@@ -55,6 +55,8 @@ def parse():
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="budget of the cpu_baseline sample")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-train", action="store_true", help="skip the informational training-step block")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the maps the last timed step rendered as DIR/<name>.npy (float32; a seeded row sample if over 64 MB)")
     ap.add_argument("--cpu-procs", type=int, default=0,
                     help="cpu_baseline: also run this many concurrent CPU workers (whole-box figure); 0 = cores // 16")
     ap.add_argument("--cpu-worker", type=int, default=0, help=argparse.SUPPRESS)    # internal: one whole-box worker, N threads
@@ -267,6 +269,26 @@ class ClockSampler:
 
 
 # --------------------------------------------------------------------------------------------- our arm
+DUMP_LIMIT = 64 * 10 ** 6          # bytes of all files together, .npy headers included
+NPY_HEADER = 128                    # bytes per .npy header (numpy pads the header to a multiple of 64; 128 covers these shapes)
+
+
+def dump_outputs(path, out):
+    """The arrays the timed render call returned, as float32 .npy files.  Over DUMP_LIMIT in all, the same seeded sample of
+    rays is kept from every map, and its ray indices are written as rows.npy (float64, 8 bytes per kept ray)."""
+    os.makedirs(path, exist_ok=True)
+    maps = {k: v.detach().float().cpu().numpy() for k, v in out.items() if torch.is_tensor(v) and v.numel() > 0}
+    n = min(v.shape[0] for v in maps.values())
+    per_row = sum(v[0].size * 4 for v in maps.values())
+    if n * per_row + NPY_HEADER * len(maps) > DUMP_LIMIT:
+        budget = DUMP_LIMIT - NPY_HEADER * (len(maps) + 1)
+        rows = np.sort(np.random.default_rng(0).choice(n, budget // (per_row + 8), replace=False))
+        np.save(os.path.join(path, "rows.npy"), rows.astype(np.float64))
+        maps = {k: v[rows] for k, v in maps.items()}
+    for k, v in maps.items():
+        np.save(os.path.join(path, k + ".npy"), np.ascontiguousarray(v, dtype=np.float32))
+
+
 def run_ours(args):
     import ctypes as C
     from dmnerf_b200 import synth, _lib
@@ -295,7 +317,7 @@ def run_ours(args):
     from dmnerf_b200.parallel import gather_image
     ro, rd = torch.from_numpy(wl["rays_o"]).to(dev), torch.from_numpy(wl["rays_d"]).to(dev)
     z = (torch.linspace(0, 1, N_COARSE) * (wl["far"] - wl["near"]) + wl["near"]).to(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2
 
     strong = args.scaling == "strong"
     gather_ev = []
@@ -309,12 +331,15 @@ def run_ours(args):
         poses = [torch.from_numpy(synth.workload(args.workload, frame=f)["c2w"]).to(dev) for f in range(8)]
         step_no = [0]
 
+    rendered = {}                   # this rank's maps of the latest step (before any all-gather)
+
     def step_device():
         if strong:
             c2w = poses[step_no[0] % len(poses)]
             step_no[0] += 1
             ro_r, rd_r = get_rays_at(wl["H"], wl["W"], wl["K"], c2w, pix)
             out = render_rays(ro_r, rd_r, nc, nf, z, want_raw=False, want_coarse=False, want_samples=False, impl=impl)
+            rendered["out"] = out
             if world > 1:
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()
@@ -324,6 +349,7 @@ def run_ours(args):
                 return full
             return out
         out = render_rays(ro, rd, nc, nf, z, want_raw=False, want_coarse=False, want_samples=False, impl=impl)
+        rendered["out"] = out
         if world > 1:
             return gather_image(out, world)
         return out
@@ -367,6 +393,8 @@ def run_ours(args):
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         dev_ms = float(t.item())
         gather_ms = sum(a.elapsed_time(b) for a, b in gather_ev) if gather_ev else 0.0
+        if args.dump_outputs and rank == 0 and "out" in rendered:
+            dump_outputs(args.dump_outputs, rendered["out"])
 
         # ---- end to end through the C ABI with HOST buffers (pinned), H2D + D2H inside the timed region
         h = {k: torch.empty(shape, dtype=torch.float32).pin_memory() for k, shape in
@@ -429,7 +457,7 @@ def run_ours(args):
         peaks = json.load(open(peaks_path))
         peak_tf, peak_src = float(peaks["bf16_tflops_sustained"]), "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"
     else:
-        peak_tf, peak_src = 1400.0, "fallback (B200_PROFILING.md sustained)"
+        peak_tf, peak_src = 989.0, "H100 SXM data sheet, dense BF16 (not a measured rate)"
 
     # ---- BASELINE configs[3]: training step, 1024 random rays, forward + backward through the native path + Adam
     train = None
@@ -602,7 +630,7 @@ def run_ours(args):
     line = {
         "metric": "rays/sec (64c+128f samples)", "value": value, "unit": "rays/s", "n_gpus": world, "steps": args.steps,
         "warmup": max(3, args.warmup), "ms_per_step": dev_ms / args.steps, "higher_is_better": True, "scaling": args.scaling,
-        "vs_baseline": None, "dtype": "f32 (bf16x3 split operands on tcgen05, fp32 accumulate)" if args.mlp != "simt" else "f32",
+        "vs_baseline": None, "dtype": "f32 (bf16x3 split operands on wgmma, fp32 accumulate)" if args.mlp != "simt" else "f32",
         "data": "synthetic",
         "config": {"workload": workload_text(args.workload, ins_num, n_rays, args.scaling, world),
                    "name": args.workload, "rays_per_step_per_gpu": rays_rank, "l2": "256 MiB write between timed steps",

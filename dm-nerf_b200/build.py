@@ -1,4 +1,4 @@
-"""Build recipe for libdmnerf_b200.so (nvcc, sm_100a only, in-tree so the .so travels with gpurun).
+"""Build recipe for libdmnerf_b200.so (nvcc, sm_90a, built in-tree next to the package).
 
     python -m dmnerf_b200.build           # or __graft_entry__.build()
 """
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdmnerf_b200.so")
 SOURCES = ["abi.cu", "ray_kernels.cu", "mlp_simt.cu", "mlp_umma.cu", "backward.cu", "gemm_umma.cu", "penalizer.cu", "exchanger.cu", "evaluator.cu", "bwd_chain.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -35,7 +35,7 @@ def _digest():
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu under csrc/ for sm_100a and link the shared library.  Returns the .so path."""
+    """Compile every .cu under csrc/ for sm_90a and link the shared library.  Returns the .so path."""
     os.makedirs(LIBDIR, exist_ok=True)
     stamp = os.path.join(LIBDIR, "build.sha256")
     dig = _digest()

@@ -79,8 +79,7 @@ DMNERF_API int dmnerf_ctx_create(int device, dmnerf_ctx** out) {
   DMN_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   DMN_CUDA(cudaGetDeviceProperties(&prop, device));
-  DMN_CHECK(prop.major == 10, "ctx_create: this library is built for sm_100a only (device is sm_%d%d)", prop.major,
-            prop.minor);
+  DMN_CHECK(prop.major == 9 && prop.minor == 0, "ctx_create: this library is built for sm_90a only (device is sm_%d%d)", prop.major, prop.minor);
   dmnerf_ctx* c = new dmnerf_ctx();
   c->device = device;
   *out = c;

@@ -468,7 +468,7 @@ static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, i
   const bool aligned = ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0);
   if (aligned && !b_cm && N % 4 == 0 && K % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 && N >= 64 && K >= 64) {
     const int tiles_b = ((N + BT - 1) / BT) * ((K + BT - 1) / BT);
-    int64_t splits = (3 * 148 + tiles_b - 1) / tiles_b;
+    int64_t splits = (3 * 132 + tiles_b - 1) / tiles_b;
     int64_t rows = (M + splits - 1) / splits;
     rows = ((rows + BK - 1) / BK) * BK;
     if (rows < 512) rows = 512;
@@ -479,7 +479,7 @@ static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, i
     return 0;
   }
   const int tiles = ((N + GT - 1) / GT) * ((K + GT - 1) / GT);
-  int64_t splits = (4 * 148 + tiles - 1) / tiles;
+  int64_t splits = (4 * 132 + tiles - 1) / tiles;
   int64_t rows = (M + splits - 1) / splits;
   rows = ((rows + GK - 1) / GK) * GK;
   if (rows < 256) rows = 256;
@@ -500,7 +500,7 @@ static int colsum(const float* A, int lda, float* out, int64_t M, int N, cudaStr
 
 size_t mlp_backward_scratch_floats(int64_t m) { return (size_t)m * (256 + 8 * 256) + 256 * 256 + 256 + 256; }
 
-// DMNERF_BWD_IMPL=gemm: per-layer dX GEMM kernels instead of the fused gradient chain (round-1 path; cross-check / A-B timing).
+// DMNERF_BWD_IMPL=gemm: the unfolded per-layer path below instead of the folded-head gradient chain (cross-check / A-B timing).
 static bool bwd_use_chain() {
   static int v = -1;
   if (v < 0) {
@@ -563,10 +563,10 @@ static int small_tn(const float* A, int lda, const float* B, int ldb, float* C, 
   return 0;
 }
 
-// The training backward with the fused gradient chain (bwd_chain.cu) and the heads folded like in the forward:
+// The training backward with the gradient chain (bwd_chain.cu) and the heads folded like in the forward:
 //   S1 = d rgb_hid, S2 = d ins_hid                      (bwd_heads_kernel, masks from ActPlanes::bits)
-//   dY7..dY0                                            (bwd_chain_kernel: one launch, gradients stay in tensor memory)
-//   dW(l) = dY(l)^T X(l-1), db(l) = colsum dY(l)         (tcgen05 dW GEMMs over the saved planes)
+//   dY7..dY0                                            (launch_bwd_chain: one masked wgmma dX GEMM per layer)
+//   dW(l) = dY(l)^T X(l-1), db(l) = colsum dY(l)         (batched wgmma dW GEMMs over the saved planes)
 //   P = S1^T h7, Q = S2^T h7  ->  the four feature / hidden head gradients by small dense products:
 //     dW_rgb_hid[:, :256] = P W_rf^T + c1 (x) b_rf,  dW_rgb_feat = W_rh[:, :256]^T P,  db_rgb_feat = W_rh[:, :256]^T c1   (c1 = colsum S1)
 //     (rgb_feat = h7 W_rf^T + b_rf is never materialised; same for the instance branch with Q, c2)
@@ -633,7 +633,7 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
   const float* d_sig = d_out + 3;
   const float* d_ins = d_out + 4;
   R(launch_bwd_heads(p, d_out, m, ap.bits, S12, st));
-  R(launch_bwd_chain(packed, p, S12, d_out, ap.bits, m, dY, st));
+  R(launch_bwd_chain(packed, p, S12, d_out, ap, m, dY, st));
   // ---- folded head layers (dm_nerf.py:89-99): one product against h7 for both branches; trunk (dm_nerf.py:83-87)
   R(dW(S12, 256, ap.h[7], 256, PQ, 256, 256, 256, c12));
   for (int l = 7; l >= 1; --l) R(dW(dY[l], 256, ap.h[l - 1], 256, gw(l), layer_in(l), 256, 256, gb(l)));
@@ -649,7 +649,7 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
   R(dW(S12, 256, ap.emb + (int64_t)CH_POS * m, CH_IN, gw(L_RGB_HID) + 256, 283, 128, CH_DIR, nullptr, m));
   R(flush(q_in128));
   // the three output bias gradients from one sweep over d_out
-  colsum_flat_kernel<<<148 * 4, 256, 0, st>>>(d_out, C, m * C, cs);
+  colsum_flat_kernel<<<132 * 4, 256, 0, st>>>(d_out, C, m * C, cs);
   DMN_LAUNCH_OK();
   DMN_CUDA(cudaMemcpyAsync(gb(L_RGB_OUT), cs, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   DMN_CUDA(cudaMemcpyAsync(gb(L_DENSITY), cs + 3, sizeof(float), cudaMemcpyDeviceToDevice, st));

@@ -1,263 +1,18 @@
-// Fused gradient chain of the training backward (BASELINE config 4; reference train_dmsr.py:62-64, the dX half of
-// total_loss.backward() through DM_NeRF.forward, networks/dm_nerf.py:80-106).
-//
-// One persistent tcgen05 kernel per network walks the trunk backwards for one 128-sample tile at a time and never lets a
-// gradient leave the SM between layers:
-//     dY7 = mask(h7) . (d_rgb_hid W_fold + d_sigma (x) w_density)            W_fold = W_rgb_hid[:, :256] W_rgb_feat  (folded heads)
-//     dY(l-1) = mask(h(l-1)) . (dY(l) W(l)),  l = 7 .. 1                      (the instance branch sees h.detach(): no trunk term)
-// The running gradient lives in tensor memory exactly like the forward's activation (two 128-column slots of split bf16,
-// TS-form MMAs, three passes hi*hi + lo*hi + hi*lo into fp32 accumulators); the transposed weights stream through the same
-// 8-stage ring from a second packed image (bwd image, packed with the forward one by dmnerf_set_weights); the ReLU masks are
-// 1 bit per unit, written by the training forward (ActPlanes::bits).  Each epilogue writes its masked gradient dY(l) once to
-// HBM: those planes are what the per-layer dW = dY^T X GEMMs (gemm_umma.cu) consume -- a weight gradient needs all samples
-// of one layer at once (2.4 MB of accumulators per network against 256 KB of tensor memory), so it cannot ride along.
-//
-// Same role layout and barrier protocol as mlp_umma.cu (uk_pipe.cuh): warp 0 weight producer, warp 1 MMA issuer, warp 2
-// TMEM allocation, warps 4-19 prologue + epilogue (4 lane quadrants x 4 column groups).  16 half-steps per tile:
-// 2 (head fold, K = 128 from shared memory) + 14 (layers 7..1, K = 256 from tensor memory) = 720 MMAs.
+// Gradient chain of the training backward (BASELINE config 4; reference train_dmsr.py:62-64, the dX half of
+// total_loss.backward() through DM_NeRF.forward, networks/dm_nerf.py:80-106), with the heads folded like in the forward:
+//     S1 | S2 = mask(rgb_hid) . (d_rgb W_rgb_out) | mask(ins_hid) . (d_ins W_ins_out)     (bwd_heads_kernel)
+//     dY7 = mask(h7) . (S1 W_fold + d_sigma (x) w_density)      W_fold = W_rgb_hid[:, :256] W_rgb_feat  (folded heads)
+//     dY(l-1) = mask(h(l-1)) . (dY(l) W(l)),  l = 7 .. 1        (the instance branch sees h.detach(): no trunk term)
+// Every dX product is one split-bf16 wgmma GEMM (gemm_umma.cu) whose epilogue applies the ReLU mask from the 1-bit planes the
+// training forward writes (ActPlanes::bits).  Each dY(l) is written once to HBM: those planes are what the per-layer dW GEMMs
+// consume (a weight gradient needs all samples of one layer at once).
 #include <cstring>
 
-#include "uk_pipe.cuh"
+#include "common.cuh"
 #include "umma_api.cuh"
 
 namespace dmnerf {
 namespace bk {
-
-using namespace uk;
-
-constexpr int C_STEPS = 16;
-constexpr int C_STAGES = BWD_IMAGE_STAGES;           // 120 stages of 16 KB per tile
-constexpr uint32_t C_SMEM_BYTES = SM_FUSED;          // slabs + ring + barrier block (no fused-render state)
-
-struct CArgs {
-  const uint8_t* image;       // backward operand image
-  const float* s1;            // d rgb_hid, already masked: columns 0..127 of the [M,256] head-gradient plane (128..255 = d ins_hid)
-  const float* d_out;         // d raw [M, C]: column 3 = d sigma
-  int32_t ldc;
-  const float* w_dens;        // density_linear.weight [256]
-  const uint16_t* bits;       // ActPlanes::bits: [10 planes][16 groups][M] (row-fastest 16-bit groups)
-  float* dy[8];               // dY(l) [M,256], l = 0..7
-  int64_t m;
-  int32_t* status;
-};
-
-__global__ void __launch_bounds__(N_THREADS, 1) bwd_chain_kernel(const CArgs a) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  Misc* misc = reinterpret_cast<Misc*>(smem + SM_MISC);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int64_t n_tiles = (a.m + TILE_M - 1) / TILE_M;
-  const int64_t my_tiles = (n_tiles > blockIdx.x) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-
-  if (tid == 0) {
-    for (int i = 0; i < NS; ++i) { mbar_init(&misc->full[i], 1); mbar_init(&misc->empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&misc->acc_full[i], 1);
-      mbar_init(&misc->epi_done[i][0], CHUNK_THREADS);
-      mbar_init(&misc->epi_done[i][1], CHUNK_THREADS);
-    }
-    mbar_init(&misc->inputs_ready, EPI_THREADS);
-    mbar_init(&misc->a_free, 1);
-    misc->abort_flag = 0;
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc(&misc->tmem_base, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  constexpr uint32_t tbase = 0;        // 1 CTA / SM owns all 512 columns (checked)
-  if (misc->tmem_base != 0 || (smem_u32(smem) & 1023u) != 0) {
-    if (tid == 0) { atomicExch(&misc->abort_flag, 911); atomicCAS(a.status, 0, 911); }
-  }
-
-  if (warp == 0) {
-    // =========================================================== weight producer
-    Ring ring{0, 0};
-    for (int64_t ti = 0; ti < my_tiles; ++ti) {
-      for (int si = 0; si < C_STAGES; ++si) {
-        wait_bar(&misc->empty[ring.slot], ring.phase ^ 1, misc, 111, a.status);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&misc->full[ring.slot], STAGE_BYTES);
-          bulk_g2s(smem + SM_RING + ring.slot * STAGE_BYTES, a.image + (size_t)si * STAGE_BYTES, STAGE_BYTES, &misc->full[ring.slot]);
-        }
-        __syncwarp();
-        ring.advance();
-      }
-    }
-  } else if (warp == 1) {
-    // =========================================================== MMA issuer (converged warp, one elected lane)
-    long long kp[16];
-    (void)kp;
-    Ring ring{0, 0};
-    uint32_t seen00 = 0, seen01 = 0, seen10 = 0, seen11 = 0, seen_in = 0;
-    const uint32_t ring_base = smem_u32(smem + SM_RING);
-    const uint64_t e_hi = make_sdesc_sw128(smem_u32(smem + SM_E_HI)), e_lo = make_sdesc_sw128(smem_u32(smem + SM_E_LO));
-    const uint64_t d_hi = make_sdesc_sw128(smem_u32(smem + SM_D_HI)), d_lo = make_sdesc_sw128(smem_u32(smem + SM_D_LO));
-    const uint32_t idesc128 = make_idesc_bf16(128, 128);
-    auto need_epi = [&](uint32_t gd, int c) {
-      uint32_t& sn = (gd & 1) ? (c ? seen11 : seen10) : (c ? seen01 : seen00);
-      const uint32_t need = gd / 2 + 1;
-      while (sn < need) {
-        wait_bar(&misc->epi_done[gd & 1][c], sn & 1, misc, 211, a.status);
-        ++sn;
-      }
-      tc_fence_after();
-    };
-    auto need_drained = [&](uint32_t gd) { need_epi(gd, 0); need_epi(gd, 1); };
-    auto slot_chunk = [&](int slot, int j, uint32_t d_tmem, uint32_t& accum) {
-      const uint32_t hi = tbase + TC_SLOT + slot * SLOT_COLS + j * 32;
-      issue_chunk<4, false>(misc, ring, ring_base, hi, hi + SLOT_LO, d_tmem, idesc128, accum, a.status, kp);
-    };
-    auto finish = [&](uint32_t acc) {
-      if (elect_one()) mma_commit(&misc->acc_full[acc]);
-      __syncwarp();
-    };
-    for (int64_t ti = 0; ti < my_tiles; ++ti) {
-      const uint32_t g0 = (uint32_t)ti * C_STEPS;
-      // ---- folded heads: d rgb_hid [128 x 128] (shared memory: cols 0..63 in the E slabs, 64..127 in the D slabs) -> d h7
-      for (uint32_t h = 0; h < 2; ++h) {
-        const uint32_t g = g0 + h, acc = g & 1, d_tmem = tbase + TC_ACC + acc * 128;
-        if (g >= 2) need_drained(g - 2);
-        while (seen_in < (uint32_t)ti + 1) {
-          wait_bar(&misc->inputs_ready, seen_in & 1, misc, 212, a.status);
-          ++seen_in;
-        }
-        tc_fence_after();
-        uint32_t accum = 0;
-        issue_chunk<4, true>(misc, ring, ring_base, e_hi, e_lo, d_tmem, idesc128, accum, a.status, kp);
-        issue_chunk<4, true>(misc, ring, ring_base, d_hi, d_lo, d_tmem, idesc128, accum, a.status, kp);
-        finish(acc);
-      }
-      // ---- trunk layers 7 .. 1: dY(l) [slots 0, 1] x W(l) -> d h(l-1)
-      for (int p = 1; p < 8; ++p) {
-        for (uint32_t h = 0; h < 2; ++h) {
-          const uint32_t g = g0 + 2 * p + h, acc = g & 1, d_tmem = tbase + TC_ACC + acc * 128;
-          need_drained(g - 2);
-          uint32_t accum = 0;
-          slot_chunk(0, 0, d_tmem, accum); slot_chunk(0, 1, d_tmem, accum);
-          if (h == 1 && p < 7) {                 // slot 0 is free for the epilogue of the even half-step issued before this one
-            if (elect_one()) mma_commit(&misc->a_free);
-            __syncwarp();
-          }
-          if (h == 0) need_epi(g - 1, 0);
-          slot_chunk(1, 0, d_tmem, accum);
-          if (h == 0) need_epi(g - 1, 1);
-          slot_chunk(1, 1, d_tmem, accum);
-          finish(acc);
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // =========================================================== prologue + epilogue warps
-    const int et = tid - 128;
-    const int cg = et >> 7;                   // column group: 32 of the 128 columns of a half-step
-    const int r = et & 127;                   // tile row == TMEM lane
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
-    uint8_t *e_hi_slab = smem + SM_E_HI, *e_lo_slab = smem + SM_E_LO, *d_hi_slab = smem + SM_D_HI, *d_lo_slab = smem + SM_D_LO;
-    // d rgb_hid of tile tp -> split bf16 slabs (32 of the 128 columns per thread), then inputs_ready
-    auto prologue = [&](int64_t tp) {
-      const int64_t rowp = (blockIdx.x + tp * gridDim.x) * TILE_M + r;
-      float v[32];
-      if (rowp < a.m) {
-        const float4* src = reinterpret_cast<const float4*>(a.s1 + rowp * 256 + cg * 32);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { const float4 q = __ldg(src + i); v[4 * i] = q.x; v[4 * i + 1] = q.y; v[4 * i + 2] = q.z; v[4 * i + 3] = q.w; }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = 0.0f;
-      }
-      uint8_t* hi = (cg < 2) ? e_hi_slab : d_hi_slab;
-      uint8_t* lo = (cg < 2) ? e_lo_slab : d_lo_slab;
-      const int k0 = (cg & 1) * 32;
-      store_split16_smem(v, hi, lo, r, k0);
-      store_split16_smem(v + 16, hi, lo, r, k0 + 16);
-      fence_proxy_async_smem();
-      mbar_arrive(&misc->inputs_ready);
-    };
-    if (my_tiles > 0) prologue(0);
-    for (int64_t ti = 0; ti < my_tiles; ++ti) {
-      const int64_t row = (blockIdx.x + ti * gridDim.x) * TILE_M + r;
-      const bool valid = row < a.m;
-      const float dsig = valid ? __ldg(a.d_out + row * a.ldc + 3) : 0.0f;
-      for (int t = 0; t < C_STEPS; ++t) {
-        const uint32_t g = (uint32_t)ti * C_STEPS + t, acc = g & 1;
-        const uint32_t acc_addr = tbase + lane_sel + TC_ACC + acc * 128;
-        const int p = t >> 1, h = t & 1, layer = 7 - p;      // this half-step produces dY(layer)[:, h*128 + ...]
-        // this thread's columns inside the half-step (uk_pipe.cuh): f[0..15] <-> colA + i, f[16..31] <-> colB + i
-        const int colA = epi_col_a(cg), colB = epi_col_b(cg);
-        const int cA = colA >> 6, cB = colB >> 6;
-        const uint32_t slot_addr = tbase + lane_sel + TC_SLOT + h * SLOT_COLS;
-        const uint32_t hiA = slot_addr + cA * 32 + ((colA & 63) >> 1), hiB = slot_addr + cB * 32 + ((colB & 63) >> 1);
-        // ReLU masks of the two 16-unit groups, fetched before the accumulator is waited for
-        const uint32_t mA = valid ? (uint32_t)__ldg(a.bits + act_bits_index(layer, (h * 128 + colA) >> 4, row, a.m)) : 0u;
-        const uint32_t mB = valid ? (uint32_t)__ldg(a.bits + act_bits_index(layer, (h * 128 + colB) >> 4, row, a.m)) : 0u;
-        wait_bar_warp(&misc->acc_full[acc], (g / 2) & 1, misc, 311, a.status);
-        tc_fence_after();
-        uint32_t v[32];
-        if constexpr (EPI_SPLIT) { tmem_ld_x16(acc_addr + colA, v); tmem_ld_x16(acc_addr + colB, v + 16); }
-        else tmem_ld_x32(acc_addr + colA, v);
-        tmem_ld_wait();
-        if (t >= 14) {                       // nothing goes back to a slot: the accumulator is all the MMA warp waits for
-          tc_fence_before();
-          if constexpr (EPI_SPLIT) { mbar_arrive(&misc->epi_done[acc][0]); mbar_arrive(&misc->epi_done[acc][1]); }
-          else mbar_arrive(&misc->epi_done[acc][cA]);
-        }
-        float f[32];
-        if (t < 2) {                         // + d sigma (x) w_density (dm_nerf.py:101)
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const float4 wd = __ldg(reinterpret_cast<const float4*>(a.w_dens + h * 128 + (jj < 4 ? colA : colB)) + (jj & 3));
-            f[4 * jj + 0] = fmaf(dsig, wd.x, __uint_as_float(v[4 * jj + 0]));
-            f[4 * jj + 1] = fmaf(dsig, wd.y, __uint_as_float(v[4 * jj + 1]));
-            f[4 * jj + 2] = fmaf(dsig, wd.z, __uint_as_float(v[4 * jj + 2]));
-            f[4 * jj + 3] = fmaf(dsig, wd.w, __uint_as_float(v[4 * jj + 3]));
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-        }
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {                         // ReLU of layer `layer` (dm_nerf.py:85)
-          f[i] = ((mA >> i) & 1u) ? f[i] : 0.0f;
-          f[16 + i] = ((mB >> i) & 1u) ? f[16 + i] : 0.0f;
-        }
-        if (t < 14) {
-          if (h == 0 && t >= 2) {            // slot 0 still feeds the odd half-step issued behind this one
-            wait_bar_warp(&misc->a_free, (uint32_t)(ti * 6 + (p - 1)) & 1u, misc, 312, a.status);
-            tc_fence_after();
-          }
-          if constexpr (EPI_SPLIT) {
-            store_split16_tmem(f, hiA, hiA + SLOT_LO);           // K chunk 0 first: published half an epilogue earlier
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&misc->epi_done[acc][0]);
-            store_split16_tmem(f + 16, hiB, hiB + SLOT_LO);
-          } else {
-            store_split32_tmem(f, hiA, hiA + SLOT_LO);
-          }
-          tmem_st_wait();
-          tc_fence_before();
-          mbar_arrive(&misc->epi_done[acc][EPI_SPLIT ? 1 : cA]);
-        }
-#ifndef DMN_EXP_CHAIN_NOSTORE      /* timing experiment: no gradient planes written (results are garbage) */
-        {
-          float* dst = a.dy[layer] + row * W_HID + h * 128;
-          if constexpr (EPI_SPLIT) {
-            const bool ok_other = (row ^ 1) < a.m;
-            store_row16_paired(dst + colA, W_HID, f, valid, ok_other, r & 31);
-            store_row16_paired(dst + colB, W_HID, f + 16, valid, ok_other, r & 31);
-          } else {
-            if (valid) store_row32(dst + colA, f);
-          }
-        }
-#endif
-        if (t == 3 && ti + 1 < my_tiles) prologue(ti + 1);   // the slabs were last read by half-step 1
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(misc->tmem_base, 512);
-}
 
 // ------------------------------------------------------------------------------------------------ head gradients
 // d rgb_hid = mask . (d_rgb W_rgb_out), d ins_hid = mask . (d_ins W_ins_out)   (dm_nerf.py:102-103 backwards, K = 3 / ins_num+1)
@@ -355,6 +110,18 @@ __global__ void mask_bits_kernel(const float* __restrict__ plane, int width, int
   bits[act_bits_index(pl, g, row, m)] = (uint16_t)b;
 }
 
+// dY7 before the mask: d sigma (x) density_linear.weight (dm_nerf.py:101 backwards); the folded rgb head is added by the GEMM.
+__global__ void dsig_outer_kernel(const float* __restrict__ d_out, int C, const float* __restrict__ w_dens, int64_t m,
+                                  float* __restrict__ dy7) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;      // one thread per 4 units of a row
+  if (idx >= m * 64) return;
+  const int64_t row = idx >> 6;
+  const int u = (int)(idx & 63) * 4;
+  const float d = __ldg(d_out + row * C + 3);
+  *reinterpret_cast<float4*>(dy7 + row * 256 + u) =
+      make_float4(d * __ldg(w_dens + u), d * __ldg(w_dens + u + 1), d * __ldg(w_dens + u + 2), d * __ldg(w_dens + u + 3));
+}
+
 }  // namespace bk
 
 // ================================================================================================ host
@@ -384,32 +151,19 @@ int launch_bwd_heads(const NetParams& p, const float* d_out, int64_t m, const ui
   return 0;
 }
 
-// dY(7..0) of one network from d rgb_hid (s1) and d sigma (column 3 of d_out).  dy: 8 planes [m,256].
-int launch_bwd_chain(const UmmaWeights& w, const NetParams& p, const float* s1, const float* d_out, const uint16_t* bits, int64_t m,
+// dY(7..0) of one network from d rgb_hid (s1, row stride 256) and d sigma (column 3 of d_out).  dy: 8 planes [m,256].
+int launch_bwd_chain(const UmmaWeights& w, const NetParams& p, const float* s1, const float* d_out, const ActPlanes& ap, int64_t m,
                      float* const* dy, cudaStream_t st) {
-  using namespace bk;
   DMN_CHECK(w.ready && w.extra, "bwd_chain: weights not packed (call dmnerf_set_weights first)");
-  DMN_CHECK(umma_status_peek(w) == 0, "bwd_chain: an earlier tcgen05 launch reported protocol error %d (bounded wait expired); its results "
-            "are invalid -- destroy the context", umma_status_peek(w));
   if (m == 0) return 0;
-  static PerDeviceOnce attr_once;
-  if (attr_once.first())
-    DMN_CUDA(cudaFuncSetAttribute(bwd_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C_SMEM_BYTES));
-  int dev = 0, sms = 148;
-  DMN_CUDA(cudaGetDevice(&dev));
-  DMN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CArgs a;
-  memset(&a, 0, sizeof(a));
-  a.image = umma_bwd_image(w);
-  a.s1 = s1; a.d_out = d_out; a.ldc = 4 + p.ins_num + 1; a.w_dens = p.w[L_DENSITY]; a.bits = bits; a.m = m;
-  for (int l = 0; l < 8; ++l) a.dy[l] = dy[l];
-  a.status = umma_status_word(w);
-  DMN_CHECK(a.image != nullptr, "bwd_chain: backward operand image missing");
-  const int64_t tiles = (m + TILE_M - 1) / TILE_M;
-  const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
-  bwd_chain_kernel<<<grid, N_THREADS, C_SMEM_BYTES, st>>>(a);
+  const int C = 4 + p.ins_num + 1;
+  bk::dsig_outer_kernel<<<(unsigned)((m * 64 + 255) / 256), 256, 0, st>>>(d_out, C, p.w[L_DENSITY], m, dy[7]);
   DMN_LAUNCH_OK();
-  return 0;
+  auto bits = [&](int plane) { return ap.bits + (int64_t)plane * ACT_BITS_GROUPS * m; };
+  int rc = launch_gemm_nn_tc(s1, 256, umma_fold_w_rgb(w), 283, dy[7], 256, m, 128, 1, nullptr, nullptr, 0, st, bits(7));
+  for (int l = 7; l >= 1 && rc == 0; --l)
+    rc = launch_gemm_nn_tc(dy[l], 256, p.w[l], layer_in(l), dy[l - 1], 256, m, 256, 0, nullptr, nullptr, 0, st, bits(l - 1));
+  return rc;
 }
 
 }  // namespace dmnerf

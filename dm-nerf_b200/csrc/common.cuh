@@ -1,4 +1,4 @@
-// Shared declarations for libdmnerf_b200.so (sm_100a only).
+// Shared declarations for libdmnerf_b200.so (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -51,8 +51,7 @@ __host__ __device__ inline int layer_in(int l) {
 //  makes every store instruction of a warp one contiguous 128-byte line; their only readers are three narrow dW GEMMs)
 // ... | bits: ReLU masks, 1 bit per unit, as 16-bit groups stored ROW-FASTEST: [10 planes][16 groups][M] uint16 (planes 0..7 =
 //           H0..H7, 8 = rgb_hid, 9 = ins_hid (8 groups used); bit c of group g = unit 16 g + c is positive).  A warp (32
-//           consecutive rows, one group) reads or writes 64 contiguous bytes -- what the fused gradient chain (bwd_chain.cu) reads
-//           instead of the planes.
+//           consecutive rows, one group) reads or writes 64 contiguous bytes.
 constexpr int ACT_BITS_PLANES = 10, ACT_BITS_WORDS = 8, ACT_BITS_GROUPS = 16;
 __host__ __device__ inline int64_t act_bits_index(int plane, int group, int64_t row, int64_t m) {
   return ((int64_t)plane * ACT_BITS_GROUPS + group) * m + row;
@@ -140,18 +139,19 @@ int launch_composite_backward(const float* raw, const float* z, const float* ray
 struct UmmaWeights;
 int launch_mlp_backward(const NetParams& p, const UmmaWeights* packed, float* acts, const float* d_out, int64_t m, float* const* grads,
                         float* scratch, int feats_missing, cudaStream_t st);
-// Fused gradient chain (bwd_chain.cu)
+// Gradient chain (bwd_chain.cu)
 int launch_mask_bits(float* acts, int64_t m, cudaStream_t st);
 int launch_bwd_heads(const NetParams& p, const float* d_out, int64_t m, const uint16_t* bits, float* s12, cudaStream_t st);
-int launch_bwd_chain(const UmmaWeights& w, const NetParams& p, const float* s1, const float* d_out, const uint16_t* bits, int64_t m,
+int launch_bwd_chain(const UmmaWeights& w, const NetParams& p, const float* s1, const float* d_out, const ActPlanes& ap, int64_t m,
                      float* const* dy, cudaStream_t st);
 size_t mlp_backward_scratch_floats(int64_t m);
 
-// Tensor-core GEMMs of the backward (gemm_umma.cu): split-bf16 three-pass tcgen05 kernels for the wide layer shapes.
+// Tensor-core GEMMs of the backward (gemm_umma.cu): split-bf16 three-pass wgmma kernels for the wide layer shapes.
 bool gemm_nn_tc_supported(int N, int K, int ldc, const float* C, const float* mask);
 bool gemm_tn_tc_supported(int N, int K);
+// mask_bits: 1-bit ReLU mask of the output, [16 groups][M] uint16 (one plane of ActPlanes::bits), or NULL.
 int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C, int ldc, int64_t M, int N, int accumulate,
-                      const float* mask, const float* bias, int w_kmajor, cudaStream_t st);
+                      const float* mask, const float* bias, int w_kmajor, cudaStream_t st, const uint16_t* mask_bits = nullptr);
 // One product of a batched dW launch (gemm_umma.cu): C[N, K] += A[M, N]^T B[M, K]; b_cm != 0: B is column-major with that column
 // stride; transpose: A is the wide operand and the result goes to C[K, N].
 constexpr int TN_MAX_BATCH = 8;

@@ -1,28 +1,21 @@
-// tcgen05 (UMMA) GEMM kernels for the training backward of the DM_NeRF network (networks/dm_nerf.py:80-106 differentiated,
-// driven by train_dmsr.py:62-64): the two wide GEMM shapes of every layer,
+// Warpgroup-MMA (wgmma) GEMM kernels for the training backward of the DM_NeRF network (networks/dm_nerf.py:80-106
+// differentiated, driven by train_dmsr.py:62-64): the two wide GEMM shapes of every layer,
 //
 //   gemm_nn:  dX[M, 256]  (+)= dY[M, N] * W[N, 256]            (N = 128 or 256; optional ReLU mask from the saved activation)
 //   gemm_tn:  dW[NA, 256]  +=  dY[M, NA]^T * X[M, 256]          (NA = 128 or 256; contraction over the M samples)
 //
 // with the same fp32-grade arithmetic as the forward kernel: every fp32 operand is split into bf16 hi + bf16 lo and each
-// product is issued as three tensor passes  A_hi*B_hi + A_lo*B_hi + A_hi*B_lo  into fp32 accumulators in tensor memory.
+// product is issued as three tensor passes  A_hi*B_hi + A_lo*B_hi + A_hi*B_lo  into fp32 accumulators in registers.
 //
 // Operands come straight from the row-major fp32 matrices in global memory; the only preparation is the hi/lo split, done by
 // the CUDA cores while the block is written into shared memory.  One loader serves every operand, because the memory image
 // of a [rows][64 columns] block in the SWIZZLE_128B layout is the same whether the tensor core reads it K-major (rows = M or
 // N index, columns = contraction index: dY in gemm_nn) or MN-major (rows = contraction index, columns = M / N index: W in
-// gemm_nn, dY and X in gemm_tn) -- only the descriptor differs: MN-major operands set the a/b "major" bits of the instruction
-// descriptor, their leading byte offset is the stride between 64-column blocks, their stride byte offset the 1024 B between
-// 8-row groups, and a K = 16 step advances the start address by two such groups (validated on hardware by
-// tools/umma_probe.cu, modes 7 / 8 -> profiles/r01_umma_probe.txt).
+// gemm_nn, dY and X in gemm_tn) -- only the descriptor and the transpose flag of the instruction differ.
 //
-// Structure (both kernels): 512 threads, persistent CTAs.  All 16 warps split the stage they fetched into registers one or two
-// stages earlier and store it (2-3 stages of shared memory), issue the global loads of a later stage, the block synchronises,
-// and one elected lane of warp 0 issues the stage's 12 MMAs and commits them to the stage's mbarrier; loads, splits and tensor
-// work of neighbouring stages overlap.  gemm_nn alternates between two [128 x 256] accumulators and drains a tile one stage
-// late, while the next tile's first chunk is multiplied (epilogue: optional bias / accumulate, ReLU mask, fp32 store);
-// gemm_tn keeps the whole [NA x NB] gradient in tensor memory for the CTA's share of the samples, writes it once to its slice
-// of a scratch buffer, and a small kernel adds the slices.
+// Structure (both kernels): persistent CTAs, two shared-memory stages.  Every thread splits the block it fetched into
+// registers one stage earlier and stores it while the tensor core multiplies the previous stage; the global loads of the stage
+// after that are in flight at the same time.  Each warpgroup issues the MMAs of its own 64-row slice of the output tile.
 #include <cstring>
 
 #include "common.cuh"
@@ -33,40 +26,16 @@ namespace tg {
 
 using namespace umma;
 
-constexpr int NT = 512;                    // threads per CTA: 16 warps load + split; one elected lane of warp 0 issues
 constexpr int NOUT = 256;                  // output columns (gemm_nn) / columns of X (gemm_tn)
 
-// SWIZZLE_128B shared-memory descriptor with explicit leading / stride byte offsets.
-__device__ __forceinline__ uint64_t sdesc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)(lbo >> 4) << 16;
-  d |= (uint64_t)(sbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-constexpr uint32_t A_MN = 1u << 15, B_MN = 1u << 16;      // instruction-descriptor bits: operand is MN-major
-
-// One 16-byte unit of a bf16 slab = 8 consecutive fp32 values of one matrix row.  Loads are issued one or two stages ahead
-// of their use (register prefetch): with a single thread of control per stage the DRAM latency would otherwise sit on the
-// critical path of every stage.
+// One 16-byte unit of a bf16 slab = 8 consecutive fp32 values of one matrix row.
 struct Unit { float v[8]; };
 
 // 8 floats of row r (valid below r_end), columns col.. (valid below c_end) of a row-major matrix; zero outside.
 __device__ __forceinline__ void load_unit(Unit& u, const float* __restrict__ src, int64_t ld, int64_t r, int64_t r_end, int col,
                                           int c_end, int vec_ok) {
   if (r < r_end && vec_ok && col + 8 <= c_end) {
-    const float* p = src + r * ld + col;
-#ifdef DMN_LD256
-    if (vec_ok & 2) {       // 32-byte aligned rows: one 256-bit load per unit instead of two 128-bit ones
-      asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                   : "=f"(u.v[0]), "=f"(u.v[1]), "=f"(u.v[2]), "=f"(u.v[3]), "=f"(u.v[4]), "=f"(u.v[5]), "=f"(u.v[6]), "=f"(u.v[7])
-                   : "l"(p));
-      return;
-    }
-#endif
-    const float4* p4 = reinterpret_cast<const float4*>(p);
+    const float4* p4 = reinterpret_cast<const float4*>(src + r * ld + col);
     const float4 x = __ldg(p4), y = __ldg(p4 + 1);
     u.v[0] = x.x; u.v[1] = x.y; u.v[2] = x.z; u.v[3] = x.w; u.v[4] = y.x; u.v[5] = y.y; u.v[6] = y.z; u.v[7] = y.w;
   } else {
@@ -100,15 +69,15 @@ __device__ __forceinline__ void fail(int32_t* status, int code) { atomicCAS(stat
 // W_KMAJOR = true:   C[M, 256]   =  A[M, N] * W[256, N]^T + bias       (y = x W^T + b: rebuilds the feature planes)
 // N = 64 * NCH.  The weight matrix is the same for every tile, so it is split ONCE per call into a packed image of ready-made
 // stage blocks (pack_w_kernel) that are streamed into the stages with bulk async copies (TMA engine, mbarrier transaction
-// counts, requested as soon as a stage is free); the 16 loader warps only handle the activation / gradient rows, fetched two
-// stages ahead.
+// counts, requested as soon as a stage is free); the threads only handle the activation / gradient rows.
+// Output tile [128 x 256]: warpgroup w owns rows 64 (w & 1) and columns 128 (w >> 1).
+constexpr int NN_THREADS = 512;
 constexpr uint32_t NN_A_BYTES = 128 * 128;               // one [128 x 64] slab
 constexpr uint32_t NN_W_BYTES = 256 * 128;               // the W block of a chunk: 4 slabs [64 x 64] or one slab [256 x 64]
 constexpr uint32_t NN_W_SLAB = 64 * 128;
 constexpr uint32_t NN_STAGE = 2 * NN_A_BYTES + 2 * NN_W_BYTES;          // A hi, A lo, W hi, W lo = 96 KB
 constexpr uint32_t NN_SMEM = 2 * NN_STAGE + 1024;
-constexpr int NN_UA = 128 * 8 / NT;                      // A units per thread and stage: 2
-constexpr int NN_THREADS = NT;
+constexpr int NN_UA = 128 * 8 / NN_THREADS;              // A units per thread and stage: 2
 
 // image[c] = { W_hi block, W_lo block } of contraction chunk c, in the shared-memory layout of a stage.
 template <bool W_KMAJOR>
@@ -131,172 +100,126 @@ __global__ void pack_w_kernel(const float* __restrict__ W, int ldw, int nch, int
 template <int NCH, bool W_KMAJOR>
 __global__ void __launch_bounds__(NN_THREADS, 1) gemm_nn_tc_kernel(const float* __restrict__ A, int lda, const uint8_t* __restrict__ wimage,
                                                                    float* __restrict__ C, int ldc, int64_t M, int accumulate,
-                                                                   const float* __restrict__ mask, const float* __restrict__ bias,
-                                                                   int vec_a, int32_t* status) {
+                                                                   const float* __restrict__ mask, const uint16_t* __restrict__ mbits,
+                                                                   const float* __restrict__ bias, int vec_a, int32_t* status) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ uint64_t done[2], wfull[2], acc_done[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t wfull[2];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    mbar_init(&done[0], 1); mbar_init(&done[1], 1); mbar_init(&wfull[0], 1); mbar_init(&wfull[1], 1);
-    mbar_init(&acc_done[0], 1); mbar_init(&acc_done[1], 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(&tmem_base_s, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tD = tmem_base_s;
-  const uint32_t idesc = make_idesc_bf16(128, NOUT) | (W_KMAJOR ? 0u : B_MN);
+  const int tid = threadIdx.x, wg = tid >> 7, wl = (tid >> 5) & 3, lane = tid & 31;
   const int64_t n_tiles = (M + 127) / 128;
   const int64_t my_tiles = (n_tiles > blockIdx.x) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
   const int64_t n_chunks = my_tiles * NCH;
   // chunk q of this CTA: tile blockIdx.x + (q / NCH) * gridDim.x, contraction columns [64 (q % NCH), +64)
-
-  {
-    // ===================================================== loaders + weight requests + MMA issuer + epilogue (16 warps)
-    auto issue = [&](Unit (&r)[NN_UA], int64_t q) {
-      const int c = (int)(q % NCH);
-      const int64_t m0 = (blockIdx.x + (q / NCH) * gridDim.x) * 128;
+  auto request_w = [&](int64_t q) {
+    const uint32_t s = (uint32_t)q & 1;
+    uint8_t* w_hi = smem + s * NN_STAGE + 2 * NN_A_BYTES;
+    const int c = (int)(q % NCH);
+    mbar_arrive_expect_tx(&wfull[s], 2 * NN_W_BYTES);
 #pragma unroll
-      for (int i = 0; i < NN_UA; ++i) {
-        const int u = tid + i * NT;
-        load_unit(r[i], A, lda, m0 + (u >> 3), M, 64 * c + (u & 7) * 8, 64 * NCH, vec_a != 0);
-      }
-    };
-    // ReLU mask of this thread's 64 output values of local tile `ti` (two 128-byte lines of the saved activation): requested
-    // into L2 at the top of a stage (no registers held while the stage runs) and read in the epilogue one chunk later.
-    auto tile_row = [&](int64_t ti) { return (blockIdx.x + ti * gridDim.x) * 128 + (warp & 3) * 32 + lane; };
-    auto prefetch_mask = [&](int64_t ti) {
-      const int64_t m_row = tile_row(ti);
-      if (mask == nullptr || m_row >= M) return;
-      const float* p0 = mask + m_row * ldc + (warp >> 2) * 64;
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(p0));
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(p0 + 32));
-    };
-    // Epilogue of local tile ti (accumulator ti & 1): warp w -> rows (w & 3) * 32 + lane, columns (w >> 2) * 64 ...
-    auto epilogue = [&](int64_t ti) {
-      if (!mbar_wait(&acc_done[ti & 1], (uint32_t)(ti >> 1) & 1)) fail(status, 602);
-      __syncwarp();                 // lanes can leave the spin at different times; tcgen05.ld below is .sync.aligned
-      tc_fence_after();
-      const int64_t m = tile_row(ti);
-      const int col0 = (warp >> 2) * 64;
-      const uint32_t taddr = tD + (uint32_t)(ti & 1) * 256 + ((uint32_t)((warp & 3) * 32) << 16) + col0;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_x32(taddr + c0, v);
-        tmem_ld_wait();
-        if (m < M) {
-          float* crow = C + m * ldc + col0 + c0;
-          uint32_t mb = 0xFFFFFFFFu;
-          if (mask) {
-            const float4* mrow4 = reinterpret_cast<const float4*>(mask + m * ldc + col0 + c0);
-            mb = 0;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 x = __ldg(mrow4 + j);
-              mb |= (x.x > 0.0f ? 1u : 0u) << (4 * j) | (x.y > 0.0f ? 1u : 0u) << (4 * j + 1) | (x.z > 0.0f ? 1u : 0u) << (4 * j + 2) |
-                    (x.w > 0.0f ? 1u : 0u) << (4 * j + 3);
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-            if (bias) {
-              const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + col0 + c0 + j));
-              o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
-            }
-            if (accumulate) {
-              const float4 old = *reinterpret_cast<const float4*>(crow + j);
-              o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-            }
-            if (!((mb >> j) & 1u)) o.x = 0.0f;
-            if (!((mb >> (j + 1)) & 1u)) o.y = 0.0f;
-            if (!((mb >> (j + 2)) & 1u)) o.z = 0.0f;
-            if (!((mb >> (j + 3)) & 1u)) o.w = 0.0f;
-            *reinterpret_cast<float4*>(crow + j) = o;
-          }
-        }
-      }
-      tc_fence_before();                 // ordered before the block barrier of the stage that reuses this accumulator
-    };
-    auto stage = [&](Unit (&r)[NN_UA], int64_t q) {
-      const int c = (int)(q % NCH);
-      const int64_t ti = q / NCH;
-      const uint32_t s = (uint32_t)q & 1;
-      uint8_t* st = smem + s * NN_STAGE;
-      uint8_t *a_hi = st, *a_lo = st + NN_A_BYTES, *w_hi = st + 2 * NN_A_BYTES, *w_lo = w_hi + NN_W_BYTES;
-      // the previous tile is drained one stage late -- after this tile's first chunk has been handed to the tensor core
-      // (the two tiles use different accumulators) -- so its epilogue overlaps tensor work instead of stalling it
-      const bool drain_prev = (c == 0) && ti > 0;
-      if (drain_prev) prefetch_mask(ti - 1);
-      if (q >= 2 && !mbar_wait(&done[s], (uint32_t)((q >> 1) - 1) & 1)) fail(status, 601);      // the MMAs that read this stage are done
-      if (tid == 0) {
-        // this chunk's weights: 64 KB from the packed image (L2); they land while the previous chunk is still being multiplied
-        mbar_arrive_expect_tx(&wfull[s], 2 * NN_W_BYTES);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) bulk_g2s(w_hi + i * 16384, wimage + (size_t)c * 2 * NN_W_BYTES + i * 16384, 16384, &wfull[s]);
-      }
-#pragma unroll
-      for (int i = 0; i < NN_UA; ++i) {
-        const int u = tid + i * NT;
-        store_unit(r[i], a_hi, a_lo, u >> 3, u & 7);
-      }
-      if (q + 2 < n_chunks) issue(r, q + 2);               // in flight while this and the next stage are multiplied
-      fence_proxy_async_smem();
-      __syncthreads();
-      if (warp == 0) {
-        if (!mbar_wait(&wfull[s], (uint32_t)(q >> 1) & 1)) fail(status, 604);                   // this stage's weights have landed
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa_hi = smem_u32(a_hi), sa_lo = smem_u32(a_lo), sw_hi = smem_u32(w_hi), sw_lo = smem_u32(w_lo);
-          const uint32_t d = tD + (uint32_t)(ti & 1) * 256;
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t da_hi = sdesc(sa_hi + ks * 32, 16, 1024), da_lo = sdesc(sa_lo + ks * 32, 16, 1024);
-            const uint64_t db_hi = W_KMAJOR ? sdesc(sw_hi + ks * 32, 16, 1024) : sdesc(sw_hi + ks * 2048, NN_W_SLAB, 1024);
-            const uint64_t db_lo = W_KMAJOR ? sdesc(sw_lo + ks * 32, 16, 1024) : sdesc(sw_lo + ks * 2048, NN_W_SLAB, 1024);
-            mma_ss(d, da_hi, db_hi, idesc, (c == 0 && ks == 0) ? 0u : 1u);
-            mma_ss(d, da_lo, db_hi, idesc, 1u);
-            mma_ss(d, da_hi, db_lo, idesc, 1u);
-          }
-          mma_commit(&done[s]);
-          if (c == NCH - 1) mma_commit(&acc_done[ti & 1]);
-        }
-        __syncwarp();
-      }
-      if (drain_prev) epilogue(ti - 1);
-    };
-    Unit r0[NN_UA], r1[NN_UA];
-    if (n_chunks > 0) issue(r0, 0);
-    if (n_chunks > 1) issue(r1, 1);
-    for (int64_t q = 0; q < n_chunks; q += 2) {
-      stage(r0, q);
-      if (q + 1 < n_chunks) stage(r1, q + 1);
-    }
-    if (my_tiles > 0) epilogue(my_tiles - 1);            // the last tile
+    for (int i = 0; i < 4; ++i) bulk_g2s(w_hi + i * 16384, wimage + (size_t)c * 2 * NN_W_BYTES + i * 16384, 16384, &wfull[s]);
+  };
+  if (tid == 0) {
+    mbar_init(&wfull[0], 1); mbar_init(&wfull[1], 1);
+    fence_barrier_init();
+    if (n_chunks > 0) request_w(0);
+    if (n_chunks > 1) request_w(1);
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 0) tmem_dealloc(tD, 512);
+  auto load = [&](Unit (&r)[NN_UA], int64_t q) {
+    const int c = (int)(q % NCH);
+    const int64_t m0 = (blockIdx.x + (q / NCH) * gridDim.x) * 128;
+#pragma unroll
+    for (int i = 0; i < NN_UA; ++i) {
+      const int u = tid + i * NN_THREADS;
+      load_unit(r[i], A, lda, m0 + (u >> 3), M, 64 * c + (u & 7) * 8, 64 * NCH, vec_a != 0);
+    }
+  };
+  auto store = [&](const Unit (&r)[NN_UA], int64_t q) {
+    uint8_t* st = smem + ((uint32_t)q & 1) * NN_STAGE;
+#pragma unroll
+    for (int i = 0; i < NN_UA; ++i) {
+      const int u = tid + i * NN_THREADS;
+      store_unit(r[i], st, st + NN_A_BYTES, u >> 3, u & 7);
+    }
+  };
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+  Unit r[NN_UA];
+  if (n_chunks > 0) { load(r, 0); store(r, 0); }
+  if (n_chunks > 1) load(r, 1);
+  for (int64_t q = 0; q < n_chunks; ++q) {
+    const int c = (int)(q % NCH);
+    const int64_t ti = q / NCH;
+    const uint32_t s = (uint32_t)q & 1;
+    fence_proxy_async_smem();
+    __syncthreads();                               // A(q) stored; every warpgroup has finished the MMAs of chunk q - 1
+    if (tid == 0 && q >= 1 && q + 1 < n_chunks) request_w(q + 1);     // into the stage chunk q - 1 used
+    if (!mbar_wait(&wfull[s], (uint32_t)(q >> 1) & 1)) fail(status, 604);
+    {
+      const uint32_t st = smem_u32(smem + s * NN_STAGE);
+      const uint32_t sa_hi = st + (wg & 1) * 8192, sa_lo = sa_hi + NN_A_BYTES;
+      const uint32_t sw_hi = st + 2 * NN_A_BYTES + (wg >> 1) * 16384, sw_lo = sw_hi + NN_W_BYTES;
+      wg_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint64_t da_hi = make_sdesc_sw128(sa_hi + ks * 32), da_lo = make_sdesc_sw128(sa_lo + ks * 32);
+        const uint64_t db_hi = W_KMAJOR ? make_sdesc_sw128(sw_hi + ks * 32) : sdesc(sw_hi + ks * 2048, NN_W_SLAB, 1024);
+        const uint64_t db_lo = W_KMAJOR ? make_sdesc_sw128(sw_lo + ks * 32) : sdesc(sw_lo + ks * 2048, NN_W_SLAB, 1024);
+        constexpr int TB = W_KMAJOR ? 0 : 1;
+        wgmma_n128<0, TB>(acc, da_hi, db_hi, (c == 0 && ks == 0) ? 0u : 1u);
+        wgmma_n128<0, TB>(acc, da_lo, db_hi, 1u);
+        wgmma_n128<0, TB>(acc, da_hi, db_lo, 1u);
+      }
+      wg_commit();
+    }
+    if (q + 1 < n_chunks) store(r, q + 1);          // split the next block while the tensor core works on this one
+    if (q + 2 < n_chunks) load(r, q + 2);
+    wg_wait<0>();
+    wg_reg_fence(acc);
+    if (c == NCH - 1) {
+      // epilogue: thread -> rows m0 + 64 (wg & 1) + 16 wl + lane / 4 (+ 8), columns 128 (wg >> 1) + 8 j + 2 (lane % 4) (+ 1)
+      const int64_t m_a = (blockIdx.x + ti * gridDim.x) * 128 + 64 * (wg & 1) + 16 * wl + (lane >> 2);
+      const int col0 = 128 * (wg >> 1) + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t m = m_a + 8 * h;
+        if (m >= M) continue;
+        float* crow = C + m * ldc;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int col = col0 + 8 * j;
+          float2 o = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          if (bias) { const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col)); o.x += bb.x; o.y += bb.y; }
+          if (accumulate) { const float2 old = *reinterpret_cast<const float2*>(crow + col); o.x += old.x; o.y += old.y; }
+          if (mask) {
+            const float2 mk = __ldg(reinterpret_cast<const float2*>(mask + m * ldc + col));
+            if (!(mk.x > 0.0f)) o.x = 0.0f;
+            if (!(mk.y > 0.0f)) o.y = 0.0f;
+          }
+          if (mbits) {                   // 1-bit ReLU mask: [16 groups][M] uint16, bit c of group g = unit 16 g + c
+            const uint32_t b = (uint32_t)__ldg(mbits + (int64_t)(col >> 4) * M + m) >> (col & 15);
+            if (!(b & 1u)) o.x = 0.0f;
+            if (!(b & 2u)) o.y = 0.0f;
+          }
+          *reinterpret_cast<float2*>(crow + col) = o;
+        }
+      }
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ gemm_tn
-// P[NA, NB] = A[mb:me, 0:NA]^T * B[mb:me, 0:nb] for this CTA's rows (NB = 256, or 64 with nb <= 64 valid columns); 32 samples
-// per stage, 3 stages in flight, loads issued two stages ahead.  Every CTA writes its partial product to its own slice of a
-// scratch buffer; reduce_partials_kernel adds the slices into the gradient (fp32 atomics from 148 CTAs onto the same 64 K
-// addresses were the slowest part of the first version).  colsum != NULL: colsum[n] += sum over the rows of A[:, n] (the bias
-// gradient, from the registers that already hold A).
-constexpr uint32_t TN_SLAB = 32 * 128;                   // one [32 x 64] slab
-constexpr int TN_STAGES = 3;
+// P[NA, NB] = A[mb:me, 0:NA]^T * B[mb:me, 0:nb] for this CTA's rows; the CTA computes one [128 x NBT] tile of P (NBT = 128, or
+// 64 with nb <= 64 valid columns) over 32 samples per stage.  Both operands are MN-major (the samples are the contraction index).
+// Every CTA writes its partial product to its own slice of a scratch buffer; reduce_partials_kernel adds the slices into the
+// gradient in a fixed order.  colsum != NULL: colsum[n] += sum over the rows of A[:, n] (the bias gradient, from the registers
+// that already hold A).
+constexpr int TN_THREADS = 256;
+constexpr uint32_t TN_SLAB = 32 * 128;                   // one [32 samples x 64 columns] block
 
 // A launch multiplies up to TN_MAX_BATCH independent products over the same M samples (the weight gradients of several layers of
-// one network: their operands are all on hand once the gradient chain has run): CTA b works on product b / slices, sample
-// slice b % slices.  With 8 products a CTA's slice is 8x longer than with one product per launch (fewer, longer pipelines:
-// the fill / drain and the 256 KB accumulator write are paid once per 8x the samples) and 8x fewer partial slices are written
-// and re-read by the reduction.
+// one network: their operands are all on hand once the gradient chain has run).  blockIdx.x = ((prob * tiles) + tile) * slices + slice.
 struct TnBatch {
   TnProblem p[TN_MAX_BATCH];
   int vec_a[TN_MAX_BATCH], vec_b[TN_MAX_BATCH];
@@ -304,39 +227,27 @@ struct TnBatch {
   int64_t rows_per_cta;
 };
 
-template <int NA, int NB>
-__global__ void __launch_bounds__(NT, 1) gemm_tn_tc_kernel(const __grid_constant__ TnBatch batch, float* __restrict__ partial,
-                                                           int64_t M, int32_t* status) {
-  const int prob = (int)blockIdx.x / batch.slices, slice = (int)blockIdx.x - prob * batch.slices;
+template <int NBT>
+__global__ void __launch_bounds__(TN_THREADS, 1) gemm_tn_tc_kernel(const __grid_constant__ TnBatch batch, float* __restrict__ partial,
+                                                                   int64_t M, int NA, int NB, int32_t* status) {
+  constexpr int SB = NBT / 64;                           // B blocks per stage
+  constexpr uint32_t STAGE = 2 * (2 + SB) * TN_SLAB;     // A (2 blocks) + B, hi + lo
+  constexpr int UPT = ((2 + SB) * 256) / TN_THREADS;     // units per thread per stage: unit U = tid + i * TN_THREADS
+  constexpr int NACC = NBT / 2;
+  const int tiles_n = NA / 128, tiles_k = NB / NBT, tiles = tiles_n * tiles_k;
+  const int slice = (int)blockIdx.x % batch.slices, pt = (int)blockIdx.x / batch.slices;
+  const int prob = pt / tiles, tile = pt % tiles, tn = tile / tiles_k, tk = tile % tiles_k;
   const float* __restrict__ A = batch.p[prob].A;
   const float* __restrict__ B = batch.p[prob].B;
-  float* __restrict__ colsum = batch.p[prob].colsum;
+  float* __restrict__ colsum = tk == 0 ? batch.p[prob].colsum : nullptr;
   const int lda = batch.p[prob].lda, ldb = batch.p[prob].ldb, nb = batch.p[prob].K;
   const int vec_a = batch.vec_a[prob], vec_b = batch.vec_b[prob];
   const int64_t b_cm = batch.p[prob].b_cm, rows_per_cta = batch.rows_per_cta;
-  constexpr int SA = NA / 64, SB = NB / 64;              // slabs per operand
-  constexpr uint32_t STAGE = 2 * (SA + SB) * TN_SLAB;   // hi + lo
-  constexpr int NH = NA / 128;                           // accumulators of 128 gradient rows
-  constexpr int UPT = ((SA + SB) * 256 + NT - 1) / NT;   // units per thread per stage; unit U = tid + i * NT
-  constexpr int ACC_COLS = (NH * NB < 32) ? 32 : NH * NB;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ uint64_t done[TN_STAGES], filled[TN_STAGES], acc_done;
-  __shared__ uint32_t tmem_base_s;
-  __shared__ float csum_s[NA];
+  __shared__ float csum_s[128];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    for (int i = 0; i < TN_STAGES; ++i) { mbar_init(&done[i], 1); mbar_init(&filled[i], NT); }
-    mbar_init(&acc_done, 1);
-    fence_barrier_init();
-  }
-  if (tid < NA) csum_s[tid] = 0.0f;
-  if (warp == 0) tmem_alloc(&tmem_base_s, ACC_COLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tD = tmem_base_s;
-  const uint32_t idesc = make_idesc_bf16(128, NB) | A_MN | B_MN;
+  const int tid = threadIdx.x, wg = tid >> 7, wl = (tid >> 5) & 3, lane = tid & 31;
+  if (tid < 128) csum_s[tid] = 0.0f;
   const int64_t mb = (int64_t)slice * rows_per_cta;
   const int64_t me = (mb + rows_per_cta < M) ? mb + rows_per_cta : M;
   const int64_t n_chunks = (me > mb) ? (me - mb + 31) / 32 : 0;
@@ -345,151 +256,104 @@ __global__ void __launch_bounds__(NT, 1) gemm_tn_tc_kernel(const __grid_constant
   for (int i = 0; i < UPT; ++i)
 #pragma unroll
     for (int j = 0; j < 8; ++j) csum[i][j] = 0.0f;
-  auto issue = [&](Unit (&r)[UPT], int64_t q) {
+  auto load = [&](Unit (&r)[UPT], int64_t q) {
     const int64_t m0 = mb + q * 32;
 #pragma unroll
     for (int i = 0; i < UPT; ++i) {
-      const int U = tid + i * NT, slab = U >> 8, u = U & 255;
-      if (slab < SA) load_unit(r[i], A, lda, m0 + (u >> 3), me, 64 * slab + (u & 7) * 8, NA, vec_a);
-      else if (slab < SA + SB) {
-        if (b_cm) load_unit_cm(r[i], B, b_cm, m0 + (u >> 3), me, 64 * (slab - SA) + (u & 7) * 8, nb);
-        else load_unit(r[i], B, ldb, m0 + (u >> 3), me, 64 * (slab - SA) + (u & 7) * 8, nb, vec_b);
-      }
+      const int U = tid + i * TN_THREADS, blk = U >> 8, u = U & 255;
+      if (blk < 2) load_unit(r[i], A, lda, m0 + (u >> 3), me, 128 * tn + 64 * blk + (u & 7) * 8, NA, vec_a);
+      else if (b_cm) load_unit_cm(r[i], B, b_cm, m0 + (u >> 3), me, NBT * tk + 64 * (blk - 2) + (u & 7) * 8, nb);
+      else load_unit(r[i], B, ldb, m0 + (u >> 3), me, NBT * tk + 64 * (blk - 2) + (u & 7) * 8, nb, vec_b);
     }
   };
-  auto stage = [&](Unit (&r)[UPT], int64_t q) {            // store chunk q from registers, prefetch chunk q + 2, multiply
-    const uint32_t s = (uint32_t)(q % TN_STAGES);
-    uint8_t* st = smem + s * STAGE;
-    uint8_t *a_hi = st, *a_lo = st + SA * TN_SLAB, *b_hi = st + 2 * SA * TN_SLAB, *b_lo = b_hi + SB * TN_SLAB;
-    if (q >= TN_STAGES && !mbar_wait(&done[s], (uint32_t)(q / TN_STAGES - 1) & 1)) fail(status, 611);
+  auto store = [&](const Unit (&r)[UPT], int64_t q) {
+    uint8_t* st = smem + ((uint32_t)q & 1) * STAGE;
 #pragma unroll
     for (int i = 0; i < UPT; ++i) {
-      const int U = tid + i * NT, slab = U >> 8, u = U & 255;
-      if (slab < SA) {
-        store_unit(r[i], a_hi + slab * TN_SLAB, a_lo + slab * TN_SLAB, u >> 3, u & 7);
-        if (colsum) {
+      const int U = tid + i * TN_THREADS, blk = U >> 8, u = U & 255;
+      const int side = blk < 2 ? 0 : 1, b = blk < 2 ? blk : blk - 2;
+      uint8_t* hi = st + (side ? 2 * 2 * TN_SLAB : 0) + b * TN_SLAB;
+      uint8_t* lo = hi + (side ? SB : 2) * TN_SLAB;
+      store_unit(r[i], hi, lo, u >> 3, u & 7);
+      if (colsum && blk < 2) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) csum[i][j] += r[i].v[j];
-        }
-      } else if (slab < SA + SB) {
-        store_unit(r[i], b_hi + (slab - SA) * TN_SLAB, b_lo + (slab - SA) * TN_SLAB, u >> 3, u & 7);
+        for (int j = 0; j < 8; ++j) csum[i][j] += r[i].v[j];
       }
-    }
-    if (q + 2 < n_chunks) issue(r, q + 2);
-    // every thread announces its part of the stage on an mbarrier; only the issuing warp waits for the stage to be complete
-    // (a block-wide barrier here held all 16 loader warps back until the slowest had stored: ncu stall_barrier 12 %)
-    fence_proxy_async_smem();
-    mbar_arrive(&filled[s]);
-    if (warp == 0) {
-      if (!mbar_wait(&filled[s], (uint32_t)(q / TN_STAGES) & 1)) fail(status, 613);
-      __syncwarp();
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa_hi = smem_u32(a_hi), sa_lo = smem_u32(a_lo), sb_hi = smem_u32(b_hi), sb_lo = smem_u32(b_lo);
-#pragma unroll
-        for (int h = 0; h < NH; ++h) {
-#pragma unroll
-          for (int ks = 0; ks < 2; ++ks) {
-            const uint64_t da_hi = sdesc(sa_hi + h * 2 * TN_SLAB + ks * 2048, TN_SLAB, 1024);
-            const uint64_t da_lo = sdesc(sa_lo + h * 2 * TN_SLAB + ks * 2048, TN_SLAB, 1024);
-            const uint64_t db_hi = sdesc(sb_hi + ks * 2048, TN_SLAB, 1024), db_lo = sdesc(sb_lo + ks * 2048, TN_SLAB, 1024);
-            const uint32_t d = tD + h * NB;
-            mma_ss(d, da_hi, db_hi, idesc, (q == 0 && ks == 0) ? 0u : 1u);
-            mma_ss(d, da_lo, db_hi, idesc, 1u);
-            mma_ss(d, da_hi, db_lo, idesc, 1u);
-          }
-        }
-        mma_commit(&done[s]);
-      }
-      __syncwarp();
     }
   };
-  Unit r0[UPT], r1[UPT];
-  if (n_chunks > 0) issue(r0, 0);
-  if (n_chunks > 1) issue(r1, 1);
-  for (int64_t q = 0; q < n_chunks; q += 2) {
-    stage(r0, q);
-    if (q + 1 < n_chunks) stage(r1, q + 1);
-  }
-  float* mine = partial + (size_t)blockIdx.x * NA * NB;
-  if (n_chunks > 0) {
-    if (warp == 0) {
-      if (elect_one()) mma_commit(&acc_done);
-      __syncwarp();
-    }
-    if (colsum) {       // bias gradient: per-thread partial sums -> shared memory -> one global atomic per column and CTA
+  float acc[NACC];
 #pragma unroll
-      for (int i = 0; i < UPT; ++i) {
-        const int U = tid + i * NT, slab = U >> 8, u = U & 255;
-        if (slab < SA) {
+  for (int i = 0; i < NACC; ++i) acc[i] = 0.0f;
+  Unit r[UPT];
+  if (n_chunks > 0) { load(r, 0); store(r, 0); }
+  if (n_chunks > 1) load(r, 1);
+  for (int64_t q = 0; q < n_chunks; ++q) {
+    const uint32_t st = smem_u32(smem + ((uint32_t)q & 1) * STAGE);
+    fence_proxy_async_smem();
+    __syncthreads();                     // chunk q stored; every warpgroup has finished the MMAs of chunk q - 1
+    const uint32_t a_hi = st + wg * TN_SLAB, a_lo = a_hi + 2 * TN_SLAB;
+    const uint32_t b_hi = st + 4 * TN_SLAB, b_lo = b_hi + SB * TN_SLAB;
+    wg_fence();
 #pragma unroll
-          for (int j = 0; j < 8; ++j) atomicAdd(&csum_s[64 * slab + (u & 7) * 8 + j], csum[i][j]);
-        }
-      }
-      __syncthreads();
-      if (tid < NA) atomicAdd(colsum + tid, csum_s[tid]);
-    }
-    if (!mbar_wait(&acc_done, 0)) fail(status, 612);
-    __syncwarp();                   // lanes can leave the spin at different times; tcgen05.ld below is .sync.aligned
-    tc_fence_after();
-    // warp w -> accumulator rows (w & 3) * 32 + lane, 32-column groups (w >> 2), (w >> 2) + 4, ...
-#pragma unroll 1
-    for (int h = 0; h < NH; ++h) {
-      const int n = h * 128 + (warp & 3) * 32 + lane;                     // gradient row
-#pragma unroll 1
-      for (int c0 = (warp >> 2) * 32; c0 < NB; c0 += 128) {
-        uint32_t v[32];
-        tmem_ld_x32(tD + h * NB + ((uint32_t)((warp & 3) * 32) << 16) + c0, v);
-        tmem_ld_wait();
-        // slice layout (private to this kernel and reduce_partials_kernel): float4 ((h * NB/32 + g) * 8 + j) * 128 + row holds
-        // columns 32 g + 4 j .. + 3 of gradient row 128 h + row: the 32 lanes of a store instruction write 512 contiguous bytes
-        (void)n;
-        float4* dst = reinterpret_cast<float4*>(mine) + ((size_t)(h * (NB / 32) + c0 / 32) * 8) * 128 + (warp & 3) * 32 + lane;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          dst[(size_t)j * 128] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
+    for (int ks = 0; ks < 2; ++ks) {
+      const uint64_t da_hi = sdesc(a_hi + ks * 2048, TN_SLAB, 1024), da_lo = sdesc(a_lo + ks * 2048, TN_SLAB, 1024);
+      const uint64_t db_hi = sdesc(b_hi + ks * 2048, TN_SLAB, 1024), db_lo = sdesc(b_lo + ks * 2048, TN_SLAB, 1024);
+      const uint32_t sc = (q == 0 && ks == 0) ? 0u : 1u;
+      if constexpr (NBT == 128) {
+        wgmma_n128<1, 1>(acc, da_hi, db_hi, sc); wgmma_n128<1, 1>(acc, da_lo, db_hi, 1u); wgmma_n128<1, 1>(acc, da_hi, db_lo, 1u);
+      } else {
+        wgmma_n64<1, 1>(acc, da_hi, db_hi, sc); wgmma_n64<1, 1>(acc, da_lo, db_hi, 1u); wgmma_n64<1, 1>(acc, da_hi, db_lo, 1u);
       }
     }
-  } else {
-    for (int i = tid; i < NA * NB; i += NT) mine[i] = 0.0f;
+    wg_commit();
+    if (q + 1 < n_chunks) store(r, q + 1);
+    if (q + 2 < n_chunks) load(r, q + 2);
+    wg_wait<0>();
+    wg_reg_fence(acc);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tD, ACC_COLS);
+  if (colsum) {       // bias gradient: per-thread partial sums -> shared memory -> one global atomic per column and CTA
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < UPT; ++i) {
+      const int U = tid + i * TN_THREADS, blk = U >> 8, u = U & 255;
+      if (blk < 2) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) atomicAdd(&csum_s[64 * blk + (u & 7) * 8 + j], csum[i][j]);
+      }
+    }
+    __syncthreads();
+    if (tid < 128) atomicAdd(colsum + 128 * tn + tid, csum_s[tid]);
+  }
+  // slice layout (private to this kernel and reduce_partials_kernel): [prob][slice][NA][NB] row-major
+  float* mine = partial + ((size_t)prob * batch.slices + slice) * NA * NB;
+  const int n_a = 128 * tn + 64 * wg + 16 * wl + (lane >> 2);
+  const int k0 = NBT * tk + 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < NBT / 8; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(mine + (size_t)(n_a + 8 * h) * NB + k0 + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+  (void)status;
 }
 
-// C[n, k] += sum_slice partial[slice][n][k]  (k < K valid columns of the NB-wide partials) for product blockIdx.y of the batch;
-// transpose: C[k, n] instead (the product was computed with the roles of the two operands exchanged).  64 float4 columns x 4
-// slice groups per block: every thread keeps several independent 16-byte loads in flight (the slices were just written: they
-// come from L2).  The slices of a product are added in a fixed order: the gradient is reproducible from run to run.
+// C[n, k] += sum_slice partial[prob][slice][n][k]  (k < K valid columns of the NB-wide partials) for product blockIdx.y of the
+// batch; transpose: C[k, n] instead (the product was computed with the roles of the two operands exchanged).  The slices of a
+// product are added in a fixed order: the gradient is reproducible from run to run.
 __global__ void __launch_bounds__(256) reduce_partials_kernel(const float* __restrict__ partial, const __grid_constant__ TnBatch batch,
                                                               int NA, int NB) {
-  __shared__ float4 red[4][64];
   const TnProblem& pr = batch.p[blockIdx.y];
   const int n_cta = batch.slices, kb = pr.K, ldc = pr.ldc, transpose = pr.transpose;
   float* __restrict__ C = pr.C;
-  const int q = threadIdx.x & 63, grp = threadIdx.x >> 6;
-  const int idx4 = blockIdx.x * 64 + q, total4 = NA * NB / 4;
-  float4 s0 = make_float4(0.f, 0.f, 0.f, 0.f), s1 = s0;
-  if (idx4 < total4) {
-    const float4* src = reinterpret_cast<const float4*>(partial) + (size_t)blockIdx.y * n_cta * total4 + idx4;
-    const size_t stride = (size_t)total4;
-    int c = grp;
-    for (; c + 4 < n_cta; c += 8) {
-      const float4 x = __ldcs(src + (size_t)c * stride), y = __ldcs(src + (size_t)(c + 4) * stride);
-      s0.x += x.x; s0.y += x.y; s0.z += x.z; s0.w += x.w;
-      s1.x += y.x; s1.y += y.y; s1.z += y.z; s1.w += y.w;
-    }
-    if (c < n_cta) { const float4 x = __ldcs(src + (size_t)c * stride); s0.x += x.x; s0.y += x.y; s0.z += x.z; s0.w += x.w; }
+  const int idx4 = blockIdx.x * blockDim.x + threadIdx.x, total4 = NA * NB / 4;
+  if (idx4 >= total4) return;
+  const float4* src = reinterpret_cast<const float4*>(partial) + (size_t)blockIdx.y * n_cta * total4 + idx4;
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int c = 0; c < n_cta; ++c) {
+    const float4 x = __ldcs(src + (size_t)c * total4);
+    s.x += x.x; s.y += x.y; s.z += x.z; s.w += x.w;
   }
-  red[grp][q] = make_float4(s0.x + s1.x, s0.y + s1.y, s0.z + s1.z, s0.w + s1.w);
-  __syncthreads();
-  if (grp != 0 || idx4 >= total4) return;
-  const float4 a = red[0][q], b = red[1][q], c = red[2][q], d = red[3][q];
-  const float v[4] = {(a.x + b.x) + (c.x + d.x), (a.y + b.y) + (c.y + d.y), (a.z + b.z) + (c.z + d.z), (a.w + b.w) + (c.w + d.w)};
-  // slice layout of gemm_tn_tc_kernel: float4 idx4 = ((h * NB/32 + g) * 8 + j) * 128 + row  ->  row 128 h + row, columns 32 g + 4 j ..
-  const int row = idx4 & 127, j = (idx4 >> 7) & 7, hg = idx4 >> 10, g = hg % (NB / 32), h = hg / (NB / 32);
-  const int n = h * 128 + row, k0 = g * 32 + 4 * j;
+  const float v[4] = {s.x, s.y, s.z, s.w};
+  const int n = (idx4 * 4) / NB, k0 = (idx4 * 4) % NB;
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
     const int k = k0 + e;
@@ -505,7 +369,7 @@ struct DevState {
   int32_t* status = nullptr;          // device error word of the GEMM kernels
   uint8_t* wimage = nullptr;          // packed weights of the dX GEMM in flight (4 chunks x 64 KB)
   float* partial = nullptr;           // per-CTA partial products of the dW GEMM
-  size_t partial_ctas = 0;
+  size_t partial_floats = 0;
   int sms = 0;
 };
 constexpr int MAX_DEVICES = 64;
@@ -520,29 +384,26 @@ static int dev_state(DevState** out) {
     DMN_CUDA(cudaMalloc((void**)&d.status, sizeof(int32_t)));
     DMN_CUDA(cudaMemset(d.status, 0, sizeof(int32_t)));
     DMN_CUDA(cudaMalloc((void**)&d.wimage, 4 * 2 * NN_W_BYTES));
-    if (cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sms <= 0) d.sms = 148;
+    DMN_CUDA(cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev));
   }
   *out = &d;
   return 0;
 }
 
-// bit 0: rows are 16-byte aligned (128-bit loads); bit 1: 32-byte aligned (256-bit loads)
-static int vec4_ok(const void* p, int ld) {
-  const int v16 = ((uintptr_t)p % 16 == 0) && (ld % 4 == 0), v32 = ((uintptr_t)p % 32 == 0) && (ld % 8 == 0);
-  return v16 | (v16 && v32 ? 2 : 0);
-}
+// rows are 16-byte aligned (128-bit loads)
+static int vec4_ok(const void* p, int ld) { return ((uintptr_t)p % 16 == 0) && (ld % 4 == 0); }
 
 }  // namespace tg
 
 // Shapes the tensor-core kernels are specialised for (everything else stays on the fp32 CUDA-core kernels of backward.cu).
 bool gemm_nn_tc_supported(int N, int K, int ldc, const float* C, const float* mask) {
-  return (N == 128 || N == 256) && K == 256 && ldc % 4 == 0 && ((uintptr_t)C % 16 == 0) && (!mask || (uintptr_t)mask % 16 == 0);
+  return (N == 128 || N == 256) && K == 256 && ldc % 2 == 0 && ((uintptr_t)C % 8 == 0) && (!mask || (uintptr_t)mask % 8 == 0);
 }
 bool gemm_tn_tc_supported(int N, int K) { return (N == 128 || N == 256) && (K == 256 || (K >= 1 && K <= 64)); }
 
 // w_kmajor == 0: C[M,256] (+)= A[M,N] W[N,256] (mask optional);  w_kmajor != 0: C[M,256] = A[M,N] W[256,N]^T + bias.
 int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C, int ldc, int64_t M, int N, int accumulate,
-                      const float* mask, const float* bias, int w_kmajor, cudaStream_t st) {
+                      const float* mask, const float* bias, int w_kmajor, cudaStream_t st, const uint16_t* mask_bits) {
   using namespace tg;
   if (M <= 0) return 0;
   DevState* ds = nullptr;
@@ -556,16 +417,16 @@ int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C
     DMN_CUDA(cudaFuncSetAttribute(gemm_nn_tc_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NN_SMEM));
   }
   DMN_CHECK(!w_kmajor || N == 256, "gemm_nt(tc): contraction width %d not supported", N);
-  DMN_CHECK(!bias || (uintptr_t)bias % 16 == 0, "gemm(tc): bias must be 16-byte aligned");
+  DMN_CHECK(!bias || (uintptr_t)bias % 8 == 0, "gemm(tc): bias must be 8-byte aligned");
   const int64_t tiles = (M + 127) / 128;
   const unsigned grid = (unsigned)(tiles < ds->sms ? tiles : ds->sms);
   const int va = vec4_ok(A, lda), vw = vec4_ok(W, ldw), nch = N / 64;
   if (w_kmajor) pack_w_kernel<true><<<nch, 512, 0, st>>>(W, ldw, nch, vw, wimage);
   else pack_w_kernel<false><<<nch, 512, 0, st>>>(W, ldw, nch, vw, wimage);
   DMN_LAUNCH_OK();
-  if (w_kmajor) gemm_nn_tc_kernel<4, true><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, mask, bias, va, g_status);
-  else if (N == 128) gemm_nn_tc_kernel<2, false><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, mask, bias, va, g_status);
-  else gemm_nn_tc_kernel<4, false><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, mask, bias, va, g_status);
+  if (w_kmajor) gemm_nn_tc_kernel<4, true><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, mask, mask_bits, bias, va, g_status);
+  else if (N == 128) gemm_nn_tc_kernel<2, false><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, mask, mask_bits, bias, va, g_status);
+  else gemm_nn_tc_kernel<4, false><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, mask, mask_bits, bias, va, g_status);
   DMN_LAUNCH_OK();
   return 0;
 }
@@ -591,34 +452,33 @@ int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, cud
     batch.vec_a[i] = vec4_ok(probs[i].A, probs[i].lda);
     batch.vec_b[i] = vec4_ok(probs[i].B, probs[i].ldb);
   }
-  int slices = ds->sms / n;
+  const int NBT = NB == 256 ? 128 : 64;
+  const int tiles = (N / 128) * (NB / NBT);
+  int slices = ds->sms / (n * tiles);
   if (slices < 1) slices = 1;
   int64_t rows = (M + slices - 1) / slices;
   rows = ((rows + 31) / 32) * 32;
   slices = (int)((M + rows - 1) / rows);
   batch.n = n; batch.slices = slices; batch.rows_per_cta = rows;
-  const unsigned grid = (unsigned)(n * slices);
-  if (!ds->partial || ds->partial_ctas < grid) {      // up to one [256 x 256] fp32 slice per CTA
+  const unsigned grid = (unsigned)(n * tiles * slices);
+  const size_t need = (size_t)n * slices * N * NB;
+  if (!ds->partial || ds->partial_floats < need) {
     if (ds->partial) DMN_CUDA(cudaFree(ds->partial));
     ds->partial = nullptr;
-    ds->partial_ctas = grid > (unsigned)ds->sms ? grid : (unsigned)ds->sms;
-    DMN_CUDA(cudaMalloc((void**)&ds->partial, ds->partial_ctas * 256 * 256 * sizeof(float)));
+    ds->partial_floats = need;
+    DMN_CUDA(cudaMalloc((void**)&ds->partial, need * sizeof(float)));
   }
   float* scratch = ds->partial;
   static PerDeviceOnce attr_once;
-  auto smem_of = [](int na, int nbk) { return (uint32_t)(TN_STAGES * 2 * (na / 64 + nbk / 64) * TN_SLAB + 1024); };
+  auto smem_of = [](int nbt) { return (uint32_t)(2 * 2 * (2 + nbt / 64) * TN_SLAB + 1024); };
   if (attr_once.first()) {
-    DMN_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel<128, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(128, 256)));
-    DMN_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel<256, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(256, 256)));
-    DMN_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel<128, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(128, 64)));
-    DMN_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel<256, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(256, 64)));
+    DMN_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(128)));
+    DMN_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(64)));
   }
-  if (N == 128 && NB == 256) gemm_tn_tc_kernel<128, 256><<<grid, NT, smem_of(128, 256), st>>>(batch, scratch, M, g_status);
-  else if (N == 256 && NB == 256) gemm_tn_tc_kernel<256, 256><<<grid, NT, smem_of(256, 256), st>>>(batch, scratch, M, g_status);
-  else if (N == 128) gemm_tn_tc_kernel<128, 64><<<grid, NT, smem_of(128, 64), st>>>(batch, scratch, M, g_status);
-  else gemm_tn_tc_kernel<256, 64><<<grid, NT, smem_of(256, 64), st>>>(batch, scratch, M, g_status);
+  if (NBT == 128) gemm_tn_tc_kernel<128><<<grid, TN_THREADS, smem_of(128), st>>>(batch, scratch, M, N, NB, g_status);
+  else gemm_tn_tc_kernel<64><<<grid, TN_THREADS, smem_of(64), st>>>(batch, scratch, M, N, NB, g_status);
   DMN_LAUNCH_OK();
-  reduce_partials_kernel<<<dim3((N * NB / 4 + 63) / 64, n), 256, 0, st>>>(scratch, batch, N, NB);
+  reduce_partials_kernel<<<dim3((N * NB / 4 + 255) / 256, n), 256, 0, st>>>(scratch, batch, N, NB);
   DMN_LAUNCH_OK();
   return 0;
 }

@@ -1,7 +1,7 @@
 // fp32 CUDA-core implementation of DM_NeRF.forward (reference networks/dm_nerf.py:80-106), fused with the
 // point generation + positional encoding of render.py:49-58 when called on rays.
 //
-// Role: the exact-fp32 path.  It serves (i) as the on-device cross-check for the tcgen05 kernel,
+// Role: the exact-fp32 path.  It serves (i) as the on-device cross-check for the tensor-core kernel,
 // (ii) shapes the tensor-core kernel does not cover, (iii) DMNERF_IMPL_SIMT.  It keeps every activation
 // on chip: one CTA owns a tile of 64 samples, the 256-wide hidden state lives in shared memory and each
 // layer is computed in place from an 8x8 register tile per thread; weights stream from L2 in 16-deep
@@ -190,7 +190,7 @@ int launch_mlp_simt(const NetParams& p, const float* x, const float* rays_o, con
     DMN_CUDA(cudaFuncSetAttribute(simt::mlp_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)simt::SMEM_BYTES));
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   DMN_CUDA(cudaGetDevice(&dev));
   DMN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int64_t tiles = (m + simt::TM - 1) / simt::TM;

@@ -1,27 +1,22 @@
-// tcgen05 (UMMA) implementation of the DM_NeRF network for one 128-sample tile per CTA (persistent, 1 CTA / SM).
+// Warpgroup-MMA (wgmma) implementation of the DM_NeRF network for one 128-sample tile per CTA (persistent, 1 CTA / SM).
 //
 // Arithmetic: every fp32 operand is split into bf16 hi + bf16 lo (16 significand bits); each algorithmic GEMM is issued
-// as three tensor passes  A_hi*W_hi + A_lo*W_hi + A_hi*W_lo  accumulating in fp32 in tensor memory (relative error
-// ~2^-16 per product, measured ~1e-5 on outputs, inside the 1e-4 parity budget; single-pass bf16/tf32 is not).
+// as three tensor passes  A_hi*W_hi + A_lo*W_hi + A_hi*W_lo  accumulating in fp32 registers (relative error ~2^-16 per
+// product, ~1e-5 on outputs, inside the 1e-4 parity budget; single-pass bf16/tf32 is not).
 //
 // Data flow per tile (nothing 256-wide ever leaves the SM):
-//   * activations: two 128-column "slots" in TENSOR MEMORY, each holding one K-half of the current 256-wide activation as
-//     split bf16 (64 columns of hi halves + 64 of lo halves).  Every trunk MMA takes its A operand from tensor memory
-//     (TS form: no shared-memory read for A); with the two fp32 accumulators the 512 TMEM columns are exactly used.
-//     The position / direction embeddings (4 of the 73 K chunks of a tile) are shared-memory operands (SS form).
-//   * every 256-wide layer is executed as two N=128 half-steps with separate TMEM accumulators, so the epilogue of one
-//     half-step (TMEM -> registers -> bias/ReLU/split -> slot) overlaps the tensor work of the next.  The even half-step of a
-//     layer overwrites slot 0 while the odd one still reads it: the odd half-step reads slot 0 first and releases it
-//     (a_free barrier).  Epilogue results are published per 64-column K chunk.
-//   * weights: packed once per weight update (dmnerf_set_weights) into the exact shared-memory image, streamed in
-//     16 KB stages through a ring with 1-D bulk async copies (TMA engine, mbarrier completion) from L2.
+//   * activations: the current 256-wide activation lives in shared memory as split bf16 (4 K chunks x hi / lo slabs in the
+//     128-byte-swizzled K-major layout the tensor core reads).  Each of the two consumer warpgroups owns 64 rows of the tile;
+//     a 256-wide layer is two N = 128 half-steps accumulated into two register accumulators, and the epilogue (bias, ReLU,
+//     split) overwrites the activation in place once the layer's MMAs have completed.
+//   * the position embedding is a shared-memory slab of its own (layers 0 and 5); after layer 5 the direction embedding
+//     replaces it (colour hidden layer).
+//   * weights: packed once per weight update (dmnerf_set_weights) into the exact shared-memory image, streamed in 16 KB
+//     stages through a ring with 1-D bulk async copies (TMA engine, mbarrier completion) from L2 by one producer warp; both
+//     warpgroups read every stage, and a stage is handed back when the MMAs of both have completed.
 //   * heads: rgb_feature_linear / ins_feature_linear have no activation, so they are folded into the following layer at
-//     pack time (W' = W2 W1, fp64 accumulate); density (N=1) and the 3-wide rgb head are fp32 CUDA-core dot products inside
-//     the epilogues of layer 7 / the colour hidden layer; the instance head is an N=pad16 MMA.  19 half-steps per tile.
-//
-// Warp roles (640 threads): warp 0 weight producer, warp 1 MMA issuer (converged warp, one elected lane), warp 2 TMEM
-// allocator, warps 4-19 prologue (points + positional encoding, sliced into the idle time of the previous tile's
-// epilogues) and epilogue: 4 TMEM lane quadrants x 4 column groups, i.e. one row and 32 accumulator columns per thread.
+//     pack time (W' = W2 W1, fp64 accumulate); density (N=1) and the 3-wide rgb head are fp32 CUDA-core dot products in the
+//     epilogues of layer 7 / the colour hidden layer; the instance head is one more MMA.  19 half-steps per tile.
 // All waits are bounded: a protocol bug raises an error code, never a hang.
 //
 #include <cstring>
@@ -36,32 +31,16 @@ namespace dmnerf {
 namespace uk {
 
 using namespace umma;
-enum ChunkKind : int8_t { CK_E = 6, CK_D = 7 };              // 0..3 = slot*2 + chunk
-
-#ifdef DMN_DEBUG_STALL
-}  // namespace uk
-}  // namespace dmnerf
-extern "C" __attribute__((visibility("default"))) int dmnerf_debug_stall(int* out) {
-  cudaDeviceSynchronize();
-  return (int)cudaMemcpyFromSymbol(out, dmnerf::uk::g_stall_dbg, sizeof(int) * 641);
-}
-namespace dmnerf {
-namespace uk {
-#endif
-
-#ifdef DMN_KPROF
-__device__ long long g_kprof[160][16];
-__device__ long long g_ktrace[4][64];     // CTA 0, tile KTRACE_TILE: [mma step ready | mma step issued | epi acc_full seen | epi arrived][step]
-#endif
+enum ChunkKind : int8_t { CK_E = 6, CK_D = 7 };              // 0..3 = activation K chunk
 
 struct Step {
   int8_t n_chunks;
-  int8_t chunk[MAX_CHUNKS];   // ChunkKind or slot*2+j
+  int8_t chunk[MAX_CHUNKS];   // ChunkKind or activation chunk
   int8_t dep[MAX_CHUNKS];     // tile-relative step whose epilogue produces the chunk; -1 = tile inputs
   int8_t ksteps[MAX_CHUNKS];  // K/16 MMAs for this chunk (4, or 2 for the direction embedding)
-  int8_t out_slot;            // destination slot, or -1 = write network outputs
+  int8_t out_slot;            // destination half of the activation, or -1 = network outputs
   int8_t relu;
-  int16_t n;                  // MMA N (multiple of 16, <= 128)
+  int16_t n;                  // rows of the packed weight stage (multiple of 16, <= 128)
 };
 
 struct Program {
@@ -75,7 +54,7 @@ struct Program {
 constexpr int FS = 64, FI = 128, FF = FS + FI;        // the fused path is specialised for 64 + 128 samples
 constexpr int ACC_W = 5 + DMNERF_MAX_INS + 1 + 3;      // rgb3, depth, acc, ins_num+1 (padded)
 struct Fused {
-  float ray[2][2][8];         // [pair parity][ray]: o(3), d(3), |d|, valid (the next pair is loaded while this one finishes)
+  float ray[2][8];            // per ray: o(3), d(3), |d|, valid
   float zc[2][FS];            // coarse depths (after jitter)
   float zf[2][FF];            // fine depths (sorted union)
   float w[TILE_M];            // compositing weights of the current tile's rows
@@ -86,7 +65,6 @@ struct Fused {
   float bins[2][FS], cdf[2][FS], vals[2][FF];
 };
 static_assert(sizeof(Fused) <= 12288, "Fused state does not fit its shared-memory block");
-
 
 struct KArgs {
   const uint8_t* image;        // packed bf16 operand image (fused: coarse network)
@@ -110,8 +88,7 @@ struct KArgs {
 // ------------------------------------------------------------------------------------------------ prologue helpers
 // sin and cos of one argument with |a| < ~1e5: three-constant Cody-Waite reduction by pi/2 + the single-precision minimax
 // polynomials on [-pi/4, pi/4] (the textbook algorithm behind the library's own fast path, <= 2 ulp), written without the
-// large-argument branch so that the compiler can interleave the independent evaluations of a row (the prologue is a long
-// chain of these; with the library call's branch in between they serialise at ~550 cycles each).
+// large-argument branch so that the compiler can interleave the independent evaluations of a row.
 __device__ __forceinline__ void sincos_cw(float a, float& sn, float& cs) {
   const float t = fmaf(a, 0.636619772f, 12582912.0f);          // 1.5 * 2^23: the integer n = rint(a * 2/pi) lands in the mantissa
   const int n = __float_as_int(t);
@@ -163,13 +140,14 @@ __device__ __forceinline__ void fill_embedding(const float v[3], float* vals /* 
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
+// Warps 0-7: two consumer warpgroups (MMA issue, epilogues, prologue); warp 8: weight producer.
 template <bool FUSED>
 __global__ void __launch_bounds__(N_THREADS, 1) mlp_umma_kernel(const __grid_constant__ Program prog, const KArgs a) {
   // The kernel has no static shared memory, so the dynamic block starts at offset 0 of the CTA's shared window and
-  // is 1024-aligned by construction (checked below); addresses derived from it stay compile-time / uniform.
+  // is 1024-aligned by construction (checked below).
   extern __shared__ __align__(1024) uint8_t smem[];
   Misc* misc = reinterpret_cast<Misc*>(smem + SM_MISC);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // RAW: work item = one 128-row tile of a.m samples.  FUSED: work item = ray pair = 4 tiles (1 coarse + 3 fine).
   const int64_t n_items = FUSED ? (a.n_rays + 1) / 2 : (a.m + TILE_M - 1) / TILE_M;
   const int64_t my_items = (n_items > blockIdx.x) ? (n_items - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
@@ -178,29 +156,16 @@ __global__ void __launch_bounds__(N_THREADS, 1) mlp_umma_kernel(const __grid_con
   const int C = 4 + prog.ins_num + 1;
 
   if (tid == 0) {
-    for (int i = 0; i < NS; ++i) { mbar_init(&misc->full[i], 1); mbar_init(&misc->empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&misc->acc_full[i], 1);
-      mbar_init(&misc->epi_done[i][0], CHUNK_THREADS);
-      mbar_init(&misc->epi_done[i][1], CHUNK_THREADS);
-    }
-    mbar_init(&misc->inputs_ready, EPI_THREADS);
-    mbar_init(&misc->a_free, 1);
+    for (int i = 0; i < NS; ++i) { mbar_init(&misc->full[i], 1); mbar_init(&misc->empty[i], 8); }
     misc->abort_flag = 0;
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(&misc->tmem_base, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  // This CTA owns the whole tensor memory of its SM (512 columns, 1 CTA/SM), so the allocation starts at column 0.
-  // Treating the base as the constant 0 keeps every TMEM address in uniform registers / immediates.
-  constexpr uint32_t tbase = 0;
-  if (misc->tmem_base != 0 || (smem_u32(smem) & 1023u) != 0) {
+  if ((smem_u32(smem) & 1023u) != 0) {
     if (tid == 0) { atomicExch(&misc->abort_flag, 901); atomicCAS(a.status, 0, 901); }
   }
 
-  if (warp == 0) {
+  if (warp == 8) {
     // =========================================================== weight producer (converged warp, one elected lane issues)
     Ring ring{0, 0};
     const int n_stages = prog.n_stages;
@@ -208,268 +173,151 @@ __global__ void __launch_bounds__(N_THREADS, 1) mlp_umma_kernel(const __grid_con
       const uint8_t* image = (FUSED && (ti & 3) != 0) ? a.image_fine : a.image;
       for (int si = 0; si < n_stages; ++si) {
         const uint32_t off = prog.stage_off[si], bytes = prog.stage_off[si + 1] - off;
-        DBG_SITE(20000 + si);
         wait_bar(&misc->empty[ring.slot], ring.phase ^ 1, misc, 101, a.status);
         if (elect_one()) {
-#ifdef DMN_EXP_NOWEIGHTS     /* timing experiment only: no weight traffic (results are garbage) */
-          (void)image; (void)off; (void)bytes;
-          mbar_arrive(&misc->full[ring.slot]);
-#else
           mbar_arrive_expect_tx(&misc->full[ring.slot], bytes);
           bulk_g2s(smem + SM_RING + ring.slot * STAGE_BYTES, image + off, bytes, &misc->full[ring.slot]);
-#endif
         }
         __syncwarp();
         ring.advance();
       }
     }
-  } else if (warp == 1) {
-    // =========================================================== MMA issuer (converged warp, one elected lane issues)
-    // The per-tile schedule is written out structurally (it mirrors build_program(), which drives the producer, the
-    // epilogue and the weight packing): 8 trunk layers x 2 half-steps, two folded hidden heads, two output heads.
-#ifdef DMN_KPROF
-    int64_t kt_tile = 0; int kt_step = 0; long long kt_ww = 0, kt_we = 0;
-#endif
-    long long kp[16] = {0};
-    (void)kp;
-    const long long kp_role0 = clock64();
-    (void)kp_role0;
-    Ring ring{0, 0};
-    uint32_t seen00 = 0, seen01 = 0, seen10 = 0, seen11 = 0, seen_in = 0;
-    const uint32_t ring_base = smem_u32(smem + SM_RING);
-    const uint64_t e_hi = make_sdesc_sw128(smem_u32(smem + SM_E_HI)), e_lo = make_sdesc_sw128(smem_u32(smem + SM_E_LO));
-    const uint64_t d_hi = make_sdesc_sw128(smem_u32(smem + SM_D_HI)), d_lo = make_sdesc_sw128(smem_u32(smem + SM_D_LO));
-    const uint32_t idesc128 = make_idesc_bf16(128, 128), idesc16 = make_idesc_bf16(128, 16);
-    const uint32_t idesc_ins = make_idesc_bf16(128, prog.step[N_STEPS - 1].n);
-    // The epilogue of global step gd has finished 64-column chunk c: that K chunk of its output slot is readable and
-    // that part of its accumulator is drained.  (Chunk granularity lets the next layer's MMAs on chunk 0 overlap the
-    // epilogue of chunk 1.)
-    auto need_epi = [&](uint32_t gd, int c) {
-      uint32_t& sn = (gd & 1) ? (c ? seen11 : seen10) : (c ? seen01 : seen00);
-      const uint32_t need = gd / 2 + 1;
-      while (sn < need) {
-        DBG_SITE(10000 + (int)(gd % 1000) * 4 + c);
-        wait_bar(&misc->epi_done[gd & 1][c], sn & 1, misc, 201, a.status);
-        ++sn;
-      }
-      tc_fence_after();
-    };
-    auto need_drained = [&](uint32_t gd) { need_epi(gd, 0); need_epi(gd, 1); };
-    // K chunk j of activation slot `slot` (both bf16 halves in tensor memory)
-    auto slot_chunk = [&](int slot, int j, uint32_t d_tmem, uint32_t idesc, uint32_t& accum) {
-      const uint32_t hi = tbase + TC_SLOT + slot * SLOT_COLS + j * 32;
-      issue_chunk<4, false>(misc, ring, ring_base, hi, hi + SLOT_LO, d_tmem, idesc, accum, a.status, kp);
-    };
-    auto finish = [&](uint32_t acc) {
-      if (elect_one()) mma_commit(&misc->acc_full[acc]);
-      __syncwarp();
-#ifdef DMN_KPROF
-      if (blockIdx.x == 0 && kt_tile >= KTRACE_TILE && kt_tile < KTRACE_TILE + 2 && (tid & 31) == 0) {
-        g_ktrace[1][(kt_tile - KTRACE_TILE) * 20 + kt_step] = clock64();
-        const long long ww = kp[4] + kp[5], we = kp[0] + kp[1] + kp[2] + kp[3] + kp[7];
-        g_ktrace[0][(kt_tile - KTRACE_TILE) * 20 + kt_step] = ((ww - kt_ww) << 32) | (we - kt_we);
-        kt_ww = ww; kt_we = we;
-      } else if ((tid & 31) == 0) { kt_ww = kp[4] + kp[5]; kt_we = kp[0] + kp[1] + kp[2] + kp[3] + kp[7]; }
-      ++kt_step;
-#endif
-    };
-    // Slot 0 has been read by everything issued so far: the epilogue of the preceding even half-step may overwrite it.
-    auto release_slot0 = [&]() {
-      if (elect_one()) mma_commit(&misc->a_free);
-      __syncwarp();
-    };
-    // Slot 0 always holds K-half 0 of the current activation (written by the even half-step of the previous layer),
-    // slot 1 K-half 1 (odd half-step).  The even epilogue of a layer runs while the odd half-step's MMAs are in flight,
-    // so the odd half-step reads slot 0 first and releases it (a_free) before it turns to slot 1.
-    // Accumulators alternate with the GLOBAL half-step counter g (a tile has an odd number of half-steps).
-    for (int64_t ti = 0; ti < my_tiles; ++ti) {
-      const uint32_t g0 = (uint32_t)ti * N_STEPS;
-#ifdef DMN_KPROF
-      kt_tile = ti; kt_step = 0;
-#endif
-      // ---- layer 0: E -> slots 0, 1
-      for (uint32_t h = 0; h < 2; ++h) {
-        const uint32_t g = g0 + h, acc = g & 1;
-        if (g >= 2) { KP_T0(); need_drained(g - 2); KP_ADD(0); }
-        {
-          KP_T0();
-          while (seen_in < (uint32_t)ti + 1) {
-            wait_bar(&misc->inputs_ready, seen_in & 1, misc, 202, a.status);
-            ++seen_in;
-          }
-          KP_ADD(3);
-        }
-        tc_fence_after();
-        uint32_t accum = 0;
-        issue_chunk<4, true>(misc, ring, ring_base, e_hi, e_lo, tbase + TC_ACC + acc * 128, idesc128, accum, a.status, kp);
-        finish(acc);
-      }
-      // ---- layers 1..7
-      for (int l = 1; l < 8; ++l) {
-        for (uint32_t h = 0; h < 2; ++h) {
-          const uint32_t g = g0 + 2 * l + h, acc = g & 1, d_tmem = tbase + TC_ACC + acc * 128;
-          { KP_T0(); need_drained(g - 2); KP_ADD(0); }   // accumulator free (and, for h == 0, K-half 0 of the input complete)
-          uint32_t accum = 0;
-          slot_chunk(0, 0, d_tmem, idesc128, accum); slot_chunk(0, 1, d_tmem, idesc128, accum);
-          if (h == 1) release_slot0();
-#ifndef DMN_EXP_NO_NEEDEPI    /* timing experiment only (results are garbage): slot 1 is read without waiting for its epilogue */
-          if (h == 0) { KP_T0(); need_epi(g - 1, 0); KP_ADD(1); }
-#endif
-          slot_chunk(1, 0, d_tmem, idesc128, accum);
-#ifndef DMN_EXP_NO_NEEDEPI
-          if (h == 0) { KP_T0(); need_epi(g - 1, 1); KP_ADD(2); }
-#endif
-          slot_chunk(1, 1, d_tmem, idesc128, accum);
-          if (l == 5) issue_chunk<4, true>(misc, ring, ring_base, e_hi, e_lo, d_tmem, idesc128, accum, a.status, kp);
-          finish(acc);
-        }
-      }
-      {
-        // ---- folded instance hidden layer (half-step 16): h -> slot 0 (an even half-step like those of the trunk)
-        uint32_t g = g0 + T_INS_HID, acc = g & 1, d_tmem = tbase + TC_ACC + acc * 128, accum = 0;
-        { KP_T0(); need_drained(g - 2); KP_ADD(7); }
-        slot_chunk(0, 0, d_tmem, idesc128, accum); slot_chunk(0, 1, d_tmem, idesc128, accum);
-        { KP_T0(); need_epi(g - 1, 0); KP_ADD(7); }
-        slot_chunk(1, 0, d_tmem, idesc128, accum);
-        { KP_T0(); need_epi(g - 1, 1); KP_ADD(7); }
-        slot_chunk(1, 1, d_tmem, idesc128, accum);
-        finish(acc);
-        // ---- folded colour hidden layer (half-step 17): [h | dir]; its epilogue evaluates the 3-wide rgb head and the
-        //      density on CUDA cores, so nothing is written back to a slot.  Its MMAs hide the epilogue of half-step 16.
-        g = g0 + T_RGB_HID; acc = g & 1; d_tmem = tbase + TC_ACC + acc * 128; accum = 0;
-        { KP_T0(); need_drained(g - 2); KP_ADD(7); }
-        slot_chunk(0, 0, d_tmem, idesc128, accum); slot_chunk(0, 1, d_tmem, idesc128, accum);
-        release_slot0();
-        slot_chunk(1, 0, d_tmem, idesc128, accum); slot_chunk(1, 1, d_tmem, idesc128, accum);
-        issue_chunk<2, true>(misc, ring, ring_base, d_hi, d_lo, d_tmem, idesc128, accum, a.status, kp);
-        finish(acc);
-        // ---- instance head (half-step 18, N = pad16(ins_num+1)) on the instance hidden activation (slot 0)
-        g = g0 + T_INS_OUT; acc = g & 1; d_tmem = tbase + TC_ACC + acc * 128; accum = 0;
-        { KP_T0(); need_drained(g - 2); KP_ADD(7); }    // slot 0 complete, accumulator of half-step 16 drained
-        slot_chunk(0, 0, d_tmem, idesc_ins, accum); slot_chunk(0, 1, d_tmem, idesc_ins, accum);
-        finish(acc);
+    return;
+  }
+
+  // =========================================================== consumer warpgroups
+  const int g = tid >> 7;                       // warpgroup: tile rows [64 g, 64 g + 64)
+  const int wl = warp & 3;
+  const int ra = 64 * g + 16 * wl + (lane >> 2);  // tile rows of this thread's accumulator fragment: ra, ra + 8
+  const int q4 = lane & 3;                      // fragment columns 8 j + 2 q4 (+ 1)
+  const int pr = 64 * g + (tid & 63);           // prologue: tile row of this thread
+  const int ph = (tid >> 6) & 1;                // prologue: which half of the row's embedding columns
+  const int bar_wg = 1 + g;                     // named barrier of this warpgroup
+  uint8_t *e_hi = smem + SM_E_HI, *e_lo = smem + SM_E_LO;
+  const uint32_t ring_base = smem_u32(smem + SM_RING);
+  const uint32_t act_base = smem_u32(smem + SM_ACT) + 8192u * g;     // this warpgroup's 64 rows inside every slab
+  const uint32_t e_base = smem_u32(e_hi) + 8192u * g;
+  Ring ring{0, 0};
+  int prev_slot = -1;
+  float acc0[64], acc1[64];
+
+  // One weight stage: wait for it, issue its MMAs (A_hi * W and, for a W_hi stage, A_lo * W), hand the previous stage back
+  // once its MMAs have completed (the ring holds the stage in flight, the stage issued before it and the one being filled).
+  auto stage = [&](float (&acc)[64], uint32_t a_hi, uint32_t a_lo, bool with_lo, int ks, uint32_t scale0) {
+    const uint32_t s = ring.slot;
+    wait_bar(&misc->full[s], ring.phase, misc, 204, a.status);
+    const uint32_t w = ring_base + s * STAGE_BYTES;
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (k < ks) {
+        wgmma_n128<0, 0>(acc, make_sdesc_sw128(a_hi + 32 * k), make_sdesc_sw128(w + 32 * k), k == 0 ? scale0 : 1u);
+        if (with_lo) wgmma_n128<0, 0>(acc, make_sdesc_sw128(a_lo + 32 * k), make_sdesc_sw128(w + 32 * k), 1u);
       }
     }
-#ifdef DMN_KPROF
-    kp[6] = clock64() - kp_role0;
-    if ((tid & 31) == 0) for (int i = 0; i < 8; ++i) g_kprof[blockIdx.x][i] = kp[i];
-#endif
-  } else if (warp >= 4) {
-    // =========================================================== prologue + epilogue warps
-    // 16 warps = 4 TMEM lane quadrants (warp % 4: rows) x 4 column groups (cg): in a hidden half-step every thread owns
-    // one row and 32 of the 128 output columns; the two column groups of a 64-column K chunk publish it together.
-    const int et = tid - 128;                 // 0..511
-    const int cg = et >> 7;                   // column group
-    const int r = et & 127;                   // tile row == TMEM lane
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
-    uint8_t *e_hi_slab = smem + SM_E_HI, *e_lo_slab = smem + SM_E_LO, *d_hi_slab = smem + SM_D_HI, *d_lo_slab = smem + SM_D_LO;
-    float dens_acc = 0.0f;
-    const int n_ins1 = prog.ins_num + 1;
-    long long kp[16] = {0};
-    (void)kp;
-    const long long kp_role0 = clock64();
-    (void)kp_role0;
-    // Operands (points, embeddings) of tile `tp`, split bf16 hi / lo into the shared-memory slabs, then inputs_ready.
-    // The work comes in parts so that it can be spread over the idle time of several epilogues of the PREVIOUS tile:
-    //   PRO_E0 / PRO_E1: position-embedding columns [16 cg, 16 cg + 8) / [16 cg + 8, 16 cg + 16) of this thread's row
-    //                    (the E slabs are free once half-step 11, the skip layer, has completed)
-    //   PRO_D:           direction embedding, 16 columns each by column groups 2 and 3 (free after half-step 16)
-    //   PRO_DONE:        make the slabs visible to the tensor core and arrive on inputs_ready
-    // Only the first tile of a CTA and the first fine tile of a ray pair (whose depths come out of the coarse tile's
-    // importance sampling) are prepared in one piece (PRO_ALL) at the tile boundary.
-    constexpr int PRO_E0 = 1, PRO_E1 = 2, PRO_D = 4, PRO_DONE = 8, PRO_ALL = 15;
-    auto prologue = [&](int64_t tp, const int parts) {
-      const int jp = FUSED ? (int)(tp & 3) : 0;
-      const int64_t itemp = blockIdx.x + (FUSED ? (tp >> 2) : tp) * gridDim.x;
-      const int up = FUSED ? (int)((tp >> 2) & 1) : 0;                   // ray-data buffer of that ray pair
-      int64_t rowp = 0;
-      int rlp = 0, sip = 0;
-      bool validp;
+    wg_commit();
+    wg_wait<1>();
+    if (prev_slot >= 0 && lane == 0) mbar_arrive(&misc->empty[prev_slot]);
+    prev_slot = (int)s;
+    ring.advance();
+  };
+  auto drain = [&]() {
+    wg_wait<0>();
+    wg_reg_fence(acc0);
+    wg_reg_fence(acc1);
+    if (prev_slot >= 0 && lane == 0) mbar_arrive(&misc->empty[prev_slot]);
+    prev_slot = -1;
+  };
+  // One 64-wide K chunk (W_hi stage, then W_lo stage) of a half-step
+  auto chunk = [&](float (&acc)[64], uint32_t a_hi, uint32_t a_lo, int ks, bool first) {
+    stage(acc, a_hi, a_lo, true, ks, first ? 0u : 1u);
+    stage(acc, a_hi, a_lo, false, ks, 1u);
+  };
+  auto act_chunk = [&](float (&acc)[64], int c, bool first) {
+    const uint32_t hi = act_base + c * ACT_CHUNK;
+    chunk(acc, hi, hi + CHUNK_BYTES, 4, first);
+  };
+  auto all_act = [&](float (&acc)[64]) { for (int c = 0; c < 4; ++c) act_chunk(acc, c, c == 0); };
+  auto e_chunk = [&](float (&acc)[64], int ks, bool first) { chunk(acc, e_base, e_base + CHUNK_BYTES, ks, first); };
+  auto wg_sync = [&]() { named_bar_sync_id(bar_wg, 128); };
+  auto all_sync = [&]() { named_bar_sync<3, CONSUMERS>(); };
+
+  for (int64_t ti = 0; ti < my_tiles; ++ti) {
+    const int j = FUSED ? (int)(ti & 3) : 0;                            // fused: 0 = coarse tile, 1..3 = fine tiles
+    const int64_t item = blockIdx.x + (FUSED ? (ti >> 2) : ti) * gridDim.x;
+    const float* bias_base = (FUSED && j != 0) ? a.bias_fine : a.bias;
+    // ---------------- rows of this tile: which sample a tile row is
+    auto row_of = [&](int r, int& rl, int& si, int64_t& row, bool& valid) {
       if constexpr (FUSED) {
-        if (jp == 0) {
-          if (parts & PRO_E0) {                                           // first part: fetch the pair's rays
-            if (et < 2) {
-              const int64_t ray = itemp * 2 + et;
-              const bool ok = ray < a.n_rays;
-              float* rs = fz->ray[up][et];
-              for (int c = 0; c < 3; ++c) { rs[c] = ok ? a.rays_o[ray * 3 + c] : 0.0f; rs[3 + c] = ok ? a.rays_d[ray * 3 + c] : 0.0f; }
-              rs[6] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(rs[3], rs[3]), __fmul_rn(rs[4], rs[4])), __fmul_rn(rs[5], rs[5])));
-              rs[7] = ok ? 1.0f : 0.0f;
-            }
-            named_bar_sync<3, 512>();
-          }
-          rlp = r >> 6; sip = r & 63;
-        } else {
-          const int gr = (jp - 1) * TILE_M + r;
-          rlp = gr / FF; sip = gr % FF;
-        }
-        validp = fz->ray[up][rlp][7] != 0.0f;
+        if (j == 0) { rl = r >> 6; si = r & 63; }
+        else { const int gr = (j - 1) * TILE_M + r; rl = gr / FF; si = gr % FF; }
+        row = 0;
+        valid = fz->ray[rl][7] != 0.0f;
       } else {
-        rowp = itemp * TILE_M + r;
-        validp = rowp < a.m;
+        rl = 0; si = 0;
+        row = item * TILE_M + r;
+        valid = row < a.m;
       }
-      const bool do_d = (parts & PRO_D) && cg >= 2;
-      const int d_col0 = (cg == 2) ? 0 : 16;
-      float vals[16];
-      auto save_emb = [&](int col0, auto cntc) {          // training forward: keep the embedded inputs (ActPlanes.emb)
-        constexpr int CNT = decltype(cntc)::value;
-        if constexpr (!FUSED) {
-          if (a.acts && validp) {
-            float* dst = act_planes(a.acts, a.m).emb + (int64_t)col0 * a.m + rowp;      // column-major [90][M]: coalesced per column
-#pragma unroll
-            for (int i = 0; i < CNT; ++i)
-              if (col0 + i < CH_IN && (col0 >= CH_POS || col0 + i < CH_POS)) dst[(int64_t)i * a.m] = vals[i];
-          }
+    };
+    // ---------------- prologue: points + position embedding of row pr, columns [32 ph, 32 ph + 32)
+    if (FUSED && j == 0) {
+      if (tid < 2) {
+        const int64_t ray = item * 2 + tid;
+        const bool ok = ray < a.n_rays;
+        float* rs = fz->ray[tid];
+        for (int c = 0; c < 3; ++c) { rs[c] = ok ? a.rays_o[ray * 3 + c] : 0.0f; rs[3 + c] = ok ? a.rays_d[ray * 3 + c] : 0.0f; }
+        rs[6] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(rs[3], rs[3]), __fmul_rn(rs[4], rs[4])), __fmul_rn(rs[5], rs[5])));
+        rs[7] = ok ? 1.0f : 0.0f;
+      }
+      all_sync();
+    }
+    int p_rl, p_si;
+    int64_t p_row;
+    bool p_valid;
+    row_of(pr, p_rl, p_si, p_row, p_valid);
+    float pt[3] = {0.f, 0.f, 0.f}, vd[3] = {0.f, 0.f, 0.f};
+    auto save_emb = [&](int col0, const float* vals, int cnt) {          // training forward: keep the embedded inputs
+      if constexpr (!FUSED) {
+        if (a.acts && p_valid) {
+          float* dst = act_planes(a.acts, a.m).emb + (int64_t)col0 * a.m + p_row;      // column-major [90][M]
+          for (int i = 0; i < cnt; ++i)
+            if (col0 + i < CH_IN && (col0 >= CH_POS || col0 + i < CH_POS)) dst[(int64_t)i * a.m] = vals[i];
         }
-      };
-      using c8 = std::integral_constant<int, 8>;
-      using c16 = std::integral_constant<int, 16>;
+      }
+    };
+    {
+      float vals[32];
       if (!FUSED && a.x) {
-        // pre-embedded input rows [M, 90]
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          if (!(parts & (half ? PRO_E1 : PRO_E0))) continue;
-          const int e0 = 16 * cg + 8 * half;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) vals[i] = (validp && e0 + i < CH_POS) ? a.x[rowp * CH_IN + e0 + i] : 0.0f;
-          save_emb(e0, c8{});
-          store_split8_smem(vals, e_hi_slab, e_lo_slab, r, e0);
-        }
-        if (do_d) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) vals[i] = (validp && d_col0 + i < CH_DIR) ? a.x[rowp * CH_IN + CH_POS + d_col0 + i] : 0.0f;
-          save_emb(CH_POS + d_col0, c16{});
-          store_split16_smem(vals, d_hi_slab, d_lo_slab, r, d_col0);
-        }
-      } else if ((parts & (PRO_E0 | PRO_E1)) || do_d) {
-        float pt[3] = {0.f, 0.f, 0.f}, vd[3] = {0.f, 0.f, 0.f};
-        if (validp) {
+        for (int i = 0; i < 32; ++i) vals[i] = (p_valid && 32 * ph + i < CH_POS) ? a.x[p_row * CH_IN + 32 * ph + i] : 0.0f;
+      } else {
+        if (p_valid) {
           float o0, o1, o2, d0, d1, d2, nrm, zz;
           if constexpr (FUSED) {
-            const float* rs = fz->ray[up][rlp];
+            const float* rs = fz->ray[p_rl];
             o0 = rs[0]; o1 = rs[1]; o2 = rs[2]; d0 = rs[3]; d1 = rs[4]; d2 = rs[5]; nrm = rs[6];
-            if (jp == 0) {
+            if (j == 0) {
               // render.py:40-47: shared / per-ray coarse row, jittered inside its stratum when t_rand is given
-              const int64_t ray = itemp * 2 + rlp;
+              const int64_t ray = item * 2 + p_rl;
               const float* zr = a.z_in + ray * a.z_stride;
-              zz = zr[sip];
+              zz = zr[p_si];
               if (a.t_rand) {
-                const float lower = (sip == 0) ? zz : __fmul_rn(0.5f, __fadd_rn(zz, zr[sip - 1]));
-                const float upper = (sip == FS - 1) ? zz : __fmul_rn(0.5f, __fadd_rn(zr[sip + 1], zz));
-                zz = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), a.t_rand[ray * FS + sip]));
+                const float lower = (p_si == 0) ? zz : __fmul_rn(0.5f, __fadd_rn(zz, zr[p_si - 1]));
+                const float upper = (p_si == FS - 1) ? zz : __fmul_rn(0.5f, __fadd_rn(zr[p_si + 1], zz));
+                zz = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), a.t_rand[ray * FS + p_si]));
               }
-              if (cg == 0 && (parts & PRO_E0)) {
-                fz->zc[rlp][sip] = zz;
-                if (a.zc_out) a.zc_out[ray * FS + sip] = zz;
+              if (ph == 0) {
+                fz->zc[p_rl][p_si] = zz;
+                if (a.zc_out) a.zc_out[ray * FS + p_si] = zz;
               }
             } else {
-              zz = fz->zf[rlp][sip];
+              zz = fz->zf[p_rl][p_si];
             }
           } else {
             // rays mode: sample s of ray r at depth z.  Points mode (z == NULL, s == 1): rays_o holds the query points and
             // rays_d the view directions exactly as they go into the embedding (mesh_generator.py:40-44 passes zeros).
-            const int64_t ray = rowp / a.s;
-            zz = a.z ? a.z[rowp] : 0.0f;
+            const int64_t ray = p_row / a.s;
+            zz = a.z ? a.z[p_row] : 0.0f;
             o0 = a.rays_o[ray * 3]; o1 = a.rays_o[ray * 3 + 1]; o2 = a.rays_o[ray * 3 + 2];
             d0 = a.rays_d[ray * 3]; d1 = a.rays_d[ray * 3 + 1]; d2 = a.rays_d[ray * 3 + 2];
             nrm = a.z ? sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2))) : 1.0f;
@@ -481,463 +329,309 @@ __global__ void __launch_bounds__(N_THREADS, 1) mlp_umma_kernel(const __grid_con
           } else {
             pt[0] = o0; pt[1] = o1; pt[2] = o2;
           }
-          if (do_d) { vd[0] = __fdiv_rn(d0, nrm); vd[1] = __fdiv_rn(d1, nrm); vd[2] = __fdiv_rn(d2, nrm); }   // render.py:37
+          vd[0] = __fdiv_rn(d0, nrm); vd[1] = __fdiv_rn(d1, nrm); vd[2] = __fdiv_rn(d2, nrm);      // render.py:37
         }
         // |2^9 x| small enough for the branch-free sin/cos in every lane?  (warp-uniform choice; scenes are a few units wide)
         const float amax = fmaxf(fmaxf(fabsf(pt[0]), fabsf(pt[1])), fabsf(pt[2]));
-        const bool fast = __all_sync(FULL, amax < 64.0f);
-        auto embed_pos8 = [&](auto fastc, auto halfc) {
-          constexpr bool F = decltype(fastc)::value;
-          constexpr int H = decltype(halfc)::value;
-          if (cg == 0) fill_embedding<0 + 8 * H, 8, L_POS, F>(pt, vals);
-          else if (cg == 1) fill_embedding<16 + 8 * H, 8, L_POS, F>(pt, vals);
-          else if (cg == 2) fill_embedding<32 + 8 * H, 8, L_POS, F>(pt, vals);
-          else fill_embedding<48 + 8 * H, 8, L_POS, F>(pt, vals);           // entries 48..62, entry 63 is the zero pad
-          if (!validp) {
+        const bool fast = __all_sync(0xffffffffu, amax < 64.0f);
+        if (ph == 0) { if (fast) fill_embedding<0, 32, L_POS, true>(pt, vals); else fill_embedding<0, 32, L_POS, false>(pt, vals); }
+        else { if (fast) fill_embedding<32, 32, L_POS, true>(pt, vals); else fill_embedding<32, 32, L_POS, false>(pt, vals); }
+        if (!p_valid) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) vals[i] = 0.0f;
+          for (int i = 0; i < 32; ++i) vals[i] = 0.0f;
+        }
+      }
+      save_emb(32 * ph, vals, 32);
+#pragma unroll
+      for (int u = 0; u < 4; ++u) store_split8_smem(vals + 8 * u, e_hi, e_lo, pr, 32 * ph + 8 * u);
+    }
+    fence_proxy_async_smem();            // the embeddings are read by the tensor core through the async proxy
+    wg_sync();
+
+    // ---------------- epilogue helpers
+    const float* bias_t = bias_base;
+    const ActPlanes ap = act_planes(a.acts, a.m);
+    int64_t row_ab[2];
+    bool valid_ab[2];
+    {
+      int rl_, si_;
+      row_of(ra, rl_, si_, row_ab[0], valid_ab[0]);
+      row_of(ra + 8, rl_, si_, row_ab[1], valid_ab[1]);
+    }
+    // bias + ReLU of one 128-column half-step accumulator; store as split bf16 into activation half `half` (or nowhere)
+    auto hidden = [&](float (&acc)[64], int t, int half, int plane, int width, int col_off) {
+      const float* bias = bias_t + t * 128;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        const int col = 8 * jj + 2 * q4;
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          acc[4 * jj + 2 * h] = fmaxf(acc[4 * jj + 2 * h] + bb.x, 0.0f);
+          acc[4 * jj + 2 * h + 1] = fmaxf(acc[4 * jj + 2 * h + 1] + bb.y, 0.0f);
+          if (half >= 0) {
+            uint32_t hi, lo;
+            split_bf16x2(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1], hi, lo);
+            const int c256 = 128 * half + col;
+            const uint32_t o = SM_ACT + (c256 >> 6) * ACT_CHUNK + sw128_offset(ra + 8 * h, c256 & 63);
+            *reinterpret_cast<uint32_t*>(smem + o) = hi;
+            *reinterpret_cast<uint32_t*>(smem + o + CHUNK_BYTES) = lo;
           }
-          save_emb(16 * cg + 8 * H, c8{});
-          store_split8_smem(vals, e_hi_slab, e_lo_slab, r, 16 * cg + 8 * H);
-        };
-        using h0 = std::integral_constant<int, 0>;
-        using h1 = std::integral_constant<int, 1>;
-        if (parts & PRO_E0) { if (fast) embed_pos8(std::true_type{}, h0{}); else embed_pos8(std::false_type{}, h0{}); }
-        if (parts & PRO_E1) { if (fast) embed_pos8(std::true_type{}, h1{}); else embed_pos8(std::false_type{}, h1{}); }
-        if (do_d) {                                      // |vd| <= 1: always the branch-free path; 27 valid entries, rest 0
-          if (cg == 2) fill_embedding<0, 16, L_DIR, true>(vd, vals);
-          else fill_embedding<16, 16, L_DIR, true>(vd, vals);
-          if (!validp) {
+        }
+      }
+      if constexpr (!FUSED) {
+        if (a.acts) {                            // training forward: keep the post-activation values and their ReLU masks
+          float* base = (plane < 8) ? ap.h[plane] : (plane == 8 ? ap.rgb_hid : ap.ins_hid);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (!valid_ab[h]) continue;
+            float* dst = base + row_ab[h] * width + col_off + 2 * q4;
+#pragma unroll
+            for (int jj = 0; jj < 16; ++jj)
+              *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1]);
+          }
+#pragma unroll
+          for (int grp = 0; grp < 8; ++grp) {      // 16 units = n8 blocks 2 grp, 2 grp + 1
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              uint32_t b = 0;
+              b |= (acc[4 * (2 * grp) + 2 * h] > 0.0f ? 1u : 0u) << (2 * q4);
+              b |= (acc[4 * (2 * grp) + 2 * h + 1] > 0.0f ? 1u : 0u) << (2 * q4 + 1);
+              b |= (acc[4 * (2 * grp + 1) + 2 * h] > 0.0f ? 1u : 0u) << (8 + 2 * q4);
+              b |= (acc[4 * (2 * grp + 1) + 2 * h + 1] > 0.0f ? 1u : 0u) << (9 + 2 * q4);
+              b |= __shfl_xor_sync(0xffffffffu, b, 1);
+              b |= __shfl_xor_sync(0xffffffffu, b, 2);
+              if (q4 == 0 && valid_ab[h]) ap.bits[act_bits_index(plane, (col_off >> 4) + grp, row_ab[h], a.m)] = (uint16_t)b;
+            }
+          }
+        }
+      }
+    };
+    // sum over the four lanes of a quad (the four column owners of a row), fixed order
+    auto quad_sum = [&](float v) { v += __shfl_xor_sync(0xffffffffu, v, 1); v += __shfl_xor_sync(0xffffffffu, v, 2); return v; };
+
+    // ---------------- trunk: layers 0..7
+    float dens[2] = {0.f, 0.f};
+    for (int l = 0; l < 8; ++l) {
+      if (l == 0) { e_chunk(acc0, 4, true); e_chunk(acc1, 4, true); }
+      else {
+        all_act(acc0); if (l == 5) e_chunk(acc0, 4, false);
+        all_act(acc1); if (l == 5) e_chunk(acc1, 4, false);
+      }
+      drain();
+      wg_sync();                                   // every warp's MMAs on the old activation have completed
+      hidden(acc0, 2 * l, 0, l, W_HID, 0);
+      hidden(acc1, 2 * l + 1, 1, l, W_HID, 128);
+      if (l == 7) {                                // density_linear (dm_nerf.py:101) on the final trunk activation
+        const float* wd = bias_t + B_WD;
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          const int col = 8 * jj + 2 * q4;
+          const float2 w0 = __ldg(reinterpret_cast<const float2*>(wd + col)), w1 = __ldg(reinterpret_cast<const float2*>(wd + 128 + col));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            dens[h] = fmaf(acc0[4 * jj + 2 * h], w0.x, dens[h]); dens[h] = fmaf(acc0[4 * jj + 2 * h + 1], w0.y, dens[h]);
+            dens[h] = fmaf(acc1[4 * jj + 2 * h], w1.x, dens[h]); dens[h] = fmaf(acc1[4 * jj + 2 * h + 1], w1.y, dens[h]);
+          }
+        }
+      }
+      if (l == 5) {
+        // the position embedding has been read for the last time: the direction embedding takes its place (columns 0..31)
+        float vals[16];
+        if (!FUSED && a.x) {
+#pragma unroll
+          for (int i = 0; i < 16; ++i) vals[i] = (p_valid && 16 * ph + i < CH_DIR) ? a.x[p_row * CH_IN + CH_POS + 16 * ph + i] : 0.0f;
+        } else {
+          if (ph == 0) fill_embedding<0, 16, L_DIR, true>(vd, vals); else fill_embedding<16, 16, L_DIR, true>(vd, vals);
+          if (!p_valid) {
 #pragma unroll
             for (int i = 0; i < 16; ++i) vals[i] = 0.0f;
           }
-          save_emb(CH_POS + d_col0, c16{});
-          store_split16_smem(vals, d_hi_slab, d_lo_slab, r, d_col0);
         }
+        save_emb(CH_POS + 16 * ph, vals, 16);
+        store_split8_smem(vals, e_hi, e_lo, pr, 16 * ph);
+        store_split8_smem(vals + 8, e_hi, e_lo, pr, 16 * ph + 8);
       }
-      if (parts & PRO_DONE) {
-        fence_proxy_async_smem();          // the embeddings are read by the tensor core through the async proxy
-        mbar_arrive(&misc->inputs_ready);
-      }
-    };
-    (void)0;
-    // may tile tp be prepared during tile tp-1?  (the first fine tile of a pair needs this tile's importance samples)
-    auto early_ok = [&](int64_t tp) { return tp < my_tiles && (!FUSED || (tp & 3) != 1); };
-
-    if (my_tiles > 0) { KP_T0(); prologue(0, PRO_ALL); KP_ADD(10); }
-    for (int64_t ti = 0; ti < my_tiles; ++ti) {
-      // ---- which rows does this tile hold
-      const int j = FUSED ? (int)(ti & 3) : 0;                            // fused: 0 = coarse tile, 1..3 = fine tiles
-      const int64_t item = blockIdx.x + (FUSED ? (ti >> 2) : ti) * gridDim.x;
-      const int u_cur = FUSED ? (int)((ti >> 2) & 1) : 0;
-      int64_t row = 0;                                                    // RAW: global sample row
-      int rl = 0, si = 0, S = 0;                                          // fused: local ray (0/1), sample index, samples per ray
-      bool valid;
-      if constexpr (FUSED) {
-        if (j == 0) { rl = r >> 6; si = r & 63; S = FS; }
-        else { const int gr = (j - 1) * TILE_M + r; rl = gr / FF; si = gr % FF; S = FF; }
-        valid = fz->ray[u_cur][rl][7] != 0.0f;
-      } else {
-        row = item * TILE_M + r;
-        valid = row < a.m;
-      }
-      const float* bias_base = (FUSED && j != 0) ? a.bias_fine : a.bias;
-      // ---------------- epilogues of the 20 half-steps
-      for (int t = 0; t < N_STEPS; ++t) {
-        const uint32_t g = (uint32_t)ti * N_STEPS + t, acc = g & 1;
-        const uint32_t acc_addr = tbase + lane_sel + TC_ACC + acc * 128;
-        const float* bias = bias_base + t * 128;
-        const int q = cg;                             // output heads: 64-column half (column groups 0 and 1 only)
-        if (t <= T_RGB_HID) {
-          // hidden half-step (ReLU layers; even steps fill slot 0, odd steps slot 1): this thread's 32 columns -> bias,
-          // ReLU, split, store into the destination slot; the K chunk is published on its own barrier as soon as its two
-          // column groups are done.  The bias is fetched before the accumulator is waited for (L1 is tiny next to 224 KB of
-          // shared memory: these loads usually come from L2).
-          const int slot = t & 1;
-          // this thread's columns inside the half-step: f[0..15] <-> colA + i (K chunk cA), f[16..31] <-> colB + i (K chunk cB)
-          const int colA = epi_col_a(cg), colB = epi_col_b(cg);
-          const int cA = colA >> 6, cB = colB >> 6;
-          const uint32_t slot_addr = tbase + lane_sel + TC_SLOT + slot * SLOT_COLS;
-          const uint32_t hiA = slot_addr + cA * 32 + ((colA & 63) >> 1), hiB = slot_addr + cB * 32 + ((colB & 63) >> 1);
-          float4 bb[8];
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            bb[jj] = __ldg(reinterpret_cast<const float4*>(bias + colA) + jj);
-            bb[4 + jj] = __ldg(reinterpret_cast<const float4*>(bias + colB) + jj);
-          }
-          DBG_SITE(t * 100 + 1);
-          { KP_T0(); wait_bar_warp(&misc->acc_full[acc], (g / 2) & 1, misc, 301, a.status); KP_ADD(8); }
-          DBG_SITE(t * 100 + 2);
-          tc_fence_after();
-#ifdef DMN_KPROF
-          const long long kp_body0 = clock64();
-          if (blockIdx.x == 0 && ti >= KTRACE_TILE && ti < KTRACE_TILE + 2 && et == 0) g_ktrace[2][(ti - KTRACE_TILE) * 20 + t] = kp_body0;
-#endif
-          uint32_t v[32];
-#ifdef DMN_EXP_EPI_NOTMEM     /* timing experiment only (results are garbage): after a CTA's first tile the epilogue neither reads */
-          const bool exp_skip = ti > 0;   /* the accumulator nor writes a slot; the slots keep tile 0's activations as MMA operands */
-          if (exp_skip) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = 0x3f800000u + (uint32_t)(i + r);
-          } else
-#endif
-          {
-            if constexpr (EPI_SPLIT) { tmem_ld_x16(acc_addr + colA, v); tmem_ld_x16(acc_addr + colB, v + 16); }
-            else tmem_ld_x32(acc_addr + colA, v);
-            tmem_ld_wait();
-          }
-          if (t == T_RGB_HID) {       // nothing goes back to a slot: the accumulator is all the MMA warp waits for
-            tc_fence_before();
-            if constexpr (EPI_SPLIT) { mbar_arrive(&misc->epi_done[acc][0]); mbar_arrive(&misc->epi_done[acc][1]); }
-            else mbar_arrive(&misc->epi_done[acc][cA]);
-          }
-          float f[32];
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            f[4 * jj + 0] = fmaxf(__uint_as_float(v[4 * jj + 0]) + bb[jj].x, 0.0f);
-            f[4 * jj + 1] = fmaxf(__uint_as_float(v[4 * jj + 1]) + bb[jj].y, 0.0f);
-            f[4 * jj + 2] = fmaxf(__uint_as_float(v[4 * jj + 2]) + bb[jj].z, 0.0f);
-            f[4 * jj + 3] = fmaxf(__uint_as_float(v[4 * jj + 3]) + bb[jj].w, 0.0f);
-          }
-          auto density_partial = [&]() {   // density_linear (dm_nerf.py:101) on the final trunk activation, fp32 CUDA cores
-            const float* wbase = bias_base + B_WD + (t - 14) * 128;
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-              const float4 ww = __ldg(reinterpret_cast<const float4*>(wbase + (jj < 4 ? colA : colB)) + (jj & 3));
-              dens_acc = fmaf(f[4 * jj + 0], ww.x, dens_acc);
-              dens_acc = fmaf(f[4 * jj + 1], ww.y, dens_acc);
-              dens_acc = fmaf(f[4 * jj + 2], ww.z, dens_acc);
-              dens_acc = fmaf(f[4 * jj + 3], ww.w, dens_acc);
-            }
-          };
-          if (t < T_RGB_HID) {
-            if ((t & 1) == 0 && t >= 2) {
-              // slot 0 still feeds the MMAs of the odd half-step issued behind this one: wait until it has released it
-              KP_T0();
-              DBG_SITE(t * 100 + 3);
-#ifndef DMN_EXP_NO_AFREE      /* timing experiment only (results are garbage): the even epilogue does not wait for slot 0 */
-              wait_bar_warp(&misc->a_free, (uint32_t)((t >> 1) - 1) & 1u, misc, 302, a.status);
-#endif
-              KP_ADD(9);
-              tc_fence_after();
-            }
-#if defined(DMN_EXP_EPI_NOTMEM)
-            if (exp_skip) {
-              if (__float_as_uint(f[3]) == 0x7fc12345u) misc->part[cg][r].x = f[7] + f[19] + f[30];   // keeps the arithmetic alive
-              tc_fence_before(); mbar_arrive(&misc->epi_done[acc][0]);
-            } else {
-              store_split16_tmem(f, hiA, hiA + SLOT_LO);
-              tmem_st_wait();
-              tc_fence_before();
-              mbar_arrive(&misc->epi_done[acc][0]);
-              store_split16_tmem(f + 16, hiB, hiB + SLOT_LO);
-            }
-#elif defined(DMN_EXP_EPI_NOMATH)   /* timing experiment only: raw accumulator words go back to the slot, no bias / ReLU / split arithmetic */
-            if constexpr (EPI_SPLIT) {
-              tmem_st_x8(hiA, v); tmem_st_x8(hiA + SLOT_LO, v + 8);
-              tmem_st_wait();
-              tc_fence_before();
-              mbar_arrive(&misc->epi_done[acc][0]);
-              tmem_st_x8(hiB, v + 16); tmem_st_x8(hiB + SLOT_LO, v + 24);
-            }
-#else
-            if constexpr (EPI_SPLIT) {
-              store_split16_tmem(f, hiA, hiA + SLOT_LO);             // K chunk 0 first: published half an epilogue earlier
-              tmem_st_wait();
-              tc_fence_before();
-              mbar_arrive(&misc->epi_done[acc][0]);
-              store_split16_tmem(f + 16, hiB, hiB + SLOT_LO);
-            } else
-#endif
-            if constexpr (!EPI_SPLIT) {
-              store_split32_tmem(f, hiA, hiA + SLOT_LO);
-            }
-            if (t == 15) {            // publish before this half-step's arrive: the arrive orders it ahead of the reader
-              density_partial();      // (epi_done 15 -> MMA warp -> acc_full 17 -> colour-head epilogue)
-              misc->part[cg][r].w = dens_acc;
-              dens_acc = 0.0f;
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&misc->epi_done[acc][EPI_SPLIT ? 1 : cA]);
-#ifdef DMN_KPROF
-            if (blockIdx.x == 0 && ti >= KTRACE_TILE && ti < KTRACE_TILE + 2 && et == 0) g_ktrace[3][(ti - KTRACE_TILE) * 20 + t] = clock64();
-#endif
-            DBG_SITE(t * 100 + 4);
-            if (t == 14) density_partial();      // off the critical path
-          }
-          if constexpr (!FUSED) {
-            if (a.acts) {                            // training forward: keep the post-activation values (ActPlanes)
-              const ActPlanes ap = act_planes(a.acts, a.m);
-              const int width = (t < 16) ? W_HID : W_HID / 2;
-              float* dst = (t < 16) ? ap.h[t >> 1] + row * W_HID + (t & 1) * 128
-                                    : ((t == T_RGB_HID) ? ap.rgb_hid : ap.ins_hid) + row * (W_HID / 2);
-#ifndef DMN_EXP_FWD_NOACTSTORE      /* timing experiment: activation planes not written (results are garbage) */
-              if constexpr (EPI_SPLIT) {
-                const bool ok_other = (row ^ 1) < a.m;
-                store_row16_paired(dst + colA, width, f, valid, ok_other, r & 31);
-                store_row16_paired(dst + colB, width, f + 16, valid, ok_other, r & 31);
-              } else {
-#ifdef DMN_QUAD_STORE
-                DBG_SITE(t * 100 + 50);
-                store_row32_quad(dst + colA, width, f, row - (r & 3), a.m, r & 31);
-                DBG_SITE(t * 100 + 51);
-#else
-                if (valid) store_row32(dst + colA, f);
-#endif
-              }
-#endif
-              if (valid) {
-                uint32_t bwa = 0, bwb = 0;           // ReLU masks of these 2 x 16 units, 1 bit each (ActPlanes::bits)
-#pragma unroll
-                for (int i = 0; i < 16; ++i) { bwa |= (f[i] > 0.0f ? 1u : 0u) << i; bwb |= (f[16 + i] > 0.0f ? 1u : 0u) << i; }
-                const int plane = (t < 16) ? (t >> 1) : ((t == T_RGB_HID) ? 8 : 9);
-                const int ua = ((t < 16) ? (t & 1) * 128 : 0) + colA, ub = ((t < 16) ? (t & 1) * 128 : 0) + colB;   // unit index
-                ap.bits[act_bits_index(plane, ua >> 4, row, a.m)] = (uint16_t)bwa;     // row-fastest: a warp writes 64 contiguous bytes
-                ap.bits[act_bits_index(plane, ub >> 4, row, a.m)] = (uint16_t)bwb;
-              }
-            }
-          }
-          // Prepare the next tile in the idle time after odd half-steps: E was last read by half-step 11.
-          DBG_SITE(t * 100 + 6);
-          if ((t == 11 || t == 13) && early_ok(ti + 1)) {
-            KP_T0();
-            prologue(ti + 1, t == 11 ? PRO_E0 : PRO_E1);
-            KP_ADD(10);
-          }
-          if (t < T_RGB_HID) continue;
-          // ---------------- colour hidden layer: the 3-wide rgb head on CUDA cores (fp32), 32 columns per thread
-          {
-            float p0 = 0.0f, p1 = 0.0f, p2 = 0.0f;
-            const int colA = epi_col_a(cg), colB = epi_col_b(cg);
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-              const float4* w0 = reinterpret_cast<const float4*>(bias_base + B_WRGB + (jj < 4 ? colA : colB)) + (jj & 3);
-              const float4 wa = __ldg(w0), wb = __ldg(w0 + 32), wc = __ldg(w0 + 64);
-              p0 = fmaf(f[4 * jj + 0], wa.x, p0); p0 = fmaf(f[4 * jj + 1], wa.y, p0); p0 = fmaf(f[4 * jj + 2], wa.z, p0); p0 = fmaf(f[4 * jj + 3], wa.w, p0);
-              p1 = fmaf(f[4 * jj + 0], wb.x, p1); p1 = fmaf(f[4 * jj + 1], wb.y, p1); p1 = fmaf(f[4 * jj + 2], wb.z, p1); p1 = fmaf(f[4 * jj + 3], wb.w, p1);
-              p2 = fmaf(f[4 * jj + 0], wc.x, p2); p2 = fmaf(f[4 * jj + 1], wc.y, p2); p2 = fmaf(f[4 * jj + 2], wc.z, p2); p2 = fmaf(f[4 * jj + 3], wc.w, p2);
-            }
-            float4* dstp = &misc->part[cg][r];
-            dstp->x = p0; dstp->y = p1; dstp->z = p2;
-          }
-          // D was last read by this half-step: finish the next tile's operands (column groups 2 and 3 embed the direction).
-          // After a coarse tile of the fused kernel the next tile's depths do not exist yet: everybody waits for column
-          // group 0 to composite this tile and draw the importance samples, then prepares the first fine tile in one piece
-          // (the instance head of this tile is drained afterwards, off the critical path).
-          DBG_SITE(t * 100 + 7);
-          if (cg != 0) {
-            named_bar_arrive<4, 512>();
-            if (early_ok(ti + 1)) { KP_T0(); prologue(ti + 1, PRO_D | PRO_DONE); KP_ADD(10); }
-          } else {
-            if (early_ok(ti + 1)) prologue(ti + 1, PRO_DONE);
-            named_bar_sync<4, 512>();
-            // rgb_linear (dm_nerf.py:102,105) and density_linear (dm_nerf.py:101): add the four column groups' partial
-            // dot products in a fixed order
-            const float4 s0 = misc->part[0][r], s1 = misc->part[1][r], s2 = misc->part[2][r], s3 = misc->part[3][r];
-            const float c0 = ((s0.x + s1.x) + (s2.x + s3.x)) + __ldg(bias_base + B_BRGB + 0);
-            const float c1 = ((s0.y + s1.y) + (s2.y + s3.y)) + __ldg(bias_base + B_BRGB + 1);
-            const float c2 = ((s0.z + s1.z) + (s2.z + s3.z)) + __ldg(bias_base + B_BRGB + 2);
-            const float sigma = ((s0.w + s1.w) + (s2.w + s3.w)) + __ldg(bias_base + B_BD);
-            if constexpr (!FUSED) {
-              if (valid) {
-                float* o = a.out + row * C;
-                o[0] = c0; o[1] = c1; o[2] = c2; o[3] = sigma;
-              }
-            } else {
-              // ---- sigma -> alpha -> transmittance (render.py:7-18): warp scan + cross-warp carry
-              const float* zs = (j == 0) ? fz->zc[rl] : fz->zf[rl];
-              const float zi = zs[si];
-              float dist = (si == S - 1) ? 1e10f : __fsub_rn(zs[si + 1], zi);
-              dist = __fmul_rn(dist, fz->ray[u_cur][rl][6]);
-              const float alpha = __fsub_rn(1.0f, expf(-__fmul_rn(fmaxf(sigma, 0.0f), dist)));
-              const float f = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
-              const int lane_i = r & 31, wi = r >> 5;
-              const float incl = warp_scan_mul(f, lane_i);
-              float excl = __shfl_up_sync(FULL, incl, 1);
-              if (lane_i == 0) excl = 1.0f;
-              if (lane_i == 31) fz->tot[wi] = incl;
-              named_bar_sync<1, 128>();
-              // transmittance entering this warp = carry of the ray x products of earlier warps of the same ray in this tile
-              const int first_w = (j == 0) ? (rl * 2) : ((j == 2) ? (rl * 2) : 0);   // first warp of my ray inside this tile
-              float pre = (FUSED && j >= 2) ? fz->carry[j][rl] : 1.0f;
-              for (int w2 = first_w; w2 < wi; ++w2) pre = __fmul_rn(pre, fz->tot[w2]);
-              const float wgt = valid ? __fmul_rn(alpha, __fmul_rn(pre, excl)) : 0.0f;
-              fz->w[r] = wgt;
-              if (j >= 1 && j <= 2 && wi == 0 && lane_i < 2) {
-                // carry into the next fine tile for ray `lane_i` (ray A ends inside tile 2, ray B starts there)
-                float cpre = (j == 2) ? fz->carry[2][lane_i] : 1.0f;
-                const int wa = (j == 1) ? (lane_i == 0 ? 0 : 4) : (lane_i == 0 ? 0 : 2);    // warps of that ray in this tile
-                const int wb = (j == 1) ? (lane_i == 0 ? 4 : 4) : (lane_i == 0 ? 2 : 4);
-                for (int w2 = wa; w2 < wb; ++w2) cpre = __fmul_rn(cpre, fz->tot[w2]);
-                fz->carry[j + 1][lane_i] = cpre;
-              }
-              if (j == 0 && a.wc_out && valid) a.wc_out[(item * 2 + rl) * FS + si] = wgt;
-              if (j != 0 && a.wf_out && valid) a.wf_out[(item * 2 + rl) * FF + si] = wgt;
-              // ---- weighted sums (render.py:19-20 + acc): warp reduce, one shared-memory atomic per warp and channel
-              float p0 = __fmul_rn(wgt, sigmoidf_acc(c0)), p1 = __fmul_rn(wgt, sigmoidf_acc(c1)), p2 = __fmul_rn(wgt, sigmoidf_acc(c2));
-              float p3 = __fmul_rn(wgt, zi), p4 = wgt;
-              p0 = warp_sum(p0); p1 = warp_sum(p1); p2 = warp_sum(p2); p3 = warp_sum(p3); p4 = warp_sum(p4);
-              if (lane_i == 0) {
-                float* ac = fz->accum[rl][si >> 5];
-                ac[0] = p0; ac[1] = p1; ac[2] = p2; ac[3] = p3; ac[4] = p4;
-              }
-            }
-          if constexpr (FUSED) {
-            if (j == 0) {
-              // ---- hierarchical sampling (render.py:66-70) by this column group: 64 threads per ray, results stay in
-              //      shared memory.  (Barrier 1 = the 128 threads of column group 0.)
-              const int rr = r >> 6, t64 = r & 63;
-              fz->vals[rr][t64] = fz->zc[rr][t64];
-              if (t64 < FS - 1) fz->bins[rr][t64] = __fmul_rn(0.5f, __fadd_rn(fz->zc[rr][t64 + 1], fz->zc[rr][t64]));
-              named_bar_sync<1, 128>();          // bins and this tile's weights fz->w are complete
-              const int64_t ray = item * 2 + rr;
-              const float* wr = fz->w + rr * FS;
-              const float* uu = (a.u && fz->ray[u_cur][rr][7] != 0.0f) ? a.u + ray * FI : nullptr;
-              if (t64 < 32) ray_build_cdf([&](int k) { return wr[k + 1]; }, FS - 1, fz->cdf[rr], t64);
-              named_bar_sync<1, 128>();
-              for (int sidx = t64; sidx < FI; sidx += 64)
-                fz->vals[rr][FS + sidx] = ray_sample_at(fz->bins[rr], fz->cdf[rr], FS - 1, uu ? uu[sidx] : linspace01(sidx, FI));
-              named_bar_sync<1, 128>();
-              // both runs ascending (always, for the deterministic linspace)?  One vote for the pair keeps the barrier simple.
-              const bool mine = (uu == nullptr) && ray_sorted_part(fz->vals[rr] + FS, FI, t64, 64) && ray_sorted_part(fz->vals[rr], FS, t64, 64);
-              int all_sorted;
-              __syncwarp();
-              asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.s32 p, %1, 0;\n\tbarrier.red.and.pred q, 1, 128, p;\n\tselp.s32 %0, 1, 0, q;\n\t}"
-                           : "=r"(all_sorted) : "r"((int)mine) : "memory");
-              if (all_sorted) ray_merge_part(fz->vals[rr], FS, fz->vals[rr] + FS, FI, fz->zf[rr], t64, 64);
-              else ray_rank_part(fz->vals[rr], FF, fz->zf[rr], t64, 64);
-              named_bar_sync<1, 128>();
-              if (a.zf_out && fz->ray[u_cur][rr][7] != 0.0f)
-                for (int k = t64; k < FF; k += 64) a.zf_out[ray * FF + k] = fz->zf[rr][k];
-            }
-          }
-          }
-          if (FUSED && j == 0) {
-            named_bar_sync<3, 512>();            // fine depths visible to every prologue thread
-            if (ti + 1 < my_tiles) { KP_T0(); prologue(ti + 1, PRO_ALL); KP_ADD(10); }
-          }
-          continue;
-        }
-        const Step& st = prog.step[t];
-        DBG_SITE(t * 100 + 11);
-        { KP_T0(); wait_bar_warp(&misc->acc_full[acc], (g / 2) & 1, misc, 301, a.status); KP_ADD(8); }
-        DBG_SITE(t * 100 + 12);
-        tc_fence_after();
-        if (cg >= 2) {
-          // the instance head is drained by column groups 0 and 1 (256 threads, q = 64-column half) alone
-          if constexpr (EPI_SPLIT) {                 // every epilogue thread is counted on the chunk barriers
-            mbar_arrive(&misc->epi_done[acc][0]);
-            mbar_arrive(&misc->epi_done[acc][1]);
-          }
-        } else {
-          // instance head (N = pad16(ins_num+1))                                 (dm_nerf.py:103,105)
-          if constexpr (!FUSED) {
-            for (int c0 = q * 64; c0 < st.n && c0 < q * 64 + 64; c0 += 16) {
-              uint32_t v[16];
-              tmem_ld_x16(acc_addr + c0, v);
-              tmem_ld_wait();
-              if (valid) {
-                float* o = a.out + row * C + 4;
-#pragma unroll
-                for (int jj = 0; jj < 16; ++jj)
-                  if (c0 + jj < n_ins1) o[c0 + jj] = __uint_as_float(v[jj]) + __ldg(bias + c0 + jj);
-              }
-            }
-            tc_fence_before();
-            mbar_arrive(&misc->epi_done[acc][0]);
-            mbar_arrive(&misc->epi_done[acc][1]);
-          } else {
-            // instance logits weighted by the (detached) weights: sum_i w_i raw_i[4+k]   (render.py:22-24)
-            named_bar_sync<2, 256>();     // weights of this tile (fz->w) are complete
-            const float wgt = fz->w[r];
-            const int lane_i = r & 31;
-            const int c_end = (st.n < q * 64 + 64) ? st.n : q * 64 + 64;
-            bool arrived = false;
-            for (int c0 = q * 64; c0 < c_end; c0 += 16) {
-              uint32_t v[16];
-              tmem_ld_x16(acc_addr + c0, v);
-              tmem_ld_wait();
-              if (c0 + 16 >= c_end) {                  // last block in registers: the accumulator is drained
-                tc_fence_before();
-                mbar_arrive(&misc->epi_done[acc][0]);
-                mbar_arrive(&misc->epi_done[acc][1]);
-                arrived = true;
-              }
-              // 16 channels x 32 rows (one ray, one 32-sample chunk per warp) -> 16 sums with a transposing butterfly: every
-              // round halves the channels a lane carries (8 + 4 + 2 + 1 + 1 shuffles instead of 16 x 5); lanes 2c, 2c + 1 end up
-              // with channel c0 + c.  Fixed order: bit-reproducible.
-              float x[16];
-#pragma unroll
-              for (int jj = 0; jj < 16; ++jj)
-                x[jj] = (c0 + jj < n_ins1) ? __fmul_rn(wgt, __uint_as_float(v[jj]) + __ldg(bias + c0 + jj)) : 0.0f;
-#pragma unroll
-              for (int half = 8, bit = 16; half >= 1; half >>= 1, bit >>= 1) {
-                const bool up = (lane_i & bit) != 0;
-#pragma unroll
-                for (int i = 0; i < half; ++i) {
-                  const float send = up ? x[i] : x[half + i], keep = up ? x[half + i] : x[i];
-                  x[i] = __fadd_rn(keep, __shfl_xor_sync(FULL, send, bit));
-                }
-              }
-              const float tot = __fadd_rn(x[0], __shfl_xor_sync(FULL, x[0], 1));
-              const int ch = c0 + (lane_i >> 1);
-              if ((lane_i & 1) == 0 && ch < n_ins1) fz->accum[rl][si >> 5][5 + ch] = tot;
-            }
-            if (!arrived) {                            // no channel block in this 64-column half
-              tc_fence_before();
-              mbar_arrive(&misc->epi_done[acc][0]);
-              mbar_arrive(&misc->epi_done[acc][1]);
-            }
-            named_bar_sync<2, 256>();     // all running sums of this tile are in
-            // ---- rays that end in this tile: write their maps (render.py:19-26) and clear the sums
-            const int done_lo = (j == 0) ? 0 : ((j == 2) ? 0 : ((j == 3) ? 1 : 2));
-            const int done_hi = (j == 0) ? 2 : ((j == 2) ? 1 : ((j == 3) ? 2 : 2));
-            for (int rr = done_lo; rr < done_hi; ++rr) {
-              const int64_t ray = item * 2 + rr;
-              if (fz->ray[u_cur][rr][7] != 0.0f && et < 5 + n_ins1) {
-                float vsum = 0.0f;
-                for (int cj = 0; cj < S / 32; ++cj) vsum = __fadd_rn(vsum, fz->accum[rr][cj][et]);
-                float* o_rgb = (j == 0) ? a.rgb_c : a.rgb_f;
-                float* o_dep = (j == 0) ? a.depth_c : a.depth_f;
-                float* o_acc = (j == 0) ? a.acc_c : a.acc_f;
-                float* o_ins = (j == 0) ? a.ins_c : a.ins_f;
-                const int n_out = a.keep_all_ins ? n_ins1 : n_ins1 - 1;
-                if (et < 3) { if (o_rgb) o_rgb[ray * 3 + et] = vsum; }
-                else if (et == 3) { if (o_dep) o_dep[ray] = vsum; }
-                else if (et == 4) { if (o_acc) o_acc[ray] = vsum; }
-                else if (et - 5 < n_out) { if (o_ins) o_ins[ray * n_out + (et - 5)] = sigmoidf_acc(vsum); }
-              }
-            }
-          }
-        }
-      }
-      if (ti + 1 < my_tiles && !early_ok(ti + 1) && !(FUSED && j == 0)) { KP_T0(); prologue(ti + 1, PRO_ALL); KP_ADD(10); }
+      fence_proxy_async_smem();
+      wg_sync();
     }
-#ifdef DMN_KPROF
-    kp[11] = clock64() - kp_role0;
-    if (et == 0) for (int i = 8; i < 16; ++i) g_kprof[blockIdx.x][i] = kp[i];
-#endif
+    // ---------------- folded instance hidden layer (acc0) and folded colour hidden layer [h | dir] (acc1)
+    all_act(acc0);
+    all_act(acc1); e_chunk(acc1, 2, false);
+    drain();
+    wg_sync();
+    float rgb[2][3];
+    hidden(acc1, T_RGB_HID, -1, 8, W_HID / 2, 0);
+    {
+      // rgb_linear (dm_nerf.py:102,105) on CUDA cores
+#pragma unroll
+      for (int h = 0; h < 2; ++h) rgb[h][0] = rgb[h][1] = rgb[h][2] = 0.0f;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        const int col = 8 * jj + 2 * q4;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const float2 w = __ldg(reinterpret_cast<const float2*>(bias_t + B_WRGB + c * 128 + col));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            rgb[h][c] = fmaf(acc1[4 * jj + 2 * h], w.x, rgb[h][c]);
+            rgb[h][c] = fmaf(acc1[4 * jj + 2 * h + 1], w.y, rgb[h][c]);
+          }
+        }
+      }
+    }
+    hidden(acc0, T_INS_HID, 0, 9, W_HID / 2, 0);
+    fence_proxy_async_smem();
+    wg_sync();
+    // ---------------- instance head (dm_nerf.py:103,105) on the instance hidden activation (activation half 0)
+    // The weight stages of this step hold n = pad16(ins_num + 1) rows, but the MMA is issued with N = 128 like every other
+    // step: rows n..127 of the ring slot are stale bytes of an earlier stage.  Output column c depends only on B row c, so
+    // columns >= n are garbage and are never read (only columns < ins_num + 1 are stored below).  The head is 1 of 19
+    // half-steps of a tile.
+    act_chunk(acc0, 0, true); act_chunk(acc0, 1, false);
+    drain();
+    wg_sync();
+    const int n_ins1 = prog.ins_num + 1;
+    float c3[2][4];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      c3[h][0] = quad_sum(rgb[h][0]) + __ldg(bias_t + B_BRGB + 0);
+      c3[h][1] = quad_sum(rgb[h][1]) + __ldg(bias_t + B_BRGB + 1);
+      c3[h][2] = quad_sum(rgb[h][2]) + __ldg(bias_t + B_BRGB + 2);
+      c3[h][3] = quad_sum(dens[h]) + __ldg(bias_t + B_BD);
+    }
+    const float* bias_ins = bias_t + T_INS_OUT * 128;
+    if constexpr (!FUSED) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!valid_ab[h]) continue;
+        float* o = a.out + row_ab[h] * C;
+        if (q4 == 0) { o[0] = c3[h][0]; o[1] = c3[h][1]; o[2] = c3[h][2]; o[3] = c3[h][3]; }
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          const int col = 8 * jj + 2 * q4;
+          if (col < n_ins1) o[4 + col] = acc0[4 * jj + 2 * h] + __ldg(bias_ins + col);
+          if (col + 1 < n_ins1) o[5 + col] = acc0[4 * jj + 2 * h + 1] + __ldg(bias_ins + col + 1);
+        }
+      }
+    } else {
+      // per-row outputs into shared memory: rgb / density in misc->rowv, instance logits [128][128] over the activation
+      float* logit = reinterpret_cast<float*>(smem + SM_ACT);
+      all_sync();                        // both warpgroups' instance-head MMAs have read the activation
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (q4 == 0) misc->rowv[ra + 8 * h] = make_float4(c3[h][0], c3[h][1], c3[h][2], c3[h][3]);
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          const int col = 8 * jj + 2 * q4;
+          if (col < n_ins1) logit[(ra + 8 * h) * 128 + col] = acc0[4 * jj + 2 * h] + __ldg(bias_ins + col);
+          if (col + 1 < n_ins1) logit[(ra + 8 * h) * 128 + col + 1] = acc0[4 * jj + 2 * h + 1] + __ldg(bias_ins + col + 1);
+        }
+      }
+      all_sync();
+      if (tid < TILE_M) {
+        // ---- sigma -> alpha -> transmittance (render.py:7-18): warp scan + cross-warp carry; thread = tile row
+        const int r = tid;
+        int rl, si;
+        int64_t row_unused;
+        bool valid;
+        row_of(r, rl, si, row_unused, valid);
+        const int S = (j == 0) ? FS : FF;
+        const float4 rv = misc->rowv[r];
+        const float* zs = (j == 0) ? fz->zc[rl] : fz->zf[rl];
+        const float zi = zs[si];
+        float dist = (si == S - 1) ? 1e10f : __fsub_rn(zs[si + 1], zi);
+        dist = __fmul_rn(dist, fz->ray[rl][6]);
+        const float alpha = __fsub_rn(1.0f, expf(-__fmul_rn(fmaxf(rv.w, 0.0f), dist)));
+        const float f = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
+        const int lane_i = r & 31, wi = r >> 5;
+        const float incl = warp_scan_mul(f, lane_i);
+        float excl = __shfl_up_sync(FULL, incl, 1);
+        if (lane_i == 0) excl = 1.0f;
+        if (lane_i == 31) fz->tot[wi] = incl;
+        named_bar_sync<4, 128>();
+        // transmittance entering this warp = carry of the ray x products of earlier warps of the same ray in this tile
+        const int first_w = (j == 0) ? (rl * 2) : ((j == 2) ? (rl * 2) : 0);   // first warp of my ray inside this tile
+        float pre = (j >= 2) ? fz->carry[j][rl] : 1.0f;
+        for (int w2 = first_w; w2 < wi; ++w2) pre = __fmul_rn(pre, fz->tot[w2]);
+        const float wgt = valid ? __fmul_rn(alpha, __fmul_rn(pre, excl)) : 0.0f;
+        fz->w[r] = wgt;
+        if (j >= 1 && j <= 2 && wi == 0 && lane_i < 2) {
+          // carry into the next fine tile for ray `lane_i` (ray A ends inside tile 2, ray B starts there)
+          float cpre = (j == 2) ? fz->carry[2][lane_i] : 1.0f;
+          const int wa = (j == 1) ? (lane_i == 0 ? 0 : 4) : (lane_i == 0 ? 0 : 2);    // warps of that ray in this tile
+          const int wb = (j == 1) ? (lane_i == 0 ? 4 : 4) : (lane_i == 0 ? 2 : 4);
+          for (int w2 = wa; w2 < wb; ++w2) cpre = __fmul_rn(cpre, fz->tot[w2]);
+          fz->carry[j + 1][lane_i] = cpre;
+        }
+        if (j == 0 && a.wc_out && valid) a.wc_out[(item * 2 + rl) * FS + si] = wgt;
+        if (j != 0 && a.wf_out && valid) a.wf_out[(item * 2 + rl) * FF + si] = wgt;
+        // ---- weighted sums (render.py:19-20 + acc): warp reduce per 32-sample chunk
+        float p0 = __fmul_rn(wgt, sigmoidf_acc(rv.x)), p1 = __fmul_rn(wgt, sigmoidf_acc(rv.y)), p2 = __fmul_rn(wgt, sigmoidf_acc(rv.z));
+        float p3 = __fmul_rn(wgt, zi), p4 = wgt;
+        p0 = warp_sum(p0); p1 = warp_sum(p1); p2 = warp_sum(p2); p3 = warp_sum(p3); p4 = warp_sum(p4);
+        float* ac = fz->accum[rl][si >> 5];
+        if (lane_i == 0) { ac[0] = p0; ac[1] = p1; ac[2] = p2; ac[3] = p3; ac[4] = p4; }
+        named_bar_sync<4, 128>();        // weights of the tile complete
+        // instance logits weighted by the (detached) weights: sum_i w_i raw_i[4+k] (render.py:22-24); lane = channel,
+        // the 32 rows of this warp's chunk added in order
+        for (int ch = lane_i; ch < n_ins1; ch += 32) {
+          float sacc = 0.0f;
+          for (int rr = 0; rr < 32; ++rr) sacc = __fadd_rn(sacc, __fmul_rn(fz->w[32 * wi + rr], logit[(32 * wi + rr) * 128 + ch]));
+          ac[5 + ch] = sacc;
+        }
+        named_bar_sync<4, 128>();        // all running sums of this tile are in
+        // ---- rays that end in this tile: write their maps (render.py:19-26) and clear the sums
+        const int done_lo = (j == 0) ? 0 : ((j == 2) ? 0 : ((j == 3) ? 1 : 2));
+        const int done_hi = (j == 0) ? 2 : ((j == 2) ? 1 : ((j == 3) ? 2 : 2));
+        for (int rr = done_lo; rr < done_hi; ++rr) {
+          const int64_t ray = item * 2 + rr;
+          if (fz->ray[rr][7] == 0.0f) continue;
+          for (int e = r; e < 5 + n_ins1; e += TILE_M) {
+            float vsum = 0.0f;
+            for (int cj = 0; cj < S / 32; ++cj) vsum = __fadd_rn(vsum, fz->accum[rr][cj][e]);
+            float* o_rgb = (j == 0) ? a.rgb_c : a.rgb_f;
+            float* o_dep = (j == 0) ? a.depth_c : a.depth_f;
+            float* o_acc = (j == 0) ? a.acc_c : a.acc_f;
+            float* o_ins = (j == 0) ? a.ins_c : a.ins_f;
+            const int n_out = a.keep_all_ins ? n_ins1 : n_ins1 - 1;
+            if (e < 3) { if (o_rgb) o_rgb[ray * 3 + e] = vsum; }
+            else if (e == 3) { if (o_dep) o_dep[ray] = vsum; }
+            else if (e == 4) { if (o_acc) o_acc[ray] = vsum; }
+            else if (e - 5 < n_out) { if (o_ins) o_ins[ray * n_out + (e - 5)] = sigmoidf_acc(vsum); }
+          }
+        }
+        if (j == 0) {
+          // ---- hierarchical sampling (render.py:66-70): 64 threads per ray, results stay in shared memory
+          const int rr = r >> 6, t64 = r & 63;
+          fz->vals[rr][t64] = fz->zc[rr][t64];
+          if (t64 < FS - 1) fz->bins[rr][t64] = __fmul_rn(0.5f, __fadd_rn(fz->zc[rr][t64 + 1], fz->zc[rr][t64]));
+          named_bar_sync<4, 128>();          // bins complete
+          const int64_t ray = item * 2 + rr;
+          const float* wr = fz->w + rr * FS;
+          const float* uu = (a.u && fz->ray[rr][7] != 0.0f) ? a.u + ray * FI : nullptr;
+          if (t64 < 32) ray_build_cdf([&](int k) { return wr[k + 1]; }, FS - 1, fz->cdf[rr], t64);
+          named_bar_sync<4, 128>();
+          for (int sidx = t64; sidx < FI; sidx += 64)
+            fz->vals[rr][FS + sidx] = ray_sample_at(fz->bins[rr], fz->cdf[rr], FS - 1, uu ? uu[sidx] : linspace01(sidx, FI));
+          named_bar_sync<4, 128>();
+          // both runs ascending (always, for the deterministic linspace)?  One vote for the pair keeps the barrier simple.
+          const bool mine = (uu == nullptr) && ray_sorted_part(fz->vals[rr] + FS, FI, t64, 64) && ray_sorted_part(fz->vals[rr], FS, t64, 64);
+          int all_sorted;
+          __syncwarp();
+          asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.s32 p, %1, 0;\n\tbarrier.red.and.pred q, 4, 128, p;\n\tselp.s32 %0, 1, 0, q;\n\t}"
+                       : "=r"(all_sorted) : "r"((int)mine) : "memory");
+          if (all_sorted) ray_merge_part(fz->vals[rr], FS, fz->vals[rr] + FS, FI, fz->zf[rr], t64, 64);
+          else ray_rank_part(fz->vals[rr], FF, fz->zf[rr], t64, 64);
+          named_bar_sync<4, 128>();
+          if (a.zf_out && fz->ray[rr][7] != 0.0f)
+            for (int k = t64; k < FF; k += 64) a.zf_out[ray * FF + k] = fz->zf[rr][k];
+        }
+      }
+      all_sync();                        // the logits region is free again; fine depths visible to the next prologue
+    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(misc->tmem_base, 512);
 }
-
-#ifdef DMN_KPROF
-}  // namespace uk
-}  // namespace dmnerf
-extern "C" __attribute__((visibility("default"))) int dmnerf_debug_kprof(long long* out, int n_blocks) {
-  cudaDeviceSynchronize();
-  return (int)cudaMemcpyFromSymbol(out, dmnerf::uk::g_kprof, sizeof(long long) * 16 * (size_t)n_blocks);
-}
-extern "C" __attribute__((visibility("default"))) int dmnerf_debug_ktrace(long long* out) {
-  cudaDeviceSynchronize();
-  return (int)cudaMemcpyFromSymbol(out, dmnerf::uk::g_ktrace, sizeof(long long) * 4 * 64);
-}
-namespace dmnerf {
-namespace uk {
-#endif
 
 // ------------------------------------------------------------------------------------------------ host: program
 static void build_program(Program& P, int ins_num) {
@@ -1060,7 +754,6 @@ struct UmmaExtra {            // hangs off UmmaWeights::image allocation bookkee
   int32_t* d_status;          // device alias of h_status
   volatile int32_t* h_status;  // error word in mapped host memory: a kernel that gave up on a barrier writes its code here, and the
                               // NEXT launch through this weight set refuses to start (a stalled launch can never pass silently)
-  uint8_t* bwd_image;         // operand image of the gradient chain (bwd_chain.cu)
 };
 
 static UmmaExtra* extra_of(const UmmaWeights& w) { return reinterpret_cast<UmmaExtra*>(w.extra); }
@@ -1075,14 +768,12 @@ void umma_weights_free(UmmaWeights& w) {
     if (x->fold_b) cudaFree(x->fold_b);
     if (x->d_entries) cudaFree(x->d_entries);
     if (x->h_status) cudaFreeHost((void*)x->h_status);
-    if (x->bwd_image) cudaFree(x->bwd_image);
     delete x;
   }
   w = UmmaWeights();
 }
 
 bool umma_available(const UmmaWeights& w) { return w.ready; }
-const uint8_t* umma_bwd_image(const UmmaWeights& w) { return w.extra ? extra_of(w)->bwd_image : nullptr; }
 const float* umma_fold_w_rgb(const UmmaWeights& w) { return w.extra ? extra_of(w)->fold_w_rgb : nullptr; }
 int32_t* umma_status_word(const UmmaWeights& w) { return w.extra ? extra_of(w)->d_status : nullptr; }
 int umma_status_peek(const UmmaWeights& w) { return (w.extra && extra_of(w)->h_status) ? (int)*extra_of(w)->h_status : 0; }
@@ -1102,8 +793,7 @@ int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
     DMN_CUDA(cudaMalloc((void**)&x->fold_w_rgb, 128 * 283 * sizeof(float)));
     DMN_CUDA(cudaMalloc((void**)&x->fold_w_ins, 128 * 256 * sizeof(float)));
     DMN_CUDA(cudaMalloc((void**)&x->fold_b, 256 * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->d_entries, (MAX_STAGES + BWD_IMAGE_STAGES / 2) * sizeof(PackStage)));
-    DMN_CUDA(cudaMalloc((void**)&x->bwd_image, (size_t)BWD_IMAGE_STAGES * STAGE_BYTES));
+    DMN_CUDA(cudaMalloc((void**)&x->d_entries, MAX_STAGES * sizeof(PackStage)));
     DMN_CUDA(cudaHostAlloc((void**)&x->h_status, sizeof(int32_t), cudaHostAllocMapped));
     *x->h_status = 0;
     DMN_CUDA(cudaHostGetDevicePointer((void**)&x->d_status, (void*)x->h_status, 0));
@@ -1142,29 +832,9 @@ int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
   }
   DMN_CHECK((int)ent.size() * 2 == x->prog.n_stages && (int)ent.size() <= MAX_STAGES, "umma pack: stage table mismatch");
   const size_t n_fwd = ent.size();
-  // gradient chain (bwd_chain.cu): transposed operands, B[n = input unit][k = output unit] = W[k][n], in consumption order
-  {
-    uint32_t off = 0;
-    auto add = [&](const float* src, int ld, int n_base, int row_base) {
-      PackStage e;
-      memset(&e, 0, sizeof(e));
-      e.src = src; e.ld = ld; e.n_base = n_base; e.n_valid = 128; e.col_base = row_base; e.k_valid = 64; e.n_rows = 128;
-      e.transposed = 1; e.off_hi = off; e.off_lo = off + STAGE_BYTES;
-      off += 2 * STAGE_BYTES;
-      ent.push_back(e);
-    };
-    for (int h = 0; h < 2; ++h)                       // d h7 = d rgb_hid [., 128] x W_fold [128][256 (+27)]
-      for (int c = 0; c < 2; ++c) add(x->fold_w_rgb, 283, h * 128, 64 * c);
-    for (int l = 7; l >= 1; --l)                      // d h(l-1) = dY(l) [., 256] x W(l) [256][256 (+63 for the skip layer)]
-      for (int h = 0; h < 2; ++h)
-        for (int c = 0; c < 4; ++c) add(p.w[l], layer_in(l), h * 128, 64 * c);
-    DMN_CHECK((ent.size() - n_fwd) * 2 == (size_t)BWD_IMAGE_STAGES, "umma pack: backward stage table mismatch");
-  }
   DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), ent.size() * sizeof(PackStage), cudaMemcpyHostToDevice, st));
   DMN_CUDA(cudaStreamSynchronize(st));               // `ent` is a host temporary
   pack_kernel<<<(unsigned)n_fwd, 256, 0, st>>>(x->d_entries, (int)n_fwd, (uint8_t*)w.image);
-  DMN_LAUNCH_OK();
-  pack_kernel<<<(unsigned)(ent.size() - n_fwd), 256, 0, st>>>(x->d_entries + n_fwd, (int)(ent.size() - n_fwd), x->bwd_image);
   DMN_LAUNCH_OK();
   bias_kernel<<<8, 256, 0, st>>>(p, x->fold_b, x->fold_b + 128, w.bias);
   DMN_LAUNCH_OK();
@@ -1178,7 +848,7 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
   DMN_CHECK(w.ready && w.extra, "mlp(umma): weights not packed (call dmnerf_set_weights first)");
   DMN_CHECK((x != nullptr) != (rays_o != nullptr && rays_d != nullptr), "mlp(umma): pass either x or rays");
   DMN_CHECK(x != nullptr || z != nullptr || s == 1, "mlp(umma): points mode (z == NULL) takes one sample per row");
-  DMN_CHECK(umma_status_peek(w) == 0, "mlp(umma): an earlier tcgen05 launch reported protocol error %d (bounded wait expired); its results "
+  DMN_CHECK(umma_status_peek(w) == 0, "mlp(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); its results "
             "are invalid -- destroy the context", umma_status_peek(w));
   if (m == 0) return 0;
   UmmaExtra* ex = extra_of(w);
@@ -1186,7 +856,7 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
   if (attr_once.first()) {
     DMN_CUDA(cudaFuncSetAttribute(mlp_umma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   DMN_CUDA(cudaGetDevice(&dev));
   DMN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int64_t tiles = (m + TILE_M - 1) / TILE_M;
@@ -1207,7 +877,7 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   using namespace uk;
   DMN_CHECK(wc.ready && wf.ready && wc.extra && wf.extra, "render(umma): weights not packed");
   DMN_CHECK(wc.ins_num == wf.ins_num, "render(umma): coarse/fine ins_num differ");
-  DMN_CHECK(umma_status_peek(wc) == 0, "render(umma): an earlier tcgen05 launch reported protocol error %d (bounded wait expired); its "
+  DMN_CHECK(umma_status_peek(wc) == 0, "render(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); its "
             "results are invalid -- destroy the context", umma_status_peek(wc));
   if (n == 0) return 0;
   UmmaExtra* ex = extra_of(wc);
@@ -1215,7 +885,7 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   if (attr_once.first()) {
     DMN_CUDA(cudaFuncSetAttribute(mlp_umma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   DMN_CUDA(cudaGetDevice(&dev));
   DMN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   KArgs a;
@@ -1243,7 +913,7 @@ int umma_check_status(const UmmaWeights& w, cudaStream_t st) {
   int32_t code = 0;
   DMN_CUDA(cudaStreamSynchronize(st));
   code = (int32_t)*extra_of(w)->h_status;
-  DMN_CHECK(code == 0, "tcgen05 MLP kernel reported protocol error %d (bounded wait expired)", code);
+  DMN_CHECK(code == 0, "tensor-core MLP kernel reported protocol error %d (bounded wait expired)", code);
   return 0;
 }
 

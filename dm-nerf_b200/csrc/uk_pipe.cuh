@@ -1,12 +1,6 @@
-// Shared device-side pieces of the persistent tcgen05 pipelines (mlp_umma.cu: forward network / fused render kernel;
-// bwd_chain.cu: fused gradient chain of the training backward): tensor-memory and shared-memory maps, the barrier block,
-// bounded waits, the weight ring and the issue of one 64-wide K chunk, and the split-bf16 store helpers.
+// Shared device-side pieces of the persistent warpgroup-MMA network kernel (mlp_umma.cu: forward network / fused render
+// kernel): shared-memory map, the barrier block, bounded waits, the weight ring and the split-bf16 store helpers.
 #pragma once
-
-// Cache operator of the 256-bit activation / gradient plane stores of the training kernels (A/B knob: -DDMN_ST_COP='".cs"').
-#ifndef DMN_ST_COP
-#define DMN_ST_COP ""
-#endif
 
 #include "common.cuh"
 #include "umma.cuh"
@@ -16,8 +10,8 @@ namespace uk {
 
 using namespace umma;
 
-constexpr int TILE_M = 128;
-constexpr int NS = 8;                      // weight ring stages
+constexpr int TILE_M = 128;                // rows per tile: two consumer warpgroups of 64 rows
+constexpr int NS = 3;                      // weight ring stages
 constexpr int STAGE_BYTES = 16384;         // up to [128 rows][64 bf16]
 constexpr int CHUNK_BYTES = 16384;         // activation slab [128 rows][64 bf16]
 constexpr int N_STEPS = 19;                 // 16 trunk half-steps, instance hidden, colour hidden (+ head on CUDA cores), instance head
@@ -30,73 +24,29 @@ constexpr int B_BRGB = B_WRGB + 3 * 128;   // rgb_linear bias (+1 pad)
 constexpr int B_TOTAL = B_BRGB + 4;
 constexpr int MAX_CHUNKS = 5;
 constexpr int MAX_STAGES = 160;
-constexpr int EPI_THREADS = 512;           // 16 prologue / epilogue warps: 4 TMEM lane quadrants x 4 column groups
-// Column ownership of an epilogue thread inside a 128-column half-step.  EPI_SPLIT: 16 columns of K chunk 0 (columns
-// [16 cg, +16)) and then 16 columns of K chunk 1 ([64 + 16 cg, +16)): chunk 0 of a half-step's output is published after half of
-// the epilogue, so the next layer's MMAs on it are queued well before the tensor pipe runs dry (with 32 contiguous columns per
-// thread both chunks appear at the very end, a hair later than the pipe needs them: ~0.7 k idle cycles per layer).
-// Measured (profiles/r02_ab_and_kprof.md): the split mapping changes the fused render kernel by < 0.5 % (the kernel is bound by
-// board power, not by these dependency waits).  DMN_EPI_SPLIT=0 selects 32 contiguous columns per thread (round-1 mapping).
-#ifndef DMN_EPI_SPLIT
-#define DMN_EPI_SPLIT 1
-#endif
-constexpr bool EPI_SPLIT = DMN_EPI_SPLIT != 0;
-constexpr int CHUNK_THREADS = EPI_SPLIT ? 512 : 256;   // arrivals that publish one 64-column K chunk of a half-step's output
-__host__ __device__ constexpr int epi_col_a(int cg) { return EPI_SPLIT ? 16 * cg : 32 * cg; }
-__host__ __device__ constexpr int epi_col_b(int cg) { return EPI_SPLIT ? 64 + 16 * cg : 32 * cg + 16; }
-constexpr int N_THREADS = 128 + EPI_THREADS;
-
-// tensor-memory column map (512 columns x 128 lanes x 32 bit) -- completely used:
-//   two fp32 accumulators [128 x 128] and two activation slots, each holding a [128 x 128] activation block (one K-half of
-//   a 256-wide layer input) as split bf16: 64 columns of hi halves + 64 columns of lo halves (2 bf16 per 32-bit column).
-// Every trunk MMA therefore takes its A operand from tensor memory (no shared-memory read for A); the position / direction
-// embeddings, used by 4 of the 73 K chunks of a tile, live in shared memory instead.
-constexpr uint32_t TC_ACC = 0;             // two accumulators: [0,128) and [128,256)
-constexpr uint32_t TC_SLOT = 256;          // slot s at 256 + 128 s: hi of chunk c at +32 c, lo of chunk c at +64 + 32 c
-constexpr uint32_t SLOT_COLS = 128, SLOT_LO = 64;
+constexpr int CONSUMERS = 256;             // two warpgroups: MMA issue, epilogues, prologue
+constexpr int N_THREADS = CONSUMERS + 32;  // + one weight-producer warp
 
 // shared-memory map (offsets from the 1024-aligned base)
-constexpr uint32_t SM_E_HI = 0;                                 // position embedding, K-major SW128 slabs [128 rows][64 bf16]
+//   activation: 4 K chunks of the current 256-wide activation, each as a bf16 hi and a bf16 lo slab [128 rows][64]
+//   (warpgroup g reads and writes rows [64 g, 64 g + 64)).  After the instance head the region holds the instance logits
+//   of the tile (fused render kernel).
+constexpr uint32_t SM_ACT = 0;
+constexpr uint32_t ACT_CHUNK = 2 * CHUNK_BYTES;                  // hi slab, then lo slab
+constexpr uint32_t SM_E_HI = SM_ACT + 4 * ACT_CHUNK;             // position embedding; the direction embedding after layer 5
 constexpr uint32_t SM_E_LO = SM_E_HI + CHUNK_BYTES;
-constexpr uint32_t SM_D_HI = SM_E_LO + CHUNK_BYTES;             // direction embedding (32 of the 64 K columns used)
-constexpr uint32_t SM_D_LO = SM_D_HI + CHUNK_BYTES;
-constexpr uint32_t SM_RING = SM_D_LO + CHUNK_BYTES;
+constexpr uint32_t SM_RING = SM_E_LO + CHUNK_BYTES;
 constexpr uint32_t SM_MISC = SM_RING + NS * STAGE_BYTES;
-constexpr uint32_t SM_FUSED = SM_MISC + 9216;                   // per-unit state of the fused render kernel
+constexpr uint32_t SM_FUSED = SM_MISC + 3072;                   // per-unit state of the fused render kernel
 constexpr uint32_t SMEM_BYTES = SM_FUSED + 12288;
 static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB shared memory of an SM");
 
 struct Misc {                  // lives at SM_MISC
   uint64_t full[NS], empty[NS];
-  uint64_t acc_full[2], epi_done[2][2], inputs_ready;   // epi_done[accumulator][64-column chunk]
-  uint64_t a_free;             // the odd half-step of a layer has finished reading slot 0 (its even half-step may overwrite it)
-  uint32_t tmem_base;
   int32_t abort_flag;
-  float4 part[4][TILE_M];      // per column group and row: partial dot products of the rgb head (xyz) and of the density (w)
+  float4 rowv[TILE_M];         // fused render kernel: per row rgb (xyz) and density (w) of the current tile
 };
-
-static_assert(sizeof(Misc) <= 9216, "Misc does not fit its shared-memory block");
-
-// ------------------------------------------------------------------------------------------------ in-kernel cycle profile
-// Diagnostics build only (-DDMN_KPROF, tools/kprof.py): where do the MMA warp and one epilogue thread spend their cycles.
-#ifdef DMN_KPROF
-#define KTRACE_TILE 100
-#define KP_T0() const long long kp_t0 = clock64()
-#define KP_ADD(i) kp[i] += clock64() - kp_t0
-#else
-#define KP_T0() ((void)0)
-#define KP_ADD(i) ((void)0)
-#endif
-
-// ------------------------------------------------------------------------------------------------ stall diagnostics
-// Diagnostics build only (-DDMN_DEBUG_STALL, tools/stall_debug.py): every thread keeps the id of the last "site" it passed in
-// shared memory; the first thread whose bounded wait expires snapshots all 640 of them for the host.
-#ifdef DMN_DEBUG_STALL
-static __device__ int g_stall_dbg[641];     // one copy per translation unit (the export in mlp_umma.cu reads its own)
-#define DBG_SITE(site_) (reinterpret_cast<volatile int*>(smem + SM_FUSED)[threadIdx.x] = (site_))
-#else
-#define DBG_SITE(site_) ((void)0)
-#endif
+static_assert(sizeof(Misc) <= 3072, "Misc does not fit its shared-memory block");
 
 // ------------------------------------------------------------------------------------------------ bounded waits
 // Slow path of a barrier wait (kept out of line so the hot path is one try_wait + branch).
@@ -104,36 +54,17 @@ static __device__ int g_stall_dbg[641];     // one copy per translation unit (th
 // drains (with garbage results) and the host sees the status word -- no divergent early exits in the role loops.
 static __device__ __noinline__ void slow_wait(uint64_t* bar, uint32_t parity, Misc* misc, int code, int32_t* status) {
   const long long t0 = clock64();
-#ifdef DMN_WAIT_HINT_NS
-  while (!mbar_try_wait_hint(bar, parity, DMN_WAIT_HINT_NS)) {
-#else
   while (!mbar_try_wait(bar, parity)) {
-#endif
     if (*(volatile int32_t*)&misc->abort_flag) return;
     if (clock64() - t0 > 4000000000LL) {           // ~2 s: protocol failure
       atomicExch(&misc->abort_flag, code);
-#ifdef DMN_DEBUG_STALL
-      if (atomicCAS(status, 0, code) == 0) {
-        const volatile int* sd = reinterpret_cast<const volatile int*>(reinterpret_cast<uint8_t*>(misc) - SM_MISC + SM_FUSED);
-        for (int i = 0; i < 640; ++i) g_stall_dbg[i] = sd[i];
-        g_stall_dbg[640] = (int)blockIdx.x * 100000 + code * 1000 + (int)threadIdx.x;
-      }
-#else
       atomicCAS(status, 0, code);
-#endif
       return;
     }
   }
 }
 __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity, Misc* misc, int code, int32_t* status) {
   if (!mbar_try_wait(bar, parity)) slow_wait(bar, parity, misc, code, status);
-}
-
-// Wait executed by a WHOLE warp (prologue / epilogue roles): the lanes can leave the spin at different times, and what follows
-// (tcgen05.ld/st .sync.aligned, named barriers, warp shuffles) needs all 32 of them together -- reconverge explicitly.
-__device__ __forceinline__ void wait_bar_warp(uint64_t* bar, uint32_t parity, Misc* misc, int code, int32_t* status) {
-  wait_bar(bar, parity, misc, code, status);
-  __syncwarp();
 }
 
 // Named barriers are executed by whole warps and are .aligned: reconverge first (the lanes of a warp can be in different
@@ -143,10 +74,9 @@ __device__ __forceinline__ void named_bar_sync() {
   __syncwarp();
   asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(COUNT) : "memory");
 }
-template <int ID, int COUNT>
-__device__ __forceinline__ void named_bar_arrive() {
+__device__ __forceinline__ void named_bar_sync_id(int id, int count) {
   __syncwarp();
-  asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(COUNT) : "memory");
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // Position in the weight ring (warp-uniform).
@@ -157,46 +87,6 @@ struct Ring {
   }
 };
 
-// One 64-wide K chunk of one half-step: consumes the W_hi stage (A_hi*W_hi and A_lo*W_hi) and the W_lo stage (A_hi*W_lo).
-// Executed by the whole (converged) MMA warp; one elected lane issues.
-// A_SMEM = false: a_hi / a_lo are tensor-memory addresses (activation slots);  true: shared-memory descriptors (embeddings).
-template <int KS, bool A_SMEM>
-__device__ __forceinline__ void issue_chunk(Misc* misc, Ring& ring, uint32_t ring_base, uint64_t a_hi, uint64_t a_lo,
-                                            uint32_t d_tmem, uint32_t idesc, uint32_t& accum, int32_t* status,
-                                            long long* kp) {
-  const uint32_t s_hi = ring.slot, p_hi = ring.phase;
-  ring.advance();
-  const uint32_t s_lo = ring.slot, p_lo = ring.phase;
-  ring.advance();
-  const uint64_t wh = make_sdesc_sw128(ring_base + s_hi * STAGE_BYTES);
-  const uint64_t wl = make_sdesc_sw128(ring_base + s_lo * STAGE_BYTES);
-  if (elect_one()) {
-    { KP_T0(); wait_bar(&misc->full[s_hi], p_hi, misc, 204, status); KP_ADD(4); }
-    tc_fence_after();
-#pragma unroll
-    for (int k = 0; k < KS; ++k) {               // +2 on a descriptor = +32 bytes = 16 bf16 along K; +8 TMEM columns likewise
-      if (A_SMEM) {
-        mma_ss(d_tmem, a_hi + 2 * k, wh + 2 * k, idesc, k == 0 ? accum : 1u);
-        mma_ss(d_tmem, a_lo + 2 * k, wh + 2 * k, idesc, 1u);
-      } else {
-        mma_ts(d_tmem, (uint32_t)a_hi + k * 8, wh + 2 * k, idesc, k == 0 ? accum : 1u);
-        mma_ts(d_tmem, (uint32_t)a_lo + k * 8, wh + 2 * k, idesc, 1u);
-      }
-    }
-    mma_commit(&misc->empty[s_hi]);
-    { KP_T0(); wait_bar(&misc->full[s_lo], p_lo, misc, 205, status); KP_ADD(5); }
-    tc_fence_after();
-#pragma unroll
-    for (int k = 0; k < KS; ++k) {
-      if (A_SMEM) mma_ss(d_tmem, a_hi + 2 * k, wl + 2 * k, idesc, 1u);
-      else mma_ts(d_tmem, (uint32_t)a_hi + k * 8, wl + 2 * k, idesc, 1u);
-    }
-    mma_commit(&misc->empty[s_lo]);
-  }
-  __syncwarp();
-  accum = 1;
-}
-
 // 8 fp32 values -> bf16 hi and bf16 lo into two K-major SW128 slabs (row `row`, K columns [k0, k0+8): one 16-byte unit each).
 __device__ __forceinline__ void store_split8_smem(const float* vals, uint8_t* slab_hi, uint8_t* slab_lo, int row, int k0) {
   uint32_t hi[4], lo[4];
@@ -205,122 +95,6 @@ __device__ __forceinline__ void store_split8_smem(const float* vals, uint8_t* sl
   const uint32_t o = sw128_offset(row, k0);
   *reinterpret_cast<uint4*>(slab_hi + o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
   *reinterpret_cast<uint4*>(slab_lo + o) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-}
-
-// 16 fp32 values -> bf16 hi and bf16 lo into two K-major SW128 slabs (row `row`, K columns [k0, k0+16)).
-__device__ __forceinline__ void store_split16_smem(const float* vals, uint8_t* slab_hi, uint8_t* slab_lo, int row, int k0) {
-  uint32_t hi[8], lo[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) split_bf16x2(vals[2 * j], vals[2 * j + 1], hi[j], lo[j]);
-#pragma unroll
-  for (int u = 0; u < 2; ++u) {
-    const uint32_t o = sw128_offset(row, k0 + 8 * u);
-    *reinterpret_cast<uint4*>(slab_hi + o) = make_uint4(hi[4 * u], hi[4 * u + 1], hi[4 * u + 2], hi[4 * u + 3]);
-    *reinterpret_cast<uint4*>(slab_lo + o) = make_uint4(lo[4 * u], lo[4 * u + 1], lo[4 * u + 2], lo[4 * u + 3]);
-  }
-}
-
-// 32 fp32 values -> bf16 hi and bf16 lo, both into TMEM (16 columns each).
-__device__ __forceinline__ void store_split32_tmem(const float* vals, uint32_t tmem_hi, uint32_t tmem_lo) {
-  uint32_t hi[16], lo[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) split_bf16x2(vals[2 * j], vals[2 * j + 1], hi[j], lo[j]);
-  tmem_st_x16(tmem_hi, hi);
-  tmem_st_x16(tmem_lo, lo);
-}
-
-// 16 fp32 values -> bf16 hi and bf16 lo, both into TMEM (8 columns each).
-__device__ __forceinline__ void store_split16_tmem(const float* vals, uint32_t tmem_hi, uint32_t tmem_lo) {
-  uint32_t hi[8], lo[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) split_bf16x2(vals[2 * j], vals[2 * j + 1], hi[j], lo[j]);
-  tmem_st_x8(tmem_hi, hi);
-  tmem_st_x8(tmem_lo, lo);
-}
-
-// 16 consecutive fp32 values of one row (64 B, 32-byte aligned) to global memory as two 256-bit stores.
-__device__ __forceinline__ void store_row16(float* __restrict__ dst, const float* v) {
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-    asm volatile("st.global" DMN_ST_COP ".v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst + 8 * i), "f"(v[8 * i]), "f"(v[8 * i + 1]),
-                 "f"(v[8 * i + 2]), "f"(v[8 * i + 3]), "f"(v[8 * i + 4]), "f"(v[8 * i + 5]), "f"(v[8 * i + 6]), "f"(v[8 * i + 7])
-                 : "memory");
-}
-
-// Two neighbouring lanes (rows r, r ^ 1 of the tile) store their 16-column groups TOGETHER: they swap halves with one shuffle
-// round, so that every 256-bit store instruction writes 64 contiguous bytes per lane pair (16 row pieces per instruction
-// instead of 32 scattered sectors: half the L1 store wavefronts, which is what bounds the activation / gradient plane
-// stores -- ncu: l1tex 64-67 %, DRAM 22-33 %).  `dst` = this lane's own row (column of v[0]); row_stride in floats;
-// ok_own / ok_other: the two rows exist.  All 32 lanes must call it.
-__device__ __forceinline__ void store_row16_paired(float* __restrict__ dst, int64_t row_stride, const float* v, bool ok_own,
-                                                   bool ok_other, int lane) {
-  __syncwarp();
-  const bool odd = (lane & 1) != 0;
-  float x[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) x[i] = __shfl_xor_sync(0xffffffffu, odd ? v[i] : v[8 + i], 1);
-  float* even_row = odd ? dst - row_stride : dst;      // the pair's even lane's row
-  float* odd_row = odd ? dst : dst + row_stride;
-  const bool ok_even = odd ? ok_other : ok_own, ok_odd = odd ? ok_own : ok_other;
-  float a[8], b[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) { a[i] = odd ? x[i] : v[i]; b[i] = odd ? v[8 + i] : x[i]; }
-  float* pa = even_row + (odd ? 8 : 0);                // instruction 1: the even row's 64 bytes, 32 per lane
-  float* pb = odd_row + (odd ? 8 : 0);                 // instruction 2: the odd row's
-  if (ok_even)
-    asm volatile("st.global" DMN_ST_COP ".v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(pa), "f"(a[0]), "f"(a[1]), "f"(a[2]), "f"(a[3]), "f"(a[4]),
-                 "f"(a[5]), "f"(a[6]), "f"(a[7]) : "memory");
-  if (ok_odd)
-    asm volatile("st.global" DMN_ST_COP ".v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(pb), "f"(b[0]), "f"(b[1]), "f"(b[2]), "f"(b[3]), "f"(b[4]),
-                 "f"(b[5]), "f"(b[6]), "f"(b[7]) : "memory");
-}
-
-#ifdef DMN_QUAD_STORE      /* diagnostics only: the four-lane store variant that stalled intermittently (tools/stall_debug.py) */
-// Four neighbouring lanes (rows 4k..4k+3 of the tile) store their 32-column groups TOGETHER: a 4 x 4 transpose of 8-float
-// blocks in two shuffle rounds, after which lane q holds block q of all four rows and every 256-bit store instruction writes
-// whole 128-byte lines (8 per instruction instead of 32 scattered sectors).  `dst` = this lane's own row (column of v[0]);
-// row_base = index of the quad's first row; all 32 lanes must call it.
-__device__ __forceinline__ void store_row32_quad(float* __restrict__ dst, int64_t row_stride, const float* v, int64_t row_base,
-                                                 int64_t n_rows, int lane) {
-  __syncwarp();
-  const int q = lane & 3;
-  const bool b0 = (q & 1) != 0, b1 = (q & 2) != 0;
-  // round 1 (xor 1): lanes with bit 0 clear keep blocks 0, 2 and receive the partner's blocks 0, 2; the others blocks 1, 3
-  float xe[2][8], xo[2][8];             // [lower / upper block][8 floats] of the pair's even row / odd row
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float r0 = __shfl_xor_sync(0xffffffffu, b0 ? v[i] : v[8 + i], 1);          // partner's lower block of MY parity
-    const float r1 = __shfl_xor_sync(0xffffffffu, b0 ? v[16 + i] : v[24 + i], 1);    // partner's upper block of MY parity
-    xe[0][i] = b0 ? r0 : v[i];        xe[1][i] = b0 ? r1 : v[16 + i];
-    xo[0][i] = b0 ? v[8 + i] : r0;    xo[1][i] = b0 ? v[24 + i] : r1;
-  }
-  // round 2 (xor 2): lanes with bit 1 clear keep the lower blocks and receive the other pair's lower blocks; the others upper
-  float t[4][8];                         // block q of rows row_base + 0..3
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float re = __shfl_xor_sync(0xffffffffu, b1 ? xe[0][i] : xe[1][i], 2);
-    const float ro = __shfl_xor_sync(0xffffffffu, b1 ? xo[0][i] : xo[1][i], 2);
-    t[0][i] = b1 ? re : xe[0][i];   t[1][i] = b1 ? ro : xo[0][i];       // rows of pair A (quad rows 0, 1)
-    t[2][i] = b1 ? xe[1][i] : re;   t[3][i] = b1 ? xo[1][i] : ro;       // rows of pair B (quad rows 2, 3)
-  }
-  float* base = dst - (int64_t)q * row_stride + 8 * q;      // quad row 0, this lane's 8-float block
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-    if (row_base + i < n_rows)
-      asm volatile("st.global" DMN_ST_COP ".v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(base + (int64_t)i * row_stride), "f"(t[i][0]),
-                   "f"(t[i][1]), "f"(t[i][2]), "f"(t[i][3]), "f"(t[i][4]), "f"(t[i][5]), "f"(t[i][6]), "f"(t[i][7]) : "memory");
-}
-
-#endif
-
-// 32 consecutive fp32 values of one row (128 B, 32-byte aligned) to global memory as four 256-bit stores: every store is a
-// whole 32-byte sector (a 128-bit store leaves half-sector partial writes for the L2 to merge, at twice the request count).
-__device__ __forceinline__ void store_row32(float* __restrict__ dst, const float* v) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-    asm volatile("st.global" DMN_ST_COP ".v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst + 8 * i), "f"(v[8 * i]), "f"(v[8 * i + 1]),
-                 "f"(v[8 * i + 2]), "f"(v[8 * i + 3]), "f"(v[8 * i + 4]), "f"(v[8 * i + 5]), "f"(v[8 * i + 6]), "f"(v[8 * i + 7])
-                 : "memory");
 }
 
 }  // namespace uk

@@ -1,14 +1,15 @@
-// Thin inline-PTX layer over the Blackwell tensor-core path (sm_100a): tcgen05.mma (UMMA) with shared-memory or
-// tensor-memory A operand, TMEM allocation / load / store, mbarrier, bulk async copy (TMA engine, 1-D).
+// Thin inline-PTX layer over the Hopper tensor-core path (sm_90a): warpgroup MMA (wgmma.mma_async) with both operands in
+// shared memory and the fp32 accumulator in registers, mbarrier, bulk async copy (TMA engine, 1-D).
 // Layout conventions used everywhere in this library:
 //   * K-major bf16 operand "slab": [rows][64 bf16] = 128 B per row, rows grouped by 8 into 1024 B swizzle atoms,
 //     16-byte unit u of row r stored at unit (u ^ (r & 7))  (the canonical SWIZZLE_128B K-major layout).
 //     A slab of R rows occupies R * 128 bytes and must start 1024 B aligned.
-//   * UMMA shared-memory descriptor for such a slab: start address, LBO = 16 B (ignored for swizzled K-major),
-//     SBO = 1024 B (stride between 8-row groups), version 1, layout type SWIZZLE_128B.  Advancing K by 16 elements
-//     inside the slab = +32 B on the start address.
-//   * TMEM: lane = accumulator row (M = 128 uses all 128 lanes), column = fp32 accumulator column; a bf16 A operand in
-//     TMEM packs two consecutive K elements per 32-bit column (K = 16 per MMA -> 8 columns).
+//   * wgmma shared-memory descriptor for such a slab: start address, LBO = 16 B (ignored for swizzled K-major),
+//     SBO = 1024 B (stride between 8-row groups), layout type SWIZZLE_128B.  Advancing K by 16 elements inside the slab =
+//     +32 B on the start address.  The same bytes read MN-major (rows = contraction index) take LBO = stride between
+//     64-element MN blocks, SBO = 1024 B, and a K = 16 step advances the start address by 2048 B.
+//   * accumulator fragment of m64nNk16 (fp32): thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and
+//     columns 8 j + 2 (t % 4) (+ 1): d[4 j + 0, 1] = row r, columns c, c + 1; d[4 j + 2, 3] = row r + 8, same columns.
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
@@ -17,8 +18,7 @@ namespace umma {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// One lane of a converged warp (all 32 lanes must execute this).  Keeping the issuing warp converged lets the compiler hold
-// MMA operands in uniform registers instead of emitting a per-instruction R2UR waterfall.
+// One lane of a converged warp (all 32 lanes must execute this).
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
@@ -26,26 +26,17 @@ __device__ __forceinline__ bool elect_one() {
 }
 
 // ---------------------------------------------------------------- descriptors
-// Instruction descriptor, kind::f16, A/B = bf16 (K-major), D = fp32.  (cute/arch/mma_sm100_desc.hpp bit layout)
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4)                     // c_format  = F32
-         | (1u << 7)                   // a_format  = BF16
-         | (1u << 10)                  // b_format  = BF16
-         | (0u << 15) | (0u << 16)     // a_major = b_major = K
-         | ((uint32_t)(N >> 3) << 17)  // n_dim
-         | ((uint32_t)(M >> 4) << 24); // m_dim
-}
-
-// Shared-memory matrix descriptor for a K-major SWIZZLE_128B slab starting at shared address `saddr`.
-__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t saddr) {
+// Shared-memory matrix descriptor (SWIZZLE_128B) with explicit leading / stride byte offsets.
+__device__ __forceinline__ uint64_t sdesc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);        // start address   bits [0,14)
-  d |= (uint64_t)(16u >> 4) << 16;                 // leading byte offset (unused for swizzled K-major)
-  d |= (uint64_t)(1024u >> 4) << 32;               // stride byte offset: 8 rows * 128 B
-  d |= (uint64_t)1 << 46;                          // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                          // layout type: SWIZZLE_128B
+  d |= (uint64_t)((lbo & 0x3FFFFu) >> 4) << 16;    // leading byte offset
+  d |= (uint64_t)((sbo & 0x3FFFFu) >> 4) << 32;    // stride byte offset
+  d |= (uint64_t)1 << 62;                          // layout type: SWIZZLE_128B
   return d;
 }
+// K-major SWIZZLE_128B slab starting at shared address `saddr`.
+__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t saddr) { return sdesc(saddr, 16, 1024); }
 
 // Byte offset of element (row, k) inside a K-major SW128 slab (k in [0,64)).
 __host__ __device__ __forceinline__ uint32_t sw128_offset(int row, int k) {
@@ -75,18 +66,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// try_wait with a suspend-time hint (ns): the warp may sleep in hardware up to that long instead of spinning on the barrier.
-__device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t parity, uint32_t hint_ns) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity), "r"(hint_ns)
-      : "memory");
-  return ok != 0;
-}
 // Bounded wait: returns false (and the caller must bail out) instead of hanging the GPU if the barrier never flips.
 __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, uint32_t max_spins = 1u << 26) {
   for (uint32_t i = 0; i < max_spins; ++i)
@@ -95,9 +74,8 @@ __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, uint32
 }
 
 // ---------------------------------------------------------------- proxies / fences
+// Generic-proxy shared-memory writes (operand slabs stored by threads) made visible to the tensor core (async proxy).
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ---------------------------------------------------------------- bulk async copy (TMA engine, 1-D)
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
@@ -107,74 +85,54 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                : "memory");
 }
 
-// ---------------------------------------------------------------- TMEM management (one full warp executes these)
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// ---------------------------------------------------------------- warpgroup MMA (all 128 threads of a warpgroup)
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// Keeps the compiler from moving accumulator reads / writes across an asynchronous MMA.
+template <int R>
+__device__ __forceinline__ void wg_reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------- MMA issue (ONE thread)
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T; TA / TB = 1: that operand is MN-major.  scale_d = 0 overwrites D.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,"
+      "%62,%63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
       : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]^T
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All previously issued MMAs of this thread arrive on `bar` when complete (implies fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-// ---------------------------------------------------------------- TMEM <-> registers (warp-collective, 32 lanes x 32-bit)
-// Warp w may touch TMEM lanes [32*(w%4), 32*(w%4)+32).  taddr = base | (lane_base << 16) | column.
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t* r) {
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31},"
+      " %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_st_x8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------- bf16 hi/lo split (round-to-nearest)
 // x ~= hi + lo with hi = bf16(x), lo = bf16(x - hi): 16 significand bits in total.

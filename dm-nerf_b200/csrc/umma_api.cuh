@@ -1,4 +1,4 @@
-// Interface between the C-ABI layer and the tcgen05 (UMMA) MLP kernel.
+// Interface between the C-ABI layer and the tensor-core (wgmma) MLP kernel.
 #pragma once
 #include "common.cuh"
 
@@ -16,10 +16,6 @@ struct UmmaWeights {
   bool ready = false;
 };
 
-// Backward operand image (bwd_chain.cu): the transposed weights of the gradient chain in consumption order, 16 KB stages:
-// head fold 2 half-steps x 2 chunks, layers 7..1 x 2 half-steps x 4 chunks, hi + lo each.
-constexpr int BWD_IMAGE_STAGES = (2 * 2 + 14 * 4) * 2;
-const uint8_t* umma_bwd_image(const UmmaWeights& w);
 const float* umma_fold_w_rgb(const UmmaWeights& w);      // [128][283]: W_rgb_hid[:, :256] W_rgb_feat | W_rgb_hid[:, 256:]
 int32_t* umma_status_word(const UmmaWeights& w);
 int umma_status_peek(const UmmaWeights& w);            // host-side read of the error word (mapped memory, no synchronisation)

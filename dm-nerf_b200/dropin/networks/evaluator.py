@@ -1,5 +1,5 @@
 """networks.evaluator (reference networks/evaluator.py): the Hungarian-matched instance loss of the training step
-(ins_criterion / hungarian) and the small loss lambdas run on the B200 kernels; the evaluation-time metrics (ins_eval,
+(ins_criterion / hungarian) and the small loss lambdas run on the native kernels; the evaluation-time metrics (ins_eval,
 calculate_ap: CPU numpy code outside the hot path) are re-exported from the reference checkout when DMNERF_REFERENCE_ROOT
 points at one."""
 import importlib.util as _ilu

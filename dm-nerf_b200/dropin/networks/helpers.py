@@ -1,4 +1,4 @@
-"""networks.helpers (reference networks/helpers.py): the hot-path functions come from the B200 package;
+"""networks.helpers (reference networks/helpers.py): the hot-path functions come from the native package;
 everything else (ray selection for training, rotation helpers) is re-exported from the reference when
 DMNERF_REFERENCE_ROOT points at a checkout."""
 import importlib.util as _ilu

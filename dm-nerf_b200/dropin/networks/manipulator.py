@@ -1,4 +1,4 @@
-"""networks.manipulator (reference networks/manipulator.py): the edit path runs on the B200 kernels; the reference's
+"""networks.manipulator (reference networks/manipulator.py): the edit path runs on the native kernels; the reference's
 evaluation / demo loops (manipulator_eval, manipulator_demo: image IO, LPIPS, ...) are re-exported from the reference checkout
 when DMNERF_REFERENCE_ROOT points at one and its dependencies are installed."""
 import importlib.util as _ilu

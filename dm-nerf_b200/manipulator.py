@@ -3,7 +3,7 @@ of the edit path with the reference's names and signatures.
 
     exchanger(ori_raw, tar_raws, ori_raw_pred, tar_raw_preds, move_labels)               manipulator.py:18-83   (one kernel)
     manipulator_render(raw, z_vals, rays_d)                                              manipulator.py:86-105  (composite, all instance channels)
-    manipulator_nerf(rays, position_embedder, view_embedder, model, N_samples, near, far, z_vals)   manipulator.py:108-134 (tcgen05 network)
+    manipulator_nerf(rays, position_embedder, view_embedder, model, N_samples, near, far, z_vals)   manipulator.py:108-134 (tensor-core network)
     manipulator(position_embedder, view_embedder, model_coarse, model_fine, ori_rays, f_tar_rays, args)   manipulator.py:137-205
 
 The evaluation / demo loops of the reference module (image IO, metrics) are not part of the path and are not provided.

@@ -18,7 +18,7 @@ class DM_NeRF(nn.Module):
         self.skips, self.input_ch_pts, self.input_ch_views = skips, input_ch_pts, input_ch_views
         if not (D == 8 and W == 256 and input_ch_pts == 63 and input_ch_views == 27 and list(skips) == [4]):
             raise NotImplementedError(
-                "the B200 kernels are specialised for DM_NeRF(D=8, W=256, input_ch_pts=63, input_ch_views=27, "
+                "the native kernels are specialised for DM_NeRF(D=8, W=256, input_ch_pts=63, input_ch_views=27, "
                 "skips=[4]) -- the only configuration config.create_nerf builds (config.py:126-138)")
         if ins_num is None or not (1 <= int(ins_num) <= _lib.N_PARAMS * 0 + 127):
             raise ValueError("ins_num must be in [1, 127], got %r" % (ins_num,))

@@ -1,5 +1,5 @@
 """Drop-in for reference networks/render.py: `dm_nerf` (:31-96, the north_star's render_rays) and
-`render_train` (:6-28, raw2outputs), running on the fused B200 kernels through the C ABI."""
+`render_train` (:6-28, raw2outputs), running on the fused native kernels through the C ABI."""
 import ctypes as C
 
 import torch

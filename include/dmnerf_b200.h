@@ -1,5 +1,5 @@
 /*
- * dmnerf_b200.h -- C ABI of the B200-native DM-NeRF volumetric renderer (libdmnerf_b200.so).
+ * dmnerf_b200.h -- C ABI of the H100-native (sm_90a) DM-NeRF volumetric renderer (libdmnerf_b200.so).
  *
  * The reference (vLAR-group/DM-NeRF) has no FFI: its boundary is the Python call surface
  *   networks/render.py:31   dm_nerf(rays, pos_embedder, view_embedder, model_coarse, model_fine, z_vals_coarse, args)
@@ -35,9 +35,9 @@ extern "C" {
 #define DMNERF_MAX_INS 127          /* ins_num + 1 <= 128 */
 
 /* MLP implementation selector */
-#define DMNERF_IMPL_AUTO 0          /* tcgen05 path when available for the shape, else SIMT */
+#define DMNERF_IMPL_AUTO 0          /* tensor-core path when available for the shape, else SIMT */
 #define DMNERF_IMPL_SIMT 1          /* fp32 CUDA-core reference kernel */
-#define DMNERF_IMPL_UMMA 2          /* tcgen05 tensor-core kernel, bf16x3 split operands, fp32 accumulate */
+#define DMNERF_IMPL_UMMA 2          /* wgmma tensor-core kernel, bf16x3 split operands, fp32 accumulate */
 
 /* dmnerf_render_* flags */
 #define DMNERF_FLAG_PERTURB   1     /* args.perturb > 0: t_rand and u must be given (render.py:40-47, helpers.py:135) */
@@ -187,8 +187,9 @@ DMNERF_API int dmnerf_mlp_forward_train(dmnerf_ctx* ctx, int net, const float* x
  * Gradient routing follows the reference (networks/dm_nerf.py:95: the instance branch reads h.detach()).
  * scratch: dmnerf_mlp_backward_scratch_floats(m) floats.  feats_missing is a flag word: bit 0 = the forward did not write the
  * feature planes (tensor-core forward), bit 1 = the caller has already zero-filled `grads` (one fill instead of 30 memsets).
- * M >= 512: one fused tcgen05 kernel carries the gradient through the trunk (it never leaves the SM between layers) and
- * tcgen05 GEMMs form the weight gradients; smaller batches and DMNERF_BWD_IMPL=simt use fp32 CUDA-core kernels. */
+ * M >= 512: the heads are folded like in the forward, one masked split-bf16 wgmma GEMM per layer carries the gradient
+ * through the trunk and batched wgmma GEMMs form the weight gradients; smaller batches and DMNERF_BWD_IMPL=simt use fp32
+ * CUDA-core kernels. */
 DMNERF_API int dmnerf_mlp_backward(dmnerf_ctx* ctx, int net, float* acts, const float* d_out, int64_t m, float* const* grads,
                         float* scratch, int feats_missing, void* stream);
 

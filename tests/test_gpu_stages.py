@@ -59,7 +59,7 @@ IMPLS = [pytest.param(_lib.IMPL_SIMT, id="simt"), pytest.param(_lib.IMPL_UMMA, i
 @pytest.mark.parametrize("impl", IMPLS)
 @pytest.mark.parametrize("ins_num", [13, 59])
 def test_mlp(golden_dir, ins_num, impl):
-    """DM_NeRF.forward: fp32 CUDA-core kernel and the tcgen05 bf16x3 kernel against the reference fixture."""
+    """DM_NeRF.forward: fp32 CUDA-core kernel and the wgmma bf16x3 kernel against the reference fixture."""
     from dmnerf_b200.engine import get_context
     g = load(golden_dir, "mlp_ins%d.npz" % ins_num)
     net = model_from_weights(synth.make_weights(int(g["seed"]), ins_num), DEV).eval()

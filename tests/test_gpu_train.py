@@ -216,12 +216,10 @@ def test_tensor_core_training_forward_saves_the_reference_activations(m):
 
 @pytest.mark.parametrize("ins_num", [13, 59, 127])
 def test_mlp_backward_tensor_core_gemms(ins_num):
-    """Batches of >= 512 samples run the backward on the tensor cores: the fused gradient chain (bwd_chain.cu: head gradients,
-    dY7..dY0 in one launch, masks from bit planes -- here produced from the exact forward's planes by mask_bits_kernel), the dW
-    GEMMs (gemm_umma.cu) and the folded head products; with the exact-fp32 forward the 30 parameter gradients must still agree
-    with torch autograd on the oracle to fp32 noise.  1333 samples: ten full 128-row tiles + a ragged one, 32-sample stages with
-    a ragged tail; ins_num = 127 is the widest object head the library accepts (128 instance logits, 66 KB of head weights in
-    the head-gradient kernel's shared memory)."""
+    """Batches of >= 512 samples run the backward on the tensor cores: the split-bf16 wgmma dX and dW GEMMs (gemm_umma.cu) layer
+    by layer; with the exact-fp32 forward the 30 parameter gradients must still agree with torch autograd on the oracle to fp32
+    noise.  1333 samples: ten full 128-row tiles + a ragged one, 32-sample stages with a ragged tail; ins_num = 127 is the widest
+    object head the library accepts (128 instance logits)."""
     m = 1333
     w = synth.make_weights(21, ins_num)
     p = O.to_torch(w)

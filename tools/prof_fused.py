@@ -11,7 +11,7 @@ from dmnerf_b200.engine import get_context               # noqa: E402
 from dmnerf_b200.testing import make_models              # noqa: E402
 from dmnerf_b200.render import render_rays               # noqa: E402
 
-n = int(sys.argv[1]) if len(sys.argv) > 1 else 148 * 2 * 96
+n = int(sys.argv[1]) if len(sys.argv) > 1 else 132 * 2 * 96
 dev = "cuda"
 wl = synth.workload("dmsr_study")
 nc, nf, _, _ = make_models(101, 202, wl["ins_num"], dev)

@@ -1,4 +1,4 @@
-"""Minimal driver for ncu: a few launches of the fine-network tcgen05 kernel (rays mode) on one GPU."""
+"""Minimal driver for a profiler: a few launches of the fine-network tensor-core kernel (rays mode) on one GPU."""
 import os
 import sys
 
@@ -11,7 +11,7 @@ from dmnerf_b200.engine import get_context               # noqa: E402
 from dmnerf_b200.testing import model_from_weights       # noqa: E402
 from dmnerf_b200.autograd import mlp_forward_rays        # noqa: E402
 
-n = int(sys.argv[1]) if len(sys.argv) > 1 else 148 * 256
+n = int(sys.argv[1]) if len(sys.argv) > 1 else 132 * 256
 dev = "cuda"
 wl = synth.workload("dmsr_study")
 net = model_from_weights(synth.make_weights(202, 13), dev).eval()

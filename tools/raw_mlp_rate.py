@@ -1,11 +1,11 @@
 import sys, torch
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, __import__("os").path.dirname(__import__("os").path.dirname(__import__("os").path.abspath(__file__))))
 from dmnerf_b200 import synth
 from dmnerf_b200.autograd import mlp_forward_points
 from dmnerf_b200.testing import make_models
 dev = "cuda"
 _, nf, _, _ = make_models(101, 202, 13, dev)
-n = 148 * 128 * 96          # 96 tiles per CTA
+n = 132 * 128 * 96          # 96 tiles per CTA
 pts = (torch.rand(n, 3, device=dev) * 6 - 3)
 with torch.no_grad():
     for _ in range(3): out = mlp_forward_points(nf, pts)

@@ -16,7 +16,7 @@ from dmnerf_b200.render import render_rays               # noqa: E402
 launches = int(sys.argv[1]) if len(sys.argv) > 1 else 300
 dev = "cuda"
 slow = []
-for name, n in (("dmsr_study", 148 * 2 * 8), ("replica_room0_93", 4096), ("dmsr_study", 1001)):
+for name, n in (("dmsr_study", 132 * 2 * 8), ("replica_room0_93", 4096), ("dmsr_study", 1001)):
     wl = synth.workload(name)
     nc, nf, _, _ = make_models(101, 202, wl["ins_num"], dev)
     ro, rd = torch.from_numpy(wl["rays_o"][:n]).to(dev), torch.from_numpy(wl["rays_d"][:n]).to(dev)
