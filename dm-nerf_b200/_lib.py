@@ -90,6 +90,19 @@ PROTOTYPES = {
     "dmnerf_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.c_int]),
     "dmnerf_render_forward_host": (C.c_int, [C.c_void_p, C.POINTER(RenderIO), C.c_int64, C.c_int, C.c_int, C.c_int,
                                              C.c_int, C.c_void_p]),
+    "dmnerf_mesh_grid_points": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_int64, C.c_int64, _f32p,
+                                          C.c_void_p]),
+    "dmnerf_mesh_occupancy": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_float,
+                                        C.c_int64, _f32p, C.c_void_p]),
+    "dmnerf_mesh_mc_count": (C.c_int, [C.c_void_p, _f32p, C.c_int, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_mesh_mc_emit": (C.c_int, [C.c_void_p, _f32p, C.c_int, C.c_int, C.c_int, C.c_float, _f32p, C.c_void_p, C.c_void_p]),
+    "dmnerf_mesh_to_scene": (C.c_int, [_f32p, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, _f32p, C.c_void_p]),
+    "dmnerf_mesh_normals": (C.c_int, [C.c_void_p, _f32p, C.c_int64, C.c_void_p, C.c_int64, _f32p, C.c_void_p]),
+    "dmnerf_mesh_clusters": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dmnerf_mesh_clean": (C.c_int, [C.c_void_p, _f32p, _f32p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, _f32p, _f32p,
+                                    C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_mesh_label_rays": (C.c_int, [_f32p, _f32p, C.c_int64, C.c_float, _f32p, _f32p, C.c_void_p]),
+    "dmnerf_argmax_rows": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

@@ -53,6 +53,8 @@ struct dmnerf_ctx {
   Scratch ws_raw_c, ws_raw_f, ws_z_c, ws_z_f, ws_w_c, ws_w_f;
   Scratch host_in, host_out;      // device staging for the *_host entry point
   Scratch frame_rays;             // rays of the frame being rendered by dmnerf_render_frame_host
+  Scratch mesh_pts, mesh_raw;     // one slab of the occupancy sweep: points + zero view directions, network output
+  MeshState* mesh = nullptr;      // buffers of the other mesh entry points (mesh.cu)
   bool train_feats_missing[2] = {false, false};
   bool profiling = false;
   bool last_fused = false;       // the last render call took the single-kernel path
@@ -91,8 +93,9 @@ DMNERF_API int dmnerf_ctx_destroy(dmnerf_ctx* ctx) {
   cudaSetDevice(ctx->device);
   for (int i = 0; i < 2; ++i) umma_weights_free(ctx->packed[i]);
   Scratch* all[] = {&ctx->ws_raw_c, &ctx->ws_raw_f, &ctx->ws_z_c, &ctx->ws_z_f, &ctx->ws_w_c, &ctx->ws_w_f,
-                    &ctx->host_in, &ctx->host_out, &ctx->frame_rays};
+                    &ctx->host_in, &ctx->host_out, &ctx->frame_rays, &ctx->mesh_pts, &ctx->mesh_raw};
   for (Scratch* s : all) s->release();
+  mesh_state_free(ctx->mesh);
   for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_in) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_done) if (e) cudaEventDestroy(e);
@@ -591,6 +594,98 @@ DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, co
   h.rays_o = nullptr; h.rays_d = nullptr; h.t_rand = nullptr; h.u = nullptr;
   h.z_coarse = z.data(); h.z_row_stride = 0;
   return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, stream);
+}
+
+// ---- mesh extraction (tools/mesh_generator.py mesh_main) ------------------------------------------------------------------
+
+DMNERF_API int dmnerf_mesh_grid_points(const double* transform_host, const double* extents_host, int dim, int64_t begin, int64_t count,
+                                       float* pts, void* stream) {
+  DMN_CHECK(transform_host && extents_host && (count == 0 || pts), "mesh_grid_points: NULL argument");
+  return launch_grid_points(transform_host, extents_host, dim, begin, count, pts, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
+                                     float voxel, int64_t slab, float* occ, void* stream) {
+  DMN_CHECK(ctx && (net == 0 || net == 1), "mesh_occupancy: bad ctx / net");
+  DMN_CHECK(transform_host && extents_host && occ, "mesh_occupancy: NULL argument");
+  DMN_CHECK(dim >= 2 && dim <= 2048, "mesh_occupancy: dim %d out of range [2, 2048]", dim);
+  DMN_CHECK(umma_available(ctx->packed[net]), "mesh_occupancy: bind the network with dmnerf_set_weights first");
+  cudaStream_t st = (cudaStream_t)stream;
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  const int64_t n = (int64_t)dim * dim * dim;
+  if (slab <= 0) slab = (int64_t)1 << 20;
+  if (slab > n) slab = n;
+  const int C = 4 + ctx->net[net].ins_num + 1;
+  if (ctx->mesh_pts.reserve((size_t)slab * 6 * sizeof(float)) || ctx->mesh_raw.reserve((size_t)slab * C * sizeof(float))) return 2;
+  float* pts = (float*)ctx->mesh_pts.ptr;
+  float* dirs = pts + slab * 3;                                   // mesh_generator.py:42: zero view directions
+  float* raw = (float*)ctx->mesh_raw.ptr;
+  DMN_CUDA(cudaMemsetAsync(dirs, 0, (size_t)slab * 3 * sizeof(float), st));
+  // slab by slab: the [dim^3, C] network output of the original never exists, only [slab, C]
+  for (int64_t b = 0; b < n; b += slab) {
+    const int64_t cnt = n - b < slab ? n - b : slab;
+    int rc = launch_grid_points(transform_host, extents_host, dim, b, cnt, pts, st);
+    if (!rc) rc = launch_mlp_umma(ctx->packed[net], ctx->net[net], nullptr, pts, dirs, nullptr, cnt, 1, raw, nullptr, st);
+    if (!rc) rc = launch_occupancy(raw, cnt, C, voxel, occ + b, st);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+DMNERF_API int dmnerf_mesh_mc_count(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, int64_t* counts_host,
+                                    void* stream) {
+  DMN_CHECK(ctx && grid && counts_host, "mesh_mc_count: NULL argument");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return mc_count(&ctx->mesh, grid, nx, ny, nz, level, counts_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_mesh_mc_emit(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris,
+                                   void* stream) {
+  DMN_CHECK(ctx && grid, "mesh_mc_emit: NULL argument");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return mc_emit(ctx->mesh, grid, nx, ny, nz, level, verts, tris, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_mesh_to_scene(const float* verts, int64_t n, const double* transform_host, const double* extents_host, int dim,
+                                    float* out, void* stream) {
+  DMN_CHECK(n >= 0 && transform_host && extents_host && (n == 0 || (verts && out)), "mesh_to_scene: bad argument");
+  return launch_to_scene(verts, n, transform_host, extents_host, dim, out, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_mesh_normals(dmnerf_ctx* ctx, const float* verts, int64_t nv, const int32_t* tris, int64_t nt, float* normals,
+                                   void* stream) {
+  DMN_CHECK(ctx && (nv == 0 || (verts && normals)) && (nt == 0 || tris), "mesh_normals: NULL argument");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return mesh_normals(&ctx->mesh, verts, nv, tris, nt, normals, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_mesh_clusters(dmnerf_ctx* ctx, const int32_t* tris, int64_t nt, int64_t nv, int32_t* cluster, int32_t* cluster_size,
+                                    void* stream) {
+  DMN_CHECK(ctx && (nt == 0 || (tris && cluster && cluster_size)), "mesh_clusters: NULL argument");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return mesh_clusters(&ctx->mesh, tris, nt, nv, cluster, cluster_size, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_mesh_clean(dmnerf_ctx* ctx, const float* verts, const float* normals, int64_t nv, const int32_t* tris, int64_t nt,
+                                 const int32_t* cluster_size, int min_cluster, float* out_verts, float* out_normals, int32_t* out_tris,
+                                 int64_t* counts_host, void* stream) {
+  DMN_CHECK(ctx && counts_host, "mesh_clean: NULL argument");
+  DMN_CHECK(nv == 0 || (verts && out_verts && (!normals == !out_normals)), "mesh_clean: NULL vertex buffer");
+  DMN_CHECK(nt == 0 || (tris && cluster_size && out_tris), "mesh_clean: NULL triangle buffer");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return mesh_clean(&ctx->mesh, verts, normals, nv, tris, nt, cluster_size, min_cluster, out_verts, out_normals, out_tris, counts_host,
+                    (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_mesh_label_rays(const float* verts, const float* normals, int64_t n, float near_z, float* rays_o, float* rays_d,
+                                      void* stream) {
+  DMN_CHECK(n >= 0 && (n == 0 || (verts && normals && rays_o && rays_d)), "mesh_label_rays: bad argument");
+  return launch_label_rays(verts, normals, n, near_z, rays_o, rays_d, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_argmax_rows(const float* x, int64_t n, int c, int64_t* out, void* stream) {
+  DMN_CHECK(n >= 0 && c >= 1 && (n == 0 || (x && out)), "argmax_rows: bad argument");
+  return launch_argmax_rows(x, n, c, out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -184,4 +184,19 @@ int launch_hungarian_assign(const float* cost_ce, const float* cost_siou, const 
                             int32_t* row_of_col, float* loss3, cudaStream_t st);
 int ins_status_take();
 
+// Mesh extraction (mesh.cu).  Transforms are row-major 4x4 float64 host arrays, extents 3 float64 host values.
+struct MeshState;                 // per-context device buffers of the mesh entry points
+void mesh_state_free(MeshState* s);
+int launch_grid_points(const double* T16, const double* ext3, int dim, int64_t begin, int64_t count, float* pts, cudaStream_t st);
+int launch_occupancy(const float* raw, int64_t n, int c, float voxel, float* occ, cudaStream_t st);
+int mc_count(MeshState** s, const float* grid, int nx, int ny, int nz, float level, int64_t* counts, cudaStream_t st);
+int mc_emit(MeshState* s, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris, cudaStream_t st);
+int launch_to_scene(const float* v, int64_t n, const double* T16, const double* ext3, int dim, float* out, cudaStream_t st);
+int mesh_normals(MeshState** s, const float* v, int64_t nv, const int32_t* tris, int64_t nt, float* normals, cudaStream_t st);
+int mesh_clusters(MeshState** s, const int32_t* tris, int64_t nt, int64_t nv, int32_t* cluster, int32_t* cluster_size, cudaStream_t st);
+int mesh_clean(MeshState** s, const float* v, const float* nrm, int64_t nv, const int32_t* tris, int64_t nt, const int32_t* csize,
+               int min_cluster, float* out_v, float* out_n, int32_t* out_t, int64_t* counts, cudaStream_t st);
+int launch_label_rays(const float* v, const float* nrm, int64_t n, float near_z, float* ro, float* rd, cudaStream_t st);
+int launch_argmax_rows(const float* x, int64_t n, int c, int64_t* out, cudaStream_t st);
+
 }  // namespace dmnerf

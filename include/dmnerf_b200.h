@@ -260,6 +260,49 @@ DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream);
 DMNERF_API int dmnerf_profile_enable(dmnerf_ctx* ctx, int enable);
 DMNERF_API int dmnerf_profile_read(dmnerf_ctx* ctx, float* ms_out, int n_out);
 
+/* ---- mesh extraction: mesh_main, tools/mesh_generator.py (+ tools/visualizer.py) ----------------------------------------
+ * transform_host: row-major 4x4 float64 (scene_transform = inv(to_origin), :23-25); extents_host: 3 float64 ([1.9, 7, 7], :26).
+ * Conventions (vertex position, numbering, face-ambiguity rule, winding): DESIGN.md, "Mesh extraction".
+ *
+ * dmnerf_mesh_grid_points: points [begin, begin + count) of the dim^3 query grid (C order of the grid index), in the network's
+ *   frame: make_3D_grid / grid_within_bound in float32 + the axis swap and flip of :28-29.  pts [count,3].
+ * dmnerf_mesh_occupancy: the occupancy sweep (:33-63): network `net` at every grid point with zero view directions, slab points
+ *   at a time (slab <= 0: 2^20), each slab reduced to occ = 1 - exp(-relu(sigma) * voxel) -> occ [dim,dim,dim].
+ * dmnerf_mesh_mc_count / _mc_emit: marching cubes (:68-69) on any grid [nx,ny,nz] (DEVICE, C order), inside = value > level.
+ *   count classifies, scans and reads back counts_host[0] = vertices, [1] = triangles (the one device->host read; fails on a grid
+ *   holding NaN); emit (same grid and level) writes verts [V,3] in index units and tris [T,3] int32.
+ * dmnerf_mesh_to_scene: index-space vertices -> scene space (:70-86): v / (dim - 1) in float32, then (q - 0.5) * 2 * extents / 2
+ *   and the transform in float64, rounded to float32.
+ * dmnerf_mesh_normals: area-weighted vertex normals (open3d compute_vertex_normals, visualizer.py:164), deterministic.
+ * dmnerf_mesh_clusters: edge-connected triangle clusters (cluster_connected_triangles, visualizer.py:174): cluster [T] = smallest
+ *   triangle index of the cluster, cluster_size [T] = its triangle count.
+ * dmnerf_mesh_clean: clean_mesh (visualizer.py:169-194): triangles with cluster_size < min_cluster removed, then unreferenced
+ *   vertices; order kept.  Outputs need room for nv / nt rows; counts_host[0..1] = kept vertices / triangles.  normals and
+ *   out_normals may both be NULL.
+ * dmnerf_mesh_label_rays: the per-vertex label rays (:106-113): rays_d = -normal, rays_o = v - rays_d * 0.03 * near, both in the
+ *   network's frame.
+ * dmnerf_argmax_rows: torch.argmax(x, -1) of x [n,c] -> int64 [n] (first maximum; NaN counts as the maximum). */
+DMNERF_API int dmnerf_mesh_grid_points(const double* transform_host, const double* extents_host, int dim, int64_t begin, int64_t count,
+                                       float* pts, void* stream);
+DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
+                                     float voxel, int64_t slab, float* occ, void* stream);
+DMNERF_API int dmnerf_mesh_mc_count(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, int64_t* counts_host,
+                                    void* stream);
+DMNERF_API int dmnerf_mesh_mc_emit(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris,
+                                   void* stream);
+DMNERF_API int dmnerf_mesh_to_scene(const float* verts, int64_t n, const double* transform_host, const double* extents_host, int dim,
+                                    float* out, void* stream);
+DMNERF_API int dmnerf_mesh_normals(dmnerf_ctx* ctx, const float* verts, int64_t nv, const int32_t* tris, int64_t nt, float* normals,
+                                   void* stream);
+DMNERF_API int dmnerf_mesh_clusters(dmnerf_ctx* ctx, const int32_t* tris, int64_t nt, int64_t nv, int32_t* cluster, int32_t* cluster_size,
+                                    void* stream);
+DMNERF_API int dmnerf_mesh_clean(dmnerf_ctx* ctx, const float* verts, const float* normals, int64_t nv, const int32_t* tris, int64_t nt,
+                                 const int32_t* cluster_size, int min_cluster, float* out_verts, float* out_normals, int32_t* out_tris,
+                                 int64_t* counts_host, void* stream);
+DMNERF_API int dmnerf_mesh_label_rays(const float* verts, const float* normals, int64_t n, float near_z, float* rays_o, float* rays_d,
+                                      void* stream);
+DMNERF_API int dmnerf_argmax_rows(const float* x, int64_t n, int c, int64_t* out, void* stream);
+
 /* Number of kernels this library has launched on the calling thread's contexts since load. */
 DMNERF_API int64_t dmnerf_launch_count(void);
 
