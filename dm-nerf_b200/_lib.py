@@ -103,7 +103,20 @@ PROTOTYPES = {
                                     C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_mesh_label_rays": (C.c_int, [_f32p, _f32p, C.c_int64, C.c_float, _f32p, _f32p, C.c_void_p]),
     "dmnerf_argmax_rows": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "dmnerf_eval_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int, C.c_int, C.c_int]),
+    "dmnerf_eval_image": (C.c_int, [_f32p, _f32p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dmnerf_ins_eval": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_void_p, C.c_int, _f32p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p]),
+    "dmnerf_calculate_ap": (C.c_int, [_f32p, _f32p, C.c_int, C.c_int, _f32p, C.c_void_p]),
+    "dmnerf_ins_dense_rows": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "dmnerf_label_colors": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
 }
+
+
+class EvalResult(C.Structure):
+    """Mirror of `struct dmnerf_eval_result`."""
+    _fields_ = [("ap", C.c_float * 6), ("gt_num", C.c_int32), ("pred_num", C.c_int32), ("status", C.c_int32),
+                ("reserved", C.c_int32), ("psnr", C.c_double), ("ssim", C.c_double), ("return_labels", C.c_int32 * 128)]
 
 _lib = None
 _lock = threading.Lock()

@@ -688,4 +688,40 @@ DMNERF_API int dmnerf_argmax_rows(const float* x, int64_t n, int c, int64_t* out
   return launch_argmax_rows(x, n, c, out, (cudaStream_t)stream);
 }
 
+// ---- test-view evaluation (networks/tester.py render_test, networks/evaluator.py ins_eval) --------------------------------
+
+DMNERF_API int64_t dmnerf_eval_workspace_bytes(int64_t n, int k, int H, int W) {
+  if (n < 0 || k < 0 || H < 0 || W < 0) return -1;
+  return eval_workspace_bytes(n, k, H, W);
+}
+
+DMNERF_API int dmnerf_eval_image(const float* rgb, const float* gt, int H, int W, void* ws, dmnerf_eval_result* res, void* stream) {
+  DMN_CHECK(rgb && gt && ws && res, "eval_image: NULL argument");
+  return eval_image(rgb, gt, H, W, ws, res, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_ins_eval(const float* ins, int64_t n, int k, const int32_t* gt_row, int gt_num, const float* mask,
+                               const int32_t* mask_labels, int mask_below, int64_t* pred_label, void* ws, dmnerf_eval_result* res,
+                               void* stream) {
+  DMN_CHECK(ins && gt_row && pred_label && ws && res, "ins_eval: NULL argument");
+  DMN_CHECK(!(mask && mask_labels), "ins_eval: pass either mask or mask_labels, not both");
+  return ins_eval(ins, n, k, gt_row, gt_num, mask, mask_labels, mask_below, pred_label, ws, res, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_calculate_ap(const float* ious, const float* conf, int m, int gt_number, float* ap6, void* stream) {
+  DMN_CHECK(ious && ap6, "calculate_ap: NULL argument");
+  return calculate_ap(ious, conf, m, gt_number, ap6, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_ins_dense_rows(const float* gt_ins, int64_t n, int k, int gt_num, int32_t* gt_row, void* stream) {
+  DMN_CHECK(n >= 0 && k >= 1 && (n == 0 || (gt_ins && gt_row)), "ins_dense_rows: bad argument");
+  return ins_dense_rows(gt_ins, n, k, gt_num, gt_row, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_label_colors(const void* labels, int labels_are_64bit, int64_t n, const uint8_t* lut, int n_lut, uint8_t* out,
+                                   void* stream) {
+  DMN_CHECK(n >= 0 && n_lut >= 0 && (n == 0 || (labels && out)) && (n_lut == 0 || lut), "label_colors: bad argument");
+  return label_colors(labels, labels_are_64bit, n, lut, n_lut, out, (cudaStream_t)stream);
+}
+
 }  // extern "C"

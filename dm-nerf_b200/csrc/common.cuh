@@ -199,4 +199,13 @@ int mesh_clean(MeshState** s, const float* v, const float* nrm, int64_t nv, cons
 int launch_label_rays(const float* v, const float* nrm, int64_t n, float near_z, float* ro, float* rd, cudaStream_t st);
 int launch_argmax_rows(const float* x, int64_t n, int c, int64_t* out, cudaStream_t st);
 
+// Test-view evaluation (metrics.cu)
+int64_t eval_workspace_bytes(int64_t n, int k, int H, int W);
+int eval_image(const float* rgb, const float* gt, int H, int W, void* ws, dmnerf_eval_result* res, cudaStream_t st);
+int ins_eval(const float* ins, int64_t n, int k, const int32_t* gt_row, int gt_num, const float* mask, const int32_t* mask_labels,
+             int mask_below, int64_t* pred_label, void* ws, dmnerf_eval_result* res, cudaStream_t st);
+int calculate_ap(const float* iou, const float* conf, int m, int gt_number, float* ap6, cudaStream_t st);
+int ins_dense_rows(const float* gt_ins, int64_t n, int k, int gt_num, int32_t* rows, cudaStream_t st);
+int label_colors(const void* labels, int is64, int64_t n, const uint8_t* lut, int n_lut, uint8_t* out, cudaStream_t st);
+
 }  // namespace dmnerf

@@ -1,7 +1,7 @@
 """networks.evaluator (reference networks/evaluator.py): the Hungarian-matched instance loss of the training step
 (ins_criterion / hungarian) and the small loss lambdas run on the native kernels; the evaluation-time metrics (ins_eval,
-calculate_ap: CPU numpy code outside the hot path) are re-exported from the reference checkout when DMNERF_REFERENCE_ROOT
-points at one."""
+calculate_ap) are re-exported from the reference checkout when DMNERF_REFERENCE_ROOT points at one, and are the native
+device versions (dmnerf_b200.tester) otherwise."""
 import importlib.util as _ilu
 import os as _os
 
@@ -20,3 +20,4 @@ if "_mod" in globals():
     _mod.ins_criterion = ins_criterion
 else:
     from dmnerf_b200.evaluator import hungarian   # noqa: F401,E402
+    from dmnerf_b200.tester import ins_eval, calculate_ap   # noqa: F401,E402

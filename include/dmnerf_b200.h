@@ -303,6 +303,39 @@ DMNERF_API int dmnerf_mesh_label_rays(const float* verts, const float* normals, 
                                       void* stream);
 DMNERF_API int dmnerf_argmax_rows(const float* x, int64_t n, int c, int64_t* out, void* stream);
 
+/* ---- test-view evaluation: render_test, networks/tester.py (+ ins_eval / calculate_ap, networks/evaluator.py:77-175) -------
+ * Rules and deviations: DESIGN.md, "Evaluation metrics".  Every result is deterministic (fixed-order reductions, integer atomics
+ * only).  `res` is DEVICE memory; reading it back is the caller's one device->host transfer per frame.  `ws` is caller-provided
+ * device scratch of dmnerf_eval_workspace_bytes(n, k, H, W) bytes, shared by both calls (stream-ordered).
+ *
+ * dmnerf_eval_image: PSNR (skimage 0.18.3 peak_signal_noise_ratio, data_range 1: fp32 difference and square, fp64 mean) and SSIM
+ *   (structural_similarity, multichannel, data_range 1: 7x7 uniform filter in fp64, mean over the interior cropped by 3, mean of
+ *   the channels) of rgb vs gt [H,W,3] float32 -> res->psnr, res->ssim.  H and W must be >= 7.
+ * dmnerf_ins_eval: ins_eval of the instance map ins [n,k] float32 against gt ranks gt_row [n] int32 (rank in [0, gt_num), anything
+ *   else = no gt object).  Mask (crop path): a pixel is masked where mask[i] == 0 (mask: float32 [n]) or mask_labels[i] >=
+ *   mask_below (mask_labels: int32 [n]); at most one of the two is non-NULL.  Writes pred_label [n] int64 (first maximum, k where
+ *   masked) and res->ap, gt_num, pred_num, return_labels[0..gt_num), status (0 ok, 1 NaN in the instance map).
+ * dmnerf_calculate_ap: calculate_ap(ious, gt_number, confidence, 'integral') of m <= 128 matches (conf may be NULL: ordered by
+ *   IoU) -> ap6 [6] float32 (device).
+ * dmnerf_ins_dense_rows: one-hot gt_ins [n,k] float32 -> rank of the first non-zero column among the first gt_num, or -1.
+ * dmnerf_label_colors: out [n,3] uint8 = lut[labels[i]] (lut [n_lut,3] uint8, device), black outside [0, n_lut); labels int64 when
+ *   labels_are_64bit, otherwise int32. */
+typedef struct dmnerf_eval_result {
+  float ap[6];                      /* AP50, AP75, AP80, AP85, AP90, AP95 */
+  int32_t gt_num, pred_num, status, reserved;
+  double psnr, ssim;
+  int32_t return_labels[DMNERF_MAX_INS + 1];   /* matched predicted label per gt object, or -1 */
+} dmnerf_eval_result;
+DMNERF_API int64_t dmnerf_eval_workspace_bytes(int64_t n, int k, int H, int W);
+DMNERF_API int dmnerf_eval_image(const float* rgb, const float* gt, int H, int W, void* ws, dmnerf_eval_result* res, void* stream);
+DMNERF_API int dmnerf_ins_eval(const float* ins, int64_t n, int k, const int32_t* gt_row, int gt_num, const float* mask,
+                               const int32_t* mask_labels, int mask_below, int64_t* pred_label, void* ws, dmnerf_eval_result* res,
+                               void* stream);
+DMNERF_API int dmnerf_calculate_ap(const float* ious, const float* conf, int m, int gt_number, float* ap6, void* stream);
+DMNERF_API int dmnerf_ins_dense_rows(const float* gt_ins, int64_t n, int k, int gt_num, int32_t* gt_row, void* stream);
+DMNERF_API int dmnerf_label_colors(const void* labels, int labels_are_64bit, int64_t n, const uint8_t* lut, int n_lut, uint8_t* out,
+                                   void* stream);
+
 /* Number of kernels this library has launched on the calling thread's contexts since load. */
 DMNERF_API int64_t dmnerf_launch_count(void);
 
