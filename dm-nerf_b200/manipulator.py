@@ -6,17 +6,30 @@ of the edit path with the reference's names and signatures.
     manipulator_nerf(rays, position_embedder, view_embedder, model, N_samples, near, far, z_vals)   manipulator.py:108-134 (tensor-core network)
     manipulator(position_embedder, view_embedder, model_coarse, model_fine, ori_rays, f_tar_rays, args)   manipulator.py:137-205
 
-The evaluation / demo loops of the reference module (image IO, metrics) are not part of the path and are not provided.
+The two loops that drive it, with the reference's signatures, printed lines and output files (no lpips, skimage, cv2 or imageio):
+
+    manipulator_eval(position_embedder, view_embedder, model_coarse, model_fine, ori_poses, hwk, trans_dicts, save_dir, ins_rgbs,
+                     args, gt_rgbs=None, gt_labels=None)                                  manipulator.py:208-364
+    manipulator_demo(position_embedder, view_embedder, model_coarse, model_fine, ori_poses, hwk, objs_trans, save_dir, ins_rgbs,
+                     objs, view_poses, ins_map, args)                                     manipulator.py:367-491
+
+Both render through manipulate_frame (one edited frame, args.N_test rays per manipulator() call, outputs preallocated on the
+device) and keep every per-pixel step on the device: rays, metrics (dmnerf_b200.tester), label arg-max and colours.  The host
+reads back the metric result struct and the PNG images once per frame.  Rules and deviations: DESIGN.md, "Manipulation loops".
 """
 import ctypes as C
+import json
+import os
+import time
 
+import numpy as np
 import torch
 
 from . import _lib
 from .engine import get_context
 from .autograd import mlp_forward_rays
 from .render import composite, _check_embedders
-from .helpers import sample_pdf, sort_concat
+from .helpers import sample_pdf, sort_concat, get_rays_k
 
 
 def exchanger(ori_raw, tar_raws, ori_raw_pred, tar_raw_preds, move_labels):
@@ -107,3 +120,215 @@ def manipulator(position_embedder, view_embedder, model_coarse, model_fine, ori_
         ori_raw2, _, _, _ = exchanger(ori_raw2, tar_raws, ori_ins_acc, tar_accs, args.target_labels)
         final_rgb, _, _, final_ins = manipulator_render(ori_raw2, ori_z2, ori_rays[1])
     return final_rgb, final_ins, tar_rgb, tar_accs[-1]
+
+
+# ----------------------------------------------------------------------------------------------------------------- frame loops
+def manipulate_frame(H, W, K, ori_pose, tar_rays_o, tar_rays_d, position_embedder, view_embedder, model_coarse, model_fine, args,
+                     impl=_lib.IMPL_AUTO):
+    """One edited frame (the chunk loops of manipulator.py:246-269 and :445-466): manipulator() over the H*W rays of
+    get_rays_k(H, W, K, ori_pose), args.N_test rays per call with the last call partial, targets labelled args.target_labels.
+    tar_rays_o / tar_rays_d: [T, H*W, 3] CUDA rays of the T targets.  The sample_pdf draws keep the reference's order (per
+    chunk: the original rays, every target, the original rays again), so a run seeded like the reference consumes the default
+    CUDA generator identically.  Returns final rgb [H*W, 3], final ins [H*W, ins_num + 1], tar_rgb [H*W, 3] and
+    tar_ins_accum [H*W, ins_num + 1] (of the last target), written chunk by chunk into preallocated device tensors."""
+    dev = tar_rays_o.device
+    ori_o, ori_d = get_rays_k(H, W, K, torch.as_tensor(ori_pose, dtype=torch.float32, device=dev))
+    ori_o, ori_d = ori_o.reshape(-1, 3), ori_d.reshape(-1, 3)
+    n, chunk = H * W, int(args.N_test)
+    if tuple(tar_rays_o.shape[1:]) != (n, 3) or tar_rays_d.shape != tar_rays_o.shape or tar_rays_o.shape[0] < 1:
+        raise ValueError("manipulate_frame: target rays must be [T, %d, 3], got %s and %s"
+                         % (n, tuple(tar_rays_o.shape), tuple(tar_rays_d.shape)))
+    out = None
+    with torch.no_grad():
+        for step in range(0, n, chunk):
+            end = min(step + chunk, n)
+            ori = torch.stack([ori_o[step:end], ori_d[step:end]], 0)
+            tar = torch.stack([tar_rays_o[:, step:end], tar_rays_d[:, step:end]], 1)               # [T, 2, cnt, 3]
+            maps = manipulator(position_embedder, view_embedder, model_coarse, model_fine, ori, tar, args, impl=impl)
+            if out is None:
+                out = [torch.empty((n,) + tuple(m.shape[1:]), device=dev, dtype=m.dtype) for m in maps]
+            for o, m in zip(out, maps):
+                o[step:end] = m
+    return tuple(out)
+
+
+# deform_v of manipulator.py:381-382: one x amplitude per demo view of the 'sin' deformation
+_DEFORM_V = np.concatenate((np.linspace(0, 0.18, 2), np.linspace(0.18, 0, 2), np.linspace(0, -0.18, 2), np.linspace(-0.18, 0, 2)))
+DEFORM_FUNCS = ("sin", "ex", "linear", "abs_linear", "ln")
+
+
+def deform_offsets(deform_func, H, view):
+    """Per-row x offsets [H] float64 of a deformed object in demo view `view`, with the numpy expressions of
+    manipulator.py:398-426 (the reference repeats each row's value over the W columns)."""
+    v_1 = np.linspace(1, H, H)
+    if deform_func == 'sin':
+        if not 0 <= view < len(_DEFORM_V):
+            raise ValueError("manipulator_demo: the 'sin' deformation has amplitudes for %d views, view %d asked"
+                             % (len(_DEFORM_V), view))
+        return np.sin(((8 * np.pi) / 400) * v_1) * _DEFORM_V[view]
+    if deform_func == 'ex':
+        return np.exp(-1 * v_1 / 50)
+    if deform_func == 'linear':
+        return (v_1 - 200) / 215
+    if deform_func == 'abs_linear':
+        return np.abs(v_1 - 200) / 200
+    if deform_func == 'ln':
+        return np.log(v_1 / 200)
+    raise ValueError("manipulator_demo: unknown deform_func %r (one of %s)" % (deform_func, ", ".join(DEFORM_FUNCS)))
+
+
+def deformed_rays(ori_o, ori_d, offsets, H, W):
+    """Target rays of a deformed object (manipulator.py:427-429): origins [H*W, 3] shifted in x by the row's float64 offset, the
+    sum taken in float64 and rounded once to float32 like the reference's fp32 + fp64 tensor add; directions unchanged."""
+    off = torch.as_tensor(np.ascontiguousarray(offsets, dtype=np.float64)).to(ori_o.device)
+    tar_o = ori_o.clone()
+    x = tar_o.view(H, W, 3)[..., 0]
+    x.copy_(x.double() + off[:, None])
+    return tar_o, ori_d.clone()
+
+
+def rigid_rays(H, W, K, trans, pose):
+    """Target rays of a moved object: get_rays_k(trans @ pose), the product taken with torch in float32 on pose's device."""
+    t = torch.as_tensor(np.asarray(trans, dtype=np.float32) if not torch.is_tensor(trans) else trans, dtype=torch.float32,
+                        device=pose.device)
+    o, d = get_rays_k(H, W, K, t @ pose)
+    return o.reshape(-1, 3), d.reshape(-1, 3)
+
+
+def _models_device(args, model_fine, who):
+    dev = torch.device(getattr(args, "device", None) or next(model_fine.parameters()).device)
+    if dev.type != "cuda":
+        raise RuntimeError("%s: the models must be on a CUDA device (no CPU fallback)" % who)
+    return dev
+
+
+def _color_dict(args):
+    data_info = args.datadir.split('/')
+    with open('./data/color_dict.json', 'r') as fh:
+        return json.load(fh)[data_info[2]][data_info[-1]]
+
+
+def _u8(rgb):
+    """to8b (evaluator.py:14) on the device, copied to the host: (255 * clip(x, 0, 1)).astype(uint8)."""
+    return (255 * torch.clamp(rgb, 0, 1)).to(torch.uint8).cpu().numpy()
+
+
+def manipulator_eval(position_embedder, view_embedder, model_coarse, model_fine, ori_poses, hwk, trans_dicts, save_dir, ins_rgbs,
+                     args, gt_rgbs=None, gt_labels=None):
+    """networks/manipulator.py manipulator_eval: object args.target_label moved by trans_dicts['transformations'][0] in every
+    view of ori_poses.  Files in save_dir/<mode>/: {i}_rgb.png, {i}_ins.png, {i}_rgb_gt.png, {i}_ins_gt.png (the two label
+    images in the channel order cv2.imwrite stores), matching_log.json and test_results.txt (PSNR SSIM LPIPS AP50..AP95 per
+    frame, then the mean row).  Poses may be numpy arrays, CPU or CUDA tensors; gt_labels any integer type (test_dmsr.py passes
+    int8).  With gt_rgbs=None only {i}_rgb.png is written."""
+    from . import tester as T
+    from .mesh import argmax_rows
+    H, W, K = hwk
+    H, W = int(H), int(W)
+    dev = _models_device(args, model_fine, "manipulator_eval")
+    ins_num = int(args.ins_num)
+    color_dict = _color_dict(args)
+    have_gt = gt_rgbs is not None
+    if have_gt:
+        gt_img_dev = torch.as_tensor(gt_rgbs).to(dev, torch.float32).contiguous()
+        lab_cpu = torch.as_tensor(gt_labels).cpu()
+        if lab_cpu.numel() and (int(lab_cpu.min()) < 0 or int(lab_cpu.max()) >= T._MAX_LABEL):
+            raise ValueError("manipulator_eval: gt labels must be integers in [0, %d)" % T._MAX_LABEL)
+        lab_dev = lab_cpu.to(torch.int32).to(dev).reshape(lab_cpu.shape[0], -1).contiguous()
+        gt_lut = T.gt_label_lut(ins_rgbs, color_dict, int(lab_cpu.max()) + 1 if lab_cpu.numel() else 1)[:, ::-1]   # cv2: BGR
+        lpips_vgg = T._lpips_model(dev)
+        gt_row = torch.empty(H * W, device=dev, dtype=torch.int32)
+        n_valid = torch.empty(1, device=dev, dtype=torch.int32)
+    trans_dict = trans_dicts['transformations'][0]
+    trans = trans_dict['transformation']
+    save_dir = os.path.join(save_dir, trans_dict["mode"])
+    os.makedirs(save_dir, exist_ok=True)
+    args.target_labels = [args.target_label]
+    full_map, psnrs, ssims, lpipses, aps = {}, [], [], [], []
+
+    with torch.no_grad():
+        for i, ori_pose in enumerate(ori_poses):
+            pose = torch.as_tensor(ori_pose, dtype=torch.float32, device=dev)
+            tar_o, tar_d = rigid_rays(H, W, K, trans, pose)
+            rgb, ins, _, _ = manipulate_frame(H, W, K, pose, tar_o[None], tar_d[None], position_embedder, view_embedder, model_coarse,
+                                              model_fine, args)
+            rgb = rgb.reshape(H, W, 3).contiguous()
+            ins_map = {}
+            if have_gt:
+                print('=' * 50, i, '=' * 50)
+                valid_gt = torch.unique(lab_cpu[i])
+                psnr_i, ssim_i, lpips_i, ap, ins_map, _ = T._frame_metrics(
+                    "manipulator_eval", i, rgb, gt_img_dev[i], ins[:, :ins_num].contiguous(), lab_dev[i], valid_gt, ins_num,
+                    lpips_vgg, gt_row, n_valid)
+                psnrs.append(psnr_i)
+                ssims.append(ssim_i)
+                lpipses.append(lpips_i)
+                full_map[i] = ins_map
+                aps.append(ap)
+
+            T.write_png(os.path.join(save_dir, f'{i}_rgb.png'), _u8(rgb))
+            if have_gt:
+                label = argmax_rows(ins).reshape(H, W)                           # all ins_num + 1 channels
+                lut = T.pred_label_lut(ins_map, ins_rgbs, color_dict, ins.shape[1])[:, ::-1]
+                T.write_png(os.path.join(save_dir, f'{i}_ins.png'), T.colorize(label, lut).cpu().numpy())
+                T.write_png(os.path.join(save_dir, f'{i}_rgb_gt.png'), _u8(gt_img_dev[i]))
+                T.write_png(os.path.join(save_dir, f'{i}_ins_gt.png'), T.colorize(lab_dev[i].reshape(H, W), gt_lut).cpu().numpy())
+
+    if have_gt:
+        with open(os.path.join(save_dir, 'matching_log.json'), 'w') as f:
+            json.dump(full_map, f)
+        aps = np.array(aps)
+        output = np.stack([psnrs, ssims, lpipses, aps[:, 0], aps[:, 1], aps[:, 2], aps[:, 3], aps[:, 4], aps[:, 5]])
+        output = output.transpose([1, 0])
+        out_ap = np.mean(aps, axis=0)
+        mean_output = np.array([np.nanmean(psnrs), np.nanmean(ssims), np.nanmean(lpipses), out_ap[0],
+                                out_ap[1], out_ap[2], out_ap[3], out_ap[4], out_ap[5]]).reshape([1, 9])
+        output = np.concatenate([output, mean_output], 0)
+        np.savetxt(fname=os.path.join(save_dir, 'test_results.txt'), X=output, fmt='%.6f', delimiter=' ')
+        print('=' * 49, 'Avg', '=' * 49)
+        print('PSNR: {:.4f}, SSIM: {:.4f},  LPIPS: {:.4f} '.format(np.mean(psnrs), np.mean(ssims), np.mean(lpipses)))
+        print('AP50: {:.4f}, AP75: {:.4f}, AP80: {:.4f}, AP85: {:.4f}, AP90: {:.4f}, AP95: {:.4f}'
+              .format(out_ap[0], out_ap[1], out_ap[2], out_ap[3], out_ap[4], out_ap[5]))
+
+
+def manipulator_demo(position_embedder, view_embedder, model_coarse, model_fine, ori_poses, hwk, objs_trans, save_dir, ins_rgbs,
+                     objs, view_poses, ins_map, args):
+    """networks/manipulator.py manipulator_demo: every object of `objs` edited at once in every view of view_poses (ori_poses
+    is unused, as in the reference).  Rigid objects move by objs_trans[obj_name][i]['transformation']; deformed ones shift
+    the origins of the view's rays in x (deform_func sin / ex / linear / abs_linear / ln).  Files in save_dir/<args.mani_type>/:
+    {i}_rgb.png, {i}_ins.png (label colours through ins_map, cv2's channel order) and {i}_ins_pred_mask.png (the labels as
+    uint8); prints `Image{i}: <seconds>` per view."""
+    from . import tester as T
+    from .mesh import argmax_rows
+    H, W, K = hwk
+    H, W = int(H), int(W)
+    dev = _models_device(args, model_fine, "manipulator_demo")
+    color_dict = _color_dict(args)
+    save_dir = os.path.join(save_dir, args.mani_type)
+    os.makedirs(save_dir, exist_ok=True)
+    lut = T.pred_label_lut(ins_map, ins_rgbs, color_dict, int(args.ins_num) + 1)[:, ::-1]
+
+    with torch.no_grad():
+        for i, view_pose in enumerate(view_poses):
+            time_0 = time.time()
+            pose = torch.as_tensor(view_pose, dtype=torch.float32, device=dev)
+            ori_o = ori_d = None
+            tar_os, tar_ds, target_labels = [], [], []
+            for obj in objs:
+                target_labels.append(obj['tar_id'])
+                if obj['mani_mode'] == 'deform':
+                    if ori_o is None:
+                        ori_o, ori_d = (r.reshape(-1, 3) for r in get_rays_k(H, W, K, pose))
+                    o, d = deformed_rays(ori_o, ori_d, deform_offsets(obj['deform_func'], H, i), H, W)
+                else:
+                    o, d = rigid_rays(H, W, K, objs_trans[obj['obj_name']][i]['transformation'], pose)
+                tar_os.append(o)
+                tar_ds.append(d)
+            args.target_labels = target_labels
+            rgb, ins, _, _ = manipulate_frame(H, W, K, pose, torch.stack(tar_os), torch.stack(tar_ds), position_embedder,
+                                              view_embedder, model_coarse, model_fine, args)
+            label = argmax_rows(ins).reshape(H, W)
+            T.write_png(os.path.join(save_dir, f'{i}_rgb.png'), _u8(rgb.reshape(H, W, 3)))
+            T.write_png(os.path.join(save_dir, f'{i}_ins.png'), T.colorize(label, lut).cpu().numpy())
+            T.write_png(os.path.join(save_dir, f'{i}_ins_pred_mask.png'), label.to(torch.uint8).cpu().numpy())
+            time_1 = time.time()
+            print(f"Image{i}: {time_1 - time_0}")

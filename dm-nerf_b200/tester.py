@@ -256,6 +256,48 @@ def _render_frame_device(H, W, K, c2w, position_embedder, view_embedder, model_c
     return torch.cat(rgbs, 0), torch.cat(inss, 0)
 
 
+def _frame_metrics(who, i, rgb, gt_img, ins, labels, valid_gt, ins_num, lpips_vgg, gt_row, n_valid, mask_labels=None):
+    """The per-frame metric block of render_test (tester.py:86-120) and manipulator_eval (manipulator.py:276-307), with their
+    two printed lines.  rgb, gt_img [H, W, 3], ins [n, k] and labels [n] int32 on the device; valid_gt: the frame's gt object
+    ids (CPU tensor); gt_row [n] int32 and n_valid [1] int32: scratch.  PSNR and SSIM (one dmnerf_eval_image), LPIPS (NaN when
+    lpips_vgg is None) and ins_eval on the gt ranks of `labels`; mask_labels: the crop path's mask (labels >= ins_num masked).
+    One read-back.  Returns (psnr, ssim, lpips, 6 APs, ins_map {predicted label: gt id}, pred_label [n] int64 on the device).
+    A frame with no gt object gets AP 1.0, an empty map and pred_label -1."""
+    n_px = ins.shape[0]
+    dev = ins.device
+    gt_num = int(valid_gt.numel())
+    if gt_num > ins_num or valid_gt.numel() >= _RANK_SLOTS:
+        raise ValueError("%s: frame %d has %d gt objects for ins_num %d" % (who, i, gt_num, ins_num))
+    ctx = get_context(dev)
+    res = _result_buffer(dev)
+    _image_into(rgb, gt_img, res)
+    lpips_i = float("nan")
+    if lpips_vgg is not None:
+        lpips_i = lpips_vgg(rgb.permute(2, 0, 1).unsqueeze(0), gt_img.permute(2, 0, 1).unsqueeze(0)).item()
+    if gt_num > 0:
+        _lib.check(ctx.lib.dmnerf_ins_label_rows(_vp(labels), n_px, _RANK_SLOTS, _vp(gt_row), _vp(n_valid), ctx.stream()),
+                   "dmnerf_ins_label_rows")
+        pred_label = _ins_eval_rows(ins, gt_row, gt_num, res, mask_labels=mask_labels, mask_below=ins_num)
+    r = _read_result(res)
+    if gt_num > 0:
+        _check_status(r)
+        ap = [float(v) for v in r.ap]
+        matched = list(r.return_labels[:gt_num])
+    else:                                                                 # no gt object: AP 1.0, labels -1
+        ap = [1.0] * 6
+        matched = []
+        pred_label = torch.full((n_px,), -1, device=dev, dtype=torch.int64)
+    psnr_i, ssim_i = float(r.psnr), float(r.ssim)
+    print(f"PSNR: {psnr_i} SSIM: {ssim_i} LPIPS: {lpips_i}")
+    gt_np = valid_gt.numpy()
+    ins_map = {}
+    for idx, lab in enumerate(matched):
+        if lab != -1:
+            ins_map[str(lab)] = int(gt_np[idx])
+    print(f"APs: {ap}")
+    return psnr_i, ssim_i, lpips_i, ap, ins_map, pred_label
+
+
 def render_test(position_embedder, view_embedder, model_coarse, model_fine, render_poses, hwk, args, gt_imgs=None, gt_labels=None,
                 ins_rgbs=None, savedir=None, matched_file=None, crop_mask=None):
     """networks/tester.py render_test, same signature, printed lines and files in `savedir`:
@@ -302,7 +344,6 @@ def render_test(position_embedder, view_embedder, model_coarse, model_fine, rend
     gt_lut = None
     if have_gt and savedir is not None:
         gt_lut = gt_label_lut(ins_rgbs, color_dict, int(lab_cpu.max()) + 1 if lab_cpu.numel() else 1)[:, ::-1]   # cv2: BGR
-    ctx = get_context(dev)
     gt_row = torch.empty(n_px, device=dev, dtype=torch.int32)
     n_valid = torch.empty(1, device=dev, dtype=torch.int32)
 
@@ -321,40 +362,14 @@ def render_test(position_embedder, view_embedder, model_coarse, model_fine, rend
                 valid_gt = torch.unique(gt_label)
                 if crop_idx is not None:
                     valid_gt = valid_gt[:-1]                                          # tester.py:99
-                gt_num = int(valid_gt.numel())
-                if gt_num > ins_num or valid_gt.numel() >= _RANK_SLOTS:
-                    raise ValueError("render_test: frame %d has %d gt objects for ins_num %d" % (i, gt_num, ins_num))
-                res = _result_buffer(dev)
-                _image_into(rgb, gt_img_dev[i], res)
-                lpips_i = float("nan")
-                if lpips_vgg is not None:
-                    lpips_i = lpips_vgg(rgb.permute(2, 0, 1).unsqueeze(0), gt_img_dev[i].permute(2, 0, 1).unsqueeze(0)).item()
-                if gt_num > 0:
-                    _lib.check(ctx.lib.dmnerf_ins_label_rows(_vp(lab_dev[i]), n_px, _RANK_SLOTS, _vp(gt_row), _vp(n_valid),
-                                                             ctx.stream()), "dmnerf_ins_label_rows")
-                    pred_label = _ins_eval_rows(ins, gt_row, gt_num, res, mask_labels=lab_dev[i] if crop_idx is not None else None,
-                                                mask_below=ins_num)
-                r = _read_result(res)
-                if gt_num > 0:
-                    _check_status(r)
-                    ap = [float(v) for v in r.ap]
-                    matched = list(r.return_labels[:gt_num])
-                else:                                                                 # no gt object: AP 1.0, labels -1
-                    ap = [1.0] * 6
-                    matched = []
-                    pred_label = torch.full((n_px,), -1, device=dev, dtype=torch.int64)
-                psnr_i, ssim_i = float(r.psnr), float(r.ssim)
+                psnr_i, ssim_i, lpips_i, ap, ins_map, pred_label = _frame_metrics(
+                    "render_test", i, rgb, gt_img_dev[i], ins, lab_dev[i], valid_gt, ins_num, lpips_vgg, gt_row, n_valid,
+                    mask_labels=lab_dev[i] if crop_idx is not None else None)
                 psnrs.append(psnr_i)
                 ssims.append(ssim_i)
                 lpipses.append(lpips_i)
-                print(f"PSNR: {psnr_i} SSIM: {ssim_i} LPIPS: {lpips_i}")
-                gt_np = valid_gt.numpy()
-                for idx, lab in enumerate(matched):
-                    if lab != -1:
-                        ins_map[str(lab)] = int(gt_np[idx])
                 full_map[i] = ins_map
                 aps.append(ap)
-                print(f"APs: {ap}")
 
             if savedir is not None:
                 rgb8 = (255 * np.clip(rgb.cpu().numpy(), 0, 1)).astype(np.uint8)      # to8b
