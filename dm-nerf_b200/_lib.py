@@ -110,6 +110,15 @@ PROTOTYPES = {
     "dmnerf_calculate_ap": (C.c_int, [_f32p, _f32p, C.c_int, C.c_int, _f32p, C.c_void_p]),
     "dmnerf_ins_dense_rows": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "dmnerf_label_colors": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "dmnerf_composite_objects": (C.c_int, [_f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint32), _f32p,
+                                           _f32p, _f32p, _f32p, _f32p, C.c_void_p]),
+    "dmnerf_render_forward_objects": (C.c_int, [C.c_void_p, C.POINTER(RenderIO), C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                C.POINTER(C.c_uint32), C.c_void_p]),
+    "dmnerf_render_frame_objects_host": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int, C.c_int, C.c_float,
+                                                   C.c_float, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                   C.POINTER(C.c_uint32), C.POINTER(RenderIO), C.c_void_p]),
+    "dmnerf_mesh_occupancy_objects": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_float,
+                                                C.c_int64, C.POINTER(C.c_uint32), _f32p, C.c_void_p, C.c_void_p]),
 }
 
 

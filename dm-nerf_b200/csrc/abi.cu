@@ -39,6 +39,15 @@ struct Scratch {
   void release() { if (ptr) cudaFree(ptr); ptr = nullptr; cap = 0; }
 };
 
+// A host-side object selection mask (4 words) -> ObjMask; only labels 0 .. n_labels - 1 may be set.
+static int object_mask(const uint32_t* keep_host, int n_labels, ObjMask& m, const char* who) {
+  DMN_CHECK(keep_host != nullptr, "%s: the object mask is NULL (pass 4 words)", who);
+  for (int b = n_labels; b < 128; ++b)
+    DMN_CHECK(!((keep_host[b >> 5] >> (b & 31)) & 1u), "%s: object mask keeps label %d, outside [0, %d]", who, b, n_labels - 1);
+  for (int i = 0; i < 4; ++i) m.w[i] = keep_host[i];
+  return 0;
+}
+
 }  // namespace dmnerf
 
 using namespace dmnerf;
@@ -171,6 +180,17 @@ DMNERF_API int dmnerf_composite(const float* raw, const float* z, const float* r
   DMN_CHECK(n >= 0, "composite: negative ray count");
   DMN_CHECK(n == 0 || (raw && z && rays_d), "composite: NULL input");
   return launch_composite(raw, z, rays_d, n, s, c, keep_all_ins, rgb, weights, depth, ins, acc, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_composite_objects(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c,
+                                        int keep_all_ins, const uint32_t* keep_host, float* rgb, float* weights, float* depth,
+                                        float* ins, float* acc, void* stream) {
+  DMN_CHECK(n >= 0, "composite_objects: negative ray count");
+  DMN_CHECK(n == 0 || (raw && z && rays_d), "composite_objects: NULL input");
+  DMN_CHECK(c >= 5 && c <= 4 + DMNERF_MAX_INS + 1, "composite_objects: channels=%d out of range", c);
+  ObjMask m;
+  if (object_mask(keep_host, c - 4, m, "composite_objects")) return 1;
+  return launch_composite(raw, z, rays_d, n, s, c, keep_all_ins, rgb, weights, depth, ins, acc, (cudaStream_t)stream, &m);
 }
 
 DMNERF_API int dmnerf_sample_pdf(const float* bins, const float* weights, int64_t n, int n_bins, int n_samples, const float* u,
@@ -319,8 +339,11 @@ DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, 
                                    (cudaStream_t)stream);
 }
 
-DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
-                          void* stream) {
+}  // extern "C"
+
+// dm_nerf() on device buffers; keep: object selection (NULL = none, the unselected kernels)
+static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                               const ObjMask* keep, void* stream) {
   DMN_CHECK(ctx && io, "render_forward: NULL ctx/io");
   DMN_CHECK(n >= 0 && S >= 3 && NI >= 2, "render_forward: bad sizes n=%lld S=%d I=%d", (long long)n, S, NI);
   DMN_CHECK(ctx->net[0].bound && ctx->net[1].bound, "render_forward: bind both networks with dmnerf_set_weights first");
@@ -332,7 +355,7 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
   DMN_CHECK(io->z_row_stride == 0 || io->z_row_stride >= S, "render_forward: bad z_row_stride");
   cudaStream_t st = (cudaStream_t)stream;
   const int C = 4 + ctx->net[0].ins_num + 1, F = S + NI;
-  const int keep = (flags & DMNERF_FLAG_KEEP_INS) ? 1 : 0;
+  const int keep_ins = (flags & DMNERF_FLAG_KEEP_INS) ? 1 : 0;
   DMN_CUDA(cudaSetDevice(ctx->device));
 
   // ---- fully fused path: one launch, no intermediate tensor in HBM
@@ -341,7 +364,7 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
   if (can_fuse) {
     const bool prof = ctx->profiling;
     if (prof) DMN_CUDA(cudaEventRecord(ctx->ev[0], st));
-    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st);
+    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep);
     if (rc) return rc;
     if (prof) for (int i = 1; i <= DMNERF_N_STAGES; ++i) DMN_CUDA(cudaEventRecord(ctx->ev[i], st));
     ctx->profile_valid = prof;
@@ -374,8 +397,8 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
   if ((rc = mlp_dispatch(ctx, 0, nullptr, io->rays_o, io->rays_d, z_c, n * S, S, raw_c, impl, st))) return rc;
   DMN_STAGE_MARK();
   // render.py:63     coarse composite
-  if ((rc = launch_composite(raw_c, z_c, io->rays_d, n, S, C, keep, io->rgb_coarse, w_c, io->depth_coarse,
-                             io->ins_coarse, io->acc_coarse, st))) return rc;
+  if ((rc = launch_composite(raw_c, z_c, io->rays_d, n, S, C, keep_ins, io->rgb_coarse, w_c, io->depth_coarse,
+                             io->ins_coarse, io->acc_coarse, st, keep))) return rc;
   DMN_STAGE_MARK();
   // render.py:66-70  importance sampling + merge
   if ((rc = launch_hier_sample(z_c, w_c, perturb ? io->u : nullptr, n, S, NI, z_f, st))) return rc;
@@ -384,12 +407,34 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
   if ((rc = mlp_dispatch(ctx, 1, nullptr, io->rays_o, io->rays_d, z_f, n * F, F, raw_f, impl, st))) return rc;
   DMN_STAGE_MARK();
   // render.py:86     fine composite
-  if ((rc = launch_composite(raw_f, z_f, io->rays_d, n, F, C, keep, io->rgb_fine, io->weights_fine, io->depth_fine,
-                             io->ins_fine, io->acc_fine, st))) return rc;
+  if ((rc = launch_composite(raw_f, z_f, io->rays_d, n, F, C, keep_ins, io->rgb_fine, io->weights_fine, io->depth_fine,
+                             io->ins_fine, io->acc_fine, st, keep))) return rc;
   DMN_STAGE_MARK();
 #undef DMN_STAGE_MARK
   ctx->profile_valid = prof;
   return 0;
+}
+
+// Both networks bound with the same ins_num, and a valid mask for them.
+static int render_object_mask(const dmnerf_ctx* ctx, const uint32_t* keep_host, ObjMask& m, const char* who) {
+  DMN_CHECK(ctx != nullptr, "%s: ctx is NULL", who);
+  DMN_CHECK(ctx->net[0].bound && ctx->net[1].bound, "%s: bind both networks with dmnerf_set_weights first", who);
+  DMN_CHECK(ctx->net[0].ins_num == ctx->net[1].ins_num, "%s: coarse/fine ins_num differ", who);
+  return object_mask(keep_host, ctx->net[0].ins_num + 1, m, who);
+}
+
+extern "C" {
+
+DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                          void* stream) {
+  return render_forward_impl(ctx, io, n, S, NI, flags, impl, nullptr, stream);
+}
+
+DMNERF_API int dmnerf_render_forward_objects(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                             const uint32_t* keep_host, void* stream) {
+  ObjMask m;
+  if (render_object_mask(ctx, keep_host, m, "render_forward_objects")) return 1;
+  return render_forward_impl(ctx, io, n, S, NI, flags, impl, &m, stream);
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
@@ -428,7 +473,7 @@ DMNERF_API int dmnerf_profile_read(dmnerf_ctx* ctx, float* ms_out, int n_out) {
 // Host-buffer render: `h` holds HOST pointers for the outputs (and for the inputs unless dev_rays_o / dev_rays_d are given:
 // rays that are already resident on the device, e.g. generated there from the camera).
 static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const float* dev_rays_o, const float* dev_rays_d, int64_t n,
-                            int S, int NI, int flags, int impl, void* stream) {
+                            int S, int NI, int flags, int impl, const ObjMask* keep, void* stream) {
   DMN_CHECK(ctx && h, "render_forward_host: NULL ctx/io");
   DMN_CHECK(n >= 0, "render_forward_host: negative ray count");
   if (n == 0) return 0;
@@ -518,7 +563,7 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
   const bool parts = n >= HOST_PART_MIN_RAYS && !ctx->profiling;
   if (!parts) {
     if (copy_in(0, n, st)) return 1;
-    int rc = dmnerf_render_forward(ctx, &io, n, S, NI, flags, impl, stream);
+    int rc = render_forward_impl(ctx, &io, n, S, NI, flags, impl, keep, stream);
     if (rc) return rc;
     if (copy_out(0, n, st)) return 1;
     return dmnerf_sync_check(ctx, stream);
@@ -548,7 +593,7 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
   for (int i = 0; i < HOST_PARTS && !rc; ++i) {
     if (i > 0) DMN_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[i], 0));
     const dmnerf_render_io pi = part_io(edge[i]);
-    rc = dmnerf_render_forward(ctx, &pi, edge[i + 1] - edge[i], S, NI, flags, impl, stream);
+    rc = render_forward_impl(ctx, &pi, edge[i + 1] - edge[i], S, NI, flags, impl, keep, stream);
     if (rc) break;
     DMN_CUDA(cudaEventRecord(ctx->ev_done[i], st));
     DMN_CUDA(cudaStreamWaitEvent(cs, ctx->ev_done[i], 0));
@@ -564,12 +609,14 @@ extern "C" {
 
 DMNERF_API int dmnerf_render_forward_host(dmnerf_ctx* ctx, const dmnerf_render_io* h, int64_t n, int S, int NI, int flags,
                                int impl, void* stream) {
-  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, stream);
+  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, nullptr, stream);
 }
 
-DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
-                                        float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
-                                        int flags, int impl, const dmnerf_render_io* out_host, void* stream) {
+}  // extern "C"
+
+static int render_frame_impl(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z, float far_z,
+                             int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance, int flags, int impl,
+                             const dmnerf_render_io* out_host, const ObjMask* keep, void* stream) {
   DMN_CHECK(ctx && K_host && c2w_host && out_host, "render_frame_host: NULL argument");
   DMN_CHECK(H > 0 && W > 0 && n_coarse >= 3 && n_coarse <= 4096, "render_frame_host: bad sizes H=%d W=%d S=%d", H, W, n_coarse);
   DMN_CHECK(ray_begin >= 0 && ray_count >= 0 && ray_begin + ray_count <= (int64_t)H * W,
@@ -593,7 +640,26 @@ DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, co
   dmnerf_render_io h = *out_host;
   h.rays_o = nullptr; h.rays_d = nullptr; h.t_rand = nullptr; h.u = nullptr;
   h.z_coarse = z.data(); h.z_row_stride = 0;
-  return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, stream);
+  return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, keep, stream);
+}
+
+extern "C" {
+
+DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
+                                        float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
+                                        int flags, int impl, const dmnerf_render_io* out_host, void* stream) {
+  return render_frame_impl(ctx, K_host, c2w_host, H, W, near_z, far_z, ray_begin, ray_count, n_coarse, n_importance, flags, impl,
+                           out_host, nullptr, stream);
+}
+
+DMNERF_API int dmnerf_render_frame_objects_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
+                                                float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
+                                                int flags, int impl, const uint32_t* keep_host, const dmnerf_render_io* out_host,
+                                                void* stream) {
+  ObjMask m;
+  if (render_object_mask(ctx, keep_host, m, "render_frame_objects_host")) return 1;
+  return render_frame_impl(ctx, K_host, c2w_host, H, W, near_z, far_z, ray_begin, ray_count, n_coarse, n_importance, flags, impl,
+                           out_host, &m, stream);
 }
 
 // ---- mesh extraction (tools/mesh_generator.py mesh_main) ------------------------------------------------------------------
@@ -604,8 +670,11 @@ DMNERF_API int dmnerf_mesh_grid_points(const double* transform_host, const doubl
   return launch_grid_points(transform_host, extents_host, dim, begin, count, pts, (cudaStream_t)stream);
 }
 
-DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
-                                     float voxel, int64_t slab, float* occ, void* stream) {
+}  // extern "C"
+
+// The occupancy sweep; keep != NULL: with the object selection (and the per-point labels when labels != NULL)
+static int mesh_occupancy_impl(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim, float voxel,
+                               int64_t slab, const ObjMask* keep, float* occ, int16_t* labels, void* stream) {
   DMN_CHECK(ctx && (net == 0 || net == 1), "mesh_occupancy: bad ctx / net");
   DMN_CHECK(transform_host && extents_host && occ, "mesh_occupancy: NULL argument");
   DMN_CHECK(dim >= 2 && dim <= 2048, "mesh_occupancy: dim %d out of range [2, 2048]", dim);
@@ -626,10 +695,28 @@ DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* tra
     const int64_t cnt = n - b < slab ? n - b : slab;
     int rc = launch_grid_points(transform_host, extents_host, dim, b, cnt, pts, st);
     if (!rc) rc = launch_mlp_umma(ctx->packed[net], ctx->net[net], nullptr, pts, dirs, nullptr, cnt, 1, raw, nullptr, st);
-    if (!rc) rc = launch_occupancy(raw, cnt, C, voxel, occ + b, st);
+    if (!rc) rc = keep ? launch_occupancy_objects(raw, cnt, C, voxel, *keep, occ + b, labels ? labels + b : nullptr, st)
+                       : launch_occupancy(raw, cnt, C, voxel, occ + b, st);
     if (rc) return rc;
   }
   return 0;
+}
+
+extern "C" {
+
+DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
+                                     float voxel, int64_t slab, float* occ, void* stream) {
+  return mesh_occupancy_impl(ctx, net, transform_host, extents_host, dim, voxel, slab, nullptr, occ, nullptr, stream);
+}
+
+DMNERF_API int dmnerf_mesh_occupancy_objects(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
+                                             float voxel, int64_t slab, const uint32_t* keep_host, float* occ, int16_t* labels,
+                                             void* stream) {
+  DMN_CHECK(ctx && (net == 0 || net == 1), "mesh_occupancy_objects: bad ctx / net");
+  DMN_CHECK(ctx->net[net].bound, "mesh_occupancy_objects: bind the network with dmnerf_set_weights first");
+  ObjMask m;
+  if (object_mask(keep_host, ctx->net[net].ins_num + 1, m, "mesh_occupancy_objects")) return 1;
+  return mesh_occupancy_impl(ctx, net, transform_host, extents_host, dim, voxel, slab, &m, occ, labels, stream);
 }
 
 DMNERF_API int dmnerf_mesh_mc_count(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, int64_t* counts_host,

@@ -112,10 +112,22 @@ extern std::atomic<int64_t> g_launches;
     DMN_CUDA(cudaGetLastError());                           \
   } while (0)
 
+// Object selection (DESIGN.md, "Object selection"): the set of kept labels 0 .. ins_num as a 128-bit mask, bit k of word
+// k / 32.  A sample whose arg-max label (argmax_sigmoid, ray_ops.cuh) is not kept has alpha = 0 in the composite.
+struct ObjMask {
+  uint32_t w[4];
+};
+__host__ __device__ inline bool obj_kept(const ObjMask& m, int label) {
+  const uint32_t word = label < 64 ? (label < 32 ? m.w[0] : m.w[1]) : (label < 96 ? m.w[2] : m.w[3]);   // no dynamic indexing
+  return (word >> (label & 31)) & 1u;
+}
+
 // ---- launchers implemented in the individual .cu files (all return 0 / non-zero status) ----
 int launch_posenc(const float* x, int64_t m, int n_freqs, float* out, cudaStream_t st);
+// keep: object selection, or NULL for none (the unselected kernel)
 int launch_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all,
-                     float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st);
+                     float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st,
+                     const ObjMask* keep = nullptr);
 int launch_sample_pdf(const float* bins, const float* weights, int64_t n, int nb, int ns, const float* u, float* out,
                       cudaStream_t st);
 int launch_sort_concat(const float* a, const float* b, int64_t n, int na, int nb, float* out, cudaStream_t st);
@@ -189,6 +201,9 @@ struct MeshState;                 // per-context device buffers of the mesh entr
 void mesh_state_free(MeshState* s);
 int launch_grid_points(const double* T16, const double* ext3, int dim, int64_t begin, int64_t count, float* pts, cudaStream_t st);
 int launch_occupancy(const float* raw, int64_t n, int c, float voxel, float* occ, cudaStream_t st);
+// the same with an object selection: occ = 0 where the point's label is not kept; labels [n] int16 (may be NULL)
+int launch_occupancy_objects(const float* raw, int64_t n, int c, float voxel, const ObjMask& keep, float* occ, int16_t* labels,
+                             cudaStream_t st);
 int mc_count(MeshState** s, const float* grid, int nx, int ny, int nz, float level, int64_t* counts, cudaStream_t st);
 int mc_emit(MeshState* s, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris, cudaStream_t st);
 int launch_to_scene(const float* v, int64_t n, const double* T16, const double* ext3, int dim, float* out, cudaStream_t st);

@@ -25,17 +25,6 @@ struct ExchangeArgs {
   int64_t* tar_label;                    // [N,S] out: per-sample label of the LAST target (after its occlusion fix)
 };
 
-// torch.argmax(torch.sigmoid(v[0:n])): first maximum wins (manipulator.py:19-25, 45-53).
-__device__ __forceinline__ int argmax_sigmoid(const float* __restrict__ v, int n) {
-  int best = 0;
-  float bv = sigmoidf_acc(v[0]);
-  for (int k = 1; k < n; ++k) {
-    const float x = sigmoidf_acc(v[k]);
-    if (x > bv) { bv = x; best = k; }
-  }
-  return best;
-}
-
 __global__ void exchanger_kernel(const ExchangeArgs a) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= a.total) return;

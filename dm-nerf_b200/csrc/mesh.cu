@@ -4,6 +4,7 @@
 #include <cub/cub.cuh>
 
 #include "common.cuh"
+#include "ray_ops.cuh"
 
 namespace dmnerf {
 
@@ -217,6 +218,28 @@ __global__ void occupancy_kernel(const float* __restrict__ raw, int64_t n, int c
 int launch_occupancy(const float* raw, int64_t n, int c, float voxel, float* occ, cudaStream_t st) {
   if (n == 0) return 0;
   occupancy_kernel<<<blocks(n, 256), 256, 0, st>>>(raw, n, c, voxel, occ);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+// The same occupancy with an object selection: the point's label is argmax_sigmoid of its c - 4 instance logits (the rule of
+// the selected composites), occ = 0 where that label is not kept; labels (optional) receives the label of every point.
+__global__ void occupancy_objects_kernel(const float* __restrict__ raw, int64_t n, int c, float voxel, const ObjMask keep,
+                                         float* __restrict__ occ, int16_t* __restrict__ labels) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float* ri = raw + i * c;
+  const int label = argmax_sigmoid(ri + 4, c - 4);
+  const float a = ri[3];
+  const float r = a > 0.f ? a : (a != a ? a : 0.f);
+  occ[i] = obj_kept(keep, label) ? __fsub_rn(1.0f, expf(__fmul_rn(-r, voxel))) : 0.0f;
+  if (labels) labels[i] = (int16_t)label;
+}
+
+int launch_occupancy_objects(const float* raw, int64_t n, int c, float voxel, const ObjMask& keep, float* occ, int16_t* labels,
+                             cudaStream_t st) {
+  if (n == 0) return 0;
+  occupancy_objects_kernel<<<blocks(n, 256), 256, 0, st>>>(raw, n, c, voxel, keep, occ, labels);
   DMN_LAUNCH_OK();
   return 0;
 }

@@ -83,6 +83,7 @@ struct KArgs {
   float* out;                  // [M, C]
   float* acts;                 // training forward (RAW mode): ActPlanes base, or nullptr
   int32_t* status;             // device error word
+  ObjMask keep;                // render_objects_kernel: kept object labels
 };
 
 // ------------------------------------------------------------------------------------------------ prologue helpers
@@ -141,8 +142,10 @@ __device__ __forceinline__ void fill_embedding(const float v[3], float* vals /* 
 
 // ------------------------------------------------------------------------------------------------ the kernel
 // Warps 0-7: two consumer warpgroups (MMA issue, epilogues, prologue); warp 8: weight producer.
-template <bool FUSED>
-__global__ void __launch_bounds__(N_THREADS, 1) mlp_umma_kernel(const __grid_constant__ Program prog, const KArgs a) {
+// SELECT (fused only): object selection -- samples whose label is not in a.keep get alpha = 0 in both composites.  The body is
+// shared by mlp_umma_kernel (no selection) and render_objects_kernel (FUSED + SELECT) below.
+template <bool FUSED, bool SELECT>
+__device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& a) {
   // The kernel has no static shared memory, so the dynamic block starts at offset 0 of the CTA's shared window and
   // is 1024-aligned by construction (checked below).
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -542,7 +545,12 @@ __global__ void __launch_bounds__(N_THREADS, 1) mlp_umma_kernel(const __grid_con
         const float zi = zs[si];
         float dist = (si == S - 1) ? 1e10f : __fsub_rn(zs[si + 1], zi);
         dist = __fmul_rn(dist, fz->ray[rl][6]);
-        const float alpha = __fsub_rn(1.0f, expf(-__fmul_rn(fmaxf(rv.w, 0.0f), dist)));
+        float alpha = __fsub_rn(1.0f, expf(-__fmul_rn(fmaxf(rv.w, 0.0f), dist)));
+        if constexpr (SELECT) {
+          // the row's label from its logits (128 floats apart per row, i.e. one bank): each lane starts its walk at channel
+          // lane mod n, so the 32 rows of a warp read ceil(32 / n) rows per bank below 32 channels and at most 2 above
+          if (!obj_kept(a.keep, argmax_sigmoid(logit + r * 128, n_ins1, (r & 31) % n_ins1))) alpha = 0.0f;
+        }
         const float f = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
         const int lane_i = r & 31, wi = r >> 5;
         const float incl = warp_scan_mul(f, lane_i);
@@ -631,6 +639,17 @@ __global__ void __launch_bounds__(N_THREADS, 1) mlp_umma_kernel(const __grid_con
       all_sync();                        // the logits region is free again; fine depths visible to the next prologue
     }
   }
+}
+
+template <bool FUSED>
+__global__ void __launch_bounds__(N_THREADS, 1) mlp_umma_kernel(const __grid_constant__ Program prog, const __grid_constant__ KArgs a) {
+  mlp_umma_body<FUSED, false>(prog, a);
+}
+
+// The fused render kernel with an object selection (a.keep): a kernel of its own, so that the unselected one carries no branch.
+__global__ void __launch_bounds__(N_THREADS, 1) render_objects_kernel(const __grid_constant__ Program prog,
+                                                                      const __grid_constant__ KArgs a) {
+  mlp_umma_body<true, true>(prog, a);
 }
 
 // ------------------------------------------------------------------------------------------------ host: program
@@ -873,7 +892,7 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
 // Whole dm_nerf() pipeline (render.py:31-96) in ONE launch: coarse network -> composite -> importance sampling -> fine
 // network -> composite, per pair of rays, nothing but rays in and per-ray maps out crossing HBM.  64 + 128 samples only.
 int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmnerf_render_io* io, int64_t n, int flags,
-                       cudaStream_t st) {
+                       cudaStream_t st, const ObjMask* keep) {
   using namespace uk;
   DMN_CHECK(wc.ready && wf.ready && wc.extra && wf.extra, "render(umma): weights not packed");
   DMN_CHECK(wc.ins_num == wf.ins_num, "render(umma): coarse/fine ins_num differ");
@@ -881,9 +900,12 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
             "results are invalid -- destroy the context", umma_status_peek(wc));
   if (n == 0) return 0;
   UmmaExtra* ex = extra_of(wc);
-  static PerDeviceOnce attr_once;
-  if (attr_once.first()) {
+  static PerDeviceOnce attr_once, attr_once_sel;
+  if (!keep && attr_once.first()) {
     DMN_CUDA(cudaFuncSetAttribute(mlp_umma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  }
+  if (keep && attr_once_sel.first()) {
+    DMN_CUDA(cudaFuncSetAttribute(render_objects_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   }
   int dev = 0, sms = 0;
   DMN_CUDA(cudaGetDevice(&dev));
@@ -903,7 +925,12 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   a.status = ex->d_status;
   const int64_t units = (n + 1) / 2;
   const unsigned grid = (unsigned)(units < sms ? units : sms);
-  mlp_umma_kernel<true><<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog, a);
+  if (keep) {
+    a.keep = *keep;
+    render_objects_kernel<<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog, a);
+  } else {
+    mlp_umma_kernel<true><<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog, a);
+  }
   DMN_LAUNCH_OK();
   return 0;
 }

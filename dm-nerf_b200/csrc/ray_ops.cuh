@@ -11,6 +11,22 @@ constexpr unsigned FULL = 0xffffffffu;
 
 __device__ __forceinline__ float sigmoidf_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// The per-sample object label: torch.argmax(torch.sigmoid(v[0:n])), first maximum wins (manipulator.py:19-25, 45-53).  The one
+// label rule of the library: the exchanger, the object-selected composites and the selected occupancy sweep all call this, so
+// ties from fp32 saturation of the sigmoid resolve the same way everywhere.  `start`: the channel the walk begins at, wrapping
+// around (the fused kernel staggers it across the lanes of a warp to spread shared-memory banks); the result does not depend on
+// it for NaN-free logits: the largest sigmoid wins, the lowest channel among equal ones.
+__device__ __forceinline__ int argmax_sigmoid(const float* __restrict__ v, int n, int start = 0) {
+  int best = start, k = start;
+  float bv = sigmoidf_acc(v[start]);
+  for (int i = 1; i < n; ++i) {
+    if (++k == n) k = 0;
+    const float x = sigmoidf_acc(v[k]);
+    if (x > bv || (x == bv && k < best)) { bv = x; best = k; }
+  }
+  return best;
+}
+
 // [x, sin(2^k x), cos(2^k x)]_k for one 3-vector; out has 3 + 6*L entries (networks/dm_nerf.py:37-38).
 __device__ __forceinline__ void posenc_one_freq(const float v[3], int k, float* out /* 6 */) {
   const float f = (float)(1 << k);

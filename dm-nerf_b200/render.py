@@ -21,7 +21,9 @@ def render_train(raw, z_vals, rays_d, keep_all_ins=False):
     return rgb, w, depth, ins
 
 
-def composite(raw, z_vals, rays_d, keep_all_ins=False):
+def composite(raw, z_vals, rays_d, keep_all_ins=False, keep_objects=None):
+    """Inference composite -> (rgb, weights, depth, ins, acc).  keep_objects: object selection (labels in [0, C - 5]) as in
+    render_rays: samples labelled otherwise enter with alpha = 0."""
     if not raw.is_cuda:
         raise RuntimeError("render_train: expected CUDA tensors (no CPU fallback)")
     n, s, c = raw.shape
@@ -32,10 +34,21 @@ def composite(raw, z_vals, rays_d, keep_all_ins=False):
     depth = torch.empty((n,), device=dev); acc = torch.empty((n,), device=dev)
     ins = torch.empty((n, n_ins), device=dev)
     ctx = get_context(dev)
-    _lib.check(ctx.lib.dmnerf_composite(_lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins),
-                                        _lib.ptr(rgb), _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc),
-                                        ctx.stream()), "dmnerf_composite")
+    if keep_objects is None:
+        _lib.check(ctx.lib.dmnerf_composite(_lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins),
+                                            _lib.ptr(rgb), _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc),
+                                            ctx.stream()), "dmnerf_composite")
+    else:
+        from .objects import object_mask
+        keep = (C.c_uint32 * 4)(*object_mask(c - 5, keep=keep_objects))
+        _lib.check(ctx.lib.dmnerf_composite_objects(_lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins), keep,
+                                                    _lib.ptr(rgb), _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc),
+                                                    ctx.stream()), "dmnerf_composite_objects")
     return rgb, w, depth, ins, acc
+
+
+def _keep_arg(words):
+    return (C.c_uint32 * 4)(*words)
 
 
 def _check_embedders(position_embedder, view_embedder):
@@ -48,11 +61,13 @@ def _check_embedders(position_embedder, view_embedder):
 
 def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb=0.0, N_importance=128,
                 t_rand=None, u=None, want_raw=True, want_coarse=True, want_samples=None, keep_all_ins=False,
-                impl=_lib.IMPL_AUTO):
+                impl=_lib.IMPL_AUTO, keep_objects=None):
     """Whole per-ray pipeline on the device.  Returns the reference's dict keys plus acc / weights maps.
     want_raw: per-sample network outputs raw_* (forces the stage-by-stage kernels); want_samples: per-sample depths and
     weights (z_vals_*, weights_*; default = want_raw); want_coarse: the coarse pass' maps.  With want_raw=False and
-    64 + 128 samples the whole call is ONE kernel and only the requested per-ray maps are written."""
+    64 + 128 samples the whole call is ONE kernel and only the requested per-ray maps are written.
+    keep_objects: an iterable of object labels in [0, ins_num]; samples labelled otherwise get alpha = 0 in both passes
+    (DESIGN.md, "Object selection").  raw_* stay the network's output.  Inference only."""
     if want_samples is None:
         want_samples = want_raw
     dev = rays_o.device
@@ -62,6 +77,14 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     ins_num = ctx.bind(0, model_coarse)
     if ctx.bind(1, model_fine) != ins_num:
         raise RuntimeError("coarse and fine networks disagree on ins_num")
+    keep = None
+    if keep_objects is not None:
+        from .autograd import _needs_grad
+        from .objects import object_mask
+        if _needs_grad(model_coarse, model_fine):
+            raise RuntimeError("render_rays: object selection is inference-only; call it under torch.no_grad() or with "
+                               "parameters that do not require grad")
+        keep = object_mask(ins_num, keep=keep_objects)
     rays_o = rays_o.reshape(-1, 3).contiguous().float()
     rays_d = rays_d.reshape(-1, 3).contiguous().float()
     n = rays_o.shape[0]
@@ -104,8 +127,12 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     io.t_rand, io.u = (_lib.ptr(t_rand), _lib.ptr(u)) if perturb > 0.0 else (None, None)
     for k, v in out.items():
         setattr(io, k, _lib.ptr(v))
-    _lib.check(ctx.lib.dmnerf_render_forward(ctx.handle, io, n, S, N_importance, flags, impl, ctx.stream()),
-               "dmnerf_render_forward")
+    if keep is None:
+        _lib.check(ctx.lib.dmnerf_render_forward(ctx.handle, io, n, S, N_importance, flags, impl, ctx.stream()),
+                   "dmnerf_render_forward")
+    else:
+        _lib.check(ctx.lib.dmnerf_render_forward_objects(ctx.handle, io, n, S, N_importance, flags, impl, _keep_arg(keep),
+                                                         ctx.stream()), "dmnerf_render_forward_objects")
     return out
 
 
@@ -195,17 +222,25 @@ raw2outputs = render_train
 
 
 def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64, N_importance=128, pixel_range=None,
-                 keep_all_ins=False, impl=_lib.IMPL_AUTO, device="cuda"):
+                 keep_all_ins=False, impl=_lib.IMPL_AUTO, device="cuda", keep_objects=None):
     """One camera of the reference's test-time loop (render_test, networks/tester.py:55-76) through the frame entry point of
     the C ABI: rays are generated on the device from K / c2w (get_rays_k), the coarse depth row from near / far
     (z_val_sample), the pixels are rendered by the fused kernel and the maps come back as HOST tensors:
     rgb [H,W,3], ins [H,W,ins_num], depth [H,W], acc [H,W] (or [n, ...] rows when a pixel_range = (begin, count) is given --
-    the per-rank slice of a sharded frame)."""
+    the per-rank slice of a sharded frame).  keep_objects: object selection as in render_rays."""
     dev = torch.device(device)
     ctx = get_context(dev)
     ins_num = ctx.bind(0, model_coarse)
     if ctx.bind(1, model_fine) != ins_num:
         raise RuntimeError("render_frame: coarse and fine networks disagree on ins_num")
+    keep = None
+    if keep_objects is not None:
+        from .autograd import _needs_grad
+        from .objects import object_mask
+        if _needs_grad(model_coarse, model_fine):
+            raise RuntimeError("render_frame: object selection is inference-only; call it under torch.no_grad() or with "
+                               "parameters that do not require grad")
+        keep = object_mask(ins_num, keep=keep_objects)
     begin, count = (0, H * W) if pixel_range is None else (int(pixel_range[0]), int(pixel_range[1]))
     n_ins = ins_num + 1 if keep_all_ins else ins_num
     pin = dev.type == "cuda"
@@ -217,8 +252,13 @@ def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64
     c2 = torch.as_tensor(c2w, dtype=torch.float32).reshape(-1, 4)[:3].reshape(-1)
     Cf = (C.c_float * 12)(*[float(v) for v in c2])
     flags = _lib.FLAG_KEEP_INS if keep_all_ins else 0
-    _lib.check(ctx.lib.dmnerf_render_frame_host(ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples,
-                                                N_importance, flags, impl, C.byref(io), ctx.stream()), "dmnerf_render_frame_host")
+    if keep is None:
+        _lib.check(ctx.lib.dmnerf_render_frame_host(ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples,
+                                                    N_importance, flags, impl, C.byref(io), ctx.stream()), "dmnerf_render_frame_host")
+    else:
+        _lib.check(ctx.lib.dmnerf_render_frame_objects_host(ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count,
+                                                            N_samples, N_importance, flags, impl, _keep_arg(keep),
+                                                            C.byref(io), ctx.stream()), "dmnerf_render_frame_objects_host")
     if pixel_range is None:
         out = {"rgb": out["rgb"].reshape(H, W, 3), "ins": out["ins"].reshape(H, W, n_ins), "depth": out["depth"].reshape(H, W),
                "acc": out["acc"].reshape(H, W)}

@@ -6,7 +6,7 @@
                                             data_range=1                                               tester.py:89-90
     ins_eval(pred_ins, gt_ins, gt_ins_num, ins_num, mask=None) -> (pred_label, ap_list, return_labels)  evaluator.py:125-175
     calculate_ap(IoUs_Metrics, gt_number, confidence=None, function_select='integral')                evaluator.py:77-122
-    write_png(path, array)                  8-bit grey or RGB PNG (zlib + struct; no imageio / cv2 / PIL)
+    write_png(path, array)                  8-bit grey, RGB or RGBA PNG (zlib + struct; no imageio / cv2 / PIL)
 
 Every metric is computed on the device by csrc/metrics.cu: PSNR, SSIM, the predicted labels, the joint histogram of predicted and
 gt labels, per-label median confidences, the cost matrices, the assignment (the device LSAP solver of the training loss) and
@@ -155,10 +155,11 @@ def calculate_ap(IoUs_Metrics, gt_number, confidence=None, function_select='inte
 
 # ----------------------------------------------------------------------------------------------------------------- images
 def write_png(path, img):
-    """8-bit PNG of a uint8 array [H, W] (grey) or [H, W, 3] (RGB), no filtering, zlib level 6."""
+    """8-bit PNG of a uint8 array [H, W] (grey), [H, W, 3] (RGB) or [H, W, 4] (RGBA, straight alpha), no filtering, zlib
+    level 6."""
     a = np.ascontiguousarray(np.asarray(img))
-    if a.dtype != np.uint8 or a.ndim not in (2, 3) or (a.ndim == 3 and a.shape[2] != 3):
-        raise ValueError("write_png: expected uint8 [H, W] or [H, W, 3], got %s %s" % (a.dtype, a.shape))
+    if a.dtype != np.uint8 or a.ndim not in (2, 3) or (a.ndim == 3 and a.shape[2] not in (3, 4)):
+        raise ValueError("write_png: expected uint8 [H, W], [H, W, 3] or [H, W, 4], got %s %s" % (a.dtype, a.shape))
     h, w = a.shape[:2]
     rows = a.reshape(h, -1)
     raw = np.concatenate([np.zeros((h, 1), np.uint8), rows], axis=1).tobytes()       # filter byte 0 per scanline
@@ -166,7 +167,8 @@ def write_png(path, img):
     def chunk(tag, data):
         return struct.pack(">I", len(data)) + tag + data + struct.pack(">I", zlib.crc32(tag + data) & 0xffffffff)
 
-    ihdr = struct.pack(">IIBBBBB", w, h, 8, 2 if a.ndim == 3 else 0, 0, 0, 0)
+    color_type = 0 if a.ndim == 2 else (2 if a.shape[2] == 3 else 6)                 # grey, RGB, RGBA
+    ihdr = struct.pack(">IIBBBBB", w, h, 8, color_type, 0, 0, 0)
     with open(path, "wb") as fh:
         fh.write(b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", ihdr) + chunk(b"IDAT", zlib.compress(raw, 6)) + chunk(b"IEND", b""))
 

@@ -241,6 +241,30 @@ DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, 
 DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n_rays, int n_coarse,
                           int n_importance, int flags, int impl, void* stream);
 
+/* ---- object selection (DESIGN.md, "Object selection") ----------------------------------------------------------------------
+ * keep_host: HOST array of 4 uint32 words, a bitmask of the KEPT object labels 0 .. ins_num (bit k of word k / 32).  Every network
+ * sample gets the label argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the exchanger's
+ * rule); a sample whose label is not kept enters the composite with alpha = 0.  This applies to the coarse and the fine pass, so
+ * the coarse weights of the selected scene drive the importance sampling.  raw_* (when asked for) stay the network's output.
+ * All three reject a NULL mask and a bit set at or above ins_num + 1.
+ * dmnerf_composite_objects: dmnerf_composite with a selection (labels 0 .. c - 5; raw is read, not edited).
+ * dmnerf_render_forward_objects: dmnerf_render_forward with a selection (fused kernel or stage kernels, chosen as there).
+ * dmnerf_render_frame_objects_host: dmnerf_render_frame_host with a selection.
+ * dmnerf_mesh_occupancy_objects: dmnerf_mesh_occupancy with the rule applied per grid point (occ = 0 where the point's label is
+ *   not kept); labels (DEVICE int16 [dim^3], may be NULL) receives every point's label. */
+DMNERF_API int dmnerf_composite_objects(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c,
+                                        int keep_all_ins, const uint32_t* keep_host, float* rgb, float* weights, float* depth,
+                                        float* ins, float* acc, void* stream);
+DMNERF_API int dmnerf_render_forward_objects(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n_rays, int n_coarse,
+                                             int n_importance, int flags, int impl, const uint32_t* keep_host, void* stream);
+DMNERF_API int dmnerf_render_frame_objects_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
+                                                float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
+                                                int flags, int impl, const uint32_t* keep_host, const dmnerf_render_io* out_host,
+                                                void* stream);
+DMNERF_API int dmnerf_mesh_occupancy_objects(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
+                                             float voxel, int64_t slab, const uint32_t* keep_host, float* occ, int16_t* labels,
+                                             void* stream);
+
 /* Same call with HOST buffers (pageable or pinned): copies rays in, renders, copies every non-NULL
  * output back, and synchronises the stream.  This is the end-to-end entry point bench.py times.
  * A batch of >= 131 072 rays is rendered in four parts (same bits: rays are independent) whose uploads / downloads travel on a

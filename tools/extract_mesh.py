@@ -7,7 +7,9 @@ CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict` (the 
 scene transform, inv(to_origin) of the scene mesh's oriented bounds, as a .npy file or as text (16 numbers).  Writes
 DIR/NAME.ply (the marching-cubes mesh in scene space) and DIR/color_NAME.ply (cleaned, every vertex coloured by its object label).
 Without --color-dict (JSON: label -> colour index) and --palette (.npy [K, 3] uint8), label k gets colour k of a fixed
-seeded palette."""
+seeded palette.  --per-object also writes DIR/NAME_obj{k}.ply for every object k: the cleaned mesh of that object alone, from
+a selected occupancy sweep whose grid points are labelled by the network (closed wherever the object does not touch the grid
+boundary); --objects limits it to the labels given."""
 import argparse
 import json
 import os
@@ -20,7 +22,7 @@ import numpy as np   # noqa: E402
 import torch         # noqa: E402
 
 
-def main(argv=None):
+def parse(argv=None):
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("checkpoint")
     ap.add_argument("transform")
@@ -35,8 +37,14 @@ def main(argv=None):
     ap.add_argument("--min-cluster", type=int, default=400)
     ap.add_argument("--color-dict", default=None)
     ap.add_argument("--palette", default=None)
+    ap.add_argument("--per-object", action="store_true", help="also write NAME_obj{k}.ply, one mesh per object")
+    ap.add_argument("--objects", type=int, nargs="+", default=None, help="with --per-object: only these labels")
     ap.add_argument("--device", default="cuda")
-    a = ap.parse_args(argv)
+    return ap.parse_args(argv)
+
+
+def main(argv=None):
+    a = parse(argv)
 
     from dmnerf_b200 import mesh as M
     from dmnerf_b200.testing import model_from_weights
@@ -57,9 +65,23 @@ def main(argv=None):
     ins_map = {str(k): k for k in range(n_col)}
     colors = M.label_colors(labels, palette, color_dict, ins_map)
     M.write_ply(os.path.join(a.out, "color_" + a.name + ".ply"), out["clean_vertices"], out["clean_triangles"], colors)
-    print(json.dumps({"vertices": int(out["vertices"].shape[0]), "triangles": int(out["triangles"].shape[0]),
-                      "clean_vertices": int(out["clean_vertices"].shape[0]), "clean_triangles": int(out["clean_triangles"].shape[0]),
-                      "files": [a.name + ".ply", "color_" + a.name + ".ply"]}))
+    files = [a.name + ".ply", "color_" + a.name + ".ply"]
+    per_object = {}
+    if a.per_object:
+        from dmnerf_b200.objects import object_meshes
+        meshes = object_meshes(nets[1], nets[0], T, objects=a.objects, grid_dim=a.grid_dim, near=a.near, far=a.far,
+                               N_importance=a.N_importance, min_cluster=a.min_cluster)
+        for k, m in meshes.items():
+            name = "%s_obj%d.ply" % (a.name, k)
+            M.write_ply(os.path.join(a.out, name), m["clean_vertices"], m["clean_triangles"])
+            files.append(name)
+            per_object[str(k)] = int(m["clean_triangles"].shape[0])
+    res = {"vertices": int(out["vertices"].shape[0]), "triangles": int(out["triangles"].shape[0]),
+           "clean_vertices": int(out["clean_vertices"].shape[0]), "clean_triangles": int(out["clean_triangles"].shape[0]),
+           "files": files}
+    if a.per_object:
+        res["object_triangles"] = per_object
+    print(json.dumps(res))
 
 
 if __name__ == "__main__":
