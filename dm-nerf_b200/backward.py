@@ -2,7 +2,8 @@
 
 The training forward evaluates the networks with the tensor-core kernel (or the exact-fp32 CUDA-core kernel, see
 TRAIN_IMPL) and keeps the activations the backward needs (dmnerf_mlp_forward_train); the backward is composite_backward
-(closed-form reverse scan) followed by the per-layer GEMMs of dmnerf_mlp_backward.  Gradient topology is the reference's (SURVEY.md 3.3): no gradient through sample_pdf
+(closed-form reverse scan) followed by dmnerf_mlp_backward (heads folded like in the forward, one masked wgmma GEMM per
+trunk layer, batched wgmma weight gradients).  Gradient topology is the reference's (SURVEY.md 3.3): no gradient through sample_pdf
 (render.py:68), the instance map sees detached weights (render.py:22-23), the instance branch sees h.detach()
 (dm_nerf.py:95), rays / depths carry no gradient.
 """
@@ -37,14 +38,14 @@ def _zeros_like_params(params):
     return [flat[o:o + p.numel()].view(p.shape) for o, p in zip(offs, params)]
 
 
-def _mlp_backward(ctx, slot, acts, d_out, m, params, feats_missing):
+def _mlp_backward(ctx, slot, acts, d_out, m, params, masks_saved):
     grads = _zeros_like_params(params)
-    feats_missing = int(feats_missing) | 2            # flags: bit 1 = the gradient buffers are already zero
+    flags = int(masks_saved) | 2            # bit 0 = ReLU bit planes saved by the forward, bit 1 = gradient buffers already zero
     n_scratch = int(ctx.lib.dmnerf_mlp_backward_scratch_floats(m))
     scratch = torch.empty(max(n_scratch, 1), device=d_out.device, dtype=torch.float32)
     arr = (C.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
     _lib.check(ctx.lib.dmnerf_mlp_backward(ctx.handle, slot, _lib.ptr(acts), _lib.ptr(d_out), m, arr, _lib.ptr(scratch),
-                                           int(feats_missing), ctx.stream()), "dmnerf_mlp_backward")
+                                           flags, ctx.stream()), "dmnerf_mlp_backward")
     return grads
 
 
@@ -64,7 +65,7 @@ class MLPFunction(torch.autograd.Function):
         impl = _train_impl(impl)
         _lib.check(ctx.lib.dmnerf_mlp_forward_train(ctx.handle, slot, _lib.ptr(x2), None, None, None, m, 1, _lib.ptr(out),
                                                     _lib.ptr(acts), impl, ctx.stream()), "dmnerf_mlp_forward_train")
-        fctx.model, fctx.m, fctx.acts, fctx.params, fctx.feats_missing = model, m, acts, params, impl != _lib.IMPL_SIMT
+        fctx.model, fctx.m, fctx.acts, fctx.params, fctx.masks_saved = model, m, acts, params, impl != _lib.IMPL_SIMT
         return out.reshape(*x.shape[:-1], out.shape[-1])
 
     @staticmethod
@@ -73,7 +74,7 @@ class MLPFunction(torch.autograd.Function):
         slot = ctx.slot_for(fctx.model)
         ctx.bind(slot, fctx.model)
         d_out = _f32(g_out.reshape(fctx.m, -1))
-        grads = _mlp_backward(ctx, slot, fctx.acts, d_out, fctx.m, fctx.params, fctx.feats_missing)
+        grads = _mlp_backward(ctx, slot, fctx.acts, d_out, fctx.m, fctx.params, fctx.masks_saved)
         return (None, None, None) + tuple(grads)
 
 
@@ -153,7 +154,7 @@ class RenderFunction(torch.autograd.Function):
         fctx.models = (model_c, model_f)
         fctx.n, fctx.S, fctx.F, fctx.C, fctx.n_c = n, S, F, Cc, n_c
         fctx.acts = saved
-        fctx.feats_missing = impl != _lib.IMPL_SIMT
+        fctx.masks_saved = impl != _lib.IMPL_SIMT
         fctx.params = params
         fctx.save_for_backward(rays_d, o["z_vals_coarse"], o["z_vals_fine"], o["raw_coarse"], o["raw_fine"])
         outs = tuple(o[k] for k in _OUT_KEYS)
@@ -180,7 +181,7 @@ class RenderFunction(torch.autograd.Function):
                                                      _lib.ptr(keep[0]), _lib.ptr(keep[1]), _lib.ptr(keep[2]), _lib.ptr(keep[3]),
                                                      _lib.ptr(keep[4]), _lib.ptr(d_raw), accumulate, st), "dmnerf_composite_backward")
             params = fctx.params[:fctx.n_c] if net == 0 else fctx.params[fctx.n_c:]
-            all_grads += _mlp_backward(ctx, net, fctx.acts[net], d_raw.reshape(n * ns, Cc), n * ns, params, fctx.feats_missing)
+            all_grads += _mlp_backward(ctx, net, fctx.acts[net], d_raw.reshape(n * ns, Cc), n * ns, params, fctx.masks_saved)
         fctx.acts = None
         return (None,) * 11 + tuple(all_grads)
 

@@ -64,7 +64,6 @@ struct dmnerf_ctx {
   Scratch frame_rays;             // rays of the frame being rendered by dmnerf_render_frame_host
   Scratch mesh_pts, mesh_raw;     // one slab of the occupancy sweep: points + zero view directions, network output
   MeshState* mesh = nullptr;      // buffers of the other mesh entry points (mesh.cu)
-  bool train_feats_missing[2] = {false, false};
   bool profiling = false;
   bool last_fused = false;       // the last render call took the single-kernel path
   bool profile_valid = false;
@@ -296,19 +295,18 @@ DMNERF_API int dmnerf_mlp_forward_train(dmnerf_ctx* ctx, int net, const float* x
   DMN_CHECK(out && acts, "mlp_forward_train: out / acts is NULL");
   DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA, "mlp_forward_train: unknown impl %d", impl);
   if (impl == DMNERF_IMPL_AUTO) impl = umma_available(ctx->packed[net]) ? DMNERF_IMPL_UMMA : DMNERF_IMPL_SIMT;
-  ctx->train_feats_missing[net] = (impl == DMNERF_IMPL_UMMA);
   if (impl == DMNERF_IMPL_UMMA)
     return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
   return launch_mlp_simt(ctx->net[net], x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_mlp_backward(dmnerf_ctx* ctx, int net, float* acts, const float* d_out, int64_t m, float* const* grads,
-                                   float* scratch, int feats_missing, void* stream) {
+                                   float* scratch, int flags, void* stream) {
   DMN_CHECK(ctx != nullptr, "mlp_backward: ctx is NULL");
   DMN_CHECK(net == 0 || net == 1, "mlp_backward: net must be 0 or 1");
   DMN_CHECK(m >= 0 && grads, "mlp_backward: bad arguments");
   DMN_CHECK(m == 0 || (acts && d_out && scratch), "mlp_backward: NULL buffer");
-  return launch_mlp_backward(ctx->net[net], &ctx->packed[net], acts, d_out, m, grads, scratch, feats_missing, (cudaStream_t)stream);
+  return launch_mlp_backward(ctx->net[net], ctx->packed[net], acts, d_out, m, grads, scratch, flags, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_composite_backward(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c,

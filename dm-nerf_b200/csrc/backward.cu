@@ -1,15 +1,12 @@
-// Backward of the render path (BASELINE config 4: training step, reference train_dmsr.py:62-64), fp32 CUDA cores.
+// Backward of the render path (BASELINE config 4: training step, reference train_dmsr.py:62-64).
 //
 //   * composite_backward_kernel: d(rgb_map, depth_map, acc_map, ins_map) -> d raw, one warp per ray.  The transmittance
 //     product is differentiated in closed form with a reverse warp scan:  dL/dalpha_i = gw_i T_i - (sum_{j>i} gw_j w_j) / f_i.
 //     Honours the reference's detach topology (render.py:22-23: the instance map sees detached weights).
-//   * MLP backward over the activations saved by the training forward (mlp_simt.cu, ActPlanes): per layer
-//       dX = (dY W) (.) relu-mask   -> gemm_nn_kernel        dW += dY^T X -> gemm_tn_kernel (split over samples, fp32 atomics)
-//       db += column sums of dY     -> colsum_kernel
-//     with the reference's gradient routing (dm_nerf.py:95: the instance branch reads h.detach(), so it contributes to
-//     ins_feature_linear and below only).
-#include <cstdlib>
-#include <cstring>
+//   * MLP backward over the activations saved by the training forward (ActPlanes), with the heads folded like in the forward
+//     (mlp_backward_chain): the gradient chain of bwd_chain.cu carries dY through the trunk, batched split-bf16 wgmma GEMMs
+//     (gemm_umma.cu) form the weight gradients, small fp32 products give the folded head layers.  Gradient routing is the
+//     reference's (dm_nerf.py:95: the instance branch reads h.detach(), so it contributes to ins_feature_linear and below only).
 
 #include "ray_ops.cuh"
 #include "umma_api.cuh"
@@ -131,65 +128,15 @@ int launch_composite_backward(const float* raw, const float* z, const float* ray
   return 0;
 }
 
-// ================================================================================================ fp32 GEMMs
+// ================================================================================================ fp32 dW GEMMs
+// The weight-gradient products the wgmma kernel does not take (gemm_tn_tc_supported): on this network only ins_linear with more
+// than 64 instance logits.
 constexpr int GT = 64;      // output tile GT x GT
 constexpr int GK = 16;      // inner chunk
 
-// C[m, k] (= | +=) sum_n A[m, n] B[n, k];  optionally C = (mask[m, k] > 0) ? C : 0   (mask shares ldc).
-__global__ void __launch_bounds__(256) gemm_nn_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                      float* __restrict__ Cm, int ldc, int64_t M, int N, int K, int accumulate,
-                                                      const float* __restrict__ mask) {
-  __shared__ float As[GK][GT + 1];
-  __shared__ float Bs[GK][GT];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int64_t m0 = (int64_t)blockIdx.x * GT;
-  const int k0 = blockIdx.y * GT;
-  float acc[4][4] = {};
-  for (int n0 = 0; n0 < N; n0 += GK) {
-    for (int idx = tid; idx < GT * GK; idx += 256) {           // A tile [GT rows][GK inner], coalesced along inner
-      const int r = idx / GK, c = idx % GK;
-      const int64_t m = m0 + r;
-      As[c][r] = (m < M && n0 + c < N) ? A[m * lda + n0 + c] : 0.0f;
-    }
-    for (int idx = tid; idx < GK * GT; idx += 256) {           // B tile [GK inner][GT cols]
-      const int r = idx / GT, c = idx % GT;
-      Bs[r][c] = (n0 + r < N && k0 + c < K) ? B[(size_t)(n0 + r) * ldb + k0 + c] : 0.0f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < GK; ++kk) {
-      float a[4], b[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) b[j] = Bs[kk][tx + 16 * j];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int64_t m = m0 + ty * 4 + i;
-    if (m >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int k = k0 + tx + 16 * j;
-      if (k >= K) continue;
-      float v = acc[i][j];
-      if (accumulate) v += Cm[m * ldc + k];
-      if (mask && !(mask[m * ldc + k] > 0.0f)) v = 0.0f;
-      Cm[m * ldc + k] = v;
-    }
-  }
-}
-
 // C[n, k] += sum_{m in split} A[m, n] B[m, k]   (C zero-initialised by the caller; fp32 atomics across splits)
 __global__ void __launch_bounds__(256) gemm_tn_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                      float* __restrict__ Cm, int ldc, int64_t M, int N, int K, int64_t rows_per_split,
-                                                      int64_t b_cm) {
+                                                      float* __restrict__ Cm, int ldc, int64_t M, int N, int K, int64_t rows_per_split) {
   __shared__ float As[GK][GT];
   __shared__ float Bs[GK][GT];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -202,7 +149,7 @@ __global__ void __launch_bounds__(256) gemm_tn_kernel(const float* __restrict__ 
       const int r = idx / GT, c = idx % GT;
       const int64_t m = m0 + r;
       As[r][c] = (m < me && n0 + c < N) ? A[m * lda + n0 + c] : 0.0f;
-      Bs[r][c] = (m < me && k0 + c < K) ? (b_cm ? B[(int64_t)(k0 + c) * b_cm + m] : B[m * ldb + k0 + c]) : 0.0f;
+      Bs[r][c] = (m < me && k0 + c < K) ? B[m * ldb + k0 + c] : 0.0f;
     }
     __syncthreads();
 #pragma unroll
@@ -231,30 +178,8 @@ __global__ void __launch_bounds__(256) gemm_tn_kernel(const float* __restrict__ 
   }
 }
 
-// out[n] += sum_m A[m, n]
-__global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ A, int lda, float* __restrict__ out, int64_t M, int N,
-                                                     int64_t rows_per_block) {
-  __shared__ float red[8][32];
-  const int c = blockIdx.x * 32 + (threadIdx.x & 31), r = threadIdx.x >> 5;
-  const int64_t mb = (int64_t)blockIdx.y * rows_per_block;
-  const int64_t me = (mb + rows_per_block < M) ? mb + rows_per_block : M;
-  float s = 0.0f;
-  if (c < N)
-    for (int64_t m = mb + r; m < me; m += 8) s += A[m * lda + c];
-  red[r][threadIdx.x & 31] = s;
-  __syncthreads();
-  if (r == 0 && c < N) {
-    float t = 0.0f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) t += red[i][threadIdx.x & 31];
-    atomicAdd(&out[c], t);
-  }
-}
-
-
-// ================================================================================================ 128x128 register-tiled GEMMs
-// Used for the 256/128-wide layers (row strides multiple of 4 floats, inner dimension multiple of 8); the small generic
-// kernels above keep the odd shapes (3 / 1 / ins_num+1 wide heads, 63- and 27-wide embeddings).
+// 128x128 register-tiled variant for operands whose widths and row strides are multiples of 4 floats (e.g. ins_num 127); the
+// generic kernel above takes the other widths (e.g. ins_num 93).
 constexpr int BT = 128;     // output tile BT x BT, 256 threads, 8x8 outputs per thread
 constexpr int BK = 8;       // inner slice
 
@@ -267,60 +192,6 @@ __device__ __forceinline__ void fma_8x8(float (&acc)[8][8], const float* __restr
   for (int i = 0; i < 8; ++i)
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-}
-
-// C[m, k] (= | +=) sum_n A[m, n] B[n, k], optional ReLU mask.  M arbitrary, N % 8 == 0, K % 4 == 0, lda/ldb/ldc % 4 == 0.
-__global__ void __launch_bounds__(256) gemm_nn_big_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                          float* __restrict__ Cm, int ldc, int64_t M, int N, int K, int accumulate,
-                                                          const float* __restrict__ mask) {
-  __shared__ __align__(16) float As[2][BK][BT];
-  __shared__ __align__(16) float Bs[2][BK][BT];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int64_t m0 = (int64_t)blockIdx.x * BT;
-  const int k0 = blockIdx.y * BT;
-  const int ar = tid >> 1, ac = (tid & 1) * 4;          // A slice: row ar, inner offset ac (float4 along the inner dimension)
-  const int br = tid >> 5, bc = (tid & 31) * 4;         // B slice: inner row br, columns bc..bc+3
-  float acc[8][8] = {};
-  float4 ra, rb;
-  auto load = [&](int n0) {
-    const int64_t m = m0 + ar;
-    ra = (m < M) ? *reinterpret_cast<const float4*>(A + m * lda + n0 + ac) : make_float4(0.f, 0.f, 0.f, 0.f);
-    rb = (k0 + bc < K) ? *reinterpret_cast<const float4*>(B + (size_t)(n0 + br) * ldb + k0 + bc) : make_float4(0.f, 0.f, 0.f, 0.f);
-  };
-  auto stash = [&](int buf) {
-    As[buf][ac + 0][ar] = ra.x; As[buf][ac + 1][ar] = ra.y; As[buf][ac + 2][ar] = ra.z; As[buf][ac + 3][ar] = ra.w;
-    *reinterpret_cast<float4*>(&Bs[buf][br][bc]) = rb;
-  };
-  load(0);
-  stash(0);
-  __syncthreads();
-  int buf = 0;
-  for (int n0 = 0; n0 < N; n0 += BK) {
-    if (n0 + BK < N) load(n0 + BK);                     // prefetch the next slice into registers
-#pragma unroll
-    for (int kk = 0; kk < BK; ++kk) fma_8x8(acc, As[buf][kk], Bs[buf][kk], ty, tx);
-    if (n0 + BK < N) stash(buf ^ 1);
-    __syncthreads();
-    buf ^= 1;
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int64_t m = m0 + ty * 8 + i;
-    if (m >= M) continue;
-#pragma unroll
-    for (int j4 = 0; j4 < 8; j4 += 4) {
-      const int k = k0 + tx * 8 + j4;
-      if (k >= K) continue;
-      float4 v = make_float4(acc[i][j4], acc[i][j4 + 1], acc[i][j4 + 2], acc[i][j4 + 3]);
-      float* cp = Cm + m * ldc + k;
-      if (accumulate) { const float4 o = *reinterpret_cast<const float4*>(cp); v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w; }
-      if (mask) {
-        const float4 mk = *reinterpret_cast<const float4*>(mask + m * ldc + k);
-        if (!(mk.x > 0.f)) v.x = 0.f; if (!(mk.y > 0.f)) v.y = 0.f; if (!(mk.z > 0.f)) v.z = 0.f; if (!(mk.w > 0.f)) v.w = 0.f;
-      }
-      *reinterpret_cast<float4*>(cp) = v;
-    }
-  }
 }
 
 // C[n, k] += sum_{m in split} A[m, n] B[m, k].  N % 4 == 0, K % 4 == 0, lda/ldb % 4 == 0; rows_per_split % 8 == 0.
@@ -369,104 +240,9 @@ __global__ void __launch_bounds__(256) gemm_tn_big_kernel(const float* __restric
   }
 }
 
-// DMNERF_BWD_IMPL=simt keeps every backward GEMM on the fp32 CUDA-core kernels (cross-check / A-B timing).
-static bool bwd_use_tc() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("DMNERF_BWD_IMPL");
-    v = (e && strcmp(e, "simt") == 0) ? 0 : 1;
-  }
-  return v != 0;
-}
-
-static int gemm_nn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K, int accumulate,
-                   const float* mask, cudaStream_t st) {
-  if (bwd_use_tc() && M >= 512 && gemm_nn_tc_supported(N, K, ldc, C, mask))
-    return launch_gemm_nn_tc(A, lda, B, ldb, C, ldc, M, N, accumulate, mask, nullptr, 0, st);
-  const bool aligned = ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0) && ((uintptr_t)C % 16 == 0) &&
-                       (!mask || (uintptr_t)mask % 16 == 0);
-  if (aligned && N % BK == 0 && K % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 && ldc % 4 == 0 && N >= 64 && K >= 64) {
-    dim3 grid((unsigned)((M + BT - 1) / BT), (unsigned)((K + BT - 1) / BT));
-    gemm_nn_big_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, N, K, accumulate, mask);
-    DMN_LAUNCH_OK();
-    return 0;
-  }
-  dim3 grid((unsigned)((M + GT - 1) / GT), (unsigned)((K + GT - 1) / GT));
-  gemm_nn_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, N, K, accumulate, mask);
-  DMN_LAUNCH_OK();
-  return 0;
-}
-
-// C[m, n] = bias[n] + sum_k A[m, k] W[n, k]   (a Linear layer: W row-major [N, K])
-__global__ void __launch_bounds__(256) gemm_nt_bias_kernel(const float* __restrict__ A, int lda, const float* __restrict__ W, int ldw,
-                                                           const float* __restrict__ bias, float* __restrict__ Cm, int ldc,
-                                                           int64_t M, int N, int K) {
-  __shared__ float As[GK][GT + 1];
-  __shared__ float Ws[GK][GT + 1];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int64_t m0 = (int64_t)blockIdx.x * GT;
-  const int n0 = blockIdx.y * GT;
-  float acc[4][4] = {};
-  for (int k0 = 0; k0 < K; k0 += GK) {
-    for (int idx = tid; idx < GT * GK; idx += 256) {
-      const int r = idx / GK, c = idx % GK;
-      const int64_t mm = m0 + r;
-      As[c][r] = (mm < M && k0 + c < K) ? A[mm * lda + k0 + c] : 0.0f;
-      Ws[c][r] = (n0 + r < N && k0 + c < K) ? W[(size_t)(n0 + r) * ldw + k0 + c] : 0.0f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < GK; ++kk) {
-      float a[4], b[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) b[j] = Ws[kk][tx + 16 * j];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int64_t mm = m0 + ty * 4 + i;
-    if (mm >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int n = n0 + tx + 16 * j;
-      if (n < N) Cm[mm * ldc + n] = acc[i][j] + bias[n];
-    }
-  }
-}
-
-static int gemm_nt_bias(const float* A, int lda, const float* W, int ldw, const float* bias, float* C, int ldc, int64_t M, int N,
-                        int K, cudaStream_t st) {
-  if (bwd_use_tc() && M >= 512 && N == 256 && K == 256 && ldc % 4 == 0 && (uintptr_t)C % 16 == 0 && (uintptr_t)bias % 16 == 0)
-    return launch_gemm_nn_tc(A, lda, W, ldw, C, ldc, M, K, 0, nullptr, bias, 1, st);
-  dim3 grid((unsigned)((M + GT - 1) / GT), (unsigned)((N + GT - 1) / GT));
-  gemm_nt_bias_kernel<<<grid, 256, 0, st>>>(A, lda, W, ldw, bias, C, ldc, M, N, K);
-  DMN_LAUNCH_OK();
-  return 0;
-}
-
-static int colsum(const float* A, int lda, float* out, int64_t M, int N, cudaStream_t st);
-
-// colsum_out != NULL: also colsum_out[n] += sum_m A[m, n] (the bias gradient of the same layer, zero-initialised by the caller).
-// b_cm != 0: B is column-major (element (m, k) at B[k * b_cm + m]) -- the embedded-input plane of the training forward.
-static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K, cudaStream_t st,
-                   float* colsum_out = nullptr, int64_t b_cm = 0) {
-  if (bwd_use_tc() && M >= 512 && gemm_tn_tc_supported(N, K))
-    return launch_gemm_tn_tc(A, lda, B, ldb, C, ldc, colsum_out, M, N, K, 0, st, b_cm);
-  if (bwd_use_tc() && M >= 512 && !colsum_out && !b_cm && gemm_tn_tc_supported(K, N))      // narrow dY, wide X: compute (X^T dY)^T
-    return launch_gemm_tn_tc(B, ldb, A, lda, C, ldc, nullptr, M, K, N, 1, st);
-  if (colsum_out) {
-    int rc = colsum(A, lda, colsum_out, M, N, st);
-    if (rc) return rc;
-  }
+static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K, cudaStream_t st) {
   const bool aligned = ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0);
-  if (aligned && !b_cm && N % 4 == 0 && K % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 && N >= 64 && K >= 64) {
+  if (aligned && N % 4 == 0 && K % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 && N >= 64 && K >= 64) {
     const int tiles_b = ((N + BT - 1) / BT) * ((K + BT - 1) / BT);
     int64_t splits = (3 * 132 + tiles_b - 1) / tiles_b;
     int64_t rows = (M + splits - 1) / splits;
@@ -485,30 +261,12 @@ static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, i
   if (rows < 256) rows = 256;
   splits = (M + rows - 1) / rows;
   dim3 grid((unsigned)((N + GT - 1) / GT), (unsigned)((K + GT - 1) / GT), (unsigned)splits);
-  gemm_tn_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, N, K, rows, b_cm);
-  DMN_LAUNCH_OK();
-  return 0;
-}
-
-static int colsum(const float* A, int lda, float* out, int64_t M, int N, cudaStream_t st) {
-  const int64_t rows = 2048;
-  dim3 grid((unsigned)((N + 31) / 32), (unsigned)((M + rows - 1) / rows));
-  colsum_kernel<<<grid, 256, 0, st>>>(A, lda, out, M, N, rows);
+  gemm_tn_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, N, K, rows);
   DMN_LAUNCH_OK();
   return 0;
 }
 
 size_t mlp_backward_scratch_floats(int64_t m) { return (size_t)m * (256 + 8 * 256) + 256 * 256 + 256 + 256; }
-
-// DMNERF_BWD_IMPL=gemm: the unfolded per-layer path below instead of the folded-head gradient chain (cross-check / A-B timing).
-static bool bwd_use_chain() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("DMNERF_BWD_IMPL");
-    v = (e && (strcmp(e, "simt") == 0 || strcmp(e, "gemm") == 0)) ? 0 : 1;
-  }
-  return v != 0;
-}
 
 // Small dense products of the folded head gradients (128..256 x 256 outputs, contraction 128..256): 16 x 16 output tiles, one
 // output per thread, so that the launch fills the machine (a 64 x 64 tiling runs these on 8-16 CTAs at ~35 us apiece).
@@ -582,7 +340,7 @@ __global__ void __launch_bounds__(256) colsum_flat_kernel(const float* __restric
 }
 
 static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, float* acts, const float* d_out, int64_t m,
-                              float* const* grads, float* scratch, int feats_missing, cudaStream_t st) {
+                              float* const* grads, float* scratch, bool masks_saved, cudaStream_t st) {
   const int ins1 = p.ins_num + 1, C = 4 + ins1;
   const ActPlanes ap = act_planes(acts, m);
   float* S12 = scratch;                               // d rgb_hid | d ins_hid  [m,256]
@@ -601,7 +359,6 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
   // gradient chain has run: they are queued by shape class and each class goes out as ONE batched tensor-core launch
   // (launch_gemm_tn_tc_batch) -- 3 GEMM + 3 reduction launches per network instead of 14 + 14.
   struct Queue { TnProblem p[TN_MAX_BATCH]; int n = 0, N = 0; } q_wide, q_in256, q_in128;      // [256 x 256], [256 x <=64], [128 x <=64]
-  const bool batched = bwd_use_tc() && m >= 512;
   auto flush = [&](Queue& q) -> int {
     const int r = q.n ? launch_gemm_tn_tc_batch(q.p, q.n, m, q.N, st) : 0;
     q.n = 0;
@@ -611,24 +368,24 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
                 int64_t b_cm = 0) -> int {
     TnProblem pr;
     Queue* q = nullptr;
-    if (batched && gemm_tn_tc_supported(N, K)) {
+    if (gemm_tn_tc_supported(N, K) && (K <= 64 || N == 256)) {
       pr.A = A; pr.lda = lda; pr.B = B; pr.ldb = ldb; pr.K = K; pr.transpose = 0; pr.colsum = colsum_out; pr.b_cm = b_cm;
       q = (K > 64) ? &q_wide : (N == 256 ? &q_in256 : &q_in128);
-      if (K > 64 && N != 256) q = nullptr;                                      // [128 x 256]: not a shape of this network
-      pr.ldc = ldc; pr.C = Cw;
-      if (q) q->N = N;
-    } else if (batched && !colsum_out && !b_cm && K > 64 && gemm_tn_tc_supported(K, N)) {      // narrow dY, wide X: (X^T dY)^T
+      q->N = N;
+    } else if (!colsum_out && !b_cm && K > 64 && gemm_tn_tc_supported(K, N)) {      // narrow dY, wide X: (X^T dY)^T
       pr.A = B; pr.lda = ldb; pr.B = A; pr.ldb = lda; pr.K = N; pr.transpose = 1; pr.colsum = nullptr; pr.b_cm = 0;
-      pr.ldc = ldc; pr.C = Cw;
       q = (K == 256) ? &q_in256 : &q_in128;
       q->N = K;
+    } else {
+      DMN_CHECK(!colsum_out && !b_cm, "mlp_backward: no kernel for the %d x %d weight gradient", N, K);
+      return gemm_tn(A, lda, B, ldb, Cw, ldc, m, N, K, st);
     }
-    if (!q) return gemm_tn(A, lda, B, ldb, Cw, ldc, m, N, K, st, colsum_out, b_cm);
+    pr.ldc = ldc; pr.C = Cw;
     if (q->n == TN_MAX_BATCH) { const int r = flush(*q); if (r) return r; }
     q->p[q->n++] = pr;
     return 0;
   };
-  if (!feats_missing) R(launch_mask_bits(acts, m, st));          // exact-fp32 forward: masks from its planes
+  if (!masks_saved) R(launch_mask_bits(acts, m, st));          // exact-fp32 forward: masks from its planes
   const float* d_rgb = d_out;
   const float* d_sig = d_out + 3;
   const float* d_ins = d_out + 4;
@@ -668,12 +425,11 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
 }
 
 // grads: 30 device pointers in state_dict order (weight, bias per layer); overwritten with the gradient of this call.
-int launch_mlp_backward(const NetParams& p, const UmmaWeights* packed, float* acts, const float* d_out, int64_t m, float* const* grads,
-                        float* scratch, int feats_missing, cudaStream_t st) {
+int launch_mlp_backward(const NetParams& p, const UmmaWeights& packed, float* acts, const float* d_out, int64_t m, float* const* grads,
+                        float* scratch, int flags, cudaStream_t st) {
   DMN_CHECK(p.bound, "mlp_backward: weights not bound");
-  const int ins1 = p.ins_num + 1, C = 4 + ins1;
-  const bool prezeroed = (feats_missing & 2) != 0;      // flags: bit 0 = feature planes missing, bit 1 = grads already zero
-  feats_missing &= 1;
+  DMN_CHECK(umma_available(packed), "mlp_backward: weights not packed (call dmnerf_set_weights first)");
+  const bool prezeroed = (flags & 2) != 0;      // flags: bit 0 = the forward wrote the ReLU bit planes, bit 1 = grads already zero
   for (int l = 0; l < N_LAYERS; ++l) {
     DMN_CHECK(grads[2 * l] && grads[2 * l + 1], "mlp_backward: gradient buffer %d is NULL", 2 * l);
     if (prezeroed) continue;
@@ -681,64 +437,7 @@ int launch_mlp_backward(const NetParams& p, const UmmaWeights* packed, float* ac
     DMN_CUDA(cudaMemsetAsync(grads[2 * l + 1], 0, (size_t)layer_out(l, p.ins_num) * sizeof(float), st));
   }
   if (m == 0) return 0;
-  if (bwd_use_tc() && bwd_use_chain() && packed && umma_available(*packed) && m >= 512)
-    return mlp_backward_chain(p, *packed, acts, d_out, m, grads, scratch, feats_missing, st);
-  const ActPlanes ap = act_planes(acts, m);
-  float* S1 = scratch;                  // d rgb_hid  [m,128]
-  float* S2 = S1 + m * 128;             // d ins_hid  [m,128]
-  float* S3 = S2 + m * 128;             // d rgb_feat [m,256]
-  float* S4 = S3 + m * 256;             // d ins_feat [m,256]
-  float* G = S4 + m * 256;              // d h (masked), ping
-  float* G2 = G + m * 256;              //               pong
-  auto gw = [&](int l) { return grads[2 * l]; };
-  auto gb = [&](int l) { return grads[2 * l + 1]; };
-  int rc = 0;
-#define R(x) do { if ((rc = (x))) return rc; } while (0)
-  if (feats_missing) {
-    // the tensor-core forward folds rgb_feature_linear / ins_feature_linear away: rebuild the two planes from h7
-    R(gemm_nt_bias(ap.h[7], 256, p.w[L_RGB_FEAT], 256, p.b[L_RGB_FEAT], ap.rgb_feat, 256, m, 256, 256, st));
-    R(gemm_nt_bias(ap.h[7], 256, p.w[L_INS_FEAT], 256, p.b[L_INS_FEAT], ap.ins_feat, 256, m, 256, 256, st));
-  }
-  const float* d_rgb = d_out;           // [m, 3]       lda = C
-  const float* d_sig = d_out + 3;       // [m, 1]
-  const float* d_ins = d_out + 4;       // [m, ins1]
-  // ---- output layers (dm_nerf.py:101-103)
-  R(gemm_tn(d_rgb, C, ap.rgb_hid, 128, gw(L_RGB_OUT), 128, m, 3, 128, st));     R(colsum(d_rgb, C, gb(L_RGB_OUT), m, 3, st));
-  R(gemm_tn(d_ins, C, ap.ins_hid, 128, gw(L_INS_OUT), 128, m, ins1, 128, st));  R(colsum(d_ins, C, gb(L_INS_OUT), m, ins1, st));
-  R(gemm_tn(d_sig, C, ap.h[7], 256, gw(L_DENSITY), 256, m, 1, 256, st));        R(colsum(d_sig, C, gb(L_DENSITY), m, 1, st));
-  R(gemm_nn(d_rgb, C, p.w[L_RGB_OUT], 128, S1, 128, m, 3, 128, 0, ap.rgb_hid, st));       // through ReLU of rgb_hid
-  R(gemm_nn(d_ins, C, p.w[L_INS_OUT], 128, S2, 128, m, ins1, 128, 0, ap.ins_hid, st));    // through ReLU of ins_hid
-  // ---- hidden head layers (dm_nerf.py:90-99)
-  R(gemm_tn(S1, 128, ap.rgb_feat, 256, gw(L_RGB_HID), 283, m, 128, 256, st, gb(L_RGB_HID)));      // + bias gradient
-  R(gemm_tn(S1, 128, ap.emb + (int64_t)CH_POS * m, CH_IN, gw(L_RGB_HID) + 256, 283, m, 128, CH_DIR, st, nullptr, m));
-  R(gemm_tn(S2, 128, ap.ins_feat, 256, gw(L_INS_HID), 256, m, 128, 256, st, gb(L_INS_HID)));      // + bias gradient
-  R(gemm_nn(S1, 128, p.w[L_RGB_HID], 283, S3, 256, m, 128, 256, 0, nullptr, st));         // d rgb_feature (no activation)
-  R(gemm_nn(S2, 128, p.w[L_INS_HID], 256, S4, 256, m, 128, 256, 0, nullptr, st));         // d ins_feature
-  // ---- feature layers on the final trunk activation (dm_nerf.py:89,95-96)
-  R(gemm_tn(S3, 256, ap.h[7], 256, gw(L_RGB_FEAT), 256, m, 256, 256, st, gb(L_RGB_FEAT)));
-  R(gemm_tn(S4, 256, ap.h[7], 256, gw(L_INS_FEAT), 256, m, 256, 256, st, gb(L_INS_FEAT)));
-  // d h8 = d sigma (x) w_density + d rgb_feat W_rgb_feat   (the instance branch saw h.detach()), then ReLU mask of layer 7
-  R(gemm_nn(d_sig, C, p.w[L_DENSITY], 256, G, 256, m, 1, 256, 0, nullptr, st));
-  R(gemm_nn(S3, 256, p.w[L_RGB_FEAT], 256, G, 256, m, 256, 256, 1, ap.h[7], st));
-  // ---- trunk, layers 7..0 (dm_nerf.py:83-87)
-  float* cur = G;
-  float* nxt = G2;
-  for (int l = 7; l >= 0; --l) {
-    const int kin = layer_in(l);
-    if (l == 0) {
-      R(gemm_tn(cur, 256, ap.emb, CH_IN, gw(0), kin, m, 256, CH_POS, st, nullptr, m));
-      R(colsum(cur, 256, gb(0), m, 256, st));
-    } else {
-      R(gemm_tn(cur, 256, ap.h[l - 1], 256, gw(l), kin, m, 256, 256, st, gb(l)));             // dW and db of layer l
-      if (l == 5) R(gemm_tn(cur, 256, ap.emb, CH_IN, gw(5) + 256, kin, m, 256, CH_POS, st, nullptr, m));   // skip input [h, pts]
-    }
-    if (l > 0) {
-      R(gemm_nn(cur, 256, p.w[l], kin, nxt, 256, m, 256, 256, 0, ap.h[l - 1], st));
-      float* t = cur; cur = nxt; nxt = t;
-    }
-  }
-#undef R
-  return 0;
+  return mlp_backward_chain(p, packed, acts, d_out, m, grads, scratch, (flags & 1) != 0, st);
 }
 
 }  // namespace dmnerf

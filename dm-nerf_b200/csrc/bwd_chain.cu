@@ -160,9 +160,9 @@ int launch_bwd_chain(const UmmaWeights& w, const NetParams& p, const float* s1, 
   bk::dsig_outer_kernel<<<(unsigned)((m * 64 + 255) / 256), 256, 0, st>>>(d_out, C, p.w[L_DENSITY], m, dy[7]);
   DMN_LAUNCH_OK();
   auto bits = [&](int plane) { return ap.bits + (int64_t)plane * ACT_BITS_GROUPS * m; };
-  int rc = launch_gemm_nn_tc(s1, 256, umma_fold_w_rgb(w), 283, dy[7], 256, m, 128, 1, nullptr, nullptr, 0, st, bits(7));
+  int rc = launch_gemm_nn_tc(s1, 256, umma_fold_w_rgb(w), 283, dy[7], 256, m, 128, 1, bits(7), st);
   for (int l = 7; l >= 1 && rc == 0; --l)
-    rc = launch_gemm_nn_tc(dy[l], 256, p.w[l], layer_in(l), dy[l - 1], 256, m, 256, 0, nullptr, nullptr, 0, st, bits(l - 1));
+    rc = launch_gemm_nn_tc(dy[l], 256, p.w[l], layer_in(l), dy[l - 1], 256, m, 256, 0, bits(l - 1), st);
   return rc;
 }
 

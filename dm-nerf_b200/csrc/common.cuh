@@ -46,7 +46,7 @@ __host__ __device__ inline int layer_in(int l) {
 }
 
 // Activations saved by the training forward of one network (planes of row-major [M, width] matrices, in this order):
-//   H0..H7 [M,256] (post-ReLU trunk outputs) | rgb_feat [M,256] | ins_feat [M,256] | rgb_hid [M,128] | ins_hid [M,128] | emb [90,M]
+//   H0..H7 [M,256] (post-ReLU trunk outputs) | rgb_hid [M,128] | ins_hid [M,128] | emb [90,M]
 // (the embedded inputs are stored COLUMN-major, [90][M]: their writers own one row and a few columns each, so row-fastest storage
 //  makes every store instruction of a warp one contiguous 128-byte line; their only readers are three narrow dW GEMMs)
 // ... | bits: ReLU masks, 1 bit per unit, as 16-bit groups stored ROW-FASTEST: [10 planes][16 groups][M] uint16 (planes 0..7 =
@@ -56,16 +56,14 @@ constexpr int ACT_BITS_PLANES = 10, ACT_BITS_WORDS = 8, ACT_BITS_GROUPS = 16;
 __host__ __device__ inline int64_t act_bits_index(int plane, int group, int64_t row, int64_t m) {
   return ((int64_t)plane * ACT_BITS_GROUPS + group) * m + row;
 }
-constexpr int ACT_FLOATS_PER_SAMPLE = CH_IN + 8 * W_HID + 2 * W_HID + 2 * (W_HID / 2) + ACT_BITS_PLANES * ACT_BITS_WORDS;   // 2986
+constexpr int ACT_FLOATS_PER_SAMPLE = CH_IN + 8 * W_HID + 2 * (W_HID / 2) + ACT_BITS_PLANES * ACT_BITS_WORDS;   // 2474
 struct ActPlanes {
-  float* emb; float* h[8]; float* rgb_feat; float* ins_feat; float* rgb_hid; float* ins_hid; uint16_t* bits;
+  float* emb; float* h[8]; float* rgb_hid; float* ins_hid; uint16_t* bits;
 };
 __host__ __device__ inline ActPlanes act_planes(float* base, int64_t m) {
   ActPlanes a;
   float* p = base;
   for (int l = 0; l < 8; ++l) { a.h[l] = p; p += m * W_HID; }
-  a.rgb_feat = p; p += m * W_HID;
-  a.ins_feat = p; p += m * W_HID;
   a.rgb_hid = p; p += m * (W_HID / 2);
   a.ins_hid = p; p += m * (W_HID / 2);
   a.emb = p; p += m * CH_IN;
@@ -146,11 +144,11 @@ int launch_mlp_simt(const NetParams& p, const float* x, const float* rays_o, con
 int launch_composite_backward(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all,
                               const float* g_rgb, const float* g_depth, const float* g_acc, const float* g_ins,
                               const float* g_weights, float* d_raw, int accumulate, cudaStream_t st);
-// feats_missing != 0: the forward that filled `acts` did not materialise rgb_feat / ins_feat (tensor-core kernel, folded
-// heads); the backward recomputes those two planes from h7 first.
+// flags: bit 0 = the forward that filled `acts` wrote the ReLU bit planes (tensor-core kernel; otherwise the backward derives
+// them from the saved activations first), bit 1 = grads are already zero.
 struct UmmaWeights;
-int launch_mlp_backward(const NetParams& p, const UmmaWeights* packed, float* acts, const float* d_out, int64_t m, float* const* grads,
-                        float* scratch, int feats_missing, cudaStream_t st);
+int launch_mlp_backward(const NetParams& p, const UmmaWeights& packed, float* acts, const float* d_out, int64_t m, float* const* grads,
+                        float* scratch, int flags, cudaStream_t st);
 // Gradient chain (bwd_chain.cu)
 int launch_mask_bits(float* acts, int64_t m, cudaStream_t st);
 int launch_bwd_heads(const NetParams& p, const float* d_out, int64_t m, const uint16_t* bits, float* s12, cudaStream_t st);
@@ -159,11 +157,10 @@ int launch_bwd_chain(const UmmaWeights& w, const NetParams& p, const float* s1, 
 size_t mlp_backward_scratch_floats(int64_t m);
 
 // Tensor-core GEMMs of the backward (gemm_umma.cu): split-bf16 three-pass wgmma kernels for the wide layer shapes.
-bool gemm_nn_tc_supported(int N, int K, int ldc, const float* C, const float* mask);
 bool gemm_tn_tc_supported(int N, int K);
 // mask_bits: 1-bit ReLU mask of the output, [16 groups][M] uint16 (one plane of ActPlanes::bits), or NULL.
 int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C, int ldc, int64_t M, int N, int accumulate,
-                      const float* mask, const float* bias, int w_kmajor, cudaStream_t st, const uint16_t* mask_bits = nullptr);
+                      const uint16_t* mask_bits, cudaStream_t st);
 // One product of a batched dW launch (gemm_umma.cu): C[N, K] += A[M, N]^T B[M, K]; b_cm != 0: B is column-major with that column
 // stride; transpose: A is the wide operand and the result goes to C[K, N].
 constexpr int TN_MAX_BATCH = 8;
@@ -173,8 +170,6 @@ struct TnProblem {
   int lda, ldb, ldc, K, transpose;
 };
 int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, cudaStream_t st);
-int launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* C, int ldc, float* colsum, int64_t M, int N, int K,
-                      int transpose, cudaStream_t st, int64_t b_cm = 0);
 int gemm_tc_check_status(cudaStream_t st);
 
 // Emptiness regulariser (penalizer.cu)

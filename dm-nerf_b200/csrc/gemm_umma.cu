@@ -1,7 +1,7 @@
 // Warpgroup-MMA (wgmma) GEMM kernels for the training backward of the DM_NeRF network (networks/dm_nerf.py:80-106
 // differentiated, driven by train_dmsr.py:62-64): the two wide GEMM shapes of every layer,
 //
-//   gemm_nn:  dX[M, 256]  (+)= dY[M, N] * W[N, 256]            (N = 128 or 256; optional ReLU mask from the saved activation)
+//   gemm_nn:  dX[M, 256]  (+)= dY[M, N] * W[N, 256]            (N = 128 or 256; optional ReLU mask from the saved bit planes)
 //   gemm_tn:  dW[NA, 256]  +=  dY[M, NA]^T * X[M, 256]          (NA = 128 or 256; contraction over the M samples)
 //
 // with the same fp32-grade arithmetic as the forward kernel: every fp32 operand is split into bf16 hi + bf16 lo and each
@@ -64,40 +64,35 @@ __device__ __forceinline__ void store_unit(const Unit& u, uint8_t* hi, uint8_t* 
 
 __device__ __forceinline__ void fail(int32_t* status, int code) { atomicCAS(status, 0, code); }
 
-// ------------------------------------------------------------------------------------------------ gemm_nn / gemm_nt
-// W_KMAJOR = false:  C[M, 256] (+)= A[M, N] * W[N, 256]                (dX = dY W; W rows are the contraction index)
-// W_KMAJOR = true:   C[M, 256]   =  A[M, N] * W[256, N]^T + bias       (y = x W^T + b: rebuilds the feature planes)
-// N = 64 * NCH.  The weight matrix is the same for every tile, so it is split ONCE per call into a packed image of ready-made
-// stage blocks (pack_w_kernel) that are streamed into the stages with bulk async copies (TMA engine, mbarrier transaction
+// ------------------------------------------------------------------------------------------------ gemm_nn
+// C[M, 256] (+)= A[M, N] * W[N, 256]   (dX = dY W; W rows are the contraction index), N = 64 * NCH.
+// The weight matrix is the same for every tile, so it is split ONCE per call into a packed image of ready-made stage blocks (pack_w_kernel) that are streamed into the stages with bulk async copies (TMA engine, mbarrier transaction
 // counts, requested as soon as a stage is free); the threads only handle the activation / gradient rows.
 // Output tile [128 x 256]: warpgroup w owns rows 64 (w & 1) and columns 128 (w >> 1).
 constexpr int NN_THREADS = 512;
 constexpr uint32_t NN_A_BYTES = 128 * 128;               // one [128 x 64] slab
-constexpr uint32_t NN_W_BYTES = 256 * 128;               // the W block of a chunk: 4 slabs [64 x 64] or one slab [256 x 64]
+constexpr uint32_t NN_W_BYTES = 256 * 128;               // the W block of a chunk: 4 slabs [64 x 64]
 constexpr uint32_t NN_W_SLAB = 64 * 128;
 constexpr uint32_t NN_STAGE = 2 * NN_A_BYTES + 2 * NN_W_BYTES;          // A hi, A lo, W hi, W lo = 96 KB
 constexpr uint32_t NN_SMEM = 2 * NN_STAGE + 1024;
 constexpr int NN_UA = 128 * 8 / NN_THREADS;              // A units per thread and stage: 2
 
 // image[c] = { W_hi block, W_lo block } of contraction chunk c, in the shared-memory layout of a stage.
-template <bool W_KMAJOR>
 __global__ void pack_w_kernel(const float* __restrict__ W, int ldw, int nch, int vec_w, uint8_t* __restrict__ image) {
   const int c = blockIdx.x;
   uint8_t* w_hi = image + (size_t)c * 2 * NN_W_BYTES;
   uint8_t* w_lo = w_hi + NN_W_BYTES;
   for (int u = threadIdx.x; u < 256 * 8; u += blockDim.x) {
     Unit r;
-    if (W_KMAJOR) {
-      load_unit(r, W, ldw, u >> 3, NOUT, 64 * c + (u & 7) * 8, 64 * nch, vec_w != 0);                 // row = output column
-      store_unit(r, w_hi, w_lo, u >> 3, u & 7);
-    } else {
-      load_unit(r, W, ldw, 64 * c + ((u >> 3) & 63), 64 * nch, 64 * (u >> 9) + (u & 7) * 8, NOUT, vec_w != 0);
-      store_unit(r, w_hi + (u >> 9) * NN_W_SLAB, w_lo + (u >> 9) * NN_W_SLAB, (u >> 3) & 63, u & 7);
-    }
+    load_unit(r, W, ldw, 64 * c + ((u >> 3) & 63), 64 * nch, 64 * (u >> 9) + (u & 7) * 8, NOUT, vec_w != 0);
+    store_unit(r, w_hi + (u >> 9) * NN_W_SLAB, w_lo + (u >> 9) * NN_W_SLAB, (u >> 3) & 63, u & 7);
   }
 }
 
-template <int NCH, bool W_KMAJOR>
+// mask (fp32 ReLU mask sharing ldc) and bias are always NULL: without these two branches nvcc schedules the epilogue so that
+// the accumulating N = 128 launch of the gradient chain takes twice as long (H100 80GB HBM3 at 700 W: 264 -> 515 us per call
+// at M = 196608), which outweighs the 5 % the N = 256 launches gain.  Keep them until the epilogue is restructured.
+template <int NCH>
 __global__ void __launch_bounds__(NN_THREADS, 1) gemm_nn_tc_kernel(const float* __restrict__ A, int lda, const uint8_t* __restrict__ wimage,
                                                                    float* __restrict__ C, int ldc, int64_t M, int accumulate,
                                                                    const float* __restrict__ mask, const uint16_t* __restrict__ mbits,
@@ -164,12 +159,11 @@ __global__ void __launch_bounds__(NN_THREADS, 1) gemm_nn_tc_kernel(const float* 
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
         const uint64_t da_hi = make_sdesc_sw128(sa_hi + ks * 32), da_lo = make_sdesc_sw128(sa_lo + ks * 32);
-        const uint64_t db_hi = W_KMAJOR ? make_sdesc_sw128(sw_hi + ks * 32) : sdesc(sw_hi + ks * 2048, NN_W_SLAB, 1024);
-        const uint64_t db_lo = W_KMAJOR ? make_sdesc_sw128(sw_lo + ks * 32) : sdesc(sw_lo + ks * 2048, NN_W_SLAB, 1024);
-        constexpr int TB = W_KMAJOR ? 0 : 1;
-        wgmma_n128<0, TB>(acc, da_hi, db_hi, (c == 0 && ks == 0) ? 0u : 1u);
-        wgmma_n128<0, TB>(acc, da_lo, db_hi, 1u);
-        wgmma_n128<0, TB>(acc, da_hi, db_lo, 1u);
+        const uint64_t db_hi = sdesc(sw_hi + ks * 2048, NN_W_SLAB, 1024);
+        const uint64_t db_lo = sdesc(sw_lo + ks * 2048, NN_W_SLAB, 1024);
+        wgmma_n128<0, 1>(acc, da_hi, db_hi, (c == 0 && ks == 0) ? 0u : 1u);
+        wgmma_n128<0, 1>(acc, da_lo, db_hi, 1u);
+        wgmma_n128<0, 1>(acc, da_hi, db_lo, 1u);
       }
       wg_commit();
     }
@@ -395,15 +389,12 @@ static int vec4_ok(const void* p, int ld) { return ((uintptr_t)p % 16 == 0) && (
 
 }  // namespace tg
 
-// Shapes the tensor-core kernels are specialised for (everything else stays on the fp32 CUDA-core kernels of backward.cu).
-bool gemm_nn_tc_supported(int N, int K, int ldc, const float* C, const float* mask) {
-  return (N == 128 || N == 256) && K == 256 && ldc % 2 == 0 && ((uintptr_t)C % 8 == 0) && (!mask || (uintptr_t)mask % 8 == 0);
-}
+// Shapes the dW kernel is specialised for (the rest goes to the fp32 CUDA-core kernels of backward.cu).
 bool gemm_tn_tc_supported(int N, int K) { return (N == 128 || N == 256) && (K == 256 || (K >= 1 && K <= 64)); }
 
-// w_kmajor == 0: C[M,256] (+)= A[M,N] W[N,256] (mask optional);  w_kmajor != 0: C[M,256] = A[M,N] W[256,N]^T + bias.
+// C[M,256] (+)= A[M,N] W[N,256], N = 128 or 256, masked by mask_bits when given.
 int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C, int ldc, int64_t M, int N, int accumulate,
-                      const float* mask, const float* bias, int w_kmajor, cudaStream_t st, const uint16_t* mask_bits) {
+                      const uint16_t* mask_bits, cudaStream_t st) {
   using namespace tg;
   if (M <= 0) return 0;
   DevState* ds = nullptr;
@@ -412,21 +403,16 @@ int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C
   int32_t* g_status = ds->status;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
-    DMN_CUDA(cudaFuncSetAttribute(gemm_nn_tc_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NN_SMEM));
-    DMN_CUDA(cudaFuncSetAttribute(gemm_nn_tc_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NN_SMEM));
-    DMN_CUDA(cudaFuncSetAttribute(gemm_nn_tc_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NN_SMEM));
+    DMN_CUDA(cudaFuncSetAttribute(gemm_nn_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NN_SMEM));
+    DMN_CUDA(cudaFuncSetAttribute(gemm_nn_tc_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NN_SMEM));
   }
-  DMN_CHECK(!w_kmajor || N == 256, "gemm_nt(tc): contraction width %d not supported", N);
-  DMN_CHECK(!bias || (uintptr_t)bias % 8 == 0, "gemm(tc): bias must be 8-byte aligned");
   const int64_t tiles = (M + 127) / 128;
   const unsigned grid = (unsigned)(tiles < ds->sms ? tiles : ds->sms);
   const int va = vec4_ok(A, lda), vw = vec4_ok(W, ldw), nch = N / 64;
-  if (w_kmajor) pack_w_kernel<true><<<nch, 512, 0, st>>>(W, ldw, nch, vw, wimage);
-  else pack_w_kernel<false><<<nch, 512, 0, st>>>(W, ldw, nch, vw, wimage);
+  pack_w_kernel<<<nch, 512, 0, st>>>(W, ldw, nch, vw, wimage);
   DMN_LAUNCH_OK();
-  if (w_kmajor) gemm_nn_tc_kernel<4, true><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, mask, mask_bits, bias, va, g_status);
-  else if (N == 128) gemm_nn_tc_kernel<2, false><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, mask, mask_bits, bias, va, g_status);
-  else gemm_nn_tc_kernel<4, false><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, mask, mask_bits, bias, va, g_status);
+  if (N == 128) gemm_nn_tc_kernel<2><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, nullptr, mask_bits, nullptr, va, g_status);
+  else gemm_nn_tc_kernel<4><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, nullptr, mask_bits, nullptr, va, g_status);
   DMN_LAUNCH_OK();
   return 0;
 }
@@ -481,15 +467,6 @@ int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, cud
   reduce_partials_kernel<<<dim3((N * NB / 4 + 255) / 256, n), 256, 0, st>>>(scratch, batch, N, NB);
   DMN_LAUNCH_OK();
   return 0;
-}
-
-// The single product C[N, K] += A[M, N]^T B[M, K] (a batch of one: every SM takes a slice of the samples).
-int launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* C, int ldc, float* colsum, int64_t M, int N, int K,
-                      int transpose, cudaStream_t st, int64_t b_cm) {
-  TnProblem pr;
-  pr.A = A; pr.lda = lda; pr.B = B; pr.ldb = ldb; pr.C = C; pr.ldc = ldc; pr.colsum = colsum; pr.K = K; pr.transpose = transpose;
-  pr.b_cm = b_cm;
-  return launch_gemm_tn_tc_batch(&pr, 1, M, N, st);
 }
 
 // Asynchronous failure word of the GEMM kernels (0 = fine); checked by dmnerf_sync_check.

@@ -162,9 +162,9 @@ mlp_simt_kernel(NetParams p, const float* __restrict__ x, const float* __restric
     // ---- density (dm_nerf.py:101) -> channel 3
     head(X, LDX, W_HID, p.w[L_DENSITY], p.b[L_DENSITY], 1, orow, C, 3, rows_valid);
     // ---- instance branch (dm_nerf.py:95-99,103) -> channels 4..
-    layer<false>(X, LDX, W_HID, p.w[L_INS_FEAT], p.b[L_INS_FEAT], W_HID, B, LDB, Wt, ACT(ap.ins_feat, W_HID));
+    layer<false>(X, LDX, W_HID, p.w[L_INS_FEAT], p.b[L_INS_FEAT], W_HID, B, LDB, Wt);
     // ---- colour branch (dm_nerf.py:89-93,102) -> channels 0..2   (h is dead after this layer: in place)
-    layer<false>(X, LDX, W_HID, p.w[L_RGB_FEAT], p.b[L_RGB_FEAT], W_HID, X, LDX, Wt, ACT(ap.rgb_feat, W_HID));
+    layer<false>(X, LDX, W_HID, p.w[L_RGB_FEAT], p.b[L_RGB_FEAT], W_HID, X, LDX, Wt);
     for (int idx = tid; idx < TM * CH_DIR; idx += NT) {            // cat([rgb_feature, input_dirs])
       const int r = idx / CH_DIR, c = idx % CH_DIR;
       X[r * LDX + W_HID + c] = E[r * LDE + CH_POS + c];

@@ -176,22 +176,23 @@ DMNERF_API int dmnerf_act_floats_per_sample(void);
 DMNERF_API int64_t dmnerf_mlp_backward_scratch_floats(int64_t m);
 
 /* DM_NeRF.forward with saved activations.  Pass either x [M,90] (rays_* NULL) or rays_o/rays_d [N,3] + z [N,S] (x NULL,
- * m = N*S).  out [M,C].  impl: DMNERF_IMPL_SIMT = exact fp32; DMNERF_IMPL_UMMA / AUTO = the tensor-core kernel, whose folded heads
- * do not produce the rgb_feature / ins_feature planes -- pass feats_missing = 1 to dmnerf_mlp_backward in that case.  Both
- * kernels also keep the ReLU masks (1 bit per unit) the fused gradient chain of the backward reads. */
+ * m = N*S).  out [M,C].  impl: DMNERF_IMPL_SIMT = exact fp32; DMNERF_IMPL_UMMA / AUTO = the tensor-core kernel, which also
+ * keeps the ReLU masks (1 bit per unit) the gradient chain of the backward reads -- pass bit 0 of `flags` to
+ * dmnerf_mlp_backward in that case.  The exact-fp32 kernel does not write the masks; the backward derives them from the saved
+ * activations. */
 DMNERF_API int dmnerf_mlp_forward_train(dmnerf_ctx* ctx, int net, const float* x, const float* rays_o, const float* rays_d,
                              const float* z, int64_t m, int s, float* out, float* acts, int impl, void* stream);
 
 /* Gradient of a scalar loss w.r.t. the 30 parameters of network `net` given d_out = dL/d(out) [M,C] and the activations
  * saved by dmnerf_mlp_forward_train.  grads: 30 device buffers (state_dict order, parameter shapes), overwritten.
  * Gradient routing follows the reference (networks/dm_nerf.py:95: the instance branch reads h.detach()).
- * scratch: dmnerf_mlp_backward_scratch_floats(m) floats.  feats_missing is a flag word: bit 0 = the forward did not write the
- * feature planes (tensor-core forward), bit 1 = the caller has already zero-filled `grads` (one fill instead of 30 memsets).
- * M >= 512: the heads are folded like in the forward, one masked split-bf16 wgmma GEMM per layer carries the gradient
- * through the trunk and batched wgmma GEMMs form the weight gradients; smaller batches and DMNERF_BWD_IMPL=simt use fp32
- * CUDA-core kernels. */
+ * scratch: dmnerf_mlp_backward_scratch_floats(m) floats.  flags is a flag word: bit 0 = the forward wrote the ReLU bit planes
+ * (tensor-core forward), bit 1 = the caller has already zero-filled `grads` (one fill instead of 30 memsets).
+ * The heads are folded like in the forward, one masked split-bf16 wgmma GEMM per layer carries the gradient through the trunk
+ * and batched wgmma GEMMs form the weight gradients (on the CUDA cores for ins_linear with more than 64 instance logits), for
+ * any M. */
 DMNERF_API int dmnerf_mlp_backward(dmnerf_ctx* ctx, int net, float* acts, const float* d_out, int64_t m, float* const* grads,
-                        float* scratch, int feats_missing, void* stream);
+                        float* scratch, int flags, void* stream);
 
 /* Backward of render_train (networks/render.py:6-28): upstream gradients of rgb_map [N,3], depth_map [N], acc_map [N],
  * ins_map [N, C-5 | C-4] and weights [N,S] (any may be NULL) -> d_raw [N,S,C] (added to d_raw when accumulate != 0).

@@ -147,10 +147,11 @@ def test_dropin_training_loop_runs_and_rebinds_updated_weights():
 
 
 @pytest.mark.parametrize("m", [300, 128 * 5])
-def test_tensor_core_training_forward_saves_the_reference_activations(m):
+def test_tensor_core_training_forward_saves_only_the_planes_the_backward_reads(m):
     """dmnerf_mlp_forward_train(impl=UMMA, rays mode): the planes kept for the backward -- the embedded inputs produced by the
     kernel's own branch-free sin/cos (dm_nerf.py:37-38), H0..H7 (dm_nerf.py:84-87) and the two hidden head activations
-    (dm_nerf.py:93,99) -- against the oracle on the same rays; a ragged last tile included."""
+    (dm_nerf.py:93,99) -- against the oracle on the same rays; a ragged last tile included.  The layout holds these planes and
+    the ReLU bit planes and nothing else."""
     from dmnerf_b200.engine import get_context
     wl = synth.workload("dmsr_study")
     w = synth.make_weights(11, 13)
@@ -173,8 +174,7 @@ def test_tensor_core_training_forward_saves_the_reference_activations(m):
     acts = acts.cpu().numpy()
     off = 0
     planes = {}
-    for name, width in [("h%d" % l, 256) for l in range(8)] + [("rgb_feat", 256), ("ins_feat", 256), ("rgb_hid", 128),
-                                                              ("ins_hid", 128), ("emb", 90)]:
+    for name, width in [("h%d" % l, 256) for l in range(8)] + [("rgb_hid", 128), ("ins_hid", 128), ("emb", 90)]:
         block = acts[off:off + m * width]
         planes[name] = block.reshape(width, m).T if name == "emb" else block.reshape(m, width)      # emb is stored column-major
         off += m * width
@@ -206,6 +206,7 @@ def test_tensor_core_training_forward_saves_the_reference_activations(m):
     assert scale_err(raw.cpu().numpy(), out) <= 1e-4
     # ReLU masks, 1 bit per unit (what the fused gradient chain reads): [10 planes][16 groups][m] uint16, rows fastest, after
     # the embedded inputs; bit c of group g = unit 16 g + c
+    assert apf * m == off + 10 * m * 8                       # nothing saved beyond these planes
     bits = acts[off:off + 10 * m * 8].view(np.uint16).reshape(10, 16, m)
     for pl, name in enumerate(["h%d" % l for l in range(8)] + ["rgb_hid", "ins_hid"]):
         width = planes[name].shape[1]
@@ -214,13 +215,14 @@ def test_tensor_core_training_forward_saves_the_reference_activations(m):
         assert np.array_equal(unpacked.astype(bool), planes[name] > 0), name
 
 
+@pytest.mark.parametrize("m", [1, 37, 511, 1333])
 @pytest.mark.parametrize("ins_num", [13, 59, 127])
-def test_mlp_backward_tensor_core_gemms(ins_num):
-    """Batches of >= 512 samples run the backward on the tensor cores: the split-bf16 wgmma dX and dW GEMMs (gemm_umma.cu) layer
+def test_mlp_backward_tensor_core_gemms(ins_num, m):
+    """The backward runs on the tensor cores for every batch size: the split-bf16 wgmma dX and dW GEMMs (gemm_umma.cu) layer
     by layer; with the exact-fp32 forward the 30 parameter gradients must still agree with torch autograd on the oracle to fp32
-    noise.  1333 samples: ten full 128-row tiles + a ragged one, 32-sample stages with a ragged tail; ins_num = 127 is the widest
-    object head the library accepts (128 instance logits)."""
-    m = 1333
+    noise.  1333 samples: ten full 128-row tiles + a ragged one, 32-sample stages with a ragged tail; 1, 37 and 511 samples: a
+    single sample, a tail shorter than one 32-sample stage, one row short of four full tiles.  ins_num = 127 is the widest
+    object head the library accepts (128 instance logits; its weight gradient runs on the fp32 CUDA-core kernels)."""
     w = synth.make_weights(21, ins_num)
     p = O.to_torch(w)
     for v in p.values():
