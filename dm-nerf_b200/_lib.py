@@ -1,12 +1,16 @@
 """ctypes binding of libdmnerf_b200.so (C ABI: include/dmnerf_b200.h).
 
-No torch types cross the boundary: tensors are passed as raw device pointers (`tensor.data_ptr()`)
-plus sizes and the current CUDA stream handle.  There is NO CPU fallback: if the shared library is
+No torch types cross the boundary: tensors are passed as raw pointers (`ptr` / `ptrs`, which check dtype and
+contiguity: ctypes itself checks nothing) plus sizes and the current CUDA stream handle; host-side matrices and masks
+are built by `floats` / `doubles` / `camera` / `keep_mask`.  There is NO CPU fallback: if the shared library is
 missing or a call fails, a RuntimeError is raised with the library's own message.
 """
 import ctypes as C
 import os
 import threading
+
+import numpy as np
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # DMNERF_LIB_PATH: diagnostics builds of the same ABI (tools/kprof.py); the default is the in-tree product library
@@ -160,15 +164,58 @@ def check(rc, what):
         raise RuntimeError("%s failed (status %d): %s" % (what, rc, (msg or b"").decode("utf-8", "replace")))
 
 
-def ptr(t):
-    """Device (or host) pointer of a contiguous float32 tensor, or None."""
-    if t is None:
-        return None
-    import torch
-    if not t.is_contiguous() or t.dtype != torch.float32:
-        raise RuntimeError("native call needs a contiguous float32 tensor (got %s, contiguous=%s): convert it into a local "
-                           "first so the copy outlives the launch" % (t.dtype, t.is_contiguous()))
-    return C.c_void_p(t.data_ptr())
+def _addr(t, dtype, strided=False):
+    if t.dtype != dtype or not (strided or t.is_contiguous()):
+        raise RuntimeError("native call needs a contiguous %s tensor (got %s, contiguous=%s): convert it into a local "
+                           "first so the copy outlives the launch" % (str(dtype).replace("torch.", ""), t.dtype,
+                                                                      t.is_contiguous()))
+    return t.data_ptr()
+
+
+def ptr(t, dtype=torch.float32, strided=False):
+    """Device (or host) pointer of a contiguous `dtype` tensor, or None.  strided=True is for an argument whose row stride
+    is passed to the entry point beside it: only the dtype is checked."""
+    return None if t is None else C.c_void_p(_addr(t, dtype, strided))
+
+
+def ptrs(tensors, dtype=torch.float32):
+    """Host array of the pointers of `tensors` (each checked like `ptr`), for the entry points that take `T* const*`."""
+    return (C.c_void_p * len(tensors))(*[_addr(t, dtype) for t in tensors])
+
+
+def _host_array(ctype, dtype, a, n):
+    a = np.asarray(a.detach().cpu().double().numpy() if torch.is_tensor(a) else a, dtype=dtype).reshape(-1)
+    if a.size != n:
+        raise ValueError("expected %d values, got %d" % (n, a.size))
+    return (ctype * n)(*a.tolist())
+
+
+def floats(a, n):
+    """Host float array of the n values of `a` (array, nested list or tensor, read row-major); ValueError for another count."""
+    return _host_array(C.c_float, np.float32, a, n)
+
+
+def doubles(a, n):
+    """`floats` in float64."""
+    return _host_array(C.c_double, np.float64, a, n)
+
+
+def camera(K, c2w):
+    """Host arrays of a camera entry point: the intrinsics K (3x3: 9 values) and the top 3x4 of the pose c2w (12 values)."""
+    pose = c2w.detach()[:3, :4] if torch.is_tensor(c2w) else np.asarray(c2w)[:3, :4]
+    return floats(K, 9), floats(pose, 12)
+
+
+def keep_mask(words):
+    """The 4-word object-selection mask (objects.object_mask) as the ABI's host uint32[4]."""
+    return (C.c_uint32 * 4)(*words)
+
+
+def need_cuda(what, *ts):
+    """RuntimeError unless every tensor of `ts` that is not None is a CUDA tensor."""
+    for t in ts:
+        if t is not None and not (torch.is_tensor(t) and t.is_cuda):
+            raise RuntimeError("%s: expected CUDA tensors (no CPU fallback)" % what)
 
 
 def launch_count():

@@ -32,8 +32,7 @@ def mlp_forward(model, x, impl=_lib.IMPL_AUTO):
     if x2.shape[1] != 90:
         raise RuntimeError("DM_NeRF.forward: expected 90 input channels (63 pos + 27 dir), got %d" % x2.shape[1])
     out = torch.empty((x2.shape[0], 4 + ins_num + 1), device=x.device, dtype=torch.float32)
-    _lib.check(ctx.lib.dmnerf_mlp_forward(ctx.handle, slot, _lib.ptr(x2), x2.shape[0], _lib.ptr(out), impl, ctx.stream()),
-               "dmnerf_mlp_forward")
+    ctx.call("dmnerf_mlp_forward", ctx.handle, slot, _lib.ptr(x2), x2.shape[0], _lib.ptr(out), impl)
     return out.reshape(*x.shape[:-1], out.shape[-1])
 
 
@@ -49,8 +48,7 @@ def mlp_forward_rays(model, rays_o, rays_d, z, impl=_lib.IMPL_AUTO):
     if ro.shape[0] != n or rd.shape[0] != n:
         raise RuntimeError("mlp_forward_rays: %d / %d rays for %d depth rows" % (ro.shape[0], rd.shape[0], n))
     out = torch.empty((n, s, 4 + ins_num + 1), device=z.device, dtype=torch.float32)
-    _lib.check(ctx.lib.dmnerf_mlp_forward_rays(ctx.handle, slot, _lib.ptr(ro), _lib.ptr(rd), _lib.ptr(zz),
-                                               n, s, _lib.ptr(out), impl, ctx.stream()), "dmnerf_mlp_forward_rays")
+    ctx.call("dmnerf_mlp_forward_rays", ctx.handle, slot, _lib.ptr(ro), _lib.ptr(rd), _lib.ptr(zz), n, s, _lib.ptr(out), impl)
     return out
 
 
@@ -65,6 +63,5 @@ def mlp_forward_points(model, pts, viewdirs=None, impl=_lib.IMPL_AUTO):
     p2 = pts.reshape(-1, 3).contiguous().float()
     v2 = torch.zeros_like(p2) if viewdirs is None else viewdirs.reshape(-1, 3).contiguous().float()
     out = torch.empty((p2.shape[0], 4 + ins_num + 1), device=pts.device, dtype=torch.float32)
-    _lib.check(ctx.lib.dmnerf_mlp_forward_points(ctx.handle, slot, _lib.ptr(p2), _lib.ptr(v2), p2.shape[0], _lib.ptr(out), impl,
-                                                 ctx.stream()), "dmnerf_mlp_forward_points")
+    ctx.call("dmnerf_mlp_forward_points", ctx.handle, slot, _lib.ptr(p2), _lib.ptr(v2), p2.shape[0], _lib.ptr(out), impl)
     return out.reshape(*pts.shape[:-1], out.shape[-1])

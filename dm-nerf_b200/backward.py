@@ -7,13 +7,13 @@ trunk layer, batched wgmma weight gradients).  Gradient topology is the referenc
 (render.py:68), the instance map sees detached weights (render.py:22-23), the instance branch sees h.detach()
 (dm_nerf.py:95), rays / depths carry no gradient.
 """
-import ctypes as C
 import os
 
 import torch
 
 from . import _lib
 from .engine import get_context, ordered_params
+from .render import bind_pair, coarse_depths, reference_draws
 
 # Kernel used by the training forward: the tensor-core kernel by default ("umma"), or the exact-fp32 CUDA-core kernel ("simt").
 TRAIN_IMPL = _lib.IMPL_SIMT if os.environ.get("DMNERF_TRAIN_IMPL", "umma").lower() == "simt" else _lib.IMPL_UMMA
@@ -43,9 +43,8 @@ def _mlp_backward(ctx, slot, acts, d_out, m, params, masks_saved):
     flags = int(masks_saved) | 2            # bit 0 = ReLU bit planes saved by the forward, bit 1 = gradient buffers already zero
     n_scratch = int(ctx.lib.dmnerf_mlp_backward_scratch_floats(m))
     scratch = torch.empty(max(n_scratch, 1), device=d_out.device, dtype=torch.float32)
-    arr = (C.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
-    _lib.check(ctx.lib.dmnerf_mlp_backward(ctx.handle, slot, _lib.ptr(acts), _lib.ptr(d_out), m, arr, _lib.ptr(scratch),
-                                           flags, ctx.stream()), "dmnerf_mlp_backward")
+    ctx.call("dmnerf_mlp_backward", ctx.handle, slot, _lib.ptr(acts), _lib.ptr(d_out), m, _lib.ptrs(grads), _lib.ptr(scratch),
+             flags)
     return grads
 
 
@@ -63,8 +62,8 @@ class MLPFunction(torch.autograd.Function):
         out = torch.empty((m, 4 + ins_num + 1), device=x.device, dtype=torch.float32)
         acts = torch.empty(max(m * ctx.lib.dmnerf_act_floats_per_sample(), 1), device=x.device, dtype=torch.float32)
         impl = _train_impl(impl)
-        _lib.check(ctx.lib.dmnerf_mlp_forward_train(ctx.handle, slot, _lib.ptr(x2), None, None, None, m, 1, _lib.ptr(out),
-                                                    _lib.ptr(acts), impl, ctx.stream()), "dmnerf_mlp_forward_train")
+        ctx.call("dmnerf_mlp_forward_train", ctx.handle, slot, _lib.ptr(x2), None, None, None, m, 1, _lib.ptr(out), _lib.ptr(acts),
+                 impl)
         fctx.model, fctx.m, fctx.acts, fctx.params, fctx.masks_saved = model, m, acts, params, impl != _lib.IMPL_SIMT
         return out.reshape(*x.shape[:-1], out.shape[-1])
 
@@ -103,10 +102,8 @@ class CompositeFunction(torch.autograd.Function):
         d_raw = torch.empty_like(raw)
         # converted grads stay alive across the launch (a stride-0 expand from .sum().backward() is copied by _f32)
         keep = [_f32(g) if g is not None else None for g in (g_rgb, g_depth, g_ins, g_w)]
-        _lib.check(ctx.lib.dmnerf_composite_backward(_lib.ptr(raw), _lib.ptr(z), _lib.ptr(rd), n, s, c, int(fctx.keep),
-                                                     _lib.ptr(keep[0]), _lib.ptr(keep[1]), None, _lib.ptr(keep[2]),
-                                                     _lib.ptr(keep[3]), _lib.ptr(d_raw), 0,
-                                                     ctx.stream()), "dmnerf_composite_backward")
+        ctx.call("dmnerf_composite_backward", _lib.ptr(raw), _lib.ptr(z), _lib.ptr(rd), n, s, c, int(fctx.keep), _lib.ptr(keep[0]),
+                 _lib.ptr(keep[1]), None, _lib.ptr(keep[2]), _lib.ptr(keep[3]), _lib.ptr(d_raw), 0)
         return d_raw, None, None, None
 
 
@@ -121,33 +118,29 @@ class RenderFunction(torch.autograd.Function):
     def forward(fctx, model_c, model_f, rays_o, rays_d, z_in, z_stride, t_rand, u, n_importance, n_c, impl, *params):
         dev = rays_o.device
         ctx = get_context(dev)
-        lib = ctx.lib
         impl = _train_impl(impl)
-        ins_num = ctx.bind(0, model_c)
-        if ctx.bind(1, model_f) != ins_num:
-            raise RuntimeError("coarse and fine networks disagree on ins_num")
+        ins_num = bind_pair(ctx, model_c, model_f)
         n, S = rays_o.shape[0], z_in.shape[-1]
         F, Cc = S + n_importance, 4 + ins_num + 1
         e = lambda *shape: torch.empty(shape, device=dev, dtype=torch.float32)
-        st = ctx.stream()
-        apf = lib.dmnerf_act_floats_per_sample()
+        apf = ctx.lib.dmnerf_act_floats_per_sample()
         o = {}
         # render.py:40-47 coarse depths
         o["z_vals_coarse"] = e(n, S)
-        _lib.check(lib.dmnerf_stratify(_lib.ptr(z_in), z_stride, _lib.ptr(t_rand), n, S, _lib.ptr(o["z_vals_coarse"]), st), "dmnerf_stratify")
+        ctx.call("dmnerf_stratify", _lib.ptr(z_in), z_stride, _lib.ptr(t_rand), n, S, _lib.ptr(o["z_vals_coarse"]))
         saved = []
         for net, zkey, tag, ns in ((0, "z_vals_coarse", "coarse", S), (1, "z_vals_fine", "fine", F)):
             if net == 1:       # render.py:66-70 importance sampling on the (detached) coarse weights
                 o["z_vals_fine"] = e(n, F)
-                _lib.check(lib.dmnerf_hier_sample(_lib.ptr(o["z_vals_coarse"]), _lib.ptr(o["weights_coarse"]), _lib.ptr(u), n, S,
-                                                  n_importance, _lib.ptr(o["z_vals_fine"]), st), "dmnerf_hier_sample")
+                ctx.call("dmnerf_hier_sample", _lib.ptr(o["z_vals_coarse"]), _lib.ptr(o["weights_coarse"]), _lib.ptr(u), n, S,
+                         n_importance, _lib.ptr(o["z_vals_fine"]))
             raw = e(n, ns, Cc)
             acts = e(max(n * ns * apf, 1))
-            _lib.check(lib.dmnerf_mlp_forward_train(ctx.handle, net, None, _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(o[zkey]),
-                                                    n * ns, ns, _lib.ptr(raw), _lib.ptr(acts), impl, st), "dmnerf_mlp_forward_train")
+            ctx.call("dmnerf_mlp_forward_train", ctx.handle, net, None, _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(o[zkey]), n * ns,
+                     ns, _lib.ptr(raw), _lib.ptr(acts), impl)
             rgb, w, depth, acc, ins = e(n, 3), e(n, ns), e(n), e(n), e(n, ins_num)
-            _lib.check(lib.dmnerf_composite(_lib.ptr(raw), _lib.ptr(o[zkey]), _lib.ptr(rays_d), n, ns, Cc, 0, _lib.ptr(rgb),
-                                            _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc), st), "dmnerf_composite")
+            ctx.call("dmnerf_composite", _lib.ptr(raw), _lib.ptr(o[zkey]), _lib.ptr(rays_d), n, ns, Cc, 0, _lib.ptr(rgb), _lib.ptr(w),
+                     _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc))
             o["raw_" + tag], o["rgb_" + tag], o["weights_" + tag] = raw, rgb, w
             o["depth_" + tag], o["acc_" + tag], o["ins_" + tag] = depth, acc, ins
             saved.append(acts)
@@ -166,7 +159,6 @@ class RenderFunction(torch.autograd.Function):
         gd = dict(zip(_OUT_KEYS, g))
         rays_d, z_c, z_f, raw_c, raw_f = fctx.saved_tensors
         ctx = get_context(rays_d.device)
-        lib, st = ctx.lib, ctx.stream()
         ctx.bind(0, fctx.models[0]); ctx.bind(1, fctx.models[1])
         n, Cc = fctx.n, fctx.C
         all_grads = []
@@ -177,9 +169,8 @@ class RenderFunction(torch.autograd.Function):
             else:
                 d_raw, accumulate = torch.empty_like(raw), 0
             keep = [_f32(gd[k + tag]) if gd[k + tag] is not None else None for k in ("rgb_", "depth_", "acc_", "ins_", "weights_")]
-            _lib.check(lib.dmnerf_composite_backward(_lib.ptr(raw), _lib.ptr(z), _lib.ptr(rays_d), n, ns, Cc, 0,
-                                                     _lib.ptr(keep[0]), _lib.ptr(keep[1]), _lib.ptr(keep[2]), _lib.ptr(keep[3]),
-                                                     _lib.ptr(keep[4]), _lib.ptr(d_raw), accumulate, st), "dmnerf_composite_backward")
+            ctx.call("dmnerf_composite_backward", _lib.ptr(raw), _lib.ptr(z), _lib.ptr(rays_d), n, ns, Cc, 0, _lib.ptr(keep[0]),
+                     _lib.ptr(keep[1]), _lib.ptr(keep[2]), _lib.ptr(keep[3]), _lib.ptr(keep[4]), _lib.ptr(d_raw), accumulate)
             params = fctx.params[:fctx.n_c] if net == 0 else fctx.params[fctx.n_c:]
             all_grads += _mlp_backward(ctx, net, fctx.acts[net], d_raw.reshape(n * ns, Cc), n * ns, params, fctx.masks_saved)
         fctx.acts = None
@@ -193,19 +184,9 @@ def render_rays_grad(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, pe
     if dev.type != "cuda":
         raise RuntimeError("dm_nerf: expected CUDA tensors (no CPU fallback)")
     rays_o, rays_d = _f32(rays_o.reshape(-1, 3)), _f32(rays_d.reshape(-1, 3))
-    n, S = rays_o.shape[0], z_vals_coarse.shape[-1]
-    if (z_vals_coarse.dim() == 2 and z_vals_coarse.shape[0] > 1 and z_vals_coarse.stride(0) == 0) or z_vals_coarse.dim() == 1:
-        z_in, z_stride = _f32(z_vals_coarse[0] if z_vals_coarse.dim() == 2 else z_vals_coarse), 0
-    else:
-        z_in, z_stride = _f32(z_vals_coarse), S
-    if perturb > 0.0:
-        if t_rand is None:
-            t_rand = torch.rand((n, S), device=dev)          # render.py:46
-        if u is None:
-            u = torch.rand((n, N_importance), device=dev)    # helpers.py:135
-        t_rand, u = _f32(t_rand), _f32(u)
-    else:
-        t_rand = u = None
+    n = rays_o.shape[0]
+    z_in, z_stride = coarse_depths(z_vals_coarse, n)
+    t_rand, u = reference_draws(perturb, n, z_vals_coarse.shape[-1], N_importance, dev, t_rand, u)
     pc, _ = ordered_params(model_coarse)
     pf, _ = ordered_params(model_fine)
     outs = RenderFunction.apply(model_coarse, model_fine, rays_o, rays_d, z_in, z_stride, t_rand, u, N_importance, len(pc),

@@ -24,8 +24,7 @@ class Embedder:
         x = inputs.reshape(-1, 3).contiguous().float()
         out = torch.empty((x.shape[0], self.out_dim), device=x.device, dtype=torch.float32)
         ctx = get_context(x.device)
-        _lib.check(ctx.lib.dmnerf_posenc(_lib.ptr(x), x.shape[0], self.num_freqs, _lib.ptr(out), ctx.stream()),
-                   "dmnerf_posenc")
+        ctx.call("dmnerf_posenc", _lib.ptr(x), x.shape[0], self.num_freqs, _lib.ptr(out))
         return out.reshape(*inputs.shape[:-1], self.out_dim)
 
 

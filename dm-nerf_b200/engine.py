@@ -77,7 +77,8 @@ class Context:
         self._keepalive = [None, None]
 
     def stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.index).cuda_stream)
+        # every native call looks the stream up: take the raw handle rather than building a torch.cuda.Stream each time
+        return C.c_void_p(torch._C._cuda_getCurrentRawStream(self.index))
 
     def bind(self, slot, model):
         params, ins_num = ordered_params(model)
@@ -87,16 +88,19 @@ class Context:
         for p in params:
             if p.dtype != torch.float32 or not p.is_cuda or not p.is_contiguous() or p.device.index != self.index:
                 raise RuntimeError("DM_NeRF parameters must be contiguous float32 tensors on cuda:%d" % self.index)
-        arr = (C.c_void_p * len(params))(*[p.data_ptr() for p in params])
-        _lib.check(self.lib.dmnerf_set_weights(self.handle, slot, arr, len(params), ins_num, self.stream()),
-                   "dmnerf_set_weights")
+        self.call("dmnerf_set_weights", self.handle, slot, _lib.ptrs(params), len(params), ins_num)
         self._bound[slot] = key
         self._keepalive[slot] = params
         return ins_num
 
+    def call(self, name, *args):
+        """Call the status-returning entry point `name` with `args` and the current stream; RuntimeError on a non-zero
+        status, with the library's message."""
+        _lib.check(getattr(self.lib, name)(*args, self.stream()), name)
+
     def sync_check(self):
         """Synchronise the current stream and raise if any native kernel reported an asynchronous failure."""
-        _lib.check(self.lib.dmnerf_sync_check(self.handle, self.stream()), "dmnerf_sync_check")
+        self.call("dmnerf_sync_check", self.handle)
 
     def slot_for(self, model):
         """Slot to evaluate `model` alone (DM_NeRF.forward): reuse a slot it already occupies."""

@@ -30,9 +30,8 @@ def _costs(pred, gt_row):
     e = lambda *s: torch.empty(s, device=dev, dtype=torch.float32)
     out = {"cost_ce": e(k, k), "cost_siou": e(k, k), "tp": e(k, k), "col_sum": e(k), "row_count": e(k)}
     ctx = get_context(dev)
-    _lib.check(ctx.lib.dmnerf_hungarian_costs(_lib.ptr(pred), gt_row.data_ptr(), n, k, _lib.ptr(out["cost_ce"]),
-                                              _lib.ptr(out["cost_siou"]), _lib.ptr(out["tp"]), _lib.ptr(out["col_sum"]),
-                                              _lib.ptr(out["row_count"]), ctx.stream()), "dmnerf_hungarian_costs")
+    ctx.call("dmnerf_hungarian_costs", _lib.ptr(pred), _lib.ptr(gt_row, torch.int32), n, k, _lib.ptr(out["cost_ce"]),
+             _lib.ptr(out["cost_siou"]), _lib.ptr(out["tp"]), _lib.ptr(out["col_sum"]), _lib.ptr(out["row_count"]))
     return out
 
 
@@ -115,9 +114,8 @@ class _MatchedLoss(torch.autograd.Function):
         g3 = torch.stack([(g if g is not None else zero).reshape(()).float() for g in (g_ce, g_inv, g_siou)]).contiguous()
         d_pred = torch.empty_like(pred)
         ctx = get_context(pred.device)
-        _lib.check(ctx.lib.dmnerf_ins_loss_backward(_lib.ptr(pred), gt_row.data_ptr(), n, k, row_of_col.data_ptr(), fctx.n_valid,
-                                                    _lib.ptr(tp), _lib.ptr(col_sum), _lib.ptr(row_count), _lib.ptr(g3),
-                                                    _lib.ptr(d_pred), ctx.stream()), "dmnerf_ins_loss_backward")
+        ctx.call("dmnerf_ins_loss_backward", _lib.ptr(pred), _lib.ptr(gt_row, torch.int32), n, k, _lib.ptr(row_of_col, torch.int32),
+                 fctx.n_valid, _lib.ptr(tp), _lib.ptr(col_sum), _lib.ptr(row_count), _lib.ptr(g3), _lib.ptr(d_pred))
         return d_pred.reshape(fctx.in_shape), None, None
 
 
@@ -138,14 +136,13 @@ class _MatchedLossDevice(torch.autograd.Function):
         ctx = get_context(dev)
         gt_row = torch.empty(n, device=dev, dtype=torch.int32)
         n_valid = torch.empty(1, device=dev, dtype=torch.int32)
-        _lib.check(ctx.lib.dmnerf_ins_label_rows(labels.data_ptr(), n, k, gt_row.data_ptr(), n_valid.data_ptr(), ctx.stream()),
-                   "dmnerf_ins_label_rows")
+        ctx.call("dmnerf_ins_label_rows", _lib.ptr(labels, torch.int32), n, k, _lib.ptr(gt_row, torch.int32),
+                 _lib.ptr(n_valid, torch.int32))
         c = _costs(pred, gt_row)
         row_of_col = torch.empty(k, device=dev, dtype=torch.int32)
         losses = torch.empty(3, device=dev, dtype=torch.float32)
-        _lib.check(ctx.lib.dmnerf_hungarian_assign(_lib.ptr(c["cost_ce"]), _lib.ptr(c["cost_siou"]), _lib.ptr(c["col_sum"]),
-                                                   n_valid.data_ptr(), n, k, row_of_col.data_ptr(), _lib.ptr(losses), ctx.stream()),
-                   "dmnerf_hungarian_assign")
+        ctx.call("dmnerf_hungarian_assign", _lib.ptr(c["cost_ce"]), _lib.ptr(c["cost_siou"]), _lib.ptr(c["col_sum"]),
+                 _lib.ptr(n_valid, torch.int32), n, k, _lib.ptr(row_of_col, torch.int32), _lib.ptr(losses))
         fctx.save_for_backward(pred, gt_row, row_of_col, n_valid, c["tp"], c["col_sum"], c["row_count"])
         fctx.in_shape = pred_ins.shape
         fctx.mark_non_differentiable(n_valid, row_of_col)
@@ -160,9 +157,8 @@ class _MatchedLossDevice(torch.autograd.Function):
         g3 = torch.stack([(g if g is not None else zero).reshape(()).float() for g in (g_ce, g_inv, g_siou)]).contiguous()
         d_pred = torch.empty_like(pred)
         ctx = get_context(pred.device)
-        _lib.check(ctx.lib.dmnerf_ins_loss_backward_dev(_lib.ptr(pred), gt_row.data_ptr(), n, k, row_of_col.data_ptr(),
-                                                        n_valid.data_ptr(), _lib.ptr(tp), _lib.ptr(col_sum), _lib.ptr(row_count),
-                                                        _lib.ptr(g3), _lib.ptr(d_pred), ctx.stream()), "dmnerf_ins_loss_backward_dev")
+        ctx.call("dmnerf_ins_loss_backward_dev", _lib.ptr(pred), _lib.ptr(gt_row, torch.int32), n, k, _lib.ptr(row_of_col, torch.int32),
+                 _lib.ptr(n_valid, torch.int32), _lib.ptr(tp), _lib.ptr(col_sum), _lib.ptr(row_count), _lib.ptr(g3), _lib.ptr(d_pred))
         return d_pred.reshape(fctx.in_shape), None
 
 

@@ -48,11 +48,9 @@ def exchanger(ori_raw, tar_raws, ori_raw_pred, tar_raw_preds, move_labels):
     ctx = get_context(ori_raw.device)
     ori_label = torch.empty((n, s), device=ori_raw.device, dtype=torch.int64)
     tar_label = torch.empty((n, s), device=ori_raw.device, dtype=torch.int64)
-    tp = (C.c_void_p * m)(*[t.data_ptr() for t in tars[:m]])
-    ap = (C.c_void_p * m)(*[a.data_ptr() for a in accs[:m]])
     mv = (C.c_int * m)(*[int(v) for v in move_labels])
-    _lib.check(ctx.lib.dmnerf_exchanger(_lib.ptr(ori_raw), tp, _lib.ptr(acc_o), ap, mv, m, n, s, c, ori_label.data_ptr(),
-                                        tar_label.data_ptr(), ctx.stream()), "dmnerf_exchanger")
+    ctx.call("dmnerf_exchanger", _lib.ptr(ori_raw), _lib.ptrs(tars[:m]), _lib.ptr(acc_o), _lib.ptrs(accs[:m]), mv, m, n, s, c,
+             _lib.ptr(ori_label, torch.int64), _lib.ptr(tar_label, torch.int64))
     return ori_raw, tar_raws, ori_label, tar_label
 
 

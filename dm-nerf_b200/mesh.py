@@ -19,29 +19,6 @@ from .engine import get_context
 EXTENTS = (1.9, 7.0, 7.0)          # mesh_generator.py:26
 
 
-def _p(t, dtype):
-    if t is None:
-        return None
-    if not t.is_cuda or not t.is_contiguous() or t.dtype != dtype:
-        raise RuntimeError("native mesh call needs a contiguous CUDA %s tensor (got %s, %s)" % (dtype, t.dtype, t.device))
-    return C.c_void_p(t.data_ptr())
-
-
-def _f(t):
-    return _p(t, torch.float32)
-
-
-def _i(t):
-    return _p(t, torch.int32)
-
-
-def _doubles(a, n):
-    a = np.asarray(a, dtype=np.float64).reshape(-1)
-    if a.size != n:
-        raise ValueError("expected %d values, got %d" % (n, a.size))
-    return (C.c_double * n)(*a.tolist())
-
-
 def check_transform(scene_transform):
     """The 4x4 scene transform (inv(to_origin) of the scene's oriented bounds) as float64; a reflection is rejected."""
     T = np.asarray(scene_transform, dtype=np.float64)
@@ -59,8 +36,7 @@ def grid_points(scene_transform, dim, extents=EXTENTS, begin=0, count=None, devi
     count = dim ** 3 - begin if count is None else count
     ctx = get_context(device)
     out = torch.empty((count, 3), device=device, dtype=torch.float32)
-    _lib.check(ctx.lib.dmnerf_mesh_grid_points(_doubles(T, 16), _doubles(extents, 3), dim, begin, count, _f(out), ctx.stream()),
-               "dmnerf_mesh_grid_points")
+    ctx.call("dmnerf_mesh_grid_points", _lib.doubles(T, 16), _lib.doubles(extents, 3), dim, begin, count, _lib.ptr(out))
     return out
 
 
@@ -74,8 +50,8 @@ def occupancy_grid(model, scene_transform, grid_dim=256, extents=EXTENTS, near=4
     ctx.bind(slot, model)
     occ = torch.empty((grid_dim,) * 3, device=device, dtype=torch.float32)
     voxel = (far - near) / N_importance
-    _lib.check(ctx.lib.dmnerf_mesh_occupancy(ctx.handle, slot, _doubles(T, 16), _doubles(extents, 3), grid_dim, voxel, slab, _f(occ),
-                                             ctx.stream()), "dmnerf_mesh_occupancy")
+    ctx.call("dmnerf_mesh_occupancy", ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(extents, 3), grid_dim, voxel, slab,
+             _lib.ptr(occ))
     return occ
 
 
@@ -89,11 +65,10 @@ def marching_cubes(grid, level=0.45):
     ctx = get_context(g.device)
     nx, ny, nz = g.shape
     counts = (C.c_int64 * 2)()
-    _lib.check(ctx.lib.dmnerf_mesh_mc_count(ctx.handle, _f(g), nx, ny, nz, level, counts, ctx.stream()), "dmnerf_mesh_mc_count")
+    ctx.call("dmnerf_mesh_mc_count", ctx.handle, _lib.ptr(g), nx, ny, nz, level, counts)
     verts = torch.empty((counts[0], 3), device=g.device, dtype=torch.float32)
     tris = torch.empty((counts[1], 3), device=g.device, dtype=torch.int32)
-    _lib.check(ctx.lib.dmnerf_mesh_mc_emit(ctx.handle, _f(g), nx, ny, nz, level, _f(verts), _i(tris), ctx.stream()),
-               "dmnerf_mesh_mc_emit")
+    ctx.call("dmnerf_mesh_mc_emit", ctx.handle, _lib.ptr(g), nx, ny, nz, level, _lib.ptr(verts), _lib.ptr(tris, torch.int32))
     return verts, tris
 
 
@@ -102,17 +77,18 @@ def to_scene(verts, scene_transform, grid_dim, extents=EXTENTS):
     T = check_transform(scene_transform)
     ctx = get_context(verts.device)
     out = torch.empty_like(verts)
-    _lib.check(ctx.lib.dmnerf_mesh_to_scene(_f(verts), verts.shape[0], _doubles(T, 16), _doubles(extents, 3), grid_dim, _f(out),
-                                            ctx.stream()), "dmnerf_mesh_to_scene")
+    ctx.call("dmnerf_mesh_to_scene", _lib.ptr(verts), verts.shape[0], _lib.doubles(T, 16), _lib.doubles(extents, 3), grid_dim,
+             _lib.ptr(out))
     return out
 
 
 def vertex_normals(verts, tris):
     """Area-weighted unit vertex normals (open3d compute_vertex_normals, visualizer.py:164)."""
+    _lib.need_cuda("vertex_normals", verts, tris)
     ctx = get_context(verts.device)
     out = torch.empty_like(verts)
-    _lib.check(ctx.lib.dmnerf_mesh_normals(ctx.handle, _f(verts), verts.shape[0], _i(tris), tris.shape[0], _f(out), ctx.stream()),
-               "dmnerf_mesh_normals")
+    ctx.call("dmnerf_mesh_normals", ctx.handle, _lib.ptr(verts), verts.shape[0], _lib.ptr(tris, torch.int32), tris.shape[0],
+             _lib.ptr(out))
     return out
 
 
@@ -121,31 +97,33 @@ def triangle_clusters(tris, n_verts):
     ctx = get_context(tris.device)
     cluster = torch.empty(tris.shape[0], device=tris.device, dtype=torch.int32)
     size = torch.empty_like(cluster)
-    _lib.check(ctx.lib.dmnerf_mesh_clusters(ctx.handle, _i(tris), tris.shape[0], n_verts, _i(cluster), _i(size), ctx.stream()),
-               "dmnerf_mesh_clusters")
+    ctx.call("dmnerf_mesh_clusters", ctx.handle, _lib.ptr(tris, torch.int32), tris.shape[0], n_verts, _lib.ptr(cluster, torch.int32),
+             _lib.ptr(size, torch.int32))
     return cluster, size
 
 
 def clean_mesh(verts, normals, tris, min_cluster=400):
     """visualizer.clean_mesh(min_num_cluster=min_cluster): triangles of clusters with fewer than min_cluster triangles removed,
     then unreferenced vertices; relative order kept.  Returns (verts, normals, tris)."""
+    _lib.need_cuda("clean_mesh", verts, normals, tris)
     ctx = get_context(verts.device)
     _, size = triangle_clusters(tris, verts.shape[0])
     ov, on = torch.empty_like(verts), (None if normals is None else torch.empty_like(normals))
     ot = torch.empty_like(tris)
     counts = (C.c_int64 * 2)()
-    _lib.check(ctx.lib.dmnerf_mesh_clean(ctx.handle, _f(verts), _f(normals), verts.shape[0], _i(tris), tris.shape[0], _i(size),
-                                         int(min_cluster), _f(ov), _f(on), _i(ot), counts, ctx.stream()), "dmnerf_mesh_clean")
+    i32 = torch.int32
+    ctx.call("dmnerf_mesh_clean", ctx.handle, _lib.ptr(verts), _lib.ptr(normals), verts.shape[0], _lib.ptr(tris, i32), tris.shape[0],
+             _lib.ptr(size, i32), int(min_cluster), _lib.ptr(ov), _lib.ptr(on), _lib.ptr(ot, i32), counts)
     nv, nt = counts[0], counts[1]
     return ov[:nv], (None if on is None else on[:nv]), ot[:nt]
 
 
 def label_rays(verts, normals, near):
     """Per-vertex label rays in the network's frame (mesh_generator.py:106-113) -> rays_o, rays_d [V, 3]."""
+    _lib.need_cuda("label_rays", verts, normals)
     ctx = get_context(verts.device)
     ro, rd = torch.empty_like(verts), torch.empty_like(verts)
-    _lib.check(ctx.lib.dmnerf_mesh_label_rays(_f(verts), _f(normals), verts.shape[0], near, _f(ro), _f(rd), ctx.stream()),
-               "dmnerf_mesh_label_rays")
+    ctx.call("dmnerf_mesh_label_rays", _lib.ptr(verts), _lib.ptr(normals), verts.shape[0], near, _lib.ptr(ro), _lib.ptr(rd))
     return ro, rd
 
 
@@ -154,8 +132,7 @@ def argmax_rows(x):
     ctx = get_context(x.device)
     x = x.contiguous()
     out = torch.empty(x.shape[0], device=x.device, dtype=torch.int64)
-    _lib.check(ctx.lib.dmnerf_argmax_rows(_f(x), x.shape[0], x.shape[1], C.c_void_p(out.data_ptr()), ctx.stream()),
-               "dmnerf_argmax_rows")
+    ctx.call("dmnerf_argmax_rows", _lib.ptr(x), x.shape[0], x.shape[1], _lib.ptr(out, torch.int64))
     return out
 
 

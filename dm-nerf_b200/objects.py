@@ -107,8 +107,7 @@ def occupancy_objects(model, scene_transform, keep_words, grid_dim=256, extents=
                       slab=0, device="cuda"):
     """The occupancy sweep of mesh.occupancy_grid with the selection applied per grid point -> (occ [dim]^3 float32, labels
     [dim]^3 int16): occ is 0 where the point's label is not kept, labels is every point's label."""
-    import ctypes as C
-    from .mesh import EXTENTS, _doubles, _f, check_transform
+    from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
     extents = EXTENTS if extents is None else extents
     ctx = get_context(device)
@@ -117,9 +116,8 @@ def occupancy_objects(model, scene_transform, keep_words, grid_dim=256, extents=
     occ = torch.empty((grid_dim,) * 3, device=device, dtype=torch.float32)
     labels = torch.empty((grid_dim,) * 3, device=device, dtype=torch.int16)
     voxel = (far - near) / N_importance
-    _lib.check(ctx.lib.dmnerf_mesh_occupancy_objects(ctx.handle, slot, _doubles(T, 16), _doubles(extents, 3), grid_dim, voxel, slab,
-                                                     (C.c_uint32 * 4)(*keep_words), _f(occ), C.c_void_p(labels.data_ptr()),
-                                                     ctx.stream()), "dmnerf_mesh_occupancy_objects")
+    ctx.call("dmnerf_mesh_occupancy_objects", ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(extents, 3), grid_dim, voxel, slab,
+             _lib.keep_mask(keep_words), _lib.ptr(occ), _lib.ptr(labels, torch.int16))
     return occ, labels
 
 

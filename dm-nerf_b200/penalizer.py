@@ -19,7 +19,6 @@ class _Penalizer(torch.autograd.Function):
         if not raw.is_cuda:
             raise RuntimeError("emptiness_penalizer: expected CUDA tensors (no CPU fallback)")
         ctx = get_context(raw.device)
-        lib = ctx.lib
         raw_c = raw.detach().contiguous().float()
         z_c = z_vals.detach().contiguous().float()
         d_c = depth.detach().reshape(-1).contiguous().float()
@@ -28,11 +27,10 @@ class _Penalizer(torch.autograd.Function):
         if z_c.shape != (n, s) or d_c.shape != (n,) or rd_c.shape != (n, 3):
             raise RuntimeError("emptiness_penalizer: inconsistent shapes raw %s z_vals %s depth %s rays_d %s"
                                % (tuple(raw.shape), tuple(z_vals.shape), tuple(depth.shape), tuple(rays_d.shape)))
-        state = torch.empty(int(lib.dmnerf_penalizer_state_bytes()), device=raw.device, dtype=torch.uint8)
+        state = torch.empty(int(ctx.lib.dmnerf_penalizer_state_bytes()), device=raw.device, dtype=torch.uint8)
         loss = torch.empty(1, device=raw.device, dtype=torch.float32)
-        _lib.check(lib.dmnerf_penalizer_forward(_lib.ptr(raw_c), _lib.ptr(z_c), _lib.ptr(d_c), _lib.ptr(rd_c), n, s, c,
-                                                float(tolerance), float(deta_w), state.data_ptr(), _lib.ptr(loss), ctx.stream()),
-                   "dmnerf_penalizer_forward")
+        ctx.call("dmnerf_penalizer_forward", _lib.ptr(raw_c), _lib.ptr(z_c), _lib.ptr(d_c), _lib.ptr(rd_c), n, s, c, float(tolerance),
+                 float(deta_w), _lib.ptr(state, torch.uint8), _lib.ptr(loss))
         fctx.save_for_backward(raw_c, z_c, d_c, rd_c, state)
         fctx.cfg = (float(tolerance), float(deta_w))
         return loss
@@ -44,9 +42,8 @@ class _Penalizer(torch.autograd.Function):
         n, s, c = raw_c.shape
         d_raw = torch.empty_like(raw_c)           # the kernel writes every channel (zeros for rgb / sigma)
         g = g_loss.detach().reshape(-1)[:1].contiguous().float()
-        _lib.check(ctx.lib.dmnerf_penalizer_backward(_lib.ptr(raw_c), _lib.ptr(z_c), _lib.ptr(d_c), _lib.ptr(rd_c), n, s, c,
-                                                     fctx.cfg[0], fctx.cfg[1], state.data_ptr(), _lib.ptr(g), _lib.ptr(d_raw), 0,
-                                                     ctx.stream()), "dmnerf_penalizer_backward")
+        ctx.call("dmnerf_penalizer_backward", _lib.ptr(raw_c), _lib.ptr(z_c), _lib.ptr(d_c), _lib.ptr(rd_c), n, s, c, fctx.cfg[0],
+                 fctx.cfg[1], _lib.ptr(state, torch.uint8), _lib.ptr(g), _lib.ptr(d_raw), 0)
         return d_raw, None, None, None, None, None
 
 

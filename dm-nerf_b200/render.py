@@ -34,21 +34,60 @@ def composite(raw, z_vals, rays_d, keep_all_ins=False, keep_objects=None):
     depth = torch.empty((n,), device=dev); acc = torch.empty((n,), device=dev)
     ins = torch.empty((n, n_ins), device=dev)
     ctx = get_context(dev)
+    outs = (_lib.ptr(rgb), _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc))
     if keep_objects is None:
-        _lib.check(ctx.lib.dmnerf_composite(_lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins),
-                                            _lib.ptr(rgb), _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc),
-                                            ctx.stream()), "dmnerf_composite")
+        ctx.call("dmnerf_composite", _lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins), *outs)
     else:
         from .objects import object_mask
-        keep = (C.c_uint32 * 4)(*object_mask(c - 5, keep=keep_objects))
-        _lib.check(ctx.lib.dmnerf_composite_objects(_lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins), keep,
-                                                    _lib.ptr(rgb), _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc),
-                                                    ctx.stream()), "dmnerf_composite_objects")
+        keep = _lib.keep_mask(object_mask(c - 5, keep=keep_objects))
+        ctx.call("dmnerf_composite_objects", _lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins), keep,
+                 *outs)
     return rgb, w, depth, ins, acc
 
 
-def _keep_arg(words):
-    return (C.c_uint32 * 4)(*words)
+def bind_pair(ctx, model_coarse, model_fine):
+    """Bind the coarse network to slot 0 and the fine one to slot 1 -> their common ins_num."""
+    ins_num = ctx.bind(0, model_coarse)
+    if ctx.bind(1, model_fine) != ins_num:
+        raise RuntimeError("coarse and fine networks disagree on ins_num")
+    return ins_num
+
+
+def coarse_depths(z_vals_coarse, n):
+    """z_vals_coarse of n rays -> (z_in, z_row_stride) of the C ABI: one shared row (a [S] tensor or the stride-0 expand of
+    z_val_sample) with stride 0, or one row per ray with stride S."""
+    if z_vals_coarse.dim() == 1:
+        return z_vals_coarse.contiguous().float(), 0
+    if z_vals_coarse.dim() == 2 and z_vals_coarse.shape[0] > 1 and z_vals_coarse.stride(0) == 0:
+        return z_vals_coarse[0].contiguous().float(), 0
+    z_in = z_vals_coarse.contiguous().float()
+    if z_in.shape[0] != n:
+        raise RuntimeError("z_vals_coarse has %d rows for %d rays" % (z_in.shape[0], n))
+    return z_in, z_vals_coarse.shape[-1]
+
+
+def reference_draws(perturb, n, S, N_importance, device, t_rand=None, u=None):
+    """The uniforms of a perturbed render, drawn where the caller did not pass them, in the reference's order: t_rand [n, S]
+    (render.py:46), then u [n, N_importance] (helpers.py:135).  (None, None) when perturb <= 0."""
+    if perturb <= 0.0:
+        return None, None
+    if t_rand is None:
+        t_rand = torch.rand((n, S), device=device)
+    if u is None:
+        u = torch.rand((n, N_importance), device=device)
+    return t_rand.contiguous().float(), u.contiguous().float()
+
+
+def selection(who, keep_objects, ins_num, model_coarse, model_fine):
+    """The host mask of an inference entry point's keep_objects, or None without a selection."""
+    if keep_objects is None:
+        return None
+    from .autograd import _needs_grad
+    from .objects import object_mask
+    if _needs_grad(model_coarse, model_fine):
+        raise RuntimeError("%s: object selection is inference-only; call it under torch.no_grad() or with parameters that "
+                           "do not require grad" % who)
+    return _lib.keep_mask(object_mask(ins_num, keep=keep_objects))
 
 
 def _check_embedders(position_embedder, view_embedder):
@@ -74,39 +113,16 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     if dev.type != "cuda":
         raise RuntimeError("dm_nerf: expected CUDA tensors (no CPU fallback)")
     ctx = get_context(dev)
-    ins_num = ctx.bind(0, model_coarse)
-    if ctx.bind(1, model_fine) != ins_num:
-        raise RuntimeError("coarse and fine networks disagree on ins_num")
-    keep = None
-    if keep_objects is not None:
-        from .autograd import _needs_grad
-        from .objects import object_mask
-        if _needs_grad(model_coarse, model_fine):
-            raise RuntimeError("render_rays: object selection is inference-only; call it under torch.no_grad() or with "
-                               "parameters that do not require grad")
-        keep = object_mask(ins_num, keep=keep_objects)
+    ins_num = bind_pair(ctx, model_coarse, model_fine)
+    keep = selection("render_rays", keep_objects, ins_num, model_coarse, model_fine)
     rays_o = rays_o.reshape(-1, 3).contiguous().float()
     rays_d = rays_d.reshape(-1, 3).contiguous().float()
     n = rays_o.shape[0]
     S = z_vals_coarse.shape[-1]
     F, C = S + N_importance, 4 + ins_num + 1
-    if z_vals_coarse.dim() == 2 and z_vals_coarse.shape[0] > 1 and z_vals_coarse.stride(0) == 0:
-        z_in, z_stride = z_vals_coarse[0].contiguous().float(), 0          # the stride-0 expand of z_val_sample
-    elif z_vals_coarse.dim() == 1:
-        z_in, z_stride = z_vals_coarse.contiguous().float(), 0
-    else:
-        z_in, z_stride = z_vals_coarse.contiguous().float(), S
-        if z_in.shape[0] != n:
-            raise RuntimeError("z_vals_coarse has %d rows for %d rays" % (z_in.shape[0], n))
-    flags = 0
-    if perturb > 0.0:
-        flags |= _lib.FLAG_PERTURB
-        # same two draws, in the same order, as the reference (render.py:46, helpers.py:135)
-        if t_rand is None:
-            t_rand = torch.rand((n, S), device=dev)
-        if u is None:
-            u = torch.rand((n, N_importance), device=dev)
-        t_rand, u = t_rand.contiguous().float(), u.contiguous().float()
+    z_in, z_stride = coarse_depths(z_vals_coarse, n)
+    t_rand, u = reference_draws(perturb, n, S, N_importance, dev, t_rand, u)
+    flags = _lib.FLAG_PERTURB if perturb > 0.0 else 0
     if want_raw:
         flags |= _lib.FLAG_WANT_RAW
     if keep_all_ins:
@@ -124,15 +140,13 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
         out.update({"raw_fine": e(n, F, C), "raw_coarse": e(n, S, C)})
     io = _lib.RenderIO()
     io.rays_o, io.rays_d, io.z_coarse, io.z_row_stride = _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(z_in), z_stride
-    io.t_rand, io.u = (_lib.ptr(t_rand), _lib.ptr(u)) if perturb > 0.0 else (None, None)
+    io.t_rand, io.u = _lib.ptr(t_rand), _lib.ptr(u)
     for k, v in out.items():
         setattr(io, k, _lib.ptr(v))
     if keep is None:
-        _lib.check(ctx.lib.dmnerf_render_forward(ctx.handle, io, n, S, N_importance, flags, impl, ctx.stream()),
-                   "dmnerf_render_forward")
+        ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags, impl)
     else:
-        _lib.check(ctx.lib.dmnerf_render_forward_objects(ctx.handle, io, n, S, N_importance, flags, impl, _keep_arg(keep),
-                                                         ctx.stream()), "dmnerf_render_forward_objects")
+        ctx.call("dmnerf_render_forward_objects", ctx.handle, io, n, S, N_importance, flags, impl, keep)
     return out
 
 
@@ -202,11 +216,9 @@ def dm_nerf(rays, position_embedder, view_embedder, model_coarse, model_fine, z_
         from .backward import render_rays_grad
         out = render_rays_grad(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb, args.N_importance)
     else:
-        t_rand = u = None
-        if perturb > 0.0:          # the reference's two draws, in its order (render.py:46, helpers.py:135)
-            n, S = rays_o.reshape(-1, 3).shape[0], z_vals_coarse.shape[-1]
-            t_rand = torch.rand((n, S), device=rays_o.device)
-            u = torch.rand((n, args.N_importance), device=rays_o.device)
+        # drawn once here: the lazy re-render must see the fused render's uniforms
+        t_rand, u = reference_draws(perturb, rays_o.reshape(-1, 3).shape[0], z_vals_coarse.shape[-1], args.N_importance,
+                                    rays_o.device)
         kw = dict(perturb=perturb, N_importance=args.N_importance, t_rand=t_rand, u=u)
         fused = render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, want_raw=False, want_samples=False, **kw)
         out = LazyRenderDict(fused, lambda: render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse,
@@ -230,35 +242,22 @@ def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64
     the per-rank slice of a sharded frame).  keep_objects: object selection as in render_rays."""
     dev = torch.device(device)
     ctx = get_context(dev)
-    ins_num = ctx.bind(0, model_coarse)
-    if ctx.bind(1, model_fine) != ins_num:
-        raise RuntimeError("render_frame: coarse and fine networks disagree on ins_num")
-    keep = None
-    if keep_objects is not None:
-        from .autograd import _needs_grad
-        from .objects import object_mask
-        if _needs_grad(model_coarse, model_fine):
-            raise RuntimeError("render_frame: object selection is inference-only; call it under torch.no_grad() or with "
-                               "parameters that do not require grad")
-        keep = object_mask(ins_num, keep=keep_objects)
+    ins_num = bind_pair(ctx, model_coarse, model_fine)
+    keep = selection("render_frame", keep_objects, ins_num, model_coarse, model_fine)
     begin, count = (0, H * W) if pixel_range is None else (int(pixel_range[0]), int(pixel_range[1]))
     n_ins = ins_num + 1 if keep_all_ins else ins_num
     pin = dev.type == "cuda"
     out = {"rgb": torch.empty(count, 3, pin_memory=pin), "ins": torch.empty(count, n_ins, pin_memory=pin),
            "depth": torch.empty(count, pin_memory=pin), "acc": torch.empty(count, pin_memory=pin)}
-    io = _lib.RenderIO(rgb_fine=out["rgb"].data_ptr(), ins_fine=out["ins"].data_ptr(), depth_fine=out["depth"].data_ptr(),
-                       acc_fine=out["acc"].data_ptr())
-    Kf = (C.c_float * 9)(*[float(v) for v in torch.as_tensor(K, dtype=torch.float32).reshape(-1)[:9]])
-    c2 = torch.as_tensor(c2w, dtype=torch.float32).reshape(-1, 4)[:3].reshape(-1)
-    Cf = (C.c_float * 12)(*[float(v) for v in c2])
+    io = _lib.RenderIO(rgb_fine=_lib.ptr(out["rgb"]), ins_fine=_lib.ptr(out["ins"]), depth_fine=_lib.ptr(out["depth"]),
+                       acc_fine=_lib.ptr(out["acc"]))
+    Kf, Cf = _lib.camera(K, c2w)
     flags = _lib.FLAG_KEEP_INS if keep_all_ins else 0
+    args = (ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples, N_importance, flags, impl)
     if keep is None:
-        _lib.check(ctx.lib.dmnerf_render_frame_host(ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples,
-                                                    N_importance, flags, impl, C.byref(io), ctx.stream()), "dmnerf_render_frame_host")
+        ctx.call("dmnerf_render_frame_host", *args, C.byref(io))
     else:
-        _lib.check(ctx.lib.dmnerf_render_frame_objects_host(ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count,
-                                                            N_samples, N_importance, flags, impl, _keep_arg(keep),
-                                                            C.byref(io), ctx.stream()), "dmnerf_render_frame_objects_host")
+        ctx.call("dmnerf_render_frame_objects_host", *args, keep, C.byref(io))
     if pixel_range is None:
         out = {"rgb": out["rgb"].reshape(H, W, 3), "ins": out["ins"].reshape(H, W, n_ins), "depth": out["depth"].reshape(H, W),
                "acc": out["acc"].reshape(H, W)}

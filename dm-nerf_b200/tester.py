@@ -36,16 +36,6 @@ _RANK_SLOTS = 128                     # distinct labels it ranks at most (ins_nu
 _workspaces = {}
 
 
-def _need_cuda(what, *ts):
-    for t in ts:
-        if t is not None and not (torch.is_tensor(t) and t.is_cuda):
-            raise RuntimeError("%s: expected CUDA tensors (no CPU fallback)" % what)
-
-
-def _vp(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
 def _workspace(dev, n, k, H, W):
     ctx = get_context(dev)
     need = int(ctx.lib.dmnerf_eval_workspace_bytes(int(n), int(k), int(H), int(W)))
@@ -73,12 +63,12 @@ def _image_into(rgb, gt, res):
     rgb, gt = rgb.detach().contiguous().float(), gt.detach().to(rgb.device).contiguous().float()
     ctx = get_context(rgb.device)
     ws = _workspace(rgb.device, 0, 0, H, W)
-    _lib.check(ctx.lib.dmnerf_eval_image(_lib.ptr(rgb), _lib.ptr(gt), H, W, _vp(ws), _vp(res), ctx.stream()), "dmnerf_eval_image")
+    ctx.call("dmnerf_eval_image", _lib.ptr(rgb), _lib.ptr(gt), H, W, _lib.ptr(ws, torch.uint8), _lib.ptr(res, torch.uint8))
 
 
 def image_metrics(rgb, gt):
     """(psnr, ssim) of two [H, W, 3] CUDA images with data_range 1, one read-back."""
-    _need_cuda("image_metrics", rgb, gt)
+    _lib.need_cuda("image_metrics", rgb, gt)
     res = _result_buffer(rgb.device)
     _image_into(rgb, gt, res)
     r = _read_result(res)
@@ -102,8 +92,9 @@ def _ins_eval_rows(ins, gt_row, gt_num, res, mask=None, mask_labels=None, mask_b
     ctx = get_context(dev)
     ws = _workspace(dev, n, k, 0, 0)
     pred_label = torch.empty(n, device=dev, dtype=torch.int64)
-    _lib.check(ctx.lib.dmnerf_ins_eval(_lib.ptr(ins), n, k, _vp(gt_row), int(gt_num), _lib.ptr(mask), _vp(mask_labels), int(mask_below),
-                                       _vp(pred_label), _vp(ws), _vp(res), ctx.stream()), "dmnerf_ins_eval")
+    i32 = torch.int32
+    ctx.call("dmnerf_ins_eval", _lib.ptr(ins), n, k, _lib.ptr(gt_row, i32), int(gt_num), _lib.ptr(mask), _lib.ptr(mask_labels, i32),
+             int(mask_below), _lib.ptr(pred_label, torch.int64), _lib.ptr(ws, torch.uint8), _lib.ptr(res, torch.uint8))
     return pred_label
 
 
@@ -118,7 +109,7 @@ def ins_eval(pred_ins, gt_ins, gt_ins_num, ins_num, mask=None):
     """evaluator.py:125-175.  pred_ins, gt_ins [..., ins_num] (gt_ins one-hot in its first gt_ins_num columns), mask [...] (0 =
     masked, the crop path).  Returns (pred_label [...] int64 CUDA tensor, ap_list (6 floats), return_labels int64 numpy array:
     the matched predicted label per gt object, or -1)."""
-    _need_cuda("ins_eval", pred_ins, gt_ins, mask)
+    _lib.need_cuda("ins_eval", pred_ins, gt_ins, mask)
     if pred_ins.shape[-1] != ins_num or tuple(gt_ins.shape) != tuple(pred_ins.shape):
         raise ValueError("ins_eval: pred_ins %s / gt_ins %s / ins_num %d are inconsistent"
                          % (tuple(pred_ins.shape), tuple(gt_ins.shape), ins_num))
@@ -129,8 +120,7 @@ def ins_eval(pred_ins, gt_ins, gt_ins_num, ins_num, mask=None):
     dev = ins.device
     ctx = get_context(dev)
     gt_row = torch.empty(n, device=dev, dtype=torch.int32)
-    _lib.check(ctx.lib.dmnerf_ins_dense_rows(_lib.ptr(gt), n, ins_num, int(gt_ins_num), _vp(gt_row), ctx.stream()),
-               "dmnerf_ins_dense_rows")
+    ctx.call("dmnerf_ins_dense_rows", _lib.ptr(gt), n, ins_num, int(gt_ins_num), _lib.ptr(gt_row, torch.int32))
     m = None if mask is None else mask.detach().reshape(-1).contiguous().float()
     res = _result_buffer(dev)
     pred_label = _ins_eval_rows(ins, gt_row, gt_ins_num, res, mask=m)
@@ -143,13 +133,12 @@ def calculate_ap(IoUs_Metrics, gt_number, confidence=None, function_select='inte
     """evaluator.py:77-122 (integral method only).  Matches are ordered by confidence, descending, ties in index order."""
     if function_select != 'integral':
         raise NotImplementedError("calculate_ap: only function_select='integral' (the one ins_eval uses) is implemented")
-    _need_cuda("calculate_ap", IoUs_Metrics, confidence)
+    _lib.need_cuda("calculate_ap", IoUs_Metrics, confidence)
     iou = IoUs_Metrics.detach().reshape(-1).contiguous().float()
     conf = None if confidence is None else confidence.detach().to(iou.device).reshape(-1).contiguous().float()
     ap = torch.empty(6, device=iou.device, dtype=torch.float32)
     ctx = get_context(iou.device)
-    _lib.check(ctx.lib.dmnerf_calculate_ap(_lib.ptr(iou), _lib.ptr(conf), iou.numel(), int(gt_number), _lib.ptr(ap), ctx.stream()),
-               "dmnerf_calculate_ap")
+    ctx.call("dmnerf_calculate_ap", _lib.ptr(iou), _lib.ptr(conf), iou.numel(), int(gt_number), _lib.ptr(ap))
     return [float(v) for v in ap.cpu()]
 
 
@@ -179,15 +168,15 @@ def _rgb_u8(rgb):
 
 def colorize(labels, lut):
     """Device gather: out [..., 3] uint8 = lut[label] (lut [L, 3] uint8), black for labels outside [0, L)."""
-    _need_cuda("colorize", labels)
+    _lib.need_cuda("colorize", labels)
     lab = labels.contiguous()
     if lab.dtype not in (torch.int64, torch.int32):
         lab = lab.to(torch.int64)
     lut_d = torch.as_tensor(np.ascontiguousarray(lut, dtype=np.uint8).reshape(-1, 3)).to(lab.device)
     out = torch.empty(tuple(lab.shape) + (3,), device=lab.device, dtype=torch.uint8)
     ctx = get_context(lab.device)
-    _lib.check(ctx.lib.dmnerf_label_colors(_vp(lab), int(lab.dtype == torch.int64), lab.numel(), _vp(lut_d), lut_d.shape[0], _vp(out),
-                                           ctx.stream()), "dmnerf_label_colors")
+    ctx.call("dmnerf_label_colors", _lib.ptr(lab, lab.dtype), int(lab.dtype == torch.int64), lab.numel(), _lib.ptr(lut_d, torch.uint8),
+             lut_d.shape[0], _lib.ptr(out, torch.uint8))
     return out
 
 
@@ -277,8 +266,8 @@ def _frame_metrics(who, i, rgb, gt_img, ins, labels, valid_gt, ins_num, lpips_vg
     if lpips_vgg is not None:
         lpips_i = lpips_vgg(rgb.permute(2, 0, 1).unsqueeze(0), gt_img.permute(2, 0, 1).unsqueeze(0)).item()
     if gt_num > 0:
-        _lib.check(ctx.lib.dmnerf_ins_label_rows(_vp(labels), n_px, _RANK_SLOTS, _vp(gt_row), _vp(n_valid), ctx.stream()),
-                   "dmnerf_ins_label_rows")
+        i32 = torch.int32
+        ctx.call("dmnerf_ins_label_rows", _lib.ptr(labels, i32), n_px, _RANK_SLOTS, _lib.ptr(gt_row, i32), _lib.ptr(n_valid, i32))
         pred_label = _ins_eval_rows(ins, gt_row, gt_num, res, mask_labels=mask_labels, mask_below=ins_num)
     r = _read_result(res)
     if gt_num > 0:

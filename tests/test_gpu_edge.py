@@ -53,6 +53,23 @@ def test_per_ray_coarse_depths_match_shared_row(want_raw):
         assert torch.equal(a[k], b[k]), k
 
 
+def test_per_ray_coarse_depths_with_too_few_rows_are_rejected():
+    """A per-ray z_vals_coarse with fewer rows than rays is an error for inference and training alike; training raises
+    before its first launch instead of reading past the end of the depths."""
+    from dmnerf_b200.render import dm_nerf, render_rays
+    from dmnerf_b200.embedder import get_embedder
+    wl, ro, rd = _rays(130)
+    nc, nf, _, _ = make_models(1, 2, 13, DEV)
+    z = torch.linspace(wl["near"], wl["far"], 64, device=DEV).repeat(129, 1)
+    with torch.no_grad(), pytest.raises(RuntimeError, match="129 rows for 130 rays"):
+        render_rays(ro, rd, nc, nf, z)
+    args = types.SimpleNamespace(perturb=1.0, N_importance=128)
+    before = _lib.launch_count()
+    with pytest.raises(RuntimeError, match="129 rows for 130 rays"):
+        dm_nerf(torch.stack([ro, rd], 0), get_embedder(10)[0], get_embedder(4)[0], nc, nf, z, args)
+    assert _lib.launch_count() == before
+
+
 def test_scannet_n_ins_slice_and_perturb_without_grad():
     """render.py:88-90: with args.is_train and args.N_ins only the last N_ins rays keep instance maps; perturb > 0 under
     no_grad (manipulator-style) must consume the two uniform draws in the reference's order."""

@@ -67,8 +67,8 @@ def one(ins_num, frames, warmup, H=480, W=640):
             ev[1].record()
             res = T._result_buffer(dev)
             T._image_into(rgb.reshape(H, W, 3), gt_img, res)
-            _lib.check(ctx.lib.dmnerf_ins_label_rows(T._vp(labels), H * W, 128, T._vp(gt_row), T._vp(n_valid), ctx.stream()),
-                       "dmnerf_ins_label_rows")
+            ctx.call("dmnerf_ins_label_rows", _lib.ptr(labels, torch.int32), H * W, 128, _lib.ptr(gt_row, torch.int32),
+                     _lib.ptr(n_valid, torch.int32))
             T._ins_eval_rows(ins, gt_row, gt_num, res)
             r = T._read_result(res)
             ev[2].record()
