@@ -102,7 +102,11 @@ __global__ void composite_backward_kernel(const float* __restrict__ raw, const f
       const float o = __shfl_down_sync(FULL, incl, d);
       if (lane + d < 32) incl += o;
     }
-    const float R = suffix + (incl - p);                 // sum_{j > i} gw_j w_j
+    // sum_{j > i} gw_j w_j from the next lane's inclusive sum, not as incl - p: where alpha_i -> 1, p = gw_i w_i is large next
+    // to the suffix, and the rounding of that difference would be amplified by 1 / f_i below
+    float after = __shfl_down_sync(FULL, incl, 1);
+    if (lane == 31) after = 0.0f;
+    const float R = suffix + after;
     if (i < S) {
       const float dalpha = gw[i] * T[i] - R / fi[i];
       float v = (rr[(size_t)i * C + 3] > 0.0f) ? dalpha * ex[i] : 0.0f;
@@ -134,9 +138,9 @@ int launch_composite_backward(const float* raw, const float* z, const float* ray
 constexpr int GT = 64;      // output tile GT x GT
 constexpr int GK = 16;      // inner chunk
 
-// C[n, k] += sum_{m in split} A[m, n] B[m, k]   (C zero-initialised by the caller; fp32 atomics across splits)
+// part[split][n][k] = sum_{m in split} A[m, n] B[m, k]   (reduce_splits_kernel adds the splits into C in split order)
 __global__ void __launch_bounds__(256) gemm_tn_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                      float* __restrict__ Cm, int ldc, int64_t M, int N, int K, int64_t rows_per_split) {
+                                                      float* __restrict__ part, int64_t M, int N, int K, int64_t rows_per_split) {
   __shared__ float As[GK][GT];
   __shared__ float Bs[GK][GT];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -166,6 +170,7 @@ __global__ void __launch_bounds__(256) gemm_tn_kernel(const float* __restrict__ 
     }
     __syncthreads();
   }
+  float* mine = part + (size_t)blockIdx.z * N * K;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int nn = n0 + ty + 16 * i;
@@ -173,7 +178,7 @@ __global__ void __launch_bounds__(256) gemm_tn_kernel(const float* __restrict__ 
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int k = k0 + tx + 16 * j;
-      if (k < K) atomicAdd(&Cm[(size_t)nn * ldc + k], acc[i][j]);
+      if (k < K) mine[(size_t)nn * K + k] = acc[i][j];
     }
   }
 }
@@ -194,9 +199,9 @@ __device__ __forceinline__ void fma_8x8(float (&acc)[8][8], const float* __restr
     for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
 }
 
-// C[n, k] += sum_{m in split} A[m, n] B[m, k].  N % 4 == 0, K % 4 == 0, lda/ldb % 4 == 0; rows_per_split % 8 == 0.
+// part[split][n][k] = sum_{m in split} A[m, n] B[m, k].  N % 4 == 0, K % 4 == 0, lda/ldb % 4 == 0; rows_per_split % 8 == 0.
 __global__ void __launch_bounds__(256) gemm_tn_big_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                          float* __restrict__ Cm, int ldc, int64_t M, int N, int K, int64_t rows_per_split) {
+                                                          float* __restrict__ part, int64_t M, int N, int K, int64_t rows_per_split) {
   __shared__ __align__(16) float As[2][BK][BT];
   __shared__ __align__(16) float Bs[2][BK][BT];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -228,6 +233,7 @@ __global__ void __launch_bounds__(256) gemm_tn_big_kernel(const float* __restric
     __syncthreads();
     buf ^= 1;
   }
+  float* mine = part + (size_t)blockIdx.z * N * K;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int nn = n0 + ty * 8 + i;
@@ -235,38 +241,113 @@ __global__ void __launch_bounds__(256) gemm_tn_big_kernel(const float* __restric
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int k = k0 + tx * 8 + j;
-      if (k < K) atomicAdd(&Cm[(size_t)nn * ldc + k], acc[i][j]);
+      if (k < K) mine[(size_t)nn * K + k] = acc[i][j];
     }
   }
 }
 
-static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K, cudaStream_t st) {
-  const bool aligned = ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0);
-  if (aligned && N % 4 == 0 && K % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 && N >= 64 && K >= 64) {
-    const int tiles_b = ((N + BT - 1) / BT) * ((K + BT - 1) / BT);
-    int64_t splits = (3 * 132 + tiles_b - 1) / tiles_b;
-    int64_t rows = (M + splits - 1) / splits;
-    rows = ((rows + BK - 1) / BK) * BK;
-    if (rows < 512) rows = 512;
-    splits = (M + rows - 1) / rows;
-    dim3 grid((unsigned)((N + BT - 1) / BT), (unsigned)((K + BT - 1) / BT), (unsigned)splits);
-    gemm_tn_big_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, N, K, rows);
-    DMN_LAUNCH_OK();
-    return 0;
+// C[n, k] += sum_split part[split][n][k], the splits added in order (reproducible bit for bit).  A block owns 32 consecutive
+// entries; its 8 warps take the splits round robin and their 8 sums are added in warp order.
+__global__ void __launch_bounds__(256) reduce_splits_kernel(const float* __restrict__ part, int splits, int N, int K,
+                                                            float* __restrict__ Cm, int ldc) {
+  __shared__ float red[8][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t nk = (int64_t)N * K, e = (int64_t)blockIdx.x * 32 + lane;
+  float s = 0.0f;
+  if (e < nk)
+    for (int z = warp; z < splits; z += 8) s += __ldcs(part + (size_t)z * nk + e);
+  red[warp][lane] = s;
+  __syncthreads();
+  if (warp == 0 && e < nk) {
+    float t = 0.0f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) t += red[w][lane];
+    Cm[(size_t)(e / K) * ldc + e % K] += t;
   }
-  const int tiles = ((N + GT - 1) / GT) * ((K + GT - 1) / GT);
-  int64_t splits = (4 * 132 + tiles - 1) / tiles;
+}
+
+// Splits of the fp32 dW GEMMs: at most this many for m samples (the split heights below are at least 256 rows, the counts at
+// most 4 * 132), each a [N x K] partial with N * K <= TN_PART_ENTRIES (ins_linear: up to 128 logits x 128 hidden units).
+constexpr int64_t TN_MAX_SPLITS = 4 * 132;
+constexpr int64_t TN_PART_ENTRIES = 128 * 128;
+static int64_t tn_part_floats(int64_t m) {
+  const int64_t s = (m + 255) / 256;
+  return (s < TN_MAX_SPLITS ? s : TN_MAX_SPLITS) * TN_PART_ENTRIES;
+}
+
+// C[n, k] += sum_m A[m, n] B[m, k] (C zero-initialised by the caller); part: tn_part_floats(M) floats of scratch.
+static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K, float* part,
+                   cudaStream_t st) {
+  DMN_CHECK((int64_t)N * K <= TN_PART_ENTRIES, "mlp_backward: %d x %d weight gradient exceeds the split scratch", N, K);
+  const bool aligned = ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0);
+  const bool big = aligned && N % 4 == 0 && K % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 && N >= 64 && K >= 64;
+  const int tile = big ? BT : GT, step = big ? BK : GK, min_rows = big ? 512 : 256;
+  const int tiles = ((N + tile - 1) / tile) * ((K + tile - 1) / tile);
+  int64_t splits = ((big ? 3 : 4) * 132 + tiles - 1) / tiles;
   int64_t rows = (M + splits - 1) / splits;
-  rows = ((rows + GK - 1) / GK) * GK;
-  if (rows < 256) rows = 256;
+  rows = ((rows + step - 1) / step) * step;
+  if (rows < min_rows) rows = min_rows;
   splits = (M + rows - 1) / rows;
-  dim3 grid((unsigned)((N + GT - 1) / GT), (unsigned)((K + GT - 1) / GT), (unsigned)splits);
-  gemm_tn_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, N, K, rows);
+  DMN_CHECK(splits * N * K <= tn_part_floats(M), "mlp_backward: %lld splits exceed the split scratch", (long long)splits);
+  dim3 grid((unsigned)((N + tile - 1) / tile), (unsigned)((K + tile - 1) / tile), (unsigned)splits);
+  if (big) gemm_tn_big_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, part, M, N, K, rows);
+  else gemm_tn_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, part, M, N, K, rows);
+  DMN_LAUNCH_OK();
+  reduce_splits_kernel<<<(unsigned)(((int64_t)N * K + 31) / 32), 256, 0, st>>>(part, (int)splits, N, K, C, ldc);
   DMN_LAUNCH_OK();
   return 0;
 }
 
-size_t mlp_backward_scratch_floats(int64_t m) { return (size_t)m * (256 + 8 * 256) + 256 * 256 + 256 + 256; }
+// Column sums of d_out (the output-layer bias gradients) in a fixed order: pass 1 gives one partial row per block (warps over
+// rows, lanes over 32 columns, the 8 warp sums added in warp order), pass 2 adds the partial rows in block order.
+constexpr int COLSUM_BLOCKS = 4 * 132;
+constexpr int COLSUM_MAX_C = 4 + DMNERF_MAX_INS + 1;
+__global__ void __launch_bounds__(256) colsum_rows_kernel(const float* __restrict__ A, int C, int64_t m, int64_t rows_per_block,
+                                                          float* __restrict__ part) {
+  __shared__ float red[8][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t r0 = (int64_t)blockIdx.x * rows_per_block;
+  const int64_t r1 = (r0 + rows_per_block < m) ? r0 + rows_per_block : m;
+  for (int c0 = 0; c0 < C; c0 += 32) {
+    const int c = c0 + lane;
+    float s = 0.0f;
+    if (c < C)
+      for (int64_t r = r0 + warp; r < r1; r += 8) s += __ldg(A + r * C + c);
+    red[warp][lane] = s;
+    __syncthreads();
+    if (warp == 0 && c < C) {
+      float t = 0.0f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) t += red[w][lane];
+      part[(size_t)blockIdx.x * C + c] = t;
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void colsum_finish_kernel(const float* __restrict__ part, int C, int blocks, float* __restrict__ out) {
+  const int c = threadIdx.x;
+  if (c >= C) return;
+  float s = 0.0f;
+  for (int b = 0; b < blocks; ++b) s += part[(size_t)b * C + c];
+  out[c] = s;
+}
+
+static int colsum_fixed(const float* A, int C, int64_t m, float* part, float* out, cudaStream_t st) {
+  const int64_t rows = (m + COLSUM_BLOCKS - 1) / COLSUM_BLOCKS;
+  const int blocks = (int)((m + rows - 1) / rows);
+  colsum_rows_kernel<<<blocks, 256, 0, st>>>(A, C, m, rows, part);
+  DMN_LAUNCH_OK();
+  colsum_finish_kernel<<<1, COLSUM_MAX_C, 0, st>>>(part, C, blocks, out);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+// [S1 | S2], dY0..dY7, [S1 | S2]^T h7, its column sums, the column sums of d_out, then the partial rows of those column sums and
+// the split partials of the fp32 dW GEMMs
+size_t mlp_backward_scratch_floats(int64_t m) {
+  return (size_t)m * (256 + 8 * 256) + 256 * 256 + 256 + 256 + (size_t)COLSUM_BLOCKS * COLSUM_MAX_C + (size_t)tn_part_floats(m);
+}
 
 // Small dense products of the folded head gradients (128..256 x 256 outputs, contraction 128..256): 16 x 16 output tiles, one
 // output per thread, so that the launch fills the machine (a 64 x 64 tiling runs these on 8-16 CTAs at ~35 us apiece).
@@ -328,17 +409,7 @@ static int small_tn(const float* A, int lda, const float* B, int ldb, float* C, 
 //   P = S1^T h7, Q = S2^T h7  ->  the four feature / hidden head gradients by small dense products:
 //     dW_rgb_hid[:, :256] = P W_rf^T + c1 (x) b_rf,  dW_rgb_feat = W_rh[:, :256]^T P,  db_rgb_feat = W_rh[:, :256]^T c1   (c1 = colsum S1)
 //     (rgb_feat = h7 W_rf^T + b_rf is never materialised; same for the instance branch with Q, c2)
-// out[c] += sum_m A[m, c] for a narrow row-major matrix (C <= 132 columns): coalesced sweep of the flat array, per-block bins.
-__global__ void __launch_bounds__(256) colsum_flat_kernel(const float* __restrict__ A, int C, int64_t total, float* __restrict__ out) {
-  __shared__ float bins[4 + DMNERF_MAX_INS + 1];
-  for (int c = threadIdx.x; c < C; c += blockDim.x) bins[c] = 0.0f;
-  __syncthreads();
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x)
-    atomicAdd(&bins[(int)(i % C)], A[i]);
-  __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) atomicAdd(&out[c], bins[c]);
-}
-
+// Every sum over the samples runs in a fixed order, so the 30 gradients are reproducible bit for bit from run to run.
 static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, float* acts, const float* d_out, int64_t m,
                               float* const* grads, float* scratch, bool masks_saved, cudaStream_t st) {
   const int ins1 = p.ins_num + 1, C = 4 + ins1;
@@ -349,6 +420,8 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
   float* PQ = dY[7] + m * 256;                        // [S1 | S2]^T h7: rows 0..127 = P, 128..255 = Q
   float* c12 = PQ + 256 * 256;                        // column sums of S1 | S2
   float* cs = c12 + 256;                              // column sums of d_out [C]
+  float* cs_part = cs + 256;                          // their partial rows [COLSUM_BLOCKS][C]
+  float* tn_part = cs_part + (size_t)COLSUM_BLOCKS * COLSUM_MAX_C;        // split partials of the fp32 dW GEMM
   float* P = PQ, *Q = PQ + 128 * 256, *c1 = c12, *c2 = c12 + 128;
   auto gw = [&](int l) { return grads[2 * l]; };
   auto gb = [&](int l) { return grads[2 * l + 1]; };
@@ -378,7 +451,7 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
       q->N = K;
     } else {
       DMN_CHECK(!colsum_out && !b_cm, "mlp_backward: no kernel for the %d x %d weight gradient", N, K);
-      return gemm_tn(A, lda, B, ldb, Cw, ldc, m, N, K, st);
+      return gemm_tn(A, lda, B, ldb, Cw, ldc, m, N, K, tn_part, st);
     }
     pr.ldc = ldc; pr.C = Cw;
     if (q->n == TN_MAX_BATCH) { const int r = flush(*q); if (r) return r; }
@@ -406,8 +479,7 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
   R(dW(S12, 256, ap.emb + (int64_t)CH_POS * m, CH_IN, gw(L_RGB_HID) + 256, 283, 128, CH_DIR, nullptr, m));
   R(flush(q_in128));
   // the three output bias gradients from one sweep over d_out
-  colsum_flat_kernel<<<132 * 4, 256, 0, st>>>(d_out, C, m * C, cs);
-  DMN_LAUNCH_OK();
+  R(colsum_fixed(d_out, C, m, cs_part, cs, st));
   DMN_CUDA(cudaMemcpyAsync(gb(L_RGB_OUT), cs, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   DMN_CUDA(cudaMemcpyAsync(gb(L_DENSITY), cs + 3, sizeof(float), cudaMemcpyDeviceToDevice, st));
   DMN_CUDA(cudaMemcpyAsync(gb(L_INS_OUT), cs + 4, ins1 * sizeof(float), cudaMemcpyDeviceToDevice, st));
