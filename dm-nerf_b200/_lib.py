@@ -20,6 +20,7 @@ ABI_VERSION = 1
 N_PARAMS = 30
 IMPL_AUTO, IMPL_SIMT, IMPL_UMMA = 0, 1, 2
 FLAG_PERTURB, FLAG_WANT_RAW, FLAG_KEEP_INS = 1, 2, 4
+LABEL_WORDS = 2049           # DMNERF_LABEL_WORDS
 
 _f32p = C.c_void_p
 
@@ -66,6 +67,14 @@ PROTOTYPES = {
     "dmnerf_ins_loss_backward_dev": (C.c_int, [_f32p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, _f32p, _f32p, _f32p,
                                                _f32p, _f32p, C.c_void_p]),
     "dmnerf_ins_status_take": (C.c_int, []),
+    "dmnerf_ins_label_bitmap": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "dmnerf_ins_label_rows_merged": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                               C.c_void_p]),
+    "dmnerf_hungarian_partials": (C.c_int, [_f32p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "dmnerf_hungarian_costs_merged": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, _f32p, _f32p, _f32p, _f32p, _f32p,
+                                                C.c_void_p]),
+    "dmnerf_ins_loss_backward_shard": (C.c_int, [_f32p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, _f32p,
+                                                 _f32p, _f32p, _f32p, _f32p, C.c_void_p]),
     "dmnerf_stratify": (C.c_int, [_f32p, C.c_int64, _f32p, C.c_int64, C.c_int, _f32p, C.c_void_p]),
     "dmnerf_hier_sample": (C.c_int, [_f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, _f32p, C.c_void_p]),
     "dmnerf_act_floats_per_sample": (C.c_int, []),
@@ -90,6 +99,10 @@ PROTOTYPES = {
                                           _f32p, C.c_void_p]),
     "dmnerf_penalizer_backward": (C.c_int, [_f32p, _f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_float, C.c_float,
                                            C.c_void_p, _f32p, _f32p, C.c_int, C.c_void_p]),
+    "dmnerf_penalizer_partials_bytes": (C.c_int64, [C.c_int64, C.c_int, C.c_int]),
+    "dmnerf_penalizer_partials": (C.c_int, [_f32p, _f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_float, C.c_float,
+                                            C.c_void_p, C.c_void_p]),
+    "dmnerf_penalizer_merge": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, _f32p, C.c_void_p]),
     "dmnerf_profile_enable": (C.c_int, [C.c_void_p, C.c_int]),
     "dmnerf_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.c_int]),
     "dmnerf_render_forward_host": (C.c_int, [C.c_void_p, C.POINTER(RenderIO), C.c_int64, C.c_int, C.c_int, C.c_int,

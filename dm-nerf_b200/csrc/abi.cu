@@ -241,7 +241,7 @@ DMNERF_API int dmnerf_ins_loss_backward(const float* pred, const int32_t* gt_row
   DMN_CHECK(n >= 0, "ins_loss_backward: negative ray count");
   DMN_CHECK(n == 0 || (pred && gt_row && row_of_col && tp && col_sum && row_count && g_losses && d_pred),
             "ins_loss_backward: NULL buffer");
-  return launch_ins_loss_grad(pred, gt_row, n, ins_num, row_of_col, n_valid, nullptr, tp, col_sum, row_count, g_losses, d_pred,
+  return launch_ins_loss_grad(pred, gt_row, n, n, ins_num, row_of_col, n_valid, nullptr, tp, col_sum, row_count, g_losses, d_pred,
                               (cudaStream_t)stream);
 }
 
@@ -262,7 +262,41 @@ DMNERF_API int dmnerf_ins_loss_backward_dev(const float* pred, const int32_t* gt
   DMN_CHECK(n >= 0, "ins_loss_backward_dev: negative ray count");
   DMN_CHECK(n == 0 || (pred && gt_row && row_of_col && n_valid && tp && col_sum && row_count && g_losses && d_pred),
             "ins_loss_backward_dev: NULL buffer");
-  return launch_ins_loss_grad(pred, gt_row, n, ins_num, row_of_col, 0, n_valid, tp, col_sum, row_count, g_losses, d_pred,
+  return launch_ins_loss_grad(pred, gt_row, n, n, ins_num, row_of_col, 0, n_valid, tp, col_sum, row_count, g_losses, d_pred,
+                              (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_ins_label_bitmap(const int32_t* labels, int64_t n, uint32_t* bitmap, void* stream) {
+  DMN_CHECK(bitmap && (n == 0 || labels), "ins_label_bitmap: NULL buffer");
+  return launch_label_bitmap(labels, n, bitmap, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_ins_label_rows_merged(const uint32_t* bitmaps, int world, const int32_t* labels, int64_t n, int ins_num,
+                                            int32_t* gt_row, int32_t* n_valid, void* stream) {
+  DMN_CHECK(bitmaps && n_valid && (n == 0 || (labels && gt_row)), "ins_label_rows_merged: NULL buffer");
+  return launch_label_rows_merged(bitmaps, world, labels, n, ins_num, gt_row, n_valid, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_hungarian_partials(const float* pred, const int32_t* gt_row, int64_t n, int ins_num, double* partials,
+                                         void* stream) {
+  DMN_CHECK(partials && (n == 0 || (pred && gt_row)), "hungarian_partials: NULL buffer");
+  return launch_hungarian_partials(pred, gt_row, n, ins_num, partials, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_hungarian_costs_merged(const double* partials, int world, int64_t n_global, int ins_num, float* cost_ce,
+                                             float* cost_siou, float* tp, float* col_sum, float* row_count, void* stream) {
+  DMN_CHECK(partials && cost_ce && cost_siou && tp && col_sum && row_count, "hungarian_costs_merged: NULL buffer");
+  return launch_hungarian_costs_merged(partials, world, n_global, ins_num, cost_ce, cost_siou, tp, col_sum, row_count,
+                                       (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_ins_loss_backward_shard(const float* pred, const int32_t* gt_row, int64_t n, int64_t n_global, int ins_num,
+                                              const int32_t* row_of_col, const int32_t* n_valid, const float* tp, const float* col_sum,
+                                              const float* row_count, const float* g_losses, float* d_pred, void* stream) {
+  DMN_CHECK(n >= 0, "ins_loss_backward_shard: negative ray count");
+  DMN_CHECK(n == 0 || (pred && gt_row && row_of_col && n_valid && tp && col_sum && row_count && g_losses && d_pred),
+            "ins_loss_backward_shard: NULL buffer");
+  return launch_ins_loss_grad(pred, gt_row, n, n_global, ins_num, row_of_col, 0, n_valid, tp, col_sum, row_count, g_losses, d_pred,
                               (cudaStream_t)stream);
 }
 
@@ -319,6 +353,23 @@ DMNERF_API int dmnerf_composite_backward(const float* raw, const float* z, const
 }
 
 DMNERF_API int64_t dmnerf_penalizer_state_bytes(void) { return (int64_t)penalizer_state_bytes(); }
+
+DMNERF_API int64_t dmnerf_penalizer_partials_bytes(int64_t n, int s, int c) {
+  return (n < 0 || s < 1) ? -1 : (int64_t)penalizer_partials_bytes(n, s, c);
+}
+
+DMNERF_API int dmnerf_penalizer_partials(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,
+                                         int s, int c, float tolerance, float deta_w, void* partials, void* stream) {
+  DMN_CHECK(n >= 0, "penalizer_partials: negative ray count");
+  DMN_CHECK(partials && (n == 0 || (raw && z_vals && depth && rays_d)), "penalizer_partials: NULL buffer");
+  DMN_CHECK(deta_w > 0.0f, "penalizer_partials: deta_w must be positive");
+  return launch_penalizer_partials(raw, z_vals, depth, rays_d, n, s, c, tolerance, deta_w, partials, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_penalizer_merge(const void* states, int world, int c, void* state, float* loss, void* stream) {
+  DMN_CHECK(states && state && loss, "penalizer_merge: NULL buffer");
+  return launch_penalizer_merge(states, world, c, state, loss, (cudaStream_t)stream);
+}
 
 DMNERF_API int dmnerf_penalizer_forward(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,
                                         int s, int c, float tolerance, float deta_w, void* state, float* loss, void* stream) {

@@ -22,6 +22,19 @@ namespace dmnerf {
 
 constexpr int EV_MAX_K = DMNERF_MAX_INS + 1;
 
+// cost_ce / cost_siou / tp of cell (g, p), and col_sum / row_count, from the fp64 sums of the batch of n rays.
+__device__ __forceinline__ void write_costs(int g, int p, int k, int64_t n, double A, double S, double B, double C, double TP,
+                                            double cnt, float* __restrict__ cost_ce, float* __restrict__ cost_siou,
+                                            float* __restrict__ tp_out, float* __restrict__ cnt_out) {
+  cost_ce[(size_t)g * k + p] = (float)(-(B + A - C) / (double)n);
+  // the reference evaluates TP, FP = sum(pred) - TP, FN = sum(gt) - TP in fp32 and then TP / (TP + FP + FN + 1e-6)
+  const float tpf = (float)TP, fp = __fsub_rn((float)S, tpf), fn = __fsub_rn((float)cnt, tpf);
+  const float den = __fadd_rn(__fadd_rn(__fadd_rn(tpf, fp), fn), 1e-6f);
+  cost_siou[(size_t)g * k + p] = __fsub_rn(1.0f, __fdiv_rn(tpf, den));
+  tp_out[(size_t)g * k + p] = tpf;
+  if (p == 0) cnt_out[g] = (float)cnt;
+}
+
 // One block per prediction column p.
 __global__ void hungarian_cost_kernel(const float* __restrict__ pred, const int32_t* __restrict__ gt_row, int64_t n, int k,
                                       float* __restrict__ cost_ce, float* __restrict__ cost_siou, float* __restrict__ tp_out,
@@ -51,26 +64,103 @@ __global__ void hungarian_cost_kernel(const float* __restrict__ pred, const int3
   for (int d = 16; d > 0; d >>= 1) { a += __shfl_xor_sync(FULL, a, d); s += __shfl_xor_sync(FULL, s, d); }
   if ((threadIdx.x & 31) == 0) { atomicAdd(&sA, a); atomicAdd(&sS, s); }
   __syncthreads();
-  for (int g = threadIdx.x; g < k; g += blockDim.x) {
-    const double tp = sTP[g], cnt = (double)sCnt[g];
-    cost_ce[(size_t)g * k + p] = (float)(-(sB[g] + sA - sC[g]) / (double)n);
-    // the reference evaluates TP, FP = sum(pred) - TP, FN = sum(gt) - TP in fp32 and then TP / (TP + FP + FN + 1e-6)
-    const float tpf = (float)tp, fp = __fsub_rn((float)sS, tpf), fn = __fsub_rn((float)cnt, tpf);
-    const float den = __fadd_rn(__fadd_rn(__fadd_rn(tpf, fp), fn), 1e-6f);
-    cost_siou[(size_t)g * k + p] = __fsub_rn(1.0f, __fdiv_rn(tpf, den));
-    tp_out[(size_t)g * k + p] = tpf;
-    if (p == 0) cnt_out[g] = (float)cnt;
-  }
+  for (int g = threadIdx.x; g < k; g += blockDim.x)
+    write_costs(g, p, k, n, sA, sS, sB[g], sC[g], sTP[g], (double)sCnt[g], cost_ce, cost_siou, tp_out, cnt_out);
   if (threadIdx.x == 0) s_out[p] = (float)sS;
+}
+
+// ---------------------------------------------------------------------------------------------------- sharded batch
+// The sums above for one contiguous shard of the batch, in fp64, summed in an order fixed by the shard's size alone (no
+// floating-point atomics): partials = A[k] | S[k] | B[k x k] | C[k x k] | TP[k x k] | cnt[k] (row g, column p at g * k + p).
+// One block per column p; every warp walks 32-row chunks, adds the rows of one label in lane order and keeps its own
+// per-label sums; the warps' sums are added in warp order at the end.
+constexpr int HP_WARPS = 8;
+__global__ void __launch_bounds__(HP_WARPS * 32) hungarian_partials_kernel(const float* __restrict__ pred,
+                                                                             const int32_t* __restrict__ gt_row, int64_t n, int k,
+                                                                             double* __restrict__ out) {
+  __shared__ double wB[HP_WARPS][EV_MAX_K], wC[HP_WARPS][EV_MAX_K], wTP[HP_WARPS][EV_MAX_K];
+  __shared__ unsigned int wCnt[HP_WARPS][EV_MAX_K];
+  __shared__ double stage[HP_WARPS][3][32];
+  __shared__ double wA[HP_WARPS], wS[HP_WARPS];
+  const int p = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int g = lane; g < k; g += 32) { wB[warp][g] = 0.0; wC[warp][g] = 0.0; wTP[warp][g] = 0.0; wCnt[warp][g] = 0u; }
+  __syncwarp();
+  double a = 0.0, s = 0.0;
+  for (int64_t base = (int64_t)warp * 32; base < n; base += HP_WARPS * 32) {      // warp-uniform trip count
+    const int64_t i = base + lane;
+    int g = -1;
+    double lb = 0.0, lc = 0.0, v = 0.0;
+    if (i < n) {
+      const float vf = pred[i * k + p];
+      const float l1 = logf(__fadd_rn(__fsub_rn(1.0f, vf), 1e-8f));
+      a += (double)l1;
+      s += (double)vf;
+      g = gt_row[i];
+      if (g >= 0 && g < k) { lb = (double)logf(__fadd_rn(vf, 1e-8f)); lc = (double)l1; v = (double)vf; }
+      else g = -1;
+    }
+    stage[warp][0][lane] = lb; stage[warp][1][lane] = lc; stage[warp][2][lane] = v;
+    const unsigned grp = __match_any_sync(FULL, g);
+    __syncwarp();
+    if (g >= 0 && lane == __ffs(grp) - 1) {                 // the lowest lane of each label adds that label's rows in lane order
+      double b = 0.0, c = 0.0, t = 0.0;
+      for (unsigned m = grp; m; m &= m - 1) {
+        const int j = __ffs(m) - 1;
+        b += stage[warp][0][j]; c += stage[warp][1][j]; t += stage[warp][2][j];
+      }
+      wB[warp][g] += b; wC[warp][g] += c; wTP[warp][g] += t; wCnt[warp][g] += __popc(grp);
+    }
+    __syncwarp();
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) { a += __shfl_xor_sync(FULL, a, d); s += __shfl_xor_sync(FULL, s, d); }
+  if (lane == 0) { wA[warp] = a; wS[warp] = s; }
+  __syncthreads();
+  const size_t kk = (size_t)k * k;
+  double* A = out; double* S = out + k; double* B = out + 2 * k; double* C = B + kk; double* TP = C + kk; double* cnt = TP + kk;
+  for (int g = threadIdx.x; g < k; g += blockDim.x) {
+    double b = 0.0, c = 0.0, t = 0.0;
+    unsigned int m = 0u;
+    for (int w = 0; w < HP_WARPS; ++w) { b += wB[w][g]; c += wC[w][g]; t += wTP[w][g]; m += wCnt[w][g]; }
+    B[(size_t)g * k + p] = b; C[(size_t)g * k + p] = c; TP[(size_t)g * k + p] = t;
+    if (p == 0) cnt[g] = (double)m;
+  }
+  if (threadIdx.x == 0) {
+    double ta = 0.0, ts = 0.0;
+    for (int w = 0; w < HP_WARPS; ++w) { ta += wA[w]; ts += wS[w]; }
+    A[p] = ta; S[p] = ts;
+  }
+}
+
+// The partials of `world` shards added in shard order, then hungarian_cost_kernel's formulas with the global ray count n.
+__global__ void hungarian_costs_merged_kernel(const double* __restrict__ partials, int world, int64_t n, int k,
+                                              float* __restrict__ cost_ce, float* __restrict__ cost_siou, float* __restrict__ tp_out,
+                                              float* __restrict__ s_out, float* __restrict__ cnt_out) {
+  const int p = blockIdx.x;
+  const size_t kk = (size_t)k * k, stride = 3 * (size_t)k + 3 * kk;
+  double A = 0.0, S = 0.0;
+  for (int w = 0; w < world; ++w) { A += partials[w * stride + p]; S += partials[w * stride + k + p]; }
+  for (int g = threadIdx.x; g < k; g += blockDim.x) {
+    const size_t cell = 2 * (size_t)k + (size_t)g * k + p;
+    double B = 0.0, C = 0.0, TP = 0.0, cnt = 0.0;
+    for (int w = 0; w < world; ++w) {
+      const double* q = partials + w * stride;
+      B += q[cell]; C += q[cell + kk]; TP += q[cell + 2 * kk]; cnt += q[2 * k + 3 * kk + g];
+    }
+    write_costs(g, p, k, n, A, S, B, C, TP, cnt, cost_ce, cost_siou, tp_out, cnt_out);
+  }
+  if (threadIdx.x == 0) s_out[p] = (float)S;
 }
 
 // d loss / d pred for  loss = g_ce * valid_ce + g_inv * invalid_ce + g_siou * valid_siou  (evaluator.py:27-36):
 //   valid_ce = mean_{g < V} cost_ce[g, col(g)],  valid_siou likewise,  invalid_ce = mean(pred[:, unmatched columns]).
 // row_of_col[p] = matched gt row of prediction column p, or -1 (unmatched).  g3 = the three upstream gradients (device).
-__global__ void ins_loss_grad_kernel(const float* __restrict__ pred, const int32_t* __restrict__ gt_row, int64_t n, int k,
-                                     const int32_t* __restrict__ row_of_col, int n_valid, const int32_t* __restrict__ n_valid_dev,
-                                     const float* __restrict__ tp, const float* __restrict__ s_sum, const float* __restrict__ cnt,
-                                     const float* __restrict__ g3, float* __restrict__ d_pred) {
+// n rows of pred are written; n_norm is the ray count of the whole batch (n_norm > n for one shard of it).
+__global__ void ins_loss_grad_kernel(const float* __restrict__ pred, const int32_t* __restrict__ gt_row, int64_t n, int64_t n_norm,
+                                     int k, const int32_t* __restrict__ row_of_col, int n_valid,
+                                     const int32_t* __restrict__ n_valid_dev, const float* __restrict__ tp,
+                                     const float* __restrict__ s_sum, const float* __restrict__ cnt, const float* __restrict__ g3,
+                                     float* __restrict__ d_pred) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n * k) return;
   if (n_valid_dev) {                         // device-side assignment: the number of distinct labels never left the device
@@ -89,9 +179,9 @@ __global__ void ins_loss_grad_kernel(const float* __restrict__ pred, const int32
     const float t = tp[(size_t)g * k + p];
     const float den = (s_sum[p] + cnt[g] - t) + 1e-6f;
     const float dsi = on ? -1.0f / den : t / (den * den);      // -(gt D - TP (1 - gt)) / D^2
-    d = g3[0] * inv_v * dce / (float)n + g3[2] * inv_v * dsi;
+    d = g3[0] * inv_v * dce / (float)n_norm + g3[2] * inv_v * dsi;
   } else {
-    d = g3[1] / ((float)n * (float)(k - n_valid));
+    d = g3[1] / ((float)n_norm * (float)(k - n_valid));
   }
   d_pred[idx] = d;
 }
@@ -102,22 +192,20 @@ __global__ void ins_loss_grad_kernel(const float* __restrict__ pred, const int32
 // distinct labels than prediction channels: n_valid = -1 (the loss comes out NaN, its gradient zero) and the code goes to the
 // status word (mapped host memory: the next ins_criterion call raises without any synchronisation).
 constexpr int LBL_WORDS = 2048;            // 65536 label values
-__global__ void __launch_bounds__(1024) label_rows_kernel(const int32_t* __restrict__ labels, int64_t n, int k,
-                                                          int32_t* __restrict__ gt_row, int32_t* __restrict__ n_valid_out,
-                                                          int32_t* status) {
-  __shared__ uint32_t bitmap[LBL_WORDS], prefix[LBL_WORDS];
-  __shared__ uint32_t warp_tot[32];
-  __shared__ int bad_s;
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  bitmap[2 * t] = 0u; bitmap[2 * t + 1] = 0u;
-  if (t == 0) bad_s = 0;
-  __syncthreads();
-  for (int64_t i = t; i < n; i += 1024) {
+static_assert(DMNERF_LABEL_WORDS == LBL_WORDS + 1, "bitmap layout of dmnerf_ins_label_bitmap");
+
+// Bitmap of the labels[0..n) into shared memory (1024 threads); bad_s = 1 when a label is outside [0, 65536).
+__device__ __forceinline__ void label_presence(const int32_t* __restrict__ labels, int64_t n, uint32_t* bitmap, int* bad_s) {
+  for (int64_t i = threadIdx.x; i < n; i += 1024) {
     const int l = labels[i];
-    if (l < 0 || l >= LBL_WORDS * 32) bad_s = 1;
+    if (l < 0 || l >= LBL_WORDS * 32) *bad_s = 1;
     else atomicOr(&bitmap[l >> 5], 1u << (l & 31));
   }
-  __syncthreads();
+}
+
+// prefix[w] = number of labels present in words 0..w-1 of the bitmap (1024 threads); returns the number of labels present.
+__device__ __forceinline__ int label_prefix(const uint32_t* bitmap, uint32_t* prefix, uint32_t* warp_tot) {
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const uint32_t c0 = __popc(bitmap[2 * t]), c1 = __popc(bitmap[2 * t + 1]);
   uint32_t incl = c0 + c1;
 #pragma unroll
@@ -134,18 +222,82 @@ __global__ void __launch_bounds__(1024) label_rows_kernel(const int32_t* __restr
   const uint32_t excl = incl - (c0 + c1) + (warp ? warp_tot[warp - 1] : 0u);
   prefix[2 * t] = excl; prefix[2 * t + 1] = excl + c0;
   __syncthreads();
-  const int n_valid = (int)warp_tot[31];
-  const bool bad = bad_s != 0 || n_valid > k || n_valid < 1;
-  for (int64_t i = t; i < n; i += 1024) {
+  return (int)warp_tot[31];
+}
+
+// gt_row[i] = rank of labels[i] among the labels of the bitmap (-1 for all rows when `bad`), n_valid_out, error code.
+__device__ __forceinline__ void label_rank_rows(const int32_t* __restrict__ labels, int64_t n, const uint32_t* bitmap,
+                                                const uint32_t* prefix, int n_valid, bool bad, int code, int32_t* __restrict__ gt_row,
+                                                int32_t* __restrict__ n_valid_out, int32_t* status) {
+  for (int64_t i = threadIdx.x; i < n; i += 1024) {
     const int l = labels[i];
     int row = -1;
     if (!bad && l >= 0 && l < LBL_WORDS * 32) row = (int)(prefix[l >> 5] + __popc(bitmap[l >> 5] & ((1u << (l & 31)) - 1u)));
     gt_row[i] = row;
   }
-  if (t == 0) {
+  if (threadIdx.x == 0) {
     *n_valid_out = bad ? -1 : n_valid;
-    if (bad && status) atomicCAS(status, 0, bad_s ? 701 : 702);
+    if (bad && status) atomicCAS(status, 0, code);
   }
+}
+
+__global__ void __launch_bounds__(1024) label_rows_kernel(const int32_t* __restrict__ labels, int64_t n, int k,
+                                                          int32_t* __restrict__ gt_row, int32_t* __restrict__ n_valid_out,
+                                                          int32_t* status) {
+  __shared__ uint32_t bitmap[LBL_WORDS], prefix[LBL_WORDS];
+  __shared__ uint32_t warp_tot[32];
+  __shared__ int bad_s;
+  const int t = threadIdx.x;
+  bitmap[2 * t] = 0u; bitmap[2 * t + 1] = 0u;
+  if (t == 0) bad_s = 0;
+  __syncthreads();
+  label_presence(labels, n, bitmap, &bad_s);
+  __syncthreads();
+  const int n_valid = label_prefix(bitmap, prefix, warp_tot);
+  const bool bad = bad_s != 0 || n_valid > k || n_valid < 1;
+  label_rank_rows(labels, n, bitmap, prefix, n_valid, bad, bad_s ? 701 : 702, gt_row, n_valid_out, status);
+}
+
+// One shard's presence bitmap: words 0..2047 over label values [0, 65536), word 2048 = 1 when a label is out of range (which
+// also goes to the status word: 701).  OR is order-free, so the bitmap does not depend on scheduling.
+__global__ void __launch_bounds__(1024) label_bitmap_kernel(const int32_t* __restrict__ labels, int64_t n, uint32_t* __restrict__ out,
+                                                            int32_t* status) {
+  __shared__ uint32_t bitmap[LBL_WORDS];
+  __shared__ int bad_s;
+  const int t = threadIdx.x;
+  bitmap[2 * t] = 0u; bitmap[2 * t + 1] = 0u;
+  if (t == 0) bad_s = 0;
+  __syncthreads();
+  label_presence(labels, n, bitmap, &bad_s);
+  __syncthreads();
+  out[2 * t] = bitmap[2 * t]; out[2 * t + 1] = bitmap[2 * t + 1];
+  if (t == 0) {
+    out[LBL_WORDS] = bad_s ? 1u : 0u;
+    if (bad_s && status) atomicCAS(status, 0, 701);
+  }
+}
+
+// label_rows_kernel on the OR of `world` shard bitmaps (rank order) for the shard's own labels: every shard ranks its rows among
+// the distinct labels of the whole batch and every shard gets the same n_valid (or -1 and the same error code).
+__global__ void __launch_bounds__(1024) label_rows_merged_kernel(const uint32_t* __restrict__ bitmaps, int world,
+                                                                 const int32_t* __restrict__ labels, int64_t n, int k,
+                                                                 int32_t* __restrict__ gt_row, int32_t* __restrict__ n_valid_out,
+                                                                 int32_t* status) {
+  __shared__ uint32_t bitmap[LBL_WORDS], prefix[LBL_WORDS];
+  __shared__ uint32_t warp_tot[32];
+  __shared__ int bad_s;
+  const int t = threadIdx.x;
+  uint32_t b0 = 0u, b1 = 0u, flag = 0u;
+  for (int w = 0; w < world; ++w) {
+    const uint32_t* q = bitmaps + (size_t)w * (LBL_WORDS + 1);
+    b0 |= q[2 * t]; b1 |= q[2 * t + 1]; flag |= q[LBL_WORDS];
+  }
+  bitmap[2 * t] = b0; bitmap[2 * t + 1] = b1;
+  if (t == 0) bad_s = flag != 0u;
+  __syncthreads();
+  const int n_valid = label_prefix(bitmap, prefix, warp_tot);
+  const bool bad = bad_s != 0 || n_valid > k || n_valid < 1;
+  label_rank_rows(labels, n, bitmap, prefix, n_valid, bad, bad_s ? 701 : 702, gt_row, n_valid_out, status);
 }
 
 // scipy.optimize.linear_sum_assignment (the rectangular shortest-augmenting-path solver of Crouse 2016 that scipy implements) on
@@ -262,15 +414,33 @@ int launch_hungarian_costs(const float* pred, const int32_t* gt_row, int64_t n, 
   return 0;
 }
 
-int launch_ins_loss_grad(const float* pred, const int32_t* gt_row, int64_t n, int k, const int32_t* row_of_col, int n_valid,
-                         const int32_t* n_valid_dev, const float* tp, const float* s_sum, const float* cnt, const float* g3,
+int launch_ins_loss_grad(const float* pred, const int32_t* gt_row, int64_t n, int64_t n_norm, int k, const int32_t* row_of_col,
+                         int n_valid, const int32_t* n_valid_dev, const float* tp, const float* s_sum, const float* cnt, const float* g3,
                          float* d_pred, cudaStream_t st) {
   DMN_CHECK(k >= 1 && k <= EV_MAX_K && (n_valid_dev || (n_valid >= 1 && n_valid <= k)), "ins_loss_grad: bad sizes (k %d, valid %d)", k,
             n_valid);
+  DMN_CHECK(n_norm >= n, "ins_loss_grad: %lld rows of a batch of %lld", (long long)n, (long long)n_norm);
   const int64_t total = n * k;
   if (total == 0) return 0;
-  ins_loss_grad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(pred, gt_row, n, k, row_of_col, n_valid, n_valid_dev, tp,
-                                                                        s_sum, cnt, g3, d_pred);
+  ins_loss_grad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(pred, gt_row, n, n_norm, k, row_of_col, n_valid, n_valid_dev,
+                                                                        tp, s_sum, cnt, g3, d_pred);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+int launch_hungarian_partials(const float* pred, const int32_t* gt_row, int64_t n, int k, double* partials, cudaStream_t st) {
+  DMN_CHECK(k >= 1 && k <= EV_MAX_K, "hungarian_partials: ins_num %d out of range (max %d)", k, EV_MAX_K);
+  DMN_CHECK(n >= 0, "hungarian_partials: negative ray count");
+  hungarian_partials_kernel<<<(unsigned)k, HP_WARPS * 32, 0, st>>>(pred, gt_row, n, k, partials);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+int launch_hungarian_costs_merged(const double* partials, int world, int64_t n, int k, float* cost_ce, float* cost_siou, float* tp,
+                                  float* s_sum, float* cnt, cudaStream_t st) {
+  DMN_CHECK(k >= 1 && k <= EV_MAX_K, "hungarian_costs_merged: ins_num %d out of range (max %d)", k, EV_MAX_K);
+  DMN_CHECK(world >= 1 && n >= 1, "hungarian_costs_merged: %d shards of a batch of %lld rays", world, (long long)n);
+  hungarian_costs_merged_kernel<<<(unsigned)k, 128, 0, st>>>(partials, world, n, k, cost_ce, cost_siou, tp, s_sum, cnt);
   DMN_LAUNCH_OK();
   return 0;
 }
@@ -300,6 +470,24 @@ int launch_label_rows(const int32_t* labels, int64_t n, int k, int32_t* gt_row, 
   DMN_CHECK(n >= 1, "ins_label_rows: empty batch");
   if (ins_status_init()) return 1;
   label_rows_kernel<<<1, 1024, 0, st>>>(labels, n, k, gt_row, n_valid, g_ins_d_status);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+int launch_label_bitmap(const int32_t* labels, int64_t n, uint32_t* bitmap, cudaStream_t st) {
+  DMN_CHECK(n >= 0, "ins_label_bitmap: negative ray count");
+  if (ins_status_init()) return 1;
+  label_bitmap_kernel<<<1, 1024, 0, st>>>(labels, n, bitmap, g_ins_d_status);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+int launch_label_rows_merged(const uint32_t* bitmaps, int world, const int32_t* labels, int64_t n, int k, int32_t* gt_row,
+                             int32_t* n_valid, cudaStream_t st) {
+  DMN_CHECK(k >= 1 && k <= EV_MAX_K, "ins_label_rows_merged: ins_num %d out of range (max %d)", k, EV_MAX_K);
+  DMN_CHECK(world >= 1 && n >= 0, "ins_label_rows_merged: %d shards, %lld rows", world, (long long)n);
+  if (ins_status_init()) return 1;
+  label_rows_merged_kernel<<<1, 1024, 0, st>>>(bitmaps, world, labels, n, k, gt_row, n_valid, g_ins_d_status);
   DMN_LAUNCH_OK();
   return 0;
 }

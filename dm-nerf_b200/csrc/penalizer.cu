@@ -54,11 +54,11 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 // traffic is fully coalesced (a thread-per-sample walk over rows of 18..132 floats touches partial sectors only).
 static int pen_tile(int c) { return c <= 48 ? 256 : (c <= 96 ? 128 : 64); }
 
-// Forward in ONE pass: mask populations (integer atomics: exact), the two masked sums (fp64 accumulation of fp32 terms), and
-// the finalisation by the last block -- the sums do not depend on the populations until the final division.
-__global__ void penalizer_loss_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ depth,
-                                      const float* __restrict__ rays_d, int64_t total, int s, int c, float tol, float w,
-                                      PenState* st, float* __restrict__ loss) {
+// This block's two masked sums (fp64 accumulation of fp32 terms) and two mask populations, valid in thread 0; the block's
+// rows of raw are staged through shared memory.
+__device__ __forceinline__ void pen_block_terms(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ depth,
+                                                const float* __restrict__ rays_d, int64_t total, int s, int c, float tol, float w,
+                                                double& tb, double& tm, unsigned long long& cb, unsigned long long& cm) {
   extern __shared__ float sraw[];
   const int tile = blockDim.x;
   const int64_t idx0 = (int64_t)blockIdx.x * tile;
@@ -96,24 +96,93 @@ __global__ void penalizer_loss_kernel(const float* __restrict__ raw, const float
   const int wid = threadIdx.x >> 5;
   if ((threadIdx.x & 31) == 0) { sh_b[wid] = sb; sh_m[wid] = sm; sh_nb[wid] = nb; sh_nm[wid] = nm; }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    double tb = 0.0, tm = 0.0;
-    unsigned long long cb = 0, cm = 0;
+  tb = 0.0; tm = 0.0; cb = 0; cm = 0;
+  if (threadIdx.x == 0)
     for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { tb += sh_b[i]; tm += sh_m[i]; cb += sh_nb[i]; cm += sh_nm[i]; }
+}
+
+// penalizer.py:42-43, 52-53
+__device__ __forceinline__ float pen_finalise(unsigned long long n_before, unsigned long long n_middle, double sum_before,
+                                              double sum_middle, int K) {
+  const double nbt = fmax((double)n_before, 1e-8), nmt = fmax((double)n_middle, 1e-8);
+  return (float)(sum_before / ((double)K * nbt) + sum_middle / nmt);
+}
+
+// Forward in ONE pass: mask populations (integer atomics: exact), the two masked sums (fp64 accumulation of fp32 terms), and
+// the finalisation by the last block -- the sums do not depend on the populations until the final division.
+__global__ void penalizer_loss_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ depth,
+                                      const float* __restrict__ rays_d, int64_t total, int s, int c, float tol, float w,
+                                      PenState* st, float* __restrict__ loss) {
+  double tb, tm;
+  unsigned long long cb, cm;
+  pen_block_terms(raw, z, depth, rays_d, total, s, c, tol, w, tb, tm, cb, cm);
+  if (threadIdx.x == 0) {
     atomicAdd(&st->sum_before, tb);
     atomicAdd(&st->sum_middle, tm);
     if (cb) atomicAdd(&st->n_before, cb);
     if (cm) atomicAdd(&st->n_middle, cm);
     __threadfence();
-    if (atomicAdd(&st->blocks_done, 1u) == gridDim.x - 1) {        // last block: finalise (penalizer.py:42-43, 52-53)
+    if (atomicAdd(&st->blocks_done, 1u) == gridDim.x - 1) {        // last block: finalise
       __threadfence();
-      const double nbt = fmax((double)*(volatile unsigned long long*)&st->n_before, 1e-8);
-      const double nmt = fmax((double)*(volatile unsigned long long*)&st->n_middle, 1e-8);
-      const double lb = *(volatile double*)&st->sum_before / ((double)K * nbt);
-      const double lm = *(volatile double*)&st->sum_middle / nmt;
-      loss[0] = (float)(lb + lm);
+      loss[0] = pen_finalise(*(volatile unsigned long long*)&st->n_before, *(volatile unsigned long long*)&st->n_middle,
+                             *(volatile double*)&st->sum_before, *(volatile double*)&st->sum_middle, c - 4);
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------------------- sharded batch
+// The populations and masked sums of one shard of the batch, unfinalised, summed in an order fixed by the shard's size alone:
+// every block writes its terms to its own slot after the PenState head, and the last block to finish adds the slots with a
+// fixed-shape reduction into the head.
+struct PenBlock {
+  double sb, sm;
+  unsigned long long nb, nm;
+};
+
+__global__ void penalizer_partial_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ depth,
+                                         const float* __restrict__ rays_d, int64_t total, int s, int c, float tol, float w,
+                                         PenState* st, PenBlock* blocks) {
+  double tb, tm;
+  unsigned long long cb, cm;
+  pen_block_terms(raw, z, depth, rays_d, total, s, c, tol, w, tb, tm, cb, cm);
+  __shared__ bool last;
+  if (threadIdx.x == 0) {
+    blocks[blockIdx.x] = PenBlock{tb, tm, cb, cm};
+    __threadfence();
+    last = atomicAdd(&st->blocks_done, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double sb = 0.0, sm = 0.0;
+  unsigned long long nb = 0, nm = 0;
+  for (unsigned b = threadIdx.x; b < gridDim.x; b += blockDim.x) {
+    sb += __ldcg(&blocks[b].sb); sm += __ldcg(&blocks[b].sm); nb += __ldcg(&blocks[b].nb); nm += __ldcg(&blocks[b].nm);
+  }
+  sb = warp_sum_d(sb);
+  sm = warp_sum_d(sm);
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) { nb += __shfl_xor_sync(FULL, nb, d); nm += __shfl_xor_sync(FULL, nm, d); }
+  __shared__ PenBlock wsum[8];
+  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = PenBlock{sb, sm, nb, nm};
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    PenBlock t{0.0, 0.0, 0, 0};
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { t.sb += wsum[i].sb; t.sm += wsum[i].sm; t.nb += wsum[i].nb; t.nm += wsum[i].nm; }
+    st->sum_before = t.sb; st->sum_middle = t.sm; st->n_before = t.nb; st->n_middle = t.nm;
+  }
+}
+
+// `world` shard heads added in shard order into `out` (what penalizer_grad_kernel reads) and the loss of the whole batch.
+__global__ void penalizer_merge_kernel(const PenState* __restrict__ parts, int world, int K, PenState* __restrict__ out,
+                                       float* __restrict__ loss) {
+  PenState t{};
+  for (int r = 0; r < world; ++r) {
+    t.n_before += parts[r].n_before; t.n_middle += parts[r].n_middle;
+    t.sum_before += parts[r].sum_before; t.sum_middle += parts[r].sum_middle;
+  }
+  *out = t;
+  loss[0] = pen_finalise(t.n_before, t.n_middle, t.sum_before, t.sum_middle, K);
 }
 
 // d_raw = g_loss * dL/d raw: every channel of every row is written (channels 0..3 get zeros), through shared memory, so the
@@ -194,5 +263,35 @@ int launch_penalizer_backward(const float* raw, const float* z, const float* dep
 }
 
 size_t penalizer_state_bytes() { return sizeof(PenState); }
+
+static_assert(sizeof(PenState) % alignof(PenBlock) == 0, "block slots follow the head");
+size_t penalizer_partials_bytes(int64_t n, int s, int c) {
+  const int64_t total = n * s;
+  const int tile = pen_tile(c);
+  return sizeof(PenState) + (size_t)((total + tile - 1) / tile) * sizeof(PenBlock);
+}
+
+int launch_penalizer_partials(const float* raw, const float* z, const float* depth, const float* rays_d, int64_t n, int s, int c,
+                              float tol, float w, void* partials, cudaStream_t st) {
+  DMN_CHECK(c > 4 && c <= 4 + DMNERF_MAX_INS + 1 && s >= 1, "penalizer: bad sizes s=%d c=%d", s, c);
+  PenState* ps = reinterpret_cast<PenState*>(partials);
+  DMN_CUDA(cudaMemsetAsync(ps, 0, sizeof(PenState), st));
+  const int64_t total = n * s;
+  if (total == 0) return 0;
+  const int tile = pen_tile(c);
+  const unsigned grid = (unsigned)((total + tile - 1) / tile);
+  penalizer_partial_kernel<<<grid, tile, (size_t)tile * c * sizeof(float), st>>>(raw, z, depth, rays_d, total, s, c, tol, w, ps,
+                                                                                 reinterpret_cast<PenBlock*>(ps + 1));
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+int launch_penalizer_merge(const void* states, int world, int c, void* state, float* loss, cudaStream_t st) {
+  DMN_CHECK(c > 4 && c <= 4 + DMNERF_MAX_INS + 1 && world >= 1, "penalizer_merge: bad sizes world=%d c=%d", world, c);
+  penalizer_merge_kernel<<<1, 1, 0, st>>>(reinterpret_cast<const PenState*>(states), world, c - 4, reinterpret_cast<PenState*>(state),
+                                          loss);
+  DMN_LAUNCH_OK();
+  return 0;
+}
 
 }  // namespace dmnerf

@@ -159,6 +159,34 @@ DMNERF_API int dmnerf_ins_loss_backward_dev(const float* pred, const int32_t* gt
                                             const float* row_count, const float* g_losses, float* d_pred, void* stream);
 DMNERF_API int dmnerf_ins_status_take(void);
 
+/* The same loss over a batch split into W contiguous shards (one per process, dmnerf_b200.distributed): each shard computes
+ * partials, the caller all-gathers them, and every shard merges the W buffers in shard order, so every shard feeds bit-identical
+ * inputs to dmnerf_hungarian_assign (which is passed the global N).  Every sum runs in an order fixed by the sizes alone: no
+ * floating-point atomics.
+ * dmnerf_ins_label_bitmap: labels [n] -> bitmap [DMNERF_LABEL_WORDS] (DEVICE uint32): words 0..2047 mark the label values
+ *   [0, 65536) present in the shard, word 2048 is 1 when a label is out of range (also posted to the status word: 701).
+ * dmnerf_ins_label_rows_merged: bitmaps [world, DMNERF_LABEL_WORDS] (the gathered bitmaps, rank order) and the shard's labels [n]
+ *   -> gt_row [n] = rank of the label among the distinct labels of the whole batch, n_valid[0] (dmnerf_ins_label_rows' rules:
+ *   -1 and status 701 / 702 for an out-of-range label in any shard or more distinct labels than ins_num).
+ * dmnerf_hungarian_partials: pred [n,ins_num], gt_row [n] -> partials [3 ins_num (ins_num + 1)] (DEVICE fp64), laid out
+ *   A[k] | S[k] | B[k,k] | C[k,k] | TP[k,k] | cnt[k] with k = ins_num, element (g, p) at g * k + p:
+ *   A[p] = sum log(1 - pred[:,p] + 1e-8), S[p] = sum pred[:,p], and over the rays of row g: B = sum log(pred + 1e-8),
+ *   C = sum log(1 - pred + 1e-8), TP = sum pred, cnt = ray count.
+ * dmnerf_hungarian_costs_merged: partials [world, 3 k (k + 1)] added in shard order -> cost_ce, cost_siou, tp, col_sum, row_count
+ *   exactly as dmnerf_hungarian_costs computes them from those sums, normalised by n_global.
+ * dmnerf_ins_loss_backward_shard: dmnerf_ins_loss_backward_dev for the shard's n rows of a batch of n_global rays. */
+#define DMNERF_LABEL_WORDS 2049
+DMNERF_API int dmnerf_ins_label_bitmap(const int32_t* labels, int64_t n, uint32_t* bitmap, void* stream);
+DMNERF_API int dmnerf_ins_label_rows_merged(const uint32_t* bitmaps, int world, const int32_t* labels, int64_t n, int ins_num,
+                                            int32_t* gt_row, int32_t* n_valid, void* stream);
+DMNERF_API int dmnerf_hungarian_partials(const float* pred, const int32_t* gt_row, int64_t n, int ins_num, double* partials,
+                                         void* stream);
+DMNERF_API int dmnerf_hungarian_costs_merged(const double* partials, int world, int64_t n_global, int ins_num, float* cost_ce,
+                                             float* cost_siou, float* tp, float* col_sum, float* row_count, void* stream);
+DMNERF_API int dmnerf_ins_loss_backward_shard(const float* pred, const int32_t* gt_row, int64_t n, int64_t n_global, int ins_num,
+                                              const int32_t* row_of_col, const int32_t* n_valid, const float* tp, const float* col_sum,
+                                              const float* row_count, const float* g_losses, float* d_pred, void* stream);
+
 /* Coarse depths, networks/render.py:40-47: z_out[n, i] = z_in row (shared when z_row_stride = 0), jittered inside its
  * stratum by t_rand [N,S] when given. */
 DMNERF_API int dmnerf_stratify(const float* z_in, int64_t z_row_stride, const float* t_rand, int64_t n, int s, float* z_out,
@@ -237,6 +265,17 @@ DMNERF_API int dmnerf_penalizer_forward(const float* raw, const float* z_vals, c
 DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,
                                          int s, int c, float tolerance, float deta_w, const void* state, const float* g_loss,
                                          float* d_raw, int accumulate, void* stream);
+
+/* The penalizer over a batch split into W shards.  dmnerf_penalizer_partials writes the shard's mask populations and masked sums,
+ * unfinalised and summed in an order fixed by the sizes, into the head (the first dmnerf_penalizer_state_bytes() bytes) of
+ * `partials`, a device buffer of dmnerf_penalizer_partials_bytes(n, s, c) bytes (the rest is per-block scratch).
+ * dmnerf_penalizer_merge: the W gathered heads (`states`, W * dmnerf_penalizer_state_bytes() bytes, rank order), added in rank
+ * order -> `state` (a dmnerf_penalizer_backward state for the whole batch; that call then gives the shard's gradient) and
+ * loss[1]. */
+DMNERF_API int64_t dmnerf_penalizer_partials_bytes(int64_t n, int s, int c);
+DMNERF_API int dmnerf_penalizer_partials(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,
+                                         int s, int c, float tolerance, float deta_w, void* partials, void* stream);
+DMNERF_API int dmnerf_penalizer_merge(const void* states, int world, int c, void* state, float* loss, void* stream);
 
 /* dm_nerf(), networks/render.py:31-96, whole per-ray pipeline on device buffers. */
 DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n_rays, int n_coarse,
