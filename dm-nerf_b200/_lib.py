@@ -18,7 +18,7 @@ LIB_PATH = os.environ.get("DMNERF_LIB_PATH") or os.path.join(_HERE, "lib", "libd
 
 ABI_VERSION = 1
 N_PARAMS = 30
-IMPL_AUTO, IMPL_SIMT, IMPL_UMMA = 0, 1, 2
+IMPL_AUTO, IMPL_SIMT, IMPL_UMMA, IMPL_UMMA_F16 = 0, 1, 2, 3
 FLAG_PERTURB, FLAG_WANT_RAW, FLAG_KEEP_INS = 1, 2, 4
 LABEL_WORDS = 2049           # DMNERF_LABEL_WORDS
 
@@ -222,6 +222,16 @@ def camera(K, c2w):
 def keep_mask(words):
     """The 4-word object-selection mask (objects.object_mask) as the ABI's host uint32[4]."""
     return (C.c_uint32 * 4)(*words)
+
+
+# DMNERF_INFER_IMPL=f16: IMPL_AUTO of an INFERENCE call means the fp16 preview network (IMPL_UMMA_F16), so that unmodified
+# scripts render previews.  Read here only; the training forward (backward._train_impl) never consults it.
+INFER_IMPL = IMPL_UMMA_F16 if os.environ.get("DMNERF_INFER_IMPL", "").strip().lower() == "f16" else IMPL_AUTO
+
+
+def infer_impl(impl):
+    """The network an inference entry point runs for `impl`: IMPL_AUTO follows DMNERF_INFER_IMPL, anything else is kept."""
+    return INFER_IMPL if impl == IMPL_AUTO else impl
 
 
 def need_cuda(what, *ts):

@@ -25,6 +25,7 @@ def mlp_forward(model, x, impl=_lib.IMPL_AUTO):
     if _needs_grad(model, x):
         from .backward import mlp_forward_grad
         return mlp_forward_grad(model, x, impl)
+    impl = _lib.infer_impl(impl)
     ctx = get_context(x.device)
     slot = ctx.slot_for(model)
     ins_num = ctx.bind(slot, model)
@@ -37,7 +38,8 @@ def mlp_forward(model, x, impl=_lib.IMPL_AUTO):
 
 
 def mlp_forward_rays(model, rays_o, rays_d, z, impl=_lib.IMPL_AUTO):
-    """Network evaluated at pts = o + d*z with both embeddings fused in (render.py:49-61)."""
+    """Network evaluated at pts = o + d*z with both embeddings fused in (render.py:49-61).  Inference only."""
+    impl = _lib.infer_impl(impl)
     ctx = get_context(z.device)
     slot = ctx.slot_for(model)
     ins_num = ctx.bind(slot, model)
@@ -57,6 +59,7 @@ def mlp_forward_points(model, pts, viewdirs=None, impl=_lib.IMPL_AUTO):
     sweep of tools/mesh_generator.py:36-49.  pts [..., 3] -> [..., 4 + ins_num + 1]."""
     if not pts.is_cuda:
         raise RuntimeError("mlp_forward_points: expected CUDA tensors (no CPU fallback)")
+    impl = _lib.infer_impl(impl)
     ctx = get_context(pts.device)
     slot = ctx.slot_for(model)
     ins_num = ctx.bind(slot, model)

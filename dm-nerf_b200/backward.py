@@ -20,6 +20,9 @@ TRAIN_IMPL = _lib.IMPL_SIMT if os.environ.get("DMNERF_TRAIN_IMPL", "umma").lower
 
 
 def _train_impl(impl):
+    if impl == _lib.IMPL_UMMA_F16:
+        raise RuntimeError("IMPL_UMMA_F16 is inference-only: training and its gradients run the exact network (IMPL_UMMA or "
+                           "IMPL_SIMT); call under torch.no_grad() for an fp16 preview")
     return TRAIN_IMPL if impl == _lib.IMPL_AUTO else impl
 
 

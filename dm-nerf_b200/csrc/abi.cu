@@ -137,14 +137,36 @@ DMNERF_API int dmnerf_posenc(const float* x, int64_t m, int n_freqs, float* out,
   return launch_posenc(x, m, n_freqs, out, (cudaStream_t)stream);
 }
 
+// The fp16 network of slot `net`: its image is packed on the first fp16 call after every dmnerf_set_weights.
+static int prepare_f16(dmnerf_ctx* ctx, int net, cudaStream_t st) {
+  DMN_CHECK(umma_available(ctx->packed[net]), "DMNERF_IMPL_UMMA_F16: bind the network with dmnerf_set_weights first");
+  return umma_weights_pack_f16(ctx->packed[net], ctx->net[net], st);
+}
+
+// An fp16 call on caller buffers returns only after its range verdict: synchronise and report (never silent inf / NaN maps).
+// A call that failed before its verdict still drains its kernels and drops their verdict: their results are not returned.
+static int f16_verdict(dmnerf_ctx* ctx, int rc, int impl, void* stream) {
+  if (impl != DMNERF_IMPL_UMMA_F16) return rc;
+  if (rc) {
+    cudaStreamSynchronize((cudaStream_t)stream);
+    for (int i = 0; i < 2; ++i) umma_take_f16_range(ctx->packed[i]);
+    return rc;
+  }
+  return dmnerf_sync_check(ctx, stream);
+}
+
 static int mlp_dispatch(dmnerf_ctx* ctx, int net, const float* x, const float* ro, const float* rd, const float* z,
                         int64_t m, int s, float* out, int impl, cudaStream_t st) {
   DMN_CHECK(ctx != nullptr, "mlp: ctx is NULL");
   DMN_CHECK(net == 0 || net == 1, "mlp: net must be 0 or 1");
   DMN_CHECK(m >= 0, "mlp: negative row count");
-  DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA, "mlp: unknown impl %d", impl);
+  DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA_F16, "mlp: unknown impl %d", impl);
   if (m == 0) return 0;
   DMN_CHECK(out != nullptr, "mlp: out is NULL");
+  if (impl == DMNERF_IMPL_UMMA_F16) {
+    if (prepare_f16(ctx, net, st)) return 1;
+    return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st, true);
+  }
   if (impl == DMNERF_IMPL_AUTO) impl = umma_available(ctx->packed[net]) ? DMNERF_IMPL_UMMA : DMNERF_IMPL_SIMT;
   if (impl == DMNERF_IMPL_UMMA)
     return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st);
@@ -153,14 +175,15 @@ static int mlp_dispatch(dmnerf_ctx* ctx, int net, const float* x, const float* r
 
 DMNERF_API int dmnerf_mlp_forward(dmnerf_ctx* ctx, int net, const float* x, int64_t m, float* out, int impl, void* stream) {
   DMN_CHECK(m <= 0 || x != nullptr, "mlp_forward: x is NULL");
-  return mlp_dispatch(ctx, net, x, nullptr, nullptr, nullptr, m, 1, out, impl, (cudaStream_t)stream);
+  return f16_verdict(ctx, mlp_dispatch(ctx, net, x, nullptr, nullptr, nullptr, m, 1, out, impl, (cudaStream_t)stream), impl, stream);
 }
 
 DMNERF_API int dmnerf_mlp_forward_rays(dmnerf_ctx* ctx, int net, const float* rays_o, const float* rays_d, const float* z,
                             int64_t n, int s, float* out, int impl, void* stream) {
   DMN_CHECK(n >= 0 && s >= 1, "mlp_forward_rays: bad sizes n=%lld s=%d", (long long)n, s);
   DMN_CHECK(n == 0 || (rays_o && rays_d && z), "mlp_forward_rays: NULL input");
-  return mlp_dispatch(ctx, net, nullptr, rays_o, rays_d, z, n * s, s, out, impl, (cudaStream_t)stream);
+  return f16_verdict(ctx, mlp_dispatch(ctx, net, nullptr, rays_o, rays_d, z, n * s, s, out, impl, (cudaStream_t)stream), impl,
+                     stream);
 }
 
 DMNERF_API int dmnerf_mlp_forward_points(dmnerf_ctx* ctx, int net, const float* pts, const float* viewdirs, int64_t m, float* out,
@@ -169,9 +192,13 @@ DMNERF_API int dmnerf_mlp_forward_points(dmnerf_ctx* ctx, int net, const float* 
   DMN_CHECK(m >= 0, "mlp_forward_points: negative point count");
   DMN_CHECK(m == 0 || (pts && viewdirs && out), "mlp_forward_points: NULL buffer");
   DMN_CHECK(impl != DMNERF_IMPL_SIMT, "mlp_forward_points: the point query runs on the tensor-core kernel only");
+  DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA_F16, "mlp_forward_points: unknown impl %d", impl);
   if (m == 0) return 0;
   DMN_CHECK(umma_available(ctx->packed[net]), "mlp_forward_points: bind the network with dmnerf_set_weights first");
-  return launch_mlp_umma(ctx->packed[net], ctx->net[net], nullptr, pts, viewdirs, nullptr, m, 1, out, nullptr, (cudaStream_t)stream);
+  const bool f16 = impl == DMNERF_IMPL_UMMA_F16;
+  if (f16 && prepare_f16(ctx, net, (cudaStream_t)stream)) return 1;
+  return f16_verdict(ctx, launch_mlp_umma(ctx->packed[net], ctx->net[net], nullptr, pts, viewdirs, nullptr, m, 1, out, nullptr,
+                                          (cudaStream_t)stream, f16), impl, stream);
 }
 
 DMNERF_API int dmnerf_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all_ins,
@@ -327,6 +354,8 @@ DMNERF_API int dmnerf_mlp_forward_train(dmnerf_ctx* ctx, int net, const float* x
   DMN_CHECK(m >= 0 && s >= 1, "mlp_forward_train: bad sizes");
   if (m == 0) return 0;
   DMN_CHECK(out && acts, "mlp_forward_train: out / acts is NULL");
+  DMN_CHECK(impl != DMNERF_IMPL_UMMA_F16, "mlp_forward_train: DMNERF_IMPL_UMMA_F16 is inference-only; training runs the exact "
+            "network (DMNERF_IMPL_UMMA or DMNERF_IMPL_SIMT)");
   DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA, "mlp_forward_train: unknown impl %d", impl);
   if (impl == DMNERF_IMPL_AUTO) impl = umma_available(ctx->packed[net]) ? DMNERF_IMPL_UMMA : DMNERF_IMPL_SIMT;
   if (impl == DMNERF_IMPL_UMMA)
@@ -412,8 +441,10 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
                         umma_available(ctx->packed[0]) && umma_available(ctx->packed[1]);
   if (can_fuse) {
     const bool prof = ctx->profiling;
+    const bool f16 = impl == DMNERF_IMPL_UMMA_F16;
+    if (f16 && (prepare_f16(ctx, 0, st) || prepare_f16(ctx, 1, st))) return 1;
     if (prof) DMN_CUDA(cudaEventRecord(ctx->ev[0], st));
-    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep);
+    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep, f16);
     if (rc) return rc;
     if (prof) for (int i = 1; i <= DMNERF_N_STAGES; ++i) DMN_CUDA(cudaEventRecord(ctx->ev[i], st));
     ctx->profile_valid = prof;
@@ -476,24 +507,29 @@ extern "C" {
 
 DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
                           void* stream) {
-  return render_forward_impl(ctx, io, n, S, NI, flags, impl, nullptr, stream);
+  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, nullptr, stream), impl, stream);
 }
 
 DMNERF_API int dmnerf_render_forward_objects(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
                                              const uint32_t* keep_host, void* stream) {
   ObjMask m;
   if (render_object_mask(ctx, keep_host, m, "render_forward_objects")) return 1;
-  return render_forward_impl(ctx, io, n, S, NI, flags, impl, &m, stream);
+  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, &m, stream), impl, stream);
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
   DMN_CHECK(ctx != nullptr, "sync_check: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
   DMN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  // fp16 range verdicts: taken from both weight sets (the stage path's coarse and fine networks each have an error word), so
+  // that none is left behind for a later call, then reported after any protocol error
+  const bool range0 = umma_take_f16_range(ctx->packed[0]), range1 = umma_take_f16_range(ctx->packed[1]);
   for (int i = 0; i < 2; ++i) {
     int rc = umma_check_status(ctx->packed[i], (cudaStream_t)stream);
     if (rc) return rc;
   }
+  DMN_CHECK(!range0 && !range1, "fp16 network: an activation exceeded the fp16 range (> 65504), so these results are invalid; "
+            "render with the exact network (DMNERF_IMPL_UMMA)");
   return gemm_tc_check_status((cudaStream_t)stream);
 }
 

@@ -19,6 +19,11 @@
 //     epilogues of layer 7 / the colour hidden layer; the instance head is one more MMA.  19 half-steps per tile.
 // All waits are bounded: a protocol bug raises an error code, never a hang.
 //
+// fp16 preview network (F16 = true: mlp_f16_kernel, render_objects_f16_kernel; inference only, DESIGN.md section 10): the same
+// body with one pass A * W per K step, fp16 operands and fp32 accumulation, streaming a second weight image that holds one fp16
+// stage per chunk (no W_lo stages).  Epilogues and embeddings store fp16 into the hi slabs; the lo slabs stay unused.  A value
+// stored above the fp16 range raises STATUS_F16_RANGE in the error word, which the host reports as an error.
+//
 #include <cstring>
 #include <type_traits>
 #include <vector>
@@ -143,8 +148,9 @@ __device__ __forceinline__ void fill_embedding(const float v[3], float* vals /* 
 // ------------------------------------------------------------------------------------------------ the kernel
 // Warps 0-7: two consumer warpgroups (MMA issue, epilogues, prologue); warp 8: weight producer.
 // SELECT (fused only): object selection -- samples whose label is not in a.keep get alpha = 0 in both composites.  The body is
-// shared by mlp_umma_kernel (no selection) and render_objects_kernel (FUSED + SELECT) below.
-template <bool FUSED, bool SELECT>
+// shared by mlp_umma_kernel (no selection) and render_objects_kernel (FUSED + SELECT) below.  F16: the fp16 preview network
+// (prog and the images are then the fp16 program and images).
+template <bool FUSED, bool SELECT, bool F16>
 __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& a) {
   // The kernel has no static shared memory, so the dynamic block starts at offset 0 of the CTA's shared window and
   // is 1024-aligned by construction (checked below).
@@ -203,6 +209,7 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
   Ring ring{0, 0};
   int prev_slot = -1;
   float acc0[64], acc1[64];
+  float f16_max = 0.0f;                         // F16: largest magnitude this thread stored as an fp16 operand
 
   // One weight stage: wait for it, issue its MMAs (A_hi * W and, for a W_hi stage, A_lo * W), hand the previous stage back
   // once its MMAs have completed (the ring holds the stage in flight, the stage issued before it and the one being filled).
@@ -214,8 +221,12 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       if (k < ks) {
-        wgmma_n128<0, 0>(acc, make_sdesc_sw128(a_hi + 32 * k), make_sdesc_sw128(w + 32 * k), k == 0 ? scale0 : 1u);
-        if (with_lo) wgmma_n128<0, 0>(acc, make_sdesc_sw128(a_lo + 32 * k), make_sdesc_sw128(w + 32 * k), 1u);
+        if constexpr (F16) {
+          wgmma_n128_f16<0, 0>(acc, make_sdesc_sw128(a_hi + 32 * k), make_sdesc_sw128(w + 32 * k), k == 0 ? scale0 : 1u);
+        } else {
+          wgmma_n128<0, 0>(acc, make_sdesc_sw128(a_hi + 32 * k), make_sdesc_sw128(w + 32 * k), k == 0 ? scale0 : 1u);
+          if (with_lo) wgmma_n128<0, 0>(acc, make_sdesc_sw128(a_lo + 32 * k), make_sdesc_sw128(w + 32 * k), 1u);
+        }
       }
     }
     wg_commit();
@@ -231,10 +242,14 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
     if (prev_slot >= 0 && lane == 0) mbar_arrive(&misc->empty[prev_slot]);
     prev_slot = -1;
   };
-  // One 64-wide K chunk (W_hi stage, then W_lo stage) of a half-step
+  // One 64-wide K chunk (W_hi stage, then W_lo stage; F16: the one fp16 stage) of a half-step
   auto chunk = [&](float (&acc)[64], uint32_t a_hi, uint32_t a_lo, int ks, bool first) {
-    stage(acc, a_hi, a_lo, true, ks, first ? 0u : 1u);
-    stage(acc, a_hi, a_lo, false, ks, 1u);
+    if constexpr (F16) {
+      stage(acc, a_hi, a_lo, false, ks, first ? 0u : 1u);
+    } else {
+      stage(acc, a_hi, a_lo, true, ks, first ? 0u : 1u);
+      stage(acc, a_hi, a_lo, false, ks, 1u);
+    }
   };
   auto act_chunk = [&](float (&acc)[64], int c, bool first) {
     const uint32_t hi = act_base + c * ACT_CHUNK;
@@ -346,7 +361,10 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
       }
       save_emb(32 * ph, vals, 32);
 #pragma unroll
-      for (int u = 0; u < 4; ++u) store_split8_smem(vals + 8 * u, e_hi, e_lo, pr, 32 * ph + 8 * u);
+      for (int u = 0; u < 4; ++u) {
+        if constexpr (F16) f16_max = fmaxf(f16_max, store_f16x8_smem(vals + 8 * u, e_hi, pr, 32 * ph + 8 * u));
+        else store_split8_smem(vals + 8 * u, e_hi, e_lo, pr, 32 * ph + 8 * u);
+      }
     }
     fence_proxy_async_smem();            // the embeddings are read by the tensor core through the async proxy
     wg_sync();
@@ -373,12 +391,18 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
           acc[4 * jj + 2 * h] = fmaxf(acc[4 * jj + 2 * h] + bb.x, 0.0f);
           acc[4 * jj + 2 * h + 1] = fmaxf(acc[4 * jj + 2 * h + 1] + bb.y, 0.0f);
           if (half >= 0) {
-            uint32_t hi, lo;
-            split_bf16x2(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1], hi, lo);
             const int c256 = 128 * half + col;
             const uint32_t o = SM_ACT + (c256 >> 6) * ACT_CHUNK + sw128_offset(ra + 8 * h, c256 & 63);
-            *reinterpret_cast<uint32_t*>(smem + o) = hi;
-            *reinterpret_cast<uint32_t*>(smem + o + CHUNK_BYTES) = lo;
+            if constexpr (F16) {
+              const float v0 = acc[4 * jj + 2 * h], v1 = acc[4 * jj + 2 * h + 1];      // >= 0 after the ReLU
+              *reinterpret_cast<uint32_t*>(smem + o) = pack_f16x2(v0, v1);
+              f16_max = fmaxf(f16_max, fmaxf(v0, v1));
+            } else {
+              uint32_t hi, lo;
+              split_bf16x2(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1], hi, lo);
+              *reinterpret_cast<uint32_t*>(smem + o) = hi;
+              *reinterpret_cast<uint32_t*>(smem + o + CHUNK_BYTES) = lo;
+            }
           }
         }
       }
@@ -452,8 +476,13 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
           }
         }
         save_emb(CH_POS + 16 * ph, vals, 16);
-        store_split8_smem(vals, e_hi, e_lo, pr, 16 * ph);
-        store_split8_smem(vals + 8, e_hi, e_lo, pr, 16 * ph + 8);
+        if constexpr (F16) {
+          f16_max = fmaxf(f16_max, store_f16x8_smem(vals, e_hi, pr, 16 * ph));
+          f16_max = fmaxf(f16_max, store_f16x8_smem(vals + 8, e_hi, pr, 16 * ph + 8));
+        } else {
+          store_split8_smem(vals, e_hi, e_lo, pr, 16 * ph);
+          store_split8_smem(vals + 8, e_hi, e_lo, pr, 16 * ph + 8);
+        }
       }
       fence_proxy_async_smem();
       wg_sync();
@@ -639,21 +668,37 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
       all_sync();                        // the logits region is free again; fine depths visible to the next prologue
     }
   }
+  if constexpr (F16) {
+    // sticky: the first code stays until the host reads and clears it (umma_take_f16_range)
+    if (f16_max > F16_MAX) atomicCAS(a.status, 0, STATUS_F16_RANGE);
+  }
 }
 
 template <bool FUSED>
 __global__ void __launch_bounds__(N_THREADS, 1) mlp_umma_kernel(const __grid_constant__ Program prog, const __grid_constant__ KArgs a) {
-  mlp_umma_body<FUSED, false>(prog, a);
+  mlp_umma_body<FUSED, false, false>(prog, a);
 }
 
 // The fused render kernel with an object selection (a.keep): a kernel of its own, so that the unselected one carries no branch.
 __global__ void __launch_bounds__(N_THREADS, 1) render_objects_kernel(const __grid_constant__ Program prog,
                                                                       const __grid_constant__ KArgs a) {
-  mlp_umma_body<true, true>(prog, a);
+  mlp_umma_body<true, true, false>(prog, a);
+}
+
+// The fp16 preview twins of the two kernels above (inference only).
+template <bool FUSED>
+__global__ void __launch_bounds__(N_THREADS, 1) mlp_f16_kernel(const __grid_constant__ Program prog, const __grid_constant__ KArgs a) {
+  mlp_umma_body<FUSED, false, true>(prog, a);
+}
+
+__global__ void __launch_bounds__(N_THREADS, 1) render_objects_f16_kernel(const __grid_constant__ Program prog,
+                                                                          const __grid_constant__ KArgs a) {
+  mlp_umma_body<true, true, true>(prog, a);
 }
 
 // ------------------------------------------------------------------------------------------------ host: program
-static void build_program(Program& P, int ins_num) {
+// f16: the fp16 program -- the same steps with one weight stage per chunk instead of a W_hi and a W_lo stage.
+static void build_program(Program& P, int ins_num, bool f16 = false) {
   memset(&P, 0, sizeof(P));
   P.ins_num = ins_num;
   // Slot 0 always holds K-half 0 of the current activation, slot 1 K-half 1 (see the MMA role of the kernel).
@@ -685,7 +730,7 @@ static void build_program(Program& P, int ins_num) {
   uint32_t off = 0;
   int si = 0;
   for (int i = 0; i < N_STEPS; ++i)
-    for (int c = 0; c < 2 * P.step[i].n_chunks; ++c) { P.stage_off[si++] = off; off += (uint32_t)P.step[i].n * 128u; }
+    for (int c = 0; c < (f16 ? 1 : 2) * P.step[i].n_chunks; ++c) { P.stage_off[si++] = off; off += (uint32_t)P.step[i].n * 128u; }
   P.stage_off[si] = off;               // sentinel: total image size
   P.n_stages = si;
 }
@@ -745,6 +790,34 @@ __global__ void pack_kernel(const PackStage* __restrict__ stages, int n_entries,
   }
 }
 
+// The fp16 image: one stage per entry at off_hi (off_lo unused).  A weight above the fp16 range sets *out_of_range = 1.
+__global__ void pack_f16_kernel(const PackStage* __restrict__ stages, int n_entries, uint8_t* __restrict__ image,
+                                int32_t* __restrict__ out_of_range) {
+  const int e = blockIdx.x;
+  if (e >= n_entries) return;
+  const PackStage ps = stages[e];
+  bool over = false;
+  for (int idx = threadIdx.x; idx < ps.n_rows * 8; idx += blockDim.x) {
+    const int n = idx >> 3, u = idx & 7;
+    uint32_t h16[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float v[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int k = 8 * u + 2 * j + h;
+        v[h] = !(n < ps.n_valid && k < ps.k_valid) ? 0.0f
+               : (ps.transposed ? ps.src[(size_t)(ps.col_base + k) * ps.ld + ps.n_base + n]
+                                : ps.src[(size_t)(ps.n_base + n) * ps.ld + ps.col_base + k]);
+        over |= !(fabsf(v[h]) <= umma::F16_MAX);      // NaN counts as out of range
+      }
+      h16[j] = umma::pack_f16x2(v[0], v[1]);
+    }
+    *reinterpret_cast<uint4*>(image + ps.off_hi + umma::sw128_offset(n, 8 * u)) = make_uint4(h16[0], h16[1], h16[2], h16[3]);
+  }
+  if (over) *out_of_range = 1;
+}
+
 __global__ void bias_kernel(NetParams p, const float* __restrict__ fold_b_rgb, const float* __restrict__ fold_b_ins,
                             float* __restrict__ bias) {
   // [N_STEPS][128] step biases, then the CUDA-core layers: density weights / bias, rgb_linear weights / bias (B_* offsets)
@@ -769,7 +842,9 @@ __global__ void bias_kernel(NetParams p, const float* __restrict__ fold_b_rgb, c
 // ================================================================================================ API
 struct UmmaExtra {            // hangs off UmmaWeights::image allocation bookkeeping
   uk::Program prog;
+  uk::Program prog16;         // the fp16 program: one stage per chunk (UmmaWeights::image16)
   float* fold_w_rgb; float* fold_w_ins; float* fold_b; uk::PackStage* d_entries;
+  int32_t* d_pack_flag;       // fp16 pack: set when a weight exceeds the fp16 range
   int32_t* d_status;          // device alias of h_status
   volatile int32_t* h_status;  // error word in mapped host memory: a kernel that gave up on a barrier writes its code here, and the
                               // NEXT launch through this weight set refuses to start (a stalled launch can never pass silently)
@@ -779,6 +854,7 @@ static UmmaExtra* extra_of(const UmmaWeights& w) { return reinterpret_cast<UmmaE
 
 void umma_weights_free(UmmaWeights& w) {
   if (w.image) cudaFree(w.image);
+  if (w.image16) cudaFree(w.image16);
   if (w.bias) cudaFree(w.bias);
   if (w.extra) {
     UmmaExtra* x = extra_of(w);
@@ -786,6 +862,7 @@ void umma_weights_free(UmmaWeights& w) {
     if (x->fold_w_ins) cudaFree(x->fold_w_ins);
     if (x->fold_b) cudaFree(x->fold_b);
     if (x->d_entries) cudaFree(x->d_entries);
+    if (x->d_pack_flag) cudaFree(x->d_pack_flag);
     if (x->h_status) cudaFreeHost((void*)x->h_status);
     delete x;
   }
@@ -797,41 +874,36 @@ const float* umma_fold_w_rgb(const UmmaWeights& w) { return w.extra ? extra_of(w
 int32_t* umma_status_word(const UmmaWeights& w) { return w.extra ? extra_of(w)->d_status : nullptr; }
 int umma_status_peek(const UmmaWeights& w) { return (w.extra && extra_of(w)->h_status) ? (int)*extra_of(w)->h_status : 0; }
 
-int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
+bool umma_take_f16_range(const UmmaWeights& w) {
+  if (umma_status_peek(w) != uk::STATUS_F16_RANGE) return false;
+  *extra_of(w)->h_status = 0;
+  return true;
+}
+
+// The error word as a new launch sees it: a protocol code, or 0.  STATUS_F16_RANGE is an fp16 verdict not reported yet.  An
+// fp16 launch meets it inside the call that raised it (the other parts of a *_host batch, the fine pass of the stage path) and
+// leaves it for that call's verdict (dmnerf_sync_check).  An exact launch can only meet one left by an fp16 call that failed for
+// another reason before its verdict; those results were never returned, so it is dropped.
+static int launch_gate(const UmmaWeights& w, bool f16) {
+  const int code = umma_status_peek(w);
+  if (code != uk::STATUS_F16_RANGE) return code;
+  if (!f16) umma_take_f16_range(w);
+  return 0;
+}
+
+// One PackStage per (step, chunk) of `prog`: the W_hi and W_lo stage of the exact image, or the one stage of the fp16 image.
+// Reads the folded head layers from the fold buffers, which umma_weights_pack fills.
+static std::vector<uk::PackStage> pack_entries(const uk::Program& prog, const NetParams& p, const UmmaExtra* x, bool f16) {
   using namespace uk;
-  if (w.extra && w.ins_num != p.ins_num) umma_weights_free(w);
-  if (!w.extra) {
-    UmmaExtra* x = new UmmaExtra();
-    memset(x, 0, sizeof(*x));
-    build_program(x->prog, p.ins_num);
-    w.extra = x;
-    w.ins_num = p.ins_num;
-    w.image_bytes = x->prog.stage_off[x->prog.n_stages];
-    DMN_CUDA(cudaMalloc(&w.image, w.image_bytes));
-    DMN_CUDA(cudaMalloc((void**)&w.bias, B_TOTAL * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->fold_w_rgb, 128 * 283 * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->fold_w_ins, 128 * 256 * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->fold_b, 256 * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->d_entries, MAX_STAGES * sizeof(PackStage)));
-    DMN_CUDA(cudaHostAlloc((void**)&x->h_status, sizeof(int32_t), cudaHostAllocMapped));
-    *x->h_status = 0;
-    DMN_CUDA(cudaHostGetDevicePointer((void**)&x->d_status, (void*)x->h_status, 0));
-  }
-  UmmaExtra* x = extra_of(w);
-  // fold the activation-free feature layers into the following hidden layers (fp64 accumulate)
-  fold_kernel<<<dim3(128, 5), 256, 0, st>>>(p.w[L_RGB_HID], 283, p.w[L_RGB_FEAT], p.b[L_RGB_FEAT], p.b[L_RGB_HID], 27, x->fold_w_rgb, x->fold_b);
-  DMN_LAUNCH_OK();
-  fold_kernel<<<dim3(128, 5), 256, 0, st>>>(p.w[L_INS_HID], 256, p.w[L_INS_FEAT], p.b[L_INS_FEAT], p.b[L_INS_HID], 0, x->fold_w_ins, x->fold_b + 128);
-  DMN_LAUNCH_OK();
-  // one PackStage per (step, chunk)
   std::vector<PackStage> ent;
+  const int per_chunk = f16 ? 1 : 2;
   int si = 0;
   for (int t = 0; t < N_STEPS; ++t) {
-    const Step& s = x->prog.step[t];
-    for (int c = 0; c < s.n_chunks; ++c, si += 2) {
+    const Step& s = prog.step[t];
+    for (int c = 0; c < s.n_chunks; ++c, si += per_chunk) {
       PackStage e;
       memset(&e, 0, sizeof(e));
-      e.n_rows = s.n; e.off_hi = x->prog.stage_off[si]; e.off_lo = x->prog.stage_off[si + 1];
+      e.n_rows = s.n; e.off_hi = prog.stage_off[si]; e.off_lo = f16 ? 0u : prog.stage_off[si + 1];
       const int kind = s.chunk[c];
       if (t < 16) {                                   // trunk layer l, output half h
         const int l = t / 2, h = t % 2;
@@ -849,6 +921,38 @@ int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
       ent.push_back(e);
     }
   }
+  return ent;
+}
+
+int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
+  using namespace uk;
+  if (w.extra && w.ins_num != p.ins_num) umma_weights_free(w);
+  if (!w.extra) {
+    UmmaExtra* x = new UmmaExtra();
+    memset(x, 0, sizeof(*x));
+    build_program(x->prog, p.ins_num);
+    build_program(x->prog16, p.ins_num, true);
+    w.extra = x;
+    w.ins_num = p.ins_num;
+    w.image_bytes = x->prog.stage_off[x->prog.n_stages];
+    DMN_CUDA(cudaMalloc(&w.image, w.image_bytes));
+    DMN_CUDA(cudaMalloc((void**)&w.bias, B_TOTAL * sizeof(float)));
+    DMN_CUDA(cudaMalloc((void**)&x->fold_w_rgb, 128 * 283 * sizeof(float)));
+    DMN_CUDA(cudaMalloc((void**)&x->fold_w_ins, 128 * 256 * sizeof(float)));
+    DMN_CUDA(cudaMalloc((void**)&x->fold_b, 256 * sizeof(float)));
+    DMN_CUDA(cudaMalloc((void**)&x->d_entries, MAX_STAGES * sizeof(PackStage)));
+    DMN_CUDA(cudaHostAlloc((void**)&x->h_status, sizeof(int32_t), cudaHostAllocMapped));
+    *x->h_status = 0;
+    DMN_CUDA(cudaHostGetDevicePointer((void**)&x->d_status, (void*)x->h_status, 0));
+  }
+  UmmaExtra* x = extra_of(w);
+  w.f16_ready = false;                                // the fp16 image is re-packed from these weights on its next use
+  // fold the activation-free feature layers into the following hidden layers (fp64 accumulate)
+  fold_kernel<<<dim3(128, 5), 256, 0, st>>>(p.w[L_RGB_HID], 283, p.w[L_RGB_FEAT], p.b[L_RGB_FEAT], p.b[L_RGB_HID], 27, x->fold_w_rgb, x->fold_b);
+  DMN_LAUNCH_OK();
+  fold_kernel<<<dim3(128, 5), 256, 0, st>>>(p.w[L_INS_HID], 256, p.w[L_INS_FEAT], p.b[L_INS_FEAT], p.b[L_INS_HID], 0, x->fold_w_ins, x->fold_b + 128);
+  DMN_LAUNCH_OK();
+  const std::vector<PackStage> ent = pack_entries(x->prog, p, x, false);
   DMN_CHECK((int)ent.size() * 2 == x->prog.n_stages && (int)ent.size() <= MAX_STAGES, "umma pack: stage table mismatch");
   const size_t n_fwd = ent.size();
   DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), ent.size() * sizeof(PackStage), cudaMemcpyHostToDevice, st));
@@ -861,19 +965,45 @@ int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
   return 0;
 }
 
+int umma_weights_pack_f16(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
+  using namespace uk;
+  DMN_CHECK(w.ready && w.extra, "fp16 network: weights not packed (call dmnerf_set_weights first)");
+  if (w.f16_ready) return 0;
+  UmmaExtra* x = extra_of(w);
+  if (!w.image16) DMN_CUDA(cudaMalloc(&w.image16, x->prog16.stage_off[x->prog16.n_stages]));
+  if (!x->d_pack_flag) DMN_CUDA(cudaMalloc((void**)&x->d_pack_flag, sizeof(int32_t)));
+  // the folded head layers are the fp32 fold of the exact pack (fp64 accumulate), rounded to fp16 here
+  const std::vector<PackStage> ent = pack_entries(x->prog16, p, x, true);
+  DMN_CHECK((int)ent.size() == x->prog16.n_stages && (int)ent.size() <= MAX_STAGES, "fp16 pack: stage table mismatch");
+  DMN_CUDA(cudaMemsetAsync(x->d_pack_flag, 0, sizeof(int32_t), st));
+  DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), ent.size() * sizeof(PackStage), cudaMemcpyHostToDevice, st));
+  pack_f16_kernel<<<(unsigned)ent.size(), 256, 0, st>>>(x->d_entries, (int)ent.size(), (uint8_t*)w.image16, x->d_pack_flag);
+  DMN_LAUNCH_OK();
+  int32_t out_of_range = 0;
+  DMN_CUDA(cudaMemcpyAsync(&out_of_range, x->d_pack_flag, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  DMN_CUDA(cudaStreamSynchronize(st));               // `ent` is a host temporary; the range verdict is read below
+  DMN_CHECK(!out_of_range, "fp16 network: a weight exceeds the fp16 range (|w| > 65504); use the exact network (DMNERF_IMPL_UMMA)");
+  w.f16_ready = true;
+  return 0;
+}
+
 int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, const float* rays_o, const float* rays_d,
-                    const float* z, int64_t m, int s, float* out, float* acts, cudaStream_t st) {
+                    const float* z, int64_t m, int s, float* out, float* acts, cudaStream_t st, bool f16) {
   using namespace uk;
   DMN_CHECK(w.ready && w.extra, "mlp(umma): weights not packed (call dmnerf_set_weights first)");
   DMN_CHECK((x != nullptr) != (rays_o != nullptr && rays_d != nullptr), "mlp(umma): pass either x or rays");
   DMN_CHECK(x != nullptr || z != nullptr || s == 1, "mlp(umma): points mode (z == NULL) takes one sample per row");
-  DMN_CHECK(umma_status_peek(w) == 0, "mlp(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); its results "
+  DMN_CHECK(launch_gate(w, f16) == 0, "mlp(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); its results "
             "are invalid -- destroy the context", umma_status_peek(w));
+  DMN_CHECK(!f16 || (w.f16_ready && acts == nullptr), "mlp(umma): the fp16 network is inference-only and needs its packed image");
   if (m == 0) return 0;
   UmmaExtra* ex = extra_of(w);
-  static PerDeviceOnce attr_once;
-  if (attr_once.first()) {
+  static PerDeviceOnce attr_once, attr_once_f16;
+  if (!f16 && attr_once.first()) {
     DMN_CUDA(cudaFuncSetAttribute(mlp_umma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  }
+  if (f16 && attr_once_f16.first()) {
+    DMN_CUDA(cudaFuncSetAttribute(mlp_f16_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   }
   int dev = 0, sms = 0;
   DMN_CUDA(cudaGetDevice(&dev));
@@ -881,10 +1011,11 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
   const int64_t tiles = (m + TILE_M - 1) / TILE_M;
   KArgs a;
   memset(&a, 0, sizeof(a));
-  a.image = (const uint8_t*)w.image; a.bias = w.bias; a.x = x; a.rays_o = rays_o; a.rays_d = rays_d; a.z = z;
+  a.image = (const uint8_t*)(f16 ? w.image16 : w.image); a.bias = w.bias; a.x = x; a.rays_o = rays_o; a.rays_d = rays_d; a.z = z;
   a.m = m; a.s = s; a.out = out; a.acts = acts; a.status = ex->d_status;
   const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
-  mlp_umma_kernel<false><<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog, a);
+  if (f16) mlp_f16_kernel<false><<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog16, a);
+  else mlp_umma_kernel<false><<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog, a);
   DMN_LAUNCH_OK();
   return 0;
 }
@@ -892,28 +1023,35 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
 // Whole dm_nerf() pipeline (render.py:31-96) in ONE launch: coarse network -> composite -> importance sampling -> fine
 // network -> composite, per pair of rays, nothing but rays in and per-ray maps out crossing HBM.  64 + 128 samples only.
 int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmnerf_render_io* io, int64_t n, int flags,
-                       cudaStream_t st, const ObjMask* keep) {
+                       cudaStream_t st, const ObjMask* keep, bool f16) {
   using namespace uk;
   DMN_CHECK(wc.ready && wf.ready && wc.extra && wf.extra, "render(umma): weights not packed");
   DMN_CHECK(wc.ins_num == wf.ins_num, "render(umma): coarse/fine ins_num differ");
-  DMN_CHECK(umma_status_peek(wc) == 0, "render(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); its "
+  DMN_CHECK(launch_gate(wc, f16) == 0, "render(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); its "
             "results are invalid -- destroy the context", umma_status_peek(wc));
+  DMN_CHECK(!f16 || (wc.f16_ready && wf.f16_ready), "render(umma): the fp16 images are not packed");
   if (n == 0) return 0;
   UmmaExtra* ex = extra_of(wc);
-  static PerDeviceOnce attr_once, attr_once_sel;
-  if (!keep && attr_once.first()) {
+  static PerDeviceOnce attr_once, attr_once_sel, attr_once_f16, attr_once_sel_f16;
+  if (!f16 && !keep && attr_once.first()) {
     DMN_CUDA(cudaFuncSetAttribute(mlp_umma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   }
-  if (keep && attr_once_sel.first()) {
+  if (!f16 && keep && attr_once_sel.first()) {
     DMN_CUDA(cudaFuncSetAttribute(render_objects_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  }
+  if (f16 && !keep && attr_once_f16.first()) {
+    DMN_CUDA(cudaFuncSetAttribute(mlp_f16_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  }
+  if (f16 && keep && attr_once_sel_f16.first()) {
+    DMN_CUDA(cudaFuncSetAttribute(render_objects_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   }
   int dev = 0, sms = 0;
   DMN_CUDA(cudaGetDevice(&dev));
   DMN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   KArgs a;
   memset(&a, 0, sizeof(a));
-  a.image = (const uint8_t*)wc.image; a.bias = wc.bias;
-  a.image_fine = (const uint8_t*)wf.image; a.bias_fine = wf.bias;
+  a.image = (const uint8_t*)(f16 ? wc.image16 : wc.image); a.bias = wc.bias;
+  a.image_fine = (const uint8_t*)(f16 ? wf.image16 : wf.image); a.bias_fine = wf.bias;
   a.rays_o = io->rays_o; a.rays_d = io->rays_d;
   a.z_in = io->z_coarse; a.z_stride = io->z_row_stride;
   const bool perturb = (flags & DMNERF_FLAG_PERTURB) != 0;
@@ -925,11 +1063,14 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   a.status = ex->d_status;
   const int64_t units = (n + 1) / 2;
   const unsigned grid = (unsigned)(units < sms ? units : sms);
+  const Program& prog = f16 ? ex->prog16 : ex->prog;      // coarse and fine share ins_num, hence the program
   if (keep) {
     a.keep = *keep;
-    render_objects_kernel<<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog, a);
+    if (f16) render_objects_f16_kernel<<<grid, N_THREADS, SMEM_BYTES, st>>>(prog, a);
+    else render_objects_kernel<<<grid, N_THREADS, SMEM_BYTES, st>>>(prog, a);
   } else {
-    mlp_umma_kernel<true><<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog, a);
+    if (f16) mlp_f16_kernel<true><<<grid, N_THREADS, SMEM_BYTES, st>>>(prog, a);
+    else mlp_umma_kernel<true><<<grid, N_THREADS, SMEM_BYTES, st>>>(prog, a);
   }
   DMN_LAUNCH_OK();
   return 0;

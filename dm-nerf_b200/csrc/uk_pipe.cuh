@@ -26,6 +26,9 @@ constexpr int MAX_CHUNKS = 5;
 constexpr int MAX_STAGES = 160;
 constexpr int CONSUMERS = 256;             // two warpgroups: MMA issue, epilogues, prologue
 constexpr int N_THREADS = CONSUMERS + 32;  // + one weight-producer warp
+// Status code of the fp16 network in the error word (KArgs::status; the protocol errors are below 1000): an activation or an
+// input exceeded the fp16 range
+constexpr int STATUS_F16_RANGE = 1001;
 
 // shared-memory map (offsets from the 1024-aligned base)
 //   activation: 4 K chunks of the current 256-wide activation, each as a bf16 hi and a bf16 lo slab [128 rows][64]
@@ -95,6 +98,19 @@ __device__ __forceinline__ void store_split8_smem(const float* vals, uint8_t* sl
   const uint32_t o = sw128_offset(row, k0);
   *reinterpret_cast<uint4*>(slab_hi + o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
   *reinterpret_cast<uint4*>(slab_lo + o) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+}
+
+// fp16 network: 8 fp32 values -> fp16 into one K-major SW128 slab; returns the largest magnitude stored (range check).
+__device__ __forceinline__ float store_f16x8_smem(const float* vals, uint8_t* slab, int row, int k0) {
+  uint32_t h[4];
+  float amax = 0.0f;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    h[j] = pack_f16x2(vals[2 * j], vals[2 * j + 1]);
+    amax = fmaxf(amax, fmaxf(fabsf(vals[2 * j]), fabsf(vals[2 * j + 1])));
+  }
+  *reinterpret_cast<uint4*>(slab + sw128_offset(row, k0)) = make_uint4(h[0], h[1], h[2], h[3]);
+  return amax;
 }
 
 }  // namespace uk

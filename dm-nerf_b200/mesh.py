@@ -136,28 +136,29 @@ def argmax_rows(x):
     return out
 
 
-def render_labels(model_coarse, model_fine, rays_o, rays_d, N_samples=64, N_importance=128, N_test=4096):
+def render_labels(model_coarse, model_fine, rays_o, rays_d, N_samples=64, N_importance=128, N_test=4096, impl=_lib.IMPL_AUTO):
     """mesh_generator.py:117-136: each ray rendered deterministically with depths z_val_sample(n, 0.01, 15, N_samples), N_test rays
-    per call, label = argmax of the fine instance map."""
+    per call, label = argmax of the fine instance map.  impl: the network of the label rays, as in render_rays."""
     from .helpers import z_val_sample
     from .render import render_rays
     z = z_val_sample(1, 0.01, 15, N_samples)[0].to(rays_o.device)
     labels = torch.empty(rays_o.shape[0], device=rays_o.device, dtype=torch.int64)
     for b in range(0, rays_o.shape[0], N_test):
         out = render_rays(rays_o[b:b + N_test], rays_d[b:b + N_test], model_coarse, model_fine, z, N_importance=N_importance,
-                          want_raw=False, want_coarse=False)
+                          want_raw=False, want_coarse=False, impl=impl)
         labels[b:b + N_test] = argmax_rows(out["ins_fine"])
     return labels
 
 
 def extract_mesh(model_fine, model_coarse, scene_transform, grid_dim=256, level=0.45, extents=EXTENTS, near=4.0, far=15.0,
-                 N_samples=64, N_importance=128, N_test=4096, min_cluster=400):
+                 N_samples=64, N_importance=128, N_test=4096, min_cluster=400, impl=_lib.IMPL_AUTO):
     """The mesh of mesh_main on the device.  Defaults are the original's (mesh_generator.py:19-26, configs/dmsr/test/meshing.txt).
     Returns device tensors:
       vertices, triangles, normals        the marching-cubes mesh in scene space (written as <expname>.ply) and its normals
       clean_vertices, clean_normals, clean_triangles   after small-cluster removal (written as color_<expname>.ply)
       labels                              int64 object label per clean vertex
-      rays_o, rays_d                      the label rays, in the network's frame"""
+      rays_o, rays_d                      the label rays, in the network's frame
+    impl applies to the label rays only: the occupancy sweep always runs the exact network (its threshold decides the surface)."""
     T = check_transform(scene_transform)
     dev = next(model_fine.parameters()).device
     with torch.no_grad():
@@ -168,7 +169,7 @@ def extract_mesh(model_fine, model_coarse, scene_transform, grid_dim=256, level=
         normals = vertex_normals(verts, tris)
         cv, cn, ct = clean_mesh(verts, normals, tris, min_cluster)
         ro, rd = label_rays(cv, cn, near)
-        labels = render_labels(model_coarse, model_fine, ro, rd, N_samples, N_importance, N_test)
+        labels = render_labels(model_coarse, model_fine, ro, rd, N_samples, N_importance, N_test, impl)
     return {"vertices": verts, "triangles": tris, "normals": normals, "clean_vertices": cv, "clean_normals": cn,
             "clean_triangles": ct, "labels": labels, "rays_o": ro, "rays_d": rd}
 

@@ -61,13 +61,13 @@ def _to8b(x):
 
 
 def render_objects(position_embedder, view_embedder, model_coarse, model_fine, poses, hwk, args, keep=None, remove=None,
-                   savedir=None, ins_rgbs=None, color_dict=None):
+                   savedir=None, ins_rgbs=None, color_dict=None, impl=_lib.IMPL_AUTO):
     """Render every pose (camera-to-world, [4, 4] or [3, 4]) with the selection, deterministically, through the frame driver.
     Reads args.near, args.far, args.N_samples, args.N_importance.  Returns one dict per pose of device maps: rgb [H, W, 3],
     ins [H, W, ins_num], depth [H, W], acc [H, W].
     savedir: writes {i:03d}.png (RGBA, alpha = acc: an isolated object is a cut-out) and instance_{i:03d}.png (the arg-max label
     of the instance map, coloured as render_test colours it: ins_rgbs[color_dict[label]], channels in cv2's order).  Without
-    ins_rgbs / color_dict, label k gets colour k of a fixed seeded palette."""
+    ins_rgbs / color_dict, label k gets colour k of a fixed seeded palette.  impl: the network, as in render_frame."""
     from .render import _check_embedders, render_frame
     from .tester import colorize, pred_label_lut, write_png
     _check_embedders(position_embedder, view_embedder)
@@ -90,7 +90,7 @@ def render_objects(position_embedder, view_embedder, model_coarse, model_fine, p
         for i, c2w in enumerate(poses):
             c2w = torch.as_tensor(np.asarray(c2w.cpu() if torch.is_tensor(c2w) else c2w), dtype=torch.float32)
             m = render_frame(H, W, K, c2w, args.near, args.far, model_coarse, model_fine, N_samples=args.N_samples,
-                             N_importance=args.N_importance, device=dev, keep_objects=kept)
+                             N_importance=args.N_importance, device=dev, keep_objects=kept, impl=impl)
             m = {k: v.to(dev) for k, v in m.items()}
             out.append(m)
             if savedir is not None:

@@ -106,7 +106,9 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     weights (z_vals_*, weights_*; default = want_raw); want_coarse: the coarse pass' maps.  With want_raw=False and
     64 + 128 samples the whole call is ONE kernel and only the requested per-ray maps are written.
     keep_objects: an iterable of object labels in [0, ins_num]; samples labelled otherwise get alpha = 0 in both passes
-    (DESIGN.md, "Object selection").  raw_* stay the network's output.  Inference only."""
+    (DESIGN.md, "Object selection").  raw_* stay the network's output.  Inference only.
+    impl: _lib.IMPL_UMMA_F16 runs the fp16 preview network (DESIGN.md section 10); IMPL_AUTO follows DMNERF_INFER_IMPL."""
+    impl = _lib.infer_impl(impl)
     if want_samples is None:
         want_samples = want_raw
     dev = rays_o.device
@@ -239,7 +241,8 @@ def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64
     the C ABI: rays are generated on the device from K / c2w (get_rays_k), the coarse depth row from near / far
     (z_val_sample), the pixels are rendered by the fused kernel and the maps come back as HOST tensors:
     rgb [H,W,3], ins [H,W,ins_num], depth [H,W], acc [H,W] (or [n, ...] rows when a pixel_range = (begin, count) is given --
-    the per-rank slice of a sharded frame).  keep_objects: object selection as in render_rays."""
+    the per-rank slice of a sharded frame).  keep_objects: object selection as in render_rays; impl as in render_rays."""
+    impl = _lib.infer_impl(impl)
     dev = torch.device(device)
     ctx = get_context(dev)
     ins_num = bind_pair(ctx, model_coarse, model_fine)

@@ -38,6 +38,18 @@ extern "C" {
 #define DMNERF_IMPL_AUTO 0          /* tensor-core path when available for the shape, else SIMT */
 #define DMNERF_IMPL_SIMT 1          /* fp32 CUDA-core reference kernel */
 #define DMNERF_IMPL_UMMA 2          /* wgmma tensor-core kernel, bf16x3 split operands, fp32 accumulate */
+/* Preview precision, INFERENCE ONLY: the same tensor-core network run once with fp16 operands and fp32 accumulation (1/3 of
+ * the MMAs, 1/2 of the weight bytes).  Accepted by dmnerf_mlp_forward(_rays/_points), dmnerf_render_forward(_host/_objects)
+ * and dmnerf_render_frame(_objects)_host (with DMNERF_FLAG_WANT_RAW the stage kernels run it too).  Its weight image is packed
+ * on the first fp16 call after each dmnerf_set_weights, from the bound weights as they are then and the folded heads and
+ * biases packed by that dmnerf_set_weights: as for the exact image, weights changed in place take effect only through a new
+ * dmnerf_set_weights.  Measured against fp64 (DESIGN.md section 10, H100): network outputs rel. L2 2.8e-4 - 4.6e-4,
+ * rendered rgb 54 - 62 dB PSNR on typical rays, argmax labels >= 0.99 agreement.  fp16 stops at 65504: a weight above it fails
+ * the call at pack time, and a stored activation above it fails the call after the kernel (these fp16 calls synchronise
+ * the stream to deliver that verdict) -- render such a network with DMNERF_IMPL_UMMA.  dmnerf_mlp_forward_train rejects it
+ * (training and every backward stay exact), and dmnerf_mesh_occupancy(_objects), which has no impl, stays exact on purpose:
+ * its threshold decides the surface. */
+#define DMNERF_IMPL_UMMA_F16 3
 
 /* dmnerf_render_* flags */
 #define DMNERF_FLAG_PERTURB   1     /* args.perturb > 0: t_rand and u must be given (render.py:40-47, helpers.py:135) */
