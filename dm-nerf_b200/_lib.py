@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DMNERF_LIB_PATH: diagnostics builds of the same ABI (tools/kprof.py); the default is the in-tree product library
 LIB_PATH = os.environ.get("DMNERF_LIB_PATH") or os.path.join(_HERE, "lib", "libdmnerf_b200.so")
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 N_PARAMS = 30
 IMPL_AUTO, IMPL_SIMT, IMPL_UMMA, IMPL_UMMA_F16 = 0, 1, 2, 3
 FLAG_PERTURB, FLAG_WANT_RAW, FLAG_KEEP_INS = 1, 2, 4
@@ -60,12 +60,10 @@ PROTOTYPES = {
                                          _f32p, C.c_void_p]),
     "dmnerf_select_pixels": (C.c_int, [C.c_uint64, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p]),
     "dmnerf_hungarian_costs": (C.c_int, [_f32p, C.c_void_p, C.c_int64, C.c_int, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_void_p]),
-    "dmnerf_ins_loss_backward": (C.c_int, [_f32p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, _f32p, _f32p, _f32p, _f32p,
-                                           _f32p, C.c_void_p]),
+    "dmnerf_ins_loss_backward": (C.c_int, [_f32p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, _f32p, _f32p,
+                                           _f32p, _f32p, _f32p, C.c_void_p]),
     "dmnerf_ins_label_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dmnerf_hungarian_assign": (C.c_int, [_f32p, _f32p, _f32p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, _f32p, C.c_void_p]),
-    "dmnerf_ins_loss_backward_dev": (C.c_int, [_f32p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, _f32p, _f32p, _f32p,
-                                               _f32p, _f32p, C.c_void_p]),
     "dmnerf_ins_status_take": (C.c_int, []),
     "dmnerf_ins_label_bitmap": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "dmnerf_ins_label_rows_merged": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
@@ -73,8 +71,6 @@ PROTOTYPES = {
     "dmnerf_hungarian_partials": (C.c_int, [_f32p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "dmnerf_hungarian_costs_merged": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, _f32p, _f32p, _f32p, _f32p, _f32p,
                                                 C.c_void_p]),
-    "dmnerf_ins_loss_backward_shard": (C.c_int, [_f32p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, _f32p,
-                                                 _f32p, _f32p, _f32p, _f32p, C.c_void_p]),
     "dmnerf_stratify": (C.c_int, [_f32p, C.c_int64, _f32p, C.c_int64, C.c_int, _f32p, C.c_void_p]),
     "dmnerf_hier_sample": (C.c_int, [_f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, _f32p, C.c_void_p]),
     "dmnerf_act_floats_per_sample": (C.c_int, []),
@@ -100,8 +96,6 @@ PROTOTYPES = {
     "dmnerf_penalizer_backward": (C.c_int, [_f32p, _f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_float, C.c_float,
                                            C.c_void_p, _f32p, _f32p, C.c_int, C.c_void_p]),
     "dmnerf_penalizer_partials_bytes": (C.c_int64, [C.c_int64, C.c_int, C.c_int]),
-    "dmnerf_penalizer_partials": (C.c_int, [_f32p, _f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_float, C.c_float,
-                                            C.c_void_p, C.c_void_p]),
     "dmnerf_penalizer_merge": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, _f32p, C.c_void_p]),
     "dmnerf_profile_enable": (C.c_int, [C.c_void_p, C.c_int]),
     "dmnerf_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.c_int]),

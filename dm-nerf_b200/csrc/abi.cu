@@ -262,13 +262,13 @@ DMNERF_API int dmnerf_hungarian_costs(const float* pred, const int32_t* gt_row, 
   return launch_hungarian_costs(pred, gt_row, n, ins_num, cost_ce, cost_siou, tp, col_sum, row_count, (cudaStream_t)stream);
 }
 
-DMNERF_API int dmnerf_ins_loss_backward(const float* pred, const int32_t* gt_row, int64_t n, int ins_num,
-                                        const int32_t* row_of_col, int n_valid, const float* tp, const float* col_sum,
+DMNERF_API int dmnerf_ins_loss_backward(const float* pred, const int32_t* gt_row, int64_t n, int64_t n_global, int ins_num,
+                                        const int32_t* row_of_col, const int32_t* n_valid, const float* tp, const float* col_sum,
                                         const float* row_count, const float* g_losses, float* d_pred, void* stream) {
   DMN_CHECK(n >= 0, "ins_loss_backward: negative ray count");
-  DMN_CHECK(n == 0 || (pred && gt_row && row_of_col && tp && col_sum && row_count && g_losses && d_pred),
+  DMN_CHECK(n == 0 || (pred && gt_row && row_of_col && n_valid && tp && col_sum && row_count && g_losses && d_pred),
             "ins_loss_backward: NULL buffer");
-  return launch_ins_loss_grad(pred, gt_row, n, n, ins_num, row_of_col, n_valid, nullptr, tp, col_sum, row_count, g_losses, d_pred,
+  return launch_ins_loss_grad(pred, gt_row, n, n_global, ins_num, row_of_col, n_valid, tp, col_sum, row_count, g_losses, d_pred,
                               (cudaStream_t)stream);
 }
 
@@ -281,16 +281,6 @@ DMNERF_API int dmnerf_hungarian_assign(const float* cost_ce, const float* cost_s
                                        int64_t n, int ins_num, int32_t* row_of_col, float* losses, void* stream) {
   DMN_CHECK(cost_ce && cost_siou && col_sum && n_valid && row_of_col && losses, "hungarian_assign: NULL buffer");
   return launch_hungarian_assign(cost_ce, cost_siou, col_sum, n_valid, n, ins_num, row_of_col, losses, (cudaStream_t)stream);
-}
-
-DMNERF_API int dmnerf_ins_loss_backward_dev(const float* pred, const int32_t* gt_row, int64_t n, int ins_num,
-                                            const int32_t* row_of_col, const int32_t* n_valid, const float* tp, const float* col_sum,
-                                            const float* row_count, const float* g_losses, float* d_pred, void* stream) {
-  DMN_CHECK(n >= 0, "ins_loss_backward_dev: negative ray count");
-  DMN_CHECK(n == 0 || (pred && gt_row && row_of_col && n_valid && tp && col_sum && row_count && g_losses && d_pred),
-            "ins_loss_backward_dev: NULL buffer");
-  return launch_ins_loss_grad(pred, gt_row, n, n, ins_num, row_of_col, 0, n_valid, tp, col_sum, row_count, g_losses, d_pred,
-                              (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_ins_label_bitmap(const int32_t* labels, int64_t n, uint32_t* bitmap, void* stream) {
@@ -315,16 +305,6 @@ DMNERF_API int dmnerf_hungarian_costs_merged(const double* partials, int world, 
   DMN_CHECK(partials && cost_ce && cost_siou && tp && col_sum && row_count, "hungarian_costs_merged: NULL buffer");
   return launch_hungarian_costs_merged(partials, world, n_global, ins_num, cost_ce, cost_siou, tp, col_sum, row_count,
                                        (cudaStream_t)stream);
-}
-
-DMNERF_API int dmnerf_ins_loss_backward_shard(const float* pred, const int32_t* gt_row, int64_t n, int64_t n_global, int ins_num,
-                                              const int32_t* row_of_col, const int32_t* n_valid, const float* tp, const float* col_sum,
-                                              const float* row_count, const float* g_losses, float* d_pred, void* stream) {
-  DMN_CHECK(n >= 0, "ins_loss_backward_shard: negative ray count");
-  DMN_CHECK(n == 0 || (pred && gt_row && row_of_col && n_valid && tp && col_sum && row_count && g_losses && d_pred),
-            "ins_loss_backward_shard: NULL buffer");
-  return launch_ins_loss_grad(pred, gt_row, n, n_global, ins_num, row_of_col, 0, n_valid, tp, col_sum, row_count, g_losses, d_pred,
-                              (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_ins_status_take(void) { return ins_status_take(); }
@@ -387,25 +367,17 @@ DMNERF_API int64_t dmnerf_penalizer_partials_bytes(int64_t n, int s, int c) {
   return (n < 0 || s < 1) ? -1 : (int64_t)penalizer_partials_bytes(n, s, c);
 }
 
-DMNERF_API int dmnerf_penalizer_partials(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,
-                                         int s, int c, float tolerance, float deta_w, void* partials, void* stream) {
-  DMN_CHECK(n >= 0, "penalizer_partials: negative ray count");
-  DMN_CHECK(partials && (n == 0 || (raw && z_vals && depth && rays_d)), "penalizer_partials: NULL buffer");
-  DMN_CHECK(deta_w > 0.0f, "penalizer_partials: deta_w must be positive");
-  return launch_penalizer_partials(raw, z_vals, depth, rays_d, n, s, c, tolerance, deta_w, partials, (cudaStream_t)stream);
-}
-
 DMNERF_API int dmnerf_penalizer_merge(const void* states, int world, int c, void* state, float* loss, void* stream) {
   DMN_CHECK(states && state && loss, "penalizer_merge: NULL buffer");
   return launch_penalizer_merge(states, world, c, state, loss, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_penalizer_forward(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,
-                                        int s, int c, float tolerance, float deta_w, void* state, float* loss, void* stream) {
+                                        int s, int c, float tolerance, float deta_w, void* partials, float* loss, void* stream) {
   DMN_CHECK(n >= 0, "penalizer_forward: negative ray count");
-  DMN_CHECK(state && loss && (n == 0 || (raw && z_vals && depth && rays_d)), "penalizer_forward: NULL buffer");
+  DMN_CHECK(partials && loss && (n == 0 || (raw && z_vals && depth && rays_d)), "penalizer_forward: NULL buffer");
   DMN_CHECK(deta_w > 0.0f, "penalizer_forward: deta_w must be positive");
-  return launch_penalizer_forward(raw, z_vals, depth, rays_d, n, s, c, tolerance, deta_w, state, loss, (cudaStream_t)stream);
+  return launch_penalizer_forward(raw, z_vals, depth, rays_d, n, s, c, tolerance, deta_w, partials, loss, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,

@@ -174,22 +174,20 @@ int gemm_tc_check_status(cudaStream_t st);
 
 // Emptiness regulariser (penalizer.cu)
 int launch_penalizer_forward(const float* raw, const float* z, const float* depth, const float* rays_d, int64_t n, int s, int c,
-                             float tol, float w, void* state, float* loss, cudaStream_t st);
+                             float tol, float w, void* partials, float* loss, cudaStream_t st);
 int launch_penalizer_backward(const float* raw, const float* z, const float* depth, const float* rays_d, int64_t n, int s, int c,
                               float tol, float w, const void* state, const float* g_loss, float* d_raw, int accumulate,
                               cudaStream_t st);
 size_t penalizer_state_bytes();
 size_t penalizer_partials_bytes(int64_t n, int s, int c);
-int launch_penalizer_partials(const float* raw, const float* z, const float* depth, const float* rays_d, int64_t n, int s, int c,
-                              float tol, float w, void* partials, cudaStream_t st);
 int launch_penalizer_merge(const void* states, int world, int c, void* state, float* loss, cudaStream_t st);
 
 // Hungarian-matched instance loss (evaluator.cu)
 int launch_hungarian_costs(const float* pred, const int32_t* gt_row, int64_t n, int k, float* cost_ce, float* cost_siou,
                            float* tp, float* s_sum, float* cnt, cudaStream_t st);
 int launch_ins_loss_grad(const float* pred, const int32_t* gt_row, int64_t n, int64_t n_norm, int k, const int32_t* row_of_col,
-                         int n_valid, const int32_t* n_valid_dev, const float* tp, const float* s_sum, const float* cnt, const float* g3,
-                         float* d_pred, cudaStream_t st);
+                         const int32_t* n_valid, const float* tp, const float* s_sum, const float* cnt, const float* g3, float* d_pred,
+                         cudaStream_t st);
 int launch_label_rows(const int32_t* labels, int64_t n, int k, int32_t* gt_row, int32_t* n_valid, cudaStream_t st);
 int launch_hungarian_assign(const float* cost_ce, const float* cost_siou, const float* s_sum, const int32_t* n_valid, int64_t n, int k,
                             int32_t* row_of_col, float* loss3, cudaStream_t st);

@@ -35,49 +35,20 @@ __device__ __forceinline__ void write_costs(int g, int p, int k, int64_t n, doub
   if (p == 0) cnt_out[g] = (float)cnt;
 }
 
-// One block per prediction column p.
-__global__ void hungarian_cost_kernel(const float* __restrict__ pred, const int32_t* __restrict__ gt_row, int64_t n, int k,
-                                      float* __restrict__ cost_ce, float* __restrict__ cost_siou, float* __restrict__ tp_out,
-                                      float* __restrict__ s_out, float* __restrict__ cnt_out) {
-  __shared__ double sB[EV_MAX_K], sC[EV_MAX_K], sTP[EV_MAX_K];
-  __shared__ double sA, sS;
-  __shared__ unsigned int sCnt[EV_MAX_K];
-  const int p = blockIdx.x;
-  for (int g = threadIdx.x; g < k; g += blockDim.x) { sB[g] = 0.0; sC[g] = 0.0; sTP[g] = 0.0; sCnt[g] = 0u; }
-  if (threadIdx.x == 0) { sA = 0.0; sS = 0.0; }
-  __syncthreads();
-  double a = 0.0, s = 0.0;
-  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
-    const float v = pred[i * k + p];
-    const int g = gt_row[i];
-    const float l1 = logf(__fadd_rn(__fsub_rn(1.0f, v), 1e-8f));
-    a += (double)l1;
-    s += (double)v;
-    if (g >= 0 && g < k) {
-      atomicAdd(&sB[g], (double)logf(__fadd_rn(v, 1e-8f)));
-      atomicAdd(&sC[g], (double)l1);
-      atomicAdd(&sTP[g], (double)v);
-      atomicAdd(&sCnt[g], 1u);
-    }
-  }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) { a += __shfl_xor_sync(FULL, a, d); s += __shfl_xor_sync(FULL, s, d); }
-  if ((threadIdx.x & 31) == 0) { atomicAdd(&sA, a); atomicAdd(&sS, s); }
-  __syncthreads();
-  for (int g = threadIdx.x; g < k; g += blockDim.x)
-    write_costs(g, p, k, n, sA, sS, sB[g], sC[g], sTP[g], (double)sCnt[g], cost_ce, cost_siou, tp_out, cnt_out);
-  if (threadIdx.x == 0) s_out[p] = (float)sS;
-}
-
-// ---------------------------------------------------------------------------------------------------- sharded batch
-// The sums above for one contiguous shard of the batch, in fp64, summed in an order fixed by the shard's size alone (no
-// floating-point atomics): partials = A[k] | S[k] | B[k x k] | C[k x k] | TP[k x k] | cnt[k] (row g, column p at g * k + p).
-// One block per column p; every warp walks 32-row chunks, adds the rows of one label in lane order and keeps its own
-// per-label sums; the warps' sums are added in warp order at the end.
+// The sums above, in fp64, for the batch or for one contiguous shard of it, summed in an order fixed by the size alone (no
+// floating-point atomics).  One block per column p; every warp walks 32-row chunks, adds the rows of one label in lane order
+// and keeps its own per-label sums; the warps' sums are added in warp order at the end.  Then either
+//   FINAL = false: the shard's partials = A[k] | S[k] | B[k x k] | C[k x k] | TP[k x k] | cnt[k] (row g, column p at g * k + p),
+//                  merged by hungarian_costs_merged_kernel, or
+//   FINAL = true:  the costs of the whole batch (n rays) straight from these sums -- the one-shard case of the merge, and bit
+//                  for bit its result, since the merge adds each partial to 0.0.
 constexpr int HP_WARPS = 8;
+template <bool FINAL>
 __global__ void __launch_bounds__(HP_WARPS * 32) hungarian_partials_kernel(const float* __restrict__ pred,
                                                                              const int32_t* __restrict__ gt_row, int64_t n, int k,
-                                                                             double* __restrict__ out) {
+                                                                             double* __restrict__ out, float* __restrict__ cost_ce,
+                                                                             float* __restrict__ cost_siou, float* __restrict__ tp_out,
+                                                                             float* __restrict__ s_out, float* __restrict__ cnt_out) {
   __shared__ double wB[HP_WARPS][EV_MAX_K], wC[HP_WARPS][EV_MAX_K], wTP[HP_WARPS][EV_MAX_K];
   __shared__ unsigned int wCnt[HP_WARPS][EV_MAX_K];
   __shared__ double stage[HP_WARPS][3][32];
@@ -118,21 +89,31 @@ __global__ void __launch_bounds__(HP_WARPS * 32) hungarian_partials_kernel(const
   __syncthreads();
   const size_t kk = (size_t)k * k;
   double* A = out; double* S = out + k; double* B = out + 2 * k; double* C = B + kk; double* TP = C + kk; double* cnt = TP + kk;
+  double ta = 0.0, ts = 0.0;
+  if constexpr (FINAL)                                       // every cell of the column needs A[p] and S[p]
+    for (int w = 0; w < HP_WARPS; ++w) { ta += wA[w]; ts += wS[w]; }
   for (int g = threadIdx.x; g < k; g += blockDim.x) {
     double b = 0.0, c = 0.0, t = 0.0;
     unsigned int m = 0u;
     for (int w = 0; w < HP_WARPS; ++w) { b += wB[w][g]; c += wC[w][g]; t += wTP[w][g]; m += wCnt[w][g]; }
-    B[(size_t)g * k + p] = b; C[(size_t)g * k + p] = c; TP[(size_t)g * k + p] = t;
-    if (p == 0) cnt[g] = (double)m;
+    if constexpr (FINAL) {
+      write_costs(g, p, k, n, ta, ts, b, c, t, (double)m, cost_ce, cost_siou, tp_out, cnt_out);
+    } else {
+      B[(size_t)g * k + p] = b; C[(size_t)g * k + p] = c; TP[(size_t)g * k + p] = t;
+      if (p == 0) cnt[g] = (double)m;
+    }
   }
   if (threadIdx.x == 0) {
-    double ta = 0.0, ts = 0.0;
-    for (int w = 0; w < HP_WARPS; ++w) { ta += wA[w]; ts += wS[w]; }
-    A[p] = ta; S[p] = ts;
+    if constexpr (FINAL) {
+      s_out[p] = (float)ts;
+    } else {
+      for (int w = 0; w < HP_WARPS; ++w) { ta += wA[w]; ts += wS[w]; }
+      A[p] = ta; S[p] = ts;
+    }
   }
 }
 
-// The partials of `world` shards added in shard order, then hungarian_cost_kernel's formulas with the global ray count n.
+// The partials of `world` shards added in shard order, then the costs of the batch of n rays (write_costs).
 __global__ void hungarian_costs_merged_kernel(const double* __restrict__ partials, int world, int64_t n, int k,
                                               float* __restrict__ cost_ce, float* __restrict__ cost_siou, float* __restrict__ tp_out,
                                               float* __restrict__ s_out, float* __restrict__ cnt_out) {
@@ -155,18 +136,16 @@ __global__ void hungarian_costs_merged_kernel(const double* __restrict__ partial
 // d loss / d pred for  loss = g_ce * valid_ce + g_inv * invalid_ce + g_siou * valid_siou  (evaluator.py:27-36):
 //   valid_ce = mean_{g < V} cost_ce[g, col(g)],  valid_siou likewise,  invalid_ce = mean(pred[:, unmatched columns]).
 // row_of_col[p] = matched gt row of prediction column p, or -1 (unmatched).  g3 = the three upstream gradients (device).
-// n rows of pred are written; n_norm is the ray count of the whole batch (n_norm > n for one shard of it).
+// n rows of pred are written; n_norm is the ray count of the whole batch (n_norm > n for one shard of it).  n_valid_dev = the
+// number of distinct labels (device).
 __global__ void ins_loss_grad_kernel(const float* __restrict__ pred, const int32_t* __restrict__ gt_row, int64_t n, int64_t n_norm,
-                                     int k, const int32_t* __restrict__ row_of_col, int n_valid,
-                                     const int32_t* __restrict__ n_valid_dev, const float* __restrict__ tp,
-                                     const float* __restrict__ s_sum, const float* __restrict__ cnt, const float* __restrict__ g3,
-                                     float* __restrict__ d_pred) {
+                                     int k, const int32_t* __restrict__ row_of_col, const int32_t* __restrict__ n_valid_dev,
+                                     const float* __restrict__ tp, const float* __restrict__ s_sum, const float* __restrict__ cnt,
+                                     const float* __restrict__ g3, float* __restrict__ d_pred) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n * k) return;
-  if (n_valid_dev) {                         // device-side assignment: the number of distinct labels never left the device
-    n_valid = *n_valid_dev;
-    if (n_valid < 1) { d_pred[idx] = 0.0f; return; }        // rejected labels: NaN loss, zero gradient, error on the next call
-  }
+  const int n_valid = *n_valid_dev;
+  if (n_valid < 1) { d_pred[idx] = 0.0f; return; }          // rejected labels: NaN loss, zero gradient, error on the next call
   const int64_t i = idx / k;
   const int p = (int)(idx % k);
   const int g = row_of_col[p];
@@ -409,21 +388,21 @@ int launch_hungarian_costs(const float* pred, const int32_t* gt_row, int64_t n, 
                            float* tp, float* s_sum, float* cnt, cudaStream_t st) {
   DMN_CHECK(k >= 1 && k <= EV_MAX_K, "hungarian_costs: ins_num %d out of range (max %d)", k, EV_MAX_K);
   DMN_CHECK(n >= 1, "hungarian_costs: empty batch");
-  hungarian_cost_kernel<<<(unsigned)k, 256, 0, st>>>(pred, gt_row, n, k, cost_ce, cost_siou, tp, s_sum, cnt);
+  hungarian_partials_kernel<true><<<(unsigned)k, HP_WARPS * 32, 0, st>>>(pred, gt_row, n, k, nullptr, cost_ce, cost_siou, tp, s_sum,
+                                                                         cnt);
   DMN_LAUNCH_OK();
   return 0;
 }
 
 int launch_ins_loss_grad(const float* pred, const int32_t* gt_row, int64_t n, int64_t n_norm, int k, const int32_t* row_of_col,
-                         int n_valid, const int32_t* n_valid_dev, const float* tp, const float* s_sum, const float* cnt, const float* g3,
-                         float* d_pred, cudaStream_t st) {
-  DMN_CHECK(k >= 1 && k <= EV_MAX_K && (n_valid_dev || (n_valid >= 1 && n_valid <= k)), "ins_loss_grad: bad sizes (k %d, valid %d)", k,
-            n_valid);
+                         const int32_t* n_valid, const float* tp, const float* s_sum, const float* cnt, const float* g3, float* d_pred,
+                         cudaStream_t st) {
+  DMN_CHECK(k >= 1 && k <= EV_MAX_K, "ins_loss_grad: ins_num %d out of range (max %d)", k, EV_MAX_K);
   DMN_CHECK(n_norm >= n, "ins_loss_grad: %lld rows of a batch of %lld", (long long)n, (long long)n_norm);
   const int64_t total = n * k;
   if (total == 0) return 0;
-  ins_loss_grad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(pred, gt_row, n, n_norm, k, row_of_col, n_valid, n_valid_dev,
-                                                                        tp, s_sum, cnt, g3, d_pred);
+  ins_loss_grad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(pred, gt_row, n, n_norm, k, row_of_col, n_valid, tp, s_sum,
+                                                                        cnt, g3, d_pred);
   DMN_LAUNCH_OK();
   return 0;
 }
@@ -431,7 +410,8 @@ int launch_ins_loss_grad(const float* pred, const int32_t* gt_row, int64_t n, in
 int launch_hungarian_partials(const float* pred, const int32_t* gt_row, int64_t n, int k, double* partials, cudaStream_t st) {
   DMN_CHECK(k >= 1 && k <= EV_MAX_K, "hungarian_partials: ins_num %d out of range (max %d)", k, EV_MAX_K);
   DMN_CHECK(n >= 0, "hungarian_partials: negative ray count");
-  hungarian_partials_kernel<<<(unsigned)k, HP_WARPS * 32, 0, st>>>(pred, gt_row, n, k, partials);
+  hungarian_partials_kernel<false><<<(unsigned)k, HP_WARPS * 32, 0, st>>>(pred, gt_row, n, k, partials, nullptr, nullptr, nullptr,
+                                                                          nullptr, nullptr);
   DMN_LAUNCH_OK();
   return 0;
 }

@@ -7,8 +7,8 @@
 //   before: z |d| < (depth - tol) |d|;  after: z |d| > (depth + tol) |d|;  middle = 1 - (before + after)   (penalizer.py:27-29)
 //
 // Two launches, both HBM-streaming with the rows of raw staged through shared memory (coalesced):
-//   penalizer_loss_kernel    the two mask populations (integers: exact), the two masked sums (fp64 accumulation of fp32
-//                            terms) and the finalisation by the last block, in one pass over raw
+//   penalizer_partial_kernel the two mask populations (integers: exact), the two masked sums (fp64 accumulation of fp32
+//                            terms, in an order fixed by the sizes) and the finalisation by the last block, in one pass over raw
 //   penalizer_grad_kernel    d L / d raw * upstream gradient (a device scalar: no host synchronisation); writes every channel
 //                            (zeros for rgb / sigma), so the caller needs no zero-fill
 // Not folded into the composite kernel: the masks need the finished depth map of the ray (a second sweep over its samples either
@@ -108,32 +108,11 @@ __device__ __forceinline__ float pen_finalise(unsigned long long n_before, unsig
   return (float)(sum_before / ((double)K * nbt) + sum_middle / nmt);
 }
 
-// Forward in ONE pass: mask populations (integer atomics: exact), the two masked sums (fp64 accumulation of fp32 terms), and
-// the finalisation by the last block -- the sums do not depend on the populations until the final division.
-__global__ void penalizer_loss_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ depth,
-                                      const float* __restrict__ rays_d, int64_t total, int s, int c, float tol, float w,
-                                      PenState* st, float* __restrict__ loss) {
-  double tb, tm;
-  unsigned long long cb, cm;
-  pen_block_terms(raw, z, depth, rays_d, total, s, c, tol, w, tb, tm, cb, cm);
-  if (threadIdx.x == 0) {
-    atomicAdd(&st->sum_before, tb);
-    atomicAdd(&st->sum_middle, tm);
-    if (cb) atomicAdd(&st->n_before, cb);
-    if (cm) atomicAdd(&st->n_middle, cm);
-    __threadfence();
-    if (atomicAdd(&st->blocks_done, 1u) == gridDim.x - 1) {        // last block: finalise
-      __threadfence();
-      loss[0] = pen_finalise(*(volatile unsigned long long*)&st->n_before, *(volatile unsigned long long*)&st->n_middle,
-                             *(volatile double*)&st->sum_before, *(volatile double*)&st->sum_middle, c - 4);
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------- sharded batch
-// The populations and masked sums of one shard of the batch, unfinalised, summed in an order fixed by the shard's size alone:
-// every block writes its terms to its own slot after the PenState head, and the last block to finish adds the slots with a
-// fixed-shape reduction into the head.
+// Forward in ONE pass over the batch or over one shard of it: the populations and masked sums, summed in an order fixed by the
+// size alone (no floating-point atomics).  Every block writes its terms to its own slot after the PenState head, and the last
+// block to finish adds the slots with a fixed-shape reduction into the head and writes the loss of those sums.  A single
+// process reads that loss; the shards of a batch gather their heads and merge them (penalizer_merge_kernel), which at one
+// shard gives the same head and loss bit for bit.
 struct PenBlock {
   double sb, sm;
   unsigned long long nb, nm;
@@ -141,7 +120,7 @@ struct PenBlock {
 
 __global__ void penalizer_partial_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ depth,
                                          const float* __restrict__ rays_d, int64_t total, int s, int c, float tol, float w,
-                                         PenState* st, PenBlock* blocks) {
+                                         PenState* st, PenBlock* blocks, float* __restrict__ loss) {
   double tb, tm;
   unsigned long long cb, cm;
   pen_block_terms(raw, z, depth, rays_d, total, s, c, tol, w, tb, tm, cb, cm);
@@ -156,6 +135,7 @@ __global__ void penalizer_partial_kernel(const float* __restrict__ raw, const fl
   __threadfence();
   double sb = 0.0, sm = 0.0;
   unsigned long long nb = 0, nm = 0;
+#pragma unroll 4
   for (unsigned b = threadIdx.x; b < gridDim.x; b += blockDim.x) {
     sb += __ldcg(&blocks[b].sb); sm += __ldcg(&blocks[b].sm); nb += __ldcg(&blocks[b].nb); nm += __ldcg(&blocks[b].nm);
   }
@@ -170,6 +150,7 @@ __global__ void penalizer_partial_kernel(const float* __restrict__ raw, const fl
     PenBlock t{0.0, 0.0, 0, 0};
     for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { t.sb += wsum[i].sb; t.sm += wsum[i].sm; t.nb += wsum[i].nb; t.nm += wsum[i].nm; }
     st->sum_before = t.sb; st->sum_middle = t.sm; st->n_before = t.nb; st->n_middle = t.nm;
+    loss[0] = pen_finalise(t.nb, t.nm, t.sb, t.sm, c - 4);
   }
 }
 
@@ -230,23 +211,6 @@ __global__ void penalizer_grad_kernel(const float* __restrict__ raw, const float
   }
 }
 
-int launch_penalizer_forward(const float* raw, const float* z, const float* depth, const float* rays_d, int64_t n, int s, int c,
-                             float tol, float w, void* state, float* loss, cudaStream_t st) {
-  DMN_CHECK(c > 4 && c <= 4 + DMNERF_MAX_INS + 1 && s >= 1, "penalizer: bad sizes s=%d c=%d", s, c);
-  PenState* ps = reinterpret_cast<PenState*>(state);
-  DMN_CUDA(cudaMemsetAsync(ps, 0, sizeof(PenState), st));
-  const int64_t total = n * s;
-  if (total == 0) {
-    DMN_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), st));
-    return 0;
-  }
-  const int tile = pen_tile(c);
-  const unsigned grid = (unsigned)((total + tile - 1) / tile);
-  penalizer_loss_kernel<<<grid, tile, (size_t)tile * c * sizeof(float), st>>>(raw, z, depth, rays_d, total, s, c, tol, w, ps, loss);
-  DMN_LAUNCH_OK();
-  return 0;
-}
-
 int launch_penalizer_backward(const float* raw, const float* z, const float* depth, const float* rays_d, int64_t n, int s, int c,
                               float tol, float w, const void* state, const float* g_loss, float* d_raw, int accumulate,
                               cudaStream_t st) {
@@ -271,17 +235,20 @@ size_t penalizer_partials_bytes(int64_t n, int s, int c) {
   return sizeof(PenState) + (size_t)((total + tile - 1) / tile) * sizeof(PenBlock);
 }
 
-int launch_penalizer_partials(const float* raw, const float* z, const float* depth, const float* rays_d, int64_t n, int s, int c,
-                              float tol, float w, void* partials, cudaStream_t st) {
+int launch_penalizer_forward(const float* raw, const float* z, const float* depth, const float* rays_d, int64_t n, int s, int c,
+                             float tol, float w, void* partials, float* loss, cudaStream_t st) {
   DMN_CHECK(c > 4 && c <= 4 + DMNERF_MAX_INS + 1 && s >= 1, "penalizer: bad sizes s=%d c=%d", s, c);
   PenState* ps = reinterpret_cast<PenState*>(partials);
   DMN_CUDA(cudaMemsetAsync(ps, 0, sizeof(PenState), st));
   const int64_t total = n * s;
-  if (total == 0) return 0;
+  if (total == 0) {
+    DMN_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), st));
+    return 0;
+  }
   const int tile = pen_tile(c);
   const unsigned grid = (unsigned)((total + tile - 1) / tile);
   penalizer_partial_kernel<<<grid, tile, (size_t)tile * c * sizeof(float), st>>>(raw, z, depth, rays_d, total, s, c, tol, w, ps,
-                                                                                 reinterpret_cast<PenBlock*>(ps + 1));
+                                                                                 reinterpret_cast<PenBlock*>(ps + 1), loss);
   DMN_LAUNCH_OK();
   return 0;
 }

@@ -15,57 +15,12 @@ replica takes the same Adam step.  DESIGN.md, "Data-parallel training", gives th
 """
 import torch
 
-from . import _lib
 from .backward import render_rays_grad
-from .engine import get_context, ordered_params
-from .parallel import shard_range
+from .engine import ordered_params
+from .evaluator import _MatchedLossDevice, _check_status
+from .parallel import all_gather, all_reduce_sum_, shard_range, world_of
+from .penalizer import _Penalizer
 from .render import reference_draws
-
-
-def world_of(group=None):
-    """(world size, rank) of `group`; (1, 0) when torch.distributed is not initialised (one process)."""
-    import torch.distributed as dist
-    if not (dist.is_available() and dist.is_initialized()):
-        return 1, 0
-    return dist.get_world_size(group), dist.get_rank(group)
-
-
-def _nccl(group):
-    import torch.distributed as dist
-    return dist.get_backend(group) == "nccl"
-
-
-def all_gather(t, group=None):
-    """[W, *t.shape] on t's device, rank order.  NCCL gathers device tensors; gloo has no CUDA all-gather, so a gloo group is
-    staged through host memory."""
-    world, _ = world_of(group)
-    if world == 1:
-        return t[None]
-    import torch.distributed as dist
-    t = t.contiguous()
-    if _nccl(group):
-        out = t.new_empty((world,) + tuple(t.shape))
-        dist.all_gather_into_tensor(out, t, group=group)
-        return out
-    host = t.cpu()
-    parts = [torch.empty_like(host) for _ in range(world)]
-    dist.all_gather(parts, host, group=group)
-    return torch.stack(parts).to(t.device)
-
-
-def all_reduce_sum_(t, group=None):
-    """In-place sum of `t` over the ranks (staged through host memory for gloo)."""
-    world, _ = world_of(group)
-    if world == 1:
-        return t
-    import torch.distributed as dist
-    if _nccl(group):
-        dist.all_reduce(t, group=group)
-    else:
-        host = t.cpu()
-        dist.all_reduce(host, group=group)
-        t.copy_(host)
-    return t
 
 
 def instance_rows(lo, hi, n_global, n_ins=None):
@@ -78,60 +33,6 @@ def instance_rows(lo, hi, n_global, n_ins=None):
 
 
 # ------------------------------------------------------------------------------------------------------------- instance loss
-class _InsSharded(torch.autograd.Function):
-    @staticmethod
-    def forward(fctx, pred_ins, labels, ins_num, n_global, group):
-        pred = pred_ins.detach().reshape(-1, ins_num).contiguous().float()
-        n, k = pred.shape
-        dev = pred.device
-        ctx = get_context(dev)
-        world, _ = world_of(group)
-        i32 = torch.int32
-        bitmap = torch.empty(_lib.LABEL_WORDS, device=dev, dtype=i32)         # uint32 words in int32 storage
-        ctx.call("dmnerf_ins_label_bitmap", _lib.ptr(labels, i32), n, _lib.ptr(bitmap, i32))
-        bitmaps = all_gather(bitmap, group)
-        gt_row = torch.empty(n, device=dev, dtype=i32)
-        n_valid = torch.empty(1, device=dev, dtype=i32)
-        ctx.call("dmnerf_ins_label_rows_merged", _lib.ptr(bitmaps, i32), world, _lib.ptr(labels, i32), n, k, _lib.ptr(gt_row, i32),
-                 _lib.ptr(n_valid, i32))
-        part = torch.empty(3 * k * (k + 1), device=dev, dtype=torch.float64)
-        ctx.call("dmnerf_hungarian_partials", _lib.ptr(pred), _lib.ptr(gt_row, i32), n, k, _lib.ptr(part, torch.float64))
-        parts = all_gather(part, group)
-        e = lambda *s: torch.empty(s, device=dev, dtype=torch.float32)
-        c = {"cost_ce": e(k, k), "cost_siou": e(k, k), "tp": e(k, k), "col_sum": e(k), "row_count": e(k)}
-        ctx.call("dmnerf_hungarian_costs_merged", _lib.ptr(parts, torch.float64), world, n_global, k, _lib.ptr(c["cost_ce"]),
-                 _lib.ptr(c["cost_siou"]), _lib.ptr(c["tp"]), _lib.ptr(c["col_sum"]), _lib.ptr(c["row_count"]))
-        row_of_col = torch.empty(k, device=dev, dtype=i32)
-        losses = e(3)
-        ctx.call("dmnerf_hungarian_assign", _lib.ptr(c["cost_ce"]), _lib.ptr(c["cost_siou"]), _lib.ptr(c["col_sum"]),
-                 _lib.ptr(n_valid, i32), n_global, k, _lib.ptr(row_of_col, i32), _lib.ptr(losses))
-        fctx.save_for_backward(pred, gt_row, row_of_col, n_valid, c["tp"], c["col_sum"], c["row_count"])
-        fctx.in_shape, fctx.n_global = pred_ins.shape, n_global
-        fctx.mark_non_differentiable(n_valid, row_of_col)
-        return losses[0].clone(), losses[1].clone(), losses[2].clone(), n_valid, row_of_col
-
-    @staticmethod
-    def backward(fctx, g_ce, g_inv, g_siou, _g_n=None, _g_r=None):
-        pred, gt_row, row_of_col, n_valid, tp, col_sum, row_count = fctx.saved_tensors
-        n, k = pred.shape
-        zero = pred.new_zeros(())
-        g3 = torch.stack([(g if g is not None else zero).reshape(()).float() for g in (g_ce, g_inv, g_siou)]).contiguous()
-        d_pred = torch.empty_like(pred)
-        i32 = torch.int32
-        get_context(pred.device).call("dmnerf_ins_loss_backward_shard", _lib.ptr(pred), _lib.ptr(gt_row, i32), n, fctx.n_global, k,
-                                      _lib.ptr(row_of_col, i32), _lib.ptr(n_valid, i32), _lib.ptr(tp), _lib.ptr(col_sum),
-                                      _lib.ptr(row_count), _lib.ptr(g3), _lib.ptr(d_pred))
-        return d_pred.reshape(fctx.in_shape), None, None, None, None
-
-
-def _check_status(device):
-    from .evaluator import _STATUS_TEXT
-    code = get_context(device).lib.dmnerf_ins_status_take()
-    if code:
-        raise RuntimeError("ins_criterion_sharded: an earlier call was given %s (code %d); its loss was NaN and its gradient zero"
-                           % (_STATUS_TEXT.get(code, "labels it cannot rank"), code))
-
-
 def ins_assignment_sharded(pred_ins, gt_labels, ins_num, n_global, group=None):
     """ins_criterion_sharded's terms plus the matching: (valid_ce, invalid_ce, valid_siou, n_valid [1], row_of_col [ins_num]),
     all on the device and identical on every rank."""
@@ -140,9 +41,9 @@ def ins_assignment_sharded(pred_ins, gt_labels, ins_num, n_global, group=None):
     if pred_ins.dim() != 2 or pred_ins.shape[1] != ins_num or gt_labels.shape[0] != pred_ins.shape[0]:
         raise RuntimeError("ins_criterion_sharded: pred_ins %s / gt_labels %s / ins_num %d are inconsistent"
                            % (tuple(pred_ins.shape), tuple(gt_labels.shape), ins_num))
-    _check_status(pred_ins.device)
+    _check_status(pred_ins.device, "ins_criterion_sharded")
     labels = gt_labels.to(pred_ins.device).reshape(-1).to(torch.int32).contiguous()
-    return _InsSharded.apply(pred_ins, labels, int(ins_num), int(n_global), group)
+    return _MatchedLossDevice.apply(pred_ins, labels, int(n_global), group)
 
 
 def ins_criterion_sharded(pred_ins, gt_labels, ins_num, n_global, group=None):
@@ -155,47 +56,11 @@ def ins_criterion_sharded(pred_ins, gt_labels, ins_num, n_global, group=None):
 
 
 # ------------------------------------------------------------------------------------------------------------------ penalizer
-class _PenSharded(torch.autograd.Function):
-    @staticmethod
-    def forward(fctx, raw, z_vals, depth, rays_d, tolerance, deta_w, group):
-        if not raw.is_cuda:
-            raise RuntimeError("ins_penalizer_sharded: expected CUDA tensors (no CPU fallback)")
-        ctx = get_context(raw.device)
-        raw_c, z_c = raw.detach().contiguous().float(), z_vals.detach().contiguous().float()
-        d_c, rd_c = depth.detach().reshape(-1).contiguous().float(), rays_d.detach().contiguous().float()
-        n, s, c = raw_c.shape
-        if z_c.shape != (n, s) or d_c.shape != (n,) or rd_c.shape != (n, 3):
-            raise RuntimeError("ins_penalizer_sharded: inconsistent shapes raw %s z_vals %s depth %s rays_d %s"
-                               % (tuple(raw.shape), tuple(z_vals.shape), tuple(depth.shape), tuple(rays_d.shape)))
-        u8 = torch.uint8
-        part = torch.empty(int(ctx.lib.dmnerf_penalizer_partials_bytes(n, s, c)), device=raw.device, dtype=u8)
-        ctx.call("dmnerf_penalizer_partials", _lib.ptr(raw_c), _lib.ptr(z_c), _lib.ptr(d_c), _lib.ptr(rd_c), n, s, c, float(tolerance),
-                 float(deta_w), _lib.ptr(part, u8))
-        head = int(ctx.lib.dmnerf_penalizer_state_bytes())
-        heads = all_gather(part[:head], group)
-        state = torch.empty(head, device=raw.device, dtype=u8)
-        loss = torch.empty(1, device=raw.device, dtype=torch.float32)
-        ctx.call("dmnerf_penalizer_merge", _lib.ptr(heads, u8), heads.shape[0], c, _lib.ptr(state, u8), _lib.ptr(loss))
-        fctx.save_for_backward(raw_c, z_c, d_c, rd_c, state)
-        fctx.cfg = (float(tolerance), float(deta_w))
-        return loss
-
-    @staticmethod
-    def backward(fctx, g_loss):
-        raw_c, z_c, d_c, rd_c, state = fctx.saved_tensors
-        n, s, c = raw_c.shape
-        d_raw = torch.empty_like(raw_c)
-        g = g_loss.detach().reshape(-1)[:1].contiguous().float()
-        get_context(raw_c.device).call("dmnerf_penalizer_backward", _lib.ptr(raw_c), _lib.ptr(z_c), _lib.ptr(d_c), _lib.ptr(rd_c), n, s,
-                                       c, fctx.cfg[0], fctx.cfg[1], _lib.ptr(state, torch.uint8), _lib.ptr(g), _lib.ptr(d_raw), 0)
-        return d_raw, None, None, None, None, None, None
-
-
 def ins_penalizer_sharded(raw, z_vals, depth, rays_d, args, group=None):
     """penalizer.ins_penalizer over the whole batch (its mask populations count the samples of every rank) from this rank's
     rows: the loss [1] of the whole batch on every rank.  The penalizer needs no global ray count: its normalisers are the
     merged populations."""
-    return _PenSharded.apply(raw, z_vals, depth[..., None].detach(), rays_d, args.tolerance, args.deta_w, group)
+    return _Penalizer.apply(raw, z_vals, depth[..., None].detach(), rays_d, args.tolerance, args.deta_w, group)
 
 
 # ----------------------------------------------------------------------------------------------------------------- colour loss

@@ -1,7 +1,8 @@
 """Multi-GPU plumbing for the render path (SURVEY.md 8e): rays are independent units, so a frame (or a
 trajectory) is split into contiguous ray ranges per rank with the weights replicated, each rank renders its
 slab with the fused kernels, and ONE all-gather of the packed image slabs assembles the result on every rank.
-No collective sits on the data path of the kernels themselves."""
+No collective sits on the data path of the kernels themselves.  world_of / all_gather / all_reduce_sum_ are the collectives
+of the training losses and of data-parallel training: one process (no process group) is world 1, where they do nothing."""
 import torch
 
 
@@ -13,6 +14,52 @@ def shard_range(n_items, world, rank, multiple=1):
     lo = min(rank * per, n_items)
     hi = min(lo + per, n_items)
     return lo, hi, per
+
+
+def world_of(group=None):
+    """(world size, rank) of `group`; (1, 0) when torch.distributed is not initialised (one process)."""
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized()):
+        return 1, 0
+    return dist.get_world_size(group), dist.get_rank(group)
+
+
+def _nccl(group):
+    import torch.distributed as dist
+    return dist.get_backend(group) == "nccl"
+
+
+def all_gather(t, group=None):
+    """[W, *t.shape] on t's device, rank order.  NCCL gathers device tensors; gloo has no CUDA all-gather, so a gloo group is
+    staged through host memory."""
+    world, _ = world_of(group)
+    if world == 1:
+        return t[None]
+    import torch.distributed as dist
+    t = t.contiguous()
+    if _nccl(group):
+        out = t.new_empty((world,) + tuple(t.shape))
+        dist.all_gather_into_tensor(out, t, group=group)
+        return out
+    host = t.cpu()
+    parts = [torch.empty_like(host) for _ in range(world)]
+    dist.all_gather(parts, host, group=group)
+    return torch.stack(parts).to(t.device)
+
+
+def all_reduce_sum_(t, group=None):
+    """In-place sum of `t` over the ranks (staged through host memory for gloo)."""
+    world, _ = world_of(group)
+    if world == 1:
+        return t
+    import torch.distributed as dist
+    if _nccl(group):
+        dist.all_reduce(t, group=group)
+    else:
+        host = t.cpu()
+        dist.all_reduce(host, group=group)
+        t.copy_(host)
+    return t
 
 
 IMAGE_KEYS = ("rgb_fine", "depth_fine", "acc_fine", "ins_fine")

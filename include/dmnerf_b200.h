@@ -28,7 +28,7 @@ extern "C" {
 #define DMNERF_API
 #endif
 
-#define DMNERF_ABI_VERSION 1
+#define DMNERF_ABI_VERSION 2
 #define DMNERF_N_PARAMS 30          /* tensors in DM_NeRF.state_dict() order, networks/dm_nerf.py:65-78 */
 #define DMNERF_CH_POS 63            /* get_embedder(10): 3 + 3*2*10, networks/dm_nerf.py:41-55 */
 #define DMNERF_CH_DIR 27            /* get_embedder(4) */
@@ -139,42 +139,41 @@ DMNERF_API int dmnerf_get_rays_at_dev(const float* K_host, const float* c2w_dev,
  * NOT numpy's random stream). */
 DMNERF_API int dmnerf_select_pixels(uint64_t seed, int H, int W, int64_t n, int64_t* pixels, void* stream);
 
-/* Hungarian-matched instance loss, networks/evaluator.py:19-74 (ins_criterion / hungarian; train_dmsr.py:38-45).
+/* Hungarian-matched instance loss, networks/evaluator.py:19-74 (ins_criterion / hungarian; train_dmsr.py:38-45).  Every sum runs
+ * in an order fixed by the sizes alone (no floating-point atomics), so the losses and gradients are reproducible bit for bit.
  * dmnerf_hungarian_costs: pred [N,ins_num] (rendered instance probabilities), gt_row [N] (int32: index of the ray's label among
- * the sorted distinct labels of the batch, evaluator.py:21-25) -> cost_ce, cost_siou [ins_num,ins_num] (row = ground-truth
- * object, column = prediction channel; evaluator.py:60-67) plus the sums the backward needs: tp [ins_num,ins_num],
- * col_sum [ins_num] (sum_n pred), row_count [ins_num].  The assignment (scipy linear_sum_assignment, evaluator.py:45-47) runs on
- * the host on the [valid x ins_num] corner of cost_ce + cost_siou, as in the reference.
- * dmnerf_ins_loss_backward: d_pred [N,ins_num] = g[0] d valid_ce + g[1] d invalid_ce + g[2] d valid_siou (evaluator.py:27-36);
- * row_of_col [ins_num] (DEVICE int32) = matched ground-truth row of every prediction channel or -1; g_losses = 3 DEVICE floats. */
-DMNERF_API int dmnerf_hungarian_costs(const float* pred, const int32_t* gt_row, int64_t n, int ins_num, float* cost_ce,
-                                      float* cost_siou, float* tp, float* col_sum, float* row_count, void* stream);
-DMNERF_API int dmnerf_ins_loss_backward(const float* pred, const int32_t* gt_row, int64_t n, int ins_num,
-                                        const int32_t* row_of_col, int n_valid, const float* tp, const float* col_sum,
-                                        const float* row_count, const float* g_losses, float* d_pred, void* stream);
-
-/* The same loss with the assignment ON THE DEVICE: no device->host hop in the training iteration (the reference's
- * valid_scores.cpu() + scipy call, evaluator.py:43-45, is its last synchronisation point).
+ *   the sorted distinct labels of the batch, evaluator.py:21-25) -> cost_ce, cost_siou [ins_num,ins_num] (row = ground-truth
+ *   object, column = prediction channel; evaluator.py:60-67) plus the sums the backward needs: tp [ins_num,ins_num],
+ *   col_sum [ins_num] (sum_n pred), row_count [ins_num].  The assignment (scipy linear_sum_assignment, evaluator.py:45-47) runs
+ *   either on the host on the [valid x ins_num] corner of cost_ce + cost_siou, as in the reference, or on the device:
  * dmnerf_ins_label_rows: labels [N] (int32 object ids in [0, 65536)) -> gt_row [N] = rank of the ray's label among the distinct
  *   labels of the batch (torch.unique order, evaluator.py:21-25) and n_valid[0] = their number (DEVICE int32; -1 when a label is
  *   out of range or there are more distinct labels than ins_num).
  * dmnerf_hungarian_assign: scipy.optimize.linear_sum_assignment's algorithm (shortest augmenting paths, fp64 duals, scipy's tie
  *   rule) on rows 0..n_valid-1 of cost_ce + cost_siou -> row_of_col [ins_num] (matched row or -1) and
- *   losses[3] = { valid_ce, invalid_ce, valid_siou } (evaluator.py:27-36; NaN after rejected labels).
- * dmnerf_ins_loss_backward_dev: dmnerf_ins_loss_backward with n_valid read from the device (zero gradient after rejected labels).
+ *   losses[3] = { valid_ce, invalid_ce, valid_siou } (evaluator.py:27-36; NaN after rejected labels).  With these two the
+ *   training iteration has no device->host hop (the reference's valid_scores.cpu() + scipy call, evaluator.py:43-45, is its
+ *   last synchronisation point).
+ * dmnerf_ins_loss_backward: d_pred [n,ins_num] = g[0] d valid_ce + g[1] d invalid_ce + g[2] d valid_siou (evaluator.py:27-36)
+ *   for n rows of a batch of n_global rays (n = n_global in one process); row_of_col [ins_num] (DEVICE int32) = matched
+ *   ground-truth row of every prediction channel or -1; n_valid[0] (DEVICE int32) = the number of distinct labels (zero gradient
+ *   when it is below 1: rejected labels); g_losses = 3 DEVICE floats.
  * dmnerf_ins_status_take: returns and clears the error word of rejected labels (0 = none; mapped host memory, no synchronisation). */
+DMNERF_API int dmnerf_hungarian_costs(const float* pred, const int32_t* gt_row, int64_t n, int ins_num, float* cost_ce,
+                                      float* cost_siou, float* tp, float* col_sum, float* row_count, void* stream);
 DMNERF_API int dmnerf_ins_label_rows(const int32_t* labels, int64_t n, int ins_num, int32_t* gt_row, int32_t* n_valid, void* stream);
 DMNERF_API int dmnerf_hungarian_assign(const float* cost_ce, const float* cost_siou, const float* col_sum, const int32_t* n_valid,
                                        int64_t n, int ins_num, int32_t* row_of_col, float* losses, void* stream);
-DMNERF_API int dmnerf_ins_loss_backward_dev(const float* pred, const int32_t* gt_row, int64_t n, int ins_num,
-                                            const int32_t* row_of_col, const int32_t* n_valid, const float* tp, const float* col_sum,
-                                            const float* row_count, const float* g_losses, float* d_pred, void* stream);
+DMNERF_API int dmnerf_ins_loss_backward(const float* pred, const int32_t* gt_row, int64_t n, int64_t n_global, int ins_num,
+                                        const int32_t* row_of_col, const int32_t* n_valid, const float* tp, const float* col_sum,
+                                        const float* row_count, const float* g_losses, float* d_pred, void* stream);
 DMNERF_API int dmnerf_ins_status_take(void);
 
 /* The same loss over a batch split into W contiguous shards (one per process, dmnerf_b200.distributed): each shard computes
  * partials, the caller all-gathers them, and every shard merges the W buffers in shard order, so every shard feeds bit-identical
- * inputs to dmnerf_hungarian_assign (which is passed the global N).  Every sum runs in an order fixed by the sizes alone: no
- * floating-point atomics.
+ * inputs to dmnerf_hungarian_assign (which is passed the global N) and then calls dmnerf_ins_loss_backward for its own rows.
+ * dmnerf_hungarian_costs is the one-shard case: it equals dmnerf_hungarian_partials followed by dmnerf_hungarian_costs_merged
+ * with world = 1 bit for bit.
  * dmnerf_ins_label_bitmap: labels [n] -> bitmap [DMNERF_LABEL_WORDS] (DEVICE uint32): words 0..2047 mark the label values
  *   [0, 65536) present in the shard, word 2048 is 1 when a label is out of range (also posted to the status word: 701).
  * dmnerf_ins_label_rows_merged: bitmaps [world, DMNERF_LABEL_WORDS] (the gathered bitmaps, rank order) and the shard's labels [n]
@@ -185,8 +184,7 @@ DMNERF_API int dmnerf_ins_status_take(void);
  *   A[p] = sum log(1 - pred[:,p] + 1e-8), S[p] = sum pred[:,p], and over the rays of row g: B = sum log(pred + 1e-8),
  *   C = sum log(1 - pred + 1e-8), TP = sum pred, cnt = ray count.
  * dmnerf_hungarian_costs_merged: partials [world, 3 k (k + 1)] added in shard order -> cost_ce, cost_siou, tp, col_sum, row_count
- *   exactly as dmnerf_hungarian_costs computes them from those sums, normalised by n_global.
- * dmnerf_ins_loss_backward_shard: dmnerf_ins_loss_backward_dev for the shard's n rows of a batch of n_global rays. */
+ *   exactly as dmnerf_hungarian_costs computes them from those sums, normalised by n_global. */
 #define DMNERF_LABEL_WORDS 2049
 DMNERF_API int dmnerf_ins_label_bitmap(const int32_t* labels, int64_t n, uint32_t* bitmap, void* stream);
 DMNERF_API int dmnerf_ins_label_rows_merged(const uint32_t* bitmaps, int world, const int32_t* labels, int64_t n, int ins_num,
@@ -195,9 +193,6 @@ DMNERF_API int dmnerf_hungarian_partials(const float* pred, const int32_t* gt_ro
                                          void* stream);
 DMNERF_API int dmnerf_hungarian_costs_merged(const double* partials, int world, int64_t n_global, int ins_num, float* cost_ce,
                                              float* cost_siou, float* tp, float* col_sum, float* row_count, void* stream);
-DMNERF_API int dmnerf_ins_loss_backward_shard(const float* pred, const int32_t* gt_row, int64_t n, int64_t n_global, int ins_num,
-                                              const int32_t* row_of_col, const int32_t* n_valid, const float* tp, const float* col_sum,
-                                              const float* row_count, const float* g_losses, float* d_pred, void* stream);
 
 /* Coarse depths, networks/render.py:40-47: z_out[n, i] = z_in row (shared when z_row_stride = 0), jittered inside its
  * stratum by t_rand [N,S] when given. */
@@ -266,27 +261,23 @@ DMNERF_API int dmnerf_exchanger(float* ori_raw, const float* const* tar_raws, co
                                 int64_t* tar_label, void* stream);
 
 /* "Emptiness" regulariser on the per-sample object logits: emptiness_penalizer / ins_penalizer, networks/penalizer.py:5-62
- * (train_dmsr.py:53-60).  raw [N,S,C], z_vals [N,S], depth [N] (the rendered depth map, treated as a constant),
- * rays_d [N,3] -> loss[1] (device).  `state` is caller-provided device scratch of dmnerf_penalizer_state_bytes() bytes that
- * carries the mask populations from the forward to the backward call.  Backward (g_loss is a DEVICE scalar): accumulate == 0
- * writes d_raw = g_loss[0] * dL/draw for EVERY channel (zeros in channels 0..3: no zero-fill needed); accumulate != 0 adds the
- * gradient to channels 4.. and leaves channels 0..3 untouched. */
+ * (train_dmsr.py:53-60).  raw [n,S,C], z_vals [n,S], depth [n] (the rendered depth map, treated as a constant),
+ * rays_d [n,3] -> loss[1] (device).  `partials` is caller-provided device scratch of dmnerf_penalizer_partials_bytes(n, S, C)
+ * bytes.  The forward writes the mask populations and masked sums, summed in an order fixed by the sizes, into its head (the
+ * first dmnerf_penalizer_state_bytes() bytes), which carries them to the backward call.  Backward (g_loss is a DEVICE scalar):
+ * accumulate == 0 writes d_raw = g_loss[0] * dL/draw for EVERY channel (zeros in channels 0..3: no zero-fill needed);
+ * accumulate != 0 adds the gradient to channels 4.. and leaves channels 0..3 untouched.
+ * Over a batch split into W shards, every shard runs the forward on its rows (and ignores its loss), and
+ * dmnerf_penalizer_merge adds the W gathered heads (`states`, W * dmnerf_penalizer_state_bytes() bytes, rank order) in rank
+ * order -> `state` (the backward's state for the whole batch; the backward on it gives the shard's gradient) and loss[1].  At
+ * W = 1 the merge gives the forward's own head and loss bit for bit. */
 DMNERF_API int64_t dmnerf_penalizer_state_bytes(void);
+DMNERF_API int64_t dmnerf_penalizer_partials_bytes(int64_t n, int s, int c);
 DMNERF_API int dmnerf_penalizer_forward(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,
-                                        int s, int c, float tolerance, float deta_w, void* state, float* loss, void* stream);
+                                        int s, int c, float tolerance, float deta_w, void* partials, float* loss, void* stream);
 DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,
                                          int s, int c, float tolerance, float deta_w, const void* state, const float* g_loss,
                                          float* d_raw, int accumulate, void* stream);
-
-/* The penalizer over a batch split into W shards.  dmnerf_penalizer_partials writes the shard's mask populations and masked sums,
- * unfinalised and summed in an order fixed by the sizes, into the head (the first dmnerf_penalizer_state_bytes() bytes) of
- * `partials`, a device buffer of dmnerf_penalizer_partials_bytes(n, s, c) bytes (the rest is per-block scratch).
- * dmnerf_penalizer_merge: the W gathered heads (`states`, W * dmnerf_penalizer_state_bytes() bytes, rank order), added in rank
- * order -> `state` (a dmnerf_penalizer_backward state for the whole batch; that call then gives the shard's gradient) and
- * loss[1]. */
-DMNERF_API int64_t dmnerf_penalizer_partials_bytes(int64_t n, int s, int c);
-DMNERF_API int dmnerf_penalizer_partials(const float* raw, const float* z_vals, const float* depth, const float* rays_d, int64_t n,
-                                         int s, int c, float tolerance, float deta_w, void* partials, void* stream);
 DMNERF_API int dmnerf_penalizer_merge(const void* states, int world, int c, void* state, float* loss, void* stream);
 
 /* dm_nerf(), networks/render.py:31-96, whole per-ray pipeline on device buffers. */

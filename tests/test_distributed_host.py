@@ -7,8 +7,8 @@ import pytest
 import torch
 
 from dmnerf_b200 import _lib
-from dmnerf_b200.distributed import img2mse_sharded, instance_rows, world_of
-from dmnerf_b200.parallel import shard_range
+from dmnerf_b200.distributed import img2mse_sharded, instance_rows
+from dmnerf_b200.parallel import shard_range, world_of
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -66,13 +66,15 @@ def test_colour_loss_at_world_one_is_img2mse_with_its_gradient():
     assert torch.allclose(x.grad, x2.grad, rtol=1e-5, atol=1e-9)
 
 
-def test_sharded_loss_entry_points_are_declared_and_bound():
+def test_loss_entry_points_are_declared_and_bound_and_the_removed_ones_are_gone():
     header = open(os.path.join(ROOT, "include", "dmnerf_b200.h")).read()
     names = ["dmnerf_ins_label_bitmap", "dmnerf_ins_label_rows_merged", "dmnerf_hungarian_partials", "dmnerf_hungarian_costs_merged",
-             "dmnerf_ins_loss_backward_shard", "dmnerf_penalizer_partials_bytes", "dmnerf_penalizer_partials", "dmnerf_penalizer_merge"]
+             "dmnerf_ins_loss_backward", "dmnerf_penalizer_partials_bytes", "dmnerf_penalizer_forward", "dmnerf_penalizer_merge"]
     for name in names:
         assert re.search(r"DMNERF_API\s+[\w\s\*]+?\b%s\s*\(" % name, header), name
         assert name in _lib.PROTOTYPES, name
     assert re.search(r"#define DMNERF_LABEL_WORDS %d\b" % _lib.LABEL_WORDS, header)
     # n and n_global of the shard's backward are both 64-bit
-    assert _lib.PROTOTYPES["dmnerf_ins_loss_backward_shard"][1][2:4] == [_lib.C.c_int64, _lib.C.c_int64]
+    assert _lib.PROTOTYPES["dmnerf_ins_loss_backward"][1][2:4] == [_lib.C.c_int64, _lib.C.c_int64]
+    for gone in ("dmnerf_ins_loss_backward_dev", "dmnerf_ins_loss_backward_shard", "dmnerf_penalizer_partials"):
+        assert gone not in _lib.PROTOTYPES and not re.search(r"\b%s\s*\(" % gone, header), gone

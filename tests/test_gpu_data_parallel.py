@@ -73,7 +73,9 @@ def _batch(n, k, seed, n_labels):
 @pytest.mark.parametrize("crop", [False, True])
 @pytest.mark.parametrize("world", [2, 3])
 @pytest.mark.parametrize("k", [13, 93])
-def test_sharded_instance_and_penalizer_kernels_match_the_unsharded_ones(k, world, crop):
+def test_sharded_instance_and_penalizer_kernels_match_the_one_shard_entries(k, world, crop):
+    """W shards of the instance loss and the penalizer against the one-process entries (dmnerf_hungarian_costs, ins_criterion,
+    emptiness_penalizer): the shards' label ranks, costs, matching, losses and gradients."""
     from dmnerf_b200.distributed import instance_rows
     from dmnerf_b200.engine import get_context
     from dmnerf_b200.evaluator import _costs, ins_criterion
@@ -114,7 +116,7 @@ def test_sharded_instance_and_penalizer_kernels_match_the_unsharded_ones(k, worl
     g3 = torch.ones(3, device=DEV)
     d = torch.empty_like(pred)
     for (lo, hi), gr in zip(pieces, rows):
-        ctx.call("dmnerf_ins_loss_backward_shard", _lib.ptr(pred[lo:hi]), _i32(gr), hi - lo, m, k, _i32(assign[1][0]), _i32(nvs[0]),
+        ctx.call("dmnerf_ins_loss_backward", _lib.ptr(pred[lo:hi]), _i32(gr), hi - lo, m, k, _i32(assign[1][0]), _i32(nvs[0]),
                  _lib.ptr(c["tp"]), _lib.ptr(c["col_sum"]), _lib.ptr(c["row_count"]), _lib.ptr(g3), _lib.ptr(d[lo:hi]))
     assert rel_l2(d.cpu(), p.grad.cpu()) <= 1e-6
     # penalizer over the shards of the whole batch (samples of every ray)
@@ -129,10 +131,11 @@ def test_sharded_instance_and_penalizer_kernels_match_the_unsharded_ones(k, worl
     pen.backward()
     head = int(ctx.lib.dmnerf_penalizer_state_bytes())
     parts = []
+    shard_loss = torch.empty(1, device=DEV)
     for lo, hi in shards:
         buf = torch.empty(int(ctx.lib.dmnerf_penalizer_partials_bytes(hi - lo, S, C)), device=DEV, dtype=torch.uint8)
-        ctx.call("dmnerf_penalizer_partials", _lib.ptr(raw[lo:hi]), _lib.ptr(z[lo:hi]), _lib.ptr(depth[lo:hi, 0].contiguous()),
-                 _lib.ptr(rays_d[lo:hi]), hi - lo, S, C, 0.05, 0.05, _lib.ptr(buf, torch.uint8))
+        ctx.call("dmnerf_penalizer_forward", _lib.ptr(raw[lo:hi]), _lib.ptr(z[lo:hi]), _lib.ptr(depth[lo:hi, 0].contiguous()),
+                 _lib.ptr(rays_d[lo:hi]), hi - lo, S, C, 0.05, 0.05, _lib.ptr(buf, torch.uint8), _lib.ptr(shard_loss))
         parts.append(buf[:head])
     state = torch.empty(head, device=DEV, dtype=torch.uint8)
     ploss = torch.empty(1, device=DEV)
@@ -146,6 +149,70 @@ def test_sharded_instance_and_penalizer_kernels_match_the_unsharded_ones(k, worl
                  _lib.ptr(rays_d[lo:hi]), hi - lo, S, C, 0.05, 0.05, _lib.ptr(state, torch.uint8), _lib.ptr(one), _lib.ptr(d_raw[lo:hi]), 0)
     assert rel_l2(d_raw.cpu(), r.grad.cpu()) <= 1e-6
     ctx.sync_check()
+
+
+@pytest.mark.parametrize("k", [13, 93, 128])
+def test_one_process_costs_are_the_one_shard_merge_bit_for_bit(k):
+    """dmnerf_hungarian_costs finalises the partials kernel's sums inside its own launch: every output equals
+    dmnerf_hungarian_partials followed by dmnerf_hungarian_costs_merged at world 1, bit for bit, with unlabelled rays (row -1)
+    and every ray count class of the kernel's 32-row chunks and 8 warps."""
+    from dmnerf_b200.engine import get_context
+    from dmnerf_b200.evaluator import _cost_buffers, _cost_ptrs, _costs
+    ctx = get_context(DEV)
+    for n in (1, 2, 31, 32, 33, 255, 256, 257, 1000, 2048, 3071, 3072):
+        gen = torch.Generator().manual_seed(n * 131 + k)
+        pred = torch.softmax(3 * torch.randn(n, k, generator=gen), -1).to(DEV).contiguous()
+        gt_row = torch.randint(-1, min(k, 9), (n,), generator=gen).to(torch.int32).to(DEV)
+        one = _costs(pred, gt_row)
+        part = torch.empty(3 * k * (k + 1), device=DEV, dtype=torch.float64)
+        ctx.call("dmnerf_hungarian_partials", _lib.ptr(pred), _i32(gt_row), n, k, _lib.ptr(part, torch.float64))
+        merged = _cost_buffers(k, DEV)
+        ctx.call("dmnerf_hungarian_costs_merged", _lib.ptr(part, torch.float64), 1, n, k, *_cost_ptrs(merged))
+        for key in one:
+            assert torch.equal(one[key], merged[key]), (n, key)
+
+
+@pytest.mark.parametrize("n, s, k", [(1, 1, 13), (37, 64, 13), (300, 64, 59), (1024, 192, 93), (200, 40, 127)])
+def test_penalizer_forward_is_the_one_shard_merge_bit_for_bit(n, s, k):
+    """The penalizer forward's own loss and head equal dmnerf_penalizer_merge of that head at world 1, bit for bit, up to
+    thousands of blocks (1024 x 192 samples at ins_num 93: 3072 block slots reduced by the last block)."""
+    from dmnerf_b200.engine import get_context
+    ctx = get_context(DEV)
+    C = 4 + k + 1
+    gen = torch.Generator().manual_seed(n + s + k)
+    raw = (2 * torch.randn(n, s, C, generator=gen)).to(DEV)
+    z = (4.0 + 11.0 * torch.sort(torch.rand(n, s, generator=gen), -1).values).to(DEV)
+    depth = (5.0 + 9.0 * torch.rand(n, generator=gen)).to(DEV)
+    rays_d = torch.randn(n, 3, generator=gen).to(DEV)
+    u8 = torch.uint8
+    part = torch.empty(int(ctx.lib.dmnerf_penalizer_partials_bytes(n, s, C)), device=DEV, dtype=u8)
+    loss = torch.empty(1, device=DEV)
+    ctx.call("dmnerf_penalizer_forward", _lib.ptr(raw), _lib.ptr(z), _lib.ptr(depth), _lib.ptr(rays_d), n, s, C, 0.05, 0.05,
+             _lib.ptr(part, u8), _lib.ptr(loss))
+    head = int(ctx.lib.dmnerf_penalizer_state_bytes())
+    state = torch.empty(head, device=DEV, dtype=u8)
+    merged = torch.empty(1, device=DEV)
+    ctx.call("dmnerf_penalizer_merge", _lib.ptr(part[:head], u8), 1, C, _lib.ptr(state, u8), _lib.ptr(merged))
+    assert torch.equal(loss, merged) and bool(torch.isfinite(loss).all())
+    assert torch.equal(part[:32], state[:32])                   # populations and sums (the block counter is the forward's own)
+
+
+def test_ins_criterion_and_its_one_process_sharded_form_agree_bit_for_bit():
+    """ins_criterion and ins_criterion_sharded(..., n_global = n) in one process run the same Function: bitwise-equal losses,
+    matchings and gradients."""
+    from dmnerf_b200.distributed import ins_assignment_sharded, ins_criterion_sharded
+    from dmnerf_b200.evaluator import ins_assignment, ins_criterion
+    n, k = 3072, 93
+    pred, labels = _batch(n, k, 17, 40)
+    got = []
+    for fn in (ins_criterion, lambda p, lab, kk: ins_criterion_sharded(p, lab, kk, n)):
+        p = pred.clone().requires_grad_(True)
+        parts = fn(p, labels, k)
+        parts[0].backward()
+        got.append(([x.detach() for x in parts], p.grad))
+    for a, b in zip(got[0][0] + [got[0][1]], got[1][0] + [got[1][1]]):
+        assert torch.equal(a, b)
+    assert torch.equal(ins_assignment(pred, labels, k)[0], ins_assignment_sharded(pred, labels, k, n)[4])
 
 
 @pytest.mark.parametrize("case", ["out_of_range", "too_many"])

@@ -20,14 +20,14 @@ def lib():
     return _lib.load()
 
 
-def test_abi_exports_every_declared_symbol(lib):
+def test_abi_version_2_exports_every_declared_symbol(lib):
     hdr = open(os.path.join(ROOT, "include", "dmnerf_b200.h")).read()
     declared = set(re.findall(r"DMNERF_API[^;(]*?\b(dmnerf_\w+)\s*\(", hdr))
     assert len(declared) >= 14
     assert declared == set(_lib.PROTOTYPES), declared ^ set(_lib.PROTOTYPES)
     for name in declared:
         assert hasattr(lib, name)
-    assert lib.dmnerf_abi_version() == 1
+    assert lib.dmnerf_abi_version() == 2
     assert ctypes.sizeof(_lib.RenderIO) == 20 * 8
 
 
