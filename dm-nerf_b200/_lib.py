@@ -16,10 +16,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DMNERF_LIB_PATH: diagnostics builds of the same ABI (tools/kprof.py); the default is the in-tree product library
 LIB_PATH = os.environ.get("DMNERF_LIB_PATH") or os.path.join(_HERE, "lib", "libdmnerf_b200.so")
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 N_PARAMS = 30
 IMPL_AUTO, IMPL_SIMT, IMPL_UMMA, IMPL_UMMA_F16 = 0, 1, 2, 3
-FLAG_PERTURB, FLAG_WANT_RAW, FLAG_KEEP_INS = 1, 2, 4
+FLAG_PERTURB, FLAG_WANT_RAW, FLAG_KEEP_INS, FLAG_SELECT = 1, 2, 4, 8
 LABEL_WORDS = 2049           # DMNERF_LABEL_WORDS
 
 _f32p = C.c_void_p
@@ -33,7 +33,7 @@ class RenderIO(C.Structure):
         ("rgb_coarse", _f32p), ("rgb_fine", _f32p), ("depth_coarse", _f32p), ("depth_fine", _f32p),
         ("acc_coarse", _f32p), ("acc_fine", _f32p), ("ins_coarse", _f32p), ("ins_fine", _f32p),
         ("z_vals_coarse", _f32p), ("z_vals_fine", _f32p), ("weights_coarse", _f32p), ("weights_fine", _f32p),
-        ("raw_coarse", _f32p), ("raw_fine", _f32p),
+        ("raw_coarse", _f32p), ("raw_fine", _f32p), ("keep", C.c_uint32 * 4),
     ]
 
 
@@ -49,8 +49,8 @@ PROTOTYPES = {
     "dmnerf_mlp_forward": (C.c_int, [C.c_void_p, C.c_int, _f32p, C.c_int64, _f32p, C.c_int, C.c_void_p]),
     "dmnerf_mlp_forward_rays": (C.c_int, [C.c_void_p, C.c_int, _f32p, _f32p, _f32p, C.c_int64, C.c_int, _f32p, C.c_int,
                                           C.c_void_p]),
-    "dmnerf_composite": (C.c_int, [_f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_int, _f32p, _f32p, _f32p, _f32p,
-                                   _f32p, C.c_void_p]),
+    "dmnerf_composite": (C.c_int, [_f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint32), _f32p, _f32p,
+                                   _f32p, _f32p, _f32p, C.c_void_p]),
     "dmnerf_sample_pdf": (C.c_int, [_f32p, _f32p, C.c_int64, C.c_int, C.c_int, _f32p, _f32p, C.c_void_p]),
     "dmnerf_sort_concat": (C.c_int, [_f32p, _f32p, C.c_int64, C.c_int, C.c_int, _f32p, C.c_void_p]),
     "dmnerf_get_rays": (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int, C.c_int, _f32p, _f32p, C.c_void_p]),
@@ -104,7 +104,7 @@ PROTOTYPES = {
     "dmnerf_mesh_grid_points": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_int64, C.c_int64, _f32p,
                                           C.c_void_p]),
     "dmnerf_mesh_occupancy": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_float,
-                                        C.c_int64, _f32p, C.c_void_p]),
+                                        C.c_int64, C.POINTER(C.c_uint32), _f32p, C.c_void_p, C.c_void_p]),
     "dmnerf_mesh_mc_count": (C.c_int, [C.c_void_p, _f32p, C.c_int, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_mesh_mc_emit": (C.c_int, [C.c_void_p, _f32p, C.c_int, C.c_int, C.c_int, C.c_float, _f32p, C.c_void_p, C.c_void_p]),
     "dmnerf_mesh_to_scene": (C.c_int, [_f32p, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, _f32p, C.c_void_p]),
@@ -121,15 +121,6 @@ PROTOTYPES = {
     "dmnerf_calculate_ap": (C.c_int, [_f32p, _f32p, C.c_int, C.c_int, _f32p, C.c_void_p]),
     "dmnerf_ins_dense_rows": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "dmnerf_label_colors": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "dmnerf_composite_objects": (C.c_int, [_f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint32), _f32p,
-                                           _f32p, _f32p, _f32p, _f32p, C.c_void_p]),
-    "dmnerf_render_forward_objects": (C.c_int, [C.c_void_p, C.POINTER(RenderIO), C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
-                                                C.POINTER(C.c_uint32), C.c_void_p]),
-    "dmnerf_render_frame_objects_host": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int, C.c_int, C.c_float,
-                                                   C.c_float, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
-                                                   C.POINTER(C.c_uint32), C.POINTER(RenderIO), C.c_void_p]),
-    "dmnerf_mesh_occupancy_objects": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_float,
-                                                C.c_int64, C.POINTER(C.c_uint32), _f32p, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -142,8 +142,8 @@ class RenderFunction(torch.autograd.Function):
             ctx.call("dmnerf_mlp_forward_train", ctx.handle, net, None, _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(o[zkey]), n * ns,
                      ns, _lib.ptr(raw), _lib.ptr(acts), impl)
             rgb, w, depth, acc, ins = e(n, 3), e(n, ns), e(n), e(n), e(n, ins_num)
-            ctx.call("dmnerf_composite", _lib.ptr(raw), _lib.ptr(o[zkey]), _lib.ptr(rays_d), n, ns, Cc, 0, _lib.ptr(rgb), _lib.ptr(w),
-                     _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc))
+            ctx.call("dmnerf_composite", _lib.ptr(raw), _lib.ptr(o[zkey]), _lib.ptr(rays_d), n, ns, Cc, 0, None, _lib.ptr(rgb),
+                     _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc))
             o["raw_" + tag], o["rgb_" + tag], o["weights_" + tag] = raw, rgb, w
             o["depth_" + tag], o["acc_" + tag], o["ins_" + tag] = depth, acc, ins
             saved.append(acts)

@@ -39,12 +39,16 @@ struct Scratch {
   void release() { if (ptr) cudaFree(ptr); ptr = nullptr; cap = 0; }
 };
 
-// A host-side object selection mask (4 words) -> ObjMask; only labels 0 .. n_labels - 1 may be set.
-static int object_mask(const uint32_t* keep_host, int n_labels, ObjMask& m, const char* who) {
-  DMN_CHECK(keep_host != nullptr, "%s: the object mask is NULL (pass 4 words)", who);
+// An entry point's object selection: keep_host (4 host words, NULL = no selection) -> keep = &m, or NULL.  Only labels
+// 0 .. n_labels - 1 may be set; n_labels = 0 means no network is bound to label the samples with.
+static int object_mask(const uint32_t* keep_host, int n_labels, ObjMask& m, const ObjMask*& keep, const char* who) {
+  keep = nullptr;
+  if (!keep_host) return 0;
+  DMN_CHECK(n_labels > 0, "%s: an object selection needs the network(s) bound with dmnerf_set_weights (one ins_num)", who);
   for (int b = n_labels; b < 128; ++b)
     DMN_CHECK(!((keep_host[b >> 5] >> (b & 31)) & 1u), "%s: object mask keeps label %d, outside [0, %d]", who, b, n_labels - 1);
   for (int i = 0; i < 4; ++i) m.w[i] = keep_host[i];
+  keep = &m;
   return 0;
 }
 
@@ -73,6 +77,14 @@ struct dmnerf_ctx {
   cudaEvent_t ev_in[HOST_PARTS] = {}, ev_done[HOST_PARTS] = {}, ev_start = nullptr;
   dmnerf_ctx() { memset(net, 0, sizeof(net)); }
 };
+
+// The selection of a render call: io->keep with DMNERF_FLAG_SELECT, over labels 0 .. ins_num of the coarse / fine pair (both
+// bound with one ins_num, else no labels).
+static int render_mask(const dmnerf_ctx* ctx, const dmnerf_render_io* io, int flags, ObjMask& m, const ObjMask*& keep,
+                       const char* who) {
+  const bool pair = ctx && ctx->net[0].bound && ctx->net[1].bound && ctx->net[0].ins_num == ctx->net[1].ins_num;
+  return object_mask((flags & DMNERF_FLAG_SELECT) && io ? io->keep : nullptr, pair ? ctx->net[0].ins_num + 1 : 0, m, keep, who);
+}
 
 extern "C" {
 
@@ -155,22 +167,27 @@ static int f16_verdict(dmnerf_ctx* ctx, int rc, int impl, void* stream) {
   return dmnerf_sync_check(ctx, stream);
 }
 
+// The network a call on slots net0 .. net1 runs: impl range-checked, DMNERF_IMPL_AUTO resolved to the tensor-core kernel when
+// every slot has its image (else SIMT), and for DMNERF_IMPL_UMMA_F16 every slot's fp16 image packed.
+static int resolve_impl(dmnerf_ctx* ctx, int& impl, int net0, int net1, cudaStream_t st, const char* who) {
+  DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA_F16, "%s: unknown impl %d", who, impl);
+  if (impl == DMNERF_IMPL_AUTO)
+    impl = umma_available(ctx->packed[net0]) && umma_available(ctx->packed[net1]) ? DMNERF_IMPL_UMMA : DMNERF_IMPL_SIMT;
+  for (int net = net0; impl == DMNERF_IMPL_UMMA_F16 && net <= net1; ++net)
+    if (prepare_f16(ctx, net, st)) return 1;
+  return 0;
+}
+
 static int mlp_dispatch(dmnerf_ctx* ctx, int net, const float* x, const float* ro, const float* rd, const float* z,
                         int64_t m, int s, float* out, int impl, cudaStream_t st) {
   DMN_CHECK(ctx != nullptr, "mlp: ctx is NULL");
   DMN_CHECK(net == 0 || net == 1, "mlp: net must be 0 or 1");
   DMN_CHECK(m >= 0, "mlp: negative row count");
-  DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA_F16, "mlp: unknown impl %d", impl);
   if (m == 0) return 0;
   DMN_CHECK(out != nullptr, "mlp: out is NULL");
-  if (impl == DMNERF_IMPL_UMMA_F16) {
-    if (prepare_f16(ctx, net, st)) return 1;
-    return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st, true);
-  }
-  if (impl == DMNERF_IMPL_AUTO) impl = umma_available(ctx->packed[net]) ? DMNERF_IMPL_UMMA : DMNERF_IMPL_SIMT;
-  if (impl == DMNERF_IMPL_UMMA)
-    return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st);
-  return launch_mlp_simt(ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st);
+  if (resolve_impl(ctx, impl, net, net, st, "mlp")) return 1;
+  if (impl == DMNERF_IMPL_SIMT) return launch_mlp_simt(ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st);
+  return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st, impl == DMNERF_IMPL_UMMA_F16);
 }
 
 DMNERF_API int dmnerf_mlp_forward(dmnerf_ctx* ctx, int net, const float* x, int64_t m, float* out, int impl, void* stream) {
@@ -192,31 +209,23 @@ DMNERF_API int dmnerf_mlp_forward_points(dmnerf_ctx* ctx, int net, const float* 
   DMN_CHECK(m >= 0, "mlp_forward_points: negative point count");
   DMN_CHECK(m == 0 || (pts && viewdirs && out), "mlp_forward_points: NULL buffer");
   DMN_CHECK(impl != DMNERF_IMPL_SIMT, "mlp_forward_points: the point query runs on the tensor-core kernel only");
-  DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA_F16, "mlp_forward_points: unknown impl %d", impl);
   if (m == 0) return 0;
   DMN_CHECK(umma_available(ctx->packed[net]), "mlp_forward_points: bind the network with dmnerf_set_weights first");
-  const bool f16 = impl == DMNERF_IMPL_UMMA_F16;
-  if (f16 && prepare_f16(ctx, net, (cudaStream_t)stream)) return 1;
+  if (resolve_impl(ctx, impl, net, net, (cudaStream_t)stream, "mlp_forward_points")) return 1;
   return f16_verdict(ctx, launch_mlp_umma(ctx->packed[net], ctx->net[net], nullptr, pts, viewdirs, nullptr, m, 1, out, nullptr,
-                                          (cudaStream_t)stream, f16), impl, stream);
+                                          (cudaStream_t)stream, impl == DMNERF_IMPL_UMMA_F16), impl, stream);
 }
 
 DMNERF_API int dmnerf_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all_ins,
-                     float* rgb, float* weights, float* depth, float* ins, float* acc, void* stream) {
+                                const uint32_t* keep_host, float* rgb, float* weights, float* depth, float* ins, float* acc,
+                                void* stream) {
   DMN_CHECK(n >= 0, "composite: negative ray count");
   DMN_CHECK(n == 0 || (raw && z && rays_d), "composite: NULL input");
-  return launch_composite(raw, z, rays_d, n, s, c, keep_all_ins, rgb, weights, depth, ins, acc, (cudaStream_t)stream);
-}
-
-DMNERF_API int dmnerf_composite_objects(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c,
-                                        int keep_all_ins, const uint32_t* keep_host, float* rgb, float* weights, float* depth,
-                                        float* ins, float* acc, void* stream) {
-  DMN_CHECK(n >= 0, "composite_objects: negative ray count");
-  DMN_CHECK(n == 0 || (raw && z && rays_d), "composite_objects: NULL input");
-  DMN_CHECK(c >= 5 && c <= 4 + DMNERF_MAX_INS + 1, "composite_objects: channels=%d out of range", c);
+  DMN_CHECK(c >= 5 && c <= 4 + DMNERF_MAX_INS + 1, "composite: channels=%d out of range", c);
   ObjMask m;
-  if (object_mask(keep_host, c - 4, m, "composite_objects")) return 1;
-  return launch_composite(raw, z, rays_d, n, s, c, keep_all_ins, rgb, weights, depth, ins, acc, (cudaStream_t)stream, &m);
+  const ObjMask* keep;
+  if (object_mask(keep_host, c - 4, m, keep, "composite")) return 1;
+  return launch_composite(raw, z, rays_d, n, s, c, keep_all_ins, rgb, weights, depth, ins, acc, (cudaStream_t)stream, keep);
 }
 
 DMNERF_API int dmnerf_sample_pdf(const float* bins, const float* weights, int64_t n, int n_bins, int n_samples, const float* u,
@@ -336,11 +345,9 @@ DMNERF_API int dmnerf_mlp_forward_train(dmnerf_ctx* ctx, int net, const float* x
   DMN_CHECK(out && acts, "mlp_forward_train: out / acts is NULL");
   DMN_CHECK(impl != DMNERF_IMPL_UMMA_F16, "mlp_forward_train: DMNERF_IMPL_UMMA_F16 is inference-only; training runs the exact "
             "network (DMNERF_IMPL_UMMA or DMNERF_IMPL_SIMT)");
-  DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA, "mlp_forward_train: unknown impl %d", impl);
-  if (impl == DMNERF_IMPL_AUTO) impl = umma_available(ctx->packed[net]) ? DMNERF_IMPL_UMMA : DMNERF_IMPL_SIMT;
-  if (impl == DMNERF_IMPL_UMMA)
-    return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
-  return launch_mlp_simt(ctx->net[net], x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
+  if (resolve_impl(ctx, impl, net, net, (cudaStream_t)stream, "mlp_forward_train")) return 1;
+  if (impl == DMNERF_IMPL_SIMT) return launch_mlp_simt(ctx->net[net], x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
+  return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_mlp_backward(dmnerf_ctx* ctx, int net, float* acts, const float* d_out, int64_t m, float* const* grads,
@@ -407,16 +414,13 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   const int C = 4 + ctx->net[0].ins_num + 1, F = S + NI;
   const int keep_ins = (flags & DMNERF_FLAG_KEEP_INS) ? 1 : 0;
   DMN_CUDA(cudaSetDevice(ctx->device));
+  if (resolve_impl(ctx, impl, 0, 1, st, "render_forward")) return 1;
 
   // ---- fully fused path: one launch, no intermediate tensor in HBM
-  const bool can_fuse = impl != DMNERF_IMPL_SIMT && S == 64 && NI == 128 && !io->raw_coarse && !io->raw_fine &&
-                        umma_available(ctx->packed[0]) && umma_available(ctx->packed[1]);
-  if (can_fuse) {
+  if (impl != DMNERF_IMPL_SIMT && S == 64 && NI == 128 && !io->raw_coarse && !io->raw_fine) {
     const bool prof = ctx->profiling;
-    const bool f16 = impl == DMNERF_IMPL_UMMA_F16;
-    if (f16 && (prepare_f16(ctx, 0, st) || prepare_f16(ctx, 1, st))) return 1;
     if (prof) DMN_CUDA(cudaEventRecord(ctx->ev[0], st));
-    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep, f16);
+    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep, impl == DMNERF_IMPL_UMMA_F16);
     if (rc) return rc;
     if (prof) for (int i = 1; i <= DMNERF_N_STAGES; ++i) DMN_CUDA(cudaEventRecord(ctx->ev[i], st));
     ctx->profile_valid = prof;
@@ -467,26 +471,14 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   return 0;
 }
 
-// Both networks bound with the same ins_num, and a valid mask for them.
-static int render_object_mask(const dmnerf_ctx* ctx, const uint32_t* keep_host, ObjMask& m, const char* who) {
-  DMN_CHECK(ctx != nullptr, "%s: ctx is NULL", who);
-  DMN_CHECK(ctx->net[0].bound && ctx->net[1].bound, "%s: bind both networks with dmnerf_set_weights first", who);
-  DMN_CHECK(ctx->net[0].ins_num == ctx->net[1].ins_num, "%s: coarse/fine ins_num differ", who);
-  return object_mask(keep_host, ctx->net[0].ins_num + 1, m, who);
-}
-
 extern "C" {
 
 DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
                           void* stream) {
-  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, nullptr, stream), impl, stream);
-}
-
-DMNERF_API int dmnerf_render_forward_objects(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
-                                             const uint32_t* keep_host, void* stream) {
   ObjMask m;
-  if (render_object_mask(ctx, keep_host, m, "render_forward_objects")) return 1;
-  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, &m, stream), impl, stream);
+  const ObjMask* keep;
+  if (render_mask(ctx, io, flags, m, keep, "render_forward")) return 1;
+  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, keep, stream), impl, stream);
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
@@ -666,15 +658,19 @@ extern "C" {
 
 DMNERF_API int dmnerf_render_forward_host(dmnerf_ctx* ctx, const dmnerf_render_io* h, int64_t n, int S, int NI, int flags,
                                int impl, void* stream) {
-  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, nullptr, stream);
+  ObjMask m;
+  const ObjMask* keep;
+  if (render_mask(ctx, h, flags, m, keep, "render_forward_host")) return 1;
+  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, keep, stream);
 }
 
-}  // extern "C"
-
-static int render_frame_impl(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z, float far_z,
-                             int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance, int flags, int impl,
-                             const dmnerf_render_io* out_host, const ObjMask* keep, void* stream) {
+DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
+                                        float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
+                                        int flags, int impl, const dmnerf_render_io* out_host, void* stream) {
   DMN_CHECK(ctx && K_host && c2w_host && out_host, "render_frame_host: NULL argument");
+  ObjMask m;
+  const ObjMask* keep;
+  if (render_mask(ctx, out_host, flags, m, keep, "render_frame_host")) return 1;
   DMN_CHECK(H > 0 && W > 0 && n_coarse >= 3 && n_coarse <= 4096, "render_frame_host: bad sizes H=%d W=%d S=%d", H, W, n_coarse);
   DMN_CHECK(ray_begin >= 0 && ray_count >= 0 && ray_begin + ray_count <= (int64_t)H * W,
             "render_frame_host: pixel range [%lld, +%lld) outside the %dx%d frame", (long long)ray_begin, (long long)ray_count, H, W);
@@ -700,25 +696,6 @@ static int render_frame_impl(dmnerf_ctx* ctx, const float* K_host, const float* 
   return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, keep, stream);
 }
 
-extern "C" {
-
-DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
-                                        float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
-                                        int flags, int impl, const dmnerf_render_io* out_host, void* stream) {
-  return render_frame_impl(ctx, K_host, c2w_host, H, W, near_z, far_z, ray_begin, ray_count, n_coarse, n_importance, flags, impl,
-                           out_host, nullptr, stream);
-}
-
-DMNERF_API int dmnerf_render_frame_objects_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
-                                                float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
-                                                int flags, int impl, const uint32_t* keep_host, const dmnerf_render_io* out_host,
-                                                void* stream) {
-  ObjMask m;
-  if (render_object_mask(ctx, keep_host, m, "render_frame_objects_host")) return 1;
-  return render_frame_impl(ctx, K_host, c2w_host, H, W, near_z, far_z, ray_begin, ray_count, n_coarse, n_importance, flags, impl,
-                           out_host, &m, stream);
-}
-
 // ---- mesh extraction (tools/mesh_generator.py mesh_main) ------------------------------------------------------------------
 
 DMNERF_API int dmnerf_mesh_grid_points(const double* transform_host, const double* extents_host, int dim, int64_t begin, int64_t count,
@@ -727,14 +704,16 @@ DMNERF_API int dmnerf_mesh_grid_points(const double* transform_host, const doubl
   return launch_grid_points(transform_host, extents_host, dim, begin, count, pts, (cudaStream_t)stream);
 }
 
-}  // extern "C"
-
-// The occupancy sweep; keep != NULL: with the object selection (and the per-point labels when labels != NULL)
-static int mesh_occupancy_impl(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim, float voxel,
-                               int64_t slab, const ObjMask* keep, float* occ, int16_t* labels, void* stream) {
+DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
+                                     float voxel, int64_t slab, const uint32_t* keep_host, float* occ, int16_t* labels,
+                                     void* stream) {
   DMN_CHECK(ctx && (net == 0 || net == 1), "mesh_occupancy: bad ctx / net");
   DMN_CHECK(transform_host && extents_host && occ, "mesh_occupancy: NULL argument");
   DMN_CHECK(dim >= 2 && dim <= 2048, "mesh_occupancy: dim %d out of range [2, 2048]", dim);
+  DMN_CHECK(keep_host || !labels, "mesh_occupancy: labels are written by the selected sweep only (pass keep_host)");
+  ObjMask m;
+  const ObjMask* keep;
+  if (object_mask(keep_host, ctx->net[net].bound ? ctx->net[net].ins_num + 1 : 0, m, keep, "mesh_occupancy")) return 1;
   DMN_CHECK(umma_available(ctx->packed[net]), "mesh_occupancy: bind the network with dmnerf_set_weights first");
   cudaStream_t st = (cudaStream_t)stream;
   DMN_CUDA(cudaSetDevice(ctx->device));
@@ -757,23 +736,6 @@ static int mesh_occupancy_impl(dmnerf_ctx* ctx, int net, const double* transform
     if (rc) return rc;
   }
   return 0;
-}
-
-extern "C" {
-
-DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
-                                     float voxel, int64_t slab, float* occ, void* stream) {
-  return mesh_occupancy_impl(ctx, net, transform_host, extents_host, dim, voxel, slab, nullptr, occ, nullptr, stream);
-}
-
-DMNERF_API int dmnerf_mesh_occupancy_objects(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
-                                             float voxel, int64_t slab, const uint32_t* keep_host, float* occ, int16_t* labels,
-                                             void* stream) {
-  DMN_CHECK(ctx && (net == 0 || net == 1), "mesh_occupancy_objects: bad ctx / net");
-  DMN_CHECK(ctx->net[net].bound, "mesh_occupancy_objects: bind the network with dmnerf_set_weights first");
-  ObjMask m;
-  if (object_mask(keep_host, ctx->net[net].ins_num + 1, m, "mesh_occupancy_objects")) return 1;
-  return mesh_occupancy_impl(ctx, net, transform_host, extents_host, dim, voxel, slab, &m, occ, labels, stream);
 }
 
 DMNERF_API int dmnerf_mesh_mc_count(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, int64_t* counts_host,

@@ -987,6 +987,21 @@ int umma_weights_pack_f16(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
   return 0;
 }
 
+// One launch of a tensor-core kernel: one persistent CTA per SM (at most `units` CTAs), the full shared-memory budget, whose
+// attribute is set once per device and kernel.
+template <void (*Kernel)(const uk::Program, const uk::KArgs)>
+static int launch_umma(int64_t units, const uk::Program& prog, const uk::KArgs& a, cudaStream_t st) {
+  using namespace uk;
+  static PerDeviceOnce attr_once;
+  if (attr_once.first()) DMN_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  int dev = 0, sms = 0;
+  DMN_CUDA(cudaGetDevice(&dev));
+  DMN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  Kernel<<<(unsigned)(units < sms ? units : sms), N_THREADS, SMEM_BYTES, st>>>(prog, a);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
 int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, const float* rays_o, const float* rays_d,
                     const float* z, int64_t m, int s, float* out, float* acts, cudaStream_t st, bool f16) {
   using namespace uk;
@@ -998,26 +1013,13 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
   DMN_CHECK(!f16 || (w.f16_ready && acts == nullptr), "mlp(umma): the fp16 network is inference-only and needs its packed image");
   if (m == 0) return 0;
   UmmaExtra* ex = extra_of(w);
-  static PerDeviceOnce attr_once, attr_once_f16;
-  if (!f16 && attr_once.first()) {
-    DMN_CUDA(cudaFuncSetAttribute(mlp_umma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  }
-  if (f16 && attr_once_f16.first()) {
-    DMN_CUDA(cudaFuncSetAttribute(mlp_f16_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  }
-  int dev = 0, sms = 0;
-  DMN_CUDA(cudaGetDevice(&dev));
-  DMN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int64_t tiles = (m + TILE_M - 1) / TILE_M;
   KArgs a;
   memset(&a, 0, sizeof(a));
   a.image = (const uint8_t*)(f16 ? w.image16 : w.image); a.bias = w.bias; a.x = x; a.rays_o = rays_o; a.rays_d = rays_d; a.z = z;
   a.m = m; a.s = s; a.out = out; a.acts = acts; a.status = ex->d_status;
-  const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
-  if (f16) mlp_f16_kernel<false><<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog16, a);
-  else mlp_umma_kernel<false><<<grid, N_THREADS, SMEM_BYTES, st>>>(ex->prog, a);
-  DMN_LAUNCH_OK();
-  return 0;
+  const int64_t tiles = (m + TILE_M - 1) / TILE_M;
+  if (f16) return launch_umma<mlp_f16_kernel<false>>(tiles, ex->prog16, a, st);
+  return launch_umma<mlp_umma_kernel<false>>(tiles, ex->prog, a, st);
 }
 
 // Whole dm_nerf() pipeline (render.py:31-96) in ONE launch: coarse network -> composite -> importance sampling -> fine
@@ -1032,22 +1034,6 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   DMN_CHECK(!f16 || (wc.f16_ready && wf.f16_ready), "render(umma): the fp16 images are not packed");
   if (n == 0) return 0;
   UmmaExtra* ex = extra_of(wc);
-  static PerDeviceOnce attr_once, attr_once_sel, attr_once_f16, attr_once_sel_f16;
-  if (!f16 && !keep && attr_once.first()) {
-    DMN_CUDA(cudaFuncSetAttribute(mlp_umma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  }
-  if (!f16 && keep && attr_once_sel.first()) {
-    DMN_CUDA(cudaFuncSetAttribute(render_objects_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  }
-  if (f16 && !keep && attr_once_f16.first()) {
-    DMN_CUDA(cudaFuncSetAttribute(mlp_f16_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  }
-  if (f16 && keep && attr_once_sel_f16.first()) {
-    DMN_CUDA(cudaFuncSetAttribute(render_objects_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  }
-  int dev = 0, sms = 0;
-  DMN_CUDA(cudaGetDevice(&dev));
-  DMN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   KArgs a;
   memset(&a, 0, sizeof(a));
   a.image = (const uint8_t*)(f16 ? wc.image16 : wc.image); a.bias = wc.bias;
@@ -1061,19 +1047,13 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   a.acc_c = io->acc_coarse; a.acc_f = io->acc_fine; a.ins_c = io->ins_coarse; a.ins_f = io->ins_fine;
   a.zc_out = io->z_vals_coarse; a.zf_out = io->z_vals_fine; a.wc_out = io->weights_coarse; a.wf_out = io->weights_fine;
   a.status = ex->d_status;
-  const int64_t units = (n + 1) / 2;
-  const unsigned grid = (unsigned)(units < sms ? units : sms);
+  if (keep) a.keep = *keep;
+  const int64_t units = (n + 1) / 2;                       // pairs of rays
   const Program& prog = f16 ? ex->prog16 : ex->prog;      // coarse and fine share ins_num, hence the program
-  if (keep) {
-    a.keep = *keep;
-    if (f16) render_objects_f16_kernel<<<grid, N_THREADS, SMEM_BYTES, st>>>(prog, a);
-    else render_objects_kernel<<<grid, N_THREADS, SMEM_BYTES, st>>>(prog, a);
-  } else {
-    if (f16) mlp_f16_kernel<true><<<grid, N_THREADS, SMEM_BYTES, st>>>(prog, a);
-    else mlp_umma_kernel<true><<<grid, N_THREADS, SMEM_BYTES, st>>>(prog, a);
-  }
-  DMN_LAUNCH_OK();
-  return 0;
+  if (keep && f16) return launch_umma<render_objects_f16_kernel>(units, prog, a, st);
+  if (keep) return launch_umma<render_objects_kernel>(units, prog, a, st);
+  if (f16) return launch_umma<mlp_f16_kernel<true>>(units, prog, a, st);
+  return launch_umma<mlp_umma_kernel<true>>(units, prog, a, st);
 }
 
 int umma_check_status(const UmmaWeights& w, cudaStream_t st) {

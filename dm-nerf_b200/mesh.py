@@ -44,15 +44,21 @@ def occupancy_grid(model, scene_transform, grid_dim=256, extents=EXTENTS, near=4
                    device="cuda"):
     """mesh_generator.py:23-63: occupancy 1 - exp(-relu(sigma) * (far - near) / N_importance) of `model` on the grid, with zero
     view directions, evaluated slab by slab (slab <= 0: 2^20 points) -> [grid_dim]^3 on the device."""
+    return _sweep(model, scene_transform, grid_dim, extents, near, far, N_importance, slab, device)[0]
+
+
+def _sweep(model, scene_transform, grid_dim, extents, near, far, N_importance, slab, device, keep_words=None):
+    """The sweep of occupancy_grid -> (occ, labels); keep_words: a selection (objects.occupancy_objects), else labels is None."""
     T = check_transform(scene_transform)
     ctx = get_context(device)
     slot = ctx.slot_for(model)
     ctx.bind(slot, model)
     occ = torch.empty((grid_dim,) * 3, device=device, dtype=torch.float32)
-    voxel = (far - near) / N_importance
-    ctx.call("dmnerf_mesh_occupancy", ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(extents, 3), grid_dim, voxel, slab,
-             _lib.ptr(occ))
-    return occ
+    labels = None if keep_words is None else torch.empty((grid_dim,) * 3, device=device, dtype=torch.int16)
+    keep = None if keep_words is None else _lib.keep_mask(keep_words)
+    ctx.call("dmnerf_mesh_occupancy", ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(extents, 3), grid_dim,
+             (far - near) / N_importance, slab, keep, _lib.ptr(occ), _lib.ptr(labels, torch.int16))
+    return occ, labels
 
 
 def marching_cubes(grid, level=0.45):

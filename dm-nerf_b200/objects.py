@@ -15,7 +15,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .engine import get_context
 
 MAX_LABELS = 128                     # ins_num + 1 <= 128
 
@@ -107,18 +106,9 @@ def occupancy_objects(model, scene_transform, keep_words, grid_dim=256, extents=
                       slab=0, device="cuda"):
     """The occupancy sweep of mesh.occupancy_grid with the selection applied per grid point -> (occ [dim]^3 float32, labels
     [dim]^3 int16): occ is 0 where the point's label is not kept, labels is every point's label."""
-    from .mesh import EXTENTS, check_transform
-    T = check_transform(scene_transform)
-    extents = EXTENTS if extents is None else extents
-    ctx = get_context(device)
-    slot = ctx.slot_for(model)
-    ctx.bind(slot, model)
-    occ = torch.empty((grid_dim,) * 3, device=device, dtype=torch.float32)
-    labels = torch.empty((grid_dim,) * 3, device=device, dtype=torch.int16)
-    voxel = (far - near) / N_importance
-    ctx.call("dmnerf_mesh_occupancy_objects", ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(extents, 3), grid_dim, voxel, slab,
-             _lib.keep_mask(keep_words), _lib.ptr(occ), _lib.ptr(labels, torch.int16))
-    return occ, labels
+    from .mesh import EXTENTS, _sweep
+    return _sweep(model, scene_transform, grid_dim, EXTENTS if extents is None else extents, near, far, N_importance, slab, device,
+                  keep_words)
 
 
 def meshes_from_labelled_grid(occ, labels, scene_transform, objects, level=0.45, extents=None, min_cluster=400):

@@ -33,15 +33,10 @@ def composite(raw, z_vals, rays_d, keep_all_ins=False, keep_objects=None):
     rgb = torch.empty((n, 3), device=dev); w = torch.empty((n, s), device=dev)
     depth = torch.empty((n,), device=dev); acc = torch.empty((n,), device=dev)
     ins = torch.empty((n, n_ins), device=dev)
-    ctx = get_context(dev)
-    outs = (_lib.ptr(rgb), _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc))
-    if keep_objects is None:
-        ctx.call("dmnerf_composite", _lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins), *outs)
-    else:
-        from .objects import object_mask
-        keep = _lib.keep_mask(object_mask(c - 5, keep=keep_objects))
-        ctx.call("dmnerf_composite_objects", _lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins), keep,
-                 *outs)
+    from .objects import object_mask
+    keep = None if keep_objects is None else _lib.keep_mask(object_mask(c - 5, keep=keep_objects))
+    get_context(dev).call("dmnerf_composite", _lib.ptr(raw), _lib.ptr(z_vals), _lib.ptr(rays_d), n, s, c, int(keep_all_ins), keep,
+                          _lib.ptr(rgb), _lib.ptr(w), _lib.ptr(depth), _lib.ptr(ins), _lib.ptr(acc))
     return rgb, w, depth, ins, acc
 
 
@@ -79,7 +74,8 @@ def reference_draws(perturb, n, S, N_importance, device, t_rand=None, u=None):
 
 
 def selection(who, keep_objects, ins_num, model_coarse, model_fine):
-    """The host mask of an inference entry point's keep_objects, or None without a selection."""
+    """The 4 mask words of an inference entry point's keep_objects (for io.keep with FLAG_SELECT), or None without a
+    selection."""
     if keep_objects is None:
         return None
     from .autograd import _needs_grad
@@ -87,7 +83,7 @@ def selection(who, keep_objects, ins_num, model_coarse, model_fine):
     if _needs_grad(model_coarse, model_fine):
         raise RuntimeError("%s: object selection is inference-only; call it under torch.no_grad() or with parameters that "
                            "do not require grad" % who)
-    return _lib.keep_mask(object_mask(ins_num, keep=keep_objects))
+    return object_mask(ins_num, keep=keep_objects)
 
 
 def _check_embedders(position_embedder, view_embedder):
@@ -145,10 +141,10 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     io.t_rand, io.u = _lib.ptr(t_rand), _lib.ptr(u)
     for k, v in out.items():
         setattr(io, k, _lib.ptr(v))
-    if keep is None:
-        ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags, impl)
-    else:
-        ctx.call("dmnerf_render_forward_objects", ctx.handle, io, n, S, N_importance, flags, impl, keep)
+    if keep is not None:
+        flags |= _lib.FLAG_SELECT
+        io.keep[:] = keep
+    ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags, impl)
     return out
 
 
@@ -254,13 +250,13 @@ def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64
            "depth": torch.empty(count, pin_memory=pin), "acc": torch.empty(count, pin_memory=pin)}
     io = _lib.RenderIO(rgb_fine=_lib.ptr(out["rgb"]), ins_fine=_lib.ptr(out["ins"]), depth_fine=_lib.ptr(out["depth"]),
                        acc_fine=_lib.ptr(out["acc"]))
-    Kf, Cf = _lib.camera(K, c2w)
     flags = _lib.FLAG_KEEP_INS if keep_all_ins else 0
-    args = (ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples, N_importance, flags, impl)
-    if keep is None:
-        ctx.call("dmnerf_render_frame_host", *args, C.byref(io))
-    else:
-        ctx.call("dmnerf_render_frame_objects_host", *args, keep, C.byref(io))
+    if keep is not None:
+        flags |= _lib.FLAG_SELECT
+        io.keep[:] = keep
+    Kf, Cf = _lib.camera(K, c2w)
+    ctx.call("dmnerf_render_frame_host", ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples, N_importance,
+             flags, impl, C.byref(io))
     if pixel_range is None:
         out = {"rgb": out["rgb"].reshape(H, W, 3), "ins": out["ins"].reshape(H, W, n_ins), "depth": out["depth"].reshape(H, W),
                "acc": out["acc"].reshape(H, W)}

@@ -28,7 +28,7 @@ extern "C" {
 #define DMNERF_API
 #endif
 
-#define DMNERF_ABI_VERSION 2
+#define DMNERF_ABI_VERSION 3
 #define DMNERF_N_PARAMS 30          /* tensors in DM_NeRF.state_dict() order, networks/dm_nerf.py:65-78 */
 #define DMNERF_CH_POS 63            /* get_embedder(10): 3 + 3*2*10, networks/dm_nerf.py:41-55 */
 #define DMNERF_CH_DIR 27            /* get_embedder(4) */
@@ -39,15 +39,15 @@ extern "C" {
 #define DMNERF_IMPL_SIMT 1          /* fp32 CUDA-core reference kernel */
 #define DMNERF_IMPL_UMMA 2          /* wgmma tensor-core kernel, bf16x3 split operands, fp32 accumulate */
 /* Preview precision, INFERENCE ONLY: the same tensor-core network run once with fp16 operands and fp32 accumulation (1/3 of
- * the MMAs, 1/2 of the weight bytes).  Accepted by dmnerf_mlp_forward(_rays/_points), dmnerf_render_forward(_host/_objects)
- * and dmnerf_render_frame(_objects)_host (with DMNERF_FLAG_WANT_RAW the stage kernels run it too).  Its weight image is packed
+ * the MMAs, 1/2 of the weight bytes).  Accepted by dmnerf_mlp_forward(_rays/_points), dmnerf_render_forward(_host) and
+ * dmnerf_render_frame_host (with DMNERF_FLAG_WANT_RAW the stage kernels run it too).  Its weight image is packed
  * on the first fp16 call after each dmnerf_set_weights, from the bound weights as they are then and the folded heads and
  * biases packed by that dmnerf_set_weights: as for the exact image, weights changed in place take effect only through a new
  * dmnerf_set_weights.  Measured against fp64 (DESIGN.md section 10, H100): network outputs rel. L2 2.8e-4 - 4.6e-4,
  * rendered rgb 54 - 62 dB PSNR on typical rays, argmax labels >= 0.99 agreement.  fp16 stops at 65504: a weight above it fails
  * the call at pack time, and a stored activation above it fails the call after the kernel (these fp16 calls synchronise
  * the stream to deliver that verdict) -- render such a network with DMNERF_IMPL_UMMA.  dmnerf_mlp_forward_train rejects it
- * (training and every backward stay exact), and dmnerf_mesh_occupancy(_objects), which has no impl, stays exact on purpose:
+ * (training and every backward stay exact), and dmnerf_mesh_occupancy, which has no impl, stays exact on purpose:
  * its threshold decides the surface. */
 #define DMNERF_IMPL_UMMA_F16 3
 
@@ -55,6 +55,7 @@ extern "C" {
 #define DMNERF_FLAG_PERTURB   1     /* args.perturb > 0: t_rand and u must be given (render.py:40-47, helpers.py:135) */
 #define DMNERF_FLAG_WANT_RAW  2     /* materialise raw_coarse / raw_fine (training, penalizer.py) */
 #define DMNERF_FLAG_KEEP_INS  4     /* keep all ins_num+1 instance channels, no detach: manipulator.py:86-105 */
+#define DMNERF_FLAG_SELECT    8     /* object selection: the keep field is read (see "object selection" below) */
 
 typedef struct dmnerf_ctx dmnerf_ctx;
 
@@ -82,6 +83,7 @@ typedef struct dmnerf_render_io {
   float* weights_fine;       /* [N,F] */
   float* raw_coarse;         /* [N,S,C] only with DMNERF_FLAG_WANT_RAW */
   float* raw_fine;           /* [N,F,C] */
+  uint32_t keep[4];          /* kept object labels with DMNERF_FLAG_SELECT (ignored without it): bit k of word k / 32 */
 } dmnerf_render_io;
 
 DMNERF_API int         dmnerf_abi_version(void);
@@ -109,10 +111,11 @@ DMNERF_API int dmnerf_mlp_forward_rays(dmnerf_ctx* ctx, int net, const float* ra
                             int64_t n, int s, float* out, int impl, void* stream);
 
 /* render_train, networks/render.py:6-28 (keep_all_ins != 0: manipulator_render, manipulator.py:86-105).
- * raw [N,S,C], z [N,S], rays_d [N,3] -> rgb [N,3], weights [N,S], depth [N], ins [N, C-5 or C-4], acc [N]. */
+ * raw [N,S,C], z [N,S], rays_d [N,3] -> rgb [N,3], weights [N,S], depth [N], ins [N, C-5 or C-4], acc [N].
+ * keep_host: an object selection over labels 0 .. C-5 (see "object selection" below), or NULL. */
 DMNERF_API int dmnerf_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c,
-                     int keep_all_ins, float* rgb, float* weights, float* depth, float* ins, float* acc,
-                     void* stream);
+                     int keep_all_ins, const uint32_t* keep_host, float* rgb, float* weights, float* depth, float* ins,
+                     float* acc, void* stream);
 
 /* sample_pdf, networks/helpers.py:123-155.  bins [N,nb], weights [N,nb-1]; u [N,ns] or NULL (det). */
 DMNERF_API int dmnerf_sample_pdf(const float* bins, const float* weights, int64_t n, int n_bins, int n_samples,
@@ -240,7 +243,8 @@ DMNERF_API int dmnerf_composite_backward(const float* raw, const float* z, const
  * are generated on the device from K / c2w (get_rays_k, helpers.py:50-61), the shared coarse depth row from near / far
  * (z_val_sample, helpers.py:114-119), and pixels [ray_begin, ray_begin + ray_count) of the H x W frame (pixel-major, the
  * reference's reshape(-1, 3)) are rendered by dm_nerf(); every non-NULL OUTPUT field of `out_host` (host memory, ray_count
- * rows) is filled; its input fields are ignored.  Deterministic path only (perturb = 0).  Synchronises the stream. */
+ * rows) is filled.  Of its input fields only `keep` is read (with DMNERF_FLAG_SELECT); the others are ignored.
+ * Deterministic path only (perturb = 0).  Synchronises the stream. */
 DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
                                         float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
                                         int flags, int impl, const dmnerf_render_io* out_host, void* stream);
@@ -285,28 +289,17 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
                           int n_importance, int flags, int impl, void* stream);
 
 /* ---- object selection (DESIGN.md, "Object selection") ----------------------------------------------------------------------
- * keep_host: HOST array of 4 uint32 words, a bitmask of the KEPT object labels 0 .. ins_num (bit k of word k / 32).  Every network
- * sample gets the label argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the exchanger's
- * rule); a sample whose label is not kept enters the composite with alpha = 0.  This applies to the coarse and the fine pass, so
- * the coarse weights of the selected scene drive the importance sampling.  raw_* (when asked for) stay the network's output.
- * All three reject a NULL mask and a bit set at or above ins_num + 1.
- * dmnerf_composite_objects: dmnerf_composite with a selection (labels 0 .. c - 5; raw is read, not edited).
- * dmnerf_render_forward_objects: dmnerf_render_forward with a selection (fused kernel or stage kernels, chosen as there).
- * dmnerf_render_frame_objects_host: dmnerf_render_frame_host with a selection.
- * dmnerf_mesh_occupancy_objects: dmnerf_mesh_occupancy with the rule applied per grid point (occ = 0 where the point's label is
- *   not kept); labels (DEVICE int16 [dim^3], may be NULL) receives every point's label. */
-DMNERF_API int dmnerf_composite_objects(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c,
-                                        int keep_all_ins, const uint32_t* keep_host, float* rgb, float* weights, float* depth,
-                                        float* ins, float* acc, void* stream);
-DMNERF_API int dmnerf_render_forward_objects(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n_rays, int n_coarse,
-                                             int n_importance, int flags, int impl, const uint32_t* keep_host, void* stream);
-DMNERF_API int dmnerf_render_frame_objects_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
-                                                float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
-                                                int flags, int impl, const uint32_t* keep_host, const dmnerf_render_io* out_host,
-                                                void* stream);
-DMNERF_API int dmnerf_mesh_occupancy_objects(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
-                                             float voxel, int64_t slab, const uint32_t* keep_host, float* occ, int16_t* labels,
-                                             void* stream);
+ * A bitmask of the KEPT object labels 0 .. ins_num, 4 uint32 words (bit k of word k / 32).  Every network sample gets the label
+ * argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the exchanger's rule); a sample whose
+ * label is not kept enters the composite with alpha = 0.  This applies to the coarse and the fine pass, so the coarse weights of
+ * the selected scene drive the importance sampling.  raw_* (when asked for) stay the network's output.
+ * dmnerf_render_forward(_host) and dmnerf_render_frame_host: io->keep with DMNERF_FLAG_SELECT (fused kernel or stage kernels,
+ *   chosen as without it).
+ * dmnerf_composite: keep_host (HOST, labels 0 .. c - 5; raw is read, not edited), NULL = no selection.
+ * dmnerf_mesh_occupancy: keep_host (HOST), NULL = no selection; with one the rule applies per grid point (occ = 0 where the
+ *   point's label is not kept) and labels (DEVICE int16 [dim^3], may be NULL) receives every point's label.  labels without
+ *   keep_host is rejected.
+ * Every one rejects a mask bit at or above ins_num + 1, naming the label. */
 
 /* Same call with HOST buffers (pageable or pinned): copies rays in, renders, copies every non-NULL
  * output back, and synchronises the stream.  This is the end-to-end entry point bench.py times.
@@ -334,7 +327,8 @@ DMNERF_API int dmnerf_profile_read(dmnerf_ctx* ctx, float* ms_out, int n_out);
  * dmnerf_mesh_grid_points: points [begin, begin + count) of the dim^3 query grid (C order of the grid index), in the network's
  *   frame: make_3D_grid / grid_within_bound in float32 + the axis swap and flip of :28-29.  pts [count,3].
  * dmnerf_mesh_occupancy: the occupancy sweep (:33-63): network `net` at every grid point with zero view directions, slab points
- *   at a time (slab <= 0: 2^20), each slab reduced to occ = 1 - exp(-relu(sigma) * voxel) -> occ [dim,dim,dim].
+ *   at a time (slab <= 0: 2^20), each slab reduced to occ = 1 - exp(-relu(sigma) * voxel) -> occ [dim,dim,dim].  keep_host /
+ *   labels: the object selection and the label grid (see "object selection" above), both NULL for the whole scene.
  * dmnerf_mesh_mc_count / _mc_emit: marching cubes (:68-69) on any grid [nx,ny,nz] (DEVICE, C order), inside = value > level.
  *   count classifies, scans and reads back counts_host[0] = vertices, [1] = triangles (the one device->host read; fails on a grid
  *   holding NaN); emit (same grid and level) writes verts [V,3] in index units and tris [T,3] int32.
@@ -352,7 +346,8 @@ DMNERF_API int dmnerf_profile_read(dmnerf_ctx* ctx, float* ms_out, int n_out);
 DMNERF_API int dmnerf_mesh_grid_points(const double* transform_host, const double* extents_host, int dim, int64_t begin, int64_t count,
                                        float* pts, void* stream);
 DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
-                                     float voxel, int64_t slab, float* occ, void* stream);
+                                     float voxel, int64_t slab, const uint32_t* keep_host, float* occ, int16_t* labels,
+                                     void* stream);
 DMNERF_API int dmnerf_mesh_mc_count(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, int64_t* counts_host,
                                     void* stream);
 DMNERF_API int dmnerf_mesh_mc_emit(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris,

@@ -163,16 +163,19 @@ def test_render_frame_driver_matches_explicit_rays():
 def test_host_entry_point_in_parts_is_bitwise_the_single_launch():
     """dmnerf_render_forward_host on >= 131 072 rays renders the batch in four parts whose copies overlap the neighbouring
     parts' kernels (second stream): same bits as the device-resident single launch, odd ray count, per-ray depth rows
-    (z_row_stride != 0) and the shared row (stride 0), and a small batch (single part) through the same call."""
+    (z_row_stride != 0) and the shared row (stride 0), a small batch (single part) through the same call, and an object
+    selection (io.keep with FLAG_SELECT) against dmnerf_render_forward with the same mask."""
     import ctypes as C
     from dmnerf_b200.testing import make_models
     from dmnerf_b200.engine import get_context
+    from dmnerf_b200.objects import object_mask
     from dmnerf_b200.render import render_rays
     wl = synth.workload("dmsr_study")
     nc, nf, _, _ = make_models(5, 6, 13, "cuda")
     ctx = get_context(torch.device("cuda"))
     ctx.bind(0, nc); ctx.bind(1, nf)
-    for n, per_ray_z in ((131073, False), (131080, True), (4097, False)):
+    cases = ((131073, False, None), (131080, True, None), (4097, False, None), (131073, False, [0, 2, 3, 7, 13]))
+    for n, per_ray_z, keep in cases:
         ro = torch.from_numpy(wl["rays_o"][:n]).contiguous().pin_memory()
         rd = torch.from_numpy(wl["rays_d"][:n]).contiguous().pin_memory()
         zrow = torch.linspace(float(wl["near"]), float(wl["far"]), 64)
@@ -184,15 +187,18 @@ def test_host_entry_point_in_parts_is_bitwise_the_single_launch():
         io.rays_o, io.rays_d, io.z_coarse, io.z_row_stride = _lib.ptr(ro), _lib.ptr(rd), _lib.ptr(zc), (64 if per_ray_z else 0)
         for k, v in out.items():
             setattr(io, k, _lib.ptr(v))
+        if keep is not None:
+            io.keep[:] = object_mask(13, keep=keep)
+        flags = 0 if keep is None else _lib.FLAG_SELECT
         before = _lib.launch_count()
-        _lib.check(ctx.lib.dmnerf_render_forward_host(ctx.handle, io, n, 64, 128, 0, 0, ctx.stream()), "dmnerf_render_forward_host")
+        _lib.check(ctx.lib.dmnerf_render_forward_host(ctx.handle, io, n, 64, 128, flags, 0, ctx.stream()), "dmnerf_render_forward_host")
         launches = _lib.launch_count() - before
         assert launches == (4 if n >= 131072 else 1), launches
         with torch.no_grad():
             zdev = zc.cuda() if per_ray_z else zc.cuda()[None].expand(n, 64)
-            ref = render_rays(ro.cuda(), rd.cuda(), nc, nf, zdev, N_importance=128, want_raw=False)
+            ref = render_rays(ro.cuda(), rd.cuda(), nc, nf, zdev, N_importance=128, want_raw=False, keep_objects=keep)
         for k, v in out.items():
-            assert torch.equal(v, ref[k].cpu()), (n, k)
+            assert torch.equal(v, ref[k].cpu()), (n, keep, k)
 
 
 def _manip_setup(golden_dir):

@@ -187,7 +187,7 @@ def test_empty_selection_and_reproducibility(impl):
 
 
 # ------------------------------------------------------------------------------------------ rejections
-def test_rejections():
+def test_selection_is_rejected_outside_the_labels_at_every_entry_point():
     wl, ro, rd = _rays("dmsr_study", 64)
     nc, nf, _, _ = make_models(101, 202, 13, DEV)
     with torch.no_grad():
@@ -200,19 +200,57 @@ def test_rejections():
     big, _, _, _ = make_models(303, 404, 59, DEV)
     with torch.no_grad(), pytest.raises(RuntimeError):
         render_rays(ro, rd, nc, big, _z(wl), keep_objects=[1])
-    # the C ABI itself: a bit at or above ins_num + 1, and a NULL mask
+    # the C ABI itself: a bit at or above ins_num + 1 is rejected by every entry point that takes a selection, naming the label
     ctx = get_context(DEV)
     ctx.bind(0, nc); ctx.bind(1, nf)
-    out = torch.empty(ro.shape[0], 3, device=DEV)
-    io = _lib.RenderIO(rays_o=ro.data_ptr(), rays_d=rd.data_ptr(), z_coarse=_z(wl).data_ptr(), rgb_fine=out.data_ptr())
+    n, st, lib = ro.shape[0], ctx.stream(), ctx.lib
     bad = (C.c_uint32 * 4)(1 << 14, 0, 0, 0)
-    assert ctx.lib.dmnerf_render_forward_objects(ctx.handle, io, ro.shape[0], 64, 128, 0, 0, bad, ctx.stream()) != 0
-    assert b"label 14" in ctx.lib.dmnerf_last_error()
-    assert ctx.lib.dmnerf_render_forward_objects(ctx.handle, io, ro.shape[0], 64, 128, 0, 0, None, ctx.stream()) != 0
+    z, out = _z(wl), torch.empty(n, 3, device=DEV)                        # every buffer a native call reads stays referenced
+    io = _lib.RenderIO(rays_o=ro.data_ptr(), rays_d=rd.data_ptr(), z_coarse=z.data_ptr(), rgb_fine=out.data_ptr(), keep=bad)
+    ro_h, rd_h, z_h, out_h = ro.cpu(), rd.cpu(), z.cpu(), torch.empty(n, 3)
+    io_h = _lib.RenderIO(rays_o=ro_h.data_ptr(), rays_d=rd_h.data_ptr(), z_coarse=z_h.data_ptr(), rgb_fine=out_h.data_ptr(), keep=bad)
+    Kf, Cf = _lib.camera(wl["K"], wl["c2w"])
+    raw, z_rows = torch.rand(n, 64, 18, device=DEV), z.expand(n, 64).contiguous()
+    rgb, w, depth, ins, acc = (torch.empty(n, 3, device=DEV), torch.empty(n, 64, device=DEV), torch.empty(n, device=DEV),
+                               torch.empty(n, 13, device=DEV), torch.empty(n, device=DEV))
+    comp = (raw.data_ptr(), z_rows.data_ptr(), rd.data_ptr(), n, 64, 18, 0)
+    comp_out = (rgb.data_ptr(), w.data_ptr(), depth.data_ptr(), ins.data_ptr(), acc.data_ptr(), st)
     eye = (C.c_double * 16)(*np.eye(4).reshape(-1)); ext = (C.c_double * 3)(1.9, 7.0, 7.0)
-    occ = torch.empty(8, 8, 8, device=DEV)
-    assert ctx.lib.dmnerf_mesh_occupancy_objects(ctx.handle, 1, eye, ext, 8, 0.1, 0, bad, occ.data_ptr(), None, ctx.stream()) != 0
-    assert ctx.lib.dmnerf_mesh_occupancy_objects(ctx.handle, 1, eye, ext, 8, 0.1, 0, None, occ.data_ptr(), None, ctx.stream()) != 0
+    occ, lab = torch.empty(8, 8, 8, device=DEV), torch.empty(8, 8, 8, device=DEV, dtype=torch.int16)
+    sel = _lib.FLAG_SELECT
+    calls = {
+        "render_forward": lambda: lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, sel, 0, st),
+        "render_forward_host": lambda: lib.dmnerf_render_forward_host(ctx.handle, io_h, n, 64, 128, sel, 0, st),
+        "render_frame_host": lambda: lib.dmnerf_render_frame_host(ctx.handle, Kf, Cf, 48, 64, 4.0, 15.0, 0, n, 64, 128, sel, 0,
+                                                                  C.byref(io_h), st),
+        "composite": lambda: lib.dmnerf_composite(*comp, bad, *comp_out),
+        "mesh_occupancy": lambda: lib.dmnerf_mesh_occupancy(ctx.handle, 1, eye, ext, 8, 0.1, 0, bad, occ.data_ptr(), lab.data_ptr(), st),
+    }
+    for name, call in calls.items():
+        assert call() != 0, name
+        err = lib.dmnerf_last_error()
+        assert name.encode() in err and b"keeps label 14, outside [0, 13]" in err, (name, err)
+    # without DMNERF_FLAG_SELECT, io->keep is not read; a NULL mask is no selection: both are the unselected result, bit for bit
+    with torch.no_grad():
+        ref = render_rays(ro, rd, nc, nf, z, want_raw=False, want_samples=False)
+    _lib.check(lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, 0, 0, st), "dmnerf_render_forward")
+    assert torch.equal(out, ref["rgb_fine"])
+    _lib.check(lib.dmnerf_render_forward_host(ctx.handle, io_h, n, 64, 128, 0, 0, st), "dmnerf_render_forward_host")
+    assert torch.equal(out_h, ref["rgb_fine"].cpu())
+    everything = _lib.keep_mask(object_mask(13, remove=[]))
+    _lib.check(lib.dmnerf_composite(*comp, None, *comp_out), "dmnerf_composite")
+    plain = [t.clone() for t in (rgb, w, depth, ins, acc)]
+    _lib.check(lib.dmnerf_composite(*comp, everything, *comp_out), "dmnerf_composite")
+    assert all(torch.equal(a, b) for a, b in zip(plain, (rgb, w, depth, ins, acc)))
+    _lib.check(lib.dmnerf_mesh_occupancy(ctx.handle, 1, eye, ext, 8, 0.1, 0, None, occ.data_ptr(), None, st), "dmnerf_mesh_occupancy")
+    plain = occ.clone()
+    _lib.check(lib.dmnerf_mesh_occupancy(ctx.handle, 1, eye, ext, 8, 0.1, 0, everything, occ.data_ptr(), lab.data_ptr(), st),
+               "dmnerf_mesh_occupancy")
+    assert torch.equal(occ, plain)
+    # the unselected sweep does not write labels: asking it for them is an error, not a silently untouched buffer
+    assert lib.dmnerf_mesh_occupancy(ctx.handle, 1, eye, ext, 8, 0.1, 0, None, occ.data_ptr(), lab.data_ptr(), st) != 0
+    assert b"labels" in lib.dmnerf_last_error()
+    ctx.sync_check()
 
 
 # ------------------------------------------------------------------------------------------ meshes

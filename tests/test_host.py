@@ -20,15 +20,37 @@ def lib():
     return _lib.load()
 
 
-def test_abi_version_2_exports_every_declared_symbol(lib):
+def test_abi_version_3_exports_every_declared_symbol(lib):
     hdr = open(os.path.join(ROOT, "include", "dmnerf_b200.h")).read()
     declared = set(re.findall(r"DMNERF_API[^;(]*?\b(dmnerf_\w+)\s*\(", hdr))
     assert len(declared) >= 14
     assert declared == set(_lib.PROTOTYPES), declared ^ set(_lib.PROTOTYPES)
     for name in declared:
         assert hasattr(lib, name)
-    assert lib.dmnerf_abi_version() == 2
-    assert ctypes.sizeof(_lib.RenderIO) == 20 * 8
+    assert lib.dmnerf_abi_version() == 3
+    assert ctypes.sizeof(_lib.RenderIO) == 20 * 8 + 16
+
+
+def test_object_selection_is_an_argument_and_the_objects_twins_are_gone(lib):
+    hdr = open(os.path.join(ROOT, "include", "dmnerf_b200.h")).read()
+    exports = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    exported = set(re.findall(r"\b(dmnerf_\w+)$", exports, re.M))
+    assert exported == set(_lib.PROTOTYPES), exported ^ set(_lib.PROTOTYPES)
+    for gone in ("dmnerf_composite_objects", "dmnerf_render_forward_objects", "dmnerf_render_frame_objects_host",
+                 "dmnerf_mesh_occupancy_objects"):
+        assert gone not in _lib.PROTOTYPES and gone not in exported and not hasattr(lib, gone), gone
+        assert not re.search(r"\b%s\b" % gone, hdr), gone
+    # the selection of the render calls: io->keep, read with DMNERF_FLAG_SELECT
+    assert re.search(r"#define DMNERF_FLAG_SELECT\s+%d\b" % _lib.FLAG_SELECT, hdr)
+    assert re.search(r"uint32_t keep\[4\];\s*/\*[^*]*\*/\s*\} dmnerf_render_io;", hdr)
+    assert _lib.RenderIO.keep.offset == 20 * 8 and _lib.RenderIO.keep.size == 16
+    assert not any(_lib.RenderIO().keep)                                  # ctypes zero-fills: no selection by default
+    # composite and the occupancy sweep take the 4 host words where their twins did (NULL = no selection)
+    mask = ctypes.POINTER(ctypes.c_uint32)
+    assert _lib.PROTOTYPES["dmnerf_composite"][1][7] is mask
+    assert _lib.PROTOTYPES["dmnerf_mesh_occupancy"][1][7] is mask
+    assert re.search(r"dmnerf_composite\([^;]*int keep_all_ins, const uint32_t\* keep_host, float\* rgb", hdr)
+    assert re.search(r"dmnerf_mesh_occupancy\([^;]*int64_t slab, const uint32_t\* keep_host, float\* occ, int16_t\* labels", hdr)
 
 
 def test_calls_fail_loudly_without_gpu(lib):
