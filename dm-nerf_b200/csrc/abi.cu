@@ -68,6 +68,7 @@ struct dmnerf_ctx {
   Scratch frame_rays;             // rays of the frame being rendered by dmnerf_render_frame_host
   Scratch mesh_pts, mesh_raw;     // one slab of the occupancy sweep: points + zero view directions, network output
   MeshState* mesh = nullptr;      // buffers of the other mesh entry points (mesh.cu)
+  InventoryState* inventory = nullptr;   // buffers of the object-inventory entry points (inventory.cu)
   bool profiling = false;
   bool last_fused = false;       // the last render call took the single-kernel path
   bool profile_valid = false;
@@ -116,6 +117,7 @@ DMNERF_API int dmnerf_ctx_destroy(dmnerf_ctx* ctx) {
                     &ctx->host_in, &ctx->host_out, &ctx->frame_rays, &ctx->mesh_pts, &ctx->mesh_raw};
   for (Scratch* s : all) s->release();
   mesh_state_free(ctx->mesh);
+  inventory_state_free(ctx->inventory);
   for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_in) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_done) if (e) cudaEventDestroy(e);
@@ -792,6 +794,22 @@ DMNERF_API int dmnerf_mesh_label_rays(const float* verts, const float* normals, 
 DMNERF_API int dmnerf_argmax_rows(const float* x, int64_t n, int c, int64_t* out, void* stream) {
   DMN_CHECK(n >= 0 && c >= 1 && (n == 0 || (x && out)), "argmax_rows: bad argument");
   return launch_argmax_rows(x, n, c, out, (cudaStream_t)stream);
+}
+
+// ---- object inventory (DESIGN.md, "Object inventory") ---------------------------------------------------------------------
+
+DMNERF_API int dmnerf_object_voxels(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                                    const int32_t* boxes_host, int64_t* moments_host, uint32_t* hist_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "object_voxels: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return object_voxels(&ctx->inventory, occ, labels, dim, level, n_labels, boxes_host, moments_host, hist_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_object_spans(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                                   const int32_t* boxes_host, const double* axes_host, double* spans_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "object_spans: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return object_spans(&ctx->inventory, occ, labels, dim, level, n_labels, boxes_host, axes_host, spans_host, (cudaStream_t)stream);
 }
 
 // ---- test-view evaluation (networks/tester.py render_test, networks/evaluator.py ins_eval) --------------------------------

@@ -217,6 +217,14 @@ int mesh_clean(MeshState** s, const float* v, const float* nrm, int64_t nv, cons
 int launch_label_rays(const float* v, const float* nrm, int64_t n, float near_z, float* ro, float* rd, cudaStream_t st);
 int launch_argmax_rows(const float* x, int64_t n, int c, int64_t* out, cudaStream_t st);
 
+// Object inventory (inventory.cu): per-group integer statistics and fp64 spans of the solid points of a labelled grid
+struct InventoryState;            // per-context device buffers of the inventory entry points
+void inventory_state_free(InventoryState* s);
+int object_voxels(InventoryState** s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                  const int32_t* boxes_host, int64_t* moments_host, uint32_t* hist_host, cudaStream_t st);
+int object_spans(InventoryState** s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                 const int32_t* boxes_host, const double* axes_host, double* spans_host, cudaStream_t st);
+
 // Test-view evaluation (metrics.cu)
 int64_t eval_workspace_bytes(int64_t n, int k, int H, int W);
 int eval_image(const float* rgb, const float* gt, int H, int W, void* ws, dmnerf_eval_result* res, cudaStream_t st);

@@ -5,16 +5,22 @@
                                                         -> isolated / removed views through the frame driver
     object_meshes(model_fine, model_coarse, scene_transform, objects=None, grid_dim=256, level=0.45, ...)
                                                         -> {label: closed mesh of that object}
+    object_inventory(model_fine, scene_transform, extents=None, grid_dim=256, level=0.45, trim=0.0, objects=None, ...)
+                                                        -> per object: voxels, volume, centre, covariance, aabb, obb (network frame)
+    scene_box(model_fine, poses, hwk, near, far, ...)   -> (scene_transform, extents) of the scene, from the cameras
+    manipulation_transform(centre, mode)                -> the transformation dict manipulator_eval takes, about that centre
 
 Every network sample is labelled argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the
 exchanger's rule); a sample whose label is not kept has alpha = 0 in the composite of both passes, so the coarse weights of the
 selected scene drive the importance sampling.  The instance map keeps the network's channels: selection does not re-label it."""
+import ctypes as C
 import os
 
 import numpy as np
 import torch
 
 from . import _lib
+from .engine import get_context
 
 MAX_LABELS = 128                     # ins_num + 1 <= 128
 
@@ -158,3 +164,258 @@ def object_meshes(model_fine, model_coarse, scene_transform, objects=None, grid_
         if objects is None:
             objects = [k for k in torch.unique(labels).cpu().tolist() if k != ins_num]
         return meshes_from_labelled_grid(occ, labels, T, objects, level, extents, min_cluster)
+
+
+# ----------------------------------------------------------------------------------------------------------------- inventory
+# DESIGN.md, "Object inventory": which objects the model found and where they are, from the solid points (occ > level) of a
+# labelled sweep.  Every statistic is taken over an object's points: its solid points inside its trimmed index box.
+MESH_TO_NETWORK = np.array([[1.0, 0.0, 0.0], [0.0, 0.0, -1.0], [0.0, 1.0, 0.0]])    # (x, y, z) -> (x, -z, y), grid_points_kernel
+N_MOMENTS = 10                       # count, Si, Sj, Sk, Sii, Sjj, Skk, Sij, Sik, Sjk
+
+
+def grid_affine(scene_transform, dim, extents=None):
+    """The exact map from grid index (i, j, k) to the network frame, p = A @ idx + b, in fp64: linspace(-1, 1, dim) scaled by
+    extents / 2, then [R | t], then the axis swap of the sweep.  The sweep's fp32 grid points differ from it by fp32 rounding."""
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    ext = np.asarray(EXTENTS if extents is None else extents, dtype=np.float64).reshape(3)
+    R, t = T[:3, :3], T[:3, 3]
+    A = MESH_TO_NETWORK @ (R * (ext / (dim - 1))[None, :])
+    b = MESH_TO_NETWORK @ (t - R @ (ext / 2.0))
+    return A, b
+
+
+def _check_grid(occ, labels, who):
+    _lib.need_cuda(who, occ, labels)
+    if occ.dim() != 3 or not (occ.shape[0] == occ.shape[1] == occ.shape[2]):
+        raise ValueError("%s: occ must be a cubic grid [dim, dim, dim], got %s" % (who, tuple(occ.shape)))
+    if labels is not None and (labels.shape != occ.shape or labels.device != occ.device):
+        raise ValueError("%s: labels must have occ's shape and device" % who)
+    return occ.shape[0]
+
+
+def object_voxels(occ, labels, level, n_labels, boxes=None):
+    """dmnerf_object_voxels: per group 0 .. n_labels - 1 (labels None: one group) the integer moments [n_labels, 10] int64
+    (count, Si, Sj, Sk, Sii, Sjj, Skk, Sij, Sik, Sjk of the index coordinates) and the per-axis index histograms
+    [n_labels, 3, dim] uint32 of its solid points, inside its box when boxes ([n_labels, 6] inclusive index boxes) is given."""
+    dim = _check_grid(occ, labels, "object_voxels")
+    ctx = get_context(occ.device)
+    mom = np.zeros((n_labels, N_MOMENTS), dtype=np.int64)
+    hist = np.zeros((n_labels, 3, dim), dtype=np.uint32)
+    ctx.call("dmnerf_object_voxels", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), dim, float(level), int(n_labels),
+             _int32s(boxes, n_labels * 6), mom.ctypes.data_as(C.POINTER(C.c_int64)), hist.ctypes.data_as(C.POINTER(C.c_uint32)))
+    return mom, hist
+
+
+def object_spans(occ, labels, level, n_labels, boxes, axes):
+    """dmnerf_object_spans: per group and axis r the min and max over its points (solid, inside its box) of
+    ((u0 i + u1 j) + u2 k) + o with axes[g, r] = (u0, u1, u2, o), fp64 -> [n_labels, 3, 2]; (+inf, -inf) without points."""
+    _check_grid(occ, labels, "object_spans")
+    ctx = get_context(occ.device)
+    out = np.zeros((n_labels, 3, 2), dtype=np.float64)
+    ctx.call("dmnerf_object_spans", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), occ.shape[0], float(level),
+             int(n_labels), _int32s(boxes, n_labels * 6), _lib.doubles(axes, n_labels * 12), out.ctypes.data_as(C.POINTER(C.c_double)))
+    return out
+
+
+def _int32s(a, n):
+    return None if a is None else (C.c_int32 * n)(*np.asarray(a, dtype=np.int64).reshape(-1).tolist())
+
+
+def trimmed_boxes(hist, trim):
+    """Per group and grid axis, the index range [lo, hi] left after cutting floor(trim * N) of the N solid points from each end
+    of that axis's histogram -> int32 [n_groups, 6] (i_lo, i_hi, j_lo, j_hi, k_lo, k_hi); a group without points gets (1, 0)."""
+    hist = np.asarray(hist, dtype=np.int64)
+    out = np.zeros((hist.shape[0], 6), dtype=np.int32)
+    for g in range(hist.shape[0]):
+        n = int(hist[g, 0].sum())
+        if n == 0:
+            out[g] = (1, 0) * 3
+            continue
+        cut = int(np.floor(trim * n))
+        for a in range(3):
+            c = np.cumsum(hist[g, a])
+            out[g, 2 * a] = int(np.argmax(c > cut))                                  # first index with more than cut below it
+            out[g, 2 * a + 1] = int(np.nonzero(c < n - cut)[0].size)                  # first index with more than cut above it
+    return out
+
+
+def _check_trim(trim):
+    trim = float(trim)
+    if not 0.0 <= trim < 0.5:
+        raise ValueError("trim %r outside [0, 0.5)" % trim)
+    return trim
+
+
+def describe_groups(moments, boxes, A, b, voxel_volume, groups):
+    """The host stage of the inventory: for each group of `groups` with points, its entry from the integer moments of its
+    points and its box -> (entries, spans axes [n, 3, 4]).  The OBB half-sizes come from finish_obbs."""
+    entries = []
+    axes_in = np.zeros((moments.shape[0], 3, 4))
+    for g in groups:
+        n = int(moments[g, 0])
+        if n == 0:
+            continue
+        s = [int(v) for v in moments[g]]
+        S1 = s[1:4]
+        S2 = [[s[4], s[7], s[8]], [s[7], s[5], s[9]], [s[8], s[9], s[6]]]
+        mean = np.array([S1[a] / n for a in range(3)])
+        cov_idx = np.array([[(n * S2[a][c] - S1[a] * S1[c]) / (n * n) for c in range(3)] for a in range(3)])
+        centre = A @ mean + b
+        cov = A @ cov_idx @ A.T
+        lo, hi = boxes[g, 0::2].astype(np.float64), boxes[g, 1::2].astype(np.float64)
+        corners = np.array([[(hi if (c >> a) & 1 else lo)[a] for a in range(3)] for c in range(8)]) @ A.T + b
+        w, V = np.linalg.eigh(cov)
+        axes = V[:, ::-1].T.copy()                                  # rows, descending eigenvalue
+        for r in range(2):
+            if axes[r, np.argmax(np.abs(axes[r]))] < 0:
+                axes[r] = -axes[r]
+        axes[2] = np.cross(axes[0], axes[1])
+        axes_in[g, :, :3] = axes @ A
+        axes_in[g, :, 3] = axes @ (b - centre)
+        entries.append({"label": int(g), "voxels": n, "volume": n * voxel_volume, "centre": centre, "covariance": cov,
+                        "aabb": (corners.min(0), corners.max(0)), "box": boxes[g].copy(),
+                        "obb": {"axes": axes, "eigenvalues": w[::-1].copy()}})
+    return entries, axes_in
+
+
+def finish_obbs(entries, spans):
+    """OBB centre and half-sizes of every entry from its spans [n, 3, 2] (min, max of the projections on its axes)."""
+    for e in entries:
+        lo, hi = spans[e["label"], :, 0], spans[e["label"], :, 1]
+        e["obb"]["centre"] = e["centre"] + e["obb"]["axes"].T @ ((lo + hi) / 2.0)
+        e["obb"]["half_sizes"] = (hi - lo) / 2.0
+    return entries
+
+
+def inventory_from_grid(occ, labels, scene_transform, extents=None, level=0.45, trim=0.0, objects=None):
+    """The grid-only stage of object_inventory: occ [dim]^3 float32 and labels [dim]^3 int16 (or None: one group, the scene)
+    on the device.  Returns one entry per group (of `objects`, default all) that has points, ascending label:
+      label, voxels, volume (voxels |det R| prod(extents / (dim - 1))), centre and covariance (network frame),
+      aabb (min, max of the trimmed box's corners, network frame), box (the trimmed index box),
+      obb {centre, axes (rows: eigenvectors of the covariance, descending eigenvalue, right-handed), eigenvalues, half_sizes}."""
+    from .mesh import EXTENTS, check_transform
+    trim = _check_trim(trim)
+    T = check_transform(scene_transform)
+    ext = np.asarray(EXTENTS if extents is None else extents, dtype=np.float64).reshape(3)
+    dim = _check_grid(occ, labels, "inventory_from_grid")
+    n_labels = MAX_LABELS if labels is not None else 1
+    groups = range(n_labels) if objects is None else sorted({int(k) for k in objects})
+    if any(not 0 <= g < n_labels for g in groups):
+        raise ValueError("inventory_from_grid: objects must be labels in [0, %d]" % (n_labels - 1))
+    with torch.no_grad():
+        mom, hist = object_voxels(occ, labels, level, n_labels)
+        boxes = trimmed_boxes(hist, trim)
+        if trim > 0:
+            mom, _ = object_voxels(occ, labels, level, n_labels, boxes)
+        A, b = grid_affine(T, dim, ext)
+        unit = abs(np.linalg.det(T[:3, :3])) * float(np.prod(ext / (dim - 1)))
+        entries, axes_in = describe_groups(mom, boxes, A, b, unit, groups)
+        if not entries:
+            return []
+        spans = object_spans(occ, labels, level, n_labels, boxes, axes_in)
+    return finish_obbs(entries, spans)
+
+
+def object_inventory(model_fine, scene_transform, extents=None, grid_dim=256, level=0.45, trim=0.0, objects=None, near=4.0,
+                     far=15.0, N_importance=128):
+    """Which objects the model found and where: one selected occupancy sweep of model_fine (keeping `objects`, default every
+    label except ins_num, as object_meshes) with its label grid, then inventory_from_grid."""
+    from .mesh import check_transform
+    T = check_transform(scene_transform)
+    dev = next(model_fine.parameters()).device
+    ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
+    objects = list(range(ins_num)) if objects is None else _labels(objects, ins_num, "object_inventory")
+    with torch.no_grad():
+        occ, labels = occupancy_objects(model_fine, T, object_mask(ins_num, keep=objects), grid_dim, extents, near, far,
+                                        N_importance, device=dev)
+        return inventory_from_grid(occ, labels, T, extents, level, trim, objects)
+
+
+def camera_region(poses, hwk, far):
+    """Network-frame AABB (lo, hi) of the camera centres and of every camera's four corner rays at depth far: o + far * d with
+    d = R ((u - cx) / fx, (v - cy) / fy, K[2, 2]), the direction get_rays_k gives pixel (u, v)."""
+    H, W, K = hwk
+    K = np.asarray(K, dtype=np.float64).reshape(3, 3)
+    pts = []
+    for c2w in poses:
+        c2w = np.asarray(c2w.cpu() if torch.is_tensor(c2w) else c2w, dtype=np.float64)
+        R, o = c2w[:3, :3], c2w[:3, 3]
+        pts.append(o)
+        for u in (0.0, float(W) - 1):
+            for v in (0.0, float(H) - 1):
+                d = R @ np.array([(u - K[0, 2]) / K[0, 0], (v - K[1, 2]) / K[1, 1], K[2, 2]])
+                pts.append(o + far * d)
+    pts = np.array(pts)
+    return pts.min(0), pts.max(0)
+
+
+def region_transform(lo, hi):
+    """A network-frame AABB as (scene_transform, extents): box axes = the mesh-frame axes (det +1), network -> mesh is
+    (x, y, z) -> (x, z, -y)."""
+    lo, hi = np.asarray(lo, dtype=np.float64), np.asarray(hi, dtype=np.float64)
+    m_lo = np.array([lo[0], lo[2], -hi[1]])
+    m_hi = np.array([hi[0], hi[2], -lo[1]])
+    T = np.eye(4)
+    T[:3, 3] = (m_lo + m_hi) / 2.0
+    return T, m_hi - m_lo
+
+
+def box_transform(scene_transform, extents, dim, box):
+    """The index box [lo, hi] (int [6]) of a grid with an axis-aligned transform (R = I) as (scene_transform, extents)."""
+    T = np.asarray(scene_transform, dtype=np.float64)
+    ext = np.asarray(extents, dtype=np.float64)
+    step = ext / (dim - 1)
+    lo, hi = np.asarray(box[0::2], dtype=np.float64), np.asarray(box[1::2], dtype=np.float64)
+    out = np.eye(4)
+    out[:3, 3] = T[:3, 3] - ext / 2.0 + step * (lo + hi) / 2.0
+    return out, step * (hi - lo)
+
+
+def scene_box(model_fine, poses, hwk, near, far, grid_dim=128, trim=1e-3, margin=2, level=0.45, N_importance=128):
+    """The scene's box without a ground-truth mesh -> (scene_transform, extents) for extract_mesh / object_inventory:
+    1. the camera region (camera_region), 2. one unselected coarse sweep over it, 3. the trimmed box of its solid points,
+    padded by `margin` coarse voxels and kept inside the region.  A surface thinner than the coarse spacing can be missed:
+    raise grid_dim (and margin) for thin scenes."""
+    from .mesh import occupancy_grid
+    trim = _check_trim(trim)
+    if int(margin) < 0 or int(grid_dim) < 2:
+        raise ValueError("scene_box: margin must be >= 0 and grid_dim >= 2")
+    dev = next(model_fine.parameters()).device
+    T0, ext0 = region_transform(*camera_region(poses, hwk, far))
+    with torch.no_grad():
+        occ = occupancy_grid(model_fine, T0, grid_dim, ext0, near, far, N_importance, device=dev)
+        mom, hist = object_voxels(occ, None, level, 1)
+    if mom[0, 0] == 0:
+        raise ValueError("scene_box: no grid point of the camera region has occupancy above %g" % level)
+    box = trimmed_boxes(hist, trim)[0].astype(np.int64)
+    box[0::2] = np.maximum(box[0::2] - int(margin), 0)
+    box[1::2] = np.minimum(box[1::2] + int(margin), grid_dim - 1)
+    for a in range(3):                                  # at least one coarse spacing along every axis
+        if box[2 * a] == box[2 * a + 1]:
+            if box[2 * a + 1] < grid_dim - 1:
+                box[2 * a + 1] += 1
+            else:
+                box[2 * a] -= 1
+    return box_transform(T0, ext0, grid_dim, box)
+
+
+def manipulation_transform(centre, mode, distance=-0.25, yaw=90.0, scale=1.2):
+    """The transformation dict of the original's generate_poses_eval (tools/pose_generator.py) about `centre` (network frame):
+    {'transformations': [{'transformation': 4x4 list, 'mode': mode}]}; mode translation (along y by distance), rotation (yaw
+    degrees about z), scale, or multi (scale @ rotation @ translation).  As there, the centre is held in float32 and the
+    products are taken in float64, so manipulator_eval receives the same matrix the original would build."""
+    if mode not in ("translation", "rotation", "scale", "multi"):
+        raise ValueError("manipulation_transform: unknown mode %r" % (mode,))
+    c = np.asarray(centre, dtype=np.float64).reshape(3)
+    to_origin = np.eye(4, dtype=np.float32)
+    to_origin[:3, 3] = -c
+    back = np.eye(4, dtype=np.float32)
+    back[:3, 3] = -to_origin[:3, 3]
+    move = np.eye(4)
+    move[1, 3] = distance
+    a = yaw * np.pi / 180
+    turn = np.array([[np.cos(a), -np.sin(a), 0, 0], [np.sin(a), np.cos(a), 0, 0], [0, 0, 1, 0], [0, 0, 0, 1]])
+    grow = np.diag([scale, scale, scale, 1.0])
+    op = {"translation": move, "rotation": turn, "scale": grow, "multi": grow @ turn @ move}[mode]
+    return {"transformations": [{"transformation": (back @ op @ to_origin).tolist(), "mode": mode}]}

@@ -365,6 +365,23 @@ DMNERF_API int dmnerf_mesh_label_rays(const float* verts, const float* normals, 
                                       void* stream);
 DMNERF_API int dmnerf_argmax_rows(const float* x, int64_t n, int c, int64_t* out, void* stream);
 
+/* ---- object inventory (DESIGN.md, "Object inventory"; no counterpart in the original) ---------------------------------------
+ * Per-group reductions over the solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order of the index (i, j, k)).
+ * labels [dim^3] (DEVICE int16, may be NULL: every point is group 0) assigns each point its group 0 .. n_labels - 1.
+ * boxes_host: HOST int32 [n_labels][6] = inclusive index boxes (i_lo, i_hi, j_lo, j_hi, k_lo, k_hi); with it only the solid
+ * points inside their group's box count.  Every sum is an integer, so both calls are deterministic and independent of the launch
+ * shape.  Both fail, before anything is written, when dim is outside [2, 2048], n_labels outside [1, 128], the grid holds NaN or
+ * a label is outside [0, n_labels - 1].  One device->host read per call (synchronises the stream).
+ * dmnerf_object_voxels: moments_host [n_labels][10] int64 = count, Si, Sj, Sk, Sii, Sjj, Skk, Sij, Sik, Sjk of the group's index
+ *   coordinates; hist_host (may be NULL) [n_labels][3][dim] uint32 = its per-axis index histograms.  boxes_host may be NULL.
+ * dmnerf_object_spans: axes_host [n_labels][3][4] fp64 (u0, u1, u2, o) -> spans_host [n_labels][3][2] = min and max over the
+ *   group's points of s = ((u0 i + u1 j) + u2 k) + o, each operation rounded once in fp64; a group without points gets
+ *   (+inf, -inf).  boxes_host is required. */
+DMNERF_API int dmnerf_object_voxels(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                                    const int32_t* boxes_host, int64_t* moments_host, uint32_t* hist_host, void* stream);
+DMNERF_API int dmnerf_object_spans(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                                   const int32_t* boxes_host, const double* axes_host, double* spans_host, void* stream);
+
 /* ---- test-view evaluation: render_test, networks/tester.py (+ ins_eval / calculate_ap, networks/evaluator.py:77-175) -------
  * Rules and deviations: DESIGN.md, "Evaluation metrics".  Every result is deterministic (fixed-order reductions, integer atomics
  * only).  `res` is DEVICE memory; reading it back is the caller's one device->host transfer per frame.  `ws` is caller-provided

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Labelled object mesh of a trained DM-NeRF checkpoint, without trimesh, skimage or open3d.
 
-    python tools/extract_mesh.py CHECKPOINT.tar TRANSFORM --out DIR [--name NAME] [--grid-dim 256] [--near 4 --far 15] ...
+    python tools/extract_mesh.py CHECKPOINT.tar TRANSFORM --out DIR [--name NAME] [--grid-dim 256] [--extents 1.9 7 7] ...
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict` (the original's checkpoints).  TRANSFORM is the 4x4
 scene transform, inv(to_origin) of the scene mesh's oriented bounds, as a .npy file or as text (16 numbers).  Writes
@@ -29,6 +29,9 @@ def parse(argv=None):
     ap.add_argument("--out", required=True)
     ap.add_argument("--name", default="mesh")
     ap.add_argument("--grid-dim", type=int, default=256)
+    ap.add_argument("--extents", type=float, nargs=3, default=[1.9, 7.0, 7.0], metavar=("X", "Y", "Z"),
+                    help="grid size along the transform's axes (default: the original's 1.9 7 7; tools/find_objects.py "
+                         "writes the found box's)")
     ap.add_argument("--near", type=float, default=4.0)
     ap.add_argument("--far", type=float, default=15.0)
     ap.add_argument("--N-samples", type=int, default=64)
@@ -54,7 +57,7 @@ def main(argv=None):
     nets = [model_from_weights({k: v.float().numpy() for k, v in ck[key].items()}, a.device)
             for key in ("network_coarse_state_dict", "network_fine_state_dict")]
     ins_num = nets[1].ins_linear.weight.shape[0] - 1
-    out = M.extract_mesh(nets[1], nets[0], T, grid_dim=a.grid_dim, near=a.near, far=a.far, N_samples=a.N_samples,
+    out = M.extract_mesh(nets[1], nets[0], T, grid_dim=a.grid_dim, extents=tuple(a.extents), near=a.near, far=a.far, N_samples=a.N_samples,
                          N_importance=a.N_importance, N_test=a.N_test, min_cluster=a.min_cluster)
     os.makedirs(a.out, exist_ok=True)
     M.write_ply(os.path.join(a.out, a.name + ".ply"), out["vertices"], out["triangles"])
@@ -69,7 +72,7 @@ def main(argv=None):
     per_object = {}
     if a.per_object:
         from dmnerf_b200.objects import object_meshes
-        meshes = object_meshes(nets[1], nets[0], T, objects=a.objects, grid_dim=a.grid_dim, near=a.near, far=a.far,
+        meshes = object_meshes(nets[1], nets[0], T, objects=a.objects, grid_dim=a.grid_dim, extents=tuple(a.extents), near=a.near, far=a.far,
                                N_importance=a.N_importance, min_cluster=a.min_cluster)
         for k, m in meshes.items():
             name = "%s_obj%d.ply" % (a.name, k)
