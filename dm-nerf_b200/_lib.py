@@ -118,6 +118,11 @@ PROTOTYPES = {
                                        C.POINTER(C.c_int64), C.POINTER(C.c_uint32), C.c_void_p]),
     "dmnerf_object_spans": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_int32),
                                       C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p]),
+    "dmnerf_object_components": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int, C.c_void_p,
+                                           C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_component_table": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]),
+    "dmnerf_component_groups": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "dmnerf_eval_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int, C.c_int, C.c_int]),
     "dmnerf_eval_image": (C.c_int, [_f32p, _f32p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dmnerf_ins_eval": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_void_p, C.c_int, _f32p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,

@@ -69,6 +69,7 @@ struct dmnerf_ctx {
   Scratch mesh_pts, mesh_raw;     // one slab of the occupancy sweep: points + zero view directions, network output
   MeshState* mesh = nullptr;      // buffers of the other mesh entry points (mesh.cu)
   InventoryState* inventory = nullptr;   // buffers of the object-inventory entry points (inventory.cu)
+  ComponentsState* components = nullptr;   // buffers of the connected-component entry points (components.cu)
   bool profiling = false;
   bool last_fused = false;       // the last render call took the single-kernel path
   bool profile_valid = false;
@@ -118,6 +119,7 @@ DMNERF_API int dmnerf_ctx_destroy(dmnerf_ctx* ctx) {
   for (Scratch* s : all) s->release();
   mesh_state_free(ctx->mesh);
   inventory_state_free(ctx->inventory);
+  components_state_free(ctx->components);
   for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_in) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_done) if (e) cudaEventDestroy(e);
@@ -810,6 +812,30 @@ DMNERF_API int dmnerf_object_spans(dmnerf_ctx* ctx, const float* occ, const int1
   DMN_CHECK(ctx != nullptr, "object_spans: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
   return object_spans(&ctx->inventory, occ, labels, dim, level, n_labels, boxes_host, axes_host, spans_host, (cudaStream_t)stream);
+}
+
+// ---- connected components (DESIGN.md, "Connected components") -------------------------------------------------------------
+
+DMNERF_API int dmnerf_object_components(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                                        int connectivity, int32_t* comp, int64_t* n_components_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "object_components: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return object_components(&ctx->components, occ, labels, dim, level, n_labels, connectivity, comp, n_components_host,
+                           (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_component_table(dmnerf_ctx* ctx, const int32_t* comp, const int16_t* labels, int dim, int64_t n, int16_t* label,
+                                      int64_t* voxels, int64_t* root, void* stream) {
+  DMN_CHECK(ctx != nullptr, "component_table: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return component_table(&ctx->components, comp, labels, dim, n, label, voxels, root, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_component_groups(dmnerf_ctx* ctx, const int32_t* comp, int dim, int64_t n, const int16_t* lut, int discard,
+                                       int16_t* groups, void* stream) {
+  DMN_CHECK(ctx != nullptr, "component_groups: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return component_groups(&ctx->components, comp, dim, n, lut, discard, groups, (cudaStream_t)stream);
 }
 
 // ---- test-view evaluation (networks/tester.py render_test, networks/evaluator.py ins_eval) --------------------------------

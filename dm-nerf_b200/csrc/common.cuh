@@ -225,6 +225,16 @@ int object_voxels(InventoryState** s, const float* occ, const int16_t* labels, i
 int object_spans(InventoryState** s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                  const int32_t* boxes_host, const double* axes_host, double* spans_host, cudaStream_t st);
 
+// Connected components (components.cu): the solid points of a labelled grid split into canonically numbered components
+struct ComponentsState;           // per-context device buffers of the component entry points
+void components_state_free(ComponentsState* s);
+int object_components(ComponentsState** s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                      int connectivity, int32_t* comp, int64_t* n_components_host, cudaStream_t st);
+int component_table(ComponentsState** s, const int32_t* comp, const int16_t* labels, int dim, int64_t n_comp, int16_t* label,
+                    int64_t* voxels, int64_t* root, cudaStream_t st);
+int component_groups(ComponentsState** s, const int32_t* comp, int dim, int64_t n_comp, const int16_t* lut, int discard,
+                     int16_t* groups, cudaStream_t st);
+
 // Test-view evaluation (metrics.cu)
 int64_t eval_workspace_bytes(int64_t n, int k, int H, int W);
 int eval_image(const float* rgb, const float* gt, int H, int W, void* ws, dmnerf_eval_result* res, cudaStream_t st);

@@ -7,6 +7,8 @@
                                                         -> {label: closed mesh of that object}
     object_inventory(model_fine, scene_transform, extents=None, grid_dim=256, level=0.45, trim=0.0, objects=None, ...)
                                                         -> per object: voxels, volume, centre, covariance, aabb, obb (network frame)
+    object_components(occ, labels=None, level=0.45, connectivity=26)
+                                                        -> the connected components of a labelled grid's solid points
     scene_box(model_fine, poses, hwk, near, far, ...)   -> (scene_transform, extents) of the scene, from the cameras
     manipulation_transform(centre, mode)                -> the transformation dict manipulator_eval takes, about that centre
 
@@ -145,12 +147,16 @@ def meshes_from_labelled_grid(occ, labels, scene_transform, objects, level=0.45,
 
 
 def object_meshes(model_fine, model_coarse, scene_transform, objects=None, grid_dim=256, level=0.45, extents=None, near=4.0,
-                  far=15.0, N_importance=128, min_cluster=400):
+                  far=15.0, N_importance=128, min_cluster=400, components=None):
     """One mesh per object: one selected occupancy sweep of model_fine (keeping `objects`) with the label grid, then
     meshes_from_labelled_grid.  objects: labels in [0, ins_num]; default every label present in the grid except the last
     channel (ins_num, "no object").  model_coarse is accepted for symmetry with extract_mesh and not evaluated: the labels come
-    from the fine network's per-point logits, not from rendered rays.  Returns {label: mesh dict} of device tensors."""
+    from the fine network's per-point logits, not from rendered rays.  components="largest": each object's field is occ on its
+    largest 26-connected component (object_components at `level`) and 0 elsewhere.  Returns {label: mesh dict} of device
+    tensors."""
     from .mesh import check_transform
+    if components not in (None, "largest"):
+        raise ValueError("object_meshes: components must be None or 'largest', got %r" % (components,))
     T = check_transform(scene_transform)
     dev = next(model_fine.parameters()).device
     ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
@@ -163,7 +169,20 @@ def object_meshes(model_fine, model_coarse, scene_transform, objects=None, grid_
         occ, labels = occupancy_objects(model_fine, T, words, grid_dim, extents, near, far, N_importance, device=dev)
         if objects is None:
             objects = [k for k in torch.unique(labels).cpu().tolist() if k != ins_num]
+        if components == "largest":
+            labels = largest_component_grid(occ, labels, level, objects)
         return meshes_from_labelled_grid(occ, labels, T, objects, level, extents, min_cluster)
+
+
+def largest_component_grid(occ, labels, level, objects):
+    """int16 grid: label k at the points of the largest 26-connected component of each label k of `objects`, -1 elsewhere."""
+    cc = object_components(occ, labels, level, 26)
+    best = largest_components(cc["label"], cc["voxels"])
+    lut = np.full(cc["label"].shape[0], -1, dtype=np.int16)
+    for k in objects:
+        if int(k) in best:
+            lut[best[int(k)]] = int(k)
+    return component_groups(cc["grid"], lut, -1)
 
 
 # ----------------------------------------------------------------------------------------------------------------- inventory
@@ -288,14 +307,40 @@ def finish_obbs(entries, spans):
     return entries
 
 
-def inventory_from_grid(occ, labels, scene_transform, extents=None, level=0.45, trim=0.0, objects=None):
+def _inventory_of_groups(occ, labels, n_labels, T, ext, dim, level, trim, groups):
+    """The device passes and host stage of inventory_from_grid over the groups of one group grid (labels, n_labels)."""
+    mom, hist = object_voxels(occ, labels, level, n_labels)
+    boxes = trimmed_boxes(hist, trim)
+    if trim > 0:
+        mom, _ = object_voxels(occ, labels, level, n_labels, boxes)
+    A, b = grid_affine(T, dim, ext)
+    unit = abs(np.linalg.det(T[:3, :3])) * float(np.prod(ext / (dim - 1)))
+    entries, axes_in = describe_groups(mom, boxes, A, b, unit, groups)
+    if not entries:
+        return []
+    spans = object_spans(occ, labels, level, n_labels, boxes, axes_in)
+    return finish_obbs(entries, spans)
+
+
+def inventory_from_grid(occ, labels, scene_transform, extents=None, level=0.45, trim=0.0, objects=None, components=None,
+                        connectivity=26, min_voxels=1):
     """The grid-only stage of object_inventory: occ [dim]^3 float32 and labels [dim]^3 int16 (or None: one group, the scene)
     on the device.  Returns one entry per group (of `objects`, default all) that has points, ascending label:
       label, voxels, volume (voxels |det R| prod(extents / (dim - 1))), centre and covariance (network frame),
       aabb (min, max of the trimmed box's corners, network frame), box (the trimmed index box),
-      obb {centre, axes (rows: eigenvectors of the covariance, descending eigenvalue, right-handed), eigenvalues, half_sizes}."""
+      obb {centre, axes (rows: eigenvectors of the covariance, descending eigenvalue, right-handed), eigenvalues, half_sizes}.
+    components (DESIGN.md, "Connected components"; `connectivity` 6 or 26):
+      None:      a label is one object;
+      "largest": each label's statistics over its largest component only (a tie in voxels goes to the smaller root); the
+                 entry gains components (how many the label has) and discarded_voxels (its solid points outside that one);
+      "split":   one entry per component with at least min_voxels voxels, ordered by (label, root), with component (its id).
+    trim applies after the selection, over the selected points."""
     from .mesh import EXTENTS, check_transform
     trim = _check_trim(trim)
+    if components not in (None, "largest", "split"):
+        raise ValueError("inventory_from_grid: components must be None, 'largest' or 'split', got %r" % (components,))
+    if int(min_voxels) < 1 or (int(min_voxels) != 1 and components != "split"):
+        raise ValueError("inventory_from_grid: min_voxels %r needs components='split' and must be >= 1" % (min_voxels,))
     T = check_transform(scene_transform)
     ext = np.asarray(EXTENTS if extents is None else extents, dtype=np.float64).reshape(3)
     dim = _check_grid(occ, labels, "inventory_from_grid")
@@ -304,23 +349,33 @@ def inventory_from_grid(occ, labels, scene_transform, extents=None, level=0.45, 
     if any(not 0 <= g < n_labels for g in groups):
         raise ValueError("inventory_from_grid: objects must be labels in [0, %d]" % (n_labels - 1))
     with torch.no_grad():
-        mom, hist = object_voxels(occ, labels, level, n_labels)
-        boxes = trimmed_boxes(hist, trim)
-        if trim > 0:
-            mom, _ = object_voxels(occ, labels, level, n_labels, boxes)
-        A, b = grid_affine(T, dim, ext)
-        unit = abs(np.linalg.det(T[:3, :3])) * float(np.prod(ext / (dim - 1)))
-        entries, axes_in = describe_groups(mom, boxes, A, b, unit, groups)
-        if not entries:
-            return []
-        spans = object_spans(occ, labels, level, n_labels, boxes, axes_in)
-    return finish_obbs(entries, spans)
+        if components is None:
+            return _inventory_of_groups(occ, labels, n_labels, T, ext, dim, level, trim, groups)
+        cc = object_components(occ, labels, level, connectivity)
+        sel = select_components(cc["label"], cc["voxels"], components, groups, int(min_voxels))
+        entries = []
+        for lut, ids in group_luts(sel, cc["label"].shape[0]):
+            grid = component_groups(cc["grid"], lut, DISCARD_GROUP)
+            part = _inventory_of_groups(occ, grid, MAX_LABELS, T, ext, dim, level, trim, range(len(ids)))
+            del grid
+            for e in part:
+                c = int(ids[e["label"]])
+                e["label"] = int(cc["label"][c])
+                if components == "largest":
+                    same = cc["label"] == e["label"]
+                    e["components"] = int(np.count_nonzero(same))
+                    e["discarded_voxels"] = int(cc["voxels"][same].sum() - cc["voxels"][c])
+                else:
+                    e["component"] = c
+            entries += part
+    return entries
 
 
 def object_inventory(model_fine, scene_transform, extents=None, grid_dim=256, level=0.45, trim=0.0, objects=None, near=4.0,
-                     far=15.0, N_importance=128):
+                     far=15.0, N_importance=128, components=None, connectivity=26, min_voxels=1):
     """Which objects the model found and where: one selected occupancy sweep of model_fine (keeping `objects`, default every
-    label except ins_num, as object_meshes) with its label grid, then inventory_from_grid."""
+    label except ins_num, as object_meshes) with its label grid, then inventory_from_grid (components, connectivity and
+    min_voxels as there)."""
     from .mesh import check_transform
     T = check_transform(scene_transform)
     dev = next(model_fine.parameters()).device
@@ -329,7 +384,78 @@ def object_inventory(model_fine, scene_transform, extents=None, grid_dim=256, le
     with torch.no_grad():
         occ, labels = occupancy_objects(model_fine, T, object_mask(ins_num, keep=objects), grid_dim, extents, near, far,
                                         N_importance, device=dev)
-        return inventory_from_grid(occ, labels, T, extents, level, trim, objects)
+        return inventory_from_grid(occ, labels, T, extents, level, trim, objects, components, connectivity, min_voxels)
+
+
+# ----------------------------------------------------------------------------------------------------------------- components
+# DESIGN.md, "Connected components": the solid points of a labelled grid split into components, numbered by their smallest
+# C-order index; the inventory runs on a group grid that maps the chosen components to groups 0 .. 126 and the rest to 127.
+GROUP_BATCH = MAX_LABELS - 1         # components per inventory batch
+DISCARD_GROUP = MAX_LABELS - 1       # the group of every point outside the batch
+
+
+def object_components(occ, labels=None, level=0.45, connectivity=26):
+    """dmnerf_object_components + dmnerf_component_table: the connected components of the solid points (occ > level) of
+    occ [dim]^3 float32, adjacency within one label of labels [dim]^3 int16 (None: one label) -> {"grid": int32 [dim]^3 on the
+    device (component id, -1 where not solid), "label": int16 [n], "voxels": int64 [n], "root": int64 [n] (the component's
+    smallest C-order linear index)}; ids ascend with the root."""
+    dim = _check_grid(occ, labels, "object_components")
+    ctx = get_context(occ.device)
+    grid = torch.empty(occ.shape, dtype=torch.int32, device=occ.device)
+    n = C.c_int64(0)
+    ctx.call("dmnerf_object_components", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), dim, float(level),
+             MAX_LABELS if labels is not None else 1, int(connectivity), _lib.ptr(grid, torch.int32), C.byref(n))
+    n = int(n.value)
+    label = torch.empty(n, dtype=torch.int16, device=occ.device)
+    voxels = torch.empty(n, dtype=torch.int64, device=occ.device)
+    root = torch.empty(n, dtype=torch.int64, device=occ.device)
+    ctx.call("dmnerf_component_table", ctx.handle, _lib.ptr(grid, torch.int32), _lib.ptr(labels, torch.int16), dim, n,
+             _lib.ptr(label, torch.int16), _lib.ptr(voxels, torch.int64), _lib.ptr(root, torch.int64))
+    return {"grid": grid, "label": label.cpu().numpy(), "voxels": voxels.cpu().numpy(), "root": root.cpu().numpy()}
+
+
+def component_groups(grid, lut, discard):
+    """dmnerf_component_groups: the int16 group grid lut[id] of a component id grid, `discard` where it is -1 (not solid)."""
+    _lib.need_cuda("component_groups", grid)
+    lut = torch.as_tensor(np.asarray(lut, dtype=np.int16)).to(grid.device)
+    out = torch.empty(grid.shape, dtype=torch.int16, device=grid.device)
+    ctx = get_context(grid.device)
+    ctx.call("dmnerf_component_groups", ctx.handle, _lib.ptr(grid, torch.int32), grid.shape[0], lut.shape[0],
+             _lib.ptr(lut, torch.int16), int(discard), _lib.ptr(out, torch.int16))
+    return out
+
+
+def largest_components(label, voxels):
+    """{label: id of its largest component}; on a tie in voxels the smaller id (the smaller root) wins."""
+    label, voxels = np.asarray(label, dtype=np.int64), np.asarray(voxels, dtype=np.int64)
+    order = np.lexsort((np.arange(label.shape[0]), -voxels, label))       # by label, then most voxels, then smallest id
+    first = np.ones(order.shape[0], dtype=bool)
+    first[1:] = label[order][1:] != label[order][:-1]
+    return {int(label[c]): int(c) for c in order[first]}
+
+
+def select_components(label, voxels, components, groups, min_voxels=1):
+    """The component ids an inventory reports, in entry order: "largest": each label of `groups`' largest component, ascending
+    label; "split": every component of a label of `groups` with at least min_voxels voxels, by (label, root)."""
+    groups = set(int(g) for g in groups)
+    if components == "largest":
+        best = largest_components(label, voxels)
+        return [best[k] for k in sorted(best) if k in groups]
+    label, voxels = np.asarray(label, dtype=np.int64), np.asarray(voxels, dtype=np.int64)
+    ids = np.nonzero(np.isin(label, sorted(groups)) & (voxels >= min_voxels))[0]
+    return [int(c) for c in ids[np.lexsort((ids, label[ids]))]]
+
+
+def group_luts(ids, n_components):
+    """Batches of GROUP_BATCH of the component ids `ids` -> [(lut int16 [n_components], batch ids)]: lut[batch[g]] = g, every
+    other component DISCARD_GROUP."""
+    out = []
+    for s in range(0, len(ids), GROUP_BATCH):
+        batch = list(ids[s:s + GROUP_BATCH])
+        lut = np.full(n_components, DISCARD_GROUP, dtype=np.int16)
+        lut[batch] = np.arange(len(batch), dtype=np.int16)
+        out.append((lut, batch))
+    return out
 
 
 def camera_region(poses, hwk, far):

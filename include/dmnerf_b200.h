@@ -382,6 +382,27 @@ DMNERF_API int dmnerf_object_voxels(dmnerf_ctx* ctx, const float* occ, const int
 DMNERF_API int dmnerf_object_spans(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                                    const int32_t* boxes_host, const double* axes_host, double* spans_host, void* stream);
 
+/* ---- connected components (DESIGN.md, "Connected components"; no counterpart in the original) --------------------------------
+ * The solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order, p = (i dim + j) dim + k) split into components:
+ * two solid points are adjacent when they are face neighbours (connectivity 6) or face, edge or corner neighbours (26), never
+ * across a grid face, and, with labels (DEVICE int16, may be NULL), carry the same label.  A component's root is its smallest p;
+ * components are numbered 0 .. n - 1 in ascending root order, so every result is canonical and bit-reproducible.  dim must be in
+ * [2, 1290] (dim^3 < 2^31).  Each call validates on the device and reads back once (synchronises the stream) before anything is
+ * reported.
+ * dmnerf_object_components: comp [dim^3] (DEVICE int32) = the point's component id, or -1 where not solid; n_components_host =
+ *   n.  Fails when n_labels is outside [1, 128], connectivity is not 6 or 26, the grid holds NaN or a label (of any point) is
+ *   outside [0, n_labels - 1].
+ * dmnerf_component_table: per component of comp (n components) label [n] (DEVICE int16; 0 without labels), voxels [n] and
+ *   root [n] (DEVICE int64).  Fails when comp holds an id outside [-1, n).
+ * dmnerf_component_groups: groups [dim^3] (DEVICE int16) = lut[comp[p]] (lut: DEVICE int16 [n]), or `discard` where comp is -1;
+ *   the group grid of the inventory entry points above.  Fails when comp holds an id outside [-1, n). */
+DMNERF_API int dmnerf_object_components(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                                        int connectivity, int32_t* comp, int64_t* n_components_host, void* stream);
+DMNERF_API int dmnerf_component_table(dmnerf_ctx* ctx, const int32_t* comp, const int16_t* labels, int dim, int64_t n, int16_t* label,
+                                      int64_t* voxels, int64_t* root, void* stream);
+DMNERF_API int dmnerf_component_groups(dmnerf_ctx* ctx, const int32_t* comp, int dim, int64_t n, const int16_t* lut, int discard,
+                                       int16_t* groups, void* stream);
+
 /* ---- test-view evaluation: render_test, networks/tester.py (+ ins_eval / calculate_ap, networks/evaluator.py:77-175) -------
  * Rules and deviations: DESIGN.md, "Evaluation metrics".  Every result is deterministic (fixed-order reductions, integer atomics
  * only).  `res` is DEVICE memory; reading it back is the caller's one device->host transfer per frame.  `ws` is caller-provided

@@ -9,7 +9,8 @@ DIR/NAME.ply (the marching-cubes mesh in scene space) and DIR/color_NAME.ply (cl
 Without --color-dict (JSON: label -> colour index) and --palette (.npy [K, 3] uint8), label k gets colour k of a fixed
 seeded palette.  --per-object also writes DIR/NAME_obj{k}.ply for every object k: the cleaned mesh of that object alone, from
 a selected occupancy sweep whose grid points are labelled by the network (closed wherever the object does not touch the grid
-boundary); --objects limits it to the labels given."""
+boundary); --objects limits it to the labels given, and --largest-component meshes each object's largest connected component
+alone (DESIGN.md, "Connected components")."""
 import argparse
 import json
 import os
@@ -42,8 +43,13 @@ def parse(argv=None):
     ap.add_argument("--palette", default=None)
     ap.add_argument("--per-object", action="store_true", help="also write NAME_obj{k}.ply, one mesh per object")
     ap.add_argument("--objects", type=int, nargs="+", default=None, help="with --per-object: only these labels")
+    ap.add_argument("--largest-component", action="store_true",
+                    help="with --per-object: mesh each object's largest connected component only")
     ap.add_argument("--device", default="cuda")
-    return ap.parse_args(argv)
+    a = ap.parse_args(argv)
+    if a.largest_component and not a.per_object:
+        ap.error("--largest-component needs --per-object")
+    return a
 
 
 def main(argv=None):
@@ -73,7 +79,8 @@ def main(argv=None):
     if a.per_object:
         from dmnerf_b200.objects import object_meshes
         meshes = object_meshes(nets[1], nets[0], T, objects=a.objects, grid_dim=a.grid_dim, extents=tuple(a.extents), near=a.near, far=a.far,
-                               N_importance=a.N_importance, min_cluster=a.min_cluster)
+                               N_importance=a.N_importance, min_cluster=a.min_cluster,
+                               components="largest" if a.largest_component else None)
         for k, m in meshes.items():
             name = "%s_obj%d.ply" % (a.name, k)
             M.write_ply(os.path.join(a.out, name), m["clean_vertices"], m["clean_triangles"])

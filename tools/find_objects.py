@@ -3,13 +3,16 @@
 
     python tools/find_objects.py CHECKPOINT.tar (--transform T [--extents X Y Z] | --poses POSES.npy --hwk H W K) [--trim 0]
                                  [--grid-dim 256] [--level 0.45] [--near 4 --far 15] [--out DIR]
+                                 [--components {largest,split} [--connectivity {6,26}] [--min-voxels N]]
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict`.  The grid is either given (--transform: a 4x4 as
 .npy or 16 numbers of text, with --extents, default the original's 1.9 7 7) or found from the cameras (--poses: [N, 4, 4] or
 [N, 3, 4] camera-to-world, --hwk: height, width and K as a .npy path or 9 numbers): the scene box of the fine network's solid
 points inside the cameras' view, which --out then receives as scene_transform.txt and extents.txt for tools/extract_mesh.py
 --extents.  Prints one JSON line: the box used and one entry per object (label, voxels, volume, centre, aabb, obb), all in the
-network frame, the frame of the camera poses and of manipulator_eval's transforms."""
+network frame, the frame of the camera poses and of manipulator_eval's transforms.  --components splits each label into
+connected components (DESIGN.md, "Connected components"): `largest` reports each object's largest component and adds its
+label's component count and discarded voxels; `split` reports every component of at least --min-voxels voxels, with its id."""
 import argparse
 import json
 import os
@@ -37,8 +40,18 @@ def parse(argv=None):
     ap.add_argument("--far", type=float, default=15.0)
     ap.add_argument("--N-importance", type=int, default=128)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--components", choices=("largest", "split"), default=None,
+                    help="split each label into connected components: its largest one, or every one")
+    ap.add_argument("--connectivity", type=int, choices=(6, 26), default=None, help="with --components: 6 or 26 (default)")
+    ap.add_argument("--min-voxels", type=int, default=None, help="with --components split: the smallest component reported")
     ap.add_argument("--device", default="cuda")
     a = ap.parse_args(argv)
+    if a.components is None and a.connectivity is not None:
+        ap.error("--connectivity needs --components")
+    if a.min_voxels is not None and a.components != "split":
+        ap.error("--min-voxels needs --components split")
+    if a.min_voxels is not None and a.min_voxels < 1:
+        ap.error("--min-voxels must be >= 1")
     if a.poses is not None:
         if not a.hwk or len(a.hwk) not in (3, 11):
             ap.error("--poses needs --hwk H W K (K as a .npy path or 9 numbers)")
@@ -48,10 +61,22 @@ def parse(argv=None):
 
 
 def _json(e):
-    return {"label": e["label"], "voxels": e["voxels"], "volume": e["volume"], "centre": e["centre"].tolist(),
-            "aabb": [e["aabb"][0].tolist(), e["aabb"][1].tolist()],
-            "obb": {"centre": e["obb"]["centre"].tolist(), "axes": e["obb"]["axes"].tolist(),
-                    "half_sizes": e["obb"]["half_sizes"].tolist()}}
+    out = {"label": e["label"], "voxels": e["voxels"], "volume": e["volume"], "centre": e["centre"].tolist(),
+           "aabb": [e["aabb"][0].tolist(), e["aabb"][1].tolist()],
+           "obb": {"centre": e["obb"]["centre"].tolist(), "axes": e["obb"]["axes"].tolist(),
+                   "half_sizes": e["obb"]["half_sizes"].tolist()}}
+    for k in ("component", "components", "discarded_voxels"):          # with --components
+        if k in e:
+            out[k] = e[k]
+    return out
+
+
+def components_args(a):
+    """The component arguments of object_inventory for the parsed flags: none without --components."""
+    if a.components is None:
+        return {}
+    return {"components": a.components, "connectivity": 26 if a.connectivity is None else a.connectivity,
+            "min_voxels": 1 if a.min_voxels is None else a.min_voxels}
 
 
 def main(argv=None):
@@ -70,7 +95,7 @@ def main(argv=None):
         T = np.load(a.transform) if a.transform.endswith(".npy") else np.loadtxt(a.transform)
         T, ext = M.check_transform(np.asarray(T, dtype=np.float64).reshape(4, 4)), np.asarray(a.extents, dtype=np.float64)
     inv = object_inventory(nf, T, tuple(ext), grid_dim=a.grid_dim, level=a.level, trim=a.trim, near=a.near, far=a.far,
-                           N_importance=a.N_importance)
+                           N_importance=a.N_importance, **components_args(a))
     files = []
     if a.out is not None and a.poses is not None:
         os.makedirs(a.out, exist_ok=True)
