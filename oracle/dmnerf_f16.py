@@ -77,6 +77,54 @@ def render_f16(rays_o, rays_d, p_coarse, p_fine, z_coarse, n_importance=128):
             "rgb_coarse": rgb_c, "ins_coarse": ins_c, "depth_coarse": depth_c, "z_vals_coarse": z_coarse}
 
 
+def net_inputs_fp32(rays_o, rays_d, z):
+    """The network inputs [N * S, 90] as the kernels form them in rays mode and in the fused render (mlp_umma.cu, prologue):
+    in fp32, every operation rounded, in the kernel's order -- pts = o + d * z, |d| = sqrt((d0^2 + d1^2) + d2^2), viewdir =
+    d / |d| -- then embedded with fp32 sin / cos of x * 2^k (exact scalings).  The kernel's own sin / cos is within 2 ulp of
+    these, so a comparison on these inputs is free of the fp32-vs-fp64 input term (up to 2^9 |x| ulp at frequency 2^9)."""
+    o, d, z = rays_o.float(), rays_d.float(), z.float()
+    pts = o[:, None, :] + d[:, None, :] * z[..., None]
+    nrm = torch.sqrt((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2])
+    vd = (d / nrm[:, None])[:, None, :].expand(pts.shape)
+    return points_inputs_fp32(pts.reshape(-1, 3), vd.reshape(-1, 3))
+
+
+def points_inputs_fp32(pts, viewdirs):
+    """The network inputs [M, 90] of points mode: the fp32 points and view directions embedded as they are."""
+    return torch.cat([O.embed(pts.float(), 10), O.embed(viewdirs.float(), 4)], -1)
+
+
+def embed_freq_scale(n_freqs):
+    """[3 + 6 L]: the factor 2^k each column of O.embed multiplies its input by (1 for the identity columns)."""
+    return torch.tensor([1.0] * 3 + [float(2 ** k) for k in range(n_freqs) for _ in range(6)], dtype=torch.float64)
+
+
+def render_on_depths(net_c, net_f, rays_o, rays_d, z_coarse, z_fine, fp32_inputs=True, keep=None, keep_all_ins=False):
+    """Teacher-forced render: the two networks at the caller's coarse [N, S] and fine [N, F] depths (a kernel's own), each pass
+    composited in fp64 (O.composite), optionally with the object selection objects_oracle.select_objects(raw, keep) applied
+    before the composite.  net_c / net_f: x [M, 90] -> raw [M, C] (mlp_forward_f16 or O.mlp_forward in fp64, closed over the
+    weights); either may be None to skip its pass.  fp32_inputs: the networks see net_inputs_fp32 (the kernels' inputs);
+    otherwise O._net_inputs in fp64 (O.render's own).  Returns, per pass p in (coarse, fine): rgb_p, depth_p, acc_p, ins_p,
+    weights_p, raw_p (unselected), labels_p (per-sample arg-max label, first maximum) and gap_p (per sample, the largest
+    instance sigmoid minus the second largest)."""
+    from . import objects_oracle as OO
+    ro, rd = rays_o.double(), rays_d.double()
+    viewdirs = rd / torch.norm(rd, dim=-1, keepdim=True)
+    out = {}
+    for tag, net, z in (("coarse", net_c, z_coarse), ("fine", net_f, z_fine)):
+        if net is None:
+            continue
+        z = z.double()
+        x = net_inputs_fp32(rays_o, rays_d, z) if fp32_inputs else O._net_inputs(ro, rd, viewdirs, z)[0]
+        raw = net(x).double().reshape(z.shape[0], z.shape[1], -1)
+        sel = raw if keep is None else OO.select_objects(raw, keep)
+        rgb, w, depth, ins, acc = O.composite(sel, z, rd, keep_all_ins=keep_all_ins)
+        top2 = torch.topk(torch.sigmoid(raw[..., 4:]), 2, dim=-1).values
+        out.update({"rgb_" + tag: rgb, "depth_" + tag: depth, "acc_" + tag: acc, "ins_" + tag: ins, "weights_" + tag: w,
+                    "raw_" + tag: raw, "labels_" + tag: OO.object_labels(raw), "gap_" + tag: top2[..., 0] - top2[..., 1]})
+    return out
+
+
 def psnr(got, ref):
     """rgb PSNR in dB (peak 1) of got against ref."""
     mse = float(((got.double() - ref.double()) ** 2).mean())

@@ -99,6 +99,33 @@ def sample_pdf(bins, weights, n_samples, det=False, u=None):
     return bin_b + t * (bin_a - bin_b)                                              # :153
 
 
+def sample_pdf_explained(bins, weights, n_samples, det, u, tol):
+    """Bool [N, n_samples]: which samples of sample_pdf(bins, weights, n_samples, det, u) the inverse CDF itself makes
+    ill-conditioned, so that an fp32 implementation may legitimately land more than `tol` away from the fp32 oracle there:
+      (a) u within a few ulp of a CDF knot (searchsorted picks the neighbouring bin),
+      (b) a 3e-7 perturbation of the CDF (2 ulp of a value in [0,1]) already moves the sample by more than half the tolerance
+          (tiny denom = almost empty bin, helpers.py:150-152), or
+      (c) the reference's own arithmetic in fp64 lands elsewhere too.
+    A miss outside this mask is an arithmetic error of the implementation.  bins [N, B], weights [N, B - 1], u [N, n_samples] or
+    None (det), tol: scalar or array broadcastable to [N, n_samples]."""
+    bins, weights = bins.cpu(), weights.cpu()
+    u = None if u is None else u.cpu()
+    n = bins.shape[0]
+    ref = sample_pdf(bins.float(), weights.float(), n_samples, det=det, u=None if u is None else u.float()).numpy()
+    uu = (torch.linspace(0.0, 1.0, n_samples).expand(n, n_samples) if det else u).double()
+    wd = weights.double() + 1e-5
+    cdf = torch.cat([torch.zeros(n, 1, dtype=torch.float64), torch.cumsum(wd / wd.sum(-1, keepdim=True), -1)], -1)
+    knot = (uu[..., None] - cdf[:, None, :]).abs().min(-1).values.numpy() <= 4e-7                           # (a)
+    inds = torch.searchsorted(cdf.float().contiguous(), uu.float().contiguous(), right=True)
+    below, above = (inds - 1).clamp(min=0), inds.clamp(max=cdf.shape[-1] - 1)
+    denom = (torch.gather(cdf, -1, above) - torch.gather(cdf, -1, below))
+    width = (torch.gather(bins.double(), -1, above) - torch.gather(bins.double(), -1, below)).abs()
+    cond = (width * 3e-7 / denom.clamp(min=1e-12)).numpy() > 0.5 * tol                                        # (b)
+    twin = sample_pdf(bins.double(), weights.double(), n_samples, det=det, u=None if u is None else u.double()).numpy()
+    twin_bad = np.abs(twin - ref) > tol                                                                       # (c)
+    return knot | cond | twin_bad
+
+
 def z_val_sample(n_rays, near, far, n_samples, dtype=torch.float32):
     """reference networks/helpers.py:114-119: near + linspace(0,1,S) * (far - near), expanded to N rows."""
     t = torch.linspace(0.0, 1.0, steps=n_samples, dtype=dtype)

@@ -163,8 +163,8 @@ def test_render_frame_driver_matches_explicit_rays():
 def test_host_entry_point_in_parts_is_bitwise_the_single_launch():
     """dmnerf_render_forward_host on >= 131 072 rays renders the batch in four parts whose copies overlap the neighbouring
     parts' kernels (second stream): same bits as the device-resident single launch, odd ray count, per-ray depth rows
-    (z_row_stride != 0) and the shared row (stride 0), a small batch (single part) through the same call, and an object
-    selection (io.keep with FLAG_SELECT) against dmnerf_render_forward with the same mask."""
+    (z_row_stride != 0) and the shared row (stride 0), a small batch (single part) through the same call, an object
+    selection (io.keep with FLAG_SELECT) against dmnerf_render_forward with the same mask, and the fp16 preview network."""
     import ctypes as C
     from dmnerf_b200.testing import make_models
     from dmnerf_b200.engine import get_context
@@ -174,8 +174,13 @@ def test_host_entry_point_in_parts_is_bitwise_the_single_launch():
     nc, nf, _, _ = make_models(5, 6, 13, "cuda")
     ctx = get_context(torch.device("cuda"))
     ctx.bind(0, nc); ctx.bind(1, nf)
-    cases = ((131073, False, None), (131080, True, None), (4097, False, None), (131073, False, [0, 2, 3, 7, 13]))
-    for n, per_ray_z, keep in cases:
+    F16 = _lib.IMPL_UMMA_F16
+    with torch.no_grad():                                               # pack the fp16 images outside the launch count
+        render_rays(torch.from_numpy(wl["rays_o"][:2]).cuda(), torch.from_numpy(wl["rays_d"][:2]).cuda(), nc, nf,
+                    torch.linspace(float(wl["near"]), float(wl["far"]), 64, device="cuda"), want_raw=False, impl=F16)
+    cases = ((131073, False, None, 0), (131080, True, None, 0), (4097, False, None, 0), (131073, False, [0, 2, 3, 7, 13], 0),
+             (131073, True, None, F16))
+    for n, per_ray_z, keep, impl in cases:
         ro = torch.from_numpy(wl["rays_o"][:n]).contiguous().pin_memory()
         rd = torch.from_numpy(wl["rays_d"][:n]).contiguous().pin_memory()
         zrow = torch.linspace(float(wl["near"]), float(wl["far"]), 64)
@@ -191,14 +196,15 @@ def test_host_entry_point_in_parts_is_bitwise_the_single_launch():
             io.keep[:] = object_mask(13, keep=keep)
         flags = 0 if keep is None else _lib.FLAG_SELECT
         before = _lib.launch_count()
-        _lib.check(ctx.lib.dmnerf_render_forward_host(ctx.handle, io, n, 64, 128, flags, 0, ctx.stream()), "dmnerf_render_forward_host")
+        _lib.check(ctx.lib.dmnerf_render_forward_host(ctx.handle, io, n, 64, 128, flags, impl, ctx.stream()), "dmnerf_render_forward_host")
         launches = _lib.launch_count() - before
         assert launches == (4 if n >= 131072 else 1), launches
         with torch.no_grad():
             zdev = zc.cuda() if per_ray_z else zc.cuda()[None].expand(n, 64)
-            ref = render_rays(ro.cuda(), rd.cuda(), nc, nf, zdev, N_importance=128, want_raw=False, keep_objects=keep)
+            ref = render_rays(ro.cuda(), rd.cuda(), nc, nf, zdev, N_importance=128, want_raw=False, keep_objects=keep,
+                              impl=impl)
         for k, v in out.items():
-            assert torch.equal(v, ref[k].cpu()), (n, keep, k)
+            assert torch.equal(v, ref[k].cpu()), (n, keep, impl, k)
 
 
 def _manip_setup(golden_dir):

@@ -51,23 +51,31 @@ def _equal(a, b, keys):
 
 
 # ------------------------------------------------------------------------------------------ nothing changes without a selection
-@pytest.mark.parametrize("name", ["dmsr_study", "replica_room0_93"])
-def test_keep_all_is_bit_identical(name):
+@pytest.mark.parametrize("name,ins_num,impl", [
+    pytest.param("dmsr_study", 13, _lib.IMPL_AUTO, id="dmsr_study"),
+    pytest.param("replica_room0_93", 93, _lib.IMPL_AUTO, id="replica_room0_93"),
+    # the fp16 preview network's selected kernel (render_objects_f16_kernel) at 2, 14 and 128 label channels
+    pytest.param("dmsr_study", 1, _lib.IMPL_UMMA_F16, id="dmsr_study-f16-ins1"),
+    pytest.param("dmsr_study", 13, _lib.IMPL_UMMA_F16, id="dmsr_study-f16-ins13"),
+    pytest.param("dmsr_study", 127, _lib.IMPL_UMMA_F16, id="dmsr_study-f16-ins127")])
+def test_keep_all_is_bit_identical(name, ins_num, impl):
+    """A selection that keeps every label gives the unselected maps bit for bit: fused kernel (impl), stage kernels (SIMT),
+    frame driver (impl)."""
     wl, ro, rd = _rays(name, 1024)
-    ins_num = wl["ins_num"]
     nc, nf, _, _ = make_models(101, 202, ins_num, DEV)
     everything = list(range(ins_num + 1))
     with torch.no_grad():
-        fused = render_rays(ro, rd, nc, nf, _z(wl), want_raw=False, want_samples=True)
-        fused_sel = render_rays(ro, rd, nc, nf, _z(wl), want_raw=False, want_samples=True, keep_objects=everything)
+        fused = render_rays(ro, rd, nc, nf, _z(wl), want_raw=False, want_samples=True, impl=impl)
+        fused_sel = render_rays(ro, rd, nc, nf, _z(wl), want_raw=False, want_samples=True, keep_objects=everything, impl=impl)
         _equal(fused, fused_sel, fused.keys())
         simt = render_rays(ro, rd, nc, nf, _z(wl), impl=_lib.IMPL_SIMT)
         simt_sel = render_rays(ro, rd, nc, nf, _z(wl), impl=_lib.IMPL_SIMT, keep_objects=everything)
         _equal(simt, simt_sel, simt.keys())
         K, c2w = wl["K"], wl["c2w"]
-        fr = render_frame(wl["H"], wl["W"], K, c2w, wl["near"], wl["far"], nc, nf, pixel_range=(100000, 8192), device=DEV)
+        fr = render_frame(wl["H"], wl["W"], K, c2w, wl["near"], wl["far"], nc, nf, pixel_range=(100000, 8192), device=DEV,
+                          impl=impl)
         fr_sel = render_frame(wl["H"], wl["W"], K, c2w, wl["near"], wl["far"], nc, nf, pixel_range=(100000, 8192), device=DEV,
-                              keep_objects=everything)
+                              keep_objects=everything, impl=impl)
         _equal(fr, fr_sel, fr.keys())
     get_context(DEV).sync_check()
 

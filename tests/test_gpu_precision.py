@@ -9,7 +9,8 @@ boundary because of it), so FP16_TWIN_FRACTION of the fp16 error is the allowanc
 and 93).  A kernel that dropped or doubled a pass, or rounded anything differently, would sit at 1x or more.  That comparison
 uses embedded inputs, which both see bit for bit: in rays mode the kernel forms the points and their sin / cos in fp32, and at
 frequency 2^9 that input difference is as large as the fp16 rounding itself (0.3x - 0.6x measured), so rays mode is held to the
-fp64 bound only (so is points mode, which embeds fp32 points)."""
+fp64 bound only (so is points mode, which embeds fp32 points).  tests/test_gpu_preview_edges.py holds rays and points mode to
+the restatement too, run on the kernels' own fp32 inputs (oracle/dmnerf_f16.net_inputs_fp32)."""
 import copy
 import os
 import sys

@@ -73,6 +73,68 @@ def test_fp16_oracle_rounds_its_operands():
     assert e16 > 30 * e32, (e16, e32)
 
 
+@pytest.mark.parametrize("name", ["dmsr_study", "replica_room0_93"])
+def test_fp32_twin_inputs_are_within_a_few_ulp_of_the_fp64_embedding(name):
+    """net_inputs_fp32 and points_inputs_fp32 (the kernels' fp32 inputs) against O.embed of the same rays in fp64: every column
+    within 4 fp32 ulp (2^-23) of (2^k |x| + 1), where 2^k is the column's frequency and |x| the scale of its coordinate
+    (|o| + |d z| for a point, |viewdir| for a direction).  The identity columns are the fp32 point and direction themselves."""
+    ro, rd, _, _, _ = _case(name, 48)
+    ro, rd = ro.float(), rd.float()
+    gen = torch.Generator().manual_seed(3)
+    wl = synth.workload(name)
+    z = (torch.rand(48, 37, generator=gen, dtype=torch.float64) * (wl["far"] - wl["near"]) + wl["near"]).float()
+    twin = H.net_inputs_fp32(ro, rd, z).double()
+    ro64, rd64, z64 = ro.double(), rd.double(), z.double()
+    vd64 = rd64 / torch.norm(rd64, dim=-1, keepdim=True)
+    x64, _ = O._net_inputs(ro64, rd64, vd64, z64)
+    pt_scale = (ro64.abs()[:, None, :] + (rd64[:, None, :] * z64[..., None]).abs()).reshape(-1, 3)
+    vd_scale = vd64.abs()[:, None, :].expand(48, 37, 3).reshape(-1, 3)
+    ulp = 2.0 ** -23
+    tol = torch.cat([4 * ulp * (H.embed_freq_scale(10) * pt_scale.repeat(1, 21) + 1),
+                     4 * ulp * (H.embed_freq_scale(4) * vd_scale.repeat(1, 9) + 1)], -1)
+    err = (twin - x64).abs()
+    assert bool((err <= tol).all()), float((err / tol).max())
+    assert float(err[:, 3 + 6 * 9:63].max()) > 0.0           # the fp32 inputs are not fp64 in disguise
+    # points mode: the fp32 points and directions embedded as they are
+    pts = (ro[:, None, :] + rd[:, None, :] * z[..., None]).reshape(-1, 3)
+    dirs = (rd / torch.norm(rd, dim=-1, keepdim=True))[:, None, :].expand(48, 37, 3).reshape(-1, 3)
+    xp = H.points_inputs_fp32(pts, dirs).double()
+    xp64 = torch.cat([O.embed(pts.double(), 10), O.embed(dirs.double(), 4)], -1)
+    assert torch.equal(xp[:, :3], pts.double()) and torch.equal(xp[:, 63:66], dirs.double())
+    assert float((xp - xp64).abs().max()) <= 2 * ulp
+
+
+@pytest.mark.parametrize("keep_all_ins", [False, True])
+def test_render_on_depths_reproduces_the_oracle_render(keep_all_ins):
+    """render_on_depths with the fp64 network and fp64 inputs, on O.render's own coarse and fine depths, gives O.render's maps
+    and weights to fp64 rounding; with an object selection, objects_oracle.render's.  Labels are the first maximum of the
+    instance sigmoids and the gap is the distance to the second largest."""
+    from oracle import objects_oracle as OO
+    ro, rd, wc, wf, z = _case("dmsr_study", 40)
+    p64c, p64f = O.to_torch(wc, torch.float64), O.to_torch(wf, torch.float64)
+    net_c, net_f = (lambda x: O.mlp_forward(p64c, x)), (lambda x: O.mlp_forward(p64f, x))
+    ins_num = wc["ins_linear.weight"].shape[0] - 1
+    keep = torch.zeros(ins_num + 1, dtype=torch.bool)
+    keep[[0, 2, 5, ins_num]] = True
+    for sel in (None, keep):
+        ref = O.render(ro, rd, p64c, p64f, z) if sel is None else OO.render(ro, rd, p64c, p64f, z, sel)
+        got = H.render_on_depths(net_c, net_f, ro, rd, ref["z_vals_coarse"], ref["z_vals_fine"], fp32_inputs=False, keep=sel,
+                                 keep_all_ins=keep_all_ins)
+        for p in ("coarse", "fine"):
+            want = O.composite(ref["raw_" + p] if sel is None else OO.select_objects(ref["raw_" + p], sel), ref["z_vals_" + p],
+                               rd, keep_all_ins=keep_all_ins)
+            for k, v in zip(("rgb", "weights", "depth", "ins", "acc"), want):
+                assert torch.allclose(got["%s_%s" % (k, p)], v, rtol=1e-12, atol=1e-12), (k, p)
+            if not keep_all_ins:
+                for k in ("rgb", "depth", "ins", "acc", "weights"):
+                    assert torch.allclose(got["%s_%s" % (k, p)], ref["%s_%s" % (k, p)], rtol=1e-12, atol=1e-12), (k, p)
+            raw = got["raw_" + p]
+            assert torch.allclose(raw, ref["raw_" + p], rtol=1e-12, atol=1e-12)
+            assert torch.equal(got["labels_" + p], OO.object_labels(raw))
+            s = torch.sigmoid(raw[..., 4:]).sort(-1, descending=True).values
+            assert torch.equal(got["gap_" + p], s[..., 0] - s[..., 1]) and bool((got["gap_" + p] >= 0).all())
+
+
 def _sass_counts():
     path = os.path.join(ROOT, "dm-nerf_b200", "lib", "libdmnerf_b200.so")
     if shutil.which("cuobjdump") is None:
