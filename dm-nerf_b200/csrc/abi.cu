@@ -70,6 +70,8 @@ struct dmnerf_ctx {
   MeshState* mesh = nullptr;      // buffers of the other mesh entry points (mesh.cu)
   InventoryState* inventory = nullptr;   // buffers of the object-inventory entry points (inventory.cu)
   ComponentsState* components = nullptr;   // buffers of the connected-component entry points (components.cu)
+  Region region = {};             // region selection read with DMNERF_FLAG_REGION (dmnerf_set_region); bits == NULL: none set
+  Scratch region_tmp;             // dmnerf_region_dilate: the second buffer of a multi-step dilation
   bool profiling = false;
   bool last_fused = false;       // the last render call took the single-kernel path
   bool profile_valid = false;
@@ -86,6 +88,22 @@ static int render_mask(const dmnerf_ctx* ctx, const dmnerf_render_io* io, int fl
                        const char* who) {
   const bool pair = ctx && ctx->net[0].bound && ctx->net[1].bound && ctx->net[0].ins_num == ctx->net[1].ins_num;
   return object_mask((flags & DMNERF_FLAG_SELECT) && io ? io->keep : nullptr, pair ? ctx->net[0].ins_num + 1 : 0, m, keep, who);
+}
+
+// The region of a render call: the context's (dmnerf_set_region) with DMNERF_FLAG_REGION, else NULL.  Its labels are checked
+// against the bound pair here, as a keep mask's are.
+static int render_region(const dmnerf_ctx* ctx, int flags, const Region*& region, const char* who) {
+  region = nullptr;
+  if (!(flags & DMNERF_FLAG_REGION)) return 0;
+  DMN_CHECK(ctx && ctx->region.bits, "%s: DMNERF_FLAG_REGION without a region (set one with dmnerf_set_region)", who);
+  const bool pair = ctx->net[0].bound && ctx->net[1].bound && ctx->net[0].ins_num == ctx->net[1].ins_num;
+  DMN_CHECK(pair, "%s: a region selection needs the network(s) bound with dmnerf_set_weights (one ins_num)", who);
+  const int n_labels = ctx->net[0].ins_num + 1;
+  for (int b = n_labels; b < 128; ++b)
+    DMN_CHECK(!((ctx->region.applies.w[b >> 5] >> (b & 31)) & 1u), "%s: region applies to label %d, outside [0, %d]", who, b,
+              n_labels - 1);
+  region = &ctx->region;
+  return 0;
 }
 
 extern "C" {
@@ -115,7 +133,7 @@ DMNERF_API int dmnerf_ctx_destroy(dmnerf_ctx* ctx) {
   cudaSetDevice(ctx->device);
   for (int i = 0; i < 2; ++i) umma_weights_free(ctx->packed[i]);
   Scratch* all[] = {&ctx->ws_raw_c, &ctx->ws_raw_f, &ctx->ws_z_c, &ctx->ws_z_f, &ctx->ws_w_c, &ctx->ws_w_f,
-                    &ctx->host_in, &ctx->host_out, &ctx->frame_rays, &ctx->mesh_pts, &ctx->mesh_raw};
+                    &ctx->host_in, &ctx->host_out, &ctx->frame_rays, &ctx->mesh_pts, &ctx->mesh_raw, &ctx->region_tmp};
   for (Scratch* s : all) s->release();
   mesh_state_free(ctx->mesh);
   inventory_state_free(ctx->inventory);
@@ -402,9 +420,9 @@ DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, 
 
 }  // extern "C"
 
-// dm_nerf() on device buffers; keep: object selection (NULL = none, the unselected kernels)
+// dm_nerf() on device buffers; keep: object selection, region: region selection (both NULL = none, the unselected kernels)
 static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
-                               const ObjMask* keep, void* stream) {
+                               const ObjMask* keep, const Region* region, void* stream) {
   DMN_CHECK(ctx && io, "render_forward: NULL ctx/io");
   DMN_CHECK(n >= 0 && S >= 3 && NI >= 2, "render_forward: bad sizes n=%lld S=%d I=%d", (long long)n, S, NI);
   DMN_CHECK(ctx->net[0].bound && ctx->net[1].bound, "render_forward: bind both networks with dmnerf_set_weights first");
@@ -424,7 +442,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   if (impl != DMNERF_IMPL_SIMT && S == 64 && NI == 128 && !io->raw_coarse && !io->raw_fine) {
     const bool prof = ctx->profiling;
     if (prof) DMN_CUDA(cudaEventRecord(ctx->ev[0], st));
-    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep, impl == DMNERF_IMPL_UMMA_F16);
+    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep, impl == DMNERF_IMPL_UMMA_F16, region);
     if (rc) return rc;
     if (prof) for (int i = 1; i <= DMNERF_N_STAGES; ++i) DMN_CUDA(cudaEventRecord(ctx->ev[i], st));
     ctx->profile_valid = prof;
@@ -458,7 +476,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:63     coarse composite
   if ((rc = launch_composite(raw_c, z_c, io->rays_d, n, S, C, keep_ins, io->rgb_coarse, w_c, io->depth_coarse,
-                             io->ins_coarse, io->acc_coarse, st, keep))) return rc;
+                             io->ins_coarse, io->acc_coarse, st, keep, io->rays_o, region))) return rc;
   DMN_STAGE_MARK();
   // render.py:66-70  importance sampling + merge
   if ((rc = launch_hier_sample(z_c, w_c, perturb ? io->u : nullptr, n, S, NI, z_f, st))) return rc;
@@ -468,7 +486,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:86     fine composite
   if ((rc = launch_composite(raw_f, z_f, io->rays_d, n, F, C, keep_ins, io->rgb_fine, io->weights_fine, io->depth_fine,
-                             io->ins_fine, io->acc_fine, st, keep))) return rc;
+                             io->ins_fine, io->acc_fine, st, keep, io->rays_o, region))) return rc;
   DMN_STAGE_MARK();
 #undef DMN_STAGE_MARK
   ctx->profile_valid = prof;
@@ -481,8 +499,9 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
                           void* stream) {
   ObjMask m;
   const ObjMask* keep;
-  if (render_mask(ctx, io, flags, m, keep, "render_forward")) return 1;
-  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, keep, stream), impl, stream);
+  const Region* region;
+  if (render_mask(ctx, io, flags, m, keep, "render_forward") || render_region(ctx, flags, region, "render_forward")) return 1;
+  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, keep, region, stream), impl, stream);
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
@@ -526,7 +545,7 @@ DMNERF_API int dmnerf_profile_read(dmnerf_ctx* ctx, float* ms_out, int n_out) {
 // Host-buffer render: `h` holds HOST pointers for the outputs (and for the inputs unless dev_rays_o / dev_rays_d are given:
 // rays that are already resident on the device, e.g. generated there from the camera).
 static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const float* dev_rays_o, const float* dev_rays_d, int64_t n,
-                            int S, int NI, int flags, int impl, const ObjMask* keep, void* stream) {
+                            int S, int NI, int flags, int impl, const ObjMask* keep, const Region* region, void* stream) {
   DMN_CHECK(ctx && h, "render_forward_host: NULL ctx/io");
   DMN_CHECK(n >= 0, "render_forward_host: negative ray count");
   if (n == 0) return 0;
@@ -616,7 +635,7 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
   const bool parts = n >= HOST_PART_MIN_RAYS && !ctx->profiling;
   if (!parts) {
     if (copy_in(0, n, st)) return 1;
-    int rc = render_forward_impl(ctx, &io, n, S, NI, flags, impl, keep, stream);
+    int rc = render_forward_impl(ctx, &io, n, S, NI, flags, impl, keep, region, stream);
     if (rc) return rc;
     if (copy_out(0, n, st)) return 1;
     return dmnerf_sync_check(ctx, stream);
@@ -646,7 +665,7 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
   for (int i = 0; i < HOST_PARTS && !rc; ++i) {
     if (i > 0) DMN_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[i], 0));
     const dmnerf_render_io pi = part_io(edge[i]);
-    rc = render_forward_impl(ctx, &pi, edge[i + 1] - edge[i], S, NI, flags, impl, keep, stream);
+    rc = render_forward_impl(ctx, &pi, edge[i + 1] - edge[i], S, NI, flags, impl, keep, region, stream);
     if (rc) break;
     DMN_CUDA(cudaEventRecord(ctx->ev_done[i], st));
     DMN_CUDA(cudaStreamWaitEvent(cs, ctx->ev_done[i], 0));
@@ -664,8 +683,9 @@ DMNERF_API int dmnerf_render_forward_host(dmnerf_ctx* ctx, const dmnerf_render_i
                                int impl, void* stream) {
   ObjMask m;
   const ObjMask* keep;
-  if (render_mask(ctx, h, flags, m, keep, "render_forward_host")) return 1;
-  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, keep, stream);
+  const Region* region;
+  if (render_mask(ctx, h, flags, m, keep, "render_forward_host") || render_region(ctx, flags, region, "render_forward_host")) return 1;
+  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, keep, region, stream);
 }
 
 DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
@@ -674,7 +694,9 @@ DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, co
   DMN_CHECK(ctx && K_host && c2w_host && out_host, "render_frame_host: NULL argument");
   ObjMask m;
   const ObjMask* keep;
-  if (render_mask(ctx, out_host, flags, m, keep, "render_frame_host")) return 1;
+  const Region* region;
+  if (render_mask(ctx, out_host, flags, m, keep, "render_frame_host") || render_region(ctx, flags, region, "render_frame_host"))
+    return 1;
   DMN_CHECK(H > 0 && W > 0 && n_coarse >= 3 && n_coarse <= 4096, "render_frame_host: bad sizes H=%d W=%d S=%d", H, W, n_coarse);
   DMN_CHECK(ray_begin >= 0 && ray_count >= 0 && ray_begin + ray_count <= (int64_t)H * W,
             "render_frame_host: pixel range [%lld, +%lld) outside the %dx%d frame", (long long)ray_begin, (long long)ray_count, H, W);
@@ -697,7 +719,7 @@ DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, co
   dmnerf_render_io h = *out_host;
   h.rays_o = nullptr; h.rays_d = nullptr; h.t_rand = nullptr; h.u = nullptr;
   h.z_coarse = z.data(); h.z_row_stride = 0;
-  return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, keep, stream);
+  return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, keep, region, stream);
 }
 
 // ---- mesh extraction (tools/mesh_generator.py mesh_main) ------------------------------------------------------------------
@@ -836,6 +858,55 @@ DMNERF_API int dmnerf_component_groups(dmnerf_ctx* ctx, const int32_t* comp, int
   DMN_CHECK(ctx != nullptr, "component_groups: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
   return component_groups(&ctx->components, comp, dim, n, lut, discard, groups, (cudaStream_t)stream);
+}
+
+// ---- region selection (DESIGN.md, "Region selection") ---------------------------------------------------------------------
+
+DMNERF_API int dmnerf_set_region(dmnerf_ctx* ctx, const uint32_t* bits_device, int dim, const float* voxel_map12,
+                                 const uint32_t* applies_host, int outside_keep) {
+  DMN_CHECK(ctx != nullptr, "set_region: ctx is NULL");
+  if (!bits_device) {
+    ctx->region = Region{};
+    return 0;
+  }
+  DMN_CHECK(voxel_map12 && applies_host, "set_region: NULL voxel map / applies mask");
+  if (region_check(dim, voxel_map12, "set_region")) return 1;
+  Region r = {};
+  r.bits = bits_device;
+  for (int i = 0; i < 12; ++i) r.map[i] = voxel_map12[i];
+  r.dim = dim;
+  r.outside_keep = outside_keep ? 1 : 0;
+  for (int i = 0; i < 4; ++i) r.applies.w[i] = applies_host[i];
+  ctx->region = r;
+  return 0;
+}
+
+DMNERF_API int dmnerf_region_pack(const int32_t* ids, int dim, const uint32_t* table, int64_t n_ids, uint32_t* bits, void* stream) {
+  return region_pack(ids, dim, table, n_ids, bits, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_region_dilate(dmnerf_ctx* ctx, const uint32_t* in, int dim, int radius, int connectivity, int invert,
+                                    uint32_t* out, void* stream) {
+  DMN_CHECK(ctx != nullptr, "region_dilate: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  if (region_check(dim, nullptr, "region_dilate")) return 1;
+  uint32_t* tmp = nullptr;
+  if (radius >= 2) {
+    if (ctx->region_tmp.reserve((size_t)region_words(dim) * sizeof(uint32_t))) return 2;
+    tmp = (uint32_t*)ctx->region_tmp.ptr;
+  }
+  return region_dilate(in, dim, radius, connectivity, invert, out, tmp, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_region_contains(const uint32_t* bits, int dim, const float* voxel_map12, const float* pts, int64_t n,
+                                      uint8_t* out, void* stream) {
+  DMN_CHECK(bits && voxel_map12, "region_contains: NULL bits / voxel map");
+  if (region_check(dim, voxel_map12, "region_contains")) return 1;
+  Region r = {};
+  r.bits = bits;
+  for (int i = 0; i < 12; ++i) r.map[i] = voxel_map12[i];
+  r.dim = dim;
+  return region_contains(r, pts, n, out, (cudaStream_t)stream);
 }
 
 // ---- test-view evaluation (networks/tester.py render_test, networks/evaluator.py ins_eval) --------------------------------

@@ -120,12 +120,27 @@ __host__ __device__ inline bool obj_kept(const ObjMask& m, int label) {
   return (word >> (label & 31)) & 1u;
 }
 
+// Region selection (DESIGN.md, "Region selection"): one bit per point of a sweep grid [dim]^3 (C order, bit v & 31 of word
+// v >> 5), the fp32 voxel map [M | c] (row-major 3x4) from the network frame to grid indices, and the rule's two settings: the
+// labels it applies to and what happens to a sample outside the grid.  bits == NULL: no region.  The per-sample test is
+// region_drops (ray_ops.cuh).
+constexpr int REGION_MAX_DIM = 1290;                          // dim^3 < 2^31, as the component grids
+struct Region {
+  const uint32_t* bits;
+  float map[12];
+  int32_t dim;
+  int32_t outside_keep;        // 1: a sample outside the grid is kept; 0: dropped
+  ObjMask applies;             // labels the region applies to
+};
+inline int64_t region_words(int dim) { return ((int64_t)dim * dim * dim + 31) / 32; }
+
 // ---- launchers implemented in the individual .cu files (all return 0 / non-zero status) ----
 int launch_posenc(const float* x, int64_t m, int n_freqs, float* out, cudaStream_t st);
-// keep: object selection, or NULL for none (the unselected kernel)
+// keep: object selection, or NULL for none (the unselected kernel); region (with rays_o): region selection, or NULL for none.
+// A region without keep runs the selected kernel with every label kept.
 int launch_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all,
                      float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st,
-                     const ObjMask* keep = nullptr);
+                     const ObjMask* keep = nullptr, const float* rays_o = nullptr, const Region* region = nullptr);
 int launch_sample_pdf(const float* bins, const float* weights, int64_t n, int nb, int ns, const float* u, float* out,
                       cudaStream_t st);
 int launch_sort_concat(const float* a, const float* b, int64_t n, int na, int nb, float* out, cudaStream_t st);
@@ -234,6 +249,13 @@ int component_table(ComponentsState** s, const int32_t* comp, const int16_t* lab
                     int64_t* voxels, int64_t* root, cudaStream_t st);
 int component_groups(ComponentsState** s, const int32_t* comp, int dim, int64_t n_comp, const int16_t* lut, int discard,
                      int16_t* groups, cudaStream_t st);
+
+// Region builders (region.cu).  Grids are [dim]^3 in C order; bits are region_words(dim) uint32 words, the tail zero.
+int region_check(int dim, const float* map12, const char* who);      // dim in range, map finite (map12 may be NULL)
+int region_pack(const int32_t* ids, int dim, const uint32_t* table, int64_t n_ids, uint32_t* bits, cudaStream_t st);
+// tmp: region_words(dim) device words, needed when r >= 2
+int region_dilate(const uint32_t* in, int dim, int r, int connectivity, int invert, uint32_t* out, uint32_t* tmp, cudaStream_t st);
+int region_contains(const Region& r, const float* pts, int64_t n, uint8_t* out, cudaStream_t st);
 
 // Test-view evaluation (metrics.cu)
 int64_t eval_workspace_bytes(int64_t n, int k, int H, int W);

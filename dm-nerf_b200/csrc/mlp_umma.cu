@@ -89,6 +89,7 @@ struct KArgs {
   float* acts;                 // training forward (RAW mode): ActPlanes base, or nullptr
   int32_t* status;             // device error word
   ObjMask keep;                // render_objects_kernel: kept object labels
+  Region region;               // render_objects_kernel: region selection (region.bits == NULL: none)
 };
 
 // ------------------------------------------------------------------------------------------------ prologue helpers
@@ -147,7 +148,8 @@ __device__ __forceinline__ void fill_embedding(const float v[3], float* vals /* 
 
 // ------------------------------------------------------------------------------------------------ the kernel
 // Warps 0-7: two consumer warpgroups (MMA issue, epilogues, prologue); warp 8: weight producer.
-// SELECT (fused only): object selection -- samples whose label is not in a.keep get alpha = 0 in both composites.  The body is
+// SELECT (fused only): object selection -- samples whose label is not in a.keep get alpha = 0 in both composites, and so do the
+// samples a.region drops (region selection, when a.region.bits is set).  The body is
 // shared by mlp_umma_kernel (no selection) and render_objects_kernel (FUSED + SELECT) below.  F16: the fp16 preview network
 // (prog and the images are then the fp16 program and images).
 template <bool FUSED, bool SELECT, bool F16>
@@ -578,7 +580,15 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
         if constexpr (SELECT) {
           // the row's label from its logits (128 floats apart per row, i.e. one bank): each lane starts its walk at channel
           // lane mod n, so the 32 rows of a warp read ceil(32 / n) rows per bank below 32 channels and at most 2 above
-          if (!obj_kept(a.keep, argmax_sigmoid(logit + r * 128, n_ins1, (r & 31) % n_ins1))) alpha = 0.0f;
+          const int label = argmax_sigmoid(logit + r * 128, n_ins1, (r & 31) % n_ins1);
+          bool drop = !obj_kept(a.keep, label);
+          if (a.region.bits && !drop) {
+            // region selection: the sample's point as the prologue computed it, from the ray and the depth zi
+            float p[3];
+            ray_point(fz->ray[rl], fz->ray[rl] + 3, zi, p);
+            drop = region_drops(a.region, label, p[0], p[1], p[2]);
+          }
+          if (drop) alpha = 0.0f;
         }
         const float f = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
         const int lane_i = r & 31, wi = r >> 5;
@@ -1025,7 +1035,7 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
 // Whole dm_nerf() pipeline (render.py:31-96) in ONE launch: coarse network -> composite -> importance sampling -> fine
 // network -> composite, per pair of rays, nothing but rays in and per-ray maps out crossing HBM.  64 + 128 samples only.
 int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmnerf_render_io* io, int64_t n, int flags,
-                       cudaStream_t st, const ObjMask* keep, bool f16) {
+                       cudaStream_t st, const ObjMask* keep, bool f16, const Region* region) {
   using namespace uk;
   DMN_CHECK(wc.ready && wf.ready && wc.extra && wf.extra, "render(umma): weights not packed");
   DMN_CHECK(wc.ins_num == wf.ins_num, "render(umma): coarse/fine ins_num differ");
@@ -1048,6 +1058,11 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   a.zc_out = io->z_vals_coarse; a.zf_out = io->z_vals_fine; a.wc_out = io->weights_coarse; a.wf_out = io->weights_fine;
   a.status = ex->d_status;
   if (keep) a.keep = *keep;
+  if (region) {                                            // a region alone runs the selected kernel with every label kept
+    if (!keep) a.keep = ObjMask{{~0u, ~0u, ~0u, ~0u}};
+    a.region = *region;
+    keep = &a.keep;
+  }
   const int64_t units = (n + 1) / 2;                       // pairs of rays
   const Program& prog = f16 ? ex->prog16 : ex->prog;      // coarse and fine share ins_num, hence the program
   if (keep && f16) return launch_umma<render_objects_f16_kernel>(units, prog, a, st);

@@ -42,12 +42,14 @@ int launch_posenc(const float* x, int64_t m, int n_freqs, float* out, cudaStream
 // One warp per ray.  Phase 1: warp-scan weights into shared memory.  Phase 2: one lane per output
 // channel walks the samples in order (coalesced across channels), mirroring torch.sum(..., -2).
 // SELECT: object selection -- a sample whose argmax_sigmoid label is not kept enters with density 0 (alpha = 0); raw is read,
-// never edited.
+// never edited.  With region.bits set (SELECT only) a sample the region drops (region_drops at o + d z) enters with alpha = 0
+// too: the same test as the fused render kernels.
 template <bool SELECT>
 __global__ void composite_kernel(const float* __restrict__ raw, const float* __restrict__ z,
                                  const float* __restrict__ rays_d, int64_t n, int S, int C, int keep_all,
                                  float* __restrict__ rgb, float* __restrict__ weights, float* __restrict__ depth,
-                                 float* __restrict__ ins, float* __restrict__ acc, const ObjMask keep) {
+                                 float* __restrict__ ins, float* __restrict__ acc, const ObjMask keep,
+                                 const float* __restrict__ rays_o, const __grid_constant__ Region region) {
   extern __shared__ float smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t ray = (int64_t)blockIdx.x * WARPS_PER_BLOCK + warp;
@@ -59,7 +61,16 @@ __global__ void composite_kernel(const float* __restrict__ raw, const float* __r
   const float dnorm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
   ray_weights(S, dnorm, [&](int i) {
     const float* ri = rr + (size_t)i * C;
-    if constexpr (SELECT) { if (!obj_kept(keep, argmax_sigmoid(ri + 4, C - 4))) return 0.0f; }
+    if constexpr (SELECT) {
+      const int label = argmax_sigmoid(ri + 4, C - 4);
+      if (!obj_kept(keep, label)) return 0.0f;
+      if (region.bits) {
+        const float o[3] = {rays_o[ray * 3], rays_o[ray * 3 + 1], rays_o[ray * 3 + 2]}, d[3] = {dx, dy, dz};
+        float p[3];
+        ray_point(o, d, zr[i], p);
+        if (region_drops(region, label, p[0], p[1], p[2])) return 0.0f;
+      }
+    }
     return ri[3];
   }, [&](int i) { return zr[i]; }, w, lane);
   __syncwarp();
@@ -88,17 +99,22 @@ __global__ void composite_kernel(const float* __restrict__ raw, const float* __r
 }
 
 int launch_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all,
-                     float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st, const ObjMask* keep) {
+                     float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st, const ObjMask* keep,
+                     const float* rays_o, const Region* region) {
   DMN_CHECK(s >= 1 && s <= 4096, "composite: n_samples=%d out of range [1,4096]", s);
   DMN_CHECK(c >= 5 && c <= 4 + DMNERF_MAX_INS + 1, "composite: channels=%d out of range", c);
+  DMN_CHECK(!region || (region->bits && rays_o), "composite: a region needs its bits and the ray origins");
   if (n == 0) return 0;
   const size_t smem = (size_t)WARPS_PER_BLOCK * s * sizeof(float);
-  auto kernel = keep ? composite_kernel<true> : composite_kernel<false>;
+  const bool select = keep || region;
+  auto kernel = select ? composite_kernel<true> : composite_kernel<false>;
   if (smem > 48 * 1024)
     DMN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const ObjMask none = {{0u, 0u, 0u, 0u}};
+  const ObjMask none = {{0u, 0u, 0u, 0u}}, all = {{~0u, ~0u, ~0u, ~0u}};
+  const Region no_region{};
   kernel<<<(unsigned)((n + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK), WARPS_PER_BLOCK * 32, smem, st>>>(
-      raw, z, rays_d, n, s, c, keep_all, rgb, weights, depth, ins, acc, keep ? *keep : none);
+      raw, z, rays_d, n, s, c, keep_all, rgb, weights, depth, ins, acc, keep ? *keep : (region ? all : none), rays_o,
+      region ? *region : no_region);
   DMN_LAUNCH_OK();
   return 0;
 }

@@ -27,6 +27,38 @@ __device__ __forceinline__ int argmax_sigmoid(const float* __restrict__ v, int n
   return best;
 }
 
+// Region selection (DESIGN.md, "Region selection").  The bit of the grid point nearest to p: u_a = ((M_a0 p0 + M_a1 p1) +
+// M_a2 p2) + c_a with every operation rounded once, i_a = rint(u_a); 1 or 0 when every i_a is in [0, dim - 1], -1 otherwise
+// (NaN and inf included).  The render kernels, the stage composite and dmnerf_region_contains all call this one function.
+__device__ __forceinline__ int region_bit(const Region& r, float p0, float p1, float p2) {
+  int idx[3];
+  const float top = (float)(r.dim - 1);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const float* m = r.map + 4 * a;
+    const float u = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[0], p0), __fmul_rn(m[1], p1)), __fmul_rn(m[2], p2)), m[3]);
+    const float i = rintf(u);
+    if (!(i >= 0.0f && i <= top)) return -1;
+    idx[a] = (int)i;
+  }
+  const int v = (idx[0] * r.dim + idx[1]) * r.dim + idx[2];
+  return (int)((__ldg(r.bits + (v >> 5)) >> (v & 31)) & 1u);
+}
+
+// Does the region give a sample with label `label` at p = o + d z alpha = 0?  Only for a label in r.applies: inside the grid
+// when its bit is 0, outside it unless r.outside_keep.
+__device__ __forceinline__ bool region_drops(const Region& r, int label, float p0, float p1, float p2) {
+  if (!obj_kept(r.applies, label)) return false;
+  const int b = region_bit(r, p0, p1, p2);
+  return b == 0 || (b < 0 && !r.outside_keep);
+}
+
+// The sample point of depth z on the ray (o, d), as the network prologue computes it.
+__device__ __forceinline__ void ray_point(const float* o, const float* d, float z, float p[3]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) p[c] = __fadd_rn(o[c], __fmul_rn(d[c], z));
+}
+
 // [x, sin(2^k x), cos(2^k x)]_k for one 3-vector; out has 3 + 6*L entries (networks/dm_nerf.py:37-38).
 __device__ __forceinline__ void posenc_one_freq(const float v[3], int k, float* out /* 6 */) {
   const float f = (float)(1 << k);

@@ -9,6 +9,9 @@
                                                         -> per object: voxels, volume, centre, covariance, aabb, obb (network frame)
     object_components(occ, labels=None, level=0.45, connectivity=26)
                                                         -> the connected components of a labelled grid's solid points
+    component_region(cc, ids, scene_transform, ...) / region_from_mask(mask, scene_transform, ...)
+                                                        -> a Region: grid bits the renderer reads per sample (render_*(region=))
+    region_contains(region, pts)                        -> which points a region keeps, by the render kernels' own test
     scene_box(model_fine, poses, hwk, near, far, ...)   -> (scene_transform, extents) of the scene, from the cameras
     manipulation_transform(centre, mode)                -> the transformation dict manipulator_eval takes, about that centre
 
@@ -68,13 +71,16 @@ def _to8b(x):
 
 
 def render_objects(position_embedder, view_embedder, model_coarse, model_fine, poses, hwk, args, keep=None, remove=None,
-                   savedir=None, ins_rgbs=None, color_dict=None, impl=_lib.IMPL_AUTO):
+                   savedir=None, ins_rgbs=None, color_dict=None, impl=_lib.IMPL_AUTO, region=None):
     """Render every pose (camera-to-world, [4, 4] or [3, 4]) with the selection, deterministically, through the frame driver.
     Reads args.near, args.far, args.N_samples, args.N_importance.  Returns one dict per pose of device maps: rgb [H, W, 3],
     ins [H, W, ins_num], depth [H, W], acc [H, W].
     savedir: writes {i:03d}.png (RGBA, alpha = acc: an isolated object is a cut-out) and instance_{i:03d}.png (the arg-max label
     of the instance map, coloured as render_test colours it: ins_rgbs[color_dict[label]], channels in cv2's order).  Without
-    ins_rgbs / color_dict, label k gets colour k of a fixed seeded palette.  impl: the network, as in render_frame."""
+    ins_rgbs / color_dict, label k gets colour k of a fixed seeded palette.  impl: the network, as in render_frame.
+    region: a Region (region selection, DESIGN.md "Region selection") applied with the label selection; with a region, keep and
+    remove may both be left out (every label kept).  Floater cleanup, for example, is the component_region of each object
+    label's largest piece (see component_region)."""
     from .render import _check_embedders, render_frame
     from .tester import colorize, pred_label_lut, write_png
     _check_embedders(position_embedder, view_embedder)
@@ -82,7 +88,10 @@ def render_objects(position_embedder, view_embedder, model_coarse, model_fine, p
     H, W = int(H), int(W)
     dev = next(model_fine.parameters()).device
     ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
-    kept = kept_labels(object_mask(ins_num, keep=keep, remove=remove))
+    if region is not None and keep is None and remove is None:
+        kept = None
+    else:
+        kept = kept_labels(object_mask(ins_num, keep=keep, remove=remove))
     lut = None
     if savedir is not None:
         os.makedirs(savedir, exist_ok=True)
@@ -97,7 +106,7 @@ def render_objects(position_embedder, view_embedder, model_coarse, model_fine, p
         for i, c2w in enumerate(poses):
             c2w = torch.as_tensor(np.asarray(c2w.cpu() if torch.is_tensor(c2w) else c2w), dtype=torch.float32)
             m = render_frame(H, W, K, c2w, args.near, args.far, model_coarse, model_fine, N_samples=args.N_samples,
-                             N_importance=args.N_importance, device=dev, keep_objects=kept, impl=impl)
+                             N_importance=args.N_importance, device=dev, keep_objects=kept, impl=impl, region=region)
             m = {k: v.to(dev) for k, v in m.items()}
             out.append(m)
             if savedir is not None:
@@ -456,6 +465,156 @@ def group_luts(ids, n_components):
         lut[batch] = np.arange(len(batch), dtype=np.int16)
         out.append((lut, batch))
     return out
+
+
+# ----------------------------------------------------------------------------------------------------------------- regions
+# DESIGN.md, "Region selection": one bit per point of the sweep grid, read per sample by the render kernels.  A sample whose label
+# is in the region's `applies` labels gets alpha = 0 when its nearest grid point's bit is 0, or when it lies outside the grid and
+# `outside` is "drop".
+REGION_MAX_DIM = 1290                # dim^3 < 2^31, as object_components
+
+
+def voxel_map(scene_transform, dim, extents=None):
+    """The fp32 map [M | c] (3x4) from the network frame to grid indices of the sweep grid: grid_affine (A, b) in fp64, M =
+    inv(A), c = -inv(A) b, each of the 12 numbers rounded once to fp32."""
+    A, b = grid_affine(scene_transform, dim, extents)
+    M = np.linalg.inv(A)
+    return np.concatenate([M, (-M @ b)[:, None]], 1).astype(np.float32)
+
+
+class Region:
+    """A region of the sweep grid: bits (int32 CUDA tensor, ceil(dim^3 / 32) words; point v = (i dim + j) dim + k is bit v & 31
+    of word v >> 5), dim, voxel_map (float32 [3, 4], voxel_map()), applies (the 4 label words it applies to, or None: every
+    label of the networks it renders with) and outside ("keep" or "drop": samples outside the grid)."""
+
+    def __init__(self, bits, dim, voxel_map, applies=None, outside="keep"):
+        dim = int(dim)
+        if not 2 <= dim <= REGION_MAX_DIM:
+            raise ValueError("Region: dim %d outside [2, %d]" % (dim, REGION_MAX_DIM))
+        words = (dim ** 3 + 31) // 32
+        if not torch.is_tensor(bits) or bits.dtype != torch.int32 or not bits.is_cuda or bits.dim() != 1 or \
+                bits.shape[0] != words or not bits.is_contiguous():
+            raise ValueError("Region: bits must be a contiguous int32 CUDA tensor of %d words for dim %d" % (words, dim))
+        vm = np.asarray(voxel_map, dtype=np.float32).reshape(3, 4)
+        if not np.isfinite(vm).all():
+            raise ValueError("Region: the voxel map is not finite")
+        if outside not in ("keep", "drop"):
+            raise ValueError("Region: outside must be 'keep' or 'drop', got %r" % (outside,))
+        if applies is not None:
+            applies = [int(w) & 0xFFFFFFFF for w in applies]
+            if len(applies) != 4:
+                raise ValueError("Region: applies takes 4 label words")
+        self.bits, self.dim, self.voxel_map, self.applies, self.outside = bits, dim, vm, applies, outside
+
+    def applies_words(self, ins_num):
+        """The 4 label words for networks with ins_num: applies, or every label 0 .. ins_num."""
+        return object_mask(ins_num, remove=[]) if self.applies is None else list(self.applies)
+
+
+def label_words(labels):
+    """The 4 label words of an iterable of labels in [0, 127] (a region's applies)."""
+    words = [0, 0, 0, 0]
+    for k in labels:
+        k = int(k)
+        if not 0 <= k < MAX_LABELS:
+            raise ValueError("label %d outside [0, %d]" % (k, MAX_LABELS - 1))
+        words[k >> 5] |= 1 << (k & 31)
+    return words
+
+
+def _check_build(dilate, connectivity, outside):
+    if int(dilate) != dilate or int(dilate) < 0:
+        raise ValueError("region: dilate must be an integer >= 0, got %r" % (dilate,))
+    if connectivity not in (6, 26):
+        raise ValueError("region: connectivity %r is not 6 or 26" % (connectivity,))
+    if outside not in ("keep", "drop"):
+        raise ValueError("region: outside must be 'keep' or 'drop', got %r" % (outside,))
+
+
+def _region_bits(ids, table, n_ids, dim, dilate, connectivity, invert):
+    """dmnerf_region_pack of an int32 id grid with a table over ids, then dmnerf_region_dilate -> int32 words."""
+    dilate, connectivity = int(dilate), int(connectivity)
+    words = (dim ** 3 + 31) // 32
+    packed = torch.empty(words, dtype=torch.int32, device=ids.device)
+    ctx = get_context(ids.device)
+    tab = torch.as_tensor(np.asarray(table, dtype=np.uint32).view(np.int32)).to(ids.device)
+    ctx.call("dmnerf_region_pack", _lib.ptr(ids, torch.int32), dim, _lib.ptr(tab, torch.int32), int(n_ids),
+             _lib.ptr(packed, torch.int32))
+    if dilate == 0 and not invert:
+        return packed
+    out = torch.empty_like(packed)
+    ctx.call("dmnerf_region_dilate", ctx.handle, _lib.ptr(packed, torch.int32), dim, dilate, connectivity, int(bool(invert)),
+             _lib.ptr(out, torch.int32))
+    return out
+
+
+def _check_cube(grid, who):
+    _lib.need_cuda(who, grid)
+    if grid.dim() != 3 or not (grid.shape[0] == grid.shape[1] == grid.shape[2]):
+        raise ValueError("%s: expected a cubic grid [dim, dim, dim], got %s" % (who, tuple(grid.shape)))
+    dim = int(grid.shape[0])
+    if not 2 <= dim <= REGION_MAX_DIM:
+        raise ValueError("%s: dim %d outside [2, %d]" % (who, dim, REGION_MAX_DIM))
+    return dim
+
+
+def region_from_mask(mask, scene_transform, extents=None, applies=None, outside="keep", dilate=0, connectivity=26):
+    """A Region from a boolean grid mask [dim]^3 (CUDA) over the sweep grid of (scene_transform, extents): the points where mask
+    is True, grown by `dilate` dilation steps.  applies: labels it applies to (default every label); outside as in Region.  An
+    index box [i0:i1, j0:j1, k0:k1] goes through here as a mask."""
+    _check_build(dilate, connectivity, outside)
+    dim = _check_cube(mask, "region_from_mask")
+    ids = torch.where(mask.bool(), 0, -1).to(torch.int32).contiguous()
+    bits = _region_bits(ids, [1], 1, dim, dilate, connectivity, False)
+    return Region(bits, dim, voxel_map(scene_transform, dim, extents), None if applies is None else label_words(applies), outside)
+
+
+def component_region(cc, ids, scene_transform, extents=None, dilate=1, connectivity=26, invert=False, outside="keep"):
+    """A Region from components of object_components' result `cc`: the points of the components `ids`, grown by `dilate`
+    dilation steps (`connectivity` 6 or 26), complemented when invert.  It applies to the labels of `ids` only.
+      one piece alone:  component_region(cc, [j], T)                 -- drops every other piece of j's label
+      one piece out:    component_region(cc, [j], T, invert=True)    -- drops piece j, keeps the rest of its label
+      floater cleanup:  best = largest_components(cc["label"], cc["voxels"]);
+                        component_region(cc, [best[k] for k in best if k != ins_num], T)
+                        -- every object label keeps its largest piece (dilated by a voxel), its floaters go; labels as
+                        object_inventory: every label but ins_num, from a sweep of object_inventory's selection."""
+    _check_build(dilate, connectivity, outside)
+    grid = cc["grid"]
+    dim = _check_cube(grid, "component_region")
+    n = int(np.asarray(cc["label"]).shape[0])
+    ids = [int(c) for c in ids]
+    if any(not 0 <= c < n for c in ids):
+        raise ValueError("component_region: component ids must be in [0, %d)" % n)
+    table = np.zeros(max(1, (n + 31) // 32), dtype=np.uint32)
+    for c in ids:
+        table[c >> 5] |= np.uint32(1 << (c & 31))
+    bits = _region_bits(grid, table, n, dim, dilate, connectivity, invert)
+    applies = label_words(sorted({int(cc["label"][c]) for c in ids}))
+    return Region(bits, dim, voxel_map(scene_transform, dim, extents), applies, outside)
+
+
+def region_contains(region, pts):
+    """dmnerf_region_contains: bool [n] -- the point pts [n, 3] (network frame, CUDA) is inside the grid and its bit is set, by the
+    render kernels' own test."""
+    _lib.need_cuda("region_contains", pts)
+    pts = pts.reshape(-1, 3).contiguous().float()
+    out = torch.empty(pts.shape[0], dtype=torch.uint8, device=pts.device)
+    get_context(pts.device).call("dmnerf_region_contains", _lib.ptr(region.bits, torch.int32), region.dim,
+                                 _lib.floats(region.voxel_map, 12), _lib.ptr(pts), pts.shape[0], _lib.ptr(out, torch.uint8))
+    return out.bool()
+
+
+def set_region(ctx, region, ins_num):
+    """Make `region` the context's region (dmnerf_set_region) for networks with ins_num; None clears it."""
+    lib = ctx.lib
+    if region is None:
+        _lib.check(lib.dmnerf_set_region(ctx.handle, None, 0, None, None, 0), "dmnerf_set_region")
+        return
+    if region.bits.device.index != ctx.index:
+        raise ValueError("region: bits live on %s, the render on cuda:%d" % (region.bits.device, ctx.index))
+    _lib.check(lib.dmnerf_set_region(ctx.handle, _lib.ptr(region.bits, torch.int32), region.dim, _lib.floats(region.voxel_map, 12),
+                                     _lib.keep_mask(region.applies_words(ins_num)), int(region.outside == "keep")),
+               "dmnerf_set_region")
 
 
 def camera_region(poses, hwk, far):

@@ -1,5 +1,6 @@
 """Drop-in for reference networks/render.py: `dm_nerf` (:31-96, the north_star's render_rays) and
 `render_train` (:6-28, raw2outputs), running on the fused native kernels through the C ABI."""
+import contextlib
 import ctypes as C
 
 import torch
@@ -86,6 +87,25 @@ def selection(who, keep_objects, ins_num, model_coarse, model_fine):
     return object_mask(ins_num, keep=keep_objects)
 
 
+@contextlib.contextmanager
+def region_scope(ctx, who, region, ins_num, model_coarse, model_fine):
+    """`region` (objects.Region, or None) as the context's region for the calls inside the block; yields the flag those calls
+    add (DMNERF_FLAG_REGION, or 0 without a region).  Inference only, as object selection."""
+    if region is None:
+        yield 0
+        return
+    from .autograd import _needs_grad
+    from .objects import set_region
+    if _needs_grad(model_coarse, model_fine):
+        raise RuntimeError("%s: region selection is inference-only; call it under torch.no_grad() or with parameters that "
+                           "do not require grad" % who)
+    set_region(ctx, region, ins_num)
+    try:
+        yield _lib.FLAG_REGION
+    finally:
+        set_region(ctx, None, ins_num)
+
+
 def _check_embedders(position_embedder, view_embedder):
     pd = getattr(position_embedder, "out_dim", None)
     vd = getattr(view_embedder, "out_dim", None)
@@ -96,13 +116,14 @@ def _check_embedders(position_embedder, view_embedder):
 
 def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb=0.0, N_importance=128,
                 t_rand=None, u=None, want_raw=True, want_coarse=True, want_samples=None, keep_all_ins=False,
-                impl=_lib.IMPL_AUTO, keep_objects=None):
+                impl=_lib.IMPL_AUTO, keep_objects=None, region=None):
     """Whole per-ray pipeline on the device.  Returns the reference's dict keys plus acc / weights maps.
     want_raw: per-sample network outputs raw_* (forces the stage-by-stage kernels); want_samples: per-sample depths and
     weights (z_vals_*, weights_*; default = want_raw); want_coarse: the coarse pass' maps.  With want_raw=False and
     64 + 128 samples the whole call is ONE kernel and only the requested per-ray maps are written.
     keep_objects: an iterable of object labels in [0, ins_num]; samples labelled otherwise get alpha = 0 in both passes
     (DESIGN.md, "Object selection").  raw_* stay the network's output.  Inference only.
+    region: an objects.Region; samples it drops get alpha = 0 in both passes as well (DESIGN.md, "Region selection").
     impl: _lib.IMPL_UMMA_F16 runs the fp16 preview network (DESIGN.md section 10); IMPL_AUTO follows DMNERF_INFER_IMPL."""
     impl = _lib.infer_impl(impl)
     if want_samples is None:
@@ -144,7 +165,8 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     if keep is not None:
         flags |= _lib.FLAG_SELECT
         io.keep[:] = keep
-    ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags, impl)
+    with region_scope(ctx, "render_rays", region, ins_num, model_coarse, model_fine) as region_flag:
+        ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags | region_flag, impl)
     return out
 
 
@@ -232,12 +254,13 @@ raw2outputs = render_train
 
 
 def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64, N_importance=128, pixel_range=None,
-                 keep_all_ins=False, impl=_lib.IMPL_AUTO, device="cuda", keep_objects=None):
+                 keep_all_ins=False, impl=_lib.IMPL_AUTO, device="cuda", keep_objects=None, region=None):
     """One camera of the reference's test-time loop (render_test, networks/tester.py:55-76) through the frame entry point of
     the C ABI: rays are generated on the device from K / c2w (get_rays_k), the coarse depth row from near / far
     (z_val_sample), the pixels are rendered by the fused kernel and the maps come back as HOST tensors:
     rgb [H,W,3], ins [H,W,ins_num], depth [H,W], acc [H,W] (or [n, ...] rows when a pixel_range = (begin, count) is given --
-    the per-rank slice of a sharded frame).  keep_objects: object selection as in render_rays; impl as in render_rays."""
+    the per-rank slice of a sharded frame).  keep_objects and region: object and region selection as in render_rays; impl as in
+    render_rays."""
     impl = _lib.infer_impl(impl)
     dev = torch.device(device)
     ctx = get_context(dev)
@@ -255,8 +278,9 @@ def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64
         flags |= _lib.FLAG_SELECT
         io.keep[:] = keep
     Kf, Cf = _lib.camera(K, c2w)
-    ctx.call("dmnerf_render_frame_host", ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples, N_importance,
-             flags, impl, C.byref(io))
+    with region_scope(ctx, "render_frame", region, ins_num, model_coarse, model_fine) as region_flag:
+        ctx.call("dmnerf_render_frame_host", ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples,
+                 N_importance, flags | region_flag, impl, C.byref(io))
     if pixel_range is None:
         out = {"rgb": out["rgb"].reshape(H, W, 3), "ins": out["ins"].reshape(H, W, n_ins), "depth": out["depth"].reshape(H, W),
                "acc": out["acc"].reshape(H, W)}

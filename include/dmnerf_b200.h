@@ -56,6 +56,7 @@ extern "C" {
 #define DMNERF_FLAG_WANT_RAW  2     /* materialise raw_coarse / raw_fine (training, penalizer.py) */
 #define DMNERF_FLAG_KEEP_INS  4     /* keep all ins_num+1 instance channels, no detach: manipulator.py:86-105 */
 #define DMNERF_FLAG_SELECT    8     /* object selection: the keep field is read (see "object selection" below) */
+#define DMNERF_FLAG_REGION   16     /* region selection: the context's region is read (see "region selection" below) */
 
 typedef struct dmnerf_ctx dmnerf_ctx;
 
@@ -402,6 +403,32 @@ DMNERF_API int dmnerf_component_table(dmnerf_ctx* ctx, const int32_t* comp, cons
                                       int64_t* voxels, int64_t* root, void* stream);
 DMNERF_API int dmnerf_component_groups(dmnerf_ctx* ctx, const int32_t* comp, int dim, int64_t n, const int16_t* lut, int discard,
                                        int16_t* groups, void* stream);
+
+/* ---- region selection (DESIGN.md, "Region selection"; no counterpart in the original) ------------------------------------
+ * A region is one bit per point of a sweep grid [dim,dim,dim] (dim in [2, 1290]; point v = (i dim + j) dim + k is bit v & 31 of
+ * word v >> 5, ceil(dim^3 / 32) uint32 words, the bits past dim^3 zero), the voxel map [M | c] (row-major 3x4 float32, network
+ * frame -> grid index), the labels it applies to (4 words, as a keep mask) and the rule for samples outside the grid.  A render
+ * sample at p = o + d z (fp32, as the network prologue computes it) with label l (argmax_sigmoid, as object selection) gets alpha
+ * = 0 when l is in `applies` and either p's nearest grid point (i_a = rint(((M_a0 p0 + M_a1 p1) + M_a2 p2) + c_a), every
+ * operation rounded once) is inside the grid with bit 0, or p is outside it and outside_keep is 0.  NaN and inf are outside.
+ * dmnerf_set_region: the region DMNERF_FLAG_REGION reads in dmnerf_render_forward(_host) and dmnerf_render_frame_host (fused
+ *   kernels or stage kernels, chosen as without it; with or without DMNERF_FLAG_SELECT).  bits_device stays the caller's and must
+ *   outlive the renders; NULL clears the region.  Fails for dim out of range or a non-finite map.  A render with the flag fails
+ *   when no region is set or `applies` holds a label above the bound networks' ins_num.
+ * dmnerf_region_pack: bits (DEVICE) = for every point, the bit of its id in table (DEVICE uint32, bit id of word id / 32, over
+ *   ids 0 .. n_ids - 1); an id outside [0, n_ids) (-1: no component) gives 0.  ids: DEVICE int32 [dim^3].
+ * dmnerf_region_dilate: out = `radius` steps of binary dilation of in (6: face neighbours, 26: also edge and corner neighbours;
+ *   never across a grid face; radius 0 copies), then the complement when invert != 0 (tail bits stay 0).  in and out are
+ *   distinct DEVICE buffers.
+ * dmnerf_region_contains: out [n] (DEVICE uint8) = 1 where the point pts [n,3] (DEVICE) is inside the grid and its bit is 1: the
+ *   render kernels' own test. */
+DMNERF_API int dmnerf_set_region(dmnerf_ctx* ctx, const uint32_t* bits_device, int dim, const float* voxel_map12,
+                                 const uint32_t* applies_host, int outside_keep);
+DMNERF_API int dmnerf_region_pack(const int32_t* ids, int dim, const uint32_t* table, int64_t n_ids, uint32_t* bits, void* stream);
+DMNERF_API int dmnerf_region_dilate(dmnerf_ctx* ctx, const uint32_t* in, int dim, int radius, int connectivity, int invert,
+                                    uint32_t* out, void* stream);
+DMNERF_API int dmnerf_region_contains(const uint32_t* bits, int dim, const float* voxel_map12, const float* pts, int64_t n,
+                                      uint8_t* out, void* stream);
 
 /* ---- test-view evaluation: render_test, networks/tester.py (+ ins_eval / calculate_ap, networks/evaluator.py:77-175) -------
  * Rules and deviations: DESIGN.md, "Evaluation metrics".  Every result is deterministic (fixed-order reductions, integer atomics
