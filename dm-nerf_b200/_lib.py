@@ -37,6 +37,25 @@ class RenderIO(C.Structure):
     ]
 
 
+MAX_MOVES = 8                # DMNERF_MAX_MOVES
+
+
+class PieceRegion(C.Structure):
+    """Mirror of `struct dmnerf_piece_region` (bits NULL: no region)."""
+    _fields_ = [("bits", C.c_void_p), ("dim", C.c_int32), ("outside_keep", C.c_int32), ("voxel_map", C.c_float * 12),
+                ("applies", C.c_uint32 * 4)]
+
+
+class Pieces(C.Structure):
+    """Mirror of `struct dmnerf_pieces`."""
+    _fields_ = [
+        ("region", PieceRegion * MAX_MOVES), ("rest_drop", C.c_int32 * MAX_MOVES),
+        ("ori_vote", C.c_void_p * MAX_MOVES), ("tar_vote", C.c_void_p * MAX_MOVES),
+        ("ori_rays_o", _f32p), ("ori_rays_d", _f32p), ("ori_z", _f32p),
+        ("tar_rays_o", _f32p * MAX_MOVES), ("tar_rays_d", _f32p * MAX_MOVES), ("tar_z", _f32p * MAX_MOVES),
+    ]
+
+
 # name -> (restype, argtypes); every symbol declared in include/dmnerf_b200.h
 PROTOTYPES = {
     "dmnerf_abi_version": (C.c_int, []),
@@ -89,7 +108,9 @@ PROTOTYPES = {
                                           C.c_void_p]),
     "dmnerf_mlp_forward_points": (C.c_int, [C.c_void_p, C.c_int, _f32p, _f32p, C.c_int64, _f32p, C.c_int, C.c_void_p]),
     "dmnerf_exchanger": (C.c_int, [_f32p, C.POINTER(C.c_void_p), _f32p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.c_int, C.c_int64,
-                                  C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+                                  C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Pieces), C.c_void_p]),
+    "dmnerf_piece_vote": (C.c_int, [_f32p, _f32p, _f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_int),
+                                    C.POINTER(PieceRegion), C.c_int, C.c_void_p, C.c_void_p]),
     "dmnerf_penalizer_state_bytes": (C.c_int64, []),
     "dmnerf_penalizer_forward": (C.c_int, [_f32p, _f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p,
                                           _f32p, C.c_void_p]),

@@ -16,6 +16,10 @@ The two loops that drive it, with the reference's signatures, printed lines and 
 Both render through manipulate_frame (one edited frame, args.N_test rays per manipulator() call, outputs preallocated on the
 device) and keep every per-pixel step on the device: rays, metrics (dmnerf_b200.tester), label arg-max and colours.  The host
 reads back the metric result struct and the PNG images once per frame.  Rules and deviations: DESIGN.md, "Manipulation loops".
+
+Each of them also takes the keywords pieces= and rest= (no counterpart in the original; DESIGN.md, "Moving pieces"): a move may
+carry a region, so that one piece of its label moves and the rest of the label is kept or dropped.  Without them the edit is the
+original's.
 """
 import ctypes as C
 import json
@@ -32,8 +36,9 @@ from .render import composite, _check_embedders
 from .helpers import sample_pdf, sort_concat, get_rays_k
 
 
-def exchanger(ori_raw, tar_raws, ori_raw_pred, tar_raw_preds, move_labels):
-    """Edits `ori_raw` in place like the reference and returns (ori_raw, tar_raws, ori_pred_label, tar_pred_label)."""
+def exchanger(ori_raw, tar_raws, ori_raw_pred, tar_raw_preds, move_labels, pieces=None):
+    """Edits `ori_raw` in place like the reference and returns (ori_raw, tar_raws, ori_pred_label, tar_pred_label).
+    pieces: an ExchangePieces (DESIGN.md, "Moving pieces"), or None for the reference's exchanger."""
     if not ori_raw.is_cuda:
         raise RuntimeError("exchanger: expected CUDA tensors (no CPU fallback)")
     if not (ori_raw.is_contiguous() and ori_raw.dtype == torch.float32):
@@ -49,9 +54,125 @@ def exchanger(ori_raw, tar_raws, ori_raw_pred, tar_raw_preds, move_labels):
     ori_label = torch.empty((n, s), device=ori_raw.device, dtype=torch.int64)
     tar_label = torch.empty((n, s), device=ori_raw.device, dtype=torch.int64)
     mv = (C.c_int * m)(*[int(v) for v in move_labels])
+    # desc points into the tensors of `alive`, which stay referenced until the call returns
+    desc, alive = (None, ()) if pieces is None else pieces.describe(move_labels, n, s, c - 5, ori_raw.device)
     ctx.call("dmnerf_exchanger", _lib.ptr(ori_raw), _lib.ptrs(tars[:m]), _lib.ptr(acc_o), _lib.ptrs(accs[:m]), mv, m, n, s, c,
-             _lib.ptr(ori_label, torch.int64), _lib.ptr(tar_label, torch.int64))
+             _lib.ptr(ori_label, torch.int64), _lib.ptr(tar_label, torch.int64), None if desc is None else C.byref(desc))
     return ori_raw, tar_raws, ori_label, tar_label
+
+
+# ----------------------------------------------------------------------------------------------------------------- pieces
+# DESIGN.md, "Moving pieces": a move may carry a region (objects.Region), so that only the samples of its label inside that piece
+# move; the rest of the label is kept or dropped.  Rays are judged by a per-ray vote on their first fine pass.
+RESTS = ("keep", "drop")
+
+
+def move_rests(rest, m):
+    """rest ("keep" / "drop", or one of them per move) -> [bool] of m: True where the rest of the label is dropped."""
+    rests = [rest] * m if isinstance(rest, str) else list(rest)
+    if len(rests) != m or any(r not in RESTS for r in rests):
+        raise ValueError("rest must be 'keep' or 'drop', or one of them for each of the %d moves, got %r" % (m, rest))
+    return [r == "drop" for r in rests]
+
+
+def move_pieces(pieces, move_labels, ins_num, device):
+    """pieces (None, or a Region or None per move of move_labels) checked -> a list of m Regions / None, or None when no move has
+    a region.  ValueError for a wrong length, a region on another device or a moved label outside the region's labels."""
+    m = len(move_labels)
+    if pieces is None:
+        return None
+    pieces = list(pieces)
+    if len(pieces) != m:
+        raise ValueError("pieces: %d entries for %d moved labels" % (len(pieces), m))
+    for r, mv in zip(pieces, move_labels):
+        if r is not None:
+            _piece_region(r, int(mv), ins_num, device)
+    return pieces if any(r is not None for r in pieces) else None
+
+
+def _piece_region(region, mv, ins_num, device):
+    """The C struct of one move's region (None: bits NULL)."""
+    d = _lib.PieceRegion()
+    if region is None:
+        return d
+    from .objects import Region
+    if not isinstance(region, Region):
+        raise ValueError("pieces: each entry must be an objects.Region or None, got %r" % (type(region).__name__,))
+    if region.bits.device != torch.device(device):
+        raise ValueError("pieces: a region's bits live on %s, the edit on %s" % (region.bits.device, device))
+    words = region.applies_words(ins_num)
+    if not (0 <= mv <= ins_num and (int(words[mv >> 5]) >> (mv & 31)) & 1):
+        raise ValueError("pieces: moved label %d is not among the labels its region applies to" % mv)
+    d.bits = _lib.ptr(region.bits, torch.int32).value
+    d.dim = region.dim
+    d.outside_keep = int(region.outside == "keep")
+    d.voxel_map[:] = [float(v) for v in np.asarray(region.voxel_map, dtype=np.float32).reshape(-1)]
+    d.applies[:] = [int(w) & 0xFFFFFFFF for w in words]
+    return d
+
+
+def piece_vote(raw, z, weights, rays_o, rays_d, move_labels, regions):
+    """dmnerf_piece_vote: per move, does a ray's accumulated label stand for the piece?  raw [N,S,C], depths z [N,S], composite
+    weights [N,S] and rays [N,3] of one fine pass -> uint8 [m, N] = (weight of mv's samples the region keeps) >= (weight of those
+    it drops), each summed in ascending sample order in fp32; 1 for a move without a region."""
+    _lib.need_cuda("piece_vote", raw, z, weights, rays_o, rays_d)
+    n, s, c = raw.shape
+    m = len(move_labels)
+    if len(regions) != m or not 1 <= m <= _lib.MAX_MOVES:
+        raise ValueError("piece_vote: between 1 and %d moves, one region (or None) each" % _lib.MAX_MOVES)
+    raw, z, weights = raw.contiguous().float(), z.contiguous().float(), weights.contiguous().float()
+    rays_o, rays_d = rays_o.contiguous().float(), rays_d.contiguous().float()
+    if z.shape != (n, s) or weights.shape != (n, s) or rays_o.shape != (n, 3) or rays_d.shape != (n, 3):
+        raise RuntimeError("piece_vote: inconsistent shapes")
+    descs = (_lib.PieceRegion * m)(*[_piece_region(r, int(mv), c - 5, raw.device) for r, mv in zip(regions, move_labels)])
+    votes = torch.empty((m, n), dtype=torch.uint8, device=raw.device)
+    get_context(raw.device).call("dmnerf_piece_vote", _lib.ptr(raw), _lib.ptr(z), _lib.ptr(weights), _lib.ptr(rays_o),
+                                 _lib.ptr(rays_d), n, s, c, (C.c_int * m)(*[int(v) for v in move_labels]), descs, m,
+                                 _lib.ptr(votes, torch.uint8))
+    return votes
+
+
+class ExchangePieces:
+    """The pieces of one exchange: regions (a Region or None per move), rest_drop (bool per move), the original's rays (o, d)
+    [N,3] and the depths ori_z [N,S] of ori_raw's samples, each target's rays tar_rays[i] = (o, d) and depths tar_zs[i] [N,S],
+    and the votes of the first fine pass: ori_votes uint8 [m, N] (piece_vote of the original rays) and tar_votes[i] uint8 [N]
+    (target i's vote for move i)."""
+
+    def __init__(self, regions, rest_drop, ori_rays, ori_z, tar_rays, tar_zs, ori_votes, tar_votes):
+        self.regions, self.rest_drop = list(regions), list(rest_drop)
+        self.ori_rays, self.ori_z, self.tar_rays, self.tar_zs = ori_rays, ori_z, list(tar_rays), list(tar_zs)
+        self.ori_votes, self.tar_votes = ori_votes, list(tar_votes)
+
+    def describe(self, move_labels, n, s, ins_num, device):
+        """-> (the dmnerf_pieces struct, the tensors it points into, to be kept alive for the call)."""
+        m = len(move_labels)
+        if len(self.regions) != m or len(self.rest_drop) != m:
+            raise ValueError("exchanger: pieces describe %d moves, %d moved labels given" % (len(self.regions), m))
+        d = _lib.Pieces()
+        keep = []
+
+        def dev(t, shape, dtype=torch.float32):
+            _lib.need_cuda("exchanger", t)
+            t = t.contiguous().to(dtype)
+            if tuple(t.shape) != shape or t.device != torch.device(device):
+                raise RuntimeError("exchanger: a pieces tensor has shape %s on %s, expected %s on %s"
+                                   % (tuple(t.shape), t.device, shape, device))
+            keep.append(t)
+            return _lib.ptr(t, dtype).value
+        for i, (r, mv) in enumerate(zip(self.regions, move_labels)):
+            d.region[i] = _piece_region(r, int(mv), ins_num, device)
+            if r is None:
+                continue
+            d.rest_drop[i] = int(bool(self.rest_drop[i]))
+            d.ori_vote[i] = dev(self.ori_votes[i], (n,), torch.uint8)
+            d.tar_vote[i] = dev(self.tar_votes[i], (n,), torch.uint8)
+            d.tar_rays_o[i] = dev(self.tar_rays[i][0], (n, 3))
+            d.tar_rays_d[i] = dev(self.tar_rays[i][1], (n, 3))
+            d.tar_z[i] = dev(self.tar_zs[i], (n, s))
+        if any(r is not None for r in self.regions):
+            d.ori_rays_o, d.ori_rays_d = dev(self.ori_rays[0], (n, 3)), dev(self.ori_rays[1], (n, 3))
+            d.ori_z = dev(self.ori_z, (n, s))
+        return d, keep
 
 
 def manipulator_render(raw, z_vals, rays_d):
@@ -73,12 +194,22 @@ def manipulator_nerf(rays, position_embedder, view_embedder, model, N_samples=No
     return raw, z_vals
 
 
+def _ins_num(model):
+    return int(model.ins_linear.weight.shape[0]) - 1
+
+
 def manipulator(position_embedder, view_embedder, model_coarse, model_fine, ori_rays, f_tar_rays, args, us=None,
-                impl=_lib.IMPL_AUTO):
+                impl=_lib.IMPL_AUTO, pieces=None, rest="keep"):
     """manipulator.py:137-205.  `us`: optional list of [N, N_importance] uniforms replacing the torch.rand draws of the
-    sample_pdf calls (order: original rays, every target, original rays again) -- used by the parity tests."""
+    sample_pdf calls (order: original rays, every target, original rays again) -- used by the parity tests.
+    pieces (DESIGN.md, "Moving pieces"): None, or one objects.Region or None per label of args.target_labels: a move with a
+    region moves only the samples of its label inside that piece; rest ("keep" / "drop", or one per move) says what becomes of
+    the label's other samples.  Without any region the edit is the reference's."""
     N_samples, N_importance, near, far = args.N_samples, args.N_importance, args.near, args.far
     us = list(us) if us is not None else None
+    labels = list(args.target_labels)
+    drops = move_rests(rest, len(labels))
+    regions = move_pieces(pieces, labels, _ins_num(model_fine), ori_rays.device)
 
     def draw(bins, w):
         return sample_pdf(bins, w, N_importance, u=(us.pop(0) if us is not None else None))
@@ -86,50 +217,63 @@ def manipulator(position_embedder, view_embedder, model_coarse, model_fine, ori_
     def nerf(rays, model, z=None):
         return manipulator_nerf(rays, position_embedder, view_embedder, model, N_samples, near, far, z_vals=z, impl=impl)
 
-    def fine_pass(rays, coarse_raw, coarse_z):
+    def fine_pass(rays, coarse_raw, coarse_z, moves=None):
         _, w, _, _ = manipulator_render(coarse_raw, coarse_z, rays[1])
         mid = .5 * (coarse_z[..., 1:] + coarse_z[..., :-1])
         z_s = draw(mid, w[..., 1:-1])
         z_full = sort_concat(coarse_z, z_s)                                   # sort(cat(.)) as one kernel
         raw_full, _ = nerf(rays, model_fine, z_full)
-        _, _, _, ins_acc = manipulator_render(raw_full, z_full, rays[1])
-        return z_s, ins_acc
+        _, w_full, _, ins_acc = manipulator_render(raw_full, z_full, rays[1])
+        vote = None if moves is None else piece_vote(raw_full, z_full, w_full, rays[0], rays[1], *moves)
+        return z_s, ins_acc, vote
 
     with torch.no_grad():
         ori_raw, ori_z = nerf(ori_rays, model_coarse)
-        _, ori_ins_acc = fine_pass(ori_rays, ori_raw, ori_z)
-        tar_raws, tar_zs, tar_samples, tar_accs = [], [], [], []
+        _, ori_ins_acc, ori_votes = fine_pass(ori_rays, ori_raw, ori_z, None if regions is None else (labels, regions))
+        tar_raws, tar_zs, tar_samples, tar_accs, tar_votes = [], [], [], [], []
         tar_rgb = None
-        for tar_rays in f_tar_rays:
+        for idx, tar_rays in enumerate(f_tar_rays):
             t_raw, t_z = nerf(tar_rays, model_coarse)
             tar_rgb, _, _, _ = manipulator_render(t_raw, t_z, tar_rays[1])
-            z_s, acc = fine_pass(tar_rays, t_raw, t_z)
+            moves = None if regions is None or idx >= len(labels) else ([labels[idx]], [regions[idx]])
+            z_s, acc, vote = fine_pass(tar_rays, t_raw, t_z, moves)
             tar_raws.append(t_raw); tar_zs.append(t_z); tar_samples.append(z_s); tar_accs.append(acc)
-        ori_raw, _, _, _ = exchanger(ori_raw, tar_raws, ori_ins_acc, tar_accs, args.target_labels)
+            tar_votes.append(None if vote is None else vote[0])
+
+        def pieces_on(ori_depths, tar_depths):
+            if regions is None:
+                return None
+            return ExchangePieces(regions, drops, ori_rays, ori_depths, f_tar_rays, tar_depths, ori_votes, tar_votes)
+        ori_raw, _, _, _ = exchanger(ori_raw, tar_raws, ori_ins_acc, tar_accs, labels, pieces=pieces_on(ori_z, tar_zs))
         _, ori_w, _, _ = manipulator_render(ori_raw, ori_z, ori_rays[1])
         mid = .5 * (ori_z[..., 1:] + ori_z[..., :-1])
         ori_samples = draw(mid, ori_w[..., 1:-1])
         extra = torch.cat([ori_samples] + tar_samples, -1)                     # samples every second-pass ray set shares
         ori_z2 = sort_concat(ori_z, extra)
         ori_raw2, _ = nerf(ori_rays, model_fine, ori_z2)
+        tar_z2s = []
         for idx, tar_rays in enumerate(f_tar_rays):
             t_z2 = sort_concat(tar_zs[idx], extra)
             tar_raws[idx], _ = nerf(tar_rays, model_fine, t_z2)
-        ori_raw2, _, _, _ = exchanger(ori_raw2, tar_raws, ori_ins_acc, tar_accs, args.target_labels)
+            tar_z2s.append(t_z2)
+        ori_raw2, _, _, _ = exchanger(ori_raw2, tar_raws, ori_ins_acc, tar_accs, labels, pieces=pieces_on(ori_z2, tar_z2s))
         final_rgb, _, _, final_ins = manipulator_render(ori_raw2, ori_z2, ori_rays[1])
     return final_rgb, final_ins, tar_rgb, tar_accs[-1]
 
 
 # ----------------------------------------------------------------------------------------------------------------- frame loops
 def manipulate_frame(H, W, K, ori_pose, tar_rays_o, tar_rays_d, position_embedder, view_embedder, model_coarse, model_fine, args,
-                     impl=_lib.IMPL_AUTO):
+                     impl=_lib.IMPL_AUTO, pieces=None, rest="keep"):
     """One edited frame (the chunk loops of manipulator.py:246-269 and :445-466): manipulator() over the H*W rays of
     get_rays_k(H, W, K, ori_pose), args.N_test rays per call with the last call partial, targets labelled args.target_labels.
     tar_rays_o / tar_rays_d: [T, H*W, 3] CUDA rays of the T targets.  The sample_pdf draws keep the reference's order (per
     chunk: the original rays, every target, the original rays again), so a run seeded like the reference consumes the default
     CUDA generator identically.  Returns final rgb [H*W, 3], final ins [H*W, ins_num + 1], tar_rgb [H*W, 3] and
-    tar_ins_accum [H*W, ins_num + 1] (of the last target), written chunk by chunk into preallocated device tensors."""
+    tar_ins_accum [H*W, ins_num + 1] (of the last target), written chunk by chunk into preallocated device tensors.
+    pieces / rest: as manipulator() (one Region or None per label of args.target_labels; "keep" / "drop"), checked once here."""
     dev = tar_rays_o.device
+    move_rests(rest, len(args.target_labels))
+    move_pieces(pieces, list(args.target_labels), _ins_num(model_fine), dev)
     ori_o, ori_d = get_rays_k(H, W, K, torch.as_tensor(ori_pose, dtype=torch.float32, device=dev))
     ori_o, ori_d = ori_o.reshape(-1, 3), ori_d.reshape(-1, 3)
     n, chunk = H * W, int(args.N_test)
@@ -142,7 +286,8 @@ def manipulate_frame(H, W, K, ori_pose, tar_rays_o, tar_rays_d, position_embedde
             end = min(step + chunk, n)
             ori = torch.stack([ori_o[step:end], ori_d[step:end]], 0)
             tar = torch.stack([tar_rays_o[:, step:end], tar_rays_d[:, step:end]], 1)               # [T, 2, cnt, 3]
-            maps = manipulator(position_embedder, view_embedder, model_coarse, model_fine, ori, tar, args, impl=impl)
+            maps = manipulator(position_embedder, view_embedder, model_coarse, model_fine, ori, tar, args, impl=impl, pieces=pieces,
+                               rest=rest)
             if out is None:
                 out = [torch.empty((n,) + tuple(m.shape[1:]), device=dev, dtype=m.dtype) for m in maps]
             for o, m in zip(out, maps):
@@ -212,9 +357,9 @@ def _u8(rgb):
 
 
 def manipulator_eval(position_embedder, view_embedder, model_coarse, model_fine, ori_poses, hwk, trans_dicts, save_dir, ins_rgbs,
-                     args, gt_rgbs=None, gt_labels=None):
+                     args, gt_rgbs=None, gt_labels=None, pieces=None, rest="keep"):
     """networks/manipulator.py manipulator_eval: object args.target_label moved by trans_dicts['transformations'][0] in every
-    view of ori_poses.  Files in save_dir/<mode>/: {i}_rgb.png, {i}_ins.png, {i}_rgb_gt.png, {i}_ins_gt.png (the two label
+    view of ori_poses.  pieces / rest: as manipulate_frame (a list of one Region or None; DESIGN.md, "Moving pieces").  Files in save_dir/<mode>/: {i}_rgb.png, {i}_ins.png, {i}_rgb_gt.png, {i}_ins_gt.png (the two label
     images in the channel order cv2.imwrite stores), matching_log.json and test_results.txt (PSNR SSIM LPIPS AP50..AP95 per
     frame, then the mean row).  Poses may be numpy arrays, CPU or CUDA tensors; gt_labels any integer type (test_dmsr.py passes
     int8).  With gt_rgbs=None only {i}_rgb.png is written."""
@@ -248,7 +393,7 @@ def manipulator_eval(position_embedder, view_embedder, model_coarse, model_fine,
             pose = torch.as_tensor(ori_pose, dtype=torch.float32, device=dev)
             tar_o, tar_d = rigid_rays(H, W, K, trans, pose)
             rgb, ins, _, _ = manipulate_frame(H, W, K, pose, tar_o[None], tar_d[None], position_embedder, view_embedder, model_coarse,
-                                              model_fine, args)
+                                              model_fine, args, pieces=pieces, rest=rest)
             rgb = rgb.reshape(H, W, 3).contiguous()
             ins_map = {}
             if have_gt:
@@ -289,9 +434,9 @@ def manipulator_eval(position_embedder, view_embedder, model_coarse, model_fine,
 
 
 def manipulator_demo(position_embedder, view_embedder, model_coarse, model_fine, ori_poses, hwk, objs_trans, save_dir, ins_rgbs,
-                     objs, view_poses, ins_map, args):
+                     objs, view_poses, ins_map, args, pieces=None, rest="keep"):
     """networks/manipulator.py manipulator_demo: every object of `objs` edited at once in every view of view_poses (ori_poses
-    is unused, as in the reference).  Rigid objects move by objs_trans[obj_name][i]['transformation']; deformed ones shift
+    is unused, as in the reference).  pieces / rest: as manipulate_frame, aligned with `objs` (DESIGN.md, "Moving pieces").  Rigid objects move by objs_trans[obj_name][i]['transformation']; deformed ones shift
     the origins of the view's rays in x (deform_func sin / ex / linear / abs_linear / ln).  Files in save_dir/<args.mani_type>/:
     {i}_rgb.png, {i}_ins.png (label colours through ins_map, cv2's channel order) and {i}_ins_pred_mask.png (the labels as
     uint8); prints `Image{i}: <seconds>` per view."""
@@ -323,7 +468,7 @@ def manipulator_demo(position_embedder, view_embedder, model_coarse, model_fine,
                 tar_ds.append(d)
             args.target_labels = target_labels
             rgb, ins, _, _ = manipulate_frame(H, W, K, pose, torch.stack(tar_os), torch.stack(tar_ds), position_embedder,
-                                              view_embedder, model_coarse, model_fine, args)
+                                              view_embedder, model_coarse, model_fine, args, pieces=pieces, rest=rest)
             label = argmax_rows(ins).reshape(H, W)
             T.write_png(os.path.join(save_dir, f'{i}_rgb.png'), _u8(rgb.reshape(H, W, 3)))
             T.write_png(os.path.join(save_dir, f'{i}_ins.png'), T.colorize(label, lut).cpu().numpy())

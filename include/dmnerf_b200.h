@@ -260,10 +260,47 @@ DMNERF_API int dmnerf_mlp_forward_points(dmnerf_ctx* ctx, int net, const float* 
  * transformed ("target") ray sets of an object edit.  ori_raw [N,S,C] is edited IN PLACE; tar_raws / tar_accs are HOST arrays
  * of n_moves DEVICE pointers ([N,S,C] / [N,C-4]); ori_acc [N,C-4] and tar_accs are the rendered instance maps with every
  * channel kept (manipulator_render); move_labels is a HOST array.  Outputs: int64 per-sample labels of the original and of the
- * last target after the occlusion fixes. */
+ * last target after the occlusion fixes.  pieces (HOST, see "moving pieces" below): NULL is the reference's exchanger.
+ *
+ * ---- moving pieces (DESIGN.md, "Moving pieces"; no counterpart in the original) -------------------------------------------
+ * A move may carry a region (as in "region selection" below: bits, dim, voxel map, the labels it applies to, outside_keep), so
+ * that only its label's samples inside that piece move.  A sample of label mv at p = o + d z (fp32, the network prologue's
+ * expression) is in the piece when the region does not drop it (the render kernels' per-sample test); mv must be among the
+ * labels the region applies to.  A ray's accumulated label is the moving piece when it equals mv and the ray's vote is 1.
+ * dmnerf_piece_vote: the votes of one fine pass: raw [N,S,C], its depths z [N,S], composite weights [N,S] and rays [N,3] ->
+ *   votes [n_moves, N] (DEVICE uint8) = in >= out, where in (out) is the sum of w_s over the samples labelled move_labels[i]
+ *   (argmax_sigmoid over all C - 4 channels) that the region keeps (drops), added in ascending sample order in fp32.  A move
+ *   without a region (bits NULL) votes 1.  move_labels and regions are HOST arrays of n_moves.
+ * dmnerf_exchanger with pieces: per move i with a region, the rays and this pass's depths of target i, the votes of the
+ *   original rays and of target i's rays (their first fine pass), and rest_drop (1: the samples of mv outside the piece are
+ *   zeroed, 0: kept); the original's rays and depths once.  A move whose region bits are NULL takes its whole label.  Every
+ *   region is checked (dim in [2, 1290], finite map, mv among its labels, non-NULL votes, rays and depths) before any launch. */
+#define DMNERF_MAX_MOVES 8
+typedef struct dmnerf_piece_region {
+  const uint32_t* bits;      /* DEVICE region bits, or NULL: no region */
+  int32_t dim;
+  int32_t outside_keep;      /* 1: a sample outside the grid is in the piece */
+  float voxel_map[12];       /* row-major 3x4 [M | c]: network frame -> grid index */
+  uint32_t applies[4];       /* labels the region applies to, bit k of word k / 32 */
+} dmnerf_piece_region;
+typedef struct dmnerf_pieces {
+  dmnerf_piece_region region[DMNERF_MAX_MOVES];
+  int32_t rest_drop[DMNERF_MAX_MOVES];
+  const uint8_t* ori_vote[DMNERF_MAX_MOVES];    /* [N] DEVICE: row i of the original rays' dmnerf_piece_vote */
+  const uint8_t* tar_vote[DMNERF_MAX_MOVES];    /* [N] DEVICE: target i's vote for move i */
+  const float* ori_rays_o;                      /* [N,3] DEVICE */
+  const float* ori_rays_d;                      /* [N,3] */
+  const float* ori_z;                           /* [N,S] the depths of ori_raw's samples */
+  const float* tar_rays_o[DMNERF_MAX_MOVES];    /* [N,3] */
+  const float* tar_rays_d[DMNERF_MAX_MOVES];    /* [N,3] */
+  const float* tar_z[DMNERF_MAX_MOVES];         /* [N,S] the depths of tar_raws[i]'s samples */
+} dmnerf_pieces;
 DMNERF_API int dmnerf_exchanger(float* ori_raw, const float* const* tar_raws, const float* ori_acc, const float* const* tar_accs,
                                 const int* move_labels, int n_moves, int64_t n, int s, int c, int64_t* ori_label,
-                                int64_t* tar_label, void* stream);
+                                int64_t* tar_label, const dmnerf_pieces* pieces, void* stream);
+DMNERF_API int dmnerf_piece_vote(const float* raw, const float* z, const float* weights, const float* rays_o, const float* rays_d,
+                                 int64_t n, int s, int c, const int* move_labels, const dmnerf_piece_region* regions, int n_moves,
+                                 uint8_t* votes, void* stream);
 
 /* "Emptiness" regulariser on the per-sample object logits: emptiness_penalizer / ins_penalizer, networks/penalizer.py:5-62
  * (train_dmsr.py:53-60).  raw [n,S,C], z_vals [n,S], depth [n] (the rendered depth map, treated as a constant),
