@@ -52,6 +52,7 @@ struct Program {
   Step step[N_STEPS];
   uint32_t stage_off[MAX_STAGES];     // byte offset of every weight stage in the packed image
   int32_t n_stages;
+  int32_t head_stage;                 // first stage of the head steps (T_INS_HID): a tile without heads streams stages below it
   int32_t ins_num;
 };
 
@@ -165,6 +166,9 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
   const int64_t my_tiles = FUSED ? 4 * my_items : my_items;
   Fused* fz = reinterpret_cast<Fused*>(smem + SM_FUSED);
   const int C = 4 + prog.ins_num + 1;
+  // Fused: the coarse tile runs the instance and colour heads only when a coarse map is written (the selected kernels always
+  // need its labels).  The coarse weights and the fine samples depend on the coarse density alone.
+  const bool coarse_heads = SELECT || a.rgb_c || a.ins_c || a.depth_c || a.acc_c;
 
   if (tid == 0) {
     for (int i = 0; i < NS; ++i) { mbar_init(&misc->full[i], 1); mbar_init(&misc->empty[i], 8); }
@@ -179,9 +183,9 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
   if (warp == 8) {
     // =========================================================== weight producer (converged warp, one elected lane issues)
     Ring ring{0, 0};
-    const int n_stages = prog.n_stages;
     for (int64_t ti = 0; ti < my_tiles; ++ti) {
       const uint8_t* image = (FUSED && (ti & 3) != 0) ? a.image_fine : a.image;
+      const int n_stages = (FUSED && (ti & 3) == 0 && !coarse_heads) ? prog.head_stage : prog.n_stages;
       for (int si = 0; si < n_stages; ++si) {
         const uint32_t off = prog.stage_off[si], bytes = prog.stage_off[si + 1] - off;
         wait_bar(&misc->empty[ring.slot], ring.phase ^ 1, misc, 101, a.status);
@@ -490,41 +494,46 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
       wg_sync();
     }
     // ---------------- folded instance hidden layer (acc0) and folded colour hidden layer [h | dir] (acc1)
-    all_act(acc0);
-    all_act(acc1); e_chunk(acc1, 2, false);
-    drain();
-    wg_sync();
+    // A fused coarse tile whose coarse maps nobody reads stops after the density (Program::head_stage: the producer skips the
+    // same stages); its composite then takes the weights from the density alone.
+    const bool heads = !FUSED || j != 0 || coarse_heads;
     float rgb[2][3];
-    hidden(acc1, T_RGB_HID, -1, 8, W_HID / 2, 0);
-    {
-      // rgb_linear (dm_nerf.py:102,105) on CUDA cores
 #pragma unroll
-      for (int h = 0; h < 2; ++h) rgb[h][0] = rgb[h][1] = rgb[h][2] = 0.0f;
+    for (int h = 0; h < 2; ++h) rgb[h][0] = rgb[h][1] = rgb[h][2] = 0.0f;
+    if (heads) {
+      all_act(acc0);
+      all_act(acc1); e_chunk(acc1, 2, false);
+      drain();
+      wg_sync();
+      hidden(acc1, T_RGB_HID, -1, 8, W_HID / 2, 0);
+      {
+        // rgb_linear (dm_nerf.py:102,105) on CUDA cores
 #pragma unroll
-      for (int jj = 0; jj < 16; ++jj) {
-        const int col = 8 * jj + 2 * q4;
+        for (int jj = 0; jj < 16; ++jj) {
+          const int col = 8 * jj + 2 * q4;
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const float2 w = __ldg(reinterpret_cast<const float2*>(bias_t + B_WRGB + c * 128 + col));
+          for (int c = 0; c < 3; ++c) {
+            const float2 w = __ldg(reinterpret_cast<const float2*>(bias_t + B_WRGB + c * 128 + col));
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            rgb[h][c] = fmaf(acc1[4 * jj + 2 * h], w.x, rgb[h][c]);
-            rgb[h][c] = fmaf(acc1[4 * jj + 2 * h + 1], w.y, rgb[h][c]);
+            for (int h = 0; h < 2; ++h) {
+              rgb[h][c] = fmaf(acc1[4 * jj + 2 * h], w.x, rgb[h][c]);
+              rgb[h][c] = fmaf(acc1[4 * jj + 2 * h + 1], w.y, rgb[h][c]);
+            }
           }
         }
       }
+      hidden(acc0, T_INS_HID, 0, 9, W_HID / 2, 0);
+      fence_proxy_async_smem();
+      wg_sync();
+      // ---------------- instance head (dm_nerf.py:103,105) on the instance hidden activation (activation half 0)
+      // The weight stages of this step hold n = pad16(ins_num + 1) rows, but the MMA is issued with N = 128 like every other
+      // step: rows n..127 of the ring slot are stale bytes of an earlier stage.  Output column c depends only on B row c, so
+      // columns >= n are garbage and are never read (only columns < ins_num + 1 are stored below).  The head is 1 of 19
+      // half-steps of a tile.
+      act_chunk(acc0, 0, true); act_chunk(acc0, 1, false);
+      drain();
+      wg_sync();
     }
-    hidden(acc0, T_INS_HID, 0, 9, W_HID / 2, 0);
-    fence_proxy_async_smem();
-    wg_sync();
-    // ---------------- instance head (dm_nerf.py:103,105) on the instance hidden activation (activation half 0)
-    // The weight stages of this step hold n = pad16(ins_num + 1) rows, but the MMA is issued with N = 128 like every other
-    // step: rows n..127 of the ring slot are stale bytes of an earlier stage.  Output column c depends only on B row c, so
-    // columns >= n are garbage and are never read (only columns < ins_num + 1 are stored below).  The head is 1 of 19
-    // half-steps of a tile.
-    act_chunk(acc0, 0, true); act_chunk(acc0, 1, false);
-    drain();
-    wg_sync();
     const int n_ins1 = prog.ins_num + 1;
     float c3[2][4];
 #pragma unroll
@@ -555,6 +564,7 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (q4 == 0) misc->rowv[ra + 8 * h] = make_float4(c3[h][0], c3[h][1], c3[h][2], c3[h][3]);
+        if (!heads) continue;
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj) {
           const int col = 8 * jj + 2 * q4;
@@ -621,8 +631,8 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
         if (lane_i == 0) { ac[0] = p0; ac[1] = p1; ac[2] = p2; ac[3] = p3; ac[4] = p4; }
         named_bar_sync<4, 128>();        // weights of the tile complete
         // instance logits weighted by the (detached) weights: sum_i w_i raw_i[4+k] (render.py:22-24); lane = channel,
-        // the 32 rows of this warp's chunk added in order
-        for (int ch = lane_i; ch < n_ins1; ch += 32) {
+        // the 32 rows of this warp's chunk added in order (a tile without heads has no logits)
+        for (int ch = lane_i; ch < (heads ? n_ins1 : 0); ch += 32) {
           float sacc = 0.0f;
           for (int rr = 0; rr < 32; ++rr) sacc = __fadd_rn(sacc, __fmul_rn(fz->w[32 * wi + rr], logit[(32 * wi + rr) * 128 + ch]));
           ac[5 + ch] = sacc;
@@ -739,8 +749,10 @@ static void build_program(Program& P, int ins_num, bool f16 = false) {
   // stage offsets
   uint32_t off = 0;
   int si = 0;
-  for (int i = 0; i < N_STEPS; ++i)
+  for (int i = 0; i < N_STEPS; ++i) {
+    if (i == T_INS_HID) P.head_stage = si;
     for (int c = 0; c < (f16 ? 1 : 2) * P.step[i].n_chunks; ++c) { P.stage_off[si++] = off; off += (uint32_t)P.step[i].n * 128u; }
+  }
   P.stage_off[si] = off;               // sentinel: total image size
   P.n_stages = si;
 }
