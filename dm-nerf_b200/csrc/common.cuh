@@ -41,7 +41,7 @@ struct NetParams {
 __host__ __device__ inline int layer_out(int l, int ins_num) {
   return l < 10 ? W_HID : (l < 12 ? W_HID / 2 : (l == L_DENSITY ? 1 : (l == L_INS_OUT ? ins_num + 1 : 3)));
 }
-__host__ __device__ inline int layer_in(int l) {
+__host__ __device__ constexpr int layer_in(int l) {
   return l == 0 ? CH_POS : (l == 5 ? W_HID + CH_POS : (l == L_RGB_HID ? W_HID + CH_DIR : (l >= L_INS_OUT ? W_HID / 2 : W_HID)));
 }
 

@@ -24,9 +24,9 @@
 // stage per chunk (no W_lo stages).  Epilogues and embeddings store fp16 into the hi slabs; the lo slabs stay unused.  A value
 // stored above the fp16 range raises STATUS_F16_RANGE in the error word, which the host reports as an error.
 //
+#include <array>
 #include <cstring>
 #include <type_traits>
-#include <vector>
 
 #include "ray_ops.cuh"
 #include "uk_pipe.cuh"
@@ -36,25 +36,6 @@ namespace dmnerf {
 namespace uk {
 
 using namespace umma;
-enum ChunkKind : int8_t { CK_E = 6, CK_D = 7 };              // 0..3 = activation K chunk
-
-struct Step {
-  int8_t n_chunks;
-  int8_t chunk[MAX_CHUNKS];   // ChunkKind or activation chunk
-  int8_t dep[MAX_CHUNKS];     // tile-relative step whose epilogue produces the chunk; -1 = tile inputs
-  int8_t ksteps[MAX_CHUNKS];  // K/16 MMAs for this chunk (4, or 2 for the direction embedding)
-  int8_t out_slot;            // destination half of the activation, or -1 = network outputs
-  int8_t relu;
-  int16_t n;                  // rows of the packed weight stage (multiple of 16, <= 128)
-};
-
-struct Program {
-  Step step[N_STEPS];
-  uint32_t stage_off[MAX_STAGES];     // byte offset of every weight stage in the packed image
-  int32_t n_stages;
-  int32_t head_stage;                 // first stage of the head steps (T_INS_HID): a tile without heads streams stages below it
-  int32_t ins_num;
-};
 
 // Shared state of the fused render kernel: one work unit = 2 rays = 1 coarse tile (2 x 64 samples) + 3 fine tiles (2 x 192).
 constexpr int FS = 64, FI = 128, FF = FS + FI;        // the fused path is specialised for 64 + 128 samples
@@ -148,6 +129,23 @@ __device__ __forceinline__ void fill_embedding(const float v[3], float* vals /* 
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
+// The 64-wide weight chunks the consumer issues per tile, in this order: trunk layers 0..7, two half-steps each (layer 0:
+// the position embedding; layers 1..7: the four activation chunks, then at layer 5 the position embedding again), then the
+// heads: the folded instance hidden layer (four activation chunks), the folded colour hidden layer (four activation chunks,
+// then the direction embedding) and the instance head (two activation chunks).  weight_chunks() lists them for the producer
+// and the packer and is checked against these counts.
+constexpr int HEAD_CHUNK = 2 * (1 + 7 * 4 + 1);             // 60: the first chunk of the heads
+constexpr int TILE_CHUNKS = HEAD_CHUNK + 4 + (4 + 1) + 2;   // 71
+constexpr int MAX_STAGES = 2 * TILE_CHUNKS;                // the exact stream: a W_hi and a W_lo stage per chunk
+
+// The weight stream of one image, derived from weight_chunks() by make_program: all the kernel reads of it.
+struct Program {
+  uint32_t stage_off[MAX_STAGES + 1];  // byte offset of every weight stage in the image; stage_off[n_stages] = image size
+  int32_t n_stages;
+  int32_t head_stage;                  // first stage of the heads: a tile without heads streams the stages below it
+  int32_t ins_num;
+};
+
 // Warps 0-7: two consumer warpgroups (MMA issue, epilogues, prologue); warp 8: weight producer.
 // SELECT (fused only): object selection -- samples whose label is not in a.keep get alpha = 0 in both composites, and so do the
 // samples a.region drops (region selection, when a.region.bits is set).  The body is
@@ -716,51 +714,62 @@ __global__ void __launch_bounds__(N_THREADS, 1) render_objects_f16_kernel(const 
   mlp_umma_body<true, true, true>(prog, a);
 }
 
-// ------------------------------------------------------------------------------------------------ host: program
-// f16: the fp16 program -- the same steps with one weight stage per chunk instead of a W_hi and a W_lo stage.
-static void build_program(Program& P, int ins_num, bool f16 = false) {
-  memset(&P, 0, sizeof(P));
-  P.ins_num = ins_num;
-  // Slot 0 always holds K-half 0 of the current activation, slot 1 K-half 1 (see the MMA role of the kernel).
-  int a_step = -1, b_step = -1;                        // steps that produced them
-  int t = 0;
-  auto add_chunk = [&](Step& s, int kind, int dep, int ks) {
-    s.chunk[s.n_chunks] = (int8_t)kind; s.dep[s.n_chunks] = (int8_t)dep; s.ksteps[s.n_chunks] = (int8_t)ks; ++s.n_chunks;
+// ------------------------------------------------------------------------------------------------ host: the weight stream
+// One weight chunk: the [rows x 64] block B[n][k] = src[n_base + n][col_base + k] of its source matrix (row stride ld), zero
+// for n >= n_valid or k >= k_valid.  The exact image holds it as a W_hi and a W_lo stage, the fp16 image as one fp16 stage.
+enum WeightSrc : int8_t { SRC_TRUNK, SRC_INS_HID, SRC_RGB_HID, SRC_INS_OUT };   // trunk layer `layer`, the folded instance
+                                                                                 // and colour hidden layers, ins_linear
+struct WeightChunk {
+  int8_t src, layer;
+  int16_t ld, n_base, n_valid, col_base, k_valid;
+  int16_t rows;               // rows of its stage: 128, or pad16(ins_num + 1) for the instance head
+};
+struct WeightChunks { WeightChunk c[TILE_CHUNKS]; int n, head; };
+
+// The one description of the weight stream: every chunk of a tile, in the order the consumer issues them (mlp_umma_body).
+constexpr WeightChunks weight_chunks(int ins_num) {
+  WeightChunks w{};
+  auto add = [&](WeightSrc src, int layer, int ld, int n_base, int n_valid, int col_base, int k_valid, int rows) {
+    w.c[w.n++] = WeightChunk{(int8_t)src, (int8_t)layer, (int16_t)ld, (int16_t)n_base, (int16_t)n_valid, (int16_t)col_base,
+                             (int16_t)k_valid, (int16_t)rows};
   };
-  auto add_act = [&](Step& s) {
-    add_chunk(s, 0, a_step, 4); add_chunk(s, 1, a_step, 4);
-    add_chunk(s, 2, b_step, 4); add_chunk(s, 3, b_step, 4);
-  };
-  for (int l = 0; l < 8; ++l) {
+  for (int l = 0; l < 8; ++l) {                       // trunk layer l, output half h
     for (int h = 0; h < 2; ++h) {
-      Step& s = P.step[t];
-      s.n = 128; s.relu = 1; s.out_slot = (int8_t)h;
-      if (l == 0) add_chunk(s, CK_E, -1, 4);
-      else { add_act(s); if (l == 5) add_chunk(s, CK_E, -1, 4); }
-      ++t;
+      if (l != 0)
+        for (int c = 0; c < 4; ++c) add(SRC_TRUNK, l, layer_in(l), 128 * h, 128, 64 * c, 64, 128);
+      if (l == 0 || l == 5) add(SRC_TRUNK, l, layer_in(l), 128 * h, 128, l == 0 ? 0 : 256, CH_POS, 128);
     }
-    a_step = t - 2; b_step = t - 1;
   }
-  // folded instance branch -> slot 0; folded colour branch (its 3-wide head runs on CUDA cores); instance head on slot 0
-  { Step& s = P.step[t]; s.n = 128; s.relu = 1; s.out_slot = 0; add_act(s); ++t; }                              // T_INS_HID
-  { Step& s = P.step[t]; s.n = 128; s.relu = 1; s.out_slot = -1; add_act(s); add_chunk(s, CK_D, -1, 2); ++t; }  // T_RGB_HID
-  { Step& s = P.step[t]; s.n = (int16_t)(((ins_num + 1) + 15) / 16 * 16); s.relu = 0; s.out_slot = -1;        // T_INS_OUT
-    add_chunk(s, 0, t - 2, 4); add_chunk(s, 1, t - 2, 4); ++t; }
-  // stage offsets
+  w.head = w.n;
+  for (int c = 0; c < 4; ++c) add(SRC_INS_HID, 0, 256, 0, 128, 64 * c, 64, 128);    // folded instance hidden layer [128][256]
+  for (int c = 0; c < 4; ++c) add(SRC_RGB_HID, 0, 283, 0, 128, 64 * c, 64, 128);    // folded colour hidden layer [128][283]
+  add(SRC_RGB_HID, 0, 283, 0, 128, 256, CH_DIR, 128);
+  const int n_ins1 = ins_num + 1, head_rows = (n_ins1 + 15) / 16 * 16;
+  for (int c = 0; c < 2; ++c) add(SRC_INS_OUT, 0, 128, 0, n_ins1, 64 * c, 64, head_rows);   // ins_linear [ins_num + 1][128]
+  return w;
+}
+static_assert(weight_chunks(1).n == TILE_CHUNKS && weight_chunks(1).head == HEAD_CHUNK,
+              "weight_chunks() does not match the chunks the consumer issues");
+
+// The stream of the exact image (a W_hi and a W_lo stage per chunk) or of the fp16 image (one stage per chunk).
+static Program make_program(int ins_num, bool f16) {
+  const WeightChunks w = weight_chunks(ins_num);
+  const int per_chunk = f16 ? 1 : 2;
+  Program P;
+  memset(&P, 0, sizeof(P));
   uint32_t off = 0;
-  int si = 0;
-  for (int i = 0; i < N_STEPS; ++i) {
-    if (i == T_INS_HID) P.head_stage = si;
-    for (int c = 0; c < (f16 ? 1 : 2) * P.step[i].n_chunks; ++c) { P.stage_off[si++] = off; off += (uint32_t)P.step[i].n * 128u; }
-  }
-  P.stage_off[si] = off;               // sentinel: total image size
-  P.n_stages = si;
+  for (int i = 0; i < w.n; ++i)
+    for (int s = 0; s < per_chunk; ++s) { P.stage_off[per_chunk * i + s] = off; off += (uint32_t)w.c[i].rows * 128u; }
+  P.n_stages = per_chunk * w.n;
+  P.stage_off[P.n_stages] = off;
+  P.head_stage = per_chunk * w.head;
+  P.ins_num = ins_num;
+  return P;
 }
 
 // ------------------------------------------------------------------------------------------------ host: packing
-struct PackStage {            // one entry per (step, chunk): produces the W_hi and the W_lo stage
-  const float* src; int ld; int n_base; int n_valid; int col_base; int k_valid; int n_rows; uint32_t off_hi; uint32_t off_lo;
-  int transposed;             // 0: B[n][k] = src[n_base + n][col_base + k];  1: B[n][k] = src[col_base + k][n_base + n]
+struct PackStage {            // one per chunk: its stages at off_hi (W_hi, or the fp16 stage) and off_lo (W_lo)
+  const float* src; WeightChunk c; uint32_t off_hi; uint32_t off_lo;
 };
 
 __global__ void fold_kernel(const float* __restrict__ w2, int ld2, const float* __restrict__ w1, const float* __restrict__ b1,
@@ -787,11 +796,17 @@ __global__ void fold_kernel(const float* __restrict__ w2, int ld2, const float* 
   }
 }
 
-__global__ void pack_kernel(const PackStage* __restrict__ stages, int n_entries, uint8_t* __restrict__ image) {
+// One block per chunk.  Exact image: B as bf16 hi and lo stages.  F16: as one fp16 stage; a weight above the fp16 range sets
+// *out_of_range = 1.
+template <bool F16>
+__global__ void pack_kernel(const PackStage* __restrict__ stages, int n_entries, uint8_t* __restrict__ image,
+                            int32_t* __restrict__ out_of_range) {
   const int e = blockIdx.x;
   if (e >= n_entries) return;
   const PackStage ps = stages[e];
-  for (int idx = threadIdx.x; idx < ps.n_rows * 8; idx += blockDim.x) {
+  const WeightChunk& c = ps.c;
+  bool over = false;
+  for (int idx = threadIdx.x; idx < c.rows * 8; idx += blockDim.x) {
     const int n = idx >> 3, u = idx & 7;
     uint32_t hi[4], lo[4];
 #pragma unroll
@@ -800,42 +815,15 @@ __global__ void pack_kernel(const PackStage* __restrict__ stages, int n_entries,
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int k = 8 * u + 2 * j + h;
-        v[h] = !(n < ps.n_valid && k < ps.k_valid) ? 0.0f
-               : (ps.transposed ? ps.src[(size_t)(ps.col_base + k) * ps.ld + ps.n_base + n]
-                                : ps.src[(size_t)(ps.n_base + n) * ps.ld + ps.col_base + k]);
+        v[h] = (n < c.n_valid && k < c.k_valid) ? ps.src[(size_t)(c.n_base + n) * c.ld + c.col_base + k] : 0.0f;
+        if (F16) over |= !(fabsf(v[h]) <= umma::F16_MAX);      // NaN counts as out of range
       }
-      umma::split_bf16x2(v[0], v[1], hi[j], lo[j]);
+      if constexpr (F16) hi[j] = umma::pack_f16x2(v[0], v[1]);
+      else umma::split_bf16x2(v[0], v[1], hi[j], lo[j]);
     }
     const uint32_t o = umma::sw128_offset(n, 8 * u);
     *reinterpret_cast<uint4*>(image + ps.off_hi + o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    *reinterpret_cast<uint4*>(image + ps.off_lo + o) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-  }
-}
-
-// The fp16 image: one stage per entry at off_hi (off_lo unused).  A weight above the fp16 range sets *out_of_range = 1.
-__global__ void pack_f16_kernel(const PackStage* __restrict__ stages, int n_entries, uint8_t* __restrict__ image,
-                                int32_t* __restrict__ out_of_range) {
-  const int e = blockIdx.x;
-  if (e >= n_entries) return;
-  const PackStage ps = stages[e];
-  bool over = false;
-  for (int idx = threadIdx.x; idx < ps.n_rows * 8; idx += blockDim.x) {
-    const int n = idx >> 3, u = idx & 7;
-    uint32_t h16[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float v[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int k = 8 * u + 2 * j + h;
-        v[h] = !(n < ps.n_valid && k < ps.k_valid) ? 0.0f
-               : (ps.transposed ? ps.src[(size_t)(ps.col_base + k) * ps.ld + ps.n_base + n]
-                                : ps.src[(size_t)(ps.n_base + n) * ps.ld + ps.col_base + k]);
-        over |= !(fabsf(v[h]) <= umma::F16_MAX);      // NaN counts as out of range
-      }
-      h16[j] = umma::pack_f16x2(v[0], v[1]);
-    }
-    *reinterpret_cast<uint4*>(image + ps.off_hi + umma::sw128_offset(n, 8 * u)) = make_uint4(h16[0], h16[1], h16[2], h16[3]);
+    if constexpr (!F16) *reinterpret_cast<uint4*>(image + ps.off_lo + o) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
   }
   if (over) *out_of_range = 1;
 }
@@ -863,8 +851,8 @@ __global__ void bias_kernel(NetParams p, const float* __restrict__ fold_b_rgb, c
 
 // ================================================================================================ API
 struct UmmaExtra {            // hangs off UmmaWeights::image allocation bookkeeping
-  uk::Program prog;
-  uk::Program prog16;         // the fp16 program: one stage per chunk (UmmaWeights::image16)
+  uk::Program prog;           // the stream of UmmaWeights::image
+  uk::Program prog16;         // the stream of UmmaWeights::image16: one stage per chunk
   float* fold_w_rgb; float* fold_w_ins; float* fold_b; uk::PackStage* d_entries;
   int32_t* d_pack_flag;       // fp16 pack: set when a weight exceeds the fp16 range
   int32_t* d_status;          // device alias of h_status
@@ -913,35 +901,19 @@ static int launch_gate(const UmmaWeights& w, bool f16) {
   return 0;
 }
 
-// One PackStage per (step, chunk) of `prog`: the W_hi and W_lo stage of the exact image, or the one stage of the fp16 image.
-// Reads the folded head layers from the fold buffers, which umma_weights_pack fills.
-static std::vector<uk::PackStage> pack_entries(const uk::Program& prog, const NetParams& p, const UmmaExtra* x, bool f16) {
+// One PackStage per chunk of weight_chunks(), placed by `prog` (the exact or the fp16 stream).  Reads the folded head layers
+// from the fold buffers, which umma_weights_pack fills.
+static std::array<uk::PackStage, uk::TILE_CHUNKS> pack_entries(const uk::Program& prog, const NetParams& p, const UmmaExtra* x,
+                                                               bool f16) {
   using namespace uk;
-  std::vector<PackStage> ent;
+  const WeightChunks w = weight_chunks(p.ins_num);
   const int per_chunk = f16 ? 1 : 2;
-  int si = 0;
-  for (int t = 0; t < N_STEPS; ++t) {
-    const Step& s = prog.step[t];
-    for (int c = 0; c < s.n_chunks; ++c, si += per_chunk) {
-      PackStage e;
-      memset(&e, 0, sizeof(e));
-      e.n_rows = s.n; e.off_hi = prog.stage_off[si]; e.off_lo = f16 ? 0u : prog.stage_off[si + 1];
-      const int kind = s.chunk[c];
-      if (t < 16) {                                   // trunk layer l, output half h
-        const int l = t / 2, h = t % 2;
-        e.src = p.w[l]; e.ld = layer_in(l); e.n_base = h * 128; e.n_valid = 128;
-        if (kind == CK_E) { e.col_base = (l == 0) ? 0 : 256; e.k_valid = 63; }
-        else { e.col_base = 64 * c; e.k_valid = 64; }
-      } else if (t == T_RGB_HID) {                    // folded rgb hidden layer: [128][283]
-        e.src = x->fold_w_rgb; e.ld = 283; e.n_base = 0; e.n_valid = 128;
-        if (kind == CK_D) { e.col_base = 256; e.k_valid = 27; } else { e.col_base = 64 * c; e.k_valid = 64; }
-      } else if (t == T_INS_HID) {                    // folded instance hidden layer: [128][256]
-        e.src = x->fold_w_ins; e.ld = 256; e.n_base = 0; e.n_valid = 128; e.col_base = 64 * c; e.k_valid = 64;
-      } else {                                        // ins_linear [ins_num+1][128]
-        e.src = p.w[L_INS_OUT]; e.ld = 128; e.n_base = 0; e.n_valid = p.ins_num + 1; e.col_base = 64 * c; e.k_valid = 64;
-      }
-      ent.push_back(e);
-    }
+  std::array<PackStage, TILE_CHUNKS> ent;
+  for (int i = 0; i < TILE_CHUNKS; ++i) {
+    const WeightChunk& c = w.c[i];
+    const float* src = c.src == SRC_TRUNK ? p.w[c.layer] : c.src == SRC_INS_HID ? x->fold_w_ins
+                     : c.src == SRC_RGB_HID ? x->fold_w_rgb : p.w[L_INS_OUT];
+    ent[i] = PackStage{src, c, prog.stage_off[per_chunk * i], f16 ? 0u : prog.stage_off[per_chunk * i + 1]};
   }
   return ent;
 }
@@ -952,8 +924,8 @@ int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
   if (!w.extra) {
     UmmaExtra* x = new UmmaExtra();
     memset(x, 0, sizeof(*x));
-    build_program(x->prog, p.ins_num);
-    build_program(x->prog16, p.ins_num, true);
+    x->prog = make_program(p.ins_num, false);
+    x->prog16 = make_program(p.ins_num, true);
     w.extra = x;
     w.ins_num = p.ins_num;
     w.image_bytes = x->prog.stage_off[x->prog.n_stages];
@@ -962,7 +934,7 @@ int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
     DMN_CUDA(cudaMalloc((void**)&x->fold_w_rgb, 128 * 283 * sizeof(float)));
     DMN_CUDA(cudaMalloc((void**)&x->fold_w_ins, 128 * 256 * sizeof(float)));
     DMN_CUDA(cudaMalloc((void**)&x->fold_b, 256 * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->d_entries, MAX_STAGES * sizeof(PackStage)));
+    DMN_CUDA(cudaMalloc((void**)&x->d_entries, TILE_CHUNKS * sizeof(PackStage)));
     DMN_CUDA(cudaHostAlloc((void**)&x->h_status, sizeof(int32_t), cudaHostAllocMapped));
     *x->h_status = 0;
     DMN_CUDA(cudaHostGetDevicePointer((void**)&x->d_status, (void*)x->h_status, 0));
@@ -974,12 +946,10 @@ int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
   DMN_LAUNCH_OK();
   fold_kernel<<<dim3(128, 5), 256, 0, st>>>(p.w[L_INS_HID], 256, p.w[L_INS_FEAT], p.b[L_INS_FEAT], p.b[L_INS_HID], 0, x->fold_w_ins, x->fold_b + 128);
   DMN_LAUNCH_OK();
-  const std::vector<PackStage> ent = pack_entries(x->prog, p, x, false);
-  DMN_CHECK((int)ent.size() * 2 == x->prog.n_stages && (int)ent.size() <= MAX_STAGES, "umma pack: stage table mismatch");
-  const size_t n_fwd = ent.size();
-  DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), ent.size() * sizeof(PackStage), cudaMemcpyHostToDevice, st));
+  const auto ent = pack_entries(x->prog, p, x, false);
+  DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), sizeof(ent), cudaMemcpyHostToDevice, st));
   DMN_CUDA(cudaStreamSynchronize(st));               // `ent` is a host temporary
-  pack_kernel<<<(unsigned)n_fwd, 256, 0, st>>>(x->d_entries, (int)n_fwd, (uint8_t*)w.image);
+  pack_kernel<false><<<TILE_CHUNKS, 256, 0, st>>>(x->d_entries, TILE_CHUNKS, (uint8_t*)w.image, nullptr);
   DMN_LAUNCH_OK();
   bias_kernel<<<8, 256, 0, st>>>(p, x->fold_b, x->fold_b + 128, w.bias);
   DMN_LAUNCH_OK();
@@ -995,11 +965,10 @@ int umma_weights_pack_f16(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
   if (!w.image16) DMN_CUDA(cudaMalloc(&w.image16, x->prog16.stage_off[x->prog16.n_stages]));
   if (!x->d_pack_flag) DMN_CUDA(cudaMalloc((void**)&x->d_pack_flag, sizeof(int32_t)));
   // the folded head layers are the fp32 fold of the exact pack (fp64 accumulate), rounded to fp16 here
-  const std::vector<PackStage> ent = pack_entries(x->prog16, p, x, true);
-  DMN_CHECK((int)ent.size() == x->prog16.n_stages && (int)ent.size() <= MAX_STAGES, "fp16 pack: stage table mismatch");
+  const auto ent = pack_entries(x->prog16, p, x, true);
   DMN_CUDA(cudaMemsetAsync(x->d_pack_flag, 0, sizeof(int32_t), st));
-  DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), ent.size() * sizeof(PackStage), cudaMemcpyHostToDevice, st));
-  pack_f16_kernel<<<(unsigned)ent.size(), 256, 0, st>>>(x->d_entries, (int)ent.size(), (uint8_t*)w.image16, x->d_pack_flag);
+  DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), sizeof(ent), cudaMemcpyHostToDevice, st));
+  pack_kernel<true><<<TILE_CHUNKS, 256, 0, st>>>(x->d_entries, TILE_CHUNKS, (uint8_t*)w.image16, x->d_pack_flag);
   DMN_LAUNCH_OK();
   int32_t out_of_range = 0;
   DMN_CUDA(cudaMemcpyAsync(&out_of_range, x->d_pack_flag, sizeof(int32_t), cudaMemcpyDeviceToHost, st));

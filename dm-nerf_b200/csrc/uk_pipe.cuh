@@ -22,8 +22,6 @@ constexpr int B_BD = B_WD + 256;           // density bias (+3 pad)
 constexpr int B_WRGB = B_BD + 4;           // rgb_linear weights [3][128]
 constexpr int B_BRGB = B_WRGB + 3 * 128;   // rgb_linear bias (+1 pad)
 constexpr int B_TOTAL = B_BRGB + 4;
-constexpr int MAX_CHUNKS = 5;
-constexpr int MAX_STAGES = 160;
 constexpr int CONSUMERS = 256;             // two warpgroups: MMA issue, epilogues, prologue
 constexpr int N_THREADS = CONSUMERS + 32;  // + one weight-producer warp
 // Status code of the fp16 network in the error word (KArgs::status; the protocol errors are below 1000): an activation or an

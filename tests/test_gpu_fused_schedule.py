@@ -1,6 +1,8 @@
 """GPU: the fused render kernel and the RAW-mode training forward return exactly the bits pinned in tests/golden/fused_bits.npz
-(oracle/make_golden_fused_bits.py), and a render without the coarse maps (want_coarse=False: the coarse tile skips its heads)
-gives the same fine maps, fine depths and fine weights bit for bit as one with them, at every instance-head width."""
+(oracle/make_golden_fused_bits.py); the selected fused kernels, renders at the instance-head widths and a points-mode query
+return those pinned in tests/golden/fused_edge_bits.npz; and a render without the coarse maps (want_coarse=False: the coarse
+tile skips its heads) gives the same fine maps, fine depths and fine weights bit for bit as one with them, at every
+instance-head width."""
 import os
 import sys
 
@@ -18,6 +20,7 @@ from oracle import make_golden_fused_bits as G  # noqa: E402
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 FIXTURE = os.path.join(ROOT, "tests", "golden", "fused_bits.npz")
+EDGE_FIXTURE = os.path.join(ROOT, "tests", "golden", "fused_edge_bits.npz")
 FINE_KEYS = ("rgb_fine", "depth_fine", "acc_fine", "ins_fine", "z_vals_fine", "weights_fine")
 
 
@@ -51,6 +54,23 @@ def test_fused_renders_match_fixture(golden):
 def test_training_forward_matches_fixture(golden):
     seen = _check(golden, G.train_cases(DEV))
     assert sorted(seen) == ["train/acts", "train/out"]
+
+
+@pytest.fixture(scope="module")
+def edge_golden():
+    with np.load(EDGE_FIXTURE) as z:
+        return {k: z[k] for k in z.files}
+
+
+def test_selected_and_head_width_renders_match_fixture(edge_golden):
+    seen = _check(edge_golden, G.edge_render_cases(DEV))
+    expected = [k[:-len("#sha256")] for k in edge_golden if k.endswith("#sha256") and not k.startswith("points/")]
+    assert sorted(seen) == sorted(expected)
+
+
+def test_points_query_matches_fixture(edge_golden):
+    seen = _check(edge_golden, G.points_cases(DEV))
+    assert sorted(seen) == ["points/exact/out", "points/f16/out"]
 
 
 @pytest.mark.parametrize("impl", [_lib.IMPL_UMMA, _lib.IMPL_UMMA_F16], ids=["exact", "fp16"])
