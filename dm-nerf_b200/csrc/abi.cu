@@ -23,22 +23,6 @@ void set_error(const char* fmt, ...) {
   g_error = buf;
 }
 
-// Grow-only device scratch buffer.
-struct Scratch {
-  void* ptr = nullptr;
-  size_t cap = 0;
-  int reserve(size_t bytes) {
-    if (bytes <= cap) return 0;
-    if (ptr) DMN_CUDA(cudaFree(ptr));
-    ptr = nullptr; cap = 0;
-    const size_t want = bytes + bytes / 4;
-    DMN_CUDA(cudaMalloc(&ptr, want));
-    cap = want;
-    return 0;
-  }
-  void release() { if (ptr) cudaFree(ptr); ptr = nullptr; cap = 0; }
-};
-
 // An entry point's object selection: keep_host (4 host words, NULL = no selection) -> keep = &m, or NULL.  Only labels
 // 0 .. n_labels - 1 may be set; n_labels = 0 means no network is bound to label the samples with.
 static int object_mask(const uint32_t* keep_host, int n_labels, ObjMask& m, const ObjMask*& keep, const char* who) {
@@ -63,17 +47,17 @@ struct dmnerf_ctx {
   int device = 0;
   NetParams net[2];
   UmmaWeights packed[2];          // tensor-core operand images (umma_api.cuh)
-  Scratch ws_raw_c, ws_raw_f, ws_z_c, ws_z_f, ws_w_c, ws_w_f;
-  Scratch host_in, host_out;      // device staging for the *_host entry point
-  Scratch frame_rays;             // rays of the frame being rendered by dmnerf_render_frame_host
-  Scratch mesh_pts, mesh_raw;     // one slab of the occupancy sweep: points + zero view directions, network output
-  MeshState* mesh = nullptr;      // buffers of the other mesh entry points (mesh.cu)
-  InventoryState* inventory = nullptr;   // buffers of the object-inventory entry points (inventory.cu)
-  ComponentsState* components = nullptr;   // buffers of the connected-component entry points (components.cu)
+  DeviceBuffer ws_raw_c, ws_raw_f, ws_z_c, ws_z_f, ws_w_c, ws_w_f;
+  DeviceBuffer host_in, host_out; // device staging for the *_host entry point
+  DeviceBuffer frame_rays;        // rays of the frame being rendered by dmnerf_render_frame_host
+  DeviceBuffer mesh_pts, mesh_raw;   // one slab of the occupancy sweep: points + zero view directions, network output
+  DeviceBuffer gemm_wimage, gemm_partial;   // dmnerf_mlp_backward: scratch of the tensor-core GEMMs (gemm_umma.cu)
+  MeshState mesh;                 // buffers of the other mesh entry points (mesh.cu)
+  InventoryState inventory;       // buffers of the object-inventory entry points (inventory.cu)
+  ComponentsState components;     // buffers of the connected-component entry points (components.cu)
   Region region = {};             // region selection read with DMNERF_FLAG_REGION (dmnerf_set_region); bits == NULL: none set
-  Scratch region_tmp;             // dmnerf_region_dilate: the second buffer of a multi-step dilation
+  DeviceBuffer region_tmp;        // dmnerf_region_dilate: the second buffer of a multi-step dilation
   bool profiling = false;
-  bool last_fused = false;       // the last render call took the single-kernel path
   bool profile_valid = false;
   cudaEvent_t ev[DMNERF_N_STAGES + 1] = {};
   // *_host entry points: second stream + events so that the copies of one part of a large batch overlap the kernels of the next
@@ -132,12 +116,6 @@ DMNERF_API int dmnerf_ctx_destroy(dmnerf_ctx* ctx) {
   if (!ctx) return 0;
   cudaSetDevice(ctx->device);
   for (int i = 0; i < 2; ++i) umma_weights_free(ctx->packed[i]);
-  Scratch* all[] = {&ctx->ws_raw_c, &ctx->ws_raw_f, &ctx->ws_z_c, &ctx->ws_z_f, &ctx->ws_w_c, &ctx->ws_w_f,
-                    &ctx->host_in, &ctx->host_out, &ctx->frame_rays, &ctx->mesh_pts, &ctx->mesh_raw, &ctx->region_tmp};
-  for (Scratch* s : all) s->release();
-  mesh_state_free(ctx->mesh);
-  inventory_state_free(ctx->inventory);
-  components_state_free(ctx->components);
   for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_in) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_done) if (e) cudaEventDestroy(e);
@@ -378,7 +356,8 @@ DMNERF_API int dmnerf_mlp_backward(dmnerf_ctx* ctx, int net, float* acts, const 
   DMN_CHECK(net == 0 || net == 1, "mlp_backward: net must be 0 or 1");
   DMN_CHECK(m >= 0 && grads, "mlp_backward: bad arguments");
   DMN_CHECK(m == 0 || (acts && d_out && scratch), "mlp_backward: NULL buffer");
-  return launch_mlp_backward(ctx->net[net], ctx->packed[net], acts, d_out, m, grads, scratch, flags, (cudaStream_t)stream);
+  return launch_mlp_backward(ctx->net[net], ctx->packed[net], acts, d_out, m, grads, scratch, flags, ctx->gemm_wimage,
+                             ctx->gemm_partial, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_composite_backward(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c,
@@ -446,22 +425,20 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
     if (rc) return rc;
     if (prof) for (int i = 1; i <= DMNERF_N_STAGES; ++i) DMN_CUDA(cudaEventRecord(ctx->ev[i], st));
     ctx->profile_valid = prof;
-    ctx->last_fused = true;
     return 0;
   }
-  ctx->last_fused = false;
 
   // scratch for whatever the caller does not want back
   float* z_c = io->z_vals_coarse;
-  if (!z_c) { if (ctx->ws_z_c.reserve((size_t)n * S * 4)) return 2; z_c = (float*)ctx->ws_z_c.ptr; }
+  if (!z_c && ctx->ws_z_c.get((size_t)n * S, &z_c)) return 2;
   float* z_f = io->z_vals_fine;
-  if (!z_f) { if (ctx->ws_z_f.reserve((size_t)n * F * 4)) return 2; z_f = (float*)ctx->ws_z_f.ptr; }
+  if (!z_f && ctx->ws_z_f.get((size_t)n * F, &z_f)) return 2;
   float* w_c = io->weights_coarse;
-  if (!w_c) { if (ctx->ws_w_c.reserve((size_t)n * S * 4)) return 2; w_c = (float*)ctx->ws_w_c.ptr; }
+  if (!w_c && ctx->ws_w_c.get((size_t)n * S, &w_c)) return 2;
   float* raw_c = io->raw_coarse;
-  if (!raw_c) { if (ctx->ws_raw_c.reserve((size_t)n * S * C * 4)) return 2; raw_c = (float*)ctx->ws_raw_c.ptr; }
+  if (!raw_c && ctx->ws_raw_c.get((size_t)n * S * C, &raw_c)) return 2;
   float* raw_f = io->raw_fine;
-  if (!raw_f) { if (ctx->ws_raw_f.reserve((size_t)n * F * C * 4)) return 2; raw_f = (float*)ctx->ws_raw_f.ptr; }
+  if (!raw_f && ctx->ws_raw_f.get((size_t)n * F * C, &raw_f)) return 2;
 
   int rc;
   const bool prof = ctx->profiling;
@@ -517,7 +494,7 @@ DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
   }
   DMN_CHECK(!range0 && !range1, "fp16 network: an activation exceeded the fp16 range (> 65504), so these results are invalid; "
             "render with the exact network (DMNERF_IMPL_UMMA)");
-  return gemm_tc_check_status((cudaStream_t)stream);
+  return 0;
 }
 
 DMNERF_API int dmnerf_profile_enable(dmnerf_ctx* ctx, int enable) {
@@ -561,8 +538,8 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
 
   // ---- inputs: one device arena
   size_t in_floats = (dev_rays ? 0 : (size_t)n * 6) + zin + (perturb ? (size_t)n * (S + NI) : 0);
-  if (ctx->host_in.reserve(in_floats * 4)) return 2;
-  float* d = (float*)ctx->host_in.ptr;
+  float* d;
+  if (ctx->host_in.get(in_floats, &d)) return 2;
   dmnerf_render_io io;
   memset(&io, 0, sizeof(io));
   float* p = d;
@@ -593,8 +570,8 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
   };
   size_t out_floats = 0;
   for (const Out& o : outs) if (h->*(o.hp)) out_floats += (size_t)n * o.per_ray;
-  if (ctx->host_out.reserve(out_floats * 4 + 16)) return 2;
-  float* q = (float*)ctx->host_out.ptr;
+  float* q;
+  if (ctx->host_out.get(out_floats, &q)) return 2;
   for (const Out& o : outs) if (h->*(o.hp)) { io.*(o.hp) = q; q += (size_t)n * o.per_ray; }
 
   // Copies of rows [r0, r1) of the batch.  Every ray is rendered independently of its neighbours (the rows of a tile never
@@ -704,8 +681,8 @@ DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, co
   if (ray_count == 0) return 0;
   DMN_CUDA(cudaSetDevice(ctx->device));
   // rays of the whole frame on the device (helpers.py:50-61; tester.py:59-61), the range asked for is rendered
-  if (ctx->frame_rays.reserve((size_t)H * W * 6 * sizeof(float))) return 2;
-  float* ro = (float*)ctx->frame_rays.ptr;
+  float* ro;
+  if (ctx->frame_rays.get((size_t)H * W * 6, &ro)) return 2;
   float* rd = ro + (size_t)H * W * 3;
   int rc = dmnerf_get_rays(K_host, c2w_host, H, W, ro, rd, stream);
   if (rc) return rc;
@@ -747,10 +724,9 @@ DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* tra
   if (slab <= 0) slab = (int64_t)1 << 20;
   if (slab > n) slab = n;
   const int C = 4 + ctx->net[net].ins_num + 1;
-  if (ctx->mesh_pts.reserve((size_t)slab * 6 * sizeof(float)) || ctx->mesh_raw.reserve((size_t)slab * C * sizeof(float))) return 2;
-  float* pts = (float*)ctx->mesh_pts.ptr;
+  float *pts, *raw;
+  if (ctx->mesh_pts.get((size_t)slab * 6, &pts) || ctx->mesh_raw.get((size_t)slab * C, &raw)) return 2;
   float* dirs = pts + slab * 3;                                   // mesh_generator.py:42: zero view directions
-  float* raw = (float*)ctx->mesh_raw.ptr;
   DMN_CUDA(cudaMemsetAsync(dirs, 0, (size_t)slab * 3 * sizeof(float), st));
   // slab by slab: the [dim^3, C] network output of the original never exists, only [slab, C]
   for (int64_t b = 0; b < n; b += slab) {
@@ -768,7 +744,7 @@ DMNERF_API int dmnerf_mesh_mc_count(dmnerf_ctx* ctx, const float* grid, int nx, 
                                     void* stream) {
   DMN_CHECK(ctx && grid && counts_host, "mesh_mc_count: NULL argument");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return mc_count(&ctx->mesh, grid, nx, ny, nz, level, counts_host, (cudaStream_t)stream);
+  return mc_count(ctx->mesh, grid, nx, ny, nz, level, counts_host, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_mesh_mc_emit(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris,
@@ -788,14 +764,14 @@ DMNERF_API int dmnerf_mesh_normals(dmnerf_ctx* ctx, const float* verts, int64_t 
                                    void* stream) {
   DMN_CHECK(ctx && (nv == 0 || (verts && normals)) && (nt == 0 || tris), "mesh_normals: NULL argument");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return mesh_normals(&ctx->mesh, verts, nv, tris, nt, normals, (cudaStream_t)stream);
+  return mesh_normals(ctx->mesh, verts, nv, tris, nt, normals, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_mesh_clusters(dmnerf_ctx* ctx, const int32_t* tris, int64_t nt, int64_t nv, int32_t* cluster, int32_t* cluster_size,
                                     void* stream) {
   DMN_CHECK(ctx && (nt == 0 || (tris && cluster && cluster_size)), "mesh_clusters: NULL argument");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return mesh_clusters(&ctx->mesh, tris, nt, nv, cluster, cluster_size, (cudaStream_t)stream);
+  return mesh_clusters(ctx->mesh, tris, nt, nv, cluster, cluster_size, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_mesh_clean(dmnerf_ctx* ctx, const float* verts, const float* normals, int64_t nv, const int32_t* tris, int64_t nt,
@@ -805,7 +781,7 @@ DMNERF_API int dmnerf_mesh_clean(dmnerf_ctx* ctx, const float* verts, const floa
   DMN_CHECK(nv == 0 || (verts && out_verts && (!normals == !out_normals)), "mesh_clean: NULL vertex buffer");
   DMN_CHECK(nt == 0 || (tris && cluster_size && out_tris), "mesh_clean: NULL triangle buffer");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return mesh_clean(&ctx->mesh, verts, normals, nv, tris, nt, cluster_size, min_cluster, out_verts, out_normals, out_tris, counts_host,
+  return mesh_clean(ctx->mesh, verts, normals, nv, tris, nt, cluster_size, min_cluster, out_verts, out_normals, out_tris, counts_host,
                     (cudaStream_t)stream);
 }
 
@@ -826,14 +802,14 @@ DMNERF_API int dmnerf_object_voxels(dmnerf_ctx* ctx, const float* occ, const int
                                     const int32_t* boxes_host, int64_t* moments_host, uint32_t* hist_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "object_voxels: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return object_voxels(&ctx->inventory, occ, labels, dim, level, n_labels, boxes_host, moments_host, hist_host, (cudaStream_t)stream);
+  return object_voxels(ctx->inventory, occ, labels, dim, level, n_labels, boxes_host, moments_host, hist_host, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_object_spans(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                                    const int32_t* boxes_host, const double* axes_host, double* spans_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "object_spans: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return object_spans(&ctx->inventory, occ, labels, dim, level, n_labels, boxes_host, axes_host, spans_host, (cudaStream_t)stream);
+  return object_spans(ctx->inventory, occ, labels, dim, level, n_labels, boxes_host, axes_host, spans_host, (cudaStream_t)stream);
 }
 
 // ---- connected components (DESIGN.md, "Connected components") -------------------------------------------------------------
@@ -842,7 +818,7 @@ DMNERF_API int dmnerf_object_components(dmnerf_ctx* ctx, const float* occ, const
                                         int connectivity, int32_t* comp, int64_t* n_components_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "object_components: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return object_components(&ctx->components, occ, labels, dim, level, n_labels, connectivity, comp, n_components_host,
+  return object_components(ctx->components, occ, labels, dim, level, n_labels, connectivity, comp, n_components_host,
                            (cudaStream_t)stream);
 }
 
@@ -850,14 +826,14 @@ DMNERF_API int dmnerf_component_table(dmnerf_ctx* ctx, const int32_t* comp, cons
                                       int64_t* voxels, int64_t* root, void* stream) {
   DMN_CHECK(ctx != nullptr, "component_table: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return component_table(&ctx->components, comp, labels, dim, n, label, voxels, root, (cudaStream_t)stream);
+  return component_table(ctx->components, comp, labels, dim, n, label, voxels, root, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_component_groups(dmnerf_ctx* ctx, const int32_t* comp, int dim, int64_t n, const int16_t* lut, int discard,
                                        int16_t* groups, void* stream) {
   DMN_CHECK(ctx != nullptr, "component_groups: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return component_groups(&ctx->components, comp, dim, n, lut, discard, groups, (cudaStream_t)stream);
+  return component_groups(ctx->components, comp, dim, n, lut, discard, groups, (cudaStream_t)stream);
 }
 
 // ---- region selection (DESIGN.md, "Region selection") ---------------------------------------------------------------------
@@ -891,10 +867,7 @@ DMNERF_API int dmnerf_region_dilate(dmnerf_ctx* ctx, const uint32_t* in, int dim
   DMN_CUDA(cudaSetDevice(ctx->device));
   if (region_check(dim, nullptr, "region_dilate")) return 1;
   uint32_t* tmp = nullptr;
-  if (radius >= 2) {
-    if (ctx->region_tmp.reserve((size_t)region_words(dim) * sizeof(uint32_t))) return 2;
-    tmp = (uint32_t*)ctx->region_tmp.ptr;
-  }
+  if (radius >= 2 && ctx->region_tmp.get((size_t)region_words(dim), &tmp)) return 2;
   return region_dilate(in, dim, radius, connectivity, invert, out, tmp, (cudaStream_t)stream);
 }
 

@@ -110,6 +110,41 @@ extern std::atomic<int64_t> g_launches;
     DMN_CUDA(cudaGetLastError());                           \
   } while (0)
 
+// Grow-only device buffer, the only owner of device memory in the library: get() returns room for n values of T, reallocating
+// (contents lost) with 25 % headroom when a request outgrows it.  Every request carries a 16-byte tail, so that an empty one
+// still yields a valid pointer (a NULL scratch pointer would turn a cub call into a size query).
+class DeviceBuffer {
+ public:
+  DeviceBuffer() = default;
+  DeviceBuffer(const DeviceBuffer&) = delete;
+  DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+  ~DeviceBuffer() { if (ptr_) cudaFree(ptr_); }
+  template <class T>
+  int get(size_t n, T** out) {
+    const size_t bytes = n * sizeof(T) + 16;
+    if (bytes > cap_) {
+      if (ptr_) DMN_CUDA(cudaFree(ptr_));
+      ptr_ = nullptr; cap_ = 0;
+      DMN_CUDA(cudaMalloc(&ptr_, bytes + bytes / 4));
+      cap_ = bytes + bytes / 4;
+    }
+    *out = static_cast<T*>(ptr_);
+    return 0;
+  }
+
+ private:
+  void* ptr_ = nullptr;
+  size_t cap_ = 0;
+};
+
+// Number of SMs of the current device (the grid of a persistent kernel).
+inline int sm_count(int* sms) {
+  int dev = 0;
+  DMN_CUDA(cudaGetDevice(&dev));
+  DMN_CUDA(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+  return 0;
+}
+
 // Object selection (DESIGN.md, "Object selection"): the set of kept labels 0 .. ins_num as a 128-bit mask, bit k of word
 // k / 32.  A sample whose arg-max label (argmax_sigmoid, ray_ops.cuh) is not kept has alpha = 0 in the composite.
 struct ObjMask {
@@ -160,22 +195,24 @@ int launch_composite_backward(const float* raw, const float* z, const float* ray
                               const float* g_rgb, const float* g_depth, const float* g_acc, const float* g_ins,
                               const float* g_weights, float* d_raw, int accumulate, cudaStream_t st);
 // flags: bit 0 = the forward that filled `acts` wrote the ReLU bit planes (tensor-core kernel; otherwise the backward derives
-// them from the saved activations first), bit 1 = grads are already zero.
+// them from the saved activations first), bit 1 = grads are already zero.  wimage / partial: the scratch of the tensor-core
+// GEMMs (launch_gemm_nn_tc / launch_gemm_tn_tc_batch).
 struct UmmaWeights;
 int launch_mlp_backward(const NetParams& p, const UmmaWeights& packed, float* acts, const float* d_out, int64_t m, float* const* grads,
-                        float* scratch, int flags, cudaStream_t st);
+                        float* scratch, int flags, DeviceBuffer& wimage, DeviceBuffer& partial, cudaStream_t st);
 // Gradient chain (bwd_chain.cu)
 int launch_mask_bits(float* acts, int64_t m, cudaStream_t st);
 int launch_bwd_heads(const NetParams& p, const float* d_out, int64_t m, const uint16_t* bits, float* s12, cudaStream_t st);
 int launch_bwd_chain(const UmmaWeights& w, const NetParams& p, const float* s1, const float* d_out, const ActPlanes& ap, int64_t m,
-                     float* const* dy, cudaStream_t st);
+                     float* const* dy, DeviceBuffer& wimage, cudaStream_t st);
 size_t mlp_backward_scratch_floats(int64_t m);
 
-// Tensor-core GEMMs of the backward (gemm_umma.cu): split-bf16 three-pass wgmma kernels for the wide layer shapes.
+// Tensor-core GEMMs of the backward (gemm_umma.cu): split-bf16 three-pass wgmma kernels for the wide layer shapes.  A kernel that
+// gives up on a barrier writes its code (6xx) to `status`, the error word of the weight set being differentiated.
 bool gemm_tn_tc_supported(int N, int K);
-// mask_bits: 1-bit ReLU mask of the output, [16 groups][M] uint16 (one plane of ActPlanes::bits), or NULL.
+// mask_bits: 1-bit ReLU mask of the output, [16 groups][M] uint16 (one plane of ActPlanes::bits), or NULL.  wimage: the packed W.
 int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C, int ldc, int64_t M, int N, int accumulate,
-                      const uint16_t* mask_bits, cudaStream_t st);
+                      const uint16_t* mask_bits, DeviceBuffer& wimage, int32_t* status, cudaStream_t st);
 // One product of a batched dW launch (gemm_umma.cu): C[N, K] += A[M, N]^T B[M, K]; b_cm != 0: B is column-major with that column
 // stride; transpose: A is the wide operand and the result goes to C[K, N].
 constexpr int TN_MAX_BATCH = 8;
@@ -184,8 +221,8 @@ struct TnProblem {
   int64_t b_cm;
   int lda, ldb, ldc, K, transpose;
 };
-int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, cudaStream_t st);
-int gemm_tc_check_status(cudaStream_t st);
+// partial: the per-CTA partial products, reduced in a fixed order.
+int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, DeviceBuffer& partial, int32_t* status, cudaStream_t st);
 
 // Emptiness regulariser (penalizer.cu)
 int launch_penalizer_forward(const float* raw, const float* z, const float* depth, const float* rays_d, int64_t n, int s, int c,
@@ -215,39 +252,50 @@ int launch_hungarian_costs_merged(const double* partials, int world, int64_t n, 
                                   float* s_sum, float* cnt, cudaStream_t st);
 
 // Mesh extraction (mesh.cu).  Transforms are row-major 4x4 float64 host arrays, extents 3 float64 host values.
-struct MeshState;                 // per-context device buffers of the mesh entry points
-void mesh_state_free(MeshState* s);
+// Per-context device buffers of the mesh entry points (the marching-cubes scans and the cleanup's compaction share some), and
+// what the last marching-cubes count pass classified: mc_emit must see the same grid.
+struct MeshState {
+  DeviceBuffer eflags, cases, vcnt, vscan, tcnt, tscan, temp, totals, keys_in, keys_out, vals_in, vals_out, parent, size;
+  const float* grid = nullptr;
+  int nx = 0, ny = 0, nz = 0;
+  float level = 0.f;
+  int64_t nv = -1, nt = -1;
+};
 int launch_grid_points(const double* T16, const double* ext3, int dim, int64_t begin, int64_t count, float* pts, cudaStream_t st);
 int launch_occupancy(const float* raw, int64_t n, int c, float voxel, float* occ, cudaStream_t st);
 // the same with an object selection: occ = 0 where the point's label is not kept; labels [n] int16 (may be NULL)
 int launch_occupancy_objects(const float* raw, int64_t n, int c, float voxel, const ObjMask& keep, float* occ, int16_t* labels,
                              cudaStream_t st);
-int mc_count(MeshState** s, const float* grid, int nx, int ny, int nz, float level, int64_t* counts, cudaStream_t st);
-int mc_emit(MeshState* s, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris, cudaStream_t st);
+int mc_count(MeshState& s, const float* grid, int nx, int ny, int nz, float level, int64_t* counts, cudaStream_t st);
+int mc_emit(MeshState& s, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris, cudaStream_t st);
 int launch_to_scene(const float* v, int64_t n, const double* T16, const double* ext3, int dim, float* out, cudaStream_t st);
-int mesh_normals(MeshState** s, const float* v, int64_t nv, const int32_t* tris, int64_t nt, float* normals, cudaStream_t st);
-int mesh_clusters(MeshState** s, const int32_t* tris, int64_t nt, int64_t nv, int32_t* cluster, int32_t* cluster_size, cudaStream_t st);
-int mesh_clean(MeshState** s, const float* v, const float* nrm, int64_t nv, const int32_t* tris, int64_t nt, const int32_t* csize,
+int mesh_normals(MeshState& s, const float* v, int64_t nv, const int32_t* tris, int64_t nt, float* normals, cudaStream_t st);
+int mesh_clusters(MeshState& s, const int32_t* tris, int64_t nt, int64_t nv, int32_t* cluster, int32_t* cluster_size, cudaStream_t st);
+int mesh_clean(MeshState& s, const float* v, const float* nrm, int64_t nv, const int32_t* tris, int64_t nt, const int32_t* csize,
                int min_cluster, float* out_v, float* out_n, int32_t* out_t, int64_t* counts, cudaStream_t st);
 int launch_label_rays(const float* v, const float* nrm, int64_t n, float near_z, float* ro, float* rd, cudaStream_t st);
 int launch_argmax_rows(const float* x, int64_t n, int c, int64_t* out, cudaStream_t st);
 
-// Object inventory (inventory.cu): per-group integer statistics and fp64 spans of the solid points of a labelled grid
-struct InventoryState;            // per-context device buffers of the inventory entry points
-void inventory_state_free(InventoryState* s);
-int object_voxels(InventoryState** s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+// Object inventory (inventory.cu): per-group integer statistics and fp64 spans of the solid points of a labelled grid.
+// Per-context device buffers: everything a call reads back (status word first), and its inputs.
+struct InventoryState {
+  DeviceBuffer out, in;
+};
+int object_voxels(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                   const int32_t* boxes_host, int64_t* moments_host, uint32_t* hist_host, cudaStream_t st);
-int object_spans(InventoryState** s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+int object_spans(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                  const int32_t* boxes_host, const double* axes_host, double* spans_host, cudaStream_t st);
 
-// Connected components (components.cu): the solid points of a labelled grid split into canonically numbered components
-struct ComponentsState;           // per-context device buffers of the component entry points
-void components_state_free(ComponentsState* s);
-int object_components(ComponentsState** s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+// Connected components (components.cu): the solid points of a labelled grid split into canonically numbered components.
+// Per-context device buffers: the status words a call reads back, the chunk counts and the scan's storage.
+struct ComponentsState {
+  DeviceBuffer status, counts, temp;
+};
+int object_components(ComponentsState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                       int connectivity, int32_t* comp, int64_t* n_components_host, cudaStream_t st);
-int component_table(ComponentsState** s, const int32_t* comp, const int16_t* labels, int dim, int64_t n_comp, int16_t* label,
+int component_table(ComponentsState& s, const int32_t* comp, const int16_t* labels, int dim, int64_t n_comp, int16_t* label,
                     int64_t* voxels, int64_t* root, cudaStream_t st);
-int component_groups(ComponentsState** s, const int32_t* comp, int dim, int64_t n_comp, const int16_t* lut, int discard,
+int component_groups(ComponentsState& s, const int32_t* comp, int dim, int64_t n_comp, const int16_t* lut, int discard,
                      int16_t* groups, cudaStream_t st);
 
 // Region builders (region.cu).  Grids are [dim]^3 in C order; bits are region_words(dim) uint32 words, the tail zero.

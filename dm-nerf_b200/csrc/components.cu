@@ -230,32 +230,8 @@ int check_dim(int dim, const char* who) {
 
 }  // namespace
 
-// Device scratch of the component entry points: the status words a call reads back, the chunk counts and the scan's storage.
-struct ComponentsState {
-  enum { STATUS, COUNTS, TEMP, N_BUF };
-  void* p[N_BUF] = {};
-  size_t cap[N_BUF] = {};
-  int get(int i, size_t bytes, void** out) {
-    if (bytes > cap[i]) {
-      if (p[i]) DMN_CUDA(cudaFree(p[i]));
-      p[i] = nullptr; cap[i] = 0;
-      DMN_CUDA(cudaMalloc(&p[i], bytes));
-      cap[i] = bytes;
-    }
-    *out = p[i];
-    return 0;
-  }
-};
-
-void components_state_free(ComponentsState* s) {
-  if (!s) return;
-  for (void* q : s->p)
-    if (q) cudaFree(q);
-  delete s;
-}
-
 // the call's one device->host read: the status word and (object_components) the int32 total in the low half of the second word
-static int read_status(void* status, int64_t* total_host, cudaStream_t st, const char* who, int n_labels) {
+static int read_status(const int64_t* status, int64_t* total_host, cudaStream_t st, const char* who, int n_labels) {
   int64_t h[2];
   DMN_CUDA(cudaMemcpyAsync(h, status, sizeof(h), cudaMemcpyDeviceToHost, st));
   DMN_CUDA(cudaStreamSynchronize(st));
@@ -267,7 +243,7 @@ static int read_status(void* status, int64_t* total_host, cudaStream_t st, const
   return 0;
 }
 
-int object_components(ComponentsState** sp, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+int object_components(ComponentsState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                       int connectivity, int32_t* comp, int64_t* n_components_host, cudaStream_t st) {
   const char* who = "object_components";
   DMN_CHECK(occ && comp && n_components_host, "%s: NULL occ / comp / n_components", who);
@@ -275,22 +251,19 @@ int object_components(ComponentsState** sp, const float* occ, const int16_t* lab
   DMN_CHECK(n_labels >= 1 && n_labels <= DMNERF_MAX_INS + 1, "%s: n_labels %d out of range [1, %d]", who, n_labels, DMNERF_MAX_INS + 1);
   DMN_CHECK(connectivity == 6 || connectivity == 26, "%s: connectivity %d is not 6 or 26", who, connectivity);
   DMN_CHECK(!(level != level), "%s: level is NaN", who);
-  if (!*sp) *sp = new ComponentsState();
-  ComponentsState* s = *sp;
   const int64_t n = (int64_t)dim * dim * dim;
   const int64_t n_chunks = (n + CC_CHUNK - 1) / CC_CHUNK;
-  void *status, *counts_v, *tmp;
+  int64_t* status;
+  int32_t* counts;
+  uint8_t* tmp;
   // status: [bad, total]; counts: n_chunks + 1 root counts (the last one 0), then their exclusive scan, the chunks' first ids
   // (its last entry is the total)
-  if (s->get(ComponentsState::STATUS, 16, &status) ||
-      s->get(ComponentsState::COUNTS, (size_t)2 * (n_chunks + 1) * sizeof(int32_t), &counts_v))
-    return 2;
-  auto* counts = static_cast<int32_t*>(counts_v);
+  if (s.status.get(2, &status) || s.counts.get((size_t)2 * (n_chunks + 1), &counts)) return 2;
   int32_t* offsets = counts + n_chunks + 1;
   size_t tmp_bytes = 0;
   DMN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts, offsets, (int)(n_chunks + 1), st));
-  if (s->get(ComponentsState::TEMP, tmp_bytes, &tmp)) return 2;
-  int* bad = static_cast<int*>(status);
+  if (s.temp.get(tmp_bytes, &tmp)) return 2;
+  int* bad = reinterpret_cast<int*>(status);
   DMN_CUDA(cudaMemsetAsync(status, 0, 16, st));
   DMN_CUDA(cudaMemsetAsync(counts + n_chunks, 0, sizeof(int32_t), st));
   const int blocks = blocks_for(n);
@@ -311,11 +284,11 @@ int object_components(ComponentsState** sp, const float* occ, const int16_t* lab
   cc_decode_roots_kernel<<<blocks, CC_THREADS, 0, st>>>(n, comp);
   DMN_LAUNCH_OK();
   // the total is offsets[n_chunks]: next to the status word, so that one read brings both
-  DMN_CUDA(cudaMemcpyAsync(static_cast<char*>(status) + 8, offsets + n_chunks, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  DMN_CUDA(cudaMemcpyAsync(status + 1, offsets + n_chunks, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   return read_status(status, n_components_host, st, who, n_labels);
 }
 
-int component_table(ComponentsState** sp, const int32_t* comp, const int16_t* labels, int dim, int64_t n_comp, int16_t* label,
+int component_table(ComponentsState& s, const int32_t* comp, const int16_t* labels, int dim, int64_t n_comp, int16_t* label,
                     int64_t* voxels, int64_t* root, cudaStream_t st) {
   const char* who = "component_table";
   DMN_CHECK(comp != nullptr, "%s: comp is NULL", who);
@@ -323,22 +296,20 @@ int component_table(ComponentsState** sp, const int32_t* comp, const int16_t* la
   const int64_t n = (int64_t)dim * dim * dim;
   DMN_CHECK(n_comp >= 0 && n_comp <= n, "%s: %lld components out of range [0, %lld]", who, (long long)n_comp, (long long)n);
   DMN_CHECK(n_comp == 0 || (label && voxels && root), "%s: NULL label / voxels / root", who);
-  if (!*sp) *sp = new ComponentsState();
-  ComponentsState* s = *sp;
-  void* status;
-  if (s->get(ComponentsState::STATUS, 16, &status)) return 2;
+  int64_t* status;
+  if (s.status.get(2, &status)) return 2;
   DMN_CUDA(cudaMemsetAsync(status, 0, 16, st));
   if (n_comp) {
     DMN_CUDA(cudaMemsetAsync(voxels, 0, (size_t)n_comp * sizeof(int64_t), st));
     DMN_CUDA(cudaMemsetAsync(root, 0x7f, (size_t)n_comp * sizeof(int64_t), st));     // above every index: the empty minimum
   }
   cc_table_kernel<<<blocks_for(n), CC_THREADS, 0, st>>>(comp, labels, n, n_comp, label, reinterpret_cast<unsigned long long*>(voxels),
-                                                        reinterpret_cast<long long*>(root), static_cast<int*>(status));
+                                                        reinterpret_cast<long long*>(root), reinterpret_cast<int*>(status));
   DMN_LAUNCH_OK();
   return read_status(status, nullptr, st, who, 1);
 }
 
-int component_groups(ComponentsState** sp, const int32_t* comp, int dim, int64_t n_comp, const int16_t* lut, int discard,
+int component_groups(ComponentsState& s, const int32_t* comp, int dim, int64_t n_comp, const int16_t* lut, int discard,
                      int16_t* groups, cudaStream_t st) {
   const char* who = "component_groups";
   DMN_CHECK(comp && groups, "%s: NULL comp / groups", who);
@@ -347,12 +318,10 @@ int component_groups(ComponentsState** sp, const int32_t* comp, int dim, int64_t
   DMN_CHECK(n_comp >= 0 && n_comp <= n, "%s: %lld components out of range [0, %lld]", who, (long long)n_comp, (long long)n);
   DMN_CHECK(n_comp == 0 || lut, "%s: lut is NULL", who);
   DMN_CHECK(discard >= -32768 && discard <= 32767, "%s: discard group %d is not an int16", who, discard);
-  if (!*sp) *sp = new ComponentsState();
-  ComponentsState* s = *sp;
-  void* status;
-  if (s->get(ComponentsState::STATUS, 16, &status)) return 2;
+  int64_t* status;
+  if (s.status.get(2, &status)) return 2;
   DMN_CUDA(cudaMemsetAsync(status, 0, 16, st));
-  cc_groups_kernel<<<blocks_for(n), CC_THREADS, 0, st>>>(comp, n, n_comp, lut, (int16_t)discard, groups, static_cast<int*>(status));
+  cc_groups_kernel<<<blocks_for(n), CC_THREADS, 0, st>>>(comp, n, n_comp, lut, (int16_t)discard, groups, reinterpret_cast<int*>(status));
   DMN_LAUNCH_OK();
   return read_status(status, nullptr, st, who, 1);
 }

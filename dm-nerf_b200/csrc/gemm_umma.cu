@@ -368,33 +368,6 @@ __global__ void __launch_bounds__(256) reduce_partials_kernel(const float* __res
   }
 }
 
-// Scratch of the GEMM launches, one set per CUDA device of the process (launches on a device are stream-ordered, so one packed
-// weight image and one partial-product buffer per device are enough; they live until the process exits).
-struct DevState {
-  int32_t* status = nullptr;          // device error word of the GEMM kernels
-  uint8_t* wimage = nullptr;          // packed weights of the dX GEMM in flight (4 chunks x 64 KB)
-  float* partial = nullptr;           // per-CTA partial products of the dW GEMM
-  size_t partial_floats = 0;
-  int sms = 0;
-};
-constexpr int MAX_DEVICES = 64;
-static DevState g_dev[MAX_DEVICES];
-
-static int dev_state(DevState** out) {
-  int dev = 0;
-  DMN_CUDA(cudaGetDevice(&dev));
-  DMN_CHECK(dev >= 0 && dev < MAX_DEVICES, "gemm(tc): device index %d out of range", dev);
-  DevState& d = g_dev[dev];
-  if (!d.status) {
-    DMN_CUDA(cudaMalloc((void**)&d.status, sizeof(int32_t)));
-    DMN_CUDA(cudaMemset(d.status, 0, sizeof(int32_t)));
-    DMN_CUDA(cudaMalloc((void**)&d.wimage, 4 * 2 * NN_W_BYTES));
-    DMN_CUDA(cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev));
-  }
-  *out = &d;
-  return 0;
-}
-
 // rows are 16-byte aligned (128-bit loads)
 static int vec4_ok(const void* p, int ld) { return ((uintptr_t)p % 16 == 0) && (ld % 4 == 0); }
 
@@ -405,25 +378,24 @@ bool gemm_tn_tc_supported(int N, int K) { return (N == 128 || N == 256) && (K ==
 
 // C[M,256] (+)= A[M,N] W[N,256], N = 128 or 256, masked by mask_bits when given.
 int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C, int ldc, int64_t M, int N, int accumulate,
-                      const uint16_t* mask_bits, cudaStream_t st) {
+                      const uint16_t* mask_bits, DeviceBuffer& wimage_buf, int32_t* status, cudaStream_t st) {
   using namespace tg;
   if (M <= 0) return 0;
-  DevState* ds = nullptr;
-  if (dev_state(&ds)) return 1;
-  uint8_t* wimage = ds->wimage;
-  int32_t* g_status = ds->status;
+  uint8_t* wimage;
+  int sms = 0;
+  if (wimage_buf.get(4 * 2 * NN_W_BYTES, &wimage) || sm_count(&sms)) return 2;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
     DMN_CUDA(cudaFuncSetAttribute(gemm_nn_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NN_SMEM));
     DMN_CUDA(cudaFuncSetAttribute(gemm_nn_tc_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NN_SMEM));
   }
   const int64_t tiles = (M + 127) / 128;
-  const unsigned grid = (unsigned)(tiles < ds->sms ? tiles : ds->sms);
+  const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
   const int va = vec4_ok(A, lda), vw = vec4_ok(W, ldw), nch = N / 64;
   pack_w_kernel<<<nch, 512, 0, st>>>(W, ldw, nch, vw, wimage);
   DMN_LAUNCH_OK();
-  if (N == 128) gemm_nn_tc_kernel<2><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, nullptr, mask_bits, nullptr, va, g_status);
-  else gemm_nn_tc_kernel<4><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, nullptr, mask_bits, nullptr, va, g_status);
+  if (N == 128) gemm_nn_tc_kernel<2><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, nullptr, mask_bits, nullptr, va, status);
+  else gemm_nn_tc_kernel<4><<<grid, NN_THREADS, NN_SMEM, st>>>(A, lda, wimage, C, ldc, M, accumulate, nullptr, mask_bits, nullptr, va, status);
   DMN_LAUNCH_OK();
   return 0;
 }
@@ -431,12 +403,10 @@ int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C
 // For every product i < n:  C_i[N, K_i] += A_i[M, N]^T B_i[M, K_i]  (N = 128 or 256; every K_i = 256, or every K_i <= 64);
 // transpose != 0: the caller passes the WIDE matrix as A and the narrow one (K <= 64 columns) as B and wants C[K, N] += B^T A.
 // One GEMM launch + one reduction launch for the whole batch.
-int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, cudaStream_t st) {
+int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, DeviceBuffer& partial, int32_t* status,
+                            cudaStream_t st) {
   using namespace tg;
   if (M <= 0 || n <= 0) return 0;
-  DevState* ds = nullptr;
-  if (dev_state(&ds)) return 1;
-  int32_t* g_status = ds->status;
   DMN_CHECK(n <= TN_MAX_BATCH, "gemm_tn(tc): %d products in one batch (max %d)", n, TN_MAX_BATCH);
   const int NB = (probs[0].K > 64) ? 256 : 64;
   TnBatch batch;
@@ -451,7 +421,9 @@ int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, cud
   }
   const int NBT = NB == 256 ? 128 : 64;
   const int tiles = (N / 128) * (NB / NBT);
-  int slices = ds->sms / (n * tiles);
+  int sms = 0;
+  if (sm_count(&sms)) return 2;
+  int slices = sms / (n * tiles);
   if (slices < 1) slices = 1;
   // A CTA sums at most TN_MAX_ROWS samples into its fp32 tensor-core accumulators: the error of that chain grows with its
   // length (H100, 8 products x 4 tiles = 4 slices: relative L2 error of the weight gradients 5.5e-5 at 16 384 samples per
@@ -462,37 +434,19 @@ int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, cud
   slices = (int)((M + rows - 1) / rows);
   batch.n = n; batch.slices = slices; batch.rows_per_cta = rows;
   const unsigned grid = (unsigned)(n * tiles * slices);
-  const size_t need = (size_t)n * slices * N * NB + (size_t)n * slices * N;       // products, then the column sums
-  if (!ds->partial || ds->partial_floats < need) {
-    if (ds->partial) DMN_CUDA(cudaFree(ds->partial));
-    ds->partial = nullptr;
-    ds->partial_floats = need;
-    DMN_CUDA(cudaMalloc((void**)&ds->partial, need * sizeof(float)));
-  }
-  float* scratch = ds->partial;
+  float* scratch;
+  if (partial.get((size_t)n * slices * N * NB + (size_t)n * slices * N, &scratch)) return 2;      // products, then the column sums
   static PerDeviceOnce attr_once;
   auto smem_of = [](int nbt) { return (uint32_t)(2 * 2 * (2 + nbt / 64) * TN_SLAB + 1024); };
   if (attr_once.first()) {
     DMN_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(128)));
     DMN_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(64)));
   }
-  if (NBT == 128) gemm_tn_tc_kernel<128><<<grid, TN_THREADS, smem_of(128), st>>>(batch, scratch, M, N, NB, g_status);
-  else gemm_tn_tc_kernel<64><<<grid, TN_THREADS, smem_of(64), st>>>(batch, scratch, M, N, NB, g_status);
+  if (NBT == 128) gemm_tn_tc_kernel<128><<<grid, TN_THREADS, smem_of(128), st>>>(batch, scratch, M, N, NB, status);
+  else gemm_tn_tc_kernel<64><<<grid, TN_THREADS, smem_of(64), st>>>(batch, scratch, M, N, NB, status);
   DMN_LAUNCH_OK();
   reduce_partials_kernel<<<dim3((N * NB / 4 + N + 255) / 256, n), 256, 0, st>>>(scratch, batch, N, NB);
   DMN_LAUNCH_OK();
-  return 0;
-}
-
-// Asynchronous failure word of the GEMM kernels (0 = fine); checked by dmnerf_sync_check.
-int gemm_tc_check_status(cudaStream_t st) {
-  int dev = 0;
-  DMN_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= tg::MAX_DEVICES || !tg::g_dev[dev].status) return 0;
-  int32_t h = 0;
-  DMN_CUDA(cudaMemcpyAsync(&h, tg::g_dev[dev].status, sizeof(h), cudaMemcpyDeviceToHost, st));
-  DMN_CUDA(cudaStreamSynchronize(st));
-  DMN_CHECK(h == 0, "tensor-core backward GEMM: barrier protocol failure (code %d)", h);
   return 0;
 }
 

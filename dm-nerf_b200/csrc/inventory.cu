@@ -270,73 +270,49 @@ static int grid_blocks(const InvTiling& t, size_t smem, const void* kernel) {
   return (int)(t.n_tiles < want ? t.n_tiles : want);
 }
 
-static int reject(int bad, int n_labels, const char* who) {
+// The call's one device->host read: the first h.size() bytes of its out buffer, status word first; fails on a bad status.
+static int read_back(const char* out, std::vector<char>& h, int n_labels, const char* who, cudaStream_t st) {
+  DMN_CUDA(cudaMemcpyAsync(h.data(), out, h.size(), cudaMemcpyDeviceToHost, st));
+  DMN_CUDA(cudaStreamSynchronize(st));
+  int bad;
+  memcpy(&bad, h.data(), sizeof(int));
   DMN_CHECK(!(bad & INV_BAD_NAN), "%s: the grid holds NaN values", who);
   DMN_CHECK(!(bad & INV_BAD_LABEL), "%s: the label grid holds a label outside [0, %d]", who, n_labels - 1);
   return 0;
 }
 
-// Device scratch of the inventory entry points: one buffer for everything a call reads back (status word first), one for inputs.
-struct InventoryState {
-  void* out = nullptr;
-  size_t out_cap = 0;
-  void* in = nullptr;
-  size_t in_cap = 0;
-  static int grow(void** p, size_t* cap, size_t bytes) {
-    if (bytes <= *cap) return 0;
-    if (*p) DMN_CUDA(cudaFree(*p));
-    *p = nullptr; *cap = 0;
-    DMN_CUDA(cudaMalloc(p, bytes));
-    *cap = bytes;
-    return 0;
-  }
-};
-
-void inventory_state_free(InventoryState* s) {
-  if (!s) return;
-  if (s->out) cudaFree(s->out);
-  if (s->in) cudaFree(s->in);
-  delete s;
-}
-
-int object_voxels(InventoryState** sp, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+int object_voxels(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                   const int32_t* boxes_host, int64_t* moments_host, uint32_t* hist_host, cudaStream_t st) {
   const char* who = "object_voxels";
   if (check_args(occ, dim, n_labels, who)) return 1;
   DMN_CHECK(moments_host != nullptr, "%s: moments is NULL", who);
   DMN_CHECK(!(level != level), "%s: level is NaN", who);
-  if (!*sp) *sp = new InventoryState();
-  InventoryState* s = *sp;
   const size_t mom_bytes = (size_t)n_labels * N_MOM * sizeof(uint64_t), hist_bytes = (size_t)n_labels * 3 * dim * sizeof(uint32_t);
   const size_t out_bytes = 16 + mom_bytes + hist_bytes;
-  if (InventoryState::grow(&s->out, &s->out_cap, out_bytes)) return 2;
-  int* bad = static_cast<int*>(s->out);
-  auto* mom = reinterpret_cast<unsigned long long*>(static_cast<char*>(s->out) + 16);
-  auto* hist = reinterpret_cast<uint32_t*>(static_cast<char*>(s->out) + 16 + mom_bytes);
-  const int* boxes = nullptr;
+  char* out;
+  if (s.out.get(out_bytes, &out)) return 2;
+  int* bad = reinterpret_cast<int*>(out);
+  auto* mom = reinterpret_cast<unsigned long long*>(out + 16);
+  auto* hist = reinterpret_cast<uint32_t*>(out + 16 + mom_bytes);
+  int* boxes = nullptr;
   if (boxes_host) {
-    if (InventoryState::grow(&s->in, &s->in_cap, (size_t)n_labels * 6 * sizeof(int))) return 2;
-    DMN_CUDA(cudaMemcpyAsync(s->in, boxes_host, (size_t)n_labels * 6 * sizeof(int), cudaMemcpyHostToDevice, st));
-    boxes = static_cast<const int*>(s->in);
+    if (s.in.get((size_t)n_labels * 6, &boxes)) return 2;
+    DMN_CUDA(cudaMemcpyAsync(boxes, boxes_host, (size_t)n_labels * 6 * sizeof(int), cudaMemcpyHostToDevice, st));
   }
-  DMN_CUDA(cudaMemsetAsync(s->out, 0, out_bytes, st));
+  DMN_CUDA(cudaMemsetAsync(out, 0, out_bytes, st));
   const InvTiling tl = tiling(dim);
   const size_t smem = (size_t)n_labels * (2 * TILE + 2) * sizeof(uint32_t) + (boxes ? (size_t)n_labels * 6 * sizeof(int) : 0);
   object_voxels_kernel<<<grid_blocks(tl, smem, (const void*)object_voxels_kernel), THREADS, smem, st>>>(
       occ, labels, tl, level, n_labels, boxes, mom, hist, bad);
   DMN_LAUNCH_OK();
   std::vector<char> h(out_bytes);
-  DMN_CUDA(cudaMemcpyAsync(h.data(), s->out, out_bytes, cudaMemcpyDeviceToHost, st));
-  DMN_CUDA(cudaStreamSynchronize(st));
-  int hbad;
-  memcpy(&hbad, h.data(), sizeof(int));
-  if (reject(hbad, n_labels, who)) return 1;
+  if (const int rc = read_back(out, h, n_labels, who, st)) return rc;
   memcpy(moments_host, h.data() + 16, mom_bytes);
   if (hist_host) memcpy(hist_host, h.data() + 16 + mom_bytes, hist_bytes);
   return 0;
 }
 
-int object_spans(InventoryState** sp, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+int object_spans(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                  const int32_t* boxes_host, const double* axes_host, double* spans_host, cudaStream_t st) {
   const char* who = "object_spans";
   if (check_args(occ, dim, n_labels, who)) return 1;
@@ -344,11 +320,10 @@ int object_spans(InventoryState** sp, const float* occ, const int16_t* labels, i
   DMN_CHECK(!(level != level), "%s: level is NaN", who);
   for (int q = 0; q < n_labels * 12; ++q)
     DMN_CHECK(std::isfinite(axes_host[q]), "%s: axis coefficient %d of label %d is not finite", who, q % 12, q / 12);
-  if (!*sp) *sp = new InventoryState();
-  InventoryState* s = *sp;
   const size_t key_bytes = (size_t)n_labels * 6 * sizeof(long long), out_bytes = 16 + key_bytes;
   const size_t axes_bytes = (size_t)n_labels * 12 * sizeof(double), box_bytes = (size_t)n_labels * 6 * sizeof(int);
-  if (InventoryState::grow(&s->out, &s->out_cap, out_bytes) || InventoryState::grow(&s->in, &s->in_cap, axes_bytes + box_bytes)) return 2;
+  char *out, *in_d;
+  if (s.out.get(out_bytes, &out) || s.in.get(axes_bytes + box_bytes, &in_d)) return 2;
   // inputs and the empty extrema go up in one copy each: [status | keys] and [axes | boxes]
   std::vector<char> init(out_bytes, 0);
   for (int q = 0; q < n_labels * 6; ++q) {
@@ -358,23 +333,19 @@ int object_spans(InventoryState** sp, const float* occ, const int16_t* labels, i
   std::vector<char> in(axes_bytes + box_bytes);
   memcpy(in.data(), axes_host, axes_bytes);
   memcpy(in.data() + axes_bytes, boxes_host, box_bytes);
-  DMN_CUDA(cudaMemcpyAsync(s->out, init.data(), out_bytes, cudaMemcpyHostToDevice, st));
-  DMN_CUDA(cudaMemcpyAsync(s->in, in.data(), in.size(), cudaMemcpyHostToDevice, st));
-  int* bad = static_cast<int*>(s->out);
-  auto* keys = reinterpret_cast<long long*>(static_cast<char*>(s->out) + 16);
-  const auto* axes = static_cast<const double*>(s->in);
-  const auto* boxes = reinterpret_cast<const int*>(static_cast<const char*>(s->in) + axes_bytes);
+  DMN_CUDA(cudaMemcpyAsync(out, init.data(), out_bytes, cudaMemcpyHostToDevice, st));
+  DMN_CUDA(cudaMemcpyAsync(in_d, in.data(), in.size(), cudaMemcpyHostToDevice, st));
+  int* bad = reinterpret_cast<int*>(out);
+  auto* keys = reinterpret_cast<long long*>(out + 16);
+  const auto* axes = reinterpret_cast<const double*>(in_d);
+  const auto* boxes = reinterpret_cast<const int*>(in_d + axes_bytes);
   const InvTiling tl = tiling(dim);
   const size_t smem = key_bytes + (size_t)n_labels * sizeof(int) + box_bytes;
   object_spans_kernel<<<grid_blocks(tl, smem, (const void*)object_spans_kernel), THREADS, smem, st>>>(
       occ, labels, tl, level, n_labels, boxes, axes, keys, bad);
   DMN_LAUNCH_OK();
   std::vector<char> h(out_bytes);
-  DMN_CUDA(cudaMemcpyAsync(h.data(), s->out, out_bytes, cudaMemcpyDeviceToHost, st));
-  DMN_CUDA(cudaStreamSynchronize(st));
-  int hbad;
-  memcpy(&hbad, h.data(), sizeof(int));
-  if (reject(hbad, n_labels, who)) return 1;
+  if (const int rc = read_back(out, h, n_labels, who, st)) return rc;
   for (int q = 0; q < n_labels * 6; ++q) {
     long long key;
     memcpy(&key, h.data() + 16 + q * sizeof(long long), sizeof(key));

@@ -121,41 +121,6 @@ constexpr McTable kTable = make_table();
 
 __constant__ McTable c_mc = mcgen::kTable;
 
-// ---- device buffers of the mesh entry points (grow-only, owned by the context) ---------------------------------------------
-struct MeshState {
-  enum { EFLAGS, CASES, VCNT, VSCAN, TCNT, TSCAN, TEMP, TOTALS, KEYS_IN, KEYS_OUT, VALS_IN, VALS_OUT, PARENT, SIZE, N_BUF };
-  void* p[N_BUF] = {};
-  size_t cap[N_BUF] = {};
-  // what the last marching-cubes count pass classified (mc_emit must see the same grid)
-  const float* grid = nullptr;
-  int nx = 0, ny = 0, nz = 0;
-  float level = 0.f;
-  int64_t nv = -1, nt = -1;
-  template <class T>
-  int get(int i, size_t n, T** out) {
-    const size_t bytes = n * sizeof(T) + 16;
-    if (bytes > cap[i]) {
-      if (p[i]) DMN_CUDA(cudaFree(p[i]));
-      p[i] = nullptr; cap[i] = 0;
-      DMN_CUDA(cudaMalloc(&p[i], bytes + bytes / 4));
-      cap[i] = bytes + bytes / 4;
-    }
-    *out = static_cast<T*>(p[i]);
-    return 0;
-  }
-};
-
-void mesh_state_free(MeshState* s) {
-  if (!s) return;
-  for (void* q : s->p) if (q) cudaFree(q);
-  delete s;
-}
-
-static MeshState* state(MeshState** s) {
-  if (!*s) *s = new MeshState();
-  return *s;
-}
-
 static inline unsigned blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
 // ---- query grid and occupancy -------------------------------------------------------------------------------------------
@@ -319,40 +284,38 @@ __global__ void mc_triangle_kernel(int nx, int ny, int nz, const uint8_t* __rest
 }
 
 template <class F>
-static int cub_temp(MeshState* s, F&& run) {
+static int cub_temp(MeshState& s, F&& run) {
   size_t bytes = 0;
   DMN_CUDA(run(nullptr, bytes));
   uint8_t* tmp = nullptr;
-  if (s->get(MeshState::TEMP, bytes, &tmp)) return 2;
+  if (s.temp.get(bytes, &tmp)) return 2;
   DMN_CUDA(run(tmp, bytes));
   return 0;
 }
 
-static int exclusive_sum(MeshState* s, const int32_t* in, int32_t* out, int64_t n, cudaStream_t st) {
+static int exclusive_sum(MeshState& s, const int32_t* in, int32_t* out, int64_t n, cudaStream_t st) {
   return cub_temp(s, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, in, out, (int)n, st); });
 }
 
-static int read_back(MeshState* s, int64_t* host, int n, cudaStream_t st) {
+static int read_back(MeshState& s, int64_t* host, int n, cudaStream_t st) {
   int64_t* d = nullptr;
-  if (s->get(MeshState::TOTALS, 4, &d)) return 2;
+  if (s.totals.get(4, &d)) return 2;
   DMN_CUDA(cudaMemcpyAsync(host, d, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
   DMN_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
 
-int mc_count(MeshState** sp, const float* grid, int nx, int ny, int nz, float level, int64_t* counts, cudaStream_t st) {
+int mc_count(MeshState& s, const float* grid, int nx, int ny, int nz, float level, int64_t* counts, cudaStream_t st) {
   DMN_CHECK(nx >= 2 && ny >= 2 && nz >= 2, "mc_count: grid %dx%dx%d is smaller than one cell", nx, ny, nz);
   const int64_t n = (int64_t)nx * ny * nz;
   DMN_CHECK(n * MC_MAX_TRI < INT32_MAX, "mc_count: grid of %lld points exceeds the 32-bit vertex / triangle numbering", (long long)n);
   DMN_CHECK(!(level != level), "mc_count: level is NaN");
-  MeshState* s = state(sp);
-  s->grid = nullptr;
+  s.grid = nullptr;
   uint8_t *ef, *cs;
   int32_t *vc, *vs, *tc, *ts;
   int64_t* tot;
-  if (s->get(MeshState::EFLAGS, n, &ef) || s->get(MeshState::CASES, n, &cs) || s->get(MeshState::VCNT, n, &vc) ||
-      s->get(MeshState::VSCAN, n, &vs) || s->get(MeshState::TCNT, n, &tc) || s->get(MeshState::TSCAN, n, &ts) ||
-      s->get(MeshState::TOTALS, 4, &tot))
+  if (s.eflags.get(n, &ef) || s.cases.get(n, &cs) || s.vcnt.get(n, &vc) || s.vscan.get(n, &vs) || s.tcnt.get(n, &tc) ||
+      s.tscan.get(n, &ts) || s.totals.get(4, &tot))
     return 2;
   int32_t* nan_seen = reinterpret_cast<int32_t*>(tot + 3);
   DMN_CUDA(cudaMemsetAsync(nan_seen, 0, sizeof(int32_t), st));
@@ -364,27 +327,26 @@ int mc_count(MeshState** sp, const float* grid, int nx, int ny, int nz, float le
   int64_t h[3];
   if (read_back(s, h, 3, st)) return 2;
   DMN_CHECK(h[2] == 0, "mc_count: the grid holds NaN values");
-  s->grid = grid; s->nx = nx; s->ny = ny; s->nz = nz; s->level = level;
-  s->nv = h[0]; s->nt = h[1];
+  s.grid = grid; s.nx = nx; s.ny = ny; s.nz = nz; s.level = level;
+  s.nv = h[0]; s.nt = h[1];
   counts[0] = h[0];
   counts[1] = h[1];
   return 0;
 }
 
-int mc_emit(MeshState* s, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris, cudaStream_t st) {
-  DMN_CHECK(s && s->grid == grid && s->nx == nx && s->ny == ny && s->nz == nz && s->level == level,
+int mc_emit(MeshState& s, const float* grid, int nx, int ny, int nz, float level, float* verts, int32_t* tris, cudaStream_t st) {
+  DMN_CHECK(s.grid == grid && s.nx == nx && s.ny == ny && s.nz == nz && s.level == level,
             "mc_emit: call dmnerf_mesh_mc_count on the same grid and level first");
-  DMN_CHECK((s->nv == 0 || verts) && (s->nt == 0 || tris), "mc_emit: NULL output");
+  DMN_CHECK((s.nv == 0 || verts) && (s.nt == 0 || tris), "mc_emit: NULL output");
   const int64_t n = (int64_t)nx * ny * nz;
-  auto* ef = static_cast<const uint8_t*>(s->p[MeshState::EFLAGS]);
-  auto* cs = static_cast<const uint8_t*>(s->p[MeshState::CASES]);
-  auto* vs = static_cast<const int32_t*>(s->p[MeshState::VSCAN]);
-  auto* ts = static_cast<const int32_t*>(s->p[MeshState::TSCAN]);
-  if (s->nv) {
+  uint8_t *ef, *cs;
+  int32_t *vs, *ts;
+  if (s.eflags.get(n, &ef) || s.cases.get(n, &cs) || s.vscan.get(n, &vs) || s.tscan.get(n, &ts)) return 2;   // as mc_count left them
+  if (s.nv) {
     mc_vertex_kernel<<<blocks(n, 256), 256, 0, st>>>(grid, nx, ny, nz, level, ef, vs, verts);
     DMN_LAUNCH_OK();
   }
-  if (s->nt) {
+  if (s.nt) {
     mc_triangle_kernel<<<blocks(n, 256), 256, 0, st>>>(nx, ny, nz, cs, ts, ef, vs, tris);
     DMN_LAUNCH_OK();
   }
@@ -462,13 +424,12 @@ __global__ void normals_kernel(const float* __restrict__ v, const int32_t* __res
   normals[3 * i + 2] = (float)(sz * inv);
 }
 
-int mesh_normals(MeshState** sp, const float* v, int64_t nv, const int32_t* tris, int64_t nt, float* normals, cudaStream_t st) {
+int mesh_normals(MeshState& s, const float* v, int64_t nv, const int32_t* tris, int64_t nt, float* normals, cudaStream_t st) {
   DMN_CHECK(nv >= 0 && nt >= 0 && nv < INT32_MAX && 3 * nt < INT32_MAX, "mesh_normals: bad sizes");
   if (nv == 0) return 0;
-  MeshState* s = state(sp);
   const int64_t n3 = 3 * nt;
   int32_t *kout, *vin, *vout;
-  if (s->get(MeshState::KEYS_OUT, n3, &kout) || s->get(MeshState::VALS_IN, n3, &vin) || s->get(MeshState::VALS_OUT, n3, &vout)) return 2;
+  if (s.keys_out.get(n3, &kout) || s.vals_in.get(n3, &vin) || s.vals_out.get(n3, &vout)) return 2;
   if (n3) {
     iota_tri_kernel<<<blocks(n3, 256), 256, 0, st>>>(n3, vin);
     DMN_LAUNCH_OK();
@@ -539,16 +500,15 @@ __global__ void cluster_size_kernel(int64_t nt, const int32_t* __restrict__ clus
   if (t < nt) out[t] = size[cluster[t]];
 }
 
-int mesh_clusters(MeshState** sp, const int32_t* tris, int64_t nt, int64_t nv, int32_t* cluster, int32_t* cluster_size,
+int mesh_clusters(MeshState& s, const int32_t* tris, int64_t nt, int64_t nv, int32_t* cluster, int32_t* cluster_size,
                   cudaStream_t st) {
   DMN_CHECK(nt >= 0 && nv >= 0 && 3 * nt < INT32_MAX && nv < INT32_MAX, "mesh_clusters: bad sizes");
   if (nt == 0) return 0;
-  MeshState* s = state(sp);
   const int64_t n3 = 3 * nt;
   uint64_t *kin, *kout;
   int32_t *vin, *vout, *parent, *size;
-  if (s->get(MeshState::KEYS_IN, n3, &kin) || s->get(MeshState::KEYS_OUT, n3, &kout) || s->get(MeshState::VALS_IN, n3, &vin) ||
-      s->get(MeshState::VALS_OUT, n3, &vout) || s->get(MeshState::PARENT, nt, &parent) || s->get(MeshState::SIZE, nt, &size))
+  if (s.keys_in.get(n3, &kin) || s.keys_out.get(n3, &kout) || s.vals_in.get(n3, &vin) || s.vals_out.get(n3, &vout) ||
+      s.parent.get(nt, &parent) || s.size.get(nt, &size))
     return 2;
   edge_keys_kernel<<<blocks(n3, 256), 256, 0, st>>>(tris, nt, nv, kin, vin);
   DMN_LAUNCH_OK();
@@ -604,18 +564,17 @@ __global__ void clean_totals_kernel(const int32_t* vref, const int32_t* vpos, in
   out[1] = nt ? (int64_t)tpos[nt - 1] + keep[nt - 1] : 0;
 }
 
-int mesh_clean(MeshState** sp, const float* v, const float* nrm, int64_t nv, const int32_t* tris, int64_t nt, const int32_t* csize,
+int mesh_clean(MeshState& s, const float* v, const float* nrm, int64_t nv, const int32_t* tris, int64_t nt, const int32_t* csize,
                int min_cluster, float* out_v, float* out_n, int32_t* out_t, int64_t* counts, cudaStream_t st) {
   DMN_CHECK(nt >= 0 && nv >= 0 && 3 * nt < INT32_MAX && nv < INT32_MAX, "mesh_clean: bad sizes");
-  MeshState* s = state(sp);
   counts[0] = counts[1] = 0;
   if (nt == 0 && nv == 0) return 0;
   int32_t *keep, *tpos, *vref, *vpos;
   int64_t* tot;
-  if (s->get(MeshState::VCNT, nt + 1, &keep) || s->get(MeshState::VSCAN, nt + 1, &tpos) || s->get(MeshState::TCNT, nv + 1, &vref) ||
-      s->get(MeshState::TSCAN, nv + 1, &vpos) || s->get(MeshState::TOTALS, 4, &tot))
+  if (s.vcnt.get(nt + 1, &keep) || s.vscan.get(nt + 1, &tpos) || s.tcnt.get(nv + 1, &vref) || s.tscan.get(nv + 1, &vpos) ||
+      s.totals.get(4, &tot))
     return 2;
-  s->grid = nullptr;                            // the marching-cubes scans share these buffers
+  s.grid = nullptr;                             // the marching-cubes scans share these buffers
   if (nt) {
     keep_kernel<<<blocks(nt, 256), 256, 0, st>>>(csize, nt, min_cluster, keep);
     DMN_LAUNCH_OK();

@@ -850,29 +850,23 @@ __global__ void bias_kernel(NetParams p, const float* __restrict__ fold_b_rgb, c
 }  // namespace uk
 
 // ================================================================================================ API
-struct UmmaExtra {            // hangs off UmmaWeights::image allocation bookkeeping
+struct UmmaExtra {            // hangs off UmmaWeights::extra
   uk::Program prog;           // the stream of UmmaWeights::image
   uk::Program prog16;         // the stream of UmmaWeights::image16: one stage per chunk
-  float* fold_w_rgb; float* fold_w_ins; float* fold_b; uk::PackStage* d_entries;
-  int32_t* d_pack_flag;       // fp16 pack: set when a weight exceeds the fp16 range
-  int32_t* d_status;          // device alias of h_status
-  volatile int32_t* h_status;  // error word in mapped host memory: a kernel that gave up on a barrier writes its code here, and the
-                              // NEXT launch through this weight set refuses to start (a stalled launch can never pass silently)
+  struct {                    // the memory behind UmmaWeights' pointers and the ones below
+    DeviceBuffer image, image16, bias, fold_w_rgb, fold_w_ins, fold_b, entries, pack_flag;
+  } mem;
+  float* fold_w_rgb = nullptr; float* fold_w_ins = nullptr; float* fold_b = nullptr; uk::PackStage* d_entries = nullptr;
+  int32_t* d_status = nullptr;           // device alias of h_status
+  volatile int32_t* h_status = nullptr;  // error word in mapped host memory: a kernel (network or backward GEMM) that gave up on a
+                                         // barrier writes its code here, and the NEXT launch through this weight set refuses to
+                                         // start (a stalled launch can never pass silently)
 };
 
 static UmmaExtra* extra_of(const UmmaWeights& w) { return reinterpret_cast<UmmaExtra*>(w.extra); }
 
 void umma_weights_free(UmmaWeights& w) {
-  if (w.image) cudaFree(w.image);
-  if (w.image16) cudaFree(w.image16);
-  if (w.bias) cudaFree(w.bias);
-  if (w.extra) {
-    UmmaExtra* x = extra_of(w);
-    if (x->fold_w_rgb) cudaFree(x->fold_w_rgb);
-    if (x->fold_w_ins) cudaFree(x->fold_w_ins);
-    if (x->fold_b) cudaFree(x->fold_b);
-    if (x->d_entries) cudaFree(x->d_entries);
-    if (x->d_pack_flag) cudaFree(x->d_pack_flag);
+  if (UmmaExtra* x = extra_of(w)) {
     if (x->h_status) cudaFreeHost((void*)x->h_status);
     delete x;
   }
@@ -923,18 +917,14 @@ int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
   if (w.extra && w.ins_num != p.ins_num) umma_weights_free(w);
   if (!w.extra) {
     UmmaExtra* x = new UmmaExtra();
-    memset(x, 0, sizeof(*x));
     x->prog = make_program(p.ins_num, false);
     x->prog16 = make_program(p.ins_num, true);
     w.extra = x;
     w.ins_num = p.ins_num;
-    w.image_bytes = x->prog.stage_off[x->prog.n_stages];
-    DMN_CUDA(cudaMalloc(&w.image, w.image_bytes));
-    DMN_CUDA(cudaMalloc((void**)&w.bias, B_TOTAL * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->fold_w_rgb, 128 * 283 * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->fold_w_ins, 128 * 256 * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->fold_b, 256 * sizeof(float)));
-    DMN_CUDA(cudaMalloc((void**)&x->d_entries, TILE_CHUNKS * sizeof(PackStage)));
+    if (x->mem.image.get(x->prog.stage_off[x->prog.n_stages], &w.image) || x->mem.bias.get(B_TOTAL, &w.bias) ||
+        x->mem.fold_w_rgb.get(128 * 283, &x->fold_w_rgb) || x->mem.fold_w_ins.get(128 * 256, &x->fold_w_ins) ||
+        x->mem.fold_b.get(256, &x->fold_b) || x->mem.entries.get(TILE_CHUNKS, &x->d_entries))
+      return 2;
     DMN_CUDA(cudaHostAlloc((void**)&x->h_status, sizeof(int32_t), cudaHostAllocMapped));
     *x->h_status = 0;
     DMN_CUDA(cudaHostGetDevicePointer((void**)&x->d_status, (void*)x->h_status, 0));
@@ -949,7 +939,7 @@ int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
   const auto ent = pack_entries(x->prog, p, x, false);
   DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), sizeof(ent), cudaMemcpyHostToDevice, st));
   DMN_CUDA(cudaStreamSynchronize(st));               // `ent` is a host temporary
-  pack_kernel<false><<<TILE_CHUNKS, 256, 0, st>>>(x->d_entries, TILE_CHUNKS, (uint8_t*)w.image, nullptr);
+  pack_kernel<false><<<TILE_CHUNKS, 256, 0, st>>>(x->d_entries, TILE_CHUNKS, w.image, nullptr);
   DMN_LAUNCH_OK();
   bias_kernel<<<8, 256, 0, st>>>(p, x->fold_b, x->fold_b + 128, w.bias);
   DMN_LAUNCH_OK();
@@ -962,16 +952,16 @@ int umma_weights_pack_f16(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
   DMN_CHECK(w.ready && w.extra, "fp16 network: weights not packed (call dmnerf_set_weights first)");
   if (w.f16_ready) return 0;
   UmmaExtra* x = extra_of(w);
-  if (!w.image16) DMN_CUDA(cudaMalloc(&w.image16, x->prog16.stage_off[x->prog16.n_stages]));
-  if (!x->d_pack_flag) DMN_CUDA(cudaMalloc((void**)&x->d_pack_flag, sizeof(int32_t)));
+  int32_t* pack_flag;
+  if (x->mem.image16.get(x->prog16.stage_off[x->prog16.n_stages], &w.image16) || x->mem.pack_flag.get(1, &pack_flag)) return 2;
   // the folded head layers are the fp32 fold of the exact pack (fp64 accumulate), rounded to fp16 here
   const auto ent = pack_entries(x->prog16, p, x, true);
-  DMN_CUDA(cudaMemsetAsync(x->d_pack_flag, 0, sizeof(int32_t), st));
+  DMN_CUDA(cudaMemsetAsync(pack_flag, 0, sizeof(int32_t), st));
   DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), sizeof(ent), cudaMemcpyHostToDevice, st));
-  pack_kernel<true><<<TILE_CHUNKS, 256, 0, st>>>(x->d_entries, TILE_CHUNKS, (uint8_t*)w.image16, x->d_pack_flag);
+  pack_kernel<true><<<TILE_CHUNKS, 256, 0, st>>>(x->d_entries, TILE_CHUNKS, w.image16, pack_flag);
   DMN_LAUNCH_OK();
   int32_t out_of_range = 0;
-  DMN_CUDA(cudaMemcpyAsync(&out_of_range, x->d_pack_flag, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  DMN_CUDA(cudaMemcpyAsync(&out_of_range, pack_flag, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   DMN_CUDA(cudaStreamSynchronize(st));               // `ent` is a host temporary; the range verdict is read below
   DMN_CHECK(!out_of_range, "fp16 network: a weight exceeds the fp16 range (|w| > 65504); use the exact network (DMNERF_IMPL_UMMA)");
   w.f16_ready = true;
@@ -985,9 +975,8 @@ static int launch_umma(int64_t units, const uk::Program& prog, const uk::KArgs& 
   using namespace uk;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) DMN_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  int dev = 0, sms = 0;
-  DMN_CUDA(cudaGetDevice(&dev));
-  DMN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms = 0;
+  if (sm_count(&sms)) return 2;
   Kernel<<<(unsigned)(units < sms ? units : sms), N_THREADS, SMEM_BYTES, st>>>(prog, a);
   DMN_LAUNCH_OK();
   return 0;
@@ -1006,7 +995,7 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
   UmmaExtra* ex = extra_of(w);
   KArgs a;
   memset(&a, 0, sizeof(a));
-  a.image = (const uint8_t*)(f16 ? w.image16 : w.image); a.bias = w.bias; a.x = x; a.rays_o = rays_o; a.rays_d = rays_d; a.z = z;
+  a.image = f16 ? w.image16 : w.image; a.bias = w.bias; a.x = x; a.rays_o = rays_o; a.rays_d = rays_d; a.z = z;
   a.m = m; a.s = s; a.out = out; a.acts = acts; a.status = ex->d_status;
   const int64_t tiles = (m + TILE_M - 1) / TILE_M;
   if (f16) return launch_umma<mlp_f16_kernel<false>>(tiles, ex->prog16, a, st);
@@ -1027,8 +1016,8 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   UmmaExtra* ex = extra_of(wc);
   KArgs a;
   memset(&a, 0, sizeof(a));
-  a.image = (const uint8_t*)(f16 ? wc.image16 : wc.image); a.bias = wc.bias;
-  a.image_fine = (const uint8_t*)(f16 ? wf.image16 : wf.image); a.bias_fine = wf.bias;
+  a.image = f16 ? wc.image16 : wc.image; a.bias = wc.bias;
+  a.image_fine = f16 ? wf.image16 : wf.image; a.bias_fine = wf.bias;
   a.rays_o = io->rays_o; a.rays_d = io->rays_d;
   a.z_in = io->z_coarse; a.z_stride = io->z_row_stride;
   const bool perturb = (flags & DMNERF_FLAG_PERTURB) != 0;
@@ -1053,10 +1042,9 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
 }
 
 int umma_check_status(const UmmaWeights& w, cudaStream_t st) {
-  if (!w.extra) return 0;
-  int32_t code = 0;
   DMN_CUDA(cudaStreamSynchronize(st));
-  code = (int32_t)*extra_of(w)->h_status;
+  const int code = umma_status_peek(w);
+  DMN_CHECK(code / 100 != 6, "tensor-core backward GEMM: barrier protocol failure (code %d)", code);     // gemm_umma.cu: 6xx
   DMN_CHECK(code == 0, "tensor-core MLP kernel reported protocol error %d (bounded wait expired)", code);
   return 0;
 }

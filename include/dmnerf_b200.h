@@ -347,7 +347,8 @@ DMNERF_API int dmnerf_render_forward_host(dmnerf_ctx* ctx, const dmnerf_render_i
                                int n_importance, int flags, int impl, void* stream);
 
 /* Synchronise `stream` and report any asynchronous failure of the kernels launched through `ctx` (CUDA errors and
- * the tensor-core kernel's bounded-wait protocol check). */
+ * the bounded-wait protocol checks of the tensor-core network kernels and backward GEMMs).  A protocol failure stays with the
+ * weight set it ran with: later tensor-core launches through it refuse to start until the context is destroyed. */
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream);
 
 /* Per-stage device timing of dmnerf_render_forward (CUDA events recorded on the launch stream around each stage):
