@@ -19,7 +19,7 @@ LIB_PATH = os.environ.get("DMNERF_LIB_PATH") or os.path.join(_HERE, "lib", "libd
 ABI_VERSION = 3
 N_PARAMS = 30
 IMPL_AUTO, IMPL_SIMT, IMPL_UMMA, IMPL_UMMA_F16 = 0, 1, 2, 3
-FLAG_PERTURB, FLAG_WANT_RAW, FLAG_KEEP_INS, FLAG_SELECT, FLAG_REGION = 1, 2, 4, 8, 16
+FLAG_PERTURB, FLAG_WANT_RAW, FLAG_KEEP_INS, FLAG_SELECT, FLAG_REGION, FLAG_APPEARANCE = 1, 2, 4, 8, 16, 32
 LABEL_WORDS = 2049           # DMNERF_LABEL_WORDS
 
 _f32p = C.c_void_p
@@ -148,6 +148,7 @@ PROTOTYPES = {
     "dmnerf_region_pack": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "dmnerf_region_dilate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "dmnerf_region_contains": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_float), _f32p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "dmnerf_set_appearance": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.c_int, C.c_void_p]),
     "dmnerf_eval_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int, C.c_int, C.c_int]),
     "dmnerf_eval_image": (C.c_int, [_f32p, _f32p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dmnerf_ins_eval": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_void_p, C.c_int, _f32p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,

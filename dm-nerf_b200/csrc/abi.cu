@@ -57,6 +57,11 @@ struct dmnerf_ctx {
   ComponentsState components;     // buffers of the connected-component entry points (components.cu)
   Region region = {};             // region selection read with DMNERF_FLAG_REGION (dmnerf_set_region); bits == NULL: none set
   DeviceBuffer region_tmp;        // dmnerf_region_dilate: the second buffer of a multi-step dilation
+  // object appearance read with DMNERF_FLAG_APPEARANCE (dmnerf_set_appearance): appearance_labels rows of APPEARANCE_ROW floats
+  // at `appearance`, in a buffer of its own sized for DMNERF_MAX_INS + 1 rows, so that it is never reallocated; 0 labels: none set
+  DeviceBuffer appearance_buf;
+  const float* appearance = nullptr;
+  int appearance_labels = 0;
   bool profiling = false;
   bool profile_valid = false;
   cudaEvent_t ev[DMNERF_N_STAGES + 1] = {};
@@ -87,6 +92,21 @@ static int render_region(const dmnerf_ctx* ctx, int flags, const Region*& region
     DMN_CHECK(!((ctx->region.applies.w[b >> 5] >> (b & 31)) & 1u), "%s: region applies to label %d, outside [0, %d]", who, b,
               n_labels - 1);
   region = &ctx->region;
+  return 0;
+}
+
+// The appearance table of a render call: the context's (dmnerf_set_appearance) with DMNERF_FLAG_APPEARANCE, else NULL.  It must
+// have one row per label of the bound pair.
+static int render_appearance(const dmnerf_ctx* ctx, int flags, const float*& table, const char* who) {
+  table = nullptr;
+  if (!(flags & DMNERF_FLAG_APPEARANCE)) return 0;
+  DMN_CHECK(ctx && ctx->appearance_labels > 0, "%s: DMNERF_FLAG_APPEARANCE without an appearance (set one with "
+            "dmnerf_set_appearance)", who);
+  const bool pair = ctx->net[0].bound && ctx->net[1].bound && ctx->net[0].ins_num == ctx->net[1].ins_num;
+  DMN_CHECK(pair, "%s: an appearance needs the network(s) bound with dmnerf_set_weights (one ins_num)", who);
+  DMN_CHECK(ctx->appearance_labels == ctx->net[0].ins_num + 1, "%s: the appearance has %d rows for %d labels (ins_num + 1)", who,
+            ctx->appearance_labels, ctx->net[0].ins_num + 1);
+  table = ctx->appearance;
   return 0;
 }
 
@@ -399,9 +419,10 @@ DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, 
 
 }  // extern "C"
 
-// dm_nerf() on device buffers; keep: object selection, region: region selection (both NULL = none, the unselected kernels)
+// dm_nerf() on device buffers; keep: object selection, region: region selection, appearance: object appearance table (all NULL =
+// none, the unselected kernels)
 static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
-                               const ObjMask* keep, const Region* region, void* stream) {
+                               const ObjMask* keep, const Region* region, const float* appearance, void* stream) {
   DMN_CHECK(ctx && io, "render_forward: NULL ctx/io");
   DMN_CHECK(n >= 0 && S >= 3 && NI >= 2, "render_forward: bad sizes n=%lld S=%d I=%d", (long long)n, S, NI);
   DMN_CHECK(ctx->net[0].bound && ctx->net[1].bound, "render_forward: bind both networks with dmnerf_set_weights first");
@@ -421,7 +442,8 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   if (impl != DMNERF_IMPL_SIMT && S == 64 && NI == 128 && !io->raw_coarse && !io->raw_fine) {
     const bool prof = ctx->profiling;
     if (prof) DMN_CUDA(cudaEventRecord(ctx->ev[0], st));
-    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep, impl == DMNERF_IMPL_UMMA_F16, region);
+    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep, impl == DMNERF_IMPL_UMMA_F16, region,
+                                appearance);
     if (rc) return rc;
     if (prof) for (int i = 1; i <= DMNERF_N_STAGES; ++i) DMN_CUDA(cudaEventRecord(ctx->ev[i], st));
     ctx->profile_valid = prof;
@@ -453,7 +475,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:63     coarse composite
   if ((rc = launch_composite(raw_c, z_c, io->rays_d, n, S, C, keep_ins, io->rgb_coarse, w_c, io->depth_coarse,
-                             io->ins_coarse, io->acc_coarse, st, keep, io->rays_o, region))) return rc;
+                             io->ins_coarse, io->acc_coarse, st, keep, io->rays_o, region, appearance))) return rc;
   DMN_STAGE_MARK();
   // render.py:66-70  importance sampling + merge
   if ((rc = launch_hier_sample(z_c, w_c, perturb ? io->u : nullptr, n, S, NI, z_f, st))) return rc;
@@ -463,7 +485,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:86     fine composite
   if ((rc = launch_composite(raw_f, z_f, io->rays_d, n, F, C, keep_ins, io->rgb_fine, io->weights_fine, io->depth_fine,
-                             io->ins_fine, io->acc_fine, st, keep, io->rays_o, region))) return rc;
+                             io->ins_fine, io->acc_fine, st, keep, io->rays_o, region, appearance))) return rc;
   DMN_STAGE_MARK();
 #undef DMN_STAGE_MARK
   ctx->profile_valid = prof;
@@ -477,8 +499,11 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
   ObjMask m;
   const ObjMask* keep;
   const Region* region;
-  if (render_mask(ctx, io, flags, m, keep, "render_forward") || render_region(ctx, flags, region, "render_forward")) return 1;
-  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, keep, region, stream), impl, stream);
+  const float* appearance;
+  if (render_mask(ctx, io, flags, m, keep, "render_forward") || render_region(ctx, flags, region, "render_forward") ||
+      render_appearance(ctx, flags, appearance, "render_forward"))
+    return 1;
+  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, keep, region, appearance, stream), impl, stream);
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
@@ -522,7 +547,8 @@ DMNERF_API int dmnerf_profile_read(dmnerf_ctx* ctx, float* ms_out, int n_out) {
 // Host-buffer render: `h` holds HOST pointers for the outputs (and for the inputs unless dev_rays_o / dev_rays_d are given:
 // rays that are already resident on the device, e.g. generated there from the camera).
 static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const float* dev_rays_o, const float* dev_rays_d, int64_t n,
-                            int S, int NI, int flags, int impl, const ObjMask* keep, const Region* region, void* stream) {
+                            int S, int NI, int flags, int impl, const ObjMask* keep, const Region* region,
+                            const float* appearance, void* stream) {
   DMN_CHECK(ctx && h, "render_forward_host: NULL ctx/io");
   DMN_CHECK(n >= 0, "render_forward_host: negative ray count");
   if (n == 0) return 0;
@@ -612,7 +638,7 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
   const bool parts = n >= HOST_PART_MIN_RAYS && !ctx->profiling;
   if (!parts) {
     if (copy_in(0, n, st)) return 1;
-    int rc = render_forward_impl(ctx, &io, n, S, NI, flags, impl, keep, region, stream);
+    int rc = render_forward_impl(ctx, &io, n, S, NI, flags, impl, keep, region, appearance, stream);
     if (rc) return rc;
     if (copy_out(0, n, st)) return 1;
     return dmnerf_sync_check(ctx, stream);
@@ -642,7 +668,7 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
   for (int i = 0; i < HOST_PARTS && !rc; ++i) {
     if (i > 0) DMN_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[i], 0));
     const dmnerf_render_io pi = part_io(edge[i]);
-    rc = render_forward_impl(ctx, &pi, edge[i + 1] - edge[i], S, NI, flags, impl, keep, region, stream);
+    rc = render_forward_impl(ctx, &pi, edge[i + 1] - edge[i], S, NI, flags, impl, keep, region, appearance, stream);
     if (rc) break;
     DMN_CUDA(cudaEventRecord(ctx->ev_done[i], st));
     DMN_CUDA(cudaStreamWaitEvent(cs, ctx->ev_done[i], 0));
@@ -661,8 +687,11 @@ DMNERF_API int dmnerf_render_forward_host(dmnerf_ctx* ctx, const dmnerf_render_i
   ObjMask m;
   const ObjMask* keep;
   const Region* region;
-  if (render_mask(ctx, h, flags, m, keep, "render_forward_host") || render_region(ctx, flags, region, "render_forward_host")) return 1;
-  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, keep, region, stream);
+  const float* appearance;
+  if (render_mask(ctx, h, flags, m, keep, "render_forward_host") || render_region(ctx, flags, region, "render_forward_host") ||
+      render_appearance(ctx, flags, appearance, "render_forward_host"))
+    return 1;
+  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, keep, region, appearance, stream);
 }
 
 DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
@@ -672,7 +701,9 @@ DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, co
   ObjMask m;
   const ObjMask* keep;
   const Region* region;
-  if (render_mask(ctx, out_host, flags, m, keep, "render_frame_host") || render_region(ctx, flags, region, "render_frame_host"))
+  const float* appearance;
+  if (render_mask(ctx, out_host, flags, m, keep, "render_frame_host") || render_region(ctx, flags, region, "render_frame_host") ||
+      render_appearance(ctx, flags, appearance, "render_frame_host"))
     return 1;
   DMN_CHECK(H > 0 && W > 0 && n_coarse >= 3 && n_coarse <= 4096, "render_frame_host: bad sizes H=%d W=%d S=%d", H, W, n_coarse);
   DMN_CHECK(ray_begin >= 0 && ray_count >= 0 && ray_begin + ray_count <= (int64_t)H * W,
@@ -696,7 +727,8 @@ DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, co
   dmnerf_render_io h = *out_host;
   h.rays_o = nullptr; h.rays_d = nullptr; h.t_rand = nullptr; h.u = nullptr;
   h.z_coarse = z.data(); h.z_row_stride = 0;
-  return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, keep, region, stream);
+  return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, keep, region,
+                          appearance, stream);
 }
 
 // ---- mesh extraction (tools/mesh_generator.py mesh_main) ------------------------------------------------------------------
@@ -854,6 +886,33 @@ DMNERF_API int dmnerf_set_region(dmnerf_ctx* ctx, const uint32_t* bits_device, i
   r.outside_keep = outside_keep ? 1 : 0;
   for (int i = 0; i < 4; ++i) r.applies.w[i] = applies_host[i];
   ctx->region = r;
+  return 0;
+}
+
+// ---- object appearance (DESIGN.md, "Object appearance") -------------------------------------------------------------------
+
+DMNERF_API int dmnerf_set_appearance(dmnerf_ctx* ctx, const float* table_host, int n_labels, void* stream) {
+  DMN_CHECK(ctx != nullptr, "set_appearance: ctx is NULL");
+  if (!table_host) {
+    ctx->appearance = nullptr;
+    ctx->appearance_labels = 0;
+    return 0;
+  }
+  DMN_CHECK(n_labels >= 2 && n_labels <= DMNERF_MAX_INS + 1, "set_appearance: %d labels outside [2, %d]", n_labels,
+            DMNERF_MAX_INS + 1);
+  for (int l = 0; l < n_labels; ++l) {
+    const float* row = table_host + (size_t)l * APPEARANCE_ROW;
+    for (int i = 0; i < APPEARANCE_ROW; ++i)
+      DMN_CHECK(std::isfinite(row[i]), "set_appearance: entry %d of label %d is not finite", i, l);
+    DMN_CHECK(row[12] >= 0.0f, "set_appearance: label %d has a negative density scale %g", l, (double)row[12]);
+  }
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  float* d;
+  if (ctx->appearance_buf.get((size_t)(DMNERF_MAX_INS + 1) * APPEARANCE_ROW, &d)) return 2;
+  DMN_CUDA(cudaMemcpyAsync(d, table_host, (size_t)n_labels * APPEARANCE_ROW * sizeof(float), cudaMemcpyHostToDevice,
+                           (cudaStream_t)stream));
+  ctx->appearance = d;
+  ctx->appearance_labels = n_labels;
   return 0;
 }
 

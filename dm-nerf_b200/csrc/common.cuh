@@ -169,13 +169,20 @@ struct Region {
 };
 inline int64_t region_words(int dim) { return ((int64_t)dim * dim * dim + 31) / 32; }
 
+// Object appearance (DESIGN.md, "Object appearance"): one row per label 0 .. ins_num of APPEARANCE_ROW floats, the colour map
+// [M | b] (row-major 3x4), the density scale and 3 floats of padding (a row is 4 aligned float4).  The per-sample step is
+// appearance_apply (ray_ops.cuh).
+constexpr int APPEARANCE_ROW = 16;
+
 // ---- launchers implemented in the individual .cu files (all return 0 / non-zero status) ----
 int launch_posenc(const float* x, int64_t m, int n_freqs, float* out, cudaStream_t st);
 // keep: object selection, or NULL for none (the unselected kernel); region (with rays_o): region selection, or NULL for none.
-// A region without keep runs the selected kernel with every label kept.
+// A region without keep runs the selected kernel with every label kept.  appearance: the table of object appearance (device,
+// c - 4 rows), or NULL for none; without keep or a region it too runs the selected kernel with every label kept.
 int launch_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all,
                      float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st,
-                     const ObjMask* keep = nullptr, const float* rays_o = nullptr, const Region* region = nullptr);
+                     const ObjMask* keep = nullptr, const float* rays_o = nullptr, const Region* region = nullptr,
+                     const float* appearance = nullptr);
 int launch_sample_pdf(const float* bins, const float* weights, int64_t n, int nb, int ns, const float* u, float* out,
                       cudaStream_t st);
 int launch_sort_concat(const float* a, const float* b, int64_t n, int na, int nb, float* out, cudaStream_t st);

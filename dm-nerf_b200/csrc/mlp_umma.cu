@@ -72,6 +72,7 @@ struct KArgs {
   int32_t* status;             // device error word
   ObjMask keep;                // render_objects_kernel: kept object labels
   Region region;               // render_objects_kernel: region selection (region.bits == NULL: none)
+  const float* appearance;     // render_objects_kernel: object appearance table (ins_num + 1 rows), or NULL for none
 };
 
 // ------------------------------------------------------------------------------------------------ prologue helpers
@@ -148,9 +149,10 @@ struct Program {
 
 // Warps 0-7: two consumer warpgroups (MMA issue, epilogues, prologue); warp 8: weight producer.
 // SELECT (fused only): object selection -- samples whose label is not in a.keep get alpha = 0 in both composites, and so do the
-// samples a.region drops (region selection, when a.region.bits is set).  The body is
-// shared by mlp_umma_kernel (no selection) and render_objects_kernel (FUSED + SELECT) below.  F16: the fp16 preview network
-// (prog and the images are then the fp16 program and images).
+// samples a.region drops (region selection, when a.region.bits is set); with a.appearance set, every other sample's density and
+// colour go through its label's appearance row (appearance_apply).  The body is shared by mlp_umma_kernel (no selection) and
+// render_objects_kernel (FUSED + SELECT) below.  F16: the fp16 preview network (prog and the images are then the fp16 program
+// and images).
 template <bool FUSED, bool SELECT, bool F16>
 __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& a) {
   // The kernel has no static shared memory, so the dynamic block starts at offset 0 of the CTA's shared window and
@@ -585,10 +587,11 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
         float dist = (si == S - 1) ? 1e10f : __fsub_rn(zs[si + 1], zi);
         dist = __fmul_rn(dist, fz->ray[rl][6]);
         float alpha = __fsub_rn(1.0f, expf(-__fmul_rn(fmaxf(rv.w, 0.0f), dist)));
+        int label = 0;
         if constexpr (SELECT) {
           // the row's label from its logits (128 floats apart per row, i.e. one bank): each lane starts its walk at channel
           // lane mod n, so the 32 rows of a warp read ceil(32 / n) rows per bank below 32 channels and at most 2 above
-          const int label = argmax_sigmoid(logit + r * 128, n_ins1, (r & 31) % n_ins1);
+          label = argmax_sigmoid(logit + r * 128, n_ins1, (r & 31) % n_ins1);
           bool drop = !obj_kept(a.keep, label);
           if (a.region.bits && !drop) {
             // region selection: the sample's point as the prologue computed it, from the ray and the depth zi
@@ -596,7 +599,13 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
             ray_point(fz->ray[rl], fz->ray[rl] + 3, zi, p);
             drop = region_drops(a.region, label, p[0], p[1], p[2]);
           }
-          if (drop) alpha = 0.0f;
+          if (drop) {
+            alpha = 0.0f;
+          } else if (a.appearance) {
+            float sg = fmaxf(rv.w, 0.0f), c[3] = {0.0f, 0.0f, 0.0f};
+            appearance_apply(a.appearance, label, sg, c);
+            alpha = __fsub_rn(1.0f, expf(-__fmul_rn(sg, dist)));
+          }
         }
         const float f = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
         const int lane_i = r & 31, wi = r >> 5;
@@ -622,7 +631,14 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
         if (j == 0 && a.wc_out && valid) a.wc_out[(item * 2 + rl) * FS + si] = wgt;
         if (j != 0 && a.wf_out && valid) a.wf_out[(item * 2 + rl) * FF + si] = wgt;
         // ---- weighted sums (render.py:19-20 + acc): warp reduce per 32-sample chunk
-        float p0 = __fmul_rn(wgt, sigmoidf_acc(rv.x)), p1 = __fmul_rn(wgt, sigmoidf_acc(rv.y)), p2 = __fmul_rn(wgt, sigmoidf_acc(rv.z));
+        float p0, p1, p2;
+        if constexpr (SELECT) {
+          float c[3] = {sigmoidf_acc(rv.x), sigmoidf_acc(rv.y), sigmoidf_acc(rv.z)}, sg = 0.0f;
+          if (a.appearance) appearance_apply(a.appearance, label, sg, c);
+          p0 = __fmul_rn(wgt, c[0]); p1 = __fmul_rn(wgt, c[1]); p2 = __fmul_rn(wgt, c[2]);
+        } else {
+          p0 = __fmul_rn(wgt, sigmoidf_acc(rv.x)); p1 = __fmul_rn(wgt, sigmoidf_acc(rv.y)); p2 = __fmul_rn(wgt, sigmoidf_acc(rv.z));
+        }
         float p3 = __fmul_rn(wgt, zi), p4 = wgt;
         p0 = warp_sum(p0); p1 = warp_sum(p1); p2 = warp_sum(p2); p3 = warp_sum(p3); p4 = warp_sum(p4);
         float* ac = fz->accum[rl][si >> 5];
@@ -1005,7 +1021,7 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
 // Whole dm_nerf() pipeline (render.py:31-96) in ONE launch: coarse network -> composite -> importance sampling -> fine
 // network -> composite, per pair of rays, nothing but rays in and per-ray maps out crossing HBM.  64 + 128 samples only.
 int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmnerf_render_io* io, int64_t n, int flags,
-                       cudaStream_t st, const ObjMask* keep, bool f16, const Region* region) {
+                       cudaStream_t st, const ObjMask* keep, bool f16, const Region* region, const float* appearance) {
   using namespace uk;
   DMN_CHECK(wc.ready && wf.ready && wc.extra && wf.extra, "render(umma): weights not packed");
   DMN_CHECK(wc.ins_num == wf.ins_num, "render(umma): coarse/fine ins_num differ");
@@ -1028,9 +1044,10 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   a.zc_out = io->z_vals_coarse; a.zf_out = io->z_vals_fine; a.wc_out = io->weights_coarse; a.wf_out = io->weights_fine;
   a.status = ex->d_status;
   if (keep) a.keep = *keep;
-  if (region) {                                            // a region alone runs the selected kernel with every label kept
-    if (!keep) a.keep = ObjMask{{~0u, ~0u, ~0u, ~0u}};
-    a.region = *region;
+  if (region) a.region = *region;
+  a.appearance = appearance;
+  if (!keep && (region || appearance)) {                  // a region or an appearance alone: the selected kernel, every label kept
+    a.keep = ObjMask{{~0u, ~0u, ~0u, ~0u}};
     keep = &a.keep;
   }
   const int64_t units = (n + 1) / 2;                       // pairs of rays

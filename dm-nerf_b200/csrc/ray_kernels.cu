@@ -43,13 +43,15 @@ int launch_posenc(const float* x, int64_t m, int n_freqs, float* out, cudaStream
 // channel walks the samples in order (coalesced across channels), mirroring torch.sum(..., -2).
 // SELECT: object selection -- a sample whose argmax_sigmoid label is not kept enters with density 0 (alpha = 0); raw is read,
 // never edited.  With region.bits set (SELECT only) a sample the region drops (region_drops at o + d z) enters with alpha = 0
-// too: the same test as the fused render kernels.
+// too: the same test as the fused render kernels.  With an appearance table (SELECT only) a kept sample's density is scaled and
+// its colour mapped by appearance_apply; the rgb lanes take the sample's label again from its logits.
 template <bool SELECT>
 __global__ void composite_kernel(const float* __restrict__ raw, const float* __restrict__ z,
                                  const float* __restrict__ rays_d, int64_t n, int S, int C, int keep_all,
                                  float* __restrict__ rgb, float* __restrict__ weights, float* __restrict__ depth,
                                  float* __restrict__ ins, float* __restrict__ acc, const ObjMask keep,
-                                 const float* __restrict__ rays_o, const __grid_constant__ Region region) {
+                                 const float* __restrict__ rays_o, const __grid_constant__ Region region,
+                                 const float* __restrict__ appearance) {
   extern __shared__ float smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t ray = (int64_t)blockIdx.x * WARPS_PER_BLOCK + warp;
@@ -70,6 +72,11 @@ __global__ void composite_kernel(const float* __restrict__ raw, const float* __r
         ray_point(o, d, zr[i], p);
         if (region_drops(region, label, p[0], p[1], p[2])) return 0.0f;
       }
+      if (appearance) {
+        float sg = fmaxf(ri[3], 0.0f), c[3] = {0.0f, 0.0f, 0.0f};
+        appearance_apply(appearance, label, sg, c);
+        return sg;                                 // >= 0: ray_weights' max(sigma, 0) leaves it as it is
+      }
     }
     return ri[3];
   }, [&](int i) { return zr[i]; }, w, lane);
@@ -80,7 +87,18 @@ __global__ void composite_kernel(const float* __restrict__ raw, const float* __r
   for (int k = lane; k < C; k += 32) {
     if (k < 3) {
       float a = 0.0f;
-      for (int i = 0; i < S; ++i) a = __fadd_rn(a, __fmul_rn(w[i], sigmoidf_acc(rr[(size_t)i * C + k])));
+      for (int i = 0; i < S; ++i) {
+        float c = sigmoidf_acc(rr[(size_t)i * C + k]);
+        if constexpr (SELECT) {
+          if (appearance) {
+            const float* ri = rr + (size_t)i * C;
+            float sg = 0.0f, col[3] = {sigmoidf_acc(ri[0]), sigmoidf_acc(ri[1]), sigmoidf_acc(ri[2])};
+            appearance_apply(appearance, argmax_sigmoid(ri + 4, C - 4), sg, col);
+            c = k == 0 ? col[0] : (k == 1 ? col[1] : col[2]);
+          }
+        }
+        a = __fadd_rn(a, __fmul_rn(w[i], c));
+      }
       if (rgb) rgb[ray * 3 + k] = a;
     } else if (k == 3) {
       float d = 0.0f, s = 0.0f;
@@ -100,21 +118,21 @@ __global__ void composite_kernel(const float* __restrict__ raw, const float* __r
 
 int launch_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all,
                      float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st, const ObjMask* keep,
-                     const float* rays_o, const Region* region) {
+                     const float* rays_o, const Region* region, const float* appearance) {
   DMN_CHECK(s >= 1 && s <= 4096, "composite: n_samples=%d out of range [1,4096]", s);
   DMN_CHECK(c >= 5 && c <= 4 + DMNERF_MAX_INS + 1, "composite: channels=%d out of range", c);
   DMN_CHECK(!region || (region->bits && rays_o), "composite: a region needs its bits and the ray origins");
   if (n == 0) return 0;
   const size_t smem = (size_t)WARPS_PER_BLOCK * s * sizeof(float);
-  const bool select = keep || region;
+  const bool select = keep || region || appearance;
   auto kernel = select ? composite_kernel<true> : composite_kernel<false>;
   if (smem > 48 * 1024)
     DMN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const ObjMask none = {{0u, 0u, 0u, 0u}}, all = {{~0u, ~0u, ~0u, ~0u}};
   const Region no_region{};
   kernel<<<(unsigned)((n + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK), WARPS_PER_BLOCK * 32, smem, st>>>(
-      raw, z, rays_d, n, s, c, keep_all, rgb, weights, depth, ins, acc, keep ? *keep : (region ? all : none), rays_o,
-      region ? *region : no_region);
+      raw, z, rays_d, n, s, c, keep_all, rgb, weights, depth, ins, acc, keep ? *keep : (select ? all : none), rays_o,
+      region ? *region : no_region, appearance);
   DMN_LAUNCH_OK();
   return 0;
 }

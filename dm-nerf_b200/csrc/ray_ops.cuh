@@ -53,6 +53,23 @@ __device__ __forceinline__ bool region_drops(const Region& r, int label, float p
   return b == 0 || (b < 0 && !r.outside_keep);
 }
 
+// Object appearance (DESIGN.md, "Object appearance").  Row `label` of the table (APPEARANCE_ROW floats: the colour map [M | b],
+// row-major 3x4, then the density scale s) applied to a kept sample: sg (its max(sigma, 0)) becomes s sg, and each channel of
+// its sigmoid colour c becomes min(max(((M_a0 c0 + M_a1 c1) + M_a2 c2) + b_a, 0), 1), every operation rounded once.  The fused
+// render kernels and the stage composite call this one function; a caller that needs only one of the two results discards the
+// other, and the compiler drops that half.
+__device__ __forceinline__ void appearance_apply(const float* __restrict__ table, int label, float& sg, float c[3]) {
+  const float4* row = reinterpret_cast<const float4*>(table + APPEARANCE_ROW * label);
+  sg = __fmul_rn(__ldg(row + 3).x, sg);
+  const float4 m[3] = {__ldg(row), __ldg(row + 1), __ldg(row + 2)};
+  const float c0 = c[0], c1 = c[1], c2 = c[2];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const float u = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[a].x, c0), __fmul_rn(m[a].y, c1)), __fmul_rn(m[a].z, c2)), m[a].w);
+    c[a] = fminf(fmaxf(u, 0.0f), 1.0f);
+  }
+}
+
 // The sample point of depth z on the ray (o, d), as the network prologue computes it.
 __device__ __forceinline__ void ray_point(const float* o, const float* d, float z, float p[3]) {
 #pragma unroll

@@ -39,6 +39,7 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
 int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmnerf_render_io* io, int64_t n, int flags,
                        cudaStream_t st, const ObjMask* keep = nullptr,     // keep: object selection, or NULL
                        bool f16 = false,
-                       const Region* region = nullptr);                    // region selection, or NULL
+                       const Region* region = nullptr,                     // region selection, or NULL
+                       const float* appearance = nullptr);                 // object appearance table (device), or NULL
 
 }  // namespace dmnerf

@@ -12,6 +12,8 @@
     component_region(cc, ids, scene_transform, ...) / region_from_mask(mask, scene_transform, ...)
                                                         -> a Region: grid bits the renderer reads per sample (render_*(region=))
     region_contains(region, pts)                        -> which points a region keeps, by the render kernels' own test
+    Appearance(ins_num, colour=None, density=None), tint(rgb)
+                                                        -> per-object colour maps and density scales (render_*(appearance=))
     scene_box(model_fine, poses, hwk, near, far, ...)   -> (scene_transform, extents) of the scene, from the cameras
     manipulation_transform(centre, mode)                -> the transformation dict manipulator_eval takes, about that centre
 
@@ -71,7 +73,7 @@ def _to8b(x):
 
 
 def render_objects(position_embedder, view_embedder, model_coarse, model_fine, poses, hwk, args, keep=None, remove=None,
-                   savedir=None, ins_rgbs=None, color_dict=None, impl=_lib.IMPL_AUTO, region=None):
+                   savedir=None, ins_rgbs=None, color_dict=None, impl=_lib.IMPL_AUTO, region=None, appearance=None):
     """Render every pose (camera-to-world, [4, 4] or [3, 4]) with the selection, deterministically, through the frame driver.
     Reads args.near, args.far, args.N_samples, args.N_importance.  Returns one dict per pose of device maps: rgb [H, W, 3],
     ins [H, W, ins_num], depth [H, W], acc [H, W].
@@ -80,7 +82,9 @@ def render_objects(position_embedder, view_embedder, model_coarse, model_fine, p
     ins_rgbs / color_dict, label k gets colour k of a fixed seeded palette.  impl: the network, as in render_frame.
     region: a Region (region selection, DESIGN.md "Region selection") applied with the label selection; with a region, keep and
     remove may both be left out (every label kept).  Floater cleanup, for example, is the component_region of each object
-    label's largest piece (see component_region)."""
+    label's largest piece (see component_region).
+    appearance: an Appearance (object appearance, DESIGN.md "Object appearance") applied to the samples the selection and the
+    region keep; with one, keep and remove may both be left out as well."""
     from .render import _check_embedders, render_frame
     from .tester import colorize, pred_label_lut, write_png
     _check_embedders(position_embedder, view_embedder)
@@ -88,7 +92,7 @@ def render_objects(position_embedder, view_embedder, model_coarse, model_fine, p
     H, W = int(H), int(W)
     dev = next(model_fine.parameters()).device
     ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
-    if region is not None and keep is None and remove is None:
+    if (region is not None or appearance is not None) and keep is None and remove is None:
         kept = None
     else:
         kept = kept_labels(object_mask(ins_num, keep=keep, remove=remove))
@@ -106,7 +110,8 @@ def render_objects(position_embedder, view_embedder, model_coarse, model_fine, p
         for i, c2w in enumerate(poses):
             c2w = torch.as_tensor(np.asarray(c2w.cpu() if torch.is_tensor(c2w) else c2w), dtype=torch.float32)
             m = render_frame(H, W, K, c2w, args.near, args.far, model_coarse, model_fine, N_samples=args.N_samples,
-                             N_importance=args.N_importance, device=dev, keep_objects=kept, impl=impl, region=region)
+                             N_importance=args.N_importance, device=dev, keep_objects=kept, impl=impl, region=region,
+                             appearance=appearance)
             m = {k: v.to(dev) for k, v in m.items()}
             out.append(m)
             if savedir is not None:
@@ -615,6 +620,67 @@ def set_region(ctx, region, ins_num):
     _lib.check(lib.dmnerf_set_region(ctx.handle, _lib.ptr(region.bits, torch.int32), region.dim, _lib.floats(region.voxel_map, 12),
                                      _lib.keep_mask(region.applies_words(ins_num)), int(region.outside == "keep")),
                "dmnerf_set_region")
+
+
+# ----------------------------------------------------------------------------------------------------------------- appearance
+# DESIGN.md, "Object appearance": per label a colour map and a density scale, applied per sample by the render kernels to every
+# sample the selection and the region keep.
+APPEARANCE_ROW = 16                  # floats per label: [M | b] row-major 3x4, the density scale, 3 of padding
+LUMA = (0.299, 0.587, 0.114)
+
+
+def tint(rgb):
+    """The colour map (3x4, float64) that keeps a sample's shading and replaces its hue with rgb: c'_a = rgb_a (0.299 c0 +
+    0.587 c1 + 0.114 c2), no offset.  tint((1, 1, 1)) is greyscale."""
+    rgb = np.asarray(rgb, dtype=np.float64).reshape(-1)
+    if rgb.shape != (3,) or not np.isfinite(rgb).all():
+        raise ValueError("tint: rgb must be 3 finite numbers, got %r" % (rgb.tolist(),))
+    return np.concatenate([np.outer(rgb, LUMA), np.zeros((3, 1))], 1)
+
+
+class Appearance:
+    """An object appearance for networks with ins_num: per label, the colour map [M | b] applied to a sample's sigmoid colour c
+    (c' = clamp(M c + b, 0, 1)) and the scale s >= 0 of its density (alpha = 1 - exp(-s relu(sigma) dist)).
+    colour: {label: 3x4 matrix [M | b], or 3x3 M (b = 0)}; density: {label: s}.  A label without an entry keeps its look
+    (M = I, b = 0, s = 1).  `table` is the float32 [ins_num + 1, 16] table dmnerf_set_appearance takes."""
+
+    def __init__(self, ins_num, colour=None, density=None):
+        ins_num = int(ins_num)
+        if not 1 <= ins_num <= MAX_LABELS - 1:
+            raise ValueError("Appearance: ins_num %d outside [1, %d]" % (ins_num, MAX_LABELS - 1))
+        table = np.zeros((ins_num + 1, APPEARANCE_ROW), dtype=np.float32)
+        table[:, :12] = np.eye(3, 4, dtype=np.float32).reshape(12)
+        table[:, 12] = 1.0
+        for label, m in dict(colour or {}).items():
+            k = _labels([label], ins_num, "Appearance")[0]
+            m = np.asarray(m, dtype=np.float64)
+            if m.shape == (3, 3):
+                m = np.concatenate([m, np.zeros((3, 1))], 1)
+            if m.shape != (3, 4):
+                raise ValueError("Appearance: the colour map of label %d must be 3x4 or 3x3, got shape %s" % (k, m.shape))
+            with np.errstate(over="ignore", invalid="ignore"):
+                m = m.astype(np.float32)
+            if not np.isfinite(m).all():
+                raise ValueError("Appearance: the colour map of label %d is not finite in float32" % k)
+            table[k, :12] = m.reshape(12)
+        for label, s in dict(density or {}).items():
+            k = _labels([label], ins_num, "Appearance")[0]
+            with np.errstate(over="ignore", invalid="ignore"):
+                s = np.float32(s)
+            if not (np.isfinite(s) and s >= 0):
+                raise ValueError("Appearance: the density scale of label %d must be finite and >= 0, got %r" % (k, float(s)))
+            table[k, 12] = s
+        self.ins_num, self.table = ins_num, table
+
+
+def set_appearance(ctx, appearance, ins_num):
+    """Make `appearance` the context's appearance (dmnerf_set_appearance) for networks with ins_num; None clears it."""
+    if appearance is None:
+        ctx.call("dmnerf_set_appearance", ctx.handle, None, 0)
+        return
+    if appearance.ins_num != ins_num:
+        raise ValueError("appearance: built for ins_num %d, the networks have ins_num %d" % (appearance.ins_num, ins_num))
+    ctx.call("dmnerf_set_appearance", ctx.handle, _lib.floats(appearance.table, appearance.table.size), ins_num + 1)
 
 
 def camera_region(poses, hwk, far):

@@ -79,12 +79,18 @@ def selection(who, keep_objects, ins_num, model_coarse, model_fine):
     selection."""
     if keep_objects is None:
         return None
-    from .autograd import _needs_grad
     from .objects import object_mask
-    if _needs_grad(model_coarse, model_fine):
-        raise RuntimeError("%s: object selection is inference-only; call it under torch.no_grad() or with parameters that "
-                           "do not require grad" % who)
+    inference_only(who, "object selection", model_coarse, model_fine)
     return object_mask(ins_num, keep=keep_objects)
+
+
+def inference_only(who, what, model_coarse, model_fine):
+    """RuntimeError when the networks would record gradients: the scene edits (object selection, region, appearance) render
+    inference only."""
+    from .autograd import _needs_grad
+    if _needs_grad(model_coarse, model_fine):
+        raise RuntimeError("%s: %s is inference-only; call it under torch.no_grad() or with parameters that do not require "
+                           "grad" % (who, what))
 
 
 @contextlib.contextmanager
@@ -94,16 +100,29 @@ def region_scope(ctx, who, region, ins_num, model_coarse, model_fine):
     if region is None:
         yield 0
         return
-    from .autograd import _needs_grad
     from .objects import set_region
-    if _needs_grad(model_coarse, model_fine):
-        raise RuntimeError("%s: region selection is inference-only; call it under torch.no_grad() or with parameters that "
-                           "do not require grad" % who)
+    inference_only(who, "region selection", model_coarse, model_fine)
     set_region(ctx, region, ins_num)
     try:
         yield _lib.FLAG_REGION
     finally:
         set_region(ctx, None, ins_num)
+
+
+@contextlib.contextmanager
+def appearance_scope(ctx, who, appearance, ins_num, model_coarse, model_fine):
+    """`appearance` (objects.Appearance, or None) as the context's appearance for the calls inside the block; yields the flag
+    those calls add (DMNERF_FLAG_APPEARANCE, or 0 without one).  Inference only, as object selection."""
+    if appearance is None:
+        yield 0
+        return
+    from .objects import set_appearance
+    inference_only(who, "object appearance", model_coarse, model_fine)
+    set_appearance(ctx, appearance, ins_num)
+    try:
+        yield _lib.FLAG_APPEARANCE
+    finally:
+        set_appearance(ctx, None, ins_num)
 
 
 def _check_embedders(position_embedder, view_embedder):
@@ -116,7 +135,7 @@ def _check_embedders(position_embedder, view_embedder):
 
 def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb=0.0, N_importance=128,
                 t_rand=None, u=None, want_raw=True, want_coarse=True, want_samples=None, keep_all_ins=False,
-                impl=_lib.IMPL_AUTO, keep_objects=None, region=None):
+                impl=_lib.IMPL_AUTO, keep_objects=None, region=None, appearance=None):
     """Whole per-ray pipeline on the device.  Returns the reference's dict keys plus acc / weights maps.
     want_raw: per-sample network outputs raw_* (forces the stage-by-stage kernels); want_samples: per-sample depths and
     weights (z_vals_*, weights_*; default = want_raw); want_coarse: the coarse pass' maps.  With want_raw=False and
@@ -124,6 +143,8 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     keep_objects: an iterable of object labels in [0, ins_num]; samples labelled otherwise get alpha = 0 in both passes
     (DESIGN.md, "Object selection").  raw_* stay the network's output.  Inference only.
     region: an objects.Region; samples it drops get alpha = 0 in both passes as well (DESIGN.md, "Region selection").
+    appearance: an objects.Appearance; every sample the selection and the region keep has its label's density scale and colour
+    map applied in both passes (DESIGN.md, "Object appearance").  Inference only.
     impl: _lib.IMPL_UMMA_F16 runs the fp16 preview network (DESIGN.md section 10); IMPL_AUTO follows DMNERF_INFER_IMPL."""
     impl = _lib.infer_impl(impl)
     if want_samples is None:
@@ -165,8 +186,9 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     if keep is not None:
         flags |= _lib.FLAG_SELECT
         io.keep[:] = keep
-    with region_scope(ctx, "render_rays", region, ins_num, model_coarse, model_fine) as region_flag:
-        ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags | region_flag, impl)
+    with region_scope(ctx, "render_rays", region, ins_num, model_coarse, model_fine) as region_flag, \
+            appearance_scope(ctx, "render_rays", appearance, ins_num, model_coarse, model_fine) as appearance_flag:
+        ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags | region_flag | appearance_flag, impl)
     return out
 
 
@@ -254,13 +276,13 @@ raw2outputs = render_train
 
 
 def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64, N_importance=128, pixel_range=None,
-                 keep_all_ins=False, impl=_lib.IMPL_AUTO, device="cuda", keep_objects=None, region=None):
+                 keep_all_ins=False, impl=_lib.IMPL_AUTO, device="cuda", keep_objects=None, region=None, appearance=None):
     """One camera of the reference's test-time loop (render_test, networks/tester.py:55-76) through the frame entry point of
     the C ABI: rays are generated on the device from K / c2w (get_rays_k), the coarse depth row from near / far
     (z_val_sample), the pixels are rendered by the fused kernel and the maps come back as HOST tensors:
     rgb [H,W,3], ins [H,W,ins_num], depth [H,W], acc [H,W] (or [n, ...] rows when a pixel_range = (begin, count) is given --
-    the per-rank slice of a sharded frame).  keep_objects and region: object and region selection as in render_rays; impl as in
-    render_rays."""
+    the per-rank slice of a sharded frame).  keep_objects, region and appearance: object selection, region selection and object
+    appearance as in render_rays; impl as in render_rays."""
     impl = _lib.infer_impl(impl)
     dev = torch.device(device)
     ctx = get_context(dev)
@@ -278,9 +300,10 @@ def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64
         flags |= _lib.FLAG_SELECT
         io.keep[:] = keep
     Kf, Cf = _lib.camera(K, c2w)
-    with region_scope(ctx, "render_frame", region, ins_num, model_coarse, model_fine) as region_flag:
+    with region_scope(ctx, "render_frame", region, ins_num, model_coarse, model_fine) as region_flag, \
+            appearance_scope(ctx, "render_frame", appearance, ins_num, model_coarse, model_fine) as appearance_flag:
         ctx.call("dmnerf_render_frame_host", ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples,
-                 N_importance, flags | region_flag, impl, C.byref(io))
+                 N_importance, flags | region_flag | appearance_flag, impl, C.byref(io))
     if pixel_range is None:
         out = {"rgb": out["rgb"].reshape(H, W, 3), "ins": out["ins"].reshape(H, W, n_ins), "depth": out["depth"].reshape(H, W),
                "acc": out["acc"].reshape(H, W)}

@@ -57,6 +57,7 @@ extern "C" {
 #define DMNERF_FLAG_KEEP_INS  4     /* keep all ins_num+1 instance channels, no detach: manipulator.py:86-105 */
 #define DMNERF_FLAG_SELECT    8     /* object selection: the keep field is read (see "object selection" below) */
 #define DMNERF_FLAG_REGION   16     /* region selection: the context's region is read (see "region selection" below) */
+#define DMNERF_FLAG_APPEARANCE 32   /* object appearance: the context's appearance is read (see "object appearance" below) */
 
 typedef struct dmnerf_ctx dmnerf_ctx;
 
@@ -467,6 +468,20 @@ DMNERF_API int dmnerf_region_dilate(dmnerf_ctx* ctx, const uint32_t* in, int dim
                                     uint32_t* out, void* stream);
 DMNERF_API int dmnerf_region_contains(const uint32_t* bits, int dim, const float* voxel_map12, const float* pts, int64_t n,
                                       uint8_t* out, void* stream);
+
+/* ---- object appearance (DESIGN.md, "Object appearance"; no counterpart in the original) -----------------------------------
+ * An appearance is one row of 16 floats per label l in [0, ins_num]: the colour map [M_l | b_l] (row-major 3x4), the density
+ * scale s_l (finite, >= 0) and 3 floats of padding (finite, ignored).  The identity row is [I | 0], s = 1.  A render sample with
+ * label l (argmax_sigmoid, as object selection) that the selection and the region keep gets alpha = 1 - expf(-(s_l max(sigma,
+ * 0)) dist) and the colour c'_a = min(max(((M_a0 c0 + M_a1 c1) + M_a2 c2) + b_a, 0), 1) of its sigmoid colour c, every
+ * operation rounded once in fp32; a dropped sample keeps alpha = 0.  Depth, acc and the instance maps use the edited weights,
+ * raw_* stay the network's output, and the coarse weights of the edited scene drive the importance sampling.
+ * dmnerf_set_appearance: the table DMNERF_FLAG_APPEARANCE reads in dmnerf_render_forward(_host) and dmnerf_render_frame_host
+ *   (fused kernels or stage kernels, chosen as without it; with or without DMNERF_FLAG_SELECT and DMNERF_FLAG_REGION).
+ *   table_host (HOST, n_labels x 16 floats) is copied on `stream` into the context, so it may be freed on return; NULL clears
+ *   the appearance.  Fails for n_labels outside [2, DMNERF_MAX_INS + 1], an entry that is not finite or a negative scale.  A
+ *   render with the flag fails when no appearance is set or n_labels is not the bound networks' ins_num + 1. */
+DMNERF_API int dmnerf_set_appearance(dmnerf_ctx* ctx, const float* table_host, int n_labels, void* stream);
 
 /* ---- test-view evaluation: render_test, networks/tester.py (+ ins_eval / calculate_ap, networks/evaluator.py:77-175) -------
  * Rules and deviations: DESIGN.md, "Evaluation metrics".  Every result is deterministic (fixed-order reductions, integer atomics

@@ -5,6 +5,7 @@
            [--near 4 --far 15 --N-samples 64 --N-importance 128]
            [(--no-floaters | --keep-piece ID [ID ...] | --drop-piece ID [ID ...]) --transform T [--extents X Y Z]
             [--grid-dim 256] [--level 0.45] [--connectivity {6,26}] [--dilate 1]]
+           [--tint L R G B ...] [--opacity L S ...]
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict` (the original's checkpoints).  POSE.npy holds one
 camera-to-world pose [4, 4] (or [3, 4]) or several [N, 4, 4].  K is the 3x3 intrinsics, as a .npy file or as 9 numbers.  Writes
@@ -16,7 +17,11 @@ fine network over the grid of --transform / --extents / --grid-dim (every label 
 --level into --connectivity-connected components.  --no-floaters keeps each object's largest piece, --keep-piece keeps only the
 given pieces of their objects, --drop-piece removes the given pieces and leaves the rest of their objects; a kept piece is grown
 by --dilate voxels.  Piece IDs are the `component` ids of tools/find_objects.py --components split with the same sweep arguments.
-A region combines with --keep / --remove, or stands alone (every label kept)."""
+A region combines with --keep / --remove, or stands alone (every label kept).
+
+Object appearance (DESIGN.md, "Object appearance") changes how objects look: --tint L R G B gives label L the hue (R, G, B) and
+keeps its shading (objects.tint; 1 1 1 is grey), --opacity L S scales label L's density by S >= 0 (0 removes it, below 1 fades
+it, above 1 makes it more solid).  Both repeat, and combine with every flag above or stand alone."""
 import argparse
 import json
 import os
@@ -53,10 +58,21 @@ def parse(argv=None):
     ap.add_argument("--level", type=float, default=0.45)
     ap.add_argument("--connectivity", type=int, choices=(6, 26), default=26)
     ap.add_argument("--dilate", type=int, default=1, help="voxels a kept piece is grown by")
+    ap.add_argument("--tint", type=float, nargs=4, action="append", default=[], metavar=("L", "R", "G", "B"),
+                    help="give object label L the hue (R, G, B), keeping its shading (repeatable)")
+    ap.add_argument("--opacity", type=float, nargs=2, action="append", default=[], metavar=("L", "S"),
+                    help="scale object label L's density by S >= 0 (repeatable)")
     a = ap.parse_args(argv)
     a.region = "no_floaters" if a.no_floaters else ("keep" if a.keep_piece else ("drop" if a.drop_piece else None))
-    if a.keep is None and a.remove is None and a.region is None:
-        ap.error("one of --keep, --remove, --no-floaters, --keep-piece or --drop-piece is required")
+    if a.keep is None and a.remove is None and a.region is None and not a.tint and not a.opacity:
+        ap.error("one of --keep, --remove, --no-floaters, --keep-piece, --drop-piece, --tint or --opacity is required")
+    for flag, entries in (("--tint", a.tint), ("--opacity", a.opacity)):
+        if any(e[0] != int(e[0]) for e in entries):
+            ap.error("%s takes an integer label first" % flag)
+    if any(not s >= 0 for _, s in a.opacity):
+        ap.error("--opacity S must be >= 0")
+    a.tint = {int(e[0]): tuple(e[1:]) for e in a.tint}
+    a.opacity = {int(e[0]): e[1] for e in a.opacity}
     if a.region is not None and a.transform is None:
         ap.error("a piece selection needs --transform (the sweep grid)")
     if a.dilate < 0:
@@ -94,7 +110,7 @@ def main(argv=None):
     a = parse(argv)
     import torch
     from dmnerf_b200.embedder import get_embedder
-    from dmnerf_b200.objects import render_objects
+    from dmnerf_b200.objects import Appearance, render_objects, tint
     from dmnerf_b200.testing import model_from_weights
     ck = torch.load(a.checkpoint, map_location="cpu")
     nets = [model_from_weights({k: v.float().numpy() for k, v in ck[key].items()}, a.device)
@@ -106,8 +122,12 @@ def main(argv=None):
     ve, _ = get_embedder(4)
     args = types.SimpleNamespace(near=a.near, far=a.far, N_samples=a.N_samples, N_importance=a.N_importance)
     region = piece_region(a, nets[1]) if a.region is not None else None
+    appearance = None
+    if a.tint or a.opacity:
+        ins_num = int(nets[1].ins_linear.weight.shape[0]) - 1
+        appearance = Appearance(ins_num, colour={k: tint(rgb) for k, rgb in a.tint.items()}, density=a.opacity)
     maps = render_objects(pe, ve, nets[0], nets[1], poses, (a.H, a.W, a.K), args, keep=a.keep, remove=a.remove, savedir=a.out,
-                          region=region)
+                          region=region, appearance=appearance)
     print(json.dumps({"frames": len(maps), "mean_acc": [float(m["acc"].mean()) for m in maps],
                       "files": sorted(os.listdir(a.out))}))
 
