@@ -16,13 +16,25 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DMNERF_LIB_PATH: diagnostics builds of the same ABI (tools/kprof.py); the default is the in-tree product library
 LIB_PATH = os.environ.get("DMNERF_LIB_PATH") or os.path.join(_HERE, "lib", "libdmnerf_b200.so")
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 N_PARAMS = 30
 IMPL_AUTO, IMPL_SIMT, IMPL_UMMA, IMPL_UMMA_F16 = 0, 1, 2, 3
-FLAG_PERTURB, FLAG_WANT_RAW, FLAG_KEEP_INS, FLAG_SELECT, FLAG_REGION, FLAG_APPEARANCE = 1, 2, 4, 8, 16, 32
+FLAG_PERTURB, FLAG_WANT_RAW, FLAG_KEEP_INS = 1, 2, 4
 LABEL_WORDS = 2049           # DMNERF_LABEL_WORDS
 
 _f32p = C.c_void_p
+
+
+class RegionDesc(C.Structure):
+    """Mirror of `struct dmnerf_region` (objects.Region.abi builds one)."""
+    _fields_ = [("bits", C.c_void_p), ("dim", C.c_int32), ("outside_keep", C.c_int32), ("voxel_map", C.c_float * 12),
+                ("applies", C.c_uint32 * 4)]
+
+
+class Edit(C.Structure):
+    """Mirror of `struct dmnerf_edit` (render.scene_edit builds one)."""
+    _fields_ = [("keep", C.POINTER(C.c_uint32)), ("region", C.POINTER(RegionDesc)), ("appearance", C.POINTER(C.c_float)),
+                ("appearance_labels", C.c_int32)]
 
 
 class RenderIO(C.Structure):
@@ -33,23 +45,17 @@ class RenderIO(C.Structure):
         ("rgb_coarse", _f32p), ("rgb_fine", _f32p), ("depth_coarse", _f32p), ("depth_fine", _f32p),
         ("acc_coarse", _f32p), ("acc_fine", _f32p), ("ins_coarse", _f32p), ("ins_fine", _f32p),
         ("z_vals_coarse", _f32p), ("z_vals_fine", _f32p), ("weights_coarse", _f32p), ("weights_fine", _f32p),
-        ("raw_coarse", _f32p), ("raw_fine", _f32p), ("keep", C.c_uint32 * 4),
+        ("raw_coarse", _f32p), ("raw_fine", _f32p), ("edit", C.POINTER(Edit)),
     ]
 
 
 MAX_MOVES = 8                # DMNERF_MAX_MOVES
 
 
-class PieceRegion(C.Structure):
-    """Mirror of `struct dmnerf_piece_region` (bits NULL: no region)."""
-    _fields_ = [("bits", C.c_void_p), ("dim", C.c_int32), ("outside_keep", C.c_int32), ("voxel_map", C.c_float * 12),
-                ("applies", C.c_uint32 * 4)]
-
-
 class Pieces(C.Structure):
     """Mirror of `struct dmnerf_pieces`."""
     _fields_ = [
-        ("region", PieceRegion * MAX_MOVES), ("rest_drop", C.c_int32 * MAX_MOVES),
+        ("region", RegionDesc * MAX_MOVES), ("rest_drop", C.c_int32 * MAX_MOVES),
         ("ori_vote", C.c_void_p * MAX_MOVES), ("tar_vote", C.c_void_p * MAX_MOVES),
         ("ori_rays_o", _f32p), ("ori_rays_d", _f32p), ("ori_z", _f32p),
         ("tar_rays_o", _f32p * MAX_MOVES), ("tar_rays_d", _f32p * MAX_MOVES), ("tar_z", _f32p * MAX_MOVES),
@@ -110,7 +116,7 @@ PROTOTYPES = {
     "dmnerf_exchanger": (C.c_int, [_f32p, C.POINTER(C.c_void_p), _f32p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.c_int, C.c_int64,
                                   C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Pieces), C.c_void_p]),
     "dmnerf_piece_vote": (C.c_int, [_f32p, _f32p, _f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_int),
-                                    C.POINTER(PieceRegion), C.c_int, C.c_void_p, C.c_void_p]),
+                                    C.POINTER(RegionDesc), C.c_int, C.c_void_p, C.c_void_p]),
     "dmnerf_penalizer_state_bytes": (C.c_int64, []),
     "dmnerf_penalizer_forward": (C.c_int, [_f32p, _f32p, _f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p,
                                           _f32p, C.c_void_p]),
@@ -144,11 +150,9 @@ PROTOTYPES = {
     "dmnerf_component_table": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p]),
     "dmnerf_component_groups": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "dmnerf_set_region": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_uint32), C.c_int]),
     "dmnerf_region_pack": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "dmnerf_region_dilate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
-    "dmnerf_region_contains": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_float), _f32p, C.c_int64, C.c_void_p, C.c_void_p]),
-    "dmnerf_set_appearance": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.c_int, C.c_void_p]),
+    "dmnerf_region_contains": (C.c_int, [C.POINTER(RegionDesc), _f32p, C.c_int64, C.c_void_p, C.c_void_p]),
     "dmnerf_eval_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int, C.c_int, C.c_int]),
     "dmnerf_eval_image": (C.c_int, [_f32p, _f32p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dmnerf_ins_eval": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_void_p, C.c_int, _f32p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,

@@ -23,16 +23,15 @@ void set_error(const char* fmt, ...) {
   g_error = buf;
 }
 
-// An entry point's object selection: keep_host (4 host words, NULL = no selection) -> keep = &m, or NULL.  Only labels
+// An entry point's object selection: keep_host (4 host words) -> m, or every label when keep_host is NULL.  Only labels
 // 0 .. n_labels - 1 may be set; n_labels = 0 means no network is bound to label the samples with.
-static int object_mask(const uint32_t* keep_host, int n_labels, ObjMask& m, const ObjMask*& keep, const char* who) {
-  keep = nullptr;
+static int object_mask(const uint32_t* keep_host, int n_labels, ObjMask& m, const char* who) {
+  m = ObjMask{{~0u, ~0u, ~0u, ~0u}};
   if (!keep_host) return 0;
   DMN_CHECK(n_labels > 0, "%s: an object selection needs the network(s) bound with dmnerf_set_weights (one ins_num)", who);
   for (int b = n_labels; b < 128; ++b)
     DMN_CHECK(!((keep_host[b >> 5] >> (b & 31)) & 1u), "%s: object mask keeps label %d, outside [0, %d]", who, b, n_labels - 1);
   for (int i = 0; i < 4; ++i) m.w[i] = keep_host[i];
-  keep = &m;
   return 0;
 }
 
@@ -55,13 +54,9 @@ struct dmnerf_ctx {
   MeshState mesh;                 // buffers of the other mesh entry points (mesh.cu)
   InventoryState inventory;       // buffers of the object-inventory entry points (inventory.cu)
   ComponentsState components;     // buffers of the connected-component entry points (components.cu)
-  Region region = {};             // region selection read with DMNERF_FLAG_REGION (dmnerf_set_region); bits == NULL: none set
   DeviceBuffer region_tmp;        // dmnerf_region_dilate: the second buffer of a multi-step dilation
-  // object appearance read with DMNERF_FLAG_APPEARANCE (dmnerf_set_appearance): appearance_labels rows of APPEARANCE_ROW floats
-  // at `appearance`, in a buffer of its own sized for DMNERF_MAX_INS + 1 rows, so that it is never reallocated; 0 labels: none set
+  // the appearance table of the render call (scene_edit), sized for DMNERF_MAX_INS + 1 rows so that it is never reallocated
   DeviceBuffer appearance_buf;
-  const float* appearance = nullptr;
-  int appearance_labels = 0;
   bool profiling = false;
   bool profile_valid = false;
   cudaEvent_t ev[DMNERF_N_STAGES + 1] = {};
@@ -71,42 +66,44 @@ struct dmnerf_ctx {
   dmnerf_ctx() { memset(net, 0, sizeof(net)); }
 };
 
-// The selection of a render call: io->keep with DMNERF_FLAG_SELECT, over labels 0 .. ins_num of the coarse / fine pair (both
-// bound with one ins_num, else no labels).
-static int render_mask(const dmnerf_ctx* ctx, const dmnerf_render_io* io, int flags, ObjMask& m, const ObjMask*& keep,
-                       const char* who) {
+// The flags the render entry points take.
+constexpr int RENDER_FLAGS = DMNERF_FLAG_PERTURB | DMNERF_FLAG_WANT_RAW | DMNERF_FLAG_KEEP_INS;
+
+// The scene edit of a render call, checked against the coarse / fine pair (both bound with one ins_num): in (NULL, or all three
+// members NULL: no edit) -> e and edit = &e, or edit = NULL for the unselected kernels.  The appearance table is copied on `st`
+// into the context's staging buffer.  Without a selection every label is kept (object_mask).
+static int scene_edit(dmnerf_ctx* ctx, const dmnerf_edit* in, cudaStream_t st, Edit& e, const Edit*& edit, const char* who) {
+  edit = nullptr;
+  if (!in || (!in->keep && !in->region && !in->appearance)) return 0;
   const bool pair = ctx && ctx->net[0].bound && ctx->net[1].bound && ctx->net[0].ins_num == ctx->net[1].ins_num;
-  return object_mask((flags & DMNERF_FLAG_SELECT) && io ? io->keep : nullptr, pair ? ctx->net[0].ins_num + 1 : 0, m, keep, who);
-}
-
-// The region of a render call: the context's (dmnerf_set_region) with DMNERF_FLAG_REGION, else NULL.  Its labels are checked
-// against the bound pair here, as a keep mask's are.
-static int render_region(const dmnerf_ctx* ctx, int flags, const Region*& region, const char* who) {
-  region = nullptr;
-  if (!(flags & DMNERF_FLAG_REGION)) return 0;
-  DMN_CHECK(ctx && ctx->region.bits, "%s: DMNERF_FLAG_REGION without a region (set one with dmnerf_set_region)", who);
-  const bool pair = ctx->net[0].bound && ctx->net[1].bound && ctx->net[0].ins_num == ctx->net[1].ins_num;
-  DMN_CHECK(pair, "%s: a region selection needs the network(s) bound with dmnerf_set_weights (one ins_num)", who);
+  DMN_CHECK(pair, "%s: a scene edit needs the network(s) bound with dmnerf_set_weights (one ins_num)", who);
   const int n_labels = ctx->net[0].ins_num + 1;
-  for (int b = n_labels; b < 128; ++b)
-    DMN_CHECK(!((ctx->region.applies.w[b >> 5] >> (b & 31)) & 1u), "%s: region applies to label %d, outside [0, %d]", who, b,
-              n_labels - 1);
-  region = &ctx->region;
-  return 0;
-}
-
-// The appearance table of a render call: the context's (dmnerf_set_appearance) with DMNERF_FLAG_APPEARANCE, else NULL.  It must
-// have one row per label of the bound pair.
-static int render_appearance(const dmnerf_ctx* ctx, int flags, const float*& table, const char* who) {
-  table = nullptr;
-  if (!(flags & DMNERF_FLAG_APPEARANCE)) return 0;
-  DMN_CHECK(ctx && ctx->appearance_labels > 0, "%s: DMNERF_FLAG_APPEARANCE without an appearance (set one with "
-            "dmnerf_set_appearance)", who);
-  const bool pair = ctx->net[0].bound && ctx->net[1].bound && ctx->net[0].ins_num == ctx->net[1].ins_num;
-  DMN_CHECK(pair, "%s: an appearance needs the network(s) bound with dmnerf_set_weights (one ins_num)", who);
-  DMN_CHECK(ctx->appearance_labels == ctx->net[0].ins_num + 1, "%s: the appearance has %d rows for %d labels (ins_num + 1)", who,
-            ctx->appearance_labels, ctx->net[0].ins_num + 1);
-  table = ctx->appearance;
+  if (object_mask(in->keep, n_labels, e.keep, who)) return 1;
+  e.region = Region{};
+  if (in->region) {
+    if (region_from_abi(*in->region, e.region, who)) return 1;
+    for (int b = n_labels; b < 128; ++b)
+      DMN_CHECK(!obj_kept(e.region.applies, b), "%s: region applies to label %d, outside [0, %d]", who, b, n_labels - 1);
+  }
+  e.appearance = nullptr;
+  if (in->appearance) {
+    const int rows = in->appearance_labels;
+    DMN_CHECK(rows >= 2 && rows <= DMNERF_MAX_INS + 1, "%s: an appearance of %d labels outside [2, %d]", who, rows,
+              DMNERF_MAX_INS + 1);
+    DMN_CHECK(rows == n_labels, "%s: the appearance has %d rows for %d labels (ins_num + 1)", who, rows, n_labels);
+    for (int l = 0; l < rows; ++l) {
+      const float* row = in->appearance + (size_t)l * APPEARANCE_ROW;
+      for (int i = 0; i < APPEARANCE_ROW; ++i)
+        DMN_CHECK(std::isfinite(row[i]), "%s: appearance entry %d of label %d is not finite", who, i, l);
+      DMN_CHECK(row[12] >= 0.0f, "%s: label %d has a negative density scale %g", who, l, (double)row[12]);
+    }
+    DMN_CUDA(cudaSetDevice(ctx->device));
+    float* d;
+    if (ctx->appearance_buf.get((size_t)(DMNERF_MAX_INS + 1) * APPEARANCE_ROW, &d)) return 2;
+    DMN_CUDA(cudaMemcpyAsync(d, in->appearance, (size_t)rows * APPEARANCE_ROW * sizeof(float), cudaMemcpyHostToDevice, st));
+    e.appearance = d;
+  }
+  edit = &e;
   return 0;
 }
 
@@ -242,10 +239,10 @@ DMNERF_API int dmnerf_composite(const float* raw, const float* z, const float* r
   DMN_CHECK(n >= 0, "composite: negative ray count");
   DMN_CHECK(n == 0 || (raw && z && rays_d), "composite: NULL input");
   DMN_CHECK(c >= 5 && c <= 4 + DMNERF_MAX_INS + 1, "composite: channels=%d out of range", c);
-  ObjMask m;
-  const ObjMask* keep;
-  if (object_mask(keep_host, c - 4, m, keep, "composite")) return 1;
-  return launch_composite(raw, z, rays_d, n, s, c, keep_all_ins, rgb, weights, depth, ins, acc, (cudaStream_t)stream, keep);
+  Edit e = {};
+  if (object_mask(keep_host, c - 4, e.keep, "composite")) return 1;
+  return launch_composite(raw, z, rays_d, n, s, c, keep_all_ins, rgb, weights, depth, ins, acc, (cudaStream_t)stream,
+                          keep_host ? &e : nullptr);
 }
 
 DMNERF_API int dmnerf_sample_pdf(const float* bins, const float* weights, int64_t n, int n_bins, int n_samples, const float* u,
@@ -419,10 +416,9 @@ DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, 
 
 }  // extern "C"
 
-// dm_nerf() on device buffers; keep: object selection, region: region selection, appearance: object appearance table (all NULL =
-// none, the unselected kernels)
+// dm_nerf() on device buffers; edit: the checked scene edit, or NULL for none (the unselected kernels)
 static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
-                               const ObjMask* keep, const Region* region, const float* appearance, void* stream) {
+                               const Edit* edit, void* stream) {
   DMN_CHECK(ctx && io, "render_forward: NULL ctx/io");
   DMN_CHECK(n >= 0 && S >= 3 && NI >= 2, "render_forward: bad sizes n=%lld S=%d I=%d", (long long)n, S, NI);
   DMN_CHECK(ctx->net[0].bound && ctx->net[1].bound, "render_forward: bind both networks with dmnerf_set_weights first");
@@ -442,8 +438,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   if (impl != DMNERF_IMPL_SIMT && S == 64 && NI == 128 && !io->raw_coarse && !io->raw_fine) {
     const bool prof = ctx->profiling;
     if (prof) DMN_CUDA(cudaEventRecord(ctx->ev[0], st));
-    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, keep, impl == DMNERF_IMPL_UMMA_F16, region,
-                                appearance);
+    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, edit, impl == DMNERF_IMPL_UMMA_F16);
     if (rc) return rc;
     if (prof) for (int i = 1; i <= DMNERF_N_STAGES; ++i) DMN_CUDA(cudaEventRecord(ctx->ev[i], st));
     ctx->profile_valid = prof;
@@ -475,7 +470,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:63     coarse composite
   if ((rc = launch_composite(raw_c, z_c, io->rays_d, n, S, C, keep_ins, io->rgb_coarse, w_c, io->depth_coarse,
-                             io->ins_coarse, io->acc_coarse, st, keep, io->rays_o, region, appearance))) return rc;
+                             io->ins_coarse, io->acc_coarse, st, edit, io->rays_o))) return rc;
   DMN_STAGE_MARK();
   // render.py:66-70  importance sampling + merge
   if ((rc = launch_hier_sample(z_c, w_c, perturb ? io->u : nullptr, n, S, NI, z_f, st))) return rc;
@@ -485,7 +480,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:86     fine composite
   if ((rc = launch_composite(raw_f, z_f, io->rays_d, n, F, C, keep_ins, io->rgb_fine, io->weights_fine, io->depth_fine,
-                             io->ins_fine, io->acc_fine, st, keep, io->rays_o, region, appearance))) return rc;
+                             io->ins_fine, io->acc_fine, st, edit, io->rays_o))) return rc;
   DMN_STAGE_MARK();
 #undef DMN_STAGE_MARK
   ctx->profile_valid = prof;
@@ -496,14 +491,11 @@ extern "C" {
 
 DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
                           void* stream) {
-  ObjMask m;
-  const ObjMask* keep;
-  const Region* region;
-  const float* appearance;
-  if (render_mask(ctx, io, flags, m, keep, "render_forward") || render_region(ctx, flags, region, "render_forward") ||
-      render_appearance(ctx, flags, appearance, "render_forward"))
-    return 1;
-  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, keep, region, appearance, stream), impl, stream);
+  DMN_CHECK(!(flags & ~RENDER_FLAGS), "render_forward: unknown flag bits 0x%x", flags & ~RENDER_FLAGS);
+  Edit e;
+  const Edit* edit;
+  if (int rc = scene_edit(ctx, io ? io->edit : nullptr, (cudaStream_t)stream, e, edit, "render_forward")) return rc;
+  return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, edit, stream), impl, stream);
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
@@ -545,10 +537,10 @@ DMNERF_API int dmnerf_profile_read(dmnerf_ctx* ctx, float* ms_out, int n_out) {
 }  // extern "C"
 
 // Host-buffer render: `h` holds HOST pointers for the outputs (and for the inputs unless dev_rays_o / dev_rays_d are given:
-// rays that are already resident on the device, e.g. generated there from the camera).
+// rays that are already resident on the device, e.g. generated there from the camera).  edit: as for render_forward_impl, its
+// appearance table already on the device, so that every part reads the one copy.
 static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const float* dev_rays_o, const float* dev_rays_d, int64_t n,
-                            int S, int NI, int flags, int impl, const ObjMask* keep, const Region* region,
-                            const float* appearance, void* stream) {
+                            int S, int NI, int flags, int impl, const Edit* edit, void* stream) {
   DMN_CHECK(ctx && h, "render_forward_host: NULL ctx/io");
   DMN_CHECK(n >= 0, "render_forward_host: negative ray count");
   if (n == 0) return 0;
@@ -638,7 +630,7 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
   const bool parts = n >= HOST_PART_MIN_RAYS && !ctx->profiling;
   if (!parts) {
     if (copy_in(0, n, st)) return 1;
-    int rc = render_forward_impl(ctx, &io, n, S, NI, flags, impl, keep, region, appearance, stream);
+    int rc = render_forward_impl(ctx, &io, n, S, NI, flags, impl, edit, stream);
     if (rc) return rc;
     if (copy_out(0, n, st)) return 1;
     return dmnerf_sync_check(ctx, stream);
@@ -668,7 +660,7 @@ static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const fl
   for (int i = 0; i < HOST_PARTS && !rc; ++i) {
     if (i > 0) DMN_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[i], 0));
     const dmnerf_render_io pi = part_io(edge[i]);
-    rc = render_forward_impl(ctx, &pi, edge[i + 1] - edge[i], S, NI, flags, impl, keep, region, appearance, stream);
+    rc = render_forward_impl(ctx, &pi, edge[i + 1] - edge[i], S, NI, flags, impl, edit, stream);
     if (rc) break;
     DMN_CUDA(cudaEventRecord(ctx->ev_done[i], st));
     DMN_CUDA(cudaStreamWaitEvent(cs, ctx->ev_done[i], 0));
@@ -684,27 +676,21 @@ extern "C" {
 
 DMNERF_API int dmnerf_render_forward_host(dmnerf_ctx* ctx, const dmnerf_render_io* h, int64_t n, int S, int NI, int flags,
                                int impl, void* stream) {
-  ObjMask m;
-  const ObjMask* keep;
-  const Region* region;
-  const float* appearance;
-  if (render_mask(ctx, h, flags, m, keep, "render_forward_host") || render_region(ctx, flags, region, "render_forward_host") ||
-      render_appearance(ctx, flags, appearance, "render_forward_host"))
-    return 1;
-  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, keep, region, appearance, stream);
+  DMN_CHECK(!(flags & ~RENDER_FLAGS), "render_forward_host: unknown flag bits 0x%x", flags & ~RENDER_FLAGS);
+  Edit e;
+  const Edit* edit;
+  if (int rc = scene_edit(ctx, h ? h->edit : nullptr, (cudaStream_t)stream, e, edit, "render_forward_host")) return rc;
+  return render_host_impl(ctx, h, nullptr, nullptr, n, S, NI, flags, impl, edit, stream);
 }
 
 DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
                                         float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
                                         int flags, int impl, const dmnerf_render_io* out_host, void* stream) {
   DMN_CHECK(ctx && K_host && c2w_host && out_host, "render_frame_host: NULL argument");
-  ObjMask m;
-  const ObjMask* keep;
-  const Region* region;
-  const float* appearance;
-  if (render_mask(ctx, out_host, flags, m, keep, "render_frame_host") || render_region(ctx, flags, region, "render_frame_host") ||
-      render_appearance(ctx, flags, appearance, "render_frame_host"))
-    return 1;
+  DMN_CHECK(!(flags & ~RENDER_FLAGS), "render_frame_host: unknown flag bits 0x%x", flags & ~RENDER_FLAGS);
+  Edit e;
+  const Edit* edit;
+  if (int rc = scene_edit(ctx, out_host->edit, (cudaStream_t)stream, e, edit, "render_frame_host")) return rc;
   DMN_CHECK(H > 0 && W > 0 && n_coarse >= 3 && n_coarse <= 4096, "render_frame_host: bad sizes H=%d W=%d S=%d", H, W, n_coarse);
   DMN_CHECK(ray_begin >= 0 && ray_count >= 0 && ray_begin + ray_count <= (int64_t)H * W,
             "render_frame_host: pixel range [%lld, +%lld) outside the %dx%d frame", (long long)ray_begin, (long long)ray_count, H, W);
@@ -727,8 +713,8 @@ DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, co
   dmnerf_render_io h = *out_host;
   h.rays_o = nullptr; h.rays_d = nullptr; h.t_rand = nullptr; h.u = nullptr;
   h.z_coarse = z.data(); h.z_row_stride = 0;
-  return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, keep, region,
-                          appearance, stream);
+  return render_host_impl(ctx, &h, ro + ray_begin * 3, rd + ray_begin * 3, ray_count, n_coarse, n_importance, flags, impl, edit,
+                          stream);
 }
 
 // ---- mesh extraction (tools/mesh_generator.py mesh_main) ------------------------------------------------------------------
@@ -746,9 +732,8 @@ DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* tra
   DMN_CHECK(transform_host && extents_host && occ, "mesh_occupancy: NULL argument");
   DMN_CHECK(dim >= 2 && dim <= 2048, "mesh_occupancy: dim %d out of range [2, 2048]", dim);
   DMN_CHECK(keep_host || !labels, "mesh_occupancy: labels are written by the selected sweep only (pass keep_host)");
-  ObjMask m;
-  const ObjMask* keep;
-  if (object_mask(keep_host, ctx->net[net].bound ? ctx->net[net].ins_num + 1 : 0, m, keep, "mesh_occupancy")) return 1;
+  ObjMask keep;
+  if (object_mask(keep_host, ctx->net[net].bound ? ctx->net[net].ins_num + 1 : 0, keep, "mesh_occupancy")) return 1;
   DMN_CHECK(umma_available(ctx->packed[net]), "mesh_occupancy: bind the network with dmnerf_set_weights first");
   cudaStream_t st = (cudaStream_t)stream;
   DMN_CUDA(cudaSetDevice(ctx->device));
@@ -765,8 +750,8 @@ DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* tra
     const int64_t cnt = n - b < slab ? n - b : slab;
     int rc = launch_grid_points(transform_host, extents_host, dim, b, cnt, pts, st);
     if (!rc) rc = launch_mlp_umma(ctx->packed[net], ctx->net[net], nullptr, pts, dirs, nullptr, cnt, 1, raw, nullptr, st);
-    if (!rc) rc = keep ? launch_occupancy_objects(raw, cnt, C, voxel, *keep, occ + b, labels ? labels + b : nullptr, st)
-                       : launch_occupancy(raw, cnt, C, voxel, occ + b, st);
+    if (!rc) rc = keep_host ? launch_occupancy_objects(raw, cnt, C, voxel, keep, occ + b, labels ? labels + b : nullptr, st)
+                            : launch_occupancy(raw, cnt, C, voxel, occ + b, st);
     if (rc) return rc;
   }
   return 0;
@@ -870,52 +855,6 @@ DMNERF_API int dmnerf_component_groups(dmnerf_ctx* ctx, const int32_t* comp, int
 
 // ---- region selection (DESIGN.md, "Region selection") ---------------------------------------------------------------------
 
-DMNERF_API int dmnerf_set_region(dmnerf_ctx* ctx, const uint32_t* bits_device, int dim, const float* voxel_map12,
-                                 const uint32_t* applies_host, int outside_keep) {
-  DMN_CHECK(ctx != nullptr, "set_region: ctx is NULL");
-  if (!bits_device) {
-    ctx->region = Region{};
-    return 0;
-  }
-  DMN_CHECK(voxel_map12 && applies_host, "set_region: NULL voxel map / applies mask");
-  if (region_check(dim, voxel_map12, "set_region")) return 1;
-  Region r = {};
-  r.bits = bits_device;
-  for (int i = 0; i < 12; ++i) r.map[i] = voxel_map12[i];
-  r.dim = dim;
-  r.outside_keep = outside_keep ? 1 : 0;
-  for (int i = 0; i < 4; ++i) r.applies.w[i] = applies_host[i];
-  ctx->region = r;
-  return 0;
-}
-
-// ---- object appearance (DESIGN.md, "Object appearance") -------------------------------------------------------------------
-
-DMNERF_API int dmnerf_set_appearance(dmnerf_ctx* ctx, const float* table_host, int n_labels, void* stream) {
-  DMN_CHECK(ctx != nullptr, "set_appearance: ctx is NULL");
-  if (!table_host) {
-    ctx->appearance = nullptr;
-    ctx->appearance_labels = 0;
-    return 0;
-  }
-  DMN_CHECK(n_labels >= 2 && n_labels <= DMNERF_MAX_INS + 1, "set_appearance: %d labels outside [2, %d]", n_labels,
-            DMNERF_MAX_INS + 1);
-  for (int l = 0; l < n_labels; ++l) {
-    const float* row = table_host + (size_t)l * APPEARANCE_ROW;
-    for (int i = 0; i < APPEARANCE_ROW; ++i)
-      DMN_CHECK(std::isfinite(row[i]), "set_appearance: entry %d of label %d is not finite", i, l);
-    DMN_CHECK(row[12] >= 0.0f, "set_appearance: label %d has a negative density scale %g", l, (double)row[12]);
-  }
-  DMN_CUDA(cudaSetDevice(ctx->device));
-  float* d;
-  if (ctx->appearance_buf.get((size_t)(DMNERF_MAX_INS + 1) * APPEARANCE_ROW, &d)) return 2;
-  DMN_CUDA(cudaMemcpyAsync(d, table_host, (size_t)n_labels * APPEARANCE_ROW * sizeof(float), cudaMemcpyHostToDevice,
-                           (cudaStream_t)stream));
-  ctx->appearance = d;
-  ctx->appearance_labels = n_labels;
-  return 0;
-}
-
 DMNERF_API int dmnerf_region_pack(const int32_t* ids, int dim, const uint32_t* table, int64_t n_ids, uint32_t* bits, void* stream) {
   return region_pack(ids, dim, table, n_ids, bits, (cudaStream_t)stream);
 }
@@ -930,14 +869,10 @@ DMNERF_API int dmnerf_region_dilate(dmnerf_ctx* ctx, const uint32_t* in, int dim
   return region_dilate(in, dim, radius, connectivity, invert, out, tmp, (cudaStream_t)stream);
 }
 
-DMNERF_API int dmnerf_region_contains(const uint32_t* bits, int dim, const float* voxel_map12, const float* pts, int64_t n,
-                                      uint8_t* out, void* stream) {
-  DMN_CHECK(bits && voxel_map12, "region_contains: NULL bits / voxel map");
-  if (region_check(dim, voxel_map12, "region_contains")) return 1;
-  Region r = {};
-  r.bits = bits;
-  for (int i = 0; i < 12; ++i) r.map[i] = voxel_map12[i];
-  r.dim = dim;
+DMNERF_API int dmnerf_region_contains(const dmnerf_region* region, const float* pts, int64_t n, uint8_t* out, void* stream) {
+  DMN_CHECK(region != nullptr, "region_contains: region is NULL");
+  Region r;
+  if (region_from_abi(*region, r, "region_contains")) return 1;
   return region_contains(r, pts, n, out, (cudaStream_t)stream);
 }
 

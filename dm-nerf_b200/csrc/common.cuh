@@ -174,15 +174,21 @@ inline int64_t region_words(int dim) { return ((int64_t)dim * dim * dim + 31) / 
 // appearance_apply (ray_ops.cuh).
 constexpr int APPEARANCE_ROW = 16;
 
+// The scene edit of a render call, checked (abi.cu scene_edit): the kept labels (every label when the caller gave no selection),
+// the region (bits == NULL: none) and the appearance table (device, ins_num + 1 rows, or NULL: none).  A launcher given an Edit
+// runs the selected kernels; given NULL, the unselected ones.
+struct Edit {
+  ObjMask keep;
+  Region region;
+  const float* appearance;
+};
+
 // ---- launchers implemented in the individual .cu files (all return 0 / non-zero status) ----
 int launch_posenc(const float* x, int64_t m, int n_freqs, float* out, cudaStream_t st);
-// keep: object selection, or NULL for none (the unselected kernel); region (with rays_o): region selection, or NULL for none.
-// A region without keep runs the selected kernel with every label kept.  appearance: the table of object appearance (device,
-// c - 4 rows), or NULL for none; without keep or a region it too runs the selected kernel with every label kept.
+// edit: the scene edit (the selected kernel; a region needs rays_o), or NULL for none (the unselected kernel).
 int launch_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all,
                      float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st,
-                     const ObjMask* keep = nullptr, const float* rays_o = nullptr, const Region* region = nullptr,
-                     const float* appearance = nullptr);
+                     const Edit* edit = nullptr, const float* rays_o = nullptr);
 int launch_sample_pdf(const float* bins, const float* weights, int64_t n, int nb, int ns, const float* u, float* out,
                       cudaStream_t st);
 int launch_sort_concat(const float* a, const float* b, int64_t n, int na, int nb, float* out, cudaStream_t st);
@@ -307,10 +313,12 @@ int component_groups(ComponentsState& s, const int32_t* comp, int dim, int64_t n
 
 // Region builders (region.cu).  Grids are [dim]^3 in C order; bits are region_words(dim) uint32 words, the tail zero.
 int region_check(int dim, const float* map12, const char* who);      // dim in range, map finite (map12 may be NULL)
+// The ABI region d as r, checked: bits not NULL, then region_check.
+int region_from_abi(const dmnerf_region& d, Region& r, const char* who);
 int region_pack(const int32_t* ids, int dim, const uint32_t* table, int64_t n_ids, uint32_t* bits, cudaStream_t st);
 // tmp: region_words(dim) device words, needed when r >= 2
 int region_dilate(const uint32_t* in, int dim, int r, int connectivity, int invert, uint32_t* out, uint32_t* tmp, cudaStream_t st);
-int region_contains(const Region& r, const float* pts, int64_t n, uint8_t* out, cudaStream_t st);
+int region_contains(const Region& r, const float* pts, int64_t n, uint8_t* out, cudaStream_t st);   // r from region_from_abi
 
 // Test-view evaluation (metrics.cu)
 int64_t eval_workspace_bytes(int64_t n, int k, int H, int W);

@@ -186,18 +186,13 @@ __global__ void __launch_bounds__(VOTE_WARPS * 32) piece_vote_kernel(const VoteA
   }
 }
 
-// The region of a move, checked: dim and map, the moved label among the labels it applies to.
-int piece_region(const dmnerf_piece_region& d, int mv, Region& r, const char* who, int i) {
+// The region of a move (bits NULL: none), checked: dim and map, the moved label among the labels it applies to.
+int piece_region(const dmnerf_region& d, int mv, Region& r, const char* who, int i) {
   r = Region{};
   if (!d.bits) return 0;
-  if (region_check(d.dim, d.voxel_map, who)) return 1;
-  DMN_CHECK(mv >= 0 && mv <= DMNERF_MAX_INS && ((d.applies[mv >> 5] >> (mv & 31)) & 1u),
+  if (region_from_abi(d, r, who)) return 1;
+  DMN_CHECK(mv >= 0 && mv <= DMNERF_MAX_INS && obj_kept(r.applies, mv),
             "%s: move %d: moved label %d is not among the labels its region applies to", who, i, mv);
-  r.bits = d.bits;
-  for (int k = 0; k < 12; ++k) r.map[k] = d.voxel_map[k];
-  r.dim = d.dim;
-  r.outside_keep = d.outside_keep ? 1 : 0;
-  for (int k = 0; k < 4; ++k) r.applies.w[k] = d.applies[k];
   return 0;
 }
 
@@ -244,7 +239,7 @@ extern "C" DMNERF_API int dmnerf_exchanger(float* ori_raw, const float* const* t
 
 extern "C" DMNERF_API int dmnerf_piece_vote(const float* raw, const float* z, const float* weights, const float* rays_o,
                                             const float* rays_d, int64_t n, int s, int c, const int* move_labels,
-                                            const dmnerf_piece_region* regions, int n_moves, uint8_t* votes, void* stream) {
+                                            const dmnerf_region* regions, int n_moves, uint8_t* votes, void* stream) {
   const char* who = "piece_vote";
   DMN_CHECK(n >= 0 && s >= 1 && c > 5, "%s: bad sizes n=%lld s=%d c=%d", who, (long long)n, s, c);
   DMN_CHECK(n_moves >= 1 && n_moves <= EX_MAX_MOVES, "%s: between 1 and %d moves are supported, got %d", who, EX_MAX_MOVES, n_moves);

@@ -1021,7 +1021,7 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
 // Whole dm_nerf() pipeline (render.py:31-96) in ONE launch: coarse network -> composite -> importance sampling -> fine
 // network -> composite, per pair of rays, nothing but rays in and per-ray maps out crossing HBM.  64 + 128 samples only.
 int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmnerf_render_io* io, int64_t n, int flags,
-                       cudaStream_t st, const ObjMask* keep, bool f16, const Region* region, const float* appearance) {
+                       cudaStream_t st, const Edit* edit, bool f16) {
   using namespace uk;
   DMN_CHECK(wc.ready && wf.ready && wc.extra && wf.extra, "render(umma): weights not packed");
   DMN_CHECK(wc.ins_num == wf.ins_num, "render(umma): coarse/fine ins_num differ");
@@ -1043,17 +1043,15 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   a.acc_c = io->acc_coarse; a.acc_f = io->acc_fine; a.ins_c = io->ins_coarse; a.ins_f = io->ins_fine;
   a.zc_out = io->z_vals_coarse; a.zf_out = io->z_vals_fine; a.wc_out = io->weights_coarse; a.wf_out = io->weights_fine;
   a.status = ex->d_status;
-  if (keep) a.keep = *keep;
-  if (region) a.region = *region;
-  a.appearance = appearance;
-  if (!keep && (region || appearance)) {                  // a region or an appearance alone: the selected kernel, every label kept
-    a.keep = ObjMask{{~0u, ~0u, ~0u, ~0u}};
-    keep = &a.keep;
+  if (edit) {
+    a.keep = edit->keep;
+    a.region = edit->region;
+    a.appearance = edit->appearance;
   }
   const int64_t units = (n + 1) / 2;                       // pairs of rays
   const Program& prog = f16 ? ex->prog16 : ex->prog;      // coarse and fine share ins_num, hence the program
-  if (keep && f16) return launch_umma<render_objects_f16_kernel>(units, prog, a, st);
-  if (keep) return launch_umma<render_objects_kernel>(units, prog, a, st);
+  if (edit && f16) return launch_umma<render_objects_f16_kernel>(units, prog, a, st);
+  if (edit) return launch_umma<render_objects_kernel>(units, prog, a, st);
   if (f16) return launch_umma<mlp_f16_kernel<true>>(units, prog, a, st);
   return launch_umma<mlp_umma_kernel<true>>(units, prog, a, st);
 }

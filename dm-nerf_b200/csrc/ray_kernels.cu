@@ -117,22 +117,20 @@ __global__ void composite_kernel(const float* __restrict__ raw, const float* __r
 }
 
 int launch_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all,
-                     float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st, const ObjMask* keep,
-                     const float* rays_o, const Region* region, const float* appearance) {
+                     float* rgb, float* weights, float* depth, float* ins, float* acc, cudaStream_t st, const Edit* edit,
+                     const float* rays_o) {
   DMN_CHECK(s >= 1 && s <= 4096, "composite: n_samples=%d out of range [1,4096]", s);
   DMN_CHECK(c >= 5 && c <= 4 + DMNERF_MAX_INS + 1, "composite: channels=%d out of range", c);
-  DMN_CHECK(!region || (region->bits && rays_o), "composite: a region needs its bits and the ray origins");
+  DMN_CHECK(!edit || !edit->region.bits || rays_o, "composite: a region needs the ray origins");
   if (n == 0) return 0;
   const size_t smem = (size_t)WARPS_PER_BLOCK * s * sizeof(float);
-  const bool select = keep || region || appearance;
-  auto kernel = select ? composite_kernel<true> : composite_kernel<false>;
+  auto kernel = edit ? composite_kernel<true> : composite_kernel<false>;
   if (smem > 48 * 1024)
     DMN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const ObjMask none = {{0u, 0u, 0u, 0u}}, all = {{~0u, ~0u, ~0u, ~0u}};
-  const Region no_region{};
+  const Edit none = {};
+  const Edit& e = edit ? *edit : none;
   kernel<<<(unsigned)((n + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK), WARPS_PER_BLOCK * 32, smem, st>>>(
-      raw, z, rays_d, n, s, c, keep_all, rgb, weights, depth, ins, acc, keep ? *keep : (select ? all : none), rays_o,
-      region ? *region : no_region, appearance);
+      raw, z, rays_d, n, s, c, keep_all, rgb, weights, depth, ins, acc, e.keep, rays_o, e.region, e.appearance);
   DMN_LAUNCH_OK();
   return 0;
 }

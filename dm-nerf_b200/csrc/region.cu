@@ -98,6 +98,18 @@ int region_check(int dim, const float* map12, const char* who) {
   return 0;
 }
 
+int region_from_abi(const dmnerf_region& d, Region& r, const char* who) {
+  DMN_CHECK(d.bits != nullptr, "%s: a region with NULL bits", who);
+  if (region_check(d.dim, d.voxel_map, who)) return 1;
+  r = Region{};
+  r.bits = d.bits;
+  for (int i = 0; i < 12; ++i) r.map[i] = d.voxel_map[i];
+  r.dim = d.dim;
+  r.outside_keep = d.outside_keep ? 1 : 0;
+  for (int i = 0; i < 4; ++i) r.applies.w[i] = d.applies[i];
+  return 0;
+}
+
 int region_pack(const int32_t* ids, int dim, const uint32_t* table, int64_t n_ids, uint32_t* bits, cudaStream_t st) {
   const char* who = "region_pack";
   if (region_check(dim, nullptr, who)) return 1;
@@ -141,10 +153,7 @@ int region_dilate(const uint32_t* in, int dim, int r, int connectivity, int inve
 }
 
 int region_contains(const Region& r, const float* pts, int64_t n, uint8_t* out, cudaStream_t st) {
-  const char* who = "region_contains";
-  if (region_check(r.dim, r.map, who)) return 1;
-  DMN_CHECK(r.bits != nullptr, "%s: NULL bits", who);
-  DMN_CHECK(n >= 0 && (n == 0 || (pts && out)), "%s: bad points", who);
+  DMN_CHECK(n >= 0 && (n == 0 || (pts && out)), "region_contains: bad points");
   if (n == 0) return 0;
   region_contains_kernel<<<blocks_for(n), RG_THREADS, 0, st>>>(r, pts, n, out);
   DMN_LAUNCH_OK();

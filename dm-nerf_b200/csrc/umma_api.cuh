@@ -36,10 +36,8 @@ int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, co
                     const float* z, int64_t m, int s, float* out, float* acts, cudaStream_t st, bool f16 = false);
 
 // Fused whole-pipeline launch (64 + 128 samples, no raw output): see mlp_umma.cu.
+// edit: the scene edit (the selected kernel), or NULL for none (the unselected kernel).
 int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmnerf_render_io* io, int64_t n, int flags,
-                       cudaStream_t st, const ObjMask* keep = nullptr,     // keep: object selection, or NULL
-                       bool f16 = false,
-                       const Region* region = nullptr,                     // region selection, or NULL
-                       const float* appearance = nullptr);                 // object appearance table (device), or NULL
+                       cudaStream_t st, const Edit* edit, bool f16);
 
 }  // namespace dmnerf

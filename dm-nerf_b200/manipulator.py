@@ -92,22 +92,16 @@ def move_pieces(pieces, move_labels, ins_num, device):
 
 def _piece_region(region, mv, ins_num, device):
     """The C struct of one move's region (None: bits NULL)."""
-    d = _lib.PieceRegion()
     if region is None:
-        return d
+        return _lib.RegionDesc()
     from .objects import Region
     if not isinstance(region, Region):
         raise ValueError("pieces: each entry must be an objects.Region or None, got %r" % (type(region).__name__,))
     if region.bits.device != torch.device(device):
         raise ValueError("pieces: a region's bits live on %s, the edit on %s" % (region.bits.device, device))
-    words = region.applies_words(ins_num)
-    if not (0 <= mv <= ins_num and (int(words[mv >> 5]) >> (mv & 31)) & 1):
+    d = region.abi(ins_num)
+    if not (0 <= mv <= ins_num and (d.applies[mv >> 5] >> (mv & 31)) & 1):
         raise ValueError("pieces: moved label %d is not among the labels its region applies to" % mv)
-    d.bits = _lib.ptr(region.bits, torch.int32).value
-    d.dim = region.dim
-    d.outside_keep = int(region.outside == "keep")
-    d.voxel_map[:] = [float(v) for v in np.asarray(region.voxel_map, dtype=np.float32).reshape(-1)]
-    d.applies[:] = [int(w) & 0xFFFFFFFF for w in words]
     return d
 
 
@@ -124,7 +118,7 @@ def piece_vote(raw, z, weights, rays_o, rays_d, move_labels, regions):
     rays_o, rays_d = rays_o.contiguous().float(), rays_d.contiguous().float()
     if z.shape != (n, s) or weights.shape != (n, s) or rays_o.shape != (n, 3) or rays_d.shape != (n, 3):
         raise RuntimeError("piece_vote: inconsistent shapes")
-    descs = (_lib.PieceRegion * m)(*[_piece_region(r, int(mv), c - 5, raw.device) for r, mv in zip(regions, move_labels)])
+    descs = (_lib.RegionDesc * m)(*[_piece_region(r, int(mv), c - 5, raw.device) for r, mv in zip(regions, move_labels)])
     votes = torch.empty((m, n), dtype=torch.uint8, device=raw.device)
     get_context(raw.device).call("dmnerf_piece_vote", _lib.ptr(raw), _lib.ptr(z), _lib.ptr(weights), _lib.ptr(rays_o),
                                  _lib.ptr(rays_d), n, s, c, (C.c_int * m)(*[int(v) for v in move_labels]), descs, m,

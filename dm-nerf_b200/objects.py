@@ -515,6 +515,14 @@ class Region:
         """The 4 label words for networks with ins_num: applies, or every label 0 .. ins_num."""
         return object_mask(ins_num, remove=[]) if self.applies is None else list(self.applies)
 
+    def abi(self, ins_num):
+        """The C ABI's dmnerf_region (_lib.RegionDesc) of this region for networks with ins_num.  It points at self.bits: keep
+        this Region alive until the call that reads it returns."""
+        d = _lib.RegionDesc(bits=_lib.ptr(self.bits, torch.int32).value, dim=self.dim, outside_keep=int(self.outside == "keep"))
+        d.voxel_map[:] = [float(v) for v in np.asarray(self.voxel_map, dtype=np.float32).reshape(-1)]
+        d.applies[:] = self.applies_words(ins_num)
+        return d
+
 
 def label_words(labels):
     """The 4 label words of an iterable of labels in [0, 127] (a region's applies)."""
@@ -604,22 +612,9 @@ def region_contains(region, pts):
     _lib.need_cuda("region_contains", pts)
     pts = pts.reshape(-1, 3).contiguous().float()
     out = torch.empty(pts.shape[0], dtype=torch.uint8, device=pts.device)
-    get_context(pts.device).call("dmnerf_region_contains", _lib.ptr(region.bits, torch.int32), region.dim,
-                                 _lib.floats(region.voxel_map, 12), _lib.ptr(pts), pts.shape[0], _lib.ptr(out, torch.uint8))
+    desc = region.abi(MAX_LABELS - 1)                   # applies is not read here
+    get_context(pts.device).call("dmnerf_region_contains", C.byref(desc), _lib.ptr(pts), pts.shape[0], _lib.ptr(out, torch.uint8))
     return out.bool()
-
-
-def set_region(ctx, region, ins_num):
-    """Make `region` the context's region (dmnerf_set_region) for networks with ins_num; None clears it."""
-    lib = ctx.lib
-    if region is None:
-        _lib.check(lib.dmnerf_set_region(ctx.handle, None, 0, None, None, 0), "dmnerf_set_region")
-        return
-    if region.bits.device.index != ctx.index:
-        raise ValueError("region: bits live on %s, the render on cuda:%d" % (region.bits.device, ctx.index))
-    _lib.check(lib.dmnerf_set_region(ctx.handle, _lib.ptr(region.bits, torch.int32), region.dim, _lib.floats(region.voxel_map, 12),
-                                     _lib.keep_mask(region.applies_words(ins_num)), int(region.outside == "keep")),
-               "dmnerf_set_region")
 
 
 # ----------------------------------------------------------------------------------------------------------------- appearance
@@ -642,7 +637,7 @@ class Appearance:
     """An object appearance for networks with ins_num: per label, the colour map [M | b] applied to a sample's sigmoid colour c
     (c' = clamp(M c + b, 0, 1)) and the scale s >= 0 of its density (alpha = 1 - exp(-s relu(sigma) dist)).
     colour: {label: 3x4 matrix [M | b], or 3x3 M (b = 0)}; density: {label: s}.  A label without an entry keeps its look
-    (M = I, b = 0, s = 1).  `table` is the float32 [ins_num + 1, 16] table dmnerf_set_appearance takes."""
+    (M = I, b = 0, s = 1).  `table` is the float32 [ins_num + 1, 16] table of dmnerf_edit.appearance."""
 
     def __init__(self, ins_num, colour=None, density=None):
         ins_num = int(ins_num)
@@ -671,16 +666,6 @@ class Appearance:
                 raise ValueError("Appearance: the density scale of label %d must be finite and >= 0, got %r" % (k, float(s)))
             table[k, 12] = s
         self.ins_num, self.table = ins_num, table
-
-
-def set_appearance(ctx, appearance, ins_num):
-    """Make `appearance` the context's appearance (dmnerf_set_appearance) for networks with ins_num; None clears it."""
-    if appearance is None:
-        ctx.call("dmnerf_set_appearance", ctx.handle, None, 0)
-        return
-    if appearance.ins_num != ins_num:
-        raise ValueError("appearance: built for ins_num %d, the networks have ins_num %d" % (appearance.ins_num, ins_num))
-    ctx.call("dmnerf_set_appearance", ctx.handle, _lib.floats(appearance.table, appearance.table.size), ins_num + 1)
 
 
 def camera_region(poses, hwk, far):

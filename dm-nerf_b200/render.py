@@ -1,6 +1,5 @@
 """Drop-in for reference networks/render.py: `dm_nerf` (:31-96, the north_star's render_rays) and
 `render_train` (:6-28, raw2outputs), running on the fused native kernels through the C ABI."""
-import contextlib
 import ctypes as C
 
 import torch
@@ -74,55 +73,37 @@ def reference_draws(perturb, n, S, N_importance, device, t_rand=None, u=None):
     return t_rand.contiguous().float(), u.contiguous().float()
 
 
-def selection(who, keep_objects, ins_num, model_coarse, model_fine):
-    """The 4 mask words of an inference entry point's keep_objects (for io.keep with FLAG_SELECT), or None without a
-    selection."""
-    if keep_objects is None:
-        return None
-    from .objects import object_mask
-    inference_only(who, "object selection", model_coarse, model_fine)
-    return object_mask(ins_num, keep=keep_objects)
-
-
-def inference_only(who, what, model_coarse, model_fine):
-    """RuntimeError when the networks would record gradients: the scene edits (object selection, region, appearance) render
-    inference only."""
+def scene_edit(who, ins_num, device, model_coarse, model_fine, keep_objects=None, region=None, appearance=None):
+    """The scene edit of an inference entry point rendering on `device` with networks of ins_num: keep_objects (labels in
+    [0, ins_num]), region (objects.Region) and appearance (objects.Appearance) -> (a pointer to the _lib.Edit for io.edit, or
+    None without an edit; the ctypes objects it points into, which the caller holds until the native call returns).  The
+    edits render inference only: RuntimeError when the networks would record gradients.  ValueError for a region whose bits
+    live on another device or an appearance built for another ins_num."""
+    if keep_objects is None and region is None and appearance is None:
+        return None, ()
     from .autograd import _needs_grad
     if _needs_grad(model_coarse, model_fine):
-        raise RuntimeError("%s: %s is inference-only; call it under torch.no_grad() or with parameters that do not require "
-                           "grad" % (who, what))
-
-
-@contextlib.contextmanager
-def region_scope(ctx, who, region, ins_num, model_coarse, model_fine):
-    """`region` (objects.Region, or None) as the context's region for the calls inside the block; yields the flag those calls
-    add (DMNERF_FLAG_REGION, or 0 without a region).  Inference only, as object selection."""
-    if region is None:
-        yield 0
-        return
-    from .objects import set_region
-    inference_only(who, "region selection", model_coarse, model_fine)
-    set_region(ctx, region, ins_num)
-    try:
-        yield _lib.FLAG_REGION
-    finally:
-        set_region(ctx, None, ins_num)
-
-
-@contextlib.contextmanager
-def appearance_scope(ctx, who, appearance, ins_num, model_coarse, model_fine):
-    """`appearance` (objects.Appearance, or None) as the context's appearance for the calls inside the block; yields the flag
-    those calls add (DMNERF_FLAG_APPEARANCE, or 0 without one).  Inference only, as object selection."""
-    if appearance is None:
-        yield 0
-        return
-    from .objects import set_appearance
-    inference_only(who, "object appearance", model_coarse, model_fine)
-    set_appearance(ctx, appearance, ins_num)
-    try:
-        yield _lib.FLAG_APPEARANCE
-    finally:
-        set_appearance(ctx, None, ins_num)
+        raise RuntimeError("%s: a scene edit (object selection, region, appearance) is inference-only; call it under "
+                           "torch.no_grad() or with parameters that do not require grad" % who)
+    edit, held = _lib.Edit(), []
+    if keep_objects is not None:
+        from .objects import object_mask
+        keep = _lib.keep_mask(object_mask(ins_num, keep=keep_objects))
+        edit.keep = C.cast(keep, C.POINTER(C.c_uint32))
+        held.append(keep)
+    if region is not None:
+        if region.bits.device != torch.device(device):
+            raise ValueError("region: bits live on %s, the render on %s" % (region.bits.device, device))
+        desc = region.abi(ins_num)
+        edit.region = C.pointer(desc)
+        held += [desc, region.bits]
+    if appearance is not None:
+        if appearance.ins_num != ins_num:
+            raise ValueError("appearance: built for ins_num %d, the networks have ins_num %d" % (appearance.ins_num, ins_num))
+        table = _lib.floats(appearance.table, appearance.table.size)
+        edit.appearance, edit.appearance_labels = C.cast(table, C.POINTER(C.c_float)), ins_num + 1
+        held.append(table)
+    return C.pointer(edit), held
 
 
 def _check_embedders(position_embedder, view_embedder):
@@ -154,7 +135,7 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
         raise RuntimeError("dm_nerf: expected CUDA tensors (no CPU fallback)")
     ctx = get_context(dev)
     ins_num = bind_pair(ctx, model_coarse, model_fine)
-    keep = selection("render_rays", keep_objects, ins_num, model_coarse, model_fine)
+    edit, held = scene_edit("render_rays", ins_num, dev, model_coarse, model_fine, keep_objects, region, appearance)
     rays_o = rays_o.reshape(-1, 3).contiguous().float()
     rays_d = rays_d.reshape(-1, 3).contiguous().float()
     n = rays_o.shape[0]
@@ -183,12 +164,8 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     io.t_rand, io.u = _lib.ptr(t_rand), _lib.ptr(u)
     for k, v in out.items():
         setattr(io, k, _lib.ptr(v))
-    if keep is not None:
-        flags |= _lib.FLAG_SELECT
-        io.keep[:] = keep
-    with region_scope(ctx, "render_rays", region, ins_num, model_coarse, model_fine) as region_flag, \
-            appearance_scope(ctx, "render_rays", appearance, ins_num, model_coarse, model_fine) as appearance_flag:
-        ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags | region_flag | appearance_flag, impl)
+    io.edit = edit
+    ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags, impl)
     return out
 
 
@@ -287,23 +264,19 @@ def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64
     dev = torch.device(device)
     ctx = get_context(dev)
     ins_num = bind_pair(ctx, model_coarse, model_fine)
-    keep = selection("render_frame", keep_objects, ins_num, model_coarse, model_fine)
+    edit, held = scene_edit("render_frame", ins_num, torch.device("cuda", ctx.index), model_coarse, model_fine, keep_objects,
+                            region, appearance)
     begin, count = (0, H * W) if pixel_range is None else (int(pixel_range[0]), int(pixel_range[1]))
     n_ins = ins_num + 1 if keep_all_ins else ins_num
     pin = dev.type == "cuda"
     out = {"rgb": torch.empty(count, 3, pin_memory=pin), "ins": torch.empty(count, n_ins, pin_memory=pin),
            "depth": torch.empty(count, pin_memory=pin), "acc": torch.empty(count, pin_memory=pin)}
     io = _lib.RenderIO(rgb_fine=_lib.ptr(out["rgb"]), ins_fine=_lib.ptr(out["ins"]), depth_fine=_lib.ptr(out["depth"]),
-                       acc_fine=_lib.ptr(out["acc"]))
+                       acc_fine=_lib.ptr(out["acc"]), edit=edit)
     flags = _lib.FLAG_KEEP_INS if keep_all_ins else 0
-    if keep is not None:
-        flags |= _lib.FLAG_SELECT
-        io.keep[:] = keep
     Kf, Cf = _lib.camera(K, c2w)
-    with region_scope(ctx, "render_frame", region, ins_num, model_coarse, model_fine) as region_flag, \
-            appearance_scope(ctx, "render_frame", appearance, ins_num, model_coarse, model_fine) as appearance_flag:
-        ctx.call("dmnerf_render_frame_host", ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples,
-                 N_importance, flags | region_flag | appearance_flag, impl, C.byref(io))
+    ctx.call("dmnerf_render_frame_host", ctx.handle, Kf, Cf, H, W, float(near), float(far), begin, count, N_samples,
+             N_importance, flags, impl, C.byref(io))
     if pixel_range is None:
         out = {"rgb": out["rgb"].reshape(H, W, 3), "ins": out["ins"].reshape(H, W, n_ins), "depth": out["depth"].reshape(H, W),
                "acc": out["acc"].reshape(H, W)}

@@ -28,7 +28,7 @@ extern "C" {
 #define DMNERF_API
 #endif
 
-#define DMNERF_ABI_VERSION 3
+#define DMNERF_ABI_VERSION 4
 #define DMNERF_N_PARAMS 30          /* tensors in DM_NeRF.state_dict() order, networks/dm_nerf.py:65-78 */
 #define DMNERF_CH_POS 63            /* get_embedder(10): 3 + 3*2*10, networks/dm_nerf.py:41-55 */
 #define DMNERF_CH_DIR 27            /* get_embedder(4) */
@@ -55,11 +55,27 @@ extern "C" {
 #define DMNERF_FLAG_PERTURB   1     /* args.perturb > 0: t_rand and u must be given (render.py:40-47, helpers.py:135) */
 #define DMNERF_FLAG_WANT_RAW  2     /* materialise raw_coarse / raw_fine (training, penalizer.py) */
 #define DMNERF_FLAG_KEEP_INS  4     /* keep all ins_num+1 instance channels, no detach: manipulator.py:86-105 */
-#define DMNERF_FLAG_SELECT    8     /* object selection: the keep field is read (see "object selection" below) */
-#define DMNERF_FLAG_REGION   16     /* region selection: the context's region is read (see "region selection" below) */
-#define DMNERF_FLAG_APPEARANCE 32   /* object appearance: the context's appearance is read (see "object appearance" below) */
+/* The render entry points reject any other flag bit. */
 
 typedef struct dmnerf_ctx dmnerf_ctx;
+
+/* A region (see "region selection" below). */
+typedef struct dmnerf_region {
+  const uint32_t* bits;      /* DEVICE, ceil(dim^3 / 32) words; the caller keeps them alive for the call */
+  int32_t dim;
+  int32_t outside_keep;      /* 1: a sample outside the grid is kept (in the piece); 0: dropped */
+  float voxel_map[12];       /* row-major 3x4 [M | c]: network frame -> grid index */
+  uint32_t applies[4];       /* labels the region applies to, bit k of word k / 32 */
+} dmnerf_region;
+
+/* The scene edit of one render call (see "object selection", "region selection" and "object appearance" below).  An edit
+ * whose three members are all NULL is no edit. */
+typedef struct dmnerf_edit {
+  const uint32_t* keep;            /* HOST, 4 words of kept labels (bit k of word k / 32); NULL: every label */
+  const dmnerf_region* region;     /* HOST struct; NULL: no region */
+  const float* appearance;         /* HOST [appearance_labels][16]; NULL: no appearance */
+  int32_t appearance_labels;
+} dmnerf_edit;
 
 /* All per-ray inputs/outputs of one dm_nerf() call (networks/render.py:31-96).  Any output pointer
  * may be NULL (not written).  Shapes: N rays, S coarse samples, I importance samples, F = S + I,
@@ -85,7 +101,7 @@ typedef struct dmnerf_render_io {
   float* weights_fine;       /* [N,F] */
   float* raw_coarse;         /* [N,S,C] only with DMNERF_FLAG_WANT_RAW */
   float* raw_fine;           /* [N,F,C] */
-  uint32_t keep[4];          /* kept object labels with DMNERF_FLAG_SELECT (ignored without it): bit k of word k / 32 */
+  const dmnerf_edit* edit;   /* HOST: the scene edit, or NULL for none */
 } dmnerf_render_io;
 
 DMNERF_API int         dmnerf_abi_version(void);
@@ -245,7 +261,7 @@ DMNERF_API int dmnerf_composite_backward(const float* raw, const float* z, const
  * are generated on the device from K / c2w (get_rays_k, helpers.py:50-61), the shared coarse depth row from near / far
  * (z_val_sample, helpers.py:114-119), and pixels [ray_begin, ray_begin + ray_count) of the H x W frame (pixel-major, the
  * reference's reshape(-1, 3)) are rendered by dm_nerf(); every non-NULL OUTPUT field of `out_host` (host memory, ray_count
- * rows) is filled.  Of its input fields only `keep` is read (with DMNERF_FLAG_SELECT); the others are ignored.
+ * rows) is filled.  Of its input fields only `edit` is read; the others are ignored.
  * Deterministic path only (perturb = 0).  Synchronises the stream. */
 DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
                                         float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
@@ -264,8 +280,8 @@ DMNERF_API int dmnerf_mlp_forward_points(dmnerf_ctx* ctx, int net, const float* 
  * last target after the occlusion fixes.  pieces (HOST, see "moving pieces" below): NULL is the reference's exchanger.
  *
  * ---- moving pieces (DESIGN.md, "Moving pieces"; no counterpart in the original) -------------------------------------------
- * A move may carry a region (as in "region selection" below: bits, dim, voxel map, the labels it applies to, outside_keep), so
- * that only its label's samples inside that piece move.  A sample of label mv at p = o + d z (fp32, the network prologue's
+ * A move may carry a region (a dmnerf_region, as in "region selection" below), so that only its label's samples inside that
+ * piece move.  A sample of label mv at p = o + d z (fp32, the network prologue's
  * expression) is in the piece when the region does not drop it (the render kernels' per-sample test); mv must be among the
  * labels the region applies to.  A ray's accumulated label is the moving piece when it equals mv and the ray's vote is 1.
  * dmnerf_piece_vote: the votes of one fine pass: raw [N,S,C], its depths z [N,S], composite weights [N,S] and rays [N,3] ->
@@ -277,15 +293,8 @@ DMNERF_API int dmnerf_mlp_forward_points(dmnerf_ctx* ctx, int net, const float* 
  *   zeroed, 0: kept); the original's rays and depths once.  A move whose region bits are NULL takes its whole label.  Every
  *   region is checked (dim in [2, 1290], finite map, mv among its labels, non-NULL votes, rays and depths) before any launch. */
 #define DMNERF_MAX_MOVES 8
-typedef struct dmnerf_piece_region {
-  const uint32_t* bits;      /* DEVICE region bits, or NULL: no region */
-  int32_t dim;
-  int32_t outside_keep;      /* 1: a sample outside the grid is in the piece */
-  float voxel_map[12];       /* row-major 3x4 [M | c]: network frame -> grid index */
-  uint32_t applies[4];       /* labels the region applies to, bit k of word k / 32 */
-} dmnerf_piece_region;
 typedef struct dmnerf_pieces {
-  dmnerf_piece_region region[DMNERF_MAX_MOVES];
+  dmnerf_region region[DMNERF_MAX_MOVES];       /* bits NULL: the move takes its whole label */
   int32_t rest_drop[DMNERF_MAX_MOVES];
   const uint8_t* ori_vote[DMNERF_MAX_MOVES];    /* [N] DEVICE: row i of the original rays' dmnerf_piece_vote */
   const uint8_t* tar_vote[DMNERF_MAX_MOVES];    /* [N] DEVICE: target i's vote for move i */
@@ -300,7 +309,7 @@ DMNERF_API int dmnerf_exchanger(float* ori_raw, const float* const* tar_raws, co
                                 const int* move_labels, int n_moves, int64_t n, int s, int c, int64_t* ori_label,
                                 int64_t* tar_label, const dmnerf_pieces* pieces, void* stream);
 DMNERF_API int dmnerf_piece_vote(const float* raw, const float* z, const float* weights, const float* rays_o, const float* rays_d,
-                                 int64_t n, int s, int c, const int* move_labels, const dmnerf_piece_region* regions, int n_moves,
+                                 int64_t n, int s, int c, const int* move_labels, const dmnerf_region* regions, int n_moves,
                                  uint8_t* votes, void* stream);
 
 /* "Emptiness" regulariser on the per-sample object logits: emptiness_penalizer / ins_penalizer, networks/penalizer.py:5-62
@@ -332,8 +341,8 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
  * argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the exchanger's rule); a sample whose
  * label is not kept enters the composite with alpha = 0.  This applies to the coarse and the fine pass, so the coarse weights of
  * the selected scene drive the importance sampling.  raw_* (when asked for) stay the network's output.
- * dmnerf_render_forward(_host) and dmnerf_render_frame_host: io->keep with DMNERF_FLAG_SELECT (fused kernel or stage kernels,
- *   chosen as without it).
+ * dmnerf_render_forward(_host) and dmnerf_render_frame_host: io->edit->keep (fused kernel or stage kernels, chosen as without
+ *   an edit).  A region or an appearance without keep keeps every label.
  * dmnerf_composite: keep_host (HOST, labels 0 .. c - 5; raw is read, not edited), NULL = no selection.
  * dmnerf_mesh_occupancy: keep_host (HOST), NULL = no selection; with one the rule applies per grid point (occ = 0 where the
  *   point's label is not kept) and labels (DEVICE int16 [dim^3], may be NULL) receives every point's label.  labels without
@@ -444,30 +453,27 @@ DMNERF_API int dmnerf_component_groups(dmnerf_ctx* ctx, const int32_t* comp, int
                                        int16_t* groups, void* stream);
 
 /* ---- region selection (DESIGN.md, "Region selection"; no counterpart in the original) ------------------------------------
- * A region is one bit per point of a sweep grid [dim,dim,dim] (dim in [2, 1290]; point v = (i dim + j) dim + k is bit v & 31 of
- * word v >> 5, ceil(dim^3 / 32) uint32 words, the bits past dim^3 zero), the voxel map [M | c] (row-major 3x4 float32, network
- * frame -> grid index), the labels it applies to (4 words, as a keep mask) and the rule for samples outside the grid.  A render
- * sample at p = o + d z (fp32, as the network prologue computes it) with label l (argmax_sigmoid, as object selection) gets alpha
- * = 0 when l is in `applies` and either p's nearest grid point (i_a = rint(((M_a0 p0 + M_a1 p1) + M_a2 p2) + c_a), every
- * operation rounded once) is inside the grid with bit 0, or p is outside it and outside_keep is 0.  NaN and inf are outside.
- * dmnerf_set_region: the region DMNERF_FLAG_REGION reads in dmnerf_render_forward(_host) and dmnerf_render_frame_host (fused
- *   kernels or stage kernels, chosen as without it; with or without DMNERF_FLAG_SELECT).  bits_device stays the caller's and must
- *   outlive the renders; NULL clears the region.  Fails for dim out of range or a non-finite map.  A render with the flag fails
- *   when no region is set or `applies` holds a label above the bound networks' ins_num.
+ * A region (dmnerf_region) is one bit per point of a sweep grid [dim,dim,dim] (dim in [2, 1290]; point v = (i dim + j) dim + k
+ * is bit v & 31 of word v >> 5, ceil(dim^3 / 32) uint32 words, the bits past dim^3 zero), the voxel map [M | c] (row-major 3x4
+ * float32, network frame -> grid index), the labels it applies to (4 words, as a keep mask) and the rule for samples outside the
+ * grid.  A render sample at p = o + d z (fp32, as the network prologue computes it) with label l (argmax_sigmoid, as object
+ * selection) gets alpha = 0 when l is in `applies` and either p's nearest grid point (i_a = rint(((M_a0 p0 + M_a1 p1) + M_a2 p2)
+ * + c_a), every operation rounded once) is inside the grid with bit 0, or p is outside it and outside_keep is 0.  NaN and inf
+ * are outside.
+ * dmnerf_render_forward(_host) and dmnerf_render_frame_host: io->edit->region (fused kernels or stage kernels, chosen as without
+ *   an edit; with or without keep).  The render fails for NULL bits, dim out of range, a non-finite map or `applies` holding a
+ *   label above the bound networks' ins_num.
  * dmnerf_region_pack: bits (DEVICE) = for every point, the bit of its id in table (DEVICE uint32, bit id of word id / 32, over
  *   ids 0 .. n_ids - 1); an id outside [0, n_ids) (-1: no component) gives 0.  ids: DEVICE int32 [dim^3].
  * dmnerf_region_dilate: out = `radius` steps of binary dilation of in (6: face neighbours, 26: also edge and corner neighbours;
  *   never across a grid face; radius 0 copies), then the complement when invert != 0 (tail bits stay 0).  in and out are
  *   distinct DEVICE buffers.
- * dmnerf_region_contains: out [n] (DEVICE uint8) = 1 where the point pts [n,3] (DEVICE) is inside the grid and its bit is 1: the
- *   render kernels' own test. */
-DMNERF_API int dmnerf_set_region(dmnerf_ctx* ctx, const uint32_t* bits_device, int dim, const float* voxel_map12,
-                                 const uint32_t* applies_host, int outside_keep);
+ * dmnerf_region_contains: out [n] (DEVICE uint8) = 1 where the point pts [n,3] (DEVICE) is inside the grid of `region` (bits,
+ *   dim and voxel map are read) and its bit is 1: the render kernels' own test. */
 DMNERF_API int dmnerf_region_pack(const int32_t* ids, int dim, const uint32_t* table, int64_t n_ids, uint32_t* bits, void* stream);
 DMNERF_API int dmnerf_region_dilate(dmnerf_ctx* ctx, const uint32_t* in, int dim, int radius, int connectivity, int invert,
                                     uint32_t* out, void* stream);
-DMNERF_API int dmnerf_region_contains(const uint32_t* bits, int dim, const float* voxel_map12, const float* pts, int64_t n,
-                                      uint8_t* out, void* stream);
+DMNERF_API int dmnerf_region_contains(const dmnerf_region* region, const float* pts, int64_t n, uint8_t* out, void* stream);
 
 /* ---- object appearance (DESIGN.md, "Object appearance"; no counterpart in the original) -----------------------------------
  * An appearance is one row of 16 floats per label l in [0, ins_num]: the colour map [M_l | b_l] (row-major 3x4), the density
@@ -476,12 +482,10 @@ DMNERF_API int dmnerf_region_contains(const uint32_t* bits, int dim, const float
  * 0)) dist) and the colour c'_a = min(max(((M_a0 c0 + M_a1 c1) + M_a2 c2) + b_a, 0), 1) of its sigmoid colour c, every
  * operation rounded once in fp32; a dropped sample keeps alpha = 0.  Depth, acc and the instance maps use the edited weights,
  * raw_* stay the network's output, and the coarse weights of the edited scene drive the importance sampling.
- * dmnerf_set_appearance: the table DMNERF_FLAG_APPEARANCE reads in dmnerf_render_forward(_host) and dmnerf_render_frame_host
- *   (fused kernels or stage kernels, chosen as without it; with or without DMNERF_FLAG_SELECT and DMNERF_FLAG_REGION).
- *   table_host (HOST, n_labels x 16 floats) is copied on `stream` into the context, so it may be freed on return; NULL clears
- *   the appearance.  Fails for n_labels outside [2, DMNERF_MAX_INS + 1], an entry that is not finite or a negative scale.  A
- *   render with the flag fails when no appearance is set or n_labels is not the bound networks' ins_num + 1. */
-DMNERF_API int dmnerf_set_appearance(dmnerf_ctx* ctx, const float* table_host, int n_labels, void* stream);
+ * dmnerf_render_forward(_host) and dmnerf_render_frame_host: io->edit->appearance with appearance_labels rows (fused kernels or
+ *   stage kernels, chosen as without an edit; with or without keep and a region).  The table is copied on the call's stream into
+ *   the context once per call, so it may be freed on return.  The render fails for appearance_labels outside
+ *   [2, DMNERF_MAX_INS + 1] or other than the bound networks' ins_num + 1, an entry that is not finite or a negative scale. */
 
 /* ---- test-view evaluation: render_test, networks/tester.py (+ ins_eval / calculate_ap, networks/evaluator.py:77-175) -------
  * Rules and deviations: DESIGN.md, "Evaluation metrics".  Every result is deterministic (fixed-order reductions, integer atomics

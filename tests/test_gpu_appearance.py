@@ -255,31 +255,31 @@ def test_rejections_leave_the_next_render_unchanged():
     lib, st, n = ctx.lib, ctx.stream(), ro.shape[0]
     z, out = _z(wl), torch.empty(n, 3, device=DEV)
     io = _lib.RenderIO(rays_o=ro.data_ptr(), rays_d=rd.data_ptr(), z_coarse=z.data_ptr(), rgb_fine=out.data_ptr())
-    # the flag without a table
-    assert lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, _lib.FLAG_APPEARANCE, 0, st) != 0
-    assert b"without an appearance" in lib.dmnerf_last_error()
+
+    def render(table, n_labels):
+        rows = _lib.floats(table, table.size)
+        edit = _lib.Edit(appearance=C.cast(rows, C.POINTER(C.c_float)), appearance_labels=n_labels)
+        io.edit = C.pointer(edit)
+        return lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, 0, 0, st)
     good = OB.Appearance(13).table
-    # label counts outside [2, 128], NaN and inf entries, a negative scale
-    for n_labels in (1, 129):
+    # a table of 0 labels, label counts outside [2, 128], NaN and inf entries, a negative scale
+    for n_labels in (0, 1, 129):
         big = np.tile(good[:1], (max(n_labels, 1), 1))
-        assert lib.dmnerf_set_appearance(ctx.handle, _lib.floats(big, big.size), n_labels, st) != 0
+        assert render(big, n_labels) != 0
         assert b"labels outside" in lib.dmnerf_last_error()
     for i, v in ((3, float("nan")), (12, float("inf")), (14, float("nan"))):
         bad = good.copy()
         bad[5, i] = v
-        assert lib.dmnerf_set_appearance(ctx.handle, _lib.floats(bad, bad.size), 14, st) != 0
+        assert render(bad, 14) != 0
         assert b"not finite" in lib.dmnerf_last_error()
     bad = good.copy()
     bad[2, 12] = -0.5
-    assert lib.dmnerf_set_appearance(ctx.handle, _lib.floats(bad, bad.size), 14, st) != 0
+    assert render(bad, 14) != 0
     assert b"negative density scale" in lib.dmnerf_last_error()
-    # a table of the wrong length for the bound networks: accepted when set, rejected at render time
+    # a table of the wrong length for the bound networks
     short = OB.Appearance(12).table
-    assert lib.dmnerf_set_appearance(ctx.handle, _lib.floats(short, short.size), 13, st) == 0
-    assert lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, _lib.FLAG_APPEARANCE, 0, st) != 0
+    assert render(short, 13) != 0
     assert b"13 rows for 14 labels" in lib.dmnerf_last_error()
-    assert lib.dmnerf_set_appearance(ctx.handle, None, 0, st) == 0
-    assert lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, _lib.FLAG_APPEARANCE, 0, st) != 0
     with torch.no_grad(), pytest.raises(ValueError, match="ins_num 12"):
         render_rays(ro, rd, nc, nf, z, appearance=OB.Appearance(12))
     # grad mode
@@ -287,13 +287,11 @@ def test_rejections_leave_the_next_render_unchanged():
         render_rays(ro, rd, nc, nf, z, appearance=OB.Appearance(13))
     with pytest.raises(RuntimeError, match="inference-only"):
         render_frame(48, 64, wl["K"], wl["c2w"], 4.0, 15.0, nc, nf, device=DEV, appearance=OB.Appearance(13))
-    with torch.no_grad():
-        after = render_rays(ro, rd, nc, nf, _z(wl), want_raw=False, want_samples=True)
-    _equal(before, after, before.keys())
-    # the appearance is cleared after every call: the flag alone is an error again
+    # nor does a render with an appearance leave anything behind: the next render without one is the unedited result
     with torch.no_grad():
         render_rays(ro, rd, nc, nf, z, want_raw=False, appearance=OB.Appearance(13, density={1: 0.5}))
-    assert lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, _lib.FLAG_APPEARANCE, 0, st) != 0
+        after = render_rays(ro, rd, nc, nf, _z(wl), want_raw=False, want_samples=True)
+    _equal(before, after, before.keys())
     ctx.sync_check()
 
 

@@ -164,7 +164,7 @@ def test_host_entry_point_in_parts_is_bitwise_the_single_launch():
     """dmnerf_render_forward_host on >= 131 072 rays renders the batch in four parts whose copies overlap the neighbouring
     parts' kernels (second stream): same bits as the device-resident single launch, odd ray count, per-ray depth rows
     (z_row_stride != 0) and the shared row (stride 0), a small batch (single part) through the same call, an object
-    selection (io.keep with FLAG_SELECT) against dmnerf_render_forward with the same mask, and the fp16 preview network."""
+    selection (io.edit->keep) against dmnerf_render_forward with the same mask, and the fp16 preview network."""
     import ctypes as C
     from dmnerf_b200.testing import make_models
     from dmnerf_b200.engine import get_context
@@ -193,10 +193,11 @@ def test_host_entry_point_in_parts_is_bitwise_the_single_launch():
         for k, v in out.items():
             setattr(io, k, _lib.ptr(v))
         if keep is not None:
-            io.keep[:] = object_mask(13, keep=keep)
-        flags = 0 if keep is None else _lib.FLAG_SELECT
+            words = _lib.keep_mask(object_mask(13, keep=keep))
+            edit = _lib.Edit(keep=C.cast(words, C.POINTER(C.c_uint32)))
+            io.edit = C.pointer(edit)
         before = _lib.launch_count()
-        _lib.check(ctx.lib.dmnerf_render_forward_host(ctx.handle, io, n, 64, 128, flags, impl, ctx.stream()), "dmnerf_render_forward_host")
+        _lib.check(ctx.lib.dmnerf_render_forward_host(ctx.handle, io, n, 64, 128, 0, impl, ctx.stream()), "dmnerf_render_forward_host")
         launches = _lib.launch_count() - before
         assert launches == (4 if n >= 131072 else 1), launches
         with torch.no_grad():

@@ -291,10 +291,10 @@ def test_rejections(gold):
         assert call(edit) != 0
         assert len(ctx.lib.dmnerf_last_error()) > 0
     with pytest.raises(RuntimeError, match="applies"):
-        bad = _lib.PieceRegion()
+        bad = _lib.RegionDesc()
         bad.bits, bad.dim = ok.bits.data_ptr(), ok.dim
         ctx.call("dmnerf_piece_vote", _lib.ptr(raw), _lib.ptr(z), _lib.ptr(z), _lib.ptr(ro), _lib.ptr(rd), n, s, c,
-                 (C.c_int * 1)(mv), (_lib.PieceRegion * 1)(bad), 1, _lib.ptr(votes, torch.uint8))
+                 (C.c_int * 1)(mv), (_lib.RegionDesc * 1)(bad), 1, _lib.ptr(votes, torch.uint8))
     ctx.sync_check()
 
 

@@ -213,10 +213,13 @@ def test_selection_is_rejected_outside_the_labels_at_every_entry_point():
     ctx.bind(0, nc); ctx.bind(1, nf)
     n, st, lib = ro.shape[0], ctx.stream(), ctx.lib
     bad = (C.c_uint32 * 4)(1 << 14, 0, 0, 0)
+    edit = _lib.Edit(keep=C.cast(bad, C.POINTER(C.c_uint32)))
     z, out = _z(wl), torch.empty(n, 3, device=DEV)                        # every buffer a native call reads stays referenced
-    io = _lib.RenderIO(rays_o=ro.data_ptr(), rays_d=rd.data_ptr(), z_coarse=z.data_ptr(), rgb_fine=out.data_ptr(), keep=bad)
+    io = _lib.RenderIO(rays_o=ro.data_ptr(), rays_d=rd.data_ptr(), z_coarse=z.data_ptr(), rgb_fine=out.data_ptr(),
+                       edit=C.pointer(edit))
     ro_h, rd_h, z_h, out_h = ro.cpu(), rd.cpu(), z.cpu(), torch.empty(n, 3)
-    io_h = _lib.RenderIO(rays_o=ro_h.data_ptr(), rays_d=rd_h.data_ptr(), z_coarse=z_h.data_ptr(), rgb_fine=out_h.data_ptr(), keep=bad)
+    io_h = _lib.RenderIO(rays_o=ro_h.data_ptr(), rays_d=rd_h.data_ptr(), z_coarse=z_h.data_ptr(), rgb_fine=out_h.data_ptr(),
+                         edit=C.pointer(edit))
     Kf, Cf = _lib.camera(wl["K"], wl["c2w"])
     raw, z_rows = torch.rand(n, 64, 18, device=DEV), z.expand(n, 64).contiguous()
     rgb, w, depth, ins, acc = (torch.empty(n, 3, device=DEV), torch.empty(n, 64, device=DEV), torch.empty(n, device=DEV),
@@ -225,11 +228,10 @@ def test_selection_is_rejected_outside_the_labels_at_every_entry_point():
     comp_out = (rgb.data_ptr(), w.data_ptr(), depth.data_ptr(), ins.data_ptr(), acc.data_ptr(), st)
     eye = (C.c_double * 16)(*np.eye(4).reshape(-1)); ext = (C.c_double * 3)(1.9, 7.0, 7.0)
     occ, lab = torch.empty(8, 8, 8, device=DEV), torch.empty(8, 8, 8, device=DEV, dtype=torch.int16)
-    sel = _lib.FLAG_SELECT
     calls = {
-        "render_forward": lambda: lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, sel, 0, st),
-        "render_forward_host": lambda: lib.dmnerf_render_forward_host(ctx.handle, io_h, n, 64, 128, sel, 0, st),
-        "render_frame_host": lambda: lib.dmnerf_render_frame_host(ctx.handle, Kf, Cf, 48, 64, 4.0, 15.0, 0, n, 64, 128, sel, 0,
+        "render_forward": lambda: lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, 0, 0, st),
+        "render_forward_host": lambda: lib.dmnerf_render_forward_host(ctx.handle, io_h, n, 64, 128, 0, 0, st),
+        "render_frame_host": lambda: lib.dmnerf_render_frame_host(ctx.handle, Kf, Cf, 48, 64, 4.0, 15.0, 0, n, 64, 128, 0, 0,
                                                                   C.byref(io_h), st),
         "composite": lambda: lib.dmnerf_composite(*comp, bad, *comp_out),
         "mesh_occupancy": lambda: lib.dmnerf_mesh_occupancy(ctx.handle, 1, eye, ext, 8, 0.1, 0, bad, occ.data_ptr(), lab.data_ptr(), st),
@@ -238,13 +240,16 @@ def test_selection_is_rejected_outside_the_labels_at_every_entry_point():
         assert call() != 0, name
         err = lib.dmnerf_last_error()
         assert name.encode() in err and b"keeps label 14, outside [0, 13]" in err, (name, err)
-    # without DMNERF_FLAG_SELECT, io->keep is not read; a NULL mask is no selection: both are the unselected result, bit for bit
+    # without an edit (io->edit NULL, or an edit whose members are all NULL) and with a NULL mask: the unselected result, bit
+    # for bit
     with torch.no_grad():
         ref = render_rays(ro, rd, nc, nf, z, want_raw=False, want_samples=False)
-    _lib.check(lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, 0, 0, st), "dmnerf_render_forward")
-    assert torch.equal(out, ref["rgb_fine"])
-    _lib.check(lib.dmnerf_render_forward_host(ctx.handle, io_h, n, 64, 128, 0, 0, st), "dmnerf_render_forward_host")
-    assert torch.equal(out_h, ref["rgb_fine"].cpu())
+    for e in (None, C.pointer(_lib.Edit())):
+        io.edit = io_h.edit = e
+        _lib.check(lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, 0, 0, st), "dmnerf_render_forward")
+        assert torch.equal(out, ref["rgb_fine"])
+        _lib.check(lib.dmnerf_render_forward_host(ctx.handle, io_h, n, 64, 128, 0, 0, st), "dmnerf_render_forward_host")
+        assert torch.equal(out_h, ref["rgb_fine"].cpu())
     everything = _lib.keep_mask(object_mask(13, remove=[]))
     _lib.check(lib.dmnerf_composite(*comp, None, *comp_out), "dmnerf_composite")
     plain = [t.clone() for t in (rgb, w, depth, ins, acc)]

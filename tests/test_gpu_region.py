@@ -338,20 +338,34 @@ def test_rejections():
     ctx.bind(0, nc); ctx.bind(1, nf)
     lib, st, n = ctx.lib, ctx.stream(), ro.shape[0]
     z, out = _z(wl), torch.empty(n, 3, device=DEV)
+    with torch.no_grad():
+        plain = render_rays(ro, rd, nc, nf, z, want_raw=False, want_samples=False)["rgb_fine"]
     io = _lib.RenderIO(rays_o=ro.data_ptr(), rays_d=rd.data_ptr(), z_coarse=z.data_ptr(), rgb_fine=out.data_ptr())
-    assert lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, _lib.FLAG_REGION, 0, st) != 0
-    assert b"without a region" in lib.dmnerf_last_error()
-    vm = _lib.floats(OB.voxel_map(_transform(), 8), 12)
     words = torch.zeros(16, dtype=torch.int32, device=DEV)
-    every = _lib.keep_mask(OB.object_mask(13, remove=[]))
+
+    def render(desc, flags=0):
+        edit = _lib.Edit(region=C.pointer(desc))
+        io.edit = C.pointer(edit)
+        return lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, flags, 0, st)
+    good = OB.Region(words, 8, OB.voxel_map(_transform(), 8))
+    # a region without bits, dim out of range, a non-finite map, applies above ins_num (naming the label)
+    desc = good.abi(13)
+    desc.bits = None
+    assert render(desc) != 0 and b"NULL bits" in lib.dmnerf_last_error()
     for dim in (1, 1291):
-        assert lib.dmnerf_set_region(ctx.handle, C.c_void_p(words.data_ptr()), dim, vm, every, 1) != 0
-        assert b"dim" in lib.dmnerf_last_error()
-    bad_map = _lib.floats([float("nan")] + [0.0] * 11, 12)
-    assert lib.dmnerf_set_region(ctx.handle, C.c_void_p(words.data_ptr()), 8, bad_map, every, 1) != 0
-    assert b"not finite" in lib.dmnerf_last_error()
-    # applies above ins_num: rejected at render time, naming the label
+        desc = good.abi(13)
+        desc.dim = dim
+        assert render(desc) != 0 and b"dim" in lib.dmnerf_last_error()
+    desc = good.abi(13)
+    desc.voxel_map[0] = float("nan")
+    assert render(desc) != 0 and b"not finite" in lib.dmnerf_last_error()
     reg = OB.Region(words, 8, OB.voxel_map(_transform(), 8), applies=OB.label_words([2, 14]))
+    assert render(reg.abi(13)) != 0 and b"applies to label 14, outside [0, 13]" in lib.dmnerf_last_error()
+    # the flags that once selected the context's edits: rejected, not ignored
+    io.edit = None
+    for flag in (8, 16, 32):
+        assert lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, flag, 0, st) != 0
+        assert b"unknown flag" in lib.dmnerf_last_error()
     with torch.no_grad(), pytest.raises(RuntimeError, match="applies to label 14, outside \\[0, 13\\]"):
         render_rays(ro, rd, nc, nf, z, region=reg)
     with torch.no_grad(), pytest.raises(RuntimeError, match="applies to label 14"):
@@ -370,8 +384,11 @@ def test_rejections():
             OB.region_from_mask(mask, _transform(), **kw)
     assert lib.dmnerf_region_dilate(ctx.handle, C.c_void_p(words.data_ptr()), 8, -1, 26, 0, C.c_void_p(out.data_ptr()), st) != 0
     assert lib.dmnerf_region_dilate(ctx.handle, C.c_void_p(words.data_ptr()), 8, 1, 18, 0, C.c_void_p(out.data_ptr()), st) != 0
-    # the region is cleared after every call: the flag alone is an error again
-    assert lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, _lib.FLAG_REGION, 0, st) != 0
+    # a render with a region leaves nothing behind: the next render without an edit is the unselected one, bit for bit
+    _lib.check(render(good.abi(13)), "dmnerf_render_forward")
+    io.edit = None
+    _lib.check(lib.dmnerf_render_forward(ctx.handle, io, n, 64, 128, 0, 0, st), "dmnerf_render_forward")
+    assert torch.equal(out, plain)
     ctx.sync_check()
 
 

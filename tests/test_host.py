@@ -20,15 +20,15 @@ def lib():
     return _lib.load()
 
 
-def test_abi_version_3_exports_every_declared_symbol(lib):
+def test_abi_version_4_exports_every_declared_symbol(lib):
     hdr = open(os.path.join(ROOT, "include", "dmnerf_b200.h")).read()
     declared = set(re.findall(r"DMNERF_API[^;(]*?\b(dmnerf_\w+)\s*\(", hdr))
     assert len(declared) >= 14
     assert declared == set(_lib.PROTOTYPES), declared ^ set(_lib.PROTOTYPES)
     for name in declared:
         assert hasattr(lib, name)
-    assert lib.dmnerf_abi_version() == 3
-    assert ctypes.sizeof(_lib.RenderIO) == 20 * 8 + 16
+    assert lib.dmnerf_abi_version() == 4
+    assert ctypes.sizeof(_lib.RenderIO) == 20 * 8 + 8
 
 
 def test_object_selection_is_an_argument_and_the_objects_twins_are_gone(lib):
@@ -36,21 +36,46 @@ def test_object_selection_is_an_argument_and_the_objects_twins_are_gone(lib):
     exports = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
     exported = set(re.findall(r"\b(dmnerf_\w+)$", exports, re.M))
     assert exported == set(_lib.PROTOTYPES), exported ^ set(_lib.PROTOTYPES)
-    for gone in ("dmnerf_composite_objects", "dmnerf_render_forward_objects", "dmnerf_render_frame_objects_host",
-                 "dmnerf_mesh_occupancy_objects"):
+    setters = ["dmnerf_set_" + edit for edit in ("region", "appearance")]          # the context-held edits of ABI version 3
+    for gone in ["dmnerf_composite_objects", "dmnerf_render_forward_objects", "dmnerf_render_frame_objects_host",
+                 "dmnerf_mesh_occupancy_objects"] + setters:
         assert gone not in _lib.PROTOTYPES and gone not in exported and not hasattr(lib, gone), gone
         assert not re.search(r"\b%s\b" % gone, hdr), gone
-    # the selection of the render calls: io->keep, read with DMNERF_FLAG_SELECT
-    assert re.search(r"#define DMNERF_FLAG_SELECT\s+%d\b" % _lib.FLAG_SELECT, hdr)
-    assert re.search(r"uint32_t keep\[4\];\s*/\*[^*]*\*/\s*\} dmnerf_render_io;", hdr)
-    assert _lib.RenderIO.keep.offset == 20 * 8 and _lib.RenderIO.keep.size == 16
-    assert not any(_lib.RenderIO().keep)                                  # ctypes zero-fills: no selection by default
+    # the scene edit of the render calls: io->edit, the last field; the flags that once selected the context's edits are gone
+    for flag in ("SELECT", "REGION", "APPEARANCE"):
+        assert not re.search(r"\bDMNERF_FLAG_%s\b" % flag, hdr) and not hasattr(_lib, "FLAG_" + flag), flag
+    assert re.search(r"const dmnerf_edit\* edit;\s*/\*[^*]*\*/\s*\} dmnerf_render_io;", hdr)
+    assert _lib.RenderIO.edit.offset == 20 * 8 and _lib.RenderIO.edit.size == 8
+    assert not _lib.RenderIO().edit                                       # ctypes zero-fills: no edit by default
     # composite and the occupancy sweep take the 4 host words where their twins did (NULL = no selection)
     mask = ctypes.POINTER(ctypes.c_uint32)
     assert _lib.PROTOTYPES["dmnerf_composite"][1][7] is mask
     assert _lib.PROTOTYPES["dmnerf_mesh_occupancy"][1][7] is mask
     assert re.search(r"dmnerf_composite\([^;]*int keep_all_ins, const uint32_t\* keep_host, float\* rgb", hdr)
     assert re.search(r"dmnerf_mesh_occupancy\([^;]*int64_t slab, const uint32_t\* keep_host, float\* occ, int16_t\* labels", hdr)
+
+
+def test_abi_structs_match_their_ctypes_mirrors(tmp_path):
+    """The host C compiler's layout of every struct the binding mirrors (include/dmnerf_b200.h): its size and the offset of every
+    field equal the ctypes mirror's."""
+    mirrors = {"dmnerf_render_io": _lib.RenderIO, "dmnerf_edit": _lib.Edit, "dmnerf_region": _lib.RegionDesc,
+               "dmnerf_pieces": _lib.Pieces, "dmnerf_eval_result": _lib.EvalResult}
+    lines = []
+    for struct, cls in mirrors.items():
+        lines.append('  printf("%s sizeof %%zu\\n", sizeof(%s));' % (struct, struct))
+        lines += ['  printf("%s %s %%zu\\n", offsetof(%s, %s));' % (struct, f[0], struct, f[0]) for f in cls._fields_]
+    src = tmp_path / "layout.c"
+    src.write_text("#include <stddef.h>\n#include <stdio.h>\n#include \"dmnerf_b200.h\"\nint main(void) {\n%s\n  return 0;\n}\n"
+                   % "\n".join(lines))
+    exe = str(tmp_path / "layout")
+    subprocess.run(["cc", "-std=c11", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", exe], check=True)
+    got = dict((tuple(line.split()[:2]), int(line.split()[2])) for line in
+               subprocess.run([exe], capture_output=True, text=True, check=True).stdout.splitlines())
+    want = {}
+    for struct, cls in mirrors.items():
+        want[(struct, "sizeof")] = ctypes.sizeof(cls)
+        want.update({(struct, f[0]): getattr(cls, f[0]).offset for f in cls._fields_})
+    assert got == want, {k: (got.get(k), want[k]) for k in want if got.get(k) != want[k]}
 
 
 def test_calls_fail_loudly_without_gpu(lib):
