@@ -147,7 +147,8 @@ struct Program {
   int32_t ins_num;
 };
 
-// Warps 0-7: two consumer warpgroups (MMA issue, epilogues, prologue); warp 8: weight producer.
+// Warps 0-7: two consumer warpgroups (MMA issue, epilogues, prologue), CONSUMER_REGS registers each; warps 8-11: the producer
+// warpgroup at PRODUCER_REGS, of which warp 8 streams the weights.
 // SELECT (fused only): object selection -- samples whose label is not in a.keep get alpha = 0 in both composites, and so do the
 // samples a.region drops (region selection, when a.region.bits is set); with a.appearance set, every other sample's density and
 // colour go through its label's appearance row (appearance_apply).  The body is shared by mlp_umma_kernel (no selection) and
@@ -180,8 +181,11 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
     if (tid == 0) { atomicExch(&misc->abort_flag, 901); atomicCAS(a.status, 0, 901); }
   }
 
-  if (warp == 8) {
-    // =========================================================== weight producer (converged warp, one elected lane issues)
+  if (warp >= 8) {
+    // =========================================================== producer warpgroup: hands its registers to the consumers;
+    // warp 8 streams the weights (converged warp, one elected lane issues), warps 9-11 have nothing to do
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp != 8) return;
     Ring ring{0, 0};
     for (int64_t ti = 0; ti < my_tiles; ++ti) {
       const uint8_t* image = (FUSED && (ti & 3) != 0) ? a.image_fine : a.image;
@@ -201,6 +205,7 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
   }
 
   // =========================================================== consumer warpgroups
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int g = tid >> 7;                       // warpgroup: tile rows [64 g, 64 g + 64)
   const int wl = warp & 3;
   const int ra = 64 * g + 16 * wl + (lane >> 2);  // tile rows of this thread's accumulator fragment: ra, ra + 8
@@ -445,6 +450,10 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
 
     // ---------------- trunk: layers 0..7
     float dens[2] = {0.f, 0.f};
+    // The first MMA of a half-step overwrites its accumulator (scale0 = 0), but the MMA's register operands are read-write:
+    // without a definition here the accumulators of the last tile would stay live through the composite and the prologue.
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.0f;
     for (int l = 0; l < 8; ++l) {
       if (l == 0) { e_chunk(acc0, 4, true); e_chunk(acc1, 4, true); }
       else {

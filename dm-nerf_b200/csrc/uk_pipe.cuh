@@ -23,7 +23,10 @@ constexpr int B_WRGB = B_BD + 4;           // rgb_linear weights [3][128]
 constexpr int B_BRGB = B_WRGB + 3 * 128;   // rgb_linear bias (+1 pad)
 constexpr int B_TOTAL = B_BRGB + 4;
 constexpr int CONSUMERS = 256;             // two warpgroups: MMA issue, epilogues, prologue
-constexpr int N_THREADS = CONSUMERS + 32;  // + one weight-producer warp
+constexpr int N_THREADS = CONSUMERS + 128; // + the producer warpgroup (its first warp streams the weights)
+// Registers per thread after the role split (setmaxnreg): 128 x 24 + 256 x 240 = 64 512, the 168 x 384 of the launch
+constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 240;
+static_assert(128 * PRODUCER_REGS + CONSUMERS * CONSUMER_REGS <= 168 * N_THREADS, "register budget exceeds the launch's");
 // Status code of the fp16 network in the error word (KArgs::status; the protocol errors are below 1000): an activation or an
 // input exceeded the fp16 range
 constexpr int STATUS_F16_RANGE = 1001;
@@ -50,10 +53,11 @@ struct Misc {                  // lives at SM_MISC
 static_assert(sizeof(Misc) <= 3072, "Misc does not fit its shared-memory block");
 
 // ------------------------------------------------------------------------------------------------ bounded waits
-// Slow path of a barrier wait (kept out of line so the hot path is one try_wait + branch).
+// Slow path of a barrier wait.  Inline, although it is cold: with a call in the consumer body, whose accumulators are live
+// across it, ptxas fails register allocation at the CONSUMER_REGS budget (C7600).
 // On a timeout the abort flag is raised and execution simply continues: every later wait returns at once, the kernel
 // drains (with garbage results) and the host sees the status word -- no divergent early exits in the role loops.
-static __device__ __noinline__ void slow_wait(uint64_t* bar, uint32_t parity, Misc* misc, int code, int32_t* status) {
+__device__ __forceinline__ void slow_wait(uint64_t* bar, uint32_t parity, Misc* misc, int code, int32_t* status) {
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
     if (*(volatile int32_t*)&misc->abort_flag) return;

@@ -78,6 +78,14 @@ __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, uint32
 // Generic-proxy shared-memory writes (operand slabs stored by threads) made visible to the tensor core (async proxy).
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ---------------------------------------------------------------- per-warpgroup register budget
+// Every warp of a warpgroup executes the same one.  The CTA's register file is fixed at launch: a warpgroup can only grow by
+// what another one has handed back.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------- bulk async copy (TMA engine, 1-D)
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
