@@ -7,7 +7,7 @@
 #include <vector>
 
 #include "common.cuh"
-#include "umma_api.cuh"
+#include "network.cuh"
 
 namespace dmnerf {
 
@@ -24,11 +24,10 @@ void set_error(const char* fmt, ...) {
 }
 
 // An entry point's object selection: keep_host (4 host words) -> m, or every label when keep_host is NULL.  Only labels
-// 0 .. n_labels - 1 may be set; n_labels = 0 means no network is bound to label the samples with.
+// 0 .. n_labels - 1 may be set.
 static int object_mask(const uint32_t* keep_host, int n_labels, ObjMask& m, const char* who) {
   m = ObjMask{{~0u, ~0u, ~0u, ~0u}};
   if (!keep_host) return 0;
-  DMN_CHECK(n_labels > 0, "%s: an object selection needs the network(s) bound with dmnerf_set_weights (one ins_num)", who);
   for (int b = n_labels; b < 128; ++b)
     DMN_CHECK(!((keep_host[b >> 5] >> (b & 31)) & 1u), "%s: object mask keeps label %d, outside [0, %d]", who, b, n_labels - 1);
   for (int i = 0; i < 4; ++i) m.w[i] = keep_host[i];
@@ -44,8 +43,7 @@ constexpr int64_t HOST_PART_MIN_RAYS = 131072;
 
 struct dmnerf_ctx {
   int device = 0;
-  NetParams net[2];
-  UmmaWeights packed[2];          // tensor-core operand images (umma_api.cuh)
+  Network net[2];                 // 0: coarse, 1: fine (network.cuh)
   DeviceBuffer ws_raw_c, ws_raw_f, ws_z_c, ws_z_f, ws_w_c, ws_w_f;
   DeviceBuffer host_in, host_out; // device staging for the *_host entry point
   DeviceBuffer frame_rays;        // rays of the frame being rendered by dmnerf_render_frame_host
@@ -63,21 +61,34 @@ struct dmnerf_ctx {
   // *_host entry points: second stream + events so that the copies of one part of a large batch overlap the kernels of the next
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_in[HOST_PARTS] = {}, ev_done[HOST_PARTS] = {}, ev_start = nullptr;
-  dmnerf_ctx() { memset(net, 0, sizeof(net)); }
 };
+
+// The precondition of every entry point that runs a network: slot `net` bound with dmnerf_set_weights (and so packed).
+static int bound_net(const dmnerf_ctx* ctx, int net, const char* who) {
+  DMN_CHECK(ctx != nullptr, "%s: ctx is NULL", who);
+  DMN_CHECK(net == 0 || net == 1, "%s: net must be 0 (coarse) or 1 (fine), got %d", who, net);
+  DMN_CHECK(ctx->net[net].bound, "%s: bind the network with dmnerf_set_weights first", who);
+  return 0;
+}
+
+// The precondition of every render entry point: the coarse / fine pair bound with one ins_num.
+static int bound_pair(const dmnerf_ctx* ctx, const char* who) {
+  DMN_CHECK(ctx != nullptr, "%s: ctx is NULL", who);
+  DMN_CHECK(ctx->net[0].bound && ctx->net[1].bound, "%s: bind both networks with dmnerf_set_weights first", who);
+  DMN_CHECK(ctx->net[0].p.ins_num == ctx->net[1].p.ins_num, "%s: coarse/fine ins_num differ", who);
+  return 0;
+}
 
 // The flags the render entry points take.
 constexpr int RENDER_FLAGS = DMNERF_FLAG_PERTURB | DMNERF_FLAG_WANT_RAW | DMNERF_FLAG_KEEP_INS;
 
-// The scene edit of a render call, checked against the coarse / fine pair (both bound with one ins_num): in (NULL, or all three
-// members NULL: no edit) -> e and edit = &e, or edit = NULL for the unselected kernels.  The appearance table is copied on `st`
+// The scene edit of a render call, checked against the coarse / fine pair (bound_pair): in (NULL, or all three members NULL: no
+// edit) -> e and edit = &e, or edit = NULL for the unselected kernels.  The appearance table is copied on `st`
 // into the context's staging buffer.  Without a selection every label is kept (object_mask).
 static int scene_edit(dmnerf_ctx* ctx, const dmnerf_edit* in, cudaStream_t st, Edit& e, const Edit*& edit, const char* who) {
   edit = nullptr;
   if (!in || (!in->keep && !in->region && !in->appearance)) return 0;
-  const bool pair = ctx && ctx->net[0].bound && ctx->net[1].bound && ctx->net[0].ins_num == ctx->net[1].ins_num;
-  DMN_CHECK(pair, "%s: a scene edit needs the network(s) bound with dmnerf_set_weights (one ins_num)", who);
-  const int n_labels = ctx->net[0].ins_num + 1;
+  const int n_labels = ctx->net[0].p.ins_num + 1;
   if (object_mask(in->keep, n_labels, e.keep, who)) return 1;
   e.region = Region{};
   if (in->region) {
@@ -132,7 +143,6 @@ DMNERF_API int dmnerf_ctx_create(int device, dmnerf_ctx** out) {
 DMNERF_API int dmnerf_ctx_destroy(dmnerf_ctx* ctx) {
   if (!ctx) return 0;
   cudaSetDevice(ctx->device);
-  for (int i = 0; i < 2; ++i) umma_weights_free(ctx->packed[i]);
   for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_in) if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_done) if (e) cudaEventDestroy(e);
@@ -149,15 +159,15 @@ DMNERF_API int dmnerf_set_weights(dmnerf_ctx* ctx, int net, const float* const* 
             DMNERF_N_PARAMS, n_params);
   DMN_CHECK(ins_num >= 1 && ins_num <= DMNERF_MAX_INS, "set_weights: ins_num=%d out of range [1,%d]", ins_num,
             DMNERF_MAX_INS);
-  NetParams& p = ctx->net[net];
+  DMN_CHECK(params != nullptr, "set_weights: params is NULL");
+  for (int i = 0; i < DMNERF_N_PARAMS; ++i) DMN_CHECK(params[i], "set_weights: parameter %d is NULL", i);
+  NetParams p;
   for (int l = 0; l < N_LAYERS; ++l) {
-    DMN_CHECK(params[2 * l] && params[2 * l + 1], "set_weights: parameter %d is NULL", 2 * l);
     p.w[l] = params[2 * l];
     p.b[l] = params[2 * l + 1];
   }
   p.ins_num = ins_num;
-  p.bound = true;
-  return umma_weights_pack(ctx->packed[net], p, (cudaStream_t)stream);
+  return ctx->net[net].bind(p, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_posenc(const float* x, int64_t m, int n_freqs, float* out, void* stream) {
@@ -166,54 +176,48 @@ DMNERF_API int dmnerf_posenc(const float* x, int64_t m, int n_freqs, float* out,
   return launch_posenc(x, m, n_freqs, out, (cudaStream_t)stream);
 }
 
-// The fp16 network of slot `net`: its image is packed on the first fp16 call after every dmnerf_set_weights.
-static int prepare_f16(dmnerf_ctx* ctx, int net, cudaStream_t st) {
-  DMN_CHECK(umma_available(ctx->packed[net]), "DMNERF_IMPL_UMMA_F16: bind the network with dmnerf_set_weights first");
-  return umma_weights_pack_f16(ctx->packed[net], ctx->net[net], st);
-}
-
 // An fp16 call on caller buffers returns only after its range verdict: synchronise and report (never silent inf / NaN maps).
 // A call that failed before its verdict still drains its kernels and drops their verdict: their results are not returned.
 static int f16_verdict(dmnerf_ctx* ctx, int rc, int impl, void* stream) {
   if (impl != DMNERF_IMPL_UMMA_F16) return rc;
   if (rc) {
     cudaStreamSynchronize((cudaStream_t)stream);
-    for (int i = 0; i < 2; ++i) umma_take_f16_range(ctx->packed[i]);
+    for (const Network& n : ctx->net) n.take_f16_range();
     return rc;
   }
   return dmnerf_sync_check(ctx, stream);
 }
 
-// The network a call on slots net0 .. net1 runs: impl range-checked, DMNERF_IMPL_AUTO resolved to the tensor-core kernel when
-// every slot has its image (else SIMT), and for DMNERF_IMPL_UMMA_F16 every slot's fp16 image packed.
+// The network a call on the bound slots net0 .. net1 runs: impl range-checked, DMNERF_IMPL_AUTO resolved to the tensor-core
+// kernel (a bound slot always has its image), and for DMNERF_IMPL_UMMA_F16 every slot's fp16 image packed.
 static int resolve_impl(dmnerf_ctx* ctx, int& impl, int net0, int net1, cudaStream_t st, const char* who) {
   DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA_F16, "%s: unknown impl %d", who, impl);
-  if (impl == DMNERF_IMPL_AUTO)
-    impl = umma_available(ctx->packed[net0]) && umma_available(ctx->packed[net1]) ? DMNERF_IMPL_UMMA : DMNERF_IMPL_SIMT;
+  if (impl == DMNERF_IMPL_AUTO) impl = DMNERF_IMPL_UMMA;
   for (int net = net0; impl == DMNERF_IMPL_UMMA_F16 && net <= net1; ++net)
-    if (prepare_f16(ctx, net, st)) return 1;
+    if (ctx->net[net].pack_f16(st)) return 1;
   return 0;
 }
 
+// The network of the bound slot `net` on m rows.
 static int mlp_dispatch(dmnerf_ctx* ctx, int net, const float* x, const float* ro, const float* rd, const float* z,
                         int64_t m, int s, float* out, int impl, cudaStream_t st) {
-  DMN_CHECK(ctx != nullptr, "mlp: ctx is NULL");
-  DMN_CHECK(net == 0 || net == 1, "mlp: net must be 0 or 1");
   DMN_CHECK(m >= 0, "mlp: negative row count");
   if (m == 0) return 0;
   DMN_CHECK(out != nullptr, "mlp: out is NULL");
   if (resolve_impl(ctx, impl, net, net, st, "mlp")) return 1;
-  if (impl == DMNERF_IMPL_SIMT) return launch_mlp_simt(ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st);
-  return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st, impl == DMNERF_IMPL_UMMA_F16);
+  if (impl == DMNERF_IMPL_SIMT) return launch_mlp_simt(ctx->net[net].p, x, ro, rd, z, m, s, out, nullptr, st);
+  return launch_mlp_tc(ctx->net[net], x, ro, rd, z, m, s, out, nullptr, st, impl == DMNERF_IMPL_UMMA_F16);
 }
 
 DMNERF_API int dmnerf_mlp_forward(dmnerf_ctx* ctx, int net, const float* x, int64_t m, float* out, int impl, void* stream) {
+  if (bound_net(ctx, net, "mlp_forward")) return 1;
   DMN_CHECK(m <= 0 || x != nullptr, "mlp_forward: x is NULL");
   return f16_verdict(ctx, mlp_dispatch(ctx, net, x, nullptr, nullptr, nullptr, m, 1, out, impl, (cudaStream_t)stream), impl, stream);
 }
 
 DMNERF_API int dmnerf_mlp_forward_rays(dmnerf_ctx* ctx, int net, const float* rays_o, const float* rays_d, const float* z,
                             int64_t n, int s, float* out, int impl, void* stream) {
+  if (bound_net(ctx, net, "mlp_forward_rays")) return 1;
   DMN_CHECK(n >= 0 && s >= 1, "mlp_forward_rays: bad sizes n=%lld s=%d", (long long)n, s);
   DMN_CHECK(n == 0 || (rays_o && rays_d && z), "mlp_forward_rays: NULL input");
   return f16_verdict(ctx, mlp_dispatch(ctx, net, nullptr, rays_o, rays_d, z, n * s, s, out, impl, (cudaStream_t)stream), impl,
@@ -222,15 +226,14 @@ DMNERF_API int dmnerf_mlp_forward_rays(dmnerf_ctx* ctx, int net, const float* ra
 
 DMNERF_API int dmnerf_mlp_forward_points(dmnerf_ctx* ctx, int net, const float* pts, const float* viewdirs, int64_t m, float* out,
                                          int impl, void* stream) {
-  DMN_CHECK(ctx != nullptr && (net == 0 || net == 1), "mlp_forward_points: bad ctx / net");
+  if (bound_net(ctx, net, "mlp_forward_points")) return 1;
   DMN_CHECK(m >= 0, "mlp_forward_points: negative point count");
   DMN_CHECK(m == 0 || (pts && viewdirs && out), "mlp_forward_points: NULL buffer");
   DMN_CHECK(impl != DMNERF_IMPL_SIMT, "mlp_forward_points: the point query runs on the tensor-core kernel only");
   if (m == 0) return 0;
-  DMN_CHECK(umma_available(ctx->packed[net]), "mlp_forward_points: bind the network with dmnerf_set_weights first");
   if (resolve_impl(ctx, impl, net, net, (cudaStream_t)stream, "mlp_forward_points")) return 1;
-  return f16_verdict(ctx, launch_mlp_umma(ctx->packed[net], ctx->net[net], nullptr, pts, viewdirs, nullptr, m, 1, out, nullptr,
-                                          (cudaStream_t)stream, impl == DMNERF_IMPL_UMMA_F16), impl, stream);
+  return f16_verdict(ctx, launch_mlp_tc(ctx->net[net], nullptr, pts, viewdirs, nullptr, m, 1, out, nullptr, (cudaStream_t)stream,
+                                        impl == DMNERF_IMPL_UMMA_F16), impl, stream);
 }
 
 DMNERF_API int dmnerf_composite(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c, int keep_all_ins,
@@ -355,26 +358,24 @@ DMNERF_API int64_t dmnerf_mlp_backward_scratch_floats(int64_t m) { return (int64
 
 DMNERF_API int dmnerf_mlp_forward_train(dmnerf_ctx* ctx, int net, const float* x, const float* rays_o, const float* rays_d,
                                         const float* z, int64_t m, int s, float* out, float* acts, int impl, void* stream) {
-  DMN_CHECK(ctx != nullptr, "mlp_forward_train: ctx is NULL");
-  DMN_CHECK(net == 0 || net == 1, "mlp_forward_train: net must be 0 or 1");
+  if (bound_net(ctx, net, "mlp_forward_train")) return 1;
   DMN_CHECK(m >= 0 && s >= 1, "mlp_forward_train: bad sizes");
   if (m == 0) return 0;
   DMN_CHECK(out && acts, "mlp_forward_train: out / acts is NULL");
   DMN_CHECK(impl != DMNERF_IMPL_UMMA_F16, "mlp_forward_train: DMNERF_IMPL_UMMA_F16 is inference-only; training runs the exact "
             "network (DMNERF_IMPL_UMMA or DMNERF_IMPL_SIMT)");
   if (resolve_impl(ctx, impl, net, net, (cudaStream_t)stream, "mlp_forward_train")) return 1;
-  if (impl == DMNERF_IMPL_SIMT) return launch_mlp_simt(ctx->net[net], x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
-  return launch_mlp_umma(ctx->packed[net], ctx->net[net], x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
+  if (impl == DMNERF_IMPL_SIMT) return launch_mlp_simt(ctx->net[net].p, x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
+  return launch_mlp_tc(ctx->net[net], x, rays_o, rays_d, z, m, s, out, acts, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_mlp_backward(dmnerf_ctx* ctx, int net, float* acts, const float* d_out, int64_t m, float* const* grads,
                                    float* scratch, int flags, void* stream) {
-  DMN_CHECK(ctx != nullptr, "mlp_backward: ctx is NULL");
-  DMN_CHECK(net == 0 || net == 1, "mlp_backward: net must be 0 or 1");
+  if (bound_net(ctx, net, "mlp_backward")) return 1;
   DMN_CHECK(m >= 0 && grads, "mlp_backward: bad arguments");
   DMN_CHECK(m == 0 || (acts && d_out && scratch), "mlp_backward: NULL buffer");
-  return launch_mlp_backward(ctx->net[net], ctx->packed[net], acts, d_out, m, grads, scratch, flags, ctx->gemm_wimage,
-                             ctx->gemm_partial, (cudaStream_t)stream);
+  return launch_mlp_backward(ctx->net[net], acts, d_out, m, grads, scratch, flags, ctx->gemm_wimage, ctx->gemm_partial,
+                             (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_composite_backward(const float* raw, const float* z, const float* rays_d, int64_t n, int s, int c,
@@ -416,20 +417,19 @@ DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, 
 
 }  // extern "C"
 
-// dm_nerf() on device buffers; edit: the checked scene edit, or NULL for none (the unselected kernels)
+// dm_nerf() on device buffers with the bound pair (bound_pair); edit: the checked scene edit, or NULL for none (the
+// unselected kernels)
 static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
                                const Edit* edit, void* stream) {
-  DMN_CHECK(ctx && io, "render_forward: NULL ctx/io");
+  DMN_CHECK(io, "render_forward: io is NULL");
   DMN_CHECK(n >= 0 && S >= 3 && NI >= 2, "render_forward: bad sizes n=%lld S=%d I=%d", (long long)n, S, NI);
-  DMN_CHECK(ctx->net[0].bound && ctx->net[1].bound, "render_forward: bind both networks with dmnerf_set_weights first");
-  DMN_CHECK(ctx->net[0].ins_num == ctx->net[1].ins_num, "render_forward: coarse/fine ins_num differ");
   if (n == 0) return 0;
   DMN_CHECK(io->rays_o && io->rays_d && io->z_coarse, "render_forward: rays_o / rays_d / z_coarse is NULL");
   const bool perturb = (flags & DMNERF_FLAG_PERTURB) != 0;
   DMN_CHECK(!perturb || (io->t_rand && io->u), "render_forward: PERTURB needs t_rand and u");
   DMN_CHECK(io->z_row_stride == 0 || io->z_row_stride >= S, "render_forward: bad z_row_stride");
   cudaStream_t st = (cudaStream_t)stream;
-  const int C = 4 + ctx->net[0].ins_num + 1, F = S + NI;
+  const int C = 4 + ctx->net[0].p.ins_num + 1, F = S + NI;
   const int keep_ins = (flags & DMNERF_FLAG_KEEP_INS) ? 1 : 0;
   DMN_CUDA(cudaSetDevice(ctx->device));
   if (resolve_impl(ctx, impl, 0, 1, st, "render_forward")) return 1;
@@ -438,7 +438,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   if (impl != DMNERF_IMPL_SIMT && S == 64 && NI == 128 && !io->raw_coarse && !io->raw_fine) {
     const bool prof = ctx->profiling;
     if (prof) DMN_CUDA(cudaEventRecord(ctx->ev[0], st));
-    int rc = launch_render_umma(ctx->packed[0], ctx->packed[1], io, n, flags, st, edit, impl == DMNERF_IMPL_UMMA_F16);
+    int rc = launch_render_tc(ctx->net[0], ctx->net[1], io, n, flags, st, edit, impl == DMNERF_IMPL_UMMA_F16);
     if (rc) return rc;
     if (prof) for (int i = 1; i <= DMNERF_N_STAGES; ++i) DMN_CUDA(cudaEventRecord(ctx->ev[i], st));
     ctx->profile_valid = prof;
@@ -491,6 +491,7 @@ extern "C" {
 
 DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
                           void* stream) {
+  if (bound_pair(ctx, "render_forward")) return 1;
   DMN_CHECK(!(flags & ~RENDER_FLAGS), "render_forward: unknown flag bits 0x%x", flags & ~RENDER_FLAGS);
   Edit e;
   const Edit* edit;
@@ -504,11 +505,9 @@ DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
   DMN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
   // fp16 range verdicts: taken from both weight sets (the stage path's coarse and fine networks each have an error word), so
   // that none is left behind for a later call, then reported after any protocol error
-  const bool range0 = umma_take_f16_range(ctx->packed[0]), range1 = umma_take_f16_range(ctx->packed[1]);
-  for (int i = 0; i < 2; ++i) {
-    int rc = umma_check_status(ctx->packed[i], (cudaStream_t)stream);
-    if (rc) return rc;
-  }
+  const bool range0 = ctx->net[0].take_f16_range(), range1 = ctx->net[1].take_f16_range();
+  for (const Network& n : ctx->net)
+    if (int rc = n.check_status((cudaStream_t)stream)) return rc;
   DMN_CHECK(!range0 && !range1, "fp16 network: an activation exceeded the fp16 range (> 65504), so these results are invalid; "
             "render with the exact network (DMNERF_IMPL_UMMA)");
   return 0;
@@ -536,20 +535,19 @@ DMNERF_API int dmnerf_profile_read(dmnerf_ctx* ctx, float* ms_out, int n_out) {
 
 }  // extern "C"
 
-// Host-buffer render: `h` holds HOST pointers for the outputs (and for the inputs unless dev_rays_o / dev_rays_d are given:
-// rays that are already resident on the device, e.g. generated there from the camera).  edit: as for render_forward_impl, its
-// appearance table already on the device, so that every part reads the one copy.
+// Host-buffer render with the bound pair (bound_pair): `h` holds HOST pointers for the outputs (and for the inputs unless
+// dev_rays_o / dev_rays_d are given: rays that are already resident on the device, e.g. generated there from the camera).
+// edit: as for render_forward_impl, its appearance table already on the device, so that every part reads the one copy.
 static int render_host_impl(dmnerf_ctx* ctx, const dmnerf_render_io* h, const float* dev_rays_o, const float* dev_rays_d, int64_t n,
                             int S, int NI, int flags, int impl, const Edit* edit, void* stream) {
-  DMN_CHECK(ctx && h, "render_forward_host: NULL ctx/io");
+  DMN_CHECK(h, "render_forward_host: io is NULL");
   DMN_CHECK(n >= 0, "render_forward_host: negative ray count");
   if (n == 0) return 0;
   const bool dev_rays = dev_rays_o != nullptr && dev_rays_d != nullptr;
   DMN_CHECK((dev_rays || (h->rays_o && h->rays_d)) && h->z_coarse, "render_forward_host: rays_o / rays_d / z_coarse is NULL");
-  DMN_CHECK(ctx->net[0].bound && ctx->net[1].bound, "render_forward_host: bind both networks first");
   cudaStream_t st = (cudaStream_t)stream;
   DMN_CUDA(cudaSetDevice(ctx->device));
-  const int ins = ctx->net[0].ins_num, C = 4 + ins + 1, F = S + NI;
+  const int ins = ctx->net[0].p.ins_num, C = 4 + ins + 1, F = S + NI;
   const int n_ins_out = (flags & DMNERF_FLAG_KEEP_INS) ? ins + 1 : ins;
   const bool perturb = (flags & DMNERF_FLAG_PERTURB) != 0;
   const size_t zin = (h->z_row_stride == 0) ? (size_t)S : (size_t)n * h->z_row_stride;
@@ -676,6 +674,7 @@ extern "C" {
 
 DMNERF_API int dmnerf_render_forward_host(dmnerf_ctx* ctx, const dmnerf_render_io* h, int64_t n, int S, int NI, int flags,
                                int impl, void* stream) {
+  if (bound_pair(ctx, "render_forward_host")) return 1;
   DMN_CHECK(!(flags & ~RENDER_FLAGS), "render_forward_host: unknown flag bits 0x%x", flags & ~RENDER_FLAGS);
   Edit e;
   const Edit* edit;
@@ -686,7 +685,8 @@ DMNERF_API int dmnerf_render_forward_host(dmnerf_ctx* ctx, const dmnerf_render_i
 DMNERF_API int dmnerf_render_frame_host(dmnerf_ctx* ctx, const float* K_host, const float* c2w_host, int H, int W, float near_z,
                                         float far_z, int64_t ray_begin, int64_t ray_count, int n_coarse, int n_importance,
                                         int flags, int impl, const dmnerf_render_io* out_host, void* stream) {
-  DMN_CHECK(ctx && K_host && c2w_host && out_host, "render_frame_host: NULL argument");
+  if (bound_pair(ctx, "render_frame_host")) return 1;
+  DMN_CHECK(K_host && c2w_host && out_host, "render_frame_host: NULL argument");
   DMN_CHECK(!(flags & ~RENDER_FLAGS), "render_frame_host: unknown flag bits 0x%x", flags & ~RENDER_FLAGS);
   Edit e;
   const Edit* edit;
@@ -728,19 +728,18 @@ DMNERF_API int dmnerf_mesh_grid_points(const double* transform_host, const doubl
 DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
                                      float voxel, int64_t slab, const uint32_t* keep_host, float* occ, int16_t* labels,
                                      void* stream) {
-  DMN_CHECK(ctx && (net == 0 || net == 1), "mesh_occupancy: bad ctx / net");
+  if (bound_net(ctx, net, "mesh_occupancy")) return 1;
   DMN_CHECK(transform_host && extents_host && occ, "mesh_occupancy: NULL argument");
   DMN_CHECK(dim >= 2 && dim <= 2048, "mesh_occupancy: dim %d out of range [2, 2048]", dim);
   DMN_CHECK(keep_host || !labels, "mesh_occupancy: labels are written by the selected sweep only (pass keep_host)");
   ObjMask keep;
-  if (object_mask(keep_host, ctx->net[net].bound ? ctx->net[net].ins_num + 1 : 0, keep, "mesh_occupancy")) return 1;
-  DMN_CHECK(umma_available(ctx->packed[net]), "mesh_occupancy: bind the network with dmnerf_set_weights first");
+  if (object_mask(keep_host, ctx->net[net].p.ins_num + 1, keep, "mesh_occupancy")) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   DMN_CUDA(cudaSetDevice(ctx->device));
   const int64_t n = (int64_t)dim * dim * dim;
   if (slab <= 0) slab = (int64_t)1 << 20;
   if (slab > n) slab = n;
-  const int C = 4 + ctx->net[net].ins_num + 1;
+  const int C = 4 + ctx->net[net].p.ins_num + 1;
   float *pts, *raw;
   if (ctx->mesh_pts.get((size_t)slab * 6, &pts) || ctx->mesh_raw.get((size_t)slab * C, &raw)) return 2;
   float* dirs = pts + slab * 3;                                   // mesh_generator.py:42: zero view directions
@@ -749,7 +748,7 @@ DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* tra
   for (int64_t b = 0; b < n; b += slab) {
     const int64_t cnt = n - b < slab ? n - b : slab;
     int rc = launch_grid_points(transform_host, extents_host, dim, b, cnt, pts, st);
-    if (!rc) rc = launch_mlp_umma(ctx->packed[net], ctx->net[net], nullptr, pts, dirs, nullptr, cnt, 1, raw, nullptr, st);
+    if (!rc) rc = launch_mlp_tc(ctx->net[net], nullptr, pts, dirs, nullptr, cnt, 1, raw, nullptr, st);
     if (!rc) rc = keep_host ? launch_occupancy_objects(raw, cnt, C, voxel, keep, occ + b, labels ? labels + b : nullptr, st)
                             : launch_occupancy(raw, cnt, C, voxel, occ + b, st);
     if (rc) return rc;

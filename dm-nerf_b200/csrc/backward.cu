@@ -9,7 +9,7 @@
 //     reference's (dm_nerf.py:95: the instance branch reads h.detach(), so it contributes to ins_feature_linear and below only).
 
 #include "ray_ops.cuh"
-#include "umma_api.cuh"
+#include "network.cuh"
 
 namespace dmnerf {
 
@@ -410,9 +410,9 @@ static int small_tn(const float* A, int lda, const float* B, int ldb, float* C, 
 //     dW_rgb_hid[:, :256] = P W_rf^T + c1 (x) b_rf,  dW_rgb_feat = W_rh[:, :256]^T P,  db_rgb_feat = W_rh[:, :256]^T c1   (c1 = colsum S1)
 //     (rgb_feat = h7 W_rf^T + b_rf is never materialised; same for the instance branch with Q, c2)
 // Every sum over the samples runs in a fixed order, so the 30 gradients are reproducible bit for bit from run to run.
-static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, float* acts, const float* d_out, int64_t m,
-                              float* const* grads, float* scratch, bool masks_saved, DeviceBuffer& wimage, DeviceBuffer& partial,
-                              cudaStream_t st) {
+static int mlp_backward_chain(const Network& net, float* acts, const float* d_out, int64_t m, float* const* grads, float* scratch,
+                              bool masks_saved, DeviceBuffer& wimage, DeviceBuffer& partial, cudaStream_t st) {
+  const NetParams& p = net.p;
   const int ins1 = p.ins_num + 1, C = 4 + ins1;
   const ActPlanes ap = act_planes(acts, m);
   float* S12 = scratch;                               // d rgb_hid | d ins_hid  [m,256]
@@ -434,7 +434,7 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
   // (launch_gemm_tn_tc_batch) -- 3 GEMM + 3 reduction launches per network instead of 14 + 14.
   struct Queue { TnProblem p[TN_MAX_BATCH]; int n = 0, N = 0; } q_wide, q_in256, q_in128;      // [256 x 256], [256 x <=64], [128 x <=64]
   auto flush = [&](Queue& q) -> int {
-    const int r = q.n ? launch_gemm_tn_tc_batch(q.p, q.n, m, q.N, partial, umma_status_word(packed), st) : 0;
+    const int r = q.n ? launch_gemm_tn_tc_batch(q.p, q.n, m, q.N, partial, net.status.device(), st) : 0;
     q.n = 0;
     return r;
   };
@@ -464,7 +464,7 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
   const float* d_sig = d_out + 3;
   const float* d_ins = d_out + 4;
   R(launch_bwd_heads(p, d_out, m, ap.bits, S12, st));
-  R(launch_bwd_chain(packed, p, S12, d_out, ap, m, dY, wimage, st));
+  R(launch_bwd_chain(net, S12, d_out, ap, m, dY, wimage, st));
   // ---- folded head layers (dm_nerf.py:89-99): one product against h7 for both branches; trunk (dm_nerf.py:83-87)
   R(dW(S12, 256, ap.h[7], 256, PQ, 256, 256, 256, c12));
   for (int l = 7; l >= 1; --l) R(dW(dY[l], 256, ap.h[l - 1], 256, gw(l), layer_in(l), 256, 256, gb(l)));
@@ -498,19 +498,17 @@ static int mlp_backward_chain(const NetParams& p, const UmmaWeights& packed, flo
 }
 
 // grads: 30 device pointers in state_dict order (weight, bias per layer); overwritten with the gradient of this call.
-int launch_mlp_backward(const NetParams& p, const UmmaWeights& packed, float* acts, const float* d_out, int64_t m, float* const* grads,
-                        float* scratch, int flags, DeviceBuffer& wimage, DeviceBuffer& partial, cudaStream_t st) {
-  DMN_CHECK(p.bound, "mlp_backward: weights not bound");
-  DMN_CHECK(umma_available(packed), "mlp_backward: weights not packed (call dmnerf_set_weights first)");
+int launch_mlp_backward(const Network& net, float* acts, const float* d_out, int64_t m, float* const* grads, float* scratch, int flags,
+                        DeviceBuffer& wimage, DeviceBuffer& partial, cudaStream_t st) {
   const bool prezeroed = (flags & 2) != 0;      // flags: bit 0 = the forward wrote the ReLU bit planes, bit 1 = grads already zero
   for (int l = 0; l < N_LAYERS; ++l) {
     DMN_CHECK(grads[2 * l] && grads[2 * l + 1], "mlp_backward: gradient buffer %d is NULL", 2 * l);
     if (prezeroed) continue;
-    DMN_CUDA(cudaMemsetAsync(grads[2 * l], 0, (size_t)layer_out(l, p.ins_num) * layer_in(l) * sizeof(float), st));
-    DMN_CUDA(cudaMemsetAsync(grads[2 * l + 1], 0, (size_t)layer_out(l, p.ins_num) * sizeof(float), st));
+    DMN_CUDA(cudaMemsetAsync(grads[2 * l], 0, (size_t)layer_out(l, net.p.ins_num) * layer_in(l) * sizeof(float), st));
+    DMN_CUDA(cudaMemsetAsync(grads[2 * l + 1], 0, (size_t)layer_out(l, net.p.ins_num) * sizeof(float), st));
   }
   if (m == 0) return 0;
-  return mlp_backward_chain(p, packed, acts, d_out, m, grads, scratch, (flags & 1) != 0, wimage, partial, st);
+  return mlp_backward_chain(net, acts, d_out, m, grads, scratch, (flags & 1) != 0, wimage, partial, st);
 }
 
 }  // namespace dmnerf

@@ -9,7 +9,7 @@
 #include <cstring>
 
 #include "common.cuh"
-#include "umma_api.cuh"
+#include "network.cuh"
 
 namespace dmnerf {
 namespace bk {
@@ -152,16 +152,16 @@ int launch_bwd_heads(const NetParams& p, const float* d_out, int64_t m, const ui
 }
 
 // dY(7..0) of one network from d rgb_hid (s1, row stride 256) and d sigma (column 3 of d_out).  dy: 8 planes [m,256].
-int launch_bwd_chain(const UmmaWeights& w, const NetParams& p, const float* s1, const float* d_out, const ActPlanes& ap, int64_t m,
-                     float* const* dy, DeviceBuffer& wimage, cudaStream_t st) {
-  DMN_CHECK(w.ready && w.extra, "bwd_chain: weights not packed (call dmnerf_set_weights first)");
+int launch_bwd_chain(const Network& net, const float* s1, const float* d_out, const ActPlanes& ap, int64_t m, float* const* dy,
+                     DeviceBuffer& wimage, cudaStream_t st) {
   if (m == 0) return 0;
+  const NetParams& p = net.p;
   const int C = 4 + p.ins_num + 1;
   bk::dsig_outer_kernel<<<(unsigned)((m * 64 + 255) / 256), 256, 0, st>>>(d_out, C, p.w[L_DENSITY], m, dy[7]);
   DMN_LAUNCH_OK();
   auto bits = [&](int plane) { return ap.bits + (int64_t)plane * ACT_BITS_GROUPS * m; };
-  int32_t* status = umma_status_word(w);
-  int rc = launch_gemm_nn_tc(s1, 256, umma_fold_w_rgb(w), 283, dy[7], 256, m, 128, 1, bits(7), wimage, status, st);
+  int32_t* status = net.status.device();
+  int rc = launch_gemm_nn_tc(s1, 256, net.fold_w_rgb.data<float>(), 283, dy[7], 256, m, 128, 1, bits(7), wimage, status, st);
   for (int l = 7; l >= 1 && rc == 0; --l)
     rc = launch_gemm_nn_tc(dy[l], 256, p.w[l], layer_in(l), dy[l - 1], 256, m, 256, 0, bits(l - 1), wimage, status, st);
   return rc;

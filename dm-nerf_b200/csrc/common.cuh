@@ -35,7 +35,6 @@ struct NetParams {
   const float* w[N_LAYERS];
   const float* b[N_LAYERS];
   int ins_num;
-  bool bound;
 };
 
 __host__ __device__ inline int layer_out(int l, int ins_num) {
@@ -131,6 +130,8 @@ class DeviceBuffer {
     *out = static_cast<T*>(ptr_);
     return 0;
   }
+  template <class T>
+  T* data() const { return static_cast<T*>(ptr_); }   // what the last get() returned
 
  private:
   void* ptr_ = nullptr;
@@ -210,18 +211,18 @@ int launch_composite_backward(const float* raw, const float* z, const float* ray
 // flags: bit 0 = the forward that filled `acts` wrote the ReLU bit planes (tensor-core kernel; otherwise the backward derives
 // them from the saved activations first), bit 1 = grads are already zero.  wimage / partial: the scratch of the tensor-core
 // GEMMs (launch_gemm_nn_tc / launch_gemm_tn_tc_batch).
-struct UmmaWeights;
-int launch_mlp_backward(const NetParams& p, const UmmaWeights& packed, float* acts, const float* d_out, int64_t m, float* const* grads,
-                        float* scratch, int flags, DeviceBuffer& wimage, DeviceBuffer& partial, cudaStream_t st);
+struct Network;
+int launch_mlp_backward(const Network& net, float* acts, const float* d_out, int64_t m, float* const* grads, float* scratch, int flags,
+                        DeviceBuffer& wimage, DeviceBuffer& partial, cudaStream_t st);
 // Gradient chain (bwd_chain.cu)
 int launch_mask_bits(float* acts, int64_t m, cudaStream_t st);
 int launch_bwd_heads(const NetParams& p, const float* d_out, int64_t m, const uint16_t* bits, float* s12, cudaStream_t st);
-int launch_bwd_chain(const UmmaWeights& w, const NetParams& p, const float* s1, const float* d_out, const ActPlanes& ap, int64_t m,
-                     float* const* dy, DeviceBuffer& wimage, cudaStream_t st);
+int launch_bwd_chain(const Network& net, const float* s1, const float* d_out, const ActPlanes& ap, int64_t m, float* const* dy,
+                     DeviceBuffer& wimage, cudaStream_t st);
 size_t mlp_backward_scratch_floats(int64_t m);
 
 // Tensor-core GEMMs of the backward (gemm_umma.cu): split-bf16 three-pass wgmma kernels for the wide layer shapes.  A kernel that
-// gives up on a barrier writes its code (6xx) to `status`, the error word of the weight set being differentiated.
+// gives up on a barrier writes its code (6xx) to `status`, the error word of the network being differentiated.
 bool gemm_tn_tc_supported(int N, int K);
 // mask_bits: 1-bit ReLU mask of the output, [16 groups][M] uint16 (one plane of ActPlanes::bits), or NULL.  wimage: the packed W.
 int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C, int ldc, int64_t M, int N, int accumulate,

@@ -181,7 +181,6 @@ mlp_simt_kernel(NetParams p, const float* __restrict__ x, const float* __restric
 
 int launch_mlp_simt(const NetParams& p, const float* x, const float* rays_o, const float* rays_d, const float* z,
                     int64_t m, int s, float* out, float* acts, cudaStream_t st) {
-  DMN_CHECK(p.bound, "mlp: weights not bound (call dmnerf_set_weights first)");
   DMN_CHECK((x != nullptr) != (rays_o != nullptr && rays_d != nullptr && z != nullptr),
             "mlp: pass either x or (rays_o, rays_d, z)");
   if (m == 0) return 0;

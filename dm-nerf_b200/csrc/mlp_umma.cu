@@ -30,7 +30,7 @@
 
 #include "ray_ops.cuh"
 #include "uk_pipe.cuh"
-#include "umma_api.cuh"
+#include "network.cuh"
 
 namespace dmnerf {
 namespace uk {
@@ -130,23 +130,7 @@ __device__ __forceinline__ void fill_embedding(const float v[3], float* vals /* 
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
-// The 64-wide weight chunks the consumer issues per tile, in this order: trunk layers 0..7, two half-steps each (layer 0:
-// the position embedding; layers 1..7: the four activation chunks, then at layer 5 the position embedding again), then the
-// heads: the folded instance hidden layer (four activation chunks), the folded colour hidden layer (four activation chunks,
-// then the direction embedding) and the instance head (two activation chunks).  weight_chunks() lists them for the producer
-// and the packer and is checked against these counts.
-constexpr int HEAD_CHUNK = 2 * (1 + 7 * 4 + 1);             // 60: the first chunk of the heads
-constexpr int TILE_CHUNKS = HEAD_CHUNK + 4 + (4 + 1) + 2;   // 71
-constexpr int MAX_STAGES = 2 * TILE_CHUNKS;                // the exact stream: a W_hi and a W_lo stage per chunk
-
-// The weight stream of one image, derived from weight_chunks() by make_program: all the kernel reads of it.
-struct Program {
-  uint32_t stage_off[MAX_STAGES + 1];  // byte offset of every weight stage in the image; stage_off[n_stages] = image size
-  int32_t n_stages;
-  int32_t head_stage;                  // first stage of the heads: a tile without heads streams the stages below it
-  int32_t ins_num;
-};
-
+// The chunks of a tile (TILE_CHUNKS, HEAD_CHUNK) and the weight stream the kernel reads (Program): network.cuh.
 // Warps 0-7: two consumer warpgroups (MMA issue, epilogues, prologue), CONSUMER_REGS registers each; warps 8-11: the producer
 // warpgroup at PRODUCER_REGS, of which warp 8 streams the weights.
 // SELECT (fused only): object selection -- samples whose label is not in a.keep get alpha = 0 in both composites, and so do the
@@ -712,7 +696,7 @@ __device__ __forceinline__ void mlp_umma_body(const Program& prog, const KArgs& 
     }
   }
   if constexpr (F16) {
-    // sticky: the first code stays until the host reads and clears it (umma_take_f16_range)
+    // sticky: the first code stays until the host reads and clears it (Network::take_f16_range)
     if (f16_max > F16_MAX) atomicCAS(a.status, 0, STATUS_F16_RANGE);
   }
 }
@@ -875,121 +859,92 @@ __global__ void bias_kernel(NetParams p, const float* __restrict__ fold_b_rgb, c
 }  // namespace uk
 
 // ================================================================================================ API
-struct UmmaExtra {            // hangs off UmmaWeights::extra
-  uk::Program prog;           // the stream of UmmaWeights::image
-  uk::Program prog16;         // the stream of UmmaWeights::image16: one stage per chunk
-  struct {                    // the memory behind UmmaWeights' pointers and the ones below
-    DeviceBuffer image, image16, bias, fold_w_rgb, fold_w_ins, fold_b, entries, pack_flag;
-  } mem;
-  float* fold_w_rgb = nullptr; float* fold_w_ins = nullptr; float* fold_b = nullptr; uk::PackStage* d_entries = nullptr;
-  int32_t* d_status = nullptr;           // device alias of h_status
-  volatile int32_t* h_status = nullptr;  // error word in mapped host memory: a kernel (network or backward GEMM) that gave up on a
-                                         // barrier writes its code here, and the NEXT launch through this weight set refuses to
-                                         // start (a stalled launch can never pass silently)
-};
-
-static UmmaExtra* extra_of(const UmmaWeights& w) { return reinterpret_cast<UmmaExtra*>(w.extra); }
-
-void umma_weights_free(UmmaWeights& w) {
-  if (UmmaExtra* x = extra_of(w)) {
-    if (x->h_status) cudaFreeHost((void*)x->h_status);
-    delete x;
-  }
-  w = UmmaWeights();
-}
-
-bool umma_available(const UmmaWeights& w) { return w.ready; }
-const float* umma_fold_w_rgb(const UmmaWeights& w) { return w.extra ? extra_of(w)->fold_w_rgb : nullptr; }
-int32_t* umma_status_word(const UmmaWeights& w) { return w.extra ? extra_of(w)->d_status : nullptr; }
-int umma_status_peek(const UmmaWeights& w) { return (w.extra && extra_of(w)->h_status) ? (int)*extra_of(w)->h_status : 0; }
-
-bool umma_take_f16_range(const UmmaWeights& w) {
-  if (umma_status_peek(w) != uk::STATUS_F16_RANGE) return false;
-  *extra_of(w)->h_status = 0;
-  return true;
-}
-
 // The error word as a new launch sees it: a protocol code, or 0.  STATUS_F16_RANGE is an fp16 verdict not reported yet.  An
 // fp16 launch meets it inside the call that raised it (the other parts of a *_host batch, the fine pass of the stage path) and
 // leaves it for that call's verdict (dmnerf_sync_check).  An exact launch can only meet one left by an fp16 call that failed for
 // another reason before its verdict; those results were never returned, so it is dropped.
-static int launch_gate(const UmmaWeights& w, bool f16) {
-  const int code = umma_status_peek(w);
+int Network::launch_gate(bool f16) const {
+  const int code = status.read();
   if (code != uk::STATUS_F16_RANGE) return code;
-  if (!f16) umma_take_f16_range(w);
+  if (!f16) status.clear();
+  return 0;
+}
+
+bool Network::take_f16_range() const {
+  if (status.read() != uk::STATUS_F16_RANGE) return false;
+  status.clear();
+  return true;
+}
+
+int Network::check_status(cudaStream_t st) const {
+  DMN_CUDA(cudaStreamSynchronize(st));
+  const int code = status.read();
+  DMN_CHECK(code / 100 != 6, "tensor-core backward GEMM: barrier protocol failure (code %d)", code);     // gemm_umma.cu: 6xx
+  DMN_CHECK(code == 0, "tensor-core MLP kernel reported protocol error %d (bounded wait expired)", code);
   return 0;
 }
 
 // One PackStage per chunk of weight_chunks(), placed by `prog` (the exact or the fp16 stream).  Reads the folded head layers
-// from the fold buffers, which umma_weights_pack fills.
-static std::array<uk::PackStage, uk::TILE_CHUNKS> pack_entries(const uk::Program& prog, const NetParams& p, const UmmaExtra* x,
-                                                               bool f16) {
+// from the fold buffers, which bind() fills.
+static std::array<uk::PackStage, uk::TILE_CHUNKS> pack_entries(const uk::Program& prog, const Network& net, bool f16) {
   using namespace uk;
+  const NetParams& p = net.p;
   const WeightChunks w = weight_chunks(p.ins_num);
   const int per_chunk = f16 ? 1 : 2;
   std::array<PackStage, TILE_CHUNKS> ent;
   for (int i = 0; i < TILE_CHUNKS; ++i) {
     const WeightChunk& c = w.c[i];
-    const float* src = c.src == SRC_TRUNK ? p.w[c.layer] : c.src == SRC_INS_HID ? x->fold_w_ins
-                     : c.src == SRC_RGB_HID ? x->fold_w_rgb : p.w[L_INS_OUT];
+    const float* src = c.src == SRC_TRUNK ? p.w[c.layer] : c.src == SRC_INS_HID ? net.fold_w_ins.data<float>()
+                     : c.src == SRC_RGB_HID ? net.fold_w_rgb.data<float>() : p.w[L_INS_OUT];
     ent[i] = PackStage{src, c, prog.stage_off[per_chunk * i], f16 ? 0u : prog.stage_off[per_chunk * i + 1]};
   }
   return ent;
 }
 
-int umma_weights_pack(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
+int Network::bind(const NetParams& params, cudaStream_t st) {
   using namespace uk;
-  if (w.extra && w.ins_num != p.ins_num) umma_weights_free(w);
-  if (!w.extra) {
-    UmmaExtra* x = new UmmaExtra();
-    x->prog = make_program(p.ins_num, false);
-    x->prog16 = make_program(p.ins_num, true);
-    w.extra = x;
-    w.ins_num = p.ins_num;
-    if (x->mem.image.get(x->prog.stage_off[x->prog.n_stages], &w.image) || x->mem.bias.get(B_TOTAL, &w.bias) ||
-        x->mem.fold_w_rgb.get(128 * 283, &x->fold_w_rgb) || x->mem.fold_w_ins.get(128 * 256, &x->fold_w_ins) ||
-        x->mem.fold_b.get(256, &x->fold_b) || x->mem.entries.get(TILE_CHUNKS, &x->d_entries))
-      return 2;
-    DMN_CUDA(cudaHostAlloc((void**)&x->h_status, sizeof(int32_t), cudaHostAllocMapped));
-    *x->h_status = 0;
-    DMN_CUDA(cudaHostGetDevicePointer((void**)&x->d_status, (void*)x->h_status, 0));
-  }
-  UmmaExtra* x = extra_of(w);
-  w.f16_ready = false;                                // the fp16 image is re-packed from these weights on its next use
+  bound = false;                                      // until the pack below has succeeded
+  f16_ready = false;                                  // the fp16 image is re-packed from these weights on its next use
+  p = params;
+  prog = make_program(p.ins_num, false);
+  prog16 = make_program(p.ins_num, true);
+  uint8_t* img; float *b, *fw_rgb, *fw_ins, *fb; PackStage* d_entries;
+  if (image.get(prog.stage_off[prog.n_stages], &img) || bias.get(B_TOTAL, &b) || fold_w_rgb.get(128 * 283, &fw_rgb) ||
+      fold_w_ins.get(128 * 256, &fw_ins) || fold_b.get(256, &fb) || entries.get(TILE_CHUNKS, &d_entries) || status.init())
+    return 2;
   // fold the activation-free feature layers into the following hidden layers (fp64 accumulate)
-  fold_kernel<<<dim3(128, 5), 256, 0, st>>>(p.w[L_RGB_HID], 283, p.w[L_RGB_FEAT], p.b[L_RGB_FEAT], p.b[L_RGB_HID], 27, x->fold_w_rgb, x->fold_b);
+  fold_kernel<<<dim3(128, 5), 256, 0, st>>>(p.w[L_RGB_HID], 283, p.w[L_RGB_FEAT], p.b[L_RGB_FEAT], p.b[L_RGB_HID], 27, fw_rgb, fb);
   DMN_LAUNCH_OK();
-  fold_kernel<<<dim3(128, 5), 256, 0, st>>>(p.w[L_INS_HID], 256, p.w[L_INS_FEAT], p.b[L_INS_FEAT], p.b[L_INS_HID], 0, x->fold_w_ins, x->fold_b + 128);
+  fold_kernel<<<dim3(128, 5), 256, 0, st>>>(p.w[L_INS_HID], 256, p.w[L_INS_FEAT], p.b[L_INS_FEAT], p.b[L_INS_HID], 0, fw_ins, fb + 128);
   DMN_LAUNCH_OK();
-  const auto ent = pack_entries(x->prog, p, x, false);
-  DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), sizeof(ent), cudaMemcpyHostToDevice, st));
+  const auto ent = pack_entries(prog, *this, false);
+  DMN_CUDA(cudaMemcpyAsync(d_entries, ent.data(), sizeof(ent), cudaMemcpyHostToDevice, st));
   DMN_CUDA(cudaStreamSynchronize(st));               // `ent` is a host temporary
-  pack_kernel<false><<<TILE_CHUNKS, 256, 0, st>>>(x->d_entries, TILE_CHUNKS, w.image, nullptr);
+  pack_kernel<false><<<TILE_CHUNKS, 256, 0, st>>>(d_entries, TILE_CHUNKS, img, nullptr);
   DMN_LAUNCH_OK();
-  bias_kernel<<<8, 256, 0, st>>>(p, x->fold_b, x->fold_b + 128, w.bias);
+  bias_kernel<<<8, 256, 0, st>>>(p, fb, fb + 128, b);
   DMN_LAUNCH_OK();
-  w.ready = true;
+  bound = true;
   return 0;
 }
 
-int umma_weights_pack_f16(UmmaWeights& w, const NetParams& p, cudaStream_t st) {
+int Network::pack_f16(cudaStream_t st) {
   using namespace uk;
-  DMN_CHECK(w.ready && w.extra, "fp16 network: weights not packed (call dmnerf_set_weights first)");
-  if (w.f16_ready) return 0;
-  UmmaExtra* x = extra_of(w);
-  int32_t* pack_flag;
-  if (x->mem.image16.get(x->prog16.stage_off[x->prog16.n_stages], &w.image16) || x->mem.pack_flag.get(1, &pack_flag)) return 2;
+  if (f16_ready) return 0;
+  uint8_t* img; int32_t* pack_flag_d; PackStage* d_entries;
+  if (image16.get(prog16.stage_off[prog16.n_stages], &img) || pack_flag.get(1, &pack_flag_d) || entries.get(TILE_CHUNKS, &d_entries))
+    return 2;
   // the folded head layers are the fp32 fold of the exact pack (fp64 accumulate), rounded to fp16 here
-  const auto ent = pack_entries(x->prog16, p, x, true);
-  DMN_CUDA(cudaMemsetAsync(pack_flag, 0, sizeof(int32_t), st));
-  DMN_CUDA(cudaMemcpyAsync(x->d_entries, ent.data(), sizeof(ent), cudaMemcpyHostToDevice, st));
-  pack_kernel<true><<<TILE_CHUNKS, 256, 0, st>>>(x->d_entries, TILE_CHUNKS, w.image16, pack_flag);
+  const auto ent = pack_entries(prog16, *this, true);
+  DMN_CUDA(cudaMemsetAsync(pack_flag_d, 0, sizeof(int32_t), st));
+  DMN_CUDA(cudaMemcpyAsync(d_entries, ent.data(), sizeof(ent), cudaMemcpyHostToDevice, st));
+  pack_kernel<true><<<TILE_CHUNKS, 256, 0, st>>>(d_entries, TILE_CHUNKS, img, pack_flag_d);
   DMN_LAUNCH_OK();
   int32_t out_of_range = 0;
-  DMN_CUDA(cudaMemcpyAsync(&out_of_range, pack_flag, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  DMN_CUDA(cudaMemcpyAsync(&out_of_range, pack_flag_d, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   DMN_CUDA(cudaStreamSynchronize(st));               // `ent` is a host temporary; the range verdict is read below
   DMN_CHECK(!out_of_range, "fp16 network: a weight exceeds the fp16 range (|w| > 65504); use the exact network (DMNERF_IMPL_UMMA)");
-  w.f16_ready = true;
+  f16_ready = true;
   return 0;
 }
 
@@ -1007,42 +962,38 @@ static int launch_umma(int64_t units, const uk::Program& prog, const uk::KArgs& 
   return 0;
 }
 
-int launch_mlp_umma(const UmmaWeights& w, const NetParams& p, const float* x, const float* rays_o, const float* rays_d,
-                    const float* z, int64_t m, int s, float* out, float* acts, cudaStream_t st, bool f16) {
+int launch_mlp_tc(const Network& net, const float* x, const float* rays_o, const float* rays_d, const float* z, int64_t m, int s,
+                  float* out, float* acts, cudaStream_t st, bool f16) {
   using namespace uk;
-  DMN_CHECK(w.ready && w.extra, "mlp(umma): weights not packed (call dmnerf_set_weights first)");
   DMN_CHECK((x != nullptr) != (rays_o != nullptr && rays_d != nullptr), "mlp(umma): pass either x or rays");
   DMN_CHECK(x != nullptr || z != nullptr || s == 1, "mlp(umma): points mode (z == NULL) takes one sample per row");
-  DMN_CHECK(launch_gate(w, f16) == 0, "mlp(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); its results "
-            "are invalid -- destroy the context", umma_status_peek(w));
-  DMN_CHECK(!f16 || (w.f16_ready && acts == nullptr), "mlp(umma): the fp16 network is inference-only and needs its packed image");
+  DMN_CHECK(net.launch_gate(f16) == 0, "mlp(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); its "
+            "results are invalid -- destroy the context", net.status.read());
+  DMN_CHECK(!f16 || (net.f16_ready && acts == nullptr), "mlp(umma): the fp16 network is inference-only and needs its packed image");
   if (m == 0) return 0;
-  UmmaExtra* ex = extra_of(w);
   KArgs a;
   memset(&a, 0, sizeof(a));
-  a.image = f16 ? w.image16 : w.image; a.bias = w.bias; a.x = x; a.rays_o = rays_o; a.rays_d = rays_d; a.z = z;
-  a.m = m; a.s = s; a.out = out; a.acts = acts; a.status = ex->d_status;
+  a.image = f16 ? net.image16.data<uint8_t>() : net.image.data<uint8_t>(); a.bias = net.bias.data<float>();
+  a.x = x; a.rays_o = rays_o; a.rays_d = rays_d; a.z = z;
+  a.m = m; a.s = s; a.out = out; a.acts = acts; a.status = net.status.device();
   const int64_t tiles = (m + TILE_M - 1) / TILE_M;
-  if (f16) return launch_umma<mlp_f16_kernel<false>>(tiles, ex->prog16, a, st);
-  return launch_umma<mlp_umma_kernel<false>>(tiles, ex->prog, a, st);
+  if (f16) return launch_umma<mlp_f16_kernel<false>>(tiles, net.prog16, a, st);
+  return launch_umma<mlp_umma_kernel<false>>(tiles, net.prog, a, st);
 }
 
 // Whole dm_nerf() pipeline (render.py:31-96) in ONE launch: coarse network -> composite -> importance sampling -> fine
 // network -> composite, per pair of rays, nothing but rays in and per-ray maps out crossing HBM.  64 + 128 samples only.
-int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmnerf_render_io* io, int64_t n, int flags,
-                       cudaStream_t st, const Edit* edit, bool f16) {
+int launch_render_tc(const Network& coarse, const Network& fine, const dmnerf_render_io* io, int64_t n, int flags, cudaStream_t st,
+                     const Edit* edit, bool f16) {
   using namespace uk;
-  DMN_CHECK(wc.ready && wf.ready && wc.extra && wf.extra, "render(umma): weights not packed");
-  DMN_CHECK(wc.ins_num == wf.ins_num, "render(umma): coarse/fine ins_num differ");
-  DMN_CHECK(launch_gate(wc, f16) == 0, "render(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); its "
-            "results are invalid -- destroy the context", umma_status_peek(wc));
-  DMN_CHECK(!f16 || (wc.f16_ready && wf.f16_ready), "render(umma): the fp16 images are not packed");
+  DMN_CHECK(coarse.launch_gate(f16) == 0, "render(umma): an earlier tensor-core launch reported protocol error %d (bounded wait expired); "
+            "its results are invalid -- destroy the context", coarse.status.read());
+  DMN_CHECK(!f16 || (coarse.f16_ready && fine.f16_ready), "render(umma): the fp16 images are not packed");
   if (n == 0) return 0;
-  UmmaExtra* ex = extra_of(wc);
   KArgs a;
   memset(&a, 0, sizeof(a));
-  a.image = f16 ? wc.image16 : wc.image; a.bias = wc.bias;
-  a.image_fine = f16 ? wf.image16 : wf.image; a.bias_fine = wf.bias;
+  a.image = f16 ? coarse.image16.data<uint8_t>() : coarse.image.data<uint8_t>(); a.bias = coarse.bias.data<float>();
+  a.image_fine = f16 ? fine.image16.data<uint8_t>() : fine.image.data<uint8_t>(); a.bias_fine = fine.bias.data<float>();
   a.rays_o = io->rays_o; a.rays_d = io->rays_d;
   a.z_in = io->z_coarse; a.z_stride = io->z_row_stride;
   const bool perturb = (flags & DMNERF_FLAG_PERTURB) != 0;
@@ -1051,26 +1002,18 @@ int launch_render_umma(const UmmaWeights& wc, const UmmaWeights& wf, const dmner
   a.rgb_c = io->rgb_coarse; a.rgb_f = io->rgb_fine; a.depth_c = io->depth_coarse; a.depth_f = io->depth_fine;
   a.acc_c = io->acc_coarse; a.acc_f = io->acc_fine; a.ins_c = io->ins_coarse; a.ins_f = io->ins_fine;
   a.zc_out = io->z_vals_coarse; a.zf_out = io->z_vals_fine; a.wc_out = io->weights_coarse; a.wf_out = io->weights_fine;
-  a.status = ex->d_status;
+  a.status = coarse.status.device();
   if (edit) {
     a.keep = edit->keep;
     a.region = edit->region;
     a.appearance = edit->appearance;
   }
   const int64_t units = (n + 1) / 2;                       // pairs of rays
-  const Program& prog = f16 ? ex->prog16 : ex->prog;      // coarse and fine share ins_num, hence the program
+  const Program& prog = f16 ? coarse.prog16 : coarse.prog;   // coarse and fine share ins_num, hence the program
   if (edit && f16) return launch_umma<render_objects_f16_kernel>(units, prog, a, st);
   if (edit) return launch_umma<render_objects_kernel>(units, prog, a, st);
   if (f16) return launch_umma<mlp_f16_kernel<true>>(units, prog, a, st);
   return launch_umma<mlp_umma_kernel<true>>(units, prog, a, st);
-}
-
-int umma_check_status(const UmmaWeights& w, cudaStream_t st) {
-  DMN_CUDA(cudaStreamSynchronize(st));
-  const int code = umma_status_peek(w);
-  DMN_CHECK(code / 100 != 6, "tensor-core backward GEMM: barrier protocol failure (code %d)", code);     // gemm_umma.cu: 6xx
-  DMN_CHECK(code == 0, "tensor-core MLP kernel reported protocol error %d (bounded wait expired)", code);
-  return 0;
 }
 
 }  // namespace dmnerf

@@ -88,6 +88,7 @@ class Context:
         for p in params:
             if p.dtype != torch.float32 or not p.is_cuda or not p.is_contiguous() or p.device.index != self.index:
                 raise RuntimeError("DM_NeRF parameters must be contiguous float32 tensors on cuda:%d" % self.index)
+        self._bound[slot] = None       # a pack that fails leaves the slot unbound
         self.call("dmnerf_set_weights", self.handle, slot, _lib.ptrs(params), len(params), ins_num)
         self._bound[slot] = key
         self._keepalive[slot] = params

@@ -35,7 +35,7 @@ extern "C" {
 #define DMNERF_MAX_INS 127          /* ins_num + 1 <= 128 */
 
 /* MLP implementation selector */
-#define DMNERF_IMPL_AUTO 0          /* tensor-core path when available for the shape, else SIMT */
+#define DMNERF_IMPL_AUTO 0          /* DMNERF_IMPL_UMMA: a bound network always has its tensor-core image */
 #define DMNERF_IMPL_SIMT 1          /* fp32 CUDA-core reference kernel */
 #define DMNERF_IMPL_UMMA 2          /* wgmma tensor-core kernel, bf16x3 split operands, fp32 accumulate */
 /* Preview precision, INFERENCE ONLY: the same tensor-core network run once with fp16 operands and fp32 accumulation (1/3 of
@@ -113,7 +113,9 @@ DMNERF_API int dmnerf_ctx_destroy(dmnerf_ctx* ctx);
 /* Bind one network's LIVE parameter storage (30 device pointers, state_dict order) and re-pack the
  * tensor-core operand image.  net: 0 = coarse, 1 = fine.  Replaces model.load_state_dict()/the
  * nn.Module parameter reads of DM_NeRF.forward (networks/dm_nerf.py:80-106).  Call again after every
- * in-place optimizer update. */
+ * in-place optimizer update.  A call whose arguments are rejected (ctx, net, n_params, ins_num or a NULL
+ * pointer) leaves the slot exactly as it was.  Otherwise the slot is bound only if the pack succeeds: after a
+ * failed pack it is unbound, and every call that runs it fails until a dmnerf_set_weights succeeds. */
 DMNERF_API int dmnerf_set_weights(dmnerf_ctx* ctx, int net, const float* const* params, int n_params, int ins_num,
                        void* stream);
 
