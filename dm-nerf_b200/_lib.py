@@ -62,6 +62,12 @@ class Pieces(C.Structure):
     ]
 
 
+class EditMove(C.Structure):
+    """Mirror of `struct dmnerf_edit_move` (objects.edited_sweep builds them)."""
+    _fields_ = [("label", C.c_int32), ("rest_drop", C.c_int32), ("trans", C.c_double * 12), ("box", C.c_int32 * 6),
+                ("piece", RegionDesc)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/dmnerf_b200.h
 PROTOTYPES = {
     "dmnerf_abi_version": (C.c_int, []),
@@ -141,6 +147,10 @@ PROTOTYPES = {
                                     C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_mesh_label_rays": (C.c_int, [_f32p, _f32p, C.c_int64, C.c_float, _f32p, _f32p, C.c_void_p]),
     "dmnerf_argmax_rows": (C.c_int, [_f32p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "dmnerf_mesh_occupancy_edit": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_float,
+                                             C.c_float, C.c_int64, C.POINTER(EditMove), C.c_int, _f32p, C.c_void_p,
+                                             C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_mesh_vertex_labels": (C.c_int, [_f32p, C.c_int64, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "dmnerf_object_voxels": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_int32),
                                        C.POINTER(C.c_int64), C.POINTER(C.c_uint32), C.c_void_p]),
     "dmnerf_object_spans": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_int32),

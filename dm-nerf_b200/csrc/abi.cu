@@ -756,6 +756,58 @@ DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* tra
   return 0;
 }
 
+DMNERF_API int dmnerf_mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
+                                          float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host, int n_moves,
+                                          float* occ, int16_t* labels, int64_t* evaluated_host, void* stream) {
+  const char* who = "mesh_occupancy_edit";
+  if (bound_net(ctx, net, who)) return 1;
+  if (evaluated_host) *evaluated_host = 0;
+  DMN_CHECK(transform_host && extents_host && occ && labels, "%s: NULL argument", who);
+  DMN_CHECK(dim >= 2 && dim <= 2048, "%s: dim %d out of range [2, 2048]", who, dim);
+  DMN_CHECK(n_moves >= 0 && n_moves <= DMNERF_MAX_MOVES, "%s: between 0 and %d moves are supported, got %d", who, DMNERF_MAX_MOVES,
+            n_moves);
+  DMN_CHECK(n_moves == 0 || moves_host, "%s: moves is NULL", who);
+  DMN_CHECK(level > 0.0f && level < 1.0f, "%s: level %g outside (0, 1)", who, (double)level);
+  const double* T = transform_host;
+  const double det = T[0] * (T[5] * T[10] - T[6] * T[9]) - T[1] * (T[4] * T[10] - T[6] * T[8]) + T[2] * (T[4] * T[9] - T[5] * T[8]);
+  DMN_CHECK(det > 0.0, "%s: the scene transform has det %g <= 0", who, det);
+  for (int a = 0; a < 3; ++a) DMN_CHECK(extents_host[a] > 0.0 && std::isfinite(extents_host[a]), "%s: extents must be finite and > 0", who);
+  EditMove mv[DMNERF_MAX_MOVES];
+  for (int i = 0; i < n_moves; ++i)
+    if (edit_move_from_abi(moves_host[i], transform_host, extents_host, dim, ctx->net[net].p.ins_num, mv[i], who, i)) return 1;
+  if (n_moves == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  const int64_t n = (int64_t)dim * dim * dim;
+  if (slab <= 0) slab = (int64_t)1 << 20;
+  if (slab > n) slab = n;
+  const int C = 4 + ctx->net[net].p.ins_num + 1;
+  float *pts, *raw;
+  if (ctx->mesh_pts.get((size_t)slab * 6, &pts) || ctx->mesh_raw.get((size_t)slab * C, &raw)) return 2;
+  float* dirs = pts + slab * 3;                                   // zero view directions, as the sweep
+  DMN_CUDA(cudaMemsetAsync(dirs, 0, (size_t)slab * 3 * sizeof(float), st));
+  int64_t evaluated = 0;
+  // slab by slab, move by move: a point's moves only read its own earlier state, so this is the moves applied in order
+  for (int64_t b = 0; b < n; b += slab) {
+    const int64_t cnt = n - b < slab ? n - b : slab;
+    for (int i = 0; i < n_moves; ++i) {
+      int64_t m = 0;
+      int rc = edit_targets(ctx->mesh, transform_host, extents_host, dim, mv[i], b, cnt, pts, &m, st);
+      if (!rc && m) rc = launch_mlp_tc(ctx->net[net], nullptr, pts, dirs, nullptr, m, 1, raw, nullptr, st);
+      if (!rc) rc = edit_apply(ctx->mesh, transform_host, extents_host, dim, mv[i], b, cnt, raw, C, voxel, level, occ, labels, st);
+      if (rc) return rc;
+      evaluated += m;
+    }
+  }
+  if (evaluated_host) *evaluated_host = evaluated;
+  return 0;
+}
+
+DMNERF_API int dmnerf_mesh_vertex_labels(const float* verts, int64_t n, const float* occ, const int16_t* labels, int dim, float level,
+                                         int16_t* out, void* stream) {
+  return launch_vertex_labels(verts, n, occ, labels, dim, level, out, (cudaStream_t)stream);
+}
+
 DMNERF_API int dmnerf_mesh_mc_count(dmnerf_ctx* ctx, const float* grid, int nx, int ny, int nz, float level, int64_t* counts_host,
                                     void* stream) {
   DMN_CHECK(ctx && grid && counts_host, "mesh_mc_count: NULL argument");

@@ -270,6 +270,7 @@ int launch_hungarian_costs_merged(const double* partials, int world, int64_t n, 
 // what the last marching-cubes count pass classified: mc_emit must see the same grid.
 struct MeshState {
   DeviceBuffer eflags, cases, vcnt, vscan, tcnt, tscan, temp, totals, keys_in, keys_out, vals_in, vals_out, parent, size;
+  DeviceBuffer edit_t, edit_flag, edit_pos;   // the edited sweep's slab: target points, in-box flags and their scan
   const float* grid = nullptr;
   int nx = 0, ny = 0, nz = 0;
   float level = 0.f;
@@ -289,6 +290,31 @@ int mesh_clean(MeshState& s, const float* v, const float* nrm, int64_t nv, const
                int min_cluster, float* out_v, float* out_n, int32_t* out_t, int64_t* counts, cudaStream_t st);
 int launch_label_rays(const float* v, const float* nrm, int64_t n, float near_z, float* ro, float* rd, cudaStream_t st);
 int launch_argmax_rows(const float* x, int64_t n, int c, int64_t* out, cudaStream_t st);
+
+// Meshing an edited scene (mesh.cu; DESIGN.md, "Meshing an edited scene").  One checked move of dmnerf_mesh_occupancy_edit: the
+// 3x4 move and the grid's index map u = inv (t - b) in fp64, the box in index units, the piece (bits NULL: none).
+struct EditMove {
+  double trans[12];
+  double inv[9];
+  double b[3];
+  double lo[3], hi[3];
+  Region piece;
+  int32_t label, rest_drop, empty;   // empty: the box holds no point, nothing is evaluated
+};
+// d -> m, checked against the grid (dim, transform, extents) and the bound network's ins_num
+int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const double* ext3, int dim, int ins_num, EditMove& m,
+                       const char* who, int i);
+// Points [begin, begin + count) of the grid: their targets under m, the boxed ones compacted in order into pts [*n_eval, 3];
+// *n_eval read back (synchronises).
+int edit_targets(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
+                 float* pts, int64_t* n_eval, cudaStream_t st);
+// take / vacate of m on the same points, raw [n_eval, c]: the network at the compacted targets of the last edit_targets
+int edit_apply(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
+               const float* raw, int c, float voxel, float level, float* occ, int16_t* labels, cudaStream_t st);
+int launch_vertex_labels(const float* v, int64_t n, const float* occ, const int16_t* labels, int dim, float level, int16_t* out,
+                         cudaStream_t st);
+// The region of a move (bits NULL: none), checked: dim and map, the moved label among the labels it applies to (exchanger.cu).
+int piece_region(const dmnerf_region& d, int mv, Region& r, const char* who, int i);
 
 // Object inventory (inventory.cu): per-group integer statistics and fp64 spans of the solid points of a labelled grid.
 // Per-context device buffers: everything a call reads back (status word first), and its inputs.

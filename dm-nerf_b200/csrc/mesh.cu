@@ -1,6 +1,9 @@
 // Mesh extraction, tools/mesh_generator.py + tools/visualizer.py of the original project: query grid of the occupancy sweep and
 // its epilogue, marching cubes on a caller-provided grid, scene-space vertices, area-weighted vertex normals, edge-connected
 // triangle clusters, small-cluster removal and the per-vertex label rays.  Conventions: DESIGN.md, "Mesh extraction".
+#include <cmath>
+#include <cstring>
+
 #include <cub/cub.cuh>
 
 #include "common.cuh"
@@ -139,10 +142,8 @@ __device__ __forceinline__ float linspace_m11(int i, const GridXform& g) {
 
 // visualizer.make_3D_grid / grid_within_bound + mesh_generator.py:28-29, in the original's fp32 operation order:
 // q = (R q_scaled summed left to right) + t, then (x, y, z) -> (x, -z, y)
-__global__ void grid_points_kernel(GridXform g, int64_t begin, int64_t count, float* __restrict__ pts) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  const int64_t p = begin + i, d = g.dim;
+__device__ __forceinline__ void sweep_point(const GridXform& g, int64_t p, float out[3]) {
+  const int64_t d = g.dim;
   const float q[3] = {__fmul_rn(linspace_m11((int)(p / (d * d)), g), g.s[0]), __fmul_rn(linspace_m11((int)((p / d) % d), g), g.s[1]),
                       __fmul_rn(linspace_m11((int)(p % d), g), g.s[2])};
   float w[3];
@@ -151,33 +152,50 @@ __global__ void grid_points_kernel(GridXform g, int64_t begin, int64_t count, fl
     const float* row = g.r + 4 * r;
     w[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(row[0], q[0]), __fmul_rn(row[1], q[1])), __fmul_rn(row[2], q[2])), row[3]);
   }
-  pts[3 * i] = w[0];
-  pts[3 * i + 1] = -w[2];
-  pts[3 * i + 2] = w[1];
+  out[0] = w[0];
+  out[1] = -w[2];
+  out[2] = w[1];
 }
 
-int launch_grid_points(const double* T16, const double* ext3, int dim, int64_t begin, int64_t count, float* pts, cudaStream_t st) {
-  DMN_CHECK(dim >= 2 && dim <= 2048, "grid_points: dim %d out of range [2, 2048]", dim);
-  DMN_CHECK(begin >= 0 && count >= 0 && begin + count <= (int64_t)dim * dim * dim, "grid_points: range outside the grid");
-  if (count == 0) return 0;
+__global__ void grid_points_kernel(GridXform g, int64_t begin, int64_t count, float* __restrict__ pts) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  float w[3];
+  sweep_point(g, begin + i, w);
+  pts[3 * i] = w[0];
+  pts[3 * i + 1] = w[1];
+  pts[3 * i + 2] = w[2];
+}
+
+static GridXform make_xform(const double* T16, const double* ext3, int dim) {
   GridXform g;
   for (int r = 0; r < 3; ++r)
     for (int c = 0; c < 4; ++c) g.r[4 * r + c] = (float)T16[4 * r + c];
   for (int a = 0; a < 3; ++a) g.s[a] = (float)(ext3[a] / 2.0);
   g.step = 2.0f / (float)(dim - 1);
   g.dim = dim;
-  grid_points_kernel<<<blocks(count, 256), 256, 0, st>>>(g, begin, count, pts);
+  return g;
+}
+
+int launch_grid_points(const double* T16, const double* ext3, int dim, int64_t begin, int64_t count, float* pts, cudaStream_t st) {
+  DMN_CHECK(dim >= 2 && dim <= 2048, "grid_points: dim %d out of range [2, 2048]", dim);
+  DMN_CHECK(begin >= 0 && count >= 0 && begin + count <= (int64_t)dim * dim * dim, "grid_points: range outside the grid");
+  if (count == 0) return 0;
+  grid_points_kernel<<<blocks(count, 256), 256, 0, st>>>(make_xform(T16, ext3, dim), begin, count, pts);
   DMN_LAUNCH_OK();
   return 0;
 }
 
 // mesh_generator.py:51-62: occ = 1 - exp(-relu(sigma) * voxel), sigma = channel 3 of the network output [n, c]
+__device__ __forceinline__ float occupancy_of(float a, float voxel) {
+  const float r = a > 0.f ? a : (a != a ? a : 0.f);           // torch.relu keeps NaN
+  return __fsub_rn(1.0f, expf(__fmul_rn(-r, voxel)));
+}
+
 __global__ void occupancy_kernel(const float* __restrict__ raw, int64_t n, int c, float voxel, float* __restrict__ occ) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float a = raw[i * c + 3];
-  const float r = a > 0.f ? a : (a != a ? a : 0.f);           // torch.relu keeps NaN
-  occ[i] = __fsub_rn(1.0f, expf(__fmul_rn(-r, voxel)));
+  occ[i] = occupancy_of(raw[i * c + 3], voxel);
 }
 
 int launch_occupancy(const float* raw, int64_t n, int c, float voxel, float* occ, cudaStream_t st) {
@@ -195,9 +213,7 @@ __global__ void occupancy_objects_kernel(const float* __restrict__ raw, int64_t 
   if (i >= n) return;
   const float* ri = raw + i * c;
   const int label = argmax_sigmoid(ri + 4, c - 4);
-  const float a = ri[3];
-  const float r = a > 0.f ? a : (a != a ? a : 0.f);
-  occ[i] = obj_kept(keep, label) ? __fsub_rn(1.0f, expf(__fmul_rn(-r, voxel))) : 0.0f;
+  occ[i] = obj_kept(keep, label) ? occupancy_of(ri[3], voxel) : 0.0f;
   if (labels) labels[i] = (int16_t)label;
 }
 
@@ -638,6 +654,226 @@ __global__ void argmax_rows_kernel(const float* __restrict__ x, int64_t n, int c
 int launch_argmax_rows(const float* x, int64_t n, int c, int64_t* out, cudaStream_t st) {
   if (n == 0) return 0;
   argmax_rows_kernel<<<blocks(n, 256), 256, 0, st>>>(x, n, c, out);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+// ---- meshing an edited scene (DESIGN.md, "Meshing an edited scene") ---------------------------------------------------------
+// Every fp64 expression below is written with one rounding per operation (no contraction), so that a numpy restatement
+// (oracle/edit_sweep_oracle.py) takes the same decisions.
+
+// The grid's index map of objects.grid_affine: p = A idx + b with A = S R diag(h), b = S (t - R e), h = extents / (dim - 1),
+// e = extents / 2 and S the axis swap (x, y, z) -> (x, -z, y); inv = diag(1 / h) R^-1 S^T, R^-1 = adj(R) / det(R).
+static void grid_index_map(const double* T, const double* ext, int dim, double inv[9], double b[3]) {
+  const double R[3][3] = {{T[0], T[1], T[2]}, {T[4], T[5], T[6]}, {T[8], T[9], T[10]}};
+  double adj[3][3];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      const int i1 = (j + 1) % 3, i2 = (j + 2) % 3, j1 = (i + 1) % 3, j2 = (i + 2) % 3;
+      adj[i][j] = R[i1][j1] * R[i2][j2] - R[i1][j2] * R[i2][j1];       // cofactor (j, i)
+    }
+  const double det = (R[0][0] * adj[0][0] + R[0][1] * adj[1][0]) + R[0][2] * adj[2][0];
+  double w[3];
+  for (int r = 0; r < 3; ++r)
+    w[r] = T[4 * r + 3] - ((R[r][0] * (ext[0] / 2.0) + R[r][1] * (ext[1] / 2.0)) + R[r][2] * (ext[2] / 2.0));
+  b[0] = w[0]; b[1] = -w[2]; b[2] = w[1];
+  for (int a = 0; a < 3; ++a) {
+    const double scale = (double)(dim - 1) / ext[a];
+    const double ri[3] = {adj[a][0] / det, adj[a][1] / det, adj[a][2] / det};
+    // column c of S^T: S^T e_0 = e_0, S^T e_1 = -e_2, S^T e_2 = e_1
+    inv[3 * a] = scale * ri[0];
+    inv[3 * a + 1] = scale * -ri[2];
+    inv[3 * a + 2] = scale * ri[1];
+  }
+}
+
+int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const double* ext3, int dim, int ins_num, EditMove& m,
+                       const char* who, int i) {
+  memset(&m, 0, sizeof(m));
+  DMN_CHECK(d.label >= 0 && d.label <= ins_num, "%s: move %d: label %d outside [0, %d]", who, i, d.label, ins_num);
+  for (int k = 0; k < 12; ++k) DMN_CHECK(std::isfinite(d.trans[k]), "%s: move %d: the transformation is not finite", who, i);
+  const double* t = d.trans;
+  const double det = t[0] * (t[5] * t[10] - t[6] * t[9]) - t[1] * (t[4] * t[10] - t[6] * t[8]) + t[2] * (t[4] * t[9] - t[5] * t[8]);
+  DMN_CHECK(det > 0.0, "%s: move %d: the transformation has det %g <= 0 (a reflection or a degenerate matrix)", who, i, det);
+  const int* bx = d.box;
+  const bool empty = bx[0] == 1 && bx[1] == 0 && bx[2] == 1 && bx[3] == 0 && bx[4] == 1 && bx[5] == 0;
+  if (!empty)
+    for (int a = 0; a < 3; ++a)
+      DMN_CHECK(bx[2 * a] >= 0 && bx[2 * a] <= bx[2 * a + 1] && bx[2 * a + 1] <= dim - 1,
+                "%s: move %d: box [%d, %d] x [%d, %d] x [%d, %d] is inverted or outside the grid [0, %d]", who, i, bx[0], bx[1], bx[2],
+                bx[3], bx[4], bx[5], dim - 1);
+  if (piece_region(d.piece, d.label, m.piece, who, i)) return 1;
+  memcpy(m.trans, d.trans, sizeof(m.trans));
+  grid_index_map(T16, ext3, dim, m.inv, m.b);
+  for (int a = 0; a < 3; ++a) { m.lo[a] = bx[2 * a]; m.hi[a] = bx[2 * a + 1]; }
+  m.label = d.label;
+  m.rest_drop = d.rest_drop ? 1 : 0;
+  m.empty = empty ? 1 : 0;
+  return 0;
+}
+
+// One thread per grid point of the slab: its target t = trans p (fp64, rounded once to fp32) and whether the nearest grid index
+// of t, rint(A^-1 (t - b)), lies in the box (an fp32 sweep point maps to its own index, also on the grid's faces).
+__global__ void edit_target_kernel(const GridXform g, const EditMove m, int64_t begin, int64_t count, float* __restrict__ tgt,
+                                   int32_t* __restrict__ flag) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  float p[3];
+  sweep_point(g, begin + i, p);
+  float t[3];
+  double dt[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const double* r = m.trans + 4 * a;
+    const double v = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)p[0]), __dmul_rn(r[1], (double)p[1])),
+                                         __dmul_rn(r[2], (double)p[2])), r[3]);
+    t[a] = __double2float_rn(v);
+    dt[a] = __dsub_rn((double)t[a], m.b[a]);
+  }
+  bool in = !m.empty;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const double* row = m.inv + 3 * a;
+    const double u = __dadd_rn(__dadd_rn(__dmul_rn(row[0], dt[0]), __dmul_rn(row[1], dt[1])), __dmul_rn(row[2], dt[2]));
+    const double i = rint(u);                                     // the nearest grid index, half to even
+    in = in && i >= m.lo[a] && i <= m.hi[a];
+  }
+  tgt[3 * i] = t[0];
+  tgt[3 * i + 1] = t[1];
+  tgt[3 * i + 2] = t[2];
+  flag[i] = in ? 1 : 0;
+}
+
+// order-keeping compaction of the boxed targets (pos: exclusive scan of flag)
+__global__ void edit_compact_kernel(const float* __restrict__ tgt, const int32_t* __restrict__ flag, const int32_t* __restrict__ pos,
+                                    int64_t count, float* __restrict__ pts) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count || !flag[i]) return;
+  const int64_t o = pos[i];
+  pts[3 * o] = tgt[3 * i];
+  pts[3 * o + 1] = tgt[3 * i + 1];
+  pts[3 * o + 2] = tgt[3 * i + 2];
+}
+
+__global__ void edit_count_kernel(const int32_t* flag, const int32_t* pos, int64_t count, int64_t* out) {
+  out[0] = (int64_t)pos[count - 1] + flag[count - 1];
+}
+
+// One thread per grid point of the slab: take the target's (occ, label), or vacate the point.
+__global__ void edit_apply_kernel(const GridXform g, const EditMove m, int64_t begin, int64_t count, const int32_t* __restrict__ flag,
+                                  const int32_t* __restrict__ pos, const float* __restrict__ tgt, const float* __restrict__ raw, int c,
+                                  float voxel, float level, float* __restrict__ occ, int16_t* __restrict__ labels) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const int64_t p = begin + i;
+  const float o = occ[p];
+  const int l = labels[p];
+  const bool has_piece = m.piece.bits != nullptr;
+  if (flag[i]) {
+    const float* r = raw + (int64_t)pos[i] * c;
+    const int lt = argmax_sigmoid(r + 4, c - 4);
+    const float ot = occupancy_of(r[3], voxel);
+    if (lt == m.label && (ot > level || o <= level) &&
+        (!has_piece || !region_drops(m.piece, m.label, tgt[3 * i], tgt[3 * i + 1], tgt[3 * i + 2]))) {
+      occ[p] = ot;
+      labels[p] = (int16_t)m.label;
+      return;
+    }
+  }
+  if (l == m.label && o > level) {
+    bool in_piece = true;
+    if (has_piece) {
+      float q[3];
+      sweep_point(g, p, q);
+      in_piece = !region_drops(m.piece, m.label, q[0], q[1], q[2]);
+    }
+    if (in_piece || m.rest_drop) occ[p] = 0.0f;
+  }
+}
+
+int edit_targets(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
+                 float* pts, int64_t* n_eval, cudaStream_t st) {
+  *n_eval = 0;
+  DMN_CHECK(count >= 1 && count < INT32_MAX, "edit_targets: slab of %lld points outside [1, 2^31)", (long long)count);
+  float* tgt;
+  int32_t *flag, *pos;
+  int64_t* tot;
+  if (s.edit_t.get((size_t)count * 3, &tgt) || s.edit_flag.get((size_t)count, &flag) || s.edit_pos.get((size_t)count, &pos) ||
+      s.totals.get(4, &tot))
+    return 2;
+  const GridXform g = make_xform(T16, ext3, dim);
+  edit_target_kernel<<<blocks(count, 256), 256, 0, st>>>(g, m, begin, count, tgt, flag);
+  DMN_LAUNCH_OK();
+  if (exclusive_sum(s, flag, pos, count, st)) return 2;
+  edit_count_kernel<<<1, 1, 0, st>>>(flag, pos, count, tot);
+  DMN_LAUNCH_OK();
+  int64_t n = 0;
+  if (read_back(s, &n, 1, st)) return 2;
+  if (n) {
+    edit_compact_kernel<<<blocks(count, 256), 256, 0, st>>>(tgt, flag, pos, count, pts);
+    DMN_LAUNCH_OK();
+  }
+  *n_eval = n;
+  return 0;
+}
+
+int edit_apply(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
+               const float* raw, int c, float voxel, float level, float* occ, int16_t* labels, cudaStream_t st) {
+  float* tgt;
+  int32_t *flag, *pos;
+  if (s.edit_t.get((size_t)count * 3, &tgt) || s.edit_flag.get((size_t)count, &flag) || s.edit_pos.get((size_t)count, &pos))
+    return 2;                                                     // as edit_targets left them
+  edit_apply_kernel<<<blocks(count, 256), 256, 0, st>>>(make_xform(T16, ext3, dim), m, begin, count, flag, pos, tgt, raw, c, voxel,
+                                                        level, occ, labels);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+// The label of the nearest solid grid point closer than 2 to an index-space vertex: the 4^3 block floor(v) - 1 .. floor(v) + 2
+// holds every grid point closer than 2; it is walked in ascending linear index and only a strictly smaller squared distance
+// replaces the best, so an exact tie goes to the lowest index.
+__global__ void vertex_labels_kernel(const float* __restrict__ v, int64_t n, const float* __restrict__ occ,
+                                     const int16_t* __restrict__ labels, int dim, float level, int16_t* __restrict__ out) {
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n) return;
+  const float x[3] = {v[3 * q], v[3 * q + 1], v[3 * q + 2]};
+  int lo[3], hi[3];
+  bool ok = true;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    ok = ok && x[a] > -2.0f && x[a] < (float)(dim + 1);           // also false for NaN
+    const int f = ok ? (int)floorf(x[a]) : 0;
+    lo[a] = max(f - 1, 0);
+    hi[a] = min(f + 2, dim - 1);
+  }
+  int best = -1;
+  double bd = 4.0;
+  if (ok) {
+    for (int i = lo[0]; i <= hi[0]; ++i) {
+      const double dx = __dsub_rn((double)x[0], (double)i);
+      for (int j = lo[1]; j <= hi[1]; ++j) {
+        const double dy = __dsub_rn((double)x[1], (double)j);
+        const double dxy = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
+        for (int k = lo[2]; k <= hi[2]; ++k) {
+          const double dz = __dsub_rn((double)x[2], (double)k);
+          const double d2 = __dadd_rn(dxy, __dmul_rn(dz, dz));
+          const int64_t p = ((int64_t)i * dim + j) * dim + k;
+          if (d2 < bd && occ[p] > level) { bd = d2; best = labels[p]; }
+        }
+      }
+    }
+  }
+  out[q] = (int16_t)best;
+}
+
+int launch_vertex_labels(const float* v, int64_t n, const float* occ, const int16_t* labels, int dim, float level, int16_t* out,
+                         cudaStream_t st) {
+  DMN_CHECK(n >= 0, "mesh_vertex_labels: negative vertex count");
+  DMN_CHECK(dim >= 2 && dim <= 2048, "mesh_vertex_labels: dim %d out of range [2, 2048]", dim);
+  DMN_CHECK(std::isfinite(level), "mesh_vertex_labels: level is not finite");
+  DMN_CHECK(occ && labels && (n == 0 || (v && out)), "mesh_vertex_labels: NULL argument");
+  if (n == 0) return 0;
+  vertex_labels_kernel<<<blocks(n, 256), 256, 0, st>>>(v, n, occ, labels, dim, level, out);
   DMN_LAUNCH_OK();
   return 0;
 }

@@ -142,6 +142,20 @@ def argmax_rows(x):
     return out
 
 
+def vertex_labels(verts, occ, labels, level=0.45):
+    """dmnerf_mesh_vertex_labels: per index-space vertex [V, 3] the label (labels [dim]^3 int16) of the nearest solid grid point
+    (occ > level) closer than 2, an exact tie to the lowest linear index, -1 without one -> int16 [V].  For the marching-cubes
+    vertices of (occ, level) this is the inside end of each vertex's edge."""
+    _lib.need_cuda("vertex_labels", verts, occ, labels)
+    if occ.dim() != 3 or not (occ.shape[0] == occ.shape[1] == occ.shape[2]) or labels.shape != occ.shape:
+        raise ValueError("vertex_labels: occ and labels must be one cubic grid [dim, dim, dim]")
+    v = verts.contiguous().float()
+    out = torch.empty(v.shape[0], device=v.device, dtype=torch.int16)
+    get_context(v.device).call("dmnerf_mesh_vertex_labels", _lib.ptr(v), v.shape[0], _lib.ptr(occ), _lib.ptr(labels, torch.int16),
+                               occ.shape[0], float(level), _lib.ptr(out, torch.int16))
+    return out
+
+
 def render_labels(model_coarse, model_fine, rays_o, rays_d, N_samples=64, N_importance=128, N_test=4096, impl=_lib.IMPL_AUTO):
     """mesh_generator.py:117-136: each ray rendered deterministically with depths z_val_sample(n, 0.01, 15, N_samples), N_test rays
     per call, label = argmax of the fine instance map.  impl: the network of the label rays, as in render_rays."""

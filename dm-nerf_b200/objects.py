@@ -16,6 +16,8 @@
                                                         -> per-object colour maps and density scales (render_*(appearance=))
     scene_box(model_fine, poses, hwk, near, far, ...)   -> (scene_transform, extents) of the scene, from the cameras
     manipulation_transform(centre, mode)                -> the transformation dict manipulator_eval takes, about that centre
+    edited_sweep(model_fine, scene_transform, moves, ...) / edited_mesh(...)
+                                                        -> the labelled sweep / the mesh of a scene with objects moved
 
 Every network sample is labelled argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the
 exchanger's rule); a sample whose label is not kept has alpha = 0 in the composite of both passes, so the coarse weights of the
@@ -188,6 +190,209 @@ def object_meshes(model_fine, model_coarse, scene_transform, objects=None, grid_
         return meshes_from_labelled_grid(occ, labels, T, objects, level, extents, min_cluster)
 
 
+# ----------------------------------------------------------------------------------------------------------------- edited meshes
+# DESIGN.md, "Meshing an edited scene": the moves of manipulator_eval / manipulate_frame applied per grid point to the labelled
+# keep-all sweep, so that an edited scene can be meshed.  The network runs only at the target points inside each move's box.
+EMPTY_BOX = (1, 0, 1, 0, 1, 0)       # the inventory's box of a group without points: a move with it evaluates nothing
+
+
+def _move_matrix(trans, i):
+    m = np.asarray(trans, dtype=np.float64)
+    if m.shape != (4, 4) or not np.isfinite(m).all():
+        raise ValueError("edit: move %d: the transformation must be a finite 4x4 matrix, got shape %s" % (i, m.shape))
+    if not np.array_equal(m[3], [0.0, 0.0, 0.0, 1.0]):
+        raise ValueError("edit: move %d: the transformation's last row must be (0, 0, 0, 1)" % i)
+    if np.linalg.det(m[:3, :3]) <= 0:
+        raise ValueError("edit: move %d: the transformation has a non-positive determinant (a reflection or a degenerate "
+                         "matrix)" % i)
+    return m
+
+
+def _check_moves(moves, ins_num):
+    """moves [(label, 4x4)] -> (labels, matrices); ValueError for more than MAX_MOVES, a label outside [0, ins_num] or a bad
+    matrix.  A matrix may be manipulation_transform(...)["transformations"][0]["transformation"] (a nested list)."""
+    moves = list(moves)
+    if len(moves) > _lib.MAX_MOVES:
+        raise ValueError("edit: at most %d moves are supported, got %d" % (_lib.MAX_MOVES, len(moves)))
+    labels, mats = [], []
+    for i, mv in enumerate(moves):
+        try:
+            label, trans = mv
+        except (TypeError, ValueError):
+            raise ValueError("edit: move %d must be a pair (label, 4x4 transformation)" % i) from None
+        labels.append(_labels([label], ins_num, "edit")[0])
+        mats.append(_move_matrix(trans, i))
+    return labels, mats
+
+
+def _check_level(level):
+    level = float(level)
+    if not 0.0 < level < 1.0:
+        raise ValueError("edit: level %r outside (0, 1)" % level)
+    return level
+
+
+def _check_boxes(boxes, m, dim):
+    b = np.asarray(boxes, dtype=np.int64)
+    if b.shape != (m, 6):
+        raise ValueError("edit: boxes must be [%d, 6] inclusive index boxes, got shape %s" % (m, b.shape))
+    for i in range(m):
+        if tuple(b[i]) == EMPTY_BOX:
+            continue
+        if not all(0 <= b[i, 2 * a] <= b[i, 2 * a + 1] <= dim - 1 for a in range(3)):
+            raise ValueError("edit: box %d %s is inverted or outside the grid [0, %d]" % (i, b[i].tolist(), dim - 1))
+    return b
+
+
+def _region_keeps(region, T, dim, extents, device, slab=1 << 20):
+    """bool [dim]^3: the sweep grid points a piece keeps for a label it applies to -- inside its grid with the bit set, or
+    outside it when it keeps outside samples -- by the render kernels' own test (region_contains)."""
+    from .mesh import EXTENTS, grid_points
+    ext = EXTENTS if extents is None else extents
+    whole = None
+    if region.outside == "keep":
+        words = np.full((region.dim ** 3 + 31) // 32, -1, dtype=np.int32)
+        tail = region.dim ** 3 % 32
+        if tail:
+            words[-1] = (1 << tail) - 1
+        whole = Region(torch.as_tensor(words).to(region.bits.device), region.dim, region.voxel_map, region.applies, "keep")
+    keep = torch.empty(dim ** 3, dtype=torch.bool, device=device)
+    for b in range(0, dim ** 3, slab):
+        pts = grid_points(T, dim, ext, b, min(slab, dim ** 3 - b), device)
+        k = region_contains(region, pts)
+        if whole is not None:
+            k |= ~region_contains(whole, pts)
+        keep[b:b + pts.shape[0]] = k
+    return keep.reshape((dim,) * 3)
+
+
+def solid_box(occ, labels, label, level=0.45, margin=2, keep=None):
+    """The inclusive index box (i_lo, i_hi, j_lo, j_hi, k_lo, k_hi) of the solid points (occ > level) of `label` (and of `keep`,
+    a bool grid, when given), grown by `margin` voxels on every side and clipped to the grid; EMPTY_BOX without points."""
+    mask = (labels == int(label)) & (occ > level)
+    if keep is not None:
+        mask &= keep
+    if not bool(mask.any()):
+        return EMPTY_BOX
+    dim = occ.shape[0]
+    box = []
+    for a in range(3):
+        idx = torch.nonzero(mask.any(dim=tuple(c for c in range(3) if c != a))).flatten()
+        box += [max(int(idx[0]) - int(margin), 0), min(int(idx[-1]) + int(margin), dim - 1)]
+    return tuple(box)
+
+
+def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, extents=None, level=0.45, near=4.0, far=15.0,
+                   N_importance=128, pieces=None, rest="keep", slab=0):
+    """dmnerf_mesh_occupancy_edit: the moves [(label, 4x4)] applied in order, in place, to occ / labels ([dim]^3 float32 /
+    int16 on the device: the keep-all sweep of model_fine on this grid), the network evaluated only at the target points
+    inside each move's box (boxes: [m, 6] inclusive index boxes, EMPTY_BOX for none).  pieces / rest: as manipulator.  Returns
+    the number of target points evaluated."""
+    from .manipulator import _piece_region, move_pieces, move_rests
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    dim = _check_grid(occ, labels, "edit_occupancy")
+    if labels is None or labels.dtype != torch.int16 or occ.dtype != torch.float32:
+        raise ValueError("edit_occupancy: occ must be float32 and labels int16")
+    ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
+    mv, mats = _check_moves(moves, ins_num)
+    level = _check_level(level)
+    boxes = _check_boxes(boxes, len(mv), dim)
+    drops = move_rests(rest, len(mv))
+    regions = move_pieces(pieces, mv, ins_num, occ.device) or [None] * len(mv)
+    if not mv:
+        return 0
+    descs = (_lib.EditMove * len(mv))()
+    for i in range(len(mv)):
+        d = descs[i]
+        d.label, d.rest_drop = mv[i], int(drops[i])
+        d.trans[:] = mats[i][:3].reshape(-1).tolist()
+        d.box[:] = [int(v) for v in boxes[i]]
+        d.piece = _piece_region(regions[i], mv[i], ins_num, occ.device)
+    ctx = get_context(occ.device)
+    slot = ctx.slot_for(model_fine)
+    ctx.bind(slot, model_fine)
+    ext = EXTENTS if extents is None else extents
+    n = C.c_int64(0)
+    with torch.no_grad():
+        ctx.call("dmnerf_mesh_occupancy_edit", ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(ext, 3), dim,
+                 (far - near) / N_importance, level, int(slab), descs, len(mv), _lib.ptr(occ), _lib.ptr(labels, torch.int16),
+                 C.byref(n))
+    return int(n.value)
+
+
+def edit_boxes(occ, labels, moves, scene_transform, extents=None, level=0.45, margin=2, pieces=None):
+    """The default boxes of edited_sweep from the unedited sweep: per move, solid_box of its label's solid points (those its
+    piece keeps, with a piece) grown by margin -> int [m, 6]."""
+    if int(margin) != margin or int(margin) < 0:
+        raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
+    mv = [int(m[0]) for m in moves]
+    regions = list(pieces) if pieces is not None else [None] * len(mv)
+    dim = occ.shape[0]
+    out = []
+    for k, r in zip(mv, regions):
+        keep = None if r is None else _region_keeps(r, scene_transform, dim, extents, occ.device)
+        out.append(solid_box(occ, labels, k, level, int(margin), keep))
+        del keep
+    return np.asarray(out, dtype=np.int64).reshape(len(mv), 6)
+
+
+def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128,
+                 margin=2, boxes=None, pieces=None, rest="keep"):
+    """The labelled sweep of the edited scene -> (occ [dim]^3 float32, labels [dim]^3 int16) on the device: the keep-all sweep of
+    model_fine (occupancy_objects), then the moves [(label, 4x4 in the network frame, as manipulator_eval's transformation)]
+    applied in order (edit_occupancy).  A move shows at p what the network holds at trans p, as rigid_rays renders it: the
+    object lands at inv(trans) x.  boxes: per move the index box of the target points evaluated; by default the box of the
+    moved label's solid points in the unedited grid (of those its piece keeps, with a piece) grown by `margin` voxels.
+    pieces / rest: as manipulator (a Region or None per move; "keep" / "drop", or one per move)."""
+    from .manipulator import move_pieces, move_rests
+    from .mesh import check_transform
+    T = check_transform(scene_transform)
+    dev = next(model_fine.parameters()).device
+    ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
+    mv, _ = _check_moves(moves, ins_num)
+    level = _check_level(level)
+    move_rests(rest, len(mv))
+    move_pieces(pieces, mv, ins_num, dev)
+    if int(margin) != margin or int(margin) < 0:
+        raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
+    if boxes is not None:
+        boxes = _check_boxes(boxes, len(mv), int(grid_dim))
+    with torch.no_grad():
+        occ, labels = occupancy_objects(model_fine, T, object_mask(ins_num, remove=[]), grid_dim, extents, near, far, N_importance,
+                                        device=dev)
+        if boxes is None:
+            boxes = edit_boxes(occ, labels, moves, T, extents, level, margin, pieces)
+        edit_occupancy(model_fine, T, occ, labels, moves, boxes, extents, level, near, far, N_importance, pieces, rest)
+    return occ, labels
+
+
+def edited_mesh(model_fine, scene_transform, moves, grid_dim=256, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128,
+                margin=2, boxes=None, pieces=None, rest="keep", min_cluster=400, per_object=False):
+    """The mesh of an edited scene: edited_sweep (same arguments) -> marching cubes -> scene space -> normals -> small-cluster
+    removal.  Returns extract_mesh's keys as device tensors -- vertices, triangles, normals, clean_vertices, clean_normals,
+    clean_triangles -- and labels (int64 per clean vertex: mesh.vertex_labels of its index-space vertex, the label of the
+    inside end of its edge, from the edited grid; no label rays are rendered).  per_object: also objects, the
+    meshes_from_labelled_grid of the edited grid for every label with solid points except ins_num."""
+    from .mesh import EXTENTS, check_transform, clean_mesh, marching_cubes, to_scene, vertex_labels, vertex_normals
+    T = check_transform(scene_transform)
+    ext = EXTENTS if extents is None else extents
+    ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
+    with torch.no_grad():
+        occ, labels = edited_sweep(model_fine, T, moves, grid_dim, ext, level, near, far, N_importance, margin, boxes, pieces, rest)
+        v_idx, tris = marching_cubes(occ, level)
+        verts = to_scene(v_idx, T, grid_dim, ext)
+        normals = vertex_normals(verts, tris)
+        cv, cn, ct = clean_mesh(verts, normals, tris, min_cluster)
+        ci, _, _ = clean_mesh(v_idx, None, tris, min_cluster)         # the same topological cleanup, index space
+        out = {"vertices": verts, "triangles": tris, "normals": normals, "clean_vertices": cv, "clean_normals": cn,
+               "clean_triangles": ct, "labels": vertex_labels(ci, occ, labels, level).long()}
+        if per_object:
+            objects = [k for k in torch.unique(labels[occ > level]).cpu().tolist() if k != ins_num]
+            out["objects"] = meshes_from_labelled_grid(occ, labels, T, objects, level, ext, min_cluster)
+    return out
+
+
 def largest_component_grid(occ, labels, level, objects):
     """int16 grid: label k at the points of the largest 26-connected component of each label k of `objects`, -1 elsewhere."""
     cc = object_components(occ, labels, level, 26)
@@ -348,7 +553,8 @@ def inventory_from_grid(occ, labels, scene_transform, extents=None, level=0.45, 
       "largest": each label's statistics over its largest component only (a tie in voxels goes to the smaller root); the
                  entry gains components (how many the label has) and discarded_voxels (its solid points outside that one);
       "split":   one entry per component with at least min_voxels voxels, ordered by (label, root), with component (its id).
-    trim applies after the selection, over the selected points."""
+    trim applies after the selection, over the selected points.  An edited grid (edited_sweep) is a labelled grid like any
+    other: its inventory reports the objects where the moves put them."""
     from .mesh import EXTENTS, check_transform
     trim = _check_trim(trim)
     if components not in (None, "largest", "split"):
@@ -412,7 +618,7 @@ def object_components(occ, labels=None, level=0.45, connectivity=26):
     """dmnerf_object_components + dmnerf_component_table: the connected components of the solid points (occ > level) of
     occ [dim]^3 float32, adjacency within one label of labels [dim]^3 int16 (None: one label) -> {"grid": int32 [dim]^3 on the
     device (component id, -1 where not solid), "label": int16 [n], "voxels": int64 [n], "root": int64 [n] (the component's
-    smallest C-order linear index)}; ids ascend with the root."""
+    smallest C-order linear index)}; ids ascend with the root.  An edited grid (edited_sweep) is accepted unchanged."""
     dim = _check_grid(occ, labels, "object_components")
     ctx = get_context(occ.device)
     grid = torch.empty(occ.shape, dtype=torch.int32, device=occ.device)

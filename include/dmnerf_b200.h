@@ -416,6 +416,36 @@ DMNERF_API int dmnerf_mesh_label_rays(const float* verts, const float* normals, 
                                       void* stream);
 DMNERF_API int dmnerf_argmax_rows(const float* x, int64_t n, int c, int64_t* out, void* stream);
 
+/* ---- meshing an edited scene (DESIGN.md, "Meshing an edited scene"; no counterpart in the original) -------------------------
+ * dmnerf_mesh_occupancy_edit: object moves applied per grid point to a labelled sweep.  occ / labels [dim^3] (DEVICE, in-out) hold
+ *   the unedited keep-all sweep of network `net` on the grid of (transform_host, extents_host, dim) with this voxel; moves_host
+ *   (HOST, n_moves in [0, DMNERF_MAX_MOVES]) are applied in order, each to the result of the previous ones.  Per move and grid
+ *   point p (the sweep's fp32 point): t = trans p in fp64, rounded once to fp32; the network runs at t (zero view directions)
+ *   only when its nearest grid index rint(A^-1 (t - b)) (the grid's index map, fp64) lies in the move's box.
+ *   take = in box && label(t) == label && (occ(t) > level || occ_p <= level) && (no piece || the piece keeps t):
+ *   (occ_p, label_p) = (occ(t), label).  Otherwise a point with label_p == label and occ_p > level that is in the piece (every
+ *   point without a piece) or whose move has rest_drop gets occ_p = 0, its label kept.  slab <= 0: 2^20 points per slab.  evaluated_host (may be NULL) receives the number of
+ *   target points evaluated.  Rejected on the host, before any launch: more than DMNERF_MAX_MOVES moves, a label outside
+ *   [0, ins_num], a non-finite trans or one whose 3x3 part has det <= 0, a box outside the grid or inverted (the empty box
+ *   (1, 0, 1, 0, 1, 0) is accepted and evaluates nothing), level outside (0, 1), a piece whose `applies` lacks the label.
+ *   Synchronises the stream once per slab and move (the number of boxed points sizes the network launch).
+ * dmnerf_mesh_vertex_labels: out [n] (DEVICE int16) = the label (labels, DEVICE int16 [dim^3]) of the solid grid point
+ *   (occ > level) nearest to the index-space vertex verts [n,3] (DEVICE), among those closer than 2 (fp64 squared distances,
+ *   ((dx^2 + dy^2) + dz^2)); an exact tie goes to the lowest linear index; -1 when there is none.  For a marching-cubes vertex of
+ *   the same grid and level this is the inside end of its edge. */
+typedef struct dmnerf_edit_move {
+  int32_t label;
+  int32_t rest_drop;          /* 1: the solid points of the label outside the piece are vacated too */
+  double trans[12];           /* row-major 3x4 of the move, network frame: the edited scene shows at p what the network has at trans p */
+  int32_t box[6];             /* inclusive index box (i_lo, i_hi, j_lo, j_hi, k_lo, k_hi) of the target points evaluated */
+  dmnerf_region piece;        /* bits NULL: the whole label moves */
+} dmnerf_edit_move;
+DMNERF_API int dmnerf_mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
+                                          float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host, int n_moves,
+                                          float* occ, int16_t* labels, int64_t* evaluated_host, void* stream);
+DMNERF_API int dmnerf_mesh_vertex_labels(const float* verts, int64_t n, const float* occ, const int16_t* labels, int dim, float level,
+                                         int16_t* out, void* stream);
+
 /* ---- object inventory (DESIGN.md, "Object inventory"; no counterpart in the original) ---------------------------------------
  * Per-group reductions over the solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order of the index (i, j, k)).
  * labels [dim^3] (DEVICE int16, may be NULL: every point is group 0) assigns each point its group 0 .. n_labels - 1.

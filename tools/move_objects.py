@@ -4,7 +4,7 @@
     python tools/move_objects.py CHECKPOINT.tar --pose POSE.npy --hwk H W K (--move-label L | --move-piece ID)
            --mode {translation,rotation,scale,multi} [--distance -0.25 --yaw 90 --scale 1.2] [--rest keep|drop]
            --transform T [--extents X Y Z] [--grid-dim 256] [--level 0.45] [--connectivity {6,26}] [--dilate 1] --out DIR
-           [--near 4 --far 15 --N-samples 64 --N-importance 128 --N-test 4096]
+           [--near 4 --far 15 --N-samples 64 --N-importance 128 --N-test 4096] [--mesh [--min-cluster 400]]
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict`.  POSE.npy holds the camera-to-world pose [4, 4] (or
 [3, 4]; of several [N, 4, 4] the first is used).  K is the 3x3 intrinsics, as a .npy file or as 9 numbers.
@@ -18,7 +18,9 @@ the rest of its label: `--move-label L --rest drop` moves object L without its f
 
 Writes DIR/rgb.png, DIR/instance.png (the arg-max label of the edited instance map; label k gets colour k of a fixed seeded
 palette, as tools/render_objects.py) and DIR/transform.json (the transformation dict, the moved label, piece and centre), and
-prints one JSON line."""
+prints one JSON line.  --mesh also writes DIR/edited.ply (the marching-cubes mesh of the edited scene, scene space) and
+DIR/color_edited.ply (the cleaned mesh, every vertex in its label's colour of instance.png) of the same edit: the same piece,
+rest and transformation, applied per grid point to the labelled sweep (DESIGN.md, "Meshing an edited scene")."""
 import argparse
 import json
 import os
@@ -57,6 +59,8 @@ def parse(argv=None):
     ap.add_argument("--N-importance", type=int, default=128)
     ap.add_argument("--N-test", type=int, default=4096, help="rays per edit call")
     ap.add_argument("--device", default="cuda")
+    ap.add_argument("--mesh", action="store_true", help="also write edited.ply and color_edited.ply of the edit")
+    ap.add_argument("--min-cluster", type=int, default=400, help="--mesh: smallest triangle cluster kept in color_edited.ply")
     a = ap.parse_args(argv)
     if a.dilate < 0:
         ap.error("--dilate must be >= 0")
@@ -134,6 +138,16 @@ def main(argv=None):
     write_png(os.path.join(a.out, "instance.png"), colorize(argmax_rows(ins).reshape(a.H, a.W), lut).cpu().numpy())
     record = {"transformations": trans["transformations"], "label": label, "piece": piece, "centre": centre.tolist(),
               "rest": a.rest}
+    if a.mesh:
+        from dmnerf_b200.objects import edited_mesh
+        m = edited_mesh(nets[1], T, [(label, trans["transformations"][0]["transformation"])], a.grid_dim, ext, a.level, a.near,
+                        a.far, a.N_importance, pieces=[region], rest=a.rest, min_cluster=a.min_cluster)
+        M.write_ply(os.path.join(a.out, "edited.ply"), m["vertices"], m["triangles"])
+        lab = m["labels"].cpu().numpy()
+        colors = np.where((lab >= 0)[:, None], lut[np.clip(lab, 0, ins_num)], 0).astype(np.uint8)   # instance.png's colours
+        M.write_ply(os.path.join(a.out, "color_edited.ply"), m["clean_vertices"], m["clean_triangles"], colors)
+        record["mesh"] = {"vertices": int(m["vertices"].shape[0]), "triangles": int(m["triangles"].shape[0]),
+                          "clean_vertices": int(m["clean_vertices"].shape[0]), "clean_triangles": int(m["clean_triangles"].shape[0])}
     with open(os.path.join(a.out, "transform.json"), "w") as fh:
         json.dump(record, fh, indent=1)
     print(json.dumps(dict(record, files=sorted(os.listdir(a.out)))))
