@@ -5,8 +5,9 @@
 //     Honours the reference's detach topology (render.py:22-23: the instance map sees detached weights).
 //   * MLP backward over the activations saved by the training forward (ActPlanes), with the heads folded like in the forward
 //     (mlp_backward_chain): the gradient chain of bwd_chain.cu carries dY through the trunk, batched split-bf16 wgmma GEMMs
-//     (gemm_umma.cu) form the weight gradients, small fp32 products give the folded head layers.  Gradient routing is the
-//     reference's (dm_nerf.py:95: the instance branch reads h.detach(), so it contributes to ins_feature_linear and below only).
+//     (gemm_umma.cu) form the weight gradients at every object-head width, small fp32 products give the folded head layers.
+//     Gradient routing is the reference's (dm_nerf.py:95: the instance branch reads h.detach(), so it contributes to
+//     ins_feature_linear and below only).
 
 #include "ray_ops.cuh"
 #include "network.cuh"
@@ -132,172 +133,6 @@ int launch_composite_backward(const float* raw, const float* z, const float* ray
   return 0;
 }
 
-// ================================================================================================ fp32 dW GEMMs
-// The weight-gradient products the wgmma kernel does not take (gemm_tn_tc_supported): on this network only ins_linear with more
-// than 64 instance logits.
-constexpr int GT = 64;      // output tile GT x GT
-constexpr int GK = 16;      // inner chunk
-
-// part[split][n][k] = sum_{m in split} A[m, n] B[m, k]   (reduce_splits_kernel adds the splits into C in split order)
-__global__ void __launch_bounds__(256) gemm_tn_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                      float* __restrict__ part, int64_t M, int N, int K, int64_t rows_per_split) {
-  __shared__ float As[GK][GT];
-  __shared__ float Bs[GK][GT];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int n0 = blockIdx.x * GT, k0 = blockIdx.y * GT;
-  const int64_t mb = (int64_t)blockIdx.z * rows_per_split;
-  const int64_t me = (mb + rows_per_split < M) ? mb + rows_per_split : M;
-  float acc[4][4] = {};
-  for (int64_t m0 = mb; m0 < me; m0 += GK) {
-    for (int idx = tid; idx < GK * GT; idx += 256) {
-      const int r = idx / GT, c = idx % GT;
-      const int64_t m = m0 + r;
-      As[r][c] = (m < me && n0 + c < N) ? A[m * lda + n0 + c] : 0.0f;
-      Bs[r][c] = (m < me && k0 + c < K) ? B[m * ldb + k0 + c] : 0.0f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < GK; ++kk) {
-      float a[4], b[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) a[i] = As[kk][ty + 16 * i];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) b[j] = Bs[kk][tx + 16 * j];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-  float* mine = part + (size_t)blockIdx.z * N * K;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int nn = n0 + ty + 16 * i;
-    if (nn >= N) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int k = k0 + tx + 16 * j;
-      if (k < K) mine[(size_t)nn * K + k] = acc[i][j];
-    }
-  }
-}
-
-// 128x128 register-tiled variant for operands whose widths and row strides are multiples of 4 floats (e.g. ins_num 127); the
-// generic kernel above takes the other widths (e.g. ins_num 93).
-constexpr int BT = 128;     // output tile BT x BT, 256 threads, 8x8 outputs per thread
-constexpr int BK = 8;       // inner slice
-
-__device__ __forceinline__ void fma_8x8(float (&acc)[8][8], const float* __restrict__ as, const float* __restrict__ bs, int ty, int tx) {
-  const float4 a0 = *reinterpret_cast<const float4*>(as + ty * 8), a1 = *reinterpret_cast<const float4*>(as + ty * 8 + 4);
-  const float4 b0 = *reinterpret_cast<const float4*>(bs + tx * 8), b1 = *reinterpret_cast<const float4*>(bs + tx * 8 + 4);
-  const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-  const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-}
-
-// part[split][n][k] = sum_{m in split} A[m, n] B[m, k].  N % 4 == 0, K % 4 == 0, lda/ldb % 4 == 0; rows_per_split % 8 == 0.
-__global__ void __launch_bounds__(256) gemm_tn_big_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                          float* __restrict__ part, int64_t M, int N, int K, int64_t rows_per_split) {
-  __shared__ __align__(16) float As[2][BK][BT];
-  __shared__ __align__(16) float Bs[2][BK][BT];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int n0 = blockIdx.x * BT, k0 = blockIdx.y * BT;
-  const int64_t mb = (int64_t)blockIdx.z * rows_per_split;
-  const int64_t me = (mb + rows_per_split < M) ? mb + rows_per_split : M;
-  const int lr = tid >> 5, lc = (tid & 31) * 4;         // slice row lr (sample), columns lc..lc+3
-  float acc[8][8] = {};
-  float4 ra, rb;
-  auto load = [&](int64_t m0) {
-    const int64_t m = m0 + lr;
-    const bool ok = m < me;
-    ra = (ok && n0 + lc < N) ? *reinterpret_cast<const float4*>(A + m * lda + n0 + lc) : make_float4(0.f, 0.f, 0.f, 0.f);
-    rb = (ok && k0 + lc < K) ? *reinterpret_cast<const float4*>(B + m * ldb + k0 + lc) : make_float4(0.f, 0.f, 0.f, 0.f);
-  };
-  auto stash = [&](int buf) {
-    *reinterpret_cast<float4*>(&As[buf][lr][lc]) = ra;
-    *reinterpret_cast<float4*>(&Bs[buf][lr][lc]) = rb;
-  };
-  load(mb);
-  stash(0);
-  __syncthreads();
-  int buf = 0;
-  for (int64_t m0 = mb; m0 < me; m0 += BK) {
-    if (m0 + BK < me) load(m0 + BK);
-#pragma unroll
-    for (int kk = 0; kk < BK; ++kk) fma_8x8(acc, As[buf][kk], Bs[buf][kk], ty, tx);
-    if (m0 + BK < me) stash(buf ^ 1);
-    __syncthreads();
-    buf ^= 1;
-  }
-  float* mine = part + (size_t)blockIdx.z * N * K;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int nn = n0 + ty * 8 + i;
-    if (nn >= N) continue;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int k = k0 + tx * 8 + j;
-      if (k < K) mine[(size_t)nn * K + k] = acc[i][j];
-    }
-  }
-}
-
-// C[n, k] += sum_split part[split][n][k], the splits added in order (reproducible bit for bit).  A block owns 32 consecutive
-// entries; its 8 warps take the splits round robin and their 8 sums are added in warp order.
-__global__ void __launch_bounds__(256) reduce_splits_kernel(const float* __restrict__ part, int splits, int N, int K,
-                                                            float* __restrict__ Cm, int ldc) {
-  __shared__ float red[8][32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t nk = (int64_t)N * K, e = (int64_t)blockIdx.x * 32 + lane;
-  float s = 0.0f;
-  if (e < nk)
-    for (int z = warp; z < splits; z += 8) s += __ldcs(part + (size_t)z * nk + e);
-  red[warp][lane] = s;
-  __syncthreads();
-  if (warp == 0 && e < nk) {
-    float t = 0.0f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) t += red[w][lane];
-    Cm[(size_t)(e / K) * ldc + e % K] += t;
-  }
-}
-
-// Splits of the fp32 dW GEMMs: at most this many for m samples (the split heights below are at least 256 rows, the counts at
-// most 4 * 132), each a [N x K] partial with N * K <= TN_PART_ENTRIES (ins_linear: up to 128 logits x 128 hidden units).
-constexpr int64_t TN_MAX_SPLITS = 4 * 132;
-constexpr int64_t TN_PART_ENTRIES = 128 * 128;
-static int64_t tn_part_floats(int64_t m) {
-  const int64_t s = (m + 255) / 256;
-  return (s < TN_MAX_SPLITS ? s : TN_MAX_SPLITS) * TN_PART_ENTRIES;
-}
-
-// C[n, k] += sum_m A[m, n] B[m, k] (C zero-initialised by the caller); part: tn_part_floats(M) floats of scratch.
-static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K, float* part,
-                   cudaStream_t st) {
-  DMN_CHECK((int64_t)N * K <= TN_PART_ENTRIES, "mlp_backward: %d x %d weight gradient exceeds the split scratch", N, K);
-  const bool aligned = ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0);
-  const bool big = aligned && N % 4 == 0 && K % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 && N >= 64 && K >= 64;
-  const int tile = big ? BT : GT, step = big ? BK : GK, min_rows = big ? 512 : 256;
-  const int tiles = ((N + tile - 1) / tile) * ((K + tile - 1) / tile);
-  int64_t splits = ((big ? 3 : 4) * 132 + tiles - 1) / tiles;
-  int64_t rows = (M + splits - 1) / splits;
-  rows = ((rows + step - 1) / step) * step;
-  if (rows < min_rows) rows = min_rows;
-  splits = (M + rows - 1) / rows;
-  DMN_CHECK(splits * N * K <= tn_part_floats(M), "mlp_backward: %lld splits exceed the split scratch", (long long)splits);
-  dim3 grid((unsigned)((N + tile - 1) / tile), (unsigned)((K + tile - 1) / tile), (unsigned)splits);
-  if (big) gemm_tn_big_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, part, M, N, K, rows);
-  else gemm_tn_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, part, M, N, K, rows);
-  DMN_LAUNCH_OK();
-  reduce_splits_kernel<<<(unsigned)(((int64_t)N * K + 31) / 32), 256, 0, st>>>(part, (int)splits, N, K, C, ldc);
-  DMN_LAUNCH_OK();
-  return 0;
-}
-
 // Column sums of d_out (the output-layer bias gradients) in a fixed order: pass 1 gives one partial row per block (warps over
 // rows, lanes over 32 columns, the 8 warp sums added in warp order), pass 2 adds the partial rows in block order.
 constexpr int COLSUM_BLOCKS = 4 * 132;
@@ -343,10 +178,9 @@ static int colsum_fixed(const float* A, int C, int64_t m, float* part, float* ou
   return 0;
 }
 
-// [S1 | S2], dY0..dY7, [S1 | S2]^T h7, its column sums, the column sums of d_out, then the partial rows of those column sums and
-// the split partials of the fp32 dW GEMMs
+// [S1 | S2], dY0..dY7, [S1 | S2]^T h7, its column sums, the column sums of d_out, then the partial rows of those column sums
 size_t mlp_backward_scratch_floats(int64_t m) {
-  return (size_t)m * (256 + 8 * 256) + 256 * 256 + 256 + 256 + (size_t)COLSUM_BLOCKS * COLSUM_MAX_C + (size_t)tn_part_floats(m);
+  return (size_t)m * (256 + 8 * 256) + 256 * 256 + 256 + 256 + (size_t)COLSUM_BLOCKS * COLSUM_MAX_C;
 }
 
 // Small dense products of the folded head gradients (128..256 x 256 outputs, contraction 128..256): 16 x 16 output tiles, one
@@ -422,7 +256,6 @@ static int mlp_backward_chain(const Network& net, float* acts, const float* d_ou
   float* c12 = PQ + 256 * 256;                        // column sums of S1 | S2
   float* cs = c12 + 256;                              // column sums of d_out [C]
   float* cs_part = cs + 256;                          // their partial rows [COLSUM_BLOCKS][C]
-  float* tn_part = cs_part + (size_t)COLSUM_BLOCKS * COLSUM_MAX_C;        // split partials of the fp32 dW GEMM
   float* P = PQ, *Q = PQ + 128 * 256, *c1 = c12, *c2 = c12 + 128;
   auto gw = [&](int l) { return grads[2 * l]; };
   auto gb = [&](int l) { return grads[2 * l + 1]; };
@@ -431,8 +264,10 @@ static int mlp_backward_chain(const Network& net, float* acts, const float* d_ou
 #define R(x) do { if ((rc = (x))) return rc; } while (0)
   // Every weight-gradient product of the network contracts over the same m samples and all their operands exist once the
   // gradient chain has run: they are queued by shape class and each class goes out as ONE batched tensor-core launch
-  // (launch_gemm_tn_tc_batch) -- 3 GEMM + 3 reduction launches per network instead of 14 + 14.
-  struct Queue { TnProblem p[TN_MAX_BATCH]; int n = 0, N = 0; } q_wide, q_in256, q_in128;      // [256 x 256], [256 x <=64], [128 x <=64]
+  // (launch_gemm_tn_tc_batch) -- 3 GEMM + 3 reduction launches per network instead of 14 + 14, one more pair for ins_linear
+  // with more than 64 instance logits.
+  struct Queue { TnProblem p[TN_MAX_BATCH]; int n = 0, N = 0; };
+  Queue q_wide, q_in256, q_in128, q_ins;      // [256 x 256], [256 x <=64], [128 x <=64], [128 x 65..128]
   auto flush = [&](Queue& q) -> int {
     const int r = q.n ? launch_gemm_tn_tc_batch(q.p, q.n, m, q.N, partial, net.status.device(), st) : 0;
     q.n = 0;
@@ -446,13 +281,11 @@ static int mlp_backward_chain(const Network& net, float* acts, const float* d_ou
       pr.A = A; pr.lda = lda; pr.B = B; pr.ldb = ldb; pr.K = K; pr.transpose = 0; pr.colsum = colsum_out; pr.b_cm = b_cm;
       q = (K > 64) ? &q_wide : (N == 256 ? &q_in256 : &q_in128);
       q->N = N;
-    } else if (!colsum_out && !b_cm && K > 64 && gemm_tn_tc_supported(K, N)) {      // narrow dY, wide X: (X^T dY)^T
-      pr.A = B; pr.lda = ldb; pr.B = A; pr.ldb = lda; pr.K = N; pr.transpose = 1; pr.colsum = nullptr; pr.b_cm = 0;
-      q = (K == 256) ? &q_in256 : &q_in128;
-      q->N = K;
-    } else {
+    } else {                                                    // narrow dY, wide X: (X^T dY)^T
       DMN_CHECK(!colsum_out && !b_cm, "mlp_backward: no kernel for the %d x %d weight gradient", N, K);
-      return gemm_tn(A, lda, B, ldb, Cw, ldc, m, N, K, tn_part, st);
+      pr.A = B; pr.lda = ldb; pr.B = A; pr.ldb = lda; pr.K = N; pr.transpose = 1; pr.colsum = nullptr; pr.b_cm = 0;
+      q = (K == 256) ? &q_in256 : (N <= 64 ? &q_in128 : &q_ins);
+      q->N = K;
     }
     pr.ldc = ldc; pr.C = Cw;
     if (q->n == TN_MAX_BATCH) { const int r = flush(*q); if (r) return r; }
@@ -479,6 +312,7 @@ static int mlp_backward_chain(const Network& net, float* acts, const float* d_ou
   R(dW(d_ins, C, ap.ins_hid, 128, gw(L_INS_OUT), 128, ins1, 128));
   R(dW(S12, 256, ap.emb + (int64_t)CH_POS * m, CH_IN, gw(L_RGB_HID) + 256, 283, 128, CH_DIR, nullptr, m));
   R(flush(q_in128));
+  R(flush(q_ins));
   // the three output bias gradients from one sweep over d_out
   R(colsum_fixed(d_out, C, m, cs_part, cs, st));
   DMN_CUDA(cudaMemcpyAsync(gb(L_RGB_OUT), cs, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));

@@ -204,8 +204,9 @@ __global__ void __launch_bounds__(NN_THREADS, 1) gemm_nn_tc_kernel(const float* 
 }
 
 // ------------------------------------------------------------------------------------------------ gemm_tn
-// P[NA, NB] = A[mb:me, 0:NA]^T * B[mb:me, 0:nb] for this CTA's rows; the CTA computes one [128 x NBT] tile of P (NBT = 128, or
-// 64 with nb <= 64 valid columns) over 32 samples per stage.  Both operands are MN-major (the samples are the contraction index).
+// P[NA, NB] = A[mb:me, 0:NA]^T * B[mb:me, 0:nb] for this CTA's rows; the CTA computes one [128 x NBT] tile of P (NBT = 64 with
+// NB = 64, else 128; columns from nb on are zero) over 32 samples per stage.  Both operands are MN-major (the samples are the
+// contraction index).
 // Every CTA writes its partial product to its own slice of a scratch buffer; reduce_partials_kernel adds the slices into the
 // gradient in a fixed order.  colsum != NULL: colsum[n] += sum over the rows of A[:, n] (the bias gradient, from the registers
 // that already hold A); each CTA sums its rows in a fixed order into one row of column sums per slice, which
@@ -373,8 +374,8 @@ static int vec4_ok(const void* p, int ld) { return ((uintptr_t)p % 16 == 0) && (
 
 }  // namespace tg
 
-// Shapes the dW kernel is specialised for (the rest goes to the fp32 CUDA-core kernels of backward.cu).
-bool gemm_tn_tc_supported(int N, int K) { return (N == 128 || N == 256) && (K == 256 || (K >= 1 && K <= 64)); }
+// Shapes the dW kernel is specialised for.
+bool gemm_tn_tc_supported(int N, int K) { return (N == 128 || N == 256) && (K == 256 || (K >= 1 && K <= 128)); }
 
 // C[M,256] (+)= A[M,N] W[N,256], N = 128 or 256, masked by mask_bits when given.
 int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C, int ldc, int64_t M, int N, int accumulate,
@@ -400,26 +401,26 @@ int launch_gemm_nn_tc(const float* A, int lda, const float* W, int ldw, float* C
   return 0;
 }
 
-// For every product i < n:  C_i[N, K_i] += A_i[M, N]^T B_i[M, K_i]  (N = 128 or 256; every K_i = 256, or every K_i <= 64);
-// transpose != 0: the caller passes the WIDE matrix as A and the narrow one (K <= 64 columns) as B and wants C[K, N] += B^T A.
-// One GEMM launch + one reduction launch for the whole batch.
+// For every product i < n:  C_i[N, K_i] += A_i[M, N]^T B_i[M, K_i]  (N = 128 or 256; the K_i of one batch are all in one class
+// NB: K_i <= 64 -> 64, 65..128 -> 128, 256 -> 256); transpose != 0: the caller passes the WIDE matrix as A and the narrow one
+// (K <= 128 columns) as B and wants C[K, N] += B^T A.  One GEMM launch + one reduction launch for the whole batch.
 int launch_gemm_tn_tc_batch(const TnProblem* probs, int n, int64_t M, int N, DeviceBuffer& partial, int32_t* status,
                             cudaStream_t st) {
   using namespace tg;
   if (M <= 0 || n <= 0) return 0;
   DMN_CHECK(n <= TN_MAX_BATCH, "gemm_tn(tc): %d products in one batch (max %d)", n, TN_MAX_BATCH);
-  const int NB = (probs[0].K > 64) ? 256 : 64;
+  auto nb_class = [](int K) { return K <= 64 ? 64 : K <= 128 ? 128 : 256; };
+  const int NB = nb_class(probs[0].K);
   TnBatch batch;
   memset(&batch, 0, sizeof(batch));
   for (int i = 0; i < n; ++i) {
     const int K = probs[i].K;
-    DMN_CHECK((N == 128 || N == 256) && K >= 1 && K <= 256 && ((K > 64) ? 256 : 64) == NB && (NB == 64 || K == 256),
-              "gemm_tn(tc): shape %d x %d not supported", N, K);
+    DMN_CHECK(gemm_tn_tc_supported(N, K) && nb_class(K) == NB, "gemm_tn(tc): shape %d x %d not supported", N, K);
     batch.p[i] = probs[i];
     batch.vec_a[i] = vec4_ok(probs[i].A, probs[i].lda);
     batch.vec_b[i] = vec4_ok(probs[i].B, probs[i].ldb);
   }
-  const int NBT = NB == 256 ? 128 : 64;
+  const int NBT = NB == 64 ? 64 : 128;
   const int tiles = (N / 128) * (NB / NBT);
   int sms = 0;
   if (sm_count(&sms)) return 2;

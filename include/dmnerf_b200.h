@@ -247,8 +247,7 @@ DMNERF_API int dmnerf_mlp_forward_train(dmnerf_ctx* ctx, int net, const float* x
  * scratch: dmnerf_mlp_backward_scratch_floats(m) floats.  flags is a flag word: bit 0 = the forward wrote the ReLU bit planes
  * (tensor-core forward), bit 1 = the caller has already zero-filled `grads` (one fill instead of 30 memsets).
  * The heads are folded like in the forward, one masked split-bf16 wgmma GEMM per layer carries the gradient through the trunk
- * and batched wgmma GEMMs form the weight gradients (on the CUDA cores for ins_linear with more than 64 instance logits), for
- * any M. */
+ * and batched wgmma GEMMs form the weight gradients, for any M. */
 DMNERF_API int dmnerf_mlp_backward(dmnerf_ctx* ctx, int net, float* acts, const float* d_out, int64_t m, float* const* grads,
                         float* scratch, int flags, void* stream);
 

@@ -195,8 +195,9 @@ WIDTHS = [1, 13, 59, 63, 64, 67, 69, 93, 127]
 @pytest.mark.parametrize("ins_num", WIDTHS)
 def test_backward_matches_teacher_forced_fp64(ins_num, impl, m):
     """All 30 gradients within the exact-forward bounds with either forward.  ins_num 63 / 64 sit on either side of the
-    64-logit switch of the ins_linear weight gradient (tensor cores / fp32 CUDA cores); 67 and 127 take the 128x128 fp32 kernel,
-    64, 69 and 93 the generic one.  Batch sizes around the 32-sample stage and the 128-row tile."""
+    64-logit switch of the ins_linear weight gradient from the 64-column to the 128-column tensor-core tile; 64, 67, 69, 93
+    and 127 take ragged and full 128-column tiles, aligned and unaligned rows.  Batch sizes around the 32-sample stage and the
+    128-row tile."""
     net = _net(ins_num, 40 + ins_num)
     x = _x_inputs(m, 7 * m + ins_num)
     d_out = torch.randn(m, 5 + ins_num, generator=torch.Generator().manual_seed(m + ins_num)).to(DEV)

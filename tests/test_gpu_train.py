@@ -222,7 +222,7 @@ def test_mlp_backward_tensor_core_gemms(ins_num, m):
     by layer; with the exact-fp32 forward the 30 parameter gradients must still agree with torch autograd on the oracle to fp32
     noise.  1333 samples: ten full 128-row tiles + a ragged one, 32-sample stages with a ragged tail; 1, 37 and 511 samples: a
     single sample, a tail shorter than one 32-sample stage, one row short of four full tiles.  ins_num = 127 is the widest
-    object head the library accepts (128 instance logits; its weight gradient runs on the fp32 CUDA-core kernels)."""
+    object head the library accepts (128 instance logits: a full 128-column tile of the ins_linear weight gradient)."""
     w = synth.make_weights(21, ins_num)
     p = O.to_torch(w)
     for v in p.values():
