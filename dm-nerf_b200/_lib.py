@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# DMNERF_LIB_PATH: diagnostics builds of the same ABI (tools/kprof.py); the default is the in-tree product library
+# DMNERF_LIB_PATH: diagnostics builds of the same ABI; the default is the in-tree product library
 LIB_PATH = os.environ.get("DMNERF_LIB_PATH") or os.path.join(_HERE, "lib", "libdmnerf_b200.so")
 
 ABI_VERSION = 4

@@ -9,20 +9,15 @@ Rays/s: median of --reps frames per variant, the variants alternated frame by fr
 appearance is set and cleared around every frame, as render_frame does.  Nothing is written to disk."""
 import argparse
 import json
-import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import objects as OB                         # noqa: E402
-from dmnerf_b200 import synth                                 # noqa: E402
-from dmnerf_b200.render import render_frame                   # noqa: E402
-from dmnerf_b200.testing import make_models                   # noqa: E402
+from _harness import alternate, cuda_device, gpu_identity, host_ms
+from dmnerf_b200 import objects as OB
+from dmnerf_b200 import synth
+from dmnerf_b200.render import render_frame
+from dmnerf_b200.testing import make_models
 
 
 def frames(name, reps, dev):
@@ -36,17 +31,12 @@ def frames(name, reps, dev):
                 "tint_all": {"appearance": OB.Appearance(ins_num, colour=tinted)},
                 "tint_density_half": {"appearance": OB.Appearance(ins_num, colour=tinted,
                                                                   density={k: 0.3 for k in everything[::2]})}}
-    times = {k: [] for k in variants}
+
+    def frame(kw):
+        return lambda: render_frame(H, W, wl["K"], wl["c2w"], wl["near"], wl["far"], nc, nf, device=dev, **kw)
     with torch.no_grad():
-        for r in range(reps + 1):
-            for k, kw in variants.items():
-                torch.cuda.synchronize()
-                t0 = time.perf_counter()
-                render_frame(H, W, wl["K"], wl["c2w"], wl["near"], wl["far"], nc, nf, device=dev, **kw)
-                torch.cuda.synchronize()
-                if r:
-                    times[k].append(time.perf_counter() - t0)
-    rate = {k: H * W / float(np.median(v)) for k, v in times.items()}
+        ms = alternate({k: frame(kw) for k, kw in variants.items()}, reps, clock=host_ms)
+    rate = {k: H * W / (float(np.median(v)) * 1e-3) for k, v in ms.items()}
     return {"workload": name, "ins_num": ins_num, "rays_per_s": rate,
             "tint_all_vs_keep_all": rate["tint_all"] / rate["keep_all"],
             "tint_density_half_vs_keep_all": rate["tint_density_half"] / rate["keep_all"]}
@@ -56,16 +46,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "tools/appearance_bench.py needs a CUDA device; there is no CPU fallback"
-    dev = torch.device("cuda", 0)
+    dev = cuda_device("appearance_bench.py")
     runs = [frames(n, a.reps, dev) for n in ("dmsr_study", "replica_room0_93")]
-    try:
-        gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=20).stdout.strip()
-    except Exception as exc:
-        gpu = "nvidia-smi unavailable: %s" % exc
-    print(json.dumps({"metric": "object appearance cost", "reps": a.reps, "frames": runs, "gpu": gpu,
-                      "gpu_name": torch.cuda.get_device_name(dev),
+    name, smi, _ = gpu_identity(dev)
+    print(json.dumps({"metric": "object appearance cost", "reps": a.reps, "frames": runs, "gpu": smi, "gpu_name": name,
                       "what": "640x480 frames through the frame driver (host maps), rays/s median of %d, variants alternated"
                               % a.reps}))
 

@@ -10,31 +10,23 @@ events around each call, median of --reps after one warm-up; the sweep is timed 
 label (int16) grids over the call's time.  Nothing is written to disk."""
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import objects as OB                         # noqa: E402
-from dmnerf_b200.testing import make_models                   # noqa: E402
-from oracle.components_oracle import serpentine               # noqa: E402
+from _harness import cuda_device, event_ms, gpu_identity
+from dmnerf_b200 import objects as OB
+from dmnerf_b200.testing import make_models
+from oracle.components_oracle import serpentine
 
 
 def timed(fn, reps):
-    out, ms = None, []
-    for r in range(reps + 1):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        out = fn()
-        b.record()
-        torch.cuda.synchronize()
-        if r or reps == 0:
-            ms.append(a.elapsed_time(b))
-    return out, float(np.median(ms))
+    """(result, median ms) of reps calls after one warm-up; at reps 0 the time of the one cold call."""
+    ms = []
+    for _ in range(reps + 1):
+        t, out = event_ms(fn)
+        ms.append(t)
+    return out, float(np.median(ms[1:] or ms))
 
 
 def components(occ, labels, level, reps):
@@ -70,8 +62,7 @@ def main():
     ap.add_argument("--grid-dims", type=int, nargs="+", default=[256, 512])
     ap.add_argument("--reps", type=int, default=3)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "tools/components_bench.py needs a CUDA device; there is no CPU fallback"
-    dev = torch.device("cuda", 0)
+    dev = cuda_device("components_bench.py")
     runs = []
     for dim in a.grid_dims:
         for k in (13, 93):
@@ -82,13 +73,8 @@ def main():
                      "object_components": components(occ, None, 0.45, a.reps)})
         del occ
         torch.cuda.empty_cache()
-    try:
-        gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=20).stdout.strip()
-    except Exception as exc:
-        gpu = "nvidia-smi unavailable: %s" % exc
-    print(json.dumps({"metric": "connected components device time", "reps": a.reps, "runs": runs, "gpu": gpu,
-                      "gpu_name": torch.cuda.get_device_name(dev),
+    name, smi, _ = gpu_identity(dev)
+    print(json.dumps({"metric": "connected components device time", "reps": a.reps, "runs": runs, "gpu": smi, "gpu_name": name,
                       "what": "object_components (labelling, per-component table, read-backs) per connectivity; the whole "
                               "inventory_from_grid with components='largest' and without, trim 0.01, against one selected "
                               "sweep; CUDA events, median of %d after one warm-up; GB/s = occ + label grid bytes over the "

@@ -11,31 +11,24 @@ grid's centre.  CUDA events, mean of --reps runs after one warm-up; the edit pas
 round trips.  Nothing is written to disk."""
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import objects as OB                         # noqa: E402
-from dmnerf_b200.testing import make_models                   # noqa: E402
+from _harness import cuda_device, event_ms, gpu_identity
+from dmnerf_b200 import objects as OB
+from dmnerf_b200.testing import make_models
 
 NEAR, FAR, N_IMPORTANCE, EXT = 4.0, 15.0, 128, (1.9, 7.0, 7.0)
 
 
 def _timed(fn, reps):
+    """(mean ms, result) of reps calls after one warm-up: the mean, not the median, is what DESIGN.md quotes of this bench."""
     fn()
-    out, ms = None, []
+    ms = []
     for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        out = fn()
-        b.record()
-        torch.cuda.synchronize()
-        ms.append(a.elapsed_time(b))
+        t, out = event_ms(fn)
+        ms.append(t)
     return float(np.mean(ms)), out
 
 
@@ -44,8 +37,7 @@ def main():
     ap.add_argument("--grid-dim", type=int, default=256)
     ap.add_argument("--reps", type=int, default=2)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "tools/edit_mesh_bench.py needs a CUDA device; there is no CPU fallback"
-    dev = torch.device("cuda", 0)
+    dev = cuda_device("edit_mesh_bench.py")
     dim = a.grid_dim
     T = np.eye(4)
     T[:3, 3] = (0.1, -0.2, 0.3)
@@ -88,13 +80,9 @@ def main():
                                   "evaluated_fraction": evaluated / dim ** 3, "edit_over_sweep": edit_ms / sweep_ms,
                                   "edited_mesh_ms": mesh_ms, "clean_vertices": int(m["clean_vertices"].shape[0])})
             del occ0, lab0
-    try:
-        gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=20).stdout.strip()
-    except Exception as exc:
-        gpu = "nvidia-smi unavailable: %s" % exc
+    name, smi, _ = gpu_identity(dev)
     print(json.dumps({"metric": "edited mesh device time", "grid_dim": dim, "reps": a.reps, "cases": cases,
-                      "gpu": gpu, "gpu_name": torch.cuda.get_device_name(dev),
+                      "gpu": smi, "gpu_name": name,
                       "what": "unedited keep-all sweep, edit pass on a copy of it, whole edited_mesh (sweep + edit + marching "
                               "cubes + cleanup + vertex labels) with explicit boxes; synthetic trained-like networks; CUDA events, "
                               "mean of %d runs after one warm-up" % a.reps}))

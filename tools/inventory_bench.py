@@ -8,30 +8,22 @@ Every pass ends with its one device->host read (it synchronises), so a pass's ti
 each call, median of --reps after one warm-up.  Nothing is written to disk."""
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import objects as OB                         # noqa: E402
-from dmnerf_b200.testing import make_models                   # noqa: E402
+from _harness import cuda_device, event_ms, gpu_identity
+from dmnerf_b200 import objects as OB
+from dmnerf_b200.testing import make_models
 
 
 def timed(fn, reps):
-    out, ms = None, []
-    for r in range(reps + 1):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        out = fn()
-        b.record()
-        torch.cuda.synchronize()
-        if r:
-            ms.append(a.elapsed_time(b))
-    return out, float(np.median(ms))
+    """(result, median ms) of reps calls after one warm-up."""
+    ms = []
+    for _ in range(reps + 1):
+        t, out = event_ms(fn)
+        ms.append(t)
+    return out, float(np.median(ms[1:]))
 
 
 def one(ins_num, dim, reps, dev):
@@ -62,16 +54,11 @@ def main():
     ap.add_argument("--grid-dim", type=int, default=256)
     ap.add_argument("--reps", type=int, default=3)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "tools/inventory_bench.py needs a CUDA device; there is no CPU fallback"
-    dev = torch.device("cuda", 0)
+    dev = cuda_device("inventory_bench.py")
     runs = [one(k, a.grid_dim, a.reps, dev) for k in (13, 93)]
-    try:
-        gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=20).stdout.strip()
-    except Exception as exc:
-        gpu = "nvidia-smi unavailable: %s" % exc
-    print(json.dumps({"metric": "object inventory device time", "grid_dim": a.grid_dim, "reps": a.reps, "runs": runs, "gpu": gpu,
-                      "gpu_name": torch.cuda.get_device_name(dev),
+    name, smi, _ = gpu_identity(dev)
+    print(json.dumps({"metric": "object inventory device time", "grid_dim": a.grid_dim, "reps": a.reps, "runs": runs, "gpu": smi,
+                      "gpu_name": name,
                       "what": "selected sweep with the label grid, then each pass over the occ (fp32) + label (int16) grids "
                               "with its read-back; trim 0.01; CUDA events, median of %d after one warm-up; GB/s = grid bytes "
                               "read once over the pass time" % a.reps}))

@@ -9,22 +9,16 @@ import argparse
 import contextlib
 import io
 import json
-import os
-import sys
 import types
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from dmnerf_b200 import synth, tester as T                 # noqa: E402
-from dmnerf_b200.manipulator import manipulate_frame, rigid_rays   # noqa: E402
-from dmnerf_b200.embedder import get_embedder              # noqa: E402
-from dmnerf_b200.testing import make_models                # noqa: E402
-from eval_bench import gpu_info                            # noqa: E402
+from _harness import cuda_device, event_ms, gpu_identity, stages_ms
+from dmnerf_b200 import synth, tester as T
+from dmnerf_b200.manipulator import manipulate_frame, rigid_rays
+from dmnerf_b200.embedder import get_embedder
+from dmnerf_b200.testing import make_models
 
 H, W, INS_NUM = 480, 640, 13
 
@@ -39,15 +33,11 @@ def one(m, frames, warmup, nc, nf, pe, ve, K, pose, args):
     args.target_labels = [2 + 3 * k for k in range(m)]
     tars = [rigid_rays(H, W, K, _move(k), pose) for k in range(m)]
     to, td = torch.stack([t[0] for t in tars]), torch.stack([t[1] for t in tars])
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     ms = []
     for f in range(warmup + frames):
-        ev[0].record()
-        out = manipulate_frame(H, W, K, pose, to, td, pe, ve, nc, nf, args)
-        ev[1].record()
-        torch.cuda.synchronize()
+        t, out = event_ms(lambda: manipulate_frame(H, W, K, pose, to, td, pe, ve, nc, nf, args))
         if f >= warmup:
-            ms.append(ev[0].elapsed_time(ev[1]))
+            ms.append(t)
     per_px = (m + 1) * (448 + 128 * m)
     med = float(np.median(ms))
     return {"targets": m, "frame_ms": [round(v, 1) for v in ms], "frame_ms_median": round(med, 1),
@@ -59,11 +49,11 @@ def main():
     ap.add_argument("--frames", type=int, default=2)
     ap.add_argument("--warmup", type=int, default=1)
     a = ap.parse_args()
-    dev = torch.device("cuda")
+    dev = cuda_device("mani_bench.py")
     wl = synth.workload("dmsr_study")
     K = np.array(wl["K"], dtype=np.float32)
     pose = torch.from_numpy(np.asarray(wl["c2w"], dtype=np.float32)).to(dev)
-    nc, nf, _, _ = make_models(1, 2, INS_NUM, "cuda")
+    nc, nf, _, _ = make_models(1, 2, INS_NUM, dev)
     pe, ve = get_embedder(10)[0], get_embedder(4)[0]
     args = types.SimpleNamespace(N_test=4096, near=float(wl["near"]), far=float(wl["far"]), N_samples=64, N_importance=128,
                                  ins_num=INS_NUM)
@@ -84,17 +74,17 @@ def main():
         labels = torch.from_numpy(region).to(dev).reshape(-1).contiguous()
         valid_gt = torch.unique(torch.from_numpy(region))
         scratch = torch.empty(H * W, device=dev, dtype=torch.int32), torch.empty(1, device=dev, dtype=torch.int32)
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-        metric_ms = []
-        for f in range(2 + 5):
-            ev[0].record()
+
+        def metrics(f):
             with contextlib.redirect_stdout(io.StringIO()):
                 T._frame_metrics("mani_bench", f, rgb, gt_img, ins[:, :INS_NUM].contiguous(), labels, valid_gt, INS_NUM, None, *scratch)
-            ev[1].record()
-            torch.cuda.synchronize()
+        metric_ms = []
+        for f in range(2 + 5):
+            (t,), _ = stages_ms(lambda: metrics(f))     # one pair of events, reused every frame
             if f >= 2:
-                metric_ms.append(ev[0].elapsed_time(ev[1]))
-    name, power = gpu_info()
+                metric_ms.append(t)
+    name, _, card = gpu_identity(dev)
+    name, power = card or (name, "unknown")
     print(json.dumps({"bench": "mani_frame_640x480", "gpu": name, "power_limit": power, "ins_num": INS_NUM, "N_test": args.N_test,
                       "cases": cases, "metrics_ms": [round(v, 3) for v in metric_ms],
                       "metrics_ms_median": round(float(np.median(metric_ms)), 3)}))

@@ -12,21 +12,17 @@ networks (its label is the moved one), as a component_region dilated by one voxe
 samples), on random network outputs; median of 20 launches after 3 warm-ups.  Nothing is written to disk."""
 import argparse
 import json
-import os
-import subprocess
-import sys
 import types
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import objects as OB                                   # noqa: E402
-from dmnerf_b200 import synth                                           # noqa: E402
-from dmnerf_b200.embedder import get_embedder                           # noqa: E402
-from dmnerf_b200.manipulator import ExchangePieces, exchanger, manipulate_frame, piece_vote, rigid_rays   # noqa: E402
-from dmnerf_b200.testing import make_models                             # noqa: E402
+from _harness import alternate, cuda_device, event_ms, gpu_identity
+from dmnerf_b200 import objects as OB
+from dmnerf_b200 import synth
+from dmnerf_b200.embedder import get_embedder
+from dmnerf_b200.manipulator import ExchangePieces, exchanger, manipulate_frame, piece_vote, rigid_rays
+from dmnerf_b200.testing import make_models
 
 
 def largest_piece(nf, ins_num, dim, dev):
@@ -45,15 +41,6 @@ def largest_piece(nf, ins_num, dim, dev):
     return OB.component_region(cc, [piece], T, dilate=1), label, info
 
 
-def _timed(fn):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b)
-
-
 def frames(name, reps, sweep_dim, n_test, dev):
     wl = synth.workload(name)
     ins_num = wl["ins_num"]
@@ -68,13 +55,11 @@ def frames(name, reps, sweep_dim, n_test, dev):
     pe, ve = get_embedder(10)[0], get_embedder(4)[0]
     variants = {"whole_label": {}, "piece_keep": {"pieces": [region], "rest": "keep"},
                 "piece_drop": {"pieces": [region], "rest": "drop"}}
-    ms = {k: [] for k in variants}
+
+    def frame(kw):
+        return lambda: manipulate_frame(H, W, K, pose, tar_o[None], tar_d[None], pe, ve, nc, nf, args, **kw)
     with torch.no_grad():
-        for r in range(reps + 1):
-            for k, kw in variants.items():
-                t = _timed(lambda: manipulate_frame(H, W, K, pose, tar_o[None], tar_d[None], pe, ve, nc, nf, args, **kw))
-                if r:
-                    ms[k].append(t)
+        ms = alternate({k: frame(kw) for k, kw in variants.items()}, reps)
     frame_ms = {k: float(np.median(v)) for k, v in ms.items()}
     return {"workload": name, "ins_num": ins_num, "moved_label": label, "sweep_dim": sweep_dim, **info, "frame_ms": frame_ms,
             "piece_keep_vs_whole": frame_ms["piece_keep"] / frame_ms["whole_label"],
@@ -109,7 +94,7 @@ def kernels(wl, region, label, ins_num, n, dev):
         t = []
         for r in range(23):
             work.copy_(ori)
-            x = _timed(fn)
+            x, _ = event_ms(fn)
             if r >= 3:
                 t.append(x)
         out[k + "_ms"] = float(np.median(t))
@@ -123,16 +108,10 @@ def main():
     ap.add_argument("--sweep-dim", type=int, default=256)
     ap.add_argument("--n-test", type=int, default=4096)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "tools/mani_pieces_bench.py needs a CUDA device; there is no CPU fallback"
-    dev = torch.device("cuda", 0)
+    dev = cuda_device("mani_pieces_bench.py")
     runs = [frames(n, a.reps, a.sweep_dim, a.n_test, dev) for n in ("dmsr_study", "replica_room0_93")]
-    try:
-        gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=20).stdout.strip()
-    except Exception as exc:
-        gpu = "nvidia-smi unavailable: %s" % exc
-    print(json.dumps({"metric": "moving pieces cost", "reps": a.reps, "runs": runs, "gpu": gpu,
-                      "gpu_name": torch.cuda.get_device_name(dev),
+    name, smi, _ = gpu_identity(dev)
+    print(json.dumps({"metric": "moving pieces cost", "reps": a.reps, "runs": runs, "gpu": smi, "gpu_name": name,
                       "what": "640x480 edited frames (manipulate_frame, N_test %d), CUDA events, median of %d, variants "
                               "alternated; kernels: median of 20 launches" % (a.n_test, a.reps)}))
 

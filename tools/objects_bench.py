@@ -8,41 +8,17 @@
 Synthetic trained-like networks (the bench.py ones).       python tools/objects_bench.py [--reps 3]"""
 import argparse
 import json
-import os
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import numpy as np
+import torch
 
-import numpy as np   # noqa: E402
-import torch         # noqa: E402
-
-from dmnerf_b200 import synth                                   # noqa: E402
-from dmnerf_b200 import mesh as M                               # noqa: E402
-from dmnerf_b200.helpers import z_val_sample                    # noqa: E402
-from dmnerf_b200.objects import meshes_from_labelled_grid, object_mask, occupancy_objects   # noqa: E402
-from dmnerf_b200.render import render_rays                      # noqa: E402
-from dmnerf_b200.testing import make_models                     # noqa: E402
-
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=20).stdout.strip()
-        name, power = [s.strip() for s in q.split(",")]
-    except Exception:
-        name, power = torch.cuda.get_device_name(0), "unknown"
-    return name, power
-
-
-def timed(fn, dev):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    fn()
-    b.record()
-    torch.cuda.synchronize(dev)
-    return a.elapsed_time(b)
+from _harness import alternate, cuda_device, event_ms, gpu_identity
+from dmnerf_b200 import synth
+from dmnerf_b200 import mesh as M
+from dmnerf_b200.helpers import z_val_sample
+from dmnerf_b200.objects import meshes_from_labelled_grid, object_mask, occupancy_objects
+from dmnerf_b200.render import render_rays
+from dmnerf_b200.testing import make_models
 
 
 def frame_rates(name, reps, dev):
@@ -60,12 +36,7 @@ def frame_rates(name, reps, dev):
                     "remove_one": [k for k in range(ins_num + 1) if k != one]}
         run = {k: (lambda keep=keep: render_rays(ro, rd, nc, nf, z, want_raw=False, want_samples=False, want_coarse=False,
                                                  keep_objects=keep)) for k, keep in variants.items()}
-        for f in run.values():
-            f()                                                             # warm-up of every variant
-        ms = {k: [] for k in run}
-        for _ in range(reps):
-            for k, f in run.items():
-                ms[k].append(timed(f, dev))
+        ms = alternate(run, reps)
     return {"ins_num": ins_num, "rays": n, "label": one,
             "rays_per_s": {k: n / (np.median(v) * 1e-3) for k, v in ms.items()},
             "ms": {k: [round(x, 3) for x in v] for k, v in ms.items()}}
@@ -87,14 +58,12 @@ def mesh_times(reps, dev, dim=256, ins_num=13):
         del occ, labels, sample
         sweep, per_obj, tris = [], [], None
         for _ in range(reps + 1):
-            holder = {}
-            t_sweep = timed(lambda: holder.update(zip(("occ", "labels"), occupancy_objects(nf, T, keep, dim, near=near, far=far,
-                                                                                             device=dev))), dev)
-            t_mesh = timed(lambda: holder.update(meshes=meshes_from_labelled_grid(holder["occ"], holder["labels"], T, objects, level)),
-                           dev)
+            t_sweep, (occ, labels) = event_ms(lambda: occupancy_objects(nf, T, keep, dim, near=near, far=far, device=dev))
+            t_mesh, meshes = event_ms(lambda: meshes_from_labelled_grid(occ, labels, T, objects, level))
             sweep.append(t_sweep)
             per_obj.append(t_mesh)
-            tris = {k: int(m["clean_triangles"].shape[0]) for k, m in holder["meshes"].items()}
+            tris = {k: int(m["clean_triangles"].shape[0]) for k, m in meshes.items()}
+            del occ, labels, meshes                         # freed before the next timed sweep
     return {"grid_dim": dim, "ins_num": ins_num, "level": level, "objects": len(objects), "clean_triangles": tris,
             "sweep_ms": [round(x, 2) for x in sweep[1:]], "per_object_mesh_ms": [round(x, 2) for x in per_obj[1:]]}
 
@@ -103,9 +72,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "tools/objects_bench.py needs a CUDA device; there is no CPU fallback"
-    dev = torch.device("cuda", 0)
-    name, power = gpu_info()
+    dev = cuda_device("objects_bench.py")
+    name, _, card = gpu_identity(dev)
+    name, power = card or (name, "unknown")
     res = {"bench": "object_selection", "gpu": name, "power_limit": power,
            "frame_640x480": {wl: frame_rates(wl, a.reps, dev) for wl in ("dmsr_study", "replica_room0_93")},
            "mesh": mesh_times(a.reps, dev)}

@@ -9,13 +9,12 @@ import time
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import synth                                                  # noqa: E402
-from dmnerf_b200.render import render_rays                                     # noqa: E402
-from dmnerf_b200.testing import make_models, parity_table, format_parity_table  # noqa: E402
-from dmnerf_b200.engine import get_context                                     # noqa: E402
-from oracle import dmnerf_oracle as O                                          # noqa: E402
+from _harness import ROOT, cuda_device, gpu_identity
+from dmnerf_b200 import synth
+from dmnerf_b200.render import render_rays
+from dmnerf_b200.testing import make_models, parity_table, format_parity_table
+from dmnerf_b200.engine import get_context
+from oracle import dmnerf_oracle as O
 
 CONFIGS = ("dmsr_study", "replica_room0", "replica_room0_93", "replica_office2")
 
@@ -45,6 +44,7 @@ def run_config(name, n_rays, dev="cuda", seeds=(101, 202)):
 
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 2048
+    print("GPU: %s" % gpu_identity(cuda_device("parity_at_scale.py"))[1])
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     res, md = {}, []
     for name in CONFIGS:

@@ -1,23 +1,20 @@
 """SURVEY section 8 row f4: the 256^3 density sweep of tools/mesh_generator.py:36-49 through the point-query entry point
 (dmnerf_mlp_forward_points: points and zero view directions embedded inside the tensor-core kernel), timed on the device, plus
 the CPU oracle on a bounded sample of the same points.      python tools/point_sweep.py [grid]"""
-import os
 import sys
 import time
 
-import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import synth                                 # noqa: E402
-from dmnerf_b200.autograd import mlp_forward_points           # noqa: E402
-from dmnerf_b200.engine import get_context                    # noqa: E402
-from dmnerf_b200.testing import make_models, raw_errs         # noqa: E402
-from oracle import dmnerf_oracle as O                         # noqa: E402
+from _harness import cuda_device, event_ms, gpu_identity
+from dmnerf_b200 import synth
+from dmnerf_b200.autograd import mlp_forward_points
+from dmnerf_b200.engine import get_context
+from dmnerf_b200.testing import make_models, raw_errs
+from oracle import dmnerf_oracle as O
 
 grid = int(sys.argv[1]) if len(sys.argv) > 1 else 256
-dev = "cuda"
+dev = cuda_device("point_sweep.py")
 _, nf, _, wf = make_models(101, 202, 13, dev)
 t = torch.linspace(-3.0, 3.0, grid, device=dev)
 chunk = grid * grid * 16                                      # 16 z-slabs per call (mesh_generator.py sweeps in chunks too)
@@ -31,15 +28,11 @@ with torch.no_grad():
             sigma.view(grid, grid, grid)[:, :, z0:z0 + 16] = out[:, 3].view(grid, grid, -1)
     sweep()
     torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    sweep()
-    e1.record()
-    torch.cuda.synchronize()
+    ms, _ = event_ms(sweep)
     get_context(dev).sync_check()
-    ms = e0.elapsed_time(e1)
     n = grid ** 3
     flops = 2.0 * synth.macs_per_sample(13) * n
+    print("GPU: %s" % gpu_identity(dev)[1])
     print("point query sweep: %d^3 = %d points in %.1f ms = %.1f M points/s, %.0f algorithmic TFLOP/s (incl. grid generation and the sigma scatter in torch)"
           % (grid, n, ms, n / ms / 1e3, flops / (ms * 1e-3) / 1e12))
     # CPU oracle on a sample of the same points

@@ -10,34 +10,19 @@ One manipulate_frame with one moved object is timed in both precisions too.  --p
 import argparse
 import ctypes as C
 import json
-import os
-import sys
 import types
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from dmnerf_b200 import _lib, synth                        # noqa: E402
-from dmnerf_b200.engine import get_context                 # noqa: E402
-from dmnerf_b200.render import render_frame, render_rays   # noqa: E402
-from dmnerf_b200.testing import make_models                # noqa: E402
-from eval_bench import gpu_info                            # noqa: E402
+from _harness import alternate, cuda_device, event_ms, gpu_identity
+from dmnerf_b200 import _lib, synth
+from dmnerf_b200.engine import get_context
+from dmnerf_b200.render import render_frame, render_rays
+from dmnerf_b200.testing import make_models
 
 IMPLS = {"exact": _lib.IMPL_UMMA, "fp16": _lib.IMPL_UMMA_F16}
 STAGES = ("prep_z", "coarse_net", "coarse_composite", "hier_sample", "fine_net", "fine_composite")
-
-
-def _timed(fn):
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-    ev[0].record()
-    out = fn()
-    ev[1].record()
-    torch.cuda.synchronize()
-    return ev[0].elapsed_time(ev[1]), out
 
 
 def _psnr(a, b):
@@ -50,14 +35,9 @@ def frames(name, reps, warmup):
     H, W = wl["H"], wl["W"]
     nc, nf, _, _ = make_models(101, 202, wl["ins_num"], "cuda")
     call = lambda impl: render_frame(H, W, wl["K"], wl["c2w"], wl["near"], wl["far"], nc, nf, impl=impl)
-    ms = {k: [] for k in IMPLS}
-    maps = {}
+    maps = {}                                   # the last frame of each precision, held as the next frames run
     with torch.no_grad():
-        for r in range(warmup + reps):
-            for k, impl in IMPLS.items():
-                t, maps[k] = _timed(lambda: call(impl))
-                if r >= warmup:
-                    ms[k].append(t)
+        ms = alternate({k: lambda k=k, impl=impl: maps.update({k: call(impl)}) for k, impl in IMPLS.items()}, reps, warmup)
     med = {k: float(np.median(v)) for k, v in ms.items()}
     rate = {k: H * W / (med[k] / 1e3) for k in IMPLS}
     agree = float((maps["fp16"]["ins"].argmax(-1) == maps["exact"]["ins"].argmax(-1)).double().mean())
@@ -85,8 +65,8 @@ def manipulation(reps, warmup):
     rgb = {}
     for r in range(warmup + reps):
         for k, impl in IMPLS.items():
-            torch.cuda.manual_seed(7)
-            t, out = _timed(lambda: manipulate_frame(H, W, wl["K"], pose, to[None], td[None], pe, ve, nc, nf, args, impl=impl))
+            torch.cuda.manual_seed(7)                   # outside the timed call
+            t, out = event_ms(lambda: manipulate_frame(H, W, wl["K"], pose, to[None], td[None], pe, ve, nc, nf, args, impl=impl))
             rgb[k] = out[0]
             if r >= warmup:
                 ms[k].append(t)
@@ -121,9 +101,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--profile", action="store_true")
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("precision_bench: needs a CUDA device")
-    name, power = gpu_info()
+    name, _, card = gpu_identity(cuda_device("precision_bench.py"))
+    name, power = card or (name, "unknown")
     res = {"gpu": name, "power_limit": power, "frames": [frames(w, a.reps, a.warmup) for w in ("dmsr_study", "replica_room0_93")],
            "manipulate_frame": manipulation(max(1, a.reps // 2), 1)}
     if a.profile:

@@ -2,24 +2,22 @@
 event-timed iteration, GPU-busy time (sum of kernel durations from CUPTI), host-issue time (the same loop with the GPU idle at
 the start of every iteration cannot run faster than the host can issue it), top kernels.  python tools/prof_full_iter.py"""
 import os
-import sys
 import time
 import types
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import synth                              # noqa: E402
-from dmnerf_b200.testing import make_models                # noqa: E402
-from dmnerf_b200.render import dm_nerf                     # noqa: E402
-from dmnerf_b200.embedder import get_embedder              # noqa: E402
-from dmnerf_b200.helpers import get_select_full            # noqa: E402
-from dmnerf_b200.evaluator import ins_criterion, img2mse   # noqa: E402
-from dmnerf_b200.penalizer import ins_penalizer            # noqa: E402
+from _harness import cuda_device, event_ms, gpu_identity
+from dmnerf_b200 import synth
+from dmnerf_b200.testing import make_models
+from dmnerf_b200.render import dm_nerf
+from dmnerf_b200.embedder import get_embedder
+from dmnerf_b200.helpers import get_select_full
+from dmnerf_b200.evaluator import ins_criterion, img2mse
+from dmnerf_b200.penalizer import ins_penalizer
 
-dev = "cuda"
+dev = cuda_device("prof_full_iter.py")
 ins_num = 13
 wl = synth.workload("dmsr_study")
 H, W = wl["H"], wl["W"]
@@ -57,13 +55,10 @@ def full_iteration():
 for _ in range(4):
     full_iteration()
 torch.cuda.synchronize()
-e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-e0.record()
-for _ in range(10):
-    full_iteration()
-e1.record(); torch.cuda.synchronize()
+ms, _ = event_ms(lambda: [full_iteration() for _ in range(10)])
+print("GPU: %s" % gpu_identity(dev)[1])
 print("adam=%s " % os.environ.get("ADAM", "foreach (torch default)"), end="")
-print("parts=%s: %.3f ms per iteration (CUDA events, 10 iterations back to back)" % (",".join(parts), e0.elapsed_time(e1) / 10))
+print("parts=%s: %.3f ms per iteration (CUDA events, 10 iterations back to back)" % (",".join(parts), ms / 10))
 host = []
 for _ in range(6):
     torch.cuda.synchronize()

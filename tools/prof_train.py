@@ -1,20 +1,17 @@
 """Kernel-level time breakdown of one training step (BASELINE config 4) with torch.profiler (CUPTI sees every kernel of the
 process, including the native library's).  python tools/prof_train.py"""
-import os
-import sys
 import types
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import synth                              # noqa: E402
-from dmnerf_b200.testing import make_models                # noqa: E402
-from dmnerf_b200.render import dm_nerf                     # noqa: E402
-from dmnerf_b200.embedder import get_embedder              # noqa: E402
+from _harness import cuda_device, gpu_identity
+from dmnerf_b200 import synth
+from dmnerf_b200.testing import make_models
+from dmnerf_b200.render import dm_nerf
+from dmnerf_b200.embedder import get_embedder
 
-dev = "cuda"
+dev = cuda_device("prof_train.py")
 wl = synth.workload("dmsr_study")
 nc, nf, _, _ = make_models(201, 202, 13, dev)
 sel = np.random.Generator(np.random.PCG64(0)).choice(307200, 1024, replace=False)
@@ -47,6 +44,7 @@ with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
 rows = [(e.key, e.device_time_total / 3.0, e.count // 3) for e in prof.key_averages() if e.device_time_total > 0]
 rows.sort(key=lambda r: -r[1])
 tot = sum(r[1] for r in rows)
+print("GPU: %s" % gpu_identity(dev)[1])
 print("device time per step: %.2f ms over %d kernel kinds" % (tot / 1e3, len(rows)))
 for k, t, c in rows[:28]:
     print("%8.1f us  %5.1f%%  x%-3d %s" % (t, 100 * t / tot, c, k[:110]))

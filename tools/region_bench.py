@@ -13,20 +13,15 @@ than a picture of a trained scene.  Build times: CUDA events, median of --reps a
 0.3.  Nothing is written to disk."""
 import argparse
 import json
-import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from dmnerf_b200 import objects as OB                         # noqa: E402
-from dmnerf_b200 import synth                                 # noqa: E402
-from dmnerf_b200.render import render_frame                   # noqa: E402
-from dmnerf_b200.testing import make_models                   # noqa: E402
+from _harness import alternate, cuda_device, gpu_identity, host_ms
+from dmnerf_b200 import objects as OB
+from dmnerf_b200 import synth
+from dmnerf_b200.render import render_frame
+from dmnerf_b200.testing import make_models
 
 
 def floater_region(nf, ins_num, dim, dev):
@@ -51,17 +46,12 @@ def frames(name, reps, sweep_dim, dev):
     H, W = 480, 640
     everything = list(range(ins_num + 1))
     variants = {"unselected": {}, "keep_all": {"keep_objects": everything}, "floater_region": {"region": reg}}
-    times = {k: [] for k in variants}
+
+    def frame(kw):
+        return lambda: render_frame(H, W, wl["K"], wl["c2w"], wl["near"], wl["far"], nc, nf, device=dev, **kw)
     with torch.no_grad():
-        for r in range(reps + 1):
-            for k, kw in variants.items():
-                torch.cuda.synchronize()
-                t0 = time.perf_counter()
-                render_frame(H, W, wl["K"], wl["c2w"], wl["near"], wl["far"], nc, nf, device=dev, **kw)
-                torch.cuda.synchronize()
-                if r:
-                    times[k].append(time.perf_counter() - t0)
-    rate = {k: H * W / float(np.median(v)) for k, v in times.items()}
+        ms = alternate({k: frame(kw) for k, kw in variants.items()}, reps, clock=host_ms)
+    rate = {k: H * W / (float(np.median(v)) * 1e-3) for k, v in ms.items()}
     return {"workload": name, "ins_num": ins_num, "rays_per_s": rate, "sweep_dim": sweep_dim, **info,
             "keep_all_vs_unselected": rate["keep_all"] / rate["unselected"],
             "region_vs_keep_all": rate["floater_region"] / rate["keep_all"]}
@@ -69,15 +59,7 @@ def frames(name, reps, sweep_dim, dev):
 
 def build_times(dim, reps, dev):
     mask = torch.rand((dim,) * 3, device=dev) < 0.3
-    ms = []
-    for r in range(reps + 1):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        OB.region_from_mask(mask, np.eye(4), dilate=1, connectivity=26)
-        b.record()
-        torch.cuda.synchronize()
-        if r:
-            ms.append(a.elapsed_time(b))
+    ms = alternate({"build": lambda: OB.region_from_mask(mask, np.eye(4), dilate=1, connectivity=26)}, reps)["build"]
     return {"grid_dim": dim, "pack_dilate1_ms": float(np.median(ms)), "bits_MB": (dim ** 3 + 31) // 32 * 4 / 1e6}
 
 
@@ -87,17 +69,12 @@ def main():
     ap.add_argument("--grid-dims", type=int, nargs="+", default=[256, 512])
     ap.add_argument("--sweep-dim", type=int, default=256)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "tools/region_bench.py needs a CUDA device; there is no CPU fallback"
-    dev = torch.device("cuda", 0)
+    dev = cuda_device("region_bench.py")
     runs = [frames(n, a.reps, a.sweep_dim, dev) for n in ("dmsr_study", "replica_room0_93")]
     builds = [build_times(d, a.reps, dev) for d in a.grid_dims]
-    try:
-        gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=20).stdout.strip()
-    except Exception as exc:
-        gpu = "nvidia-smi unavailable: %s" % exc
-    print(json.dumps({"metric": "region selection cost", "reps": a.reps, "frames": runs, "build": builds, "gpu": gpu,
-                      "gpu_name": torch.cuda.get_device_name(dev),
+    name, smi, _ = gpu_identity(dev)
+    print(json.dumps({"metric": "region selection cost", "reps": a.reps, "frames": runs, "build": builds, "gpu": smi,
+                      "gpu_name": name,
                       "what": "640x480 frames through the frame driver (host maps), rays/s median of %d, variants alternated; "
                               "region build = pack + dilate 1 (26), CUDA events" % a.reps}))
 
