@@ -50,6 +50,7 @@ class RenderIO(C.Structure):
 
 
 MAX_MOVES = 8                # DMNERF_MAX_MOVES
+MAX_CANDIDATES = 4096        # DMNERF_MAX_CANDIDATES
 
 
 class Pieces(C.Structure):
@@ -155,6 +156,11 @@ PROTOTYPES = {
                                        C.POINTER(C.c_int64), C.POINTER(C.c_uint32), C.c_void_p]),
     "dmnerf_object_spans": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_int32),
                                       C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p]),
+    "dmnerf_move_overlap": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                      C.POINTER(EditMove), C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_int64),
+                                      C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_object_contacts": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_int64),
+                                         C.c_void_p]),
     "dmnerf_object_components": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int, C.c_void_p,
                                            C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_component_table": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -763,15 +763,10 @@ DMNERF_API int dmnerf_mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double
   if (bound_net(ctx, net, who)) return 1;
   if (evaluated_host) *evaluated_host = 0;
   DMN_CHECK(transform_host && extents_host && occ && labels, "%s: NULL argument", who);
-  DMN_CHECK(dim >= 2 && dim <= 2048, "%s: dim %d out of range [2, 2048]", who, dim);
+  if (sweep_grid_check(transform_host, extents_host, dim, level, who)) return 1;
   DMN_CHECK(n_moves >= 0 && n_moves <= DMNERF_MAX_MOVES, "%s: between 0 and %d moves are supported, got %d", who, DMNERF_MAX_MOVES,
             n_moves);
   DMN_CHECK(n_moves == 0 || moves_host, "%s: moves is NULL", who);
-  DMN_CHECK(level > 0.0f && level < 1.0f, "%s: level %g outside (0, 1)", who, (double)level);
-  const double* T = transform_host;
-  const double det = T[0] * (T[5] * T[10] - T[6] * T[9]) - T[1] * (T[4] * T[10] - T[6] * T[8]) + T[2] * (T[4] * T[9] - T[5] * T[8]);
-  DMN_CHECK(det > 0.0, "%s: the scene transform has det %g <= 0", who, det);
-  for (int a = 0; a < 3; ++a) DMN_CHECK(extents_host[a] > 0.0 && std::isfinite(extents_host[a]), "%s: extents must be finite and > 0", who);
   EditMove mv[DMNERF_MAX_MOVES];
   for (int i = 0; i < n_moves; ++i)
     if (edit_move_from_abi(moves_host[i], transform_host, extents_host, dim, ctx->net[net].p.ins_num, mv[i], who, i)) return 1;
@@ -878,6 +873,25 @@ DMNERF_API int dmnerf_object_spans(dmnerf_ctx* ctx, const float* occ, const int1
   DMN_CHECK(ctx != nullptr, "object_spans: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
   return object_spans(ctx->inventory, occ, labels, dim, level, n_labels, boxes_host, axes_host, spans_host, (cudaStream_t)stream);
+}
+
+// ---- collision checks (DESIGN.md, "Collision checks") ---------------------------------------------------------------------
+
+DMNERF_API int dmnerf_move_overlap(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                   const double* transform_host, const double* extents_host, const dmnerf_edit_move* candidates_host,
+                                   int n_candidates, const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host,
+                                   void* stream) {
+  DMN_CHECK(ctx != nullptr, "move_overlap: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, n_candidates,
+                      obstacles_host, overlap_host, landed_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_object_contacts(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                                      int64_t* faces_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "object_contacts: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return object_contacts(ctx->inventory, occ, labels, dim, level, n_labels, faces_host, (cudaStream_t)stream);
 }
 
 // ---- connected components (DESIGN.md, "Connected components") -------------------------------------------------------------

@@ -301,6 +301,9 @@ struct EditMove {
   Region piece;
   int32_t label, rest_drop, empty;   // empty: the box holds no point, nothing is evaluated
 };
+// The grid and level of an edit or a collision check: dim in [2, 2048], level in (0, 1), a scene transform with det > 0 and
+// finite extents > 0.
+int sweep_grid_check(const double* T16, const double* ext3, int dim, float level, const char* who);
 // d -> m, checked against the grid (dim, transform, extents) and the bound network's ins_num
 int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const double* ext3, int dim, int ins_num, EditMove& m,
                        const char* who, int i);
@@ -325,6 +328,14 @@ int object_voxels(InventoryState& s, const float* occ, const int16_t* labels, in
                   const int32_t* boxes_host, int64_t* moments_host, uint32_t* hist_host, cudaStream_t st);
 int object_spans(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                  const int32_t* boxes_host, const double* axes_host, double* spans_host, cudaStream_t st);
+
+// Collision checks (collide.cu; DESIGN.md, "Collision checks"), in the inventory's buffers: grid-only counts over a labelled
+// keep-all sweep, one device->host read per call.
+int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
+                 const dmnerf_edit_move* cands_host, int n, const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host,
+                 cudaStream_t st);
+int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels, int64_t* faces_host,
+                    cudaStream_t st);
 
 // Connected components (components.cu): the solid points of a labelled grid split into canonically numbered components.
 // Per-context device buffers: the status words a call reads back, the chunk counts and the scan's storage.

@@ -8,6 +8,7 @@
 
 #include "common.cuh"
 #include "ray_ops.cuh"
+#include "sweep_grid.cuh"
 
 namespace dmnerf {
 
@@ -127,36 +128,6 @@ __constant__ McTable c_mc = mcgen::kTable;
 static inline unsigned blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
 // ---- query grid and occupancy -------------------------------------------------------------------------------------------
-struct GridXform {
-  float r[12];     // rows of [R | t], float32 like the original's torch.from_numpy(transform).float()
-  float s[3];      // extents / 2 (float32)
-  float step;      // torch.linspace(-1, 1, dim) step
-  int dim;
-};
-
-// torch.linspace(-1, 1, dim) on the CPU in float32: start + step * i below the half, end - step * (dim - 1 - i) above it, each a
-// single rounding (fused multiply-add)
-__device__ __forceinline__ float linspace_m11(int i, const GridXform& g) {
-  return i < g.dim / 2 ? __fmaf_rn(g.step, (float)i, -1.0f) : __fmaf_rn(-g.step, (float)(g.dim - 1 - i), 1.0f);
-}
-
-// visualizer.make_3D_grid / grid_within_bound + mesh_generator.py:28-29, in the original's fp32 operation order:
-// q = (R q_scaled summed left to right) + t, then (x, y, z) -> (x, -z, y)
-__device__ __forceinline__ void sweep_point(const GridXform& g, int64_t p, float out[3]) {
-  const int64_t d = g.dim;
-  const float q[3] = {__fmul_rn(linspace_m11((int)(p / (d * d)), g), g.s[0]), __fmul_rn(linspace_m11((int)((p / d) % d), g), g.s[1]),
-                      __fmul_rn(linspace_m11((int)(p % d), g), g.s[2])};
-  float w[3];
-#pragma unroll
-  for (int r = 0; r < 3; ++r) {
-    const float* row = g.r + 4 * r;
-    w[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(row[0], q[0]), __fmul_rn(row[1], q[1])), __fmul_rn(row[2], q[2])), row[3]);
-  }
-  out[0] = w[0];
-  out[1] = -w[2];
-  out[2] = w[1];
-}
-
 __global__ void grid_points_kernel(GridXform g, int64_t begin, int64_t count, float* __restrict__ pts) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
@@ -165,16 +136,6 @@ __global__ void grid_points_kernel(GridXform g, int64_t begin, int64_t count, fl
   pts[3 * i] = w[0];
   pts[3 * i + 1] = w[1];
   pts[3 * i + 2] = w[2];
-}
-
-static GridXform make_xform(const double* T16, const double* ext3, int dim) {
-  GridXform g;
-  for (int r = 0; r < 3; ++r)
-    for (int c = 0; c < 4; ++c) g.r[4 * r + c] = (float)T16[4 * r + c];
-  for (int a = 0; a < 3; ++a) g.s[a] = (float)(ext3[a] / 2.0);
-  g.step = 2.0f / (float)(dim - 1);
-  g.dim = dim;
-  return g;
 }
 
 int launch_grid_points(const double* T16, const double* ext3, int dim, int64_t begin, int64_t count, float* pts, cudaStream_t st) {
@@ -687,6 +648,15 @@ static void grid_index_map(const double* T, const double* ext, int dim, double i
   }
 }
 
+int sweep_grid_check(const double* T, const double* ext3, int dim, float level, const char* who) {
+  DMN_CHECK(dim >= 2 && dim <= 2048, "%s: dim %d out of range [2, 2048]", who, dim);
+  DMN_CHECK(level > 0.0f && level < 1.0f, "%s: level %g outside (0, 1)", who, (double)level);
+  const double det = T[0] * (T[5] * T[10] - T[6] * T[9]) - T[1] * (T[4] * T[10] - T[6] * T[8]) + T[2] * (T[4] * T[9] - T[5] * T[8]);
+  DMN_CHECK(det > 0.0, "%s: the scene transform has det %g <= 0", who, det);
+  for (int a = 0; a < 3; ++a) DMN_CHECK(ext3[a] > 0.0 && std::isfinite(ext3[a]), "%s: extents must be finite and > 0", who);
+  return 0;
+}
+
 int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const double* ext3, int dim, int ins_num, EditMove& m,
                        const char* who, int i) {
   memset(&m, 0, sizeof(m));
@@ -712,8 +682,7 @@ int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const doubl
   return 0;
 }
 
-// One thread per grid point of the slab: its target t = trans p (fp64, rounded once to fp32) and whether the nearest grid index
-// of t, rint(A^-1 (t - b)), lies in the box (an fp32 sweep point maps to its own index, also on the grid's faces).
+// One thread per grid point of the slab: its target t (edit_target) and whether the nearest grid index of t lies in the box.
 __global__ void edit_target_kernel(const GridXform g, const EditMove m, int64_t begin, int64_t count, float* __restrict__ tgt,
                                    int32_t* __restrict__ flag) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -721,23 +690,8 @@ __global__ void edit_target_kernel(const GridXform g, const EditMove m, int64_t 
   float p[3];
   sweep_point(g, begin + i, p);
   float t[3];
-  double dt[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const double* r = m.trans + 4 * a;
-    const double v = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)p[0]), __dmul_rn(r[1], (double)p[1])),
-                                         __dmul_rn(r[2], (double)p[2])), r[3]);
-    t[a] = __double2float_rn(v);
-    dt[a] = __dsub_rn((double)t[a], m.b[a]);
-  }
-  bool in = !m.empty;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const double* row = m.inv + 3 * a;
-    const double u = __dadd_rn(__dadd_rn(__dmul_rn(row[0], dt[0]), __dmul_rn(row[1], dt[1])), __dmul_rn(row[2], dt[2]));
-    const double i = rint(u);                                     // the nearest grid index, half to even
-    in = in && i >= m.lo[a] && i <= m.hi[a];
-  }
+  double q[3];
+  const bool in = edit_target(m.trans, m.inv, m.b, m.lo, m.hi, !m.empty, p, t, q);
   tgt[3 * i] = t[0];
   tgt[3 * i + 1] = t[1];
   tgt[3 * i + 2] = t[2];

@@ -1,0 +1,74 @@
+// The occupancy sweep's grid as the device sees it (DESIGN.md, "Mesh extraction" and "Meshing an edited scene"): its fp32 grid
+// points, and the target and nearest grid index of a point under a move.  Shared by the edited sweep (mesh.cu) and the collision
+// checks (collide.cu), so that both take the same decisions.
+#pragma once
+#include "common.cuh"
+
+namespace dmnerf {
+
+struct GridXform {
+  float r[12];     // rows of [R | t], float32 like the original's torch.from_numpy(transform).float()
+  float s[3];      // extents / 2 (float32)
+  float step;      // torch.linspace(-1, 1, dim) step
+  int dim;
+};
+
+inline GridXform make_xform(const double* T16, const double* ext3, int dim) {
+  GridXform g;
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 4; ++c) g.r[4 * r + c] = (float)T16[4 * r + c];
+  for (int a = 0; a < 3; ++a) g.s[a] = (float)(ext3[a] / 2.0);
+  g.step = 2.0f / (float)(dim - 1);
+  g.dim = dim;
+  return g;
+}
+
+// torch.linspace(-1, 1, dim) on the CPU in float32: start + step * i below the half, end - step * (dim - 1 - i) above it, each a
+// single rounding (fused multiply-add)
+__device__ __forceinline__ float linspace_m11(int i, const GridXform& g) {
+  return i < g.dim / 2 ? __fmaf_rn(g.step, (float)i, -1.0f) : __fmaf_rn(-g.step, (float)(g.dim - 1 - i), 1.0f);
+}
+
+// visualizer.make_3D_grid / grid_within_bound + mesh_generator.py:28-29, in the original's fp32 operation order:
+// q = (R q_scaled summed left to right) + t, then (x, y, z) -> (x, -z, y)
+__device__ __forceinline__ void sweep_point(const GridXform& g, int64_t p, float out[3]) {
+  const int64_t d = g.dim;
+  const float q[3] = {__fmul_rn(linspace_m11((int)(p / (d * d)), g), g.s[0]), __fmul_rn(linspace_m11((int)((p / d) % d), g), g.s[1]),
+                      __fmul_rn(linspace_m11((int)(p % d), g), g.s[2])};
+  float w[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    const float* row = g.r + 4 * r;
+    w[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(row[0], q[0]), __fmul_rn(row[1], q[1])), __fmul_rn(row[2], q[2])), row[3]);
+  }
+  out[0] = w[0];
+  out[1] = -w[2];
+  out[2] = w[1];
+}
+
+// The target of sweep point p under a move: t = trans p (row-major 3x4, fp64, rounded once to fp32), the nearest grid index
+// q = rint(inv (t - b)) of t (fp64, half to even; inv and b: the grid's index map), and whether q lies in the inclusive box
+// [lo, hi] (`in` false: never).  An fp32 sweep point maps to its own index, also on the grid's faces.  Every operation is rounded
+// once (no contraction), so that a numpy restatement takes the same decisions.
+__device__ __forceinline__ bool edit_target(const double* trans, const double* inv, const double* b, const double* lo,
+                                            const double* hi, bool in, const float p[3], float t[3], double q[3]) {
+  double dt[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const double* r = trans + 4 * a;
+    const double v = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)p[0]), __dmul_rn(r[1], (double)p[1])),
+                                         __dmul_rn(r[2], (double)p[2])), r[3]);
+    t[a] = __double2float_rn(v);
+    dt[a] = __dsub_rn((double)t[a], b[a]);
+  }
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const double* row = inv + 3 * a;
+    const double u = __dadd_rn(__dadd_rn(__dmul_rn(row[0], dt[0]), __dmul_rn(row[1], dt[1])), __dmul_rn(row[2], dt[2]));
+    q[a] = rint(u);
+    in = in && q[a] >= lo[a] && q[a] <= hi[a];
+  }
+  return in;
+}
+
+}  // namespace dmnerf

@@ -18,6 +18,8 @@
     manipulation_transform(centre, mode)                -> the transformation dict manipulator_eval takes, about that centre
     edited_sweep(model_fine, scene_transform, moves, ...) / edited_mesh(...)
                                                         -> the labelled sweep / the mesh of a scene with objects moved
+    move_overlap(occ, labels, scene_transform, moves, ...) / slide_until_contact(...) / object_contacts(...) / supports(...)
+                                                        -> collision checks of moves, and which objects touch, from a sweep
 
 Every network sample is labelled argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the
 exchanger's rule); a sample whose label is not kept has alpha = 0 in the composite of both passes, so the coarse weights of the
@@ -208,12 +210,12 @@ def _move_matrix(trans, i):
     return m
 
 
-def _check_moves(moves, ins_num):
-    """moves [(label, 4x4)] -> (labels, matrices); ValueError for more than MAX_MOVES, a label outside [0, ins_num] or a bad
+def _check_moves(moves, ins_num, limit=_lib.MAX_MOVES):
+    """moves [(label, 4x4)] -> (labels, matrices); ValueError for more than `limit`, a label outside [0, ins_num] or a bad
     matrix.  A matrix may be manipulation_transform(...)["transformations"][0]["transformation"] (a nested list)."""
     moves = list(moves)
-    if len(moves) > _lib.MAX_MOVES:
-        raise ValueError("edit: at most %d moves are supported, got %d" % (_lib.MAX_MOVES, len(moves)))
+    if len(moves) > limit:
+        raise ValueError("edit: at most %d moves are supported, got %d" % (limit, len(moves)))
     labels, mats = [], []
     for i, mv in enumerate(moves):
         try:
@@ -391,6 +393,183 @@ def edited_mesh(model_fine, scene_transform, moves, grid_dim=256, extents=None, 
             objects = [k for k in torch.unique(labels[occ > level]).cpu().tolist() if k != ins_num]
             out["objects"] = meshes_from_labelled_grid(occ, labels, T, objects, level, ext, min_cluster)
     return out
+
+
+# ----------------------------------------------------------------------------------------------------------------- collisions
+# DESIGN.md, "Collision checks": grid-only checks of moves on the labelled keep-all sweep (edited_sweep's), each candidate on its
+# own.  The moved object at p is the unedited grid at the nearest grid index of trans p, as edited_sweep samples it on an exact
+# grid; off the grid points it is the sweep resampled at its own resolution, not the network at trans p.
+ALL_LABELS = [0xFFFFFFFF] * 4
+
+
+def _voxel_volume(T, ext, dim):
+    return abs(np.linalg.det(T[:3, :3])) * float(np.prod(np.asarray(ext, dtype=np.float64) / (dim - 1)))
+
+
+def _check_sweep(occ, labels, who):
+    dim = _check_grid(occ, labels, who)
+    if labels is None or labels.dtype != torch.int16 or occ.dtype != torch.float32:
+        raise ValueError("%s: occ must be float32 and labels int16" % who)
+    return dim
+
+
+def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, boxes=None, margin=2, pieces=None, rest="keep",
+                 obstacles=None):
+    """dmnerf_move_overlap: each move [(label, 4x4 in the network frame)] checked on its own against the labelled keep-all sweep
+    occ / labels ([dim]^3 float32 / int16 on the device; an edited_sweep result is accepted unchanged).  boxes, margin, pieces,
+    rest: as edited_sweep (default boxes: edit_boxes).  obstacles: the labels that count as obstacles (default every label).
+    Returns one dict per move: label, landed (the voxels the moved object occupies after the move), overlap {label: voxels}
+    (labels with voxels > 0: solid obstacle points the moved object lands on; the points the move vacates are not obstacles),
+    overlap_volume {label: voxels times the inventory's voxel volume} and total (the overlapping voxels)."""
+    from .manipulator import _piece_region, move_pieces, move_rests
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    dim = _check_sweep(occ, labels, "move_overlap")
+    ext = EXTENTS if extents is None else extents
+    ins_num = MAX_LABELS - 1
+    mv, mats = _check_moves(moves, ins_num, _lib.MAX_CANDIDATES)
+    level = _check_level(level)
+    drops = move_rests(rest, len(mv))
+    regions = move_pieces(pieces, mv, ins_num, occ.device) or [None] * len(mv)
+    words = ALL_LABELS if obstacles is None else label_words(obstacles)
+    if not mv:
+        return []
+    if boxes is None:
+        boxes = edit_boxes(occ, labels, moves, T, ext, level, margin, pieces)
+    boxes = _check_boxes(boxes, len(mv), dim)
+    descs = (_lib.EditMove * len(mv))()
+    for i in range(len(mv)):
+        d = descs[i]
+        d.label, d.rest_drop = mv[i], int(drops[i])
+        d.trans[:] = mats[i][:3].reshape(-1).tolist()
+        d.box[:] = [int(v) for v in boxes[i]]
+        d.piece = _piece_region(regions[i], mv[i], ins_num, occ.device)
+    overlap = np.zeros((len(mv), MAX_LABELS), dtype=np.int64)
+    landed = np.zeros(len(mv), dtype=np.int64)
+    ctx = get_context(occ.device)
+    ctx.call("dmnerf_move_overlap", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), dim, level, _lib.doubles(T, 16),
+             _lib.doubles(ext, 3), descs, len(mv), (C.c_uint32 * 4)(*words), overlap.ctypes.data_as(C.POINTER(C.c_int64)),
+             landed.ctypes.data_as(C.POINTER(C.c_int64)))
+    unit = _voxel_volume(T, ext, dim)
+    out = []
+    for i in range(len(mv)):
+        hit = {int(k): int(overlap[i, k]) for k in np.nonzero(overlap[i])[0]}
+        out.append({"label": mv[i], "landed": int(landed[i]), "overlap": hit,
+                    "overlap_volume": {k: v * unit for k, v in hit.items()}, "total": int(overlap[i].sum())})
+    return out
+
+
+def _translate(v):
+    m = np.eye(4)
+    m[:3, 3] = v
+    return m
+
+
+def slide_steps(direction, max_distance, step, base=None):
+    """The candidates of slide_until_contact -> (unit direction, distances s_k, 4x4 moves base @ translate(-s_k d)).  s_k =
+    k step for k = 0 .. K - 1, the last one max_distance itself; ValueError for more than MAX_CANDIDATES steps."""
+    d = np.asarray(direction, dtype=np.float64).reshape(-1)
+    if d.shape != (3,) or not np.isfinite(d).all() or not np.linalg.norm(d) > 0:
+        raise ValueError("slide: direction must be 3 finite numbers, not all 0, got %r" % (d.tolist(),))
+    d = d / np.linalg.norm(d)
+    max_distance, step = float(max_distance), float(step)
+    if not (np.isfinite(max_distance) and max_distance >= 0):
+        raise ValueError("slide: max_distance must be finite and >= 0, got %r" % max_distance)
+    if not (np.isfinite(step) and step > 0):
+        raise ValueError("slide: step must be finite and > 0, got %r" % step)
+    n = int(np.ceil(max_distance / step)) + 1
+    if n > _lib.MAX_CANDIDATES:
+        raise ValueError("slide: %d steps of %g to %g exceed the %d candidates of one check" % (n, step, max_distance,
+                                                                                              _lib.MAX_CANDIDATES))
+    base = np.eye(4) if base is None else _move_matrix(base, 0)
+    s = np.minimum(np.arange(n, dtype=np.float64) * step, max_distance)
+    return d, s, [base @ _translate(-sk * d) for sk in s]
+
+
+def slide_result(d, steps, results, tolerance, base=None):
+    """The answer of slide_until_contact from the move_overlap results of its steps."""
+    base = np.eye(4) if base is None else np.asarray(base, dtype=np.float64)
+    profile = [r["total"] for r in results]
+    first = next((k for k, v in enumerate(profile) if v > tolerance), None)
+    if first is None:
+        distance, contact = float(steps[-1]), None
+    else:
+        contact = {"distance": float(steps[first]), "overlap": results[first]["overlap"]}
+        distance = float(steps[first - 1]) if first > 0 else None
+    trans = None if distance is None else (base @ _translate(-distance * d)).tolist()
+    return {"distance": distance, "transformation": trans, "contact": contact, "steps": [float(v) for v in steps],
+            "profile": profile}
+
+
+def slide_until_contact(occ, labels, scene_transform, label, direction, max_distance, step=None, base=None, tolerance=0,
+                        extents=None, level=0.45, margin=2, piece=None, rest="keep", obstacles=None):
+    """How far object `label` (or its piece) can slide along `direction` (network frame) before it overlaps an obstacle of the
+    sweep occ / labels by more than `tolerance` voxels.  The candidates base @ translate(-s_k d) (d the unit direction): the
+    object moved by base (it lands at inv(base) x), then shifted by s_k d, s_k = k step up to max_distance (step: default the
+    smallest grid spacing), all checked in one move_overlap call (at most MAX_CANDIDATES steps).  Returns
+      distance:       the largest s_k before the first step that overlaps, max_distance without contact, None when base
+                      itself overlaps;
+      transformation: the 4x4 (nested list) at that distance, as rigid_rays, manipulator_eval and edited_sweep take it;
+      contact:        None, or {distance, overlap} of the first overlapping step;
+      steps, profile: every s_k and its total overlap.
+    The object is checked at the steps only: an obstacle thinner than one step can be passed through."""
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    ext = EXTENTS if extents is None else extents
+    if int(tolerance) != tolerance or int(tolerance) < 0:
+        raise ValueError("slide: tolerance must be an integer >= 0 voxels, got %r" % (tolerance,))
+    if step is None:
+        A, _ = grid_affine(T, occ.shape[0], ext)
+        step = float(np.linalg.norm(A, axis=0).min())
+    d, s, mats = slide_steps(direction, max_distance, step, base)
+    pieces = None if piece is None else [piece]
+    box = edit_boxes(occ, labels, [(label, mats[0])], T, ext, _check_level(level), margin, pieces)[0]
+    results = move_overlap(occ, labels, T, [(label, m) for m in mats], ext, level, [box] * len(mats), margin,
+                           None if piece is None else [piece] * len(mats), rest, obstacles)
+    return slide_result(d, s, results, int(tolerance), mats[0])
+
+
+def object_contacts(occ, labels, scene_transform, extents=None, level=0.45):
+    """dmnerf_object_contacts: which objects of a labelled sweep touch.  Returns faces int64 [3, 128, 128] (faces[a, l1, l2]:
+    the solid points of l1 whose +a index neighbour is a solid point of l2 != l1), axes [3, 3] (the unit network-frame direction
+    of each index axis) and face_area [3] (the network-frame area of one voxel face across each axis)."""
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    dim = _check_sweep(occ, labels, "object_contacts")
+    ext = EXTENTS if extents is None else extents
+    level = _check_level(level)
+    faces = np.zeros((3, MAX_LABELS, MAX_LABELS), dtype=np.int64)
+    ctx = get_context(occ.device)
+    ctx.call("dmnerf_object_contacts", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), dim, level, MAX_LABELS,
+             faces.ctypes.data_as(C.POINTER(C.c_int64)))
+    return contacts_from_faces(faces, T, dim, ext)
+
+
+def contacts_from_faces(faces, scene_transform, dim, extents=None):
+    """object_contacts' dict from its face counts and the grid."""
+    A, _ = grid_affine(scene_transform, dim, extents)
+    area = [float(np.linalg.norm(np.cross(A[:, (a + 1) % 3], A[:, (a + 2) % 3]))) for a in range(3)]
+    return {"faces": faces, "axes": (A / np.linalg.norm(A, axis=0)).T.copy(), "face_area": np.array(area)}
+
+
+def supports(contacts, down, min_faces=1):
+    """Which object rests on which, from object_contacts: along the index axis closest to +-down (network frame), the labels
+    below each label's solid points -> {label: [(label_below, faces), ...]}, most faces first (then ascending label); pairs
+    with fewer than min_faces faces are left out."""
+    dn = np.asarray(down, dtype=np.float64).reshape(-1)
+    if dn.shape != (3,) or not np.isfinite(dn).all() or not np.linalg.norm(dn) > 0:
+        raise ValueError("supports: down must be 3 finite numbers, not all 0, got %r" % (dn.tolist(),))
+    if int(min_faces) != min_faces or int(min_faces) < 1:
+        raise ValueError("supports: min_faces must be an integer >= 1, got %r" % (min_faces,))
+    dots = np.asarray(contacts["axes"]) @ (dn / np.linalg.norm(dn))
+    a = int(np.argmax(np.abs(dots)))
+    f = np.asarray(contacts["faces"])[a]
+    if dots[a] < 0:                                    # +e_a points up: the neighbour at p + e_a is above
+        f = f.T
+    out = {}
+    for top, below in zip(*np.nonzero(f >= int(min_faces))):
+        out.setdefault(int(top), []).append((int(below), int(f[top, below])))
+    return {k: sorted(v, key=lambda x: (-x[1], x[0])) for k, v in sorted(out.items())}
 
 
 def largest_component_grid(occ, labels, level, objects):

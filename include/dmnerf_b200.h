@@ -462,6 +462,34 @@ DMNERF_API int dmnerf_object_voxels(dmnerf_ctx* ctx, const float* occ, const int
 DMNERF_API int dmnerf_object_spans(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                                    const int32_t* boxes_host, const double* axes_host, double* spans_host, void* stream);
 
+/* ---- collision checks (DESIGN.md, "Collision checks"; no counterpart in the original) ----------------------------------------
+ * Grid-only checks of object moves on a labelled keep-all sweep occ / labels [dim^3] (DEVICE float32 / int16, C order of the
+ * index (i, j, k)) of the grid (transform_host, extents_host, dim); the network is not evaluated.  A point is solid when
+ * occ > level.  Every count is an integer, so both calls are bit-reproducible and independent of the launch shape.  Both fail,
+ * before anything is written, when the grid holds NaN or a label outside their range; one device->host read per call
+ * (synchronises the stream).
+ * dmnerf_move_overlap: each of the n_candidates moves (HOST, in [1, DMNERF_MAX_CANDIDATES]; fields as dmnerf_mesh_occupancy_edit,
+ *   box = the source box B) is checked on its own against the grid.  Per grid point p (the sweep's fp32 point) and candidate:
+ *   t = trans p in fp64, rounded once to fp32, q = rint(A^-1 (t - b)) as dmnerf_mesh_occupancy_edit computes them;
+ *   src(p) = q in B && labels[q] == label && occ[q] > level && (no piece || the piece keeps t): the moved object covers p;
+ *   obstacle(p) = occ[p] > level && labels[p] in obstacles_host (4 words of 32 labels; NULL: every label), except a point the
+ *   move vacates (labels[p] == label and p in the piece -- every point without a piece -- or rest_drop).
+ *   landed_host [n] (HOST int64) = #{p : src(p)}; overlap_host [n][128] (HOST int64) = #{p : src(p) && obstacle(p) &&
+ *   labels[p] == l} per l.  Only the points of each candidate's destination box are visited: B grown by half a voxel, mapped
+ *   back through the move, plus one voxel; this never changes a count.  Rejected on the host: dim outside [2, 2048], level
+ *   outside (0, 1), a scene transform with det <= 0 or extents not finite and > 0, a candidate count out of range, and every
+ *   candidate dmnerf_mesh_occupancy_edit rejects (labels in [0, 127]).  Fails on the device for a label outside [0, 127].
+ * dmnerf_object_contacts: faces_host [3][n_labels][n_labels] (HOST int64) = per index axis a, #{p : solid l1 at p, solid l2 at
+ *   p + e_a, l1 != l2}, never across a grid face.  Rejected: dim outside [2, 2048], n_labels outside [1, 128], level outside
+ *   (0, 1); fails on the device for a label outside [0, n_labels - 1]. */
+#define DMNERF_MAX_CANDIDATES 4096
+DMNERF_API int dmnerf_move_overlap(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                   const double* transform_host, const double* extents_host,
+                                   const dmnerf_edit_move* candidates_host, int n_candidates, const uint32_t* obstacles_host,
+                                   int64_t* overlap_host /* [n][128] */, int64_t* landed_host /* [n] */, void* stream);
+DMNERF_API int dmnerf_object_contacts(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
+                                      int64_t* faces_host /* [3][n_labels][n_labels] */, void* stream);
+
 /* ---- connected components (DESIGN.md, "Connected components"; no counterpart in the original) --------------------------------
  * The solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order, p = (i dim + j) dim + k) split into components:
  * two solid points are adjacent when they are face neighbours (connectivity 6) or face, edge or corner neighbours (26), never

@@ -4,6 +4,7 @@
     python tools/find_objects.py CHECKPOINT.tar (--transform T [--extents X Y Z] | --poses POSES.npy --hwk H W K) [--trim 0]
                                  [--grid-dim 256] [--level 0.45] [--near 4 --far 15] [--out DIR]
                                  [--components {largest,split} [--connectivity {6,26}] [--min-voxels N]]
+                                 [--contacts [--down X Y Z]]
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict`.  The grid is either given (--transform: a 4x4 as
 .npy or 16 numbers of text, with --extents, default the original's 1.9 7 7) or found from the cameras (--poses: [N, 4, 4] or
@@ -12,7 +13,11 @@ points inside the cameras' view, which --out then receives as scene_transform.tx
 --extents.  Prints one JSON line: the box used and one entry per object (label, voxels, volume, centre, aabb, obb), all in the
 network frame, the frame of the camera poses and of manipulator_eval's transforms.  --components splits each label into
 connected components (DESIGN.md, "Connected components"): `largest` reports each object's largest component and adds its
-label's component count and discarded voxels; `split` reports every component of at least --min-voxels voxels, with its id."""
+label's component count and discarded voxels; `split` reports every component of at least --min-voxels voxels, with its id.
+--contacts adds the touching pairs (DESIGN.md, "Collision checks") of a sweep with the inventory's selection: per index axis its
+network-frame direction and one voxel face's area, and per pair of labels (a, b) the faces where a solid point of a has a solid
+point of b next to it along +axis, with their area.  --down (network frame) adds to each object `rests_on`: the labels below it
+along the index axis closest to that direction, with the faces they share."""
 import argparse
 import json
 import os
@@ -44,8 +49,15 @@ def parse(argv=None):
                     help="split each label into connected components: its largest one, or every one")
     ap.add_argument("--connectivity", type=int, choices=(6, 26), default=None, help="with --components: 6 or 26 (default)")
     ap.add_argument("--min-voxels", type=int, default=None, help="with --components split: the smallest component reported")
+    ap.add_argument("--contacts", action="store_true", help="also report which objects touch")
+    ap.add_argument("--down", type=float, nargs=3, default=None, metavar=("X", "Y", "Z"),
+                    help="with --contacts: the network-frame down direction; adds rests_on per object")
     ap.add_argument("--device", default="cuda")
     a = ap.parse_args(argv)
+    if a.down is not None and not a.contacts:
+        ap.error("--down needs --contacts")
+    if a.down is not None and not any(a.down):
+        ap.error("--down must not be 0 0 0")
     if a.components is None and a.connectivity is not None:
         ap.error("--connectivity needs --components")
     if a.min_voxels is not None and a.components != "split":
@@ -79,6 +91,26 @@ def components_args(a):
             "min_voxels": 1 if a.min_voxels is None else a.min_voxels}
 
 
+def contacts_json(a, nf, T, ext, objects):
+    """--contacts: object_contacts of a sweep keeping every label but the last, as object_inventory sweeps; with --down, each
+    entry of `objects` gains rests_on."""
+    import torch
+    from dmnerf_b200.objects import object_contacts, object_mask, occupancy_objects, supports
+    ins_num = int(nf.ins_linear.weight.shape[0]) - 1
+    with torch.no_grad():
+        occ, labels = occupancy_objects(nf, T, object_mask(ins_num, keep=range(ins_num)), a.grid_dim, tuple(ext), a.near, a.far,
+                                        a.N_importance, device=next(nf.parameters()).device)
+        c = object_contacts(occ, labels, T, tuple(ext), a.level)
+    del occ, labels
+    pairs = [{"labels": [int(l1), int(l2)], "axis": int(ax), "faces": int(c["faces"][ax, l1, l2]),
+              "area": float(c["faces"][ax, l1, l2] * c["face_area"][ax])} for ax, l1, l2 in zip(*np.nonzero(c["faces"]))]
+    if a.down is not None:
+        below = supports(c, a.down)
+        for e in objects:
+            e["rests_on"] = [{"label": k, "faces": n} for k, n in below.get(e["label"], [])]
+    return {"contacts": {"axes": c["axes"].tolist(), "face_area": c["face_area"].tolist(), "pairs": pairs}}
+
+
 def main(argv=None):
     a = parse(argv)
     import torch
@@ -96,6 +128,9 @@ def main(argv=None):
         T, ext = M.check_transform(np.asarray(T, dtype=np.float64).reshape(4, 4)), np.asarray(a.extents, dtype=np.float64)
     inv = object_inventory(nf, T, tuple(ext), grid_dim=a.grid_dim, level=a.level, trim=a.trim, near=a.near, far=a.far,
                            N_importance=a.N_importance, **components_args(a))
+    out = {"objects": [_json(e) for e in inv]}
+    if a.contacts:
+        out.update(contacts_json(a, nf, T, ext, out["objects"]))
     files = []
     if a.out is not None and a.poses is not None:
         os.makedirs(a.out, exist_ok=True)
@@ -103,7 +138,7 @@ def main(argv=None):
         np.savetxt(os.path.join(a.out, "extents.txt"), np.asarray(ext).reshape(1, 3), fmt="%.17g")
         files = ["scene_transform.txt", "extents.txt"]
     print(json.dumps({"scene_transform": np.asarray(T).tolist(), "extents": np.asarray(ext).tolist(), "trim": a.trim,
-                      "objects": [_json(e) for e in inv], "files": files}))
+                      **out, "files": files}))
 
 
 if __name__ == "__main__":

@@ -5,6 +5,7 @@
            --mode {translation,rotation,scale,multi} [--distance -0.25 --yaw 90 --scale 1.2] [--rest keep|drop]
            --transform T [--extents X Y Z] [--grid-dim 256] [--level 0.45] [--connectivity {6,26}] [--dilate 1] --out DIR
            [--near 4 --far 15 --N-samples 64 --N-importance 128 --N-test 4096] [--mesh [--min-cluster 400]]
+           [--check] [--until-contact [--step S] [--tolerance N]]
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict`.  POSE.npy holds the camera-to-world pose [4, 4] (or
 [3, 4]; of several [N, 4, 4] the first is used).  K is the 3x3 intrinsics, as a .npy file or as 9 numbers.
@@ -20,7 +21,14 @@ Writes DIR/rgb.png, DIR/instance.png (the arg-max label of the edited instance m
 palette, as tools/render_objects.py) and DIR/transform.json (the transformation dict, the moved label, piece and centre), and
 prints one JSON line.  --mesh also writes DIR/edited.ply (the marching-cubes mesh of the edited scene, scene space) and
 DIR/color_edited.ply (the cleaned mesh, every vertex in its label's colour of instance.png) of the same edit: the same piece,
-rest and transformation, applied per grid point to the labelled sweep (DESIGN.md, "Meshing an edited scene")."""
+rest and transformation, applied per grid point to the labelled sweep (DESIGN.md, "Meshing an edited scene").
+
+Collision checks (DESIGN.md, "Collision checks") read one keep-all labelled sweep, the one the edited mesh starts from:
+--check adds `overlap` (per label, the solid voxels of other objects the moved piece lands on, and their volume) and `landed`
+(the voxels it occupies after the move) to transform.json and the JSON line.  --until-contact (--mode translation only) slides
+the piece the way --distance moves it, by at most |--distance| in steps of --step (default one grid spacing), and stops before
+the first step that overlaps by more than --tolerance voxels; the distance found replaces --distance in the transformation that
+is rendered and meshed, and the record gains slide {requested, found, contact}."""
 import argparse
 import json
 import os
@@ -61,7 +69,22 @@ def parse(argv=None):
     ap.add_argument("--device", default="cuda")
     ap.add_argument("--mesh", action="store_true", help="also write edited.ply and color_edited.ply of the edit")
     ap.add_argument("--min-cluster", type=int, default=400, help="--mesh: smallest triangle cluster kept in color_edited.ply")
+    ap.add_argument("--check", action="store_true", help="report the overlap of the move with the other objects")
+    ap.add_argument("--until-contact", action="store_true", help="translation: slide until just before contact")
+    ap.add_argument("--step", type=float, default=None, help="--until-contact: the slide's step (default: one grid spacing)")
+    ap.add_argument("--tolerance", type=int, default=0, help="--until-contact: overlapping voxels tolerated")
     a = ap.parse_args(argv)
+    if a.until_contact:
+        if a.mode != "translation":
+            ap.error("--until-contact needs --mode translation")
+        if a.distance == 0:
+            ap.error("--until-contact needs a non-zero --distance (its sign gives the direction)")
+        if a.step is not None and not a.step > 0:
+            ap.error("--step must be > 0")
+        if a.tolerance < 0:
+            ap.error("--tolerance must be >= 0")
+    elif a.step is not None or a.tolerance != 0:
+        ap.error("--step and --tolerance need --until-contact")
     if a.dilate < 0:
         ap.error("--dilate must be >= 0")
     if len(a.hwk) not in (3, 11):
@@ -99,6 +122,17 @@ def choose_piece(a, model_fine, T, ext):
     return piece, label, np.asarray(centre, dtype=np.float64), region
 
 
+def slide_translation(a, occ, labels, T, ext, label, region):
+    """--until-contact: the slide of the piece along the way --distance moves it (manipulation_transform's translation shifts
+    the object by -distance along y) -> {requested, found, contact}; found is None when the piece overlaps where it stands."""
+    from dmnerf_b200.objects import slide_until_contact
+    r = slide_until_contact(occ, labels, T, label, (0.0, -float(np.sign(a.distance)), 0.0), abs(a.distance), step=a.step,
+                            tolerance=a.tolerance, extents=ext, level=a.level, piece=region, rest=a.rest)
+    contact = None if r["contact"] is None else {"distance": r["contact"]["distance"],
+                                                 "overlap": {str(k): v for k, v in r["contact"]["overlap"].items()}}
+    return {"requested": a.distance, "found": r["distance"], "contact": contact}
+
+
 def main(argv=None):
     a = parse(argv)
     import torch
@@ -120,6 +154,15 @@ def main(argv=None):
     T = np.load(a.transform) if a.transform.endswith(".npy") else np.loadtxt(a.transform)
     T, ext = M.check_transform(np.asarray(T, dtype=np.float64).reshape(4, 4)), tuple(a.extents)
     piece, label, centre, region = choose_piece(a, nets[1], T, ext)
+    slide = None
+    if a.check or a.until_contact:
+        from dmnerf_b200.objects import object_mask, occupancy_objects
+        with torch.no_grad():
+            occ, labels = occupancy_objects(nets[1], T, object_mask(ins_num, remove=[]), a.grid_dim, ext, a.near, a.far,
+                                            a.N_importance, device=next(nets[1].parameters()).device)
+    if a.until_contact:
+        slide = slide_translation(a, occ, labels, T, ext, label, region)
+        a.distance = np.sign(a.distance) * (slide["found"] or 0.0)
     trans = manipulation_transform(centre, a.mode, distance=a.distance, yaw=a.yaw, scale=a.scale)
     dev = next(nets[1].parameters()).device
     pose_t = torch.from_numpy(c2w).to(dev)
@@ -138,6 +181,17 @@ def main(argv=None):
     write_png(os.path.join(a.out, "instance.png"), colorize(argmax_rows(ins).reshape(a.H, a.W), lut).cpu().numpy())
     record = {"transformations": trans["transformations"], "label": label, "piece": piece, "centre": centre.tolist(),
               "rest": a.rest}
+    if slide is not None:
+        record["slide"] = slide
+    if a.check:
+        from dmnerf_b200.objects import move_overlap
+        r = move_overlap(occ, labels, T, [(label, trans["transformations"][0]["transformation"])], ext, a.level, pieces=[region],
+                         rest=a.rest)[0]
+        record["overlap"] = {"voxels": {str(k): v for k, v in r["overlap"].items()},
+                             "volume": {str(k): v for k, v in r["overlap_volume"].items()}}
+        record["landed"] = r["landed"]
+    if a.check or a.until_contact:
+        del occ, labels
     if a.mesh:
         from dmnerf_b200.objects import edited_mesh
         m = edited_mesh(nets[1], T, [(label, trans["transformations"][0]["transformation"])], a.grid_dim, ext, a.level, a.near,
