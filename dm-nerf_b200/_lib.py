@@ -69,6 +69,18 @@ class EditMove(C.Structure):
                 ("piece", RegionDesc)]
 
 
+class Placement(C.Structure):
+    """Mirror of `struct dmnerf_placement` (objects.placement_map builds one)."""
+    _fields_ = [("piece", RegionDesc), ("obstacles", C.c_uint32 * 4), ("label", C.c_int32), ("rest_drop", C.c_int32),
+                ("axis", C.c_int32), ("sign", C.c_int32), ("lift", C.c_int32)]
+
+
+class PlacementInfo(C.Structure):
+    """Mirror of `struct dmnerf_placement_info`."""
+    _fields_ = [("offset_lo", C.c_int32 * 2), ("offsets", C.c_int32 * 2), ("height", C.c_int32 * 2), ("runs", C.c_int64),
+                ("points", C.c_int64), ("sum", C.c_int64 * 3)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/dmnerf_b200.h
 PROTOTYPES = {
     "dmnerf_abi_version": (C.c_int, []),
@@ -161,6 +173,12 @@ PROTOTYPES = {
                                       C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_object_contacts": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_int64),
                                          C.c_void_p]),
+    "dmnerf_placement_map": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double),
+                                       C.POINTER(C.c_double), C.POINTER(Placement), C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.POINTER(PlacementInfo), C.c_void_p]),
+    "dmnerf_placement_contacts": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double),
+                                            C.POINTER(C.c_double), C.POINTER(Placement), C.c_int, C.c_int, C.POINTER(C.c_int32),
+                                            C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.c_void_p]),
     "dmnerf_object_components": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int, C.c_void_p,
                                            C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_component_table": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,

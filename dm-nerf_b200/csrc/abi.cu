@@ -52,6 +52,7 @@ struct dmnerf_ctx {
   MeshState mesh;                 // buffers of the other mesh entry points (mesh.cu)
   InventoryState inventory;       // buffers of the object-inventory entry points (inventory.cu)
   ComponentsState components;     // buffers of the connected-component entry points (components.cu)
+  PlaceState place;               // buffers of the placement entry points (place.cu)
   DeviceBuffer region_tmp;        // dmnerf_region_dilate: the second buffer of a multi-step dilation
   // the appearance table of the render call (scene_edit), sized for DMNERF_MAX_INS + 1 rows so that it is never reallocated
   DeviceBuffer appearance_buf;
@@ -892,6 +893,27 @@ DMNERF_API int dmnerf_object_contacts(dmnerf_ctx* ctx, const float* occ, const i
   DMN_CHECK(ctx != nullptr, "object_contacts: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
   return object_contacts(ctx->inventory, occ, labels, dim, level, n_labels, faces_host, (cudaStream_t)stream);
+}
+
+// ---- object placement (DESIGN.md, "Object placement") --------------------------------------------------------------------
+
+DMNERF_API int dmnerf_placement_map(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                    const double* transform_host, const double* extents_host, const dmnerf_placement* placement,
+                                    int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_map: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_map(ctx->place, occ, labels, dim, level, transform_host, extents_host, placement, drop, contacts, support,
+                       info_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_placement_contacts(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                         const double* transform_host, const double* extents_host, const dmnerf_placement* placement,
+                                         int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                                         int32_t* drop_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_contacts: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_contacts(ctx->place, occ, labels, dim, level, transform_host, extents_host, placement, u, v, cells_host, max_cells,
+                            n_cells_host, drop_host, (cudaStream_t)stream);
 }
 
 // ---- connected components (DESIGN.md, "Connected components") -------------------------------------------------------------

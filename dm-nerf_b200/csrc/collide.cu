@@ -184,13 +184,7 @@ int persistent_blocks(const void* kernel, int threads, size_t smem, int64_t min_
 
 // The call's one device->host read: status word, then the counters; fails on a bad status.
 int read_back(const char* out, std::vector<char>& h, int max_label, const char* who, cudaStream_t st) {
-  DMN_CUDA(cudaMemcpyAsync(h.data(), out, h.size(), cudaMemcpyDeviceToHost, st));
-  DMN_CUDA(cudaStreamSynchronize(st));
-  int bad;
-  memcpy(&bad, h.data(), sizeof(int));
-  DMN_CHECK(!(bad & BAD_NAN), "%s: the grid holds NaN values", who);
-  DMN_CHECK(!(bad & BAD_LABEL), "%s: the label grid holds a label outside [0, %d]", who, max_label);
-  return 0;
+  return read_checked(out, h.data(), h.size(), max_label, who, st);
 }
 
 // The grid's index map forward, x = A u + b (objects.grid_affine): A = S R diag(extents / (dim - 1)), S: (x, y, z) -> (x, -z, y).
@@ -236,6 +230,22 @@ void destination_box(const EditMove& e, const double A[9], int dim, int dlo[3], 
 }
 
 }  // namespace
+
+int launch_grid_check(const float* occ, const int16_t* labels, int64_t n, int n_labels, int* bad, cudaStream_t st) {
+  grid_check_kernel<<<persistent_blocks((const void*)grid_check_kernel, 256, 0, 1), 256, 0, st>>>(occ, labels, n, n_labels, bad);
+  DMN_LAUNCH_OK();
+  return 0;
+}
+
+int read_checked(const void* dev, void* host, size_t bytes, int max_label, const char* who, cudaStream_t st) {
+  DMN_CUDA(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, st));
+  DMN_CUDA(cudaStreamSynchronize(st));
+  int bad;
+  memcpy(&bad, host, sizeof(int));
+  DMN_CHECK(!(bad & BAD_NAN), "%s: the grid holds NaN values", who);
+  DMN_CHECK(!(bad & BAD_LABEL), "%s: the label grid holds a label outside [0, %d]", who, max_label);
+  return 0;
+}
 
 int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
                  const dmnerf_edit_move* cands_host, int n, const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host,
@@ -313,9 +323,7 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
   int* bad = reinterpret_cast<int*>(out);
   auto* counts = reinterpret_cast<unsigned long long*>(out + 16);
   const int64_t npts = (int64_t)dim * dim * dim;
-  grid_check_kernel<<<persistent_blocks((const void*)grid_check_kernel, 256, 0, 1), 256, 0, st>>>(occ, labels, npts, DMNERF_MAX_INS + 1,
-                                                                                                  bad);
-  DMN_LAUNCH_OK();
+  if (launch_grid_check(occ, labels, npts, DMNERF_MAX_INS + 1, bad, st)) return 2;
   if (blocks_total) {
     move_overlap_kernel<<<(unsigned)blocks_total, OV_THREADS, 0, st>>>(
         make_xform(T16, ext3, dim), map, occ, labels, level, obst, reinterpret_cast<const Candidate*>(in_d),

@@ -336,6 +336,23 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
                  cudaStream_t st);
 int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels, int64_t* faces_host,
                     cudaStream_t st);
+// The grid check of both: flags in *bad (device) for NaN in occ and labels outside [0, n_labels - 1].  read_checked copies
+// `bytes` from dev to host and synchronises; the buffer starts with that flag word, and a set flag fails the call.
+int launch_grid_check(const float* occ, const int16_t* labels, int64_t n, int n_labels, int* bad, cudaStream_t st);
+int read_checked(const void* dev, void* host, size_t bytes, int max_label, const char* who, cudaStream_t st);
+
+// Object placement (place.cu; DESIGN.md, "Object placement"): the column table (int16 per grid point: dim 1024 takes 2 GiB),
+// the object's bytes, per-column run counts and offsets, the scan's storage, the runs, the status word and the support cells.
+constexpr int PLACE_MAX_DIM = 1024;
+struct PlaceState {
+  DeviceBuffer table, object, counts, offsets, temp, runs, status, cells;
+};
+int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
+                  const dmnerf_placement* p, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
+                  cudaStream_t st);
+int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16,
+                       const double* ext3, const dmnerf_placement* p, int u, int v, int32_t* cells_host, int64_t max_cells,
+                       int64_t* n_cells_host, int32_t* drop_host, cudaStream_t st);
 
 // Connected components (components.cu): the solid points of a labelled grid split into canonically numbered components.
 // Per-context device buffers: the status words a call reads back, the chunk counts and the scan's storage.

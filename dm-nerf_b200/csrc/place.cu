@@ -1,0 +1,469 @@
+// Object placement (DESIGN.md, "Object placement"): where a lowered object comes to rest at every horizontal offset, from a
+// labelled keep-all sweep, in index space and in integers.  Heights y run along the down axis, away from down; a column is one
+// horizontal cell (h1, h2), numbered c = h1 dim + h2.
+//   column pass: per column and height the highest obstacle height at or below it (int16, -1: none), each column contiguous, and
+//                one byte per (column, height) that says whether the point belongs to the placed object;
+//   runs:        per column the maximal vertical runs of the object, written in (column, bottom) order at the exclusive scan of
+//                the per-column run counts, so that no atomic decides the order;
+//   map:         one warp per offset: the free fall (warp minimum) and blocked (OR) over the runs, then the runs that rest on an
+//                obstacle and a 128-bin shared histogram of the obstacle labels under them;
+//   contacts:    the support cells of one offset, in run order.
+// Only the bottom of a run can meet an obstacle when the object falls (the point below any other point of a run is the object),
+// so a run [z0, z1] needs one look-up per offset: b, the highest obstacle at or below its raised top.
+#include <cub/cub.cuh>
+
+#include <climits>
+#include <cstring>
+
+#include "common.cuh"
+#include "ray_ops.cuh"
+#include "sweep_grid.cuh"
+
+namespace dmnerf {
+
+namespace {
+
+constexpr int TILE = 32;                      // column pass: 32 columns x 32 heights per step
+constexpr int CP_WARPS = 8;
+constexpr int RUN_WARPS = 8;                  // runs: one warp per column
+constexpr int MAP_WARPS = 8;                  // map: one warp per offset
+constexpr int CT_THREADS = 256;               // contacts: one block
+constexpr int N_BINS = DMNERF_MAX_INS + 1;
+constexpr unsigned FULL = 0xffffffffu;
+
+// The placement's axes: linear index strides of h1, h2 and the down axis, and whether the height runs against the index.
+struct Frame {
+  int64_t s1, s2, sa;
+  int dim;
+  int flip;                                   // 1: y = dim - 1 - idx_axis (down is +e_axis)
+  int height_fast;                            // the down axis is the grid's fastest index
+};
+
+__device__ __forceinline__ int64_t point_of(const Frame& f, int h1, int h2, int y) {
+  return h1 * f.s1 + h2 * f.s2 + (int64_t)(f.flip ? f.dim - 1 - y : y) * f.sa;
+}
+
+// What the placed object and the obstacles are (DESIGN.md, "Object placement"): S = labels == label, solid, kept by the piece;
+// O = solid, label among the obstacles, not vacated (labels == label and in the piece -- every point without one -- or rest_drop).
+struct Placed {
+  Region piece;                               // bits NULL: the whole label
+  ObjMask obstacles;
+  int label, rest_drop;
+};
+
+// The status a call reads back: the grid check's flags, the object's box, height range and sums (over its points, of h1, h2
+// and y), its points and its runs.  Integer atomics only, so every field is independent of their order.
+struct Status {
+  int bad;
+  int box[6];                                 // h1 lo, hi, h2 lo, hi, y lo, hi
+  int n_cells;                                // contacts pass: support runs written; drop at the offset (-1: blocked)
+  int drop;
+  int pad;
+  unsigned long long points, runs, sum[3];
+};
+
+struct __align__(8) ObjRun {
+  int16_t h1, h2, z0, z1;
+};
+
+__device__ __forceinline__ void classify(const Frame& f, const GridXform& g, const Placed& m, const float* __restrict__ occ,
+                                         const int16_t* __restrict__ labels, float level, int64_t p, bool& obst, bool& obj) {
+  const float v = occ[p];
+  const int l = labels[p];
+  const bool solid = v > level && l >= 0 && l <= DMNERF_MAX_INS;
+  obst = solid && obj_kept(m.obstacles, l);
+  obj = false;
+  if (solid && l == m.label) {
+    bool keep = true;
+    if (m.piece.bits != nullptr) {
+      float q[3];
+      sweep_point(g, p, q);
+      keep = !region_drops(m.piece, m.label, q[0], q[1], q[2]);
+    }
+    obj = keep;
+    if (keep || m.rest_drop) obst = false;                       // vacated by the move
+  }
+}
+
+// A block takes 32 consecutive columns and walks their heights 32 at a time.  The load reads the grid along its fastest index
+// (the height when the down axis is the fastest, the column's h2 otherwise); each warp then scans 4 of the columns with its lanes
+// on the heights (a warp max-scan, carried from chunk to chunk) and writes 32 contiguous table entries and object bytes.
+__global__ void __launch_bounds__(CP_WARPS * 32) place_column_kernel(const Frame f, const GridXform g, const Placed m,
+                                                                     const float* __restrict__ occ, const int16_t* __restrict__ labels,
+                                                                     float level, int16_t* __restrict__ table,
+                                                                     uint8_t* __restrict__ object) {
+  __shared__ uint8_t s[TILE][TILE + 1];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t n_cols = (int64_t)f.dim * f.dim;
+  const int64_t c0 = (int64_t)blockIdx.x * TILE;
+  int carry[TILE / CP_WARPS];
+#pragma unroll
+  for (int k = 0; k < TILE / CP_WARPS; ++k) carry[k] = -1;
+  for (int y0 = 0; y0 < f.dim; y0 += TILE) {
+    for (int r = w; r < TILE; r += CP_WARPS) {
+      const int cl = f.height_fast ? r : lane, yl = f.height_fast ? lane : r;
+      const int64_t c = c0 + cl;
+      const int y = y0 + yl;
+      uint8_t bits = 0;
+      if (c < n_cols && y < f.dim) {
+        bool obst, obj;
+        classify(f, g, m, occ, labels, level, point_of(f, (int)(c / f.dim), (int)(c % f.dim), y), obst, obj);
+        bits = (obst ? 1 : 0) | (obj ? 2 : 0);
+      }
+      s[cl][yl] = bits;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < TILE / CP_WARPS; ++k) {
+      const int cl = w + k * CP_WARPS;
+      const int64_t c = c0 + cl;
+      const int y = y0 + lane;
+      const int bits = s[cl][lane];
+      int v = (bits & 1) ? y : -1;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const int o = __shfl_up_sync(FULL, v, d);
+        if (lane >= d) v = max(v, o);
+      }
+      v = max(v, carry[k]);
+      carry[k] = __shfl_sync(FULL, v, 31);
+      if (c < n_cols && y < f.dim) {
+        table[c * f.dim + y] = (int16_t)v;
+        object[c * f.dim + y] = (uint8_t)(bits >> 1);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// One warp per column: its runs (a bottom: object here, not below; a top: object here, not above) and its points, with the
+// object's box, height range and sums accumulated once per column.
+__global__ void __launch_bounds__(RUN_WARPS * 32) place_run_count_kernel(int dim, const uint8_t* __restrict__ object,
+                                                                         int32_t* __restrict__ counts, Status* __restrict__ st) {
+  const int lane = threadIdx.x & 31;
+  const int64_t c = (int64_t)blockIdx.x * RUN_WARPS + (threadIdx.x >> 5);
+  if (c >= (int64_t)dim * dim) return;
+  const uint8_t* col = object + c * dim;
+  int runs = 0, points = 0, ylo = INT_MAX, yhi = -1;
+  unsigned long long ysum = 0;
+  for (int y0 = 0; y0 < dim; y0 += 32) {
+    const int y = y0 + lane;
+    const bool here = y < dim && col[y];
+    const bool below = here && y > 0 && col[y - 1];
+    runs += __popc(__ballot_sync(FULL, here && !below));
+    points += __popc(__ballot_sync(FULL, here));
+    if (here) {
+      ylo = min(ylo, y);
+      yhi = max(yhi, y);
+      ysum += (unsigned long long)y;
+    }
+  }
+  ysum = __reduce_add_sync(FULL, (unsigned)ysum);                // < 2^32: at most 1024 heights of at most 1023
+  ylo = __reduce_min_sync(FULL, ylo);
+  yhi = __reduce_max_sync(FULL, yhi);
+  if (lane == 0) {
+    counts[c] = runs;
+    if (points) {
+      const int h1 = (int)(c / dim), h2 = (int)(c % dim);
+      atomicMin(&st->box[0], h1);
+      atomicMax(&st->box[1], h1);
+      atomicMin(&st->box[2], h2);
+      atomicMax(&st->box[3], h2);
+      atomicMin(&st->box[4], ylo);
+      atomicMax(&st->box[5], yhi);
+      atomicAdd(&st->points, (unsigned long long)points);
+      atomicAdd(&st->runs, (unsigned long long)runs);
+      atomicAdd(&st->sum[0], (unsigned long long)h1 * points);
+      atomicAdd(&st->sum[1], (unsigned long long)h2 * points);
+      atomicAdd(&st->sum[2], ysum);
+    }
+  }
+}
+
+// One warp per column: the column's runs at offsets[c] .. offsets[c] + counts[c] - 1, bottom to top.  The k-th bottom and the
+// k-th top of a column belong to its k-th run.
+__global__ void __launch_bounds__(RUN_WARPS * 32) place_run_write_kernel(int dim, const uint8_t* __restrict__ object,
+                                                                         const int32_t* __restrict__ counts,
+                                                                         const int32_t* __restrict__ offsets, ObjRun* __restrict__ runs) {
+  const int lane = threadIdx.x & 31;
+  const int64_t c = (int64_t)blockIdx.x * RUN_WARPS + (threadIdx.x >> 5);
+  if (c >= (int64_t)dim * dim || counts[c] == 0) return;
+  const uint8_t* col = object + c * dim;
+  ObjRun* out = runs + offsets[c];
+  const unsigned below_me = (1u << lane) - 1u;
+  int n_bot = 0, n_top = 0;
+  for (int y0 = 0; y0 < dim; y0 += 32) {
+    const int y = y0 + lane;
+    const bool here = y < dim && col[y];
+    const bool bot = here && !(y > 0 && col[y - 1]);
+    const bool top = here && !(y + 1 < dim && col[y + 1]);
+    const unsigned bm = __ballot_sync(FULL, bot), tm = __ballot_sync(FULL, top);
+    if (bot) {
+      ObjRun& r = out[n_bot + __popc(bm & below_me)];
+      r.h1 = (int16_t)(c / dim);
+      r.h2 = (int16_t)(c % dim);
+      r.z0 = (int16_t)y;
+    }
+    if (top) out[n_top + __popc(tm & below_me)].z1 = (int16_t)y;
+    n_bot += __popc(bm);
+    n_top += __popc(tm);
+  }
+}
+
+// b of run q at offset (u, v): the highest obstacle height at or below its raised top, -1 for none
+__device__ __forceinline__ int obstacle_below(const Frame& f, const int16_t* __restrict__ table, const ObjRun& q, int u, int v,
+                                              int lift) {
+  return table[((int64_t)(q.h1 + u) * f.dim + (q.h2 + v)) * f.dim + (q.z1 + lift)];
+}
+
+__global__ void __launch_bounds__(MAP_WARPS * 32) place_map_kernel(const Frame f, const int16_t* __restrict__ table,
+                                                                   const int16_t* __restrict__ labels, const ObjRun* __restrict__ runs,
+                                                                   int64_t n_runs, int u_lo, int v_lo, int U, int V, int lift,
+                                                                   int32_t* __restrict__ drop, int32_t* __restrict__ contacts,
+                                                                   int16_t* __restrict__ support) {
+  __shared__ uint32_t hist[MAP_WARPS][N_BINS];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t o = (int64_t)blockIdx.x * MAP_WARPS + w;
+  if (o >= (int64_t)U * V) return;                               // warp-uniform; nothing below synchronises the block
+  const int u = u_lo + (int)(o / V), v = v_lo + (int)(o % V);
+  int fall = INT_MAX;
+  bool blocked = false;
+  for (int64_t r = lane; r < n_runs; r += 32) {
+    const ObjRun q = runs[r];
+    const int b = obstacle_below(f, table, q, u, v, lift), bot = q.z0 + lift;
+    blocked |= b >= bot;
+    fall = min(fall, bot - b - 1);                               // b = -1: down to height 0
+  }
+  if (__any_sync(FULL, blocked)) {
+    if (lane == 0) {
+      drop[o] = -1;
+      contacts[o] = 0;
+      support[o] = -1;
+    }
+    return;
+  }
+  fall = __reduce_min_sync(FULL, fall);
+  for (int k = lane; k < N_BINS; k += 32) hist[w][k] = 0;
+  __syncwarp();
+  int n = 0;
+  for (int64_t r = lane; r < n_runs; r += 32) {
+    const ObjRun q = runs[r];
+    const int b = obstacle_below(f, table, q, u, v, lift);
+    if (b >= 0 && b == q.z0 + lift - fall - 1) {                 // the run's bottom rests on an obstacle point
+      ++n;
+      atomicAdd(&hist[w][labels[point_of(f, q.h1 + u, q.h2 + v, b)]], 1u);
+    }
+  }
+  n = __reduce_add_sync(FULL, (unsigned)n);
+  __syncwarp();
+  unsigned best = 0;                                             // (runs << 8) | (127 - label): most runs, then lowest label
+  for (int k = lane; k < N_BINS; k += 32) {
+    const unsigned key = (hist[w][k] << 8) | (unsigned)(N_BINS - 1 - k);
+    if (hist[w][k] && key > best) best = key;
+  }
+  best = __reduce_max_sync(FULL, best);
+  if (lane == 0) {
+    drop[o] = fall;
+    contacts[o] = n;
+    support[o] = n ? (int16_t)(N_BINS - 1 - (int)(best & 0xff)) : (int16_t)-1;
+  }
+}
+
+// One block: the drop at (u, v) as the map computes it, then (h1 + u, h2 + v, label below) of every run resting on an obstacle,
+// in run order (a block scan per 256 runs).
+__global__ void __launch_bounds__(CT_THREADS) place_contacts_kernel(const Frame f, const int16_t* __restrict__ table,
+                                                                    const int16_t* __restrict__ labels, const ObjRun* __restrict__ runs,
+                                                                    int64_t n_runs, int u, int v, int lift, Status* __restrict__ st,
+                                                                    int32_t* __restrict__ cells) {
+  typedef cub::BlockScan<int, CT_THREADS> Scan;
+  __shared__ typename Scan::TempStorage scan;
+  __shared__ int s_fall[CT_THREADS / 32], s_blocked[CT_THREADS / 32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int fall = INT_MAX, blocked = 0;
+  for (int64_t r = threadIdx.x; r < n_runs; r += CT_THREADS) {
+    const ObjRun q = runs[r];
+    const int b = obstacle_below(f, table, q, u, v, lift), bot = q.z0 + lift;
+    blocked |= b >= bot;
+    fall = min(fall, bot - b - 1);
+  }
+  fall = __reduce_min_sync(FULL, fall);
+  blocked = __reduce_or_sync(FULL, (unsigned)blocked);
+  if (lane == 0) {
+    s_fall[w] = fall;
+    s_blocked[w] = blocked;
+  }
+  __syncthreads();
+  fall = INT_MAX;
+  blocked = 0;
+  for (int k = 0; k < CT_THREADS / 32; ++k) {
+    fall = min(fall, s_fall[k]);
+    blocked |= s_blocked[k];
+  }
+  if (blocked) {
+    if (threadIdx.x == 0) {
+      st->drop = -1;
+      st->n_cells = 0;
+    }
+    return;                                                      // block-uniform
+  }
+  int written = 0;
+  for (int64_t r0 = 0; r0 < n_runs; r0 += CT_THREADS) {
+    const int64_t r = r0 + threadIdx.x;
+    int flag = 0, b = -1;
+    ObjRun q{};
+    if (r < n_runs) {
+      q = runs[r];
+      b = obstacle_below(f, table, q, u, v, lift);
+      flag = b >= 0 && b == q.z0 + lift - fall - 1;
+    }
+    int pos, total;
+    Scan(scan).ExclusiveSum(flag, pos, total);
+    if (flag) {
+      int32_t* cell = cells + 3 * (int64_t)(written + pos);
+      cell[0] = q.h1 + u;
+      cell[1] = q.h2 + v;
+      cell[2] = labels[point_of(f, q.h1 + u, q.h2 + v, b)];
+    }
+    written += total;
+    __syncthreads();                                             // the scan's storage is reused
+  }
+  if (threadIdx.x == 0) {
+    st->drop = fall;
+    st->n_cells = written;
+  }
+}
+
+// The checked grid, placement and object of a placement call, with its table and runs on the device.
+struct Prepared {
+  Frame f;
+  Status st;
+  int16_t* table;
+  ObjRun* runs;
+  Status* st_dev;
+  int u_lo, v_lo, U, V;
+};
+
+// Host checks, then the grid check, the column pass and the runs, with the call's one status read-back in between.
+int prepare(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
+            const dmnerf_placement* p, const char* who, Prepared& out, cudaStream_t stream) {
+  DMN_CHECK(occ && labels && T16 && ext3 && p, "%s: NULL argument", who);
+  DMN_CHECK(dim >= 2 && dim <= PLACE_MAX_DIM, "%s: dim %d out of range [2, %d]", who, dim, PLACE_MAX_DIM);
+  if (sweep_grid_check(T16, ext3, dim, level, who)) return 1;
+  DMN_CHECK(p->label >= 0 && p->label <= DMNERF_MAX_INS, "%s: label %d outside [0, %d]", who, p->label, DMNERF_MAX_INS);
+  DMN_CHECK(p->axis >= 0 && p->axis <= 2, "%s: down axis %d is not 0, 1 or 2", who, p->axis);
+  DMN_CHECK(p->sign == 1 || p->sign == -1, "%s: the sign of down along its axis must be +1 or -1, got %d", who, p->sign);
+  DMN_CHECK(p->lift >= 0 && p->lift <= dim - 1, "%s: lift %d takes the object out of the grid [0, %d]", who, p->lift, dim - 1);
+  Placed m;
+  if (piece_region(p->piece, p->label, m.piece, who, 0)) return 1;
+  for (int k = 0; k < 4; ++k) m.obstacles.w[k] = p->obstacles[k];
+  m.label = p->label;
+  m.rest_drop = p->rest_drop ? 1 : 0;
+  const int64_t d = dim, stride[3] = {d * d, d, 1};
+  const int h1 = p->axis == 0 ? 1 : 0, h2 = p->axis == 2 ? 1 : 2;
+  Frame& f = out.f;
+  f.s1 = stride[h1];
+  f.s2 = stride[h2];
+  f.sa = stride[p->axis];
+  f.dim = dim;
+  f.flip = p->sign == 1 ? 1 : 0;
+  f.height_fast = p->axis == 2 ? 1 : 0;
+  const int64_t n = d * d * d, n_cols = d * d;
+  uint8_t* object;
+  int32_t *counts, *offsets;
+  if (s.table.get((size_t)n, &out.table) || s.object.get((size_t)n, &object) || s.counts.get((size_t)n_cols, &counts) ||
+      s.offsets.get((size_t)n_cols, &offsets) || s.status.get(1, &out.st_dev))
+    return 2;
+  Status init{};
+  for (int a = 0; a < 3; ++a) {
+    init.box[2 * a] = INT_MAX;
+    init.box[2 * a + 1] = -1;
+  }
+  DMN_CUDA(cudaMemcpyAsync(out.st_dev, &init, sizeof(init), cudaMemcpyHostToDevice, stream));
+  if (launch_grid_check(occ, labels, n, DMNERF_MAX_INS + 1, &out.st_dev->bad, stream)) return 2;
+  place_column_kernel<<<(unsigned)((n_cols + TILE - 1) / TILE), CP_WARPS * 32, 0, stream>>>(f, make_xform(T16, ext3, dim), m, occ, labels,
+                                                                                             level, out.table, object);
+  DMN_LAUNCH_OK();
+  const unsigned col_blocks = (unsigned)((n_cols + RUN_WARPS - 1) / RUN_WARPS);
+  place_run_count_kernel<<<col_blocks, RUN_WARPS * 32, 0, stream>>>(dim, object, counts, out.st_dev);
+  DMN_LAUNCH_OK();
+  size_t tmp_bytes = 0;
+  DMN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts, offsets, (int)n_cols, stream));
+  char* tmp;
+  if (s.temp.get(tmp_bytes, &tmp)) return 2;
+  DMN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, counts, offsets, (int)n_cols, stream));
+  if (const int rc = read_checked(out.st_dev, &out.st, sizeof(Status), DMNERF_MAX_INS, who, stream)) return rc;
+  const Status& st = out.st;
+  DMN_CHECK(st.points > 0, "%s: label %d has no solid points%s", who, p->label, m.piece.bits ? " in its piece" : "");
+  DMN_CHECK(st.box[5] + p->lift <= dim - 1, "%s: lift %d takes the object's top (height %d) out of the grid [0, %d]", who, p->lift,
+            st.box[5], dim - 1);
+  if (s.runs.get((size_t)st.runs, &out.runs)) return 2;
+  place_run_write_kernel<<<col_blocks, RUN_WARPS * 32, 0, stream>>>(dim, object, counts, offsets, out.runs);
+  DMN_LAUNCH_OK();
+  out.u_lo = -st.box[0];
+  out.v_lo = -st.box[2];
+  out.U = dim - (st.box[1] - st.box[0]);
+  out.V = dim - (st.box[3] - st.box[2]);
+  return 0;
+}
+
+void fill_info(const Prepared& q, dmnerf_placement_info* info) {
+  memset(info, 0, sizeof(*info));
+  info->offset_lo[0] = q.u_lo;
+  info->offset_lo[1] = q.v_lo;
+  info->offsets[0] = q.U;
+  info->offsets[1] = q.V;
+  info->height[0] = q.st.box[4];
+  info->height[1] = q.st.box[5];
+  info->runs = (int64_t)q.st.runs;
+  info->points = (int64_t)q.st.points;
+  for (int a = 0; a < 3; ++a) info->sum[a] = (int64_t)q.st.sum[a];
+}
+
+}  // namespace
+
+int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
+                  const dmnerf_placement* p, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
+                  cudaStream_t st) {
+  const char* who = "placement_map";
+  DMN_CHECK(drop && contacts && support && info, "%s: NULL argument", who);
+  memset(info, 0, sizeof(*info));
+  Prepared q;
+  if (const int rc = prepare(s, occ, labels, dim, level, T16, ext3, p, who, q, st)) return rc;
+  const int64_t offsets = (int64_t)q.U * q.V;
+  place_map_kernel<<<(unsigned)((offsets + MAP_WARPS - 1) / MAP_WARPS), MAP_WARPS * 32, 0, st>>>(
+      q.f, q.table, labels, q.runs, (int64_t)q.st.runs, q.u_lo, q.v_lo, q.U, q.V, p->lift, drop, contacts, support);
+  DMN_LAUNCH_OK();
+  fill_info(q, info);
+  return 0;
+}
+
+int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16,
+                       const double* ext3, const dmnerf_placement* p, int u, int v, int32_t* cells_host, int64_t max_cells,
+                       int64_t* n_cells_host, int32_t* drop_host, cudaStream_t st) {
+  const char* who = "placement_contacts";
+  DMN_CHECK(n_cells_host && drop_host && max_cells >= 0 && (max_cells == 0 || cells_host), "%s: bad output arguments", who);
+  *n_cells_host = 0;
+  *drop_host = -1;
+  Prepared q;
+  if (const int rc = prepare(s, occ, labels, dim, level, T16, ext3, p, who, q, st)) return rc;
+  DMN_CHECK(u >= q.u_lo && u < q.u_lo + q.U && v >= q.v_lo && v < q.v_lo + q.V,
+            "%s: offset (%d, %d) outside the offsets [%d, %d] x [%d, %d] that keep the object inside the grid", who, u, v, q.u_lo,
+            q.u_lo + q.U - 1, q.v_lo, q.v_lo + q.V - 1);
+  int32_t* cells;
+  if (s.cells.get((size_t)3 * q.st.runs, &cells)) return 2;
+  place_contacts_kernel<<<1, CT_THREADS, 0, st>>>(q.f, q.table, labels, q.runs, (int64_t)q.st.runs, u, v, p->lift, q.st_dev, cells);
+  DMN_LAUNCH_OK();
+  Status h;
+  DMN_CUDA(cudaMemcpyAsync(&h, q.st_dev, sizeof(h), cudaMemcpyDeviceToHost, st));
+  DMN_CUDA(cudaStreamSynchronize(st));
+  DMN_CHECK(h.n_cells <= max_cells, "%s: %d support runs need room for as many cells, got %lld", who, h.n_cells, (long long)max_cells);
+  if (h.n_cells) {
+    DMN_CUDA(cudaMemcpyAsync(cells_host, cells, (size_t)h.n_cells * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    DMN_CUDA(cudaStreamSynchronize(st));
+  }
+  *n_cells_host = h.n_cells;
+  *drop_host = h.drop;
+  return 0;
+}
+
+}  // namespace dmnerf

@@ -20,12 +20,15 @@
                                                         -> the labelled sweep / the mesh of a scene with objects moved
     move_overlap(occ, labels, scene_transform, moves, ...) / slide_until_contact(...) / object_contacts(...) / supports(...)
                                                         -> collision checks of moves, and which objects touch, from a sweep
+    placement_map(occ, labels, scene_transform, label, down, ...) / placement(map, u, v) / place_object(..., near, ...)
+                                                        -> where a lowered object comes to rest, on what, and whether it stands
 
 Every network sample is labelled argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the
 exchanger's rule); a sample whose label is not kept has alpha = 0 in the composite of both passes, so the coarse weights of the
 selected scene drive the importance sampling.  The instance map keeps the network's channels: selection does not re-label it."""
 import ctypes as C
 import os
+from fractions import Fraction
 
 import numpy as np
 import torch
@@ -556,20 +559,221 @@ def supports(contacts, down, min_faces=1):
     """Which object rests on which, from object_contacts: along the index axis closest to +-down (network frame), the labels
     below each label's solid points -> {label: [(label_below, faces), ...]}, most faces first (then ascending label); pairs
     with fewer than min_faces faces are left out."""
-    dn = np.asarray(down, dtype=np.float64).reshape(-1)
-    if dn.shape != (3,) or not np.isfinite(dn).all() or not np.linalg.norm(dn) > 0:
-        raise ValueError("supports: down must be 3 finite numbers, not all 0, got %r" % (dn.tolist(),))
+    a, sign = down_axis(contacts["axes"], down, "supports")
     if int(min_faces) != min_faces or int(min_faces) < 1:
         raise ValueError("supports: min_faces must be an integer >= 1, got %r" % (min_faces,))
-    dots = np.asarray(contacts["axes"]) @ (dn / np.linalg.norm(dn))
-    a = int(np.argmax(np.abs(dots)))
     f = np.asarray(contacts["faces"])[a]
-    if dots[a] < 0:                                    # +e_a points up: the neighbour at p + e_a is above
+    if sign < 0:                                       # +e_a points up: the neighbour at p + e_a is above
         f = f.T
     out = {}
     for top, below in zip(*np.nonzero(f >= int(min_faces))):
         out.setdefault(int(top), []).append((int(below), int(f[top, below])))
     return {k: sorted(v, key=lambda x: (-x[1], x[0])) for k, v in sorted(out.items())}
+
+
+def down_axis(axes, down, who):
+    """The index axis closest to +-down (network frame), given the unit network-frame direction of each index axis as the rows
+    of axes [3, 3] -> (axis, sign): sign +1 when +e_axis points down, -1 when it points up."""
+    dn = np.asarray(down, dtype=np.float64).reshape(-1)
+    if dn.shape != (3,) or not np.isfinite(dn).all() or not np.linalg.norm(dn) > 0:
+        raise ValueError("%s: down must be 3 finite numbers, not all 0, got %r" % (who, dn.tolist()))
+    dots = np.asarray(axes) @ (dn / np.linalg.norm(dn))
+    a = int(np.argmax(np.abs(dots)))
+    return a, (1 if dots[a] > 0 else -1)
+
+
+# ----------------------------------------------------------------------------------------------------------------- placement
+# DESIGN.md, "Object placement": where an object lowered along the down axis comes to rest at every horizontal offset of the
+# labelled keep-all sweep, what holds it up and whether it stands; index space, integers.
+PLACE_MAX_DIM = 1024                 # int16 heights in the column table
+
+
+def _check_point(x, what):
+    p = np.asarray(x, dtype=np.float64).reshape(-1)
+    if p.shape != (3,) or not np.isfinite(p).all():
+        raise ValueError("placement: %s must be 3 finite numbers, got %r" % (what, p.tolist()))
+    return p
+
+
+def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=None, level=0.45, piece=None, rest="keep",
+                  obstacles=None):
+    """dmnerf_placement_map: object `label` (or its piece, with rest "keep" / "drop" as move_overlap) raised by `lift` voxels and
+    lowered along the index axis closest to +-down (network frame, chosen as supports chooses it), at every horizontal offset
+    that keeps it inside the grid of the labelled keep-all sweep occ / labels.  obstacles: the labels that count (default all).
+    Returns a dict:
+      drop, support, contacts: device maps [U, V] (int32, int16, int32): the voxels it falls (-1: blocked where it is raised),
+                      the obstacle label under most of its resting runs (-1: blocked, or resting on the grid's floor), and the
+                      runs that rest on an obstacle;
+      offset_lo:      the offset (u, v) of entry [0, 0], in voxels along the horizontal axes;
+      axis, sign, horizontal: the down axis, +1 when +e_axis points down, and the two horizontal index axes (ascending);
+      centre:         the object's exact centre of mass in index space (3 Fractions, axes i, j, k), from its runs;
+      runs, points:   its vertical runs and its points;
+    and what placement() needs to describe one offset."""
+    from .manipulator import _piece_region, move_pieces, move_rests
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    ext = EXTENTS if extents is None else extents
+    label = _labels([label], MAX_LABELS - 1, "placement")[0]
+    level = _check_level(level)
+    if isinstance(lift, (bool, np.bool_)) or int(lift) != lift or int(lift) < 0:
+        raise ValueError("placement: lift must be an integer >= 0 voxels, got %r" % (lift,))
+    rest_drop = move_rests(rest, 1)[0]
+    words = ALL_LABELS if obstacles is None else label_words(obstacles)
+    A, _ = grid_affine(T, 2, ext)
+    axis, sign = down_axis((A / np.linalg.norm(A, axis=0)).T, down, "placement")
+    dim = _check_sweep(occ, labels, "placement_map")
+    if not 2 <= dim <= PLACE_MAX_DIM:
+        raise ValueError("placement: dim %d outside [2, %d]" % (dim, PLACE_MAX_DIM))
+    if int(lift) > dim - 1:
+        raise ValueError("placement: lift %d takes the object out of the grid [0, %d]" % (int(lift), dim - 1))
+    move_pieces(None if piece is None else [piece], [label], MAX_LABELS - 1, occ.device)
+    desc = _lib.Placement(piece=_piece_region(piece, label, MAX_LABELS - 1, occ.device), label=label, rest_drop=int(rest_drop),
+                          axis=axis, sign=sign, lift=int(lift))
+    desc.obstacles[:] = words
+    drop = torch.empty(dim * dim, dtype=torch.int32, device=occ.device)
+    contacts = torch.empty(dim * dim, dtype=torch.int32, device=occ.device)
+    support = torch.empty(dim * dim, dtype=torch.int16, device=occ.device)
+    info = _lib.PlacementInfo()
+    try:
+        get_context(occ.device).call("dmnerf_placement_map", get_context(occ.device).handle, _lib.ptr(occ),
+                                     _lib.ptr(labels, torch.int16), dim, level, _lib.doubles(T, 16), _lib.doubles(ext, 3),
+                                     C.byref(desc), _lib.ptr(drop, torch.int32), _lib.ptr(contacts, torch.int32),
+                                     _lib.ptr(support, torch.int16), C.byref(info))
+    except RuntimeError as e:
+        if "(status 1)" in str(e):                     # the library rejected the input: a label without points, the lift, the grid
+            raise ValueError(str(e)) from None
+        raise
+    U, V = int(info.offsets[0]), int(info.offsets[1])
+    horizontal = [a for a in range(3) if a != axis]
+    n = int(info.points)
+    centre = [None] * 3
+    for a, s in zip(horizontal, info.sum[:2]):
+        centre[a] = Fraction(int(s), n)
+    ysum = Fraction(int(info.sum[2]), n)                 # heights y: idx_axis, or dim - 1 - idx_axis when +e_axis points down
+    centre[axis] = dim - 1 - ysum if sign > 0 else ysum
+    return {"drop": drop[:U * V].view(U, V), "support": support[:U * V].view(U, V), "contacts": contacts[:U * V].view(U, V),
+            "offset_lo": (int(info.offset_lo[0]), int(info.offset_lo[1])), "axis": axis, "sign": sign, "horizontal": horizontal,
+            "centre": centre, "runs": int(info.runs), "points": n, "height": (int(info.height[0]), int(info.height[1])),
+            "lift": int(lift), "label": label, "dim": dim,
+            "_call": (occ, labels, T, ext, level, desc, piece)}
+
+
+def placement_delta(m, u, v, drop):
+    """The index displacement [3] (int) of the placement at offset (u, v) with `drop`: (u, v) on the horizontal axes and
+    lift - drop in height, along -sign on the down axis."""
+    delta = [0, 0, 0]
+    delta[m["horizontal"][0]], delta[m["horizontal"][1]] = int(u), int(v)
+    delta[m["axis"]] = -m["sign"] * (m["lift"] - int(drop))
+    return delta
+
+
+def placement_transform(A, delta):
+    """translate(-A delta) (4x4 float64): the move that lands the object at x + A delta, as move_overlap and edited_sweep read it."""
+    return _translate(-(np.asarray(A, dtype=np.float64) @ np.asarray(delta, dtype=np.float64)))
+
+
+def hull_contains(cells, num, den):
+    """Whether the point num / den (num: 2 integers, den: an integer > 0) lies in the closed convex hull of the integer points
+    `cells` [n, 2]; exact: integer cross products on the points scaled by den.  False without cells."""
+    pts = sorted({(int(a) * den, int(b) * den) for a, b in cells})
+    q = (int(num[0]), int(num[1]))
+    if not pts:
+        return False
+
+    def cross(o, a, b):
+        return (a[0] - o[0]) * (b[1] - o[1]) - (a[1] - o[1]) * (b[0] - o[0])
+    hull = []
+    for part in (pts, pts[::-1]):                      # Andrew's monotone chain, collinear points dropped
+        chain = []
+        for p in part:
+            while len(chain) >= 2 and cross(chain[-2], chain[-1], p) <= 0:
+                chain.pop()
+            chain.append(p)
+        hull += chain[:-1]
+    if len(hull) <= 2:                                 # a point or a segment: q on it
+        a, b = pts[0], pts[-1]
+        return cross(a, b, q) == 0 and min(a[0], b[0]) <= q[0] <= max(a[0], b[0]) and min(a[1], b[1]) <= q[1] <= max(a[1], b[1])
+    return all(cross(hull[i], hull[(i + 1) % len(hull)], q) >= 0 for i in range(len(hull)))
+
+
+def placement(m, u, v):
+    """The placement of placement_map's result `m` at offset (u, v) (voxels; ValueError outside the map or where it is blocked):
+      transformation: the 4x4 (nested list) that lands the object there, as rigid_rays, manipulate_frame, edited_sweep and
+                      move_overlap read it;
+      offset, drop, support, supported (support >= 0);
+      contacts:       the support cells [(h1, h2, label below), ...] (dmnerf_placement_contacts), one per resting run;
+      stable:         the object's centre of mass projects into the closed convex hull of the support cells (exact);
+      centre:         the placed centre of mass, network frame."""
+    u, v = int(u), int(v)
+    (u0, v0), (U, V) = m["offset_lo"], tuple(m["drop"].shape)
+    if not (u0 <= u < u0 + U and v0 <= v < v0 + V):
+        raise ValueError("placement: offset (%d, %d) outside [%d, %d] x [%d, %d]" % (u, v, u0, u0 + U - 1, v0, v0 + V - 1))
+    drop = int(m["drop"][u - u0, v - v0])
+    if drop < 0:
+        raise ValueError("placement: offset (%d, %d) is blocked: the raised object overlaps an obstacle" % (u, v))
+    support, n = int(m["support"][u - u0, v - v0]), int(m["contacts"][u - u0, v - v0])
+    occ, labels, T, ext, level, desc, _ = m["_call"]
+    cells = np.zeros((max(n, 1), 3), dtype=np.int32)
+    got, dr = C.c_int64(0), C.c_int32(0)
+    ctx = get_context(occ.device)
+    ctx.call("dmnerf_placement_contacts", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), m["dim"], level,
+             _lib.doubles(T, 16), _lib.doubles(ext, 3), C.byref(desc), u, v, cells.ctypes.data_as(C.POINTER(C.c_int32)), n,
+             C.byref(got), C.byref(dr))
+    if int(got.value) != n or int(dr.value) != drop:
+        raise RuntimeError("placement: the grid changed since placement_map (offset (%d, %d): drop %d, %d resting runs; now %d, %d)"
+                           % (u, v, drop, n, int(dr.value), int(got.value)))
+    cells = cells[:n]
+    h1, h2 = m["horizontal"]
+    den = m["points"]
+    num = (m["centre"][h1] * den + u * den, m["centre"][h2] * den + v * den)
+    delta = placement_delta(m, u, v, drop)
+    A, b = grid_affine(T, m["dim"], ext)
+    centre = A @ (np.array([float(c) for c in m["centre"]]) + np.asarray(delta, dtype=np.float64)) + b
+    return {"transformation": placement_transform(A, delta).tolist(), "offset": (u, v), "drop": drop, "support": support,
+            "supported": support >= 0, "contacts": [tuple(int(x) for x in c) for c in cells],
+            "stable": hull_contains(cells[:, :2], num, den), "centre": centre, "delta": delta}
+
+
+def place_object(occ, labels, scene_transform, label, down, near, on=None, stable=True, lift=0, max_tests=64, extents=None,
+                 level=0.45, piece=None, rest="keep", obstacles=None):
+    """The placement of object `label` (or its piece) closest to the network-frame point `near`: over placement_map's offsets
+    that are not blocked and rest on an obstacle whose label is in `on` (default: any), ordered by the distance of the placed
+    centre of mass from `near` across the down axis (ties: the lowest (u, v)), the first that is stable -- testing at most
+    max_tests of them -- or, with stable=False, the first.  Returns {"placement": placement() of it, or None; "reason": None, or
+    why there is none; "candidates": how many offsets qualified; "tested": stability tests run; "map": placement_map's result}."""
+    near = _check_point(near, "near")
+    if isinstance(max_tests, (bool, np.bool_)) or int(max_tests) != max_tests or int(max_tests) < 1:
+        raise ValueError("placement: max_tests must be an integer >= 1, got %r" % (max_tests,))
+    on = None if on is None else set(_labels(on, MAX_LABELS - 1, "placement"))
+    m = placement_map(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles)
+    drop, support = m["drop"].cpu().numpy(), m["support"].cpu().numpy()
+    ok = (drop >= 0) & (support >= 0)
+    if on is not None:
+        ok &= np.isin(support, sorted(on))
+    iu, iv = np.nonzero(ok)
+    out = {"placement": None, "reason": None, "candidates": int(iu.size), "tested": 0, "map": m}
+    if iu.size == 0:
+        out["reason"] = "no offset rests on %s" % ("an obstacle" if on is None else "label(s) %s" % sorted(on))
+        return out
+    T, ext = m["_call"][2], m["_call"][3]
+    A, b = grid_affine(T, m["dim"], ext)
+    u, v = iu + m["offset_lo"][0], iv + m["offset_lo"][1]
+    c = np.array([float(x) for x in m["centre"]])
+    delta = np.zeros((iu.size, 3))
+    delta[:, m["horizontal"][0]], delta[:, m["horizontal"][1]] = u, v
+    delta[:, m["axis"]] = -m["sign"] * (m["lift"] - drop[iu, iv])
+    gap = (c[None, :] + delta) @ A.T + b - near[None, :]
+    axis_dir = A[:, m["axis"]] / np.linalg.norm(A[:, m["axis"]])
+    gap -= np.outer(gap @ axis_dir, axis_dir)
+    order = np.lexsort((v, u, np.linalg.norm(gap, axis=1)))
+    for k in order[:int(max_tests)]:
+        p = placement(m, u[k], v[k])
+        out["tested"] += 1
+        if p["stable"] or not stable:
+            out["placement"] = p
+            return out
+    out["reason"] = "none of the %d nearest of %d resting offsets is stable" % (min(int(max_tests), iu.size), iu.size)
+    return out
 
 
 def largest_component_grid(occ, labels, level, objects):

@@ -490,6 +490,58 @@ DMNERF_API int dmnerf_move_overlap(dmnerf_ctx* ctx, const float* occ, const int1
 DMNERF_API int dmnerf_object_contacts(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                                       int64_t* faces_host /* [3][n_labels][n_labels] */, void* stream);
 
+/* ---- object placement (DESIGN.md, "Object placement"; no counterpart in the original) ---------------------------------------
+ * Where object `label` (or its piece) comes to rest when it is lowered at every horizontal offset, from the labelled keep-all
+ * sweep occ / labels [dim^3] (DEVICE float32 / int16, C order) of the grid (transform_host, extents_host, dim), in index space
+ * and in integers: every result is bit-reproducible.  Heights y run along index axis `axis`, away from down: y = dim - 1 - idx
+ * when sign is +1 (down is +e_axis), y = idx when sign is -1.  The horizontal axes (h1, h2) are the other two, ascending.
+ *   object S:    labels[p] == label, occ[p] > level, and the piece keeps p's fp32 sweep point (every p without a piece);
+ *   obstacles O: occ[p] > level, labels[p] in obstacles, and p not vacated (labels[p] == label and p in the piece -- every point
+ *                without one -- or rest_drop), as dmnerf_move_overlap.
+ * At offset (u, v) the object is raised by lift and lowered a voxel at a time: drop = -1 (blocked) when S + (u, v, lift)
+ * overlaps O, otherwise the largest h such that no S + (u, v, lift - h') with h' in 0..h overlaps O or reaches below height 0.
+ * At rest, contacts = the runs of S (maximal vertical runs of one column) whose bottom sits directly on an obstacle point, and
+ * support = the obstacle label under the most of them (ties: the lowest label), -1 when there is none or the offset is blocked.
+ * The offsets are those that keep S's horizontal index box inside the grid: u in [-h1_lo, dim - 1 - h1_hi], and as much for v.
+ * The object lands at trans^-1 x for trans = translate(-A delta), delta the index displacement (dmnerf_move_overlap's convention).
+ * Each call re-reads the grid: the grid check, a column pass that writes the column table (the highest obstacle height at or
+ * below every height of every column, int16, in the context: 2 bytes per grid point, 2 GiB at dim 1024) and the object's runs.
+ * Rejected on the host, before any launch: dim outside [2, 1024], level outside (0, 1), a scene transform with det <= 0 or
+ * extents not finite and > 0, a label outside [0, 127], an axis outside {0, 1, 2}, a sign other than +-1, a lift outside
+ * [0, dim - 1], a piece whose `applies` lacks the label.  After the one status read-back, before the map is computed: NaN in
+ * occ, a label outside [0, 127] in labels, a label without solid points (in its piece), a lift that takes the object's top out
+ * of the grid.
+ * dmnerf_placement_map: drop, contacts (DEVICE int32) and support (DEVICE int16), each with room for dim * dim entries, receive
+ *   the [U][V] row-major map; entry [i][j] is offset (offset_lo[0] + i, offset_lo[1] + j).  info_host gets the offsets, the
+ *   object's height range, its runs, its points |S| and its sums over S of (h1, h2, y), so that its centre is exact.
+ * dmnerf_placement_contacts: the support of one offset (u, v) inside the map's range: cells_host [n][3] (HOST int32, room for
+ *   max_cells) = (h1 + u, h2 + v, label below) of every run resting on an obstacle, in (column, bottom) order of the runs;
+ *   n_cells_host = n; drop_host = the map's drop there (no cells when it is -1).  Synchronises the stream. */
+typedef struct dmnerf_placement {
+  dmnerf_region piece;        /* bits NULL: the whole label is placed */
+  uint32_t obstacles[4];      /* the labels that are obstacles, bit k of word k / 32 */
+  int32_t label;
+  int32_t rest_drop;          /* 1: the solid points of the label outside the piece are vacated too */
+  int32_t axis;               /* the down axis: index axis 0, 1 or 2 */
+  int32_t sign;               /* +1: down is +e_axis; -1: down is -e_axis */
+  int32_t lift;               /* voxels the object is raised by before it is lowered */
+} dmnerf_placement;
+typedef struct dmnerf_placement_info {
+  int32_t offset_lo[2];       /* the offset (u, v) of map entry [0][0] */
+  int32_t offsets[2];         /* U, V */
+  int32_t height[2];          /* the lowest and highest height of the object's points */
+  int64_t runs;               /* its vertical runs */
+  int64_t points;             /* |S| */
+  int64_t sum[3];             /* sums over S of h1, h2 and y */
+} dmnerf_placement_info;
+DMNERF_API int dmnerf_placement_map(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                    const double* transform_host, const double* extents_host, const dmnerf_placement* placement,
+                                    int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info_host, void* stream);
+DMNERF_API int dmnerf_placement_contacts(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                         const double* transform_host, const double* extents_host, const dmnerf_placement* placement,
+                                         int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                                         int32_t* drop_host, void* stream);
+
 /* ---- connected components (DESIGN.md, "Connected components"; no counterpart in the original) --------------------------------
  * The solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order, p = (i dim + j) dim + k) split into components:
  * two solid points are adjacent when they are face neighbours (connectivity 6) or face, edge or corner neighbours (26), never

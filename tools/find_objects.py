@@ -4,7 +4,7 @@
     python tools/find_objects.py CHECKPOINT.tar (--transform T [--extents X Y Z] | --poses POSES.npy --hwk H W K) [--trim 0]
                                  [--grid-dim 256] [--level 0.45] [--near 4 --far 15] [--out DIR]
                                  [--components {largest,split} [--connectivity {6,26}] [--min-voxels N]]
-                                 [--contacts [--down X Y Z]]
+                                 [--contacts [--down X Y Z]] [--placements L --down X Y Z [--lift N] --out DIR]
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict`.  The grid is either given (--transform: a 4x4 as
 .npy or 16 numbers of text, with --extents, default the original's 1.9 7 7) or found from the cameras (--poses: [N, 4, 4] or
@@ -17,7 +17,10 @@ label's component count and discarded voxels; `split` reports every component of
 --contacts adds the touching pairs (DESIGN.md, "Collision checks") of a sweep with the inventory's selection: per index axis its
 network-frame direction and one voxel face's area, and per pair of labels (a, b) the faces where a solid point of a has a solid
 point of b next to it along +axis, with their area.  --down (network frame) adds to each object `rests_on`: the labels below it
-along the index axis closest to that direction, with the faces they share."""
+along the index axis closest to that direction, with the faces they share.  --placements L (DESIGN.md, "Object placement") writes
+DIR/placements_L.npz: the placement map of label L lowered along --down (raised by --lift voxels first) on the keep-all sweep --
+drop, support and contacts [U, V], offset_lo, axis, sign, horizontal, centre (index space), runs and points -- and names it in
+the JSON line's `placements`."""
 import argparse
 import json
 import os
@@ -52,10 +55,21 @@ def parse(argv=None):
     ap.add_argument("--contacts", action="store_true", help="also report which objects touch")
     ap.add_argument("--down", type=float, nargs=3, default=None, metavar=("X", "Y", "Z"),
                     help="with --contacts: the network-frame down direction; adds rests_on per object")
+    ap.add_argument("--placements", type=int, default=None, metavar="L", help="write the placement map of label L (needs --down)")
+    ap.add_argument("--lift", type=int, default=None, help="with --placements: voxels the object is raised by first (default 0)")
     ap.add_argument("--device", default="cuda")
     a = ap.parse_args(argv)
-    if a.down is not None and not a.contacts:
-        ap.error("--down needs --contacts")
+    if a.down is not None and not (a.contacts or a.placements is not None):
+        ap.error("--down needs --contacts or --placements")
+    if a.placements is not None:
+        if a.down is None or a.out is None:
+            ap.error("--placements needs --down and --out")
+        if not 0 <= a.placements <= 127:
+            ap.error("--placements: label %d outside [0, 127]" % a.placements)
+        if a.lift is not None and a.lift < 0:
+            ap.error("--lift must be >= 0")
+    elif a.lift is not None:
+        ap.error("--lift needs --placements")
     if a.down is not None and not any(a.down):
         ap.error("--down must not be 0 0 0")
     if a.components is None and a.connectivity is not None:
@@ -111,6 +125,23 @@ def contacts_json(a, nf, T, ext, objects):
     return {"contacts": {"axes": c["axes"].tolist(), "face_area": c["face_area"].tolist(), "pairs": pairs}}
 
 
+def placements_npz(a, nf, T, ext):
+    """--placements: placement_map of the label on the keep-all sweep, written to DIR/placements_L.npz -> its file name."""
+    import torch
+    from dmnerf_b200.objects import object_mask, occupancy_objects, placement_map
+    ins_num = int(nf.ins_linear.weight.shape[0]) - 1
+    with torch.no_grad():
+        occ, labels = occupancy_objects(nf, T, object_mask(ins_num, remove=[]), a.grid_dim, tuple(ext), a.near, a.far, a.N_importance,
+                                        device=next(nf.parameters()).device)
+        m = placement_map(occ, labels, T, a.placements, a.down, a.lift or 0, tuple(ext), a.level)
+    name = "placements_%d.npz" % a.placements
+    np.savez(os.path.join(a.out, name), drop=m["drop"].cpu().numpy(), support=m["support"].cpu().numpy(),
+             contacts=m["contacts"].cpu().numpy(), offset_lo=np.array(m["offset_lo"]), axis=m["axis"], sign=m["sign"],
+             horizontal=np.array(m["horizontal"]), centre=np.array([float(c) for c in m["centre"]]), runs=m["runs"],
+             points=m["points"], lift=m["lift"])
+    return name
+
+
 def main(argv=None):
     a = parse(argv)
     import torch
@@ -132,11 +163,15 @@ def main(argv=None):
     if a.contacts:
         out.update(contacts_json(a, nf, T, ext, out["objects"]))
     files = []
+    if a.placements is not None:
+        os.makedirs(a.out, exist_ok=True)
+        out["placements"] = placements_npz(a, nf, T, ext)
+        files.append(out["placements"])
     if a.out is not None and a.poses is not None:
         os.makedirs(a.out, exist_ok=True)
         np.savetxt(os.path.join(a.out, "scene_transform.txt"), T, fmt="%.17g")
         np.savetxt(os.path.join(a.out, "extents.txt"), np.asarray(ext).reshape(1, 3), fmt="%.17g")
-        files = ["scene_transform.txt", "extents.txt"]
+        files += ["scene_transform.txt", "extents.txt"]
     print(json.dumps({"scene_transform": np.asarray(T).tolist(), "extents": np.asarray(ext).tolist(), "trim": a.trim,
                       **out, "files": files}))
 

@@ -2,7 +2,8 @@
 """Move one piece of an object of a trained DM-NeRF checkpoint and render the edited frame (DESIGN.md, "Moving pieces").
 
     python tools/move_objects.py CHECKPOINT.tar --pose POSE.npy --hwk H W K (--move-label L | --move-piece ID)
-           --mode {translation,rotation,scale,multi} [--distance -0.25 --yaw 90 --scale 1.2] [--rest keep|drop]
+           (--mode {translation,rotation,scale,multi} [--distance -0.25 --yaw 90 --scale 1.2]
+            | --place-at X Y Z --down X Y Z [--on L ...] [--lift N] [--any-stability]) [--rest keep|drop]
            --transform T [--extents X Y Z] [--grid-dim 256] [--level 0.45] [--connectivity {6,26}] [--dilate 1] --out DIR
            [--near 4 --far 15 --N-samples 64 --N-importance 128 --N-test 4096] [--mesh [--min-cluster 400]]
            [--check] [--until-contact [--step S] [--tolerance N]]
@@ -28,7 +29,14 @@ Collision checks (DESIGN.md, "Collision checks") read one keep-all labelled swee
 (the voxels it occupies after the move) to transform.json and the JSON line.  --until-contact (--mode translation only) slides
 the piece the way --distance moves it, by at most |--distance| in steps of --step (default one grid spacing), and stops before
 the first step that overlaps by more than --tolerance voxels; the distance found replaces --distance in the transformation that
-is rendered and meshed, and the record gains slide {requested, found, contact}."""
+is rendered and meshed, and the record gains slide {requested, found, contact}.
+
+Placement (DESIGN.md, "Object placement"): --place-at chooses the move instead of --mode.  The piece is lowered along the index
+axis closest to --down (network frame), after being raised by --lift voxels, at every horizontal offset of the keep-all sweep;
+of the offsets where it rests on an object (of a label among --on, when given), the one whose centre of mass lands nearest to
+the network-frame point --place-at across the down axis, and stands (its centre over the hull of its support; --any-stability:
+the nearest, standing or not), is rendered and meshed as --until-contact's is.  The record gains place {offset, drop, support,
+stable, contacts}."""
 import argparse
 import json
 import os
@@ -49,10 +57,16 @@ def parse(argv=None):
     which = ap.add_mutually_exclusive_group(required=True)
     which.add_argument("--move-label", type=int, metavar="L", help="move the largest piece of object label L")
     which.add_argument("--move-piece", type=int, metavar="ID", help="move this piece (a component id of the sweep)")
-    ap.add_argument("--mode", required=True, choices=("translation", "rotation", "scale", "multi"))
-    ap.add_argument("--distance", type=float, default=-0.25, help="translation along y")
-    ap.add_argument("--yaw", type=float, default=90.0, help="rotation about z, degrees")
-    ap.add_argument("--scale", type=float, default=1.2)
+    ap.add_argument("--mode", choices=("translation", "rotation", "scale", "multi"))
+    ap.add_argument("--distance", type=float, default=None, help="translation along y (default -0.25)")
+    ap.add_argument("--yaw", type=float, default=None, help="rotation about z, degrees (default 90)")
+    ap.add_argument("--scale", type=float, default=None, help="(default 1.2)")
+    ap.add_argument("--place-at", type=float, nargs=3, default=None, metavar=("X", "Y", "Z"),
+                    help="place the piece where it rests nearest to this network-frame point (replaces --mode)")
+    ap.add_argument("--down", type=float, nargs=3, default=None, metavar=("X", "Y", "Z"), help="--place-at: network-frame down")
+    ap.add_argument("--on", type=int, nargs="+", default=None, metavar="L", help="--place-at: rest on one of these labels")
+    ap.add_argument("--lift", type=int, default=None, help="--place-at: voxels the piece is raised by first (default 0)")
+    ap.add_argument("--any-stability", action="store_true", help="--place-at: take the nearest resting offset, stable or not")
     ap.add_argument("--rest", choices=("keep", "drop"), default="keep", help="the rest of the moved label: kept or removed")
     ap.add_argument("--transform", required=True, help="4x4 scene transform of the sweep grid (.npy or text)")
     ap.add_argument("--extents", type=float, nargs=3, default=[1.9, 7.0, 7.0], metavar=("X", "Y", "Z"))
@@ -74,6 +88,24 @@ def parse(argv=None):
     ap.add_argument("--step", type=float, default=None, help="--until-contact: the slide's step (default: one grid spacing)")
     ap.add_argument("--tolerance", type=int, default=0, help="--until-contact: overlapping voxels tolerated")
     a = ap.parse_args(argv)
+    if a.place_at is not None:
+        for flag, given in (("--mode", a.mode is not None), ("--until-contact", a.until_contact), ("--distance", a.distance is not None),
+                            ("--yaw", a.yaw is not None), ("--scale", a.scale is not None)):
+            if given:
+                ap.error("--place-at replaces %s" % flag)
+        if a.down is None or not any(a.down):
+            ap.error("--place-at needs --down X Y Z, not 0 0 0")
+        if a.lift is not None and a.lift < 0:
+            ap.error("--lift must be >= 0")
+        a.lift = a.lift or 0
+    else:
+        if a.mode is None:
+            ap.error("give --mode or --place-at")
+        if a.down is not None or a.on is not None or a.lift is not None or a.any_stability:
+            ap.error("--down, --on, --lift and --any-stability need --place-at")
+        a.distance = -0.25 if a.distance is None else a.distance
+        a.yaw = 90.0 if a.yaw is None else a.yaw
+        a.scale = 1.2 if a.scale is None else a.scale
     if a.until_contact:
         if a.mode != "translation":
             ap.error("--until-contact needs --mode translation")
@@ -133,6 +165,19 @@ def slide_translation(a, occ, labels, T, ext, label, region):
     return {"requested": a.distance, "found": r["distance"], "contact": contact}
 
 
+def place_piece(a, occ, labels, T, ext, label, region):
+    """--place-at: place_object for the piece -> {transformation, offset, drop, support, stable, contacts}; exits when no offset
+    qualifies."""
+    from dmnerf_b200.objects import place_object
+    r = place_object(occ, labels, T, label, a.down, a.place_at, on=a.on, stable=not a.any_stability, lift=a.lift, extents=ext,
+                     level=a.level, piece=region, rest=a.rest)
+    p = r["placement"]
+    if p is None:
+        raise SystemExit("move_objects: no placement: %s" % r["reason"])
+    return {"transformation": p["transformation"], "offset": list(p["offset"]), "drop": p["drop"], "support": p["support"],
+            "stable": p["stable"], "contacts": [list(c) for c in p["contacts"]]}
+
+
 def main(argv=None):
     a = parse(argv)
     import torch
@@ -154,8 +199,8 @@ def main(argv=None):
     T = np.load(a.transform) if a.transform.endswith(".npy") else np.loadtxt(a.transform)
     T, ext = M.check_transform(np.asarray(T, dtype=np.float64).reshape(4, 4)), tuple(a.extents)
     piece, label, centre, region = choose_piece(a, nets[1], T, ext)
-    slide = None
-    if a.check or a.until_contact:
+    slide = place = None
+    if a.check or a.until_contact or a.place_at is not None:
         from dmnerf_b200.objects import object_mask, occupancy_objects
         with torch.no_grad():
             occ, labels = occupancy_objects(nets[1], T, object_mask(ins_num, remove=[]), a.grid_dim, ext, a.near, a.far,
@@ -163,7 +208,11 @@ def main(argv=None):
     if a.until_contact:
         slide = slide_translation(a, occ, labels, T, ext, label, region)
         a.distance = np.sign(a.distance) * (slide["found"] or 0.0)
-    trans = manipulation_transform(centre, a.mode, distance=a.distance, yaw=a.yaw, scale=a.scale)
+    if a.place_at is not None:
+        place = place_piece(a, occ, labels, T, ext, label, region)
+        trans = {"transformations": [{"transformation": place.pop("transformation"), "mode": "placement"}]}
+    else:
+        trans = manipulation_transform(centre, a.mode, distance=a.distance, yaw=a.yaw, scale=a.scale)
     dev = next(nets[1].parameters()).device
     pose_t = torch.from_numpy(c2w).to(dev)
     tar_o, tar_d = rigid_rays(a.H, a.W, a.K, trans["transformations"][0]["transformation"], pose_t)
@@ -183,6 +232,8 @@ def main(argv=None):
               "rest": a.rest}
     if slide is not None:
         record["slide"] = slide
+    if place is not None:
+        record["place"] = place
     if a.check:
         from dmnerf_b200.objects import move_overlap
         r = move_overlap(occ, labels, T, [(label, trans["transformations"][0]["transformation"])], ext, a.level, pieces=[region],
@@ -190,7 +241,7 @@ def main(argv=None):
         record["overlap"] = {"voxels": {str(k): v for k, v in r["overlap"].items()},
                              "volume": {str(k): v for k, v in r["overlap_volume"].items()}}
         record["landed"] = r["landed"]
-    if a.check or a.until_contact:
+    if a.check or a.until_contact or a.place_at is not None:
         del occ, labels
     if a.mesh:
         from dmnerf_b200.objects import edited_mesh
