@@ -51,6 +51,7 @@ class RenderIO(C.Structure):
 
 MAX_MOVES = 8                # DMNERF_MAX_MOVES
 MAX_CANDIDATES = 4096        # DMNERF_MAX_CANDIDATES
+MAX_BASES = 64               # DMNERF_MAX_BASES
 
 
 class Pieces(C.Structure):
@@ -179,6 +180,14 @@ PROTOTYPES = {
     "dmnerf_placement_contacts": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double),
                                             C.POINTER(C.c_double), C.POINTER(Placement), C.c_int, C.c_int, C.POINTER(C.c_int32),
                                             C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.c_void_p]),
+    "dmnerf_placement_maps": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double),
+                                        C.POINTER(C.c_double), C.POINTER(Placement), C.POINTER(C.c_double), C.POINTER(C.c_int32),
+                                        C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PlacementInfo), C.POINTER(C.c_int32),
+                                        C.c_void_p]),
+    "dmnerf_placement_contacts_moved": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double),
+                                                  C.POINTER(C.c_double), C.POINTER(Placement), C.POINTER(C.c_double),
+                                                  C.POINTER(C.c_int32), C.c_int, C.c_int, C.POINTER(C.c_int32), C.c_int64,
+                                                  C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.c_void_p]),
     "dmnerf_object_components": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int, C.c_void_p,
                                            C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_component_table": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -912,8 +912,30 @@ DMNERF_API int dmnerf_placement_contacts(dmnerf_ctx* ctx, const float* occ, cons
                                          int32_t* drop_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "placement_contacts: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_contacts(ctx->place, occ, labels, dim, level, transform_host, extents_host, placement, u, v, cells_host, max_cells,
-                            n_cells_host, drop_host, (cudaStream_t)stream);
+  return placement_contacts(ctx->place, occ, labels, dim, level, transform_host, extents_host, placement, nullptr, nullptr, u, v,
+                            cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_placement_maps(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                     const double* transform_host, const double* extents_host, const dmnerf_placement* placement,
+                                     const double* bases_host, const int32_t* box_host, int n_bases, int32_t* drop, int32_t* contacts,
+                                     int16_t* support, dmnerf_placement_info* info_host, int32_t* status_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_maps: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_maps(ctx->place, occ, labels, dim, level, transform_host, extents_host, placement, bases_host, box_host, n_bases,
+                        drop, contacts, support, info_host, status_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_placement_contacts_moved(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                               const double* transform_host, const double* extents_host,
+                                               const dmnerf_placement* placement, const double* base_host, const int32_t* box_host,
+                                               int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                                               int32_t* drop_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_contacts_moved: ctx is NULL");
+  DMN_CHECK(base_host != nullptr, "placement_contacts_moved: base is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_contacts(ctx->place, occ, labels, dim, level, transform_host, extents_host, placement, base_host, box_host, u, v,
+                            cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
 }
 
 // ---- connected components (DESIGN.md, "Connected components") -------------------------------------------------------------

@@ -350,9 +350,15 @@ struct PlaceState {
 int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
                   const dmnerf_placement* p, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
                   cudaStream_t st);
+// The same for the object as each move of bases_host [n][12] leaves it (DESIGN.md, "Turned placements"): one column table, then
+// per base the moved object's bytes, runs and map; status [n] says which were placed.
+int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
+                   const dmnerf_placement* p, const double* bases_host, const int32_t* box_host, int n_bases, int32_t* drop,
+                   int32_t* contacts, int16_t* support, dmnerf_placement_info* info, int32_t* status, cudaStream_t st);
+// base_host NULL: the object as it lies (dmnerf_placement_contacts); otherwise as base_host [12] and box_host [6] leave it.
 int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16,
-                       const double* ext3, const dmnerf_placement* p, int u, int v, int32_t* cells_host, int64_t max_cells,
-                       int64_t* n_cells_host, int32_t* drop_host, cudaStream_t st);
+                       const double* ext3, const dmnerf_placement* p, const double* base_host, const int32_t* box_host, int u, int v,
+                       int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host, int32_t* drop_host, cudaStream_t st);
 
 // Connected components (components.cu): the solid points of a labelled grid split into canonically numbered components.
 // Per-context device buffers: the status words a call reads back, the chunk counts and the scan's storage.

@@ -14,6 +14,7 @@
 
 #include <climits>
 #include <cstring>
+#include <vector>
 
 #include "common.cuh"
 #include "ray_ops.cuh"
@@ -28,6 +29,7 @@ constexpr int CP_WARPS = 8;
 constexpr int RUN_WARPS = 8;                  // runs: one warp per column
 constexpr int MAP_WARPS = 8;                  // map: one warp per offset
 constexpr int CT_THREADS = 256;               // contacts: one block
+constexpr int MV_THREADS = 256;               // moved object: one thread per (column, height)
 constexpr int N_BINS = DMNERF_MAX_INS + 1;
 constexpr unsigned FULL = 0xffffffffu;
 
@@ -87,7 +89,9 @@ __device__ __forceinline__ void classify(const Frame& f, const GridXform& g, con
 
 // A block takes 32 consecutive columns and walks their heights 32 at a time.  The load reads the grid along its fastest index
 // (the height when the down axis is the fastest, the column's h2 otherwise); each warp then scans 4 of the columns with its lanes
-// on the heights (a warp max-scan, carried from chunk to chunk) and writes 32 contiguous table entries and object bytes.
+// on the heights (a warp max-scan, carried from chunk to chunk) and writes 32 contiguous table entries and, with OBJECT (the
+// object as it lies), object bytes.  A moved object's bytes come from place_moved_kernel; the table never depends on the move.
+template <bool OBJECT>
 __global__ void __launch_bounds__(CP_WARPS * 32) place_column_kernel(const Frame f, const GridXform g, const Placed m,
                                                                      const float* __restrict__ occ, const int16_t* __restrict__ labels,
                                                                      float level, int16_t* __restrict__ table,
@@ -129,11 +133,31 @@ __global__ void __launch_bounds__(CP_WARPS * 32) place_column_kernel(const Frame
       carry[k] = __shfl_sync(FULL, v, 31);
       if (c < n_cols && y < f.dim) {
         table[c * f.dim + y] = (int16_t)v;
-        object[c * f.dim + y] = (uint8_t)(bits >> 1);
+        if (OBJECT) object[c * f.dim + y] = (uint8_t)(bits >> 1);
       }
     }
     __syncthreads();
   }
+}
+
+// The object as the move e leaves it (DESIGN.md, "Turned placements"), one thread per (column, height) in the object bytes
+// order: point p belongs to it when src(p) of the collision checks holds -- q = edit_target(e, p) in the box B, labels[q] == label,
+// occ[q] > level and the piece keeps the target t.  Points the move carries outside the grid are lost, as in the edited sweep.
+__global__ void __launch_bounds__(MV_THREADS) place_moved_kernel(const Frame f, const GridXform g, const EditMove e,
+                                                                 const float* __restrict__ occ, const int16_t* __restrict__ labels,
+                                                                 float level, uint8_t* __restrict__ object) {
+  const int64_t o = (int64_t)blockIdx.x * MV_THREADS + threadIdx.x, d = f.dim;
+  if (o >= d * d * d) return;
+  const int64_t c = o / d;
+  float p[3], t[3];
+  double q[3];
+  sweep_point(g, point_of(f, (int)(c / d), (int)(c % d), (int)(o % d)), p);
+  bool src = edit_target(e.trans, e.inv, e.b, e.lo, e.hi, !e.empty, p, t, q);
+  if (src) {
+    const int64_t qi = ((int64_t)q[0] * d + (int64_t)q[1]) * d + (int64_t)q[2];
+    src = labels[qi] == e.label && occ[qi] > level && (e.piece.bits == nullptr || !region_drops(e.piece, e.label, t[0], t[1], t[2]));
+  }
+  object[o] = src ? 1 : 0;
 }
 
 // One warp per column: its runs (a bottom: object here, not below; a top: object here, not above) and its points, with the
@@ -333,19 +357,29 @@ __global__ void __launch_bounds__(CT_THREADS) place_contacts_kernel(const Frame 
   }
 }
 
-// The checked grid, placement and object of a placement call, with its table and runs on the device.
+// The checked grid and placement of a call, its buffers, and after object_runs the object's status, runs and offset range.
 struct Prepared {
   Frame f;
+  GridXform g;
+  Placed m;
+  const float* occ;
+  const int16_t* labels;
+  float level;
+  int lift;
   Status st;
   int16_t* table;
+  uint8_t* object;
+  int32_t *counts, *offsets;
   ObjRun* runs;
   Status* st_dev;
   int u_lo, v_lo, U, V;
 };
 
-// Host checks, then the grid check, the column pass and the runs, with the call's one status read-back in between.
-int prepare(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
-            const dmnerf_placement* p, const char* who, Prepared& out, cudaStream_t stream) {
+enum { PLACED = 0, NO_POINTS = 1, TOP_OUT = 2 };   // dmnerf_placement_maps' status per base
+
+// The host checks of every placement call, before any launch.
+int check(const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
+          const dmnerf_placement* p, const char* who, Prepared& q) {
   DMN_CHECK(occ && labels && T16 && ext3 && p, "%s: NULL argument", who);
   DMN_CHECK(dim >= 2 && dim <= PLACE_MAX_DIM, "%s: dim %d out of range [2, %d]", who, dim, PLACE_MAX_DIM);
   if (sweep_grid_check(T16, ext3, dim, level, who)) return 1;
@@ -353,56 +387,117 @@ int prepare(PlaceState& s, const float* occ, const int16_t* labels, int dim, flo
   DMN_CHECK(p->axis >= 0 && p->axis <= 2, "%s: down axis %d is not 0, 1 or 2", who, p->axis);
   DMN_CHECK(p->sign == 1 || p->sign == -1, "%s: the sign of down along its axis must be +1 or -1, got %d", who, p->sign);
   DMN_CHECK(p->lift >= 0 && p->lift <= dim - 1, "%s: lift %d takes the object out of the grid [0, %d]", who, p->lift, dim - 1);
-  Placed m;
+  Placed& m = q.m;
   if (piece_region(p->piece, p->label, m.piece, who, 0)) return 1;
   for (int k = 0; k < 4; ++k) m.obstacles.w[k] = p->obstacles[k];
   m.label = p->label;
   m.rest_drop = p->rest_drop ? 1 : 0;
   const int64_t d = dim, stride[3] = {d * d, d, 1};
   const int h1 = p->axis == 0 ? 1 : 0, h2 = p->axis == 2 ? 1 : 2;
-  Frame& f = out.f;
+  Frame& f = q.f;
   f.s1 = stride[h1];
   f.s2 = stride[h2];
   f.sa = stride[p->axis];
   f.dim = dim;
   f.flip = p->sign == 1 ? 1 : 0;
   f.height_fast = p->axis == 2 ? 1 : 0;
-  const int64_t n = d * d * d, n_cols = d * d;
-  uint8_t* object;
-  int32_t *counts, *offsets;
-  if (s.table.get((size_t)n, &out.table) || s.object.get((size_t)n, &object) || s.counts.get((size_t)n_cols, &counts) ||
-      s.offsets.get((size_t)n_cols, &offsets) || s.status.get(1, &out.st_dev))
+  q.g = make_xform(T16, ext3, dim);
+  q.occ = occ;
+  q.labels = labels;
+  q.level = level;
+  q.lift = p->lift;
+  return 0;
+}
+
+// base (row-major 3x4) and the source box B of a moved placement as the edit move the shared checks take: finite, det > 0, B
+// inside the grid and not inverted (the empty box: no point), the piece applying to the label.
+int base_move(const dmnerf_placement* p, const double* base12, const int32_t* box6, const double* T16, const double* ext3, int dim,
+              EditMove& e, const char* who, int i) {
+  dmnerf_edit_move d;
+  memset(&d, 0, sizeof(d));
+  d.label = p->label;
+  d.rest_drop = p->rest_drop;
+  memcpy(d.trans, base12, sizeof(d.trans));
+  memcpy(d.box, box6, sizeof(d.box));
+  d.piece = p->piece;
+  return edit_move_from_abi(d, T16, ext3, dim, DMNERF_MAX_INS, e, who, i);
+}
+
+// The buffers, the grid check and the column pass: the column table, and the bytes of the unmoved object when `unmoved`.
+int columns(PlaceState& s, Prepared& q, bool unmoved, cudaStream_t stream) {
+  const int64_t d = q.f.dim, n = d * d * d, n_cols = d * d;
+  if (s.table.get((size_t)n, &q.table) || s.object.get((size_t)n, &q.object) || s.counts.get((size_t)n_cols, &q.counts) ||
+      s.offsets.get((size_t)n_cols, &q.offsets) || s.status.get(1, &q.st_dev))
     return 2;
   Status init{};
   for (int a = 0; a < 3; ++a) {
     init.box[2 * a] = INT_MAX;
     init.box[2 * a + 1] = -1;
   }
-  DMN_CUDA(cudaMemcpyAsync(out.st_dev, &init, sizeof(init), cudaMemcpyHostToDevice, stream));
-  if (launch_grid_check(occ, labels, n, DMNERF_MAX_INS + 1, &out.st_dev->bad, stream)) return 2;
-  place_column_kernel<<<(unsigned)((n_cols + TILE - 1) / TILE), CP_WARPS * 32, 0, stream>>>(f, make_xform(T16, ext3, dim), m, occ, labels,
-                                                                                             level, out.table, object);
+  DMN_CUDA(cudaMemcpyAsync(q.st_dev, &init, sizeof(init), cudaMemcpyHostToDevice, stream));
+  if (launch_grid_check(q.occ, q.labels, n, DMNERF_MAX_INS + 1, &q.st_dev->bad, stream)) return 2;
+  const unsigned blocks = (unsigned)((n_cols + TILE - 1) / TILE);
+  if (unmoved)
+    place_column_kernel<true><<<blocks, CP_WARPS * 32, 0, stream>>>(q.f, q.g, q.m, q.occ, q.labels, q.level, q.table, q.object);
+  else
+    place_column_kernel<false><<<blocks, CP_WARPS * 32, 0, stream>>>(q.f, q.g, q.m, q.occ, q.labels, q.level, q.table, nullptr);
   DMN_LAUNCH_OK();
+  return 0;
+}
+
+// The object's bytes when it is moved by `base` (NULL: as the column pass wrote them), its runs and the status read-back, after
+// which *why says whether it can be placed (PLACED) or why not.  The grid check's flags fail the call.
+int object_runs(PlaceState& s, Prepared& q, const EditMove* base, bool first, const char* who, int* why, cudaStream_t stream) {
+  const int64_t d = q.f.dim, n = d * d * d, n_cols = d * d;
+  if (!first) {                                                  // the grid check's flags were read with the first base
+    Status init{};
+    for (int a = 0; a < 3; ++a) {
+      init.box[2 * a] = INT_MAX;
+      init.box[2 * a + 1] = -1;
+    }
+    DMN_CUDA(cudaMemcpyAsync(q.st_dev, &init, sizeof(init), cudaMemcpyHostToDevice, stream));
+  }
+  if (base) {
+    place_moved_kernel<<<(unsigned)((n + MV_THREADS - 1) / MV_THREADS), MV_THREADS, 0, stream>>>(q.f, q.g, *base, q.occ, q.labels,
+                                                                                                 q.level, q.object);
+    DMN_LAUNCH_OK();
+  }
   const unsigned col_blocks = (unsigned)((n_cols + RUN_WARPS - 1) / RUN_WARPS);
-  place_run_count_kernel<<<col_blocks, RUN_WARPS * 32, 0, stream>>>(dim, object, counts, out.st_dev);
+  place_run_count_kernel<<<col_blocks, RUN_WARPS * 32, 0, stream>>>(q.f.dim, q.object, q.counts, q.st_dev);
   DMN_LAUNCH_OK();
   size_t tmp_bytes = 0;
-  DMN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts, offsets, (int)n_cols, stream));
+  DMN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, q.counts, q.offsets, (int)n_cols, stream));
   char* tmp;
   if (s.temp.get(tmp_bytes, &tmp)) return 2;
-  DMN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, counts, offsets, (int)n_cols, stream));
-  if (const int rc = read_checked(out.st_dev, &out.st, sizeof(Status), DMNERF_MAX_INS, who, stream)) return rc;
-  const Status& st = out.st;
-  DMN_CHECK(st.points > 0, "%s: label %d has no solid points%s", who, p->label, m.piece.bits ? " in its piece" : "");
-  DMN_CHECK(st.box[5] + p->lift <= dim - 1, "%s: lift %d takes the object's top (height %d) out of the grid [0, %d]", who, p->lift,
-            st.box[5], dim - 1);
-  if (s.runs.get((size_t)st.runs, &out.runs)) return 2;
-  place_run_write_kernel<<<col_blocks, RUN_WARPS * 32, 0, stream>>>(dim, object, counts, offsets, out.runs);
+  DMN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, q.counts, q.offsets, (int)n_cols, stream));
+  if (const int rc = read_checked(q.st_dev, &q.st, sizeof(Status), DMNERF_MAX_INS, who, stream)) return rc;
+  const Status& st = q.st;
+  *why = st.points == 0 ? NO_POINTS : (st.box[5] + q.lift > q.f.dim - 1 ? TOP_OUT : PLACED);
+  if (*why != PLACED) return 0;
+  if (s.runs.get((size_t)st.runs, &q.runs)) return 2;
+  place_run_write_kernel<<<col_blocks, RUN_WARPS * 32, 0, stream>>>(q.f.dim, q.object, q.counts, q.offsets, q.runs);
   DMN_LAUNCH_OK();
-  out.u_lo = -st.box[0];
-  out.v_lo = -st.box[2];
-  out.U = dim - (st.box[1] - st.box[0]);
-  out.V = dim - (st.box[3] - st.box[2]);
+  q.u_lo = -st.box[0];
+  q.v_lo = -st.box[2];
+  q.U = q.f.dim - (st.box[1] - st.box[0]);
+  q.V = q.f.dim - (st.box[3] - st.box[2]);
+  return 0;
+}
+
+// A placement that cannot be made fails a one-object call with its reason.
+int unplaced(const Prepared& q, int why, bool moved, const char* who) {
+  DMN_CHECK(why != NO_POINTS, "%s: label %d has no solid points%s", who, q.m.label,
+            moved ? " after the move" : (q.m.piece.bits ? " in its piece" : ""));
+  DMN_CHECK(why != TOP_OUT, "%s: lift %d takes the object's top (height %d) out of the grid [0, %d]", who, q.lift, q.st.box[5],
+            q.f.dim - 1);
+  return 0;
+}
+
+int launch_map(const Prepared& q, int32_t* drop, int32_t* contacts, int16_t* support, cudaStream_t st) {
+  const int64_t offsets = (int64_t)q.U * q.V;
+  place_map_kernel<<<(unsigned)((offsets + MAP_WARPS - 1) / MAP_WARPS), MAP_WARPS * 32, 0, st>>>(
+      q.f, q.table, q.labels, q.runs, (int64_t)q.st.runs, q.u_lo, q.v_lo, q.U, q.V, q.lift, drop, contacts, support);
+  DMN_LAUNCH_OK();
   return 0;
 }
 
@@ -419,39 +514,15 @@ void fill_info(const Prepared& q, dmnerf_placement_info* info) {
   for (int a = 0; a < 3; ++a) info->sum[a] = (int64_t)q.st.sum[a];
 }
 
-}  // namespace
-
-int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
-                  const dmnerf_placement* p, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
-                  cudaStream_t st) {
-  const char* who = "placement_map";
-  DMN_CHECK(drop && contacts && support && info, "%s: NULL argument", who);
-  memset(info, 0, sizeof(*info));
-  Prepared q;
-  if (const int rc = prepare(s, occ, labels, dim, level, T16, ext3, p, who, q, st)) return rc;
-  const int64_t offsets = (int64_t)q.U * q.V;
-  place_map_kernel<<<(unsigned)((offsets + MAP_WARPS - 1) / MAP_WARPS), MAP_WARPS * 32, 0, st>>>(
-      q.f, q.table, labels, q.runs, (int64_t)q.st.runs, q.u_lo, q.v_lo, q.U, q.V, p->lift, drop, contacts, support);
-  DMN_LAUNCH_OK();
-  fill_info(q, info);
-  return 0;
-}
-
-int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16,
-                       const double* ext3, const dmnerf_placement* p, int u, int v, int32_t* cells_host, int64_t max_cells,
-                       int64_t* n_cells_host, int32_t* drop_host, cudaStream_t st) {
-  const char* who = "placement_contacts";
-  DMN_CHECK(n_cells_host && drop_host && max_cells >= 0 && (max_cells == 0 || cells_host), "%s: bad output arguments", who);
-  *n_cells_host = 0;
-  *drop_host = -1;
-  Prepared q;
-  if (const int rc = prepare(s, occ, labels, dim, level, T16, ext3, p, who, q, st)) return rc;
+// The support cells of offset (u, v) of a prepared object, read back to the host.
+int contacts_at(PlaceState& s, const Prepared& q, int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                int32_t* drop_host, const char* who, cudaStream_t st) {
   DMN_CHECK(u >= q.u_lo && u < q.u_lo + q.U && v >= q.v_lo && v < q.v_lo + q.V,
             "%s: offset (%d, %d) outside the offsets [%d, %d] x [%d, %d] that keep the object inside the grid", who, u, v, q.u_lo,
             q.u_lo + q.U - 1, q.v_lo, q.v_lo + q.V - 1);
   int32_t* cells;
   if (s.cells.get((size_t)3 * q.st.runs, &cells)) return 2;
-  place_contacts_kernel<<<1, CT_THREADS, 0, st>>>(q.f, q.table, labels, q.runs, (int64_t)q.st.runs, u, v, p->lift, q.st_dev, cells);
+  place_contacts_kernel<<<1, CT_THREADS, 0, st>>>(q.f, q.table, q.labels, q.runs, (int64_t)q.st.runs, u, v, q.lift, q.st_dev, cells);
   DMN_LAUNCH_OK();
   Status h;
   DMN_CUDA(cudaMemcpyAsync(&h, q.st_dev, sizeof(h), cudaMemcpyDeviceToHost, st));
@@ -464,6 +535,77 @@ int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, i
   *n_cells_host = h.n_cells;
   *drop_host = h.drop;
   return 0;
+}
+
+}  // namespace
+
+int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
+                  const dmnerf_placement* p, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
+                  cudaStream_t st) {
+  const char* who = "placement_map";
+  DMN_CHECK(drop && contacts && support && info, "%s: NULL argument", who);
+  memset(info, 0, sizeof(*info));
+  Prepared q;
+  int why;
+  if (check(occ, labels, dim, level, T16, ext3, p, who, q)) return 1;
+  if (const int rc = columns(s, q, true, st)) return rc;
+  if (const int rc = object_runs(s, q, nullptr, true, who, &why, st)) return rc;
+  if (unplaced(q, why, false, who)) return 1;
+  if (const int rc = launch_map(q, drop, contacts, support, st)) return rc;
+  fill_info(q, info);
+  return 0;
+}
+
+int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
+                   const dmnerf_placement* p, const double* bases_host, const int32_t* box_host, int n_bases, int32_t* drop,
+                   int32_t* contacts, int16_t* support, dmnerf_placement_info* info, int32_t* status, cudaStream_t st) {
+  const char* who = "placement_maps";
+  DMN_CHECK(drop && contacts && support && info && status, "%s: NULL argument", who);
+  DMN_CHECK(n_bases >= 1 && n_bases <= DMNERF_MAX_BASES, "%s: between 1 and %d bases are supported, got %d", who, DMNERF_MAX_BASES,
+            n_bases);
+  DMN_CHECK(bases_host && box_host, "%s: bases or box is NULL", who);
+  for (int i = 0; i < n_bases; ++i) {
+    memset(info + i, 0, sizeof(*info));
+    status[i] = NO_POINTS;
+  }
+  Prepared q;
+  if (check(occ, labels, dim, level, T16, ext3, p, who, q)) return 1;
+  std::vector<EditMove> e(n_bases);
+  for (int i = 0; i < n_bases; ++i)
+    if (base_move(p, bases_host + 12 * i, box_host, T16, ext3, dim, e[i], who, i)) return 1;
+  if (const int rc = columns(s, q, false, st)) return rc;
+  const int64_t plane = (int64_t)dim * dim;
+  for (int i = 0; i < n_bases; ++i) {
+    int why;
+    if (const int rc = object_runs(s, q, &e[i], i == 0, who, &why, st)) return rc;
+    status[i] = why;
+    if (why != PLACED) continue;
+    if (const int rc = launch_map(q, drop + i * plane, contacts + i * plane, support + i * plane, st)) return rc;
+    fill_info(q, info + i);
+  }
+  return 0;
+}
+
+int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16,
+                       const double* ext3, const dmnerf_placement* p, const double* base_host, const int32_t* box_host, int u, int v,
+                       int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host, int32_t* drop_host, cudaStream_t st) {
+  const bool moved = base_host != nullptr;
+  const char* who = moved ? "placement_contacts_moved" : "placement_contacts";
+  DMN_CHECK(n_cells_host && drop_host && max_cells >= 0 && (max_cells == 0 || cells_host), "%s: bad output arguments", who);
+  *n_cells_host = 0;
+  *drop_host = -1;
+  Prepared q;
+  EditMove e;
+  int why;
+  if (check(occ, labels, dim, level, T16, ext3, p, who, q)) return 1;
+  if (moved) {
+    DMN_CHECK(box_host, "%s: box is NULL", who);
+    if (base_move(p, base_host, box_host, T16, ext3, dim, e, who, 0)) return 1;
+  }
+  if (const int rc = columns(s, q, !moved, st)) return rc;
+  if (const int rc = object_runs(s, q, moved ? &e : nullptr, true, who, &why, st)) return rc;
+  if (unplaced(q, why, moved, who)) return 1;
+  return contacts_at(s, q, u, v, cells_host, max_cells, n_cells_host, drop_host, who, st);
 }
 
 }  // namespace dmnerf

@@ -596,10 +596,13 @@ def _check_point(x, what):
 
 
 def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=None, level=0.45, piece=None, rest="keep",
-                  obstacles=None):
+                  obstacles=None, base=None, box=None):
     """dmnerf_placement_map: object `label` (or its piece, with rest "keep" / "drop" as move_overlap) raised by `lift` voxels and
     lowered along the index axis closest to +-down (network frame, chosen as supports chooses it), at every horizontal offset
     that keeps it inside the grid of the labelled keep-all sweep occ / labels.  obstacles: the labels that count (default all).
+    base (a 4x4 move in the network frame, as move_overlap takes it) places the object as that move leaves it instead
+    (dmnerf_placement_maps; DESIGN.md, "Turned placements"): sampled from the grid through the source box `box` (default
+    edit_boxes' box, margin 2), its points carried outside the grid lost.
     Returns a dict:
       drop, support, contacts: device maps [U, V] (int32, int16, int32): the voxels it falls (-1: blocked where it is raised),
                       the obstacle label under most of its resting runs (-1: blocked, or resting on the grid's floor), and the
@@ -608,7 +611,39 @@ def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=Non
       axis, sign, horizontal: the down axis, +1 when +e_axis points down, and the two horizontal index axes (ascending);
       centre:         the object's exact centre of mass in index space (3 Fractions, axes i, j, k), from its runs;
       runs, points:   its vertical runs and its points;
+      base, box:      the move (4x4, None without one) and its source box (None without a base);
+      points_before:  the object's points before the move (points without a base): a difference is clipping or resampling;
     and what placement() needs to describe one offset."""
+    if base is None and box is not None:
+        raise ValueError("placement: box needs a base")
+    if base is not None:
+        base = _move_matrix(base, 0)
+    if box is not None:
+        box = _check_boxes([box], 1, occ.shape[0])[0]
+    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles)
+    if base is None:
+        info = _lib.PlacementInfo()
+        drop, contacts, support = (torch.empty(c["dim"] ** 2, dtype=t, device=occ.device) for t in (torch.int32, torch.int32, torch.int16))
+        _placement_library("dmnerf_placement_map", occ, _lib.ptr(occ), _lib.ptr(labels, torch.int16), c["dim"], c["level"],
+                           _lib.doubles(c["T"], 16), _lib.doubles(c["ext"], 3), C.byref(c["desc"]), _lib.ptr(drop, torch.int32),
+                           _lib.ptr(contacts, torch.int32), _lib.ptr(support, torch.int16), C.byref(info))
+        return _map_result(c, info, drop, contacts, support, None, None, int(info.points))
+    box = _placement_box(c, box)
+    m, status = _placement_maps(c, [base], box, _object_points(c))
+    if m[0] is None:
+        raise ValueError(_unplaced(c, status[0]))
+    return m[0]
+
+
+def _unplaced(c, status):
+    """Why dmnerf_placement_maps did not place a base (its status 1 or 2)."""
+    if status == 1:
+        return "placement: label %d has no solid points after the move" % c["label"]
+    return "placement: lift %d takes the moved object's top out of the grid [0, %d]" % (c["lift"], c["dim"] - 1)
+
+
+def _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles):
+    """The checked arguments of a placement call: grid, level, label, lift, down axis and the ABI placement."""
     from .manipulator import _piece_region, move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -630,20 +665,41 @@ def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=Non
     desc = _lib.Placement(piece=_piece_region(piece, label, MAX_LABELS - 1, occ.device), label=label, rest_drop=int(rest_drop),
                           axis=axis, sign=sign, lift=int(lift))
     desc.obstacles[:] = words
-    drop = torch.empty(dim * dim, dtype=torch.int32, device=occ.device)
-    contacts = torch.empty(dim * dim, dtype=torch.int32, device=occ.device)
-    support = torch.empty(dim * dim, dtype=torch.int16, device=occ.device)
-    info = _lib.PlacementInfo()
+    return {"occ": occ, "labels": labels, "T": T, "ext": ext, "level": level, "label": label, "lift": int(lift), "axis": axis,
+            "sign": sign, "dim": dim, "desc": desc, "piece": piece}
+
+
+def _placement_library(name, occ, *args):
     try:
-        get_context(occ.device).call("dmnerf_placement_map", get_context(occ.device).handle, _lib.ptr(occ),
-                                     _lib.ptr(labels, torch.int16), dim, level, _lib.doubles(T, 16), _lib.doubles(ext, 3),
-                                     C.byref(desc), _lib.ptr(drop, torch.int32), _lib.ptr(contacts, torch.int32),
-                                     _lib.ptr(support, torch.int16), C.byref(info))
+        get_context(occ.device).call(name, get_context(occ.device).handle, *args)
     except RuntimeError as e:
         if "(status 1)" in str(e):                     # the library rejected the input: a label without points, the lift, the grid
             raise ValueError(str(e)) from None
         raise
+
+
+def _placement_box(c, box):
+    """The source box of a moved placement: edit_boxes' (margin 2) unless one is given -> int [6]."""
+    if box is not None:
+        return box
+    return edit_boxes(c["occ"], c["labels"], [(c["label"], np.eye(4))], c["T"], c["ext"], c["level"], 2,
+                      None if c["piece"] is None else [c["piece"]])[0]
+
+
+def _object_mask(c):
+    mask = (c["labels"] == c["label"]) & (c["occ"] > c["level"])
+    if c["piece"] is not None:
+        mask &= _region_keeps(c["piece"], c["T"], c["dim"], c["ext"], c["occ"].device)
+    return mask
+
+
+def _object_points(c):
+    return int(_object_mask(c).sum())
+
+
+def _map_result(c, info, drop, contacts, support, base, box, points_before):
     U, V = int(info.offsets[0]), int(info.offsets[1])
+    axis, sign, dim = c["axis"], c["sign"], c["dim"]
     horizontal = [a for a in range(3) if a != axis]
     n = int(info.points)
     centre = [None] * 3
@@ -654,8 +710,29 @@ def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=Non
     return {"drop": drop[:U * V].view(U, V), "support": support[:U * V].view(U, V), "contacts": contacts[:U * V].view(U, V),
             "offset_lo": (int(info.offset_lo[0]), int(info.offset_lo[1])), "axis": axis, "sign": sign, "horizontal": horizontal,
             "centre": centre, "runs": int(info.runs), "points": n, "height": (int(info.height[0]), int(info.height[1])),
-            "lift": int(lift), "label": label, "dim": dim,
-            "_call": (occ, labels, T, ext, level, desc, piece)}
+            "lift": c["lift"], "label": c["label"], "dim": dim, "base": base, "box": None if box is None else tuple(int(x) for x in box),
+            "points_before": points_before,
+            "_call": (c["occ"], c["labels"], c["T"], c["ext"], c["level"], c["desc"], c["piece"])}
+
+
+def _placement_maps(c, bases, box, points_before):
+    """dmnerf_placement_maps for the checked bases (at most MAX_BASES) -> (one placement_map result per base, None where the
+    base leaves no point or its top out of the grid; the statuses)."""
+    n, dim = len(bases), c["dim"]
+    occ = c["occ"]
+    drop, contacts = (torch.empty((n, dim * dim), dtype=torch.int32, device=occ.device) for _ in range(2))
+    support = torch.empty((n, dim * dim), dtype=torch.int16, device=occ.device)
+    infos = (_lib.PlacementInfo * n)()
+    status = np.zeros(n, dtype=np.int32)
+    rows = np.ascontiguousarray([np.asarray(b, dtype=np.float64)[:3].reshape(-1) for b in bases])
+    _placement_library("dmnerf_placement_maps", occ, _lib.ptr(occ), _lib.ptr(c["labels"], torch.int16), dim, c["level"],
+                       _lib.doubles(c["T"], 16), _lib.doubles(c["ext"], 3), C.byref(c["desc"]),
+                       rows.ctypes.data_as(C.POINTER(C.c_double)), (C.c_int32 * 6)(*[int(x) for x in box]), n,
+                       _lib.ptr(drop, torch.int32), _lib.ptr(contacts, torch.int32), _lib.ptr(support, torch.int16), infos,
+                       status.ctypes.data_as(C.POINTER(C.c_int32)))
+    maps = [None if status[i] else _map_result(c, infos[i], drop[i], contacts[i], support[i], np.asarray(bases[i], dtype=np.float64),
+                                               box, points_before) for i in range(n)]
+    return maps, status.tolist()
 
 
 def placement_delta(m, u, v, drop):
@@ -699,11 +776,12 @@ def hull_contains(cells, num, den):
 def placement(m, u, v):
     """The placement of placement_map's result `m` at offset (u, v) (voxels; ValueError outside the map or where it is blocked):
       transformation: the 4x4 (nested list) that lands the object there, as rigid_rays, manipulate_frame, edited_sweep and
-                      move_overlap read it;
+                      move_overlap read it: base @ translate(-A delta) (base = I without one);
       offset, drop, support, supported (support >= 0);
-      contacts:       the support cells [(h1, h2, label below), ...] (dmnerf_placement_contacts), one per resting run;
+      contacts:       the support cells [(h1, h2, label below), ...] (dmnerf_placement_contacts, or _moved with a base), one per
+                      resting run;
       stable:         the object's centre of mass projects into the closed convex hull of the support cells (exact);
-      centre:         the placed centre of mass, network frame."""
+      centre:         the placed centre of mass A (c + delta) + b, network frame (c: the object's exact centre as m has it)."""
     u, v = int(u), int(v)
     (u0, v0), (U, V) = m["offset_lo"], tuple(m["drop"].shape)
     if not (u0 <= u < u0 + U and v0 <= v < v0 + V):
@@ -716,9 +794,13 @@ def placement(m, u, v):
     cells = np.zeros((max(n, 1), 3), dtype=np.int32)
     got, dr = C.c_int64(0), C.c_int32(0)
     ctx = get_context(occ.device)
-    ctx.call("dmnerf_placement_contacts", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), m["dim"], level,
-             _lib.doubles(T, 16), _lib.doubles(ext, 3), C.byref(desc), u, v, cells.ctypes.data_as(C.POINTER(C.c_int32)), n,
-             C.byref(got), C.byref(dr))
+    head = (ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), m["dim"], level, _lib.doubles(T, 16), _lib.doubles(ext, 3),
+            C.byref(desc))
+    tail = (u, v, cells.ctypes.data_as(C.POINTER(C.c_int32)), n, C.byref(got), C.byref(dr))
+    if m.get("base") is None:
+        ctx.call("dmnerf_placement_contacts", *head, *tail)
+    else:
+        ctx.call("dmnerf_placement_contacts_moved", *head, _lib.doubles(m["base"][:3], 12), (C.c_int32 * 6)(*m["box"]), *tail)
     if int(got.value) != n or int(dr.value) != drop:
         raise RuntimeError("placement: the grid changed since placement_map (offset (%d, %d): drop %d, %d resting runs; now %d, %d)"
                            % (u, v, drop, n, int(dr.value), int(got.value)))
@@ -729,51 +811,183 @@ def placement(m, u, v):
     delta = placement_delta(m, u, v, drop)
     A, b = grid_affine(T, m["dim"], ext)
     centre = A @ (np.array([float(c) for c in m["centre"]]) + np.asarray(delta, dtype=np.float64)) + b
-    return {"transformation": placement_transform(A, delta).tolist(), "offset": (u, v), "drop": drop, "support": support,
+    trans = placement_transform(A, delta)
+    if m.get("base") is not None:
+        trans = m["base"] @ trans
+    return {"transformation": trans.tolist(), "offset": (u, v), "drop": drop, "support": support,
             "supported": support >= 0, "contacts": [tuple(int(x) for x in c) for c in cells],
             "stable": hull_contains(cells[:, :2], num, den), "centre": centre, "delta": delta}
 
 
+def _turn_cos_sin(angle):
+    """cos and sin of `angle` degrees, exactly 0 and +-1 at multiples of 90 (np.cos(np.pi / 2) is not 0)."""
+    q, r = divmod(float(angle), 90.0)
+    if r == 0.0:
+        return ((1.0, 0.0), (0.0, 1.0), (-1.0, 0.0), (0.0, -1.0))[int(q) % 4]
+    t = np.radians(float(angle))
+    return float(np.cos(t)), float(np.sin(t))
+
+
+def turn_bases(scene_transform, dim, axis, centre, box, angles, extents=None):
+    """The moves that turn an object about the down index axis (DESIGN.md, "Turned placements"), one per angle (degrees) ->
+    [(angle, 4x4 base or None when the turned object does not fit the grid horizontally)].
+      axis:   the down index axis; the turn is right-handed about A[:, axis] / |A[:, axis]| (network frame);
+      centre: the object's exact centre in index space (3 numbers or Fractions); the pivot is the grid point nearest it;
+      box:    the object's solid index box (i_lo, i_hi, j_lo, j_hi, k_lo, k_hi).
+    The object turned by theta about the pivot P, then shifted by whole voxels so that the pivot's column is the grid's middle
+    column, lands at L(x) = R (x - P) + P + A s; its base is L^-1 = [R^T | P - R^T (P + A s)], as move_overlap reads a move.  A
+    turn does not fit when a horizontal corner of the box grown by half a voxel, carried by L, leaves [-0.5, dim - 0.5]."""
+    T = np.asarray(scene_transform, dtype=np.float64)
+    A, b = grid_affine(T, dim, extents)
+    n = A[:, axis] / np.linalg.norm(A[:, axis])
+    pivot = np.array([int(np.floor(Fraction(x) + Fraction(1, 2))) for x in centre], dtype=np.float64)
+    shift = np.zeros(3)
+    for a in range(3):
+        if a != axis:
+            shift[a] = (dim - 1) // 2 - pivot[a]
+    P, Ainv = A @ pivot + b, np.linalg.inv(A)
+    box = np.asarray(box, dtype=np.float64)
+    corners = np.array([[box[2 * a + ((k >> a) & 1)] + (0.5 if (k >> a) & 1 else -0.5) for a in range(3)] for k in range(8)])
+    cross = np.array([[0.0, -n[2], n[1]], [n[2], 0.0, -n[0]], [-n[1], n[0], 0.0]])
+    out = []
+    for angle in angles:
+        c, s = _turn_cos_sin(angle)
+        R = c * np.eye(3) + s * cross + (1.0 - c) * np.outer(n, n)
+        landed = ((corners @ A.T + b - P) @ R.T + P + A @ shift - b) @ Ainv.T
+        h = [a for a in range(3) if a != axis]
+        if (landed[:, h] < -0.5 - 1e-9).any() or (landed[:, h] > dim - 0.5 + 1e-9).any():
+            out.append((float(angle), None))
+            continue
+        base = np.eye(4)
+        base[:3, :3] = R.T
+        base[:3, 3] = P - R.T @ (P + A @ shift)
+        out.append((float(angle), base))
+    return out
+
+
+def _turn_angles(turns):
+    """place_object's turns -> [degrees]: K (an integer >= 1) gives 360 k / K, k = 0 .. K - 1; else a non-empty list of finite
+    numbers."""
+    if isinstance(turns, (bool, np.bool_)):
+        raise ValueError("placement: turns must be an integer >= 1 or a list of degrees, got %r" % (turns,))
+    if isinstance(turns, (int, np.integer)):
+        if int(turns) < 1:
+            raise ValueError("placement: turns must be an integer >= 1 or a list of degrees, got %r" % (turns,))
+        return [360.0 * k / int(turns) for k in range(int(turns))]
+    try:
+        angles = [float(x) for x in turns]
+    except (TypeError, ValueError):
+        raise ValueError("placement: turns must be an integer >= 1 or a list of degrees, got %r" % (turns,)) from None
+    if not angles or not np.isfinite(angles).all():
+        raise ValueError("placement: turns must be an integer >= 1 or a non-empty list of finite degrees, got %r" % (turns,))
+    return angles
+
+
 def place_object(occ, labels, scene_transform, label, down, near, on=None, stable=True, lift=0, max_tests=64, extents=None,
-                 level=0.45, piece=None, rest="keep", obstacles=None):
+                 level=0.45, piece=None, rest="keep", obstacles=None, turns=None):
     """The placement of object `label` (or its piece) closest to the network-frame point `near`: over placement_map's offsets
     that are not blocked and rest on an obstacle whose label is in `on` (default: any), ordered by the distance of the placed
     centre of mass from `near` across the down axis (ties: the lowest (u, v)), the first that is stable -- testing at most
-    max_tests of them -- or, with stable=False, the first.  Returns {"placement": placement() of it, or None; "reason": None, or
-    why there is none; "candidates": how many offsets qualified; "tested": stability tests run; "map": placement_map's result}."""
+    max_tests of them -- or, with stable=False, the first.  turns (DESIGN.md, "Turned placements"): None places the object as it
+    lies; an integer K also turns it about the down axis by 360 k / K degrees, a list by those degrees (turn_bases), every turn
+    mapped in batched calls; candidates of all turns are ordered by distance, then turn order, then (u, v).  Returns
+    {"placement": placement() of it, or None; "reason": None, or why there is none; "candidates": how many offsets qualified;
+    "tested": stability tests run; "map": the placement_map result it came from (without turns: the map); "turn": its angle
+    (None without turns); "maps": [(angle, map)] of the turns that were mapped; "unfit": the angles whose turned object does not
+    fit the grid; "unplaced": the angles whose turned object has no point or leaves the grid at this lift}."""
     near = _check_point(near, "near")
     if isinstance(max_tests, (bool, np.bool_)) or int(max_tests) != max_tests or int(max_tests) < 1:
         raise ValueError("placement: max_tests must be an integer >= 1, got %r" % (max_tests,))
     on = None if on is None else set(_labels(on, MAX_LABELS - 1, "placement"))
-    m = placement_map(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles)
-    drop, support = m["drop"].cpu().numpy(), m["support"].cpu().numpy()
-    ok = (drop >= 0) & (support >= 0)
-    if on is not None:
-        ok &= np.isin(support, sorted(on))
-    iu, iv = np.nonzero(ok)
-    out = {"placement": None, "reason": None, "candidates": int(iu.size), "tested": 0, "map": m}
-    if iu.size == 0:
+    angles = None if turns is None else _turn_angles(turns)
+    if turns is None:
+        m = placement_map(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles)
+        maps, unfit, unplaced = [(None, m)], [], []
+    else:
+        maps, unfit, unplaced = turned_placement_maps(occ, labels, scene_transform, label, down, angles, lift, extents, level, piece,
+                                                      rest, obstacles)
+    out = {"placement": None, "reason": None, "candidates": 0, "tested": 0, "map": maps[0][1] if turns is None else None,
+           "turn": None, "maps": [] if turns is None else maps, "unfit": unfit, "unplaced": unplaced}
+    rows = placement_candidates([m for _, m in maps], near, on)
+    if rows.shape[0] == 0:
         out["reason"] = "no offset rests on %s" % ("an obstacle" if on is None else "label(s) %s" % sorted(on))
+        if turns is not None and not maps:
+            out["reason"] = "no turn fits the grid" if not unplaced else "no turned object can be placed"
         return out
-    T, ext = m["_call"][2], m["_call"][3]
-    A, b = grid_affine(T, m["dim"], ext)
-    u, v = iu + m["offset_lo"][0], iv + m["offset_lo"][1]
-    c = np.array([float(x) for x in m["centre"]])
-    delta = np.zeros((iu.size, 3))
-    delta[:, m["horizontal"][0]], delta[:, m["horizontal"][1]] = u, v
-    delta[:, m["axis"]] = -m["sign"] * (m["lift"] - drop[iu, iv])
-    gap = (c[None, :] + delta) @ A.T + b - near[None, :]
-    axis_dir = A[:, m["axis"]] / np.linalg.norm(A[:, m["axis"]])
-    gap -= np.outer(gap @ axis_dir, axis_dir)
-    order = np.lexsort((v, u, np.linalg.norm(gap, axis=1)))
-    for k in order[:int(max_tests)]:
-        p = placement(m, u[k], v[k])
+    out["candidates"] = int(rows.shape[0])
+    for k in range(min(int(max_tests), rows.shape[0])):
+        angle, m = maps[int(rows[k, 1])]
+        p = placement(m, int(rows[k, 2]), int(rows[k, 3]))
         out["tested"] += 1
         if p["stable"] or not stable:
-            out["placement"] = p
+            out.update(placement=p, map=m, turn=angle)
             return out
-    out["reason"] = "none of the %d nearest of %d resting offsets is stable" % (min(int(max_tests), iu.size), iu.size)
+    out["reason"] = "none of the %d nearest of %d resting offsets is stable" % (min(int(max_tests), rows.shape[0]), rows.shape[0])
     return out
+
+
+def turned_placement_maps(occ, labels, scene_transform, label, down, turns, lift=0, extents=None, level=0.45, piece=None,
+                          rest="keep", obstacles=None):
+    """placement_map of the object turned about the down axis by each of `turns` (degrees, or an integer K: 360 k / K), the
+    turns built by turn_bases from the object's solid box and exact centre, mapped in dmnerf_placement_maps calls of at most
+    MAX_BASES bases, with edit_boxes' source box -> ([(angle, map)] of the turns mapped, the angles that do not fit the grid,
+    the angles whose turned object has no point or its top out of the grid)."""
+    angles = _turn_angles(turns)
+    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles)
+    points, box, centre = _object_extent(_object_mask(c))
+    if points == 0:
+        raise ValueError("placement: label %d has no solid points%s" % (c["label"], " in its piece" if piece is not None else ""))
+    fitted = turn_bases(c["T"], c["dim"], c["axis"], centre, box, angles, c["ext"])
+    unfit = [a for a, bs in fitted if bs is None]
+    fitted = [(a, bs) for a, bs in fitted if bs is not None]
+    src = _placement_box(c, None)
+    maps, unplaced = [], []
+    for k in range(0, len(fitted), _lib.MAX_BASES):
+        chunk = fitted[k:k + _lib.MAX_BASES]
+        got, _ = _placement_maps(c, [bs for _, bs in chunk], src, points)
+        maps += [(a, mk) for (a, _), mk in zip(chunk, got) if mk is not None]
+        unplaced += [a for (a, _), mk in zip(chunk, got) if mk is None]
+    return maps, unfit, unplaced
+
+
+def placement_candidates(maps, near, on=None):
+    """The resting offsets of placement_map results `maps` (one per turn, in turn order) that rest on an obstacle (whose label
+    is in `on`, when given), in place_object's order: by the distance of the placed centre of mass from the network-frame point
+    `near` across the down axis, then by turn, then by (u, v) -> float [n, 4] rows (distance, turn, u, v)."""
+    rows = [np.zeros((0, 4))]
+    for t, m in enumerate(maps):
+        drop, support = m["drop"].cpu().numpy(), m["support"].cpu().numpy()
+        ok = (drop >= 0) & (support >= 0)
+        if on is not None:
+            ok &= np.isin(support, sorted(on))
+        iu, iv = np.nonzero(ok)
+        T, ext = m["_call"][2], m["_call"][3]
+        A, b = grid_affine(T, m["dim"], ext)
+        u, v = iu + m["offset_lo"][0], iv + m["offset_lo"][1]
+        cm = np.array([float(x) for x in m["centre"]])
+        delta = np.zeros((iu.size, 3))
+        delta[:, m["horizontal"][0]], delta[:, m["horizontal"][1]] = u, v
+        delta[:, m["axis"]] = -m["sign"] * (m["lift"] - drop[iu, iv])
+        gap = (cm[None, :] + delta) @ A.T + b - np.asarray(near, dtype=np.float64)[None, :]
+        axis_dir = A[:, m["axis"]] / np.linalg.norm(A[:, m["axis"]])
+        gap -= np.outer(gap @ axis_dir, axis_dir)
+        rows.append(np.stack([np.linalg.norm(gap, axis=1), np.full(iu.size, t), u, v], 1))
+    rows = np.concatenate(rows)
+    return rows[np.lexsort((rows[:, 3], rows[:, 2], rows[:, 1], rows[:, 0]))]
+
+
+def _object_extent(mask):
+    """The points, solid index box (i_lo, i_hi, j_lo, j_hi, k_lo, k_hi) and exact centre (3 Fractions) of a bool grid's points."""
+    n = int(mask.sum())
+    if n == 0:
+        return 0, EMPTY_BOX, None
+    box, centre = [], []
+    for a in range(3):
+        per = mask.sum(dim=tuple(x for x in range(3) if x != a)).long()
+        idx = torch.nonzero(per).flatten()
+        box += [int(idx[0]), int(idx[-1])]
+        centre.append(Fraction(int((per * torch.arange(per.numel(), device=per.device)).sum()), n))
+    return n, tuple(box), centre
 
 
 def largest_component_grid(occ, labels, level, objects):

@@ -542,6 +542,37 @@ DMNERF_API int dmnerf_placement_contacts(dmnerf_ctx* ctx, const float* occ, cons
                                          int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
                                          int32_t* drop_host, void* stream);
 
+/* ---- turned placements (DESIGN.md, "Turned placements"; no counterpart in the original) ------------------------------------
+ * The placement of the object as a move `base` leaves it: base is a row-major 3x4 (fp64, network frame, as dmnerf_edit_move's
+ * trans) and box_host [6] (HOST int32) the source box B (as dmnerf_move_overlap's box).  The object is S_base = {p : src(p)} with
+ * src as dmnerf_move_overlap computes it: q = rint(A^-1 (t - b)) of t = fp32(base p) in B, labels[q] == label, occ[q] > level and
+ * the piece keeps t; points carried outside the grid are lost.  The obstacles, heights, runs, drop, contacts, support and info are
+ * dmnerf_placement_map's, taken over S_base; the obstacles are unchanged (the points the move vacates are the object's points as
+ * it lies).  The placement at offset (u, v) with drop d is the move base translate(-A delta), delta as for dmnerf_placement_map:
+ * the object lands at base^-1 x + A delta.  With base = I and the box of the label's solid points (grown by any margin), S_base
+ * is dmnerf_placement_map's S and the maps are equal bit for bit.  Rejected on the host, before any launch: everything
+ * dmnerf_placement_map rejects, a base that is not finite or has det <= 0, and a box outside the grid or inverted (the empty
+ * box (1, 0, 1, 0, 1, 0) is accepted and leaves no point).
+ * dmnerf_placement_maps: n_bases (in [1, DMNERF_MAX_BASES]) bases bases_host [n][12] in one call: the column table is built once,
+ *   then per base the moved object's bytes (one reused buffer), its runs and its map.  drop, contacts, support (DEVICE, each with
+ *   room for n * dim * dim entries): base i's [U_i][V_i] map starts at entry i * dim * dim.  status_host [n] (HOST int32) = 0
+ *   placed, 1 no points after the move, 2 the object's top out of the grid at this lift; an unplaced base leaves its maps
+ *   unwritten and its info_host [n] entry zero and does not fail the call.  The run buffers are sized from each base's point and
+ *   run counts, so the call reads the status back once per base (synchronises the stream n times).
+ * dmnerf_placement_contacts_moved: dmnerf_placement_contacts for the object as base_host [12] leaves it; fails when that base
+ *   leaves no point or its top out of the grid. */
+#define DMNERF_MAX_BASES 64
+DMNERF_API int dmnerf_placement_maps(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                     const double* transform_host, const double* extents_host, const dmnerf_placement* placement,
+                                     const double* bases_host /* [n][12] */, const int32_t* box_host /* [6] */, int n_bases,
+                                     int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info_host /* [n] */,
+                                     int32_t* status_host /* [n] */, void* stream);
+DMNERF_API int dmnerf_placement_contacts_moved(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                               const double* transform_host, const double* extents_host,
+                                               const dmnerf_placement* placement, const double* base_host /* [12] */,
+                                               const int32_t* box_host /* [6] */, int u, int v, int32_t* cells_host, int64_t max_cells,
+                                               int64_t* n_cells_host, int32_t* drop_host, void* stream);
+
 /* ---- connected components (DESIGN.md, "Connected components"; no counterpart in the original) --------------------------------
  * The solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order, p = (i dim + j) dim + k) split into components:
  * two solid points are adjacent when they are face neighbours (connectivity 6) or face, edge or corner neighbours (26), never

@@ -4,7 +4,7 @@
     python tools/find_objects.py CHECKPOINT.tar (--transform T [--extents X Y Z] | --poses POSES.npy --hwk H W K) [--trim 0]
                                  [--grid-dim 256] [--level 0.45] [--near 4 --far 15] [--out DIR]
                                  [--components {largest,split} [--connectivity {6,26}] [--min-voxels N]]
-                                 [--contacts [--down X Y Z]] [--placements L --down X Y Z [--lift N] --out DIR]
+                                 [--contacts [--down X Y Z]] [--placements L --down X Y Z [--lift N] [--turns K] --out DIR]
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict`.  The grid is either given (--transform: a 4x4 as
 .npy or 16 numbers of text, with --extents, default the original's 1.9 7 7) or found from the cameras (--poses: [N, 4, 4] or
@@ -20,7 +20,10 @@ point of b next to it along +axis, with their area.  --down (network frame) adds
 along the index axis closest to that direction, with the faces they share.  --placements L (DESIGN.md, "Object placement") writes
 DIR/placements_L.npz: the placement map of label L lowered along --down (raised by --lift voxels first) on the keep-all sweep --
 drop, support and contacts [U, V], offset_lo, axis, sign, horizontal, centre (index space), runs and points -- and names it in
-the JSON line's `placements`."""
+the JSON line's `placements`.  --turns K (DESIGN.md, "Turned placements") maps the object turned about down by 360 k / K degrees
+instead: the .npz then holds angles (those mapped, in turn order), unfit and unplaced (the angles that did not fit the grid or
+left no point), axis, sign, lift, points_before, and per mapped turn t drop_t, support_t, contacts_t, offset_lo_t, base_t,
+centre_t and points_t."""
 import argparse
 import json
 import os
@@ -57,6 +60,8 @@ def parse(argv=None):
                     help="with --contacts: the network-frame down direction; adds rests_on per object")
     ap.add_argument("--placements", type=int, default=None, metavar="L", help="write the placement map of label L (needs --down)")
     ap.add_argument("--lift", type=int, default=None, help="with --placements: voxels the object is raised by first (default 0)")
+    ap.add_argument("--turns", type=int, default=None, metavar="K",
+                    help="with --placements: also the maps of the object turned about down by 360 k / K degrees (default 1)")
     ap.add_argument("--device", default="cuda")
     a = ap.parse_args(argv)
     if a.down is not None and not (a.contacts or a.placements is not None):
@@ -68,8 +73,11 @@ def parse(argv=None):
             ap.error("--placements: label %d outside [0, 127]" % a.placements)
         if a.lift is not None and a.lift < 0:
             ap.error("--lift must be >= 0")
-    elif a.lift is not None:
-        ap.error("--lift needs --placements")
+        if a.turns is not None and a.turns < 1:
+            ap.error("--turns must be >= 1")
+        a.turns = a.turns or 1
+    elif a.lift is not None or a.turns is not None:
+        ap.error("--lift and --turns need --placements")
     if a.down is not None and not any(a.down):
         ap.error("--down must not be 0 0 0")
     if a.components is None and a.connectivity is not None:
@@ -128,17 +136,34 @@ def contacts_json(a, nf, T, ext, objects):
 def placements_npz(a, nf, T, ext):
     """--placements: placement_map of the label on the keep-all sweep, written to DIR/placements_L.npz -> its file name."""
     import torch
-    from dmnerf_b200.objects import object_mask, occupancy_objects, placement_map
+    from dmnerf_b200.objects import object_mask, occupancy_objects, placement_map, turned_placement_maps
     ins_num = int(nf.ins_linear.weight.shape[0]) - 1
     with torch.no_grad():
         occ, labels = occupancy_objects(nf, T, object_mask(ins_num, remove=[]), a.grid_dim, tuple(ext), a.near, a.far, a.N_importance,
                                         device=next(nf.parameters()).device)
-        m = placement_map(occ, labels, T, a.placements, a.down, a.lift or 0, tuple(ext), a.level)
+        if a.turns == 1:
+            m = placement_map(occ, labels, T, a.placements, a.down, a.lift or 0, tuple(ext), a.level)
+        else:
+            maps, unfit, unplaced = turned_placement_maps(occ, labels, T, a.placements, a.down, a.turns, a.lift or 0, tuple(ext),
+                                                          a.level)
     name = "placements_%d.npz" % a.placements
-    np.savez(os.path.join(a.out, name), drop=m["drop"].cpu().numpy(), support=m["support"].cpu().numpy(),
-             contacts=m["contacts"].cpu().numpy(), offset_lo=np.array(m["offset_lo"]), axis=m["axis"], sign=m["sign"],
-             horizontal=np.array(m["horizontal"]), centre=np.array([float(c) for c in m["centre"]]), runs=m["runs"],
-             points=m["points"], lift=m["lift"])
+    if a.turns == 1:
+        np.savez(os.path.join(a.out, name), drop=m["drop"].cpu().numpy(), support=m["support"].cpu().numpy(),
+                 contacts=m["contacts"].cpu().numpy(), offset_lo=np.array(m["offset_lo"]), axis=m["axis"], sign=m["sign"],
+                 horizontal=np.array(m["horizontal"]), centre=np.array([float(c) for c in m["centre"]]), runs=m["runs"],
+                 points=m["points"], lift=m["lift"])
+        return name
+    per_turn = {}
+    for t, (angle, m) in enumerate(maps):
+        per_turn.update({"drop_%d" % t: m["drop"].cpu().numpy(), "support_%d" % t: m["support"].cpu().numpy(),
+                         "contacts_%d" % t: m["contacts"].cpu().numpy(), "offset_lo_%d" % t: np.array(m["offset_lo"]),
+                         "base_%d" % t: m["base"], "centre_%d" % t: np.array([float(c) for c in m["centre"]]),
+                         "points_%d" % t: m["points"]})
+    first = maps[0][1] if maps else None
+    np.savez(os.path.join(a.out, name), angles=np.array([angle for angle, _ in maps], dtype=np.float64),
+             unfit=np.array(unfit, dtype=np.float64), unplaced=np.array(unplaced, dtype=np.float64),
+             axis=-1 if first is None else first["axis"], sign=0 if first is None else first["sign"], lift=a.lift or 0,
+             points_before=0 if first is None else first["points_before"], **per_turn)
     return name
 
 

@@ -3,7 +3,7 @@
 
     python tools/move_objects.py CHECKPOINT.tar --pose POSE.npy --hwk H W K (--move-label L | --move-piece ID)
            (--mode {translation,rotation,scale,multi} [--distance -0.25 --yaw 90 --scale 1.2]
-            | --place-at X Y Z --down X Y Z [--on L ...] [--lift N] [--any-stability]) [--rest keep|drop]
+            | --place-at X Y Z --down X Y Z [--on L ...] [--lift N] [--any-stability] [--turns K]) [--rest keep|drop]
            --transform T [--extents X Y Z] [--grid-dim 256] [--level 0.45] [--connectivity {6,26}] [--dilate 1] --out DIR
            [--near 4 --far 15 --N-samples 64 --N-importance 128 --N-test 4096] [--mesh [--min-cluster 400]]
            [--check] [--until-contact [--step S] [--tolerance N]]
@@ -36,7 +36,8 @@ axis closest to --down (network frame), after being raised by --lift voxels, at 
 of the offsets where it rests on an object (of a label among --on, when given), the one whose centre of mass lands nearest to
 the network-frame point --place-at across the down axis, and stands (its centre over the hull of its support; --any-stability:
 the nearest, standing or not), is rendered and meshed as --until-contact's is.  The record gains place {offset, drop, support,
-stable, contacts}."""
+stable, contacts}.  --turns K (DESIGN.md, "Turned placements") also turns the piece about down by 360 k / K degrees and picks the
+nearest placement over every turn that fits the grid; the record's place gains turn, the angle in degrees of the one chosen."""
 import argparse
 import json
 import os
@@ -67,6 +68,8 @@ def parse(argv=None):
     ap.add_argument("--on", type=int, nargs="+", default=None, metavar="L", help="--place-at: rest on one of these labels")
     ap.add_argument("--lift", type=int, default=None, help="--place-at: voxels the piece is raised by first (default 0)")
     ap.add_argument("--any-stability", action="store_true", help="--place-at: take the nearest resting offset, stable or not")
+    ap.add_argument("--turns", type=int, default=None, metavar="K",
+                    help="--place-at: also turn the piece about down by 360 k / K degrees, k = 0 .. K - 1 (default 1: unturned)")
     ap.add_argument("--rest", choices=("keep", "drop"), default="keep", help="the rest of the moved label: kept or removed")
     ap.add_argument("--transform", required=True, help="4x4 scene transform of the sweep grid (.npy or text)")
     ap.add_argument("--extents", type=float, nargs=3, default=[1.9, 7.0, 7.0], metavar=("X", "Y", "Z"))
@@ -97,12 +100,15 @@ def parse(argv=None):
             ap.error("--place-at needs --down X Y Z, not 0 0 0")
         if a.lift is not None and a.lift < 0:
             ap.error("--lift must be >= 0")
+        if a.turns is not None and a.turns < 1:
+            ap.error("--turns must be >= 1")
         a.lift = a.lift or 0
+        a.turns = a.turns or 1
     else:
         if a.mode is None:
             ap.error("give --mode or --place-at")
-        if a.down is not None or a.on is not None or a.lift is not None or a.any_stability:
-            ap.error("--down, --on, --lift and --any-stability need --place-at")
+        if a.down is not None or a.on is not None or a.lift is not None or a.any_stability or a.turns is not None:
+            ap.error("--down, --on, --lift, --any-stability and --turns need --place-at")
         a.distance = -0.25 if a.distance is None else a.distance
         a.yaw = 90.0 if a.yaw is None else a.yaw
         a.scale = 1.2 if a.scale is None else a.scale
@@ -170,12 +176,15 @@ def place_piece(a, occ, labels, T, ext, label, region):
     qualifies."""
     from dmnerf_b200.objects import place_object
     r = place_object(occ, labels, T, label, a.down, a.place_at, on=a.on, stable=not a.any_stability, lift=a.lift, extents=ext,
-                     level=a.level, piece=region, rest=a.rest)
+                     level=a.level, piece=region, rest=a.rest, turns=None if a.turns == 1 else a.turns)
     p = r["placement"]
     if p is None:
         raise SystemExit("move_objects: no placement: %s" % r["reason"])
-    return {"transformation": p["transformation"], "offset": list(p["offset"]), "drop": p["drop"], "support": p["support"],
-            "stable": p["stable"], "contacts": [list(c) for c in p["contacts"]]}
+    out = {"transformation": p["transformation"], "offset": list(p["offset"]), "drop": p["drop"], "support": p["support"],
+           "stable": p["stable"], "contacts": [list(c) for c in p["contacts"]]}
+    if a.turns != 1:
+        out["turn"] = r["turn"]
+    return out
 
 
 def main(argv=None):

@@ -10,7 +10,10 @@ level is the 99th percentile of the sweep's occupancy (about 1 % of the grid sol
 tools/collide_bench.py the label with the most points spans the grid and leaves one offset).  The placed label is the one with
 the most solid points; down is the network's -y, the grid's fastest index axis (k) for the
 identity rotation used here, the case where the column pass reads each column contiguously.  place_object aims at the grid's
-centre and tests at most 64 offsets for stability.  The calls are timed alternately (_harness.alternate, CUDA events, one
+centre and tests at most 64 offsets for stability.  The turned cases (DESIGN.md, "Turned placements") time, at lift 0, for the
+label with the most points and for its piece inside an index cube of side grid_dim / 4 around its centre (a small object with
+many offsets), placement_map against turned_placement_maps of 8 and of 36 turns and place_object(turns=8), with the 8-turn
+call's stage split (torch.profiler) and its number of column-pass launches.  The calls are timed alternately (_harness.alternate, CUDA events, one
 warm-up round); each ends in its read-back.  Nothing is written to disk."""
 import argparse
 import json
@@ -25,6 +28,7 @@ from dmnerf_b200.testing import make_models
 NEAR, FAR, N_IMPORTANCE, EXT = 4.0, 15.0, 128, (1.9, 7.0, 7.0)
 DOWN = (0.0, -1.0, 0.0)
 STAGES = {"column_table": ("grid_check_kernel", "place_column_kernel"),
+          "moved_object": ("place_moved_kernel",),
           "runs": ("place_run_count_kernel", "DeviceScan", "place_run_write_kernel"),
           "map": ("place_map_kernel",)}
 
@@ -33,21 +37,63 @@ def _stats(ms):
     return {"mean_ms": float(np.mean(ms)), "min_ms": float(np.min(ms)), "max_ms": float(np.max(ms))}
 
 
-def _stage_ms(fn):
-    """Device time per stage of one call of fn, from the kernel records of torch.profiler."""
+def _stage_ms(fn, launches=None):
+    """Device time per stage of one call of fn, from the kernel records of torch.profiler; launches (a dict) receives the
+    number of column-pass launches."""
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         fn()
         torch.cuda.synchronize()
     out = {k: 0.0 for k in STAGES}
+    columns = 0
     for e in prof.events():
         if e.device_type != torch.autograd.DeviceType.CUDA:
             continue
+        columns += "place_column_kernel" in e.name
         for k, names in STAGES.items():
             if any(n in e.name for n in names):
                 out[k] += e.device_time / 1e3
+    if launches is not None:
+        launches["column_pass"] = columns
     return out
+
+
+def _small_piece(occ, lab, T, dim, level, label):
+    """A small object with many offsets: the piece of `label` inside the index cube of side dim / 4 centred on the label's
+    centre (the Region of that cube, applying to the label)."""
+    _, _, centre = OB._object_extent((lab == label) & (occ > level))
+    lo = [min(max(int(c) - dim // 8, 0), dim - dim // 4) for c in centre]
+    cube = torch.zeros((dim,) * 3, dtype=torch.bool, device=occ.device)
+    cube[lo[0]:lo[0] + dim // 4, lo[1]:lo[1] + dim // 4, lo[2]:lo[2] + dim // 4] = True
+    return OB.region_from_mask(cube, T, EXT, applies=[label], outside="drop")
+
+
+def turned_cases(occ, lab, T, dim, level, label, near, reps, what, piece=None):
+    """The turned path for one object: placement_map against batched maps of 8 and 36 turns and place_object(turns=8)."""
+    angles8, angles36 = [45.0 * k for k in range(8)], [10.0 * k for k in range(36)]
+    case = {"label": label, "object": what, "level": level}
+    kw = dict(extents=EXT, level=level, piece=piece)
+    m = OB.placement_map(occ, lab, T, label, DOWN, 0, **kw)
+    variants = {
+        "placement_map": lambda: OB.placement_map(occ, lab, T, label, DOWN, 0, **kw),
+        "turns_8": lambda: OB.turned_placement_maps(occ, lab, T, label, DOWN, angles8, 0, **kw),
+        "turns_36": lambda: OB.turned_placement_maps(occ, lab, T, label, DOWN, angles36, 0, **kw),
+        "place_object_turns_8": lambda: OB.place_object(occ, lab, T, label, DOWN, near, turns=8, **kw),
+    }
+    ms = alternate(variants, reps)
+    launches = {}
+    stages = [_stage_ms(lambda: OB.turned_placement_maps(occ, lab, T, label, DOWN, angles8, 0, **kw), launches)
+              for _ in range(reps)]
+    maps, unfit, unplaced = OB.turned_placement_maps(occ, lab, T, label, DOWN, angles8, 0, **kw)
+    r = OB.place_object(occ, lab, T, label, DOWN, near, turns=8, **kw)
+    case.update({"points": m["points"], "runs": m["runs"], "offsets": int(m["drop"].numel()),
+                 "turns_8": {"mapped": len(maps), "unfit": unfit, "unplaced": unplaced,
+                             "offsets": [int(x["drop"].numel()) for _, x in maps], "column_pass_launches": launches["column_pass"]},
+                 "place_object_turns_8": {"candidates": r["candidates"], "tested": r["tested"], "turn": r["turn"]},
+                 **{k + "_ms": _stats(v) for k, v in ms.items()},
+                 **{"turns_8_stage_" + k + "_ms": _stats([s[k] for s in stages]) for k in STAGES}})
+    return case
 
 
 def main():
@@ -61,7 +107,7 @@ def main():
     T[:3, 3] = (0.1, -0.2, 0.3)
     A, b = OB.grid_affine(T, dim, EXT)
     near = A @ np.full(3, (dim - 1) / 2.0) + b
-    cases = []
+    cases, turned = [], []
     for ins_num in (13, 93):
         _, nf, _, _ = make_models(101, 202, ins_num, dev, trained_like=True)
         keep_all = OB.object_mask(ins_num, remove=[])
@@ -97,9 +143,14 @@ def main():
                              **{"stage_" + k + "_ms": _stats([s[k] for s in stages]) for k in STAGES}})
                 cases.append(case)
                 del m, r
+            turned.append(dict(turned_cases(occ, lab, T, dim, level, label, near, a.reps, "whole label"), ins_num=ins_num))
+            piece = _small_piece(occ, lab, T, dim, level, label)
+            turned.append(dict(turned_cases(occ, lab, T, dim, level, label, near, a.reps, "piece in a cube of side dim / 4", piece),
+                               ins_num=ins_num))
         del occ, lab
     name, smi, _ = gpu_identity(dev)
-    print(json.dumps({"metric": "placement device time", "grid_dim": dim, "reps": a.reps, "down": DOWN, "cases": cases, "gpu": smi,
+    print(json.dumps({"metric": "placement device time", "grid_dim": dim, "reps": a.reps, "down": DOWN, "cases": cases,
+                      "turned": turned, "gpu": smi,
                       "gpu_name": name,
                       "what": "keep-all labelled sweep, placement_map (stages: torch.profiler kernel times of one call each), "
                               "place_object (at most 64 stability tests); synthetic trained-like networks; CUDA events, "
