@@ -912,7 +912,7 @@ DMNERF_API int dmnerf_placement_contacts(dmnerf_ctx* ctx, const float* occ, cons
                                          int32_t* drop_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "placement_contacts: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_contacts(ctx->place, occ, labels, dim, level, transform_host, extents_host, placement, nullptr, nullptr, u, v,
+  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, nullptr, nullptr, u, v,
                             cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
 }
 
@@ -922,7 +922,7 @@ DMNERF_API int dmnerf_placement_maps(dmnerf_ctx* ctx, const float* occ, const in
                                      int16_t* support, dmnerf_placement_info* info_host, int32_t* status_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "placement_maps: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_maps(ctx->place, occ, labels, dim, level, transform_host, extents_host, placement, bases_host, box_host, n_bases,
+  return placement_maps(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, bases_host, box_host, n_bases,
                         drop, contacts, support, info_host, status_host, (cudaStream_t)stream);
 }
 
@@ -934,8 +934,42 @@ DMNERF_API int dmnerf_placement_contacts_moved(dmnerf_ctx* ctx, const float* occ
   DMN_CHECK(ctx != nullptr, "placement_contacts_moved: ctx is NULL");
   DMN_CHECK(base_host != nullptr, "placement_contacts_moved: base is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_contacts(ctx->place, occ, labels, dim, level, transform_host, extents_host, placement, base_host, box_host, u, v,
+  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, base_host, box_host, u, v,
                             cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
+}
+
+// ---- arranging objects (DESIGN.md, "Arranging objects") -------------------------------------------------------------------
+
+DMNERF_API int dmnerf_grid_edit(dmnerf_ctx* ctx, const float* src_occ, const int16_t* src_labels, int dim, float level,
+                                const double* transform_host, const double* extents_host, const dmnerf_edit_move* moves_host, int n_moves,
+                                float* occ, int16_t* labels, int64_t* landed_host, int64_t* overwritten_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "grid_edit: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, n_moves, occ, labels,
+                   landed_host, overwritten_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_placement_maps_in_scene(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                              const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                              const double* extents_host, const dmnerf_placement* placement, const double* bases_host,
+                                              const int32_t* box_host, int n_bases, int32_t* drop, int32_t* contacts, int16_t* support,
+                                              dmnerf_placement_info* info_host, int32_t* status_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_maps_in_scene: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_maps(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, bases_host,
+                        box_host, n_bases, drop, contacts, support, info_host, status_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_placement_contacts_in_scene(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                                  const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                                  const double* extents_host, const dmnerf_placement* placement, const double* base_host,
+                                                  const int32_t* box_host, int u, int v, int32_t* cells_host, int64_t max_cells,
+                                                  int64_t* n_cells_host, int32_t* drop_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_contacts_in_scene: ctx is NULL");
+  DMN_CHECK(base_host != nullptr, "placement_contacts_in_scene: base is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_contacts(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement,
+                            base_host, box_host, u, v, cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
 }
 
 // ---- connected components (DESIGN.md, "Connected components") -------------------------------------------------------------

@@ -24,6 +24,7 @@ constexpr int OV_BLOCK_POINTS = OV_THREADS * OV_POINTS;
 constexpr int N_COUNTERS = DMNERF_MAX_INS + 2;   // overlap per label 0 .. 127, then landed
 constexpr int LANDED = DMNERF_MAX_INS + 1;
 constexpr int CT_THREADS = 512;
+constexpr int GE_THREADS = 256;
 constexpr unsigned FULL = 0xffffffffu;
 
 enum { BAD_NAN = 1, BAD_LABEL = 2 };
@@ -135,6 +136,50 @@ __global__ void __launch_bounds__(OV_THREADS) move_overlap_kernel(const GridXfor
     const uint32_t v = (&hist[0][0])[q];
     if (v) atomicAdd(counts + (int64_t)run.first * N_COUNTERS + q, (unsigned long long)v);
   }
+}
+
+// One move of the grid-only edit (DESIGN.md, "Arranging objects"), one thread per grid point p of the state: edit_rule with the
+// source grid at the target's nearest index q.  counts [129]: overwritten per label, then landed -- the takes whose target is
+// solid, and those of them that land on a solid state point the move does not vacate, by its label.  The state point is read
+// before it is written and no thread reads another's point, so the launch order of the points does not matter.
+__global__ void __launch_bounds__(GE_THREADS) grid_edit_kernel(const GridXform g, const EditMove e, const float* __restrict__ src_occ,
+                                                               const int16_t* __restrict__ src_labels, float level,
+                                                               float* __restrict__ occ, int16_t* __restrict__ labels,
+                                                               unsigned long long* __restrict__ counts) {
+  __shared__ uint32_t hist[N_COUNTERS];
+  for (int k = threadIdx.x; k < N_COUNTERS; k += GE_THREADS) hist[k] = 0;
+  __syncthreads();
+  const int64_t d = g.dim, p = (int64_t)blockIdx.x * GE_THREADS + threadIdx.x;
+  bool landed = false;
+  if (p < d * d * d) {
+    const float o = occ[p];
+    const int l = labels[p];
+    float x[3], t[3];
+    double q[3];
+    sweep_point(g, p, x);
+    const bool in_box = edit_target(e.trans, e.inv, e.b, e.lo, e.hi, !e.empty, x, t, q);
+    auto here = [&] { return e.piece.bits == nullptr || !region_drops(e.piece, e.label, x[0], x[1], x[2]); };
+    edit_rule(
+        e, in_box,
+        [&](int& lt, float& ot) {
+          const int64_t qi = ((int64_t)q[0] * d + (int64_t)q[1]) * d + (int64_t)q[2];
+          lt = src_labels[qi];
+          ot = src_occ[qi];
+        },
+        o, l, level, [&] { return region_drops(e.piece, e.label, t[0], t[1], t[2]); }, [&](bool& b) { b = here(); },
+        [&](float ot) {
+          occ[p] = ot;
+          labels[p] = (int16_t)e.label;
+          landed = ot > level;
+          if (landed && o > level && !(l == e.label && (e.rest_drop || here()))) atomicAdd(&hist[l], 1u);
+        },
+        [&] { occ[p] = 0.0f; });
+  }
+  const unsigned n = __ballot_sync(FULL, landed);
+  if ((threadIdx.x & 31) == 0 && n) atomicAdd(&hist[LANDED], (uint32_t)__popc(n));
+  __syncthreads();
+  for (int k = threadIdx.x; k < N_COUNTERS; k += GE_THREADS)
+    if (hist[k]) atomicAdd(counts + k, (unsigned long long)hist[k]);
 }
 
 // shared: faces [3][n_labels][n_labels]; a block walks points p grid-stride and counts the +a neighbours of its solid points
@@ -361,6 +406,53 @@ int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, 
   std::vector<char> h(out_bytes);
   if (const int rc = read_back(out, h, n_labels - 1, who, st)) return rc;
   memcpy(faces_host, h.data() + 16, nf * sizeof(int64_t));
+  return 0;
+}
+
+int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels, int dim, float level, const double* T16,
+              const double* ext3, const dmnerf_edit_move* moves_host, int n, float* occ, int16_t* labels, int64_t* landed_host,
+              int64_t* overwritten_host, cudaStream_t st) {
+  const char* who = "grid_edit";
+  DMN_CHECK(src_occ && src_labels && occ && labels && T16 && ext3 && landed_host && overwritten_host, "%s: NULL argument", who);
+  DMN_CHECK(n >= 1 && n <= DMNERF_MAX_MOVES, "%s: between 1 and %d moves are supported, got %d", who, DMNERF_MAX_MOVES, n);
+  DMN_CHECK(moves_host, "%s: moves is NULL", who);
+  if (sweep_grid_check(T16, ext3, dim, level, who)) return 1;
+  const int64_t npts = (int64_t)dim * dim * dim;
+  // the state is written while the source is read at other points: they must not share memory
+  auto apart = [](const void* a, size_t na, const void* b, size_t nb) {
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x + na <= y || y + nb <= x;
+  };
+  const size_t fo = (size_t)npts * sizeof(float), lb = (size_t)npts * sizeof(int16_t);
+  DMN_CHECK(apart(src_occ, fo, occ, fo) && apart(src_occ, fo, labels, lb) && apart(src_labels, lb, occ, fo) &&
+                apart(src_labels, lb, labels, lb),
+            "%s: the source and state grids overlap in memory (the state must be a separate copy)", who);
+  std::vector<EditMove> mv(n);
+  for (int i = 0; i < n; ++i)
+    if (edit_move_from_abi(moves_host[i], T16, ext3, dim, DMNERF_MAX_INS, mv[i], who, i)) return 1;
+  const size_t out_bytes = 16 + (size_t)n * N_COUNTERS * sizeof(unsigned long long);
+  char* out;
+  if (s.out.get(out_bytes, &out)) return 2;
+  DMN_CUDA(cudaMemsetAsync(out, 0, out_bytes, st));
+  int* bad = reinterpret_cast<int*>(out);
+  if (launch_grid_check(src_occ, src_labels, npts, DMNERF_MAX_INS + 1, bad, st) ||
+      launch_grid_check(occ, labels, npts, DMNERF_MAX_INS + 1, bad, st))
+    return 2;
+  std::vector<char> h(out_bytes);
+  if (const int rc = read_checked(out, h.data(), 16, DMNERF_MAX_INS, who, st)) return rc;   // a bad grid writes nothing
+  const GridXform g = make_xform(T16, ext3, dim);
+  auto* counts = reinterpret_cast<unsigned long long*>(out + 16);
+  for (int i = 0; i < n; ++i) {
+    grid_edit_kernel<<<(unsigned)((npts + GE_THREADS - 1) / GE_THREADS), GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ,
+                                                                                           labels, counts + (size_t)i * N_COUNTERS);
+    DMN_LAUNCH_OK();
+  }
+  if (const int rc = read_back(out, h, DMNERF_MAX_INS, who, st)) return rc;
+  for (int i = 0; i < n; ++i) {
+    const char* row = h.data() + 16 + (size_t)i * N_COUNTERS * sizeof(unsigned long long);
+    memcpy(overwritten_host + (size_t)i * (DMNERF_MAX_INS + 1), row, (DMNERF_MAX_INS + 1) * sizeof(int64_t));
+    memcpy(landed_host + i, row + LANDED * sizeof(int64_t), sizeof(int64_t));
+  }
   return 0;
 }
 

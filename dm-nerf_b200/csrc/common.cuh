@@ -336,6 +336,12 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
                  cudaStream_t st);
 int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels, int64_t* faces_host,
                     cudaStream_t st);
+// The grid-only edit (DESIGN.md, "Arranging objects"): the moves applied in order to the state occ / labels, each target read
+// from the source grid at its nearest index; landed [n] and overwritten [n][128] per move.  Two read-backs: the grid checks of
+// both grids before the first edit, the counts at the end.
+int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels, int dim, float level, const double* T16,
+              const double* ext3, const dmnerf_edit_move* moves_host, int n, float* occ, int16_t* labels, int64_t* landed_host,
+              int64_t* overwritten_host, cudaStream_t st);
 // The grid check of both: flags in *bad (device) for NaN in occ and labels outside [0, n_labels - 1].  read_checked copies
 // `bytes` from dev to host and synchronises; the buffer starts with that flag word, and a set flag fails the call.
 int launch_grid_check(const float* occ, const int16_t* labels, int64_t n, int n_labels, int* bad, cudaStream_t st);
@@ -351,14 +357,19 @@ int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int di
                   const dmnerf_placement* p, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
                   cudaStream_t st);
 // The same for the object as each move of bases_host [n][12] leaves it (DESIGN.md, "Turned placements"): one column table, then
-// per base the moved object's bytes, runs and map; status [n] says which were placed.
-int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
-                   const dmnerf_placement* p, const double* bases_host, const int32_t* box_host, int n_bases, int32_t* drop,
-                   int32_t* contacts, int16_t* support, dmnerf_placement_info* info, int32_t* status, cudaStream_t st);
-// base_host NULL: the object as it lies (dmnerf_placement_contacts); otherwise as base_host [12] and box_host [6] leave it.
-int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16,
-                       const double* ext3, const dmnerf_placement* p, const double* base_host, const int32_t* box_host, int u, int v,
-                       int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host, int32_t* drop_host, cudaStream_t st);
+// per base the moved object's bytes, runs and map; status [n] says which were placed.  The object is sampled from occ / labels,
+// the obstacles and support labels come from the scene scene_occ / scene_labels (DESIGN.md, "Arranging objects"); passing the
+// same grid twice is dmnerf_placement_maps.
+int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels, int dim,
+                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, const double* bases_host,
+                   const int32_t* box_host, int n_bases, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
+                   int32_t* status, cudaStream_t st);
+// base_host NULL: the object as it lies (dmnerf_placement_contacts; the scene must be the object's grid); otherwise as base_host
+// [12] and box_host [6] leave it, sampled from occ / labels, in the scene scene_occ / scene_labels.
+int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels,
+                       int dim, float level, const double* T16, const double* ext3, const dmnerf_placement* p, const double* base_host,
+                       const int32_t* box_host, int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                       int32_t* drop_host, cudaStream_t st);
 
 // Connected components (components.cu): the solid points of a labelled grid split into canonically numbered components.
 // Per-context device buffers: the status words a call reads back, the chunk counts and the scan's storage.

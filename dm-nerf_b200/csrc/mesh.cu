@@ -722,27 +722,25 @@ __global__ void edit_apply_kernel(const GridXform g, const EditMove m, int64_t b
   const int64_t p = begin + i;
   const float o = occ[p];
   const int l = labels[p];
-  const bool has_piece = m.piece.bits != nullptr;
-  if (flag[i]) {
-    const float* r = raw + (int64_t)pos[i] * c;
-    const int lt = argmax_sigmoid(r + 4, c - 4);
-    const float ot = occupancy_of(r[3], voxel);
-    if (lt == m.label && (ot > level || o <= level) &&
-        (!has_piece || !region_drops(m.piece, m.label, tgt[3 * i], tgt[3 * i + 1], tgt[3 * i + 2]))) {
-      occ[p] = ot;
-      labels[p] = (int16_t)m.label;
-      return;
-    }
-  }
-  if (l == m.label && o > level) {
-    bool in_piece = true;
-    if (has_piece) {
-      float q[3];
-      sweep_point(g, p, q);
-      in_piece = !region_drops(m.piece, m.label, q[0], q[1], q[2]);
-    }
-    if (in_piece || m.rest_drop) occ[p] = 0.0f;
-  }
+  edit_rule(
+      m, flag[i] != 0,
+      [&](int& lt, float& ot) {
+        const float* r = raw + (int64_t)pos[i] * c;
+        lt = argmax_sigmoid(r + 4, c - 4);
+        ot = occupancy_of(r[3], voxel);
+      },
+      o, l, level,
+      [&] { return region_drops(m.piece, m.label, tgt[3 * i], tgt[3 * i + 1], tgt[3 * i + 2]); },
+      [&](bool& in_piece) {
+        float q[3];
+        sweep_point(g, p, q);
+        in_piece = !region_drops(m.piece, m.label, q[0], q[1], q[2]);
+      },
+      [&](float ot) {
+        occ[p] = ot;
+        labels[p] = (int16_t)m.label;
+      },
+      [&] { occ[p] = 0.0f; });
 }
 
 int edit_targets(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,

@@ -357,13 +357,18 @@ __global__ void __launch_bounds__(CT_THREADS) place_contacts_kernel(const Frame 
   }
 }
 
-// The checked grid and placement of a call, its buffers, and after object_runs the object's status, runs and offset range.
+// The checked grids and placement of a call, its buffers, and after object_runs the object's status, runs and offset range.
+// occ / labels: the scene, which gives the obstacles, the vacated points and the labels under the object (the column pass, the
+// map and the contacts); src_occ / src_labels: the grid a moved object is sampled from (place_moved_kernel).  They are the same
+// grid except in a placement in an edited scene (DESIGN.md, "Arranging objects").
 struct Prepared {
   Frame f;
   GridXform g;
   Placed m;
   const float* occ;
   const int16_t* labels;
+  const float* src_occ;
+  const int16_t* src_labels;
   float level;
   int lift;
   Status st;
@@ -377,10 +382,10 @@ struct Prepared {
 
 enum { PLACED = 0, NO_POINTS = 1, TOP_OUT = 2 };   // dmnerf_placement_maps' status per base
 
-// The host checks of every placement call, before any launch.
-int check(const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
-          const dmnerf_placement* p, const char* who, Prepared& q) {
-  DMN_CHECK(occ && labels && T16 && ext3 && p, "%s: NULL argument", who);
+// The host checks of every placement call, before any launch: the object's grid occ / labels and the scene.
+int check(const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels, int dim, float level,
+          const double* T16, const double* ext3, const dmnerf_placement* p, const char* who, Prepared& q) {
+  DMN_CHECK(occ && labels && scene_occ && scene_labels && T16 && ext3 && p, "%s: NULL argument", who);
   DMN_CHECK(dim >= 2 && dim <= PLACE_MAX_DIM, "%s: dim %d out of range [2, %d]", who, dim, PLACE_MAX_DIM);
   if (sweep_grid_check(T16, ext3, dim, level, who)) return 1;
   DMN_CHECK(p->label >= 0 && p->label <= DMNERF_MAX_INS, "%s: label %d outside [0, %d]", who, p->label, DMNERF_MAX_INS);
@@ -402,8 +407,10 @@ int check(const float* occ, const int16_t* labels, int dim, float level, const d
   f.flip = p->sign == 1 ? 1 : 0;
   f.height_fast = p->axis == 2 ? 1 : 0;
   q.g = make_xform(T16, ext3, dim);
-  q.occ = occ;
-  q.labels = labels;
+  q.occ = scene_occ;
+  q.labels = scene_labels;
+  q.src_occ = occ;
+  q.src_labels = labels;
   q.level = level;
   q.lift = p->lift;
   return 0;
@@ -423,7 +430,8 @@ int base_move(const dmnerf_placement* p, const double* base12, const int32_t* bo
   return edit_move_from_abi(d, T16, ext3, dim, DMNERF_MAX_INS, e, who, i);
 }
 
-// The buffers, the grid check and the column pass: the column table, and the bytes of the unmoved object when `unmoved`.
+// The buffers, the grid check (of both grids when the scene is not the object's grid) and the column pass: the column table,
+// and the bytes of the unmoved object when `unmoved`.
 int columns(PlaceState& s, Prepared& q, bool unmoved, cudaStream_t stream) {
   const int64_t d = q.f.dim, n = d * d * d, n_cols = d * d;
   if (s.table.get((size_t)n, &q.table) || s.object.get((size_t)n, &q.object) || s.counts.get((size_t)n_cols, &q.counts) ||
@@ -436,6 +444,9 @@ int columns(PlaceState& s, Prepared& q, bool unmoved, cudaStream_t stream) {
   }
   DMN_CUDA(cudaMemcpyAsync(q.st_dev, &init, sizeof(init), cudaMemcpyHostToDevice, stream));
   if (launch_grid_check(q.occ, q.labels, n, DMNERF_MAX_INS + 1, &q.st_dev->bad, stream)) return 2;
+  if ((q.src_occ != q.occ || q.src_labels != q.labels) &&
+      launch_grid_check(q.src_occ, q.src_labels, n, DMNERF_MAX_INS + 1, &q.st_dev->bad, stream))
+    return 2;
   const unsigned blocks = (unsigned)((n_cols + TILE - 1) / TILE);
   if (unmoved)
     place_column_kernel<true><<<blocks, CP_WARPS * 32, 0, stream>>>(q.f, q.g, q.m, q.occ, q.labels, q.level, q.table, q.object);
@@ -458,8 +469,8 @@ int object_runs(PlaceState& s, Prepared& q, const EditMove* base, bool first, co
     DMN_CUDA(cudaMemcpyAsync(q.st_dev, &init, sizeof(init), cudaMemcpyHostToDevice, stream));
   }
   if (base) {
-    place_moved_kernel<<<(unsigned)((n + MV_THREADS - 1) / MV_THREADS), MV_THREADS, 0, stream>>>(q.f, q.g, *base, q.occ, q.labels,
-                                                                                                 q.level, q.object);
+    place_moved_kernel<<<(unsigned)((n + MV_THREADS - 1) / MV_THREADS), MV_THREADS, 0, stream>>>(q.f, q.g, *base, q.src_occ,
+                                                                                                 q.src_labels, q.level, q.object);
     DMN_LAUNCH_OK();
   }
   const unsigned col_blocks = (unsigned)((n_cols + RUN_WARPS - 1) / RUN_WARPS);
@@ -547,7 +558,7 @@ int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int di
   memset(info, 0, sizeof(*info));
   Prepared q;
   int why;
-  if (check(occ, labels, dim, level, T16, ext3, p, who, q)) return 1;
+  if (check(occ, labels, occ, labels, dim, level, T16, ext3, p, who, q)) return 1;
   if (const int rc = columns(s, q, true, st)) return rc;
   if (const int rc = object_runs(s, q, nullptr, true, who, &why, st)) return rc;
   if (unplaced(q, why, false, who)) return 1;
@@ -556,10 +567,11 @@ int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int di
   return 0;
 }
 
-int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
-                   const dmnerf_placement* p, const double* bases_host, const int32_t* box_host, int n_bases, int32_t* drop,
-                   int32_t* contacts, int16_t* support, dmnerf_placement_info* info, int32_t* status, cudaStream_t st) {
-  const char* who = "placement_maps";
+int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels, int dim,
+                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, const double* bases_host,
+                   const int32_t* box_host, int n_bases, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
+                   int32_t* status, cudaStream_t st) {
+  const char* who = occ == scene_occ && labels == scene_labels ? "placement_maps" : "placement_maps_in_scene";
   DMN_CHECK(drop && contacts && support && info && status, "%s: NULL argument", who);
   DMN_CHECK(n_bases >= 1 && n_bases <= DMNERF_MAX_BASES, "%s: between 1 and %d bases are supported, got %d", who, DMNERF_MAX_BASES,
             n_bases);
@@ -569,7 +581,7 @@ int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, int d
     status[i] = NO_POINTS;
   }
   Prepared q;
-  if (check(occ, labels, dim, level, T16, ext3, p, who, q)) return 1;
+  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, who, q)) return 1;
   std::vector<EditMove> e(n_bases);
   for (int i = 0; i < n_bases; ++i)
     if (base_move(p, bases_host + 12 * i, box_host, T16, ext3, dim, e[i], who, i)) return 1;
@@ -586,18 +598,20 @@ int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, int d
   return 0;
 }
 
-int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16,
-                       const double* ext3, const dmnerf_placement* p, const double* base_host, const int32_t* box_host, int u, int v,
-                       int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host, int32_t* drop_host, cudaStream_t st) {
+int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels,
+                       int dim, float level, const double* T16, const double* ext3, const dmnerf_placement* p, const double* base_host,
+                       const int32_t* box_host, int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                       int32_t* drop_host, cudaStream_t st) {
   const bool moved = base_host != nullptr;
-  const char* who = moved ? "placement_contacts_moved" : "placement_contacts";
+  const char* who = !moved ? "placement_contacts"
+                           : (occ == scene_occ && labels == scene_labels ? "placement_contacts_moved" : "placement_contacts_in_scene");
   DMN_CHECK(n_cells_host && drop_host && max_cells >= 0 && (max_cells == 0 || cells_host), "%s: bad output arguments", who);
   *n_cells_host = 0;
   *drop_host = -1;
   Prepared q;
   EditMove e;
   int why;
-  if (check(occ, labels, dim, level, T16, ext3, p, who, q)) return 1;
+  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, who, q)) return 1;
   if (moved) {
     DMN_CHECK(box_host, "%s: box is NULL", who);
     if (base_move(p, base_host, box_host, T16, ext3, dim, e, who, 0)) return 1;

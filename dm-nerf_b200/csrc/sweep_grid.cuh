@@ -71,4 +71,34 @@ __device__ __forceinline__ bool edit_target(const double* trans, const double* i
   return in;
 }
 
+// The edit rule at one grid point p (DESIGN.md, "Meshing an edited scene"), shared by the edited sweep (the network at the
+// target) and the grid-only edit (collide.cu: the unedited grid at the target's nearest index).  m: the move's label, rest_drop
+// and piece (taken by value, which keeps the edited sweep's SASS as it was before the rule was shared).  target(lt, ot) gives the
+// label and occupancy at the target and is called only in the box; drops_target() is the piece's region_drops at the target and
+// in_piece(b) sets b to whether the piece keeps p, both called only with a piece.
+//   take:   in the box && lt == label && (ot > level || o <= level) && (no piece || !drops_target()): take(ot) writes
+//           (o, l) <- (ot, label);
+//   vacate: otherwise l == label && o > level && (no piece || p in the piece || rest_drop): vacate() writes o <- 0, the label
+//           kept.
+template <class Move, class Target, class DropsTarget, class InPiece, class Take, class Vacate>
+__device__ __forceinline__ void edit_rule(const Move m, bool in_box, const Target& target, float o, int l, float level,
+                                          const DropsTarget& drops_target, const InPiece& in_piece_of, const Take& take,
+                                          const Vacate& vacate) {
+  const bool has_piece = m.piece.bits != nullptr;
+  if (in_box) {
+    int lt;
+    float ot;
+    target(lt, ot);
+    if (lt == m.label && (ot > level || o <= level) && (!has_piece || !drops_target())) {
+      take(ot);
+      return;
+    }
+  }
+  if (l == m.label && o > level) {
+    bool in_piece = true;
+    if (has_piece) in_piece_of(in_piece);
+    if (in_piece || m.rest_drop) vacate();
+  }
+}
+
 }  // namespace dmnerf

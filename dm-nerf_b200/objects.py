@@ -22,6 +22,8 @@
                                                         -> collision checks of moves, and which objects touch, from a sweep
     placement_map(occ, labels, scene_transform, label, down, ...) / placement(map, u, v) / place_object(..., near, ...)
                                                         -> where a lowered object comes to rest, on what, and whether it stands
+    edited_grid(occ, labels, scene_transform, moves, ...) / arrange_objects(occ, labels, scene_transform, items, down, ...)
+                                                        -> moves applied to the sweep alone, and several objects placed in turn
 
 Every network sample is labelled argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the
 exchanger's rule); a sample whose label is not kept has alpha = 0 in the composite of both passes, so the coarse weights of the
@@ -424,7 +426,7 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     Returns one dict per move: label, landed (the voxels the moved object occupies after the move), overlap {label: voxels}
     (labels with voxels > 0: solid obstacle points the moved object lands on; the points the move vacates are not obstacles),
     overlap_volume {label: voxels times the inventory's voxel volume} and total (the overlapping voxels)."""
-    from .manipulator import _piece_region, move_pieces, move_rests
+    from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
     dim = _check_sweep(occ, labels, "move_overlap")
@@ -440,13 +442,7 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     if boxes is None:
         boxes = edit_boxes(occ, labels, moves, T, ext, level, margin, pieces)
     boxes = _check_boxes(boxes, len(mv), dim)
-    descs = (_lib.EditMove * len(mv))()
-    for i in range(len(mv)):
-        d = descs[i]
-        d.label, d.rest_drop = mv[i], int(drops[i])
-        d.trans[:] = mats[i][:3].reshape(-1).tolist()
-        d.box[:] = [int(v) for v in boxes[i]]
-        d.piece = _piece_region(regions[i], mv[i], ins_num, occ.device)
+    descs = _edit_moves(mv, mats, boxes, drops, regions, occ.device)
     overlap = np.zeros((len(mv), MAX_LABELS), dtype=np.int64)
     landed = np.zeros(len(mv), dtype=np.int64)
     ctx = get_context(occ.device)
@@ -454,12 +450,28 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
              _lib.doubles(ext, 3), descs, len(mv), (C.c_uint32 * 4)(*words), overlap.ctypes.data_as(C.POINTER(C.c_int64)),
              landed.ctypes.data_as(C.POINTER(C.c_int64)))
     unit = _voxel_volume(T, ext, dim)
-    out = []
+    return [_count_report(mv[i], landed[i], overlap[i], unit, "overlap") for i in range(len(mv))]
+
+
+def _edit_moves(mv, mats, boxes, drops, regions, device):
+    """The ABI moves (dmnerf_edit_move) of checked labels, 4x4 matrices, boxes, rest drops and pieces (labels up to 127)."""
+    from .manipulator import _piece_region
+    descs = (_lib.EditMove * len(mv))()
     for i in range(len(mv)):
-        hit = {int(k): int(overlap[i, k]) for k in np.nonzero(overlap[i])[0]}
-        out.append({"label": mv[i], "landed": int(landed[i]), "overlap": hit,
-                    "overlap_volume": {k: v * unit for k, v in hit.items()}, "total": int(overlap[i].sum())})
-    return out
+        d = descs[i]
+        d.label, d.rest_drop = mv[i], int(drops[i])
+        d.trans[:] = mats[i][:3].reshape(-1).tolist()
+        d.box[:] = [int(v) for v in boxes[i]]
+        d.piece = _piece_region(regions[i], mv[i], MAX_LABELS - 1, device)
+    return descs
+
+
+def _count_report(label, landed, counts, unit, key):
+    """One move's counts as move_overlap and edited_grid report them: label, landed, key {label: voxels} (labels with voxels > 0),
+    key_volume {label: voxels times the voxel volume `unit`} and total."""
+    hit = {int(k): int(counts[k]) for k in np.nonzero(counts)[0]}
+    return {"label": label, "landed": int(landed), key: hit, key + "_volume": {k: v * unit for k, v in hit.items()},
+            "total": int(counts.sum())}
 
 
 def _translate(v):
@@ -596,13 +608,16 @@ def _check_point(x, what):
 
 
 def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=None, level=0.45, piece=None, rest="keep",
-                  obstacles=None, base=None, box=None):
+                  obstacles=None, base=None, box=None, scene=None):
     """dmnerf_placement_map: object `label` (or its piece, with rest "keep" / "drop" as move_overlap) raised by `lift` voxels and
     lowered along the index axis closest to +-down (network frame, chosen as supports chooses it), at every horizontal offset
     that keeps it inside the grid of the labelled keep-all sweep occ / labels.  obstacles: the labels that count (default all).
     base (a 4x4 move in the network frame, as move_overlap takes it) places the object as that move leaves it instead
     (dmnerf_placement_maps; DESIGN.md, "Turned placements"): sampled from the grid through the source box `box` (default
     edit_boxes' box, margin 2), its points carried outside the grid lost.
+    scene (DESIGN.md, "Arranging objects"): an (occ, labels) pair of the same shape, dtype and device, e.g. an edited_grid
+    result; the object is still sampled from occ / labels, but the obstacles, the points it vacates and the labels it rests on
+    come from the scene (dmnerf_placement_maps_in_scene; without a base, the identity base with the default box).
     Returns a dict:
       drop, support, contacts: device maps [U, V] (int32, int16, int32): the voxels it falls (-1: blocked where it is raised),
                       the obstacle label under most of its resting runs (-1: blocked, or resting on the grid's floor), and the
@@ -620,7 +635,13 @@ def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=Non
         base = _move_matrix(base, 0)
     if box is not None:
         box = _check_boxes([box], 1, occ.shape[0])[0]
-    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles)
+    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene)
+    if base is None and c["scene"] is not None:
+        m, status = _placement_maps(c, [np.eye(4)], _placement_box(c, box), _object_points(c))
+        if m[0] is None:
+            raise ValueError(_unplaced(c, status[0]))
+        m[0]["base"] = None
+        return m[0]
     if base is None:
         info = _lib.PlacementInfo()
         drop, contacts, support = (torch.empty(c["dim"] ** 2, dtype=t, device=occ.device) for t in (torch.int32, torch.int32, torch.int16))
@@ -642,8 +663,22 @@ def _unplaced(c, status):
     return "placement: lift %d takes the moved object's top out of the grid [0, %d]" % (c["lift"], c["dim"] - 1)
 
 
-def _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles):
-    """The checked arguments of a placement call: grid, level, label, lift, down axis and the ABI placement."""
+def _check_scene(scene, occ, labels):
+    """placement's scene: None, or an (occ, labels) pair with the shape, dtypes and device of occ / labels."""
+    if scene is None:
+        return None
+    try:
+        s_occ, s_lab = scene
+    except (TypeError, ValueError):
+        raise ValueError("placement: scene must be an (occ, labels) pair") from None
+    if not (torch.is_tensor(s_occ) and torch.is_tensor(s_lab)) or s_occ.shape != occ.shape or s_lab.shape != labels.shape or \
+            s_occ.dtype != occ.dtype or s_lab.dtype != labels.dtype or s_occ.device != occ.device or s_lab.device != labels.device:
+        raise ValueError("placement: the scene must be (occ, labels) tensors of the grid's shape, dtypes and device")
+    return s_occ, s_lab
+
+
+def _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene=None):
+    """The checked arguments of a placement call: grid, level, label, lift, down axis, scene and the ABI placement."""
     from .manipulator import _piece_region, move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -657,6 +692,7 @@ def _placement_call(occ, labels, scene_transform, label, down, lift, extents, le
     A, _ = grid_affine(T, 2, ext)
     axis, sign = down_axis((A / np.linalg.norm(A, axis=0)).T, down, "placement")
     dim = _check_sweep(occ, labels, "placement_map")
+    scene = _check_scene(scene, occ, labels)
     if not 2 <= dim <= PLACE_MAX_DIM:
         raise ValueError("placement: dim %d outside [2, %d]" % (dim, PLACE_MAX_DIM))
     if int(lift) > dim - 1:
@@ -666,7 +702,7 @@ def _placement_call(occ, labels, scene_transform, label, down, lift, extents, le
                           axis=axis, sign=sign, lift=int(lift))
     desc.obstacles[:] = words
     return {"occ": occ, "labels": labels, "T": T, "ext": ext, "level": level, "label": label, "lift": int(lift), "axis": axis,
-            "sign": sign, "dim": dim, "desc": desc, "piece": piece}
+            "sign": sign, "dim": dim, "desc": desc, "piece": piece, "scene": scene}
 
 
 def _placement_library(name, occ, *args):
@@ -712,7 +748,7 @@ def _map_result(c, info, drop, contacts, support, base, box, points_before):
             "centre": centre, "runs": int(info.runs), "points": n, "height": (int(info.height[0]), int(info.height[1])),
             "lift": c["lift"], "label": c["label"], "dim": dim, "base": base, "box": None if box is None else tuple(int(x) for x in box),
             "points_before": points_before,
-            "_call": (c["occ"], c["labels"], c["T"], c["ext"], c["level"], c["desc"], c["piece"])}
+            "_call": (c["occ"], c["labels"], c["T"], c["ext"], c["level"], c["desc"], c["piece"]), "_scene": c.get("scene")}
 
 
 def _placement_maps(c, bases, box, points_before):
@@ -725,8 +761,12 @@ def _placement_maps(c, bases, box, points_before):
     infos = (_lib.PlacementInfo * n)()
     status = np.zeros(n, dtype=np.int32)
     rows = np.ascontiguousarray([np.asarray(b, dtype=np.float64)[:3].reshape(-1) for b in bases])
-    _placement_library("dmnerf_placement_maps", occ, _lib.ptr(occ), _lib.ptr(c["labels"], torch.int16), dim, c["level"],
-                       _lib.doubles(c["T"], 16), _lib.doubles(c["ext"], 3), C.byref(c["desc"]),
+    grids = (_lib.ptr(occ), _lib.ptr(c["labels"], torch.int16))
+    name = "dmnerf_placement_maps"
+    if c.get("scene") is not None:
+        grids += (_lib.ptr(c["scene"][0]), _lib.ptr(c["scene"][1], torch.int16))
+        name = "dmnerf_placement_maps_in_scene"
+    _placement_library(name, occ, *grids, dim, c["level"], _lib.doubles(c["T"], 16), _lib.doubles(c["ext"], 3), C.byref(c["desc"]),
                        rows.ctypes.data_as(C.POINTER(C.c_double)), (C.c_int32 * 6)(*[int(x) for x in box]), n,
                        _lib.ptr(drop, torch.int32), _lib.ptr(contacts, torch.int32), _lib.ptr(support, torch.int16), infos,
                        status.ctypes.data_as(C.POINTER(C.c_int32)))
@@ -797,7 +837,12 @@ def placement(m, u, v):
     head = (ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), m["dim"], level, _lib.doubles(T, 16), _lib.doubles(ext, 3),
             C.byref(desc))
     tail = (u, v, cells.ctypes.data_as(C.POINTER(C.c_int32)), n, C.byref(got), C.byref(dr))
-    if m.get("base") is None:
+    scene = m.get("_scene")
+    if scene is not None:                              # the scene of the map: the object from occ / labels (identity base by default)
+        base = np.eye(4) if m.get("base") is None else m["base"]
+        ctx.call("dmnerf_placement_contacts_in_scene", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), _lib.ptr(scene[0]),
+                 _lib.ptr(scene[1], torch.int16), *head[3:], _lib.doubles(base[:3], 12), (C.c_int32 * 6)(*m["box"]), *tail)
+    elif m.get("base") is None:
         ctx.call("dmnerf_placement_contacts", *head, *tail)
     else:
         ctx.call("dmnerf_placement_contacts_moved", *head, _lib.doubles(m["base"][:3], 12), (C.c_int32 * 6)(*m["box"]), *tail)
@@ -884,7 +929,7 @@ def _turn_angles(turns):
 
 
 def place_object(occ, labels, scene_transform, label, down, near, on=None, stable=True, lift=0, max_tests=64, extents=None,
-                 level=0.45, piece=None, rest="keep", obstacles=None, turns=None):
+                 level=0.45, piece=None, rest="keep", obstacles=None, turns=None, scene=None):
     """The placement of object `label` (or its piece) closest to the network-frame point `near`: over placement_map's offsets
     that are not blocked and rest on an obstacle whose label is in `on` (default: any), ordered by the distance of the placed
     centre of mass from `near` across the down axis (ties: the lowest (u, v)), the first that is stable -- testing at most
@@ -894,18 +939,19 @@ def place_object(occ, labels, scene_transform, label, down, near, on=None, stabl
     {"placement": placement() of it, or None; "reason": None, or why there is none; "candidates": how many offsets qualified;
     "tested": stability tests run; "map": the placement_map result it came from (without turns: the map); "turn": its angle
     (None without turns); "maps": [(angle, map)] of the turns that were mapped; "unfit": the angles whose turned object does not
-    fit the grid; "unplaced": the angles whose turned object has no point or leaves the grid at this lift}."""
+    fit the grid; "unplaced": the angles whose turned object has no point or leaves the grid at this lift}.  scene: as
+    placement_map's (DESIGN.md, "Arranging objects")."""
     near = _check_point(near, "near")
     if isinstance(max_tests, (bool, np.bool_)) or int(max_tests) != max_tests or int(max_tests) < 1:
         raise ValueError("placement: max_tests must be an integer >= 1, got %r" % (max_tests,))
     on = None if on is None else set(_labels(on, MAX_LABELS - 1, "placement"))
     angles = None if turns is None else _turn_angles(turns)
     if turns is None:
-        m = placement_map(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles)
+        m = placement_map(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene=scene)
         maps, unfit, unplaced = [(None, m)], [], []
     else:
         maps, unfit, unplaced = turned_placement_maps(occ, labels, scene_transform, label, down, angles, lift, extents, level, piece,
-                                                      rest, obstacles)
+                                                      rest, obstacles, scene)
     out = {"placement": None, "reason": None, "candidates": 0, "tested": 0, "map": maps[0][1] if turns is None else None,
            "turn": None, "maps": [] if turns is None else maps, "unfit": unfit, "unplaced": unplaced}
     rows = placement_candidates([m for _, m in maps], near, on)
@@ -927,13 +973,14 @@ def place_object(occ, labels, scene_transform, label, down, near, on=None, stabl
 
 
 def turned_placement_maps(occ, labels, scene_transform, label, down, turns, lift=0, extents=None, level=0.45, piece=None,
-                          rest="keep", obstacles=None):
+                          rest="keep", obstacles=None, scene=None):
     """placement_map of the object turned about the down axis by each of `turns` (degrees, or an integer K: 360 k / K), the
     turns built by turn_bases from the object's solid box and exact centre, mapped in dmnerf_placement_maps calls of at most
     MAX_BASES bases, with edit_boxes' source box -> ([(angle, map)] of the turns mapped, the angles that do not fit the grid,
-    the angles whose turned object has no point or its top out of the grid)."""
+    the angles whose turned object has no point or its top out of the grid).  scene: as placement_map's; the turns are built from
+    the object in occ / labels."""
     angles = _turn_angles(turns)
-    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles)
+    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene)
     points, box, centre = _object_extent(_object_mask(c))
     if points == 0:
         raise ValueError("placement: label %d has no solid points%s" % (c["label"], " in its piece" if piece is not None else ""))
@@ -999,6 +1046,155 @@ def largest_component_grid(occ, labels, level, objects):
         if int(k) in best:
             lut[best[int(k)]] = int(k)
     return component_groups(cc["grid"], lut, -1)
+
+
+# ----------------------------------------------------------------------------------------------------------------- arrangement
+# DESIGN.md, "Arranging objects": the edited sweep's rule with the network replaced by the unedited grid at the nearest index
+# (edited_grid), and several objects placed one after another, each in the scene the earlier placements leave (arrange_objects).
+ARRANGE_KEYS = ("label", "near", "on", "piece", "rest", "turns", "stable", "lift", "obstacles")
+
+
+def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes, drops, regions):
+    """dmnerf_grid_edit of checked moves: applied in place to occ / labels, sampled from src_occ / src_labels -> edited_grid's
+    report."""
+    n, dim = len(mv), occ.shape[0]
+    overwritten = np.zeros((n, MAX_LABELS), dtype=np.int64)
+    landed = np.zeros(n, dtype=np.int64)
+    ctx = get_context(occ.device)
+    ctx.call("dmnerf_grid_edit", ctx.handle, _lib.ptr(src_occ), _lib.ptr(src_labels, torch.int16), dim, level, _lib.doubles(T, 16),
+             _lib.doubles(ext, 3), _edit_moves(mv, mats, boxes, drops, regions, occ.device), n, _lib.ptr(occ),
+             _lib.ptr(labels, torch.int16), landed.ctypes.data_as(C.POINTER(C.c_int64)),
+             overwritten.ctypes.data_as(C.POINTER(C.c_int64)))
+    unit = _voxel_volume(T, ext, dim)
+    return [_count_report(mv[i], landed[i], overwritten[i], unit, "overwritten") for i in range(n)]
+
+
+def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, boxes=None, margin=2, pieces=None, rest="keep"):
+    """dmnerf_grid_edit: edited_sweep's moves applied in order to the labelled keep-all sweep occ / labels ([dim]^3 float32 / int16
+    on the device) without the network: a move shows at p the unedited grid at the nearest grid index of trans p, as the collision
+    checks sample a moved object.  On a grid whose points and steps are exact in fp32, whole-voxel translations and quarter turns
+    give edited_sweep's grid bit for bit; elsewhere it is the sweep resampled at its own resolution.  boxes, margin, pieces, rest:
+    as edited_sweep (default boxes: edit_boxes of occ / labels).  Works on copies -> (occ', labels', report), report one dict per
+    move: label, landed (the voxels it takes from a solid target), overwritten {label: voxels} (labels with voxels > 0: solid
+    points of the grid as the earlier moves left it that it lands on and does not vacate), overwritten_volume and total."""
+    from .manipulator import move_pieces, move_rests
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    dim = _check_sweep(occ, labels, "edited_grid")
+    ext = EXTENTS if extents is None else extents
+    mv, mats = _check_moves(moves, MAX_LABELS - 1)
+    level = _check_level(level)
+    drops = move_rests(rest, len(mv))
+    regions = move_pieces(pieces, mv, MAX_LABELS - 1, occ.device) or [None] * len(mv)
+    if int(margin) != margin or int(margin) < 0:
+        raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
+    if boxes is None:
+        boxes = edit_boxes(occ, labels, moves, T, ext, level, margin, pieces)
+    boxes = _check_boxes(boxes, len(mv), dim)
+    out_occ, out_labels = occ.clone(memory_format=torch.contiguous_format), labels.clone(memory_format=torch.contiguous_format)
+    if not mv:
+        return out_occ, out_labels, []
+    return out_occ, out_labels, _grid_edit(occ, labels, out_occ, out_labels, T, ext, level, mv, mats, boxes, drops, regions)
+
+
+def _check_items(items, dim, device):
+    """arrange_objects' items, checked before any device work -> [dict with every key of ARRANGE_KEYS]."""
+    from .manipulator import move_pieces, move_rests
+    if isinstance(items, dict) or not hasattr(items, "__iter__"):
+        raise ValueError("arrange: items must be a list of dicts")
+    items = list(items)
+    if not 1 <= len(items) <= _lib.MAX_MOVES:
+        raise ValueError("arrange: between 1 and %d items are supported (the render and the mesh take at most %d moves), got %d"
+                         % (_lib.MAX_MOVES, _lib.MAX_MOVES, len(items)))
+    out, seen = [], {}
+    for i, it in enumerate(items):
+        if not isinstance(it, dict):
+            raise ValueError("arrange: item %d must be a dict, got %r" % (i, type(it).__name__))
+        unknown = sorted(set(it) - set(ARRANGE_KEYS))
+        if unknown:
+            raise ValueError("arrange: item %d: unknown keys %s (known: %s)" % (i, unknown, ", ".join(ARRANGE_KEYS)))
+        for k in ("label", "near"):
+            if k not in it:
+                raise ValueError("arrange: item %d needs %r" % (i, k))
+        c = {k: it.get(k) for k in ARRANGE_KEYS}
+        c["label"] = _labels([c["label"]], MAX_LABELS - 1, "arrange")[0]
+        if c["label"] in seen:
+            raise ValueError("arrange: items %d and %d share label %d (the second move would also vacate the first one's landed "
+                             "points)" % (seen[c["label"]], i, c["label"]))
+        seen[c["label"]] = i
+        c["near"] = _check_point(c["near"], "near")
+        if c["on"] is not None:
+            c["on"] = _labels(c["on"], MAX_LABELS - 1, "arrange")
+        if c["turns"] is not None:
+            _turn_angles(c["turns"])
+        c["stable"] = True if c["stable"] is None else c["stable"]
+        if not isinstance(c["stable"], (bool, np.bool_)):
+            raise ValueError("arrange: item %d: stable must be True or False, got %r" % (i, c["stable"]))
+        c["lift"] = 0 if c["lift"] is None else c["lift"]
+        if isinstance(c["lift"], (bool, np.bool_)) or int(c["lift"]) != c["lift"] or not 0 <= int(c["lift"]) <= dim - 1:
+            raise ValueError("arrange: item %d: lift must be an integer in [0, %d] voxels, got %r" % (i, dim - 1, c["lift"]))
+        c["lift"] = int(c["lift"])
+        c["rest"] = "keep" if c["rest"] is None else c["rest"]
+        move_rests(c["rest"], 1)
+        if c["piece"] is not None:
+            move_pieces([c["piece"]], [c["label"]], MAX_LABELS - 1, device)
+        if c["obstacles"] is not None:
+            label_words(c["obstacles"])
+        out.append(c)
+    return out
+
+
+def arrange_objects(occ, labels, scene_transform, items, down, extents=None, level=0.45, max_tests=64):
+    """Several objects placed one after another (DESIGN.md, "Arranging objects"), greedily in the order given, each in the scene
+    the earlier placements leave: the state starts as a copy of the labelled keep-all sweep occ / labels; item k is placed by
+    place_object with the object from the unedited grid and scene = the state, and when it is placed its move is applied to the
+    state by the grid-only edit (edited_grid's rule, the default box); an item that is not placed stays where it is and is an
+    obstacle for the items after it.  items: dicts with label and near (network frame) and optionally on (labels to rest on; an
+    earlier item keeps its label where it landed), piece, rest, turns, stable, lift and obstacles, as place_object takes them;
+    at most MAX_MOVES items, no two with one label.  down: shared by every item.  Every item is checked before any device work.
+    Returns a dict:
+      items:  per item, place_object's result and its label; placement None and a reason when it was not placed (its maps were
+              computed on the state before its own move and refer to the state's tensors, which later items edit);
+      moves:  [(label, 4x4 nested list)] of the placed items in order, and pieces / rest aligned with them: manipulate_frame,
+              manipulator_eval, edited_sweep and edited_mesh take them unchanged;
+      occ, labels: the arranged grid, equal to edited_grid(occ, labels, ..., moves, pieces=pieces, rest=rest) bit for bit;
+      report: edited_grid's report of each placed move (overwritten: what it landed on in the scene left before it)."""
+    from .manipulator import move_rests
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    ext = EXTENTS if extents is None else extents
+    if not torch.is_tensor(occ) or occ.dim() != 3:
+        raise ValueError("arrange: occ must be a [dim, dim, dim] tensor")
+    checked = _check_items(items, occ.shape[0], occ.device)
+    level = _check_level(level)
+    if isinstance(max_tests, (bool, np.bool_)) or int(max_tests) != max_tests or int(max_tests) < 1:
+        raise ValueError("placement: max_tests must be an integer >= 1, got %r" % (max_tests,))
+    A, _ = grid_affine(T, 2, ext)
+    down_axis((A / np.linalg.norm(A, axis=0)).T, down, "arrange")
+    dim = _check_sweep(occ, labels, "arrange_objects")
+    if not 2 <= dim <= PLACE_MAX_DIM:
+        raise ValueError("placement: dim %d outside [2, %d]" % (dim, PLACE_MAX_DIM))
+    state_occ, state_labels = occ.clone(memory_format=torch.contiguous_format), labels.clone(memory_format=torch.contiguous_format)
+    out = {"items": [], "moves": [], "pieces": [], "rest": [], "occ": state_occ, "labels": state_labels, "report": []}
+    for it in checked:
+        try:
+            r = place_object(occ, labels, T, it["label"], down, it["near"], it["on"], it["stable"], it["lift"], max_tests, ext, level,
+                             it["piece"], it["rest"], it["obstacles"], it["turns"], scene=(state_occ, state_labels))
+        except ValueError as e:        # found on the device: no solid points (in its piece), or the lift takes its top out
+            r = {"placement": None, "reason": str(e)}
+        out["items"].append(dict(r, label=it["label"]))
+        if r["placement"] is None:
+            continue
+        trans = r["placement"]["transformation"]
+        move = (it["label"], trans)
+        pieces = None if it["piece"] is None else [it["piece"]]
+        box = edit_boxes(occ, labels, [move], T, ext, level, 2, pieces)
+        out["report"] += _grid_edit(occ, labels, state_occ, state_labels, T, ext, level, [it["label"]],
+                                    [np.asarray(trans, dtype=np.float64)], box, move_rests(it["rest"], 1), [it["piece"]])
+        out["moves"].append(move)
+        out["pieces"].append(it["piece"])
+        out["rest"].append(it["rest"])
+    return out
 
 
 # ----------------------------------------------------------------------------------------------------------------- inventory

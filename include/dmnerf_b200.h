@@ -573,6 +573,43 @@ DMNERF_API int dmnerf_placement_contacts_moved(dmnerf_ctx* ctx, const float* occ
                                                const int32_t* box_host /* [6] */, int u, int v, int32_t* cells_host, int64_t max_cells,
                                                int64_t* n_cells_host, int32_t* drop_host, void* stream);
 
+/* ---- arranging objects (DESIGN.md, "Arranging objects"; no counterpart in the original) -------------------------------------
+ * dmnerf_grid_edit: the moves of dmnerf_mesh_occupancy_edit applied in order, in place, to the state occ / labels [dim^3] (DEVICE
+ *   float32 / int16, in-out), with the network replaced by the source grid src_occ / src_labels [dim^3] (DEVICE, never written) at
+ *   the target's nearest grid index: per move and state point p, t and q = rint(A^-1 (t - b)) as dmnerf_move_overlap computes
+ *   them, take = q in B && src_labels[q] == label && (src_occ[q] > level || occ_p <= level) && (no piece || the piece keeps t):
+ *   (occ_p, label_p) = (src_occ[q], label); otherwise dmnerf_mesh_occupancy_edit's vacate.  moves_host: n_moves in
+ *   [1, DMNERF_MAX_MOVES], fields as dmnerf_mesh_occupancy_edit (labels in [0, 127]).  Per move: landed_host [n] (HOST int64) =
+ *   the takes whose target is solid; overwritten_host [n][128] (HOST int64) = those of them that land on a solid state point of
+ *   label l that the move does not vacate (label_p == label and p in the piece -- every point without one -- or rest_drop).  With
+ *   the state equal to the source these are dmnerf_move_overlap's landed and overlap (every label an obstacle), and on a grid
+ *   whose points and steps are exact in fp32 the result of whole-voxel translations and quarter turns is the edited sweep's.
+ *   Every count is an integer and every write is per point, so the result is bit-reproducible.  Rejected on the host, before any
+ *   launch: n_moves out of range, everything dmnerf_move_overlap rejects of the grid and the moves, and source and state buffers
+ *   that overlap in memory.  Fails after the first read-back, with the state unwritten, on NaN or a label outside [0, 127] in
+ *   either grid.  Two device->host reads: the grid checks, then the counts (synchronises the stream twice).
+ * dmnerf_placement_maps_in_scene: dmnerf_placement_maps with the object S_base sampled from occ / labels and everything else --
+ *   the obstacles, the points the move vacates, the labels under the resting runs -- taken from the scene scene_occ /
+ *   scene_labels [dim^3] (DEVICE, the same grid).  The scene being occ / labels is dmnerf_placement_maps, bit for bit.  Both
+ *   grids are checked.
+ * dmnerf_placement_contacts_in_scene: dmnerf_placement_contacts_moved in the scene of dmnerf_placement_maps_in_scene. */
+DMNERF_API int dmnerf_grid_edit(dmnerf_ctx* ctx, const float* src_occ, const int16_t* src_labels, int dim, float level,
+                                const double* transform_host, const double* extents_host, const dmnerf_edit_move* moves_host, int n_moves,
+                                float* occ, int16_t* labels, int64_t* landed_host /* [n] */, int64_t* overwritten_host /* [n][128] */,
+                                void* stream);
+DMNERF_API int dmnerf_placement_maps_in_scene(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                              const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                              const double* extents_host, const dmnerf_placement* placement,
+                                              const double* bases_host /* [n][12] */, const int32_t* box_host /* [6] */, int n_bases,
+                                              int32_t* drop, int32_t* contacts, int16_t* support,
+                                              dmnerf_placement_info* info_host /* [n] */, int32_t* status_host /* [n] */, void* stream);
+DMNERF_API int dmnerf_placement_contacts_in_scene(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                                  const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                                  const double* extents_host, const dmnerf_placement* placement,
+                                                  const double* base_host /* [12] */, const int32_t* box_host /* [6] */, int u, int v,
+                                                  int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host, int32_t* drop_host,
+                                                  void* stream);
+
 /* ---- connected components (DESIGN.md, "Connected components"; no counterpart in the original) --------------------------------
  * The solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order, p = (i dim + j) dim + k) split into components:
  * two solid points are adjacent when they are face neighbours (connectivity 6) or face, edge or corner neighbours (26), never

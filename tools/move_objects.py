@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Move one piece of an object of a trained DM-NeRF checkpoint and render the edited frame (DESIGN.md, "Moving pieces").
 
-    python tools/move_objects.py CHECKPOINT.tar --pose POSE.npy --hwk H W K (--move-label L | --move-piece ID)
+    python tools/move_objects.py CHECKPOINT.tar --pose POSE.npy --hwk H W K (--move-label L | --move-piece ID | --arrange SPEC.json)
            (--mode {translation,rotation,scale,multi} [--distance -0.25 --yaw 90 --scale 1.2]
             | --place-at X Y Z --down X Y Z [--on L ...] [--lift N] [--any-stability] [--turns K]) [--rest keep|drop]
            --transform T [--extents X Y Z] [--grid-dim 256] [--level 0.45] [--connectivity {6,26}] [--dilate 1] --out DIR
@@ -37,7 +37,15 @@ of the offsets where it rests on an object (of a label among --on, when given), 
 the network-frame point --place-at across the down axis, and stands (its centre over the hull of its support; --any-stability:
 the nearest, standing or not), is rendered and meshed as --until-contact's is.  The record gains place {offset, drop, support,
 stable, contacts}.  --turns K (DESIGN.md, "Turned placements") also turns the piece about down by 360 k / K degrees and picks the
-nearest placement over every turn that fits the grid; the record's place gains turn, the angle in degrees of the one chosen."""
+nearest placement over every turn that fits the grid; the record's place gains turn, the angle in degrees of the one chosen.
+
+Arranging (DESIGN.md, "Arranging objects"): --arrange SPEC.json --down X Y Z replaces --move-label / --move-piece and places
+several objects one after another, each in the scene the earlier placements leave (objects.arrange_objects).  SPEC is a list of
+{"label": L | "piece": ID, "near": [x, y, z], "on": [...], "turns": K, "rest": "keep" | "drop", "any_stability": bool}: "label"
+moves the label's largest piece and "piece" that component, each with its region grown by --dilate voxels, as the single-move
+flags do.  The frame is rendered with every placed move (manipulate_frame), --mesh meshes the same moves (edited_mesh), and the
+record gains arrange: per item label, placed, reason, offset, drop, support, stable and turn, and each placed move's overwritten
+(the solid voxels of the scene left before it that it landed on, per label)."""
 import argparse
 import json
 import os
@@ -58,6 +66,7 @@ def parse(argv=None):
     which = ap.add_mutually_exclusive_group(required=True)
     which.add_argument("--move-label", type=int, metavar="L", help="move the largest piece of object label L")
     which.add_argument("--move-piece", type=int, metavar="ID", help="move this piece (a component id of the sweep)")
+    which.add_argument("--arrange", metavar="SPEC.json", help="place several pieces one after another (a JSON list of items)")
     ap.add_argument("--mode", choices=("translation", "rotation", "scale", "multi"))
     ap.add_argument("--distance", type=float, default=None, help="translation along y (default -0.25)")
     ap.add_argument("--yaw", type=float, default=None, help="rotation about z, degrees (default 90)")
@@ -91,7 +100,19 @@ def parse(argv=None):
     ap.add_argument("--step", type=float, default=None, help="--until-contact: the slide's step (default: one grid spacing)")
     ap.add_argument("--tolerance", type=int, default=0, help="--until-contact: overlapping voxels tolerated")
     a = ap.parse_args(argv)
-    if a.place_at is not None:
+    if a.arrange is not None:
+        for flag, given in (("--place-at", a.place_at is not None), ("--mode", a.mode is not None),
+                            ("--until-contact", a.until_contact), ("--distance", a.distance is not None), ("--yaw", a.yaw is not None),
+                            ("--scale", a.scale is not None), ("--turns", a.turns is not None), ("--check", a.check)):
+            if given:
+                ap.error("--arrange cannot be combined with %s (each item gives its own placement; the record reports what "
+                         "each placed move overwrote)" % flag)
+        if a.down is None or not any(a.down):
+            ap.error("--arrange needs --down X Y Z, not 0 0 0")
+        if a.on is not None or a.lift is not None or a.any_stability:
+            ap.error("--on, --lift and --any-stability are per item with --arrange")
+        a.lift, a.turns = 0, 1
+    elif a.place_at is not None:
         for flag, given in (("--mode", a.mode is not None), ("--until-contact", a.until_contact), ("--distance", a.distance is not None),
                             ("--yaw", a.yaw is not None), ("--scale", a.scale is not None)):
             if given:
@@ -130,6 +151,68 @@ def parse(argv=None):
     a.H, a.W = int(a.hwk[0]), int(a.hwk[1])
     a.K = (np.load(a.hwk[2]) if len(a.hwk) == 3 else np.array([float(v) for v in a.hwk[2:]])).astype(np.float32).reshape(3, 3)
     return a
+
+
+ITEM_KEYS = ("label", "piece", "near", "on", "turns", "rest", "any_stability")
+
+
+def read_spec(path):
+    """--arrange's SPEC -> [item dict]; SystemExit for a malformed one."""
+    with open(path) as fh:
+        spec = json.load(fh)
+    if not isinstance(spec, list) or not spec:
+        raise SystemExit("move_objects: %s must hold a non-empty JSON list of items" % path)
+    for i, it in enumerate(spec):
+        if not isinstance(it, dict) or set(it) - set(ITEM_KEYS) or ("label" in it) == ("piece" in it) or "near" not in it:
+            raise SystemExit("move_objects: item %d of %s needs exactly one of label / piece, near, and only the keys %s"
+                             % (i, path, ", ".join(ITEM_KEYS)))
+    return spec
+
+
+def choose_pieces(a, model_fine, T, ext, spec):
+    """choose_piece for every item of --arrange -> [(component id, label, Region)] (one sweep and one split)."""
+    import torch
+    from dmnerf_b200.objects import component_region, largest_components, object_components, object_mask, occupancy_objects
+    ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
+    with torch.no_grad():
+        occ, labels = occupancy_objects(model_fine, T, object_mask(ins_num, keep=range(ins_num)), a.grid_dim, ext, a.near, a.far,
+                                        a.N_importance, device=next(model_fine.parameters()).device)
+        cc = object_components(occ, labels, a.level, a.connectivity)
+    del occ, labels
+    best = largest_components(cc["label"], cc["voxels"])
+    out = []
+    for it in spec:
+        if "piece" in it:
+            piece = int(it["piece"])
+            if not 0 <= piece < len(cc["label"]):
+                raise SystemExit("move_objects: piece %d does not exist (the sweep has %d pieces)" % (piece, len(cc["label"])))
+        else:
+            if int(it["label"]) not in best or int(it["label"]) >= ins_num:
+                raise SystemExit("move_objects: object label %d has no piece in the sweep" % int(it["label"]))
+            piece = best[int(it["label"])]
+        out.append((piece, int(cc["label"][piece]), component_region(cc, [piece], T, ext, dilate=a.dilate, connectivity=a.connectivity)))
+    return out
+
+
+def arrange_pieces(a, occ, labels, T, ext, spec, chosen):
+    """--arrange: arrange_objects for the items -> (moves, regions, rests, the record's arrange)."""
+    from dmnerf_b200.objects import arrange_objects
+    items = []
+    for it, (_, label, region) in zip(spec, chosen):
+        items.append({"label": label, "near": it["near"], "on": it.get("on"), "piece": region, "rest": it.get("rest", "keep"),
+                      "turns": it.get("turns"), "stable": not it.get("any_stability", False)})
+    r = arrange_objects(occ, labels, T, items, a.down, ext, a.level)
+    rec, report = [], iter(r["report"])
+    for (piece, label, _), res in zip(chosen, r["items"]):
+        p = res["placement"]
+        entry = {"label": label, "piece": piece, "placed": p is not None, "reason": res.get("reason"),
+                 "offset": None if p is None else list(p["offset"]), "drop": None if p is None else p["drop"],
+                 "support": None if p is None else p["support"], "stable": None if p is None else p["stable"],
+                 "turn": res.get("turn")}
+        if p is not None:
+            entry["overwritten"] = {str(k): v for k, v in next(report)["overwritten"].items()}
+        rec.append(entry)
+    return r["moves"], r["pieces"], r["rest"], rec
 
 
 def choose_piece(a, model_fine, T, ext):
@@ -207,9 +290,14 @@ def main(argv=None):
     c2w[:pose.shape[0]] = pose[:4]
     T = np.load(a.transform) if a.transform.endswith(".npy") else np.loadtxt(a.transform)
     T, ext = M.check_transform(np.asarray(T, dtype=np.float64).reshape(4, 4)), tuple(a.extents)
-    piece, label, centre, region = choose_piece(a, nets[1], T, ext)
-    slide = place = None
-    if a.check or a.until_contact or a.place_at is not None:
+    slide = place = arranged = None
+    if a.arrange is not None:
+        spec = read_spec(a.arrange)
+        chosen = choose_pieces(a, nets[1], T, ext, spec)
+        piece, label, centre, region = None, None, None, None
+    else:
+        piece, label, centre, region = choose_piece(a, nets[1], T, ext)
+    if a.check or a.until_contact or a.place_at is not None or a.arrange is not None:
         from dmnerf_b200.objects import object_mask, occupancy_objects
         with torch.no_grad():
             occ, labels = occupancy_objects(nets[1], T, object_mask(ins_num, remove=[]), a.grid_dim, ext, a.near, a.far,
@@ -217,28 +305,39 @@ def main(argv=None):
     if a.until_contact:
         slide = slide_translation(a, occ, labels, T, ext, label, region)
         a.distance = np.sign(a.distance) * (slide["found"] or 0.0)
-    if a.place_at is not None:
+    if a.arrange is not None:
+        moves, regions, rests, arranged = arrange_pieces(a, occ, labels, T, ext, spec, chosen)
+        if not moves:
+            raise SystemExit("move_objects: no item was placed: %s" % "; ".join("%d: %s" % (e["label"], e["reason"]) for e in arranged))
+        trans = {"transformations": [{"transformation": m, "mode": "placement"} for _, m in moves]}
+    elif a.place_at is not None:
         place = place_piece(a, occ, labels, T, ext, label, region)
         trans = {"transformations": [{"transformation": place.pop("transformation"), "mode": "placement"}]}
     else:
         trans = manipulation_transform(centre, a.mode, distance=a.distance, yaw=a.yaw, scale=a.scale)
+    if a.arrange is None:
+        moves, regions, rests = [(label, trans["transformations"][0]["transformation"])], [region], [a.rest]
     dev = next(nets[1].parameters()).device
     pose_t = torch.from_numpy(c2w).to(dev)
-    tar_o, tar_d = rigid_rays(a.H, a.W, a.K, trans["transformations"][0]["transformation"], pose_t)
+    rays = [rigid_rays(a.H, a.W, a.K, m, pose_t) for _, m in moves]
+    tar_o, tar_d = torch.stack([o for o, _ in rays]), torch.stack([d for _, d in rays])
     args = types.SimpleNamespace(N_test=a.N_test, N_samples=a.N_samples, N_importance=a.N_importance, near=a.near, far=a.far,
-                                 target_labels=[label])
+                                 target_labels=[k for k, _ in moves])
     pe, _ = get_embedder(10)
     ve, _ = get_embedder(4)
-    rgb, ins, _, _ = manipulate_frame(a.H, a.W, a.K, pose_t, tar_o[None], tar_d[None], pe, ve, nets[0], nets[1], args,
-                                      pieces=[region], rest=a.rest)
+    rgb, ins, _, _ = manipulate_frame(a.H, a.W, a.K, pose_t, tar_o, tar_d, pe, ve, nets[0], nets[1], args, pieces=regions,
+                                      rest=rests)
     os.makedirs(a.out, exist_ok=True)
     write_png(os.path.join(a.out, "rgb.png"), (255 * torch.clamp(rgb, 0, 1)).to(torch.uint8).reshape(a.H, a.W, 3).cpu().numpy())
     ins_rgbs = np.random.default_rng(0).integers(0, 256, (ins_num + 1, 3))
     lut = pred_label_lut({str(k): k for k in range(ins_num + 1)}, ins_rgbs, {str(k): k for k in range(ins_num + 1)},
                          ins_num + 1)[:, ::-1]
     write_png(os.path.join(a.out, "instance.png"), colorize(argmax_rows(ins).reshape(a.H, a.W), lut).cpu().numpy())
-    record = {"transformations": trans["transformations"], "label": label, "piece": piece, "centre": centre.tolist(),
-              "rest": a.rest}
+    if a.arrange is not None:
+        record = {"transformations": trans["transformations"], "labels": [k for k, _ in moves], "rest": rests, "arrange": arranged}
+    else:
+        record = {"transformations": trans["transformations"], "label": label, "piece": piece, "centre": centre.tolist(),
+                  "rest": a.rest}
     if slide is not None:
         record["slide"] = slide
     if place is not None:
@@ -250,12 +349,12 @@ def main(argv=None):
         record["overlap"] = {"voxels": {str(k): v for k, v in r["overlap"].items()},
                              "volume": {str(k): v for k, v in r["overlap_volume"].items()}}
         record["landed"] = r["landed"]
-    if a.check or a.until_contact or a.place_at is not None:
+    if a.check or a.until_contact or a.place_at is not None or a.arrange is not None:
         del occ, labels
     if a.mesh:
         from dmnerf_b200.objects import edited_mesh
-        m = edited_mesh(nets[1], T, [(label, trans["transformations"][0]["transformation"])], a.grid_dim, ext, a.level, a.near,
-                        a.far, a.N_importance, pieces=[region], rest=a.rest, min_cluster=a.min_cluster)
+        m = edited_mesh(nets[1], T, moves, a.grid_dim, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests,
+                        min_cluster=a.min_cluster)
         M.write_ply(os.path.join(a.out, "edited.ply"), m["vertices"], m["triangles"])
         lab = m["labels"].cpu().numpy()
         colors = np.where((lab >= 0)[:, None], lut[np.clip(lab, 0, ins_num)], 0).astype(np.uint8)   # instance.png's colours

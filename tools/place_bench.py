@@ -13,8 +13,11 @@ identity rotation used here, the case where the column pass reads each column co
 centre and tests at most 64 offsets for stability.  The turned cases (DESIGN.md, "Turned placements") time, at lift 0, for the
 label with the most points and for its piece inside an index cube of side grid_dim / 4 around its centre (a small object with
 many offsets), placement_map against turned_placement_maps of 8 and of 36 turns and place_object(turns=8), with the 8-turn
-call's stage split (torch.profiler) and its number of column-pass launches.  The calls are timed alternately (_harness.alternate, CUDA events, one
-warm-up round); each ends in its read-back.  Nothing is written to disk."""
+call's stage split (torch.profiler) and its number of column-pass launches.  The arrangement cases (DESIGN.md, "Arranging
+objects") time, against the sweep, edited_grid with 1 and with 8 moves (whole-voxel shifts of the labels with the most points) and
+arrange_objects of 4 small pieces (each label's piece inside an index cube of side grid_dim / 4, as above) with turns=4, aimed at
+four points around the grid's centre.  The calls are timed alternately (_harness.alternate, CUDA events, one warm-up round); each
+ends in its read-back.  Nothing is written to disk."""
 import argparse
 import json
 
@@ -96,6 +99,29 @@ def turned_cases(occ, lab, T, dim, level, label, near, reps, what, piece=None):
     return case
 
 
+def arrange_cases(nf, keep_all, occ, lab, T, dim, level, reps, dev):
+    """edited_grid of 1 and 8 moves and arrange_objects of 4 small pieces with turns=4, alternated with the sweep."""
+    A, b = OB.grid_affine(T, dim, EXT)
+    k, c = torch.unique(lab[occ > level], return_counts=True)
+    labels = [int(x) for x in k[torch.argsort(c, descending=True)][:8]]
+    moves = [(x, OB._translate(A @ np.array([(i % 3) - 1.0, 2.0, (i % 2) * 3.0]))) for i, x in enumerate(labels)]
+    pieces = [_small_piece(occ, lab, T, dim, level, x) for x in labels[:4]]
+    aims = [A @ np.array([dim / 2.0 + di, dim / 2.0, dim / 2.0 + dk]) + b for di, dk in ((-32, -32), (-32, 32), (32, -32), (32, 32))]
+    items = [{"label": x, "near": y, "piece": pc, "turns": 4} for x, y, pc in zip(labels[:4], aims, pieces)]
+    variants = {
+        "sweep": lambda: OB.occupancy_objects(nf, T, keep_all, dim, EXT, NEAR, FAR, N_IMPORTANCE, device=dev),
+        "edited_grid_1": lambda: OB.edited_grid(occ, lab, T, moves[:1], EXT, level),
+        "edited_grid_8": lambda: OB.edited_grid(occ, lab, T, moves, EXT, level),
+        "arrange_objects_4": lambda: OB.arrange_objects(occ, lab, T, items, DOWN, EXT, level),
+    }
+    ms = alternate(variants, reps)
+    r = OB.arrange_objects(occ, lab, T, items, DOWN, EXT, level)
+    return {"labels": labels, "level": level, "moves": len(moves),
+            "arrange": [{"label": it["label"], "placed": it["placement"] is not None, "tested": it.get("tested"),
+                         "turn": it.get("turn")} for it in r["items"]],
+            **{k + "_ms": _stats(v) for k, v in ms.items()}}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--grid-dim", type=int, default=256)
@@ -107,7 +133,7 @@ def main():
     T[:3, 3] = (0.1, -0.2, 0.3)
     A, b = OB.grid_affine(T, dim, EXT)
     near = A @ np.full(3, (dim - 1) / 2.0) + b
-    cases, turned = [], []
+    cases, turned, arranged = [], [], []
     for ins_num in (13, 93):
         _, nf, _, _ = make_models(101, 202, ins_num, dev, trained_like=True)
         keep_all = OB.object_mask(ins_num, remove=[])
@@ -147,10 +173,11 @@ def main():
             piece = _small_piece(occ, lab, T, dim, level, label)
             turned.append(dict(turned_cases(occ, lab, T, dim, level, label, near, a.reps, "piece in a cube of side dim / 4", piece),
                                ins_num=ins_num))
+            arranged.append(dict(arrange_cases(nf, keep_all, occ, lab, T, dim, level, a.reps, dev), ins_num=ins_num))
         del occ, lab
     name, smi, _ = gpu_identity(dev)
     print(json.dumps({"metric": "placement device time", "grid_dim": dim, "reps": a.reps, "down": DOWN, "cases": cases,
-                      "turned": turned, "gpu": smi,
+                      "turned": turned, "arrange": arranged, "gpu": smi,
                       "gpu_name": name,
                       "what": "keep-all labelled sweep, placement_map (stages: torch.profiler kernel times of one call each), "
                               "place_object (at most 64 stability tests); synthetic trained-like networks; CUDA events, "
