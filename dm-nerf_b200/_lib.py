@@ -70,6 +70,12 @@ class EditMove(C.Structure):
                 ("piece", RegionDesc)]
 
 
+class RenderMoves(C.Structure):
+    """Mirror of `struct dmnerf_render_moves` (objects.render_moves builds one)."""
+    _fields_ = [("moves", C.POINTER(EditMove)), ("n_moves", C.c_int32), ("dim", C.c_int32), ("transform", C.c_double * 16),
+                ("extents", C.c_double * 3), ("level", C.c_float), ("voxel", C.c_float)]
+
+
 class Placement(C.Structure):
     """Mirror of `struct dmnerf_placement` (objects.placement_map builds one)."""
     _fields_ = [("piece", RegionDesc), ("obstacles", C.c_uint32 * 4), ("label", C.c_int32), ("rest_drop", C.c_int32),
@@ -164,6 +170,8 @@ PROTOTYPES = {
     "dmnerf_mesh_occupancy_edit": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_float,
                                              C.c_float, C.c_int64, C.POINTER(EditMove), C.c_int, _f32p, C.c_void_p,
                                              C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_render_moved": (C.c_int, [C.c_void_p, C.POINTER(RenderIO), C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.POINTER(RenderMoves), C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_mesh_vertex_labels": (C.c_int, [_f32p, C.c_int64, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "dmnerf_object_voxels": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_int32),
                                        C.POINTER(C.c_int64), C.POINTER(C.c_uint32), C.c_void_p]),

@@ -50,6 +50,7 @@ struct dmnerf_ctx {
   DeviceBuffer mesh_pts, mesh_raw;   // one slab of the occupancy sweep: points + zero view directions, network output
   DeviceBuffer gemm_wimage, gemm_partial;   // dmnerf_mlp_backward: scratch of the tensor-core GEMMs (gemm_umma.cu)
   MeshState mesh;                 // buffers of the other mesh entry points (mesh.cu)
+  MovesState moves;               // buffers of the moved render (render_moves.cu)
   InventoryState inventory;       // buffers of the object-inventory entry points (inventory.cu)
   ComponentsState components;     // buffers of the connected-component entry points (components.cu)
   PlaceState place;               // buffers of the placement entry points (place.cu)
@@ -418,10 +419,18 @@ DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, 
 
 }  // extern "C"
 
+// The checked moves of dmnerf_render_moved and the targets each pass evaluated.
+struct RenderMoves {
+  const EditMove* moves;
+  int n;
+  float voxel, level;
+  int64_t evaluated[2];
+};
+
 // dm_nerf() on device buffers with the bound pair (bound_pair); edit: the checked scene edit, or NULL for none (the
-// unselected kernels)
+// unselected kernels); mv: moves applied to each pass's raw after its network (the stage path), or NULL for none
 static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
-                               const Edit* edit, void* stream) {
+                               const Edit* edit, void* stream, RenderMoves* mv = nullptr) {
   DMN_CHECK(io, "render_forward: io is NULL");
   DMN_CHECK(n >= 0 && S >= 3 && NI >= 2, "render_forward: bad sizes n=%lld S=%d I=%d", (long long)n, S, NI);
   if (n == 0) return 0;
@@ -436,7 +445,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   if (resolve_impl(ctx, impl, 0, 1, st, "render_forward")) return 1;
 
   // ---- fully fused path: one launch, no intermediate tensor in HBM
-  if (impl != DMNERF_IMPL_SIMT && S == 64 && NI == 128 && !io->raw_coarse && !io->raw_fine) {
+  if (impl != DMNERF_IMPL_SIMT && S == 64 && NI == 128 && !io->raw_coarse && !io->raw_fine && !mv) {
     const bool prof = ctx->profiling;
     if (prof) DMN_CUDA(cudaEventRecord(ctx->ev[0], st));
     int rc = launch_render_tc(ctx->net[0], ctx->net[1], io, n, flags, st, edit, impl == DMNERF_IMPL_UMMA_F16);
@@ -468,6 +477,9 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:49-61  points, embeddings, coarse network
   if ((rc = mlp_dispatch(ctx, 0, nullptr, io->rays_o, io->rays_d, z_c, n * S, S, raw_c, impl, st))) return rc;
+  if (mv && (rc = render_moves_pass(ctx->moves, ctx->net[0], impl == DMNERF_IMPL_UMMA_F16, mv->moves, mv->n, io->rays_o, io->rays_d,
+                                    z_c, n, S, C, mv->voxel, mv->level, raw_c, &mv->evaluated[0], st)))
+    return rc;
   DMN_STAGE_MARK();
   // render.py:63     coarse composite
   if ((rc = launch_composite(raw_c, z_c, io->rays_d, n, S, C, keep_ins, io->rgb_coarse, w_c, io->depth_coarse,
@@ -478,6 +490,9 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:71-82  fine network on all S+I depths
   if ((rc = mlp_dispatch(ctx, 1, nullptr, io->rays_o, io->rays_d, z_f, n * F, F, raw_f, impl, st))) return rc;
+  if (mv && (rc = render_moves_pass(ctx->moves, ctx->net[1], impl == DMNERF_IMPL_UMMA_F16, mv->moves, mv->n, io->rays_o, io->rays_d,
+                                    z_f, n, F, C, mv->voxel, mv->level, raw_f, &mv->evaluated[1], st)))
+    return rc;
   DMN_STAGE_MARK();
   // render.py:86     fine composite
   if ((rc = launch_composite(raw_f, z_f, io->rays_d, n, F, C, keep_ins, io->rgb_fine, io->weights_fine, io->depth_fine,
@@ -498,6 +513,35 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
   const Edit* edit;
   if (int rc = scene_edit(ctx, io ? io->edit : nullptr, (cudaStream_t)stream, e, edit, "render_forward")) return rc;
   return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, edit, stream), impl, stream);
+}
+
+DMNERF_API int dmnerf_render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                   const dmnerf_render_moves* moves, int64_t* evaluated_host, void* stream) {
+  const char* who = "render_moved";
+  if (evaluated_host) evaluated_host[0] = evaluated_host[1] = 0;
+  if (bound_pair(ctx, who)) return 1;
+  DMN_CHECK(!(flags & ~RENDER_FLAGS), "%s: unknown flag bits 0x%x", who, flags & ~RENDER_FLAGS);
+  DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA_F16, "%s: unknown impl %d", who, impl);
+  DMN_CHECK(impl != DMNERF_IMPL_SIMT, "%s: the moved targets run in the network's points mode, which the tensor-core kernels "
+            "alone provide (DMNERF_IMPL_UMMA or DMNERF_IMPL_UMMA_F16), not DMNERF_IMPL_SIMT", who);
+  DMN_CHECK(moves != nullptr, "%s: moves is NULL", who);
+  DMN_CHECK(moves->n_moves >= 1 && moves->n_moves <= DMNERF_MAX_MOVES, "%s: between 1 and %d moves are supported, got %d", who,
+            DMNERF_MAX_MOVES, moves->n_moves);
+  DMN_CHECK(moves->moves != nullptr, "%s: moves->moves is NULL", who);
+  if (sweep_grid_check(moves->transform, moves->extents, moves->dim, moves->level, who)) return 1;
+  DMN_CHECK(std::isfinite(moves->voxel) && moves->voxel > 0.0f, "%s: voxel %g must be finite and > 0", who, (double)moves->voxel);
+  DMN_CHECK(n >= 0 && S >= 3 && NI >= 2, "%s: bad sizes n=%lld S=%d I=%d", who, (long long)n, S, NI);
+  DMN_CHECK(n * (int64_t)(S + NI) < ((int64_t)1 << 31), "%s: %lld rays of %d samples reach 2^31 samples", who, (long long)n, S + NI);
+  EditMove mv[DMNERF_MAX_MOVES];
+  for (int i = 0; i < moves->n_moves; ++i)
+    if (edit_move_from_abi(moves->moves[i], moves->transform, moves->extents, moves->dim, ctx->net[0].p.ins_num, mv[i], who, i)) return 1;
+  Edit e;
+  const Edit* edit;
+  if (int rc = scene_edit(ctx, io ? io->edit : nullptr, (cudaStream_t)stream, e, edit, who)) return rc;
+  RenderMoves r = {mv, moves->n_moves, moves->voxel, moves->level, {0, 0}};
+  const int rc = f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, edit, stream, &r), impl, stream);
+  if (evaluated_host && !rc) { evaluated_host[0] = r.evaluated[0]; evaluated_host[1] = r.evaluated[1]; }
+  return rc;
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {

@@ -319,6 +319,20 @@ int launch_vertex_labels(const float* v, int64_t n, const float* occ, const int1
 // The region of a move (bits NULL: none), checked: dim and map, the moved label among the labels it applies to (exchanger.cu).
 int piece_region(const dmnerf_region& d, int mv, Region& r, const char* who, int i);
 
+// Rendering moved objects per sample (render_moves.cu; DESIGN.md, "Rendering moved objects").  Per-context device buffers of one
+// pass and move: the targets and view directions of every sample, the in-box flags and their scan, the boxed targets compacted,
+// the network's rows at them and the count read back.
+struct MovesState {
+  DeviceBuffer tgt, flag, pin, pos, temp, pts, raw, total;
+};
+struct Network;
+// The moves applied in order, in place, to the raw rows raw [n * s, c] of one pass of a stage render (samples o + d z, z [n, s]),
+// the targets run through `net` (fp16 preview network when f16); *evaluated += the targets evaluated.  One device->host read of
+// the count per move (synchronises).
+int render_moves_pass(MovesState& s, const Network& net, bool f16, const EditMove* moves, int n_moves, const float* rays_o,
+                      const float* rays_d, const float* z, int64_t n, int s_per_ray, int c, float voxel, float level, float* raw,
+                      int64_t* evaluated, cudaStream_t st);
+
 // Object inventory (inventory.cu): per-group integer statistics and fp64 spans of the solid points of a labelled grid.
 // Per-context device buffers: everything a call reads back (status word first), and its inputs.
 struct InventoryState {

@@ -147,12 +147,7 @@ int launch_grid_points(const double* T16, const double* ext3, int dim, int64_t b
   return 0;
 }
 
-// mesh_generator.py:51-62: occ = 1 - exp(-relu(sigma) * voxel), sigma = channel 3 of the network output [n, c]
-__device__ __forceinline__ float occupancy_of(float a, float voxel) {
-  const float r = a > 0.f ? a : (a != a ? a : 0.f);           // torch.relu keeps NaN
-  return __fsub_rn(1.0f, expf(__fmul_rn(-r, voxel)));
-}
-
+// occupancy_of: sweep_grid.cuh
 __global__ void occupancy_kernel(const float* __restrict__ raw, int64_t n, int c, float voxel, float* __restrict__ occ) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;

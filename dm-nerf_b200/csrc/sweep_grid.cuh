@@ -1,6 +1,6 @@
 // The occupancy sweep's grid as the device sees it (DESIGN.md, "Mesh extraction" and "Meshing an edited scene"): its fp32 grid
-// points, and the target and nearest grid index of a point under a move.  Shared by the edited sweep (mesh.cu) and the collision
-// checks (collide.cu), so that both take the same decisions.
+// points, and the target and nearest grid index of a point under a move.  Shared by the edited sweep (mesh.cu), the collision
+// checks (collide.cu) and the moved render (render_moves.cu), so that all take the same decisions.
 #pragma once
 #include "common.cuh"
 
@@ -69,6 +69,19 @@ __device__ __forceinline__ bool edit_target(const double* trans, const double* i
     in = in && q[a] >= lo[a] && q[a] <= hi[a];
   }
   return in;
+}
+
+// mesh_generator.py:51-62: occ = 1 - exp(-relu(sigma) * voxel), sigma = channel 3 of the network output [n, c]
+__device__ __forceinline__ float occupancy_of(float a, float voxel) {
+  const float r = a > 0.f ? a : (a != a ? a : 0.f);           // torch.relu keeps NaN
+  return __fsub_rn(1.0f, expf(__fmul_rn(-r, voxel)));
+}
+
+// The take test of a move of `label` (piece aside): the target (lt, ot) is that label, and it is solid or the point it replaces
+// (occupancy o) is not.  The moved render (render_moves.cu) calls it; edit_rule below spells the same expression out, because
+// calling it there reorders the SASS of the edited sweep's and the grid-only edit's kernels.
+__device__ __forceinline__ bool edit_takes(int lt, float ot, int label, float o, float level) {
+  return lt == label && (ot > level || o <= level);
 }
 
 // The edit rule at one grid point p (DESIGN.md, "Meshing an edited scene"), shared by the edited sweep (the network at the

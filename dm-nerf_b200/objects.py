@@ -24,6 +24,9 @@
                                                         -> where a lowered object comes to rest, on what, and whether it stands
     edited_grid(occ, labels, scene_transform, moves, ...) / arrange_objects(occ, labels, scene_transform, items, down, ...)
                                                         -> moves applied to the sweep alone, and several objects placed in turn
+    render_moves(occ, labels, scene_transform, moves, ...)
+                                                        -> moves for render_rays(moves=) / render_frame(moves=): the edited
+                                                           sweep's rule applied per render sample
 
 Every network sample is labelled argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the
 exchanger's rule); a sample whose label is not kept has alpha = 0 in the composite of both passes, so the coarse weights of the
@@ -398,6 +401,66 @@ def edited_mesh(model_fine, scene_transform, moves, grid_dim=256, extents=None, 
             objects = [k for k in torch.unique(labels[occ > level]).cpu().tolist() if k != ins_num]
             out["objects"] = meshes_from_labelled_grid(occ, labels, T, objects, level, ext, min_cluster)
     return out
+
+
+# ----------------------------------------------------------------------------------------------------------------- moved renders
+# DESIGN.md, "Rendering moved objects": edited_sweep's moves applied per render sample, inside the stage render, so that a render
+# and a mesh of one edit agree.  render_rays(moves=) and render_frame(moves=) take the value render_moves returns.
+class MovedScene:
+    """Checked moves for render_rays(moves=) / render_frame(moves=): the dmnerf_render_moves the library reads, and the move
+    descriptions and region bits it points into, held for as long as the value lives.  Immutable."""
+    __slots__ = ("_desc", "_held", "device", "labels", "boxes", "rest_drop", "level", "voxel")
+
+    def __init__(self, desc, held, device, labels, boxes, rest_drop, level, voxel):
+        for k, v in zip(self.__slots__, (desc, held, device, labels, tuple(map(tuple, boxes.tolist())), tuple(rest_drop), level,
+                                         voxel)):
+            object.__setattr__(self, k, v)
+
+    def __setattr__(self, key, value):
+        raise AttributeError("MovedScene is immutable")
+
+    def abi(self):
+        """The dmnerf_render_moves of these moves."""
+        return self._desc
+
+
+def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128, margin=2,
+                 boxes=None, pieces=None, rest="keep"):
+    """The moves [(label, 4x4 in the network frame)] of edited_sweep, checked for the moved render -> a MovedScene.  occ / labels:
+    the unedited keep-all sweep ([dim]^3 float32 / int16 on the device) that the default boxes come from (edit_boxes, as
+    edited_sweep) and whose grid (scene_transform, extents, dim) the boxes index.  level, margin, boxes, pieces, rest: as
+    edited_sweep; the voxel of the occupancy test is the sweep's (far - near) / N_importance.  moves, pieces and rest may be
+    arrange_objects' moves, pieces and rest unchanged, or manipulator_eval's [(label, 4x4)].  Labels are checked against the
+    networks when the render runs."""
+    from .manipulator import move_pieces, move_rests
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    ext = EXTENTS if extents is None else extents
+    mv, mats = _check_moves(moves, MAX_LABELS - 1)
+    if not mv:
+        raise ValueError("render_moves: give between 1 and %d moves" % _lib.MAX_MOVES)
+    level = _check_level(level)
+    drops = move_rests(rest, len(mv))
+    if int(margin) != margin or int(margin) < 0:
+        raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
+    with np.errstate(divide="ignore", invalid="ignore"):
+        voxel = np.float32(np.float64(far - near) / np.float64(N_importance))
+    if not (np.isfinite(voxel) and voxel > 0):
+        raise ValueError("render_moves: the voxel (far - near) / N_importance = %r must be finite and > 0" % (float(voxel),))
+    if boxes is not None:
+        boxes = _check_boxes(boxes, len(mv), occ.shape[0])
+    regions = move_pieces(pieces, mv, MAX_LABELS - 1, occ.device) or [None] * len(mv)
+    dim = _check_sweep(occ, labels, "render_moves")
+    if boxes is None:
+        boxes = _check_boxes(edit_boxes(occ, labels, moves, T, ext, level, margin, pieces), len(mv), dim)
+    descs = _edit_moves(mv, mats, boxes, drops, regions, occ.device)
+    d = _lib.RenderMoves()
+    d.moves, d.n_moves, d.dim = C.cast(descs, C.POINTER(_lib.EditMove)), len(mv), dim
+    d.transform[:] = np.asarray(T, dtype=np.float64).reshape(-1).tolist()
+    d.extents[:] = np.asarray(ext, dtype=np.float64).reshape(-1).tolist()
+    d.level, d.voxel = level, float(voxel)
+    return MovedScene(d, (descs, [r.bits for r in regions if r is not None]), occ.device, tuple(mv), boxes, drops, level,
+                      float(voxel))
 
 
 # ----------------------------------------------------------------------------------------------------------------- collisions

@@ -116,7 +116,7 @@ def _check_embedders(position_embedder, view_embedder):
 
 def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb=0.0, N_importance=128,
                 t_rand=None, u=None, want_raw=True, want_coarse=True, want_samples=None, keep_all_ins=False,
-                impl=_lib.IMPL_AUTO, keep_objects=None, region=None, appearance=None):
+                impl=_lib.IMPL_AUTO, keep_objects=None, region=None, appearance=None, moves=None):
     """Whole per-ray pipeline on the device.  Returns the reference's dict keys plus acc / weights maps.
     want_raw: per-sample network outputs raw_* (forces the stage-by-stage kernels); want_samples: per-sample depths and
     weights (z_vals_*, weights_*; default = want_raw); want_coarse: the coarse pass' maps.  With want_raw=False and
@@ -126,7 +126,11 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     region: an objects.Region; samples it drops get alpha = 0 in both passes as well (DESIGN.md, "Region selection").
     appearance: an objects.Appearance; every sample the selection and the region keep has its label's density scale and colour
     map applied in both passes (DESIGN.md, "Object appearance").  Inference only.
-    impl: _lib.IMPL_UMMA_F16 runs the fp16 preview network (DESIGN.md section 10); IMPL_AUTO follows DMNERF_INFER_IMPL."""
+    impl: _lib.IMPL_UMMA_F16 runs the fp16 preview network (DESIGN.md section 10); IMPL_AUTO follows DMNERF_INFER_IMPL.
+    moves: an objects.MovedScene (objects.render_moves): the moves applied per sample to each pass's network output before its
+    composite, by the edited sweep's rule (DESIGN.md, "Rendering moved objects"), always on the stage kernels; raw_* are the edited
+    rows and the result gains evaluated = (coarse, fine) targets.  Composes with keep_objects, region and appearance.  Inference
+    only; not with _lib.IMPL_SIMT."""
     impl = _lib.infer_impl(impl)
     if want_samples is None:
         want_samples = want_raw
@@ -136,11 +140,13 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
     ctx = get_context(dev)
     ins_num = bind_pair(ctx, model_coarse, model_fine)
     edit, held = scene_edit("render_rays", ins_num, dev, model_coarse, model_fine, keep_objects, region, appearance)
+    if moves is not None:
+        _check_moved(moves, "render_rays", dev, model_coarse, model_fine)
     rays_o = rays_o.reshape(-1, 3).contiguous().float()
     rays_d = rays_d.reshape(-1, 3).contiguous().float()
     n = rays_o.shape[0]
     S = z_vals_coarse.shape[-1]
-    F, C = S + N_importance, 4 + ins_num + 1
+    F, ch = S + N_importance, 4 + ins_num + 1
     z_in, z_stride = coarse_depths(z_vals_coarse, n)
     t_rand, u = reference_draws(perturb, n, S, N_importance, dev, t_rand, u)
     flags = _lib.FLAG_PERTURB if perturb > 0.0 else 0
@@ -158,15 +164,34 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
         if want_samples or want_raw:
             out["weights_coarse"] = e(n, S)
     if want_raw:
-        out.update({"raw_fine": e(n, F, C), "raw_coarse": e(n, S, C)})
+        out.update({"raw_fine": e(n, F, ch), "raw_coarse": e(n, S, ch)})
     io = _lib.RenderIO()
     io.rays_o, io.rays_d, io.z_coarse, io.z_row_stride = _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(z_in), z_stride
     io.t_rand, io.u = _lib.ptr(t_rand), _lib.ptr(u)
     for k, v in out.items():
         setattr(io, k, _lib.ptr(v))
     io.edit = edit
-    ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags, impl)
+    if moves is None:
+        ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags, impl)
+        return out
+    evaluated = (C.c_int64 * 2)()
+    ctx.call("dmnerf_render_moved", ctx.handle, io, n, S, N_importance, flags, impl, C.byref(moves.abi()), evaluated)
+    out["evaluated"] = (int(evaluated[0]), int(evaluated[1]))
     return out
+
+
+def _check_moved(moves, who, device, model_coarse, model_fine):
+    """ValueError unless `moves` is an objects.MovedScene built on `device`; RuntimeError when the networks would record
+    gradients (a moved render is inference-only)."""
+    from .autograd import _needs_grad
+    from .objects import MovedScene
+    if not isinstance(moves, MovedScene):
+        raise ValueError("%s: moves must be an objects.render_moves(...) result, got %r" % (who, type(moves).__name__))
+    if moves.device != torch.device(device):
+        raise ValueError("%s: the moves were built on %s, the render runs on %s" % (who, moves.device, device))
+    if _needs_grad(model_coarse, model_fine):
+        raise RuntimeError("%s: a scene edit (object selection, region, appearance, moves) is inference-only; call it under "
+                           "torch.no_grad() or with parameters that do not require grad" % who)
 
 
 class LazyRenderDict(dict):
@@ -253,13 +278,21 @@ raw2outputs = render_train
 
 
 def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64, N_importance=128, pixel_range=None,
-                 keep_all_ins=False, impl=_lib.IMPL_AUTO, device="cuda", keep_objects=None, region=None, appearance=None):
+                 keep_all_ins=False, impl=_lib.IMPL_AUTO, device="cuda", keep_objects=None, region=None, appearance=None,
+                 moves=None, chunk=8192):
     """One camera of the reference's test-time loop (render_test, networks/tester.py:55-76) through the frame entry point of
     the C ABI: rays are generated on the device from K / c2w (get_rays_k), the coarse depth row from near / far
     (z_val_sample), the pixels are rendered by the fused kernel and the maps come back as HOST tensors:
     rgb [H,W,3], ins [H,W,ins_num], depth [H,W], acc [H,W] (or [n, ...] rows when a pixel_range = (begin, count) is given --
     the per-rank slice of a sharded frame).  keep_objects, region and appearance: object selection, region selection and object
-    appearance as in render_rays; impl as in render_rays."""
+    appearance as in render_rays; impl as in render_rays.
+    moves: an objects.MovedScene: the frame's rays (get_rays_k, on the device) are rendered by render_rays(moves=) in chunks of
+    `chunk` rays into device maps, which return as host tensors of the same shapes; the result gains evaluated = (coarse, fine)
+    targets over the frame.  `chunk` bounds the moved render's device scratch, about 190 KB per ray at ins_num 93 with 64 + 128
+    samples (1.5 GB at the default 8192; DESIGN.md, "Rendering moved objects")."""
+    if moves is not None:
+        return _render_frame_moved(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples, N_importance, pixel_range,
+                                   keep_all_ins, impl, device, keep_objects, region, appearance, moves, chunk)
     impl = _lib.infer_impl(impl)
     dev = torch.device(device)
     ctx = get_context(dev)
@@ -280,4 +313,46 @@ def render_frame(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples=64
     if pixel_range is None:
         out = {"rgb": out["rgb"].reshape(H, W, 3), "ins": out["ins"].reshape(H, W, n_ins), "depth": out["depth"].reshape(H, W),
                "acc": out["acc"].reshape(H, W)}
+    return out
+
+
+def frame_rays(H, W, K, c2w, near, far, N_samples, device):
+    """The rays [H * W, 3] (get_rays_k on the device) and the shared coarse depth row [N_samples] (z_val_sample) of one camera."""
+    from .helpers import get_rays_k, z_val_sample
+    c2w = torch.as_tensor(c2w, dtype=torch.float32).to(device)
+    ro, rd = get_rays_k(H, W, K, c2w)
+    return ro.reshape(-1, 3), rd.reshape(-1, 3), z_val_sample(1, near, far, N_samples, device=device)[0].contiguous()
+
+
+def _render_frame_moved(H, W, K, c2w, near, far, model_coarse, model_fine, N_samples, N_importance, pixel_range, keep_all_ins, impl,
+                        device, keep_objects, region, appearance, moves, chunk):
+    """render_frame(moves=): render_rays(moves=) over chunks of the frame's rays into preallocated device maps."""
+    if isinstance(chunk, (bool,)) or int(chunk) != chunk or int(chunk) < 1:
+        raise ValueError("render_frame: chunk must be an integer >= 1, got %r" % (chunk,))
+    dev = torch.device(device)
+    ctx = get_context(dev)
+    dev = torch.device("cuda", ctx.index)
+    ins_num = bind_pair(ctx, model_coarse, model_fine)
+    _check_moved(moves, "render_frame", dev, model_coarse, model_fine)
+    begin, count = (0, H * W) if pixel_range is None else (int(pixel_range[0]), int(pixel_range[1]))
+    if not (0 <= begin and 0 <= count and begin + count <= H * W):
+        raise ValueError("render_frame: pixel range [%d, +%d) outside the %dx%d frame" % (begin, count, H, W))
+    ro, rd, z = frame_rays(H, W, K, c2w, near, far, N_samples, dev)
+    n_ins = ins_num + 1 if keep_all_ins else ins_num
+    maps = {"rgb": torch.empty(count, 3, device=dev), "ins": torch.empty(count, n_ins, device=dev),
+            "depth": torch.empty(count, device=dev), "acc": torch.empty(count, device=dev)}
+    evaluated = [0, 0]
+    for b in range(0, count, int(chunk)):
+        e = min(b + int(chunk), count)
+        r = render_rays(ro[begin + b:begin + e], rd[begin + b:begin + e], model_coarse, model_fine, z, N_importance=N_importance,
+                        want_raw=False, want_coarse=False, keep_all_ins=keep_all_ins, impl=impl, keep_objects=keep_objects,
+                        region=region, appearance=appearance, moves=moves)
+        for k in maps:
+            maps[k][b:e] = r[k + "_fine"]
+        evaluated = [evaluated[0] + r["evaluated"][0], evaluated[1] + r["evaluated"][1]]
+    out = {k: v.cpu() for k, v in maps.items()}
+    if pixel_range is None:
+        out = {"rgb": out["rgb"].reshape(H, W, 3), "ins": out["ins"].reshape(H, W, n_ins), "depth": out["depth"].reshape(H, W),
+               "acc": out["acc"].reshape(H, W)}
+    out["evaluated"] = tuple(evaluated)
     return out

@@ -445,6 +445,33 @@ DMNERF_API int dmnerf_mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double
 DMNERF_API int dmnerf_mesh_vertex_labels(const float* verts, int64_t n, const float* occ, const int16_t* labels, int dim, float level,
                                          int16_t* out, void* stream);
 
+/* ---- rendering moved objects per sample (DESIGN.md, "Rendering moved objects"; no counterpart in the original) ---------------
+ * dmnerf_render_moved: dmnerf_render_forward's stage path (never the fused kernel) with the moves of dmnerf_mesh_occupancy_edit
+ *   applied to the raw rows of each pass right after its network launch, before its composite.  Per move, in order, and sample
+ *   p = o + d z (the network prologue's fp32 point) with raw row r_p and occupancy o_p = 1 - expf(-relu(r_p[3]) voxel): t and its
+ *   nearest grid index as dmnerf_mesh_occupancy_edit computes them; the target's view direction trans[:3, :3] d (fp64, rounded
+ *   once to fp32) normalised in fp32 as the prologue normalises d.  take = t's index in the box && label(t) == label &&
+ *   (occ(t) > level || o_p <= level) && (no piece || the piece keeps t): r_p = the network's row at (t, its direction) (coarse
+ *   network in the coarse pass, fine in the fine pass).  Otherwise, when label_p == label: r_p[3] = 0 (logits kept) if the piece
+ *   keeps p (every p without one) and p's nearest index is in the box, or if rest_drop and the piece does not keep p.  The edited
+ *   coarse weights drive the importance sampling; io->edit (selection, region, appearance) applies to the edited samples as in
+ *   dmnerf_render_forward, and raw_* (when asked for) are the edited rows.  evaluated_host [2] (may be NULL): the targets
+ *   evaluated in the coarse and the fine pass.  impl: DMNERF_IMPL_AUTO / _UMMA / _UMMA_F16 (the targets run on the same network).
+ *   Rejected on the host, before any launch: everything dmnerf_mesh_occupancy_edit rejects of the grid, level and moves (n_moves in
+ *   [1, DMNERF_MAX_MOVES], labels in [0, ins_num]), voxel not finite or <= 0, DMNERF_IMPL_SIMT and n (S + I) >= 2^31.  Reads the
+ *   number of boxed targets back once per move and pass (synchronises the stream). */
+typedef struct dmnerf_render_moves {
+  const dmnerf_edit_move* moves;   /* HOST [n_moves] */
+  int32_t n_moves;
+  int32_t dim;                     /* the sweep grid the boxes index */
+  double transform[16];            /* the sweep grid's scene transform, row-major */
+  double extents[3];
+  float level;                     /* (0, 1) */
+  float voxel;                     /* > 0: the sweep's (far - near) / N_importance */
+} dmnerf_render_moves;
+DMNERF_API int dmnerf_render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                   const dmnerf_render_moves* moves, int64_t* evaluated_host, void* stream);
+
 /* ---- object inventory (DESIGN.md, "Object inventory"; no counterpart in the original) ---------------------------------------
  * Per-group reductions over the solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order of the index (i, j, k)).
  * labels [dim^3] (DEVICE int16, may be NULL: every point is group 0) assigns each point its group 0 .. n_labels - 1.

@@ -6,7 +6,7 @@
             | --place-at X Y Z --down X Y Z [--on L ...] [--lift N] [--any-stability] [--turns K]) [--rest keep|drop]
            --transform T [--extents X Y Z] [--grid-dim 256] [--level 0.45] [--connectivity {6,26}] [--dilate 1] --out DIR
            [--near 4 --far 15 --N-samples 64 --N-importance 128 --N-test 4096] [--mesh [--min-cluster 400]]
-           [--check] [--until-contact [--step S] [--tolerance N]]
+           [--check] [--until-contact [--step S] [--tolerance N]] [--render {exchanger,samples}]
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict`.  POSE.npy holds the camera-to-world pose [4, 4] (or
 [3, 4]; of several [N, 4, 4] the first is used).  K is the 3x3 intrinsics, as a .npy file or as 9 numbers.
@@ -45,7 +45,13 @@ several objects one after another, each in the scene the earlier placements leav
 moves the label's largest piece and "piece" that component, each with its region grown by --dilate voxels, as the single-move
 flags do.  The frame is rendered with every placed move (manipulate_frame), --mesh meshes the same moves (edited_mesh), and the
 record gains arrange: per item label, placed, reason, offset, drop, support, stable and turn, and each placed move's overwritten
-(the solid voxels of the scene left before it that it landed on, per label)."""
+(the solid voxels of the scene left before it that it landed on, per label).
+
+Rendering (--render): `exchanger` (the default) renders the frame with manipulate_frame, the original's exchanger, which renders
+the scene again along every move.  `samples` renders the same moves, pieces and rest with render_frame(moves=) (DESIGN.md,
+"Rendering moved objects"): the edited sweep's rule applied per render sample, with the default boxes of the keep-all sweep, so
+that the frame and --mesh show the same edit.  The record gains render and evaluated (the targets the moved render evaluated in
+its coarse and fine passes; null for the exchanger)."""
 import argparse
 import json
 import os
@@ -99,6 +105,8 @@ def parse(argv=None):
     ap.add_argument("--until-contact", action="store_true", help="translation: slide until just before contact")
     ap.add_argument("--step", type=float, default=None, help="--until-contact: the slide's step (default: one grid spacing)")
     ap.add_argument("--tolerance", type=int, default=0, help="--until-contact: overlapping voxels tolerated")
+    ap.add_argument("--render", choices=("exchanger", "samples"), default="exchanger",
+                    help="render the frame with the exchanger (manipulate_frame) or per sample (render_frame(moves=))")
     a = ap.parse_args(argv)
     if a.arrange is not None:
         for flag, given in (("--place-at", a.place_at is not None), ("--mode", a.mode is not None),
@@ -297,7 +305,8 @@ def main(argv=None):
         piece, label, centre, region = None, None, None, None
     else:
         piece, label, centre, region = choose_piece(a, nets[1], T, ext)
-    if a.check or a.until_contact or a.place_at is not None or a.arrange is not None:
+    sweep = a.check or a.until_contact or a.place_at is not None or a.arrange is not None or a.render == "samples"
+    if sweep:
         from dmnerf_b200.objects import object_mask, occupancy_objects
         with torch.no_grad():
             occ, labels = occupancy_objects(nets[1], T, object_mask(ins_num, remove=[]), a.grid_dim, ext, a.near, a.far,
@@ -319,14 +328,24 @@ def main(argv=None):
         moves, regions, rests = [(label, trans["transformations"][0]["transformation"])], [region], [a.rest]
     dev = next(nets[1].parameters()).device
     pose_t = torch.from_numpy(c2w).to(dev)
-    rays = [rigid_rays(a.H, a.W, a.K, m, pose_t) for _, m in moves]
-    tar_o, tar_d = torch.stack([o for o, _ in rays]), torch.stack([d for _, d in rays])
-    args = types.SimpleNamespace(N_test=a.N_test, N_samples=a.N_samples, N_importance=a.N_importance, near=a.near, far=a.far,
-                                 target_labels=[k for k, _ in moves])
-    pe, _ = get_embedder(10)
-    ve, _ = get_embedder(4)
-    rgb, ins, _, _ = manipulate_frame(a.H, a.W, a.K, pose_t, tar_o, tar_d, pe, ve, nets[0], nets[1], args, pieces=regions,
-                                      rest=rests)
+    evaluated = None
+    if a.render == "samples":
+        from dmnerf_b200.objects import render_moves
+        from dmnerf_b200.render import render_frame
+        moved = render_moves(occ, labels, T, moves, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests)
+        with torch.no_grad():
+            fr = render_frame(a.H, a.W, a.K, pose_t, a.near, a.far, nets[0], nets[1], a.N_samples, a.N_importance, keep_all_ins=True,
+                              device=dev, moves=moved)
+        rgb, ins, evaluated = fr["rgb"].reshape(-1, 3).to(dev), fr["ins"].reshape(a.H * a.W, -1).to(dev), list(fr["evaluated"])
+    else:
+        rays = [rigid_rays(a.H, a.W, a.K, m, pose_t) for _, m in moves]
+        tar_o, tar_d = torch.stack([o for o, _ in rays]), torch.stack([d for _, d in rays])
+        args = types.SimpleNamespace(N_test=a.N_test, N_samples=a.N_samples, N_importance=a.N_importance, near=a.near, far=a.far,
+                                     target_labels=[k for k, _ in moves])
+        pe, _ = get_embedder(10)
+        ve, _ = get_embedder(4)
+        rgb, ins, _, _ = manipulate_frame(a.H, a.W, a.K, pose_t, tar_o, tar_d, pe, ve, nets[0], nets[1], args, pieces=regions,
+                                          rest=rests)
     os.makedirs(a.out, exist_ok=True)
     write_png(os.path.join(a.out, "rgb.png"), (255 * torch.clamp(rgb, 0, 1)).to(torch.uint8).reshape(a.H, a.W, 3).cpu().numpy())
     ins_rgbs = np.random.default_rng(0).integers(0, 256, (ins_num + 1, 3))
@@ -338,6 +357,7 @@ def main(argv=None):
     else:
         record = {"transformations": trans["transformations"], "label": label, "piece": piece, "centre": centre.tolist(),
                   "rest": a.rest}
+    record["render"], record["evaluated"] = a.render, evaluated
     if slide is not None:
         record["slide"] = slide
     if place is not None:
@@ -349,7 +369,7 @@ def main(argv=None):
         record["overlap"] = {"voxels": {str(k): v for k, v in r["overlap"].items()},
                              "volume": {str(k): v for k, v in r["overlap_volume"].items()}}
         record["landed"] = r["landed"]
-    if a.check or a.until_contact or a.place_at is not None or a.arrange is not None:
+    if sweep:
         del occ, labels
     if a.mesh:
         from dmnerf_b200.objects import edited_mesh
