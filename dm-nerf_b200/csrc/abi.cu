@@ -422,6 +422,7 @@ DMNERF_API int dmnerf_penalizer_backward(const float* raw, const float* z_vals, 
 // The checked moves of dmnerf_render_moved and the targets each pass evaluated.
 struct RenderMoves {
   const EditMove* moves;
+  const int32_t* copies;      // NULL: no copy
   int n;
   float voxel, level;
   int64_t evaluated[2];
@@ -477,7 +478,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:49-61  points, embeddings, coarse network
   if ((rc = mlp_dispatch(ctx, 0, nullptr, io->rays_o, io->rays_d, z_c, n * S, S, raw_c, impl, st))) return rc;
-  if (mv && (rc = render_moves_pass(ctx->moves, ctx->net[0], impl == DMNERF_IMPL_UMMA_F16, mv->moves, mv->n, io->rays_o, io->rays_d,
+  if (mv && (rc = render_moves_pass(ctx->moves, ctx->net[0], impl == DMNERF_IMPL_UMMA_F16, mv->moves, mv->copies, mv->n, io->rays_o, io->rays_d,
                                     z_c, n, S, C, mv->voxel, mv->level, raw_c, &mv->evaluated[0], st)))
     return rc;
   DMN_STAGE_MARK();
@@ -490,7 +491,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   DMN_STAGE_MARK();
   // render.py:71-82  fine network on all S+I depths
   if ((rc = mlp_dispatch(ctx, 1, nullptr, io->rays_o, io->rays_d, z_f, n * F, F, raw_f, impl, st))) return rc;
-  if (mv && (rc = render_moves_pass(ctx->moves, ctx->net[1], impl == DMNERF_IMPL_UMMA_F16, mv->moves, mv->n, io->rays_o, io->rays_d,
+  if (mv && (rc = render_moves_pass(ctx->moves, ctx->net[1], impl == DMNERF_IMPL_UMMA_F16, mv->moves, mv->copies, mv->n, io->rays_o, io->rays_d,
                                     z_f, n, F, C, mv->voxel, mv->level, raw_f, &mv->evaluated[1], st)))
     return rc;
   DMN_STAGE_MARK();
@@ -515,9 +516,12 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
   return f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, edit, stream), impl, stream);
 }
 
-DMNERF_API int dmnerf_render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
-                                   const dmnerf_render_moves* moves, int64_t* evaluated_host, void* stream) {
-  const char* who = "render_moved";
+}  // extern "C"
+
+// dmnerf_render_moved with copy flags copies_host [n_moves] (NULL: none)
+static int render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                        const dmnerf_render_moves* moves, const int32_t* copies_host, int64_t* evaluated_host, void* stream,
+                        const char* who) {
   if (evaluated_host) evaluated_host[0] = evaluated_host[1] = 0;
   if (bound_pair(ctx, who)) return 1;
   DMN_CHECK(!(flags & ~RENDER_FLAGS), "%s: unknown flag bits 0x%x", who, flags & ~RENDER_FLAGS);
@@ -535,13 +539,27 @@ DMNERF_API int dmnerf_render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, 
   EditMove mv[DMNERF_MAX_MOVES];
   for (int i = 0; i < moves->n_moves; ++i)
     if (edit_move_from_abi(moves->moves[i], moves->transform, moves->extents, moves->dim, ctx->net[0].p.ins_num, mv[i], who, i)) return 1;
+  if (copy_flags_check(moves->moves, copies_host, moves->n_moves, true, who)) return 1;
   Edit e;
   const Edit* edit;
   if (int rc = scene_edit(ctx, io ? io->edit : nullptr, (cudaStream_t)stream, e, edit, who)) return rc;
-  RenderMoves r = {mv, moves->n_moves, moves->voxel, moves->level, {0, 0}};
+  RenderMoves r = {mv, copies_host, moves->n_moves, moves->voxel, moves->level, {0, 0}};
   const int rc = f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, edit, stream, &r), impl, stream);
   if (evaluated_host && !rc) { evaluated_host[0] = r.evaluated[0]; evaluated_host[1] = r.evaluated[1]; }
   return rc;
+}
+
+extern "C" {
+
+DMNERF_API int dmnerf_render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                   const dmnerf_render_moves* moves, int64_t* evaluated_host, void* stream) {
+  return render_moved(ctx, io, n, S, NI, flags, impl, moves, nullptr, evaluated_host, stream, "render_moved");
+}
+
+DMNERF_API int dmnerf_render_moved_copies(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                          const dmnerf_render_moves* moves, const int32_t* copies_host, int64_t* evaluated_host,
+                                          void* stream) {
+  return render_moved(ctx, io, n, S, NI, flags, impl, moves, copies_host, evaluated_host, stream, "render_moved_copies");
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
@@ -801,10 +819,12 @@ DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* tra
   return 0;
 }
 
-DMNERF_API int dmnerf_mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
-                                          float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host, int n_moves,
-                                          float* occ, int16_t* labels, int64_t* evaluated_host, void* stream) {
-  const char* who = "mesh_occupancy_edit";
+}  // extern "C"
+
+// dmnerf_mesh_occupancy_edit with copy flags copies_host [n_moves] (NULL: none)
+static int mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim, float voxel,
+                               float level, int64_t slab, const dmnerf_edit_move* moves_host, const int32_t* copies_host, int n_moves,
+                               float* occ, int16_t* labels, int64_t* evaluated_host, void* stream, const char* who) {
   if (bound_net(ctx, net, who)) return 1;
   if (evaluated_host) *evaluated_host = 0;
   DMN_CHECK(transform_host && extents_host && occ && labels, "%s: NULL argument", who);
@@ -815,6 +835,7 @@ DMNERF_API int dmnerf_mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double
   EditMove mv[DMNERF_MAX_MOVES];
   for (int i = 0; i < n_moves; ++i)
     if (edit_move_from_abi(moves_host[i], transform_host, extents_host, dim, ctx->net[net].p.ins_num, mv[i], who, i)) return 1;
+  if (copy_flags_check(moves_host, copies_host, n_moves, true, who)) return 1;
   if (n_moves == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   DMN_CUDA(cudaSetDevice(ctx->device));
@@ -834,13 +855,31 @@ DMNERF_API int dmnerf_mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double
       int64_t m = 0;
       int rc = edit_targets(ctx->mesh, transform_host, extents_host, dim, mv[i], b, cnt, pts, &m, st);
       if (!rc && m) rc = launch_mlp_tc(ctx->net[net], nullptr, pts, dirs, nullptr, m, 1, raw, nullptr, st);
-      if (!rc) rc = edit_apply(ctx->mesh, transform_host, extents_host, dim, mv[i], b, cnt, raw, C, voxel, level, occ, labels, st);
+      if (!rc) rc = edit_apply(ctx->mesh, transform_host, extents_host, dim, mv[i], b, cnt, raw, C, voxel, level, occ, labels,
+                               copies_host && copies_host[i], st);
       if (rc) return rc;
       evaluated += m;
     }
   }
   if (evaluated_host) *evaluated_host = evaluated;
   return 0;
+}
+
+extern "C" {
+
+DMNERF_API int dmnerf_mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
+                                          float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host, int n_moves,
+                                          float* occ, int16_t* labels, int64_t* evaluated_host, void* stream) {
+  return mesh_occupancy_edit(ctx, net, transform_host, extents_host, dim, voxel, level, slab, moves_host, nullptr, n_moves, occ, labels,
+                             evaluated_host, stream, "mesh_occupancy_edit");
+}
+
+DMNERF_API int dmnerf_mesh_occupancy_edit_copies(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host,
+                                                 int dim, float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host,
+                                                 const int32_t* copies_host, int n_moves, float* occ, int16_t* labels,
+                                                 int64_t* evaluated_host, void* stream) {
+  return mesh_occupancy_edit(ctx, net, transform_host, extents_host, dim, voxel, level, slab, moves_host, copies_host, n_moves, occ,
+                             labels, evaluated_host, stream, "mesh_occupancy_edit_copies");
 }
 
 DMNERF_API int dmnerf_mesh_vertex_labels(const float* verts, int64_t n, const float* occ, const int16_t* labels, int dim, float level,
@@ -928,8 +967,18 @@ DMNERF_API int dmnerf_move_overlap(dmnerf_ctx* ctx, const float* occ, const int1
                                    void* stream) {
   DMN_CHECK(ctx != nullptr, "move_overlap: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, n_candidates,
+  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, nullptr, n_candidates,
                       obstacles_host, overlap_host, landed_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_move_overlap_copies(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                          const double* transform_host, const double* extents_host,
+                                          const dmnerf_edit_move* candidates_host, const int32_t* copies_host, int n_candidates,
+                                          const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "move_overlap_copies: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, copies_host, n_candidates,
+                      obstacles_host, overlap_host, landed_host, (cudaStream_t)stream, "move_overlap_copies");
 }
 
 DMNERF_API int dmnerf_object_contacts(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
@@ -956,7 +1005,7 @@ DMNERF_API int dmnerf_placement_contacts(dmnerf_ctx* ctx, const float* occ, cons
                                          int32_t* drop_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "placement_contacts: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, nullptr, nullptr, u, v,
+  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, 0, nullptr, nullptr, u, v,
                             cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
 }
 
@@ -966,7 +1015,7 @@ DMNERF_API int dmnerf_placement_maps(dmnerf_ctx* ctx, const float* occ, const in
                                      int16_t* support, dmnerf_placement_info* info_host, int32_t* status_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "placement_maps: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_maps(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, bases_host, box_host, n_bases,
+  return placement_maps(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, 0, bases_host, box_host, n_bases,
                         drop, contacts, support, info_host, status_host, (cudaStream_t)stream);
 }
 
@@ -978,7 +1027,7 @@ DMNERF_API int dmnerf_placement_contacts_moved(dmnerf_ctx* ctx, const float* occ
   DMN_CHECK(ctx != nullptr, "placement_contacts_moved: ctx is NULL");
   DMN_CHECK(base_host != nullptr, "placement_contacts_moved: base is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, base_host, box_host, u, v,
+  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, 0, base_host, box_host, u, v,
                             cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
 }
 
@@ -989,8 +1038,18 @@ DMNERF_API int dmnerf_grid_edit(dmnerf_ctx* ctx, const float* src_occ, const int
                                 float* occ, int16_t* labels, int64_t* landed_host, int64_t* overwritten_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "grid_edit: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, n_moves, occ, labels,
-                   landed_host, overwritten_host, (cudaStream_t)stream);
+  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, nullptr, n_moves, occ,
+                   labels, landed_host, overwritten_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_grid_edit_copies(dmnerf_ctx* ctx, const float* src_occ, const int16_t* src_labels, int dim, float level,
+                                       const double* transform_host, const double* extents_host, const dmnerf_edit_move* moves_host,
+                                       const int32_t* copies_host, int n_moves, float* occ, int16_t* labels, int64_t* landed_host,
+                                       int64_t* overwritten_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "grid_edit_copies: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, copies_host, n_moves, occ,
+                   labels, landed_host, overwritten_host, (cudaStream_t)stream, "grid_edit_copies");
 }
 
 DMNERF_API int dmnerf_placement_maps_in_scene(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
@@ -1000,8 +1059,21 @@ DMNERF_API int dmnerf_placement_maps_in_scene(dmnerf_ctx* ctx, const float* occ,
                                               dmnerf_placement_info* info_host, int32_t* status_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "placement_maps_in_scene: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_maps(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, bases_host,
-                        box_host, n_bases, drop, contacts, support, info_host, status_host, (cudaStream_t)stream);
+  return placement_maps(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, 0,
+                        bases_host, box_host, n_bases, drop, contacts, support, info_host, status_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_placement_maps_in_scene_copy(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                                   const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                                   const double* extents_host, const dmnerf_placement* placement, int copy,
+                                                   const double* bases_host, const int32_t* box_host, int n_bases, int32_t* drop,
+                                                   int32_t* contacts, int16_t* support, dmnerf_placement_info* info_host,
+                                                   int32_t* status_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_maps_in_scene_copy: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_maps(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, copy,
+                        bases_host, box_host, n_bases, drop, contacts, support, info_host, status_host, (cudaStream_t)stream,
+                        "placement_maps_in_scene_copy");
 }
 
 DMNERF_API int dmnerf_placement_contacts_in_scene(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
@@ -1012,8 +1084,22 @@ DMNERF_API int dmnerf_placement_contacts_in_scene(dmnerf_ctx* ctx, const float* 
   DMN_CHECK(ctx != nullptr, "placement_contacts_in_scene: ctx is NULL");
   DMN_CHECK(base_host != nullptr, "placement_contacts_in_scene: base is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_contacts(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement,
+  return placement_contacts(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, 0,
                             base_host, box_host, u, v, cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
+}
+
+DMNERF_API int dmnerf_placement_contacts_in_scene_copy(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                                       const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                                       const double* extents_host, const dmnerf_placement* placement, int copy,
+                                                       const double* base_host, const int32_t* box_host, int u, int v,
+                                                       int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                                                       int32_t* drop_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_contacts_in_scene_copy: ctx is NULL");
+  DMN_CHECK(base_host != nullptr, "placement_contacts_in_scene_copy: base is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_contacts(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, copy,
+                            base_host, box_host, u, v, cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream,
+                            "placement_contacts_in_scene_copy");
 }
 
 // ---- connected components (DESIGN.md, "Connected components") -------------------------------------------------------------

@@ -63,6 +63,9 @@ __global__ void grid_check_kernel(const float* __restrict__ occ, const int16_t* 
   if ((threadIdx.x & 31) == 0 && flags) atomicOr(bad, flags);
 }
 
+// COPY (DESIGN.md, "Copying objects"): every candidate of the launch is a copy, which vacates nothing, so its own label's solid
+// points are obstacles like any other.
+template <bool COPY>
 __global__ void __launch_bounds__(OV_THREADS) move_overlap_kernel(const GridXform g, const IndexMap map, const float* __restrict__ occ,
                                                                   const int16_t* __restrict__ labels, float level, ObjMask obstacles,
                                                                   const Candidate* __restrict__ cands, const Run* __restrict__ runs,
@@ -126,7 +129,7 @@ __global__ void __launch_bounds__(OV_THREADS) move_overlap_kernel(const GridXfor
       const unsigned landed = __ballot_sync(FULL, src);
       if (lane == 0 && landed) atomicAdd(&hist[c][LANDED], (uint32_t)__popc(landed));
       bool hit = src && blocking;
-      if (hit && l == m.label)                                   // a point the move vacates is no obstacle
+      if (!COPY && hit && l == m.label)                          // a point the move vacates is no obstacle
         hit = !(m.rest_drop || m.piece.bits == nullptr || !region_drops(m.piece, m.label, p[0], p[1], p[2]));
       if (hit) atomicAdd(&hist[c][l], 1u);
     }
@@ -141,7 +144,9 @@ __global__ void __launch_bounds__(OV_THREADS) move_overlap_kernel(const GridXfor
 // One move of the grid-only edit (DESIGN.md, "Arranging objects"), one thread per grid point p of the state: edit_rule with the
 // source grid at the target's nearest index q.  counts [129]: overwritten per label, then landed -- the takes whose target is
 // solid, and those of them that land on a solid state point the move does not vacate, by its label.  The state point is read
-// before it is written and no thread reads another's point, so the launch order of the points does not matter.
+// before it is written and no thread reads another's point, so the launch order of the points does not matter.  A COPY takes and
+// never vacates, so every solid state point it lands on counts, its own label's included.
+template <bool COPY>
 __global__ void __launch_bounds__(GE_THREADS) grid_edit_kernel(const GridXform g, const EditMove e, const float* __restrict__ src_occ,
                                                                const int16_t* __restrict__ src_labels, float level,
                                                                float* __restrict__ occ, int16_t* __restrict__ labels,
@@ -159,7 +164,7 @@ __global__ void __launch_bounds__(GE_THREADS) grid_edit_kernel(const GridXform g
     sweep_point(g, p, x);
     const bool in_box = edit_target(e.trans, e.inv, e.b, e.lo, e.hi, !e.empty, x, t, q);
     auto here = [&] { return e.piece.bits == nullptr || !region_drops(e.piece, e.label, x[0], x[1], x[2]); };
-    edit_rule(
+    edit_rule<COPY>(
         e, in_box,
         [&](int& lt, float& ot) {
           const int64_t qi = ((int64_t)q[0] * d + (int64_t)q[1]) * d + (int64_t)q[2];
@@ -171,7 +176,7 @@ __global__ void __launch_bounds__(GE_THREADS) grid_edit_kernel(const GridXform g
           occ[p] = ot;
           labels[p] = (int16_t)e.label;
           landed = ot > level;
-          if (landed && o > level && !(l == e.label && (e.rest_drop || here()))) atomicAdd(&hist[l], 1u);
+          if (landed && o > level && (COPY || !(l == e.label && (e.rest_drop || here())))) atomicAdd(&hist[l], 1u);
         },
         [&] { occ[p] = 0.0f; });
   }
@@ -293,14 +298,21 @@ int read_checked(const void* dev, void* host, size_t bytes, int max_label, const
 }
 
 int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
-                 const dmnerf_edit_move* cands_host, int n, const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host,
-                 cudaStream_t st) {
-  const char* who = "move_overlap";
+                 const dmnerf_edit_move* cands_host, const int32_t* copies_host, int n, const uint32_t* obstacles_host,
+                 int64_t* overlap_host, int64_t* landed_host, cudaStream_t st, const char* who) {
   DMN_CHECK(occ && labels && T16 && ext3 && overlap_host && landed_host, "%s: NULL argument", who);
   if (sweep_grid_check(T16, ext3, dim, level, who)) return 1;
   DMN_CHECK(n >= 1 && n <= DMNERF_MAX_CANDIDATES, "%s: between 1 and %d candidates are supported, got %d", who,
             DMNERF_MAX_CANDIDATES, n);
   DMN_CHECK(cands_host, "%s: candidates is NULL", who);
+  if (copy_flags_check(cands_host, copies_host, n, false, who)) return 1;   // each candidate on its own: no order
+  // the moves first, then the copies: one launch per kind, slot[i] the row of candidate i
+  std::vector<int> slot(n);
+  int n_moves = 0;
+  for (int i = 0; i < n; ++i)
+    if (!copies_host || !copies_host[i]) slot[i] = n_moves++;
+  for (int i = 0, k = n_moves; i < n; ++i)
+    if (copies_host && copies_host[i]) slot[i] = k++;
   std::vector<Candidate> cand(n);
   double A[9];
   grid_forward(T16, ext3, dim, A);
@@ -312,7 +324,7 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
       memcpy(map.inv, e.inv, sizeof(map.inv));
       memcpy(map.b, e.b, sizeof(map.b));
     }
-    Candidate& c = cand[i];
+    Candidate& c = cand[slot[i]];
     memset(&c, 0, sizeof(c));
     memcpy(c.trans, e.trans, sizeof(c.trans));
     memcpy(c.lo, e.lo, sizeof(c.lo));
@@ -328,34 +340,40 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
   }
   ObjMask obst;
   for (int w = 0; w < 4; ++w) obst.w[w] = obstacles_host ? obstacles_host[w] : 0xffffffffu;
-  // runs of RUN consecutive candidates over the box holding their destination boxes
+  // per kind (moves, then copies), runs of RUN consecutive candidates over the box holding their destination boxes, each kind's
+  // blocks counted from 0 for its own launch
   std::vector<Run> runs;
-  int64_t blocks_total = 0;
-  for (int f = 0; f < n; f += RUN) {
-    Run r{};
-    r.first = f;
-    r.count = n - f < RUN ? n - f : RUN;
-    int lo[3] = {dim, dim, dim}, hi[3] = {-1, -1, -1};
-    for (int i = f; i < f + r.count; ++i) {
-      const Candidate& c = cand[i];
-      if (c.dlo[0] > c.dhi[0] || c.dlo[1] > c.dhi[1] || c.dlo[2] > c.dhi[2]) continue;
-      for (int a = 0; a < 3; ++a) {
-        lo[a] = c.dlo[a] < lo[a] ? c.dlo[a] : lo[a];
-        hi[a] = c.dhi[a] > hi[a] ? c.dhi[a] : hi[a];
+  int64_t blocks_of[2] = {0, 0};
+  size_t first_run[3] = {0, 0, 0};
+  for (int kind = 0; kind < 2; ++kind) {
+    const int begin = kind ? n_moves : 0, end = kind ? n : n_moves;
+    for (int f = begin; f < end; f += RUN) {
+      Run r{};
+      r.first = f;
+      r.count = end - f < RUN ? end - f : RUN;
+      int lo[3] = {dim, dim, dim}, hi[3] = {-1, -1, -1};
+      for (int i = f; i < f + r.count; ++i) {
+        const Candidate& c = cand[i];
+        if (c.dlo[0] > c.dhi[0] || c.dlo[1] > c.dhi[1] || c.dlo[2] > c.dhi[2]) continue;
+        for (int a = 0; a < 3; ++a) {
+          lo[a] = c.dlo[a] < lo[a] ? c.dlo[a] : lo[a];
+          hi[a] = c.dhi[a] > hi[a] ? c.dhi[a] : hi[a];
+        }
       }
+      if (hi[0] < 0) continue;                                   // no candidate of the run reaches the grid
+      int64_t volume = 1;
+      for (int a = 0; a < 3; ++a) {
+        r.lo[a] = lo[a];
+        r.n[a] = hi[a] - lo[a] + 1;
+        volume *= r.n[a];
+      }
+      r.block0 = blocks_of[kind];
+      blocks_of[kind] += (volume + OV_BLOCK_POINTS - 1) / OV_BLOCK_POINTS;
+      runs.push_back(r);
     }
-    if (hi[0] < 0) continue;                                     // no candidate of the run reaches the grid
-    int64_t volume = 1;
-    for (int a = 0; a < 3; ++a) {
-      r.lo[a] = lo[a];
-      r.n[a] = hi[a] - lo[a] + 1;
-      volume *= r.n[a];
-    }
-    r.block0 = blocks_total;
-    blocks_total += (volume + OV_BLOCK_POINTS - 1) / OV_BLOCK_POINTS;
-    runs.push_back(r);
+    first_run[kind + 1] = runs.size();
+    DMN_CHECK(blocks_of[kind] < INT32_MAX, "%s: %lld blocks of work exceed one launch", who, (long long)blocks_of[kind]);
   }
-  DMN_CHECK(blocks_total < INT32_MAX, "%s: %lld blocks of work exceed one launch", who, (long long)blocks_total);
   const size_t count_bytes = (size_t)n * N_COUNTERS * sizeof(unsigned long long), out_bytes = 16 + count_bytes;
   const size_t cand_bytes = (size_t)n * sizeof(Candidate), run_bytes = runs.size() * sizeof(Run);
   char *out, *in_d;
@@ -369,16 +387,24 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
   auto* counts = reinterpret_cast<unsigned long long*>(out + 16);
   const int64_t npts = (int64_t)dim * dim * dim;
   if (launch_grid_check(occ, labels, npts, DMNERF_MAX_INS + 1, bad, st)) return 2;
-  if (blocks_total) {
-    move_overlap_kernel<<<(unsigned)blocks_total, OV_THREADS, 0, st>>>(
-        make_xform(T16, ext3, dim), map, occ, labels, level, obst, reinterpret_cast<const Candidate*>(in_d),
-        reinterpret_cast<const Run*>(in_d + cand_bytes), (int)runs.size(), counts);
+  const GridXform g = make_xform(T16, ext3, dim);
+  const Candidate* cands_d = reinterpret_cast<const Candidate*>(in_d);
+  for (int kind = 0; kind < 2; ++kind) {
+    if (!blocks_of[kind]) continue;
+    const Run* runs_d = reinterpret_cast<const Run*>(in_d + cand_bytes) + first_run[kind];
+    const int n_runs = (int)(first_run[kind + 1] - first_run[kind]);
+    if (kind)
+      move_overlap_kernel<true><<<(unsigned)blocks_of[kind], OV_THREADS, 0, st>>>(g, map, occ, labels, level, obst, cands_d, runs_d,
+                                                                                  n_runs, counts);
+    else
+      move_overlap_kernel<false><<<(unsigned)blocks_of[kind], OV_THREADS, 0, st>>>(g, map, occ, labels, level, obst, cands_d, runs_d,
+                                                                                   n_runs, counts);
     DMN_LAUNCH_OK();
   }
   std::vector<char> h(out_bytes);
   if (const int rc = read_back(out, h, DMNERF_MAX_INS, who, st)) return rc;
   for (int i = 0; i < n; ++i) {
-    const char* row = h.data() + 16 + (size_t)i * N_COUNTERS * sizeof(unsigned long long);
+    const char* row = h.data() + 16 + (size_t)slot[i] * N_COUNTERS * sizeof(unsigned long long);
     memcpy(overlap_host + (size_t)i * (DMNERF_MAX_INS + 1), row, (DMNERF_MAX_INS + 1) * sizeof(int64_t));
     memcpy(landed_host + i, row + LANDED * sizeof(int64_t), sizeof(int64_t));
   }
@@ -410,9 +436,8 @@ int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, 
 }
 
 int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels, int dim, float level, const double* T16,
-              const double* ext3, const dmnerf_edit_move* moves_host, int n, float* occ, int16_t* labels, int64_t* landed_host,
-              int64_t* overwritten_host, cudaStream_t st) {
-  const char* who = "grid_edit";
+              const double* ext3, const dmnerf_edit_move* moves_host, const int32_t* copies_host, int n, float* occ, int16_t* labels,
+              int64_t* landed_host, int64_t* overwritten_host, cudaStream_t st, const char* who) {
   DMN_CHECK(src_occ && src_labels && occ && labels && T16 && ext3 && landed_host && overwritten_host, "%s: NULL argument", who);
   DMN_CHECK(n >= 1 && n <= DMNERF_MAX_MOVES, "%s: between 1 and %d moves are supported, got %d", who, DMNERF_MAX_MOVES, n);
   DMN_CHECK(moves_host, "%s: moves is NULL", who);
@@ -430,6 +455,7 @@ int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels
   std::vector<EditMove> mv(n);
   for (int i = 0; i < n; ++i)
     if (edit_move_from_abi(moves_host[i], T16, ext3, dim, DMNERF_MAX_INS, mv[i], who, i)) return 1;
+  if (copy_flags_check(moves_host, copies_host, n, true, who)) return 1;
   const size_t out_bytes = 16 + (size_t)n * N_COUNTERS * sizeof(unsigned long long);
   char* out;
   if (s.out.get(out_bytes, &out)) return 2;
@@ -442,9 +468,13 @@ int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels
   if (const int rc = read_checked(out, h.data(), 16, DMNERF_MAX_INS, who, st)) return rc;   // a bad grid writes nothing
   const GridXform g = make_xform(T16, ext3, dim);
   auto* counts = reinterpret_cast<unsigned long long*>(out + 16);
+  const unsigned ge_blocks = (unsigned)((npts + GE_THREADS - 1) / GE_THREADS);
   for (int i = 0; i < n; ++i) {
-    grid_edit_kernel<<<(unsigned)((npts + GE_THREADS - 1) / GE_THREADS), GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ,
-                                                                                           labels, counts + (size_t)i * N_COUNTERS);
+    unsigned long long* row = counts + (size_t)i * N_COUNTERS;
+    if (copies_host && copies_host[i])
+      grid_edit_kernel<true><<<ge_blocks, GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ, labels, row);
+    else
+      grid_edit_kernel<false><<<ge_blocks, GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ, labels, row);
     DMN_LAUNCH_OK();
   }
   if (const int rc = read_back(out, h, DMNERF_MAX_INS, who, st)) return rc;

@@ -307,13 +307,17 @@ int sweep_grid_check(const double* T16, const double* ext3, int dim, float level
 // d -> m, checked against the grid (dim, transform, extents) and the bound network's ins_num
 int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const double* ext3, int dim, int ins_num, EditMove& m,
                        const char* who, int i);
+// The copy flags of n moves (DESIGN.md, "Copying objects"; copies NULL: none), checked: each 0 or 1, no copy with rest_drop and,
+// when the moves apply in order (`ordered`), no move of a label after a copy of it.
+int copy_flags_check(const dmnerf_edit_move* moves, const int32_t* copies, int n, bool ordered, const char* who);
 // Points [begin, begin + count) of the grid: their targets under m, the boxed ones compacted in order into pts [*n_eval, 3];
 // *n_eval read back (synchronises).
 int edit_targets(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
                  float* pts, int64_t* n_eval, cudaStream_t st);
-// take / vacate of m on the same points, raw [n_eval, c]: the network at the compacted targets of the last edit_targets
+// take / vacate of m on the same points, raw [n_eval, c]: the network at the compacted targets of the last edit_targets; a copy
+// takes only
 int edit_apply(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
-               const float* raw, int c, float voxel, float level, float* occ, int16_t* labels, cudaStream_t st);
+               const float* raw, int c, float voxel, float level, float* occ, int16_t* labels, bool copy, cudaStream_t st);
 int launch_vertex_labels(const float* v, int64_t n, const float* occ, const int16_t* labels, int dim, float level, int16_t* out,
                          cudaStream_t st);
 // The region of a move (bits NULL: none), checked: dim and map, the moved label among the labels it applies to (exchanger.cu).
@@ -329,9 +333,9 @@ struct Network;
 // The moves applied in order, in place, to the raw rows raw [n * s, c] of one pass of a stage render (samples o + d z, z [n, s]),
 // the targets run through `net` (fp16 preview network when f16); *evaluated += the targets evaluated.  One device->host read of
 // the count per move (synchronises).
-int render_moves_pass(MovesState& s, const Network& net, bool f16, const EditMove* moves, int n_moves, const float* rays_o,
-                      const float* rays_d, const float* z, int64_t n, int s_per_ray, int c, float voxel, float level, float* raw,
-                      int64_t* evaluated, cudaStream_t st);
+int render_moves_pass(MovesState& s, const Network& net, bool f16, const EditMove* moves, const int32_t* copies, int n_moves,
+                      const float* rays_o, const float* rays_d, const float* z, int64_t n, int s_per_ray, int c, float voxel,
+                      float level, float* raw, int64_t* evaluated, cudaStream_t st);
 
 // Object inventory (inventory.cu): per-group integer statistics and fp64 spans of the solid points of a labelled grid.
 // Per-context device buffers: everything a call reads back (status word first), and its inputs.
@@ -346,16 +350,16 @@ int object_spans(InventoryState& s, const float* occ, const int16_t* labels, int
 // Collision checks (collide.cu; DESIGN.md, "Collision checks"), in the inventory's buffers: grid-only counts over a labelled
 // keep-all sweep, one device->host read per call.
 int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
-                 const dmnerf_edit_move* cands_host, int n, const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host,
-                 cudaStream_t st);
+                 const dmnerf_edit_move* cands_host, const int32_t* copies_host, int n, const uint32_t* obstacles_host,
+                 int64_t* overlap_host, int64_t* landed_host, cudaStream_t st, const char* who = "move_overlap");
 int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels, int64_t* faces_host,
                     cudaStream_t st);
 // The grid-only edit (DESIGN.md, "Arranging objects"): the moves applied in order to the state occ / labels, each target read
 // from the source grid at its nearest index; landed [n] and overwritten [n][128] per move.  Two read-backs: the grid checks of
-// both grids before the first edit, the counts at the end.
+// both grids before the first edit, the counts at the end.  copies_host [n] (NULL: none): the copies, which take and never vacate.
 int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels, int dim, float level, const double* T16,
-              const double* ext3, const dmnerf_edit_move* moves_host, int n, float* occ, int16_t* labels, int64_t* landed_host,
-              int64_t* overwritten_host, cudaStream_t st);
+              const double* ext3, const dmnerf_edit_move* moves_host, const int32_t* copies_host, int n, float* occ, int16_t* labels,
+              int64_t* landed_host, int64_t* overwritten_host, cudaStream_t st, const char* who = "grid_edit");
 // The grid check of both: flags in *bad (device) for NaN in occ and labels outside [0, n_labels - 1].  read_checked copies
 // `bytes` from dev to host and synchronises; the buffer starts with that flag word, and a set flag fails the call.
 int launch_grid_check(const float* occ, const int16_t* labels, int64_t n, int n_labels, int* bad, cudaStream_t st);
@@ -373,17 +377,19 @@ int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int di
 // The same for the object as each move of bases_host [n][12] leaves it (DESIGN.md, "Turned placements"): one column table, then
 // per base the moved object's bytes, runs and map; status [n] says which were placed.  The object is sampled from occ / labels,
 // the obstacles and support labels come from the scene scene_occ / scene_labels (DESIGN.md, "Arranging objects"); passing the
-// same grid twice is dmnerf_placement_maps.
+// same grid twice is dmnerf_placement_maps.  copy (DESIGN.md, "Copying objects"): the object is a copy, and the scene's points of
+// its label stay obstacles.  who: the entry point's name in errors (NULL: placement_maps or placement_maps_in_scene).
 int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels, int dim,
-                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, const double* bases_host,
+                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy, const double* bases_host,
                    const int32_t* box_host, int n_bases, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
-                   int32_t* status, cudaStream_t st);
+                   int32_t* status, cudaStream_t st, const char* who = nullptr);
 // base_host NULL: the object as it lies (dmnerf_placement_contacts; the scene must be the object's grid); otherwise as base_host
 // [12] and box_host [6] leave it, sampled from occ / labels, in the scene scene_occ / scene_labels.
 int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels,
-                       int dim, float level, const double* T16, const double* ext3, const dmnerf_placement* p, const double* base_host,
+                       int dim, float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy,
+                       const double* base_host,
                        const int32_t* box_host, int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
-                       int32_t* drop_host, cudaStream_t st);
+                       int32_t* drop_host, cudaStream_t st, const char* who = nullptr);
 
 // Connected components (components.cu): the solid points of a labelled grid split into canonically numbered components.
 // Per-context device buffers: the status words a call reads back, the chunk counts and the scan's storage.

@@ -677,6 +677,20 @@ int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const doubl
   return 0;
 }
 
+int copy_flags_check(const dmnerf_edit_move* moves, const int32_t* copies, int n, bool ordered, const char* who) {
+  if (!copies) return 0;
+  for (int i = 0; i < n; ++i) {
+    DMN_CHECK(copies[i] == 0 || copies[i] == 1, "%s: move %d: copy flag %d is not 0 or 1", who, i, copies[i]);
+    DMN_CHECK(!copies[i] || !moves[i].rest_drop, "%s: move %d: a copy cannot drop the rest of its label (it vacates nothing)", who,
+              i);
+    if (!ordered || copies[i]) continue;
+    for (int j = 0; j < i; ++j)
+      DMN_CHECK(!copies[j] || moves[j].label != moves[i].label,
+                "%s: move %d of label %d follows copy %d of that label (its vacate would erase the copy)", who, i, moves[i].label, j);
+  }
+  return 0;
+}
+
 // One thread per grid point of the slab: its target t (edit_target) and whether the nearest grid index of t lies in the box.
 __global__ void edit_target_kernel(const GridXform g, const EditMove m, int64_t begin, int64_t count, float* __restrict__ tgt,
                                    int32_t* __restrict__ flag) {
@@ -708,7 +722,8 @@ __global__ void edit_count_kernel(const int32_t* flag, const int32_t* pos, int64
   out[0] = (int64_t)pos[count - 1] + flag[count - 1];
 }
 
-// One thread per grid point of the slab: take the target's (occ, label), or vacate the point.
+// One thread per grid point of the slab: take the target's (occ, label), or vacate the point (never for a COPY).
+template <bool COPY>
 __global__ void edit_apply_kernel(const GridXform g, const EditMove m, int64_t begin, int64_t count, const int32_t* __restrict__ flag,
                                   const int32_t* __restrict__ pos, const float* __restrict__ tgt, const float* __restrict__ raw, int c,
                                   float voxel, float level, float* __restrict__ occ, int16_t* __restrict__ labels) {
@@ -717,7 +732,7 @@ __global__ void edit_apply_kernel(const GridXform g, const EditMove m, int64_t b
   const int64_t p = begin + i;
   const float o = occ[p];
   const int l = labels[p];
-  edit_rule(
+  edit_rule<COPY>(
       m, flag[i] != 0,
       [&](int& lt, float& ot) {
         const float* r = raw + (int64_t)pos[i] * c;
@@ -765,13 +780,16 @@ int edit_targets(MeshState& s, const double* T16, const double* ext3, int dim, c
 }
 
 int edit_apply(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
-               const float* raw, int c, float voxel, float level, float* occ, int16_t* labels, cudaStream_t st) {
+               const float* raw, int c, float voxel, float level, float* occ, int16_t* labels, bool copy, cudaStream_t st) {
   float* tgt;
   int32_t *flag, *pos;
   if (s.edit_t.get((size_t)count * 3, &tgt) || s.edit_flag.get((size_t)count, &flag) || s.edit_pos.get((size_t)count, &pos))
     return 2;                                                     // as edit_targets left them
-  edit_apply_kernel<<<blocks(count, 256), 256, 0, st>>>(make_xform(T16, ext3, dim), m, begin, count, flag, pos, tgt, raw, c, voxel,
-                                                        level, occ, labels);
+  const GridXform g = make_xform(T16, ext3, dim);
+  if (copy)
+    edit_apply_kernel<true><<<blocks(count, 256), 256, 0, st>>>(g, m, begin, count, flag, pos, tgt, raw, c, voxel, level, occ, labels);
+  else
+    edit_apply_kernel<false><<<blocks(count, 256), 256, 0, st>>>(g, m, begin, count, flag, pos, tgt, raw, c, voxel, level, occ, labels);
   DMN_LAUNCH_OK();
   return 0;
 }

@@ -47,6 +47,7 @@ __device__ __forceinline__ int64_t point_of(const Frame& f, int h1, int h2, int 
 
 // What the placed object and the obstacles are (DESIGN.md, "Object placement"): S = labels == label, solid, kept by the piece;
 // O = solid, label among the obstacles, not vacated (labels == label and in the piece -- every point without one -- or rest_drop).
+// A COPY (DESIGN.md, "Copying objects") vacates nothing: its own label's solid points are obstacles like any other.
 struct Placed {
   Region piece;                               // bits NULL: the whole label
   ObjMask obstacles;
@@ -68,6 +69,7 @@ struct __align__(8) ObjRun {
   int16_t h1, h2, z0, z1;
 };
 
+template <bool COPY>
 __device__ __forceinline__ void classify(const Frame& f, const GridXform& g, const Placed& m, const float* __restrict__ occ,
                                          const int16_t* __restrict__ labels, float level, int64_t p, bool& obst, bool& obj) {
   const float v = occ[p];
@@ -83,7 +85,7 @@ __device__ __forceinline__ void classify(const Frame& f, const GridXform& g, con
       keep = !region_drops(m.piece, m.label, q[0], q[1], q[2]);
     }
     obj = keep;
-    if (keep || m.rest_drop) obst = false;                       // vacated by the move
+    if (!COPY && (keep || m.rest_drop)) obst = false;            // vacated by the move
   }
 }
 
@@ -91,7 +93,8 @@ __device__ __forceinline__ void classify(const Frame& f, const GridXform& g, con
 // (the height when the down axis is the fastest, the column's h2 otherwise); each warp then scans 4 of the columns with its lanes
 // on the heights (a warp max-scan, carried from chunk to chunk) and writes 32 contiguous table entries and, with OBJECT (the
 // object as it lies), object bytes.  A moved object's bytes come from place_moved_kernel; the table never depends on the move.
-template <bool OBJECT>
+// COPY: the table of a copy's scene, whose own label stays (always with a base, so never with OBJECT).
+template <bool OBJECT, bool COPY = false>
 __global__ void __launch_bounds__(CP_WARPS * 32) place_column_kernel(const Frame f, const GridXform g, const Placed m,
                                                                      const float* __restrict__ occ, const int16_t* __restrict__ labels,
                                                                      float level, int16_t* __restrict__ table,
@@ -111,7 +114,7 @@ __global__ void __launch_bounds__(CP_WARPS * 32) place_column_kernel(const Frame
       uint8_t bits = 0;
       if (c < n_cols && y < f.dim) {
         bool obst, obj;
-        classify(f, g, m, occ, labels, level, point_of(f, (int)(c / f.dim), (int)(c % f.dim), y), obst, obj);
+        classify<COPY>(f, g, m, occ, labels, level, point_of(f, (int)(c / f.dim), (int)(c % f.dim), y), obst, obj);
         bits = (obst ? 1 : 0) | (obj ? 2 : 0);
       }
       s[cl][yl] = bits;
@@ -365,6 +368,7 @@ struct Prepared {
   Frame f;
   GridXform g;
   Placed m;
+  bool copy;                                  // the object is a copy: the scene's points of its label stay obstacles
   const float* occ;
   const int16_t* labels;
   const float* src_occ;
@@ -384,7 +388,7 @@ enum { PLACED = 0, NO_POINTS = 1, TOP_OUT = 2 };   // dmnerf_placement_maps' sta
 
 // The host checks of every placement call, before any launch: the object's grid occ / labels and the scene.
 int check(const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels, int dim, float level,
-          const double* T16, const double* ext3, const dmnerf_placement* p, const char* who, Prepared& q) {
+          const double* T16, const double* ext3, const dmnerf_placement* p, int copy, const char* who, Prepared& q) {
   DMN_CHECK(occ && labels && scene_occ && scene_labels && T16 && ext3 && p, "%s: NULL argument", who);
   DMN_CHECK(dim >= 2 && dim <= PLACE_MAX_DIM, "%s: dim %d out of range [2, %d]", who, dim, PLACE_MAX_DIM);
   if (sweep_grid_check(T16, ext3, dim, level, who)) return 1;
@@ -392,6 +396,9 @@ int check(const float* occ, const int16_t* labels, const float* scene_occ, const
   DMN_CHECK(p->axis >= 0 && p->axis <= 2, "%s: down axis %d is not 0, 1 or 2", who, p->axis);
   DMN_CHECK(p->sign == 1 || p->sign == -1, "%s: the sign of down along its axis must be +1 or -1, got %d", who, p->sign);
   DMN_CHECK(p->lift >= 0 && p->lift <= dim - 1, "%s: lift %d takes the object out of the grid [0, %d]", who, p->lift, dim - 1);
+  DMN_CHECK(copy == 0 || copy == 1, "%s: copy flag %d is not 0 or 1", who, copy);
+  DMN_CHECK(!copy || !p->rest_drop, "%s: a copy cannot drop the rest of its label (it vacates nothing)", who);
+  q.copy = copy != 0;
   Placed& m = q.m;
   if (piece_region(p->piece, p->label, m.piece, who, 0)) return 1;
   for (int k = 0; k < 4; ++k) m.obstacles.w[k] = p->obstacles[k];
@@ -450,6 +457,8 @@ int columns(PlaceState& s, Prepared& q, bool unmoved, cudaStream_t stream) {
   const unsigned blocks = (unsigned)((n_cols + TILE - 1) / TILE);
   if (unmoved)
     place_column_kernel<true><<<blocks, CP_WARPS * 32, 0, stream>>>(q.f, q.g, q.m, q.occ, q.labels, q.level, q.table, q.object);
+  else if (q.copy)
+    place_column_kernel<false, true><<<blocks, CP_WARPS * 32, 0, stream>>>(q.f, q.g, q.m, q.occ, q.labels, q.level, q.table, nullptr);
   else
     place_column_kernel<false><<<blocks, CP_WARPS * 32, 0, stream>>>(q.f, q.g, q.m, q.occ, q.labels, q.level, q.table, nullptr);
   DMN_LAUNCH_OK();
@@ -558,7 +567,7 @@ int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int di
   memset(info, 0, sizeof(*info));
   Prepared q;
   int why;
-  if (check(occ, labels, occ, labels, dim, level, T16, ext3, p, who, q)) return 1;
+  if (check(occ, labels, occ, labels, dim, level, T16, ext3, p, 0, who, q)) return 1;
   if (const int rc = columns(s, q, true, st)) return rc;
   if (const int rc = object_runs(s, q, nullptr, true, who, &why, st)) return rc;
   if (unplaced(q, why, false, who)) return 1;
@@ -568,10 +577,10 @@ int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int di
 }
 
 int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels, int dim,
-                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, const double* bases_host,
+                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy, const double* bases_host,
                    const int32_t* box_host, int n_bases, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
-                   int32_t* status, cudaStream_t st) {
-  const char* who = occ == scene_occ && labels == scene_labels ? "placement_maps" : "placement_maps_in_scene";
+                   int32_t* status, cudaStream_t st, const char* who) {
+  if (!who) who = occ == scene_occ && labels == scene_labels ? "placement_maps" : "placement_maps_in_scene";
   DMN_CHECK(drop && contacts && support && info && status, "%s: NULL argument", who);
   DMN_CHECK(n_bases >= 1 && n_bases <= DMNERF_MAX_BASES, "%s: between 1 and %d bases are supported, got %d", who, DMNERF_MAX_BASES,
             n_bases);
@@ -581,7 +590,7 @@ int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const
     status[i] = NO_POINTS;
   }
   Prepared q;
-  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, who, q)) return 1;
+  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, copy, who, q)) return 1;
   std::vector<EditMove> e(n_bases);
   for (int i = 0; i < n_bases; ++i)
     if (base_move(p, bases_host + 12 * i, box_host, T16, ext3, dim, e[i], who, i)) return 1;
@@ -599,19 +608,21 @@ int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const
 }
 
 int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels,
-                       int dim, float level, const double* T16, const double* ext3, const dmnerf_placement* p, const double* base_host,
-                       const int32_t* box_host, int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
-                       int32_t* drop_host, cudaStream_t st) {
+                       int dim, float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy,
+                       const double* base_host, const int32_t* box_host, int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                       int32_t* drop_host, cudaStream_t st, const char* who) {
   const bool moved = base_host != nullptr;
-  const char* who = !moved ? "placement_contacts"
-                           : (occ == scene_occ && labels == scene_labels ? "placement_contacts_moved" : "placement_contacts_in_scene");
+  if (!who)
+    who = !moved ? "placement_contacts"
+                 : (occ == scene_occ && labels == scene_labels ? "placement_contacts_moved" : "placement_contacts_in_scene");
   DMN_CHECK(n_cells_host && drop_host && max_cells >= 0 && (max_cells == 0 || cells_host), "%s: bad output arguments", who);
   *n_cells_host = 0;
   *drop_host = -1;
   Prepared q;
   EditMove e;
   int why;
-  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, who, q)) return 1;
+  DMN_CHECK(moved || !copy, "%s: a copy is placed through a base", who);
+  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, copy, who, q)) return 1;
   if (moved) {
     DMN_CHECK(box_host, "%s: box is NULL", who);
     if (base_move(p, base_host, box_host, T16, ext3, dim, e, who, 0)) return 1;

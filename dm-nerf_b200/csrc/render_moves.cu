@@ -69,7 +69,8 @@ __global__ void move_count_kernel(const int32_t* flag, const int32_t* pos, int64
 //   vacate: otherwise label_p == label && ((the piece keeps p, every p without one) && p's index in the box
 //                                          || rest_drop && the piece does not keep p).
 // Unlike the sweep's vacate there is no occ_p > level test (a render composites every density, so a vacated object must leave no
-// haze); the box bounds the vacate instead.
+// haze); the box bounds the vacate instead.  A COPY (DESIGN.md, "Copying objects") takes the same rows and never vacates.
+template <bool COPY>
 __global__ void move_apply_kernel(const EditMove m, const float* __restrict__ rays_o, const float* __restrict__ rays_d,
                                   const float* __restrict__ z, int64_t ns, int s, int c, float voxel, float level,
                                   const int32_t* __restrict__ flag, const int32_t* __restrict__ pos, const uint8_t* __restrict__ pin,
@@ -88,6 +89,7 @@ __global__ void move_apply_kernel(const EditMove m, const float* __restrict__ ra
       return;
     }
   }
+  if (COPY) return;
   if (argmax_sigmoid(r + 4, c - 4) != m.label) return;
   bool in_piece = true;
   if (has_piece) {
@@ -101,9 +103,9 @@ __global__ void move_apply_kernel(const EditMove m, const float* __restrict__ ra
   if (in_piece ? pin[i] != 0 : m.rest_drop != 0) r[3] = 0.0f;
 }
 
-int render_moves_pass(MovesState& s, const Network& net, bool f16, const EditMove* moves, int n_moves, const float* rays_o,
-                      const float* rays_d, const float* z, int64_t n, int s_per_ray, int c, float voxel, float level, float* raw,
-                      int64_t* evaluated, cudaStream_t st) {
+int render_moves_pass(MovesState& s, const Network& net, bool f16, const EditMove* moves, const int32_t* copies, int n_moves,
+                      const float* rays_o, const float* rays_d, const float* z, int64_t n, int s_per_ray, int c, float voxel,
+                      float level, float* raw, int64_t* evaluated, cudaStream_t st) {
   const int64_t ns = n * s_per_ray;
   if (ns == 0) return 0;
   DMN_CHECK(ns < INT32_MAX, "render_moved: %lld samples in one pass exceed the 32-bit scan", (long long)ns);
@@ -136,8 +138,12 @@ int render_moves_pass(MovesState& s, const Network& net, bool f16, const EditMov
       if (s.raw.get((size_t)cnt * c, &traw)) return 2;
       if (int rc = launch_mlp_tc(net, nullptr, pts, dirs, nullptr, cnt, 1, traw, nullptr, st, f16)) return rc;
     }
-    move_apply_kernel<<<blocks(ns, 256), 256, 0, st>>>(m, rays_o, rays_d, z, ns, s_per_ray, c, voxel, level, flag, pos, pin, tgt, traw,
-                                                       raw);
+    if (copies && copies[i])
+      move_apply_kernel<true><<<blocks(ns, 256), 256, 0, st>>>(m, rays_o, rays_d, z, ns, s_per_ray, c, voxel, level, flag, pos, pin, tgt,
+                                                               traw, raw);
+    else
+      move_apply_kernel<false><<<blocks(ns, 256), 256, 0, st>>>(m, rays_o, rays_d, z, ns, s_per_ray, c, voxel, level, flag, pos, pin,
+                                                                tgt, traw, raw);
     DMN_LAUNCH_OK();
     *evaluated += cnt;
   }

@@ -92,8 +92,8 @@ __device__ __forceinline__ bool edit_takes(int lt, float ot, int label, float o,
 //   take:   in the box && lt == label && (ot > level || o <= level) && (no piece || !drops_target()): take(ot) writes
 //           (o, l) <- (ot, label);
 //   vacate: otherwise l == label && o > level && (no piece || p in the piece || rest_drop): vacate() writes o <- 0, the label
-//           kept.
-template <class Move, class Target, class DropsTarget, class InPiece, class Take, class Vacate>
+//           kept.  A copy (COPY, DESIGN.md, "Copying objects") takes as a move does and never vacates.
+template <bool COPY = false, class Move, class Target, class DropsTarget, class InPiece, class Take, class Vacate>
 __device__ __forceinline__ void edit_rule(const Move m, bool in_box, const Target& target, float o, int l, float level,
                                           const DropsTarget& drops_target, const InPiece& in_piece_of, const Take& take,
                                           const Vacate& vacate) {
@@ -107,7 +107,7 @@ __device__ __forceinline__ void edit_rule(const Move m, bool in_box, const Targe
       return;
     }
   }
-  if (l == m.label && o > level) {
+  if (!COPY && l == m.label && o > level) {
     bool in_piece = true;
     if (has_piece) in_piece_of(in_piece);
     if (in_piece || m.rest_drop) vacate();

@@ -254,6 +254,38 @@ def _check_boxes(boxes, m, dim):
     return b
 
 
+def move_copies(copies, m):
+    """copies (None, a bool, or one bool per move, like rest) -> [bool] of m: True where the move is a copy (DESIGN.md, "Copying
+    objects"), which takes as the move would and leaves its source in place."""
+    if copies is None:
+        return [False] * m
+    flags = [copies] * m if isinstance(copies, (bool, np.bool_)) else list(copies) if hasattr(copies, "__iter__") else None
+    if flags is None or len(flags) != m or any(not isinstance(c, (bool, np.bool_)) for c in flags):
+        raise ValueError("copies must be None, True / False, or one of them for each of the %d moves, got %r" % (m, copies))
+    return [bool(c) for c in flags]
+
+
+def _check_copies(copies, mv, drops, ordered=True):
+    """The copy flags of moves with labels mv and rest drops `drops`, checked -> [bool]: no copy drops the rest of its label (it
+    vacates nothing) and, when the moves apply in order, no move of a label follows a copy of it (its vacate would erase the copy,
+    which carries the label)."""
+    flags = move_copies(copies, len(mv))
+    for i, (c, d) in enumerate(zip(flags, drops)):
+        if c and d:
+            raise ValueError("copy: move %d: a copy cannot drop the rest of its label (rest 'drop'): it vacates nothing" % i)
+        if ordered and not c:
+            for j in range(i):
+                if flags[j] and mv[j] == mv[i]:
+                    raise ValueError("copy: move %d of label %d follows copy %d of that label (its vacate would erase the copy)"
+                                     % (i, mv[i], j))
+    return flags
+
+
+def _copy_flags(flags):
+    """The HOST int32 copy flags of the _copies entry points."""
+    return (C.c_int32 * len(flags))(*[int(c) for c in flags])
+
+
 def _region_keeps(region, T, dim, extents, device, slab=1 << 20):
     """bool [dim]^3: the sweep grid points a piece keeps for a label it applies to -- inside its grid with the bit set, or
     outside it when it keeps outside samples -- by the render kernels' own test (region_contains)."""
@@ -293,11 +325,12 @@ def solid_box(occ, labels, label, level=0.45, margin=2, keep=None):
 
 
 def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, extents=None, level=0.45, near=4.0, far=15.0,
-                   N_importance=128, pieces=None, rest="keep", slab=0):
+                   N_importance=128, pieces=None, rest="keep", slab=0, copies=None):
     """dmnerf_mesh_occupancy_edit: the moves [(label, 4x4)] applied in order, in place, to occ / labels ([dim]^3 float32 /
     int16 on the device: the keep-all sweep of model_fine on this grid), the network evaluated only at the target points
-    inside each move's box (boxes: [m, 6] inclusive index boxes, EMPTY_BOX for none).  pieces / rest: as manipulator.  Returns
-    the number of target points evaluated."""
+    inside each move's box (boxes: [m, 6] inclusive index boxes, EMPTY_BOX for none).  pieces / rest: as manipulator.  copies
+    (None, a bool or one per move): the moves that are copies, which take as the move would and never vacate
+    (dmnerf_mesh_occupancy_edit_copies; DESIGN.md, "Copying objects").  Returns the number of target points evaluated."""
     from .manipulator import _piece_region, move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -309,6 +342,7 @@ def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, exten
     level = _check_level(level)
     boxes = _check_boxes(boxes, len(mv), dim)
     drops = move_rests(rest, len(mv))
+    flags = _check_copies(copies, mv, drops)
     regions = move_pieces(pieces, mv, ins_num, occ.device) or [None] * len(mv)
     if not mv:
         return 0
@@ -324,10 +358,13 @@ def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, exten
     ctx.bind(slot, model_fine)
     ext = EXTENTS if extents is None else extents
     n = C.c_int64(0)
+    head = (ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(ext, 3), dim, (far - near) / N_importance, level, int(slab), descs)
+    tail = (len(mv), _lib.ptr(occ), _lib.ptr(labels, torch.int16), C.byref(n))
     with torch.no_grad():
-        ctx.call("dmnerf_mesh_occupancy_edit", ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(ext, 3), dim,
-                 (far - near) / N_importance, level, int(slab), descs, len(mv), _lib.ptr(occ), _lib.ptr(labels, torch.int16),
-                 C.byref(n))
+        if any(flags):
+            ctx.call("dmnerf_mesh_occupancy_edit_copies", *head, _copy_flags(flags), *tail)
+        else:
+            ctx.call("dmnerf_mesh_occupancy_edit", *head, *tail)
     return int(n.value)
 
 
@@ -348,13 +385,15 @@ def edit_boxes(occ, labels, moves, scene_transform, extents=None, level=0.45, ma
 
 
 def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128,
-                 margin=2, boxes=None, pieces=None, rest="keep"):
+                 margin=2, boxes=None, pieces=None, rest="keep", copies=None):
     """The labelled sweep of the edited scene -> (occ [dim]^3 float32, labels [dim]^3 int16) on the device: the keep-all sweep of
     model_fine (occupancy_objects), then the moves [(label, 4x4 in the network frame, as manipulator_eval's transformation)]
     applied in order (edit_occupancy).  A move shows at p what the network holds at trans p, as rigid_rays renders it: the
     object lands at inv(trans) x.  boxes: per move the index box of the target points evaluated; by default the box of the
     moved label's solid points in the unedited grid (of those its piece keeps, with a piece) grown by `margin` voxels.
-    pieces / rest: as manipulator (a Region or None per move; "keep" / "drop", or one per move)."""
+    pieces / rest: as manipulator (a Region or None per move; "keep" / "drop", or one per move).  copies (None, a bool or one
+    per move; DESIGN.md, "Copying objects"): a copy takes as its move would and leaves the source in place; the copy keeps the
+    source's label: a second connected piece of it where it does not touch its source, one piece with it where it does."""
     from .manipulator import move_pieces, move_rests
     from .mesh import check_transform
     T = check_transform(scene_transform)
@@ -362,7 +401,7 @@ def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None,
     ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
     mv, _ = _check_moves(moves, ins_num)
     level = _check_level(level)
-    move_rests(rest, len(mv))
+    _check_copies(copies, mv, move_rests(rest, len(mv)))
     move_pieces(pieces, mv, ins_num, dev)
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
@@ -373,23 +412,24 @@ def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None,
                                         device=dev)
         if boxes is None:
             boxes = edit_boxes(occ, labels, moves, T, extents, level, margin, pieces)
-        edit_occupancy(model_fine, T, occ, labels, moves, boxes, extents, level, near, far, N_importance, pieces, rest)
+        edit_occupancy(model_fine, T, occ, labels, moves, boxes, extents, level, near, far, N_importance, pieces, rest, copies=copies)
     return occ, labels
 
 
 def edited_mesh(model_fine, scene_transform, moves, grid_dim=256, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128,
-                margin=2, boxes=None, pieces=None, rest="keep", min_cluster=400, per_object=False):
+                margin=2, boxes=None, pieces=None, rest="keep", min_cluster=400, per_object=False, copies=None):
     """The mesh of an edited scene: edited_sweep (same arguments) -> marching cubes -> scene space -> normals -> small-cluster
     removal.  Returns extract_mesh's keys as device tensors -- vertices, triangles, normals, clean_vertices, clean_normals,
     clean_triangles -- and labels (int64 per clean vertex: mesh.vertex_labels of its index-space vertex, the label of the
     inside end of its edge, from the edited grid; no label rays are rendered).  per_object: also objects, the
-    meshes_from_labelled_grid of the edited grid for every label with solid points except ins_num."""
+    meshes_from_labelled_grid of the edited grid for every label with solid points except ins_num.  copies: as edited_sweep."""
     from .mesh import EXTENTS, check_transform, clean_mesh, marching_cubes, to_scene, vertex_labels, vertex_normals
     T = check_transform(scene_transform)
     ext = EXTENTS if extents is None else extents
     ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
     with torch.no_grad():
-        occ, labels = edited_sweep(model_fine, T, moves, grid_dim, ext, level, near, far, N_importance, margin, boxes, pieces, rest)
+        occ, labels = edited_sweep(model_fine, T, moves, grid_dim, ext, level, near, far, N_importance, margin, boxes, pieces, rest,
+                                   copies=copies)
         v_idx, tris = marching_cubes(occ, level)
         verts = to_scene(v_idx, T, grid_dim, ext)
         normals = vertex_normals(verts, tris)
@@ -408,12 +448,14 @@ def edited_mesh(model_fine, scene_transform, moves, grid_dim=256, extents=None, 
 # and a mesh of one edit agree.  render_rays(moves=) and render_frame(moves=) take the value render_moves returns.
 class MovedScene:
     """Checked moves for render_rays(moves=) / render_frame(moves=): the dmnerf_render_moves the library reads, and the move
-    descriptions and region bits it points into, held for as long as the value lives.  Immutable."""
-    __slots__ = ("_desc", "_held", "device", "labels", "boxes", "rest_drop", "level", "voxel")
+    descriptions and region bits it points into, held for as long as the value lives.  copies: per move, whether it is a copy
+    (DESIGN.md, "Copying objects").  Immutable."""
+    __slots__ = ("_desc", "_held", "device", "labels", "boxes", "rest_drop", "level", "voxel", "copies", "_flags")
 
-    def __init__(self, desc, held, device, labels, boxes, rest_drop, level, voxel):
+    def __init__(self, desc, held, device, labels, boxes, rest_drop, level, voxel, copies=None):
+        copies = tuple(bool(c) for c in copies) if copies is not None else (False,) * len(labels)
         for k, v in zip(self.__slots__, (desc, held, device, labels, tuple(map(tuple, boxes.tolist())), tuple(rest_drop), level,
-                                         voxel)):
+                                         voxel, copies, _copy_flags(copies) if any(copies) else None)):
             object.__setattr__(self, k, v)
 
     def __setattr__(self, key, value):
@@ -423,15 +465,19 @@ class MovedScene:
         """The dmnerf_render_moves of these moves."""
         return self._desc
 
+    def copy_flags(self):
+        """The copy flags dmnerf_render_moved_copies reads (HOST int32 [n_moves]), or None when no move is a copy."""
+        return self._flags
+
 
 def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128, margin=2,
-                 boxes=None, pieces=None, rest="keep"):
+                 boxes=None, pieces=None, rest="keep", copies=None):
     """The moves [(label, 4x4 in the network frame)] of edited_sweep, checked for the moved render -> a MovedScene.  occ / labels:
     the unedited keep-all sweep ([dim]^3 float32 / int16 on the device) that the default boxes come from (edit_boxes, as
     edited_sweep) and whose grid (scene_transform, extents, dim) the boxes index.  level, margin, boxes, pieces, rest: as
     edited_sweep; the voxel of the occupancy test is the sweep's (far - near) / N_importance.  moves, pieces and rest may be
     arrange_objects' moves, pieces and rest unchanged, or manipulator_eval's [(label, 4x4)].  Labels are checked against the
-    networks when the render runs."""
+    networks when the render runs.  copies: as edited_sweep (arrange_objects' copies unchanged)."""
     from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -441,6 +487,7 @@ def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, 
         raise ValueError("render_moves: give between 1 and %d moves" % _lib.MAX_MOVES)
     level = _check_level(level)
     drops = move_rests(rest, len(mv))
+    flags = _check_copies(copies, mv, drops)
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
     with np.errstate(divide="ignore", invalid="ignore"):
@@ -460,7 +507,7 @@ def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     d.extents[:] = np.asarray(ext, dtype=np.float64).reshape(-1).tolist()
     d.level, d.voxel = level, float(voxel)
     return MovedScene(d, (descs, [r.bits for r in regions if r is not None]), occ.device, tuple(mv), boxes, drops, level,
-                      float(voxel))
+                      float(voxel), flags)
 
 
 # ----------------------------------------------------------------------------------------------------------------- collisions
@@ -482,13 +529,14 @@ def _check_sweep(occ, labels, who):
 
 
 def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, boxes=None, margin=2, pieces=None, rest="keep",
-                 obstacles=None):
+                 obstacles=None, copies=None):
     """dmnerf_move_overlap: each move [(label, 4x4 in the network frame)] checked on its own against the labelled keep-all sweep
     occ / labels ([dim]^3 float32 / int16 on the device; an edited_sweep result is accepted unchanged).  boxes, margin, pieces,
     rest: as edited_sweep (default boxes: edit_boxes).  obstacles: the labels that count as obstacles (default every label).
     Returns one dict per move: label, landed (the voxels the moved object occupies after the move), overlap {label: voxels}
     (labels with voxels > 0: solid obstacle points the moved object lands on; the points the move vacates are not obstacles),
-    overlap_volume {label: voxels times the inventory's voxel volume} and total (the overlapping voxels)."""
+    overlap_volume {label: voxels times the inventory's voxel volume} and total (the overlapping voxels).  copies (None, a bool or
+    one per move; DESIGN.md, "Copying objects"): a copy vacates nothing, so its own label's solid points are obstacles too."""
     from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -498,6 +546,7 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     mv, mats = _check_moves(moves, ins_num, _lib.MAX_CANDIDATES)
     level = _check_level(level)
     drops = move_rests(rest, len(mv))
+    flags = _check_copies(copies, mv, drops, ordered=False)
     regions = move_pieces(pieces, mv, ins_num, occ.device) or [None] * len(mv)
     words = ALL_LABELS if obstacles is None else label_words(obstacles)
     if not mv:
@@ -509,9 +558,12 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     overlap = np.zeros((len(mv), MAX_LABELS), dtype=np.int64)
     landed = np.zeros(len(mv), dtype=np.int64)
     ctx = get_context(occ.device)
-    ctx.call("dmnerf_move_overlap", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), dim, level, _lib.doubles(T, 16),
-             _lib.doubles(ext, 3), descs, len(mv), (C.c_uint32 * 4)(*words), overlap.ctypes.data_as(C.POINTER(C.c_int64)),
-             landed.ctypes.data_as(C.POINTER(C.c_int64)))
+    head = (ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), dim, level, _lib.doubles(T, 16), _lib.doubles(ext, 3), descs)
+    tail = (len(mv), (C.c_uint32 * 4)(*words), overlap.ctypes.data_as(C.POINTER(C.c_int64)), landed.ctypes.data_as(C.POINTER(C.c_int64)))
+    if any(flags):
+        ctx.call("dmnerf_move_overlap_copies", *head, _copy_flags(flags), *tail)
+    else:
+        ctx.call("dmnerf_move_overlap", *head, *tail)
     unit = _voxel_volume(T, ext, dim)
     return [_count_report(mv[i], landed[i], overlap[i], unit, "overlap") for i in range(len(mv))]
 
@@ -671,7 +723,7 @@ def _check_point(x, what):
 
 
 def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=None, level=0.45, piece=None, rest="keep",
-                  obstacles=None, base=None, box=None, scene=None):
+                  obstacles=None, base=None, box=None, scene=None, copy=False):
     """dmnerf_placement_map: object `label` (or its piece, with rest "keep" / "drop" as move_overlap) raised by `lift` voxels and
     lowered along the index axis closest to +-down (network frame, chosen as supports chooses it), at every horizontal offset
     that keeps it inside the grid of the labelled keep-all sweep occ / labels.  obstacles: the labels that count (default all).
@@ -681,6 +733,9 @@ def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=Non
     scene (DESIGN.md, "Arranging objects"): an (occ, labels) pair of the same shape, dtype and device, e.g. an edited_grid
     result; the object is still sampled from occ / labels, but the obstacles, the points it vacates and the labels it rests on
     come from the scene (dmnerf_placement_maps_in_scene; without a base, the identity base with the default box).
+    copy (DESIGN.md, "Copying objects"): place a copy of the object, its source standing: the scene's solid points of the label
+    stay obstacles.  A copy always takes the based path (the identity base with the default box without one) and the scene is
+    occ / labels when none is given; rest must be "keep".
     Returns a dict:
       drop, support, contacts: device maps [U, V] (int32, int16, int32): the voxels it falls (-1: blocked where it is raised),
                       the obstacle label under most of its resting runs (-1: blocked, or resting on the grid's floor), and the
@@ -698,7 +753,7 @@ def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=Non
         base = _move_matrix(base, 0)
     if box is not None:
         box = _check_boxes([box], 1, occ.shape[0])[0]
-    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene)
+    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene, copy)
     if base is None and c["scene"] is not None:
         m, status = _placement_maps(c, [np.eye(4)], _placement_box(c, box), _object_points(c))
         if m[0] is None:
@@ -740,8 +795,8 @@ def _check_scene(scene, occ, labels):
     return s_occ, s_lab
 
 
-def _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene=None):
-    """The checked arguments of a placement call: grid, level, label, lift, down axis, scene and the ABI placement."""
+def _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene=None, copy=False):
+    """The checked arguments of a placement call: grid, level, label, lift, down axis, scene, copy and the ABI placement."""
     from .manipulator import _piece_region, move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -751,11 +806,14 @@ def _placement_call(occ, labels, scene_transform, label, down, lift, extents, le
     if isinstance(lift, (bool, np.bool_)) or int(lift) != lift or int(lift) < 0:
         raise ValueError("placement: lift must be an integer >= 0 voxels, got %r" % (lift,))
     rest_drop = move_rests(rest, 1)[0]
+    copy = _check_copies(copy, [label], [rest_drop])[0]
     words = ALL_LABELS if obstacles is None else label_words(obstacles)
     A, _ = grid_affine(T, 2, ext)
     axis, sign = down_axis((A / np.linalg.norm(A, axis=0)).T, down, "placement")
     dim = _check_sweep(occ, labels, "placement_map")
     scene = _check_scene(scene, occ, labels)
+    if copy and scene is None:                         # a copy's source stands in the grid it is sampled from
+        scene = (occ, labels)
     if not 2 <= dim <= PLACE_MAX_DIM:
         raise ValueError("placement: dim %d outside [2, %d]" % (dim, PLACE_MAX_DIM))
     if int(lift) > dim - 1:
@@ -765,7 +823,7 @@ def _placement_call(occ, labels, scene_transform, label, down, lift, extents, le
                           axis=axis, sign=sign, lift=int(lift))
     desc.obstacles[:] = words
     return {"occ": occ, "labels": labels, "T": T, "ext": ext, "level": level, "label": label, "lift": int(lift), "axis": axis,
-            "sign": sign, "dim": dim, "desc": desc, "piece": piece, "scene": scene}
+            "sign": sign, "dim": dim, "desc": desc, "piece": piece, "scene": scene, "copy": copy}
 
 
 def _placement_library(name, occ, *args):
@@ -811,7 +869,8 @@ def _map_result(c, info, drop, contacts, support, base, box, points_before):
             "centre": centre, "runs": int(info.runs), "points": n, "height": (int(info.height[0]), int(info.height[1])),
             "lift": c["lift"], "label": c["label"], "dim": dim, "base": base, "box": None if box is None else tuple(int(x) for x in box),
             "points_before": points_before,
-            "_call": (c["occ"], c["labels"], c["T"], c["ext"], c["level"], c["desc"], c["piece"]), "_scene": c.get("scene")}
+            "_call": (c["occ"], c["labels"], c["T"], c["ext"], c["level"], c["desc"], c["piece"]), "_scene": c.get("scene"),
+            "copy": bool(c.get("copy"))}
 
 
 def _placement_maps(c, bases, box, points_before):
@@ -825,12 +884,14 @@ def _placement_maps(c, bases, box, points_before):
     status = np.zeros(n, dtype=np.int32)
     rows = np.ascontiguousarray([np.asarray(b, dtype=np.float64)[:3].reshape(-1) for b in bases])
     grids = (_lib.ptr(occ), _lib.ptr(c["labels"], torch.int16))
-    name = "dmnerf_placement_maps"
+    name, copy = "dmnerf_placement_maps", ()
     if c.get("scene") is not None:
         grids += (_lib.ptr(c["scene"][0]), _lib.ptr(c["scene"][1], torch.int16))
         name = "dmnerf_placement_maps_in_scene"
+    if c.get("copy"):
+        name, copy = "dmnerf_placement_maps_in_scene_copy", (1,)
     _placement_library(name, occ, *grids, dim, c["level"], _lib.doubles(c["T"], 16), _lib.doubles(c["ext"], 3), C.byref(c["desc"]),
-                       rows.ctypes.data_as(C.POINTER(C.c_double)), (C.c_int32 * 6)(*[int(x) for x in box]), n,
+                       *copy, rows.ctypes.data_as(C.POINTER(C.c_double)), (C.c_int32 * 6)(*[int(x) for x in box]), n,
                        _lib.ptr(drop, torch.int32), _lib.ptr(contacts, torch.int32), _lib.ptr(support, torch.int16), infos,
                        status.ctypes.data_as(C.POINTER(C.c_int32)))
     maps = [None if status[i] else _map_result(c, infos[i], drop[i], contacts[i], support[i], np.asarray(bases[i], dtype=np.float64),
@@ -903,8 +964,9 @@ def placement(m, u, v):
     scene = m.get("_scene")
     if scene is not None:                              # the scene of the map: the object from occ / labels (identity base by default)
         base = np.eye(4) if m.get("base") is None else m["base"]
-        ctx.call("dmnerf_placement_contacts_in_scene", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), _lib.ptr(scene[0]),
-                 _lib.ptr(scene[1], torch.int16), *head[3:], _lib.doubles(base[:3], 12), (C.c_int32 * 6)(*m["box"]), *tail)
+        name, copy = ("dmnerf_placement_contacts_in_scene_copy", (1,)) if m.get("copy") else ("dmnerf_placement_contacts_in_scene", ())
+        ctx.call(name, ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), _lib.ptr(scene[0]), _lib.ptr(scene[1], torch.int16),
+                 *head[3:], *copy, _lib.doubles(base[:3], 12), (C.c_int32 * 6)(*m["box"]), *tail)
     elif m.get("base") is None:
         ctx.call("dmnerf_placement_contacts", *head, *tail)
     else:
@@ -992,7 +1054,7 @@ def _turn_angles(turns):
 
 
 def place_object(occ, labels, scene_transform, label, down, near, on=None, stable=True, lift=0, max_tests=64, extents=None,
-                 level=0.45, piece=None, rest="keep", obstacles=None, turns=None, scene=None):
+                 level=0.45, piece=None, rest="keep", obstacles=None, turns=None, scene=None, copy=False):
     """The placement of object `label` (or its piece) closest to the network-frame point `near`: over placement_map's offsets
     that are not blocked and rest on an obstacle whose label is in `on` (default: any), ordered by the distance of the placed
     centre of mass from `near` across the down axis (ties: the lowest (u, v)), the first that is stable -- testing at most
@@ -1002,19 +1064,20 @@ def place_object(occ, labels, scene_transform, label, down, near, on=None, stabl
     {"placement": placement() of it, or None; "reason": None, or why there is none; "candidates": how many offsets qualified;
     "tested": stability tests run; "map": the placement_map result it came from (without turns: the map); "turn": its angle
     (None without turns); "maps": [(angle, map)] of the turns that were mapped; "unfit": the angles whose turned object does not
-    fit the grid; "unplaced": the angles whose turned object has no point or leaves the grid at this lift}.  scene: as
-    placement_map's (DESIGN.md, "Arranging objects")."""
+    fit the grid; "unplaced": the angles whose turned object has no point or leaves the grid at this lift}.  scene, copy: as
+    placement_map's (DESIGN.md, "Arranging objects", "Copying objects"); the placement of a copy is the copy's move."""
     near = _check_point(near, "near")
     if isinstance(max_tests, (bool, np.bool_)) or int(max_tests) != max_tests or int(max_tests) < 1:
         raise ValueError("placement: max_tests must be an integer >= 1, got %r" % (max_tests,))
     on = None if on is None else set(_labels(on, MAX_LABELS - 1, "placement"))
     angles = None if turns is None else _turn_angles(turns)
     if turns is None:
-        m = placement_map(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene=scene)
+        m = placement_map(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene=scene,
+                          copy=copy)
         maps, unfit, unplaced = [(None, m)], [], []
     else:
         maps, unfit, unplaced = turned_placement_maps(occ, labels, scene_transform, label, down, angles, lift, extents, level, piece,
-                                                      rest, obstacles, scene)
+                                                      rest, obstacles, scene, copy)
     out = {"placement": None, "reason": None, "candidates": 0, "tested": 0, "map": maps[0][1] if turns is None else None,
            "turn": None, "maps": [] if turns is None else maps, "unfit": unfit, "unplaced": unplaced}
     rows = placement_candidates([m for _, m in maps], near, on)
@@ -1036,14 +1099,14 @@ def place_object(occ, labels, scene_transform, label, down, near, on=None, stabl
 
 
 def turned_placement_maps(occ, labels, scene_transform, label, down, turns, lift=0, extents=None, level=0.45, piece=None,
-                          rest="keep", obstacles=None, scene=None):
+                          rest="keep", obstacles=None, scene=None, copy=False):
     """placement_map of the object turned about the down axis by each of `turns` (degrees, or an integer K: 360 k / K), the
     turns built by turn_bases from the object's solid box and exact centre, mapped in dmnerf_placement_maps calls of at most
     MAX_BASES bases, with edit_boxes' source box -> ([(angle, map)] of the turns mapped, the angles that do not fit the grid,
-    the angles whose turned object has no point or its top out of the grid).  scene: as placement_map's; the turns are built from
-    the object in occ / labels."""
+    the angles whose turned object has no point or its top out of the grid).  scene, copy: as placement_map's; the turns are
+    built from the object in occ / labels."""
     angles = _turn_angles(turns)
-    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene)
+    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene, copy)
     points, box, centre = _object_extent(_object_mask(c))
     if points == 0:
         raise ValueError("placement: label %d has no solid points%s" % (c["label"], " in its piece" if piece is not None else ""))
@@ -1114,32 +1177,38 @@ def largest_component_grid(occ, labels, level, objects):
 # ----------------------------------------------------------------------------------------------------------------- arrangement
 # DESIGN.md, "Arranging objects": the edited sweep's rule with the network replaced by the unedited grid at the nearest index
 # (edited_grid), and several objects placed one after another, each in the scene the earlier placements leave (arrange_objects).
-ARRANGE_KEYS = ("label", "near", "on", "piece", "rest", "turns", "stable", "lift", "obstacles")
+ARRANGE_KEYS = ("label", "near", "on", "piece", "rest", "turns", "stable", "lift", "obstacles", "copy")
 
 
-def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes, drops, regions):
-    """dmnerf_grid_edit of checked moves: applied in place to occ / labels, sampled from src_occ / src_labels -> edited_grid's
-    report."""
+def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes, drops, regions, flags=None):
+    """dmnerf_grid_edit of checked moves (flags: the checked copy flags, None for none): applied in place to occ / labels,
+    sampled from src_occ / src_labels -> edited_grid's report."""
     n, dim = len(mv), occ.shape[0]
     overwritten = np.zeros((n, MAX_LABELS), dtype=np.int64)
     landed = np.zeros(n, dtype=np.int64)
     ctx = get_context(occ.device)
-    ctx.call("dmnerf_grid_edit", ctx.handle, _lib.ptr(src_occ), _lib.ptr(src_labels, torch.int16), dim, level, _lib.doubles(T, 16),
-             _lib.doubles(ext, 3), _edit_moves(mv, mats, boxes, drops, regions, occ.device), n, _lib.ptr(occ),
-             _lib.ptr(labels, torch.int16), landed.ctypes.data_as(C.POINTER(C.c_int64)),
-             overwritten.ctypes.data_as(C.POINTER(C.c_int64)))
+    head = (ctx.handle, _lib.ptr(src_occ), _lib.ptr(src_labels, torch.int16), dim, level, _lib.doubles(T, 16), _lib.doubles(ext, 3),
+            _edit_moves(mv, mats, boxes, drops, regions, occ.device))
+    tail = (n, _lib.ptr(occ), _lib.ptr(labels, torch.int16), landed.ctypes.data_as(C.POINTER(C.c_int64)),
+            overwritten.ctypes.data_as(C.POINTER(C.c_int64)))
+    if flags is not None and any(flags):
+        ctx.call("dmnerf_grid_edit_copies", *head, _copy_flags(flags), *tail)
+    else:
+        ctx.call("dmnerf_grid_edit", *head, *tail)
     unit = _voxel_volume(T, ext, dim)
     return [_count_report(mv[i], landed[i], overwritten[i], unit, "overwritten") for i in range(n)]
 
 
-def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, boxes=None, margin=2, pieces=None, rest="keep"):
+def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, boxes=None, margin=2, pieces=None, rest="keep",
+                copies=None):
     """dmnerf_grid_edit: edited_sweep's moves applied in order to the labelled keep-all sweep occ / labels ([dim]^3 float32 / int16
     on the device) without the network: a move shows at p the unedited grid at the nearest grid index of trans p, as the collision
     checks sample a moved object.  On a grid whose points and steps are exact in fp32, whole-voxel translations and quarter turns
     give edited_sweep's grid bit for bit; elsewhere it is the sweep resampled at its own resolution.  boxes, margin, pieces, rest:
     as edited_sweep (default boxes: edit_boxes of occ / labels).  Works on copies -> (occ', labels', report), report one dict per
     move: label, landed (the voxels it takes from a solid target), overwritten {label: voxels} (labels with voxels > 0: solid
-    points of the grid as the earlier moves left it that it lands on and does not vacate), overwritten_volume and total."""
+    points of the grid as the earlier moves left it that it lands on and does not vacate), overwritten_volume and total.
+    copies: as edited_sweep (DESIGN.md, "Copying objects"); a copy's overwritten counts its own label's points too."""
     from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -1148,6 +1217,7 @@ def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, b
     mv, mats = _check_moves(moves, MAX_LABELS - 1)
     level = _check_level(level)
     drops = move_rests(rest, len(mv))
+    flags = _check_copies(copies, mv, drops)
     regions = move_pieces(pieces, mv, MAX_LABELS - 1, occ.device) or [None] * len(mv)
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
@@ -1157,7 +1227,7 @@ def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, b
     out_occ, out_labels = occ.clone(memory_format=torch.contiguous_format), labels.clone(memory_format=torch.contiguous_format)
     if not mv:
         return out_occ, out_labels, []
-    return out_occ, out_labels, _grid_edit(occ, labels, out_occ, out_labels, T, ext, level, mv, mats, boxes, drops, regions)
+    return out_occ, out_labels, _grid_edit(occ, labels, out_occ, out_labels, T, ext, level, mv, mats, boxes, drops, regions, flags)
 
 
 def _check_items(items, dim, device):
@@ -1181,10 +1251,18 @@ def _check_items(items, dim, device):
                 raise ValueError("arrange: item %d needs %r" % (i, k))
         c = {k: it.get(k) for k in ARRANGE_KEYS}
         c["label"] = _labels([c["label"]], MAX_LABELS - 1, "arrange")[0]
-        if c["label"] in seen:
+        c["copy"] = False if c["copy"] is None else c["copy"]
+        if not isinstance(c["copy"], (bool, np.bool_)):
+            raise ValueError("arrange: item %d: copy must be True or False, got %r" % (i, c["copy"]))
+        c["copy"] = bool(c["copy"])
+        kinds = seen.setdefault(c["label"], {})
+        if not c["copy"] and "move" in kinds:
             raise ValueError("arrange: items %d and %d share label %d (the second move would also vacate the first one's landed "
-                             "points)" % (seen[c["label"]], i, c["label"]))
-        seen[c["label"]] = i
+                             "points)" % (kinds["move"], i, c["label"]))
+        if not c["copy"] and "copy" in kinds:
+            raise ValueError("arrange: item %d moves label %d after item %d copies it (the move would also vacate the copy)"
+                             % (i, c["label"], kinds["copy"]))
+        kinds.setdefault("copy" if c["copy"] else "move", i)
         c["near"] = _check_point(c["near"], "near")
         if c["on"] is not None:
             c["on"] = _labels(c["on"], MAX_LABELS - 1, "arrange")
@@ -1198,7 +1276,8 @@ def _check_items(items, dim, device):
             raise ValueError("arrange: item %d: lift must be an integer in [0, %d] voxels, got %r" % (i, dim - 1, c["lift"]))
         c["lift"] = int(c["lift"])
         c["rest"] = "keep" if c["rest"] is None else c["rest"]
-        move_rests(c["rest"], 1)
+        if move_rests(c["rest"], 1)[0] and c["copy"]:
+            raise ValueError("arrange: item %d: a copy cannot drop the rest of its label (rest 'drop'): it vacates nothing" % i)
         if c["piece"] is not None:
             move_pieces([c["piece"]], [c["label"]], MAX_LABELS - 1, device)
         if c["obstacles"] is not None:
@@ -1213,14 +1292,19 @@ def arrange_objects(occ, labels, scene_transform, items, down, extents=None, lev
     place_object with the object from the unedited grid and scene = the state, and when it is placed its move is applied to the
     state by the grid-only edit (edited_grid's rule, the default box); an item that is not placed stays where it is and is an
     obstacle for the items after it.  items: dicts with label and near (network frame) and optionally on (labels to rest on; an
-    earlier item keeps its label where it landed), piece, rest, turns, stable, lift and obstacles, as place_object takes them;
-    at most MAX_MOVES items, no two with one label.  down: shared by every item.  Every item is checked before any device work.
+    earlier item keeps its label where it landed), piece, rest, turns, stable, lift and obstacles, as place_object takes them, and
+    copy (DESIGN.md, "Copying objects"; default False): place a copy of the object from the unedited grid, its source standing as
+    an obstacle (`on` may name its own label, to stack it on its source).  At most MAX_MOVES items; no two moves of one label, no
+    move of a label after a copy of it; copies of one label may repeat and may follow its move.  down: shared by every item.
+    Every item is checked before any device work.
     Returns a dict:
       items:  per item, place_object's result and its label; placement None and a reason when it was not placed (its maps were
               computed on the state before its own move and refer to the state's tensors, which later items edit);
-      moves:  [(label, 4x4 nested list)] of the placed items in order, and pieces / rest aligned with them: manipulate_frame,
-              manipulator_eval, edited_sweep and edited_mesh take them unchanged;
-      occ, labels: the arranged grid, equal to edited_grid(occ, labels, ..., moves, pieces=pieces, rest=rest) bit for bit;
+      moves:  [(label, 4x4 nested list)] of the placed items in order, and pieces / rest / copies aligned with them:
+              manipulate_frame, manipulator_eval, edited_sweep and edited_mesh take them unchanged (copies: edited_sweep,
+              edited_mesh, edited_grid and render_moves);
+      occ, labels: the arranged grid, equal to edited_grid(occ, labels, ..., moves, pieces=pieces, rest=rest, copies=copies) bit
+              for bit;
       report: edited_grid's report of each placed move (overwritten: what it landed on in the scene left before it)."""
     from .manipulator import move_rests
     from .mesh import EXTENTS, check_transform
@@ -1238,11 +1322,11 @@ def arrange_objects(occ, labels, scene_transform, items, down, extents=None, lev
     if not 2 <= dim <= PLACE_MAX_DIM:
         raise ValueError("placement: dim %d outside [2, %d]" % (dim, PLACE_MAX_DIM))
     state_occ, state_labels = occ.clone(memory_format=torch.contiguous_format), labels.clone(memory_format=torch.contiguous_format)
-    out = {"items": [], "moves": [], "pieces": [], "rest": [], "occ": state_occ, "labels": state_labels, "report": []}
+    out = {"items": [], "moves": [], "pieces": [], "rest": [], "copies": [], "occ": state_occ, "labels": state_labels, "report": []}
     for it in checked:
         try:
             r = place_object(occ, labels, T, it["label"], down, it["near"], it["on"], it["stable"], it["lift"], max_tests, ext, level,
-                             it["piece"], it["rest"], it["obstacles"], it["turns"], scene=(state_occ, state_labels))
+                             it["piece"], it["rest"], it["obstacles"], it["turns"], scene=(state_occ, state_labels), copy=it["copy"])
         except ValueError as e:        # found on the device: no solid points (in its piece), or the lift takes its top out
             r = {"placement": None, "reason": str(e)}
         out["items"].append(dict(r, label=it["label"]))
@@ -1253,10 +1337,11 @@ def arrange_objects(occ, labels, scene_transform, items, down, extents=None, lev
         pieces = None if it["piece"] is None else [it["piece"]]
         box = edit_boxes(occ, labels, [move], T, ext, level, 2, pieces)
         out["report"] += _grid_edit(occ, labels, state_occ, state_labels, T, ext, level, [it["label"]],
-                                    [np.asarray(trans, dtype=np.float64)], box, move_rests(it["rest"], 1), [it["piece"]])
+                                    [np.asarray(trans, dtype=np.float64)], box, move_rests(it["rest"], 1), [it["piece"]], [it["copy"]])
         out["moves"].append(move)
         out["pieces"].append(it["piece"])
         out["rest"].append(it["rest"])
+        out["copies"].append(it["copy"])
     return out
 
 

@@ -637,6 +637,50 @@ DMNERF_API int dmnerf_placement_contacts_in_scene(dmnerf_ctx* ctx, const float* 
                                                   int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host, int32_t* drop_host,
                                                   void* stream);
 
+/* ---- copying objects (DESIGN.md, "Copying objects"; no counterpart in the original) ----------------------------------------
+ * A copy is a move that leaves its source in place: it takes exactly as the move with the same fields takes (same target, box,
+ * piece test and air clause) and writes the source's label, and it never vacates.  The entry points below are the ones they are
+ * named after with copy flags: copies_host [n] (HOST int32, one per move or candidate; NULL: none) or `copy` (one per call),
+ * each 0 or 1.  With every flag 0 each equals its namesake bit for bit.
+ * dmnerf_mesh_occupancy_edit_copies, dmnerf_grid_edit_copies, dmnerf_render_moved_copies: a copy skips the vacate.  In
+ *   dmnerf_grid_edit_copies a copy's overwritten_host counts every solid state point it lands on, its own label's included.
+ * dmnerf_move_overlap_copies: a copy candidate's own label's solid points are obstacles like any other (with or without a
+ *   piece).  The candidates are grouped by kind on the host, one launch per kind; the results stay in the caller's order.
+ * dmnerf_placement_maps_in_scene_copy, dmnerf_placement_contacts_in_scene_copy: with copy, the scene's solid points of the label
+ *   are obstacles (the object's source stays where it is).
+ * Rejected on the host, before any launch, beside everything the namesake rejects: a flag other than 0 or 1, a copy with
+ * rest_drop (a copy vacates nothing), and, for the moves applied in order (not dmnerf_move_overlap_copies' independent
+ * candidates), a move of a label after a copy of it (its vacate would erase the copy, which carries the label). */
+DMNERF_API int dmnerf_mesh_occupancy_edit_copies(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host,
+                                                 int dim, float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host,
+                                                 const int32_t* copies_host /* [n] */, int n_moves, float* occ, int16_t* labels,
+                                                 int64_t* evaluated_host, void* stream);
+DMNERF_API int dmnerf_grid_edit_copies(dmnerf_ctx* ctx, const float* src_occ, const int16_t* src_labels, int dim, float level,
+                                       const double* transform_host, const double* extents_host, const dmnerf_edit_move* moves_host,
+                                       const int32_t* copies_host /* [n] */, int n_moves, float* occ, int16_t* labels,
+                                       int64_t* landed_host /* [n] */, int64_t* overwritten_host /* [n][128] */, void* stream);
+DMNERF_API int dmnerf_render_moved_copies(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                          const dmnerf_render_moves* moves, const int32_t* copies_host /* [n_moves] */,
+                                          int64_t* evaluated_host, void* stream);
+DMNERF_API int dmnerf_move_overlap_copies(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                          const double* transform_host, const double* extents_host,
+                                          const dmnerf_edit_move* candidates_host, const int32_t* copies_host /* [n] */,
+                                          int n_candidates, const uint32_t* obstacles_host, int64_t* overlap_host /* [n][128] */,
+                                          int64_t* landed_host /* [n] */, void* stream);
+DMNERF_API int dmnerf_placement_maps_in_scene_copy(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                                   const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                                   const double* extents_host, const dmnerf_placement* placement, int copy,
+                                                   const double* bases_host /* [n][12] */, const int32_t* box_host /* [6] */,
+                                                   int n_bases, int32_t* drop, int32_t* contacts, int16_t* support,
+                                                   dmnerf_placement_info* info_host /* [n] */, int32_t* status_host /* [n] */,
+                                                   void* stream);
+DMNERF_API int dmnerf_placement_contacts_in_scene_copy(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                                       const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                                       const double* extents_host, const dmnerf_placement* placement, int copy,
+                                                       const double* base_host /* [12] */, const int32_t* box_host /* [6] */, int u,
+                                                       int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                                                       int32_t* drop_host, void* stream);
+
 /* ---- connected components (DESIGN.md, "Connected components"; no counterpart in the original) --------------------------------
  * The solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order, p = (i dim + j) dim + k) split into components:
  * two solid points are adjacent when they are face neighbours (connectivity 6) or face, edge or corner neighbours (26), never

@@ -107,7 +107,15 @@ def parse(argv=None):
     ap.add_argument("--tolerance", type=int, default=0, help="--until-contact: overlapping voxels tolerated")
     ap.add_argument("--render", choices=("exchanger", "samples"), default="exchanger",
                     help="render the frame with the exchanger (manipulate_frame) or per sample (render_frame(moves=))")
+    ap.add_argument("--copy", action="store_true", help="copy the piece instead of moving it: the source stays (needs --render samples)")
     a = ap.parse_args(argv)
+    if a.copy:
+        if a.render != "samples":
+            ap.error("--copy needs --render samples: the exchanger renders moves only")
+        if a.rest == "drop":
+            ap.error("--copy cannot drop the rest of the label: a copy vacates nothing")
+        if a.until_contact:
+            ap.error("--copy cannot be combined with --until-contact: a copy starts inside its source")
     if a.arrange is not None:
         for flag, given in (("--place-at", a.place_at is not None), ("--mode", a.mode is not None),
                             ("--until-contact", a.until_contact), ("--distance", a.distance is not None), ("--yaw", a.yaw is not None),
@@ -119,6 +127,8 @@ def parse(argv=None):
             ap.error("--arrange needs --down X Y Z, not 0 0 0")
         if a.on is not None or a.lift is not None or a.any_stability:
             ap.error("--on, --lift and --any-stability are per item with --arrange")
+        if a.copy:
+            ap.error('--copy is per item with --arrange: give the items "copy": true')
         a.lift, a.turns = 0, 1
     elif a.place_at is not None:
         for flag, given in (("--mode", a.mode is not None), ("--until-contact", a.until_contact), ("--distance", a.distance is not None),
@@ -161,7 +171,7 @@ def parse(argv=None):
     return a
 
 
-ITEM_KEYS = ("label", "piece", "near", "on", "turns", "rest", "any_stability")
+ITEM_KEYS = ("label", "piece", "near", "on", "turns", "rest", "any_stability", "copy")
 
 
 def read_spec(path):
@@ -174,6 +184,8 @@ def read_spec(path):
         if not isinstance(it, dict) or set(it) - set(ITEM_KEYS) or ("label" in it) == ("piece" in it) or "near" not in it:
             raise SystemExit("move_objects: item %d of %s needs exactly one of label / piece, near, and only the keys %s"
                              % (i, path, ", ".join(ITEM_KEYS)))
+        if not isinstance(it.get("copy", False), bool):
+            raise SystemExit("move_objects: item %d of %s: copy must be true or false" % (i, path))
     return spec
 
 
@@ -208,19 +220,19 @@ def arrange_pieces(a, occ, labels, T, ext, spec, chosen):
     items = []
     for it, (_, label, region) in zip(spec, chosen):
         items.append({"label": label, "near": it["near"], "on": it.get("on"), "piece": region, "rest": it.get("rest", "keep"),
-                      "turns": it.get("turns"), "stable": not it.get("any_stability", False)})
+                      "turns": it.get("turns"), "stable": not it.get("any_stability", False), "copy": it.get("copy", False)})
     r = arrange_objects(occ, labels, T, items, a.down, ext, a.level)
     rec, report = [], iter(r["report"])
-    for (piece, label, _), res in zip(chosen, r["items"]):
+    for it, (piece, label, _), res in zip(spec, chosen, r["items"]):
         p = res["placement"]
         entry = {"label": label, "piece": piece, "placed": p is not None, "reason": res.get("reason"),
                  "offset": None if p is None else list(p["offset"]), "drop": None if p is None else p["drop"],
                  "support": None if p is None else p["support"], "stable": None if p is None else p["stable"],
-                 "turn": res.get("turn")}
+                 "turn": res.get("turn"), "copy": bool(it.get("copy", False))}
         if p is not None:
             entry["overwritten"] = {str(k): v for k, v in next(report)["overwritten"].items()}
         rec.append(entry)
-    return r["moves"], r["pieces"], r["rest"], rec
+    return r["moves"], r["pieces"], r["rest"], r["copies"], rec
 
 
 def choose_piece(a, model_fine, T, ext):
@@ -267,7 +279,7 @@ def place_piece(a, occ, labels, T, ext, label, region):
     qualifies."""
     from dmnerf_b200.objects import place_object
     r = place_object(occ, labels, T, label, a.down, a.place_at, on=a.on, stable=not a.any_stability, lift=a.lift, extents=ext,
-                     level=a.level, piece=region, rest=a.rest, turns=None if a.turns == 1 else a.turns)
+                     level=a.level, piece=region, rest=a.rest, turns=None if a.turns == 1 else a.turns, copy=a.copy)
     p = r["placement"]
     if p is None:
         raise SystemExit("move_objects: no placement: %s" % r["reason"])
@@ -301,6 +313,8 @@ def main(argv=None):
     slide = place = arranged = None
     if a.arrange is not None:
         spec = read_spec(a.arrange)
+        if any(it.get("copy", False) for it in spec) and a.render != "samples":
+            raise SystemExit("move_objects: an arrangement with copies needs --render samples: the exchanger renders moves only")
         chosen = choose_pieces(a, nets[1], T, ext, spec)
         piece, label, centre, region = None, None, None, None
     else:
@@ -315,7 +329,7 @@ def main(argv=None):
         slide = slide_translation(a, occ, labels, T, ext, label, region)
         a.distance = np.sign(a.distance) * (slide["found"] or 0.0)
     if a.arrange is not None:
-        moves, regions, rests, arranged = arrange_pieces(a, occ, labels, T, ext, spec, chosen)
+        moves, regions, rests, copies, arranged = arrange_pieces(a, occ, labels, T, ext, spec, chosen)
         if not moves:
             raise SystemExit("move_objects: no item was placed: %s" % "; ".join("%d: %s" % (e["label"], e["reason"]) for e in arranged))
         trans = {"transformations": [{"transformation": m, "mode": "placement"} for _, m in moves]}
@@ -326,13 +340,15 @@ def main(argv=None):
         trans = manipulation_transform(centre, a.mode, distance=a.distance, yaw=a.yaw, scale=a.scale)
     if a.arrange is None:
         moves, regions, rests = [(label, trans["transformations"][0]["transformation"])], [region], [a.rest]
+        copies = [a.copy]
     dev = next(nets[1].parameters()).device
     pose_t = torch.from_numpy(c2w).to(dev)
     evaluated = None
     if a.render == "samples":
         from dmnerf_b200.objects import render_moves
         from dmnerf_b200.render import render_frame
-        moved = render_moves(occ, labels, T, moves, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests)
+        moved = render_moves(occ, labels, T, moves, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests,
+                             copies=copies)
         with torch.no_grad():
             fr = render_frame(a.H, a.W, a.K, pose_t, a.near, a.far, nets[0], nets[1], a.N_samples, a.N_importance, keep_all_ins=True,
                               device=dev, moves=moved)
@@ -358,6 +374,8 @@ def main(argv=None):
         record = {"transformations": trans["transformations"], "label": label, "piece": piece, "centre": centre.tolist(),
                   "rest": a.rest}
     record["render"], record["evaluated"] = a.render, evaluated
+    if any(copies):
+        record["copies"] = copies
     if slide is not None:
         record["slide"] = slide
     if place is not None:
@@ -365,7 +383,7 @@ def main(argv=None):
     if a.check:
         from dmnerf_b200.objects import move_overlap
         r = move_overlap(occ, labels, T, [(label, trans["transformations"][0]["transformation"])], ext, a.level, pieces=[region],
-                         rest=a.rest)[0]
+                         rest=a.rest, copies=a.copy)[0]
         record["overlap"] = {"voxels": {str(k): v for k, v in r["overlap"].items()},
                              "volume": {str(k): v for k, v in r["overlap_volume"].items()}}
         record["landed"] = r["landed"]
@@ -374,7 +392,7 @@ def main(argv=None):
     if a.mesh:
         from dmnerf_b200.objects import edited_mesh
         m = edited_mesh(nets[1], T, moves, a.grid_dim, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests,
-                        min_cluster=a.min_cluster)
+                        min_cluster=a.min_cluster, copies=copies)
         M.write_ply(os.path.join(a.out, "edited.ply"), m["vertices"], m["triangles"])
         lab = m["labels"].cpu().numpy()
         colors = np.where((lab >= 0)[:, None], lut[np.clip(lab, 0, ins_num)], 0).astype(np.uint8)   # instance.png's colours
