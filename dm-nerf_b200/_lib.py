@@ -227,6 +227,28 @@ PROTOTYPES = {
                                                           C.POINTER(C.c_double), C.POINTER(C.c_int32), C.c_int, C.c_int,
                                                           C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int32),
                                                           C.c_void_p]),
+    "dmnerf_mesh_occupancy_edit_groups": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int,
+                                                    C.c_float, C.c_float, C.c_int64, C.POINTER(EditMove), C.POINTER(C.c_int32),
+                                                    C.POINTER(C.c_uint32), C.c_int, _f32p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_grid_edit_groups": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double),
+                                          C.POINTER(C.c_double), C.POINTER(EditMove), C.POINTER(C.c_int32), C.POINTER(C.c_uint32),
+                                          C.c_int, _f32p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_render_moved_groups": (C.c_int, [C.c_void_p, C.POINTER(RenderIO), C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
+                                             C.POINTER(RenderMoves), C.POINTER(C.c_int32), C.POINTER(C.c_uint32), C.POINTER(C.c_int64),
+                                             C.c_void_p]),
+    "dmnerf_move_overlap_groups": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double),
+                                             C.POINTER(C.c_double), C.POINTER(EditMove), C.POINTER(C.c_int32), C.POINTER(C.c_uint32),
+                                             C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_placement_maps_in_scene_group": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float,
+                                                       C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(Placement), C.c_int,
+                                                       C.POINTER(C.c_uint32), C.POINTER(C.c_double), C.POINTER(C.c_int32), C.c_int,
+                                                       C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PlacementInfo),
+                                                       C.POINTER(C.c_int32), C.c_void_p]),
+    "dmnerf_placement_contacts_in_scene_group": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float,
+                                                           C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(Placement), C.c_int,
+                                                           C.POINTER(C.c_uint32), C.POINTER(C.c_double), C.POINTER(C.c_int32), C.c_int,
+                                                           C.c_int, C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64),
+                                                           C.POINTER(C.c_int32), C.c_void_p]),
     "dmnerf_object_components": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int, C.c_void_p,
                                            C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_component_table": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,

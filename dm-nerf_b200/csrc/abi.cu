@@ -518,10 +518,11 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
 
 }  // extern "C"
 
-// dmnerf_render_moved with copy flags copies_host [n_moves] (NULL: none)
+// dmnerf_render_moved with copy flags copies_host [n_moves] (NULL: none) and label sets groups_host [n_moves][4] (NULL: each
+// move's own label)
 static int render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
-                        const dmnerf_render_moves* moves, const int32_t* copies_host, int64_t* evaluated_host, void* stream,
-                        const char* who) {
+                        const dmnerf_render_moves* moves, const int32_t* copies_host, const uint32_t* groups_host,
+                        int64_t* evaluated_host, void* stream, const char* who) {
   if (evaluated_host) evaluated_host[0] = evaluated_host[1] = 0;
   if (bound_pair(ctx, who)) return 1;
   DMN_CHECK(!(flags & ~RENDER_FLAGS), "%s: unknown flag bits 0x%x", who, flags & ~RENDER_FLAGS);
@@ -538,8 +539,10 @@ static int render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, 
   DMN_CHECK(n * (int64_t)(S + NI) < ((int64_t)1 << 31), "%s: %lld rays of %d samples reach 2^31 samples", who, (long long)n, S + NI);
   EditMove mv[DMNERF_MAX_MOVES];
   for (int i = 0; i < moves->n_moves; ++i)
-    if (edit_move_from_abi(moves->moves[i], moves->transform, moves->extents, moves->dim, ctx->net[0].p.ins_num, mv[i], who, i)) return 1;
-  if (copy_flags_check(moves->moves, copies_host, moves->n_moves, true, who)) return 1;
+    if (edit_move_from_abi(moves->moves[i], moves->transform, moves->extents, moves->dim, ctx->net[0].p.ins_num, mv[i], who, i,
+                           groups_host ? groups_host + 4 * i : nullptr))
+      return 1;
+  if (copy_flags_check(moves->moves, copies_host, groups_host, moves->n_moves, true, who)) return 1;
   Edit e;
   const Edit* edit;
   if (int rc = scene_edit(ctx, io ? io->edit : nullptr, (cudaStream_t)stream, e, edit, who)) return rc;
@@ -553,13 +556,19 @@ extern "C" {
 
 DMNERF_API int dmnerf_render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
                                    const dmnerf_render_moves* moves, int64_t* evaluated_host, void* stream) {
-  return render_moved(ctx, io, n, S, NI, flags, impl, moves, nullptr, evaluated_host, stream, "render_moved");
+  return render_moved(ctx, io, n, S, NI, flags, impl, moves, nullptr, nullptr, evaluated_host, stream, "render_moved");
 }
 
 DMNERF_API int dmnerf_render_moved_copies(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
                                           const dmnerf_render_moves* moves, const int32_t* copies_host, int64_t* evaluated_host,
                                           void* stream) {
-  return render_moved(ctx, io, n, S, NI, flags, impl, moves, copies_host, evaluated_host, stream, "render_moved_copies");
+  return render_moved(ctx, io, n, S, NI, flags, impl, moves, copies_host, nullptr, evaluated_host, stream, "render_moved_copies");
+}
+
+DMNERF_API int dmnerf_render_moved_groups(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                          const dmnerf_render_moves* moves, const int32_t* copies_host, const uint32_t* groups_host,
+                                          int64_t* evaluated_host, void* stream) {
+  return render_moved(ctx, io, n, S, NI, flags, impl, moves, copies_host, groups_host, evaluated_host, stream, "render_moved_groups");
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
@@ -821,10 +830,12 @@ DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* tra
 
 }  // extern "C"
 
-// dmnerf_mesh_occupancy_edit with copy flags copies_host [n_moves] (NULL: none)
+// dmnerf_mesh_occupancy_edit with copy flags copies_host [n_moves] (NULL: none) and label sets groups_host [n_moves][4] (NULL:
+// each move's own label)
 static int mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim, float voxel,
-                               float level, int64_t slab, const dmnerf_edit_move* moves_host, const int32_t* copies_host, int n_moves,
-                               float* occ, int16_t* labels, int64_t* evaluated_host, void* stream, const char* who) {
+                               float level, int64_t slab, const dmnerf_edit_move* moves_host, const int32_t* copies_host,
+                               const uint32_t* groups_host, int n_moves, float* occ, int16_t* labels, int64_t* evaluated_host,
+                               void* stream, const char* who) {
   if (bound_net(ctx, net, who)) return 1;
   if (evaluated_host) *evaluated_host = 0;
   DMN_CHECK(transform_host && extents_host && occ && labels, "%s: NULL argument", who);
@@ -834,8 +845,10 @@ static int mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform
   DMN_CHECK(n_moves == 0 || moves_host, "%s: moves is NULL", who);
   EditMove mv[DMNERF_MAX_MOVES];
   for (int i = 0; i < n_moves; ++i)
-    if (edit_move_from_abi(moves_host[i], transform_host, extents_host, dim, ctx->net[net].p.ins_num, mv[i], who, i)) return 1;
-  if (copy_flags_check(moves_host, copies_host, n_moves, true, who)) return 1;
+    if (edit_move_from_abi(moves_host[i], transform_host, extents_host, dim, ctx->net[net].p.ins_num, mv[i], who, i,
+                           groups_host ? groups_host + 4 * i : nullptr))
+      return 1;
+  if (copy_flags_check(moves_host, copies_host, groups_host, n_moves, true, who)) return 1;
   if (n_moves == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   DMN_CUDA(cudaSetDevice(ctx->device));
@@ -870,16 +883,24 @@ extern "C" {
 DMNERF_API int dmnerf_mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim,
                                           float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host, int n_moves,
                                           float* occ, int16_t* labels, int64_t* evaluated_host, void* stream) {
-  return mesh_occupancy_edit(ctx, net, transform_host, extents_host, dim, voxel, level, slab, moves_host, nullptr, n_moves, occ, labels,
-                             evaluated_host, stream, "mesh_occupancy_edit");
+  return mesh_occupancy_edit(ctx, net, transform_host, extents_host, dim, voxel, level, slab, moves_host, nullptr, nullptr, n_moves, occ,
+                             labels, evaluated_host, stream, "mesh_occupancy_edit");
 }
 
 DMNERF_API int dmnerf_mesh_occupancy_edit_copies(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host,
                                                  int dim, float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host,
                                                  const int32_t* copies_host, int n_moves, float* occ, int16_t* labels,
                                                  int64_t* evaluated_host, void* stream) {
-  return mesh_occupancy_edit(ctx, net, transform_host, extents_host, dim, voxel, level, slab, moves_host, copies_host, n_moves, occ,
-                             labels, evaluated_host, stream, "mesh_occupancy_edit_copies");
+  return mesh_occupancy_edit(ctx, net, transform_host, extents_host, dim, voxel, level, slab, moves_host, copies_host, nullptr, n_moves,
+                             occ, labels, evaluated_host, stream, "mesh_occupancy_edit_copies");
+}
+
+DMNERF_API int dmnerf_mesh_occupancy_edit_groups(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host,
+                                                 int dim, float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host,
+                                                 const int32_t* copies_host, const uint32_t* groups_host, int n_moves, float* occ,
+                                                 int16_t* labels, int64_t* evaluated_host, void* stream) {
+  return mesh_occupancy_edit(ctx, net, transform_host, extents_host, dim, voxel, level, slab, moves_host, copies_host, groups_host,
+                             n_moves, occ, labels, evaluated_host, stream, "mesh_occupancy_edit_groups");
 }
 
 DMNERF_API int dmnerf_mesh_vertex_labels(const float* verts, int64_t n, const float* occ, const int16_t* labels, int dim, float level,
@@ -967,8 +988,8 @@ DMNERF_API int dmnerf_move_overlap(dmnerf_ctx* ctx, const float* occ, const int1
                                    void* stream) {
   DMN_CHECK(ctx != nullptr, "move_overlap: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, nullptr, n_candidates,
-                      obstacles_host, overlap_host, landed_host, (cudaStream_t)stream);
+  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, nullptr, nullptr,
+                      n_candidates, obstacles_host, overlap_host, landed_host, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_move_overlap_copies(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
@@ -977,8 +998,19 @@ DMNERF_API int dmnerf_move_overlap_copies(dmnerf_ctx* ctx, const float* occ, con
                                           const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "move_overlap_copies: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, copies_host, n_candidates,
-                      obstacles_host, overlap_host, landed_host, (cudaStream_t)stream, "move_overlap_copies");
+  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, copies_host, nullptr,
+                      n_candidates, obstacles_host, overlap_host, landed_host, (cudaStream_t)stream, "move_overlap_copies");
+}
+
+DMNERF_API int dmnerf_move_overlap_groups(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                          const double* transform_host, const double* extents_host,
+                                          const dmnerf_edit_move* candidates_host, const int32_t* copies_host,
+                                          const uint32_t* groups_host, int n_candidates, const uint32_t* obstacles_host,
+                                          int64_t* overlap_host, int64_t* landed_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "move_overlap_groups: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, copies_host, groups_host,
+                      n_candidates, obstacles_host, overlap_host, landed_host, (cudaStream_t)stream, "move_overlap_groups");
 }
 
 DMNERF_API int dmnerf_object_contacts(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
@@ -1005,8 +1037,8 @@ DMNERF_API int dmnerf_placement_contacts(dmnerf_ctx* ctx, const float* occ, cons
                                          int32_t* drop_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "placement_contacts: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, 0, nullptr, nullptr, u, v,
-                            cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
+  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, 0, nullptr, nullptr,
+                            nullptr, u, v, cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_placement_maps(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
@@ -1015,8 +1047,8 @@ DMNERF_API int dmnerf_placement_maps(dmnerf_ctx* ctx, const float* occ, const in
                                      int16_t* support, dmnerf_placement_info* info_host, int32_t* status_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "placement_maps: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_maps(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, 0, bases_host, box_host, n_bases,
-                        drop, contacts, support, info_host, status_host, (cudaStream_t)stream);
+  return placement_maps(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, 0, nullptr, bases_host,
+                        box_host, n_bases, drop, contacts, support, info_host, status_host, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_placement_contacts_moved(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
@@ -1027,8 +1059,8 @@ DMNERF_API int dmnerf_placement_contacts_moved(dmnerf_ctx* ctx, const float* occ
   DMN_CHECK(ctx != nullptr, "placement_contacts_moved: ctx is NULL");
   DMN_CHECK(base_host != nullptr, "placement_contacts_moved: base is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, 0, base_host, box_host, u, v,
-                            cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
+  return placement_contacts(ctx->place, occ, labels, occ, labels, dim, level, transform_host, extents_host, placement, 0, nullptr, base_host,
+                            box_host, u, v, cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
 }
 
 // ---- arranging objects (DESIGN.md, "Arranging objects") -------------------------------------------------------------------
@@ -1038,8 +1070,8 @@ DMNERF_API int dmnerf_grid_edit(dmnerf_ctx* ctx, const float* src_occ, const int
                                 float* occ, int16_t* labels, int64_t* landed_host, int64_t* overwritten_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "grid_edit: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, nullptr, n_moves, occ,
-                   labels, landed_host, overwritten_host, (cudaStream_t)stream);
+  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, nullptr, nullptr, n_moves,
+                   occ, labels, landed_host, overwritten_host, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_grid_edit_copies(dmnerf_ctx* ctx, const float* src_occ, const int16_t* src_labels, int dim, float level,
@@ -1048,8 +1080,18 @@ DMNERF_API int dmnerf_grid_edit_copies(dmnerf_ctx* ctx, const float* src_occ, co
                                        int64_t* overwritten_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "grid_edit_copies: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, copies_host, n_moves, occ,
-                   labels, landed_host, overwritten_host, (cudaStream_t)stream, "grid_edit_copies");
+  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, copies_host, nullptr,
+                   n_moves, occ, labels, landed_host, overwritten_host, (cudaStream_t)stream, "grid_edit_copies");
+}
+
+DMNERF_API int dmnerf_grid_edit_groups(dmnerf_ctx* ctx, const float* src_occ, const int16_t* src_labels, int dim, float level,
+                                       const double* transform_host, const double* extents_host, const dmnerf_edit_move* moves_host,
+                                       const int32_t* copies_host, const uint32_t* groups_host, int n_moves, float* occ,
+                                       int16_t* labels, int64_t* landed_host, int64_t* overwritten_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "grid_edit_groups: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, copies_host, groups_host,
+                   n_moves, occ, labels, landed_host, overwritten_host, (cudaStream_t)stream, "grid_edit_groups");
 }
 
 DMNERF_API int dmnerf_placement_maps_in_scene(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
@@ -1059,7 +1101,7 @@ DMNERF_API int dmnerf_placement_maps_in_scene(dmnerf_ctx* ctx, const float* occ,
                                               dmnerf_placement_info* info_host, int32_t* status_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "placement_maps_in_scene: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
-  return placement_maps(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, 0,
+  return placement_maps(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, 0, nullptr,
                         bases_host, box_host, n_bases, drop, contacts, support, info_host, status_host, (cudaStream_t)stream);
 }
 
@@ -1072,8 +1114,21 @@ DMNERF_API int dmnerf_placement_maps_in_scene_copy(dmnerf_ctx* ctx, const float*
   DMN_CHECK(ctx != nullptr, "placement_maps_in_scene_copy: ctx is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
   return placement_maps(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, copy,
-                        bases_host, box_host, n_bases, drop, contacts, support, info_host, status_host, (cudaStream_t)stream,
+                        nullptr, bases_host, box_host, n_bases, drop, contacts, support, info_host, status_host, (cudaStream_t)stream,
                         "placement_maps_in_scene_copy");
+}
+
+DMNERF_API int dmnerf_placement_maps_in_scene_group(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                                    const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                                    const double* extents_host, const dmnerf_placement* placement, int copy,
+                                                    const uint32_t* group_host, const double* bases_host, const int32_t* box_host,
+                                                    int n_bases, int32_t* drop, int32_t* contacts, int16_t* support,
+                                                    dmnerf_placement_info* info_host, int32_t* status_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_maps_in_scene_group: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_maps(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, copy,
+                        group_host, bases_host, box_host, n_bases, drop, contacts, support, info_host, status_host, (cudaStream_t)stream,
+                        "placement_maps_in_scene_group");
 }
 
 DMNERF_API int dmnerf_placement_contacts_in_scene(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
@@ -1085,7 +1140,7 @@ DMNERF_API int dmnerf_placement_contacts_in_scene(dmnerf_ctx* ctx, const float* 
   DMN_CHECK(base_host != nullptr, "placement_contacts_in_scene: base is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
   return placement_contacts(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, 0,
-                            base_host, box_host, u, v, cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
+                            nullptr, base_host, box_host, u, v, cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream);
 }
 
 DMNERF_API int dmnerf_placement_contacts_in_scene_copy(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
@@ -1098,8 +1153,23 @@ DMNERF_API int dmnerf_placement_contacts_in_scene_copy(dmnerf_ctx* ctx, const fl
   DMN_CHECK(base_host != nullptr, "placement_contacts_in_scene_copy: base is NULL");
   DMN_CUDA(cudaSetDevice(ctx->device));
   return placement_contacts(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, copy,
-                            base_host, box_host, u, v, cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream,
+                            nullptr, base_host, box_host, u, v, cells_host, max_cells, n_cells_host, drop_host, (cudaStream_t)stream,
                             "placement_contacts_in_scene_copy");
+}
+
+DMNERF_API int dmnerf_placement_contacts_in_scene_group(dmnerf_ctx* ctx, const float* occ, const int16_t* labels,
+                                                        const float* scene_occ, const int16_t* scene_labels, int dim, float level,
+                                                        const double* transform_host, const double* extents_host,
+                                                        const dmnerf_placement* placement, int copy, const uint32_t* group_host,
+                                                        const double* base_host, const int32_t* box_host, int u, int v,
+                                                        int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                                                        int32_t* drop_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "placement_contacts_in_scene_group: ctx is NULL");
+  DMN_CHECK(base_host != nullptr, "placement_contacts_in_scene_group: base is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return placement_contacts(ctx->place, occ, labels, scene_occ, scene_labels, dim, level, transform_host, extents_host, placement, copy,
+                            group_host, base_host, box_host, u, v, cells_host, max_cells, n_cells_host, drop_host,
+                            (cudaStream_t)stream, "placement_contacts_in_scene_group");
 }
 
 // ---- connected components (DESIGN.md, "Connected components") -------------------------------------------------------------

@@ -36,6 +36,7 @@ struct Candidate {
   double lo[3], hi[3];
   int dlo[3], dhi[3];
   Region piece;                 // bits NULL: the whole label moves
+  ObjMask group;                // the labels that move together
   int label, rest_drop;
 };
 
@@ -123,14 +124,15 @@ __global__ void __launch_bounds__(OV_THREADS) move_overlap_kernel(const GridXfor
         src = edit_target(m.trans, map.inv, map.b, m.lo, m.hi, true, p, t, q);
         if (src) {
           const int64_t qi = ((int64_t)q[0] * d + (int64_t)q[1]) * d + (int64_t)q[2];
-          src = labels[qi] == m.label && occ[qi] > level && (m.piece.bits == nullptr || !region_drops(m.piece, m.label, t[0], t[1], t[2]));
+          const int lq = labels[qi];
+          src = in_group(m.group, lq) && occ[qi] > level && (m.piece.bits == nullptr || !region_drops(m.piece, lq, t[0], t[1], t[2]));
         }
       }
       const unsigned landed = __ballot_sync(FULL, src);
       if (lane == 0 && landed) atomicAdd(&hist[c][LANDED], (uint32_t)__popc(landed));
       bool hit = src && blocking;
-      if (!COPY && hit && l == m.label)                          // a point the move vacates is no obstacle
-        hit = !(m.rest_drop || m.piece.bits == nullptr || !region_drops(m.piece, m.label, p[0], p[1], p[2]));
+      if (!COPY && hit && in_group(m.group, l))                  // a point the move vacates is no obstacle
+        hit = !(m.rest_drop || m.piece.bits == nullptr || !region_drops(m.piece, l, p[0], p[1], p[2]));
       if (hit) atomicAdd(&hist[c][l], 1u);
     }
   }
@@ -163,7 +165,7 @@ __global__ void __launch_bounds__(GE_THREADS) grid_edit_kernel(const GridXform g
     double q[3];
     sweep_point(g, p, x);
     const bool in_box = edit_target(e.trans, e.inv, e.b, e.lo, e.hi, !e.empty, x, t, q);
-    auto here = [&] { return e.piece.bits == nullptr || !region_drops(e.piece, e.label, x[0], x[1], x[2]); };
+    auto here = [&](int lp) { return e.piece.bits == nullptr || !region_drops(e.piece, lp, x[0], x[1], x[2]); };
     edit_rule<COPY>(
         e, in_box,
         [&](int& lt, float& ot) {
@@ -171,12 +173,12 @@ __global__ void __launch_bounds__(GE_THREADS) grid_edit_kernel(const GridXform g
           lt = src_labels[qi];
           ot = src_occ[qi];
         },
-        o, l, level, [&] { return region_drops(e.piece, e.label, t[0], t[1], t[2]); }, [&](bool& b) { b = here(); },
-        [&](float ot) {
+        o, l, level, [&](int lt) { return region_drops(e.piece, lt, t[0], t[1], t[2]); }, [&](bool& b, int lp) { b = here(lp); },
+        [&](float ot, int lt) {
           occ[p] = ot;
-          labels[p] = (int16_t)e.label;
+          labels[p] = (int16_t)lt;
           landed = ot > level;
-          if (landed && o > level && (COPY || !(l == e.label && (e.rest_drop || here())))) atomicAdd(&hist[l], 1u);
+          if (landed && o > level && (COPY || !(in_group(e.group, l) && (e.rest_drop || here(l))))) atomicAdd(&hist[l], 1u);
         },
         [&] { occ[p] = 0.0f; });
   }
@@ -298,14 +300,14 @@ int read_checked(const void* dev, void* host, size_t bytes, int max_label, const
 }
 
 int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
-                 const dmnerf_edit_move* cands_host, const int32_t* copies_host, int n, const uint32_t* obstacles_host,
-                 int64_t* overlap_host, int64_t* landed_host, cudaStream_t st, const char* who) {
+                 const dmnerf_edit_move* cands_host, const int32_t* copies_host, const uint32_t* groups_host, int n,
+                 const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host, cudaStream_t st, const char* who) {
   DMN_CHECK(occ && labels && T16 && ext3 && overlap_host && landed_host, "%s: NULL argument", who);
   if (sweep_grid_check(T16, ext3, dim, level, who)) return 1;
   DMN_CHECK(n >= 1 && n <= DMNERF_MAX_CANDIDATES, "%s: between 1 and %d candidates are supported, got %d", who,
             DMNERF_MAX_CANDIDATES, n);
   DMN_CHECK(cands_host, "%s: candidates is NULL", who);
-  if (copy_flags_check(cands_host, copies_host, n, false, who)) return 1;   // each candidate on its own: no order
+  if (copy_flags_check(cands_host, copies_host, groups_host, n, false, who)) return 1;   // each candidate on its own: no order
   // the moves first, then the copies: one launch per kind, slot[i] the row of candidate i
   std::vector<int> slot(n);
   int n_moves = 0;
@@ -319,7 +321,8 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
   IndexMap map{};
   for (int i = 0; i < n; ++i) {
     EditMove e;
-    if (edit_move_from_abi(cands_host[i], T16, ext3, dim, DMNERF_MAX_INS, e, who, i)) return 1;
+    if (edit_move_from_abi(cands_host[i], T16, ext3, dim, DMNERF_MAX_INS, e, who, i, groups_host ? groups_host + 4 * i : nullptr))
+      return 1;
     if (i == 0) {
       memcpy(map.inv, e.inv, sizeof(map.inv));
       memcpy(map.b, e.b, sizeof(map.b));
@@ -335,6 +338,7 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
       destination_box(e, A, dim, c.dlo, c.dhi);
     }
     c.piece = e.piece;
+    c.group = e.group;
     c.label = e.label;
     c.rest_drop = e.rest_drop;
   }
@@ -436,8 +440,8 @@ int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, 
 }
 
 int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels, int dim, float level, const double* T16,
-              const double* ext3, const dmnerf_edit_move* moves_host, const int32_t* copies_host, int n, float* occ, int16_t* labels,
-              int64_t* landed_host, int64_t* overwritten_host, cudaStream_t st, const char* who) {
+              const double* ext3, const dmnerf_edit_move* moves_host, const int32_t* copies_host, const uint32_t* groups_host, int n,
+              float* occ, int16_t* labels, int64_t* landed_host, int64_t* overwritten_host, cudaStream_t st, const char* who) {
   DMN_CHECK(src_occ && src_labels && occ && labels && T16 && ext3 && landed_host && overwritten_host, "%s: NULL argument", who);
   DMN_CHECK(n >= 1 && n <= DMNERF_MAX_MOVES, "%s: between 1 and %d moves are supported, got %d", who, DMNERF_MAX_MOVES, n);
   DMN_CHECK(moves_host, "%s: moves is NULL", who);
@@ -454,8 +458,9 @@ int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels
             "%s: the source and state grids overlap in memory (the state must be a separate copy)", who);
   std::vector<EditMove> mv(n);
   for (int i = 0; i < n; ++i)
-    if (edit_move_from_abi(moves_host[i], T16, ext3, dim, DMNERF_MAX_INS, mv[i], who, i)) return 1;
-  if (copy_flags_check(moves_host, copies_host, n, true, who)) return 1;
+    if (edit_move_from_abi(moves_host[i], T16, ext3, dim, DMNERF_MAX_INS, mv[i], who, i, groups_host ? groups_host + 4 * i : nullptr))
+      return 1;
+  if (copy_flags_check(moves_host, copies_host, groups_host, n, true, who)) return 1;
   const size_t out_bytes = 16 + (size_t)n * N_COUNTERS * sizeof(unsigned long long);
   char* out;
   if (s.out.get(out_bytes, &out)) return 2;

@@ -155,6 +155,10 @@ __host__ __device__ inline bool obj_kept(const ObjMask& m, int label) {
   const uint32_t word = label < 64 ? (label < 32 ? m.w[0] : m.w[1]) : (label < 96 ? m.w[2] : m.w[3]);   // no dynamic indexing
   return (word >> (label & 31)) & 1u;
 }
+// Whether label l belongs to a move's label set g (DESIGN.md, "Moving objects together"): obj_kept for a label in [0, 127], false
+// for any other, so that the set test of a move's rule, like the equality test it generalises, never matches a label outside the
+// range (a state grid of dmnerf_mesh_occupancy_edit is not checked).
+__host__ __device__ inline bool in_group(const ObjMask& g, int l) { return (unsigned)l <= (unsigned)DMNERF_MAX_INS && obj_kept(g, l); }
 
 // Region selection (DESIGN.md, "Region selection"): one bit per point of a sweep grid [dim]^3 (C order, bit v & 31 of word
 // v >> 5), the fp32 voxel map [M | c] (row-major 3x4) from the network frame to grid indices, and the rule's two settings: the
@@ -292,24 +296,32 @@ int launch_label_rays(const float* v, const float* nrm, int64_t n, float near_z,
 int launch_argmax_rows(const float* x, int64_t n, int c, int64_t* out, cudaStream_t st);
 
 // Meshing an edited scene (mesh.cu; DESIGN.md, "Meshing an edited scene").  One checked move of dmnerf_mesh_occupancy_edit: the
-// 3x4 move and the grid's index map u = inv (t - b) in fp64, the box in index units, the piece (bits NULL: none).
+// 3x4 move and the grid's index map u = inv (t - b) in fp64, the box in index units, the piece (bits NULL: none) and the labels
+// that move together (DESIGN.md, "Moving objects together"; {label} for a move of one label).
 struct EditMove {
   double trans[12];
   double inv[9];
   double b[3];
   double lo[3], hi[3];
   Region piece;
+  ObjMask group;
   int32_t label, rest_drop, empty;   // empty: the box holds no point, nothing is evaluated
 };
 // The grid and level of an edit or a collision check: dim in [2, 2048], level in (0, 1), a scene transform with det > 0 and
 // finite extents > 0.
 int sweep_grid_check(const double* T16, const double* ext3, int dim, float level, const char* who);
-// d -> m, checked against the grid (dim, transform, extents) and the bound network's ins_num
+// The label set of a move of `label` (DESIGN.md, "Moving objects together"): group4 [4] label words, or NULL for {label}; checked:
+// it holds `label` and no label above max_label.  i: the move's index in errors (< 0: none).
+int label_group(int label, const uint32_t* group4, int max_label, ObjMask& g, const char* who, int i);
+// d -> m, checked against the grid (dim, transform, extents) and the bound network's ins_num; group4: the move's label set
+// (label_group; NULL: its own label)
 int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const double* ext3, int dim, int ins_num, EditMove& m,
-                       const char* who, int i);
+                       const char* who, int i, const uint32_t* group4 = nullptr);
 // The copy flags of n moves (DESIGN.md, "Copying objects"; copies NULL: none), checked: each 0 or 1, no copy with rest_drop and,
-// when the moves apply in order (`ordered`), no move of a label after a copy of it.
-int copy_flags_check(const dmnerf_edit_move* moves, const int32_t* copies, int n, bool ordered, const char* who);
+// when the moves apply in order (`ordered`), no move whose label set (groups [n][4], NULL: each move's own label) holds a label
+// of an earlier copy's set.
+int copy_flags_check(const dmnerf_edit_move* moves, const int32_t* copies, const uint32_t* groups, int n, bool ordered,
+                     const char* who);
 // Points [begin, begin + count) of the grid: their targets under m, the boxed ones compacted in order into pts [*n_eval, 3];
 // *n_eval read back (synchronises).
 int edit_targets(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
@@ -349,16 +361,20 @@ int object_spans(InventoryState& s, const float* occ, const int16_t* labels, int
 
 // Collision checks (collide.cu; DESIGN.md, "Collision checks"), in the inventory's buffers: grid-only counts over a labelled
 // keep-all sweep, one device->host read per call.
+// groups_host [n][4] (NULL: each candidate's own label): the labels each candidate moves together.
 int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
-                 const dmnerf_edit_move* cands_host, const int32_t* copies_host, int n, const uint32_t* obstacles_host,
+                 const dmnerf_edit_move* cands_host, const int32_t* copies_host, const uint32_t* groups_host, int n,
+                 const uint32_t* obstacles_host,
                  int64_t* overlap_host, int64_t* landed_host, cudaStream_t st, const char* who = "move_overlap");
 int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels, int64_t* faces_host,
                     cudaStream_t st);
 // The grid-only edit (DESIGN.md, "Arranging objects"): the moves applied in order to the state occ / labels, each target read
 // from the source grid at its nearest index; landed [n] and overwritten [n][128] per move.  Two read-backs: the grid checks of
 // both grids before the first edit, the counts at the end.  copies_host [n] (NULL: none): the copies, which take and never vacate.
+// groups_host [n][4] (NULL: each move's own label): the labels each move carries together.
 int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels, int dim, float level, const double* T16,
-              const double* ext3, const dmnerf_edit_move* moves_host, const int32_t* copies_host, int n, float* occ, int16_t* labels,
+              const double* ext3, const dmnerf_edit_move* moves_host, const int32_t* copies_host, const uint32_t* groups_host, int n,
+              float* occ, int16_t* labels,
               int64_t* landed_host, int64_t* overwritten_host, cudaStream_t st, const char* who = "grid_edit");
 // The grid check of both: flags in *bad (device) for NaN in occ and labels outside [0, n_labels - 1].  read_checked copies
 // `bytes` from dev to host and synchronises; the buffer starts with that flag word, and a set flag fails the call.
@@ -378,16 +394,18 @@ int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int di
 // per base the moved object's bytes, runs and map; status [n] says which were placed.  The object is sampled from occ / labels,
 // the obstacles and support labels come from the scene scene_occ / scene_labels (DESIGN.md, "Arranging objects"); passing the
 // same grid twice is dmnerf_placement_maps.  copy (DESIGN.md, "Copying objects"): the object is a copy, and the scene's points of
-// its label stay obstacles.  who: the entry point's name in errors (NULL: placement_maps or placement_maps_in_scene).
+// its label stay obstacles.  group_host [4] (NULL: {p->label}): the labels placed together (DESIGN.md, "Moving objects
+// together").  who: the entry point's name in errors (NULL: placement_maps or placement_maps_in_scene).
 int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels, int dim,
-                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy, const double* bases_host,
+                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy, const uint32_t* group_host,
+                   const double* bases_host,
                    const int32_t* box_host, int n_bases, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
                    int32_t* status, cudaStream_t st, const char* who = nullptr);
 // base_host NULL: the object as it lies (dmnerf_placement_contacts; the scene must be the object's grid); otherwise as base_host
 // [12] and box_host [6] leave it, sampled from occ / labels, in the scene scene_occ / scene_labels.
 int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels,
                        int dim, float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy,
-                       const double* base_host,
+                       const uint32_t* group_host, const double* base_host,
                        const int32_t* box_host, int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
                        int32_t* drop_host, cudaStream_t st, const char* who = nullptr);
 

@@ -2,6 +2,7 @@
 // its epilogue, marching cubes on a caller-provided grid, scene-space vertices, area-weighted vertex normals, edge-connected
 // triangle clusters, small-cluster removal and the per-vertex label rays.  Conventions: DESIGN.md, "Mesh extraction".
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 
 #include <cub/cub.cuh>
@@ -652,10 +653,26 @@ int sweep_grid_check(const double* T, const double* ext3, int dim, float level, 
   return 0;
 }
 
+int label_group(int label, const uint32_t* group4, int max_label, ObjMask& g, const char* who, int i) {
+  char at[32] = "";
+  if (i >= 0) snprintf(at, sizeof(at), " move %d:", i);
+  memset(&g, 0, sizeof(g));
+  if (!group4) {
+    g.w[label >> 5] = 1u << (label & 31);
+    return 0;
+  }
+  for (int w = 0; w < 4; ++w) g.w[w] = group4[w];
+  DMN_CHECK(obj_kept(g, label), "%s:%s the label set does not hold the moved label %d", who, at, label);
+  for (int k = max_label + 1; k <= DMNERF_MAX_INS; ++k)
+    DMN_CHECK(!obj_kept(g, k), "%s:%s the label set holds label %d outside [0, %d]", who, at, k, max_label);
+  return 0;
+}
+
 int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const double* ext3, int dim, int ins_num, EditMove& m,
-                       const char* who, int i) {
+                       const char* who, int i, const uint32_t* group4) {
   memset(&m, 0, sizeof(m));
   DMN_CHECK(d.label >= 0 && d.label <= ins_num, "%s: move %d: label %d outside [0, %d]", who, i, d.label, ins_num);
+  if (label_group(d.label, group4, ins_num, m.group, who, i)) return 1;
   for (int k = 0; k < 12; ++k) DMN_CHECK(std::isfinite(d.trans[k]), "%s: move %d: the transformation is not finite", who, i);
   const double* t = d.trans;
   const double det = t[0] * (t[5] * t[10] - t[6] * t[9]) - t[1] * (t[4] * t[10] - t[6] * t[8]) + t[2] * (t[4] * t[9] - t[5] * t[8]);
@@ -677,16 +694,27 @@ int edit_move_from_abi(const dmnerf_edit_move& d, const double* T16, const doubl
   return 0;
 }
 
-int copy_flags_check(const dmnerf_edit_move* moves, const int32_t* copies, int n, bool ordered, const char* who) {
+int copy_flags_check(const dmnerf_edit_move* moves, const int32_t* copies, const uint32_t* groups, int n, bool ordered,
+                     const char* who) {
   if (!copies) return 0;
+  // bit k of word w of move i's label set
+  auto word = [&](int i, int w) -> uint32_t {
+    if (groups) return groups[4 * i + w];
+    return (moves[i].label >> 5) == w ? 1u << (moves[i].label & 31) : 0u;
+  };
   for (int i = 0; i < n; ++i) {
     DMN_CHECK(copies[i] == 0 || copies[i] == 1, "%s: move %d: copy flag %d is not 0 or 1", who, i, copies[i]);
     DMN_CHECK(!copies[i] || !moves[i].rest_drop, "%s: move %d: a copy cannot drop the rest of its label (it vacates nothing)", who,
               i);
     if (!ordered || copies[i]) continue;
-    for (int j = 0; j < i; ++j)
-      DMN_CHECK(!copies[j] || moves[j].label != moves[i].label,
-                "%s: move %d of label %d follows copy %d of that label (its vacate would erase the copy)", who, i, moves[i].label, j);
+    for (int j = 0; j < i; ++j) {
+      if (!copies[j]) continue;
+      for (int w = 0; w < 4; ++w) {
+        const uint32_t shared = word(i, w) & word(j, w);
+        DMN_CHECK(!shared, "%s: move %d of label %d follows copy %d of that label (its vacate would erase the copy)", who, i,
+                  32 * w + __builtin_ctz(shared), j);
+      }
+    }
   }
   return 0;
 }
@@ -740,15 +768,15 @@ __global__ void edit_apply_kernel(const GridXform g, const EditMove m, int64_t b
         ot = occupancy_of(r[3], voxel);
       },
       o, l, level,
-      [&] { return region_drops(m.piece, m.label, tgt[3 * i], tgt[3 * i + 1], tgt[3 * i + 2]); },
-      [&](bool& in_piece) {
+      [&](int lt) { return region_drops(m.piece, lt, tgt[3 * i], tgt[3 * i + 1], tgt[3 * i + 2]); },
+      [&](bool& in_piece, int lp) {
         float q[3];
         sweep_point(g, p, q);
-        in_piece = !region_drops(m.piece, m.label, q[0], q[1], q[2]);
+        in_piece = !region_drops(m.piece, lp, q[0], q[1], q[2]);
       },
-      [&](float ot) {
+      [&](float ot, int lt) {
         occ[p] = ot;
-        labels[p] = (int16_t)m.label;
+        labels[p] = (int16_t)lt;
       },
       [&] { occ[p] = 0.0f; });
 }

@@ -45,12 +45,14 @@ __device__ __forceinline__ int64_t point_of(const Frame& f, int h1, int h2, int 
   return h1 * f.s1 + h2 * f.s2 + (int64_t)(f.flip ? f.dim - 1 - y : y) * f.sa;
 }
 
-// What the placed object and the obstacles are (DESIGN.md, "Object placement"): S = labels == label, solid, kept by the piece;
-// O = solid, label among the obstacles, not vacated (labels == label and in the piece -- every point without one -- or rest_drop).
-// A COPY (DESIGN.md, "Copying objects") vacates nothing: its own label's solid points are obstacles like any other.
+// What the placed object and the obstacles are (DESIGN.md, "Object placement", "Moving objects together"): S = label in the
+// group, solid, kept by the piece for that label; O = solid, label among the obstacles, not vacated (label in the group and in the
+// piece -- every point without one -- or rest_drop).  A COPY (DESIGN.md, "Copying objects") vacates nothing: its own labels' solid
+// points are obstacles like any other.
 struct Placed {
-  Region piece;                               // bits NULL: the whole label
+  Region piece;                               // bits NULL: the whole labels
   ObjMask obstacles;
+  ObjMask group;                              // the labels placed together ({label} for one object)
   int label, rest_drop;
 };
 
@@ -77,12 +79,12 @@ __device__ __forceinline__ void classify(const Frame& f, const GridXform& g, con
   const bool solid = v > level && l >= 0 && l <= DMNERF_MAX_INS;
   obst = solid && obj_kept(m.obstacles, l);
   obj = false;
-  if (solid && l == m.label) {
+  if (solid && in_group(m.group, l)) {
     bool keep = true;
     if (m.piece.bits != nullptr) {
       float q[3];
       sweep_point(g, p, q);
-      keep = !region_drops(m.piece, m.label, q[0], q[1], q[2]);
+      keep = !region_drops(m.piece, l, q[0], q[1], q[2]);
     }
     obj = keep;
     if (!COPY && (keep || m.rest_drop)) obst = false;            // vacated by the move
@@ -144,8 +146,8 @@ __global__ void __launch_bounds__(CP_WARPS * 32) place_column_kernel(const Frame
 }
 
 // The object as the move e leaves it (DESIGN.md, "Turned placements"), one thread per (column, height) in the object bytes
-// order: point p belongs to it when src(p) of the collision checks holds -- q = edit_target(e, p) in the box B, labels[q] == label,
-// occ[q] > level and the piece keeps the target t.  Points the move carries outside the grid are lost, as in the edited sweep.
+// order: point p belongs to it when src(p) of the collision checks holds -- q = edit_target(e, p) in the box B, labels[q] in the
+// move's group, occ[q] > level and the piece keeps the target t for that label.  Points the move carries outside the grid are lost, as in the edited sweep.
 __global__ void __launch_bounds__(MV_THREADS) place_moved_kernel(const Frame f, const GridXform g, const EditMove e,
                                                                  const float* __restrict__ occ, const int16_t* __restrict__ labels,
                                                                  float level, uint8_t* __restrict__ object) {
@@ -158,7 +160,8 @@ __global__ void __launch_bounds__(MV_THREADS) place_moved_kernel(const Frame f, 
   bool src = edit_target(e.trans, e.inv, e.b, e.lo, e.hi, !e.empty, p, t, q);
   if (src) {
     const int64_t qi = ((int64_t)q[0] * d + (int64_t)q[1]) * d + (int64_t)q[2];
-    src = labels[qi] == e.label && occ[qi] > level && (e.piece.bits == nullptr || !region_drops(e.piece, e.label, t[0], t[1], t[2]));
+    const int lq = labels[qi];
+    src = in_group(e.group, lq) && occ[qi] > level && (e.piece.bits == nullptr || !region_drops(e.piece, lq, t[0], t[1], t[2]));
   }
   object[o] = src ? 1 : 0;
 }
@@ -388,7 +391,8 @@ enum { PLACED = 0, NO_POINTS = 1, TOP_OUT = 2 };   // dmnerf_placement_maps' sta
 
 // The host checks of every placement call, before any launch: the object's grid occ / labels and the scene.
 int check(const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels, int dim, float level,
-          const double* T16, const double* ext3, const dmnerf_placement* p, int copy, const char* who, Prepared& q) {
+          const double* T16, const double* ext3, const dmnerf_placement* p, int copy, const uint32_t* group4, const char* who,
+          Prepared& q) {
   DMN_CHECK(occ && labels && scene_occ && scene_labels && T16 && ext3 && p, "%s: NULL argument", who);
   DMN_CHECK(dim >= 2 && dim <= PLACE_MAX_DIM, "%s: dim %d out of range [2, %d]", who, dim, PLACE_MAX_DIM);
   if (sweep_grid_check(T16, ext3, dim, level, who)) return 1;
@@ -400,6 +404,7 @@ int check(const float* occ, const int16_t* labels, const float* scene_occ, const
   DMN_CHECK(!copy || !p->rest_drop, "%s: a copy cannot drop the rest of its label (it vacates nothing)", who);
   q.copy = copy != 0;
   Placed& m = q.m;
+  if (label_group(p->label, group4, DMNERF_MAX_INS, m.group, who, -1)) return 1;
   if (piece_region(p->piece, p->label, m.piece, who, 0)) return 1;
   for (int k = 0; k < 4; ++k) m.obstacles.w[k] = p->obstacles[k];
   m.label = p->label;
@@ -424,9 +429,9 @@ int check(const float* occ, const int16_t* labels, const float* scene_occ, const
 }
 
 // base (row-major 3x4) and the source box B of a moved placement as the edit move the shared checks take: finite, det > 0, B
-// inside the grid and not inverted (the empty box: no point), the piece applying to the label.
-int base_move(const dmnerf_placement* p, const double* base12, const int32_t* box6, const double* T16, const double* ext3, int dim,
-              EditMove& e, const char* who, int i) {
+// inside the grid and not inverted (the empty box: no point), the piece applying to the label; the group checked by check().
+int base_move(const dmnerf_placement* p, const ObjMask& group, const double* base12, const int32_t* box6, const double* T16,
+              const double* ext3, int dim, EditMove& e, const char* who, int i) {
   dmnerf_edit_move d;
   memset(&d, 0, sizeof(d));
   d.label = p->label;
@@ -434,7 +439,7 @@ int base_move(const dmnerf_placement* p, const double* base12, const int32_t* bo
   memcpy(d.trans, base12, sizeof(d.trans));
   memcpy(d.box, box6, sizeof(d.box));
   d.piece = p->piece;
-  return edit_move_from_abi(d, T16, ext3, dim, DMNERF_MAX_INS, e, who, i);
+  return edit_move_from_abi(d, T16, ext3, dim, DMNERF_MAX_INS, e, who, i, group.w);
 }
 
 // The buffers, the grid check (of both grids when the scene is not the object's grid) and the column pass: the column table,
@@ -567,7 +572,7 @@ int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int di
   memset(info, 0, sizeof(*info));
   Prepared q;
   int why;
-  if (check(occ, labels, occ, labels, dim, level, T16, ext3, p, 0, who, q)) return 1;
+  if (check(occ, labels, occ, labels, dim, level, T16, ext3, p, 0, nullptr, who, q)) return 1;
   if (const int rc = columns(s, q, true, st)) return rc;
   if (const int rc = object_runs(s, q, nullptr, true, who, &why, st)) return rc;
   if (unplaced(q, why, false, who)) return 1;
@@ -577,8 +582,8 @@ int placement_map(PlaceState& s, const float* occ, const int16_t* labels, int di
 }
 
 int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels, int dim,
-                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy, const double* bases_host,
-                   const int32_t* box_host, int n_bases, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
+                   float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy, const uint32_t* group_host,
+                   const double* bases_host, const int32_t* box_host, int n_bases, int32_t* drop, int32_t* contacts, int16_t* support, dmnerf_placement_info* info,
                    int32_t* status, cudaStream_t st, const char* who) {
   if (!who) who = occ == scene_occ && labels == scene_labels ? "placement_maps" : "placement_maps_in_scene";
   DMN_CHECK(drop && contacts && support && info && status, "%s: NULL argument", who);
@@ -590,10 +595,10 @@ int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const
     status[i] = NO_POINTS;
   }
   Prepared q;
-  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, copy, who, q)) return 1;
+  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, copy, group_host, who, q)) return 1;
   std::vector<EditMove> e(n_bases);
   for (int i = 0; i < n_bases; ++i)
-    if (base_move(p, bases_host + 12 * i, box_host, T16, ext3, dim, e[i], who, i)) return 1;
+    if (base_move(p, q.m.group, bases_host + 12 * i, box_host, T16, ext3, dim, e[i], who, i)) return 1;
   if (const int rc = columns(s, q, false, st)) return rc;
   const int64_t plane = (int64_t)dim * dim;
   for (int i = 0; i < n_bases; ++i) {
@@ -609,7 +614,7 @@ int placement_maps(PlaceState& s, const float* occ, const int16_t* labels, const
 
 int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, const float* scene_occ, const int16_t* scene_labels,
                        int dim, float level, const double* T16, const double* ext3, const dmnerf_placement* p, int copy,
-                       const double* base_host, const int32_t* box_host, int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
+                       const uint32_t* group_host, const double* base_host, const int32_t* box_host, int u, int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
                        int32_t* drop_host, cudaStream_t st, const char* who) {
   const bool moved = base_host != nullptr;
   if (!who)
@@ -622,10 +627,10 @@ int placement_contacts(PlaceState& s, const float* occ, const int16_t* labels, c
   EditMove e;
   int why;
   DMN_CHECK(moved || !copy, "%s: a copy is placed through a base", who);
-  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, copy, who, q)) return 1;
+  if (check(occ, labels, scene_occ, scene_labels, dim, level, T16, ext3, p, copy, group_host, who, q)) return 1;
   if (moved) {
     DMN_CHECK(box_host, "%s: box is NULL", who);
-    if (base_move(p, base_host, box_host, T16, ext3, dim, e, who, 0)) return 1;
+    if (base_move(p, q.m.group, base_host, box_host, T16, ext3, dim, e, who, 0)) return 1;
   }
   if (const int rc = columns(s, q, !moved, st)) return rc;
   if (const int rc = object_runs(s, q, moved ? &e : nullptr, true, who, &why, st)) return rc;

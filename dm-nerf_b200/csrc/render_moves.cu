@@ -65,8 +65,8 @@ __global__ void move_count_kernel(const int32_t* flag, const int32_t* pos, int64
 }
 
 // One thread per sample: take the network's row at the target (all c channels), or vacate the sample (density 0, logits kept).
-//   take:   t in the box && edit_takes(label(t), occ(t), label, occ_p) && (no piece || the piece keeps t);
-//   vacate: otherwise label_p == label && ((the piece keeps p, every p without one) && p's index in the box
+//   take:   t in the box && edit_takes(label(t), occ(t), group, occ_p) && (no piece || the piece keeps t for label(t));
+//   vacate: otherwise label_p in group && ((the piece keeps p for label_p, every p without one) && p's index in the box
 //                                          || rest_drop && the piece does not keep p).
 // Unlike the sweep's vacate there is no occ_p > level test (a render composites every density, so a vacated object must leave no
 // haze); the box bounds the vacate instead.  A COPY (DESIGN.md, "Copying objects") takes the same rows and never vacates.
@@ -83,14 +83,15 @@ __global__ void move_apply_kernel(const EditMove m, const float* __restrict__ ra
     const float* rt = traw + (int64_t)pos[i] * c;
     const int lt = argmax_sigmoid(rt + 4, c - 4);
     const float* t = tgt + 6 * i;
-    if (edit_takes(lt, occupancy_of(rt[3], voxel), m.label, occupancy_of(r[3], voxel), level) &&
-        (!has_piece || !region_drops(m.piece, m.label, t[0], t[1], t[2]))) {
+    if (edit_takes(lt, occupancy_of(rt[3], voxel), m.group, occupancy_of(r[3], voxel), level) &&
+        (!has_piece || !region_drops(m.piece, lt, t[0], t[1], t[2]))) {
       for (int k = 0; k < c; ++k) r[k] = rt[k];
       return;
     }
   }
   if (COPY) return;
-  if (argmax_sigmoid(r + 4, c - 4) != m.label) return;
+  const int lp = argmax_sigmoid(r + 4, c - 4);
+  if (!in_group(m.group, lp)) return;
   bool in_piece = true;
   if (has_piece) {
     const int64_t ray = i / s;
@@ -98,7 +99,7 @@ __global__ void move_apply_kernel(const EditMove m, const float* __restrict__ ra
     const float d[3] = {rays_d[3 * ray], rays_d[3 * ray + 1], rays_d[3 * ray + 2]};
     float p[3];
     ray_point(o, d, z[i], p);
-    in_piece = !region_drops(m.piece, m.label, p[0], p[1], p[2]);
+    in_piece = !region_drops(m.piece, lp, p[0], p[1], p[2]);
   }
   if (in_piece ? pin[i] != 0 : m.rest_drop != 0) r[3] = 0.0f;
 }

@@ -77,22 +77,24 @@ __device__ __forceinline__ float occupancy_of(float a, float voxel) {
   return __fsub_rn(1.0f, expf(__fmul_rn(-r, voxel)));
 }
 
-// The take test of a move of `label` (piece aside): the target (lt, ot) is that label, and it is solid or the point it replaces
-// (occupancy o) is not.  The moved render (render_moves.cu) calls it; edit_rule below spells the same expression out, because
-// calling it there reorders the SASS of the edited sweep's and the grid-only edit's kernels.
-__device__ __forceinline__ bool edit_takes(int lt, float ot, int label, float o, float level) {
-  return lt == label && (ot > level || o <= level);
+// The take test of a move of the labels `group` (piece aside): the target (lt, ot) holds one of them, and it is solid or the point
+// it replaces (occupancy o) is not.  The moved render (render_moves.cu) calls it; edit_rule below spells the same expression out,
+// because calling it there reorders the SASS of the edited sweep's and the grid-only edit's kernels.
+__device__ __forceinline__ bool edit_takes(int lt, float ot, const ObjMask& group, float o, float level) {
+  return in_group(group, lt) && (ot > level || o <= level);
 }
 
-// The edit rule at one grid point p (DESIGN.md, "Meshing an edited scene"), shared by the edited sweep (the network at the
-// target) and the grid-only edit (collide.cu: the unedited grid at the target's nearest index).  m: the move's label, rest_drop
-// and piece (taken by value, which keeps the edited sweep's SASS as it was before the rule was shared).  target(lt, ot) gives the
-// label and occupancy at the target and is called only in the box; drops_target() is the piece's region_drops at the target and
-// in_piece(b) sets b to whether the piece keeps p, both called only with a piece.
-//   take:   in the box && lt == label && (ot > level || o <= level) && (no piece || !drops_target()): take(ot) writes
-//           (o, l) <- (ot, label);
-//   vacate: otherwise l == label && o > level && (no piece || p in the piece || rest_drop): vacate() writes o <- 0, the label
+// The edit rule at one grid point p (DESIGN.md, "Meshing an edited scene", "Moving objects together"), shared by the edited sweep
+// (the network at the target) and the grid-only edit (collide.cu: the unedited grid at the target's nearest index).  m: the
+// move's label set `group`, rest_drop and piece (taken by value, which keeps the edited sweep's SASS as it was before the rule was
+// shared).  target(lt, ot) gives the label and occupancy at the target and is called only in the box; drops_target(lt) is the
+// piece's region_drops at the target for the target's label and in_piece(b, l) sets b to whether the piece keeps p for p's label
+// l, both called only with a piece.
+//   take:   in the box && lt in group && (ot > level || o <= level) && (no piece || !drops_target(lt)): take(ot, lt) writes
+//           (o, l) <- (ot, lt);
+//   vacate: otherwise l in group && o > level && (no piece || p in the piece || rest_drop): vacate() writes o <- 0, the label
 //           kept.  A copy (COPY, DESIGN.md, "Copying objects") takes as a move does and never vacates.
+// A move of one label has group = {label}: the set tests are that label's equality tests.
 template <bool COPY = false, class Move, class Target, class DropsTarget, class InPiece, class Take, class Vacate>
 __device__ __forceinline__ void edit_rule(const Move m, bool in_box, const Target& target, float o, int l, float level,
                                           const DropsTarget& drops_target, const InPiece& in_piece_of, const Take& take,
@@ -102,14 +104,14 @@ __device__ __forceinline__ void edit_rule(const Move m, bool in_box, const Targe
     int lt;
     float ot;
     target(lt, ot);
-    if (lt == m.label && (ot > level || o <= level) && (!has_piece || !drops_target())) {
-      take(ot);
+    if (in_group(m.group, lt) && (ot > level || o <= level) && (!has_piece || !drops_target(lt))) {
+      take(ot, lt);
       return;
     }
   }
-  if (!COPY && l == m.label && o > level) {
+  if (!COPY && in_group(m.group, l) && o > level) {
     bool in_piece = true;
-    if (has_piece) in_piece_of(in_piece);
+    if (has_piece) in_piece_of(in_piece, l);
     if (in_piece || m.rest_drop) vacate();
   }
 }

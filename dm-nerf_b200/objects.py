@@ -27,6 +27,9 @@
     render_moves(occ, labels, scene_transform, moves, ...)
                                                         -> moves for render_rays(moves=) / render_frame(moves=): the edited
                                                            sweep's rule applied per render sample
+    carried_labels(occ, labels, scene_transform, label, down, ...)
+                                                        -> what rests on an object, transitively: the group= that moves
+                                                           it together with what it carries
 
 Every network sample is labelled argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the
 exchanger's rule); a sample whose label is not kept has alpha = 0 in the composite of both passes, so the coarse weights of the
@@ -265,25 +268,76 @@ def move_copies(copies, m):
     return [bool(c) for c in flags]
 
 
-def _check_copies(copies, mv, drops, ordered=True):
+def _check_copies(copies, mv, drops, ordered=True, sets=None):
     """The copy flags of moves with labels mv and rest drops `drops`, checked -> [bool]: no copy drops the rest of its label (it
     vacates nothing) and, when the moves apply in order, no move of a label follows a copy of it (its vacate would erase the copy,
-    which carries the label)."""
+    which carries the label).  sets (move_groups; None: each move's own label): a move whose set holds a label of an earlier
+    copy's set follows a copy of that label."""
     flags = move_copies(copies, len(mv))
+    sets = sets or [(k,) for k in mv]
     for i, (c, d) in enumerate(zip(flags, drops)):
         if c and d:
             raise ValueError("copy: move %d: a copy cannot drop the rest of its label (rest 'drop'): it vacates nothing" % i)
         if ordered and not c:
             for j in range(i):
-                if flags[j] and mv[j] == mv[i]:
+                shared = sorted(set(sets[j]) & set(sets[i])) if flags[j] else []
+                if shared:
                     raise ValueError("copy: move %d of label %d follows copy %d of that label (its vacate would erase the copy)"
-                                     % (i, mv[i], j))
+                                     % (i, shared[0], j))
     return flags
 
 
 def _copy_flags(flags):
     """The HOST int32 copy flags of the _copies entry points."""
     return (C.c_int32 * len(flags))(*[int(c) for c in flags])
+
+
+def move_groups(groups, mv, ins_num, who="group"):
+    """groups (None, or one entry per move: None or an iterable of labels) -> one sorted tuple of labels per move, or None when
+    every entry is None (DESIGN.md, "Moving objects together").  A move's set G moves every label of G as one rigid body; it must
+    hold the move's label, and its labels lie in [0, ins_num].  An entry None is the move's own label."""
+    if groups is None:
+        return None
+    if isinstance(groups, (str, bytes, dict)) or not hasattr(groups, "__iter__"):
+        raise ValueError("%s: groups must be None or one entry per move, got %r" % (who, groups))
+    groups = list(groups)
+    if len(groups) != len(mv):
+        raise ValueError("%s: groups must be None or one entry per move (%d), got %d" % (who, len(mv), len(groups)))
+    if all(g is None for g in groups):
+        return None
+    out = []
+    for i, (g, label) in enumerate(zip(groups, mv)):
+        if g is None:
+            out.append((label,))
+            continue
+        if isinstance(g, (str, bytes, dict)) or not hasattr(g, "__iter__"):
+            raise ValueError("%s: move %d: a group must be None or an iterable of labels, got %r" % (who, i, g))
+        ks = sorted(set(_labels(list(g), ins_num, who)))
+        if label not in ks:
+            raise ValueError("%s: move %d: the group %s does not hold the moved label %d" % (who, i, ks, label))
+        out.append(tuple(ks))
+    return out
+
+
+def _group_words(sets):
+    """The HOST uint32 [n][4] label words of the _groups entry points."""
+    words = [w for ks in sets for w in label_words(ks)]
+    return (C.c_uint32 * len(words))(*words)
+
+
+def _group_mask(occ, labels, ks, level, piece, scene_transform, extents):
+    """bool grid: the solid points of the labels ks, each label the piece applies to cut by the piece (region_drops)."""
+    mask = torch.zeros_like(labels, dtype=torch.bool)
+    keep = None
+    applies = None if piece is None else label_words(range(MAX_LABELS)) if piece.applies is None else piece.applies
+    for k in ks:
+        mk = labels == int(k)
+        if applies is not None and (applies[k >> 5] >> (k & 31)) & 1:
+            if keep is None:
+                keep = _region_keeps(piece, scene_transform, occ.shape[0], extents, occ.device)
+            mk &= keep
+        mask |= mk
+    return mask & (occ > level)
 
 
 def _region_keeps(region, T, dim, extents, device, slab=1 << 20):
@@ -314,9 +368,14 @@ def solid_box(occ, labels, label, level=0.45, margin=2, keep=None):
     mask = (labels == int(label)) & (occ > level)
     if keep is not None:
         mask &= keep
+    return _mask_box(mask, margin)
+
+
+def _mask_box(mask, margin):
+    """solid_box of the points of a bool grid."""
     if not bool(mask.any()):
         return EMPTY_BOX
-    dim = occ.shape[0]
+    dim = mask.shape[0]
     box = []
     for a in range(3):
         idx = torch.nonzero(mask.any(dim=tuple(c for c in range(3) if c != a))).flatten()
@@ -325,12 +384,14 @@ def solid_box(occ, labels, label, level=0.45, margin=2, keep=None):
 
 
 def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, extents=None, level=0.45, near=4.0, far=15.0,
-                   N_importance=128, pieces=None, rest="keep", slab=0, copies=None):
+                   N_importance=128, pieces=None, rest="keep", slab=0, copies=None, groups=None):
     """dmnerf_mesh_occupancy_edit: the moves [(label, 4x4)] applied in order, in place, to occ / labels ([dim]^3 float32 /
     int16 on the device: the keep-all sweep of model_fine on this grid), the network evaluated only at the target points
     inside each move's box (boxes: [m, 6] inclusive index boxes, EMPTY_BOX for none).  pieces / rest: as manipulator.  copies
     (None, a bool or one per move): the moves that are copies, which take as the move would and never vacate
-    (dmnerf_mesh_occupancy_edit_copies; DESIGN.md, "Copying objects").  Returns the number of target points evaluated."""
+    (dmnerf_mesh_occupancy_edit_copies; DESIGN.md, "Copying objects").  groups (None, or per move None or labels; DESIGN.md,
+    "Moving objects together"): the labels each move carries as one body (dmnerf_mesh_occupancy_edit_groups).  Returns the number
+    of target points evaluated."""
     from .manipulator import _piece_region, move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -342,7 +403,8 @@ def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, exten
     level = _check_level(level)
     boxes = _check_boxes(boxes, len(mv), dim)
     drops = move_rests(rest, len(mv))
-    flags = _check_copies(copies, mv, drops)
+    sets = move_groups(groups, mv, ins_num)
+    flags = _check_copies(copies, mv, drops, sets=sets)
     regions = move_pieces(pieces, mv, ins_num, occ.device) or [None] * len(mv)
     if not mv:
         return 0
@@ -361,23 +423,30 @@ def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, exten
     head = (ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(ext, 3), dim, (far - near) / N_importance, level, int(slab), descs)
     tail = (len(mv), _lib.ptr(occ), _lib.ptr(labels, torch.int16), C.byref(n))
     with torch.no_grad():
-        if any(flags):
+        if sets is not None:
+            ctx.call("dmnerf_mesh_occupancy_edit_groups", *head, _copy_flags(flags), _group_words(sets), *tail)
+        elif any(flags):
             ctx.call("dmnerf_mesh_occupancy_edit_copies", *head, _copy_flags(flags), *tail)
         else:
             ctx.call("dmnerf_mesh_occupancy_edit", *head, *tail)
     return int(n.value)
 
 
-def edit_boxes(occ, labels, moves, scene_transform, extents=None, level=0.45, margin=2, pieces=None):
+def edit_boxes(occ, labels, moves, scene_transform, extents=None, level=0.45, margin=2, pieces=None, groups=None):
     """The default boxes of edited_sweep from the unedited sweep: per move, solid_box of its label's solid points (those its
-    piece keeps, with a piece) grown by margin -> int [m, 6]."""
+    piece keeps, with a piece) grown by margin -> int [m, 6].  groups (as edited_sweep): a group's box holds the solid points of
+    every label of its set, the piece applied to the labels it applies to."""
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
     mv = [int(m[0]) for m in moves]
     regions = list(pieces) if pieces is not None else [None] * len(mv)
+    sets = move_groups(groups, mv, MAX_LABELS - 1) or [(k,) for k in mv]
     dim = occ.shape[0]
     out = []
-    for k, r in zip(mv, regions):
+    for k, r, ks in zip(mv, regions, sets):
+        if len(ks) > 1:
+            out.append(_mask_box(_group_mask(occ, labels, ks, level, r, scene_transform, extents), int(margin)))
+            continue
         keep = None if r is None else _region_keeps(r, scene_transform, dim, extents, occ.device)
         out.append(solid_box(occ, labels, k, level, int(margin), keep))
         del keep
@@ -385,7 +454,7 @@ def edit_boxes(occ, labels, moves, scene_transform, extents=None, level=0.45, ma
 
 
 def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128,
-                 margin=2, boxes=None, pieces=None, rest="keep", copies=None):
+                 margin=2, boxes=None, pieces=None, rest="keep", copies=None, groups=None):
     """The labelled sweep of the edited scene -> (occ [dim]^3 float32, labels [dim]^3 int16) on the device: the keep-all sweep of
     model_fine (occupancy_objects), then the moves [(label, 4x4 in the network frame, as manipulator_eval's transformation)]
     applied in order (edit_occupancy).  A move shows at p what the network holds at trans p, as rigid_rays renders it: the
@@ -393,7 +462,11 @@ def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None,
     moved label's solid points in the unedited grid (of those its piece keeps, with a piece) grown by `margin` voxels.
     pieces / rest: as manipulator (a Region or None per move; "keep" / "drop", or one per move).  copies (None, a bool or one
     per move; DESIGN.md, "Copying objects"): a copy takes as its move would and leaves the source in place; the copy keeps the
-    source's label: a second connected piece of it where it does not touch its source, one piece with it where it does."""
+    source's label: a second connected piece of it where it does not touch its source, one piece with it where it does.
+    groups (None, or one entry per move: None or an iterable of labels holding the move's label; DESIGN.md, "Moving objects
+    together"): each move carries every label of its set as one rigid body -- a table with what stands on it -- in one pass;
+    a target of any label of the set is taken with its own label, and every label of the set is vacated.  The default box holds
+    the whole set.  carried_labels finds the set of what rests on an object."""
     from .manipulator import move_pieces, move_rests
     from .mesh import check_transform
     T = check_transform(scene_transform)
@@ -401,7 +474,7 @@ def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None,
     ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
     mv, _ = _check_moves(moves, ins_num)
     level = _check_level(level)
-    _check_copies(copies, mv, move_rests(rest, len(mv)))
+    _check_copies(copies, mv, move_rests(rest, len(mv)), sets=move_groups(groups, mv, ins_num))
     move_pieces(pieces, mv, ins_num, dev)
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
@@ -411,25 +484,27 @@ def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None,
         occ, labels = occupancy_objects(model_fine, T, object_mask(ins_num, remove=[]), grid_dim, extents, near, far, N_importance,
                                         device=dev)
         if boxes is None:
-            boxes = edit_boxes(occ, labels, moves, T, extents, level, margin, pieces)
-        edit_occupancy(model_fine, T, occ, labels, moves, boxes, extents, level, near, far, N_importance, pieces, rest, copies=copies)
+            boxes = edit_boxes(occ, labels, moves, T, extents, level, margin, pieces, groups)
+        edit_occupancy(model_fine, T, occ, labels, moves, boxes, extents, level, near, far, N_importance, pieces, rest, copies=copies,
+                       groups=groups)
     return occ, labels
 
 
 def edited_mesh(model_fine, scene_transform, moves, grid_dim=256, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128,
-                margin=2, boxes=None, pieces=None, rest="keep", min_cluster=400, per_object=False, copies=None):
+                margin=2, boxes=None, pieces=None, rest="keep", min_cluster=400, per_object=False, copies=None, groups=None):
     """The mesh of an edited scene: edited_sweep (same arguments) -> marching cubes -> scene space -> normals -> small-cluster
     removal.  Returns extract_mesh's keys as device tensors -- vertices, triangles, normals, clean_vertices, clean_normals,
     clean_triangles -- and labels (int64 per clean vertex: mesh.vertex_labels of its index-space vertex, the label of the
     inside end of its edge, from the edited grid; no label rays are rendered).  per_object: also objects, the
-    meshes_from_labelled_grid of the edited grid for every label with solid points except ins_num.  copies: as edited_sweep."""
+    meshes_from_labelled_grid of the edited grid for every label with solid points except ins_num.  copies, groups: as
+    edited_sweep."""
     from .mesh import EXTENTS, check_transform, clean_mesh, marching_cubes, to_scene, vertex_labels, vertex_normals
     T = check_transform(scene_transform)
     ext = EXTENTS if extents is None else extents
     ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
     with torch.no_grad():
         occ, labels = edited_sweep(model_fine, T, moves, grid_dim, ext, level, near, far, N_importance, margin, boxes, pieces, rest,
-                                   copies=copies)
+                                   copies=copies, groups=groups)
         v_idx, tris = marching_cubes(occ, level)
         verts = to_scene(v_idx, T, grid_dim, ext)
         normals = vertex_normals(verts, tris)
@@ -449,13 +524,15 @@ def edited_mesh(model_fine, scene_transform, moves, grid_dim=256, extents=None, 
 class MovedScene:
     """Checked moves for render_rays(moves=) / render_frame(moves=): the dmnerf_render_moves the library reads, and the move
     descriptions and region bits it points into, held for as long as the value lives.  copies: per move, whether it is a copy
-    (DESIGN.md, "Copying objects").  Immutable."""
-    __slots__ = ("_desc", "_held", "device", "labels", "boxes", "rest_drop", "level", "voxel", "copies", "_flags")
+    (DESIGN.md, "Copying objects"); groups: per move, the labels it carries (DESIGN.md, "Moving objects together").  Immutable."""
+    __slots__ = ("_desc", "_held", "device", "labels", "boxes", "rest_drop", "level", "voxel", "copies", "_flags", "groups", "_words")
 
-    def __init__(self, desc, held, device, labels, boxes, rest_drop, level, voxel, copies=None):
+    def __init__(self, desc, held, device, labels, boxes, rest_drop, level, voxel, copies=None, groups=None):
         copies = tuple(bool(c) for c in copies) if copies is not None else (False,) * len(labels)
+        sets = tuple(tuple(g) for g in groups) if groups is not None else tuple((k,) for k in labels)
         for k, v in zip(self.__slots__, (desc, held, device, labels, tuple(map(tuple, boxes.tolist())), tuple(rest_drop), level,
-                                         voxel, copies, _copy_flags(copies) if any(copies) else None)):
+                                         voxel, copies, _copy_flags(copies) if any(copies) else None, sets,
+                                         _group_words(sets) if groups is not None else None)):
             object.__setattr__(self, k, v)
 
     def __setattr__(self, key, value):
@@ -469,15 +546,19 @@ class MovedScene:
         """The copy flags dmnerf_render_moved_copies reads (HOST int32 [n_moves]), or None when no move is a copy."""
         return self._flags
 
+    def group_words(self):
+        """The label sets dmnerf_render_moved_groups reads (HOST uint32 [n_moves][4]), or None when no group was given."""
+        return self._words
+
 
 def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128, margin=2,
-                 boxes=None, pieces=None, rest="keep", copies=None):
+                 boxes=None, pieces=None, rest="keep", copies=None, groups=None):
     """The moves [(label, 4x4 in the network frame)] of edited_sweep, checked for the moved render -> a MovedScene.  occ / labels:
     the unedited keep-all sweep ([dim]^3 float32 / int16 on the device) that the default boxes come from (edit_boxes, as
     edited_sweep) and whose grid (scene_transform, extents, dim) the boxes index.  level, margin, boxes, pieces, rest: as
     edited_sweep; the voxel of the occupancy test is the sweep's (far - near) / N_importance.  moves, pieces and rest may be
     arrange_objects' moves, pieces and rest unchanged, or manipulator_eval's [(label, 4x4)].  Labels are checked against the
-    networks when the render runs.  copies: as edited_sweep (arrange_objects' copies unchanged)."""
+    networks when the render runs.  copies, groups: as edited_sweep (arrange_objects' copies and groups unchanged)."""
     from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -487,7 +568,8 @@ def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, 
         raise ValueError("render_moves: give between 1 and %d moves" % _lib.MAX_MOVES)
     level = _check_level(level)
     drops = move_rests(rest, len(mv))
-    flags = _check_copies(copies, mv, drops)
+    sets = move_groups(groups, mv, MAX_LABELS - 1)
+    flags = _check_copies(copies, mv, drops, sets=sets)
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
     with np.errstate(divide="ignore", invalid="ignore"):
@@ -499,7 +581,7 @@ def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     regions = move_pieces(pieces, mv, MAX_LABELS - 1, occ.device) or [None] * len(mv)
     dim = _check_sweep(occ, labels, "render_moves")
     if boxes is None:
-        boxes = _check_boxes(edit_boxes(occ, labels, moves, T, ext, level, margin, pieces), len(mv), dim)
+        boxes = _check_boxes(edit_boxes(occ, labels, moves, T, ext, level, margin, pieces, sets), len(mv), dim)
     descs = _edit_moves(mv, mats, boxes, drops, regions, occ.device)
     d = _lib.RenderMoves()
     d.moves, d.n_moves, d.dim = C.cast(descs, C.POINTER(_lib.EditMove)), len(mv), dim
@@ -507,7 +589,7 @@ def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     d.extents[:] = np.asarray(ext, dtype=np.float64).reshape(-1).tolist()
     d.level, d.voxel = level, float(voxel)
     return MovedScene(d, (descs, [r.bits for r in regions if r is not None]), occ.device, tuple(mv), boxes, drops, level,
-                      float(voxel), flags)
+                      float(voxel), flags, sets)
 
 
 # ----------------------------------------------------------------------------------------------------------------- collisions
@@ -529,14 +611,16 @@ def _check_sweep(occ, labels, who):
 
 
 def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, boxes=None, margin=2, pieces=None, rest="keep",
-                 obstacles=None, copies=None):
+                 obstacles=None, copies=None, groups=None):
     """dmnerf_move_overlap: each move [(label, 4x4 in the network frame)] checked on its own against the labelled keep-all sweep
     occ / labels ([dim]^3 float32 / int16 on the device; an edited_sweep result is accepted unchanged).  boxes, margin, pieces,
     rest: as edited_sweep (default boxes: edit_boxes).  obstacles: the labels that count as obstacles (default every label).
     Returns one dict per move: label, landed (the voxels the moved object occupies after the move), overlap {label: voxels}
     (labels with voxels > 0: solid obstacle points the moved object lands on; the points the move vacates are not obstacles),
     overlap_volume {label: voxels times the inventory's voxel volume} and total (the overlapping voxels).  copies (None, a bool or
-    one per move; DESIGN.md, "Copying objects"): a copy vacates nothing, so its own label's solid points are obstacles too."""
+    one per move; DESIGN.md, "Copying objects"): a copy vacates nothing, so its own label's solid points are obstacles too.
+    groups (as edited_sweep; DESIGN.md, "Moving objects together"): each candidate moves its whole set; landed and overlap count
+    every label of the set, and the points the set vacates are not obstacles (a copy's stay)."""
     from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -546,13 +630,14 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     mv, mats = _check_moves(moves, ins_num, _lib.MAX_CANDIDATES)
     level = _check_level(level)
     drops = move_rests(rest, len(mv))
+    sets = move_groups(groups, mv, ins_num)
     flags = _check_copies(copies, mv, drops, ordered=False)
     regions = move_pieces(pieces, mv, ins_num, occ.device) or [None] * len(mv)
     words = ALL_LABELS if obstacles is None else label_words(obstacles)
     if not mv:
         return []
     if boxes is None:
-        boxes = edit_boxes(occ, labels, moves, T, ext, level, margin, pieces)
+        boxes = edit_boxes(occ, labels, moves, T, ext, level, margin, pieces, sets)
     boxes = _check_boxes(boxes, len(mv), dim)
     descs = _edit_moves(mv, mats, boxes, drops, regions, occ.device)
     overlap = np.zeros((len(mv), MAX_LABELS), dtype=np.int64)
@@ -560,7 +645,9 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     ctx = get_context(occ.device)
     head = (ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), dim, level, _lib.doubles(T, 16), _lib.doubles(ext, 3), descs)
     tail = (len(mv), (C.c_uint32 * 4)(*words), overlap.ctypes.data_as(C.POINTER(C.c_int64)), landed.ctypes.data_as(C.POINTER(C.c_int64)))
-    if any(flags):
+    if sets is not None:
+        ctx.call("dmnerf_move_overlap_groups", *head, _copy_flags(flags), _group_words(sets), *tail)
+    elif any(flags):
         ctx.call("dmnerf_move_overlap_copies", *head, _copy_flags(flags), *tail)
     else:
         ctx.call("dmnerf_move_overlap", *head, *tail)
@@ -682,6 +769,34 @@ def contacts_from_faces(faces, scene_transform, dim, extents=None):
     return {"faces": faces, "axes": (A / np.linalg.norm(A, axis=0)).T.copy(), "face_area": np.array(area)}
 
 
+def carried_labels(occ, labels, scene_transform, label, down, extents=None, level=0.45, min_faces=1, exclude=()):
+    """What rests on object `label`, transitively (DESIGN.md, "Moving objects together"): the labels whose solid points lie on
+    those of `label` along the down axis (supports of object_contacts, pairs of at least min_faces faces), then what rests on
+    those, and so on -> {"group": sorted labels with `label`, "chain": {label: (the label it rests on, faces)}}, the group=
+    that moves the object with what it carries.  exclude: labels never added (a voxelised wall or floor can touch a table top
+    from above); the chain says why each label was added.  Whole labels only: a caller that moves a piece of an object passes
+    the group it wants explicitly."""
+    label = _labels([label], MAX_LABELS - 1, "carried_labels")[0]
+    exclude = set(_labels(exclude, MAX_LABELS - 1, "carried_labels"))
+    return _carried(supports(object_contacts(occ, labels, scene_transform, extents, level), down, min_faces), label, exclude)
+
+
+def _carried(on, label, exclude):
+    """carried_labels' closure over a supports() result `on`: breadth first from `label`, ascending labels at each step."""
+    group, chain, frontier = {label}, {}, [label]
+    while frontier:
+        base = frontier.pop(0)
+        for top in sorted(on):
+            if top in group or top in exclude:
+                continue
+            faces = dict(on[top]).get(base)
+            if faces is not None:
+                group.add(top)
+                chain[top] = (base, faces)
+                frontier.append(top)
+    return {"group": sorted(group), "chain": chain}
+
+
 def supports(contacts, down, min_faces=1):
     """Which object rests on which, from object_contacts: along the index axis closest to +-down (network frame), the labels
     below each label's solid points -> {label: [(label_below, faces), ...]}, most faces first (then ascending label); pairs
@@ -723,7 +838,7 @@ def _check_point(x, what):
 
 
 def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=None, level=0.45, piece=None, rest="keep",
-                  obstacles=None, base=None, box=None, scene=None, copy=False):
+                  obstacles=None, base=None, box=None, scene=None, copy=False, group=None):
     """dmnerf_placement_map: object `label` (or its piece, with rest "keep" / "drop" as move_overlap) raised by `lift` voxels and
     lowered along the index axis closest to +-down (network frame, chosen as supports chooses it), at every horizontal offset
     that keeps it inside the grid of the labelled keep-all sweep occ / labels.  obstacles: the labels that count (default all).
@@ -736,6 +851,9 @@ def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=Non
     copy (DESIGN.md, "Copying objects"): place a copy of the object, its source standing: the scene's solid points of the label
     stay obstacles.  A copy always takes the based path (the identity base with the default box without one) and the scene is
     occ / labels when none is given; rest must be "keep".
+    group (None or labels holding `label`; DESIGN.md, "Moving objects together"): place the solid points of every label of the
+    group (the piece applied to the labels it applies to) as one body, its default box the group's; what the group vacates is no
+    obstacle, and a contact inside the group is never a support.  A group takes the based path as a copy does.
     Returns a dict:
       drop, support, contacts: device maps [U, V] (int32, int16, int32): the voxels it falls (-1: blocked where it is raised),
                       the obstacle label under most of its resting runs (-1: blocked, or resting on the grid's floor), and the
@@ -753,7 +871,7 @@ def placement_map(occ, labels, scene_transform, label, down, lift=0, extents=Non
         base = _move_matrix(base, 0)
     if box is not None:
         box = _check_boxes([box], 1, occ.shape[0])[0]
-    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene, copy)
+    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene, copy, group)
     if base is None and c["scene"] is not None:
         m, status = _placement_maps(c, [np.eye(4)], _placement_box(c, box), _object_points(c))
         if m[0] is None:
@@ -795,8 +913,9 @@ def _check_scene(scene, occ, labels):
     return s_occ, s_lab
 
 
-def _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene=None, copy=False):
-    """The checked arguments of a placement call: grid, level, label, lift, down axis, scene, copy and the ABI placement."""
+def _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene=None, copy=False,
+                    group=None):
+    """The checked arguments of a placement call: grid, level, label, lift, down axis, scene, copy, group and the ABI placement."""
     from .manipulator import _piece_region, move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -807,12 +926,14 @@ def _placement_call(occ, labels, scene_transform, label, down, lift, extents, le
         raise ValueError("placement: lift must be an integer >= 0 voxels, got %r" % (lift,))
     rest_drop = move_rests(rest, 1)[0]
     copy = _check_copies(copy, [label], [rest_drop])[0]
+    sets = move_groups(None if group is None else [group], [label], MAX_LABELS - 1, "placement")
+    group = None if sets is None else sets[0]
     words = ALL_LABELS if obstacles is None else label_words(obstacles)
     A, _ = grid_affine(T, 2, ext)
     axis, sign = down_axis((A / np.linalg.norm(A, axis=0)).T, down, "placement")
     dim = _check_sweep(occ, labels, "placement_map")
     scene = _check_scene(scene, occ, labels)
-    if copy and scene is None:                         # a copy's source stands in the grid it is sampled from
+    if (copy or group is not None) and scene is None:  # a copy's source stands in the grid it is sampled from
         scene = (occ, labels)
     if not 2 <= dim <= PLACE_MAX_DIM:
         raise ValueError("placement: dim %d outside [2, %d]" % (dim, PLACE_MAX_DIM))
@@ -823,7 +944,7 @@ def _placement_call(occ, labels, scene_transform, label, down, lift, extents, le
                           axis=axis, sign=sign, lift=int(lift))
     desc.obstacles[:] = words
     return {"occ": occ, "labels": labels, "T": T, "ext": ext, "level": level, "label": label, "lift": int(lift), "axis": axis,
-            "sign": sign, "dim": dim, "desc": desc, "piece": piece, "scene": scene, "copy": copy}
+            "sign": sign, "dim": dim, "desc": desc, "piece": piece, "scene": scene, "copy": copy, "group": group}
 
 
 def _placement_library(name, occ, *args):
@@ -840,10 +961,12 @@ def _placement_box(c, box):
     if box is not None:
         return box
     return edit_boxes(c["occ"], c["labels"], [(c["label"], np.eye(4))], c["T"], c["ext"], c["level"], 2,
-                      None if c["piece"] is None else [c["piece"]])[0]
+                      None if c["piece"] is None else [c["piece"]], None if c.get("group") is None else [c["group"]])[0]
 
 
 def _object_mask(c):
+    if c.get("group") is not None:
+        return _group_mask(c["occ"], c["labels"], c["group"], c["level"], c["piece"], c["T"], c["ext"])
     mask = (c["labels"] == c["label"]) & (c["occ"] > c["level"])
     if c["piece"] is not None:
         mask &= _region_keeps(c["piece"], c["T"], c["dim"], c["ext"], c["occ"].device)
@@ -870,7 +993,7 @@ def _map_result(c, info, drop, contacts, support, base, box, points_before):
             "lift": c["lift"], "label": c["label"], "dim": dim, "base": base, "box": None if box is None else tuple(int(x) for x in box),
             "points_before": points_before,
             "_call": (c["occ"], c["labels"], c["T"], c["ext"], c["level"], c["desc"], c["piece"]), "_scene": c.get("scene"),
-            "copy": bool(c.get("copy"))}
+            "copy": bool(c.get("copy")), "group": c.get("group")}
 
 
 def _placement_maps(c, bases, box, points_before):
@@ -890,6 +1013,8 @@ def _placement_maps(c, bases, box, points_before):
         name = "dmnerf_placement_maps_in_scene"
     if c.get("copy"):
         name, copy = "dmnerf_placement_maps_in_scene_copy", (1,)
+    if c.get("group") is not None:
+        name, copy = "dmnerf_placement_maps_in_scene_group", (int(bool(c.get("copy"))), _group_words([c["group"]]))
     _placement_library(name, occ, *grids, dim, c["level"], _lib.doubles(c["T"], 16), _lib.doubles(c["ext"], 3), C.byref(c["desc"]),
                        *copy, rows.ctypes.data_as(C.POINTER(C.c_double)), (C.c_int32 * 6)(*[int(x) for x in box]), n,
                        _lib.ptr(drop, torch.int32), _lib.ptr(contacts, torch.int32), _lib.ptr(support, torch.int16), infos,
@@ -965,6 +1090,8 @@ def placement(m, u, v):
     if scene is not None:                              # the scene of the map: the object from occ / labels (identity base by default)
         base = np.eye(4) if m.get("base") is None else m["base"]
         name, copy = ("dmnerf_placement_contacts_in_scene_copy", (1,)) if m.get("copy") else ("dmnerf_placement_contacts_in_scene", ())
+        if m.get("group") is not None:
+            name, copy = "dmnerf_placement_contacts_in_scene_group", (int(bool(m.get("copy"))), _group_words([m["group"]]))
         ctx.call(name, ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), _lib.ptr(scene[0]), _lib.ptr(scene[1], torch.int16),
                  *head[3:], *copy, _lib.doubles(base[:3], 12), (C.c_int32 * 6)(*m["box"]), *tail)
     elif m.get("base") is None:
@@ -1054,7 +1181,7 @@ def _turn_angles(turns):
 
 
 def place_object(occ, labels, scene_transform, label, down, near, on=None, stable=True, lift=0, max_tests=64, extents=None,
-                 level=0.45, piece=None, rest="keep", obstacles=None, turns=None, scene=None, copy=False):
+                 level=0.45, piece=None, rest="keep", obstacles=None, turns=None, scene=None, copy=False, group=None):
     """The placement of object `label` (or its piece) closest to the network-frame point `near`: over placement_map's offsets
     that are not blocked and rest on an obstacle whose label is in `on` (default: any), ordered by the distance of the placed
     centre of mass from `near` across the down axis (ties: the lowest (u, v)), the first that is stable -- testing at most
@@ -1065,19 +1192,24 @@ def place_object(occ, labels, scene_transform, label, down, near, on=None, stabl
     "tested": stability tests run; "map": the placement_map result it came from (without turns: the map); "turn": its angle
     (None without turns); "maps": [(angle, map)] of the turns that were mapped; "unfit": the angles whose turned object does not
     fit the grid; "unplaced": the angles whose turned object has no point or leaves the grid at this lift}.  scene, copy: as
-    placement_map's (DESIGN.md, "Arranging objects", "Copying objects"); the placement of a copy is the copy's move."""
+    placement_map's (DESIGN.md, "Arranging objects", "Copying objects"); the placement of a copy is the copy's move.  group: as
+    placement_map's (DESIGN.md, "Moving objects together"); `on` may name no label of the group, except for a copy."""
     near = _check_point(near, "near")
     if isinstance(max_tests, (bool, np.bool_)) or int(max_tests) != max_tests or int(max_tests) < 1:
         raise ValueError("placement: max_tests must be an integer >= 1, got %r" % (max_tests,))
     on = None if on is None else set(_labels(on, MAX_LABELS - 1, "placement"))
+    if group is not None and on is not None and not copy:
+        inside = sorted(on & set(_labels(group, MAX_LABELS - 1, "placement")))
+        if inside:
+            raise ValueError("placement: on names label(s) %s of the moved group: a group never rests on itself" % inside)
     angles = None if turns is None else _turn_angles(turns)
     if turns is None:
         m = placement_map(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene=scene,
-                          copy=copy)
+                          copy=copy, group=group)
         maps, unfit, unplaced = [(None, m)], [], []
     else:
         maps, unfit, unplaced = turned_placement_maps(occ, labels, scene_transform, label, down, angles, lift, extents, level, piece,
-                                                      rest, obstacles, scene, copy)
+                                                      rest, obstacles, scene, copy, group)
     out = {"placement": None, "reason": None, "candidates": 0, "tested": 0, "map": maps[0][1] if turns is None else None,
            "turn": None, "maps": [] if turns is None else maps, "unfit": unfit, "unplaced": unplaced}
     rows = placement_candidates([m for _, m in maps], near, on)
@@ -1099,14 +1231,14 @@ def place_object(occ, labels, scene_transform, label, down, near, on=None, stabl
 
 
 def turned_placement_maps(occ, labels, scene_transform, label, down, turns, lift=0, extents=None, level=0.45, piece=None,
-                          rest="keep", obstacles=None, scene=None, copy=False):
+                          rest="keep", obstacles=None, scene=None, copy=False, group=None):
     """placement_map of the object turned about the down axis by each of `turns` (degrees, or an integer K: 360 k / K), the
     turns built by turn_bases from the object's solid box and exact centre, mapped in dmnerf_placement_maps calls of at most
     MAX_BASES bases, with edit_boxes' source box -> ([(angle, map)] of the turns mapped, the angles that do not fit the grid,
     the angles whose turned object has no point or its top out of the grid).  scene, copy: as placement_map's; the turns are
-    built from the object in occ / labels."""
+    built from the object in occ / labels.  group: as placement_map's; the group turns as one body about its centre."""
     angles = _turn_angles(turns)
-    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene, copy)
+    c = _placement_call(occ, labels, scene_transform, label, down, lift, extents, level, piece, rest, obstacles, scene, copy, group)
     points, box, centre = _object_extent(_object_mask(c))
     if points == 0:
         raise ValueError("placement: label %d has no solid points%s" % (c["label"], " in its piece" if piece is not None else ""))
@@ -1177,12 +1309,12 @@ def largest_component_grid(occ, labels, level, objects):
 # ----------------------------------------------------------------------------------------------------------------- arrangement
 # DESIGN.md, "Arranging objects": the edited sweep's rule with the network replaced by the unedited grid at the nearest index
 # (edited_grid), and several objects placed one after another, each in the scene the earlier placements leave (arrange_objects).
-ARRANGE_KEYS = ("label", "near", "on", "piece", "rest", "turns", "stable", "lift", "obstacles", "copy")
+ARRANGE_KEYS = ("label", "near", "on", "piece", "rest", "turns", "stable", "lift", "obstacles", "copy", "group")
 
 
-def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes, drops, regions, flags=None):
-    """dmnerf_grid_edit of checked moves (flags: the checked copy flags, None for none): applied in place to occ / labels,
-    sampled from src_occ / src_labels -> edited_grid's report."""
+def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes, drops, regions, flags=None, sets=None):
+    """dmnerf_grid_edit of checked moves (flags: the checked copy flags, None for none; sets: the checked label sets, None for
+    none): applied in place to occ / labels, sampled from src_occ / src_labels -> edited_grid's report."""
     n, dim = len(mv), occ.shape[0]
     overwritten = np.zeros((n, MAX_LABELS), dtype=np.int64)
     landed = np.zeros(n, dtype=np.int64)
@@ -1191,7 +1323,9 @@ def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes,
             _edit_moves(mv, mats, boxes, drops, regions, occ.device))
     tail = (n, _lib.ptr(occ), _lib.ptr(labels, torch.int16), landed.ctypes.data_as(C.POINTER(C.c_int64)),
             overwritten.ctypes.data_as(C.POINTER(C.c_int64)))
-    if flags is not None and any(flags):
+    if sets is not None:
+        ctx.call("dmnerf_grid_edit_groups", *head, _copy_flags(flags or [False] * n), _group_words(sets), *tail)
+    elif flags is not None and any(flags):
         ctx.call("dmnerf_grid_edit_copies", *head, _copy_flags(flags), *tail)
     else:
         ctx.call("dmnerf_grid_edit", *head, *tail)
@@ -1200,7 +1334,7 @@ def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes,
 
 
 def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, boxes=None, margin=2, pieces=None, rest="keep",
-                copies=None):
+                copies=None, groups=None):
     """dmnerf_grid_edit: edited_sweep's moves applied in order to the labelled keep-all sweep occ / labels ([dim]^3 float32 / int16
     on the device) without the network: a move shows at p the unedited grid at the nearest grid index of trans p, as the collision
     checks sample a moved object.  On a grid whose points and steps are exact in fp32, whole-voxel translations and quarter turns
@@ -1208,7 +1342,8 @@ def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, b
     as edited_sweep (default boxes: edit_boxes of occ / labels).  Works on copies -> (occ', labels', report), report one dict per
     move: label, landed (the voxels it takes from a solid target), overwritten {label: voxels} (labels with voxels > 0: solid
     points of the grid as the earlier moves left it that it lands on and does not vacate), overwritten_volume and total.
-    copies: as edited_sweep (DESIGN.md, "Copying objects"); a copy's overwritten counts its own label's points too."""
+    copies: as edited_sweep (DESIGN.md, "Copying objects"); a copy's overwritten counts its own label's points too.  groups: as
+    edited_sweep (DESIGN.md, "Moving objects together"); landed and overwritten count the whole set."""
     from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -1217,17 +1352,19 @@ def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, b
     mv, mats = _check_moves(moves, MAX_LABELS - 1)
     level = _check_level(level)
     drops = move_rests(rest, len(mv))
-    flags = _check_copies(copies, mv, drops)
+    sets = move_groups(groups, mv, MAX_LABELS - 1)
+    flags = _check_copies(copies, mv, drops, sets=sets)
     regions = move_pieces(pieces, mv, MAX_LABELS - 1, occ.device) or [None] * len(mv)
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
     if boxes is None:
-        boxes = edit_boxes(occ, labels, moves, T, ext, level, margin, pieces)
+        boxes = edit_boxes(occ, labels, moves, T, ext, level, margin, pieces, sets)
     boxes = _check_boxes(boxes, len(mv), dim)
     out_occ, out_labels = occ.clone(memory_format=torch.contiguous_format), labels.clone(memory_format=torch.contiguous_format)
     if not mv:
         return out_occ, out_labels, []
-    return out_occ, out_labels, _grid_edit(occ, labels, out_occ, out_labels, T, ext, level, mv, mats, boxes, drops, regions, flags)
+    return out_occ, out_labels, _grid_edit(occ, labels, out_occ, out_labels, T, ext, level, mv, mats, boxes, drops, regions, flags,
+                                           sets)
 
 
 def _check_items(items, dim, device):
@@ -1255,17 +1392,24 @@ def _check_items(items, dim, device):
         if not isinstance(c["copy"], (bool, np.bool_)):
             raise ValueError("arrange: item %d: copy must be True or False, got %r" % (i, c["copy"]))
         c["copy"] = bool(c["copy"])
-        kinds = seen.setdefault(c["label"], {})
-        if not c["copy"] and "move" in kinds:
-            raise ValueError("arrange: items %d and %d share label %d (the second move would also vacate the first one's landed "
-                             "points)" % (kinds["move"], i, c["label"]))
-        if not c["copy"] and "copy" in kinds:
-            raise ValueError("arrange: item %d moves label %d after item %d copies it (the move would also vacate the copy)"
-                             % (i, c["label"], kinds["copy"]))
-        kinds.setdefault("copy" if c["copy"] else "move", i)
+        sets = move_groups(None if c["group"] is None else [c["group"]], [c["label"]], MAX_LABELS - 1, "arrange")
+        c["group"] = None if sets is None else sets[0]
+        for k in c["group"] or (c["label"],):
+            kinds = seen.setdefault(k, {})
+            if not c["copy"] and "move" in kinds:
+                raise ValueError("arrange: items %d and %d share label %d (the second move would also vacate the first one's landed "
+                                 "points)" % (kinds["move"], i, k))
+            if not c["copy"] and "copy" in kinds:
+                raise ValueError("arrange: item %d moves label %d after item %d copies it (the move would also vacate the copy)"
+                                 % (i, k, kinds["copy"]))
+        for k in c["group"] or (c["label"],):
+            seen[k].setdefault("copy" if c["copy"] else "move", i)
         c["near"] = _check_point(c["near"], "near")
         if c["on"] is not None:
             c["on"] = _labels(c["on"], MAX_LABELS - 1, "arrange")
+            if c["group"] is not None and not c["copy"] and set(c["on"]) & set(c["group"]):
+                raise ValueError("arrange: item %d: on names label(s) %s of its group: a group never rests on itself"
+                                 % (i, sorted(set(c["on"]) & set(c["group"]))))
         if c["turns"] is not None:
             _turn_angles(c["turns"])
         c["stable"] = True if c["stable"] is None else c["stable"]
@@ -1295,14 +1439,17 @@ def arrange_objects(occ, labels, scene_transform, items, down, extents=None, lev
     earlier item keeps its label where it landed), piece, rest, turns, stable, lift and obstacles, as place_object takes them, and
     copy (DESIGN.md, "Copying objects"; default False): place a copy of the object from the unedited grid, its source standing as
     an obstacle (`on` may name its own label, to stack it on its source).  At most MAX_MOVES items; no two moves of one label, no
-    move of a label after a copy of it; copies of one label may repeat and may follow its move.  down: shared by every item.
+    move of a label after a copy of it; copies of one label may repeat and may follow its move.  group (DESIGN.md, "Moving
+    objects together"; labels holding the item's label): the item moves its whole set as one body, as placement_map's group; two
+    move items whose sets intersect are rejected as two moves of one label.  down: shared by every item.
     Every item is checked before any device work.
     Returns a dict:
       items:  per item, place_object's result and its label; placement None and a reason when it was not placed (its maps were
               computed on the state before its own move and refer to the state's tensors, which later items edit);
-      moves:  [(label, 4x4 nested list)] of the placed items in order, and pieces / rest / copies aligned with them:
+      moves:  [(label, 4x4 nested list)] of the placed items in order, and pieces / rest / copies / groups aligned with them:
               manipulate_frame, manipulator_eval, edited_sweep and edited_mesh take them unchanged (copies: edited_sweep,
-              edited_mesh, edited_grid and render_moves);
+              edited_mesh, edited_grid and render_moves; groups, a label tuple or None per move: edited_grid, edited_sweep,
+              edited_mesh and render_moves);
       occ, labels: the arranged grid, equal to edited_grid(occ, labels, ..., moves, pieces=pieces, rest=rest, copies=copies) bit
               for bit;
       report: edited_grid's report of each placed move (overwritten: what it landed on in the scene left before it)."""
@@ -1322,11 +1469,13 @@ def arrange_objects(occ, labels, scene_transform, items, down, extents=None, lev
     if not 2 <= dim <= PLACE_MAX_DIM:
         raise ValueError("placement: dim %d outside [2, %d]" % (dim, PLACE_MAX_DIM))
     state_occ, state_labels = occ.clone(memory_format=torch.contiguous_format), labels.clone(memory_format=torch.contiguous_format)
-    out = {"items": [], "moves": [], "pieces": [], "rest": [], "copies": [], "occ": state_occ, "labels": state_labels, "report": []}
+    out = {"items": [], "moves": [], "pieces": [], "rest": [], "copies": [], "groups": [], "occ": state_occ, "labels": state_labels,
+           "report": []}
     for it in checked:
         try:
             r = place_object(occ, labels, T, it["label"], down, it["near"], it["on"], it["stable"], it["lift"], max_tests, ext, level,
-                             it["piece"], it["rest"], it["obstacles"], it["turns"], scene=(state_occ, state_labels), copy=it["copy"])
+                             it["piece"], it["rest"], it["obstacles"], it["turns"], scene=(state_occ, state_labels), copy=it["copy"],
+                             group=it["group"])
         except ValueError as e:        # found on the device: no solid points (in its piece), or the lift takes its top out
             r = {"placement": None, "reason": str(e)}
         out["items"].append(dict(r, label=it["label"]))
@@ -1335,13 +1484,16 @@ def arrange_objects(occ, labels, scene_transform, items, down, extents=None, lev
         trans = r["placement"]["transformation"]
         move = (it["label"], trans)
         pieces = None if it["piece"] is None else [it["piece"]]
-        box = edit_boxes(occ, labels, [move], T, ext, level, 2, pieces)
+        sets = None if it["group"] is None else [it["group"]]
+        box = edit_boxes(occ, labels, [move], T, ext, level, 2, pieces, sets)
         out["report"] += _grid_edit(occ, labels, state_occ, state_labels, T, ext, level, [it["label"]],
-                                    [np.asarray(trans, dtype=np.float64)], box, move_rests(it["rest"], 1), [it["piece"]], [it["copy"]])
+                                    [np.asarray(trans, dtype=np.float64)], box, move_rests(it["rest"], 1), [it["piece"]], [it["copy"]],
+                                    sets)
         out["moves"].append(move)
         out["pieces"].append(it["piece"])
         out["rest"].append(it["rest"])
         out["copies"].append(it["copy"])
+        out["groups"].append(it["group"])
     return out
 
 

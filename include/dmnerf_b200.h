@@ -681,6 +681,53 @@ DMNERF_API int dmnerf_placement_contacts_in_scene_copy(dmnerf_ctx* ctx, const fl
                                                        int v, int32_t* cells_host, int64_t max_cells, int64_t* n_cells_host,
                                                        int32_t* drop_host, void* stream);
 
+/* ---- moving objects together (DESIGN.md, "Moving objects together"; no counterpart in the original) -------------------------
+ * A move may carry a label set G (a table and what stands on it) that holds its own label: each rule tests "label in G" where a
+ * move of one label tests "label == label".  The take writes the target's own label; the vacate clears the points of every label
+ * of G (with the piece and rest_drop tests of a single move); the piece (region_drops) is evaluated for the label of the point
+ * tested, so a piece cuts the labels of G it applies to and the others move whole.  A label outside [0, 127] (a state grid of
+ * dmnerf_mesh_occupancy_edit is not checked) belongs to no set, as it equalled no move's label before.  The collision checks do not count the points
+ * a group vacates; placement places the solid points of G (the piece applied) as one body, and a copy keeps its source's points
+ * as obstacles.  The entry points below are the _copies / _copy ones with label sets: groups_host [n][4] (HOST uint32, the label
+ * words of each move or candidate, bit k of word k / 32; NULL: each move's own label) or group_host [4] (one per call; NULL: the
+ * placement's label).  With every set {label} each equals its namesake bit for bit; a group is one move towards
+ * DMNERF_MAX_MOVES and evaluates its targets in one pass.
+ * Rejected on the host, before any launch, beside everything the namesake rejects: a set without its move's label, a set with a
+ * label outside [0, ins_num] (outside [0, 127] for the grid-only calls: dmnerf_grid_edit_groups, dmnerf_move_overlap_groups and
+ * the placement pair), and, for the moves applied in order, a move whose set holds a label of an earlier copy's set.  Each error
+ * names the entry point called. */
+DMNERF_API int dmnerf_mesh_occupancy_edit_groups(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host,
+                                                 int dim, float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host,
+                                                 const int32_t* copies_host /* [n] */, const uint32_t* groups_host /* [n][4] */,
+                                                 int n_moves, float* occ, int16_t* labels, int64_t* evaluated_host, void* stream);
+DMNERF_API int dmnerf_grid_edit_groups(dmnerf_ctx* ctx, const float* src_occ, const int16_t* src_labels, int dim, float level,
+                                       const double* transform_host, const double* extents_host, const dmnerf_edit_move* moves_host,
+                                       const int32_t* copies_host /* [n] */, const uint32_t* groups_host /* [n][4] */, int n_moves,
+                                       float* occ, int16_t* labels, int64_t* landed_host /* [n] */,
+                                       int64_t* overwritten_host /* [n][128] */, void* stream);
+DMNERF_API int dmnerf_render_moved_groups(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                          const dmnerf_render_moves* moves, const int32_t* copies_host /* [n_moves] */,
+                                          const uint32_t* groups_host /* [n_moves][4] */, int64_t* evaluated_host, void* stream);
+DMNERF_API int dmnerf_move_overlap_groups(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                          const double* transform_host, const double* extents_host,
+                                          const dmnerf_edit_move* candidates_host, const int32_t* copies_host /* [n] */,
+                                          const uint32_t* groups_host /* [n][4] */, int n_candidates, const uint32_t* obstacles_host,
+                                          int64_t* overlap_host /* [n][128] */, int64_t* landed_host /* [n] */, void* stream);
+DMNERF_API int dmnerf_placement_maps_in_scene_group(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,
+                                                    const int16_t* scene_labels, int dim, float level, const double* transform_host,
+                                                    const double* extents_host, const dmnerf_placement* placement, int copy,
+                                                    const uint32_t* group_host /* [4] */, const double* bases_host /* [n][12] */,
+                                                    const int32_t* box_host /* [6] */, int n_bases, int32_t* drop, int32_t* contacts,
+                                                    int16_t* support, dmnerf_placement_info* info_host /* [n] */,
+                                                    int32_t* status_host /* [n] */, void* stream);
+DMNERF_API int dmnerf_placement_contacts_in_scene_group(dmnerf_ctx* ctx, const float* occ, const int16_t* labels,
+                                                        const float* scene_occ, const int16_t* scene_labels, int dim, float level,
+                                                        const double* transform_host, const double* extents_host,
+                                                        const dmnerf_placement* placement, int copy,
+                                                        const uint32_t* group_host /* [4] */, const double* base_host /* [12] */,
+                                                        const int32_t* box_host /* [6] */, int u, int v, int32_t* cells_host,
+                                                        int64_t max_cells, int64_t* n_cells_host, int32_t* drop_host, void* stream);
+
 /* ---- connected components (DESIGN.md, "Connected components"; no counterpart in the original) --------------------------------
  * The solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order, p = (i dim + j) dim + k) split into components:
  * two solid points are adjacent when they are face neighbours (connectivity 6) or face, edge or corner neighbours (26), never

@@ -108,7 +108,21 @@ def parse(argv=None):
     ap.add_argument("--render", choices=("exchanger", "samples"), default="exchanger",
                     help="render the frame with the exchanger (manipulate_frame) or per sample (render_frame(moves=))")
     ap.add_argument("--copy", action="store_true", help="copy the piece instead of moving it: the source stays (needs --render samples)")
+    ap.add_argument("--with", dest="with_labels", type=int, nargs="+", default=None, metavar="L",
+                    help="move these labels together with the piece's label, as one body (needs --render samples)")
+    ap.add_argument("--carry", action="store_true",
+                    help="also move what rests on the piece's label, transitively (carried_labels; needs --down and --render samples)")
     a = ap.parse_args(argv)
+    a.grouped = a.with_labels is not None or a.carry
+    if a.grouped:
+        if a.arrange is not None:
+            ap.error('--with and --carry are per item with --arrange: give the items "group": [labels]')
+        if a.render != "samples":
+            ap.error("--with and --carry need --render samples: the exchanger renders one label per move")
+        if a.carry and (a.down is None or not any(a.down)):
+            ap.error("--carry needs --down X Y Z, not 0 0 0: what rests on the object is found along it")
+        if a.until_contact:
+            ap.error("--with and --carry cannot be combined with --until-contact: the slide moves one label")
     if a.copy:
         if a.render != "samples":
             ap.error("--copy needs --render samples: the exchanger renders moves only")
@@ -146,8 +160,8 @@ def parse(argv=None):
     else:
         if a.mode is None:
             ap.error("give --mode or --place-at")
-        if a.down is not None or a.on is not None or a.lift is not None or a.any_stability or a.turns is not None:
-            ap.error("--down, --on, --lift, --any-stability and --turns need --place-at")
+        if (a.down is not None and not a.carry) or a.on is not None or a.lift is not None or a.any_stability or a.turns is not None:
+            ap.error("--down, --on, --lift, --any-stability and --turns need --place-at (--down also serves --carry)")
         a.distance = -0.25 if a.distance is None else a.distance
         a.yaw = 90.0 if a.yaw is None else a.yaw
         a.scale = 1.2 if a.scale is None else a.scale
@@ -171,7 +185,7 @@ def parse(argv=None):
     return a
 
 
-ITEM_KEYS = ("label", "piece", "near", "on", "turns", "rest", "any_stability", "copy")
+ITEM_KEYS = ("label", "piece", "near", "on", "turns", "rest", "any_stability", "copy", "group")
 
 
 def read_spec(path):
@@ -186,6 +200,11 @@ def read_spec(path):
                              % (i, path, ", ".join(ITEM_KEYS)))
         if not isinstance(it.get("copy", False), bool):
             raise SystemExit("move_objects: item %d of %s: copy must be true or false" % (i, path))
+        g = it.get("group")
+        if g is not None and (not isinstance(g, list) or not all(isinstance(k, int) and not isinstance(k, bool) for k in g)):
+            raise SystemExit("move_objects: item %d of %s: group must be a list of labels" % (i, path))
+        if g is not None and "label" in it and it["label"] not in g:
+            raise SystemExit("move_objects: item %d of %s: the group %s does not hold the item's label %d" % (i, path, g, it["label"]))
     return spec
 
 
@@ -218,9 +237,12 @@ def arrange_pieces(a, occ, labels, T, ext, spec, chosen):
     """--arrange: arrange_objects for the items -> (moves, regions, rests, the record's arrange)."""
     from dmnerf_b200.objects import arrange_objects
     items = []
-    for it, (_, label, region) in zip(spec, chosen):
+    for i, (it, (_, label, region)) in enumerate(zip(spec, chosen)):
+        if it.get("group") is not None and label not in it["group"]:        # a piece item: its label is known from the sweep
+            raise SystemExit("move_objects: item %d: the group %s does not hold the label %d of its piece" % (i, it["group"], label))
         items.append({"label": label, "near": it["near"], "on": it.get("on"), "piece": region, "rest": it.get("rest", "keep"),
-                      "turns": it.get("turns"), "stable": not it.get("any_stability", False), "copy": it.get("copy", False)})
+                      "turns": it.get("turns"), "stable": not it.get("any_stability", False), "copy": it.get("copy", False),
+                      "group": it.get("group")})
     r = arrange_objects(occ, labels, T, items, a.down, ext, a.level)
     rec, report = [], iter(r["report"])
     for it, (piece, label, _), res in zip(spec, chosen, r["items"]):
@@ -228,11 +250,12 @@ def arrange_pieces(a, occ, labels, T, ext, spec, chosen):
         entry = {"label": label, "piece": piece, "placed": p is not None, "reason": res.get("reason"),
                  "offset": None if p is None else list(p["offset"]), "drop": None if p is None else p["drop"],
                  "support": None if p is None else p["support"], "stable": None if p is None else p["stable"],
-                 "turn": res.get("turn"), "copy": bool(it.get("copy", False))}
+                 "turn": res.get("turn"), "copy": bool(it.get("copy", False)),
+                 "group": None if it.get("group") is None else sorted(set(it["group"]))}
         if p is not None:
             entry["overwritten"] = {str(k): v for k, v in next(report)["overwritten"].items()}
         rec.append(entry)
-    return r["moves"], r["pieces"], r["rest"], r["copies"], rec
+    return r["moves"], r["pieces"], r["rest"], r["copies"], r["groups"], rec
 
 
 def choose_piece(a, model_fine, T, ext):
@@ -274,12 +297,12 @@ def slide_translation(a, occ, labels, T, ext, label, region):
     return {"requested": a.distance, "found": r["distance"], "contact": contact}
 
 
-def place_piece(a, occ, labels, T, ext, label, region):
+def place_piece(a, occ, labels, T, ext, label, region, group=None):
     """--place-at: place_object for the piece -> {transformation, offset, drop, support, stable, contacts}; exits when no offset
     qualifies."""
     from dmnerf_b200.objects import place_object
     r = place_object(occ, labels, T, label, a.down, a.place_at, on=a.on, stable=not a.any_stability, lift=a.lift, extents=ext,
-                     level=a.level, piece=region, rest=a.rest, turns=None if a.turns == 1 else a.turns, copy=a.copy)
+                     level=a.level, piece=region, rest=a.rest, turns=None if a.turns == 1 else a.turns, copy=a.copy, group=group)
     p = r["placement"]
     if p is None:
         raise SystemExit("move_objects: no placement: %s" % r["reason"])
@@ -315,32 +338,43 @@ def main(argv=None):
         spec = read_spec(a.arrange)
         if any(it.get("copy", False) for it in spec) and a.render != "samples":
             raise SystemExit("move_objects: an arrangement with copies needs --render samples: the exchanger renders moves only")
+        if any(it.get("group") is not None for it in spec) and a.render != "samples":
+            raise SystemExit("move_objects: an arrangement with groups needs --render samples: the exchanger renders one label per "
+                             "move")
         chosen = choose_pieces(a, nets[1], T, ext, spec)
         piece, label, centre, region = None, None, None, None
     else:
         piece, label, centre, region = choose_piece(a, nets[1], T, ext)
-    sweep = a.check or a.until_contact or a.place_at is not None or a.arrange is not None or a.render == "samples"
+    sweep = a.check or a.until_contact or a.place_at is not None or a.arrange is not None or a.render == "samples" or a.grouped
     if sweep:
         from dmnerf_b200.objects import object_mask, occupancy_objects
         with torch.no_grad():
             occ, labels = occupancy_objects(nets[1], T, object_mask(ins_num, remove=[]), a.grid_dim, ext, a.near, a.far,
                                             a.N_importance, device=next(nets[1].parameters()).device)
+    group = chain = None
+    if a.grouped:                                      # the piece's label and the labels moved with it
+        group = sorted(set(a.with_labels or []) | {label})
+        if a.carry:
+            from dmnerf_b200.objects import carried_labels
+            c = carried_labels(occ, labels, T, label, a.down, ext, a.level)
+            group = sorted(set(group) | set(c["group"]))
+            chain = {str(k): [b, f] for k, (b, f) in c["chain"].items()}
     if a.until_contact:
         slide = slide_translation(a, occ, labels, T, ext, label, region)
         a.distance = np.sign(a.distance) * (slide["found"] or 0.0)
     if a.arrange is not None:
-        moves, regions, rests, copies, arranged = arrange_pieces(a, occ, labels, T, ext, spec, chosen)
+        moves, regions, rests, copies, groups, arranged = arrange_pieces(a, occ, labels, T, ext, spec, chosen)
         if not moves:
             raise SystemExit("move_objects: no item was placed: %s" % "; ".join("%d: %s" % (e["label"], e["reason"]) for e in arranged))
         trans = {"transformations": [{"transformation": m, "mode": "placement"} for _, m in moves]}
     elif a.place_at is not None:
-        place = place_piece(a, occ, labels, T, ext, label, region)
+        place = place_piece(a, occ, labels, T, ext, label, region, group)
         trans = {"transformations": [{"transformation": place.pop("transformation"), "mode": "placement"}]}
     else:
         trans = manipulation_transform(centre, a.mode, distance=a.distance, yaw=a.yaw, scale=a.scale)
     if a.arrange is None:
         moves, regions, rests = [(label, trans["transformations"][0]["transformation"])], [region], [a.rest]
-        copies = [a.copy]
+        copies, groups = [a.copy], [group]
     dev = next(nets[1].parameters()).device
     pose_t = torch.from_numpy(c2w).to(dev)
     evaluated = None
@@ -348,7 +382,7 @@ def main(argv=None):
         from dmnerf_b200.objects import render_moves
         from dmnerf_b200.render import render_frame
         moved = render_moves(occ, labels, T, moves, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests,
-                             copies=copies)
+                             copies=copies, groups=groups)
         with torch.no_grad():
             fr = render_frame(a.H, a.W, a.K, pose_t, a.near, a.far, nets[0], nets[1], a.N_samples, a.N_importance, keep_all_ins=True,
                               device=dev, moves=moved)
@@ -376,6 +410,10 @@ def main(argv=None):
     record["render"], record["evaluated"] = a.render, evaluated
     if any(copies):
         record["copies"] = copies
+    if group is not None:
+        record["group"] = group
+    if chain is not None:
+        record["chain"] = chain
     if slide is not None:
         record["slide"] = slide
     if place is not None:
@@ -383,7 +421,7 @@ def main(argv=None):
     if a.check:
         from dmnerf_b200.objects import move_overlap
         r = move_overlap(occ, labels, T, [(label, trans["transformations"][0]["transformation"])], ext, a.level, pieces=[region],
-                         rest=a.rest, copies=a.copy)[0]
+                         rest=a.rest, copies=a.copy, groups=[group])[0]
         record["overlap"] = {"voxels": {str(k): v for k, v in r["overlap"].items()},
                              "volume": {str(k): v for k, v in r["overlap_volume"].items()}}
         record["landed"] = r["landed"]
@@ -392,7 +430,7 @@ def main(argv=None):
     if a.mesh:
         from dmnerf_b200.objects import edited_mesh
         m = edited_mesh(nets[1], T, moves, a.grid_dim, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests,
-                        min_cluster=a.min_cluster, copies=copies)
+                        min_cluster=a.min_cluster, copies=copies, groups=groups)
         M.write_ply(os.path.join(a.out, "edited.ply"), m["vertices"], m["triangles"])
         lab = m["labels"].cpu().numpy()
         colors = np.where((lab >= 0)[:, None], lut[np.clip(lab, 0, ins_num)], 0).astype(np.uint8)   # instance.png's colours
