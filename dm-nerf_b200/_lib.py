@@ -76,6 +76,12 @@ class RenderMoves(C.Structure):
                 ("extents", C.c_double * 3), ("level", C.c_float), ("voxel", C.c_float)]
 
 
+class Deformation(C.Structure):
+    """Mirror of `struct dmnerf_deformation` (objects.Deformation.abi builds one)."""
+    _fields_ = [("n_knots", C.c_int32), ("frame", C.c_double * 12), ("h0", C.c_double), ("dh", C.c_double),
+                ("knots", C.POINTER(C.c_double))]
+
+
 class Placement(C.Structure):
     """Mirror of `struct dmnerf_placement` (objects.placement_map builds one)."""
     _fields_ = [("piece", RegionDesc), ("obstacles", C.c_uint32 * 4), ("label", C.c_int32), ("rest_drop", C.c_int32),
@@ -249,6 +255,21 @@ PROTOTYPES = {
                                                            C.POINTER(C.c_uint32), C.POINTER(C.c_double), C.POINTER(C.c_int32), C.c_int,
                                                            C.c_int, C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64),
                                                            C.POINTER(C.c_int32), C.c_void_p]),
+    "dmnerf_mesh_occupancy_edit_deformed": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int,
+                                                      C.c_float, C.c_float, C.c_int64, C.POINTER(EditMove), C.POINTER(C.c_int32),
+                                                      C.POINTER(C.c_uint32), C.POINTER(Deformation), C.c_int, _f32p, C.c_void_p,
+                                                      C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_grid_edit_deformed": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double),
+                                            C.POINTER(C.c_double), C.POINTER(EditMove), C.POINTER(C.c_int32), C.POINTER(C.c_uint32),
+                                            C.POINTER(Deformation), C.c_int, _f32p, C.c_void_p, C.POINTER(C.c_int64),
+                                            C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_render_moved_deformed": (C.c_int, [C.c_void_p, C.POINTER(RenderIO), C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
+                                               C.POINTER(RenderMoves), C.POINTER(C.c_int32), C.POINTER(C.c_uint32),
+                                               C.POINTER(Deformation), C.POINTER(C.c_int64), C.c_void_p]),
+    "dmnerf_move_overlap_deformed": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double),
+                                               C.POINTER(C.c_double), C.POINTER(EditMove), C.POINTER(C.c_int32), C.POINTER(C.c_uint32),
+                                               C.POINTER(Deformation), C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_int64),
+                                               C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_object_components": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int, C.c_void_p,
                                            C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_component_table": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,

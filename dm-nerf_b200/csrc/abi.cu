@@ -426,6 +426,7 @@ struct RenderMoves {
   int n;
   float voxel, level;
   int64_t evaluated[2];
+  const Deform* deforms;      // [n], or NULL: every move rigid
 };
 
 // dm_nerf() on device buffers with the bound pair (bound_pair); edit: the checked scene edit, or NULL for none (the
@@ -479,7 +480,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   // render.py:49-61  points, embeddings, coarse network
   if ((rc = mlp_dispatch(ctx, 0, nullptr, io->rays_o, io->rays_d, z_c, n * S, S, raw_c, impl, st))) return rc;
   if (mv && (rc = render_moves_pass(ctx->moves, ctx->net[0], impl == DMNERF_IMPL_UMMA_F16, mv->moves, mv->copies, mv->n, io->rays_o, io->rays_d,
-                                    z_c, n, S, C, mv->voxel, mv->level, raw_c, &mv->evaluated[0], st)))
+                                    z_c, n, S, C, mv->voxel, mv->level, raw_c, &mv->evaluated[0], st, mv->deforms)))
     return rc;
   DMN_STAGE_MARK();
   // render.py:63     coarse composite
@@ -492,7 +493,7 @@ static int render_forward_impl(dmnerf_ctx* ctx, const dmnerf_render_io* io, int6
   // render.py:71-82  fine network on all S+I depths
   if ((rc = mlp_dispatch(ctx, 1, nullptr, io->rays_o, io->rays_d, z_f, n * F, F, raw_f, impl, st))) return rc;
   if (mv && (rc = render_moves_pass(ctx->moves, ctx->net[1], impl == DMNERF_IMPL_UMMA_F16, mv->moves, mv->copies, mv->n, io->rays_o, io->rays_d,
-                                    z_f, n, F, C, mv->voxel, mv->level, raw_f, &mv->evaluated[1], st)))
+                                    z_f, n, F, C, mv->voxel, mv->level, raw_f, &mv->evaluated[1], st, mv->deforms)))
     return rc;
   DMN_STAGE_MARK();
   // render.py:86     fine composite
@@ -518,12 +519,18 @@ DMNERF_API int dmnerf_render_forward(dmnerf_ctx* ctx, const dmnerf_render_io* io
 
 }  // extern "C"
 
-// dmnerf_render_moved with copy flags copies_host [n_moves] (NULL: none) and label sets groups_host [n_moves][4] (NULL: each
-// move's own label)
+// dmnerf_render_moved with copy flags copies_host [n_moves] (NULL: none), label sets groups_host [n_moves][4] (NULL: each
+// move's own label) and deformations deformations_host [n_moves] (NULL: every move rigid)
 static int render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
                         const dmnerf_render_moves* moves, const int32_t* copies_host, const uint32_t* groups_host,
-                        int64_t* evaluated_host, void* stream, const char* who) {
+                        int64_t* evaluated_host, void* stream, const char* who,
+                        const dmnerf_deformation* deformations_host = nullptr) {
   if (evaluated_host) evaluated_host[0] = evaluated_host[1] = 0;
+  if (deformations_host) {
+    DMN_CHECK(moves != nullptr, "%s: moves is NULL", who);
+    const int nm = moves->n_moves;
+    if (deformations_check(deformations_host, nm > 0 && nm <= DMNERF_MAX_MOVES ? nm : 0, who)) return 1;
+  }
   if (bound_pair(ctx, who)) return 1;
   DMN_CHECK(!(flags & ~RENDER_FLAGS), "%s: unknown flag bits 0x%x", who, flags & ~RENDER_FLAGS);
   DMN_CHECK(impl >= DMNERF_IMPL_AUTO && impl <= DMNERF_IMPL_UMMA_F16, "%s: unknown impl %d", who, impl);
@@ -546,7 +553,12 @@ static int render_moved(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, 
   Edit e;
   const Edit* edit;
   if (int rc = scene_edit(ctx, io ? io->edit : nullptr, (cudaStream_t)stream, e, edit, who)) return rc;
-  RenderMoves r = {mv, copies_host, moves->n_moves, moves->voxel, moves->level, {0, 0}};
+  Deform defs[DMNERF_MAX_MOVES];
+  bool deformed = false;
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  if (int rc = deformations_from_abi(deformations_host, moves->n_moves, ctx->moves.knots, defs, &deformed, who, (cudaStream_t)stream))
+    return rc;
+  RenderMoves r = {mv, copies_host, moves->n_moves, moves->voxel, moves->level, {0, 0}, deformed ? defs : nullptr};
   const int rc = f16_verdict(ctx, render_forward_impl(ctx, io, n, S, NI, flags, impl, edit, stream, &r), impl, stream);
   if (evaluated_host && !rc) { evaluated_host[0] = r.evaluated[0]; evaluated_host[1] = r.evaluated[1]; }
   return rc;
@@ -569,6 +581,13 @@ DMNERF_API int dmnerf_render_moved_groups(dmnerf_ctx* ctx, const dmnerf_render_i
                                           const dmnerf_render_moves* moves, const int32_t* copies_host, const uint32_t* groups_host,
                                           int64_t* evaluated_host, void* stream) {
   return render_moved(ctx, io, n, S, NI, flags, impl, moves, copies_host, groups_host, evaluated_host, stream, "render_moved_groups");
+}
+
+DMNERF_API int dmnerf_render_moved_deformed(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                            const dmnerf_render_moves* moves, const int32_t* copies_host, const uint32_t* groups_host,
+                                            const dmnerf_deformation* deformations_host, int64_t* evaluated_host, void* stream) {
+  return render_moved(ctx, io, n, S, NI, flags, impl, moves, copies_host, groups_host, evaluated_host, stream, "render_moved_deformed",
+                      deformations_host);
 }
 
 DMNERF_API int dmnerf_sync_check(dmnerf_ctx* ctx, void* stream) {
@@ -830,12 +849,13 @@ DMNERF_API int dmnerf_mesh_occupancy(dmnerf_ctx* ctx, int net, const double* tra
 
 }  // extern "C"
 
-// dmnerf_mesh_occupancy_edit with copy flags copies_host [n_moves] (NULL: none) and label sets groups_host [n_moves][4] (NULL:
-// each move's own label)
+// dmnerf_mesh_occupancy_edit with copy flags copies_host [n_moves] (NULL: none), label sets groups_host [n_moves][4] (NULL:
+// each move's own label) and deformations deformations_host [n_moves] (NULL: every move rigid)
 static int mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host, int dim, float voxel,
                                float level, int64_t slab, const dmnerf_edit_move* moves_host, const int32_t* copies_host,
                                const uint32_t* groups_host, int n_moves, float* occ, int16_t* labels, int64_t* evaluated_host,
-                               void* stream, const char* who) {
+                               void* stream, const char* who, const dmnerf_deformation* deformations_host = nullptr) {
+  if (deformations_check(deformations_host, n_moves > 0 && n_moves <= DMNERF_MAX_MOVES ? n_moves : 0, who)) return 1;
   if (bound_net(ctx, net, who)) return 1;
   if (evaluated_host) *evaluated_host = 0;
   DMN_CHECK(transform_host && extents_host && occ && labels, "%s: NULL argument", who);
@@ -860,13 +880,15 @@ static int mesh_occupancy_edit(dmnerf_ctx* ctx, int net, const double* transform
   if (ctx->mesh_pts.get((size_t)slab * 6, &pts) || ctx->mesh_raw.get((size_t)slab * C, &raw)) return 2;
   float* dirs = pts + slab * 3;                                   // zero view directions, as the sweep
   DMN_CUDA(cudaMemsetAsync(dirs, 0, (size_t)slab * 3 * sizeof(float), st));
+  Deform defs[DMNERF_MAX_MOVES];
+  if (int rc = deformations_from_abi(deformations_host, n_moves, ctx->mesh.knots, defs, nullptr, who, st)) return rc;
   int64_t evaluated = 0;
   // slab by slab, move by move: a point's moves only read its own earlier state, so this is the moves applied in order
   for (int64_t b = 0; b < n; b += slab) {
     const int64_t cnt = n - b < slab ? n - b : slab;
     for (int i = 0; i < n_moves; ++i) {
       int64_t m = 0;
-      int rc = edit_targets(ctx->mesh, transform_host, extents_host, dim, mv[i], b, cnt, pts, &m, st);
+      int rc = edit_targets(ctx->mesh, transform_host, extents_host, dim, mv[i], b, cnt, pts, &m, st, &defs[i]);
       if (!rc && m) rc = launch_mlp_tc(ctx->net[net], nullptr, pts, dirs, nullptr, m, 1, raw, nullptr, st);
       if (!rc) rc = edit_apply(ctx->mesh, transform_host, extents_host, dim, mv[i], b, cnt, raw, C, voxel, level, occ, labels,
                                copies_host && copies_host[i], st);
@@ -901,6 +923,15 @@ DMNERF_API int dmnerf_mesh_occupancy_edit_groups(dmnerf_ctx* ctx, int net, const
                                                  int16_t* labels, int64_t* evaluated_host, void* stream) {
   return mesh_occupancy_edit(ctx, net, transform_host, extents_host, dim, voxel, level, slab, moves_host, copies_host, groups_host,
                              n_moves, occ, labels, evaluated_host, stream, "mesh_occupancy_edit_groups");
+}
+
+DMNERF_API int dmnerf_mesh_occupancy_edit_deformed(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host,
+                                                   int dim, float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host,
+                                                   const int32_t* copies_host, const uint32_t* groups_host,
+                                                   const dmnerf_deformation* deformations_host, int n_moves, float* occ,
+                                                   int16_t* labels, int64_t* evaluated_host, void* stream) {
+  return mesh_occupancy_edit(ctx, net, transform_host, extents_host, dim, voxel, level, slab, moves_host, copies_host, groups_host,
+                             n_moves, occ, labels, evaluated_host, stream, "mesh_occupancy_edit_deformed", deformations_host);
 }
 
 DMNERF_API int dmnerf_mesh_vertex_labels(const float* verts, int64_t n, const float* occ, const int16_t* labels, int dim, float level,
@@ -1013,6 +1044,19 @@ DMNERF_API int dmnerf_move_overlap_groups(dmnerf_ctx* ctx, const float* occ, con
                       n_candidates, obstacles_host, overlap_host, landed_host, (cudaStream_t)stream, "move_overlap_groups");
 }
 
+DMNERF_API int dmnerf_move_overlap_deformed(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                            const double* transform_host, const double* extents_host,
+                                            const dmnerf_edit_move* candidates_host, const int32_t* copies_host,
+                                            const uint32_t* groups_host, const dmnerf_deformation* deformations_host, int n_candidates,
+                                            const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host, void* stream) {
+  const char* who = "move_overlap_deformed";
+  if (deformations_check(deformations_host, n_candidates > 0 && n_candidates <= DMNERF_MAX_CANDIDATES ? n_candidates : 0, who)) return 1;
+  DMN_CHECK(ctx != nullptr, "%s: ctx is NULL", who);
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return move_overlap(ctx->inventory, occ, labels, dim, level, transform_host, extents_host, candidates_host, copies_host, groups_host,
+                      n_candidates, obstacles_host, overlap_host, landed_host, (cudaStream_t)stream, who, deformations_host);
+}
+
 DMNERF_API int dmnerf_object_contacts(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                                       int64_t* faces_host, void* stream) {
   DMN_CHECK(ctx != nullptr, "object_contacts: ctx is NULL");
@@ -1092,6 +1136,19 @@ DMNERF_API int dmnerf_grid_edit_groups(dmnerf_ctx* ctx, const float* src_occ, co
   DMN_CUDA(cudaSetDevice(ctx->device));
   return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, copies_host, groups_host,
                    n_moves, occ, labels, landed_host, overwritten_host, (cudaStream_t)stream, "grid_edit_groups");
+}
+
+DMNERF_API int dmnerf_grid_edit_deformed(dmnerf_ctx* ctx, const float* src_occ, const int16_t* src_labels, int dim, float level,
+                                         const double* transform_host, const double* extents_host, const dmnerf_edit_move* moves_host,
+                                         const int32_t* copies_host, const uint32_t* groups_host,
+                                         const dmnerf_deformation* deformations_host, int n_moves, float* occ, int16_t* labels,
+                                         int64_t* landed_host, int64_t* overwritten_host, void* stream) {
+  const char* who = "grid_edit_deformed";
+  if (deformations_check(deformations_host, n_moves > 0 && n_moves <= DMNERF_MAX_MOVES ? n_moves : 0, who)) return 1;
+  DMN_CHECK(ctx != nullptr, "%s: ctx is NULL", who);
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return grid_edit(ctx->inventory, src_occ, src_labels, dim, level, transform_host, extents_host, moves_host, copies_host, groups_host,
+                   n_moves, occ, labels, landed_host, overwritten_host, (cudaStream_t)stream, who, deformations_host);
 }
 
 DMNERF_API int dmnerf_placement_maps_in_scene(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* scene_occ,

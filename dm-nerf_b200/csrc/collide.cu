@@ -65,12 +65,14 @@ __global__ void grid_check_kernel(const float* __restrict__ occ, const int16_t* 
 }
 
 // COPY (DESIGN.md, "Copying objects"): every candidate of the launch is a copy, which vacates nothing, so its own label's solid
-// points are obstacles like any other.
-template <bool COPY>
+// points are obstacles like any other.  DEFORM (DESIGN.md, "Deforming objects"): the candidates' targets are pulled through their
+// deformations defs [n] (one per candidate row; n_knots 0: rigid).
+template <bool COPY, bool DEFORM>
 __global__ void __launch_bounds__(OV_THREADS) move_overlap_kernel(const GridXform g, const IndexMap map, const float* __restrict__ occ,
                                                                   const int16_t* __restrict__ labels, float level, ObjMask obstacles,
                                                                   const Candidate* __restrict__ cands, const Run* __restrict__ runs,
-                                                                  int n_runs, unsigned long long* __restrict__ counts) {
+                                                                  int n_runs, unsigned long long* __restrict__ counts,
+                                                                  const Deform* __restrict__ defs) {
   __shared__ Candidate sc[RUN];
   __shared__ uint32_t hist[RUN][N_COUNTERS];
   __shared__ int s_run;
@@ -121,7 +123,12 @@ __global__ void __launch_bounds__(OV_THREADS) move_overlap_kernel(const GridXfor
       float t[3];
       if (src) {
         double q[3];
-        src = edit_target(m.trans, map.inv, map.b, m.lo, m.hi, true, p, t, q);
+        if (DEFORM && defs[run.first + c].n_knots) {
+          src = true;
+          edit_target_deformed(m.trans, defs[run.first + c], map.inv, map.b, m.lo, m.hi, src, p, t, q);
+        } else {
+          src = edit_target(m.trans, map.inv, map.b, m.lo, m.hi, true, p, t, q);
+        }
         if (src) {
           const int64_t qi = ((int64_t)q[0] * d + (int64_t)q[1]) * d + (int64_t)q[2];
           const int lq = labels[qi];
@@ -147,12 +154,13 @@ __global__ void __launch_bounds__(OV_THREADS) move_overlap_kernel(const GridXfor
 // source grid at the target's nearest index q.  counts [129]: overwritten per label, then landed -- the takes whose target is
 // solid, and those of them that land on a solid state point the move does not vacate, by its label.  The state point is read
 // before it is written and no thread reads another's point, so the launch order of the points does not matter.  A COPY takes and
-// never vacates, so every solid state point it lands on counts, its own label's included.
-template <bool COPY>
+// never vacates, so every solid state point it lands on counts, its own label's included.  DEFORM: the target is pulled through
+// the deformation df (edit_target_deformed).
+template <bool COPY, bool DEFORM>
 __global__ void __launch_bounds__(GE_THREADS) grid_edit_kernel(const GridXform g, const EditMove e, const float* __restrict__ src_occ,
                                                                const int16_t* __restrict__ src_labels, float level,
                                                                float* __restrict__ occ, int16_t* __restrict__ labels,
-                                                               unsigned long long* __restrict__ counts) {
+                                                               unsigned long long* __restrict__ counts, const Deform df) {
   __shared__ uint32_t hist[N_COUNTERS];
   for (int k = threadIdx.x; k < N_COUNTERS; k += GE_THREADS) hist[k] = 0;
   __syncthreads();
@@ -164,7 +172,11 @@ __global__ void __launch_bounds__(GE_THREADS) grid_edit_kernel(const GridXform g
     float x[3], t[3];
     double q[3];
     sweep_point(g, p, x);
-    const bool in_box = edit_target(e.trans, e.inv, e.b, e.lo, e.hi, !e.empty, x, t, q);
+    bool in_box = !e.empty;
+    if (DEFORM)
+      edit_target_deformed(e.trans, df, e.inv, e.b, e.lo, e.hi, in_box, x, t, q);
+    else
+      in_box = edit_target(e.trans, e.inv, e.b, e.lo, e.hi, in_box, x, t, q);
     auto here = [&](int lp) { return e.piece.bits == nullptr || !region_drops(e.piece, lp, x[0], x[1], x[2]); };
     edit_rule<COPY>(
         e, in_box,
@@ -247,10 +259,27 @@ void grid_forward(const double* T, const double* ext, int dim, double A[9]) {
     for (int c = 0; c < 3; ++c) A[3 * r + c] = SR[r][c] * (ext[c] / (double)(dim - 1));
 }
 
+// The forward image D(s) of a network-frame point s under the deformation d (DESIGN.md, "Deforming objects"), its frame
+// coordinates given: (u, v) -> A(h) (u, v) + t(h), h kept, the table clamped to the end knots.
+static void deform_forward(const dmnerf_deformation& d, double u, double v, double h, double out[3]) {
+  const int K = d.n_knots;
+  const double r = (h - d.h0) / d.dh;
+  const double kf = std::fmin(std::fmax(std::floor(r), 0.0), (double)(K - 2));
+  const double s = std::fmin(std::fmax(r - kf, 0.0), 1.0);
+  const double* k0 = d.knots + 6 * (int)kf;
+  double a[6];
+  for (int j = 0; j < 6; ++j) a[j] = k0[j] + s * (k0[6 + j] - k0[j]);
+  const double uu = a[0] * u + a[1] * v + a[4], vv = a[2] * u + a[3] * v + a[5];
+  for (int c = 0; c < 3; ++c) out[c] = d.frame[9 + c] + uu * d.frame[c] + vv * d.frame[3 + c] + h * d.frame[6 + c];
+}
+
 // The destination box of a move with source box B (DESIGN.md, "Collision checks", destination culling): B grown by half a voxel,
 // its 8 corners mapped by idx_p = inv (M^-1 (A u + b - m) - b), floor / ceil, one voxel of margin, clipped to the grid.  A
-// non-finite corner (a nearly degenerate move) keeps the whole grid.
-void destination_box(const EditMove& e, const double A[9], int dim, int dlo[3], int dhi[3]) {
+// non-finite corner (a nearly degenerate move) keeps the whole grid.  A deformed move (def, n_knots > 0; DESIGN.md, "Deforming
+// objects") maps D(B) instead: B bounded in frame coordinates as [u] x [v] x [h], and the images of that box's 4 horizontal
+// corners at its two heights and at every knot height between them, which hold D(B) because D is affine in (u, v) and, within a
+// knot interval, in h.
+void destination_box(const EditMove& e, const double A[9], int dim, const dmnerf_deformation* def, int dlo[3], int dhi[3]) {
   const double* t = e.trans;
   const double M[3][3] = {{t[0], t[1], t[2]}, {t[4], t[5], t[6]}, {t[8], t[9], t[10]}};
   double Mi[3][3];
@@ -262,16 +291,47 @@ void destination_box(const EditMove& e, const double A[9], int dim, int dlo[3], 
   const double det = M[0][0] * Mi[0][0] + M[0][1] * Mi[1][0] + M[0][2] * Mi[2][0];
   double lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
   bool finite = true;
-  for (int c = 0; c < 8; ++c) {
-    double u[3], x[3], y[3];
-    for (int a = 0; a < 3; ++a) u[a] = (c >> a) & 1 ? e.hi[a] + 0.5 : e.lo[a] - 0.5;
-    for (int r = 0; r < 3; ++r) x[r] = A[3 * r] * u[0] + A[3 * r + 1] * u[1] + A[3 * r + 2] * u[2] + e.b[r] - t[4 * r + 3];
+  auto add = [&](const double s[3]) {                            // a source point s of the network frame
+    double x[3], y[3];
+    for (int r = 0; r < 3; ++r) x[r] = s[r] - t[4 * r + 3];
     for (int r = 0; r < 3; ++r) y[r] = (Mi[r][0] * x[0] + Mi[r][1] * x[1] + Mi[r][2] * x[2]) / det - e.b[r];
     for (int a = 0; a < 3; ++a) {
       const double v = e.inv[3 * a] * y[0] + e.inv[3 * a + 1] * y[1] + e.inv[3 * a + 2] * y[2];
       finite = finite && std::isfinite(v);
       lo[a] = v < lo[a] ? v : lo[a];
       hi[a] = v > hi[a] ? v : hi[a];
+    }
+  };
+  const bool deformed = def && def->n_knots;
+  double flo[3] = {INFINITY, INFINITY, INFINITY}, fhi[3] = {-INFINITY, -INFINITY, -INFINITY};   // B in frame coordinates
+  for (int c = 0; c < 8; ++c) {
+    double u[3], s[3];
+    for (int a = 0; a < 3; ++a) u[a] = (c >> a) & 1 ? e.hi[a] + 0.5 : e.lo[a] - 0.5;
+    for (int r = 0; r < 3; ++r) s[r] = A[3 * r] * u[0] + A[3 * r + 1] * u[1] + A[3 * r + 2] * u[2] + e.b[r];
+    if (!deformed) {
+      add(s);
+      continue;
+    }
+    for (int a = 0; a < 3; ++a) {
+      const double* ax = def->frame + 3 * a;
+      const double f = ax[0] * (s[0] - def->frame[9]) + ax[1] * (s[1] - def->frame[10]) + ax[2] * (s[2] - def->frame[11]);
+      flo[a] = f < flo[a] ? f : flo[a];
+      fhi[a] = f > fhi[a] ? f : fhi[a];
+    }
+  }
+  if (deformed) {
+    auto level = [&](double h) {
+      for (int c = 0; c < 4; ++c) {
+        double s[3];
+        deform_forward(*def, c & 1 ? fhi[0] : flo[0], c & 2 ? fhi[1] : flo[1], h, s);
+        add(s);
+      }
+    };
+    level(flo[2]);
+    level(fhi[2]);
+    for (int k = 0; k < def->n_knots; ++k) {
+      const double h = def->h0 + k * def->dh;
+      if (h > flo[2] && h < fhi[2]) level(h);
     }
   }
   for (int a = 0; a < 3; ++a) {
@@ -301,7 +361,9 @@ int read_checked(const void* dev, void* host, size_t bytes, int max_label, const
 
 int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
                  const dmnerf_edit_move* cands_host, const int32_t* copies_host, const uint32_t* groups_host, int n,
-                 const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host, cudaStream_t st, const char* who) {
+                 const uint32_t* obstacles_host, int64_t* overlap_host, int64_t* landed_host, cudaStream_t st, const char* who,
+                 const dmnerf_deformation* deformations_host) {
+  if (deformations_check(deformations_host, n > 0 ? n : 0, who)) return 1;
   DMN_CHECK(occ && labels && T16 && ext3 && overlap_host && landed_host, "%s: NULL argument", who);
   if (sweep_grid_check(T16, ext3, dim, level, who)) return 1;
   DMN_CHECK(n >= 1 && n <= DMNERF_MAX_CANDIDATES, "%s: between 1 and %d candidates are supported, got %d", who,
@@ -335,7 +397,7 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
     if (e.empty) {
       for (int a = 0; a < 3; ++a) { c.dlo[a] = 1; c.dhi[a] = 0; }
     } else {
-      destination_box(e, A, dim, c.dlo, c.dhi);
+      destination_box(e, A, dim, deformations_host ? deformations_host + i : nullptr, c.dlo, c.dhi);
     }
     c.piece = e.piece;
     c.group = e.group;
@@ -380,11 +442,23 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
   }
   const size_t count_bytes = (size_t)n * N_COUNTERS * sizeof(unsigned long long), out_bytes = 16 + count_bytes;
   const size_t cand_bytes = (size_t)n * sizeof(Candidate), run_bytes = runs.size() * sizeof(Run);
+  // the deformations in candidate rows, after the runs (none: no bytes)
+  std::vector<Deform> defs(n), def_rows;
+  bool deformed = false;
+  if (deformations_from_abi(deformations_host, n, s.knots, defs.data(), &deformed, who, st)) return 1;
+  if (deformed) {
+    def_rows.resize(n);
+    for (int i = 0; i < n; ++i) def_rows[slot[i]] = defs[i];
+  }
+  const size_t def_bytes = def_rows.size() * sizeof(Deform);
   char *out, *in_d;
-  if (s.out.get(out_bytes, &out) || s.in.get(cand_bytes + run_bytes, &in_d)) return 2;
-  std::vector<char> in(cand_bytes + run_bytes);
+  if (s.out.get(out_bytes, &out) || s.in.get(cand_bytes + run_bytes + def_bytes + 16, &in_d)) return 2;
+  const size_t def_at = (cand_bytes + run_bytes + 15) / 16 * 16;
+  std::vector<char> in(def_at + def_bytes);
   memcpy(in.data(), cand.data(), cand_bytes);
   if (run_bytes) memcpy(in.data() + cand_bytes, runs.data(), run_bytes);
+  if (def_bytes) memcpy(in.data() + def_at, def_rows.data(), def_bytes);
+  const Deform* defs_d = deformed ? reinterpret_cast<const Deform*>(in_d + def_at) : nullptr;
   DMN_CUDA(cudaMemsetAsync(out, 0, out_bytes, st));
   DMN_CUDA(cudaMemcpyAsync(in_d, in.data(), in.size(), cudaMemcpyHostToDevice, st));
   int* bad = reinterpret_cast<int*>(out);
@@ -397,12 +471,19 @@ int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int
     if (!blocks_of[kind]) continue;
     const Run* runs_d = reinterpret_cast<const Run*>(in_d + cand_bytes) + first_run[kind];
     const int n_runs = (int)(first_run[kind + 1] - first_run[kind]);
-    if (kind)
-      move_overlap_kernel<true><<<(unsigned)blocks_of[kind], OV_THREADS, 0, st>>>(g, map, occ, labels, level, obst, cands_d, runs_d,
-                                                                                  n_runs, counts);
+    const unsigned nb = (unsigned)blocks_of[kind];
+    if (kind && deformed)
+      move_overlap_kernel<true, true><<<nb, OV_THREADS, 0, st>>>(g, map, occ, labels, level, obst, cands_d, runs_d, n_runs, counts,
+                                                                 defs_d);
+    else if (kind)
+      move_overlap_kernel<true, false><<<nb, OV_THREADS, 0, st>>>(g, map, occ, labels, level, obst, cands_d, runs_d, n_runs, counts,
+                                                                  nullptr);
+    else if (deformed)
+      move_overlap_kernel<false, true><<<nb, OV_THREADS, 0, st>>>(g, map, occ, labels, level, obst, cands_d, runs_d, n_runs, counts,
+                                                                  defs_d);
     else
-      move_overlap_kernel<false><<<(unsigned)blocks_of[kind], OV_THREADS, 0, st>>>(g, map, occ, labels, level, obst, cands_d, runs_d,
-                                                                                   n_runs, counts);
+      move_overlap_kernel<false, false><<<nb, OV_THREADS, 0, st>>>(g, map, occ, labels, level, obst, cands_d, runs_d, n_runs, counts,
+                                                                   nullptr);
     DMN_LAUNCH_OK();
   }
   std::vector<char> h(out_bytes);
@@ -441,7 +522,9 @@ int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, 
 
 int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels, int dim, float level, const double* T16,
               const double* ext3, const dmnerf_edit_move* moves_host, const int32_t* copies_host, const uint32_t* groups_host, int n,
-              float* occ, int16_t* labels, int64_t* landed_host, int64_t* overwritten_host, cudaStream_t st, const char* who) {
+              float* occ, int16_t* labels, int64_t* landed_host, int64_t* overwritten_host, cudaStream_t st, const char* who,
+              const dmnerf_deformation* deformations_host) {
+  if (deformations_check(deformations_host, n > 0 ? n : 0, who)) return 1;
   DMN_CHECK(src_occ && src_labels && occ && labels && T16 && ext3 && landed_host && overwritten_host, "%s: NULL argument", who);
   DMN_CHECK(n >= 1 && n <= DMNERF_MAX_MOVES, "%s: between 1 and %d moves are supported, got %d", who, DMNERF_MAX_MOVES, n);
   DMN_CHECK(moves_host, "%s: moves is NULL", who);
@@ -461,6 +544,8 @@ int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels
     if (edit_move_from_abi(moves_host[i], T16, ext3, dim, DMNERF_MAX_INS, mv[i], who, i, groups_host ? groups_host + 4 * i : nullptr))
       return 1;
   if (copy_flags_check(moves_host, copies_host, groups_host, n, true, who)) return 1;
+  std::vector<Deform> defs(n);
+  if (deformations_from_abi(deformations_host, n, s.knots, defs.data(), nullptr, who, st)) return 1;
   const size_t out_bytes = 16 + (size_t)n * N_COUNTERS * sizeof(unsigned long long);
   char* out;
   if (s.out.get(out_bytes, &out)) return 2;
@@ -476,10 +561,16 @@ int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels
   const unsigned ge_blocks = (unsigned)((npts + GE_THREADS - 1) / GE_THREADS);
   for (int i = 0; i < n; ++i) {
     unsigned long long* row = counts + (size_t)i * N_COUNTERS;
-    if (copies_host && copies_host[i])
-      grid_edit_kernel<true><<<ge_blocks, GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ, labels, row);
+    const bool copy = copies_host && copies_host[i], deformed = defs[i].n_knots != 0;
+    if (copy && deformed)
+      grid_edit_kernel<true, true><<<ge_blocks, GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ, labels, row, defs[i]);
+    else if (copy)
+      grid_edit_kernel<true, false><<<ge_blocks, GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ, labels, row, defs[i]);
+    else if (deformed)
+      grid_edit_kernel<false, true><<<ge_blocks, GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ, labels, row, defs[i]);
     else
-      grid_edit_kernel<false><<<ge_blocks, GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ, labels, row);
+      grid_edit_kernel<false, false><<<ge_blocks, GE_THREADS, 0, st>>>(g, mv[i], src_occ, src_labels, level, occ, labels, row,
+                                                                       defs[i]);
     DMN_LAUNCH_OK();
   }
   if (const int rc = read_back(out, h, DMNERF_MAX_INS, who, st)) return rc;

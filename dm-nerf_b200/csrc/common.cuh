@@ -275,6 +275,7 @@ int launch_hungarian_costs_merged(const double* partials, int world, int64_t n, 
 struct MeshState {
   DeviceBuffer eflags, cases, vcnt, vscan, tcnt, tscan, temp, totals, keys_in, keys_out, vals_in, vals_out, parent, size;
   DeviceBuffer edit_t, edit_flag, edit_pos;   // the edited sweep's slab: target points, in-box flags and their scan
+  DeviceBuffer knots;                         // the deformations' knot tables of the call
   const float* grid = nullptr;
   int nx = 0, ny = 0, nz = 0;
   float level = 0.f;
@@ -307,6 +308,21 @@ struct EditMove {
   ObjMask group;
   int32_t label, rest_drop, empty;   // empty: the box holds no point, nothing is evaluated
 };
+// A checked deformation of a move (DESIGN.md, "Deforming objects"): frame rows e_u, e_v, e_h, c, the knot heights h0 + k dh and
+// the DEVICE knot table [n_knots][6] (A row-major, then t).  n_knots == 0: the move is rigid.
+struct Deform {
+  double frame[12];
+  double h0, dh;
+  const double* knots;
+  int32_t n_knots;
+};
+// The deformations of n moves (deformations_host NULL: every move rigid), checked (n_knots, knots, finite values, dh, the frame
+// and det A(h) > 0 on every knot interval), their knot tables copied once into `knots` and out[i] pointing into it.  Returns
+// whether any move is deformed in *any (may be NULL).
+int deformations_from_abi(const dmnerf_deformation* deformations_host, int n, DeviceBuffer& knots, Deform* out, bool* any,
+                          const char* who, cudaStream_t st);
+// The same checks alone (no device work): what every deformed entry point runs first.
+int deformations_check(const dmnerf_deformation* deformations_host, int n, const char* who);
 // The grid and level of an edit or a collision check: dim in [2, 2048], level in (0, 1), a scene transform with det > 0 and
 // finite extents > 0.
 int sweep_grid_check(const double* T16, const double* ext3, int dim, float level, const char* who);
@@ -325,7 +341,7 @@ int copy_flags_check(const dmnerf_edit_move* moves, const int32_t* copies, const
 // Points [begin, begin + count) of the grid: their targets under m, the boxed ones compacted in order into pts [*n_eval, 3];
 // *n_eval read back (synchronises).
 int edit_targets(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
-                 float* pts, int64_t* n_eval, cudaStream_t st);
+                 float* pts, int64_t* n_eval, cudaStream_t st, const Deform* d = nullptr);
 // take / vacate of m on the same points, raw [n_eval, c]: the network at the compacted targets of the last edit_targets; a copy
 // takes only
 int edit_apply(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
@@ -339,7 +355,7 @@ int piece_region(const dmnerf_region& d, int mv, Region& r, const char* who, int
 // pass and move: the targets and view directions of every sample, the in-box flags and their scan, the boxed targets compacted,
 // the network's rows at them and the count read back.
 struct MovesState {
-  DeviceBuffer tgt, flag, pin, pos, temp, pts, raw, total;
+  DeviceBuffer tgt, flag, pin, pos, temp, pts, raw, total, knots;
 };
 struct Network;
 // The moves applied in order, in place, to the raw rows raw [n * s, c] of one pass of a stage render (samples o + d z, z [n, s]),
@@ -347,12 +363,12 @@ struct Network;
 // the count per move (synchronises).
 int render_moves_pass(MovesState& s, const Network& net, bool f16, const EditMove* moves, const int32_t* copies, int n_moves,
                       const float* rays_o, const float* rays_d, const float* z, int64_t n, int s_per_ray, int c, float voxel,
-                      float level, float* raw, int64_t* evaluated, cudaStream_t st);
+                      float level, float* raw, int64_t* evaluated, cudaStream_t st, const Deform* deforms = nullptr);
 
 // Object inventory (inventory.cu): per-group integer statistics and fp64 spans of the solid points of a labelled grid.
 // Per-context device buffers: everything a call reads back (status word first), and its inputs.
 struct InventoryState {
-  DeviceBuffer out, in;
+  DeviceBuffer out, in, knots;   // knots: the deformations' knot tables of a collision check or grid-only edit
 };
 int object_voxels(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels,
                   const int32_t* boxes_host, int64_t* moments_host, uint32_t* hist_host, cudaStream_t st);
@@ -365,7 +381,8 @@ int object_spans(InventoryState& s, const float* occ, const int16_t* labels, int
 int move_overlap(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
                  const dmnerf_edit_move* cands_host, const int32_t* copies_host, const uint32_t* groups_host, int n,
                  const uint32_t* obstacles_host,
-                 int64_t* overlap_host, int64_t* landed_host, cudaStream_t st, const char* who = "move_overlap");
+                 int64_t* overlap_host, int64_t* landed_host, cudaStream_t st, const char* who = "move_overlap",
+                 const dmnerf_deformation* deformations_host = nullptr);
 int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, int dim, float level, int n_labels, int64_t* faces_host,
                     cudaStream_t st);
 // The grid-only edit (DESIGN.md, "Arranging objects"): the moves applied in order to the state occ / labels, each target read
@@ -375,7 +392,8 @@ int object_contacts(InventoryState& s, const float* occ, const int16_t* labels, 
 int grid_edit(InventoryState& s, const float* src_occ, const int16_t* src_labels, int dim, float level, const double* T16,
               const double* ext3, const dmnerf_edit_move* moves_host, const int32_t* copies_host, const uint32_t* groups_host, int n,
               float* occ, int16_t* labels,
-              int64_t* landed_host, int64_t* overwritten_host, cudaStream_t st, const char* who = "grid_edit");
+              int64_t* landed_host, int64_t* overwritten_host, cudaStream_t st, const char* who = "grid_edit",
+              const dmnerf_deformation* deformations_host = nullptr);
 // The grid check of both: flags in *bad (device) for NaN in occ and labels outside [0, n_labels - 1].  read_checked copies
 // `bytes` from dev to host and synchronises; the buffer starts with that flag word, and a set flag fails the call.
 int launch_grid_check(const float* occ, const int16_t* labels, int64_t n, int n_labels, int* bad, cudaStream_t st);

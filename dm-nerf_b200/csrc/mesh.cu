@@ -4,6 +4,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <vector>
 
 #include <cub/cub.cuh>
 
@@ -719,16 +720,94 @@ int copy_flags_check(const dmnerf_edit_move* moves, const int32_t* copies, const
   return 0;
 }
 
-// One thread per grid point of the slab: its target t (edit_target) and whether the nearest grid index of t lies in the box.
+int deformations_check(const dmnerf_deformation* defs, int n, const char* who) {
+  if (!defs) return 0;
+  for (int i = 0; i < n; ++i) {
+    const dmnerf_deformation& d = defs[i];
+    const int K = d.n_knots;
+    if (K == 0) continue;
+    DMN_CHECK(K >= 2 && K <= 64, "%s: move %d: deformation: n_knots %d is not 0 and outside [2, 64]", who, i, K);
+    DMN_CHECK(d.knots != nullptr, "%s: move %d: deformation: the knot table is NULL", who, i);
+    bool finite = std::isfinite(d.h0) && std::isfinite(d.dh);
+    for (int k = 0; k < 12; ++k) finite = finite && std::isfinite(d.frame[k]);
+    for (int k = 0; k < 6 * K; ++k) finite = finite && std::isfinite(d.knots[k]);
+    DMN_CHECK(finite, "%s: move %d: deformation: a value is not finite", who, i);
+    DMN_CHECK(d.dh > 0.0, "%s: move %d: deformation: dh %g must be > 0", who, i, d.dh);
+    const double* e = d.frame;
+    bool ortho = true;
+    for (int a = 0; a < 3; ++a)
+      for (int b = 0; b < 3; ++b) {
+        const double dot = (e[3 * a] * e[3 * b] + e[3 * a + 1] * e[3 * b + 1]) + e[3 * a + 2] * e[3 * b + 2];
+        ortho = ortho && std::fabs(dot - (a == b ? 1.0 : 0.0)) <= 1e-9;
+      }
+    for (int a = 0; a < 3; ++a) {                                 // e_u x e_v = e_h
+      const int a1 = (a + 1) % 3, a2 = (a + 2) % 3;
+      ortho = ortho && std::fabs((e[a1] * e[3 + a2] - e[a2] * e[3 + a1]) - e[6 + a]) <= 1e-9;
+    }
+    DMN_CHECK(ortho, "%s: move %d: deformation: the frame is not orthonormal and right-handed", who, i);
+    // det A(s) on interval k, A = A_k + s D: d0 + s b1 + s^2 a2, a quadratic in s whose minimum on [0, 1] must be > 0
+    for (int k = 0; k + 1 < K; ++k) {
+      const double* A = d.knots + 6 * k;
+      const double* B = A + 6;
+      const double D[4] = {B[0] - A[0], B[1] - A[1], B[2] - A[2], B[3] - A[3]};
+      const double d0 = A[0] * A[3] - A[1] * A[2], a2 = D[0] * D[3] - D[1] * D[2];
+      const double b1 = ((A[0] * D[3] + D[0] * A[3]) - A[1] * D[2]) - D[1] * A[2];
+      double lo = std::fmin(d0, (d0 + b1) + a2);
+      if (a2 > 0.0) {
+        const double s = -b1 / (2.0 * a2);
+        if (s > 0.0 && s < 1.0) lo = std::fmin(lo, d0 - (b1 * b1) / (4.0 * a2));
+      }
+      DMN_CHECK(lo > 0.0, "%s: move %d: deformation: det A(h) <= 0 on knot interval %d", who, i, k);
+    }
+  }
+  return 0;
+}
+
+int deformations_from_abi(const dmnerf_deformation* defs, int n, DeviceBuffer& knots, Deform* out, bool* any, const char* who,
+                          cudaStream_t st) {
+  if (any) *any = false;
+  memset(out, 0, sizeof(Deform) * (size_t)n);
+  if (deformations_check(defs, n, who)) return 1;
+  if (!defs) return 0;
+  size_t total = 0;
+  for (int i = 0; i < n; ++i) total += 6 * (size_t)defs[i].n_knots;
+  if (!total) return 0;
+  std::vector<double> h(total);
+  double* dev;
+  if (knots.get(total, &dev)) return 2;
+  for (int i = 0, at = 0; i < n; ++i) {
+    const dmnerf_deformation& d = defs[i];
+    if (!d.n_knots) continue;
+    memcpy(out[i].frame, d.frame, sizeof(out[i].frame));
+    out[i].h0 = d.h0;
+    out[i].dh = d.dh;
+    out[i].n_knots = d.n_knots;
+    out[i].knots = dev + at;
+    memcpy(h.data() + at, d.knots, 6 * sizeof(double) * d.n_knots);
+    at += 6 * d.n_knots;
+  }
+  DMN_CUDA(cudaMemcpyAsync(dev, h.data(), total * sizeof(double), cudaMemcpyHostToDevice, st));
+  DMN_CUDA(cudaStreamSynchronize(st));                           // h is freed on return
+  if (any) *any = true;
+  return 0;
+}
+
+// One thread per grid point of the slab: its target t (edit_target; edit_target_deformed when DEFORM) and whether the nearest
+// grid index of t lies in the box.
+template <bool DEFORM>
 __global__ void edit_target_kernel(const GridXform g, const EditMove m, int64_t begin, int64_t count, float* __restrict__ tgt,
-                                   int32_t* __restrict__ flag) {
+                                   int32_t* __restrict__ flag, const Deform d) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
   float p[3];
   sweep_point(g, begin + i, p);
   float t[3];
   double q[3];
-  const bool in = edit_target(m.trans, m.inv, m.b, m.lo, m.hi, !m.empty, p, t, q);
+  bool in = !m.empty;
+  if (DEFORM)
+    edit_target_deformed(m.trans, d, m.inv, m.b, m.lo, m.hi, in, p, t, q);
+  else
+    in = edit_target(m.trans, m.inv, m.b, m.lo, m.hi, in, p, t, q);
   tgt[3 * i] = t[0];
   tgt[3 * i + 1] = t[1];
   tgt[3 * i + 2] = t[2];
@@ -782,7 +861,7 @@ __global__ void edit_apply_kernel(const GridXform g, const EditMove m, int64_t b
 }
 
 int edit_targets(MeshState& s, const double* T16, const double* ext3, int dim, const EditMove& m, int64_t begin, int64_t count,
-                 float* pts, int64_t* n_eval, cudaStream_t st) {
+                 float* pts, int64_t* n_eval, cudaStream_t st, const Deform* d) {
   *n_eval = 0;
   DMN_CHECK(count >= 1 && count < INT32_MAX, "edit_targets: slab of %lld points outside [1, 2^31)", (long long)count);
   float* tgt;
@@ -792,7 +871,10 @@ int edit_targets(MeshState& s, const double* T16, const double* ext3, int dim, c
       s.totals.get(4, &tot))
     return 2;
   const GridXform g = make_xform(T16, ext3, dim);
-  edit_target_kernel<<<blocks(count, 256), 256, 0, st>>>(g, m, begin, count, tgt, flag);
+  if (d && d->n_knots)
+    edit_target_kernel<true><<<blocks(count, 256), 256, 0, st>>>(g, m, begin, count, tgt, flag, *d);
+  else
+    edit_target_kernel<false><<<blocks(count, 256), 256, 0, st>>>(g, m, begin, count, tgt, flag, Deform{});
   DMN_LAUNCH_OK();
   if (exclusive_sum(s, flag, pos, count, st)) return 2;
   edit_count_kernel<<<1, 1, 0, st>>>(flag, pos, count, tot);

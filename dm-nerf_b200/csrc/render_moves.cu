@@ -18,10 +18,13 @@ static inline unsigned blocks(int64_t n, int t) { return (unsigned)((n + t - 1) 
 // One thread per sample i of the pass (ray i / s): p as the network prologue computes it; its target t and whether t's nearest grid
 // index is in the box (flag); whether p's own nearest index is (pin: edit_target under the identity, which gives t = p exactly); the
 // target's view direction trans[:3, :3] d (fp64, one rounding per operation, rounded once to fp32) normalised by the prologue's
-// own fp32 expression, since points mode embeds view directions as given.  tgt [ns, 6] = (t, direction).
+// own fp32 expression, since points mode embeds view directions as given.  tgt [ns, 6] = (t, direction).  DEFORM (DESIGN.md,
+// "Deforming objects"): t is pulled through the deformation d and the direction is the pulled-back tangent J_D^-1 trans[:3, :3] d
+// (fp64, rounded once to fp32), normalised by the same expression.
+template <bool DEFORM>
 __global__ void move_target_kernel(const EditMove m, const float* __restrict__ rays_o, const float* __restrict__ rays_d,
                                    const float* __restrict__ z, int64_t ns, int s, float* __restrict__ tgt, int32_t* __restrict__ flag,
-                                   uint8_t* __restrict__ pin) {
+                                   uint8_t* __restrict__ pin, const Deform dm) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= ns) return;
   const int64_t ray = i / s;
@@ -31,15 +34,32 @@ __global__ void move_target_kernel(const EditMove m, const float* __restrict__ r
   ray_point(o, d, z[i], p);
   float t[3];
   double q[3];
-  const bool in = edit_target(m.trans, m.inv, m.b, m.lo, m.hi, !m.empty, p, t, q);
+  bool in = !m.empty;
+  Pulled P;
+  if (DEFORM)
+    P = edit_target_deformed(m.trans, dm, m.inv, m.b, m.lo, m.hi, in, p, t, q);
+  else
+    in = edit_target(m.trans, m.inv, m.b, m.lo, m.hi, in, p, t, q);
   const double identity[12] = {1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0};
   float pp[3];
   const bool p_in = edit_target(identity, m.inv, m.b, m.lo, m.hi, !m.empty, p, pp, q);
   float dt[3];
+  if (DEFORM) {
+    double w[3], x[3];
 #pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const double* r = m.trans + 4 * a;
-    dt[a] = __double2float_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)d[0]), __dmul_rn(r[1], (double)d[1])), __dmul_rn(r[2], (double)d[2])));
+    for (int a = 0; a < 3; ++a) {
+      const double* r = m.trans + 4 * a;
+      w[a] = __dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)d[0]), __dmul_rn(r[1], (double)d[1])), __dmul_rn(r[2], (double)d[2]));
+    }
+    deform_direction(dm, P, w, x);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) dt[a] = __double2float_rn(x[a]);
+  } else {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const double* r = m.trans + 4 * a;
+      dt[a] = __double2float_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)d[0]), __dmul_rn(r[1], (double)d[1])), __dmul_rn(r[2], (double)d[2])));
+    }
   }
   const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dt[0], dt[0]), __fmul_rn(dt[1], dt[1])), __fmul_rn(dt[2], dt[2])));
   float* out = tgt + 6 * i;
@@ -106,7 +126,7 @@ __global__ void move_apply_kernel(const EditMove m, const float* __restrict__ ra
 
 int render_moves_pass(MovesState& s, const Network& net, bool f16, const EditMove* moves, const int32_t* copies, int n_moves,
                       const float* rays_o, const float* rays_d, const float* z, int64_t n, int s_per_ray, int c, float voxel,
-                      float level, float* raw, int64_t* evaluated, cudaStream_t st) {
+                      float level, float* raw, int64_t* evaluated, cudaStream_t st, const Deform* deforms) {
   const int64_t ns = n * s_per_ray;
   if (ns == 0) return 0;
   DMN_CHECK(ns < INT32_MAX, "render_moved: %lld samples in one pass exceed the 32-bit scan", (long long)ns);
@@ -124,7 +144,10 @@ int render_moves_pass(MovesState& s, const Network& net, bool f16, const EditMov
   if (s.temp.get(temp_bytes, &temp)) return 2;
   for (int i = 0; i < n_moves; ++i) {
     const EditMove& m = moves[i];
-    move_target_kernel<<<blocks(ns, 256), 256, 0, st>>>(m, rays_o, rays_d, z, ns, s_per_ray, tgt, flag, pin);
+    if (deforms && deforms[i].n_knots)
+      move_target_kernel<true><<<blocks(ns, 256), 256, 0, st>>>(m, rays_o, rays_d, z, ns, s_per_ray, tgt, flag, pin, deforms[i]);
+    else
+      move_target_kernel<false><<<blocks(ns, 256), 256, 0, st>>>(m, rays_o, rays_d, z, ns, s_per_ray, tgt, flag, pin, Deform{});
     DMN_LAUNCH_OK();
     DMN_CUDA(cub::DeviceScan::ExclusiveSum(temp, temp_bytes, flag, pos, (int)ns, st));
     move_count_kernel<<<1, 1, 0, st>>>(flag, pos, ns, tot);

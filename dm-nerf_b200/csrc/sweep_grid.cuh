@@ -50,17 +50,9 @@ __device__ __forceinline__ void sweep_point(const GridXform& g, int64_t p, float
 // q = rint(inv (t - b)) of t (fp64, half to even; inv and b: the grid's index map), and whether q lies in the inclusive box
 // [lo, hi] (`in` false: never).  An fp32 sweep point maps to its own index, also on the grid's faces.  Every operation is rounded
 // once (no contraction), so that a numpy restatement takes the same decisions.
-__device__ __forceinline__ bool edit_target(const double* trans, const double* inv, const double* b, const double* lo,
-                                            const double* hi, bool in, const float p[3], float t[3], double q[3]) {
-  double dt[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const double* r = trans + 4 * a;
-    const double v = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)p[0]), __dmul_rn(r[1], (double)p[1])),
-                                         __dmul_rn(r[2], (double)p[2])), r[3]);
-    t[a] = __double2float_rn(v);
-    dt[a] = __dsub_rn((double)t[a], b[a]);
-  }
+// q = rint(inv dt) and the box test of edit_target, dt = t - b
+__device__ __forceinline__ bool index_in_box(const double* inv, const double* lo, const double* hi, bool in, const double dt[3],
+                                             double q[3]) {
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
     const double* row = inv + 3 * a;
@@ -69,6 +61,112 @@ __device__ __forceinline__ bool edit_target(const double* trans, const double* i
     in = in && q[a] >= lo[a] && q[a] <= hi[a];
   }
   return in;
+}
+
+// y = trans p in fp64, not rounded
+__device__ __forceinline__ double moved_coord(const double* trans, int a, const float p[3]) {
+  const double* r = trans + 4 * a;
+  return __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)p[0]), __dmul_rn(r[1], (double)p[1])), __dmul_rn(r[2], (double)p[2])),
+                   r[3]);
+}
+
+__device__ __forceinline__ bool edit_target(const double* trans, const double* inv, const double* b, const double* lo,
+                                            const double* hi, bool in, const float p[3], float t[3], double q[3]) {
+  double dt[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    t[a] = __double2float_rn(moved_coord(trans, a, p));
+    dt[a] = __dsub_rn((double)t[a], b[a]);
+  }
+  return index_in_box(inv, lo, hi, in, dt, q);
+}
+
+// ---- deformations (DESIGN.md, "Deforming objects") -------------------------------------------------------------------------
+// Every expression is fp64 with one rounding per operation (the _rn intrinsics: no contraction) and nothing transcendental, so
+// that oracle/deform_oracle.py takes the same decisions.
+
+// A deformation's table at height h: the knot interval k, the interpolated A (row-major) and t, det A, and whether h lies inside
+// [h0, h0 + (K - 1) dh] (the derivative in h is zero where the table is clamped).  (u, v): the pulled frame coordinates.
+struct Pulled {
+  double a[4], t[2], det, u, v, h;
+  int k;
+  bool inside;
+};
+
+// x = D^-1(y) for y in the network frame: frame coordinates (u, v, h) of y, r = (h - h0) / dh, k = clamp(floor r, 0, K - 2),
+// s = clamp(r - k, 0, 1), A and t interpolated per entry as A_k + s (A_k+1 - A_k), (u', v') = adj(A) ((u, v) - t) / det A, and
+// x = ((c + u' e_u) + v' e_v) + h e_h.
+__device__ __forceinline__ Pulled deform_pull(const Deform& D, const double y[3], double x[3]) {
+  const double *eu = D.frame, *ev = D.frame + 3, *eh = D.frame + 6, *c = D.frame + 9;
+  const double d[3] = {__dsub_rn(y[0], c[0]), __dsub_rn(y[1], c[1]), __dsub_rn(y[2], c[2])};
+  auto dot = [&](const double* e) {
+    return __dadd_rn(__dadd_rn(__dmul_rn(e[0], d[0]), __dmul_rn(e[1], d[1])), __dmul_rn(e[2], d[2]));
+  };
+  const double u = dot(eu), v = dot(ev);
+  Pulled P;
+  P.h = dot(eh);
+  const double r = __ddiv_rn(__dsub_rn(P.h, D.h0), D.dh);
+  const double kf = fmin(fmax(floor(r), 0.0), (double)(D.n_knots - 2));
+  P.k = (int)kf;
+  P.inside = r >= 0.0 && r <= (double)(D.n_knots - 1);
+  const double s = fmin(fmax(__dsub_rn(r, kf), 0.0), 1.0);
+  const double* k0 = D.knots + 6 * P.k;
+#pragma unroll
+  for (int j = 0; j < 6; ++j) {
+    const double e = __dadd_rn(k0[j], __dmul_rn(s, __dsub_rn(k0[6 + j], k0[j])));
+    if (j < 4) P.a[j] = e;
+    else P.t[j - 4] = e;
+  }
+  P.det = __dsub_rn(__dmul_rn(P.a[0], P.a[3]), __dmul_rn(P.a[1], P.a[2]));
+  const double du = __dsub_rn(u, P.t[0]), dv = __dsub_rn(v, P.t[1]);
+  P.u = __ddiv_rn(__dsub_rn(__dmul_rn(P.a[3], du), __dmul_rn(P.a[1], dv)), P.det);
+  P.v = __ddiv_rn(__dsub_rn(__dmul_rn(P.a[0], dv), __dmul_rn(P.a[2], du)), P.det);
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+    x[a] = __dadd_rn(__dadd_rn(__dadd_rn(c[a], __dmul_rn(P.u, eu[a])), __dmul_rn(P.v, ev[a])), __dmul_rn(P.h, eh[a]));
+  return P;
+}
+
+// edit_target of a deformed move: y = trans p (fp64, not rounded), x = D^-1(y) rounded once to fp32 as t, then the same box test.
+__device__ __forceinline__ Pulled edit_target_deformed(const double* trans, const Deform& D, const double* inv, const double* b,
+                                                       const double* lo, const double* hi, bool& in, const float p[3], float t[3],
+                                                       double q[3]) {
+  double y[3], x[3], dt[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) y[a] = moved_coord(trans, a, p);
+  const Pulled P = deform_pull(D, y, x);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    t[a] = __double2float_rn(x[a]);
+    dt[a] = __dsub_rn((double)t[a], b[a]);
+  }
+  in = index_in_box(inv, lo, hi, in, dt, q);
+  return P;
+}
+
+// The pulled-back tangent J_D^-1 w of a direction w (network frame, fp64) at the pulled point P: in frame coordinates
+// (w_u, w_v, w_h), g = A' (u', v') + t' (A' = (A_k+1 - A_k) / dh and t' likewise inside the knots, zero where clamped),
+// r = (w_u, w_v) - w_h g, (d_u, d_v) = adj(A) r / det A, and out = (d_u e_u + d_v e_v) + w_h e_h.
+__device__ __forceinline__ void deform_direction(const Deform& D, const Pulled& P, const double w[3], double out[3]) {
+  const double *eu = D.frame, *ev = D.frame + 3, *eh = D.frame + 6;
+  auto dot = [&](const double* e) {
+    return __dadd_rn(__dadd_rn(__dmul_rn(e[0], w[0]), __dmul_rn(e[1], w[1])), __dmul_rn(e[2], w[2]));
+  };
+  const double wu = dot(eu), wv = dot(ev), wh = dot(eh);
+  double g0 = 0.0, g1 = 0.0;
+  if (P.inside) {
+    const double* k0 = D.knots + 6 * P.k;
+    double s[6];
+#pragma unroll
+    for (int j = 0; j < 6; ++j) s[j] = __ddiv_rn(__dsub_rn(k0[6 + j], k0[j]), D.dh);
+    g0 = __dadd_rn(__dadd_rn(__dmul_rn(s[0], P.u), __dmul_rn(s[1], P.v)), s[4]);
+    g1 = __dadd_rn(__dadd_rn(__dmul_rn(s[2], P.u), __dmul_rn(s[3], P.v)), s[5]);
+  }
+  const double r0 = __dsub_rn(wu, __dmul_rn(wh, g0)), r1 = __dsub_rn(wv, __dmul_rn(wh, g1));
+  const double du = __ddiv_rn(__dsub_rn(__dmul_rn(P.a[3], r0), __dmul_rn(P.a[1], r1)), P.det);
+  const double dv = __ddiv_rn(__dsub_rn(__dmul_rn(P.a[0], r1), __dmul_rn(P.a[2], r0)), P.det);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) out[a] = __dadd_rn(__dadd_rn(__dmul_rn(du, eu[a]), __dmul_rn(dv, ev[a])), __dmul_rn(wh, eh[a]));
 }
 
 // mesh_generator.py:51-62: occ = 1 - exp(-relu(sigma) * voxel), sigma = channel 3 of the network output [n, c]

@@ -383,15 +383,165 @@ def _mask_box(mask, margin):
     return tuple(box)
 
 
+# ----------------------------------------------------------------------------------------------------------------- deformations
+# DESIGN.md, "Deforming objects": a move bends, twists and tapers its object where it stands, before the move.
+MAX_KNOTS = 64
+
+
+def _det_interval_min(A, B):
+    """The minimum over s in [0, 1] of det(A + s (B - A)) for 2x2 row-major A, B, in the library's operation order."""
+    D = [B[0] - A[0], B[1] - A[1], B[2] - A[2], B[3] - A[3]]
+    d0, a2 = A[0] * A[3] - A[1] * A[2], D[0] * D[3] - D[1] * D[2]
+    b1 = ((A[0] * D[3] + D[0] * A[3]) - A[1] * D[2]) - D[1] * A[2]
+    lo = min(d0, (d0 + b1) + a2)
+    if a2 > 0.0:
+        s = -b1 / (2.0 * a2)
+        if 0.0 < s < 1.0:
+            lo = min(lo, d0 - (b1 * b1) / (4.0 * a2))
+    return lo
+
+
+def deformation_problem(frame, h0, dh, knots):
+    """The library's checks of a deformation (frame [12]: e_u, e_v, e_h, c; knots [K, 6]: A row-major, then t) in its order ->
+    the reason it is rejected, or None."""
+    frame = [float(v) for v in np.asarray(frame, dtype=np.float64).reshape(-1)]
+    knots = np.asarray(knots, dtype=np.float64).reshape(-1, 6)
+    K = knots.shape[0]
+    if not 2 <= K <= MAX_KNOTS:
+        return "n_knots %d is not 0 and outside [2, %d]" % (K, MAX_KNOTS)
+    if not (np.isfinite(frame).all() and np.isfinite(knots).all() and np.isfinite(h0) and np.isfinite(dh)):
+        return "a value is not finite"
+    if not dh > 0.0:
+        return "dh %g must be > 0" % dh
+    e = frame
+    ok = all(abs(((e[3 * a] * e[3 * b] + e[3 * a + 1] * e[3 * b + 1]) + e[3 * a + 2] * e[3 * b + 2]) - (1.0 if a == b else 0.0))
+             <= 1e-9 for a in range(3) for b in range(3))
+    for a in range(3):
+        a1, a2 = (a + 1) % 3, (a + 2) % 3
+        ok = ok and abs((e[a1] * e[3 + a2] - e[a2] * e[3 + a1]) - e[6 + a]) <= 1e-9
+    if not ok:
+        return "the frame is not orthonormal and right-handed"
+    for k in range(K - 1):
+        if not _det_interval_min([float(v) for v in knots[k, :4]], [float(v) for v in knots[k + 1, :4]]) > 0.0:
+            return "det A(h) <= 0 on knot interval %d" % k
+    return None
+
+
+class Deformation:
+    """A checked deformation of a move's object (DESIGN.md, "Deforming objects"): in the frame of centre `centre`, up axis `up`
+    (e_h) and forward axis `forward` (e_u; e_v = up x forward), the object's horizontal section at frame height h maps as
+    (u, v) -> A(h) (u, v) + t(h), h kept.  A [K, 2, 2] and t [K, 2] are the knots at heights h0 + k dh (dh > 0, K in [2, 64]),
+    interpolated linearly and clamped to the end knots.  ValueError with the library's message for a table it rejects: a
+    non-finite value, dh <= 0, axes that are not orthonormal to 1e-9, or det A(h) <= 0 anywhere between the knots.
+    Immutable; deformation() builds one from twist, bend and taper profiles."""
+    __slots__ = ("frame", "h0", "dh", "knots", "_abi")
+
+    def __init__(self, centre, up, forward, h0, dh, A, t):
+        up, forward = np.asarray(up, dtype=np.float64).reshape(3), np.asarray(forward, dtype=np.float64).reshape(3)
+        frame = np.concatenate([forward, np.cross(up, forward), up, np.asarray(centre, dtype=np.float64).reshape(3)])
+        A, t = np.asarray(A, dtype=np.float64), np.asarray(t, dtype=np.float64)
+        if A.ndim != 3 or A.shape[1:] != (2, 2) or t.shape != (A.shape[0], 2):
+            raise ValueError("deformation: A must be [K, 2, 2] and t [K, 2], got shapes %s and %s" % (A.shape, t.shape))
+        knots = np.concatenate([A.reshape(-1, 4), t], 1)
+        why = deformation_problem(frame, float(h0), float(dh), knots)
+        if why is not None:
+            raise ValueError("deformation: " + why)
+        d = _lib.Deformation()
+        held = (C.c_double * knots.size)(*knots.reshape(-1).tolist())
+        d.n_knots, d.h0, d.dh, d.knots = knots.shape[0], float(h0), float(dh), C.cast(held, C.POINTER(C.c_double))
+        d.frame[:] = frame.tolist()
+        for k, v in zip(self.__slots__, (frame, float(h0), float(dh), knots, (d, held))):
+            object.__setattr__(self, k, v)
+        frame.setflags(write=False)
+        knots.setflags(write=False)
+
+    def __setattr__(self, key, value):
+        raise AttributeError("Deformation is immutable")
+
+    def abi(self):
+        """The dmnerf_deformation of this table (its knots held by this value)."""
+        return self._abi[0]
+
+
+def _profile(values, knots, what):
+    if values is None:
+        return None
+    s = np.linspace(0.0, 1.0, knots)
+    v = np.asarray([values(x) for x in s] if callable(values) else values, dtype=np.float64).reshape(-1)
+    if v.shape != (knots,) or not np.isfinite(v).all():
+        raise ValueError("deformation: %s must be %d finite values or a callable of the normalised height, got %d" % (what, knots,
+                                                                                                               v.size))
+    return v
+
+
+def deformation(centre, up, h0, h1, knots=33, twist=None, bend=None, bend_dir=None, taper=None):
+    """The Deformation that twists, bends and tapers an object standing at `centre` along `up` between frame heights h0 < h1
+    (heights along up, from the centre).  Each profile is `knots` values or a callable of the normalised height in [0, 1]:
+    twist, an angle in degrees about up; bend, an offset along the horizontal direction bend_dir; taper, a horizontal scale
+    (each > 0).  Per knot A = R(twist) diag(taper, taper) and t = (bend, 0); e_u is bend_dir (made horizontal) with a bend and
+    otherwise a horizontal axis.  cos / sin are numpy's."""
+    knots = int(knots)
+    if not 2 <= knots <= MAX_KNOTS:
+        raise ValueError("deformation: n_knots %d is not 0 and outside [2, %d]" % (knots, MAX_KNOTS))
+    if not (np.isfinite([h0, h1]).all() and h1 > h0):
+        raise ValueError("deformation: the height range [%r, %r] must be finite and h1 > h0" % (h0, h1))
+    up = np.asarray(up, dtype=np.float64).reshape(3)
+    if not (np.isfinite(up).all() and np.linalg.norm(up) > 0):
+        raise ValueError("deformation: up must be a finite non-zero vector")
+    up = up / np.linalg.norm(up)
+    tw, bd, tp = _profile(twist, knots, "twist"), _profile(bend, knots, "bend"), _profile(taper, knots, "taper")
+    if bd is not None:
+        if bend_dir is None:
+            raise ValueError("deformation: a bend needs bend_dir")
+        e = np.asarray(bend_dir, dtype=np.float64).reshape(3)
+        e = e - np.dot(e, up) * up
+        if not np.linalg.norm(e) > 1e-9:
+            raise ValueError("deformation: bend_dir must not be parallel to up")
+    else:
+        e = np.eye(3)[int(np.argmin(np.abs(up)))]
+        e = e - np.dot(e, up) * up
+    e = e / np.linalg.norm(e)
+    if tp is not None and not (tp > 0).all():
+        raise ValueError("deformation: taper must be > 0")
+    th = np.radians(tw) if tw is not None else np.zeros(knots)
+    sc = tp if tp is not None else np.ones(knots)
+    c, s = np.cos(th), np.sin(th)
+    A = np.stack([np.stack([c * sc, -s * sc], -1), np.stack([s * sc, c * sc], -1)], 1)
+    t = np.stack([bd if bd is not None else np.zeros(knots), np.zeros(knots)], -1)
+    return Deformation(centre, up, e, float(h0), (float(h1) - float(h0)) / (knots - 1), A, t)
+
+
+def move_deformations(deformations, m):
+    """deformations (None, or one Deformation-or-None per move) -> a list of m, or None when every move is rigid."""
+    if deformations is None:
+        return None
+    if isinstance(deformations, Deformation) or not hasattr(deformations, "__iter__"):
+        raise ValueError("deformations must be None or one Deformation (or None) per move, got %r" % (deformations,))
+    defs = list(deformations)
+    if len(defs) != m or any(d is not None and not isinstance(d, Deformation) for d in defs):
+        raise ValueError("deformations must be None or one Deformation (or None) for each of the %d moves" % m)
+    return defs if any(d is not None for d in defs) else None
+
+
+def _deformation_array(defs):
+    """The HOST dmnerf_deformation [n] of the _deformed entry points (a rigid move: n_knots 0)."""
+    arr = (_lib.Deformation * len(defs))()
+    for i, d in enumerate(defs):
+        if d is not None:
+            arr[i] = d.abi()
+    return arr
+
+
 def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, extents=None, level=0.45, near=4.0, far=15.0,
-                   N_importance=128, pieces=None, rest="keep", slab=0, copies=None, groups=None):
+                   N_importance=128, pieces=None, rest="keep", slab=0, copies=None, groups=None, deformations=None):
     """dmnerf_mesh_occupancy_edit: the moves [(label, 4x4)] applied in order, in place, to occ / labels ([dim]^3 float32 /
     int16 on the device: the keep-all sweep of model_fine on this grid), the network evaluated only at the target points
     inside each move's box (boxes: [m, 6] inclusive index boxes, EMPTY_BOX for none).  pieces / rest: as manipulator.  copies
     (None, a bool or one per move): the moves that are copies, which take as the move would and never vacate
     (dmnerf_mesh_occupancy_edit_copies; DESIGN.md, "Copying objects").  groups (None, or per move None or labels; DESIGN.md,
-    "Moving objects together"): the labels each move carries as one body (dmnerf_mesh_occupancy_edit_groups).  Returns the number
-    of target points evaluated."""
+    "Moving objects together"): the labels each move carries as one body (dmnerf_mesh_occupancy_edit_groups).  deformations (None,
+    or one Deformation or None per move; DESIGN.md, "Deforming objects"): each deformed move bends, twists or tapers its object
+    (dmnerf_mesh_occupancy_edit_deformed).  Returns the number of target points evaluated."""
     from .manipulator import _piece_region, move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -405,6 +555,7 @@ def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, exten
     drops = move_rests(rest, len(mv))
     sets = move_groups(groups, mv, ins_num)
     flags = _check_copies(copies, mv, drops, sets=sets)
+    defs = move_deformations(deformations, len(mv))
     regions = move_pieces(pieces, mv, ins_num, occ.device) or [None] * len(mv)
     if not mv:
         return 0
@@ -423,7 +574,10 @@ def edit_occupancy(model_fine, scene_transform, occ, labels, moves, boxes, exten
     head = (ctx.handle, slot, _lib.doubles(T, 16), _lib.doubles(ext, 3), dim, (far - near) / N_importance, level, int(slab), descs)
     tail = (len(mv), _lib.ptr(occ), _lib.ptr(labels, torch.int16), C.byref(n))
     with torch.no_grad():
-        if sets is not None:
+        if defs is not None:
+            ctx.call("dmnerf_mesh_occupancy_edit_deformed", *head, _copy_flags(flags), None if sets is None else _group_words(sets),
+                     _deformation_array(defs), *tail)
+        elif sets is not None:
             ctx.call("dmnerf_mesh_occupancy_edit_groups", *head, _copy_flags(flags), _group_words(sets), *tail)
         elif any(flags):
             ctx.call("dmnerf_mesh_occupancy_edit_copies", *head, _copy_flags(flags), *tail)
@@ -454,7 +608,7 @@ def edit_boxes(occ, labels, moves, scene_transform, extents=None, level=0.45, ma
 
 
 def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128,
-                 margin=2, boxes=None, pieces=None, rest="keep", copies=None, groups=None):
+                 margin=2, boxes=None, pieces=None, rest="keep", copies=None, groups=None, deformations=None):
     """The labelled sweep of the edited scene -> (occ [dim]^3 float32, labels [dim]^3 int16) on the device: the keep-all sweep of
     model_fine (occupancy_objects), then the moves [(label, 4x4 in the network frame, as manipulator_eval's transformation)]
     applied in order (edit_occupancy).  A move shows at p what the network holds at trans p, as rigid_rays renders it: the
@@ -466,7 +620,9 @@ def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None,
     groups (None, or one entry per move: None or an iterable of labels holding the move's label; DESIGN.md, "Moving objects
     together"): each move carries every label of its set as one rigid body -- a table with what stands on it -- in one pass;
     a target of any label of the set is taken with its own label, and every label of the set is vacated.  The default box holds
-    the whole set.  carried_labels finds the set of what rests on an object."""
+    the whole set.  carried_labels finds the set of what rests on an object.  deformations (None, or one Deformation or None per
+    move; DESIGN.md, "Deforming objects"): a deformed move bends, twists or tapers its object where it stands, before the move; the
+    default box is still the source's."""
     from .manipulator import move_pieces, move_rests
     from .mesh import check_transform
     T = check_transform(scene_transform)
@@ -475,6 +631,7 @@ def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None,
     mv, _ = _check_moves(moves, ins_num)
     level = _check_level(level)
     _check_copies(copies, mv, move_rests(rest, len(mv)), sets=move_groups(groups, mv, ins_num))
+    move_deformations(deformations, len(mv))
     move_pieces(pieces, mv, ins_num, dev)
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
@@ -486,25 +643,26 @@ def edited_sweep(model_fine, scene_transform, moves, grid_dim=256, extents=None,
         if boxes is None:
             boxes = edit_boxes(occ, labels, moves, T, extents, level, margin, pieces, groups)
         edit_occupancy(model_fine, T, occ, labels, moves, boxes, extents, level, near, far, N_importance, pieces, rest, copies=copies,
-                       groups=groups)
+                       groups=groups, deformations=deformations)
     return occ, labels
 
 
 def edited_mesh(model_fine, scene_transform, moves, grid_dim=256, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128,
-                margin=2, boxes=None, pieces=None, rest="keep", min_cluster=400, per_object=False, copies=None, groups=None):
+                margin=2, boxes=None, pieces=None, rest="keep", min_cluster=400, per_object=False, copies=None, groups=None,
+                deformations=None):
     """The mesh of an edited scene: edited_sweep (same arguments) -> marching cubes -> scene space -> normals -> small-cluster
     removal.  Returns extract_mesh's keys as device tensors -- vertices, triangles, normals, clean_vertices, clean_normals,
     clean_triangles -- and labels (int64 per clean vertex: mesh.vertex_labels of its index-space vertex, the label of the
     inside end of its edge, from the edited grid; no label rays are rendered).  per_object: also objects, the
-    meshes_from_labelled_grid of the edited grid for every label with solid points except ins_num.  copies, groups: as
-    edited_sweep."""
+    meshes_from_labelled_grid of the edited grid for every label with solid points except ins_num.  copies, groups, deformations:
+    as edited_sweep."""
     from .mesh import EXTENTS, check_transform, clean_mesh, marching_cubes, to_scene, vertex_labels, vertex_normals
     T = check_transform(scene_transform)
     ext = EXTENTS if extents is None else extents
     ins_num = int(model_fine.ins_linear.weight.shape[0]) - 1
     with torch.no_grad():
         occ, labels = edited_sweep(model_fine, T, moves, grid_dim, ext, level, near, far, N_importance, margin, boxes, pieces, rest,
-                                   copies=copies, groups=groups)
+                                   copies=copies, groups=groups, deformations=deformations)
         v_idx, tris = marching_cubes(occ, level)
         verts = to_scene(v_idx, T, grid_dim, ext)
         normals = vertex_normals(verts, tris)
@@ -524,15 +682,19 @@ def edited_mesh(model_fine, scene_transform, moves, grid_dim=256, extents=None, 
 class MovedScene:
     """Checked moves for render_rays(moves=) / render_frame(moves=): the dmnerf_render_moves the library reads, and the move
     descriptions and region bits it points into, held for as long as the value lives.  copies: per move, whether it is a copy
-    (DESIGN.md, "Copying objects"); groups: per move, the labels it carries (DESIGN.md, "Moving objects together").  Immutable."""
-    __slots__ = ("_desc", "_held", "device", "labels", "boxes", "rest_drop", "level", "voxel", "copies", "_flags", "groups", "_words")
+    (DESIGN.md, "Copying objects"); groups: per move, the labels it carries (DESIGN.md, "Moving objects together");
+    deformations: per move, its Deformation or None (DESIGN.md, "Deforming objects").  Immutable."""
+    __slots__ = ("_desc", "_held", "device", "labels", "boxes", "rest_drop", "level", "voxel", "copies", "_flags", "groups", "_words",
+                 "deformations", "_defs")
 
-    def __init__(self, desc, held, device, labels, boxes, rest_drop, level, voxel, copies=None, groups=None):
+    def __init__(self, desc, held, device, labels, boxes, rest_drop, level, voxel, copies=None, groups=None, deformations=None):
         copies = tuple(bool(c) for c in copies) if copies is not None else (False,) * len(labels)
         sets = tuple(tuple(g) for g in groups) if groups is not None else tuple((k,) for k in labels)
+        defs = tuple(deformations) if deformations is not None else (None,) * len(labels)
         for k, v in zip(self.__slots__, (desc, held, device, labels, tuple(map(tuple, boxes.tolist())), tuple(rest_drop), level,
                                          voxel, copies, _copy_flags(copies) if any(copies) else None, sets,
-                                         _group_words(sets) if groups is not None else None)):
+                                         _group_words(sets) if groups is not None else None, defs,
+                                         _deformation_array(defs) if any(d is not None for d in defs) else None)):
             object.__setattr__(self, k, v)
 
     def __setattr__(self, key, value):
@@ -550,15 +712,21 @@ class MovedScene:
         """The label sets dmnerf_render_moved_groups reads (HOST uint32 [n_moves][4]), or None when no group was given."""
         return self._words
 
+    def deformation_array(self):
+        """The deformations dmnerf_render_moved_deformed reads (HOST dmnerf_deformation [n_moves]), or None when every move is
+        rigid."""
+        return self._defs
+
 
 def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, near=4.0, far=15.0, N_importance=128, margin=2,
-                 boxes=None, pieces=None, rest="keep", copies=None, groups=None):
+                 boxes=None, pieces=None, rest="keep", copies=None, groups=None, deformations=None):
     """The moves [(label, 4x4 in the network frame)] of edited_sweep, checked for the moved render -> a MovedScene.  occ / labels:
     the unedited keep-all sweep ([dim]^3 float32 / int16 on the device) that the default boxes come from (edit_boxes, as
     edited_sweep) and whose grid (scene_transform, extents, dim) the boxes index.  level, margin, boxes, pieces, rest: as
     edited_sweep; the voxel of the occupancy test is the sweep's (far - near) / N_importance.  moves, pieces and rest may be
     arrange_objects' moves, pieces and rest unchanged, or manipulator_eval's [(label, 4x4)].  Labels are checked against the
-    networks when the render runs.  copies, groups: as edited_sweep (arrange_objects' copies and groups unchanged)."""
+    networks when the render runs.  copies, groups: as edited_sweep (arrange_objects' copies and groups unchanged).
+    deformations: as edited_sweep; a deformed move's view directions are its pulled-back ray tangents."""
     from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -570,6 +738,7 @@ def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     drops = move_rests(rest, len(mv))
     sets = move_groups(groups, mv, MAX_LABELS - 1)
     flags = _check_copies(copies, mv, drops, sets=sets)
+    defs = move_deformations(deformations, len(mv))
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
     with np.errstate(divide="ignore", invalid="ignore"):
@@ -589,7 +758,7 @@ def render_moves(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     d.extents[:] = np.asarray(ext, dtype=np.float64).reshape(-1).tolist()
     d.level, d.voxel = level, float(voxel)
     return MovedScene(d, (descs, [r.bits for r in regions if r is not None]), occ.device, tuple(mv), boxes, drops, level,
-                      float(voxel), flags, sets)
+                      float(voxel), flags, sets, defs)
 
 
 # ----------------------------------------------------------------------------------------------------------------- collisions
@@ -611,7 +780,7 @@ def _check_sweep(occ, labels, who):
 
 
 def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, boxes=None, margin=2, pieces=None, rest="keep",
-                 obstacles=None, copies=None, groups=None):
+                 obstacles=None, copies=None, groups=None, deformations=None):
     """dmnerf_move_overlap: each move [(label, 4x4 in the network frame)] checked on its own against the labelled keep-all sweep
     occ / labels ([dim]^3 float32 / int16 on the device; an edited_sweep result is accepted unchanged).  boxes, margin, pieces,
     rest: as edited_sweep (default boxes: edit_boxes).  obstacles: the labels that count as obstacles (default every label).
@@ -620,7 +789,8 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     overlap_volume {label: voxels times the inventory's voxel volume} and total (the overlapping voxels).  copies (None, a bool or
     one per move; DESIGN.md, "Copying objects"): a copy vacates nothing, so its own label's solid points are obstacles too.
     groups (as edited_sweep; DESIGN.md, "Moving objects together"): each candidate moves its whole set; landed and overlap count
-    every label of the set, and the points the set vacates are not obstacles (a copy's stay)."""
+    every label of the set, and the points the set vacates are not obstacles (a copy's stay).  deformations (as edited_sweep;
+    DESIGN.md, "Deforming objects"): each candidate's object is deformed before its move."""
     from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -632,6 +802,7 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     drops = move_rests(rest, len(mv))
     sets = move_groups(groups, mv, ins_num)
     flags = _check_copies(copies, mv, drops, ordered=False)
+    defs = move_deformations(deformations, len(mv))
     regions = move_pieces(pieces, mv, ins_num, occ.device) or [None] * len(mv)
     words = ALL_LABELS if obstacles is None else label_words(obstacles)
     if not mv:
@@ -645,7 +816,10 @@ def move_overlap(occ, labels, scene_transform, moves, extents=None, level=0.45, 
     ctx = get_context(occ.device)
     head = (ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), dim, level, _lib.doubles(T, 16), _lib.doubles(ext, 3), descs)
     tail = (len(mv), (C.c_uint32 * 4)(*words), overlap.ctypes.data_as(C.POINTER(C.c_int64)), landed.ctypes.data_as(C.POINTER(C.c_int64)))
-    if sets is not None:
+    if defs is not None:
+        ctx.call("dmnerf_move_overlap_deformed", *head, _copy_flags(flags), None if sets is None else _group_words(sets),
+                 _deformation_array(defs), *tail)
+    elif sets is not None:
         ctx.call("dmnerf_move_overlap_groups", *head, _copy_flags(flags), _group_words(sets), *tail)
     elif any(flags):
         ctx.call("dmnerf_move_overlap_copies", *head, _copy_flags(flags), *tail)
@@ -1312,9 +1486,10 @@ def largest_component_grid(occ, labels, level, objects):
 ARRANGE_KEYS = ("label", "near", "on", "piece", "rest", "turns", "stable", "lift", "obstacles", "copy", "group")
 
 
-def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes, drops, regions, flags=None, sets=None):
+def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes, drops, regions, flags=None, sets=None, defs=None):
     """dmnerf_grid_edit of checked moves (flags: the checked copy flags, None for none; sets: the checked label sets, None for
-    none): applied in place to occ / labels, sampled from src_occ / src_labels -> edited_grid's report."""
+    none; defs: the checked deformations, None for none): applied in place to occ / labels, sampled from src_occ / src_labels ->
+    edited_grid's report."""
     n, dim = len(mv), occ.shape[0]
     overwritten = np.zeros((n, MAX_LABELS), dtype=np.int64)
     landed = np.zeros(n, dtype=np.int64)
@@ -1323,7 +1498,10 @@ def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes,
             _edit_moves(mv, mats, boxes, drops, regions, occ.device))
     tail = (n, _lib.ptr(occ), _lib.ptr(labels, torch.int16), landed.ctypes.data_as(C.POINTER(C.c_int64)),
             overwritten.ctypes.data_as(C.POINTER(C.c_int64)))
-    if sets is not None:
+    if defs is not None:
+        ctx.call("dmnerf_grid_edit_deformed", *head, _copy_flags(flags or [False] * n), None if sets is None else _group_words(sets),
+                 _deformation_array(defs), *tail)
+    elif sets is not None:
         ctx.call("dmnerf_grid_edit_groups", *head, _copy_flags(flags or [False] * n), _group_words(sets), *tail)
     elif flags is not None and any(flags):
         ctx.call("dmnerf_grid_edit_copies", *head, _copy_flags(flags), *tail)
@@ -1334,7 +1512,7 @@ def _grid_edit(src_occ, src_labels, occ, labels, T, ext, level, mv, mats, boxes,
 
 
 def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, boxes=None, margin=2, pieces=None, rest="keep",
-                copies=None, groups=None):
+                copies=None, groups=None, deformations=None):
     """dmnerf_grid_edit: edited_sweep's moves applied in order to the labelled keep-all sweep occ / labels ([dim]^3 float32 / int16
     on the device) without the network: a move shows at p the unedited grid at the nearest grid index of trans p, as the collision
     checks sample a moved object.  On a grid whose points and steps are exact in fp32, whole-voxel translations and quarter turns
@@ -1343,7 +1521,8 @@ def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, b
     move: label, landed (the voxels it takes from a solid target), overwritten {label: voxels} (labels with voxels > 0: solid
     points of the grid as the earlier moves left it that it lands on and does not vacate), overwritten_volume and total.
     copies: as edited_sweep (DESIGN.md, "Copying objects"); a copy's overwritten counts its own label's points too.  groups: as
-    edited_sweep (DESIGN.md, "Moving objects together"); landed and overwritten count the whole set."""
+    edited_sweep (DESIGN.md, "Moving objects together"); landed and overwritten count the whole set.  deformations: as
+    edited_sweep (DESIGN.md, "Deforming objects")."""
     from .manipulator import move_pieces, move_rests
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
@@ -1354,6 +1533,7 @@ def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, b
     drops = move_rests(rest, len(mv))
     sets = move_groups(groups, mv, MAX_LABELS - 1)
     flags = _check_copies(copies, mv, drops, sets=sets)
+    defs = move_deformations(deformations, len(mv))
     regions = move_pieces(pieces, mv, MAX_LABELS - 1, occ.device) or [None] * len(mv)
     if int(margin) != margin or int(margin) < 0:
         raise ValueError("edit: margin must be an integer >= 0, got %r" % (margin,))
@@ -1364,7 +1544,7 @@ def edited_grid(occ, labels, scene_transform, moves, extents=None, level=0.45, b
     if not mv:
         return out_occ, out_labels, []
     return out_occ, out_labels, _grid_edit(occ, labels, out_occ, out_labels, T, ext, level, mv, mats, boxes, drops, regions, flags,
-                                           sets)
+                                           sets, defs)
 
 
 def _check_items(items, dim, device):

@@ -175,7 +175,10 @@ def render_rays(rays_o, rays_d, model_coarse, model_fine, z_vals_coarse, perturb
         ctx.call("dmnerf_render_forward", ctx.handle, io, n, S, N_importance, flags, impl)
         return out
     evaluated = (C.c_int64 * 2)()
-    if moves.group_words() is not None:
+    if moves.deformation_array() is not None:
+        ctx.call("dmnerf_render_moved_deformed", ctx.handle, io, n, S, N_importance, flags, impl, C.byref(moves.abi()),
+                 moves.copy_flags(), moves.group_words(), moves.deformation_array(), evaluated)
+    elif moves.group_words() is not None:
         ctx.call("dmnerf_render_moved_groups", ctx.handle, io, n, S, N_importance, flags, impl, C.byref(moves.abi()),
                  moves.copy_flags(), moves.group_words(), evaluated)
     elif moves.copy_flags() is None:

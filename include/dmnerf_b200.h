@@ -728,6 +728,48 @@ DMNERF_API int dmnerf_placement_contacts_in_scene_group(dmnerf_ctx* ctx, const f
                                                         const int32_t* box_host /* [6] */, int u, int v, int32_t* cells_host,
                                                         int64_t max_cells, int64_t* n_cells_host, int32_t* drop_host, void* stream);
 
+/* ---- Deforming objects (DESIGN.md, "Deforming objects") ----------------------------------------------------------------------
+ * A move may bend, twist and taper its object: a height-preserving deformation D of the object where it stands, before the move,
+ * so that the forward map is x -> trans^-1 D(x) and a destination point p shows the network at x = D^-1(trans p).  D acts in a
+ * frame of the network frame: centre c and orthonormal right-handed axes e_u, e_v, e_h (e_h "up"); in frame coordinates
+ * (u, v, h) it maps (u, v) -> A(h) (u, v) + t(h) and keeps h, A(h) and t(h) interpolating n_knots knots linearly at heights
+ * h0 + k dh, clamped to the end knots outside them.  frame: the rows e_u, e_v, e_h, c; knots: HOST double [n_knots][6], A row-major
+ * then t.  n_knots == 0: a rigid move (every other field ignored).  The pull is fp64 with one rounding per operation and rounded once
+ * to fp32 before the existing box test; the moved render's view direction is the pulled-back ray's tangent.
+ * The entry points below are the _groups ones with deformations_host [n] (HOST; NULL: every move rigid).  An all-rigid array
+ * equals the namesake bit for bit.  Rejected on the host before any launch, with an error naming the entry point: n_knots outside
+ * {0} and [2, 64], NULL knots, a non-finite value, dh <= 0, a frame that is not orthonormal and right-handed to 1e-9, and
+ * det A(h) <= 0 anywhere on a knot interval. */
+typedef struct dmnerf_deformation {
+  int32_t n_knots;            /* 0: rigid; otherwise in [2, 64] */
+  double frame[12];           /* e_u, e_v, e_h, c (network frame) */
+  double h0, dh;              /* knot k at height h0 + k dh, dh > 0 */
+  const double* knots;        /* HOST [n_knots][6]: A00 A01 A10 A11 t0 t1 */
+} dmnerf_deformation;
+DMNERF_API int dmnerf_mesh_occupancy_edit_deformed(dmnerf_ctx* ctx, int net, const double* transform_host, const double* extents_host,
+                                                   int dim, float voxel, float level, int64_t slab, const dmnerf_edit_move* moves_host,
+                                                   const int32_t* copies_host /* [n] */, const uint32_t* groups_host /* [n][4] */,
+                                                   const dmnerf_deformation* deformations_host /* [n] */, int n_moves, float* occ,
+                                                   int16_t* labels, int64_t* evaluated_host, void* stream);
+DMNERF_API int dmnerf_grid_edit_deformed(dmnerf_ctx* ctx, const float* src_occ, const int16_t* src_labels, int dim, float level,
+                                         const double* transform_host, const double* extents_host, const dmnerf_edit_move* moves_host,
+                                         const int32_t* copies_host /* [n] */, const uint32_t* groups_host /* [n][4] */,
+                                         const dmnerf_deformation* deformations_host /* [n] */, int n_moves, float* occ,
+                                         int16_t* labels, int64_t* landed_host /* [n] */, int64_t* overwritten_host /* [n][128] */,
+                                         void* stream);
+DMNERF_API int dmnerf_render_moved_deformed(dmnerf_ctx* ctx, const dmnerf_render_io* io, int64_t n, int S, int NI, int flags, int impl,
+                                            const dmnerf_render_moves* moves, const int32_t* copies_host /* [n_moves] */,
+                                            const uint32_t* groups_host /* [n_moves][4] */,
+                                            const dmnerf_deformation* deformations_host /* [n_moves] */, int64_t* evaluated_host,
+                                            void* stream);
+DMNERF_API int dmnerf_move_overlap_deformed(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                            const double* transform_host, const double* extents_host,
+                                            const dmnerf_edit_move* candidates_host, const int32_t* copies_host /* [n] */,
+                                            const uint32_t* groups_host /* [n][4] */,
+                                            const dmnerf_deformation* deformations_host /* [n] */, int n_candidates,
+                                            const uint32_t* obstacles_host, int64_t* overlap_host /* [n][128] */,
+                                            int64_t* landed_host /* [n] */, void* stream);
+
 /* ---- connected components (DESIGN.md, "Connected components"; no counterpart in the original) --------------------------------
  * The solid points (occ > level) of a grid occ [dim,dim,dim] (DEVICE, C order, p = (i dim + j) dim + k) split into components:
  * two solid points are adjacent when they are face neighbours (connectivity 6) or face, edge or corner neighbours (26), never

@@ -51,7 +51,12 @@ Rendering (--render): `exchanger` (the default) renders the frame with manipulat
 the scene again along every move.  `samples` renders the same moves, pieces and rest with render_frame(moves=) (DESIGN.md,
 "Rendering moved objects"): the edited sweep's rule applied per render sample, with the default boxes of the keep-all sweep, so
 that the frame and --mesh show the same edit.  The record gains render and evaluated (the targets the moved render evaluated in
-its coarse and fine passes; null for the exchanger)."""
+its coarse and fine passes; null for the exchanger).
+
+Deforming (--twist DEG, --bend D --bend-dir X Y Z, --taper S, with --up X Y Z and --knots K; DESIGN.md, "Deforming objects"):
+the piece is twisted, bent and tapered before its move, about its inventory centre, over its extent along --up in the sweep; the
+twist (0 to DEG) and taper (1 to S) are linear in height and the bend (0 to D) quadratic.  They need --render samples, work with
+--mesh and --check, and the record gains deformation."""
 import argparse
 import json
 import os
@@ -112,7 +117,35 @@ def parse(argv=None):
                     help="move these labels together with the piece's label, as one body (needs --render samples)")
     ap.add_argument("--carry", action="store_true",
                     help="also move what rests on the piece's label, transitively (carried_labels; needs --down and --render samples)")
+    ap.add_argument("--twist", type=float, default=None, metavar="DEG",
+                    help="twist the piece about --up, 0 at its bottom to DEG at its top (needs --render samples)")
+    ap.add_argument("--bend", type=float, default=None, metavar="D",
+                    help="bend the piece: its top shifts by D along --bend-dir, quadratic in height (needs --render samples)")
+    ap.add_argument("--bend-dir", type=float, nargs=3, default=None, metavar=("X", "Y", "Z"), help="--bend: the horizontal direction")
+    ap.add_argument("--taper", type=float, default=None, metavar="S",
+                    help="taper the piece: horizontal scale 1 at its bottom to S at its top (needs --render samples)")
+    ap.add_argument("--up", type=float, nargs=3, default=None, metavar=("X", "Y", "Z"),
+                    help="--twist / --bend / --taper: the network-frame up axis of the deformation")
+    ap.add_argument("--knots", type=int, default=33, help="--twist / --bend / --taper: knots of the deformation's table")
     a = ap.parse_args(argv)
+    a.deformed = a.twist is not None or a.bend is not None or a.taper is not None
+    if a.deformed:
+        if a.render != "samples":
+            ap.error("--twist, --bend and --taper need --render samples: the exchanger renders rigid moves only")
+        for flag, given in (("--arrange", a.arrange is not None), ("--place-at", a.place_at is not None),
+                            ("--until-contact", a.until_contact)):
+            if given:
+                ap.error("--twist, --bend and --taper cannot be combined with %s: placement and the slide are rigid" % flag)
+        if a.up is None or not any(a.up):
+            ap.error("--twist, --bend and --taper need --up X Y Z, not 0 0 0")
+        if a.bend is not None and (a.bend_dir is None or not any(a.bend_dir)):
+            ap.error("--bend needs --bend-dir X Y Z, not 0 0 0")
+        if not 2 <= a.knots <= 64:
+            ap.error("deformation: n_knots %d is not 0 and outside [2, 64]" % a.knots)
+        if a.taper is not None and not a.taper > 0:
+            ap.error("deformation: taper must be > 0")
+    elif a.up is not None or a.bend_dir is not None:
+        ap.error("--up and --bend-dir need --twist, --bend or --taper")
     a.grouped = a.with_labels is not None or a.carry
     if a.grouped:
         if a.arrange is not None:
@@ -313,6 +346,22 @@ def place_piece(a, occ, labels, T, ext, label, region, group=None):
     return out
 
 
+def piece_deformation(a, occ, labels, T, ext, label, region, centre):
+    """--twist / --bend / --taper: the piece's Deformation about its inventory centre and --up, over the piece's extent along
+    --up in the sweep; the twist and taper are linear in height and the bend quadratic."""
+    from dmnerf_b200.objects import _region_keeps, deformation, grid_affine
+    up = np.asarray(a.up, dtype=np.float64) / np.linalg.norm(a.up)
+    mask = (labels == label) & (occ > a.level) & _region_keeps(region, T, occ.shape[0], ext, occ.device)
+    A, b = grid_affine(T, occ.shape[0], ext)
+    h = (np.argwhere(mask.cpu().numpy()) @ A.T + b - centre) @ up
+    h0, h1 = (float(h.min()), float(h.max())) if h.size else (-1.0, 1.0)
+    if not h1 > h0:
+        h0, h1 = h0 - 1.0, h1 + 1.0
+    return deformation(centre, up, h0, h1, a.knots, twist=None if a.twist is None else (lambda s: a.twist * s),
+                       bend=None if a.bend is None else (lambda s: a.bend * s * s), bend_dir=a.bend_dir,
+                       taper=None if a.taper is None else (lambda s: 1.0 + (a.taper - 1.0) * s))
+
+
 def main(argv=None):
     a = parse(argv)
     import torch
@@ -372,9 +421,12 @@ def main(argv=None):
         trans = {"transformations": [{"transformation": place.pop("transformation"), "mode": "placement"}]}
     else:
         trans = manipulation_transform(centre, a.mode, distance=a.distance, yaw=a.yaw, scale=a.scale)
+    deforms = None
     if a.arrange is None:
         moves, regions, rests = [(label, trans["transformations"][0]["transformation"])], [region], [a.rest]
         copies, groups = [a.copy], [group]
+        if a.deformed:
+            deforms = [piece_deformation(a, occ, labels, T, ext, label, region, centre)]
     dev = next(nets[1].parameters()).device
     pose_t = torch.from_numpy(c2w).to(dev)
     evaluated = None
@@ -382,7 +434,7 @@ def main(argv=None):
         from dmnerf_b200.objects import render_moves
         from dmnerf_b200.render import render_frame
         moved = render_moves(occ, labels, T, moves, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests,
-                             copies=copies, groups=groups)
+                             copies=copies, groups=groups, deformations=deforms)
         with torch.no_grad():
             fr = render_frame(a.H, a.W, a.K, pose_t, a.near, a.far, nets[0], nets[1], a.N_samples, a.N_importance, keep_all_ins=True,
                               device=dev, moves=moved)
@@ -414,6 +466,9 @@ def main(argv=None):
         record["group"] = group
     if chain is not None:
         record["chain"] = chain
+    if deforms is not None:
+        record["deformation"] = {"twist": a.twist, "bend": a.bend, "bend_dir": a.bend_dir, "taper": a.taper, "up": a.up,
+                                 "knots": a.knots, "h0": deforms[0].h0, "dh": deforms[0].dh}
     if slide is not None:
         record["slide"] = slide
     if place is not None:
@@ -421,7 +476,7 @@ def main(argv=None):
     if a.check:
         from dmnerf_b200.objects import move_overlap
         r = move_overlap(occ, labels, T, [(label, trans["transformations"][0]["transformation"])], ext, a.level, pieces=[region],
-                         rest=a.rest, copies=a.copy, groups=[group])[0]
+                         rest=a.rest, copies=a.copy, groups=[group], deformations=deforms)[0]
         record["overlap"] = {"voxels": {str(k): v for k, v in r["overlap"].items()},
                              "volume": {str(k): v for k, v in r["overlap_volume"].items()}}
         record["landed"] = r["landed"]
@@ -430,7 +485,7 @@ def main(argv=None):
     if a.mesh:
         from dmnerf_b200.objects import edited_mesh
         m = edited_mesh(nets[1], T, moves, a.grid_dim, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests,
-                        min_cluster=a.min_cluster, copies=copies, groups=groups)
+                        min_cluster=a.min_cluster, copies=copies, groups=groups, deformations=deforms)
         M.write_ply(os.path.join(a.out, "edited.ply"), m["vertices"], m["triangles"])
         lab = m["labels"].cpu().numpy()
         colors = np.where((lab >= 0)[:, None], lut[np.clip(lab, 0, ins_num)], 0).astype(np.uint8)   # instance.png's colours
