@@ -229,14 +229,23 @@ __device__ __forceinline__ void ray_merge_sorted(const float* a, int na, const f
   __syncwarp();
 }
 
-// Rank sort of vals[0..T) (shared) into out[0..T): ascending, ties by index (networks/render.py:70).
+// Rank sort of vals[0..T) (shared) into out[0..T): ascending, ties by index (networks/render.py:70).  A NaN ranks after every
+// number and among the NaNs by index, torch.sort's order: a NaN sample (NaN coarse weights) lands in the top slots, and every
+// slot is written once.
 __device__ __forceinline__ void ray_rank_part(const float* vals, int T, float* out, int tid, int nthr) {
   for (int e = tid; e < T; e += nthr) {
     const float v = vals[e];
     int rank = 0;
-    for (int j = 0; j < T; ++j) {
-      const float o = vals[j];
-      rank += (o < v) || (o == v && j < e);
+    if (v == v) {
+      for (int j = 0; j < T; ++j) {
+        const float o = vals[j];
+        rank += (o < v) || (o == v && j < e);
+      }
+    } else {
+      for (int j = 0; j < T; ++j) {
+        const float o = vals[j];
+        rank += (o == o) || j < e;
+      }
     }
     out[rank] = v;
   }

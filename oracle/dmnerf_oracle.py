@@ -87,6 +87,47 @@ def sample_pdf(bins, weights, n_samples, det=False, u=None):
     if det:
         u = torch.linspace(0.0, 1.0, steps=n_samples, dtype=bins.dtype)             # :132
         u = u.expand(list(cdf.shape[:-1]) + [n_samples])
+    return _inverse_cdf(bins, cdf, u)
+
+
+def warp_cdf(weights):
+    """The CDF of sample_pdf (helpers.py:125-128) in fp32, summed in the order of the library's one-warp samplers (ray_build_cdf,
+    dm-nerf_b200/csrc/ray_ops.cuh): lane l (of 32) adds w[l], w[l + 32], ... in turn, a butterfly over the lanes gives the total,
+    and each 32-wide chunk of the pdf is a Hillis-Steele inclusive scan added to the running carry.  The reference's CPU cumsum
+    accumulates in fp64 instead; the two differ in the last bits, which moves samples where the inverse CDF is ill-conditioned.
+    weights [N, B - 1] -> cdf [N, B]."""
+    w = weights.float() + 1e-5                                                      # :125
+    n, nw = w.shape
+    chunks = (nw + 31) // 32
+    lanes = torch.zeros(n, chunks * 32)
+    lanes[:, :nw] = w
+    lanes = lanes.reshape(n, chunks, 32)
+    total = torch.zeros(n, 32)
+    for c in range(chunks):
+        total = total + lanes[:, c]
+    for d in (16, 8, 4, 2, 1):
+        total = total + total[:, torch.arange(32) ^ d]
+    pdf = lanes / total[:, :1, None]
+    cdf, carry = [torch.zeros(n, 1)], torch.zeros(n)
+    for c in range(chunks):
+        v = pdf[:, c]
+        for d in (1, 2, 4, 8, 16):
+            v = torch.cat([v[:, :d], v[:, d:] + v[:, :-d]], -1)
+        cdf.append(carry[:, None] + v)
+        carry = carry + v[:, 31]
+    return torch.cat(cdf, -1)[:, :nw + 1].contiguous()
+
+
+def sample_pdf_warp(bins, weights, n_samples, det=False, u=None):
+    """sample_pdf with the CDF of warp_cdf: the library's samplers' arithmetic, operation for operation."""
+    cdf = warp_cdf(weights)
+    if det:
+        u = torch.linspace(0.0, 1.0, steps=n_samples).expand(cdf.shape[0], n_samples)
+    return _inverse_cdf(bins.float(), cdf, u.float())
+
+
+def _inverse_cdf(bins, cdf, u):
+    """helpers.py:137-153: the samples of u [N, n_samples] on the CDF cdf [N, B] over bins [N, B]."""
     u = u.contiguous()
     inds = torch.searchsorted(cdf, u, right=True)                                   # :139
     below = torch.clamp(inds - 1, min=0)
@@ -124,6 +165,15 @@ def sample_pdf_explained(bins, weights, n_samples, det, u, tol):
     twin = sample_pdf(bins.double(), weights.double(), n_samples, det=det, u=None if u is None else u.double()).numpy()
     twin_bad = np.abs(twin - ref) > tol                                                                       # (c)
     return knot | cond | twin_bad
+
+
+def hier_sample(z_c, w_c, n_importance, det, u=None):
+    """The fine depths of reference networks/render.py:66-70 from given coarse depths z_c [N, S] and weights w_c [N, S]:
+    sample_pdf on the mid-points with weights[1:-1], then sort(cat(coarse, samples)).  NaN samples sort last, as torch.sort
+    puts them."""
+    z_mid = 0.5 * (z_c[..., 1:] + z_c[..., :-1])                                    # :66
+    z_samples = sample_pdf(z_mid, w_c[..., 1:-1], n_importance, det=det, u=u).detach()   # :67-68
+    return torch.sort(torch.cat([z_c, z_samples], -1), -1)[0]                       # :70
 
 
 def z_val_sample(n_rays, near, far, n_samples, dtype=torch.float32):

@@ -87,6 +87,17 @@ def test_render_inference(golden_dir):
         assert float(out["acc_fine"].max()) <= 1.0 + 1e-5
 
 
+def test_hier_sample_restates_render(golden_dir):
+    """O.hier_sample fed the render's own coarse depths and weights gives the render's fine depths bit for bit, deterministic
+    and with given uniforms (the GPU sampler tests compare against it)."""
+    g, pc, pf, ro, rd, zc = _render_case(golden_dir, "study")
+    with torch.no_grad():
+        for perturb, t_rand, u in ((0.0, None, None), (1.0, torch.from_numpy(g["t_rand"]), torch.from_numpy(g["u"]))):
+            out = O.render(ro, rd, pc, pf, zc, perturb=perturb, t_rand=t_rand, u=u)
+            zf = O.hier_sample(out["z_vals_coarse"], out["weights_coarse"], 128, det=perturb == 0.0, u=u)
+            assert zf.shape == out["z_vals_fine"].shape and torch.equal(zf, out["z_vals_fine"])
+
+
 def test_render_train_and_grads(golden_dir):
     g, pc, pf, ro, rd, zc = _render_case(golden_dir, "study")
     for d in (pc, pf):
