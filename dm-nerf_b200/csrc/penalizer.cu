@@ -54,6 +54,13 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 // traffic is fully coalesced (a thread-per-sample walk over rows of 18..132 floats touches partial sectors only).
 static int pen_tile(int c) { return c <= 48 ? 256 : (c <= 96 ? 128 : 64); }
 
+// The tile's rows take exactly 48 KB at the widest C of a tile size (48, 96); with the forward's static shared memory that is
+// over the default per-block limit, so a launch opts in to the tile's size whenever it reaches it.
+static int pen_smem(const void* kernel, size_t smem) {
+  if (smem >= 40 * 1024) DMN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  return 0;
+}
+
 // This block's two masked sums (fp64 accumulation of fp32 terms) and two mask populations, valid in thread 0; the block's
 // rows of raw are staged through shared memory.
 __device__ __forceinline__ void pen_block_terms(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ depth,
@@ -219,6 +226,7 @@ int launch_penalizer_backward(const float* raw, const float* z, const float* dep
   if (total == 0) return 0;
   const int tile = pen_tile(c);
   const unsigned grid = (unsigned)((total + tile - 1) / tile);
+  if (pen_smem((const void*)penalizer_grad_kernel, (size_t)tile * c * sizeof(float))) return 1;
   penalizer_grad_kernel<<<grid, tile, (size_t)tile * c * sizeof(float), st>>>(raw, z, depth, rays_d, total, s, c, tol, w,
                                                                               reinterpret_cast<const PenState*>(state), g_loss, d_raw,
                                                                               accumulate);
@@ -247,6 +255,7 @@ int launch_penalizer_forward(const float* raw, const float* z, const float* dept
   }
   const int tile = pen_tile(c);
   const unsigned grid = (unsigned)((total + tile - 1) / tile);
+  if (pen_smem((const void*)penalizer_partial_kernel, (size_t)tile * c * sizeof(float))) return 1;
   penalizer_partial_kernel<<<grid, tile, (size_t)tile * c * sizeof(float), st>>>(raw, z, depth, rays_d, total, s, c, tol, w, ps,
                                                                                  reinterpret_cast<PenBlock*>(ps + 1), loss);
   DMN_LAUNCH_OK();
