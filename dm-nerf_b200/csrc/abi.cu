@@ -1276,6 +1276,18 @@ DMNERF_API int dmnerf_region_contains(const dmnerf_region* region, const float* 
   return region_contains(r, pts, n, out, (cudaStream_t)stream);
 }
 
+// ---- viewing the labelled grid (DESIGN.md, "Viewing the labelled grid") ----------------------------------------------------
+
+DMNERF_API int dmnerf_grid_cast(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                const double* transform_host, const double* extents_host, const uint32_t* keep_words_host,
+                                const float* rays_o, const float* rays_d, int64_t n, float near_t, float far_t, float* t_out,
+                                int16_t* label_out, int32_t* voxel_out, float* normal_out, void* stream) {
+  DMN_CHECK(ctx != nullptr, "grid_cast: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return grid_cast(occ, labels, dim, level, transform_host, extents_host, keep_words_host, rays_o, rays_d, n,
+                   near_t, far_t, t_out, label_out, voxel_out, normal_out, (cudaStream_t)stream);
+}
+
 // ---- test-view evaluation (networks/tester.py render_test, networks/evaluator.py ins_eval) --------------------------------
 
 DMNERF_API int64_t dmnerf_eval_workspace_bytes(int64_t n, int k, int H, int W) {

@@ -448,6 +448,12 @@ int region_pack(const int32_t* ids, int dim, const uint32_t* table, int64_t n_id
 int region_dilate(const uint32_t* in, int dim, int r, int connectivity, int invert, uint32_t* out, uint32_t* tmp, cudaStream_t st);
 int region_contains(const Region& r, const float* pts, int64_t n, uint8_t* out, cudaStream_t st);   // r from region_from_abi
 
+// Casting rays through a labelled grid (raycast.cu; DESIGN.md, "Viewing the labelled grid"): checked on the host before any launch,
+// then one voxel walk per ray.  No read-back, no atomics, no scratch.
+int grid_cast(const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
+              const uint32_t* keep_host, const float* rays_o, const float* rays_d, int64_t n, float near_t, float far_t, float* t_out,
+              int16_t* label_out, int32_t* voxel_out, float* normal_out, cudaStream_t st);
+
 // Test-view evaluation (metrics.cu)
 int64_t eval_workspace_bytes(int64_t n, int k, int H, int W);
 int eval_image(const float* rgb, const float* gt, int H, int W, void* ws, dmnerf_eval_result* res, cudaStream_t st);

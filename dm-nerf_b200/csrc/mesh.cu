@@ -620,31 +620,6 @@ int launch_argmax_rows(const float* x, int64_t n, int c, int64_t* out, cudaStrea
 // Every fp64 expression below is written with one rounding per operation (no contraction), so that a numpy restatement
 // (oracle/edit_sweep_oracle.py) takes the same decisions.
 
-// The grid's index map of objects.grid_affine: p = A idx + b with A = S R diag(h), b = S (t - R e), h = extents / (dim - 1),
-// e = extents / 2 and S the axis swap (x, y, z) -> (x, -z, y); inv = diag(1 / h) R^-1 S^T, R^-1 = adj(R) / det(R).
-static void grid_index_map(const double* T, const double* ext, int dim, double inv[9], double b[3]) {
-  const double R[3][3] = {{T[0], T[1], T[2]}, {T[4], T[5], T[6]}, {T[8], T[9], T[10]}};
-  double adj[3][3];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) {
-      const int i1 = (j + 1) % 3, i2 = (j + 2) % 3, j1 = (i + 1) % 3, j2 = (i + 2) % 3;
-      adj[i][j] = R[i1][j1] * R[i2][j2] - R[i1][j2] * R[i2][j1];       // cofactor (j, i)
-    }
-  const double det = (R[0][0] * adj[0][0] + R[0][1] * adj[1][0]) + R[0][2] * adj[2][0];
-  double w[3];
-  for (int r = 0; r < 3; ++r)
-    w[r] = T[4 * r + 3] - ((R[r][0] * (ext[0] / 2.0) + R[r][1] * (ext[1] / 2.0)) + R[r][2] * (ext[2] / 2.0));
-  b[0] = w[0]; b[1] = -w[2]; b[2] = w[1];
-  for (int a = 0; a < 3; ++a) {
-    const double scale = (double)(dim - 1) / ext[a];
-    const double ri[3] = {adj[a][0] / det, adj[a][1] / det, adj[a][2] / det};
-    // column c of S^T: S^T e_0 = e_0, S^T e_1 = -e_2, S^T e_2 = e_1
-    inv[3 * a] = scale * ri[0];
-    inv[3 * a + 1] = scale * -ri[2];
-    inv[3 * a + 2] = scale * ri[1];
-  }
-}
-
 int sweep_grid_check(const double* T, const double* ext3, int dim, float level, const char* who) {
   DMN_CHECK(dim >= 2 && dim <= 2048, "%s: dim %d out of range [2, 2048]", who, dim);
   DMN_CHECK(level > 0.0f && level < 1.0f, "%s: level %g outside (0, 1)", who, (double)level);

@@ -30,6 +30,10 @@
     carried_labels(occ, labels, scene_transform, label, down, ...)
                                                         -> what rests on an object, transitively: the group= that moves
                                                            it together with what it carries
+    cast_grid(occ, labels, scene_transform, rays_o, rays_d, near, far, ...) / grid_view(occ, labels, scene_transform, H, W, K,
+              c2w, near, far, ...)                     -> the first solid voxel along each ray (depth, label, voxel, normal,
+                                                           piece), and depth, label, normal and colour maps of the grid
+                                                           from one or several cameras, with no network
 
 Every network sample is labelled argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the
 exchanger's rule); a sample whose label is not kept has alpha = 0 in the composite of both passes, so the coarse weights of the
@@ -2234,3 +2238,132 @@ def manipulation_transform(centre, mode, distance=-0.25, yaw=90.0, scale=1.2):
     grow = np.diag([scale, scale, scale, 1.0])
     op = {"translation": move, "rotation": turn, "scale": grow, "multi": grow @ turn @ move}[mode]
     return {"transformations": [{"transformation": (back @ op @ to_origin).tolist(), "mode": mode}]}
+
+
+# ----------------------------------------------------------------------------------------------------------------- grid views
+# DESIGN.md, "Viewing the labelled grid": camera rays cast through a labelled keep-all grid to the first solid, kept voxel, with no
+# network: the look of "place, look, adjust" at the cost of one voxel walk per pixel, and the label or piece under a pixel.
+def _cast_words(keep, remove):
+    """keep= / remove= of the cast (labels in [0, 127]) -> the 4 keep words, or None for every label."""
+    if keep is not None and remove is not None:
+        raise ValueError("cast_grid: give at most one of keep= or remove=")
+    if keep is None and remove is None:
+        return None
+    words = label_words(_labels(keep if keep is not None else remove, MAX_LABELS - 1, "cast_grid"))
+    return words if keep is not None else [~w & 0xFFFFFFFF for w in words]
+
+
+def _check_rays(rays_o, rays_d, device):
+    _lib.need_cuda("cast_grid", rays_o, rays_d)
+    if rays_o.shape != rays_d.shape or rays_o.dim() < 1 or rays_o.shape[-1] != 3:
+        raise ValueError("cast_grid: rays_o and rays_d must have one shape [..., 3], got %s and %s"
+                         % (tuple(rays_o.shape), tuple(rays_d.shape)))
+    if rays_o.device != device or rays_d.device != device:
+        raise ValueError("cast_grid: the rays must be on the grid's device")
+    if rays_o.dtype != torch.float32 or rays_d.dtype != torch.float32:
+        raise ValueError("cast_grid: rays must be float32")
+
+
+def _check_range(near, far, level):
+    near, far, level = float(near), float(far), float(level)
+    if not (np.isfinite(near) and np.isfinite(far) and near <= far):
+        raise ValueError("cast_grid: near %r and far %r must be finite with near <= far" % (near, far))
+    if not np.isfinite(level):
+        raise ValueError("cast_grid: level %r is not finite" % (level,))
+    return near, far, level
+
+
+def cast_grid(occ, labels, scene_transform, rays_o, rays_d, near, far, extents=None, level=0.45, keep=None, remove=None,
+              components=None, normals=True):
+    """dmnerf_grid_cast: each ray o + t d (rays_o, rays_d [..., 3] float32 on the grid's device, network frame) cast over
+    t in [near, far] through the labelled grid occ / labels ([dim]^3 float32 / int16: occupancy_objects' keep-all sweep, or
+    edited_grid's, arrange_objects' or edited_sweep's output) to its first solid voxel (occ > level) whose label is kept (keep= or
+    remove=: labels in [0, 127]; default every label).  Grid point q owns the cube [q - 1/2, q + 1/2]^3, so depth is where the
+    ray enters that cube, in the units of rays_d as given.  Returns device tensors of the rays' leading shape: depth (float32,
+    +inf without a hit), label (int16, -1), voxel (int64 [..., 3] index (i, j, k), -1), point (o + depth d in float32, NaN
+    without a hit), normal (float32 [..., 3], 0 without a hit; None when normals=False) and hit (bool).  With components (an
+    object_components result of this grid), also piece: the component id at the hit voxel (-1 without a hit).  The picking
+    primitive: the label and piece under a pixel come from the ray of that pixel (get_rays_at)."""
+    from .mesh import EXTENTS, check_transform
+    T = check_transform(scene_transform)
+    ext = np.asarray(EXTENTS if extents is None else extents, dtype=np.float64).reshape(-1)
+    if ext.shape != (3,) or not (np.isfinite(ext).all() and (ext > 0).all()):
+        raise ValueError("cast_grid: extents must be 3 finite values > 0")
+    near, far, level = _check_range(near, far, level)
+    words = _cast_words(keep, remove)
+    if components is not None and (not isinstance(components, dict) or "grid" not in components
+                                   or tuple(components["grid"].shape) != tuple(occ.shape)):
+        raise ValueError("cast_grid: components must be an object_components result of this grid")
+    dim = _check_sweep(occ, labels, "cast_grid")
+    _check_rays(rays_o, rays_d, occ.device)
+    shape = tuple(rays_o.shape[:-1])
+    o = rays_o.reshape(-1, 3).contiguous()
+    d = rays_d.reshape(-1, 3).contiguous()
+    n, dev = o.shape[0], occ.device
+    depth = torch.empty(n, dtype=torch.float32, device=dev)
+    label = torch.empty(n, dtype=torch.int16, device=dev)
+    voxel = torch.empty(n, dtype=torch.int32, device=dev)
+    normal = torch.empty((n, 3), dtype=torch.float32, device=dev) if normals else None
+    ctx = get_context(dev)
+    ctx.call("dmnerf_grid_cast", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), dim, level, _lib.doubles(T, 16),
+             _lib.doubles(ext, 3), None if words is None else _lib.keep_mask(words), _lib.ptr(o), _lib.ptr(d), n, near, far,
+             _lib.ptr(depth), _lib.ptr(label, torch.int16), _lib.ptr(voxel, torch.int32), _lib.ptr(normal))
+    hit = voxel >= 0
+    v = voxel.to(torch.int64)
+    ijk = torch.where(hit[:, None], torch.stack([v // (dim * dim), (v // dim) % dim, v % dim], -1), torch.full_like(v[:, None], -1))
+    point = torch.where(hit[:, None], o + depth[:, None] * d, torch.full_like(o, float("nan")))
+    out = {"depth": depth.reshape(shape), "label": label.reshape(shape), "voxel": ijk.reshape(shape + (3,)),
+           "point": point.reshape(shape + (3,)), "normal": None if normal is None else normal.reshape(shape + (3,)),
+           "hit": hit.reshape(shape)}
+    if components is not None:
+        grid = components["grid"].reshape(-1)
+        out["piece"] = torch.where(hit, grid[v.clamp(min=0)], torch.full_like(voxel, -1)).reshape(shape)
+    return out
+
+
+def grid_view(occ, labels, scene_transform, H, W, K, c2w, near, far, extents=None, level=0.45, keep=None, remove=None, lut=None,
+              model_fine=None):
+    """The labelled grid seen from one camera (c2w [4, 4] or [3, 4]) or several (c2w [V, 4, 4]), all views in one cast_grid
+    launch.  Pixel (row, col) casts get_rays_k's ray, the ray render_frame renders there.  Returns device maps [V?, H, W] of depth,
+    label and hit, and normal [V?, H, W, 3].  With lut (uint8 [L, 3], e.g. tester.pred_label_lut), also image [V?, H, W, 3] uint8:
+    tester.colorize's label colours shaded by |n . d/|d||, black where nothing is hit.  With model_fine, also rgb [V?, H, W, 3]
+    float32: sigmoid of the first three outputs of mlp_forward_points(model_fine, point, d/|d|) at the hit pixels (0 elsewhere),
+    one network query per pixel.  That colour is meaningful only on an unedited grid: on an edited grid the hit points of a moved,
+    copied or deformed object are not where the network holds its colour, and this function cannot tell the two grids apart --
+    render an edited scene with render_moves and render_frame(moves=)."""
+    from .helpers import get_rays_k
+    _check_range(near, far, level)
+    if int(H) != H or int(W) != W or int(H) < 1 or int(W) < 1:
+        raise ValueError("grid_view: H and W must be integers >= 1, got %r x %r" % (H, W))
+    H, W = int(H), int(W)
+    pose = torch.as_tensor(c2w, dtype=torch.float32)
+    single = pose.dim() == 2
+    poses = pose[None] if single else pose
+    if poses.dim() != 3 or poses.shape[1] not in (3, 4) or poses.shape[2] != 4 or poses.shape[0] < 1:
+        raise ValueError("grid_view: c2w must be [4, 4], [3, 4] or [V, 4, 4], got %s" % (tuple(pose.shape),))
+    if lut is not None:
+        lut = np.asarray(lut)
+        if lut.dtype != np.uint8 or lut.ndim != 2 or lut.shape[1] != 3 or lut.shape[0] < 1:
+            raise ValueError("grid_view: lut must be uint8 [L, 3]")
+    _check_sweep(occ, labels, "grid_view")
+    poses = poses.to(occ.device)
+    rays = [get_rays_k(H, W, K, poses[v]) for v in range(poses.shape[0])]
+    o = torch.stack([r[0] for r in rays])
+    d = torch.stack([r[1] for r in rays])
+    c = cast_grid(occ, labels, scene_transform, o, d, near, far, extents, level, keep, remove)
+    out = {k: c[k] for k in ("depth", "label", "normal", "hit")}
+    if lut is not None or model_fine is not None:
+        dirs = d / torch.norm(d, dim=-1, keepdim=True)
+    if lut is not None:
+        from .tester import colorize
+        shade = (c["normal"] * dirs).sum(-1).abs()
+        out["image"] = torch.round(colorize(c["label"], lut).float() * shade[..., None]).clamp(0, 255).to(torch.uint8)
+    if model_fine is not None:
+        from .autograd import mlp_forward_points
+        rgb = torch.zeros(o.shape, dtype=torch.float32, device=occ.device)
+        hit = c["hit"]
+        if bool(hit.any()):
+            with torch.no_grad():
+                rgb[hit] = torch.sigmoid(mlp_forward_points(model_fine, c["point"][hit], dirs[hit])[:, :3])
+        out["rgb"] = rgb
+    return {k: v[0] for k, v in out.items()} if single else out

@@ -791,6 +791,27 @@ DMNERF_API int dmnerf_component_table(dmnerf_ctx* ctx, const int32_t* comp, cons
 DMNERF_API int dmnerf_component_groups(dmnerf_ctx* ctx, const int32_t* comp, int dim, int64_t n, const int16_t* lut, int discard,
                                        int16_t* groups, void* stream);
 
+/* ---- viewing the labelled grid (DESIGN.md, "Viewing the labelled grid"; no counterpart in the original) ----------------------
+ * dmnerf_grid_cast: per ray the first solid, kept voxel of a labelled grid occ [dim^3] (DEVICE float32) / labels [dim^3] (DEVICE
+ *   int16), with the scene transform and extents of the sweep (HOST float64, as dmnerf_mesh_occupancy), dim in [2, 1290].  Grid
+ *   point q owns the cube [q - 1/2, q + 1/2]^3; the ray o + t d (rays_o, rays_d [n][3], DEVICE float32, network frame; t in the
+ *   units of d as given) is cast over t in [near, far] clipped to the grid's cube [-1/2, dim - 1/2]^3 in index space
+ *   (u(t) = inv (o - b) + t inv d with the index map of dmnerf_mesh_occupancy_edit) by a voxel walk whose boundary times are
+ *   computed directly in fp64, one rounding per operation, ties stepping i before j before k.  A voxel is solid when
+ *   occ > level (NaN never is) and, with keep_words_host (HOST uint32 [4], may be NULL: every label), its label is in [0, 127]
+ *   and kept.  Per ray: t_out (DEVICE float32) = the hit voxel's entry time max(t0, t_entry) rounded once, +inf without a hit;
+ *   label_out (DEVICE int16) and voxel_out (DEVICE int32, C-order linear index) = -1 without a hit; normal_out [n][3] (DEVICE
+ *   float32, may be NULL) = -inv^T grad(occ) at the voxel normalised (central differences, one-sided at the grid's faces),
+ *   the entry face's normal when that gradient is zero or not finite, -d / |d| when the ray starts inside the voxel; 0 without
+ *   a hit.  Rays with a non-finite or zero direction, or that miss the grid, have no hit.  No atomics and no read-back: the
+ *   call does not synchronise and repeats bit for bit.  Rejected on the host before any launch, writing nothing: NULL grid, transform
+ *   or extents, NULL ray or output pointers with n > 0, dim out of range, a non-finite level, near / far not finite or
+ *   near > far, n < 0, a transform that is not finite or has det <= 0, extents not finite and > 0. */
+DMNERF_API int dmnerf_grid_cast(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, int dim, float level,
+                                const double* transform_host, const double* extents_host, const uint32_t* keep_words_host,
+                                const float* rays_o, const float* rays_d, int64_t n, float near_t, float far_t, float* t_out,
+                                int16_t* label_out, int32_t* voxel_out, float* normal_out, void* stream);
+
 /* ---- region selection (DESIGN.md, "Region selection"; no counterpart in the original) ------------------------------------
  * A region (dmnerf_region) is one bit per point of a sweep grid [dim,dim,dim] (dim in [2, 1290]; point v = (i dim + j) dim + k
  * is bit v & 31 of word v >> 5, ceil(dim^3 / 32) uint32 words, the bits past dim^3 zero), the voxel map [M | c] (row-major 3x4

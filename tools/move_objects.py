@@ -1,12 +1,13 @@
 #!/usr/bin/env python
 """Move one piece of an object of a trained DM-NeRF checkpoint and render the edited frame (DESIGN.md, "Moving pieces").
 
-    python tools/move_objects.py CHECKPOINT.tar --pose POSE.npy --hwk H W K (--move-label L | --move-piece ID | --arrange SPEC.json)
+    python tools/move_objects.py CHECKPOINT.tar --pose POSE.npy --hwk H W K
+           (--move-label L | --move-piece ID | --pick X Y | --arrange SPEC.json)
            (--mode {translation,rotation,scale,multi} [--distance -0.25 --yaw 90 --scale 1.2]
             | --place-at X Y Z --down X Y Z [--on L ...] [--lift N] [--any-stability] [--turns K]) [--rest keep|drop]
            --transform T [--extents X Y Z] [--grid-dim 256] [--level 0.45] [--connectivity {6,26}] [--dilate 1] --out DIR
            [--near 4 --far 15 --N-samples 64 --N-importance 128 --N-test 4096] [--mesh [--min-cluster 400]]
-           [--check] [--until-contact [--step S] [--tolerance N]] [--render {exchanger,samples}]
+           [--check] [--until-contact [--step S] [--tolerance N]] [--preview] [--render {exchanger,samples,none}]
 
 CHECKPOINT holds `network_coarse_state_dict` and `network_fine_state_dict`.  POSE.npy holds the camera-to-world pose [4, 4] (or
 [3, 4]; of several [N, 4, 4] the first is used).  K is the 3x3 intrinsics, as a .npy file or as 9 numbers.
@@ -16,7 +17,9 @@ as tools/find_objects.py), split at --level into --connectivity-connected pieces
 component (the `component` ids of tools/find_objects.py --components split with the same sweep arguments), --move-label the
 label's largest one.  The edit turns or shifts the piece about its own centre (manipulation_transform, the original's
 generate_poses_eval), moves only that piece (its region grown by --dilate voxels) and keeps (--rest keep) or removes (--rest drop)
-the rest of its label: `--move-label L --rest drop` moves object L without its floaters.
+the rest of its label: `--move-label L --rest drop` moves object L without its floaters.  --pick X Y takes the piece under
+column X, row Y of --pose's view: the pixel's ray (get_rays_at) cast through the same sweep (cast_grid, DESIGN.md, "Viewing the
+labelled grid"); the label, piece and network-frame point it hits are printed and recorded as pick.
 
 Writes DIR/rgb.png, DIR/instance.png (the arg-max label of the edited instance map; label k gets colour k of a fixed seeded
 palette, as tools/render_objects.py) and DIR/transform.json (the transformation dict, the moved label, piece and centre), and
@@ -51,7 +54,13 @@ Rendering (--render): `exchanger` (the default) renders the frame with manipulat
 the scene again along every move.  `samples` renders the same moves, pieces and rest with render_frame(moves=) (DESIGN.md,
 "Rendering moved objects"): the edited sweep's rule applied per render sample, with the default boxes of the keep-all sweep, so
 that the frame and --mesh show the same edit.  The record gains render and evaluated (the targets the moved render evaluated in
-its coarse and fine passes; null for the exchanger).
+its coarse and fine passes; null for the exchanger).  `none` renders no frame and meshes nothing: with --preview, the look at an
+edit costs a grid edit and a voxel walk per pixel instead of a network render.
+
+Previews (--preview; DESIGN.md, "Viewing the labelled grid"): before the frame is rendered, the keep-all sweep is cast from --pose
+(grid_view): DIR/preview.png shows the unedited grid and DIR/preview_edited.png the edited_grid of the same moves (or the
+arrangement), in instance.png's colours shaded by the angle between surface and ray, and DIR/preview_rgb.png the network's colour
+at the unedited grid's hits (one query per pixel).  The network colour of moved objects is render_moves' job (--render samples).
 
 Deforming (--twist DEG, --bend D --bend-dir X Y Z, --taper S, with --up X Y Z and --knots K; DESIGN.md, "Deforming objects"):
 the piece is twisted, bent and tapered before its move, about its inventory centre, over its extent along --up in the sweep; the
@@ -77,6 +86,7 @@ def parse(argv=None):
     which = ap.add_mutually_exclusive_group(required=True)
     which.add_argument("--move-label", type=int, metavar="L", help="move the largest piece of object label L")
     which.add_argument("--move-piece", type=int, metavar="ID", help="move this piece (a component id of the sweep)")
+    which.add_argument("--pick", type=int, nargs=2, metavar=("X", "Y"), help="move the piece under column X, row Y of --pose's view")
     which.add_argument("--arrange", metavar="SPEC.json", help="place several pieces one after another (a JSON list of items)")
     ap.add_argument("--mode", choices=("translation", "rotation", "scale", "multi"))
     ap.add_argument("--distance", type=float, default=None, help="translation along y (default -0.25)")
@@ -110,8 +120,10 @@ def parse(argv=None):
     ap.add_argument("--until-contact", action="store_true", help="translation: slide until just before contact")
     ap.add_argument("--step", type=float, default=None, help="--until-contact: the slide's step (default: one grid spacing)")
     ap.add_argument("--tolerance", type=int, default=0, help="--until-contact: overlapping voxels tolerated")
-    ap.add_argument("--render", choices=("exchanger", "samples"), default="exchanger",
-                    help="render the frame with the exchanger (manipulate_frame) or per sample (render_frame(moves=))")
+    ap.add_argument("--render", choices=("exchanger", "samples", "none"), default="exchanger",
+                    help="render the frame with the exchanger (manipulate_frame), per sample (render_frame(moves=)) or not at all")
+    ap.add_argument("--preview", action="store_true",
+                    help="write preview.png, preview_edited.png and preview_rgb.png: the sweep cast from --pose, before and after")
     ap.add_argument("--copy", action="store_true", help="copy the piece instead of moving it: the source stays (needs --render samples)")
     ap.add_argument("--with", dest="with_labels", type=int, nargs="+", default=None, metavar="L",
                     help="move these labels together with the piece's label, as one body (needs --render samples)")
@@ -129,8 +141,13 @@ def parse(argv=None):
     ap.add_argument("--knots", type=int, default=33, help="--twist / --bend / --taper: knots of the deformation's table")
     a = ap.parse_args(argv)
     a.deformed = a.twist is not None or a.bend is not None or a.taper is not None
+    if a.render == "none":
+        if not a.preview:
+            ap.error("--render none needs --preview: there would be nothing to look at")
+        if a.mesh:
+            ap.error("--render none stops after the preview: drop --mesh")
     if a.deformed:
-        if a.render != "samples":
+        if a.render == "exchanger":
             ap.error("--twist, --bend and --taper need --render samples: the exchanger renders rigid moves only")
         for flag, given in (("--arrange", a.arrange is not None), ("--place-at", a.place_at is not None),
                             ("--until-contact", a.until_contact)):
@@ -150,14 +167,14 @@ def parse(argv=None):
     if a.grouped:
         if a.arrange is not None:
             ap.error('--with and --carry are per item with --arrange: give the items "group": [labels]')
-        if a.render != "samples":
+        if a.render == "exchanger":
             ap.error("--with and --carry need --render samples: the exchanger renders one label per move")
         if a.carry and (a.down is None or not any(a.down)):
             ap.error("--carry needs --down X Y Z, not 0 0 0: what rests on the object is found along it")
         if a.until_contact:
             ap.error("--with and --carry cannot be combined with --until-contact: the slide moves one label")
     if a.copy:
-        if a.render != "samples":
+        if a.render == "exchanger":
             ap.error("--copy needs --render samples: the exchanger renders moves only")
         if a.rest == "drop":
             ap.error("--copy cannot drop the rest of the label: a copy vacates nothing")
@@ -215,6 +232,9 @@ def parse(argv=None):
         ap.error("--hwk takes H W and K as a .npy path or as 9 numbers")
     a.H, a.W = int(a.hwk[0]), int(a.hwk[1])
     a.K = (np.load(a.hwk[2]) if len(a.hwk) == 3 else np.array([float(v) for v in a.hwk[2:]])).astype(np.float32).reshape(3, 3)
+    if a.pick is not None and not (0 <= a.pick[0] < a.W and 0 <= a.pick[1] < a.H):
+        ap.error("--pick %d %d is outside the %d x %d view" % (a.pick[0], a.pick[1], a.W, a.H))
+    a.picked = None
     return a
 
 
@@ -288,11 +308,29 @@ def arrange_pieces(a, occ, labels, T, ext, spec, chosen):
         if p is not None:
             entry["overwritten"] = {str(k): v for k, v in next(report)["overwritten"].items()}
         rec.append(entry)
-    return r["moves"], r["pieces"], r["rest"], r["copies"], r["groups"], rec
+    return r["moves"], r["pieces"], r["rest"], r["copies"], r["groups"], rec, (r["occ"], r["labels"])
 
 
-def choose_piece(a, model_fine, T, ext):
-    """The sweep, its components and the moved piece -> (component id, its label, its centre, its Region)."""
+def pick_piece(a, occ, labels, T, ext, cc, pose_t):
+    """--pick: the piece under the pixel, from its ray cast through the sweep -> (component id, {label, piece, pixel, point});
+    exits on a miss."""
+    from dmnerf_b200.helpers import get_rays_at
+    from dmnerf_b200.objects import cast_grid
+    x, y = a.pick
+    o, d = get_rays_at(a.H, a.W, a.K, pose_t, [y * a.W + x])
+    c = cast_grid(occ, labels, T, o, d, a.near, a.far, ext, a.level, components=cc, normals=False)
+    piece = int(c["piece"][0])
+    if piece < 0:
+        raise SystemExit("move_objects: --pick %d %d: the pixel's ray hits no solid voxel of the sweep between near %g and far %g"
+                         % (x, y, a.near, a.far))
+    rec = {"pixel": [x, y], "label": int(c["label"][0]), "piece": piece, "point": c["point"][0].tolist()}
+    print("move_objects: picked label %d, piece %d at (%.4f, %.4f, %.4f)" % (rec["label"], piece, *rec["point"]))
+    return piece, rec
+
+
+def choose_piece(a, model_fine, T, ext, pose_t=None):
+    """The sweep, its components and the moved piece -> (component id, its label, its centre, its Region).  --pick (pose_t: the
+    pose on the device) also leaves the pick's record in a.picked."""
     import torch
     from dmnerf_b200.objects import (component_region, inventory_from_grid, largest_components, object_components, object_mask,
                                      occupancy_objects)
@@ -301,7 +339,9 @@ def choose_piece(a, model_fine, T, ext):
         occ, labels = occupancy_objects(model_fine, T, object_mask(ins_num, keep=range(ins_num)), a.grid_dim, ext, a.near, a.far,
                                         a.N_importance, device=next(model_fine.parameters()).device)
         cc = object_components(occ, labels, a.level, a.connectivity)
-        if a.move_piece is not None:
+        if a.pick is not None:
+            piece, a.picked = pick_piece(a, occ, labels, T, ext, cc, pose_t)
+        elif a.move_piece is not None:
             piece = int(a.move_piece)
             if not 0 <= piece < len(cc["label"]):
                 raise SystemExit("move_objects: piece %d does not exist (the sweep has %d pieces)" % (piece, len(cc["label"])))
@@ -362,6 +402,25 @@ def piece_deformation(a, occ, labels, T, ext, label, region, centre):
                        taper=None if a.taper is None else (lambda s: 1.0 + (a.taper - 1.0) * s))
 
 
+def write_previews(a, model_fine, occ, labels, T, ext, pose_t, lut, moves, regions, rests, copies, groups, deforms, arranged_grid):
+    """--preview: preview.png and preview_rgb.png of the keep-all sweep, preview_edited.png of its edited_grid under the moves
+    (or the arranged grid), all cast from --pose (grid_view)."""
+    import torch
+    from dmnerf_b200.objects import edited_grid, grid_view
+    from dmnerf_b200.tester import write_png
+    with torch.no_grad():
+        before = grid_view(occ, labels, T, a.H, a.W, a.K, pose_t, a.near, a.far, ext, a.level, lut=lut, model_fine=model_fine)
+        if arranged_grid is None:
+            e_occ, e_labels, _ = edited_grid(occ, labels, T, moves, ext, a.level, pieces=regions, rest=rests, copies=copies,
+                                             groups=groups, deformations=deforms)
+        else:
+            e_occ, e_labels = arranged_grid
+        after = grid_view(e_occ, e_labels, T, a.H, a.W, a.K, pose_t, a.near, a.far, ext, a.level, lut=lut)
+    write_png(os.path.join(a.out, "preview.png"), before["image"].cpu().numpy())
+    write_png(os.path.join(a.out, "preview_edited.png"), after["image"].cpu().numpy())
+    write_png(os.path.join(a.out, "preview_rgb.png"), (255 * torch.clamp(before["rgb"], 0, 1)).to(torch.uint8).cpu().numpy())
+
+
 def main(argv=None):
     a = parse(argv)
     import torch
@@ -383,24 +442,27 @@ def main(argv=None):
     T = np.load(a.transform) if a.transform.endswith(".npy") else np.loadtxt(a.transform)
     T, ext = M.check_transform(np.asarray(T, dtype=np.float64).reshape(4, 4)), tuple(a.extents)
     slide = place = arranged = None
+    dev = next(nets[1].parameters()).device
+    pose_t = torch.from_numpy(c2w).to(dev)
     if a.arrange is not None:
         spec = read_spec(a.arrange)
-        if any(it.get("copy", False) for it in spec) and a.render != "samples":
+        if any(it.get("copy", False) for it in spec) and a.render == "exchanger":
             raise SystemExit("move_objects: an arrangement with copies needs --render samples: the exchanger renders moves only")
-        if any(it.get("group") is not None for it in spec) and a.render != "samples":
+        if any(it.get("group") is not None for it in spec) and a.render == "exchanger":
             raise SystemExit("move_objects: an arrangement with groups needs --render samples: the exchanger renders one label per "
                              "move")
         chosen = choose_pieces(a, nets[1], T, ext, spec)
         piece, label, centre, region = None, None, None, None
     else:
-        piece, label, centre, region = choose_piece(a, nets[1], T, ext)
-    sweep = a.check or a.until_contact or a.place_at is not None or a.arrange is not None or a.render == "samples" or a.grouped
+        piece, label, centre, region = choose_piece(a, nets[1], T, ext, pose_t)
+    sweep = (a.check or a.until_contact or a.place_at is not None or a.arrange is not None or a.render == "samples" or a.grouped
+             or a.preview)
     if sweep:
         from dmnerf_b200.objects import object_mask, occupancy_objects
         with torch.no_grad():
             occ, labels = occupancy_objects(nets[1], T, object_mask(ins_num, remove=[]), a.grid_dim, ext, a.near, a.far,
                                             a.N_importance, device=next(nets[1].parameters()).device)
-    group = chain = None
+    group = chain = arranged_grid = None
     if a.grouped:                                      # the piece's label and the labels moved with it
         group = sorted(set(a.with_labels or []) | {label})
         if a.carry:
@@ -412,7 +474,7 @@ def main(argv=None):
         slide = slide_translation(a, occ, labels, T, ext, label, region)
         a.distance = np.sign(a.distance) * (slide["found"] or 0.0)
     if a.arrange is not None:
-        moves, regions, rests, copies, groups, arranged = arrange_pieces(a, occ, labels, T, ext, spec, chosen)
+        moves, regions, rests, copies, groups, arranged, arranged_grid = arrange_pieces(a, occ, labels, T, ext, spec, chosen)
         if not moves:
             raise SystemExit("move_objects: no item was placed: %s" % "; ".join("%d: %s" % (e["label"], e["reason"]) for e in arranged))
         trans = {"transformations": [{"transformation": m, "mode": "placement"} for _, m in moves]}
@@ -427,8 +489,12 @@ def main(argv=None):
         copies, groups = [a.copy], [group]
         if a.deformed:
             deforms = [piece_deformation(a, occ, labels, T, ext, label, region, centre)]
-    dev = next(nets[1].parameters()).device
-    pose_t = torch.from_numpy(c2w).to(dev)
+    os.makedirs(a.out, exist_ok=True)
+    ins_rgbs = np.random.default_rng(0).integers(0, 256, (ins_num + 1, 3))
+    lut = pred_label_lut({str(k): k for k in range(ins_num + 1)}, ins_rgbs, {str(k): k for k in range(ins_num + 1)},
+                         ins_num + 1)[:, ::-1]
+    if a.preview:
+        write_previews(a, nets[1], occ, labels, T, ext, pose_t, lut, moves, regions, rests, copies, groups, deforms, arranged_grid)
     evaluated = None
     if a.render == "samples":
         from dmnerf_b200.objects import render_moves
@@ -439,7 +505,7 @@ def main(argv=None):
             fr = render_frame(a.H, a.W, a.K, pose_t, a.near, a.far, nets[0], nets[1], a.N_samples, a.N_importance, keep_all_ins=True,
                               device=dev, moves=moved)
         rgb, ins, evaluated = fr["rgb"].reshape(-1, 3).to(dev), fr["ins"].reshape(a.H * a.W, -1).to(dev), list(fr["evaluated"])
-    else:
+    elif a.render == "exchanger":
         rays = [rigid_rays(a.H, a.W, a.K, m, pose_t) for _, m in moves]
         tar_o, tar_d = torch.stack([o for o, _ in rays]), torch.stack([d for _, d in rays])
         args = types.SimpleNamespace(N_test=a.N_test, N_samples=a.N_samples, N_importance=a.N_importance, near=a.near, far=a.far,
@@ -448,18 +514,17 @@ def main(argv=None):
         ve, _ = get_embedder(4)
         rgb, ins, _, _ = manipulate_frame(a.H, a.W, a.K, pose_t, tar_o, tar_d, pe, ve, nets[0], nets[1], args, pieces=regions,
                                           rest=rests)
-    os.makedirs(a.out, exist_ok=True)
-    write_png(os.path.join(a.out, "rgb.png"), (255 * torch.clamp(rgb, 0, 1)).to(torch.uint8).reshape(a.H, a.W, 3).cpu().numpy())
-    ins_rgbs = np.random.default_rng(0).integers(0, 256, (ins_num + 1, 3))
-    lut = pred_label_lut({str(k): k for k in range(ins_num + 1)}, ins_rgbs, {str(k): k for k in range(ins_num + 1)},
-                         ins_num + 1)[:, ::-1]
-    write_png(os.path.join(a.out, "instance.png"), colorize(argmax_rows(ins).reshape(a.H, a.W), lut).cpu().numpy())
+    if a.render != "none":
+        write_png(os.path.join(a.out, "rgb.png"), (255 * torch.clamp(rgb, 0, 1)).to(torch.uint8).reshape(a.H, a.W, 3).cpu().numpy())
+        write_png(os.path.join(a.out, "instance.png"), colorize(argmax_rows(ins).reshape(a.H, a.W), lut).cpu().numpy())
     if a.arrange is not None:
         record = {"transformations": trans["transformations"], "labels": [k for k, _ in moves], "rest": rests, "arrange": arranged}
     else:
         record = {"transformations": trans["transformations"], "label": label, "piece": piece, "centre": centre.tolist(),
                   "rest": a.rest}
     record["render"], record["evaluated"] = a.render, evaluated
+    if a.picked is not None:
+        record["pick"] = a.picked
     if any(copies):
         record["copies"] = copies
     if group is not None:
