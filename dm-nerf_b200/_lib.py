@@ -278,6 +278,9 @@ PROTOTYPES = {
     "dmnerf_grid_cast": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_double), C.POINTER(C.c_double),
                                    C.POINTER(C.c_uint32), _f32p, _f32p, C.c_int64, C.c_float, C.c_float, _f32p, C.c_void_p, C.c_void_p,
                                    _f32p, C.c_void_p]),
+    "dmnerf_grid_edit_source": (C.c_int, [C.c_void_p, _f32p, C.c_void_p, _f32p, C.c_void_p, C.POINTER(RenderMoves), C.POINTER(C.c_int32),
+                                          C.POINTER(C.c_uint32), C.POINTER(Deformation), _f32p, _f32p, _f32p, C.c_void_p, C.c_int64,
+                                          C.c_void_p, _f32p, _f32p, C.POINTER(C.c_int64), C.c_void_p]),
     "dmnerf_region_pack": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "dmnerf_region_dilate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "dmnerf_region_contains": (C.c_int, [C.POINTER(RegionDesc), _f32p, C.c_int64, C.c_void_p, C.c_void_p]),

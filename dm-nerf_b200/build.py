@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdmnerf_b200.so")
-SOURCES = ["abi.cu", "ray_kernels.cu", "mlp_simt.cu", "mlp_umma.cu", "backward.cu", "gemm_umma.cu", "penalizer.cu", "exchanger.cu", "evaluator.cu", "bwd_chain.cu", "mesh.cu", "metrics.cu", "inventory.cu", "components.cu", "region.cu", "collide.cu", "place.cu", "render_moves.cu", "raycast.cu"]
+SOURCES = ["abi.cu", "ray_kernels.cu", "mlp_simt.cu", "mlp_umma.cu", "backward.cu", "gemm_umma.cu", "penalizer.cu", "exchanger.cu", "evaluator.cu", "bwd_chain.cu", "mesh.cu", "metrics.cu", "inventory.cu", "components.cu", "region.cu", "collide.cu", "place.cu", "render_moves.cu", "raycast.cu", "edit_view.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 

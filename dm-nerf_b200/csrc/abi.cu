@@ -1288,6 +1288,17 @@ DMNERF_API int dmnerf_grid_cast(dmnerf_ctx* ctx, const float* occ, const int16_t
                    near_t, far_t, t_out, label_out, voxel_out, normal_out, (cudaStream_t)stream);
 }
 
+DMNERF_API int dmnerf_grid_edit_source(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* src_occ,
+                                       const int16_t* src_labels, const dmnerf_render_moves* moves, const int32_t* copies_host,
+                                       const uint32_t* groups_host, const dmnerf_deformation* deformations_host, const float* rays_o,
+                                       const float* rays_d, const float* t_out, const int32_t* voxel_out, int64_t n,
+                                       int32_t* move_out, float* point_out, float* dir_out, int64_t* mismatched_host, void* stream) {
+  DMN_CHECK(ctx != nullptr, "grid_edit_source: ctx is NULL");
+  DMN_CUDA(cudaSetDevice(ctx->device));
+  return grid_edit_source(ctx->inventory, occ, labels, src_occ, src_labels, moves, copies_host, groups_host, deformations_host, rays_o,
+                          rays_d, t_out, voxel_out, n, move_out, point_out, dir_out, mismatched_host, (cudaStream_t)stream);
+}
+
 // ---- test-view evaluation (networks/tester.py render_test, networks/evaluator.py ins_eval) --------------------------------
 
 DMNERF_API int64_t dmnerf_eval_workspace_bytes(int64_t n, int k, int H, int W) {

@@ -453,6 +453,14 @@ int region_contains(const Region& r, const float* pts, int64_t n, uint8_t* out, 
 int grid_cast(const float* occ, const int16_t* labels, int dim, float level, const double* T16, const double* ext3,
               const uint32_t* keep_host, const float* rays_o, const float* rays_d, int64_t n, float near_t, float far_t, float* t_out,
               int16_t* label_out, int32_t* voxel_out, float* normal_out, cudaStream_t st);
+// Colouring an edited view (edit_view.cu): per cast hit the move that placed it in the grid-only edit of src by `moves`, the colour
+// point and the un-normalised colour direction; *mismatched_host = the hits where the replay differs from occ / labels.  Checked
+// on the host before any launch; one read-back (fails on a voxel index outside [-1, dim^3)).
+int grid_edit_source(InventoryState& s, const float* occ, const int16_t* labels, const float* src_occ, const int16_t* src_labels,
+                     const dmnerf_render_moves* moves, const int32_t* copies_host, const uint32_t* groups_host,
+                     const dmnerf_deformation* deformations_host, const float* rays_o, const float* rays_d, const float* t_in,
+                     const int32_t* voxel_in, int64_t n, int32_t* move_out, float* point_out, float* dir_out,
+                     int64_t* mismatched_host, cudaStream_t st);
 
 // Test-view evaluation (metrics.cu)
 int64_t eval_workspace_bytes(int64_t n, int k, int H, int W);

@@ -47,19 +47,13 @@ __global__ void move_target_kernel(const EditMove m, const float* __restrict__ r
   if (DEFORM) {
     double w[3], x[3];
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      const double* r = m.trans + 4 * a;
-      w[a] = __dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)d[0]), __dmul_rn(r[1], (double)d[1])), __dmul_rn(r[2], (double)d[2]));
-    }
+    for (int a = 0; a < 3; ++a) w[a] = moved_vector(m.trans, a, d);
     deform_direction(dm, P, w, x);
 #pragma unroll
     for (int a = 0; a < 3; ++a) dt[a] = __double2float_rn(x[a]);
   } else {
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      const double* r = m.trans + 4 * a;
-      dt[a] = __double2float_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)d[0]), __dmul_rn(r[1], (double)d[1])), __dmul_rn(r[2], (double)d[2])));
-    }
+    for (int a = 0; a < 3; ++a) dt[a] = __double2float_rn(moved_vector(m.trans, a, d));
   }
   const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dt[0], dt[0]), __fmul_rn(dt[1], dt[1])), __fmul_rn(dt[2], dt[2])));
   float* out = tgt + 6 * i;

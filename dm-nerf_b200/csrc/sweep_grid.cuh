@@ -95,6 +95,13 @@ __device__ __forceinline__ double moved_coord(const double* trans, int a, const 
                    r[3]);
 }
 
+// w = trans[:3, :3] v in fp64, not rounded: the view direction of ray direction v under a move (the moved render, render_moves.cu,
+// and the edit view, edit_view.cu), before a deformation pulls it back and before it is rounded to fp32
+__device__ __forceinline__ double moved_vector(const double* trans, int a, const float v[3]) {
+  const double* r = trans + 4 * a;
+  return __dadd_rn(__dadd_rn(__dmul_rn(r[0], (double)v[0]), __dmul_rn(r[1], (double)v[1])), __dmul_rn(r[2], (double)v[2]));
+}
+
 __device__ __forceinline__ bool edit_target(const double* trans, const double* inv, const double* b, const double* lo,
                                             const double* hi, bool in, const float p[3], float t[3], double q[3]) {
   double dt[3];

@@ -33,7 +33,9 @@
     cast_grid(occ, labels, scene_transform, rays_o, rays_d, near, far, ...) / grid_view(occ, labels, scene_transform, H, W, K,
               c2w, near, far, ...)                     -> the first solid voxel along each ray (depth, label, voxel, normal,
                                                            piece), and depth, label, normal and colour maps of the grid
-                                                           from one or several cameras, with no network
+                                                           from one or several cameras, with no network; with moves= and
+                                                           source=, an edited grid's hits traced to the moves that placed
+                                                           them and coloured from the network at their source
 
 Every network sample is labelled argmax(sigmoid(instance logits)) over all ins_num + 1 channels, first maximum winning (the
 exchanger's rule); a sample whose label is not kept has alpha = 0 in the composite of both passes, so the coarse weights of the
@@ -2283,7 +2285,9 @@ def cast_grid(occ, labels, scene_transform, rays_o, rays_d, near, far, extents=N
     +inf without a hit), label (int16, -1), voxel (int64 [..., 3] index (i, j, k), -1), point (o + depth d in float32, NaN
     without a hit), normal (float32 [..., 3], 0 without a hit; None when normals=False) and hit (bool).  With components (an
     object_components result of this grid), also piece: the component id at the hit voxel (-1 without a hit).  The picking
-    primitive: the label and piece under a pixel come from the ray of that pixel (get_rays_at)."""
+    primitive: the label and piece under a pixel come from the ray of that pixel (get_rays_at).  On edited_grid's or
+    arrange_objects' grid, grid_view(moves=, source=) traces each hit voxel to the move that placed it and colours it from the
+    network at that move's source."""
     from .mesh import EXTENTS, check_transform
     T = check_transform(scene_transform)
     ext = np.asarray(EXTENTS if extents is None else extents, dtype=np.float64).reshape(-1)
@@ -2321,16 +2325,95 @@ def cast_grid(occ, labels, scene_transform, rays_o, rays_d, near, far, extents=N
     return out
 
 
+def _overlaps(a, b):
+    """Whether the storage of tensors a and b overlaps."""
+    x, y = _lib.ptr(a, a.dtype, strided=True).value, _lib.ptr(b, b.dtype, strided=True).value
+    return a.device == b.device and x < y + b.numel() * b.element_size() and y < x + a.numel() * a.element_size()
+
+
+def _check_edit_view(occ, labels, scene_transform, extents, level, moves, source):
+    """grid_view's moves= and source=, checked against the viewed grid before any device work -> True when given."""
+    from .mesh import EXTENTS, check_transform
+    if moves is None and source is None:
+        return False
+    if moves is None or source is None:
+        raise ValueError("grid_view: moves= and source= come together (the edit and the unedited sweep it was applied to)")
+    if not isinstance(moves, MovedScene):
+        raise ValueError("grid_view: moves must be an objects.render_moves(...) result, got %r" % (type(moves).__name__,))
+    if not isinstance(source, (tuple, list)) or len(source) != 2 or not all(torch.is_tensor(s) for s in source):
+        raise ValueError("grid_view: source must be the pair (occ, labels) of the unedited keep-all sweep")
+    s_occ, s_lab = source
+    if not (torch.is_tensor(occ) and torch.is_tensor(labels)):
+        raise ValueError("grid_view: occ and labels must be tensors")
+    if tuple(s_occ.shape) != tuple(occ.shape) or tuple(s_lab.shape) != tuple(occ.shape):
+        raise ValueError("grid_view: the source grid %s / %s is not the viewed grid's %s" % (tuple(s_occ.shape), tuple(s_lab.shape),
+                                                                                            tuple(occ.shape)))
+    if s_occ.dtype != torch.float32 or s_lab.dtype != torch.int16:
+        raise ValueError("grid_view: the source's occ must be float32 and its labels int16")
+    if s_occ.device != occ.device or s_lab.device != occ.device:
+        raise ValueError("grid_view: the source is on %s / %s, the viewed grid on %s" % (s_occ.device, s_lab.device, occ.device))
+    if moves.device != occ.device:
+        raise ValueError("grid_view: the moves were built on %s, the viewed grid is on %s" % (moves.device, occ.device))
+    d = moves.abi()
+    if occ.dim() != 3 or d.dim != occ.shape[0]:
+        raise ValueError("grid_view: the moves index a grid of dim %d, the viewed grid is %s" % (d.dim, tuple(occ.shape)))
+    T = check_transform(scene_transform)
+    ext = np.asarray(EXTENTS if extents is None else extents, dtype=np.float64).reshape(-1)
+    if not np.array_equal(np.asarray(d.transform[:], dtype=np.float64), T.reshape(-1)) or not (
+            ext.shape == (3,) and np.array_equal(np.asarray(d.extents[:], dtype=np.float64), ext)):
+        raise ValueError("grid_view: the moves were built on another grid (scene_transform or extents differ)")
+    if np.float32(d.level) != np.float32(level):
+        raise ValueError("grid_view: the moves were built at level %r, the view is at level %r" % (float(d.level), float(level)))
+    return True
+
+
+def _edit_view(occ, labels, moves, source, o, d, c):
+    """dmnerf_grid_edit_source on the cast c of the rays (o, d) [..., 3] -> (move int16, colour point, colour direction not
+    normalised) of the rays' shape; ValueError when a hit is not where the grid-only edit of source by moves put it."""
+    dim = occ.shape[0]
+    s_occ, s_lab = (t.contiguous() for t in source)
+    if any(_overlaps(s, g) for s in (s_occ, s_lab) for g in (occ, labels)):   # the same grid viewed as its own edit
+        s_occ, s_lab = s_occ.clone(), s_lab.clone()
+    shape = tuple(o.shape[:-1])
+    hit = c["hit"].reshape(-1)
+    v = c["voxel"].reshape(-1, 3)
+    lin = torch.where(hit, (v[:, 0] * dim + v[:, 1]) * dim + v[:, 2], torch.full_like(v[:, 0], -1)).to(torch.int32)
+    of, df = o.reshape(-1, 3).contiguous(), d.reshape(-1, 3).contiguous()
+    depth = c["depth"].reshape(-1).contiguous()
+    n = of.shape[0]
+    move = torch.empty(n, dtype=torch.int32, device=occ.device)
+    point = torch.empty((n, 3), dtype=torch.float32, device=occ.device)
+    vdir = torch.empty((n, 3), dtype=torch.float32, device=occ.device)
+    mismatched = C.c_int64(0)
+    ctx = get_context(occ.device)
+    ctx.call("dmnerf_grid_edit_source", ctx.handle, _lib.ptr(occ), _lib.ptr(labels, torch.int16), _lib.ptr(s_occ),
+             _lib.ptr(s_lab, torch.int16), C.byref(moves.abi()), moves.copy_flags(), moves.group_words(),
+             moves.deformation_array(), _lib.ptr(of), _lib.ptr(df), _lib.ptr(depth), _lib.ptr(lin, torch.int32), n,
+             _lib.ptr(move, torch.int32), _lib.ptr(point), _lib.ptr(vdir), C.byref(mismatched))
+    if mismatched.value:
+        raise ValueError("grid_view: %d of %d hit voxels differ from the grid-only edit of source by moves (the viewed grid is not "
+                         "edited_grid(source, moves) there); render it with render_moves and render_frame(moves=)"
+                         % (mismatched.value, int(hit.sum())))
+    return move.to(torch.int16).reshape(shape), point.reshape(shape + (3,)), vdir.reshape(shape + (3,))
+
+
 def grid_view(occ, labels, scene_transform, H, W, K, c2w, near, far, extents=None, level=0.45, keep=None, remove=None, lut=None,
-              model_fine=None):
+              model_fine=None, moves=None, source=None):
     """The labelled grid seen from one camera (c2w [4, 4] or [3, 4]) or several (c2w [V, 4, 4]), all views in one cast_grid
     launch.  Pixel (row, col) casts get_rays_k's ray, the ray render_frame renders there.  Returns device maps [V?, H, W] of depth,
     label and hit, and normal [V?, H, W, 3].  With lut (uint8 [L, 3], e.g. tester.pred_label_lut), also image [V?, H, W, 3] uint8:
     tester.colorize's label colours shaded by |n . d/|d||, black where nothing is hit.  With model_fine, also rgb [V?, H, W, 3]
     float32: sigmoid of the first three outputs of mlp_forward_points(model_fine, point, d/|d|) at the hit pixels (0 elsewhere),
-    one network query per pixel.  That colour is meaningful only on an unedited grid: on an edited grid the hit points of a moved,
-    copied or deformed object are not where the network holds its colour, and this function cannot tell the two grids apart --
-    render an edited scene with render_moves and render_frame(moves=)."""
+    one network query per pixel.  Without moves that colour is meaningful only on an unedited grid: on an edited grid the hit
+    points of a moved, copied or deformed object are not where the network holds its colour.
+    moves (a render_moves result, the value render_frame(moves=) takes) and source (the pair (occ, labels) of the unedited keep-all
+    sweep the moves were built on) come together, for occ / labels = edited_grid(source, moves) or arrange_objects' grid (DESIGN.md,
+    "Colouring an edited view").  Each hit voxel is traced through the moves (dmnerf_grid_edit_source): the result gains move
+    [V?, H, W] int16, the last move that placed the hit voxel (-1 off hits and where no move did), and with model_fine the colour of
+    a moved pixel is the network's at the hit point pulled back through that move, seen along the moved render's direction, as
+    render_frame(moves=) samples it; other pixels keep the colour above bit for bit.  The replay must reproduce occ / labels at
+    every hit voxel (the check covers the hits only): otherwise ValueError, with the number of differing hits, before the network
+    runs -- an edited_sweep grid, for one, holds the network's occupancies and is previewed with render_moves."""
     from .helpers import get_rays_k
     _check_range(near, far, level)
     if int(H) != H or int(W) != W or int(H) < 1 or int(W) < 1:
@@ -2345,13 +2428,18 @@ def grid_view(occ, labels, scene_transform, H, W, K, c2w, near, far, extents=Non
         lut = np.asarray(lut)
         if lut.dtype != np.uint8 or lut.ndim != 2 or lut.shape[1] != 3 or lut.shape[0] < 1:
             raise ValueError("grid_view: lut must be uint8 [L, 3]")
+    edited = _check_edit_view(occ, labels, scene_transform, extents, level, moves, source)
     _check_sweep(occ, labels, "grid_view")
+    if edited:
+        _check_sweep(source[0], source[1], "grid_view")
     poses = poses.to(occ.device)
     rays = [get_rays_k(H, W, K, poses[v]) for v in range(poses.shape[0])]
     o = torch.stack([r[0] for r in rays])
     d = torch.stack([r[1] for r in rays])
     c = cast_grid(occ, labels, scene_transform, o, d, near, far, extents, level, keep, remove)
     out = {k: c[k] for k in ("depth", "label", "normal", "hit")}
+    if edited:
+        out["move"], e_point, e_dir = _edit_view(occ, labels, moves, source, o, d, c)
     if lut is not None or model_fine is not None:
         dirs = d / torch.norm(d, dim=-1, keepdim=True)
     if lut is not None:
@@ -2362,8 +2450,13 @@ def grid_view(occ, labels, scene_transform, H, W, K, c2w, near, far, extents=Non
         from .autograd import mlp_forward_points
         rgb = torch.zeros(o.shape, dtype=torch.float32, device=occ.device)
         hit = c["hit"]
+        pts, vd = c["point"], dirs
+        if edited:                             # moved pixels: the pulled-back point and direction; the others as without moves
+            moved = (out["move"] >= 0)[..., None]
+            pts = torch.where(moved, e_point, pts)
+            vd = torch.where(moved, e_dir / torch.norm(e_dir, dim=-1, keepdim=True), vd)
         if bool(hit.any()):
             with torch.no_grad():
-                rgb[hit] = torch.sigmoid(mlp_forward_points(model_fine, c["point"][hit], dirs[hit])[:, :3])
+                rgb[hit] = torch.sigmoid(mlp_forward_points(model_fine, pts[hit], vd[hit])[:, :3])
         out["rgb"] = rgb
     return {k: v[0] for k, v in out.items()} if single else out

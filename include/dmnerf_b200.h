@@ -811,6 +811,25 @@ DMNERF_API int dmnerf_grid_cast(dmnerf_ctx* ctx, const float* occ, const int16_t
                                 const double* transform_host, const double* extents_host, const uint32_t* keep_words_host,
                                 const float* rays_o, const float* rays_d, int64_t n, float near_t, float far_t, float* t_out,
                                 int16_t* label_out, int32_t* voxel_out, float* normal_out, void* stream);
+/* dmnerf_grid_edit_source: where each hit of dmnerf_grid_cast on an edited grid came from (DESIGN.md, "Viewing the labelled grid",
+ *   "Colouring an edited view").  occ / labels [dim^3] (DEVICE) is the viewed grid, src_occ / src_labels [dim^3] (DEVICE, separate
+ *   memory) the unedited source, and moves (with copies_host [n_moves], groups_host [n_moves][4] and deformations_host [n_moves],
+ *   each HOST and may be NULL, as dmnerf_render_moved_deformed) the edit; moves->dim, transform, extents and level give the grid.
+ *   rays_o / rays_d [n][3] and t_out / voxel_out [n] (DEVICE) are the cast's rays and outputs.  Per ray with voxel q >= 0 the
+ *   moves of dmnerf_grid_edit are replayed at q's sweep point alone, from (src_occ[q], src_labels[q]), with that call's take and
+ *   vacate; move_out [n] (DEVICE int32) = the last move that took (-1: none, or no hit).  The replay's result must equal
+ *   (occ[q], labels[q]), the occupancy by its bits: *mismatched_host (HOST int64) = the hits where it does not.  x = o + t d (fp32,
+ *   multiply then add).  point_out [n][3] (DEVICE float32) = the target of x under move_out (edit_target, pulled through its
+ *   deformation), x where no move took, NaN without a hit; dir_out [n][3] (DEVICE float32) = trans[:3, :3] d in fp64 (pulled back
+ *   by the deformation's tangent at x's pulled point), rounded once, not normalised; d where no move took; 0 without a hit.
+ *   Rejected on the host before any launch: everything dmnerf_render_moved_deformed rejects of the moves (labels in [0, 127]),
+ *   dim above 1290, NULL pointers, n < 0, source and viewed grids that overlap.  One read-back (synchronises the stream); fails
+ *   after it when a voxel index lies outside [-1, dim^3). */
+DMNERF_API int dmnerf_grid_edit_source(dmnerf_ctx* ctx, const float* occ, const int16_t* labels, const float* src_occ,
+                                       const int16_t* src_labels, const dmnerf_render_moves* moves, const int32_t* copies_host,
+                                       const uint32_t* groups_host, const dmnerf_deformation* deformations_host, const float* rays_o,
+                                       const float* rays_d, const float* t_out, const int32_t* voxel_out, int64_t n,
+                                       int32_t* move_out, float* point_out, float* dir_out, int64_t* mismatched_host, void* stream);
 
 /* ---- region selection (DESIGN.md, "Region selection"; no counterpart in the original) ------------------------------------
  * A region (dmnerf_region) is one bit per point of a sweep grid [dim,dim,dim] (dim in [2, 1290]; point v = (i dim + j) dim + k

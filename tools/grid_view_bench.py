@@ -6,6 +6,10 @@
   look          for one move of the sweep's largest label at grid_dim 256: edited_grid + grid_view (the preview of the edit)
                 against render_moves + render_frame(moves=) (the network render of the same move), alternating in each round,
                 host clock around a synchronised call;
+  colour        for one and for three moves at grid_dim 256: edited_grid + grid_view(model_fine=, moves=, source=) (the preview in
+                the edit's network colour) against render_moves + render_frame(moves=) of the same moves, alternating, host clock;
+                and the preview's device stages apart (CUDA events): the cast, the replay (dmnerf_grid_edit_source) and the network
+                query at the hit pixels;
 and the GPU's name and power limit read in the same run.  Median of --reps rounds after --warmup.
     python tools/grid_view_bench.py [--reps 5] [--warmup 1]"""
 import argparse
@@ -14,9 +18,11 @@ import json
 import numpy as np
 import torch
 
-from _harness import alternate, cuda_device, event_ms, gpu_identity, host_ms
+from _harness import alternate, cuda_device, event_ms, gpu_identity, host_ms, stages_ms
 from dmnerf_b200 import objects as OB
 from dmnerf_b200 import synth
+from dmnerf_b200.autograd import mlp_forward_points
+from dmnerf_b200.helpers import get_rays_k
 from dmnerf_b200.render import render_frame
 from dmnerf_b200.testing import make_models
 
@@ -33,6 +39,54 @@ def _kernel_ms(fn):
         fn()
         torch.cuda.synchronize()
     return round(sum(e.device_time_total for e in prof.key_averages() if "grid_cast_kernel" in e.key) / 1e3, 3)
+
+
+def _colour(occ, labels, T, H, W, K, pose, near, far, level, nc, nf, dev, n_moves, a):
+    """The coloured preview of n_moves moves (the largest labels, each by 8 voxels along its own axis) against their network
+    render, and the preview's device stages."""
+    dim = occ.shape[0]
+    k, c = torch.unique(labels[occ > level], return_counts=True)
+    order = [int(v) for v in k[torch.argsort(c, descending=True, stable=True)]]
+    A, _ = OB.grid_affine(T, dim, EXT)
+    moves = []
+    for label, delta in zip(order, ([8.0, 0.0, 0.0], [0.0, 0.0, 8.0], [-8.0, 0.0, 0.0])[:n_moves]):
+        m = np.eye(4)
+        m[:3, 3] = A @ np.asarray(delta)
+        moves.append((label, m))
+    source = (occ, labels)
+
+    def preview():
+        e_occ, e_labels, _ = OB.edited_grid(occ, labels, T, moves, EXT, level)
+        moved = OB.render_moves(occ, labels, T, moves, EXT, level, near, far, NI)
+        return OB.grid_view(e_occ, e_labels, T, H, W, K, pose, near, far, EXT, level, model_fine=nf, moves=moved, source=source)
+
+    def render():
+        moved = OB.render_moves(occ, labels, T, moves, EXT, level, near, far, NI)
+        return render_frame(H, W, K, pose, near, far, nc, nf, N_samples=S, N_importance=NI, moves=moved, chunk=CHUNK, device=dev)
+    with torch.no_grad():
+        ms = alternate({"edited_grid+grid_view(moves)": preview, "render_moves+render_frame": render}, a.reps, a.warmup,
+                       clock=host_ms)
+        e_occ, e_labels, _ = OB.edited_grid(occ, labels, T, moves, EXT, level)
+        moved = OB.render_moves(occ, labels, T, moves, EXT, level, near, far, NI)
+        o, d = get_rays_k(H, W, K, pose)
+
+        def query(cr):
+            cast, (move, point, vdir) = cr
+            hit = cast["hit"]
+            return mlp_forward_points(nf, point[hit], (vdir / torch.norm(vdir, dim=-1, keepdim=True))[hit])
+        stages = []
+        for r in range(a.warmup + a.reps):
+            t, res = stages_ms(lambda: OB.cast_grid(e_occ, e_labels, T, o, d, near, far, EXT, level),
+                               lambda cast: (cast, OB._edit_view(e_occ, e_labels, moved, source, o, d, cast)), query)
+            if r >= a.warmup:
+                stages.append(t)
+        moved_px = int((res[1][1][0] >= 0).sum())
+    med = {k2: _med(v) for k2, v in ms.items()}
+    st = np.asarray(stages)
+    return {"moves": n_moves, "labels": [k2 for k2, _ in moves], "moved_pixels": moved_px,
+            "ms": {k2: [round(x, 2) for x in v] for k2, v in ms.items()}, "ms_median": med,
+            "render_over_preview": round(med["render_moves+render_frame"] / med["edited_grid+grid_view(moves)"], 1),
+            "device_ms_median": {"cast": _med(st[:, 0]), "replay": _med(st[:, 1]), "network": _med(st[:, 2])}}
 
 
 def main():
@@ -85,6 +139,7 @@ def main():
             out["look"] = {"grid_dim": dim, "label": label, "ms": {k2: [round(x, 2) for x in v] for k2, v in ms2.items()},
                            "ms_median": med,
                            "render_over_preview": round(med["render_moves+render_frame"] / med["edited_grid+grid_view"], 1)}
+            out["colour"] = [_colour(occ, labels, T, H, W, K, pose, near, far, level, nc, nf, dev, n, a) for n in (1, 3)]
         del occ, labels
     name, smi, card = gpu_identity(dev)
     name, power = card or (name, "unknown")

@@ -59,8 +59,10 @@ edit costs a grid edit and a voxel walk per pixel instead of a network render.
 
 Previews (--preview; DESIGN.md, "Viewing the labelled grid"): before the frame is rendered, the keep-all sweep is cast from --pose
 (grid_view): DIR/preview.png shows the unedited grid and DIR/preview_edited.png the edited_grid of the same moves (or the
-arrangement), in instance.png's colours shaded by the angle between surface and ray, and DIR/preview_rgb.png the network's colour
-at the unedited grid's hits (one query per pixel).  The network colour of moved objects is render_moves' job (--render samples).
+arrangement), in instance.png's colours shaded by the angle between surface and ray, DIR/preview_rgb.png the network's colour
+at the unedited grid's hits (one query per pixel) and DIR/preview_edited_rgb.png the edited grid in the edit's network colour:
+each hit traced to the move that placed it and coloured from the network at that move's source (grid_view(moves=, source=);
+DESIGN.md, "Colouring an edited view"), for every edit the tool builds.
 
 Deforming (--twist DEG, --bend D --bend-dir X Y Z, --taper S, with --up X Y Z and --knots K; DESIGN.md, "Deforming objects"):
 the piece is twisted, bent and tapered before its move, about its inventory centre, over its extent along --up in the sweep; the
@@ -123,7 +125,8 @@ def parse(argv=None):
     ap.add_argument("--render", choices=("exchanger", "samples", "none"), default="exchanger",
                     help="render the frame with the exchanger (manipulate_frame), per sample (render_frame(moves=)) or not at all")
     ap.add_argument("--preview", action="store_true",
-                    help="write preview.png, preview_edited.png and preview_rgb.png: the sweep cast from --pose, before and after")
+                    help="write preview.png, preview_edited.png, preview_rgb.png and preview_edited_rgb.png: the sweep cast "
+                         "from --pose, before and after, in label and network colours")
     ap.add_argument("--copy", action="store_true", help="copy the piece instead of moving it: the source stays (needs --render samples)")
     ap.add_argument("--with", dest="with_labels", type=int, nargs="+", default=None, metavar="L",
                     help="move these labels together with the piece's label, as one body (needs --render samples)")
@@ -403,10 +406,11 @@ def piece_deformation(a, occ, labels, T, ext, label, region, centre):
 
 
 def write_previews(a, model_fine, occ, labels, T, ext, pose_t, lut, moves, regions, rests, copies, groups, deforms, arranged_grid):
-    """--preview: preview.png and preview_rgb.png of the keep-all sweep, preview_edited.png of its edited_grid under the moves
-    (or the arranged grid), all cast from --pose (grid_view)."""
+    """--preview: preview.png and preview_rgb.png of the keep-all sweep, preview_edited.png and preview_edited_rgb.png of its
+    edited_grid under the moves (or the arranged grid), all cast from --pose (grid_view); the edited colour traces each hit to
+    the move that placed it (grid_view(moves=, source=))."""
     import torch
-    from dmnerf_b200.objects import edited_grid, grid_view
+    from dmnerf_b200.objects import edited_grid, grid_view, render_moves
     from dmnerf_b200.tester import write_png
     with torch.no_grad():
         before = grid_view(occ, labels, T, a.H, a.W, a.K, pose_t, a.near, a.far, ext, a.level, lut=lut, model_fine=model_fine)
@@ -415,10 +419,15 @@ def write_previews(a, model_fine, occ, labels, T, ext, pose_t, lut, moves, regio
                                              groups=groups, deformations=deforms)
         else:
             e_occ, e_labels = arranged_grid
-        after = grid_view(e_occ, e_labels, T, a.H, a.W, a.K, pose_t, a.near, a.far, ext, a.level, lut=lut)
+        moved = render_moves(occ, labels, T, moves, ext, a.level, a.near, a.far, a.N_importance, pieces=regions, rest=rests,
+                             copies=copies, groups=groups, deformations=deforms)
+        after = grid_view(e_occ, e_labels, T, a.H, a.W, a.K, pose_t, a.near, a.far, ext, a.level, lut=lut, model_fine=model_fine,
+                          moves=moved, source=(occ, labels))
+    to8 = lambda rgb: (255 * torch.clamp(rgb, 0, 1)).to(torch.uint8).cpu().numpy()   # noqa: E731
     write_png(os.path.join(a.out, "preview.png"), before["image"].cpu().numpy())
     write_png(os.path.join(a.out, "preview_edited.png"), after["image"].cpu().numpy())
-    write_png(os.path.join(a.out, "preview_rgb.png"), (255 * torch.clamp(before["rgb"], 0, 1)).to(torch.uint8).cpu().numpy())
+    write_png(os.path.join(a.out, "preview_rgb.png"), to8(before["rgb"]))
+    write_png(os.path.join(a.out, "preview_edited_rgb.png"), to8(after["rgb"]))
 
 
 def main(argv=None):
